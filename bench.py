@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric on its config 2 (the 1xB200 IVF_PQ case):
+"""bench.py -- BASELINE.json's metric on its config 2 (the single-GPU IVF_PQ case, 1 x H100):
 ANN queries/sec, 1M x 768 f32, IVF_PQ nlist=1024, PQ m=96x8bit, nprobes=20, k=10, batch=1024.
 
 A "step" = one pass of the hot path over one batch of 1024 synthetic queries.
@@ -11,7 +11,8 @@ A "step" = one pass of the hot path over one batch of 1024 synthetic queries.
               L2 flushed (untimed) between calls; `e2e.pipelined` = the same batches through
               lgpu_search_async with two calls in flight (no flush possible inside a pipeline);
   roofline  : algorithmic PQ-code bytes of the batch / the scan kernel's measured duration
-              (CUDA events recorded around the kernel by the library) vs the measured HBM peak;
+              (CUDA events recorded around the kernel by the library) vs the HBM peak
+              (MEASURED_PEAKS.json when present, else the H100 SXM data sheet);
   cpu_baseline : the CPU oracle (a port of the reference's lance path) on the host cores the
               process may actually use (affinity and cgroup quota), best of 3 repetitions;
   gate      : before anything is timed, the GPU results of 128 ground-truth queries must be
@@ -24,8 +25,11 @@ path (lgpu_search_sharded_device: one in-library ncclAllGather of 16-byte top-k 
 `sharded` = config 2 split N ways on ONE shared batch, gated bit-for-bit against the single-GPU
 result and the oracle; `c5` = a BASELINE configs[4]-shaped shard (12.2M rows per GPU, nlist 16384,
 batch 8192; the true 100M-row config at N = 8), oracle-checked on the probed partitions.
-`--impl reference` times the CPU oracle alone (the reference's Rust path cannot be built
-here: no cargo, lance un-vendored), rank 0 only.
+`--impl reference` times the CPU oracle alone (the reference's Rust path is not built by this
+project), rank 0 only.
+`--dump-outputs DIR` writes what the last timed step returned (ids.npy as float64, distances.npy
+and counts.npy as float32) after the timed region: the inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -251,7 +255,7 @@ def sparse_oracle_index(full_desc, sizes, goff, parts, seed):
 
 # ------------------------------------------------------------------------------------------ clocks / peaks
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -297,19 +301,8 @@ def measured_peaks():
             j = json.load(f)
         return float(j["hbm_gbs"]), float(j["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
-
-
-def profiled_traffic():
-    """dram__bytes_read+write per launch of the scan kernel from the committed ncu --set full capture
-    (profiles/): a profiler number, so it is read from the profile, never measured in this run."""
-    try:
-        cands = sorted(f for f in os.listdir(os.path.join(ROOT, "profiles")) if f.endswith("_scan_traffic.json"))
-        with open(os.path.join(ROOT, "profiles", cands[-1])) as f:
-            j = json.load(f)
-        return float(j["dram_bytes_per_launch"]), j.get("kernel")
-    except Exception:
-        return None, None
+        # H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 (at up to 700 W; never reached here)
+        return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 # ------------------------------------------------------------------------------------------ CPU arm
@@ -411,6 +404,17 @@ def same(a, b):
                 and np.array_equal(np.asarray(a[2]).view(np.uint32), np.asarray(b[2]).view(np.uint32)))
 
 
+def dump_outputs(out_dir, d_ids, d_dist, d_cnt):
+    """The arrays a caller of lgpu_search_device receives, as float npy files: row ids (u64 payload, exact in f64
+    below 2^53; UINT64_MAX marks an empty slot and is written as -1), distances, per-query result counts."""
+    os.makedirs(out_dir, exist_ok=True)
+    ids = d_ids.cpu().numpy().view(np.uint64)
+    ids_f = np.where(ids == np.iinfo(np.uint64).max, -1.0, ids.astype(np.float64))
+    np.save(os.path.join(out_dir, "ids.npy"), ids_f)
+    np.save(os.path.join(out_dir, "distances.npy"), d_dist.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "counts.npy"), d_cnt.cpu().numpy().view(np.uint32).astype(np.float32))
+
+
 # ------------------------------------------------------------------------------------------ timing helpers
 class DeviceRunner:
     """Device-resident timing of an IVF_PQ handle: CUDA events per step on the launching stream, 512 MiB L2
@@ -478,7 +482,7 @@ def ivf_extra_workload(torch, _native, name, icfg, runner, peak_gbs, steps=4, ch
     return out
 
 
-def flat_extra_workload(torch, _native, runner, peak_tf, steps=5, check=4):
+def flat_extra_workload(torch, _native, runner, peak_tf, peak_src, steps=5, check=4):
     """BASELINE configs[3]: 1M x 1536 flat L2 as a bf16 tensor-core GEMM shortlist + exact f32 re-score + top-k."""
     import oracle
     N, dim, B, k = 1_000_000, 1536, 1024, 10
@@ -503,7 +507,7 @@ def flat_extra_workload(torch, _native, runner, peak_tf, steps=5, check=4):
            "oracle_check_queries": check,
            "roofline": {"bound": "tensor", "achieved": flops / t / 1e12, "peak": peak_tf, "unit": "TFLOP/s",
                         "frac": flops / t / 1e12 / peak_tf, "note": "whole step (GEMM shortlist + exact re-score + "
-                        "top-k) over 2*B*N*d flops, vs the sustained bf16 peak"}}
+                        "top-k) over 2*B*N*d flops, vs the bf16 peak", "peak_source": peak_src}}
     fl.close()
     del v, q
     torch.cuda.empty_cache()
@@ -568,6 +572,7 @@ def main():
     ap.add_argument("--parallelism", default="replicas", choices=["replicas", "sharded"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip latency / extra_workloads / sharded / c5 blocks")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's ids / distances / counts as .npy")
     args = ap.parse_args()
     cfg = WORKLOADS[args.workload]
     args.warmup = max(args.warmup, 3) if args.impl == "native" else args.warmup
@@ -678,6 +683,8 @@ def main():
     barrier()
     launches = _native.kernel_launch_count() - launches0
     step_ms = [a.elapsed_time(b) for a, b in ev]
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, d_ids, d_dist, d_cnt)
     total_ms = torch.tensor([sum(step_ms)], dtype=torch.float64, device=device)
     if world > 1:
         dist.all_reduce(total_ms, op=dist.ReduceOp.MAX)
@@ -746,7 +753,6 @@ def main():
     _native.set_profiling(False)
     scan_avg = float(np.mean(scan_ms))
     achieved = code_bytes / (scan_avg / 1e3) / 1e9
-    traffic, traffic_kernel = profiled_traffic()
 
     out = None
     if rank == 0:
@@ -764,8 +770,9 @@ def main():
             "stage_ms": stage,
             "filter_stats": filter_stats,        # last profiled batch: candidates appended / re-scored, exact fix-ups
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs,
-                         "traffic": traffic, "traffic_kernel": traffic_kernel,
-                         "kernel": "PQ code scan (dominant kernel of the step; name in profiles/)",
+                         "kernel": "PQ code scan (dominant kernel of the step)",
+                         "note": ("algorithmic bytes count a partition's codes once per query that probes it; a tile of "
+                                  "<= 8 queries reads them from HBM once, so a value above 1.0 is on-chip reuse"),
                          "kernel_ms": scan_avg, "algorithmic_bytes_per_launch": code_bytes, "peak_source": peak_src,
                          "whole_step_frac": code_bytes / (total_ms / args.steps / 1e3) / 1e9 / peak_gbs,
                          "compulsory_bytes_per_launch": int(full_ix.codes_t.size)},
@@ -793,7 +800,7 @@ def main():
             ("c2_clustered", lambda: clustered_workload(torch, _native, oracle, args, device, runner, peak_gbs)),
             ("c3", lambda: ivf_extra_workload(torch, _native, "BASELINE.json configs[2]", dict(
                 n=10_000_000, dim=768, nlist=4096, m=96, nprobes=50, k=100, batch=4096, metric="cosine"), runner, peak_gbs)),
-            ("c4", lambda: flat_extra_workload(torch, _native, runner, peak_tf)),
+            ("c4", lambda: flat_extra_workload(torch, _native, runner, peak_tf, peak_src)),
         ):
             try:
                 t0 = time.time()

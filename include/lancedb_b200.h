@@ -1,5 +1,5 @@
 /*
- * lancedb_b200.h -- C ABI of the B200-native LanceDB vector-query hot path.
+ * lancedb_b200.h -- C ABI of the H100-native (sm_90a) LanceDB vector-query hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b): the entry points the Rust
  * `lancedb` crate would bind through `extern "C"` at the single place it hands a

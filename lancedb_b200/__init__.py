@@ -1,4 +1,4 @@
-"""lancedb_b200 -- B200-native (sm_100a) implementation of LanceDB's vector-query hot path.
+"""lancedb_b200 -- H100-native (sm_90a) implementation of LanceDB's vector-query hot path.
 
 Scope: `Table.search(...)...to_arrow()` over an IVF_PQ index and the flat brute-force path
 (SURVEY.md section 8).  Compute lives in hand-written CUDA behind the C ABI of

@@ -54,7 +54,7 @@ class SearchParams(C.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     r = subprocess.run(cmd, capture_output=not verbose, text=True)
     if r.returncode != 0:

@@ -1,5 +1,5 @@
 """Async surface mirroring the reference's `AsyncTable.query().nearest_to(...).to_arrow()` for the vector-query hot
-path (/root/reference/python/python/lancedb/query.py:3307-3405 `AsyncQuery.nearest_to`, :3551-3723
+path (python/python/lancedb/query.py:3307-3405 `AsyncQuery.nearest_to`, :3551-3723
 `AsyncVectorQueryBase`, :2867-2960 `to_batches / to_arrow / to_list / to_pandas`; SURVEY.md 8b "Surface that must stay
 unchanged").
 

@@ -516,8 +516,7 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     if (Ns == N) launch_filter_dense(Dbuf, lds, B, N, flt, st);      // the sample pass already scored every row
     else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
-    // 3. exact re-score of the admitted rows, final top-k.  (Launch shapes that skip the empty slots -- a loop
-    // over the filled slots, 32- or 64-slot CTAs -- measured no faster at C2 and slower at C4 / C5 shapes.)
+    // 3. exact re-score of the admitted rows, final top-k (one pair per slot, empty slots included)
     launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, cap, d, LGPU_L2, ws->t_exact.as<float>(), st);
     SelectArgs sb{};
     sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
@@ -602,10 +601,12 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         // the bf16 error band around the nprobes-th centroid has to fit in the shortlist, so take 3x
         // nprobes (>= 64) candidates (dense variant) or admit by threshold (filtered variant)
         const uint32_t kp = std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(64, 3 * nprobes));
-        // from ~1M (query, centroid) pairs the tensor-core shortlist wins (C2: 0.16 vs 0.19 ms)
-        const bool big = (uint64_t)B * nlist >= ((uint64_t)1 << 20) || getenv("LGPU_FORCE_TC_COARSE");
+        // the tensor-core shortlist wins at every shape measured on 1 x H100 (400 W), down to 64 queries x 1024 lists
+        // (coarse step 0.052 vs 0.063 ms; 512 x 1024: 0.082 vs 0.160 ms); smaller problems were not measured and
+        // keep the exact kernels
+        const bool big = (uint64_t)B * nlist >= ((uint64_t)1 << 16) || getenv("LGPU_FORCE_TC_COARSE");
         if (ix->has_tc && tc_enabled() && ix->metric != LGPU_DOT && B >= 8 && nlist >= 256 && kp > nprobes && big) {
-            // tcgen05 GEMM scores + one finishing kernel per query (threshold, exact re-score in lance order, top
+            // tensor-core GEMM scores + one finishing kernel per query (threshold, exact re-score in lance order, top
             // nprobes): bit-identical probe sets; queries whose candidate band overflowed are redone exactly
             mark();
             ws->qb.ensure((size_t)B * dim * 2); ws->qn2.ensure((size_t)B * 4); ws->flags.ensure((size_t)B * 4);
@@ -613,8 +614,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
             uint32_t *cgate = ws->c_wcnt.as<uint32_t>() + 2;    // 0 = no query overflowed: the exact fix-up returns at once
             launch_to_bf16(qsearch, B, dim, ws->qb.p, ws->qn2.as<float>(), st);
             if (modes.coarse_list_min && nlist >= modes.coarse_list_min && ix->cent_ns >= 4 * nprobes && nprobes <= 64) {
-                // Many lists (C5: 16384): a dense [B][nlist] score matrix is 537 MB written and read back, which bounds
-                // the GEMM (tensor pipe 34 %).  Instead: (1) dense scores of a strided SAMPLE of the centroids; their
+                // Many lists (C5: 16384): a dense [B][nlist] score matrix is 537 MB written and read back.  Instead: (1) dense scores of a strided SAMPLE of the centroids; their
                 // nprobes-th smallest + 2 E_q bounds, per query, the scores of every true probe; (2) the full GEMM runs
                 // with the filtering epilogue and appends (column, score) of the few columns under that bound to the
                 // query's list; (3) the finishing kernel works on the list (second-level threshold from the list's own
@@ -1928,7 +1928,7 @@ int lgpu_ivf_assign(const float *centroids, uint32_t nlist, uint32_t dim, int me
     });
 }
 
-// nearest centre of every row (device buffers): the search's coarse step with nprobes = 1 -- tcgen05 GEMM scores +
+// nearest centre of every row (device buffers): the search's coarse step with nprobes = 1 -- tensor-core GEMM scores +
 // coarse_finish_kernel (exact re-score, lance arithmetic) where the shape allows it, the exact kernels otherwise
 static void assign_nearest(const float *d_x, uint64_t n, uint32_t dim, const float *d_cent, uint32_t k, int num_sms,
                            uint64_t *d_ids, float *d_dist, cudaStream_t st)

@@ -36,7 +36,7 @@ void count_launches(uint64_t n);
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------
 // A search step is ~25 launches, most of them a few microseconds long, and every kernel boundary costs a drain + launch
-// gap of 2-4 us (about 50 us of BASELINE config 2's 0.66 ms step).  launch_k() launches with the programmatic-stream-
+// gap of its own.  launch_k() launches with the programmatic-stream-
 // serialization attribute and the kernels it is used for begin with pdl_entry(): they tell the scheduler that the NEXT
 // grid may be brought onto the SMs already, then wait until the PREVIOUS grid has completed and flushed before touching
 // memory.  Correctness needs nothing else: every kernel waits for its predecessor, which waited for its own.

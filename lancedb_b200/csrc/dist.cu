@@ -252,8 +252,7 @@ __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *
                                                                    const uint32_t *__restrict__ list_cnt)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
-    // long rows only are staged through shared memory: at VPT 4 / 16 the few register loads are cheaper than the
-    // extra barrier (measured: C2 and C3 coarse steps 4 % slower with staging, C5's 35 % faster)
+    // long rows only are staged through shared memory: at VPT 4 / 16 the few register loads avoid the extra barrier
     constexpr bool STAGED = VPT >= 64;
     constexpr int NV0 = STAGED ? VPT : 0;
     extern __shared__ __align__(16) unsigned char csm[];
@@ -273,8 +272,8 @@ __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *
     if constexpr (STAGED) {
         // The row goes global -> shared with cp.async (16 B per request, all VPT / 4 requests of a thread in flight at
         // once), then shared -> registers.  Register loads, however they were written, came out of ptxas as
-        // load -> use -> load: 64 serial DRAM round trips per thread, 60 % of the kernel's stall samples at nlist 16384
-        // (profiles/r02_ncu_summary.txt).  ld is a multiple of 4 floats and the buffer holds ld floats per row.
+        // load -> use -> load: 64 serial DRAM round trips per thread at nlist 16384.  ld is a multiple of 4 floats and
+        // the buffer holds ld floats per row.
         const uint32_t s_base = (uint32_t)__cvta_generic_to_shared(s_row);
         for (uint32_t i = (uint32_t)tid * 4; i < ld && i < (uint32_t)VPT * CF_THREADS; i += CF_THREADS * 4)
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s_base + i * 4), "l"(row + i) : "memory");

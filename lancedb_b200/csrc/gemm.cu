@@ -1,28 +1,27 @@
-// gemm.cu -- tcgen05 / TMEM / TMA bf16 GEMM used as a *shortlist generator*.
+// gemm.cu -- wgmma / TMA bf16 GEMM used as a *shortlist generator*.
 //
 // Where the path is a true dense Q x C contraction -- the IVF coarse step
 // (IvfModel::find_partitions, SURVEY.md 8a row a3) at large nlist and the flat
 // KNNVectorDistance (row a11, BASELINE config 4) -- the reference spends
-// B*N*d fused multiply-adds of f32 SIMD.  Here the bulk of that work runs on the 5th-gen
-// tensor cores in bf16 with f32 accumulation in TMEM:
+// B*N*d fused multiply-adds of f32 SIMD.  Here the bulk of that work runs on the Hopper
+// tensor cores in bf16 with f32 accumulation in registers:
 //     S[q][x] = |x|^2 - 2 * sum_k bf16(q_k) * bf16(x_k)          (= |q-x|^2 - |q|^2, approx.)
 // and is only used to pick candidates: the caller keeps every column whose S is within a
 // rigorous error band of the k-th best and re-scores those exactly in f32 in lance's
 // rounding order (dist.cu), so the final ids / distances are still bit-identical to the
 // oracle while >99.9% of the arithmetic is tensor-core work.
 //
-// Kernel anatomy (one persistent CTA per SM, 192 threads, cta_group::1):
-//   warp 0      TMA producer: cp.async.bulk.tensor.2d of a 128x64 Q tile and a 256x64 X tile
-//               (bf16, K-major, SWIZZLE_128B) into a 4-stage shared-memory ring, mbarrier
-//               complete_tx signalling;
-//   warp 1      TMEM allocator + MMA issuer: one elected lane issues
-//               tcgen05.mma.cta_group::1.kind::f16 (M=128, N=256, K=16) x4 per stage,
-//               tcgen05.commit releases the stage / publishes the accumulator;
-//   warps 2-5   epilogue: tcgen05.ld 32x32b.x32 of their TMEM lane quadrant, |x|^2 - 2*acc,
-//               128-byte row stores; two 256-column accumulators double-buffer MMA against
-//               the epilogue.
-// Tiles are walked N-tile-major so the eight 128-query tiles of a batch reuse an X tile
-// from L2.
+// Kernel anatomy (one persistent CTA per SM, 384 threads, 128 x 128 output tiles):
+//   warps 8-11  producer warpgroup (its registers go to the consumers, setmaxnreg); one lane
+//               issues cp.async.bulk.tensor.2d of a 128x64 Q tile and a 128x64 X tile (bf16,
+//               K-major, SWIZZLE_128B) into a 6-stage shared-memory ring, mbarrier complete_tx
+//               signalling;
+//   warps 0-7   two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: each issues
+//               wgmma.mma_async m64n128k16 x4 per stage into a 64-register f32 accumulator,
+//               keeps one stage's MMAs in flight while it waits for the next, releases a stage
+//               once its MMAs have retired, then runs the epilogue (|x|^2 - 2*acc) straight
+//               from the registers while the producer already fills the ring for the next tile.
+// Tiles are walked N-tile-major so the query tiles of a batch reuse an X tile from L2.
 #include "kernels.cuh"
 
 #include <cuda.h>
@@ -32,9 +31,9 @@ namespace lgpu {
 
 namespace {
 
-constexpr int GM = 128, GN = 256, GK = 64, GSTAGES = 4, G_THREADS = 192;
+constexpr int GM = 128, GN = 128, GK = 64, GSTAGES = 6, G_CONSUMERS = 256, G_THREADS = G_CONSUMERS + 128;
 constexpr uint32_t A_STAGE_BYTES = GM * GK * 2;     // 16 KB
-constexpr uint32_t B_STAGE_BYTES = GN * GK * 2;     // 32 KB
+constexpr uint32_t B_STAGE_BYTES = GN * GK * 2;     // 16 KB
 constexpr uint32_t G_SMEM_TILES = GSTAGES * (A_STAGE_BYTES + B_STAGE_BYTES);   // 192 KB
 constexpr uint32_t G_SMEM_BYTES = G_SMEM_TILES + 256 + 1024;                   // + barriers + alignment slack
 
@@ -70,51 +69,56 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "elect.sync _|P1, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, P1;\n\t"
-        "}\n" : "=r"(pred));
-    return pred != 0;
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-// start>>4 | LBO(=1, unused for swizzled K-major)<<16 | SBO(=1024 B between 8-row groups)>>4 <<32 |
-// version 1 <<46 | layout SWIZZLE_128B(2) <<61
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (wgmma): start>>4 | LBO(=1, unused for swizzled K-major)<<16 |
+// SBO(=1024 B between 8-row groups)>>4 <<32 | layout SWIZZLE_128B(1) <<62
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr)
 {
     uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// cute::UMMA::InstrDescriptor: c_format F32 (1<<4), a/b format BF16 (1<<7, 1<<10), K-major A and B,
-// N>>3 at bit 17, M>>4 at bit 24
-constexpr uint32_t G_IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(GN >> 3) << 17) | ((uint32_t)(GM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both bf16 K-major in shared memory; `accumulate` = 0 overwrites D.
+// Fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[4 j + 2 h + e] is row 16 w + l / 4 + 8 h,
+// column 8 j + 2 (l % 4) + e.
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// keeps the compiler from moving accumulator reads above the wgmma.wait_group that makes them valid
+__device__ __forceinline__ void fence_acc(float (&d)[64])
+{
+#pragma unroll
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 // LIST: the filtering epilogue for DENSE hit rates (coarse step at many lists), see the epilogue; a separate
-// instantiation so that the dense / sparse-filter kernel of the flat path and of the small coarse problems is
-// unchanged (staging |x|^2 through shared memory and the per-tile barrier cost the flat C4 launch 15 %).
+// instantiation so that the dense / sparse-filter kernel of the flat path and of the small coarse problems carries
+// none of its code.
 template <bool LIST>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
@@ -123,38 +127,27 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     extern __shared__ unsigned char smem_raw[];
-    __shared__ __align__(16) float s_xn[LIST ? 2 : 1][LIST ? GN : 4];  // LIST: |x|^2 of the current tile's columns, per accumulator
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;         // SWIZZLE_128B needs 1024 B alignment
     const uint32_t smem_a = base, smem_b = base + GSTAGES * A_STAGE_BYTES;
     const uint32_t bars = base + G_SMEM_TILES;
     const uint32_t full_bar = bars, empty_bar = bars + 8 * GSTAGES;
-    const uint32_t tfull_bar = bars + 16 * GSTAGES, tempty_bar = tfull_bar + 16;
-    const uint32_t tmem_slot = tempty_bar + 16;
-    unsigned char *smem_gen = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t *tmem_slot_ptr = reinterpret_cast<volatile uint32_t *>(smem_gen + G_SMEM_TILES + 16 * GSTAGES + 32);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t num_m = (B + GM - 1) / GM;
     const uint64_t num_n = (N + GN - 1) / GN;
     const uint64_t num_tiles = num_m * num_n;
 
-    if (warp == 0 && lane == 0) {
-        for (int i = 0; i < GSTAGES; i++) { mbar_init(full_bar + 8 * i, 1); mbar_init(empty_bar + 8 * i, 1); }
-        for (int i = 0; i < 2; i++) { mbar_init(tfull_bar + 8 * i, 1); mbar_init(tempty_bar + 8 * i, 128); }
+    if (warp == G_CONSUMERS / 32 && lane == 0) {
+        // full: the producer's expect_tx arrival; empty: one arrival per consumer warpgroup
+        for (int i = 0; i < GSTAGES; i++) { mbar_init(full_bar + 8 * i, 1); mbar_init(empty_bar + 8 * i, 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp == 0) {
+    if (warp >= G_CONSUMERS / 32) {
         // ===== TMA producer =====
-        if (elect_one()) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == G_CONSUMERS / 32 && lane == 0) {
             uint32_t stage = 0, phase = 0;
             for (uint64_t t = blockIdx.x; t < num_tiles; t += gridDim.x) {
                 const uint32_t m_tile = (uint32_t)(t % num_m);
@@ -168,197 +161,139 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        uint32_t stage = 0, phase = 0, it = 0;
-        for (uint64_t t = blockIdx.x; t < num_tiles; t += gridDim.x, it++) {
-            const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-            mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);              // epilogue drained this accumulator
-            tc_fence_after();
-            for (uint32_t kb = 0; kb < num_kb; kb++) {
-                mbar_wait(full_bar + 8 * stage, phase);                  // TMA bytes landed
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint64_t da = make_kmajor_sw128_desc(smem_a + stage * A_STAGE_BYTES);
-                    const uint64_t db = make_kmajor_sw128_desc(smem_b + stage * B_STAGE_BYTES);
+        return;
+    }
+
+    // ===== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of each tile =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const uint32_t wg = threadIdx.x >> 7;
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint32_t stage = 0, phase = 0;
+    float acc[64];
 #pragma unroll
-                    for (int k = 0; k < GK / 16; k++)                    // +32 B (>>4 = 2) per K=16 slice
-                        tc_mma_bf16(tmem_base + acc * GN, da + 2 * k, db + 2 * k, G_IDESC, (kb | k) != 0 ? 1u : 0u);
-                    tc_commit(empty_bar + 8 * stage);                    // frees the smem stage when the MMAs retire
-                    if (kb + 1 == num_kb) tc_commit(tfull_bar + 8 * acc);   // accumulator complete
-                }
-                __syncwarp();
-                if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
+    for (int i = 0; i < 64; i++) acc[i] = 0.f;
+    for (uint64_t t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const uint32_t m_tile = (uint32_t)(t % num_m);
+        const uint64_t n_tile = t / num_m;
+        // this thread's rows r0, r0 + 8 and columns c0 + 8 j + {0, 1}
+        const uint32_t r0 = m_tile * GM + wg * 64 + (uint32_t)(warp & 3) * 16 + (uint32_t)(lane >> 2);
+        const uint64_t c0 = n_tile * GN + 2 * (uint32_t)(lane & 3);
+        // |x|^2 of the thread's 32 columns, requested before the MMAs so that the loads land under them; past N: 0
+        float xn[32];
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const uint64_t x = c0 + 8 * j;
+            if (x + 1 < N) {
+                const float2 v = __ldg(reinterpret_cast<const float2 *>(xnorm2 + x));
+                xn[2 * j] = v.x; xn[2 * j + 1] = v.y;
+            } else {
+                xn[2 * j] = x < N ? __ldg(xnorm2 + x) : 0.f;
+                xn[2 * j + 1] = 0.f;
             }
         }
-    } else {
-        // ===== epilogue (warps 2..5 -> TMEM lane quadrants 2,3,0,1) =====
-        const int quad = warp & 3;
-        uint32_t it = 0;
-        for (uint64_t t = blockIdx.x; t < num_tiles; t += gridDim.x, it++) {
-            const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-            const uint32_t m_tile = (uint32_t)(t % num_m);
-            const uint64_t n_tile = t / num_m;
-            const uint64_t x0 = n_tile * GN;
-            if constexpr (LIST) {
-                // |x|^2 of the tile's 256 columns -> shared memory while the MMAs of the tile still run (read from global
-                // memory chunk by chunk, each chunk exposed an L2 round trip behind its TMEM load).  Columns past N read
-                // as 0 and are masked where it matters.  The barrier also keeps a warp from overwriting the buffer of tile
-                // i + 2 while another still reads tile i's.
-                const int et = (int)threadIdx.x - 64;                    // 0..127 among the epilogue threads
-                s_xn[acc][et] = x0 + et < N ? __ldg(xnorm2 + x0 + et) : 0.f;
-                s_xn[acc][et + 128] = x0 + et + 128 < N ? __ldg(xnorm2 + x0 + et + 128) : 0.f;
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-            }
-            mbar_wait(tfull_bar + 8 * acc, acc_phase);
-            tc_fence_after();
-            const uint32_t q = m_tile * GM + quad * 32 + lane;
-            float *orow = out + (size_t)q * ld_out;
-#define LGPU_TMEM_LD32(r, taddr)                                                                                        \
-    asm volatile(                                                                                                       \
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                       \
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                       \
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),               \
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),         \
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),       \
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])        \
-        : "r"(taddr));                                                                                                  \
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory")
-            [[maybe_unused]] const float *xn_s = s_xn[LIST ? acc : 0];
-            if constexpr (LIST) {
-                // Filtering epilogue for DENSE hit rates (the coarse step's lists: ~1.5 % of the columns pass, so nearly
-                // every 32-column chunk holds one).  One returning atomic per hit, as in the sparse form below, made this
-                // launch 3.5x slower than writing the dense matrix.  Two passes over the accumulator, which stays in
-                // TMEM until it is released: (1) hit masks of the tile's 8 chunks + their count, ONE atomicAdd per
-                // (query, tile) reserves the slots; (2) the chunks that hold hits are loaded again and their (column,
-                // score) pairs stored.  tcgen05.ld is warp-collective, so pass 2 re-loads a chunk when ANY lane has a hit.
+        uint32_t prev = 0;
+        for (uint32_t kb = 0; kb < num_kb; kb++) {
+            mbar_wait(full_bar + 8 * stage, phase);                      // TMA bytes landed
+            const uint64_t da = make_kmajor_sw128_desc(smem_a + stage * A_STAGE_BYTES + wg * (64 * GK * 2));
+            const uint64_t db = make_kmajor_sw128_desc(smem_b + stage * B_STAGE_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < GK / 16; k++)                            // +32 B (>>4 = 2) per K=16 slice
+                wgmma_m64n128k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();                                             // the previous stage's MMAs have retired
+            if (kb > 0 && leader) mbar_arrive(empty_bar + 8 * prev);
+            prev = stage;
+            if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_acc(acc);
+        if (leader) mbar_arrive(empty_bar + 8 * prev);
+
+        if constexpr (LIST) {
+            // Filtering epilogue for DENSE hit rates (the coarse step's lists: ~1.5 % of the columns pass).  One returning
+            // atomic per hit, as in the sparse form below, would serialise on the query's counter; instead the 4 lanes
+            // that share a row count their hits, ONE atomicAdd per (row, warpgroup tile) reserves the slots, and each
+            // lane stores its (column, score) pairs at its prefix inside the reservation.
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const uint32_t q = r0 + 8 * h;
                 const bool live = q < B;
                 const float thr = live ? flt.thr[q] : 0.f;
-                uint32_t tot = 0, slot = 0;
-                // ROLLED loops, one chunk body run 2 x 8 times: fully unrolled (masks kept in registers between the
-                // passes) the kernel grew to 17 k instructions and stalled on instruction fetch (ncu: no_inst) -- 3x
-                // slower than writing the dense matrix.  Pass 1 recomputes nothing it can keep: only the count.
-#pragma unroll 1
-                for (int pass = 0; pass < 2; pass++) {
-                    if (pass == 1) {
-                        if (!__any_sync(0xffffffffu, tot != 0u)) break;
-                        if (tot) slot = atomicAdd(flt.count + q, tot);
-                    }
-#pragma unroll 1
-                    for (int c = 0; c < GN / 32; c++) {
-                        uint32_t r[32];
-                        const uint32_t taddr = tmem_base + acc * GN + c * 32 + ((uint32_t)(quad * 32) << 16);
-                        LGPU_TMEM_LD32(r, taddr);
-                        const uint64_t xb = x0 + (uint64_t)c * 32;
-                        unsigned hit = 0;
-                        if (live && xb + 32 <= N) {
+                uint32_t hit = 0;                                        // bit 2 j + e: column c0 + 8 j + e passes
 #pragma unroll
-                            for (int j = 0; j < 32; j += 4) {
-                                const float4 xn = *reinterpret_cast<const float4 *>(xn_s + c * 32 + j);
-                                hit |= (xn.x - 2.0f * __uint_as_float(r[j]) <= thr ? 1u : 0u) << j;
-                                hit |= (xn.y - 2.0f * __uint_as_float(r[j + 1]) <= thr ? 1u : 0u) << (j + 1);
-                                hit |= (xn.z - 2.0f * __uint_as_float(r[j + 2]) <= thr ? 1u : 0u) << (j + 2);
-                                hit |= (xn.w - 2.0f * __uint_as_float(r[j + 3]) <= thr ? 1u : 0u) << (j + 3);
-                            }
-                        } else if (live) {
+                for (int j = 0; j < 16; j++)
 #pragma unroll
-                            for (int j = 0; j < 32; j++)
-                                if (xb + j < N && xn_s[c * 32 + j] - 2.0f * __uint_as_float(r[j]) <= thr) hit |= 1u << j;
-                        }
-                        if (pass == 0) {
-                            tot += __popc(hit);
-                        } else if (hit) {
+                    for (int e = 0; e < 2; e++)
+                        if (live && c0 + 8 * j + e < N && xn[2 * j + e] - 2.0f * acc[4 * j + 2 * h + e] <= thr)
+                            hit |= 1u << (2 * j + e);
+                const uint32_t n = __popc(hit);
+                uint32_t incl = n, v;                                    // inclusive prefix over the row's 4 lanes
+                v = __shfl_up_sync(0xffffffffu, incl, 1, 4); if (lane & 3) incl += v;
+                v = __shfl_up_sync(0xffffffffu, incl, 2, 4); if ((lane & 3) >= 2) incl += v;
+                const uint32_t tot = __shfl_sync(0xffffffffu, incl, 3, 4);
+                uint32_t slot = 0;
+                if ((lane & 3) == 0 && tot) slot = atomicAdd(flt.count + q, tot);
+                slot = __shfl_sync(0xffffffffu, slot, 0, 4) + incl - n;
+                if (hit) {
 #pragma unroll
-                            for (int j = 0; j < 32; j++) {
-                                if ((hit >> j) & 1u) {
-                                    if (slot < flt.cap) {
-                                        flt.cand_pos[(size_t)q * flt.cap + slot] = xb + j;
-                                        flt.cand_s[(size_t)q * flt.cap + slot] = xn_s[c * 32 + j] - 2.0f * __uint_as_float(r[j]);
-                                    }
-                                    slot++;
+                    for (int j = 0; j < 16; j++)
+#pragma unroll
+                        for (int e = 0; e < 2; e++)
+                            if ((hit >> (2 * j + e)) & 1u) {
+                                if (slot < flt.cap) {
+                                    flt.cand_pos[(size_t)q * flt.cap + slot] = c0 + 8 * j + e;
+                                    flt.cand_s[(size_t)q * flt.cap + slot] = xn[2 * j + e] - 2.0f * acc[4 * j + 2 * h + e];
                                 }
+                                slot++;
+                            }
+                }
+            }
+            continue;
+        }
+        if (flt.thr) {
+            // filtering epilogue: nothing dense is written; scores not above the per-query threshold are appended to the
+            // query's candidate list (rare: ~1e-4 of the columns)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const uint32_t q = r0 + 8 * h;
+                if (q >= B) continue;
+                const float thr = flt.thr[q];
+#pragma unroll
+                for (int j = 0; j < 16; j++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const uint64_t x = c0 + 8 * j + e;
+                        if (x < N && xn[2 * j + e] - 2.0f * acc[4 * j + 2 * h + e] <= thr) {
+                            const uint32_t slot = atomicAdd(flt.count + q, 1u);
+                            if (slot < flt.cap) {
+                                flt.cand_pos[(size_t)q * flt.cap + slot] = x;
+                                if (flt.cand_ids) flt.cand_ids[(size_t)q * flt.cap + slot] = flt.col_ids ? flt.col_ids[x] : x;
                             }
                         }
                     }
-                }
-                tc_fence_before();
-                mbar_arrive(tempty_bar + 8 * acc);
-                continue;
             }
-#pragma unroll 1
-            for (int c0 = 0; c0 < GN; c0 += 32) {
-                uint32_t r[32];
-                const uint32_t taddr = tmem_base + acc * GN + c0 + ((uint32_t)(quad * 32) << 16);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                      "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                      "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                      "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                    : "r"(taddr));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (q < B && flt.thr) {
-                    // filtering epilogue: nothing dense is written; scores not above the per-query threshold
-                    // are appended to the query's candidate list (rare: ~1e-4 of the columns)
-                    const uint64_t xb = x0 + c0;
-                    const float thr = flt.thr[q];
-                    auto admit = [&](uint64_t x) {
-                        const uint32_t slot = atomicAdd(flt.count + q, 1u);
-                        if (slot < flt.cap) {
-                            flt.cand_pos[(size_t)q * flt.cap + slot] = x;
-                            if (flt.cand_ids) flt.cand_ids[(size_t)q * flt.cap + slot] = flt.col_ids ? flt.col_ids[x] : x;
-                        }
-                    };
-                    if (xb + 32 <= N) {
-                        unsigned hit = 0;                                  // bit j: column xb+j passes
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 xn = __ldg(reinterpret_cast<const float4 *>(xnorm2 + xb + j));
-                            hit |= (xn.x - 2.0f * __uint_as_float(r[j]) <= thr ? 1u : 0u) << j;
-                            hit |= (xn.y - 2.0f * __uint_as_float(r[j + 1]) <= thr ? 1u : 0u) << (j + 1);
-                            hit |= (xn.z - 2.0f * __uint_as_float(r[j + 2]) <= thr ? 1u : 0u) << (j + 2);
-                            hit |= (xn.w - 2.0f * __uint_as_float(r[j + 3]) <= thr ? 1u : 0u) << (j + 3);
-                        }
-                        while (hit) { const int j = __ffs(hit) - 1; hit &= hit - 1; admit(xb + j); }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) {
-                            const uint64_t x = xb + j;
-                            if (x < N && __ldg(xnorm2 + x) - 2.0f * __uint_as_float(r[j]) <= thr) admit(x);
-                        }
-                    }
-                } else if (q < B) {
-                    const uint64_t xb = x0 + c0;
-                    if (xb + 32 <= N && ((ld_out & 3) == 0)) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 xn = __ldg(reinterpret_cast<const float4 *>(xnorm2 + xb + j));
-                            float4 o;
-                            o.x = xn.x - 2.0f * __uint_as_float(r[j]);
-                            o.y = xn.y - 2.0f * __uint_as_float(r[j + 1]);
-                            o.z = xn.z - 2.0f * __uint_as_float(r[j + 2]);
-                            o.w = xn.w - 2.0f * __uint_as_float(r[j + 3]);
-                            *reinterpret_cast<float4 *>(orow + xb + j) = o;
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; j++)
-                            if (xb + j < N) orow[xb + j] = __ldg(xnorm2 + xb + j) - 2.0f * __uint_as_float(r[j]);
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(tempty_bar + 8 * acc);                           // 128 arrivals free the accumulator
+            continue;
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
+        // dense scores: the 4 lanes of a row write 32 contiguous bytes per column group
+        const bool vec = (ld_out & 1) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0;
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const uint32_t q = r0 + 8 * h;
+            if (q >= B) continue;
+            float *orow = out + (size_t)q * ld_out;
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const uint64_t x = c0 + 8 * j;
+                const float s0 = xn[2 * j] - 2.0f * acc[4 * j + 2 * h], s1 = xn[2 * j + 1] - 2.0f * acc[4 * j + 2 * h + 1];
+                if (vec && x + 1 < N) {
+                    *reinterpret_cast<float2 *>(orow + x) = make_float2(s0, s1);
+                } else {
+                    if (x < N) orow[x] = s0;
+                    if (x + 1 < N) orow[x + 1] = s1;
+                }
+            }
+        }
     }
 }
 
@@ -457,8 +392,8 @@ __global__ void sample_threshold_kernel(const float *__restrict__ approx, const 
     thr[q] = t;
 }
 // The same threshold straight from the dense sample scores D[B][ld] (ns columns), one warp per query: the k-th smallest
-// by counting bisection over the lane's register copy of the row (no ids, no sorted output -- a top-k select over
-// 8192 x 2048 scores took 0.21 ms), stopped when the bracket is a quarter of the band it feeds; any hi with
+// by counting bisection over the lane's register copy of the row (no ids, no sorted output, unlike a top-k select),
+// stopped when the bracket is a quarter of the band it feeds; any hi with
 // count(S <= hi) >= k is a valid bound.  NaN scores never count.  ns <= 32 * VPL.
 template <int VPL>
 __global__ void __launch_bounds__(128) sample_kth_threshold_kernel(const float *__restrict__ D, uint64_t ld, uint32_t ns,
@@ -607,7 +542,7 @@ void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint3
     const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)num_sms);
     GemmFilter flt{};
     if (filter) flt = *filter;
-    const bool list = flt.thr && flt.cand_s;                  // dense hit rates: two-pass list epilogue
+    const bool list = flt.thr && flt.cand_s;                  // dense hit rates: one reservation per row and tile
     auto kern = list ? gemm_dist_kernel<true> : gemm_dist_kernel<false>;
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, xnorm2, out, ld_out, B, N, (uint32_t)((d + GK - 1) / GK), flt); LGPU_COUNT_LAUNCH();

@@ -31,7 +31,7 @@ __global__ void group_count_kernel(GroupArgs a, int first)
         return;
     }
     // a warp per query, a lane per probe (32 at a time): the loads and atomics of a query's probes are in flight
-    // together (one thread per query walked them one after the other: 20 dependent round trips, 14 us at C2), and the
+    // together (one thread per query walked them one after the other: 20 dependent round trips), and the
     // segment offsets come from a warp scan
     const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -71,7 +71,7 @@ __global__ void group_count_kernel(GroupArgs a, int first)
 
 // single CTA: exclusive scans over queries (segment bases) and partitions (query-list and tile offsets).  Every thread
 // sums a contiguous run of elements, one 1024-wide block scan combines the runs, the thread then writes its run back:
-// one block scan per array whatever B / nlist are (the chunked form took 72 us at nlist = 16384).
+// one block scan per array whatever B / nlist are (a chunked form needs one per chunk).
 template <class Get, class Put>
 __device__ __forceinline__ uint64_t block_exclusive_scan(uint32_t n, uint64_t *s_part, int tid, Get &&get, Put &&put)
 {
@@ -79,7 +79,7 @@ __device__ __forceinline__ uint64_t block_exclusive_scan(uint32_t n, uint64_t *s
     const uint32_t b = min(n, (uint32_t)tid * per), e = min(n, b + per);
     uint64_t sum = 0;
     // runs of up to 16 elements are read into registers first, all loads in flight (a rolled `sum += get(i)` waited for
-    // one L2 round trip per element, twice per array: 67 us at nlist 16384), and written back from the registers
+    // one L2 round trip per element, twice per array), and written back from the registers
     constexpr int RUN = 16;
     uint64_t v[RUN];
     const bool in_regs = per > 4 && per <= RUN;              // short runs: the rolled loop is cheaper than 16 predicated slots

@@ -214,7 +214,7 @@ void launch_pack_records(const uint64_t *ids, const float *dist, uint64_t n, Top
 bool gemm_shape_supported(uint32_t d);
 // X f32 [n][d] -> bf16 [n][d]; norm2[n] = |x|^2 (f32) if norm2 != nullptr
 void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *norm2, cudaStream_t st);
-// out[q][x] = xnorm2[x] - 2 * bf16(Q[q]) . bf16(X[x])   (tcgen05 + TMA), q < B, x < N
+// out[q][x] = xnorm2[x] - 2 * bf16(Q[q]) . bf16(X[x])   (wgmma + TMA), q < B, x < N
 // optional filtering epilogue: instead of writing the dense score matrix, append the columns whose score
 // is <= thr[q] to the query's candidate list (count may exceed cap: those appends are dropped)
 struct GemmFilter {

@@ -5,7 +5,7 @@
 // path and the oracle consume whatever arrays come out -- so these kernels follow plain Lloyd (random-sample init by the
 // caller, empty clusters keep their previous centre; lance's hierarchical variant above 256 lists
 // [python/python/tests/test_index.py:378] is not reproduced) and only have to be good k-means.
-//   assignment (IVF)  : the search's own coarse step (api.cu): tcgen05 GEMM scores + coarse_finish_kernel with k = 1, i.e.
+//   assignment (IVF)  : the search's own coarse step (api.cu): tensor-core GEMM scores + coarse_finish_kernel with k = 1, i.e.
 //                       the exact nearest centre in lance's arithmetic -- a training row is assigned where a query equal
 //                       to it would probe first;
 //   update (IVF)      : rows bucketed by centre (counting sort), one CTA per centre sums its rows in f64, each bucket

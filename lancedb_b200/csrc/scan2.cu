@@ -7,11 +7,11 @@
 //     d_j = sum_i LUT[i][code[i][j]]  sequentially in i      (compute_pq_distance)
 // Results are bit-identical to oracle.c: every f32 op is an explicit round-to-nearest op in the reference's
 // order (the LUT entry uses the f32x8 reduce tree, the row sum is sequential over sub-vectors).
-// Since round 2 the default search runs the filter kernel (scan3.cu) first and only the queries it cannot prove
+// The default search runs the filter kernel (scan3.cu) first and only the queries it cannot prove
 // come here (plus distance-range queries, debug entry points and LGPU_EXACT_SCAN=1); this kernel is also the
 // arithmetic pq_rescore_kernel (tables.cu) restates per candidate row.
 //
-// Work decomposition (B200-first, not the reference's per-query loop):
+// Work decomposition (GPU-first, not the reference's per-query loop):
 //   tile = (partition p, up to 8 of the queries that probe p, up to 1536 of its rows).  A persistent grid (one
 //   512-thread CTA per SM) pulls tiles from an atomic counter; tiles are ordered by partition so a partition's
 //   codes are read from HBM once and then hit in L2 for the other query groups.
@@ -19,7 +19,7 @@
 //   64 KB shared-memory buffers laid out [h][c][s][4 queries] (h = query half, c = code, s = sub-space within the
 //   chunk), so one LDS.128 returns the entries of 4 queries.  The codebook chunk is read (L2-resident) once per
 //   tile and amortised over the 8 queries.
-//   Warp specialisation: the table build is FP32-pipe work (23 flops per entry, packed FADD2/FFMA2), the scan is
+//   Warp specialisation: the table build is FP32-pipe work (23 flops per entry), the scan is
 //   shared-memory-gather work; 8 builder warps build chunk ch+1/ch+2 while 8 scanner warps scan chunk ch, handing
 //   buffers over with named barriers (bar.arrive / bar.sync).
 //   Bank conflicts: a straightforward "lane = row" scan makes 8 lanes of a quarter-warp gather at random codes =>
@@ -27,7 +27,7 @@
 //   pre-skewed by row % 8 bytes, see retile.cu), so at any instant the 8 lanes of a quarter-warp read 8
 //   *different* sub-spaces = 8 different 16-byte bank groups: conflict-free by construction, while each row still
 //   accumulates its sub-vectors strictly in order 0..m-1 in its own register.
-// Pipeline details (from the ncu stall profile of round 1, profiles/r01_scan_stalls.txt):
+// Pipeline details:
 //   * no per-tile drain: the stage counter runs on across tiles -- the all-zero "stage nch" of tile n doubles as
 //     the "stage -1" of tile n+1 -- and tile descriptors (group.cu::tile_desc_kernel) are claimed two tiles ahead
 //     by builder warp 0 into a 4-slot shared ring, so neither role ever waits for a fetch.
@@ -49,9 +49,8 @@ constexpr int S2_PW = 8, S2_CW = 8;                 // builder / scanner warps
 constexpr int S2_PT = S2_PW * 32, S2_NT = (S2_PW + S2_CW) * 32;
 constexpr int S2_CT = 128;                          // scanner threads per query half
 constexpr int S2_RMAX = 12;                         // rows per scanner thread: 128 * 12 = SCAN_ROWS_TILE_MID
-// registers per builder / scanner thread.  Measured on B200 (C2, scan stage ms per batch): 104/152 0.867,
-// 112/144 0.830, 120/136 0.823, 128/128 0.810, 136/120 0.820, 144/112 0.870 -- the builders schedule better
-// with more registers until the scanners start to spill.
+// registers per builder / scanner thread: the builders schedule better with more registers until the scanners
+// start to spill; an even split is the default (override with -DS2_PREG_V / -DS2_CREG_V).
 #ifndef S2_PREG_V
 #define S2_PREG_V 128
 #endif
@@ -133,7 +132,7 @@ struct Resid {
 
 // ---- codebook staging (DSUB == 8).  A builder warp's task needs CPT codes x 8 sub-spaces x 32 B of the
 // codebook chunk = CPT * 256 contiguous bytes.  Instead of loading them into registers a few tasks ahead
-// (round 1: the L2 round trip was the builders' largest stall), each warp streams them with cp.async
+// (each load exposes an L2 round trip), each warp streams them with cp.async
 // (LDGSTS, 16 B per lane) into a private ring of D = 3072 / (CPT * 256) slots, D tasks ahead, and reads
 // its (code, sub-space) entry back with two LDS.128 one task ahead.  16-byte unit u of a code's 256 B
 // is stored at unit u ^ ((u >> 3) & 1) so that the eight lanes of a quarter-warp (sub-spaces 0..7, 32 B

@@ -2,8 +2,8 @@
 //
 // The exact kernel (scan2.cu) has to build one f32 distance table per (query, probed partition), because
 // lance's table is on the residual q - c_p [lance, recalled; SURVEY.md 8a rows a4-a5]: 20 480 tables per
-// 1024-query batch of BASELINE config 2, and ncu showed that build -- its shared-memory staging and its f32
-// arithmetic -- not the scan, bounding the kernel (profiles/r01_ncu_summary.txt: shared pipe 76 %, FMA pipe 56 %).
+// 1024-query batch of BASELINE config 2, and that build -- its shared-memory staging and its f32 arithmetic --
+// not the scan, bounds the exact kernel.
 // Algebraically (tables.cu has the derivation)
 //     d(q, row r of partition p) = sum_i T_q[i][code_i(r)]  +  A(q,p)  +  R(r)
 // with ONE table per query, T_q[i][c] = |q_i - codebook_i[c]|^2 (1 - q_i.codebook_i[c] for dot), a scalar per

@@ -1,5 +1,5 @@
 // scan_common.cuh -- device helpers shared by the scan kernels (scan.cu, scan2.cu): named-barrier
-// wrappers and the packed f32x2 arithmetic of the distance-table build.
+// wrappers and the paired f32 arithmetic of the distance-table build.
 #pragma once
 
 #include "kernels.cuh"
@@ -36,11 +36,10 @@ __device__ __forceinline__ void load_vec(float *dst, const float *src)
     }
 }
 
-// ---- packed f32x2 arithmetic (FADD2 / FFMA2 on sm_100a): two IEEE round-to-nearest
-// f32 ops per instruction, bit-identical to the scalar ops.  ptxas contracts
-// mul.rn.f32x2 + add.rn.f32x2 into FFMA2 (even with -fmad=false), which would change
-// the rounding, so the square is written as fma(d, d, zero) with `zero` an opaque
-// kernel argument: round(d*d + 0) == round(d*d) and nothing is left to contract. ----
+// ---- f32 pairs (even, odd) held in one 64-bit register pair.  sm_90 has no packed f32x2 arithmetic, so every
+// op is two scalar IEEE round-to-nearest ops on the halves (the __f*_rn intrinsics are never contracted).  The
+// square is fma(d, d, zero) with `zero` an opaque kernel argument: round(d*d + 0) == round(d*d), and nothing is
+// left for the compiler to fold. ----
 __device__ __forceinline__ uint64_t pk2(float a, float b)
 {
     uint64_t r;
@@ -53,21 +52,21 @@ __device__ __forceinline__ void upk2(uint64_t v, float &a, float &b)
 }
 __device__ __forceinline__ uint64_t sub2(uint64_t a, uint64_t b)
 {
-    uint64_t r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    upk2(a, a0, a1); upk2(b, b0, b1);
+    return pk2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b)
 {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    upk2(a, a0, a1); upk2(b, b0, b1);
+    return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t sq2(uint64_t d, uint64_t zero)
 {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %1, %2;" : "=l"(r) : "l"(d), "l"(zero));
-    return r;
+    float d0, d1, z0, z1;
+    upk2(d, d0, d1); upk2(zero, z0, z1);
+    return pk2(__fmaf_rn(d0, d0, z0), __fmaf_rn(d1, d1, z1));
 }
 // l2_once::<f32x8>: ((s0+s4)+(s2+s6)) + ((s1+s5)+(s3+s7)), s_k = (r_k-c_k)^2
 __device__ __forceinline__ float l2_tree8_packed(const uint64_t r[4], const uint64_t c[4], uint64_t zero)

@@ -2,7 +2,7 @@
 //
 // Replaces the per-partition bounded heap + SortExec TopK(fetch=k) merge
 // [lance, recalled; SURVEY.md 8a rows a8-a9; tie-break pinned by
-// /root/reference/python/python/lancedb/query.py:1366-1368].  Also used to pick the
+// python/python/lancedb/query.py:1366-1368].  Also used to pick the
 // nprobes nearest centroids (IvfModel::find_partitions' sort_to_indices) and for the
 // flat / refine / multi-GPU merge paths.
 //
@@ -464,8 +464,8 @@ void launch_select(const SelectArgs &a, cudaStream_t st)
 {
     if (a.B == 0) return;
     LGPU_REQUIRE(a.k >= 1 && a.k <= SELECT_KMAX, "limit+offset (k) must be in [1, 2048] on the GPU path");
-    // measured on B200: with 2 / 4 entries per lane the insert path dominates (k ln(n/k) serial inserts per
-    // warp), the shared-memory stage + bitonic kernel is faster above k = 32 (C3 top-100: 1.85 vs 3.06 ms)
+    // with 2 / 4 entries per lane the insert path dominates (k ln(n/k) serial inserts per warp): above k = 32 the
+    // shared-memory stage + bitonic kernel is the faster one
     if (a.k <= 32) {
         const unsigned grid = a.B;
         const int nq = a.k <= 32 ? 1 : (a.k <= 64 ? 2 : 4);

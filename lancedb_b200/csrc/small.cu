@@ -1,6 +1,6 @@
 // small.cu -- the low-latency form of K2+K3 for tiny batches (B * nprobes <= ~1000 probe slots: a single query, or
 // the handful a micro-batch collects).  The batched kernels (group.cu -> scan3.cu / scan2.cu -> finalize) amortise
-// their ~25 launches over a thousand queries; one query pays them all (~200 us measured through lgpu_search, B = 1).
+// their ~25 launches over a thousand queries; one query pays them all.
 // Here every (query, probed partition) pair is one CTA, which is the reference's own decomposition
 // [lance, recalled: ANNIvfSubIndexExec runs per partition; SURVEY.md 8a rows a4-a7]:
 //     r   = q - centroid[p]                      (L2 / cosine; the query itself for dot)

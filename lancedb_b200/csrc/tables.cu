@@ -27,15 +27,9 @@ namespace {
 
 // ---- table entries for the FILTER.  Not lance's arithmetic (that is pq_rescore_kernel's job): the expansion
 //     |q_i - b|^2 = |q_i|^2 + |b|^2 - 2 q_i.b      (1 - q_i.b for dot)
-// with |b|^2 precomputed at open and the dot product as packed FFMA2 over (even, odd) dimension pairs: ~10
-// instructions per entry instead of ~25.  Its rounding error, <= ~12 u (|q_i| + |b|)^2 per entry, is part of the band
-// (band_check3: the 2 (|q|^2 + CB2) term).  Both table passes call this one function, so they see identical values.
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c)
-{
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
+// with |b|^2 precomputed at open and the dot product accumulated in two chains over (even, odd) dimension pairs.  Its
+// rounding error, <= ~12 u (|q_i| + |b|)^2 per entry, is part of the band (band_check3: the 2 (|q|^2 + CB2) term).
+// Both table passes call this one function, so they see identical values.
 __device__ __forceinline__ uint64_t pack2(float a, float b)
 {
     uint64_t r;
@@ -47,6 +41,15 @@ __device__ __forceinline__ float sum2(uint64_t v)
     float a, b;
     asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
     return a + b;
+}
+// (even, odd) lanes: a * b + c, each one fused multiply-add
+__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c)
+{
+    float a0, a1, b0, b1, c0, c1;
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(a));
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(b0), "=f"(b1) : "l"(b));
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(c0), "=f"(c1) : "l"(c));
+    return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 template <int DSUB>
 struct SubVec {

@@ -3,7 +3,7 @@ plain arrays of ``lgpu_index_desc`` (SURVEY.md 8f-3).
 
 STATUS: **[lance, recalled] -- UNVERIFIED against a real file.**  The reference tree holds no Lance index file and no
 Lance writer (the file format lives in the un-vendored lance crates, v11.0.0-beta.19; the only thing
-/root/reference pins is that the directory ``_indices/<uuid>/`` exists: nodejs/__test__/table.test.ts:907, 1318).
+the reference pins is that the directory ``_indices/<uuid>/`` exists: nodejs/__test__/table.test.ts:907, 1318).
 The layout below is the Lance v2 file container + the v3 vector-index layout as published in lance's
 ``protos/file2.proto``, ``protos/encodings.proto`` and ``protos/index.proto``, restated from memory:
 

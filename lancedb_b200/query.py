@@ -1,9 +1,9 @@
 """Query builder mirroring the reference's vector-search surface.
 
 Same names, argument meaning, defaults and error behaviour as
-`lancedb.query.LanceVectorQueryBuilder` (/root/reference/python/python/lancedb/query.py:1552-1862)
+`lancedb.query.LanceVectorQueryBuilder` (python/python/lancedb/query.py:1552-1862)
 and the request it lowers to, `VectorQueryRequest`
-(/root/reference/rust/lancedb/src/query.rs:1066-1114): limit 10, nprobes 20 (min == max),
+(rust/lancedb/src/query.rs:1066-1114): limit 10, nprobes 20 (min == max),
 no refine, L2.  Everything below `to_arrow()` runs on the GPU through the C ABI; only the
 `Take` of the non-vector columns for the k result rows (SURVEY.md 8a row a12) happens in
 pyarrow on the host.  `where(...)` filters: the predicate is evaluated on the host (filter.py) and its

@@ -1,7 +1,7 @@
 """In-memory table + connection mirroring the part of the reference's surface that leads
 into the vector-query hot path: `connect() -> create_table() -> create_index() ->
-search()...to_arrow()` (/root/reference/python/python/lancedb/table.py:3571-3664,
-2883-2937; /root/reference/rust/lancedb/src/table.rs:549-613 `BaseTable`).
+search()...to_arrow()` (python/python/lancedb/table.py:3571-3664,
+2883-2937; rust/lancedb/src/table.rs:549-613 `BaseTable`).
 
 The storage engine, catalog, write path and versioning of LanceDB are out of scope
 (SURVEY.md 2b rows 9-18): a table here is a pyarrow Table held in host memory whose vector

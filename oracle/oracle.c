@@ -105,7 +105,7 @@ void orc_normalize_f32(const float *x, size_t d, float *out)
 /* lance-linalg L2::l2_batch for f32 dispatches on the dimension
  * [lance, recalled]: 8 -> l2_once::<f32x8,8>, 16 -> l2_once::<f32x16,16>,
  * otherwise l2().  l2_once = ((x-y)*(x-y)).reduce_sum(), and the AVX2
- * (target-cpu=haswell, /root/reference/.cargo/config.toml:44) f32x8
+ * (target-cpu=haswell, .cargo/config.toml:44) f32x8
  * reduce_sum is permute2f128+add, permute(14)+add, hadd:
  *   ((s0+s4)+(s2+s6)) + ((s1+s5)+(s3+s7)).
  * f32x16 on AVX2 is two f32x8 halves added lane-wise first.                 */

@@ -9,9 +9,9 @@
  * PARITY STATUS: "IVF_PQ parity unpinned".  The arithmetic of the reference
  * lives in the un-vendored lance crates (lance-format/lance tag
  * v11.0.0-beta.19, commit 3128c0024427cb5bf8c04d492893ae45e78b0511, pinned in
- * /root/reference/Cargo.toml:16-29 and Cargo.lock:4817-4819,5109-5111,
- * 5234-5236).  That source is not present and cannot be built here (no
- * cargo/rustc), so every function below restates the *published algorithm*
+ * Cargo.toml:16-29 and Cargo.lock:4817-4819,5109-5111,
+ * 5234-5236).  That source is not part of the reference tree, so every
+ * function below restates the *published algorithm*
  * as recalled ("[lance, recalled]") and is anchored on the reference's own
  * call sites (rust/lancedb/src/table/query.rs:219-327) and on the flat-path
  * numeric pins the reference's tests hold (see tests/test_oracle_pins.py):

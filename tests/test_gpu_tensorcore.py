@@ -1,4 +1,4 @@
-"""tcgen05 GEMM shortlist: numerics of the GEMM itself (tolerance: it is bf16), and bit-exact
+"""Tensor-core (wgmma) GEMM shortlist: numerics of the GEMM itself (tolerance: it is bf16), and bit-exact
 parity of the paths that use it as a candidate generator (flat L2, IVF coarse step) -- the
 exact re-score decides, so ids/distances must still equal the oracle's bit for bit."""
 import numpy as np
