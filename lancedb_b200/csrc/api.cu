@@ -107,7 +107,7 @@ struct Workspace {
     DevBuf dist_out, out_ids, out_dist, out_count;
     DevBuf t_ids, t_dist, t_pos, t_cnt, t_exact;
     DevBuf widen;                       // maximum_nprobes widening: queries that found fewer than k rows
-    DevBuf qb, qn2, flags;              // tensor-core shortlist: bf16 queries, |q|^2, unproven-query flags
+    DevBuf qb, qn2, qerr, flags;        // tensor-core shortlist: bf16 queries, |q|^2, |bf16(q) - q|, unproven-query flags
     // CUDA graph of one host-buffer search (lgpu_search): the ~15 launches of a batch replayed as one
     cudaGraphExec_t graph = nullptr;
     uint64_t graph_key[4] = {0, 0, 0, 0};
@@ -249,7 +249,7 @@ struct lgpu_index {
     DevBuf cent_b, cent_n2;             // bf16 centroids + |c|^2 for the tensor-core coarse step
     DevBuf cent_sb, cent_sn2;           // every COARSE_SAMPLE_STRIDE-th centroid (bf16 + |c|^2): the threshold sample
     uint32_t cent_ns = 0;               // rows of the sample (0: none)
-    float cent_max = 0.f;
+    float cent_max = 0.f, cent_err = 0.f;   // max |c|, max |bf16(c) - c| (the error band, kernels.cuh tc_band)
     bool has_tc = false;
     bool has_vectors = false;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
@@ -264,7 +264,7 @@ struct lgpu_flat {
     uint32_t dim = 0;
     DevBuf vectors, row_ids, ysqrt;
     DevBuf vec_b, vec_n2;               // bf16 rows + |x|^2 for the tensor-core path
-    float vec_max = 0.f;
+    float vec_max = 0.f, vec_err = 0.f;     // max |x|, max |bf16(x) - x|
     int num_sms = 0;
     bool has_tc = false;
     bool has_ids = false, has_norms = false;
@@ -427,18 +427,24 @@ static bool tc_enabled()
     return v == 1;
 }
 
-// bf16 copy + squared norms + max norm of a row-major f32 matrix (open time)
-static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, cudaStream_t st)
+// bf16 copy + squared norms + max norm and max bf16 rounding error |bf16(x) - x| of a row-major f32 matrix (open time)
+static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
+                               cudaStream_t st)
 {
     Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
     n2.ensure(std::max<size_t>((size_t)n * 4, 16));
-    launch_to_bf16(X, n, d, Xb.p, n2.as<float>(), st);
-    std::vector<float> h(n);
+    DevBuf err;
+    err.ensure(std::max<size_t>((size_t)n * 4, 16));
+    launch_to_bf16(X, n, d, Xb.p, n2.as<float>(), st, err.as<float>());
+    std::vector<float> h(n), he(n);
     LGPU_CUDA(cudaMemcpyAsync(h.data(), n2.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    LGPU_CUDA(cudaMemcpyAsync(he.data(), err.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     LGPU_CUDA(cudaStreamSynchronize(st));
-    float m = 0.f;
+    float m = 0.f, me = 0.f;
     for (float v : h) m = std::max(m, v);
+    for (float v : he) me = std::max(me, v);
     xmax = std::sqrt(m) * 1.0001f;
+    xerr = me;
 }
 
 // Tensor-core shortlist + exact re-score (squared L2 only): the k best of the N rows of X for each
@@ -446,14 +452,15 @@ static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &X
 // (distance, id).  Dbuf: [B][ld] f32 scratch.  Queries whose shortlist cannot be proven complete
 // (band_check) are redone by the exact kernels in the same stream, without a host round trip.
 static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
-                       const void *Xb, const float *xnorm2, float xmax, uint64_t N, uint32_t d,
+                       const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
                        const uint64_t *col_ids, uint32_t k, uint32_t kp, uint64_t *out_ids, float *out_dist,
                        uint32_t *out_cnt, float *Dbuf, uint64_t ld)
 {
-    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->flags.ensure((size_t)B * 4);
+    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
+    ws->flags.ensure((size_t)B * 4);
     ws->t_ids.ensure((size_t)B * kp * 8); ws->t_dist.ensure((size_t)B * kp * 4);
     ws->t_pos.ensure((size_t)B * kp * 8); ws->t_cnt.ensure((size_t)B * 4); ws->t_exact.ensure((size_t)B * kp * 4);
-    launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st);
+    launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, Dbuf, ld, num_sms, st);
     SelectArgs sa{};
     sa.mode = 1; sa.dense = Dbuf; sa.ncols = N; sa.row_stride = ld; sa.col_ids = col_ids;
@@ -462,8 +469,8 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
     sa.out_count = ws->t_cnt.as<uint32_t>(); sa.out_pos = ws->t_pos.as<uint64_t>();
     launch_select(sa, st);
     if (kp >= N) LGPU_CUDA(cudaMemsetAsync(ws->flags.p, 0, (size_t)B * 4, st));   // every row is a candidate
-    else launch_band_check(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), xmax, d, B, k, kp,
-                           ws->flags.as<uint32_t>(), st);
+    else launch_band_check(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
+                           xmax, xerr, d, B, k, kp, ws->flags.as<uint32_t>(), st);
     launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, kp, d, LGPU_L2, ws->t_exact.as<float>(), st);
     SelectArgs sb{};
     sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
@@ -484,28 +491,29 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
 // filtering epilogue (no dense score matrix), the few admitted rows are re-scored exactly, and queries whose
 // candidate list overflowed are redone by the exact kernels.
 static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
-                                const void *Xb, const float *xnorm2, float xmax, uint64_t N, uint32_t d,
+                                const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
                                 const uint64_t *col_ids, uint32_t k, uint64_t *out_ids, float *out_dist,
                                 uint32_t *out_cnt, float *Dbuf, uint64_t ld, uint64_t min_sample = 65536,
                                 uint32_t cap = 1024)
 {
     const uint64_t Ns = std::min<uint64_t>(N, std::max<uint64_t>(min_sample, N / 8));
     const uint64_t lds = (Ns + 3) & ~3ull;               // Dbuf is [B][ld >= lds]
-    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->flags.ensure((size_t)B * 4);
+    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
+    ws->flags.ensure((size_t)B * 4);
     ws->t_ids.ensure((size_t)B * cap * 8); ws->t_dist.ensure((size_t)B * std::max<uint32_t>(k, 32) * 4);
     ws->t_pos.ensure((size_t)B * cap * 8); ws->t_cnt.ensure((size_t)B * 4); ws->t_exact.ensure((size_t)B * cap * 4);
     ws->probe_A.ensure((size_t)B * 4);                   // thr[q]
     ws->amax.ensure((size_t)B * 4);                      // candidate counters
     ws->sbound.ensure((size_t)B * std::max<uint32_t>(k, 32) * 8);   // sample ids (unused)
-    launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st);
+    launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
     // 1. sample pass: dense scores of the first Ns rows, k-th best per query -> threshold
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, Ns, d, Dbuf, lds, num_sms, st);
     SelectArgs sa{};
     sa.mode = 1; sa.dense = Dbuf; sa.ncols = Ns; sa.row_stride = lds; sa.B = B; sa.k = k;
     sa.out_ids = ws->sbound.as<uint64_t>(); sa.out_dist = ws->t_dist.as<float>(); sa.out_count = ws->t_cnt.as<uint32_t>();
     launch_select(sa, st);
-    launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), xmax, d, B, k,
-                            ws->probe_A.as<float>(), st);
+    launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
+                            xmax, xerr, d, B, k, ws->probe_A.as<float>(), st);
     // 2. full pass with the filtering epilogue
     LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
     LGPU_CUDA(cudaMemsetAsync(ws->t_pos.p, 0xff, (size_t)B * cap * 8, st));
@@ -609,10 +617,11 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
             // tensor-core GEMM scores + one finishing kernel per query (threshold, exact re-score in lance order, top
             // nprobes): bit-identical probe sets; queries whose candidate band overflowed are redone exactly
             mark();
-            ws->qb.ensure((size_t)B * dim * 2); ws->qn2.ensure((size_t)B * 4); ws->flags.ensure((size_t)B * 4);
+            ws->qb.ensure((size_t)B * dim * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
+            ws->flags.ensure((size_t)B * 4);
             ws->c_wcnt.ensure(16);
             uint32_t *cgate = ws->c_wcnt.as<uint32_t>() + 2;    // 0 = no query overflowed: the exact fix-up returns at once
-            launch_to_bf16(qsearch, B, dim, ws->qb.p, ws->qn2.as<float>(), st);
+            launch_to_bf16(qsearch, B, dim, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
             if (modes.coarse_list_min && nlist >= modes.coarse_list_min && ix->cent_ns >= 4 * nprobes && nprobes <= 64) {
                 // Many lists (C5: 16384): a dense [B][nlist] score matrix is 537 MB written and read back.  Instead: (1) dense scores of a strided SAMPLE of the centroids; their
                 // nprobes-th smallest + 2 E_q bounds, per query, the scores of every true probe; (2) the full GEMM runs
@@ -625,14 +634,15 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
                 ws->t_pos.ensure((size_t)B * lcap * 8); ws->t_exact.ensure((size_t)B * lcap * 4);
                 launch_gemm_dist(ws->qb.p, ix->cent_sb.p, ix->cent_sn2.as<float>(), B, ns, dim, ws->D.as<float>(), lds,
                                  ix->num_sms, st);
-                if (!launch_sample_kth_threshold(ws->D.as<float>(), lds, ns, ws->qn2.as<float>(), ix->cent_max, dim, B, nprobes,
-                                                 ws->probe_A.as<float>(), st)) {
+                if (!launch_sample_kth_threshold(ws->D.as<float>(), lds, ns, ws->qn2.as<float>(), ws->qerr.as<float>(),
+                                                 ix->cent_max, ix->cent_err, dim, B, nprobes, ws->probe_A.as<float>(), st)) {
                     SelectArgs ss{};
                     ss.mode = 1; ss.dense = ws->D.as<float>(); ss.ncols = ns; ss.row_stride = lds; ss.B = B; ss.k = nprobes;
                     ss.out_ids = ws->t_ids.as<uint64_t>(); ss.out_dist = ws->t_dist.as<float>(); ss.out_count = ws->t_cnt.as<uint32_t>();
                     launch_select(ss, st);
-                    launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ix->cent_max, dim,
-                                            B, nprobes, ws->probe_A.as<float>(), st);
+                    launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(),
+                                            ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, B, nprobes,
+                                            ws->probe_A.as<float>(), st);
                 }
                 LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
                 GemmFilter flt{};
@@ -640,14 +650,15 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
                 flt.cand_ids = nullptr; flt.col_ids = nullptr; flt.cap = lcap; flt.cand_s = ws->t_exact.as<float>();
                 launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, nullptr, 0, ix->num_sms, st, &flt);
                 launch_coarse_finish(ws->t_exact.as<float>(), lcap, B, lcap, qsearch, ix->centroids.as<float>(),
-                                     ws->qn2.as<float>(), ix->cent_max, dim, nprobes, ws->probes.as<uint64_t>(),
+                                     ws->qn2.as<float>(), ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes,
+                                     ws->probes.as<uint64_t>(),
                                      ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate,
                                      st, ws->t_pos.as<uint64_t>(), ws->amax.as<uint32_t>());
             } else {
                 launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, ws->D.as<float>(), ldc,
                                  ix->num_sms, st);
                 launch_coarse_finish(ws->D.as<float>(), ldc, B, nlist, qsearch, ix->centroids.as<float>(), ws->qn2.as<float>(),
-                                     ix->cent_max, dim, nprobes, ws->probes.as<uint64_t>(), ws->probe_dist.as<float>(),
+                                     ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes, ws->probes.as<uint64_t>(), ws->probe_dist.as<float>(),
                                      ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate, st);
             }
             launch_dist_matrix(qsearch, ix->centroids.as<float>(), B, nlist, dim, 0, nullptr, nullptr, ws->D.as<float>(), ldc,
@@ -1004,13 +1015,13 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
             !rf.bits) {
             if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
                 tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p,
-                                    fl->vec_n2.as<float>(), fl->vec_max, N, fl->dim,
+                                    fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
                                     fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k,
                                     d_ids + (size_t)q0 * sp.k, d_dist + (size_t)q0 * sp.k, d_cnt + q0,
                                     ws->D.as<float>(), ld);
             else
                 tc_topk_l2(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p, fl->vec_n2.as<float>(),
-                           fl->vec_max, N, fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp,
+                           fl->vec_max, fl->vec_err, N, fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp,
                            d_ids + (size_t)q0 * sp.k, d_dist + (size_t)q0 * sp.k, d_cnt + q0, ws->D.as<float>(), ld);
             continue;
         }
@@ -1246,7 +1257,8 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
         if (d->vectors) { up(ix->vectors, d->vectors, (size_t)d->nrows * d->dim * 4); ix->has_vectors = true; }
         if (gemm_shape_supported(d->dim) && d->metric != LGPU_DOT) {
             LGPU_CUDA(cudaStreamSynchronize(st));
-            prepare_tc_operand(ix->centroids.as<float>(), nlist, d->dim, ix->cent_b, ix->cent_n2, ix->cent_max, st);
+            prepare_tc_operand(ix->centroids.as<float>(), nlist, d->dim, ix->cent_b, ix->cent_n2, ix->cent_max, ix->cent_err,
+                               st);
             ix->device_bytes += ix->cent_b.bytes + ix->cent_n2.bytes;
             if (nlist >= 1024) {
                 // every 8th centroid, for the sampled threshold of the coarse step (strided: whatever order the
@@ -1604,7 +1616,7 @@ int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uin
         LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
         fl->num_sms = prop.multiProcessorCount;
         if (gemm_shape_supported(dim) && nrows >= 4096) {
-            prepare_tc_operand(fl->vectors.as<float>(), nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max, nullptr);
+            prepare_tc_operand(fl->vectors.as<float>(), nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max, fl->vec_err, nullptr);
             fl->has_tc = true;
         }
         if (row_ids && nrows) {
@@ -1935,14 +1947,14 @@ static void assign_nearest(const float *d_x, uint64_t n, uint32_t dim, const flo
 {
     const uint64_t ld = (k + 3ull) & ~3ull;
     const uint64_t CH = std::max<uint64_t>(256, std::min<uint64_t>(65536, ((uint64_t)1 << 28) / (ld * 4)));
-    DevBuf D, cnt, flags, gate, xb, xn2, cb, cn2;
+    DevBuf D, cnt, flags, gate, xb, xn2, xerr, cb, cn2;
     D.ensure((size_t)CH * ld * 4); cnt.ensure((size_t)CH * 4);
     const bool tc = gemm_shape_supported(dim) && k >= 256 && tc_enabled();
-    float cmax = 0.f;
+    float cmax = 0.f, cerr = 0.f;
     if (tc) {
         flags.ensure((size_t)CH * 4); gate.ensure(16);
-        xb.ensure((size_t)CH * dim * 2); xn2.ensure((size_t)CH * 4);
-        prepare_tc_operand(d_cent, k, dim, cb, cn2, cmax, st);
+        xb.ensure((size_t)CH * dim * 2); xn2.ensure((size_t)CH * 4); xerr.ensure((size_t)CH * 4);
+        prepare_tc_operand(d_cent, k, dim, cb, cn2, cmax, cerr, st);
     }
     for (uint64_t r0 = 0; r0 < n; r0 += CH) {
         const uint32_t b = (uint32_t)std::min<uint64_t>(CH, n - r0);
@@ -1951,9 +1963,10 @@ static void assign_nearest(const float *d_x, uint64_t n, uint32_t dim, const flo
         sa.mode = 1; sa.dense = D.as<float>(); sa.ncols = k; sa.row_stride = ld; sa.B = b; sa.k = 1;
         sa.out_ids = d_ids + r0; sa.out_dist = d_dist + r0; sa.out_count = cnt.as<uint32_t>();
         if (tc) {
-            launch_to_bf16(q, b, dim, xb.p, xn2.as<float>(), st);
+            launch_to_bf16(q, b, dim, xb.p, xn2.as<float>(), st, xerr.as<float>());
             launch_gemm_dist(xb.p, cb.p, cn2.as<float>(), b, k, dim, D.as<float>(), ld, num_sms, st);
-            launch_coarse_finish(D.as<float>(), ld, b, k, q, d_cent, xn2.as<float>(), cmax, dim, 1, d_ids + r0, d_dist + r0,
+            launch_coarse_finish(D.as<float>(), ld, b, k, q, d_cent, xn2.as<float>(), xerr.as<float>(), cmax, cerr, dim, 1,
+                                 d_ids + r0, d_dist + r0,
                                  cnt.as<uint32_t>(), flags.as<uint32_t>(), gate.as<uint32_t>(), st);
             launch_dist_matrix(q, d_cent, b, k, dim, 0, nullptr, nullptr, D.as<float>(), ld, st, flags.as<uint32_t>(),
                                gate.as<uint32_t>());

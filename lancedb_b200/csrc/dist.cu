@@ -243,7 +243,9 @@ constexpr int CF_THREADS = 256;
 template <int VPT>
 __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *__restrict__ S, uint64_t ld, uint32_t N_,
                                                                    const float *__restrict__ Q, const float *__restrict__ C,
-                                                                   const float *__restrict__ qn2, float xmax, uint32_t d,
+                                                                   const float *__restrict__ qn2,
+                                                                   const float *__restrict__ qerr, float xmax, float xerr,
+                                                                   uint32_t d,
                                                                    uint32_t k, uint32_t cap,
                                                                    uint64_t *__restrict__ out_ids, float *__restrict__ out_dist,
                                                                    uint32_t *__restrict__ out_cnt, uint32_t *__restrict__ flags,
@@ -314,9 +316,7 @@ __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *
     float thr = -CUDART_INF_F;
     if (kk > 0) {
         float lo = key_f32(s_lo), hi = key_f32(s_hi);               // invariant: count(S <= hi) >= kk
-        const float qn = sqrtf(qn2[q]);
-        const float sm = qn + xmax;
-        const float E = 0.0078125f * 1.00390625f * qn * xmax + 4.0f * (float)d * 5.9604645e-8f * sm * sm;
+        const float E = tc_band(qn2[q], qerr[q], xmax, xerr, d);
         if (hi < CUDART_INF_F && lo > -CUDART_INF_F) {
             for (int it = 0; it < 20 && hi - lo > 0.25f * E; it++) {    // the band is 2E wide anyway
                 const float mid = 0.5f * lo + 0.5f * hi;
@@ -404,7 +404,8 @@ __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *
 }  // namespace
 
 void launch_coarse_finish(const float *S, uint64_t ld, uint32_t B, uint32_t N, const float *Q, const float *C,
-                          const float *qn2, float xmax, uint32_t d, uint32_t k, uint64_t *out_ids, float *out_dist,
+                          const float *qn2, const float *qerr, float xmax, float xerr, uint32_t d, uint32_t k,
+                          uint64_t *out_ids, float *out_dist,
                           uint32_t *out_cnt, uint32_t *flags, uint32_t *gate, cudaStream_t st,
                           const uint64_t *list_pos, const uint32_t *list_cnt)
 {
@@ -417,7 +418,7 @@ void launch_coarse_finish(const float *S, uint64_t ld, uint32_t B, uint32_t N, c
 #define LGPU_CF(V) do { \
         const size_t smem = smem0 + ((V) >= 64 ? (size_t)(V) * CF_THREADS * 4 : 0); \
         if (smem > 48 * 1024) LGPU_CUDA(cudaFuncSetAttribute(coarse_finish_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        launch_k(coarse_finish_kernel<V>, dim3(B), dim3(CF_THREADS), smem, st, S, ld, N, Q, C, qn2, xmax, d, k, cap, out_ids, out_dist, out_cnt, flags, gate, list_pos, list_cnt); \
+        launch_k(coarse_finish_kernel<V>, dim3(B), dim3(CF_THREADS), smem, st, S, ld, N, Q, C, qn2, qerr, xmax, xerr, d, k, cap, out_ids, out_dist, out_cnt, flags, gate, list_pos, list_cnt); \
     } while (0)
     if ((list_pos == nullptr) != (list_cnt == nullptr) || (list_pos && N != ld)) {
         set_error("internal: coarse_finish list mode needs positions, counts and N == list capacity"); throw Failure{LGPU_RUNTIME};

@@ -297,9 +297,10 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     }
 }
 
-// X f32 [n][d] -> bf16 [n][d] (round to nearest even) and |x|^2 in f32; one warp per row
+// X f32 [n][d] -> bf16 [n][d] (round to nearest even), |x|^2 and the rounding error |bf16(x) - x| in f32; one warp
+// per row
 __global__ void to_bf16_norm_kernel(const float *__restrict__ X, uint64_t n, uint32_t d, __nv_bfloat16 *__restrict__ Xb,
-                                    float *__restrict__ norm2)
+                                    float *__restrict__ norm2, float *__restrict__ err)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -307,15 +308,22 @@ __global__ void to_bf16_norm_kernel(const float *__restrict__ X, uint64_t n, uin
     if (row >= n) return;
     const float *x = X + row * d;
     __nv_bfloat16 *xb = Xb + row * d;
-    float s = 0.f;
+    float s = 0.f, se = 0.f;
     for (uint32_t k = lane; k < d; k += 32) {
         float v = x[k];
-        xb[k] = __float2bfloat16_rn(v);
+        const __nv_bfloat16 b = __float2bfloat16_rn(v);
+        xb[k] = b;
         s = fmaf(v, v, s);
+        const float e = __bfloat162float(b) - v;                    // exact: b and v are within a factor of 2
+        se = fmaf(e, e, se);
     }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    for (int o = 16; o > 0; o >>= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, o);
+        se += __shfl_xor_sync(0xffffffffu, se, o);
+    }
     if (lane == 0 && norm2) norm2[row] = s;
+    if (lane == 0 && err) err[row] = sqrtf(se);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -357,16 +365,14 @@ CUtensorMap make_map(const void *ptr, uint64_t rows, uint32_t d, uint32_t box_ro
 }
 
 __global__ void band_check_kernel(const float *__restrict__ approx, const uint32_t *__restrict__ cnt,
-                                  const float *__restrict__ qnorm2, float xmax, uint32_t d, uint32_t B, uint32_t k,
-                                  uint32_t kp, uint32_t *__restrict__ flags)
+                                  const float *__restrict__ qnorm2, const float *__restrict__ qerr, float xmax, float xerr,
+                                  uint32_t d, uint32_t B, uint32_t k, uint32_t kp, uint32_t *__restrict__ flags)
 {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
     uint32_t f = 0;
     if (cnt[q] >= kp && kp > 0) {              // list is full: columns beyond it may exist
-        const float qn = sqrtf(qnorm2[q]);
-        const float s = qn + xmax;
-        const float E = 0.0078125f * 1.00390625f * qn * xmax + 4.0f * (float)d * 5.9604645e-8f * s * s;
+        const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
         const float kth = approx[(size_t)q * kp + (k - 1 < kp ? k - 1 : kp - 1)];
         const float last = approx[(size_t)q * kp + kp - 1];
         f = (k >= kp || !(last > kth + 2.0f * E)) ? 1u : 0u;
@@ -375,18 +381,16 @@ __global__ void band_check_kernel(const float *__restrict__ approx, const uint32
 }
 
 // thr[q] = (k-th smallest approximate score of the sample) + 2 E_q, or +inf when the sample holds < k rows;
-// every true top-k row of the full set has a score <= thr[q] (E_q as in band_check_kernel)
+// every true top-k row of the full set has a score <= thr[q] (E_q: tc_band)
 __global__ void sample_threshold_kernel(const float *__restrict__ approx, const uint32_t *__restrict__ cnt,
-                                        const float *__restrict__ qnorm2, float xmax, uint32_t d, uint32_t B, uint32_t k,
-                                        float *__restrict__ thr)
+                                        const float *__restrict__ qnorm2, const float *__restrict__ qerr, float xmax,
+                                        float xerr, uint32_t d, uint32_t B, uint32_t k, float *__restrict__ thr)
 {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
     float t = __int_as_float(0x7f800000);
     if (cnt[q] >= k) {
-        const float qn = sqrtf(qnorm2[q]);
-        const float s = qn + xmax;
-        const float E = 0.0078125f * 1.00390625f * qn * xmax + 4.0f * (float)d * 5.9604645e-8f * s * s;
+        const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
         t = approx[(size_t)q * k + k - 1] + 2.0f * E;
     }
     thr[q] = t;
@@ -397,8 +401,9 @@ __global__ void sample_threshold_kernel(const float *__restrict__ approx, const 
 // count(S <= hi) >= k is a valid bound.  NaN scores never count.  ns <= 32 * VPL.
 template <int VPL>
 __global__ void __launch_bounds__(128) sample_kth_threshold_kernel(const float *__restrict__ D, uint64_t ld, uint32_t ns,
-                                                                  const float *__restrict__ qnorm2, float xmax, uint32_t d,
-                                                                  uint32_t B, uint32_t k, float *__restrict__ thr)
+                                                                  const float *__restrict__ qnorm2,
+                                                                  const float *__restrict__ qerr, float xmax, float xerr,
+                                                                  uint32_t d, uint32_t B, uint32_t k, float *__restrict__ thr)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -434,9 +439,7 @@ __global__ void __launch_bounds__(128) sample_kth_threshold_kernel(const float *
     nv = __reduce_add_sync(0xffffffffu, nv);
     float t = __int_as_float(0x7f800000);
     if (nv >= k && hi < __int_as_float(0x7f800000) && lo > -__int_as_float(0x7f800000)) {
-        const float qn = sqrtf(qnorm2[q]);
-        const float s = qn + xmax;
-        const float E = 0.0078125f * 1.00390625f * qn * xmax + 4.0f * (float)d * 5.9604645e-8f * s * s;
+        const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
         for (int it = 0; it < 24 && hi - lo > 0.25f * E; it++) {        // invariant: count(S <= hi) >= k
             const float mid = 0.5f * lo + 0.5f * hi;
             uint32_t c = 0;
@@ -458,22 +461,22 @@ __global__ void overflow_flags_kernel(const uint32_t *__restrict__ count, uint32
 
 }  // namespace
 
-void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, float xmax, uint32_t d,
-                             uint32_t B, uint32_t k, float *thr, cudaStream_t st)
+void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,
+                             float xerr, uint32_t d, uint32_t B, uint32_t k, float *thr, cudaStream_t st)
 {
     if (B == 0) return;
-    sample_threshold_kernel<<<(B + 127) / 128, 128, 0, st>>>(approx, cnt, qnorm2, xmax, d, B, k, thr); LGPU_COUNT_LAUNCH();
+    sample_threshold_kernel<<<(B + 127) / 128, 128, 0, st>>>(approx, cnt, qnorm2, qerr, xmax, xerr, d, B, k, thr); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
-bool launch_sample_kth_threshold(const float *D, uint64_t ld, uint32_t ns, const float *qnorm2, float xmax, uint32_t d,
-                                 uint32_t B, uint32_t k, float *thr, cudaStream_t st)
+bool launch_sample_kth_threshold(const float *D, uint64_t ld, uint32_t ns, const float *qnorm2, const float *qerr, float xmax,
+                                 float xerr, uint32_t d, uint32_t B, uint32_t k, float *thr, cudaStream_t st)
 {
     if (B == 0) return true;
     if (ns == 0 || ns > 2048 || (ld & 3) || ld < ns) return false;       // caller falls back to select + threshold
     const unsigned grid = (B + 3) / 4;
-    if (ns <= 1024) launch_k(sample_kth_threshold_kernel<32>, dim3(grid), dim3(128), 0, st, D, ld, ns, qnorm2, xmax, d, B, k, thr);
-    else launch_k(sample_kth_threshold_kernel<64>, dim3(grid), dim3(128), 0, st, D, ld, ns, qnorm2, xmax, d, B, k, thr);
+    if (ns <= 1024) launch_k(sample_kth_threshold_kernel<32>, dim3(grid), dim3(128), 0, st, D, ld, ns, qnorm2, qerr, xmax, xerr, d, B, k, thr);
+    else launch_k(sample_kth_threshold_kernel<64>, dim3(grid), dim3(128), 0, st, D, ld, ns, qnorm2, qerr, xmax, xerr, d, B, k, thr);
     LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
     return true;
@@ -486,21 +489,21 @@ void launch_overflow_flags(const uint32_t *count, uint32_t cap, uint32_t B, uint
     LGPU_CUDA(cudaGetLastError());
 }
 
-void launch_band_check(const float *approx, const uint32_t *cnt, const float *qnorm2, float xmax, uint32_t d,
-                       uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, cudaStream_t st)
+void launch_band_check(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,
+                       float xerr, uint32_t d, uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, cudaStream_t st)
 {
     if (B == 0) return;
-    band_check_kernel<<<(B + 127) / 128, 128, 0, st>>>(approx, cnt, qnorm2, xmax, d, B, k, kp, flags); LGPU_COUNT_LAUNCH();
+    band_check_kernel<<<(B + 127) / 128, 128, 0, st>>>(approx, cnt, qnorm2, qerr, xmax, xerr, d, B, k, kp, flags); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
 bool gemm_shape_supported(uint32_t d) { return d >= 8 && d % 8 == 0; }
 
-void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *norm2, cudaStream_t st)
+void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *norm2, cudaStream_t st, float *err)
 {
     if (n == 0) return;
     uint64_t threads = n * 32;
-    launch_k(to_bf16_norm_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, X, n, d, reinterpret_cast<__nv_bfloat16 *>(Xb), norm2); LGPU_COUNT_LAUNCH();
+    launch_k(to_bf16_norm_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, X, n, d, reinterpret_cast<__nv_bfloat16 *>(Xb), norm2, err); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

@@ -143,7 +143,8 @@ void launch_dist_matrix(const float *Q, const float *C, uint32_t B, uint64_t N, 
 // columns with the smallest EXACT l2 distance (lance lane order), ascending by (distance, column); flags[q] = 1 when
 // the candidate band overflowed and the caller must redo the query with the exact kernels
 void launch_coarse_finish(const float *S, uint64_t ld, uint32_t B, uint32_t N, const float *Q, const float *C,
-                          const float *qn2, float xmax, uint32_t d, uint32_t k, uint64_t *out_ids, float *out_dist,
+                          const float *qn2, const float *qerr, float xmax, float xerr, uint32_t d, uint32_t k,
+                          uint64_t *out_ids, float *out_dist,
                           uint32_t *out_cnt, uint32_t *flags, uint32_t *gate, cudaStream_t st,
                           const uint64_t *list_pos = nullptr, const uint32_t *list_cnt = nullptr);
 // list mode (list_pos / list_cnt given, N == ld == the list capacity): S[q] holds the list_cnt[q] scores the GEMM's
@@ -212,8 +213,21 @@ void launch_pack_records(const uint64_t *ids, const float *dist, uint64_t n, Top
 
 // ---------------- tensor-core shortlist (gemm.cu) ------------------------------------
 bool gemm_shape_supported(uint32_t d);
-// X f32 [n][d] -> bf16 [n][d]; norm2[n] = |x|^2 (f32) if norm2 != nullptr
-void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *norm2, cudaStream_t st);
+// X f32 [n][d] -> bf16 [n][d]; norm2[n] = |x|^2 (f32) if norm2 != nullptr; err[n] = |bf16(x) - x| if err != nullptr
+void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *norm2, cudaStream_t st, float *err = nullptr);
+// E_q, the error band of the tensor-core scores: |S[q][x] - (|q - x|^2 - |q|^2)| <= E_q for every row x of the operand,
+// S[q][x] = |x|^2 - 2 bf16(q).bf16(x) (f32 accumulation), with r_q = |bf16(q) - q| (qerr), r_X = max_x |bf16(x) - x|
+// (xerr) and xmax >= max_x |x|:
+//   E_q = 2 ((|q| + r_q) r_X + r_q xmax)(1 + 2^-10) + 4 d 2^-24 (|q| + xmax)^2.
+// bf16(q).bf16(x) - q.x = bf16(q).(bf16(x) - x) + (bf16(q) - q).x and |bf16(q)| <= |q| + r_q; 2^-10 covers the f32
+// arithmetic of the r's and of E_q itself, the last term the f32 sums (|x|^2, the accumulation, the exact re-score).
+// Both operands round: r can reach 2^-8 of the norm each, so E_q reaches ~2^-6 |q| xmax on adversarial data.  Every
+// consumer (band check, sample thresholds, coarse finishing kernel) takes its band from here.
+__device__ __forceinline__ float tc_band(float qnorm2, float qerr, float xmax, float xerr, uint32_t d)
+{
+    const float qn = sqrtf(qnorm2), s = qn + xmax;
+    return 2.0f * 1.0009765625f * ((qn + qerr) * xerr + qerr * xmax) + 4.0f * (float)d * 5.9604645e-8f * s * s;
+}
 // out[q][x] = xnorm2[x] - 2 * bf16(Q[q]) . bf16(X[x])   (wgmma + TMA), q < B, x < N
 // optional filtering epilogue: instead of writing the dense score matrix, append the columns whose score
 // is <= thr[q] to the query's candidate list (count may exceed cap: those appends are dropped)
@@ -230,17 +244,16 @@ void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint3
                       float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter = nullptr);
 // filtering epilogue on an existing dense score matrix D[B][ld] (see gemm.cu)
 void launch_filter_dense(const float *D, uint64_t ld, uint32_t B, uint64_t N, const GemmFilter &flt, cudaStream_t st);
-void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, float xmax, uint32_t d,
-                             uint32_t B, uint32_t k, float *thr, cudaStream_t st);
+void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,
+                             float xerr, uint32_t d, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
 // the same threshold straight from dense sample scores D[B][ld] (ns <= 4096 columns; false = shape not handled)
-bool launch_sample_kth_threshold(const float *D, uint64_t ld, uint32_t ns, const float *qnorm2, float xmax, uint32_t d,
-                                 uint32_t B, uint32_t k, float *thr, cudaStream_t st);
+bool launch_sample_kth_threshold(const float *D, uint64_t ld, uint32_t ns, const float *qnorm2, const float *qerr, float xmax,
+                                 float xerr, uint32_t d, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
 void launch_overflow_flags(const uint32_t *count, uint32_t cap, uint32_t B, uint32_t *flags, cudaStream_t st);
 // flags[q] = 1 when the approximate shortlist of query q cannot be proven to contain the exact top-k:
-// approx[q][0..kp) ascending, cnt[q] entries valid; proven iff cnt < kp or approx[kp-1] > approx[k-1] + 2E_q,
-// E_q = 2^-7 (1+2^-8) |q| xmax + 4 d 2^-24 (|q| + xmax)^2
-void launch_band_check(const float *approx, const uint32_t *cnt, const float *qnorm2, float xmax, uint32_t d,
-                       uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, cudaStream_t st);
+// approx[q][0..kp) ascending, cnt[q] entries valid; proven iff cnt < kp or approx[kp-1] > approx[k-1] + 2E_q (tc_band)
+void launch_band_check(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,
+                       float xerr, uint32_t d, uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, cudaStream_t st);
 
 // ---------------- filter + verify form of the PQ scan (tables.cu, scan3.cu) -------------
 // Quantised per-query tables.  qt[q][ch][c] = 8 x u16, position j = n_q[i][c] for sub-space i = 8 ch + ((j + c) & 7):

@@ -1,6 +1,7 @@
 """Host restatement of the coarse step at many lists (api.cu: sampled bound -> list epilogue -> finishing kernel on the
 list; gemm.cu, dist.cu) checked on the CPU: with S[x] = |c_x|^2 - 2 bf16(q).bf16(c_x) (f32 accumulation of bf16
-products) and E_q = 2^-7 (1 + 2^-8) |q| cmax + 4 d 2^-24 (|q| + cmax)^2,
+products) and E_q = 2 ((|q| + r_q) r_C + r_q cmax)(1 + 2^-10) + 4 d 2^-24 (|q| + cmax)^2, r_q = |bf16(q) - q|,
+r_C = max_x |bf16(c_x) - c_x| (kernels.cuh tc_band, tests/util.py),
 
   (1) |S[x] + |q|^2 - d*(q, x)| <= E_q for every centroid (the band the kernels rely on), d* the oracle's distance;
   (2) thr1 = (k-th smallest S over every 8th centroid) + 2 E_q admits every true probe into the list;
@@ -10,29 +11,15 @@ products) and E_q = 2^-7 (1 + 2^-8) |q| cmax + 4 d 2^-24 (|q| + cmax)^2,
 
 Random centroids, centroids in tight clusters with consecutive ids (what a hierarchical trainer leaves), queries on a
 centroid, and scaled data.  The GPU tests (tests/test_gpu_tensorcore.py) check the kernels' results; this pins the
-algebra they implement."""
+algebra they implement.  tests/test_gemm_band.py puts the same steps under adversarial rounding."""
 import numpy as np
 import pytest
 
 import oracle
-from tests.util import queries, random_index
+from tests.util import queries, random_index, tc_band, tc_scores
 
 F = np.float32
 STRIDE = 8
-
-
-def _bf16(x):
-    """round-to-nearest-even f32 -> bf16 -> f32 (gemm.cu to_bf16_norm_kernel)"""
-    u = np.ascontiguousarray(x, F).view(np.uint32).astype(np.uint64)
-    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
-    return r.astype(np.uint32).view(F).reshape(np.shape(x))
-
-
-def _scores(q, C):
-    qb, Cb = _bf16(q).astype(np.float64), _bf16(C).astype(np.float64)
-    dot = (Cb @ qb).astype(F)                               # products of bf16 are exact in f32; the sum is f32
-    cn2 = (C.astype(np.float64) ** 2).sum(1).astype(F)
-    return (cn2 - F(2) * dot).astype(F)
 
 
 def _check(ix, q, k):
@@ -40,10 +27,9 @@ def _check(ix, q, k):
     orc = oracle.OracleIndex.from_data(ix)
     qn = oracle.normalize(q) if ix.metric == "cosine" else q.astype(F)
     dstar = orc.find_partitions(qn, ix.nlist)[2].astype(np.float64)      # exact distance to every centroid
-    S = _scores(qn, C)
+    S = tc_scores(qn, C)
     qn2 = float((qn.astype(np.float64) ** 2).sum())
-    cmax = float(np.sqrt((C.astype(np.float64) ** 2).sum(1).max())) * 1.0001
-    E = 0.0078125 * 1.00390625 * np.sqrt(qn2) * cmax + 4.0 * ix.dim * 5.9604645e-8 * (np.sqrt(qn2) + cmax) ** 2
+    E = tc_band(qn, C)
     assert np.abs(S.astype(np.float64) + qn2 - dstar).max() <= E                      # (1)
     truth = np.lexsort((np.arange(ix.nlist), dstar))[:k]
     sample = S[::STRIDE][: ix.nlist // STRIDE]

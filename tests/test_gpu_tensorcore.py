@@ -7,7 +7,7 @@ import torch
 
 import oracle
 from lancedb_b200 import _native
-from tests.util import queries, random_index
+from tests.util import queries, random_index, same_result, split_support_case
 
 pytestmark = pytest.mark.gpu
 
@@ -167,3 +167,48 @@ def test_coarse_tensorcore_path_bit_exact(metric, nprobes, monkeypatch):
         assert np.array_equal(parts[i], op)
     assert np.array_equal(gc, oc) and np.array_equal(gi, oi)
     assert np.array_equal(gd.view(np.uint32), od.view(np.uint32))
+
+
+# ---- adversarial bf16 rounding (tests/util.py split_support_case, tests/test_gemm_band.py): the true nearest row is
+# scored ~2^-7 |q||x| too high and k decoys as much too low, so only a band that allows for BOTH operands' rounding
+# keeps it.  Each path must still return the oracle's result bit for bit (directly, or through its exact fix-up).
+def _split_support_flat(n):
+    q, X = split_support_case(64, 1.0, n, 10)
+    Q = np.tile(q, (8, 1))
+    fl = _native.GpuFlat(X)
+    got = fl.search(Q, k=10)
+    fl.close()
+    want = oracle.flat_search(X, Q, k=10, nthreads=8)
+    assert want[0][0][0] == n - 1                                   # the construction's true nearest row
+    assert same_result(got, want)
+
+
+def test_flat_dense_shortlist_adversarial_rounding():
+    """N = 4096: the kp = 256 shortlist + band check"""
+    _split_support_flat(4096)
+
+
+def test_flat_filtered_adversarial_rounding():
+    """N = 262144: threshold from the first Ns rows (the decoys are there, the true nearest row is not) + filtering"""
+    _split_support_flat(262144)
+
+
+@pytest.mark.parametrize("list_path", [False, True])
+def test_coarse_adversarial_rounding(list_path, monkeypatch):
+    """IVF coarse step (dense finishing kernel, or the sampled bound + list with the decoys on sampled centroids): only
+    the true nearest centroid's partition holds rows, so a missed probe changes the counts"""
+    monkeypatch.setenv("LGPU_FORCE_TC_COARSE", "1")
+    if list_path:
+        monkeypatch.setenv("LGPU_COARSE_LIST_MIN", "1024")
+    nlist = 1024
+    q, C = split_support_case(64, 1.0, nlist, 10)
+    sizes = np.zeros(nlist, np.int64); sizes[-1] = 5
+    ix = random_index(np.random.default_rng(3), dim=64, nlist=nlist, m=8, sizes=sizes)
+    ix.centroids = C
+    Q = np.tile(q, (8, 1))
+    gpu = _native.GpuIvfPq(ix)
+    got = gpu.search(Q, k=10, nprobes=10)
+    gpu.close()
+    want = oracle.OracleIndex.from_data(ix).search(Q, k=10, nprobes=10, nthreads=8)
+    assert (want[2] == 5).all()
+    assert same_result(got, want)
