@@ -49,8 +49,8 @@ typedef enum {
     LGPU_OOM = 4             /* device or host allocation failure */
 } lgpu_status;
 
-/* lancedb::DistanceType, rust/lancedb/src/lib.rs:236-260 (hamming is u8-only and
- * not on this path: rust/lancedb/src/table/query.rs:230-236) */
+/* lancedb::DistanceType, rust/lancedb/src/lib.rs:236-260 (hamming is u8-only: it has its own
+ * column handle, lgpu_binary, below; rust/lancedb/src/table/query.rs:229-236) */
 typedef enum { LGPU_L2 = 0, LGPU_COSINE = 1, LGPU_DOT = 2 } lgpu_metric;
 
 typedef enum {
@@ -60,6 +60,7 @@ typedef enum {
 
 typedef struct lgpu_index lgpu_index;   /* an IVF_PQ index resident in HBM */
 typedef struct lgpu_flat lgpu_flat;     /* a raw vector column resident in HBM */
+typedef struct lgpu_binary lgpu_binary; /* a packed binary (uint8) vector column in HBM, searched by Hamming distance */
 
 /* The arrays of one IVF_PQ index (lance v2 `IvfPq`,
  * rust/lancedb/src/table/create_index.rs:283-303, :772): IVF centroids, PQ codebook
@@ -242,6 +243,25 @@ int  lgpu_flat_search_device(lgpu_flat *fl, int metric, const float *d_queries, 
                              uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count,
                              void *cuda_stream);
 
+/* ---- binary vectors: flat search by Hamming distance (the `is_binary` branch of
+ * rust/lancedb/src/table/query.rs:229-236: fixed_size_list<uint8, nbytes> columns, distance_type("hamming")) ----
+ * _distance = popcount(q XOR x) over the nbytes bytes, an integer in [0, 8 nbytes] (exact in f32; 8 nbytes <= 2^24).
+ * Results are ascending by (_distance, _rowid), as on the float flat path; k, distance_range, timeout_ms, k > nrows
+ * and nrows = 0 behave as there, nprobes and refine_factor are ignored.  vectors: [nrows][nbytes]; queries:
+ * [B][nbytes]. */
+int  lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes,
+                      const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device, lgpu_binary **out);
+void lgpu_binary_close(lgpu_binary *bx);
+int  lgpu_binary_search(lgpu_binary *bx, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
+                        uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+/* under a row-id allow-list (same bitmap as lgpu_search_filtered) */
+int  lgpu_binary_search_filtered(lgpu_binary *bx, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
+                                 const uint32_t *allow, uint64_t allow_bits,
+                                 uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+/* all five buffers in DEVICE memory, enqueued on `cuda_stream`, not synchronised */
+int  lgpu_binary_search_device(lgpu_binary *bx, const uint8_t *d_queries, uint32_t B, const lgpu_search_params *params,
+                               uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
+
 /* ---- per-stage access (parity localisation and kernel benchmarks) -------- */
 /* coarse stage only: the nprobes nearest partitions of each query and their
  * distances (host buffers, [B][nprobes]) */
@@ -255,12 +275,19 @@ int lgpu_debug_partition_distances(lgpu_index *ix, const float *query, uint32_t 
  * out is [B][N] f32); dim must be a multiple of 8 */
 int lgpu_debug_gemm(const float *queries, const float *vectors, uint32_t B, uint64_t N, uint32_t dim,
                     int device, float *out);
+/* the binary tensor-core kernel alone: out[q][x] = Hamming distance of queries[q] and vectors[x] (host buffers,
+ * queries [B][nbytes], vectors [N][nbytes], out [B][N] u32) */
+int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint32_t B, uint64_t N, uint32_t nbytes,
+                            int device, uint32_t *out);
 /* per-kernel device time (ms) of the most recent lgpu_search* call made with
  * LGPU_PROFILE=1 in the environment: coarse, select-probes, group, scan, top-k,
  * refine, total.  times: [7] */
 int lgpu_last_stage_ms(float *times);
 /* filter-scan counters of the most recent profiled lgpu_search* call on this thread (first sub-batch): candidates the
- * scanners appended, survivors re-scored exactly, queries sent to the exact fix-up pass, queries.  stats: [4] */
+ * scanners appended, survivors re-scored exactly, queries sent to the exact fix-up pass, queries.  stats: [4]
+ * After lgpu_binary_search* (whole batch): [0] candidates the tensor-core list pass appended (0 on the dense paths),
+ * [1] distances computed on the tensor cores (0 on the SIMT path), [2] queries redone densely after a list overflow,
+ * [3] queries. */
 int lgpu_last_filter_stats(uint64_t *stats);
 /* kernels this process has launched through the library so far (eager launches and graph replays alike) */
 int lgpu_kernel_launch_count(uint64_t *count);

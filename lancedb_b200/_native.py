@@ -32,6 +32,8 @@ EXPORTS = [
     "lgpu_ivf_assign", "lgpu_pq_encode", "lgpu_kmeans_train", "lgpu_pq_train",
     "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_gemm", "lgpu_last_stage_ms", "lgpu_set_profiling",
     "lgpu_kernel_launch_count", "lgpu_last_filter_stats",
+    "lgpu_binary_open", "lgpu_binary_close", "lgpu_binary_search", "lgpu_binary_search_filtered",
+    "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
 ]
 
 
@@ -113,6 +115,13 @@ def load():
     lib.lgpu_last_stage_ms.argtypes = [vp]
     lib.lgpu_set_profiling.argtypes = [i32]
     lib.lgpu_kernel_launch_count.argtypes = [C.POINTER(C.c_uint64)]
+    lib.lgpu_binary_open.argtypes = [vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
+    lib.lgpu_binary_close.argtypes = [vp]
+    lib.lgpu_binary_close.restype = None
+    lib.lgpu_binary_search.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
+    lib.lgpu_binary_search_filtered.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
+    lib.lgpu_binary_search_device.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
+    lib.lgpu_debug_hamming_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -292,6 +301,61 @@ class GpuFlat:
                                              stream))
 
 
+class GpuBinary:
+    """A packed binary vector column (fixed_size_list<uint8, nbytes>) pinned in HBM (lgpu_binary), searched by
+    Hamming distance."""
+
+    def __init__(self, vectors, row_ids=None, device: int = 0):
+        v = np.ascontiguousarray(vectors, np.uint8)
+        if v.ndim != 2:
+            raise ValueError("binary vectors must be a [rows, bytes] uint8 array")
+        self.nrows, self.nbytes = v.shape
+        rid = None if row_ids is None else np.ascontiguousarray(row_ids, np.uint64)
+        h = C.c_void_p()
+        check(load().lgpu_binary_open(_ptr(v), self.nrows, self.nbytes, _ptr(rid), device, C.byref(h)))
+        self._h = h
+        self.device = device
+
+    def close(self):
+        if getattr(self, "_h", None) and _lib is not None:
+            _lib.lgpu_binary_close(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def search(self, queries, k=10, lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
+        """Host-buffer search of queries [B, nbytes] (or one [nbytes] query) whose components are integers in
+        [0, 255]: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32)."""
+        q = self._queries(queries)
+        B = q.shape[0]
+        ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
+        p = make_params(k, 0, 0, lower, upper, 0, timeout_ms)
+        if allow is None:
+            check(load().lgpu_binary_search(self._h, _ptr(q), B, C.byref(p), _ptr(ids), _ptr(dist), _ptr(cnt)))
+        else:
+            bm = np.ascontiguousarray(allow, np.uint32)
+            if bm.size * 32 < allow_bits:
+                raise ValueError("allow bitmap shorter than allow_bits")
+            check(load().lgpu_binary_search_filtered(self._h, _ptr(q), B, C.byref(p), _ptr(bm), int(allow_bits),
+                                                     _ptr(ids), _ptr(dist), _ptr(cnt)))
+        return ids, dist, cnt
+
+    def _queries(self, queries) -> np.ndarray:
+        a = np.asarray(queries)
+        if a.ndim not in (1, 2) or a.shape[-1] != self.nbytes:
+            raise ValueError(f"binary queries must be [B, {self.nbytes}] or [{self.nbytes}], got shape {a.shape}")
+        if a.dtype != np.uint8:
+            if not (np.issubdtype(a.dtype, np.integer) or np.issubdtype(a.dtype, np.floating)) or (
+                    a.size and not (np.all(np.isfinite(a)) and np.all(a == np.round(a)) and a.min() >= 0 and
+                                    a.max() <= 255)):
+                raise ValueError("binary query components must be integers in [0, 255]")
+        return np.ascontiguousarray(a, np.uint8).reshape(-1, self.nbytes)
+
+    def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
+        """Device-pointer search (raw addresses; queries [B][nbytes] u8), enqueued on `stream`, not synchronised."""
+        check(load().lgpu_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
+
+
 def ivf_assign(centroids, vectors, metric: str = "l2", device: int = 0) -> np.ndarray:
     """Partition of every row = find_partitions(row, nprobes=1) with the search path's exact kernels."""
     c = np.ascontiguousarray(centroids, np.float32); v = np.ascontiguousarray(vectors, np.float32)
@@ -415,6 +479,16 @@ def debug_gemm(queries, vectors, device: int = 0) -> np.ndarray:
     q = np.ascontiguousarray(queries, np.float32); x = np.ascontiguousarray(vectors, np.float32)
     out = np.empty((q.shape[0], x.shape[0]), np.float32)
     check(load().lgpu_debug_gemm(_ptr(q), _ptr(x), q.shape[0], x.shape[0], q.shape[1], device, _ptr(out)))
+    return out
+
+
+def debug_hamming_gemm(queries, vectors, device: int = 0) -> np.ndarray:
+    """The binary tensor-core kernel alone: [B, N] u32 Hamming distances."""
+    q = np.ascontiguousarray(queries, np.uint8); x = np.ascontiguousarray(vectors, np.uint8)
+    if q.ndim != 2 or x.ndim != 2 or q.shape[1] != x.shape[1]:
+        raise ValueError("queries and vectors must be [rows, bytes] arrays with the same bytes per row")
+    out = np.empty((q.shape[0], x.shape[0]), np.uint32)
+    check(load().lgpu_debug_hamming_gemm(_ptr(q), _ptr(x), q.shape[0], x.shape[0], q.shape[1], device, _ptr(out)))
     return out
 
 

@@ -120,6 +120,7 @@ struct Workspace {
     DevBuf c_stats;                               // candidate-mode counters (profiling only)
     DevBuf c_work, c_wcnt, c_surv, c_exd, c_exi, c_exp;   // candidate mode: survivor work list and exact results
     DevBuf c_thr, c_slack, c_cnt, c_rec, c_key, c_last;          // filter scan (candidate mode): thresholds, bands, candidate lists
+    DevBuf hq, hq_pop, h_sample, h_list, h_cnt;   // binary search: padded queries, popc(q), sample distances, fix-up list
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -269,6 +270,19 @@ struct lgpu_flat {
     bool has_tc = false;
     bool has_ids = false, has_norms = false;
     std::mutex mu;
+    WorkspacePool pool;
+};
+
+// a packed binary vector column (fixed_size_list<uint8, nbytes>) searched by Hamming distance
+struct lgpu_binary {
+    std::atomic<int> refs{0};
+    int device = 0, num_sms = 0;
+    uint64_t nrows = 0;
+    uint32_t nbytes = 0, nbytes_pad = 0;   // caller's row bytes; stored row bytes (multiple of 32)
+    DevBuf vectors, pop, row_ids;          // [nrows][nbytes_pad] zero-padded rows, popc of each row, optional ids
+    DevBuf sample, sample_pop;             // every (nrows / nsample)-th row: the threshold sample of the list path
+    uint64_t nsample = 0;                  // 0: no sample (nrows <= HAM_SAMPLE)
+    bool has_ids = false;
     WorkspacePool pool;
 };
 
@@ -1038,6 +1052,151 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
     }
 }
 
+// ---- binary vectors (Hamming distance) ----
+// Paths, chosen from shape and request (DESIGN.md section 6):
+//   SIMT dense    ham_dense_kernel -> D[b][N] -> select mode 1.  N < HAM_TC_MIN_N, or fewer than HAM_TC_MIN_B queries
+//                 with N <= HAM_SAMPLE, prefilter or distance_range, LGPU_NO_TENSOR_CORE=1.
+//   wgmma dense   the b1 gemm_dist_kernel writes D[b][N] -> select mode 1 (N <= HAM_SAMPLE).
+//   wgmma list    N > HAM_SAMPLE, any batch size: sample pass -> threshold -> filtering pass -> select mode 2 -> dense
+//                 fix-up of the queries whose list overflowed (ham_topk_list).  On the H100 it beat the SIMT kernel at
+//                 every batch size measured, one query included: a single query's select over a dense row of N
+//                 columns runs on one SM.
+// Every path computes exact integer distances, so all three return the same rows.
+constexpr uint64_t HAM_SAMPLE = 65536;     // rows of the threshold sample
+constexpr uint32_t HAM_TC_MIN_B = 128;     // dense tensor-core path from this many queries (measured: SIMT faster at
+                                           // 64 queries x 60000 rows, wgmma at 256) ...
+constexpr uint64_t HAM_TC_MIN_N = 4096;    // ... and this many rows (not measured)
+
+// Candidate-list capacity of the list path.  Rows with d <= tau_q, tau_q the k-th smallest distance among the sample's
+// rows, number about k N / ns (more under ties): 4x that, at least 1024, at most 16384.
+static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
+{
+    const uint64_t want = 4 * (uint64_t)k * ((N + ns - 1) / ns);
+    uint32_t cap = 1024;
+    while (cap < want && cap < 16384) cap <<= 1;
+    return cap;
+}
+
+// One sub-batch through the tensor-core list path (Q: padded queries [B][nbytes_pad], qpop [B]).  The dense fix-up of
+// overflowed queries runs in chunks of `bf` queries over a [bf][N] matrix: one launch lists each chunk's flagged
+// queries, and each chunk's two launches return at once when its list is empty.
+static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
+                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, uint64_t *out_ids, float *out_dist,
+                          uint32_t *out_cnt)
+{
+    const uint64_t N = bx->nrows, ns = bx->nsample, lds = (ns + 3) & ~3ull, ld = (N + 3) & ~3ull;
+    const uint32_t nbp = bx->nbytes_pad;
+    const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    // 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest (an upper bound of the true k-th)
+    launch_ham_gemm(Q, bx->sample.p, bx->sample_pop.as<uint32_t>(), qpop, B, ns, nbp, ws->h_sample.as<float>(), lds,
+                    bx->num_sms, st);
+    SelectArgs sa{};
+    sa.mode = 1; sa.dense = ws->h_sample.as<float>(); sa.ncols = ns; sa.row_stride = lds; sa.B = B; sa.k = k;
+    sa.out_ids = ws->sbound.as<uint64_t>(); sa.out_dist = ws->t_dist.as<float>(); sa.out_count = ws->t_cnt.as<uint32_t>();
+    launch_select(sa, st);
+    launch_ham_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), B, k, ws->probe_A.as<float>(), st);
+    // 2. full pass: every row with d <= tau_q is appended as (position, id, distance); the distance is final
+    LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
+    GemmFilter flt{};
+    flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
+    flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap; flt.cand_s = ws->t_exact.as<float>();
+    launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
+    launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
+    // 3. top-k by (distance, id) of each list (an overflowed list is complete up to cap; its query is redone below)
+    SelectArgs sb{};
+    sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
+    sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0; sb.ncols_q = ws->amax.as<uint32_t>();
+    sb.B = B; sb.k = k; sb.out_ids = out_ids; sb.out_dist = out_dist; sb.out_count = out_cnt;
+    launch_select(sb, st);
+    // 4. dense fix-up of the overflowed queries only
+    launch_ham_flag_list(ws->flags.as<uint32_t>(), B, bf, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
+    for (uint32_t q0 = 0, c = 0; q0 < B; q0 += bf, c++) {
+        const uint32_t b = std::min(bf, B - q0);
+        launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld, bx->num_sms, st,
+                         ws->h_list.as<uint32_t>() + q0, ws->h_cnt.as<uint32_t>() + c);
+        SelectArgs sc{};
+        sc.mode = 1; sc.dense = ws->D.as<float>(); sc.ncols = N; sc.row_stride = ld; sc.col_ids = col_ids;
+        sc.B = b; sc.k = k; sc.out_ids = out_ids + (size_t)q0 * k; sc.out_dist = out_dist + (size_t)q0 * k;
+        sc.out_count = out_cnt + q0; sc.only = ws->flags.as<uint32_t>() + q0; sc.gate = ws->h_cnt.as<uint32_t>() + c;
+        launch_select(sc, st);
+    }
+}
+
+// d_q: raw queries [B][nbytes] in device memory
+void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *d_q, uint32_t B,
+                          const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
+                          RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
+{
+    const uint64_t N = bx->nrows, ld = (N + 3) & ~3ull;
+    const uint32_t nbp = bx->nbytes_pad, k = sp.k;
+    const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    const bool prof = profiling_enabled();
+    if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));
+    ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
+    launch_ham_pack(d_q, bx->nbytes, bx->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
+    const uint8_t *Q = ws->hq.as<uint8_t>();
+    const bool tc_ok = tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper;
+    const bool list = tc_ok && bx->nsample > 0;
+    const bool tc = list || (tc_ok && B >= HAM_TC_MIN_B && N >= HAM_TC_MIN_N);
+    const size_t budget = workspace_budget();
+    if (list) {
+        // Workspace, all inside LGPU_WS_BYTES: the fix-up matrix [bf][N] gets at most half the budget and 1 GiB (it is
+        // rarely used); the rest is split into sub-batches of bs queries, each holding its sample scores [bs][ns] and
+        // candidate lists [bs][cap] (at the default 8 GiB, 1024 queries x 10M rows run as one sub-batch).
+        const uint64_t ns = bx->nsample, lds = (ns + 3) & ~3ull;
+        const uint32_t cap = ham_list_cap(k, N, ns);
+        const uint32_t bf = (uint32_t)std::max<size_t>(1, std::min<size_t>(std::min<size_t>(budget / 2, (size_t)1 << 30) / (ld * 4), B));
+        const size_t per_q = lds * 4 + (size_t)cap * 20 + (size_t)k * 12 + 16;
+        const size_t left = budget > (size_t)bf * ld * 4 ? budget - (size_t)bf * ld * 4 : 0;
+        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
+        ws->h_sample.ensure((size_t)bs * lds * 4);
+        ws->t_dist.ensure((size_t)bs * k * 4); ws->sbound.ensure((size_t)bs * k * 8); ws->t_cnt.ensure((size_t)bs * 4);
+        ws->probe_A.ensure((size_t)bs * 4); ws->amax.ensure((size_t)bs * 4); ws->flags.ensure((size_t)bs * 4);
+        ws->t_pos.ensure((size_t)bs * cap * 8); ws->t_ids.ensure((size_t)bs * cap * 8);
+        ws->t_exact.ensure((size_t)bs * cap * 4);
+        ws->D.ensure((size_t)bf * ld * 4); ws->h_list.ensure((size_t)bs * 4);
+        ws->h_cnt.ensure((size_t)((bs + bf - 1) / bf) * 4);
+        for (uint32_t q0 = 0; q0 < B; q0 += bs) {
+            const uint32_t b = std::min(bs, B - q0);
+            if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
+            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, ws->hq_pop.as<uint32_t>() + q0, b, k, cap, bf,
+                          d_ids + (size_t)q0 * k, d_dist + (size_t)q0 * k, d_cnt + q0);
+            if (prof) {             // [0] list appends, [2] queries redone densely (over every sub-batch)
+                std::vector<uint32_t> cnt(b), fl(b);
+                LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->amax.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+                LGPU_CUDA(cudaMemcpyAsync(fl.data(), ws->flags.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+                LGPU_CUDA(cudaStreamSynchronize(st));
+                for (uint32_t q = 0; q < b; q++) { g_filter_stats[0] += cnt[q]; g_filter_stats[2] += fl[q] ? 1 : 0; }
+            }
+        }
+    } else {
+        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / std::max<size_t>(ld * 4, 4), B));
+        for (uint32_t q0 = 0; q0 < B; q0 += bs) {
+            const uint32_t b = std::min(bs, B - q0);
+            if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
+            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+            if (tc)
+                launch_ham_gemm(Q + (size_t)q0 * nbp, bx->vectors.p, bx->pop.as<uint32_t>(), ws->hq_pop.as<uint32_t>() + q0, b,
+                                N, nbp, ws->D.as<float>(), ld, bx->num_sms, st);
+            else
+                launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld,
+                                 bx->num_sms, st);
+            SelectArgs sa{};
+            sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = N; sa.row_stride = ld; sa.col_ids = col_ids;
+            sa.B = b; sa.k = k;
+            sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
+            sa.out_ids = d_ids + (size_t)q0 * k; sa.out_dist = d_dist + (size_t)q0 * k; sa.out_count = d_cnt + q0;
+            sa.allow = rf.bits; sa.allow_bits = rf.nbits;
+            launch_select(sa, st);
+        }
+    }
+    if (prof) {                     // [1] distances computed on the tensor cores, [3] queries
+        LGPU_CUDA(cudaStreamSynchronize(st));
+        g_filter_stats[1] = tc ? (uint64_t)B * (N + (list ? bx->nsample : 0)) : 0;
+        g_filter_stats[3] = B;
+    }
+}
+
 template <class F> int guarded(F &&f)
 {
     try { f(); return LGPU_OK; }
@@ -1073,25 +1232,26 @@ static bool graphs_enabled()
     return v == 1;
 }
 
-// host-buffer wrapper: stage in, run, stage out, synchronise.  `key` identifies the launch sequence
+// host-buffer wrapper: stage in, run, stage out, synchronise.  Queries are [B][dim] elements of T (f32 vectors, or the
+// bytes of packed binary vectors).  `key` identifies the launch sequence
 // (shapes + parameters): the second call with the same key is captured into a CUDA graph and later calls
 // replay it, which removes ~15 launch latencies from the synchronous end-to-end path.  Any device
 // (re)allocation anywhere in the process since the capture, profiling mode, or a failed capture falls back to
 // eager launches.
-template <class Run>
-void host_submit(WsLease &lease, const Deadline &deadline, const float *queries, uint32_t B, uint32_t dim, uint32_t k,
+template <class T, class Run>
+void host_submit(WsLease &lease, const Deadline &deadline, const T *queries, uint32_t B, uint32_t dim, uint32_t k,
                  uint64_t *out_ids, float *out_dist, uint32_t *out_count, const uint64_t (&key)[4], Run &&run,
                  bool allow_graph, bool sync)
 {
     Workspace *ws = lease.ws;
     cudaStream_t st = lease.st;
-    ws->q.ensure(std::max<size_t>((size_t)B * dim, 1) * 4);
+    ws->q.ensure(std::max<size_t>((size_t)B * dim, 1) * sizeof(T));
     ws->out_ids.ensure(std::max<size_t>((size_t)B * k, 1) * 8);
     ws->out_dist.ensure(std::max<size_t>((size_t)B * k, 1) * 4);
     ws->out_count.ensure(std::max<size_t>(B, 1) * 4);
-    LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * 4, cudaMemcpyHostToDevice, st));
+    LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * sizeof(T), cudaMemcpyHostToDevice, st));
     auto eager = [&] {
-        run(ws, st, ws->q.as<float>(), ws->out_ids.as<uint64_t>(), ws->out_dist.as<float>(), ws->out_count.as<uint32_t>(),
+        run(ws, st, ws->q.as<T>(), ws->out_ids.as<uint64_t>(), ws->out_dist.as<float>(), ws->out_count.as<uint32_t>(),
             deadline);
     };
     const bool same = memcmp(key, ws->graph_key, sizeof(key)) == 0;
@@ -1132,14 +1292,14 @@ void host_submit(WsLease &lease, const Deadline &deadline, const float *queries,
             if (g) cudaGraphDestroy(g);
             cudaGetLastError();
             ws->graph = nullptr;
-            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * 4, cudaMemcpyHostToDevice, st));
+            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * sizeof(T), cudaMemcpyHostToDevice, st));
             eager();
         } else {                                            // never try again with this workspace
             if (g) cudaGraphDestroy(g);
             cudaGetLastError();
             ws->graph = nullptr;
             ws->graph_state = -1;
-            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * 4, cudaMemcpyHostToDevice, st));
+            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * sizeof(T), cudaMemcpyHostToDevice, st));
             eager();
         }
     } else {                                                // captured, but a buffer moved since: capture again
@@ -1154,8 +1314,8 @@ void host_submit(WsLease &lease, const Deadline &deadline, const float *queries,
     if (sync) LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
-template <class Run>
-void host_call(WorkspacePool &pool, const float *queries, uint32_t B, uint32_t dim, uint32_t k, uint64_t *out_ids,
+template <class T, class Run>
+void host_call(WorkspacePool &pool, const T *queries, uint32_t B, uint32_t dim, uint32_t k, uint64_t *out_ids,
                float *out_dist, uint32_t *out_count, const uint64_t (&key)[4], uint32_t timeout_ms, Run &&run,
                bool allow_graph = true)
 {
@@ -1698,6 +1858,146 @@ int lgpu_flat_search_device(lgpu_flat *flh, int metric, const float *d_queries, 
         require_device(fl->device);
         WsLease lease(fl->pool, (cudaStream_t)cuda_stream, true);
         flat_search_device(fl.h, lease.ws, lease.st, metric, d_queries, B, *params, d_out_ids, d_out_dist, d_out_count);
+    });
+}
+
+int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, const uint64_t *row_ids, int device,
+                     lgpu_binary **out)
+{
+    lgpu_binary *bx = nullptr;
+    int rc = guarded([&] {
+        LGPU_REQUIRE(out != nullptr && nbytes > 0, "null argument / zero bytes per vector");
+        LGPU_REQUIRE((uint64_t)nbytes * 8 <= ((uint64_t)1 << 24), "binary vectors above 2^24 bits are not supported");
+        LGPU_REQUIRE(nrows == 0 || vectors != nullptr, "null vectors");
+        require_device(device);
+        bx = new lgpu_binary();
+        bx->device = device; bx->nrows = nrows; bx->nbytes = nbytes; bx->nbytes_pad = (nbytes + 31) & ~31u;
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        bx->num_sms = prop.multiProcessorCount;
+        const uint32_t nbp = bx->nbytes_pad;
+        bx->vectors.ensure(std::max<size_t>((size_t)nrows * nbp, 16));
+        bx->pop.ensure(std::max<size_t>((size_t)nrows * 4, 16));
+        if (nrows) {
+            DevBuf raw;
+            raw.ensure((size_t)nrows * nbytes);
+            LGPU_CUDA(cudaMemcpy(raw.p, vectors, (size_t)nrows * nbytes, cudaMemcpyHostToDevice));
+            launch_ham_pack(raw.as<uint8_t>(), nbytes, nbytes, nrows, bx->vectors.as<uint8_t>(), nbp, bx->pop.as<uint32_t>(),
+                            nullptr);
+        }
+        if (nrows > HAM_SAMPLE) {
+            const uint64_t stride = nrows / HAM_SAMPLE;
+            bx->nsample = HAM_SAMPLE;
+            bx->sample.ensure((size_t)HAM_SAMPLE * nbp);
+            bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
+            launch_ham_pack(bx->vectors.as<uint8_t>(), stride * nbp, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp,
+                            bx->sample_pop.as<uint32_t>(), nullptr);
+        }
+        LGPU_CUDA(cudaDeviceSynchronize());
+        if (row_ids && nrows) {
+            bx->row_ids.ensure((size_t)nrows * 8);
+            LGPU_CUDA(cudaMemcpy(bx->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
+            bx->has_ids = true;
+        }
+        register_handle(bx);
+        *out = bx;
+    });
+    if (rc != LGPU_OK && bx) delete bx;
+    return rc;
+}
+
+void lgpu_binary_close(lgpu_binary *bx)
+{
+    if (!retire_handle(bx)) return;
+    cudaSetDevice(bx->device);
+    cudaDeviceSynchronize();
+    delete bx;
+}
+
+static void check_binary_call(const void *q, uint32_t B, const lgpu_search_params *p, const void *a, const void *b,
+                              const void *c)
+{
+    check_params(p);
+    LGPU_REQUIRE(B == 0 || (q && a && b && c), "null buffer");
+}
+
+int lgpu_binary_search(lgpu_binary *bxh, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
+                       uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return guarded([&] {
+        HandleRef<lgpu_binary> bx(bxh, "binary");
+        check_binary_call(queries, B, params, out_ids, out_dist, out_count);
+        if (B == 0) return;
+        require_device(bx->device);
+        uint64_t key[4];
+        make_key(key, 0xb1a7ull, B, *params);
+        host_call(bx->pool, queries, B, bx->nbytes, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
+                  [&](Workspace *ws, cudaStream_t st, const uint8_t *dq, uint64_t *di, float *dd, uint32_t *dc,
+                      const Deadline &dl) { binary_search_device(bx.h, ws, st, dq, B, *params, di, dd, dc, RowFilter(), &dl); });
+    });
+}
+
+int lgpu_binary_search_filtered(lgpu_binary *bxh, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
+                                const uint32_t *allow, uint64_t allow_bits, uint64_t *out_ids, float *out_dist,
+                                uint32_t *out_count)
+{
+    return guarded([&] {
+        HandleRef<lgpu_binary> bx(bxh, "binary");
+        check_binary_call(queries, B, params, out_ids, out_dist, out_count);
+        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
+        if (B == 0) return;
+        require_device(bx->device);
+        uint64_t key[4];
+        make_key(key, 0xb1b7ull, B, *params);
+        host_call(bx->pool, queries, B, bx->nbytes, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
+                  [&](Workspace *ws, cudaStream_t st, const uint8_t *dq, uint64_t *di, float *dd, uint32_t *dc,
+                      const Deadline &dl) {
+                      const size_t words = (size_t)((allow_bits + 31) / 32);
+                      ws->allow.ensure(std::max<size_t>(words, 1) * 4);
+                      if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
+                      RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
+                      binary_search_device(bx.h, ws, st, dq, B, *params, di, dd, dc, rf, &dl);
+                  }, false);
+    });
+}
+
+int lgpu_binary_search_device(lgpu_binary *bxh, const uint8_t *d_queries, uint32_t B, const lgpu_search_params *params,
+                              uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream)
+{
+    return guarded([&] {
+        HandleRef<lgpu_binary> bx(bxh, "binary");
+        check_binary_call(d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
+        if (B == 0) return;
+        require_device(bx->device);
+        WsLease lease(bx->pool, (cudaStream_t)cuda_stream, true);
+        binary_search_device(bx.h, lease.ws, lease.st, d_queries, B, *params, d_out_ids, d_out_dist, d_out_count);
+    });
+}
+
+int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint32_t B, uint64_t N, uint32_t nbytes,
+                            int device, uint32_t *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(nbytes > 0 && (uint64_t)nbytes * 8 <= ((uint64_t)1 << 24), "bytes per vector out of range");
+        LGPU_REQUIRE((B == 0 || N == 0) || (queries && vectors && out), "null buffer");
+        require_device(device);
+        if (B == 0 || N == 0) return;
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        const uint32_t nbp = (nbytes + 31) & ~31u;
+        DevBuf rq, rx, q, x, qp, xp, d;
+        rq.ensure((size_t)B * nbytes); rx.ensure((size_t)N * nbytes);
+        q.ensure((size_t)B * nbp); x.ensure((size_t)N * nbp); qp.ensure((size_t)B * 4); xp.ensure((size_t)N * 4);
+        d.ensure((size_t)B * N * 4);
+        LGPU_CUDA(cudaMemcpy(rq.p, queries, (size_t)B * nbytes, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(rx.p, vectors, (size_t)N * nbytes, cudaMemcpyHostToDevice));
+        launch_ham_pack(rq.as<uint8_t>(), nbytes, nbytes, B, q.as<uint8_t>(), nbp, qp.as<uint32_t>(), nullptr);
+        launch_ham_pack(rx.as<uint8_t>(), nbytes, nbytes, N, x.as<uint8_t>(), nbp, xp.as<uint32_t>(), nullptr);
+        launch_ham_gemm(q.p, x.p, xp.as<uint32_t>(), qp.as<uint32_t>(), B, N, nbp, d.as<float>(), N, prop.multiProcessorCount,
+                        nullptr);
+        std::vector<float> h((size_t)B * N);
+        LGPU_CUDA(cudaMemcpy(h.data(), d.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < h.size(); i++) out[i] = (uint32_t)h[i];
     });
 }
 

@@ -109,21 +109,72 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
+// D[64 x 128] (+)= popc(A[64 x 256] AND B[128 x 256]^T), both b1 K-major in shared memory (32 bytes of K per row, the
+// same bytes as one k16 bf16 slice, so the descriptors and the fragment layout are those of wgmma_m64n128k16)
+__device__ __forceinline__ void wgmma_m64n128k256_b1(int (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k256.s32.b1.b1.and.popc "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p;\n\t"
+        "}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
 // keeps the compiler from moving accumulator reads above the wgmma.wait_group that makes them valid
 __device__ __forceinline__ void fence_acc(float (&d)[64])
 {
 #pragma unroll
     for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
+__device__ __forceinline__ void fence_acc(int (&d)[64])
+{
+#pragma unroll
+    for (int i = 0; i < 64; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// MMA / score policies of gemm_dist_kernel.  Bf16Dist: bf16 operands, per-row term |x|^2 (f32),
+// S = |x|^2 - 2 acc (the shortlist score above).  B1Hamming: packed bits (rows zero-padded to 32 bytes), per-row
+// term popc(x) (s32), S = popc(q) + popc(x) - 2 popc(q AND x) = popc(q XOR x) exactly: every term is an integer
+// below 2^24, so S is the final Hamming distance and needs no re-score.
+struct Bf16Dist {
+    static constexpr bool BIN = false;
+    static constexpr int K_BOX = GK;          // tensor-map elements per stage row (128 bytes)
+    using Acc = float; using Row = float; using Row2 = float2; using Filter = GemmFilter;
+    __device__ static __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k16(d, a, b, acc); }
+    __device__ static __forceinline__ int qterm(const GemmFilter &, uint32_t) { return 0; }
+    __device__ static __forceinline__ float score(float xn, float acc, int) { return xn - 2.0f * acc; }
+};
+struct B1Hamming {
+    static constexpr bool BIN = true;
+    static constexpr int K_BOX = 2 * GK;      // the map is over bytes
+    using Acc = int; using Row = int; using Row2 = int2; using Filter = HamFilter;
+    __device__ static __forceinline__ void mma(int (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k256_b1(d, a, b, acc); }
+    __device__ static __forceinline__ int qterm(const HamFilter &f, uint32_t q) { return __ldg(f.qpop + q); }
+    __device__ static __forceinline__ float score(int xn, int acc, int pq) { return (float)(pq + xn - 2 * acc); }
+};
 
 // LIST: the filtering epilogue for DENSE hit rates (coarse step at many lists), see the epilogue; a separate
 // instantiation so that the dense / sparse-filter kernel of the flat path and of the small coarse problems carries
-// none of its code.
-template <bool LIST>
+// none of its code.  Pol: Bf16Dist or B1Hamming (above).
+template <bool LIST, class Pol>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
-                 const float *__restrict__ xnorm2, float *__restrict__ out, uint64_t ld_out, uint32_t B, uint64_t N,
-                 uint32_t num_kb, GemmFilter flt)
+                 const typename Pol::Row *__restrict__ xnorm2, float *__restrict__ out, uint64_t ld_out, uint32_t B,
+                 uint64_t N, uint32_t num_kb, typename Pol::Filter flt)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     extern __shared__ unsigned char smem_raw[];
@@ -155,8 +206,8 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                 for (uint32_t kb = 0; kb < num_kb; kb++) {
                     mbar_wait(empty_bar + 8 * stage, phase ^ 1);
                     mbar_expect_tx(full_bar + 8 * stage, A_STAGE_BYTES + B_STAGE_BYTES);
-                    tma_load_2d(smem_a + stage * A_STAGE_BYTES, &tmap_q, full_bar + 8 * stage, (int)(kb * GK), (int)(m_tile * GM));
-                    tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_x, full_bar + 8 * stage, (int)(kb * GK), (int)(n_tile * GN));
+                    tma_load_2d(smem_a + stage * A_STAGE_BYTES, &tmap_q, full_bar + 8 * stage, (int)(kb * Pol::K_BOX), (int)(m_tile * GM));
+                    tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_x, full_bar + 8 * stage, (int)(kb * Pol::K_BOX), (int)(n_tile * GN));
                     if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -169,9 +220,9 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const uint32_t wg = threadIdx.x >> 7;
     const bool leader = (threadIdx.x & 127) == 0;
     uint32_t stage = 0, phase = 0;
-    float acc[64];
+    typename Pol::Acc acc[64];
 #pragma unroll
-    for (int i = 0; i < 64; i++) acc[i] = 0.f;
+    for (int i = 0; i < 64; i++) acc[i] = 0;
     for (uint64_t t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const uint32_t m_tile = (uint32_t)(t % num_m);
         const uint64_t n_tile = t / num_m;
@@ -179,16 +230,16 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         const uint32_t r0 = m_tile * GM + wg * 64 + (uint32_t)(warp & 3) * 16 + (uint32_t)(lane >> 2);
         const uint64_t c0 = n_tile * GN + 2 * (uint32_t)(lane & 3);
         // |x|^2 of the thread's 32 columns, requested before the MMAs so that the loads land under them; past N: 0
-        float xn[32];
+        typename Pol::Row xn[32];
 #pragma unroll
         for (int j = 0; j < 16; j++) {
             const uint64_t x = c0 + 8 * j;
             if (x + 1 < N) {
-                const float2 v = __ldg(reinterpret_cast<const float2 *>(xnorm2 + x));
+                const typename Pol::Row2 v = __ldg(reinterpret_cast<const typename Pol::Row2 *>(xnorm2 + x));
                 xn[2 * j] = v.x; xn[2 * j + 1] = v.y;
             } else {
-                xn[2 * j] = x < N ? __ldg(xnorm2 + x) : 0.f;
-                xn[2 * j + 1] = 0.f;
+                xn[2 * j] = x < N ? __ldg(xnorm2 + x) : 0;
+                xn[2 * j + 1] = 0;
             }
         }
         uint32_t prev = 0;
@@ -198,8 +249,8 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
             const uint64_t db = make_kmajor_sw128_desc(smem_b + stage * B_STAGE_BYTES);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < GK / 16; k++)                            // +32 B (>>4 = 2) per K=16 slice
-                wgmma_m64n128k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+            for (int k = 0; k < GK / 16; k++)                            // +32 B (>>4 = 2) per K=16 (b1: K=256) slice
+                Pol::mma(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
             wgmma_commit();
             wgmma_wait<1>();                                             // the previous stage's MMAs have retired
             if (kb > 0 && leader) mbar_arrive(empty_bar + 8 * prev);
@@ -220,12 +271,13 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                 const uint32_t q = r0 + 8 * h;
                 const bool live = q < B;
                 const float thr = live ? flt.thr[q] : 0.f;
+                const int pq = live ? Pol::qterm(flt, q) : 0;
                 uint32_t hit = 0;                                        // bit 2 j + e: column c0 + 8 j + e passes
 #pragma unroll
                 for (int j = 0; j < 16; j++)
 #pragma unroll
                     for (int e = 0; e < 2; e++)
-                        if (live && c0 + 8 * j + e < N && xn[2 * j + e] - 2.0f * acc[4 * j + 2 * h + e] <= thr)
+                        if (live && c0 + 8 * j + e < N && Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], pq) <= thr)
                             hit |= 1u << (2 * j + e);
                 const uint32_t n = __popc(hit);
                 uint32_t incl = n, v;                                    // inclusive prefix over the row's 4 lanes
@@ -243,7 +295,9 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                             if ((hit >> (2 * j + e)) & 1u) {
                                 if (slot < flt.cap) {
                                     flt.cand_pos[(size_t)q * flt.cap + slot] = c0 + 8 * j + e;
-                                    flt.cand_s[(size_t)q * flt.cap + slot] = xn[2 * j + e] - 2.0f * acc[4 * j + 2 * h + e];
+                                    flt.cand_s[(size_t)q * flt.cap + slot] = Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], pq);
+                                    if constexpr (Pol::BIN)
+                                        flt.cand_ids[(size_t)q * flt.cap + slot] = flt.col_ids ? flt.col_ids[c0 + 8 * j + e] : c0 + 8 * j + e;
                                 }
                                 slot++;
                             }
@@ -251,7 +305,7 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
             }
             continue;
         }
-        if (flt.thr) {
+        if (!Pol::BIN && flt.thr) {
             // filtering epilogue: nothing dense is written; scores not above the per-query threshold are appended to the
             // query's candidate list (rare: ~1e-4 of the columns)
 #pragma unroll
@@ -264,7 +318,7 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
                         const uint64_t x = c0 + 8 * j + e;
-                        if (x < N && xn[2 * j + e] - 2.0f * acc[4 * j + 2 * h + e] <= thr) {
+                        if (x < N && Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], 0) <= thr) {
                             const uint32_t slot = atomicAdd(flt.count + q, 1u);
                             if (slot < flt.cap) {
                                 flt.cand_pos[(size_t)q * flt.cap + slot] = x;
@@ -282,10 +336,12 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
             const uint32_t q = r0 + 8 * h;
             if (q >= B) continue;
             float *orow = out + (size_t)q * ld_out;
+            const int pq = Pol::qterm(flt, q);
 #pragma unroll
             for (int j = 0; j < 16; j++) {
                 const uint64_t x = c0 + 8 * j;
-                const float s0 = xn[2 * j] - 2.0f * acc[4 * j + 2 * h], s1 = xn[2 * j + 1] - 2.0f * acc[4 * j + 2 * h + 1];
+                const float s0 = Pol::score(xn[2 * j], acc[4 * j + 2 * h], pq);
+                const float s1 = Pol::score(xn[2 * j + 1], acc[4 * j + 2 * h + 1], pq);
                 if (vec && x + 1 < N) {
                     *reinterpret_cast<float2 *>(orow + x) = make_float2(s0, s1);
                 } else {
@@ -346,15 +402,16 @@ EncodeTiledFn get_encode_fn()
     return fn;
 }
 
-// bf16 row-major [rows][d] matrix, box = box_rows x 64 elements, 128-byte swizzle, OOB = zeros
-CUtensorMap make_map(const void *ptr, uint64_t rows, uint32_t d, uint32_t box_rows)
+// bf16 row-major [rows][d] matrix (bytes: u8 [rows][d]), box = box_rows x 128 bytes, 128-byte swizzle, OOB = zeros
+CUtensorMap make_map(const void *ptr, uint64_t rows, uint32_t d, uint32_t box_rows, bool bytes = false)
 {
     CUtensorMap m;
     cuuint64_t dims[2] = {d, rows};
-    cuuint64_t strides[1] = {(cuuint64_t)d * 2};
-    cuuint32_t box[2] = {(cuuint32_t)GK, box_rows};
+    cuuint64_t strides[1] = {(cuuint64_t)d * (bytes ? 1 : 2)};
+    cuuint32_t box[2] = {(cuuint32_t)(bytes ? 2 * GK : GK), box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(ptr), dims, strides, box, estr,
+    CUresult r = get_encode_fn()(&m, bytes ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                                 const_cast<void *>(ptr), dims, strides, box, estr,
                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -546,9 +603,28 @@ void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint3
     GemmFilter flt{};
     if (filter) flt = *filter;
     const bool list = flt.thr && flt.cand_s;                  // dense hit rates: one reservation per row and tile
-    auto kern = list ? gemm_dist_kernel<true> : gemm_dist_kernel<false>;
+    auto kern = list ? gemm_dist_kernel<true, Bf16Dist> : gemm_dist_kernel<false, Bf16Dist>;
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, xnorm2, out, ld_out, B, N, (uint32_t)((d + GK - 1) / GK), flt); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_ham_gemm(const void *Qp, const void *Xp, const uint32_t *xpop, const uint32_t *qpop, uint32_t B, uint64_t N,
+                     uint32_t nbytes_pad, float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter)
+{
+    if (B == 0 || N == 0) return;
+    LGPU_REQUIRE(nbytes_pad % 32 == 0, "binary rows must be padded to a multiple of 32 bytes");
+    CUtensorMap mq = make_map(Qp, B, nbytes_pad, GM, true);
+    CUtensorMap mx = make_map(Xp, N, nbytes_pad, GN, true);
+    const uint64_t tiles = (uint64_t)((B + GM - 1) / GM) * ((N + GN - 1) / GN);
+    const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)num_sms);
+    HamFilter flt{};
+    if (filter) static_cast<GemmFilter &>(flt) = *filter;
+    flt.qpop = reinterpret_cast<const int *>(qpop);
+    auto kern = flt.thr ? gemm_dist_kernel<true, B1Hamming> : gemm_dist_kernel<false, B1Hamming>;
+    LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
+    launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, reinterpret_cast<const int *>(xpop), out, ld_out,
+             B, N, (uint32_t)((nbytes_pad + 2 * GK - 1) / (2 * GK)), flt); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

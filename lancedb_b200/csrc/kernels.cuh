@@ -242,6 +242,34 @@ struct GemmFilter {
 };
 void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint32_t B, uint64_t N, uint32_t d,
                       float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter = nullptr);
+// the binary (Hamming) form of the same kernel: the GemmFilter fields plus popc(q) of every query
+struct HamFilter : GemmFilter {
+    const int *qpop;              // [B]
+};
+// out[q][x] = popc(Q[q] XOR X[x]) as f32 (exact), Q / X packed bits [B | N][nbytes_pad] (zero-padded to a multiple of
+// 32 bytes), xpop / qpop = popc of each row (wgmma m64n128k256 .and.popc + TMA).  With a filter (thr, count, cand_pos,
+// cand_ids, cand_s, cap required): nothing dense is written; every column with distance <= thr[q] is appended as
+// (position, id, distance) to the query's list (count may exceed cap: those appends are dropped).
+void launch_ham_gemm(const void *Qp, const void *Xp, const uint32_t *xpop, const uint32_t *qpop, uint32_t B, uint64_t N,
+                     uint32_t nbytes_pad, float *out, uint64_t ld_out, int num_sms, cudaStream_t st,
+                     const GemmFilter *filter = nullptr);
+
+// ---------------- binary vectors, SIMT side (hamming.cu) --------------------------------
+// dst[r] = src row r (src rows `src_stride` bytes apart, nbytes used) zero-padded to nbytes_pad; pop[r] = its popcount
+void launch_ham_pack(const uint8_t *src, uint64_t src_stride, uint32_t nbytes, uint64_t n, uint8_t *dst,
+                     uint32_t nbytes_pad, uint32_t *pop, cudaStream_t st);
+// D[q][x] = popc(Q[q] XOR X[x]) as f32 for x < N (LOP3 + POPC over 32-bit words; rows padded to a multiple of 32
+// bytes).  With qlist / qcount (device): only the *qcount queries qlist[0..) are computed (the fix-up of overflowed
+// queries; nothing runs when the count is 0), otherwise queries 0..B-1.
+void launch_ham_dense(const uint8_t *Q, const uint8_t *X, uint32_t B, uint64_t N, uint32_t nbytes_pad, float *D,
+                      uint64_t ldD, int num_sms, cudaStream_t st, const uint32_t *qlist = nullptr,
+                      const uint32_t *qcount = nullptr);
+// the flagged queries of each chunk of `chunk` queries: list[c chunk + i], i < count[c], = chunk-local index (one block)
+void launch_ham_flag_list(const uint32_t *flags, uint32_t B, uint32_t chunk, uint32_t *list, uint32_t *count,
+                          cudaStream_t st);
+// thr[q] = dist[q][k-1] when cnt[q] >= k, else +inf (the sample's k-th smallest distance, an upper bound of the k-th
+// smallest over all rows)
+void launch_ham_threshold(const float *dist, const uint32_t *cnt, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
 // filtering epilogue on an existing dense score matrix D[B][ld] (see gemm.cu)
 void launch_filter_dense(const float *D, uint64_t ld, uint32_t B, uint64_t N, const GemmFilter &flt, cudaStream_t st);
 void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,

@@ -20,7 +20,11 @@ from .index import IvfPqIndexData, train_ivf_pq
 from .query import LanceVectorQueryBuilder
 
 
-def _to_arrow_table(data) -> pa.Table:
+def _to_arrow_table(data, schema: Optional[pa.Schema] = None) -> pa.Table:
+    """`data` as an arrow table; with `schema`, built against it (a fixed_size_list<uint8> field holds packed binary
+    vectors, not the float32 lists that lists of numbers become without one)."""
+    if schema is not None:
+        return _to_arrow_table(data).select(schema.names).cast(schema)
     if isinstance(data, pa.Table):
         return data
     if isinstance(data, dict):
@@ -54,7 +58,22 @@ def _to_arrow_table(data) -> pa.Table:
 
 def _vector_columns(schema: pa.Schema) -> List[str]:
     return [f.name for f in schema if pa.types.is_fixed_size_list(f.type) and
-            (pa.types.is_floating(f.type.value_type))]
+            (pa.types.is_floating(f.type.value_type) or pa.types.is_uint8(f.type.value_type))]
+
+
+def _is_binary_type(t: pa.DataType) -> bool:
+    """fixed_size_list<uint8, nbytes>: packed binary vectors, searched by Hamming distance."""
+    return pa.types.is_fixed_size_list(t) and pa.types.is_uint8(t.value_type)
+
+
+def binary_query(query) -> np.ndarray:
+    """Query components for a binary column: integers in [0, 255] (checked, not wrapped as a cast would) -> uint8."""
+    a = np.asarray(query)
+    if a.dtype == object or not (np.issubdtype(a.dtype, np.integer) or np.issubdtype(a.dtype, np.floating)):
+        raise ValueError("a query on a binary vector column must hold integers in [0, 255]")
+    if a.size and not (np.all(np.isfinite(a)) and np.all(a == np.round(a)) and a.min() >= 0 and a.max() <= 255):
+        raise ValueError("a query on a binary vector column must hold integers in [0, 255]")
+    return a.astype(np.uint8)
 
 
 class Table:
@@ -63,6 +82,7 @@ class Table:
         self._data = data
         self._device = device
         self._flat: Dict[str, _native.GpuFlat] = {}
+        self._binary: Dict[str, _native.GpuBinary] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
         self._index_data: Dict[str, IvfPqIndexData] = {}
 
@@ -103,6 +123,13 @@ class Table:
     def _dim(self, column: str) -> int:
         return self._data.schema.field(column).type.list_size
 
+    def _is_binary(self, column: str) -> bool:
+        return _is_binary_type(self._data.schema.field(column).type)
+
+    def _binary_vectors(self, column: str) -> np.ndarray:
+        col = self._data.column(column).combine_chunks()
+        return np.asarray(col.flatten().to_numpy(zero_copy_only=False), np.uint8).reshape(-1, col.type.list_size)
+
     # ---- index build (parameters of Index::IvfPq; training itself is not the hot path) ----
     def create_index(self, metric: str = "l2", num_partitions: Optional[int] = None,
                      num_sub_vectors: Optional[int] = None, vector_column_name: Optional[str] = None,
@@ -113,6 +140,8 @@ class Table:
         if num_bits != 8:
             raise ValueError("only num_bits=8 is supported")
         column = vector_column_name or self._infer_vector_column(None)
+        if self._is_binary(column):
+            raise NotImplementedError("no index over binary vectors on the GPU path: search them flat (hamming)")
         if column in self._index and not replace:
             raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")   # python/python/tests/test_index.py:357
         dev = None
@@ -183,6 +212,18 @@ class Table:
         allow, allow_bits = None, 0
         if allow_mask is not None:                 # prefilter: row-id allow-list as the C ABI's bitmap
             allow, allow_bits = _native.mask_bitmap(allow_mask), int(len(allow_mask))
+        if self._is_binary(column):                # rust/lancedb/src/table/query.rs:229-236 (is_binary)
+            if distance_type is not None and distance_type != "hamming":
+                raise ValueError(f"distance type {distance_type!r} is not supported on binary column {column!r}: "
+                                 "use 'hamming'")
+            q = binary_query(queries)             # the builder's f32 copy: integers are exact up to 2^24
+            bx = self._binary.get(column)
+            if bx is None:
+                bx = self._binary[column] = _native.GpuBinary(self._binary_vectors(column), device=self._device)
+            return bx.search(q, k=k, lower=lower, upper=upper, allow=allow, allow_bits=allow_bits, timeout_ms=timeout_ms)
+        if distance_type == "hamming":
+            raise ValueError(f"distance type 'hamming' needs a binary (fixed_size_list<uint8>) column; {column!r} "
+                             "holds floats")
         idx = self._index.get(column) if use_index else None
         if idx is not None:
             if distance_type is not None and distance_type != idx.metric:
@@ -223,7 +264,7 @@ class DBConnection:
             if schema is None:
                 raise ValueError("Either data or schema must be provided")
             data = schema.empty_table()                      # an empty table is searchable (returns no rows)
-        t = Table(name, _to_arrow_table(data), self._device)
+        t = Table(name, _to_arrow_table(data, schema), self._device)
         self._tables[name] = t
         return t
 
