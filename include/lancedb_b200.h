@@ -271,6 +271,13 @@ int lgpu_debug_coarse(lgpu_index *ix, const float *queries, uint32_t B, uint32_t
  * buffers; out has n_p floats) -- exercises the LUT build + code scan kernels */
 int lgpu_debug_partition_distances(lgpu_index *ix, const float *query, uint32_t part,
                                    float *out);
+/* the filter scan (dense mode) for B queries and their nprobes nearest partitions, instead of a search
+ * result (host buffers): out_parts [B][nprobes] the probed partitions (UINT32_MAX = unused slot),
+ * out_L [B][nprobes][ld] the lower bound L the scan kernel computed for row r < min(n_p, ld) of the slot's
+ * partition, out_W / out_E [B] the band W, E of every query (unscaled: the exact distance lies in
+ * [L - s E, L + s (W + E)], s = 0.5 for cosine, else 1), out_bad [B] 1 when the query goes to the exact path */
+int lgpu_debug_filter_bounds(lgpu_index *ix, const float *queries, uint32_t B, uint32_t nprobes, uint64_t ld,
+                             uint32_t *out_parts, float *out_L, float *out_W, float *out_E, uint32_t *out_bad);
 /* the tensor-core shortlist GEMM alone: out[q][x] = |x|^2 - 2 bf16(Q[q]).bf16(X[x]) (host buffers,
  * out is [B][N] f32); dim must be a multiple of 8 */
 int lgpu_debug_gemm(const float *queries, const float *vectors, uint32_t B, uint64_t N, uint32_t dim,

@@ -30,7 +30,7 @@ EXPORTS = [
     "lgpu_comm_last_stage_ms",
     "lgpu_flat_open", "lgpu_flat_close", "lgpu_flat_search", "lgpu_flat_search_filtered", "lgpu_flat_search_device",
     "lgpu_ivf_assign", "lgpu_pq_encode", "lgpu_kmeans_train", "lgpu_pq_train",
-    "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_gemm", "lgpu_last_stage_ms", "lgpu_set_profiling",
+    "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_filter_bounds", "lgpu_debug_gemm", "lgpu_last_stage_ms", "lgpu_set_profiling",
     "lgpu_kernel_launch_count", "lgpu_last_filter_stats",
     "lgpu_binary_open", "lgpu_binary_close", "lgpu_binary_search", "lgpu_binary_search_filtered",
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
@@ -111,6 +111,7 @@ def load():
     lib.lgpu_flat_search_device.argtypes = [vp, i32, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_debug_coarse.argtypes = [vp, vp, u32, u32, vp, vp]
     lib.lgpu_debug_partition_distances.argtypes = [vp, vp, u32, vp]
+    lib.lgpu_debug_filter_bounds.argtypes = [vp, vp, u32, u32, C.c_uint64, vp, vp, vp, vp, vp]
     lib.lgpu_debug_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
     lib.lgpu_last_stage_ms.argtypes = [vp]
     lib.lgpu_set_profiling.argtypes = [i32]
@@ -245,6 +246,19 @@ class GpuIvfPq:
         parts = np.empty((B, nprobes), np.uint32); dists = np.empty((B, nprobes), np.float32)
         check(load().lgpu_debug_coarse(self._h, _ptr(q), B, nprobes, _ptr(parts), _ptr(dists)))
         return parts, dists
+
+    def debug_filter_bounds(self, queries, nprobes, ld):
+        """The dense filter scan's own numbers: (parts [B, nprobes] u32, L [B, nprobes, ld] f32 with row r < n_p of
+        the slot's partition valid, W [B], E [B] f32 (unscaled), bad [B] u32) -- see lgpu_debug_filter_bounds."""
+        q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
+        B = q.shape[0]
+        nprobes = min(nprobes, self.nlist)
+        parts = np.empty((B, nprobes), np.uint32)
+        L = np.full((B, nprobes, max(int(ld), 1)), np.nan, np.float32)
+        W, E, bad = np.empty(B, np.float32), np.empty(B, np.float32), np.empty(B, np.uint32)
+        check(load().lgpu_debug_filter_bounds(self._h, _ptr(q), B, nprobes, L.shape[2], _ptr(parts), _ptr(L), _ptr(W),
+                                              _ptr(E), _ptr(bad)))
+        return parts, L, W, E, bad
 
     def debug_partition_distances(self, query, part, n_p):
         q = np.ascontiguousarray(query, np.float32).reshape(self.dim)

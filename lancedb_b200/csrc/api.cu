@@ -563,11 +563,21 @@ void check_params(const lgpu_search_params *p)
         LGPU_REQUIRE((uint64_t)p->k * p->refine_factor <= SELECT_KMAX, "limit*refine_factor above 2048 is not supported");
 }
 
+// lgpu_debug_filter_bounds: the dense filter scan's own lower bounds and band, copied out instead of a result
+struct FilterDebug {
+    float *L;                     // host [B][nprobes][ld]: L of row r of the slot's partition at r < n_p
+    uint64_t ld;
+    uint32_t *parts;              // host [B][nprobes]
+    float *W, *E;                 // host [B]: scan_band, unscaled
+    uint32_t *bad;                // host [B]
+    bool ran = false;             // the filter scan ran (false: the index or the request cannot use it)
+};
+
 // one sub-batch of an IVF_PQ search, everything device-side on `st`
 void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
                    const lgpu_search_params &sp, uint32_t nprobes, uint64_t *d_ids, float *d_dist,
                    uint32_t *d_cnt, bool prof, const uint64_t *forced_probes = nullptr, RowFilter rf = RowFilter(),
-                   const uint32_t *only = nullptr)
+                   const uint32_t *only = nullptr, FilterDebug *dbg = nullptr)
 {
     // `only` (device, [B]): redo just the flagged queries (maximum_nprobes widening) -- exact kernels, outputs of
     // the other queries are left untouched
@@ -597,7 +607,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
                             small_scan_smem(ix->m, dim) <= 200 * 1024 &&
                             (size_t)slots * ix->pad_prefix[1] * 4 <= workspace_budget();
     const bool filter_scan = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && !forced_probes &&
-                             d_ids && kp > kk && ix->m <= 512 && !only && !small_path;
+                             (d_ids || dbg) && kp > kk && ix->m <= 512 && !only && !small_path;
     if (filter_scan) {
         ws->qt.ensure((size_t)B * ix->nch * 256 * 16); ws->qt_mm.ensure((size_t)B * ix->nch * 8 * 8);
         ws->qt_step.ensure((size_t)B * 4); ws->qt_base.ensure((size_t)B * 4); ws->qt_bad.ensure((size_t)B * 4);
@@ -815,7 +825,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
             sc.probe_A = ws->probe_A.as<float>(); sc.row_R = ix->row_R.as<float>();
         }
         launch_probe_terms(ws->probe_dist.as<float>(), qsearch, B, nprobes, dim, dot ? nullptr : ws->probe_A.as<float>(),
-                           dot ? nullptr : ws->amax.as<float>(), ws->qn2.as<float>(), st);
+                           dot ? nullptr : ws->amax.as<float>(), ws->qn2.as<float>(), ws->qt_base.as<float>(),
+                           ws->qt_bad.as<uint32_t>(), st);
         sc.qt = ws->qt.as<uint4>(); sc.qt_step = ws->qt_step.as<float>(); sc.qt_base = ws->qt_base.as<float>();
         const float mscale = ix->metric == LGPU_COSINE ? 0.5f : 1.0f;
         // candidate mode (no prefilter, k <= 32): the scanners threshold the rows themselves, nothing dense is written
@@ -845,13 +856,13 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
             const double conc = (double)np_eff * tiles_part * std::min(1.0, 2.0 * ix->num_sms / total);
             cand_fits = conc * kk <= 2.0 * cap;
         }
-        const bool cand_mode = !rf.bits && kk <= modes.cand_kmax && !modes.dense_forced && cand_fits;
+        const bool cand_mode = !rf.bits && kk <= modes.cand_kmax && !modes.dense_forced && cand_fits && !dbg;
         if (cand_mode) {
             ws->c_thr.ensure((size_t)B * 4); ws->c_slack.ensure((size_t)B * 4); ws->c_cnt.ensure((size_t)B * 4);
             ws->c_rec.ensure((size_t)B * cap * sizeof(CandRec));
             ws->c_key.ensure((size_t)B * cap * 4); ws->c_last.ensure((size_t)B * 4);
             launch_cand_prepare(ws->qt_step.as<float>(), ws->sbound.as<float>(), dot ? nullptr : ws->amax.as<float>(),
-                                dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, B,
+                                dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B,
                                 ws->c_slack.as<float>(), ws->c_thr.as<uint32_t>(), ws->c_cnt.as<uint32_t>(),
                                 ws->c_last.as<uint32_t>(), ws->c_key.as<uint32_t>(), cap, st);
             sc.cand_key = ws->c_key.as<uint32_t>(); sc.cand_last = ws->c_last.as<uint32_t>();
@@ -885,6 +896,30 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         } else {
         launch_scan3(sc, ix->num_sms, st);
         mark();
+        if (dbg) {
+            // W, E of every query (the band the consumers use) and the scan's own L, per probe slot
+            ws->s_exact.ensure((size_t)B * 8);
+            float *dW = ws->s_exact.as<float>(), *dE = dW + B;
+            launch_scan_band(ws->qt_step.as<float>(), ws->sbound.as<float>(), dot ? nullptr : ws->amax.as<float>(),
+                             dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, ix->m, dot, B, dW, dE, st);
+            std::vector<uint64_t> probes(slots), seg(slots);
+            std::vector<float> L(cap_floats);
+            LGPU_CUDA(cudaMemcpyAsync(probes.data(), ws->probes.p, (size_t)slots * 8, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaMemcpyAsync(seg.data(), ga.seg_off, (size_t)slots * 8, cudaMemcpyDeviceToHost, st));
+            if (cap_floats) LGPU_CUDA(cudaMemcpyAsync(L.data(), ws->dist_out.p, cap_floats * 4, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaMemcpyAsync(dbg->W, dW, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaMemcpyAsync(dbg->E, dE, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaMemcpyAsync(dbg->bad, ws->qt_bad.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaStreamSynchronize(st));
+            for (uint32_t sl = 0; sl < slots; sl++) {
+                const uint64_t p = probes[sl];
+                dbg->parts[sl] = p < nlist ? (uint32_t)p : UINT32_MAX;
+                const uint64_t n = p < nlist ? std::min<uint64_t>(ix->h_part_n[p], dbg->ld) : 0;
+                if (n) memcpy(dbg->L + (size_t)sl * dbg->ld, L.data() + seg[sl], n * 4);
+            }
+            dbg->ran = true;
+            return;
+        }
         // shortlist: the kp smallest lower bounds (with their storage positions)
         SelectArgs ss = sa;
         ss.k = kp; ss.out_ids = ws->s_ids.as<uint64_t>(); ss.out_dist = ws->s_lb.as<float>();
@@ -893,7 +928,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         ws->stats_mode = 2;
         launch_band_check3(ws->s_lb.as<float>(), ws->s_cnt.as<uint32_t>(), ws->qt_step.as<float>(), ws->sbound.as<float>(),
                            dot ? nullptr : ws->amax.as<float>(), dot ? nullptr : ix->rmax_bits.as<int>(),
-                           ws->qt_bad.as<uint32_t>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, B, kk, kp,
+                           ws->qt_bad.as<uint32_t>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B, kk, kp,
                            ws->flags.as<uint32_t>(), ws->c_wcnt.as<uint32_t>() + 1, ws->c_surv.as<uint32_t>(), st);
         // exact PQ distances of the shortlist (oracle arithmetic), then the kk best of those
         launch_pq_rescore(qsearch, ws->s_pos.as<uint64_t>(), B, kp, ix->codes.as<unsigned char>(),
@@ -2195,6 +2230,29 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
         uint32_t n = ix->h_part_n[part];
         if (n) LGPU_CUDA(cudaMemcpyAsync(out, ws->dist_out.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaStreamSynchronize(st));
+    });
+}
+
+int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, uint32_t nprobes, uint64_t ld,
+                             uint32_t *out_parts, float *out_L, float *out_W, float *out_E, uint32_t *out_bad)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(queries && out_parts && out_L && out_W && out_E && out_bad && B > 0 && nprobes > 0, "bad argument");
+        HandleRef<lgpu_index> ix(ixh, "index");
+        require_device(ix->device);
+        nprobes = std::min(nprobes, ix->nlist);
+        LGPU_REQUIRE(ivf_sub_batch_size(ix.h, B, nprobes) == B, "batch too large for one filter-scan launch");
+        WsLease lease(ix->pool, nullptr, false);
+        Workspace *ws = lease.ws; cudaStream_t st = lease.st;
+        ws->q.ensure((size_t)B * ix->dim * 4);
+        LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * ix->dim * 4, cudaMemcpyHostToDevice, st));
+        lgpu_search_params sp{};
+        sp.k = 10; sp.nprobes = nprobes;
+        FilterDebug dbg{out_L, ld, out_parts, out_W, out_E, out_bad};
+        ivf_sub_batch(ix.h, ws, st, ws->q.as<float>(), B, sp, nprobes, nullptr, nullptr, nullptr, false, nullptr,
+                      RowFilter(), nullptr, &dbg);
+        LGPU_CUDA(cudaStreamSynchronize(st));
+        LGPU_REQUIRE(dbg.ran, "this index or configuration does not use the filter scan");
     });
 }
 

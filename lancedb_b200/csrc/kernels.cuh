@@ -305,14 +305,37 @@ void launch_pq_rescore(const float *Q, const uint64_t *pos, uint32_t B, uint32_t
                        const float *centroids, const float *cb_tiled, uint32_t dim, uint32_t m, uint32_t dsub, int metric,
                        const uint32_t *ncols_q, float *out, cudaStream_t st);   // ncols_q: optional [B] pairs of each query (<= nc)
 // probe_A[slot] = coarse_dist[slot] - |q|^2, amax[q] = max_j coarse + |q|^2, qn2[q] = |q|^2
-// (probe_A / amax may be null: dot has no residual)
+// (probe_A / amax may be null: dot has no residual).  Sets bad[q] = 1 when |q|^2, amax[q] or base[q] + probe_A of one
+// of the query's probes is not finite: its lower bounds or its band would be, so only the exact path can serve it.
 void launch_probe_terms(const float *probe_dist, const float *Q, uint32_t B, uint32_t nprobes, uint32_t dim,
-                        float *probe_A, float *amax, float *qn2, cudaStream_t st);
-// the band of every query, for the candidate mode: slack[q] = scale (W + 2E) (same W, E as launch_band_check3);
-// also resets thr[q] = CAND_NO_THR, cand_cnt[q] = cand_last[q] = 0 and every key of cand_key to 0xffffffff
+                        float *probe_A, float *amax, float *qn2, const float *base, uint32_t *bad, cudaStream_t st);
+// The band of the filter scan (the error budget is above band_check3_kernel in tables.cu): the exact distance of a row
+// lies in [L - E, L + W + E] (times the metric scale), with
+//   W = m step (1 + 2^-10)
+//   E = 2^-15 ceil(m/96) (sbound + amax + rmax + 2 (|q|^2 + CB2) [+ m for dot]) + 2^-126.
+// For l2 and cosine every term scales with the data (E(2^j x) = 4^j E(x) in the normal range); dot's entries
+// 1 - q_i.b hold a constant 1 each, hence its m.  2^-126 is the underflow floor: 2^18 of the 2^-150 absolute errors
+// of subnormal products, quotients and conversions, more than the filter, the oracle and the coarse step make per row.
+// Every consumer (band_check3, cand_prepare) takes its band from here.
+struct ScanBand { float W, E; };
+__device__ __forceinline__ ScanBand scan_band(float step, float sbound, float amax, float rmax, float qn2, float cb2,
+                                              uint32_t m, bool dot)
+{
+    const float mag = sbound + amax + rmax + 2.0f * (qn2 + cb2) + (dot ? (float)m : 0.f);
+    ScanBand b;
+    b.W = (float)m * step * 1.0009765625f;
+    // separate roundings (no contraction into an fmaf): the band the host-side restatement computes, bit for bit
+    b.E = __fadd_rn(__fmul_rn(3.0517578125e-5f * (float)((m + 95u) / 96u), mag), 1.17549435e-38f);
+    return b;
+}
+// W[q], E[q] = scan_band of every query (lgpu_debug_filter_bounds)
+void launch_scan_band(const float *step, const float *sbound, const float *amax, const int *rmax_bits, const float *qn2,
+                      float cb2, uint32_t m, bool dot, uint32_t B, float *W, float *E, cudaStream_t st);
+// the band of every query, for the candidate mode: slack[q] = scale (W + 2E) (scan_band); also resets
+// thr[q] = CAND_NO_THR, cand_cnt[q] = cand_last[q] = 0 and every key of cand_key to 0xffffffff
 void launch_cand_prepare(const float *step, const float *sbound, const float *amax, const int *rmax_bits, const float *qn2,
-                         float cb2, float scale, uint32_t m, uint32_t B, float *slack, uint32_t *thr, uint32_t *cand_cnt,
-                         uint32_t *cand_last, uint32_t *cand_key, uint32_t cand_cap, cudaStream_t st);
+                         float cb2, float scale, uint32_t m, bool dot, uint32_t B, float *slack, uint32_t *thr,
+                         uint32_t *cand_cnt, uint32_t *cand_last, uint32_t *cand_key, uint32_t cand_cap, cudaStream_t st);
 // candidate mode, after the scan: per query, drop the candidates above the final threshold, re-score the survivors
 // exactly (oracle arithmetic, as launch_pq_rescore), and write the k best by (_distance, _rowid) -- ids, distances,
 // count and (optional) storage positions.  flags[q] = 1 when the query must be redone by the exact kernels (list
@@ -336,13 +359,14 @@ struct FinalizeArgs {
 };
 void launch_cand_finalize(const FinalizeArgs &a, cudaStream_t st);
 // flags[q] = 1 when the shortlist of q (lower bounds `lb` ascending, [B][kp], cnt valid) cannot be proven to hold
-// the exact top-k: proven iff cnt < kp or lb[kp-1] > lb[k-1] + scale (W + 2E),  W = m step (1 + 2^-10),
-// E = 2^-15 ceil(m/96) (sbound + amax + rmax + m + 2 (qn2 + cb2)); also 1 when bad[q].  amax / rmax_bits may be null
-// (dot).  cb2 = sum_i max_c |codebook_i[c]|^2.  surv (optional, [B]): the length of the ascending prefix
-// lb <= lb[k-1] + scale (W + 2E) -- the only rows that can be among the exact top-k, hence the only ones to re-score.
+// the exact top-k: proven iff cnt < kp or lb[kp-1] > lb[k-1] + scale (W + 2E), W and E from scan_band; also 1 when
+// bad[q].  amax / rmax_bits may be null (dot).  cb2 = sum_i max_c |codebook_i[c]|^2.  surv (optional, [B]): the length
+// of the ascending prefix lb <= lb[k-1] + scale (W + 2E) -- the only rows that can be among the exact top-k, hence the
+// only ones to re-score.
 void launch_band_check3(const float *lb, const uint32_t *cnt, const float *step, const float *sbound, const float *amax,
                         const int *rmax_bits, const uint32_t *bad, const float *qn2, float cb2, float scale, uint32_t m,
-                        uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, uint32_t *gate, uint32_t *surv, cudaStream_t st);
+                        bool dot, uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, uint32_t *gate, uint32_t *surv,
+                        cudaStream_t st);
 
 // ---------------- index build (build.cu) ----------------------------------------------
 // codes[row][i] = argmin_c entry(row's residual sub-vector i, codebook_i[c]) (ties: lowest c); X normalised for cosine

@@ -471,18 +471,16 @@ __global__ void __launch_bounds__(256, 2) pq_rescore_kernel(const float *__restr
 // ---- candidate mode of the filter scan: per-query band, then the final exact top-k over the survivors ----
 __global__ void cand_prepare_kernel(const float *__restrict__ step, const float *__restrict__ sbound,
                                     const float *__restrict__ amax, const int *__restrict__ rmax_bits,
-                                    const float *__restrict__ qn2, float cb2, float scale, uint32_t m, uint32_t B,
-                                    float *__restrict__ slack, uint32_t *__restrict__ thr, uint32_t *__restrict__ cand_cnt,
-                                    uint32_t *__restrict__ cand_last)
+                                    const float *__restrict__ qn2, float cb2, float scale, uint32_t m, bool dot,
+                                    uint32_t B, float *__restrict__ slack, uint32_t *__restrict__ thr,
+                                    uint32_t *__restrict__ cand_cnt, uint32_t *__restrict__ cand_last)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
-    const float mag = sbound[q] + (amax ? amax[q] : 0.f) + (rmax_bits ? __int_as_float(*rmax_bits) : 0.f) + (float)m +
-                      2.0f * (qn2[q] + cb2);
-    const float E = 3.0517578125e-5f * (float)((m + 95u) / 96u) * mag;       // same band as band_check3_kernel
-    const float W = (float)m * step[q] * 1.0009765625f;
-    slack[q] = scale * (W + 2.0f * E);
+    const ScanBand bd = scan_band(step[q], sbound[q], amax ? amax[q] : 0.f, rmax_bits ? __int_as_float(*rmax_bits) : 0.f,
+                                  qn2[q], cb2, m, dot);
+    slack[q] = scale * (bd.W + 2.0f * bd.E);
     thr[q] = CAND_NO_THR;
     cand_cnt[q] = 0u;
     cand_last[q] = 0u;
@@ -579,9 +577,12 @@ __global__ void __launch_bounds__(RSC_THREADS, 2) cand_rescore_kernel(FinalizeAr
 }
 
 // probe_A[slot] = coarse_dist - |q|^2 ; amax[q] = max_j coarse + |q|^2
+// bad[q] |= |q|^2, amax or some base + A not finite (|q|^2 above FLT_MAX with finite coarse distances makes A = -inf:
+// every L would be -inf and the candidate mode's limit tau + slack NaN)
 __global__ void probe_terms_kernel(const float *__restrict__ probe_dist, const float *__restrict__ Q, uint32_t B,
                                    uint32_t nprobes, uint32_t dim, float *__restrict__ probe_A,
-                                   float *__restrict__ amax, float *__restrict__ qn2)
+                                   float *__restrict__ amax, float *__restrict__ qn2, const float *__restrict__ base,
+                                   uint32_t *__restrict__ bad)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;    // one warp per query
@@ -593,64 +594,93 @@ __global__ void probe_terms_kernel(const float *__restrict__ probe_dist, const f
     for (int o = 16; o > 0; o >>= 1) n2d += __shfl_xor_sync(0xffffffffu, n2d, o);
     const float n2 = (float)n2d;
     float mx = 0.f;
+    bool inf = false;
     if (probe_A) {                                       // (dot: no residual, A = 0)
+        const float b = base[q];
         for (uint32_t j = lane; j < nprobes; j += 32) {
             const float cd = probe_dist[(size_t)q * nprobes + j];
-            probe_A[(size_t)q * nprobes + j] = cd - n2;
+            const float A = cd - n2;
+            probe_A[(size_t)q * nprobes + j] = A;
             mx = fmaxf(mx, fabsf(cd));
+            inf |= !(fabsf(b + A) < CUDART_INF_F);      // the same sum as scan3's epilogue
         }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    inf = __any_sync(0xffffffffu, inf);
     if (lane == 0) {
         qn2[q] = n2;
-        if (amax) amax[q] = mx + n2;                    // >= |A| and also covers the coarse distance's own rounding
+        const float am = mx + n2;                       // >= |A| and also covers the coarse distance's own rounding
+        if (amax) amax[q] = am;
+        if (inf || !(n2 < CUDART_INF_F) || !(am < CUDART_INF_F)) bad[q] = 1u;
     }
 }
 
 // flags[q] = 1 when the shortlist cannot be proven to contain the exact top-k (see the header and kernels.cuh).
-// Error budget, u = 2^-24: the exact (oracle-order) distance d* differs from the real-arithmetic distance D of the
-// same f32 inputs by <= (m + 16) u (D + |q - c_p|^2); the table entries carry <= (dsub + 2) u T each, the floor of
-// the quantiser can be off by one step when (T - min) / step lands within 2^-11 of an integer (absorbed by the
-// factor 1 + 2^-10 on W), A carries <= 70 u (coarse + |q|^2), R one ulp, the epilogue of scan3 three more roundings
-// of values bounded by sbound + amax + rmax, and the expansion form of the entries (filter_entry) <= 12 u (|q_i| + |b|)^2
-// <= 24 u (|q_i|^2 + max_c |b|^2) each.  For m <= 96 all of it is < 2^9 u = 2^-15 of
-// (sbound + amax + rmax + m + 2 (|q|^2 + CB2)), CB2 = sum_i max_c |codebook_i[c]|^2; larger m widens E proportionally.
+// Error budget of scan_band (kernels.cuh), u = 2^-24, mag = sbound + amax + rmax + 2 (|q|^2 + CB2),
+// CB2 = sum_i max_c |codebook_i[c]|^2.  In the normal range every f32 operation errs by <= u of its result:
+//   - the exact (oracle-order) distance d* differs from the real-arithmetic distance D of the same f32 inputs by
+//     <= (m + 16) u (D + |q - c_p|^2) <= 2 (m + 16) u mag: m - 1 sequential sums, <= log2(dsub) + 2 per entry;
+//   - a table entry (filter_entry) errs by <= (dsub / 2 + 2) u |q_i| |b| in its dot chain (dsub / 2 FMAs per lane, up to
+//     16 at dsub 32), as much in |q_i|^2 and in |b|^2, and u |T| in the final FMA: <= (dsub + 6) u (|q_i|^2 + |b|^2) +
+//     u |T|, summed over i <= 38 u (|q|^2 + CB2) + u sbound at dsub 32.  The entry's error enters L once through the
+//     entry itself and once through min_i (base): twice that;
+//   - the quantiser's floor can be off by one step when (T - min) / step lands within 2^-11 of an integer, and step is
+//     rounded: both are absorbed by the factor 1 + 2^-10 on W (not by E);
+//   - A carries <= 70 u (coarse + |q|^2) <= 70 u amax, R one ulp of rmax, the epilogue of scan3 (fmaf, + R) two more
+//     roundings of values bounded by sbound + amax + rmax;
+//   so for m <= 96: <= (224 + 2 + 70 + 1 + 2) u mag + 76 u (|q|^2 + CB2) < 2^9 u mag = 2^-15 mag.  For m > 96 only the
+//   first term grows, and (m + 16) <= 112 ceil(m/96): ceil(m/96) times the budget covers it.
+// dot: T = 1 - q_i.b has an absolute 1 per entry, whose rounding is not proportional to |q_i||b|: m more in mag.
+// Subnormal range: products, FMAs, quotients and conversions that underflow err by an absolute <= 2^-150 on top
+// (additions and subtractions are exact there).  Per row: 3 dsub + 1 per table entry, twice (entry and min), dsub per
+// oracle entry, dim for each of the two coarse computations, 65535 through step * S, a few in the epilogue: below
+// 2^18 x 2^-150 = 2^-132 for dim <= 16384 (m <= 512, dsub <= 32).  The floor 2^-126 covers it with a margin of 64;
+// it vanishes in the rounding of E once 2^-15 mag >= 2^-101, so E is homogeneous of degree 2 in the data there.
 __global__ void band_check3_kernel(const float *__restrict__ lb, const uint32_t *__restrict__ cnt,
                                    const float *__restrict__ step, const float *__restrict__ sbound,
                                    const float *__restrict__ amax, const int *__restrict__ rmax_bits,
                                    const uint32_t *__restrict__ bad, const float *__restrict__ qn2, float cb2, float scale,
-                                   uint32_t m, uint32_t B, uint32_t k, uint32_t kp, uint32_t *__restrict__ flags,
+                                   uint32_t m, bool dot, uint32_t B, uint32_t k, uint32_t kp, uint32_t *__restrict__ flags,
                                    uint32_t *__restrict__ gate, uint32_t *__restrict__ surv)
 {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
     uint32_t f = bad[q] ? 1u : 0u;
+    const ScanBand bd = scan_band(step[q], sbound[q], amax ? amax[q] : 0.f, rmax_bits ? __int_as_float(*rmax_bits) : 0.f,
+                                  qn2[q], cb2, m, dot);
+    const float slack = scale * (bd.W + 2.0f * bd.E);
     if (surv) {
         // the rows that can still be among the exact top-k: the ascending prefix with L <= L_(k) + scale (W + 2E)
         const uint32_t n = min(cnt[q], kp);
         uint32_t pre = n;
         if (n > k && !f) {
-            const float mag = sbound[q] + (amax ? amax[q] : 0.f) + (rmax_bits ? __int_as_float(*rmax_bits) : 0.f) + (float)m +
-                              2.0f * (qn2[q] + cb2);
-            const float lim = lb[(size_t)q * kp + k - 1] +
-                              scale * ((float)m * step[q] * 1.0009765625f + 2.0f * 3.0517578125e-5f * (float)((m + 95u) / 96u) * mag);
+            const float lim = lb[(size_t)q * kp + k - 1] + slack;
             pre = k;
             while (pre < n && !(lb[(size_t)q * kp + pre] > lim)) pre++;
         }
         surv[q] = pre;
     }
     if (!f && cnt[q] >= kp && kp > 0) {
-        const float mag = sbound[q] + (amax ? amax[q] : 0.f) + (rmax_bits ? __int_as_float(*rmax_bits) : 0.f) + (float)m +
-                          2.0f * (qn2[q] + cb2);
-        const float E = 3.0517578125e-5f * (float)((m + 95u) / 96u) * mag;
-        const float W = (float)m * step[q] * 1.0009765625f;
         const float kth = lb[(size_t)q * kp + (k - 1 < kp ? k - 1 : kp - 1)];
         const float last = lb[(size_t)q * kp + kp - 1];
-        f = (k >= kp || !(last > kth + scale * (W + 2.0f * E))) ? 1u : 0u;
+        f = (k >= kp || !(last > kth + slack)) ? 1u : 0u;
     }
     flags[q] = f;
     if (f && gate) *gate = 1u;                              // opens the gate of the exact fix-up pass
+}
+
+__global__ void scan_band_kernel(const float *__restrict__ step, const float *__restrict__ sbound,
+                                 const float *__restrict__ amax, const int *__restrict__ rmax_bits,
+                                 const float *__restrict__ qn2, float cb2, uint32_t m, bool dot, uint32_t B,
+                                 float *__restrict__ W, float *__restrict__ E)
+{
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= B) return;
+    const ScanBand bd = scan_band(step[q], sbound[q], amax ? amax[q] : 0.f, rmax_bits ? __int_as_float(*rmax_bits) : 0.f,
+                                  qn2[q], cb2, m, dot);
+    W[q] = bd.W;
+    E[q] = bd.E;
 }
 
 template <class F> void dispatch_dsub(uint32_t dsub, F &&f)
@@ -728,20 +758,21 @@ void launch_pq_rescore(const float *Q, const uint64_t *pos, uint32_t B, uint32_t
 }
 
 void launch_probe_terms(const float *probe_dist, const float *Q, uint32_t B, uint32_t nprobes, uint32_t dim,
-                        float *probe_A, float *amax, float *qn2, cudaStream_t st)
+                        float *probe_A, float *amax, float *qn2, const float *base, uint32_t *bad, cudaStream_t st)
 {
     if (B == 0) return;
-    launch_k(probe_terms_kernel, dim3((B * 32 + 255) / 256), dim3(256), 0, st, probe_dist, Q, B, nprobes, dim, probe_A, amax, qn2); LGPU_COUNT_LAUNCH();
+    launch_k(probe_terms_kernel, dim3((B * 32 + 255) / 256), dim3(256), 0, st, probe_dist, Q, B, nprobes, dim, probe_A, amax, qn2,
+             base, bad); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
 void launch_cand_prepare(const float *step, const float *sbound, const float *amax, const int *rmax_bits, const float *qn2,
-                         float cb2, float scale, uint32_t m, uint32_t B, float *slack, uint32_t *thr, uint32_t *cand_cnt,
-                         uint32_t *cand_last, uint32_t *cand_key, uint32_t cand_cap, cudaStream_t st)
+                         float cb2, float scale, uint32_t m, bool dot, uint32_t B, float *slack, uint32_t *thr,
+                         uint32_t *cand_cnt, uint32_t *cand_last, uint32_t *cand_key, uint32_t cand_cap, cudaStream_t st)
 {
     if (B == 0) return;
     LGPU_CUDA(cudaMemsetAsync(cand_key, 0xff, (size_t)B * cand_cap * 4, st));
-    launch_k(cand_prepare_kernel, dim3((B + 127) / 128), dim3(128), 0, st, step, sbound, amax, rmax_bits, qn2, cb2, scale, m, B, slack, thr, cand_cnt, cand_last); LGPU_COUNT_LAUNCH();
+    launch_k(cand_prepare_kernel, dim3((B + 127) / 128), dim3(128), 0, st, step, sbound, amax, rmax_bits, qn2, cb2, scale, m, dot, B, slack, thr, cand_cnt, cand_last); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
@@ -769,13 +800,22 @@ void launch_cand_finalize(const FinalizeArgs &a, cudaStream_t st)
     LGPU_CUDA(cudaGetLastError());
 }
 
+void launch_scan_band(const float *step, const float *sbound, const float *amax, const int *rmax_bits, const float *qn2,
+                      float cb2, uint32_t m, bool dot, uint32_t B, float *W, float *E, cudaStream_t st)
+{
+    if (B == 0) return;
+    scan_band_kernel<<<(B + 127) / 128, 128, 0, st>>>(step, sbound, amax, rmax_bits, qn2, cb2, m, dot, B, W, E); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
 void launch_band_check3(const float *lb, const uint32_t *cnt, const float *step, const float *sbound, const float *amax,
                         const int *rmax_bits, const uint32_t *bad, const float *qn2, float cb2, float scale, uint32_t m,
-                        uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, uint32_t *gate, uint32_t *surv, cudaStream_t st)
+                        bool dot, uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, uint32_t *gate, uint32_t *surv,
+                        cudaStream_t st)
 {
     if (B == 0) return;
     if (gate) LGPU_CUDA(cudaMemsetAsync(gate, 0, 4, st));
-    band_check3_kernel<<<(B + 127) / 128, 128, 0, st>>>(lb, cnt, step, sbound, amax, rmax_bits, bad, qn2, cb2, scale, m, B, k, kp, flags, gate, surv); LGPU_COUNT_LAUNCH();
+    band_check3_kernel<<<(B + 127) / 128, 128, 0, st>>>(lb, cnt, step, sbound, amax, rmax_bits, bad, qn2, cb2, scale, m, dot, B, k, kp, flags, gate, surv); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

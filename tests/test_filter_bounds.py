@@ -1,68 +1,30 @@
-"""Host restatement of the filter scan's arithmetic (lancedb_b200/csrc/tables.cu + scan3.cu) checked against the
-oracle on the CPU: the lower bound L built from the 16-bit per-query tables, the per-probe scalar A and the
-per-row constant R must bracket the oracle's exact PQ distance d*:   L - E <= d* <= L + W + E,
-with W = m * step * (1 + 2^-10) and E = 2^-15 * ceil(m/96) * (sbound + amax + rmax + m + 2 (|q|^2 + CB2)) (times 0.5
-for cosine) --
-exactly the band `band_check3_kernel` uses to prove that a shortlist contains the exact top-k.  This pins the
-algebra (|r - b|^2 = |q - b|^2 + (|c|^2 - 2 q.c) + 2 b.c), the quantiser and the error budget without a GPU;
-the GPU parity tests then check the kernels themselves."""
+"""Host restatement of the filter scan's arithmetic (lancedb_b200/csrc/tables.cu + scan3.cu, restated bit for bit in
+tests/util.py: filter_bounds) checked against the oracle on the CPU: the lower bound L built from the 16-bit per-query
+tables, the per-probe scalar A and the per-row constant R must bracket the oracle's exact PQ distance d*:
+L - E <= d* <= L + W + E (times 0.5 for cosine), with W and E of scan_band (kernels.cuh) -- exactly the band
+`band_check3_kernel` uses to prove that a shortlist contains the exact top-k.  This pins the algebra
+(|r - b|^2 = |q - b|^2 + (|c|^2 - 2 q.c) + 2 b.c), the quantiser and the error budget on random data without a GPU;
+tests/test_scan_band.py attacks the same band with constructed data, and the GPU parity tests check the kernels
+themselves."""
 import numpy as np
 import pytest
 
 import oracle
-from tests.util import queries, random_index
+from tests.util import candidate_appends, filter_bounds, queries, random_index, row_consts
 
 F = np.float32
 
 
-def _bounds(ix, orc, q, p):
-    """(L, W, E, dstar) for every row of partition p."""
-    m, dsub = ix.m, ix.dim // ix.m
-    dot, cos = ix.metric == "dot", ix.metric == "cosine"
-    qn = oracle.normalize(q) if cos else q.astype(F)
-    # the filter's table entries (tables.cu filter_entry): the expansion |q_i|^2 + |b|^2 - 2 q_i.b in f32
-    # (1 - q_i.b for dot) -- NOT lance's (q_i - b)^2 tree; its rounding error is part of E below
-    qs = qn.reshape(m, 1, dsub).astype(F)
-    cbf = ix.codebook.astype(F)                              # [m,256,dsub]
-    dotp = np.zeros((m, 256), F)
-    for t in range(dsub):
-        dotp = (dotp + qs[:, :, t] * cbf[:, :, t]).astype(F)
-    if dot:
-        T = (F(1) - dotp).astype(F)
-    else:
-        qi2 = (qs * qs).sum(2, dtype=F)
-        cbn2 = (cbf * cbf).sum(2, dtype=F)
-        T = ((qi2 + cbn2).astype(F) - F(2) * dotp).astype(F)
-    mn, mx = T.min(1), T.max(1)
-    qmax = F(65535 // m)
-    rng = F((mx - mn).max())
-    step = F(rng / qmax) if rng > 0 else F(0)
-    inv = F(qmax / rng) if rng > 0 else F(0)
-    n = np.clip(np.floor((T - mn[:, None]) * inv), 0, qmax).astype(np.int64)
-    base = F(mn.sum(dtype=F)) - (F(m - 1) if dot else F(0))
-    sbound = F(np.maximum(np.abs(mn), np.abs(mx)).sum(dtype=F))
-    codes = ix.partition_codes(p).astype(np.int64)          # [m, n_p]
-    S = n[np.arange(m)[:, None], codes].sum(0)
-    assert S.max(initial=0) <= 65535
-    if dot:
-        A, amax, R, rmax = F(0), F(0), np.zeros(codes.shape[1], F), F(0)
-    else:
-        cen = ix.centroids[p]
-        coarse = F(orc.find_partitions(qn, ix.nlist)[2][p])
-        n2 = F(np.dot(qn.astype(np.float64), qn.astype(np.float64)))
-        A = F(coarse - n2)
-        amax = F(np.abs(orc.find_partitions(qn, ix.nlist)[2]).max() + n2)
-        cb = ix.codebook.astype(np.float64)                 # [m,256,dsub]
-        cw = cb[np.arange(m)[:, None], codes]               # [m, n_p, dsub]
-        R = (2.0 * (cw * cen.reshape(m, 1, dsub).astype(np.float64)).sum((0, 2))).astype(F)
-        rmax = F(np.abs(R).max(initial=0))
-    scale = F(0.5) if cos else F(1)
-    L = ((step * S.astype(F) + F(base + A)).astype(F) + R).astype(F) * scale
-    W = F(m) * step * F(1.0009765625) * scale
-    qn2 = F(np.dot(qn.astype(np.float64), qn.astype(np.float64)))
-    cb2 = F((ix.codebook.astype(np.float64) ** 2).sum(2).max(1).sum() * 1.000001)
-    E = F(3.0517578125e-5) * F((m + 95) // 96) * F(sbound + amax + rmax + F(m) + F(2) * (qn2 + cb2)) * scale
-    return L, W, E, orc.partition_distances(q, p)
+def _bounds(ix, orc, q, p, R=None):
+    """(L, W, E, dstar) for every row of partition p, W and E scaled by the metric's scale"""
+    out, W, E, scale, bad = filter_bounds(ix, orc, q, R=R)
+    assert not bad
+    L, d = out[p]
+    return L, F(W * scale), F(E * scale), d
+
+
+def _consts(ix):
+    return None if ix.metric == "dot" else [row_consts(ix, p) for p in range(ix.nlist)]
 
 
 @pytest.mark.parametrize("metric", ["l2", "cosine", "dot"])
@@ -72,10 +34,11 @@ def test_lower_bound_brackets_the_oracle_distance(metric, dim, m, scale):
     rng = np.random.default_rng(5)
     ix = random_index(rng, dim=dim, nlist=6, m=m, metric=metric, sizes=[40, 700, 0, 1300, 5, 257], scale=scale)
     orc = oracle.OracleIndex.from_data(ix)
+    R = _consts(ix)
     worst = 0.0
     for q in queries(rng, 5, dim, scale=scale):
         for p in (0, 1, 3, 4, 5):
-            L, W, E, d = _bounds(ix, orc, q, p)
+            L, W, E, d = _bounds(ix, orc, q, p, R)
             lo, hi = L - E, L + W + E
             assert (d >= lo).all(), (metric, p, float((lo - d).max()), float(E))
             assert (d <= hi).all(), (metric, p, float((d - hi).max()), float(E), float(W))
@@ -107,36 +70,18 @@ def test_candidate_lists_hold_the_exact_topk_under_any_tile_order():
     rng = np.random.default_rng(8)
     ix = random_index(rng, dim=64, nlist=5, m=8, sizes=[900, 1500, 40, 2300, 700])
     orc = oracle.OracleIndex.from_data(ix)
+    R = _consts(ix)
     k = 10
     for q in queries(rng, 4, 64):
         rows = []                                             # (L, d*, partition, row), band per partition
         Wm, Em = F(0), F(0)
         for p in range(5):
-            L, W, E, d = _bounds(ix, orc, q, p)
+            L, W, E, d = _bounds(ix, orc, q, p, R)
             Wm, Em = max(Wm, W), max(Em, E)
             rows += [(float(L[r]), float(d[r]), p, r) for r in range(len(L))]
         slack = float(Wm + 2 * Em)
         truth = set(map(lambda t: (t[2], t[3]), sorted(rows, key=lambda t: (t[1], t[2], t[3]))[:k]))
         for trial in range(6):
-            order = rng.permutation(len(rows))
-            tiles = np.array_split(order, rng.integers(3, 40))
-            tau, stale, appended = None, None, []
-            for tile in tiles:
-                Ls = np.array([rows[i][0] for i in tile])
-                use = stale if (stale is not None and rng.random() < 0.4) else tau      # a threshold read earlier
-                rule = rng.integers(0, 3)
-                if use is None or rule == 0:                  # tile-local: an upper bound of the tile's k-th smallest
-                    if len(Ls) >= k:
-                        kth = np.sort(Ls)[k - 1]
-                        cand = kth + rng.random() * 0.1 * abs(kth)              # bisection stops above it
-                        use = cand if use is None else min(use, cand)
-                elif rule == 1 and len(appended) >= k:        # list-based: k-th smallest key of the list so far
-                    use = min(use, np.sort([rows[i][0] for i in appended])[k - 1])
-                lim = np.inf if use is None else use + slack
-                appended += [i for i in tile if rows[i][0] <= lim]
-                stale = tau
-                if use is not None:
-                    tau = use if tau is None else min(tau, use)
-            got = {(rows[i][2], rows[i][3]) for i in appended}
+            got = {(rows[i][2], rows[i][3]) for i in candidate_appends(np.array([r[0] for r in rows]), k, slack, rng)}
             assert truth <= got, (trial, len(got))
             assert len(got) < len(rows)                       # and the filter does filter

@@ -212,3 +212,48 @@ def test_coarse_adversarial_rounding(list_path, monkeypatch):
     want = oracle.OracleIndex.from_data(ix).search(Q, k=10, nprobes=10, nthreads=8)
     assert (want[2] == 5).all()
     assert same_result(got, want)
+
+
+@pytest.mark.parametrize("d", [64, 768, 1536])
+def test_gemm_accumulation_rounding(d):
+    """tc_band's 4 d 2^-24 (|q| + xmax)^2 term for the f32 sums.  bf16-exact operands make every product exact, so only
+    the accumulation (and |x|^2) rounds; the rows are ordered adversarially: one large product then many 3/4-ulp ones,
+    the same with alternating signs, and random signs.  The error against the exact score must stay within that term.
+    This holds whether wgmma rounds to nearest or truncates (either errs by <= 2 u per addition); the bound does not tell
+    them apart, test_gemm_accumulation_of_sub_ulp_products measures which.  The largest error is printed."""
+    rng = np.random.default_rng(d)
+    q = np.ones((8, d), np.float32)
+    q[1::2, 1::2] = -1                                       # queries 1, 3, ..: alternating signs
+    X = np.zeros((256, d), np.float32)
+    X[:, 0] = 2.0 ** 8
+    X[:128, 1:] = 0.75 * 2.0 ** -15                          # 3/4 of an f32 ulp of 2^8
+    X[128:192, 1:] = 0.75 * 2.0 ** -15 * np.where(np.arange(1, d) % 2, 1, -1)
+    X[192:, 1:] = _bf16(rng.standard_normal((64, d - 1)).astype(np.float32))
+    got = _native.debug_gemm(q, X).astype(np.float64)
+    qx = q.astype(np.float64) @ X.astype(np.float64).T                                     # exact
+    want = (X.astype(np.float64) ** 2).sum(1).astype(np.float32).astype(np.float64)[None, :] - 2.0 * qx
+    s = np.sqrt((q.astype(np.float64) ** 2).sum(1))[:, None] + np.sqrt((X.astype(np.float64) ** 2).sum(1).max())
+    err = np.abs(got - want)
+    assert (err <= 4.0 * d * 2.0 ** -24 * s * s).all()
+    print(f"wgmma accumulation, d={d}: largest error {float((err / (2.0 ** -24 * s * s)).max()):.3f} u (|q| + xmax)^2")
+
+
+@pytest.mark.parametrize("d", [64, 768, 1536])
+def test_gemm_accumulation_of_sub_ulp_products(d):
+    """What wgmma's f32 accumulation does with products below one ulp of the running sum: q = [256, 1, 1, ..],
+    x = [1, 3/4 ulp(256), ...] (all bf16-exact, every product exact), so q.x = 256 + (d - 1) 3/4 ulp(256) exactly and
+    the score |x|^2 - 2 q.x ~ -511 keeps q.x to 1/2 ulp(256).  Accumulating one product at a time, round-to-nearest
+    keeps ~(d - 1) ulp (each 3/4 rounds up to 1), truncation keeps none; a wider internal sum keeps (d - 1) 3/4.  The
+    kept fraction is printed; the assertion is the tc_band term (4 d u (|q| + xmax)^2), which covers all three."""
+    q = np.ones((1, d), np.float32)
+    q[0, 0] = 256
+    x = np.full((1, d), 0.75 * 2.0 ** -15, np.float32)
+    x[0, 0] = 1
+    got = float(_native.debug_gemm(q, x)[0, 0])
+    xn2 = float(np.float32((x.astype(np.float64) ** 2).sum()))
+    exact = 256 + (d - 1) * 0.75 * 2.0 ** -15
+    acc = (xn2 - got) / 2
+    s = np.sqrt(256.0 ** 2 + d - 1) + np.sqrt(1 + (d - 1) * (0.75 * 2.0 ** -15) ** 2)
+    assert abs(2 * acc - 2 * exact) <= 4.0 * d * 2.0 ** -24 * s * s
+    print(f"wgmma sub-ulp accumulation, d={d}: kept {(acc - 256) / 2.0 ** -15:.2f} ulp(256) of the exact "
+          f"{(d - 1) * 0.75:.2f} ({(d - 1):d} with round-to-nearest one at a time, 0 with truncation)")
