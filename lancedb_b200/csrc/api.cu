@@ -96,10 +96,13 @@ struct DevBuf {
 
 struct Workspace {
     cudaStream_t stream = nullptr;     // private stream (host-buffer entry points)
-    cudaStream_t aux = nullptr;        // side stream: the per-query tables are built while the coarse step runs
+    // side stream of the filter scan's front: the coarse step and the regrouping run here while the per-query tables
+    // are built on the search stream.  Created at the device's greatest priority, so that as SMs free up the block
+    // scheduler hands them to this short critical chain before the waiting table CTAs (a per-stream property)
+    cudaStream_t front = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     int stats_mode = 0;                 // profiling: 1 = the last sub-batch ran the candidate mode, 2 = the dense filter
-    bool aux_open = false;              // an EAGER fork onto `aux` has not been joined yet (a call failed half-way)
+    bool front_open = false;            // an EAGER fork onto `front` has not been joined yet (a call failed half-way)
     cudaEvent_t done = nullptr;        // last use, for cross-stream reuse
     cudaEvent_t ev[8] = {};
     DevBuf q, qn, xnorm, D, probes, probe_dist, probe_cnt;
@@ -124,7 +127,9 @@ struct Workspace {
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-        LGPU_CUDA(cudaStreamCreateWithFlags(&aux, cudaStreamNonBlocking));
+        int least = 0, greatest = 0;
+        LGPU_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        LGPU_CUDA(cudaStreamCreateWithPriority(&front, cudaStreamNonBlocking, greatest));
         LGPU_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
         LGPU_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
         LGPU_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
@@ -134,7 +139,7 @@ struct Workspace {
     {
         if (graph) cudaGraphExecDestroy(graph);
         if (stream) cudaStreamDestroy(stream);
-        if (aux) cudaStreamDestroy(aux);
+        if (front) cudaStreamDestroy(front);
         if (ev_fork) cudaEventDestroy(ev_fork);
         if (ev_join) cudaEventDestroy(ev_join);
         if (done) cudaEventDestroy(done);
@@ -359,9 +364,10 @@ struct WsLease {
         // side-stream work of a call that failed half-way.  Only after an eager fork: an event whose last record sits
         // inside a captured graph cannot be waited on outside the capture (cudaErrorInvalidValue, which would then be
         // reported by the next cudaGetLastError() of an unrelated launch).
-        if (ws->aux_open) {
-            if (cudaStreamWaitEvent(st, ws->ev_join, 0) != cudaSuccess) cudaGetLastError();
-            ws->aux_open = false;
+        if (ws->front_open) {
+            if (cudaEventRecord(ws->ev_join, ws->front) != cudaSuccess || cudaStreamWaitEvent(st, ws->ev_join, 0) != cudaSuccess)
+                cudaGetLastError();
+            ws->front_open = false;
         }
         if (cudaEventRecord(ws->done, st) != cudaSuccess) cudaGetLastError();
         pool.give(ws);
@@ -584,7 +590,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
     const uint32_t dim = ix->dim, nlist = ix->nlist;
     const uint32_t slots = B * nprobes;
     int evi = 0;
-    auto mark = [&]() { if (prof) cudaEventRecord(ws->ev[evi++], st); };
+    cudaStream_t cs = st;                                // the stream of the coarse step and the regrouping
+    auto mark = [&]() { if (prof) cudaEventRecord(ws->ev[evi++], cs); };
     mark();
     ws->stats_mode = 0;
     // ---- queries (normalised copy for cosine) ----
@@ -595,8 +602,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         qsearch = ws->qn.as<float>();
     }
     // ---- which scan: filter + verify (scan3.cu) unless the request needs every exact distance.  The filter's
-    // per-query tables depend on the queries alone, so they are built on a side stream while the coarse step and the
-    // regrouping (small kernels that leave most SMs idle) run on this one ----
+    // per-query tables depend on the queries alone, so they are built on this stream while the coarse step and the
+    // regrouping (a latency chain of small kernels) run on the high-priority side stream `front` ----
     // the PQ top-`kk` of every query (kk = k, or k * refine_factor candidates for the exact re-rank)
     const uint32_t kk = sp.refine_factor ? sp.k * sp.refine_factor : sp.k;
     const uint32_t kp = kk <= 16 ? 32u : std::min<uint32_t>(SELECT_KMAX, 2 * kk + 32);
@@ -608,24 +615,34 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
                             (size_t)slots * ix->pad_prefix[1] * 4 <= workspace_budget();
     const bool filter_scan = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && !forced_probes &&
                              (d_ids || dbg) && kp > kk && ix->m <= 512 && !only && !small_path;
+    bool tables_pending = false;
     if (filter_scan) {
         ws->qt.ensure((size_t)B * ix->nch * 256 * 16); ws->qt_mm.ensure((size_t)B * ix->nch * 8 * 8);
         ws->qt_step.ensure((size_t)B * 4); ws->qt_base.ensure((size_t)B * 4); ws->qt_bad.ensure((size_t)B * 4);
         ws->sbound.ensure((size_t)B * 4);
         LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
-        LGPU_CUDA(cudaStreamWaitEvent(ws->aux, ws->ev_fork, 0));
+        LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
+        ws->front_open = !g_capturing;
+        cs = ws->front;
+        tables_pending = true;
+    }
+    // enqueued after the coarse GEMM, so that the GEMM's CTAs (each needs most of an SM's shared memory) are not queued
+    // behind the table grids; as SMs free up, the probe selection after it is dispatched ahead of the waiting table
+    // CTAs by the priority of `front`.  (Making the tables wait for the GEMM to finish was measured slower: the tables
+    // are then the longer branch.)
+    auto launch_tables = [&]() {
+        if (!tables_pending) return;
+        tables_pending = false;
         launch_query_tables_q16(qsearch, ix->cb_tiled.as<float>(), ix->cb_n2.as<float>(), B, dim, ix->m, ix->nch, ix->dsub,
                                 ix->metric, ws->qt_mm.as<float>(), ws->qt.as<uint4>(), ws->qt_step.as<float>(),
-                                ws->qt_base.as<float>(), ws->sbound.as<float>(), ws->qt_bad.as<uint32_t>(), ws->aux);
-        LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->aux));
-        ws->aux_open = !g_capturing;
-    }
+                                ws->qt_base.as<float>(), ws->sbound.as<float>(), ws->qt_bad.as<uint32_t>(), st);
+    };
     // ---- K1: exact centroid distances + nprobes nearest ----
     ws->probes.ensure((size_t)slots * 8);
     ws->probe_dist.ensure((size_t)slots * 4);
     ws->probe_cnt.ensure((size_t)B * 4);
     if (forced_probes) {
-        LGPU_CUDA(cudaMemcpyAsync(ws->probes.p, forced_probes, (size_t)slots * 8, cudaMemcpyHostToDevice, st));
+        LGPU_CUDA(cudaMemcpyAsync(ws->probes.p, forced_probes, (size_t)slots * 8, cudaMemcpyHostToDevice, cs));
         mark();
     } else {
         const uint64_t ldc = (nlist + 3u) & ~3u;
@@ -645,7 +662,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
             ws->flags.ensure((size_t)B * 4);
             ws->c_wcnt.ensure(16);
             uint32_t *cgate = ws->c_wcnt.as<uint32_t>() + 2;    // 0 = no query overflowed: the exact fix-up returns at once
-            launch_to_bf16(qsearch, B, dim, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
+            launch_to_bf16(qsearch, B, dim, ws->qb.p, ws->qn2.as<float>(), cs, ws->qerr.as<float>());
             if (modes.coarse_list_min && nlist >= modes.coarse_list_min && ix->cent_ns >= 4 * nprobes && nprobes <= 64) {
                 // Many lists (C5: 16384): a dense [B][nlist] score matrix is 537 MB written and read back.  Instead: (1) dense scores of a strided SAMPLE of the centroids; their
                 // nprobes-th smallest + 2 E_q bounds, per query, the scores of every true probe; (2) the full GEMM runs
@@ -657,53 +674,56 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
                 ws->t_cnt.ensure((size_t)B * 4); ws->probe_A.ensure((size_t)B * 4); ws->amax.ensure((size_t)B * 4);
                 ws->t_pos.ensure((size_t)B * lcap * 8); ws->t_exact.ensure((size_t)B * lcap * 4);
                 launch_gemm_dist(ws->qb.p, ix->cent_sb.p, ix->cent_sn2.as<float>(), B, ns, dim, ws->D.as<float>(), lds,
-                                 ix->num_sms, st);
+                                 ix->num_sms, cs);
                 if (!launch_sample_kth_threshold(ws->D.as<float>(), lds, ns, ws->qn2.as<float>(), ws->qerr.as<float>(),
-                                                 ix->cent_max, ix->cent_err, dim, B, nprobes, ws->probe_A.as<float>(), st)) {
+                                                 ix->cent_max, ix->cent_err, dim, B, nprobes, ws->probe_A.as<float>(), cs)) {
                     SelectArgs ss{};
                     ss.mode = 1; ss.dense = ws->D.as<float>(); ss.ncols = ns; ss.row_stride = lds; ss.B = B; ss.k = nprobes;
                     ss.out_ids = ws->t_ids.as<uint64_t>(); ss.out_dist = ws->t_dist.as<float>(); ss.out_count = ws->t_cnt.as<uint32_t>();
-                    launch_select(ss, st);
+                    launch_select(ss, cs);
                     launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(),
                                             ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, B, nprobes,
-                                            ws->probe_A.as<float>(), st);
+                                            ws->probe_A.as<float>(), cs);
                 }
-                LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
+                LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, cs));
                 GemmFilter flt{};
                 flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
                 flt.cand_ids = nullptr; flt.col_ids = nullptr; flt.cap = lcap; flt.cand_s = ws->t_exact.as<float>();
-                launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, nullptr, 0, ix->num_sms, st, &flt);
+                launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, nullptr, 0, ix->num_sms, cs, &flt);
+                launch_tables();
                 launch_coarse_finish(ws->t_exact.as<float>(), lcap, B, lcap, qsearch, ix->centroids.as<float>(),
                                      ws->qn2.as<float>(), ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes,
                                      ws->probes.as<uint64_t>(),
                                      ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate,
-                                     st, ws->t_pos.as<uint64_t>(), ws->amax.as<uint32_t>());
+                                     cs, ws->t_pos.as<uint64_t>(), ws->amax.as<uint32_t>());
             } else {
                 launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, ws->D.as<float>(), ldc,
-                                 ix->num_sms, st);
+                                 ix->num_sms, cs);
+                launch_tables();
                 launch_coarse_finish(ws->D.as<float>(), ldc, B, nlist, qsearch, ix->centroids.as<float>(), ws->qn2.as<float>(),
                                      ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes, ws->probes.as<uint64_t>(), ws->probe_dist.as<float>(),
-                                     ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate, st);
+                                     ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate, cs);
             }
             launch_dist_matrix(qsearch, ix->centroids.as<float>(), B, nlist, dim, 0, nullptr, nullptr, ws->D.as<float>(), ldc,
-                               st, ws->flags.as<uint32_t>(), cgate);
+                               cs, ws->flags.as<uint32_t>(), cgate);
             SelectArgs sc{};
             sc.mode = 1; sc.dense = ws->D.as<float>(); sc.ncols = nlist; sc.row_stride = ldc;
             sc.B = B; sc.k = nprobes; sc.out_ids = ws->probes.as<uint64_t>(); sc.out_dist = ws->probe_dist.as<float>();
             sc.out_count = ws->probe_cnt.as<uint32_t>(); sc.only = ws->flags.as<uint32_t>(); sc.gate = cgate;
-            launch_select(sc, st);
+            launch_select(sc, cs);
         } else {
             launch_dist_matrix(qsearch, ix->centroids.as<float>(), B, nlist, dim, ix->metric == LGPU_DOT ? 1 : 0,
-                               nullptr, nullptr, ws->D.as<float>(), ldc, st);
+                               nullptr, nullptr, ws->D.as<float>(), ldc, cs);
             mark();
             SelectArgs sa{};
             sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = nlist; sa.row_stride = ldc;
             sa.B = B; sa.k = nprobes;
             sa.out_ids = ws->probes.as<uint64_t>(); sa.out_dist = ws->probe_dist.as<float>();
             sa.out_count = ws->probe_cnt.as<uint32_t>();
-            launch_select(sa, st);
+            launch_select(sa, cs);
         }
     }
+    launch_tables();
     mark();
     if (small_path) {
         mark();                                          // (no regrouping)
@@ -776,8 +796,12 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
     }
     ga.only = only;
     ga.rows_tile = filter_scan ? SCAN3_ROWS_TILE : SCAN_ROWS_TILE_MID;
-    launch_group(ga, st);
+    launch_group(ga, cs);
     mark();
+    if (filter_scan) {
+        LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
+        cs = st;
+    }
     // ---- K2+K3 ----
     uint32_t np_eff = std::min<uint32_t>(nprobes, nlist);
     size_t cap_floats = (size_t)B * ix->pad_prefix[np_eff];
@@ -817,8 +841,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         ws->flags.ensure((size_t)B * 4); ws->c_wcnt.ensure(16); ws->c_surv.ensure((size_t)B * 4);
         ws->s_ids.ensure((size_t)B * kp * 8); ws->s_lb.ensure((size_t)B * kp * 4); ws->s_pos.ensure((size_t)B * kp * 8);
         ws->s_cnt.ensure((size_t)B * 4); ws->s_exact.ensure((size_t)B * kp * 4);
-        LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));        // the tables, built on the side stream
-        ws->aux_open = false;
+        LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));        // the probes and the regrouping, from `front`
+        ws->front_open = false;
         ws->qn2.ensure((size_t)B * 4);
         if (!dot) {
             ws->probe_A.ensure((size_t)slots * 4); ws->amax.ensure((size_t)B * 4);

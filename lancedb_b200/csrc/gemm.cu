@@ -365,13 +365,23 @@ __global__ void to_bf16_norm_kernel(const float *__restrict__ X, uint64_t n, uin
     const float *x = X + row * d;
     __nv_bfloat16 *xb = Xb + row * d;
     float s = 0.f, se = 0.f;
-    for (uint32_t k = lane; k < d; k += 32) {
-        float v = x[k];
-        const __nv_bfloat16 b = __float2bfloat16_rn(v);
-        xb[k] = b;
-        s = fmaf(v, v, s);
-        const float e = __bfloat162float(b) - v;                    // exact: b and v are within a factor of 2
-        se = fmaf(e, e, se);
+    // U loads of the lane in flight at once (a rolled loop waited for one DRAM round trip per element: 13 us for
+    // 1024 x 768 on an H100); the sums still run over k = lane, lane + 32, ... in order
+    constexpr uint32_t U = 8;
+    for (uint32_t k0 = lane; k0 < d; k0 += 32 * U) {
+        float v[U];
+#pragma unroll
+        for (uint32_t u = 0; u < U; u++) v[u] = k0 + 32 * u < d ? x[k0 + 32 * u] : 0.f;
+#pragma unroll
+        for (uint32_t u = 0; u < U; u++) {
+            if (k0 + 32 * u < d) {
+                const __nv_bfloat16 b = __float2bfloat16_rn(v[u]);
+                xb[k0 + 32 * u] = b;
+                s = fmaf(v[u], v[u], s);
+                const float e = __bfloat162float(b) - v[u];         // exact: b and v are within a factor of 2
+                se = fmaf(e, e, se);
+            }
+        }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

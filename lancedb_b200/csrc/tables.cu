@@ -107,12 +107,18 @@ __device__ __forceinline__ void stage_chunk(const float *__restrict__ cb_tiled, 
                                             unsigned char *sm)
 {
     if constexpr (QtSmem<DSUB>::STAGE) {
+        // cp.async: every 16-byte request of the thread in flight at once (register copies waited for one L2 or DRAM
+        // round trip per float4)
         const float4 *src = reinterpret_cast<const float4 *>(cb_tiled + (size_t)ch * 2048 * DSUB);
-        float4 *dst = reinterpret_cast<float4 *>(sm);
-        for (int i = threadIdx.x; i < 2048 * DSUB / 4; i += 256) dst[i] = __ldg(src + i);
+        const uint32_t dst = (uint32_t)__cvta_generic_to_shared(sm);
+        for (int i = threadIdx.x; i < 2048 * DSUB / 4; i += 256)
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + 16u * i), "l"(src + i) : "memory");
         const float4 *s2 = reinterpret_cast<const float4 *>(cb_n2 + (size_t)ch * 2048);
-        float4 *d2 = reinterpret_cast<float4 *>(sm + QtSmem<DSUB>::N2);
-        for (int i = threadIdx.x; i < 512; i += 256) d2[i] = __ldg(s2 + i);
+        const uint32_t d2 = dst + (uint32_t)QtSmem<DSUB>::N2;
+        for (int i = threadIdx.x; i < 512; i += 256)
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d2 + 16u * i), "l"(s2 + i) : "memory");
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
         __syncthreads();
     }
 }
