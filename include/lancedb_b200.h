@@ -61,6 +61,7 @@ typedef enum {
 typedef struct lgpu_index lgpu_index;   /* an IVF_PQ index resident in HBM */
 typedef struct lgpu_flat lgpu_flat;     /* a raw vector column resident in HBM */
 typedef struct lgpu_binary lgpu_binary; /* a packed binary (uint8) vector column in HBM, searched by Hamming distance */
+typedef struct lgpu_multivec lgpu_multivec; /* a multivector column in HBM, searched by late interaction (MaxSim) */
 
 /* The arrays of one IVF_PQ index (lance v2 `IvfPq`,
  * rust/lancedb/src/table/create_index.rs:283-303, :772): IVF centroids, PQ codebook
@@ -262,6 +263,41 @@ int  lgpu_binary_search_filtered(lgpu_binary *bx, const uint8_t *queries, uint32
 int  lgpu_binary_search_device(lgpu_binary *bx, const uint8_t *d_queries, uint32_t B, const lgpu_search_params *params,
                                uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
 
+/* ---- multivector columns: exact late-interaction (MaxSim) flat search (the `DataType::List` branch of
+ * rust/lancedb/src/table/query.rs:180-199: list<fixed_size_list<float, dim>> columns; the query's vectors are packed
+ * into ONE query, python/python/lancedb/query.py:3376-3382) ----
+ * A row r holds n_r >= 0 vectors v_j, a query nq >= 1 vectors q_i, and
+ *     _distance = sum_i min_j cosd(q_i, v_j),  summed over i in order in f32 from 0.0f,
+ * cosd = 1 - q.v / |q| / sqrt(v.v) in lance's lane order (the flat path's cosine).  A pair whose cosd is NaN is
+ * skipped by the min; a row where some q_i has no other pair -- an empty row, a zero or NaN query vector -- has a NaN
+ * distance and is never returned.  Results are ascending by (_distance, _rowid); k, distance_range (on the summed
+ * distance), the prefilter bitmap, timeout_ms, k > nrows and nrows = 0 behave as on the float flat path; nprobes and
+ * refine_factor are ignored.
+ * values: [T][dim] f32, T = offsets[nrows]; offsets: [nrows+1] u64, offsets[0] = 0, non-decreasing; row r's vectors
+ * are values[offsets[r] .. offsets[r+1]).  Limits: dim <= 65536, n_r <= 2^20, T <= 2^40.
+ * queries: [Tq][dim] f32, Tq = q_offsets[B]; q_offsets: [B+1] u32 HOST array (also for the device entry point: it is
+ * the batch's shape), q_offsets[0] = 0, query b's vectors are queries[q_offsets[b] .. q_offsets[b+1]), 1..4096 each.
+ * Columns of at least 65536 vectors, all finite and non-zero, with dim a multiple of 8, are scored on the tensor cores
+ * (fp16 copies of the normalised vectors) when the call has no prefilter or distance_range: every row within a
+ * rigorous error band of the k-th approximate distance is re-scored exactly, and a query whose shortlist overflows or
+ * that holds a zero / non-finite vector is redone exactly, so the results are the exact ones either way.
+ * lgpu_last_filter_stats after a profiled multivector call: [0] rows admitted to the shortlists, [1] rows scored
+ * exactly (on the exact path: B x nrows), [2] queries redone densely after the shortlist, [3] queries. */
+int  lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
+                        const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device, lgpu_multivec **out);
+void lgpu_multivec_close(lgpu_multivec *mv);
+int  lgpu_multivec_search(lgpu_multivec *mv, const float *queries, const uint32_t *q_offsets, uint32_t B,
+                          const lgpu_search_params *params, uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+/* under a row-id allow-list (same bitmap as lgpu_search_filtered) */
+int  lgpu_multivec_search_filtered(lgpu_multivec *mv, const float *queries, const uint32_t *q_offsets, uint32_t B,
+                                   const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                                   uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+/* d_queries and the three outputs in DEVICE memory (q_offsets stays on the host), enqueued on `cuda_stream`, not
+ * synchronised */
+int  lgpu_multivec_search_device(lgpu_multivec *mv, const float *d_queries, const uint32_t *q_offsets, uint32_t B,
+                                 const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
+                                 uint32_t *d_out_count, void *cuda_stream);
+
 /* ---- per-stage access (parity localisation and kernel benchmarks) -------- */
 /* coarse stage only: the nprobes nearest partitions of each query and their
  * distances (host buffers, [B][nprobes]) */
@@ -286,6 +322,11 @@ int lgpu_debug_gemm(const float *queries, const float *vectors, uint32_t B, uint
  * queries [B][nbytes], vectors [N][nbytes], out [B][N] u32) */
 int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint32_t B, uint64_t N, uint32_t nbytes,
                             int device, uint32_t *out);
+/* the multivector tensor-core score alone: out[i][r] = the largest fp16(q_i / |q_i|) . fp16(v / |v|) (f32 accumulation)
+ * over row r's vectors v, NaN for an empty row (host buffers: queries [nqv][dim], values [offsets[nrows]][dim],
+ * out [nqv][nrows] f32); dim must be a multiple of 8 */
+int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
+                           uint64_t nrows, uint32_t dim, int device, float *out);
 /* per-kernel device time (ms) of the most recent lgpu_search* call made with
  * LGPU_PROFILE=1 in the environment: coarse, select-probes, group, scan, top-k,
  * refine, total.  times: [7] */
@@ -294,7 +335,7 @@ int lgpu_last_stage_ms(float *times);
  * scanners appended, survivors re-scored exactly, queries sent to the exact fix-up pass, queries.  stats: [4]
  * After lgpu_binary_search* (whole batch): [0] candidates the tensor-core list pass appended (0 on the dense paths),
  * [1] distances computed on the tensor cores (0 on the SIMT path), [2] queries redone densely after a list overflow,
- * [3] queries. */
+ * [3] queries.  After lgpu_multivec_search*: see the multivector section above. */
 int lgpu_last_filter_stats(uint64_t *stats);
 /* kernels this process has launched through the library so far (eager launches and graph replays alike) */
 int lgpu_kernel_launch_count(uint64_t *count);

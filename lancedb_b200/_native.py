@@ -34,7 +34,12 @@ EXPORTS = [
     "lgpu_kernel_launch_count", "lgpu_last_filter_stats",
     "lgpu_binary_open", "lgpu_binary_close", "lgpu_binary_search", "lgpu_binary_search_filtered",
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
+    "lgpu_multivec_open", "lgpu_multivec_close", "lgpu_multivec_search", "lgpu_multivec_search_filtered",
+    "lgpu_multivec_search_device", "lgpu_debug_maxsim_gemm",
 ]
+MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
+MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
+MULTIVEC_MAX_DIM = 65536
 
 
 class IndexDesc(C.Structure):
@@ -123,6 +128,13 @@ def load():
     lib.lgpu_binary_search_filtered.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
     lib.lgpu_binary_search_device.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_debug_hamming_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
+    lib.lgpu_multivec_open.argtypes = [vp, vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
+    lib.lgpu_multivec_close.argtypes = [vp]
+    lib.lgpu_multivec_close.restype = None
+    lib.lgpu_multivec_search.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
+    lib.lgpu_multivec_search_filtered.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
+    lib.lgpu_multivec_search_device.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
+    lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -370,6 +382,112 @@ class GpuBinary:
         check(load().lgpu_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
 
 
+def multivec_offsets(lengths) -> np.ndarray:
+    """Vector counts per row (or per query) -> the [n+1] offsets the multivector entry points take."""
+    n = np.asarray(lengths, np.int64).reshape(-1)
+    if n.size and n.min() < 0:
+        raise ValueError("vector counts must not be negative")
+    return np.concatenate([[0], np.cumsum(n)]).astype(np.uint64)
+
+
+class GpuMultivec:
+    """A multivector column (list<fixed_size_list<float, dim>>) pinned in HBM (lgpu_multivec), searched by late
+    interaction: _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors."""
+
+    def __init__(self, values, offsets, row_ids=None, device: int = 0):
+        v = np.ascontiguousarray(values, np.float32)
+        off = np.ascontiguousarray(offsets, np.uint64)
+        if v.ndim != 2:
+            raise ValueError("multivector values must be a [vectors, dim] array")
+        if off.ndim != 1 or off.size < 1 or off[0] != 0 or int(off[-1]) != v.shape[0]:
+            raise ValueError("row offsets must be [rows + 1], start at 0 and end at the number of vectors")
+        if np.any(off[1:] < off[:-1]):
+            raise ValueError("row offsets must not decrease")
+        if off.size > 1 and int(np.max(off[1:] - off[:-1])) > MULTIVEC_MAX_ROW:
+            raise ValueError(f"a multivector row holds at most {MULTIVEC_MAX_ROW} vectors")
+        if not 1 <= v.shape[1] <= MULTIVEC_MAX_DIM:
+            raise ValueError(f"multivector dimension must be in [1, {MULTIVEC_MAX_DIM}]")
+        self.nrows, self.dim = off.size - 1, v.shape[1]
+        rid = None if row_ids is None else np.ascontiguousarray(row_ids, np.uint64)
+        if rid is not None and rid.shape != (self.nrows,):
+            raise ValueError("row_ids must hold one id per row")
+        h = C.c_void_p()
+        check(load().lgpu_multivec_open(_ptr(v), _ptr(off), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
+        self._h = h
+        self.device = device
+
+    def close(self):
+        if getattr(self, "_h", None) and _lib is not None:
+            _lib.lgpu_multivec_close(self._h)
+            self._h = None
+
+    __del__ = close
+
+    def _queries(self, queries, q_offsets):
+        """(values [Tq, dim] f32, offsets [B+1] u32).  queries: a list with one [nq_b, dim] (or [dim]) array per
+        query, or [Tq, dim] values with q_offsets; a single numpy array is ONE query."""
+        if q_offsets is None:
+            qs = [queries] if isinstance(queries, np.ndarray) else list(queries)
+            arrs = []
+            for q in qs:
+                a = np.asarray(q, np.float32)
+                if a.ndim == 1:
+                    a = a[None, :]
+                if a.ndim != 2:
+                    raise ValueError("a multivector query must be [nq, dim] or [dim]")
+                arrs.append(a)
+            lens = [a.shape[0] for a in arrs]
+            vals = np.concatenate(arrs) if arrs else np.zeros((0, self.dim), np.float32)
+            off = multivec_offsets(lens)
+        else:
+            vals = np.asarray(queries, np.float32)
+            off = np.asarray(q_offsets, np.int64).reshape(-1)
+        if vals.ndim != 2 or vals.shape[1] != self.dim:
+            raise ValueError(f"multivector query vectors must have dimension {self.dim}, got shape {vals.shape}")
+        if off.size < 1 or off[0] != 0 or int(off[-1]) != vals.shape[0]:
+            raise ValueError("query offsets must be [B + 1], start at 0 and end at the number of query vectors")
+        n = np.diff(off)
+        if np.any(n < 1):
+            raise ValueError("every multivector query needs at least one vector")
+        if n.size and int(n.max()) > MULTIVEC_MAX_NQ:
+            raise ValueError(f"a multivector query holds at most {MULTIVEC_MAX_NQ} vectors")
+        if int(off[-1]) >= 1 << 32:
+            raise ValueError("too many query vectors in one call")
+        return np.ascontiguousarray(vals), np.ascontiguousarray(off, np.uint32)
+
+    def search(self, queries, k=10, q_offsets=None, lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
+        """Host-buffer search of B multivector queries: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32).
+        `queries`: a list with one [nq_b, dim] array per query, or [Tq, dim] values with `q_offsets` [B+1]; a single
+        numpy array is ONE query.  Shapes are checked before any device call."""
+        q, off = self._queries(queries, q_offsets)
+        B = off.size - 1
+        ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
+        p = make_params(k, 0, 0, lower, upper, 0, timeout_ms)
+        if allow is None:
+            check(load().lgpu_multivec_search(self._h, _ptr(q), _ptr(off), B, C.byref(p), _ptr(ids), _ptr(dist),
+                                              _ptr(cnt)))
+        else:
+            bm = np.ascontiguousarray(allow, np.uint32)
+            if bm.size * 32 < allow_bits:
+                raise ValueError("allow bitmap shorter than allow_bits")
+            check(load().lgpu_multivec_search_filtered(self._h, _ptr(q), _ptr(off), B, C.byref(p), _ptr(bm),
+                                                       int(allow_bits), _ptr(ids), _ptr(dist), _ptr(cnt)))
+        return ids, dist, cnt
+
+    def search_device(self, d_q: int, q_offsets, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
+        """Device-pointer search: d_q [Tq][dim] f32 and the outputs are raw device addresses, q_offsets [B+1] a host
+        array (checked here); enqueued on `stream`, not synchronised."""
+        off = np.asarray(q_offsets, np.int64).reshape(-1)
+        n = np.diff(off)
+        if off.size < 1 or off[0] != 0 or np.any(n < 1) or (n.size and int(n.max()) > MULTIVEC_MAX_NQ):
+            raise ValueError("query offsets must start at 0 and give every query 1..4096 vectors")
+        if int(off[-1]) >= 1 << 32:
+            raise ValueError("too many query vectors in one call")
+        off = np.ascontiguousarray(off, np.uint32)
+        check(load().lgpu_multivec_search_device(self._h, d_q, _ptr(off), off.size - 1, C.byref(p), d_ids, d_dist,
+                                                 d_cnt, stream))
+
+
 def ivf_assign(centroids, vectors, metric: str = "l2", device: int = 0) -> np.ndarray:
     """Partition of every row = find_partitions(row, nprobes=1) with the search path's exact kernels."""
     c = np.ascontiguousarray(centroids, np.float32); v = np.ascontiguousarray(vectors, np.float32)
@@ -503,6 +621,19 @@ def debug_hamming_gemm(queries, vectors, device: int = 0) -> np.ndarray:
         raise ValueError("queries and vectors must be [rows, bytes] arrays with the same bytes per row")
     out = np.empty((q.shape[0], x.shape[0]), np.uint32)
     check(load().lgpu_debug_hamming_gemm(_ptr(q), _ptr(x), q.shape[0], x.shape[0], q.shape[1], device, _ptr(out)))
+    return out
+
+
+def debug_maxsim_gemm(queries, values, offsets, device: int = 0) -> np.ndarray:
+    """The multivector tensor-core score alone: [nqv, nrows] f32, the largest fp16 normalised similarity of each query
+    vector over each row's vectors (NaN for an empty row)."""
+    q = np.ascontiguousarray(queries, np.float32); x = np.ascontiguousarray(values, np.float32)
+    off = np.ascontiguousarray(offsets, np.uint64)
+    if q.ndim != 2 or x.ndim != 2 or q.shape[1] != x.shape[1] or int(off[-1]) != x.shape[0]:
+        raise ValueError("queries [nqv, dim], values [T, dim] and offsets [nrows + 1] ending at T are required")
+    out = np.empty((q.shape[0], off.size - 1), np.float32)
+    check(load().lgpu_debug_maxsim_gemm(_ptr(q), q.shape[0], _ptr(x), _ptr(off), off.size - 1, q.shape[1], device,
+                                        _ptr(out)))
     return out
 
 

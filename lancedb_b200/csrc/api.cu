@@ -124,6 +124,9 @@ struct Workspace {
     DevBuf c_work, c_wcnt, c_surv, c_exd, c_exi, c_exp;   // candidate mode: survivor work list and exact results
     DevBuf c_thr, c_slack, c_cnt, c_rec, c_key, c_last;          // filter scan (candidate mode): thresholds, bands, candidate lists
     DevBuf hq, hq_pop, h_sample, h_list, h_cnt;   // binary search: padded queries, popc(q), sample distances, fix-up list
+    DevBuf mv_qoff, mv_P, mv_M;         // multivector search: query vector offsets, pairwise cosd block, per-row minima
+    DevBuf mv_qh, mv_qbad, mv_Mk, mv_A; // ... tensor-core path: fp16 queries, bad vectors, max-similarity keys, approx dist
+    DevBuf mv_kd, mv_ki, mv_kc, mv_thr, mv_cnt, mv_cand, mv_flags, mv_vflags, mv_gate, mv_ex, mv_exid;   // shortlist
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -287,6 +290,21 @@ struct lgpu_binary {
     DevBuf vectors, pop, row_ids;          // [nrows][nbytes_pad] zero-padded rows, popc of each row, optional ids
     DevBuf sample, sample_pop;             // every (nrows / nsample)-th row: the threshold sample of the list path
     uint64_t nsample = 0;                  // 0: no sample (nrows <= HAM_SAMPLE)
+    bool has_ids = false;
+    WorkspacePool pool;
+};
+
+// a multivector column (list<fixed_size_list<float, dim>>) searched by late interaction (MaxSim over cosine)
+struct lgpu_multivec {
+    std::atomic<int> refs{0};
+    int device = 0, num_sms = 0;
+    uint64_t nrows = 0, total = 0;         // rows; stored vectors T = offsets[nrows]
+    uint32_t dim = 0;
+    uint64_t max_row = 0;                  // largest n_r
+    DevBuf vectors, ysqrt, offsets, row_ids;   // [T][dim] f32, |v| = sqrt(dot(v, v)) per vector, [nrows+1], optional ids
+    DevBuf vec_h, col_row;                 // tensor-core path: fp16 normalised vectors [T][dim], row of each vector [T]
+    bool tc_ok = false;                    // the tensor-core path may run (see multivec_search_device)
+    std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
     bool has_ids = false;
     WorkspacePool pool;
 };
@@ -1256,6 +1274,215 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     }
 }
 
+// ---- multivector columns (late interaction: sum over the query's vectors of the min cosine distance) ----
+// Limits of one call: a query holds 1..MV_MAX_NQ vectors, a row 0..MV_MAX_ROW, a vector at most MV_MAX_DIM components.
+constexpr uint32_t MV_MAX_NQ = 4096;
+constexpr uint64_t MV_MAX_ROW = (uint64_t)1 << 20;
+constexpr uint32_t MV_MAX_DIM = 65536;
+
+// Paths (multivec.cu, DESIGN.md section 6), chosen per call:
+//   tensor cores  the F16MaxSim gemm_dist_kernel scores fp16 copies of the normalised vectors and keeps the largest
+//                 similarity per (query vector, row); approximate distances -> the k-th smallest (select mode 1) -> every
+//                 row within 2 E_q of it (mv_band) -> exact re-score of those rows (dist.cu) -> select mode 2; a query
+//                 whose list overflowed or that holds a zero / non-finite vector is redone by the exact path below in
+//                 the same stream (flags / gate: nothing runs when no query is flagged).  Taken when the column holds at
+//                 least MV_TC_MIN_T vectors (all of them finite and non-zero), dim is a multiple of 8, there is no
+//                 prefilter or distance_range, LGPU_NO_TENSOR_CORE is not set and one query's scores fit the workspace.
+//   exact         for every sub-batch of queries, blocks of consecutive query vectors against chunks of whole rows --
+//                 dist_matrix_kernel (cosine, lance order) -> per-row minimum -> in-order running sum into D[b][N] --
+//                 then select mode 1 (distance_range, prefilter, (_distance, _rowid) order, NaN dropped).
+// Workspace stays inside LGPU_WS_BYTES.
+constexpr uint64_t MV_TC_MIN_T = 65536;   // stored vectors from which the tensor-core path runs (not measured)
+
+// the exact distances of queries [qa, qb) into D[b - qa][N] (only / vflags / gate: the fix-up of flagged queries)
+static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
+                           uint32_t qa, uint32_t qb, float *D, uint64_t ld, const uint32_t *only = nullptr,
+                           const uint32_t *vflags = nullptr, const uint32_t *gate = nullptr)
+{
+    const uint64_t N = mv->nrows;
+    const uint32_t dim = mv->dim;
+    const size_t budget = workspace_budget();
+    // a chunk of rows costs (n_r + 1) floats per query vector in the block (P and M); every row fits in half a chunk
+    const size_t pair_floats = std::max<size_t>(budget / 2 / 4, 1);
+    const uint64_t row_cost = mv->max_row + 1;
+    const uint32_t qv_max = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(pair_floats / (2 * row_cost), 65535ull * 16));
+    const uint64_t *off = mv->h_offsets.data();
+    uint32_t blo = qa;
+    for (uint32_t i0 = h_qoff[qa]; i0 < h_qoff[qb]; i0 += qv_max) {
+        const uint32_t i1 = std::min(h_qoff[qb], i0 + qv_max), nqv = i1 - i0;
+        while (h_qoff[blo + 1] <= i0) blo++;                         // first query with a vector in [i0, i1)
+        uint32_t bhi = blo;
+        while (bhi < qb && h_qoff[bhi] < i1) bhi++;                  // one past the last
+        const uint64_t cap = std::max<uint64_t>(pair_floats / nqv, 2 * row_cost);
+        for (uint64_t r0 = 0; r0 < N;) {
+            uint64_t r1 = r0 + 1;
+            while (r1 < N && (off[r1 + 1] - off[r0]) + (r1 + 1 - r0) <= cap) r1++;
+            const uint64_t span = off[r1] - off[r0], ldP = (span + 3) & ~3ull;
+            const uint32_t nr = (uint32_t)(r1 - r0);
+            ws->mv_P.ensure(std::max<size_t>((size_t)nqv * ldP, 4) * 4);
+            ws->mv_M.ensure((size_t)nqv * nr * 4);
+            if (span)
+                launch_dist_matrix(d_q + (size_t)i0 * dim, mv->vectors.as<float>() + (size_t)off[r0] * dim, nqv, span,
+                                   dim, 2, ws->xnorm.as<float>() + i0, mv->ysqrt.as<float>() + off[r0],
+                                   ws->mv_P.as<float>(), ldP, st, vflags ? vflags + (i0 - h_qoff[qa]) : nullptr, gate);
+            launch_mv_rowmin(ws->mv_P.as<float>(), ldP, nqv, mv->offsets.as<uint64_t>(), r0, nr, ws->mv_M.as<float>(),
+                             nr, mv->num_sms, st, gate);
+            launch_mv_rowsum(ws->mv_M.as<float>(), nr, ws->mv_qoff.as<uint32_t>(), blo, bhi, qa, i0, i1, nr, D, ld, r0,
+                             mv->num_sms, st, only, gate);
+            r0 = r1;
+        }
+    }
+}
+
+// h_qoff: HOST [B+1] offsets of each query's vectors in d_q (validated by the caller).
+void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
+                            uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
+                            RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
+{
+    const uint64_t N = mv->nrows, ld = (N + 3) & ~3ull;
+    const uint32_t dim = mv->dim, k = sp.k, Tq = h_qoff[B];
+    const bool prof = profiling_enabled();
+    if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));
+    ws->mv_qoff.ensure((size_t)(B + 1) * 4);
+    LGPU_CUDA(cudaMemcpyAsync(ws->mv_qoff.p, h_qoff, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, st));
+    ws->xnorm.ensure(std::max<size_t>(Tq, 1) * 4);
+    launch_row_norms(d_q, Tq, dim, ws->xnorm.as<float>(), st);
+    const size_t budget = workspace_budget();
+    uint32_t max_nq = 0;
+    for (uint32_t b = 0; b < B; b++) max_nq = std::max(max_nq, h_qoff[b + 1] - h_qoff[b]);
+    const size_t quarter = budget / 4;
+    const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper &&
+                    (size_t)(max_nq + 1) * ld * 4 <= quarter;
+    if (tc) {
+        // fp16 normalised queries (and the queries holding a bad vector), then sub-batches of whole queries whose scores
+        // M [vectors][ld] u32 and approximate distances A [queries][ld] f32 take a quarter of the budget each
+        ws->mv_qh.ensure(std::max<size_t>((size_t)Tq * dim * 2, 16));
+        ws->mv_qbad.ensure(std::max<size_t>(Tq, 1) * 4);
+        launch_mv_normalize_f16(d_q, Tq, dim, ws->mv_qh.p, ws->mv_qbad.as<uint32_t>(), st);
+        uint32_t cap = 1024;
+        while (cap < 8 * k && cap < 16384) cap <<= 1;
+        for (uint32_t qa = 0; qa < B;) {
+            uint32_t qb = qa + 1;
+            while (qb < B && (size_t)(h_qoff[qb + 1] - h_qoff[qa]) * ld * 4 <= quarter && (size_t)(qb + 1 - qa) * ld * 4 <= quarter)
+                qb++;
+            if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
+            const uint32_t b = qb - qa, va = h_qoff[qa], nqv = h_qoff[qb] - va;
+            ws->mv_Mk.ensure((size_t)nqv * ld * 4);
+            ws->mv_A.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+            ws->mv_kd.ensure((size_t)b * k * 4); ws->mv_ki.ensure((size_t)b * k * 8); ws->mv_kc.ensure((size_t)b * 4);
+            ws->mv_thr.ensure((size_t)b * 4); ws->mv_cnt.ensure((size_t)b * 4); ws->mv_cand.ensure((size_t)b * cap * 4);
+            ws->mv_flags.ensure((size_t)b * 4); ws->mv_vflags.ensure((size_t)nqv * 4); ws->mv_gate.ensure(16);
+            ws->mv_ex.ensure((size_t)b * cap * 4); ws->mv_exid.ensure((size_t)b * cap * 8);
+            LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ld * 4, st));
+            MaxSimOut mo{};
+            mo.col_row = mv->col_row.as<uint32_t>(); mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ld; mo.row_base = 0;
+            mo.xdummy = mv->ysqrt.as<float>();
+            launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, mv->vec_h.p, nqv, mv->total, dim, mo,
+                               mv->num_sms, st);
+            launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ld, ws->mv_qoff.as<uint32_t>(), qa, qb, va, N,
+                                 ws->mv_A.as<float>(), ld, mv->num_sms, st);
+            SelectArgs sa{};                                   // the k-th smallest approximate distance of each query
+            sa.mode = 1; sa.dense = ws->mv_A.as<float>(); sa.ncols = N; sa.row_stride = ld; sa.B = b; sa.k = k;
+            sa.out_ids = ws->mv_ki.as<uint64_t>(); sa.out_dist = ws->mv_kd.as<float>(); sa.out_count = ws->mv_kc.as<uint32_t>();
+            launch_select(sa, st);
+            launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
+                                ws->mv_thr.as<float>(), st);
+            LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
+            launch_mv_admit(ws->mv_A.as<float>(), ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(),
+                            ws->mv_cand.as<uint32_t>(), st);
+            launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
+                            ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
+            launch_mv_rescore(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), mv->vectors.as<float>(),
+                              mv->ysqrt.as<float>(), mv->offsets.as<uint64_t>(),
+                              mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, dim, b, ws->mv_cand.as<uint32_t>(),
+                              ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), st);
+            SelectArgs sb{};
+            sb.mode = 2; sb.dense = ws->mv_ex.as<float>(); sb.cand_ids = ws->mv_exid.as<uint64_t>();
+            sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0;
+            sb.B = b; sb.k = k; sb.out_ids = d_ids + (size_t)qa * k; sb.out_dist = d_dist + (size_t)qa * k;
+            sb.out_count = d_cnt + qa;
+            launch_select(sb, st);
+            // exact fix-up of the flagged queries (A is free again: it holds their exact distances)
+            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->mv_A.as<float>(), ld, ws->mv_flags.as<uint32_t>(),
+                           ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>());
+            SelectArgs sc{};
+            sc.mode = 1; sc.dense = ws->mv_A.as<float>(); sc.ncols = N; sc.row_stride = ld;
+            sc.col_ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
+            sc.B = b; sc.k = k; sc.out_ids = d_ids + (size_t)qa * k; sc.out_dist = d_dist + (size_t)qa * k;
+            sc.out_count = d_cnt + qa; sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = ws->mv_gate.as<uint32_t>();
+            launch_select(sc, st);
+            if (prof) {             // [0] rows admitted, [1] rows re-scored exactly, [2] queries redone densely
+                std::vector<uint32_t> cnt(b), fl(b);
+                LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->mv_cnt.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+                LGPU_CUDA(cudaMemcpyAsync(fl.data(), ws->mv_flags.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+                LGPU_CUDA(cudaStreamSynchronize(st));
+                for (uint32_t q = 0; q < b; q++) {
+                    g_filter_stats[0] += cnt[q]; g_filter_stats[1] += std::min(cnt[q], cap);
+                    g_filter_stats[2] += fl[q] ? 1 : 0;
+                }
+            }
+            qa = qb;
+        }
+    } else {
+        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / 2 / std::max<size_t>(ld * 4, 4), B));
+        for (uint32_t qa = 0; qa < B; qa += bs) {
+            const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
+            if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
+            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld);
+            SelectArgs sa{};
+            sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = N; sa.row_stride = ld;
+            sa.col_ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
+            sa.B = b; sa.k = k;
+            sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
+            sa.out_ids = d_ids + (size_t)qa * k; sa.out_dist = d_dist + (size_t)qa * k; sa.out_count = d_cnt + qa;
+            sa.allow = rf.bits; sa.allow_bits = rf.nbits;
+            launch_select(sa, st);
+        }
+    }
+    if (prof) {                     // exact path: [1] rows scored exactly; both: [3] queries
+        LGPU_CUDA(cudaStreamSynchronize(st));
+        if (!tc) g_filter_stats[1] = (uint64_t)B * N;
+        g_filter_stats[3] = B;
+    }
+}
+
+// the query vector offsets of a multivector call: [B+1], starting at 0, every query holding 1..MV_MAX_NQ vectors
+static void check_multivec_offsets(const uint32_t *q_off, uint32_t B)
+{
+    LGPU_REQUIRE(q_off != nullptr, "query offsets are null");
+    LGPU_REQUIRE(q_off[0] == 0, "query offsets must start at 0");
+    for (uint32_t b = 0; b < B; b++) {
+        LGPU_REQUIRE(q_off[b + 1] > q_off[b], "every multivector query needs at least one vector (offsets must increase)");
+        LGPU_REQUIRE(q_off[b + 1] - q_off[b] <= MV_MAX_NQ, "a multivector query holds at most 4096 vectors");
+    }
+}
+
+// host-buffer multivector call: stage the query vectors in, run, stage the results out.  Not captured into a CUDA
+// graph: the launch sequence depends on every query's vector count, not only on B.
+template <class Run>
+void multivec_host_call(lgpu_multivec *mv, const float *queries, const uint32_t *q_off, uint32_t B,
+                        const lgpu_search_params &sp, uint64_t *out_ids, float *out_dist, uint32_t *out_count, Run &&run)
+{
+    const Deadline deadline(sp.timeout_ms);
+    WsLease lease(mv->pool, nullptr, false);
+    Workspace *ws = lease.ws;
+    cudaStream_t st = lease.st;
+    const size_t tq = q_off[B], k = sp.k;
+    ws->q.ensure(std::max<size_t>(tq * mv->dim, 1) * 4);
+    ws->out_ids.ensure((size_t)B * k * 8);
+    ws->out_dist.ensure((size_t)B * k * 4);
+    ws->out_count.ensure((size_t)B * 4);
+    LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, tq * mv->dim * 4, cudaMemcpyHostToDevice, st));
+    run(ws, st, ws->q.as<float>(), ws->out_ids.as<uint64_t>(), ws->out_dist.as<float>(), ws->out_count.as<uint32_t>(),
+        deadline);
+    deadline.wait(st, ws->ev[7]);
+    LGPU_CUDA(cudaMemcpyAsync(out_ids, ws->out_ids.p, (size_t)B * k * 8, cudaMemcpyDeviceToHost, st));
+    LGPU_CUDA(cudaMemcpyAsync(out_dist, ws->out_dist.p, (size_t)B * k * 4, cudaMemcpyDeviceToHost, st));
+    LGPU_CUDA(cudaMemcpyAsync(out_count, ws->out_count.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    LGPU_CUDA(cudaStreamSynchronize(st));
+}
+
 template <class F> int guarded(F &&f)
 {
     try { f(); return LGPU_OK; }
@@ -2030,6 +2257,176 @@ int lgpu_binary_search_device(lgpu_binary *bxh, const uint8_t *d_queries, uint32
         require_device(bx->device);
         WsLease lease(bx->pool, (cudaStream_t)cuda_stream, true);
         binary_search_device(bx.h, lease.ws, lease.st, d_queries, B, *params, d_out_ids, d_out_dist, d_out_count);
+    });
+}
+
+int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
+                       const uint64_t *row_ids, int device, lgpu_multivec **out)
+{
+    lgpu_multivec *mv = nullptr;
+    int rc = guarded([&] {
+        LGPU_REQUIRE(out != nullptr && offsets != nullptr, "null argument");
+        LGPU_REQUIRE(dim >= 1 && dim <= MV_MAX_DIM, "multivector dimension must be in [1, 65536]");
+        LGPU_REQUIRE(offsets[0] == 0, "row offsets must start at 0");
+        uint64_t max_row = 0;
+        for (uint64_t r = 0; r < nrows; r++) {
+            LGPU_REQUIRE(offsets[r + 1] >= offsets[r], "row offsets must not decrease");
+            LGPU_REQUIRE(offsets[r + 1] - offsets[r] <= MV_MAX_ROW, "a multivector row holds at most 2^20 vectors");
+            max_row = std::max<uint64_t>(max_row, offsets[r + 1] - offsets[r]);
+        }
+        const uint64_t T = offsets[nrows];
+        LGPU_REQUIRE(T <= ((uint64_t)1 << 40), "a multivector column holds at most 2^40 vectors");
+        LGPU_REQUIRE(T == 0 || values != nullptr, "null vectors");
+        require_device(device);
+        mv = new lgpu_multivec();
+        mv->device = device; mv->nrows = nrows; mv->total = T; mv->dim = dim; mv->max_row = max_row;
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        mv->num_sms = prop.multiProcessorCount;
+        mv->h_offsets.assign(offsets, offsets + nrows + 1);
+        mv->vectors.ensure(std::max<size_t>((size_t)T * dim * 4, 16));
+        mv->ysqrt.ensure(std::max<size_t>((size_t)T * 4, 16));
+        mv->offsets.ensure((size_t)(nrows + 1) * 8);
+        LGPU_CUDA(cudaMemcpy(mv->offsets.p, offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice));
+        if (T) {
+            LGPU_CUDA(cudaMemcpy(mv->vectors.p, values, (size_t)T * dim * 4, cudaMemcpyHostToDevice));
+            launch_row_norms(mv->vectors.as<float>(), T, dim, mv->ysqrt.as<float>(), nullptr);
+        }
+        // the tensor-core operand: only when every stored vector normalises (a zero or non-finite vector has NaN pairs,
+        // which the approximate score cannot skip as the exact min does) and the shape suits the GEMM
+        if (T >= MV_TC_MIN_T && T < ((uint64_t)1 << 31) && nrows < 0xffffffffull && gemm_shape_supported(dim)) {
+            mv->vec_h.ensure((size_t)T * dim * 2);
+            DevBuf bad;
+            bad.ensure((size_t)T * 4);
+            launch_mv_normalize_f16(mv->vectors.as<float>(), T, dim, mv->vec_h.p, bad.as<uint32_t>(), nullptr);
+            std::vector<uint32_t> hb(T), cr(T);
+            LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, (size_t)T * 4, cudaMemcpyDeviceToHost));
+            bool ok = true;
+            for (uint64_t i = 0; i < T; i++) ok = ok && !hb[i];
+            for (uint64_t r = 0; r < nrows; r++)
+                for (uint64_t j = offsets[r]; j < offsets[r + 1]; j++) cr[j] = (uint32_t)r;
+            mv->col_row.ensure((size_t)T * 4);
+            LGPU_CUDA(cudaMemcpy(mv->col_row.p, cr.data(), (size_t)T * 4, cudaMemcpyHostToDevice));
+            mv->tc_ok = ok;
+        }
+        LGPU_CUDA(cudaDeviceSynchronize());
+        if (row_ids && nrows) {
+            mv->row_ids.ensure((size_t)nrows * 8);
+            LGPU_CUDA(cudaMemcpy(mv->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
+            mv->has_ids = true;
+        }
+        register_handle(mv);
+        *out = mv;
+    });
+    if (rc != LGPU_OK && mv) delete mv;
+    return rc;
+}
+
+void lgpu_multivec_close(lgpu_multivec *mv)
+{
+    if (!retire_handle(mv)) return;
+    cudaSetDevice(mv->device);
+    cudaDeviceSynchronize();
+    delete mv;
+}
+
+static void check_multivec_call(const void *q, const uint32_t *q_off, uint32_t B, const lgpu_search_params *p,
+                                const void *a, const void *b, const void *c)
+{
+    check_params(p);
+    LGPU_REQUIRE(B == 0 || (q && a && b && c), "null buffer");
+    if (B) check_multivec_offsets(q_off, B);
+}
+
+int lgpu_multivec_search(lgpu_multivec *mvh, const float *queries, const uint32_t *q_offsets, uint32_t B,
+                         const lgpu_search_params *params, uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return guarded([&] {
+        HandleRef<lgpu_multivec> mv(mvh, "multivector");
+        check_multivec_call(queries, q_offsets, B, params, out_ids, out_dist, out_count);
+        if (B == 0) return;
+        require_device(mv->device);
+        multivec_host_call(mv.h, queries, q_offsets, B, *params, out_ids, out_dist, out_count,
+                           [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
+                               const Deadline &dl) {
+                               multivec_search_device(mv.h, ws, st, dq, q_offsets, B, *params, di, dd, dc, RowFilter(), &dl);
+                           });
+    });
+}
+
+int lgpu_multivec_search_filtered(lgpu_multivec *mvh, const float *queries, const uint32_t *q_offsets, uint32_t B,
+                                  const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                                  uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return guarded([&] {
+        HandleRef<lgpu_multivec> mv(mvh, "multivector");
+        check_multivec_call(queries, q_offsets, B, params, out_ids, out_dist, out_count);
+        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
+        if (B == 0) return;
+        require_device(mv->device);
+        multivec_host_call(mv.h, queries, q_offsets, B, *params, out_ids, out_dist, out_count,
+                           [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
+                               const Deadline &dl) {
+                               const size_t words = (size_t)((allow_bits + 31) / 32);
+                               ws->allow.ensure(std::max<size_t>(words, 1) * 4);
+                               if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
+                               RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
+                               multivec_search_device(mv.h, ws, st, dq, q_offsets, B, *params, di, dd, dc, rf, &dl);
+                           });
+    });
+}
+
+int lgpu_multivec_search_device(lgpu_multivec *mvh, const float *d_queries, const uint32_t *q_offsets, uint32_t B,
+                                const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
+                                uint32_t *d_out_count, void *cuda_stream)
+{
+    return guarded([&] {
+        HandleRef<lgpu_multivec> mv(mvh, "multivector");
+        check_multivec_call(d_queries, q_offsets, B, params, d_out_ids, d_out_dist, d_out_count);
+        if (B == 0) return;
+        require_device(mv->device);
+        WsLease lease(mv->pool, (cudaStream_t)cuda_stream, true);
+        multivec_search_device(mv.h, lease.ws, lease.st, d_queries, q_offsets, B, *params, d_out_ids, d_out_dist,
+                               d_out_count);
+    });
+}
+
+int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
+                           uint64_t nrows, uint32_t dim, int device, float *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(offsets != nullptr && (nqv == 0 || (queries && out)), "null buffer");
+        LGPU_REQUIRE(gemm_shape_supported(dim), "the tensor-core MaxSim score needs a dimension that is a multiple of 8");
+        LGPU_REQUIRE(offsets[0] == 0, "row offsets must start at 0");
+        for (uint64_t r = 0; r < nrows; r++) LGPU_REQUIRE(offsets[r + 1] >= offsets[r], "row offsets must not decrease");
+        const uint64_t T = offsets[nrows];
+        LGPU_REQUIRE(T < ((uint64_t)1 << 31) && (T == 0 || values), "bad stored vectors");
+        require_device(device);
+        if (nqv == 0 || nrows == 0) return;
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        DevBuf q, x, qh, xh, bad, cr, M;
+        q.ensure((size_t)nqv * dim * 4); x.ensure(std::max<size_t>((size_t)T * dim * 4, 16));
+        qh.ensure((size_t)nqv * dim * 2); xh.ensure(std::max<size_t>((size_t)T * dim * 2, 16));
+        bad.ensure(std::max<size_t>(std::max<uint64_t>(T, nqv), 1) * 4); cr.ensure(std::max<size_t>(T, 1) * 4);
+        M.ensure((size_t)nqv * nrows * 4);
+        std::vector<uint32_t> hcr(T);
+        for (uint64_t r = 0; r < nrows; r++)
+            for (uint64_t j = offsets[r]; j < offsets[r + 1]; j++) hcr[j] = (uint32_t)r;
+        LGPU_CUDA(cudaMemcpy(q.p, queries, (size_t)nqv * dim * 4, cudaMemcpyHostToDevice));
+        if (T) {
+            LGPU_CUDA(cudaMemcpy(x.p, values, (size_t)T * dim * 4, cudaMemcpyHostToDevice));
+            LGPU_CUDA(cudaMemcpy(cr.p, hcr.data(), (size_t)T * 4, cudaMemcpyHostToDevice));
+        }
+        LGPU_CUDA(cudaMemset(M.p, 0, (size_t)nqv * nrows * 4));
+        launch_mv_normalize_f16(q.as<float>(), nqv, dim, qh.p, bad.as<uint32_t>(), nullptr);
+        launch_mv_normalize_f16(x.as<float>(), T, dim, xh.p, bad.as<uint32_t>(), nullptr);
+        MaxSimOut mo{};
+        mo.col_row = cr.as<uint32_t>(); mo.M = M.as<uint32_t>(); mo.ldM = nrows; mo.row_base = 0; mo.xdummy = x.as<float>();
+        launch_maxsim_gemm(qh.p, xh.p, nqv, T, dim, mo, prop.multiProcessorCount, nullptr);
+        std::vector<uint32_t> keys((size_t)nqv * nrows);
+        LGPU_CUDA(cudaMemcpy(keys.data(), M.p, keys.size() * 4, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < keys.size(); i++) out[i] = keys[i] ? key_f32(keys[i]) : NAN;
     });
 }
 

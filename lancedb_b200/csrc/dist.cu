@@ -231,6 +231,42 @@ __global__ void pair_distance_kernel(const float *__restrict__ Q, const float *_
     if (hl == 0) out[pair] = v;
 }
 
+// exact MaxSim re-score of the multivector shortlist, half a warp per (query, candidate row): for each query vector i
+// in order, the NaN-skipping min over the row's vectors j of 1 - xy / |q_i| / |v_j| (xy in lance's lane order: the
+// same roundings as dist_matrix_kernel mode 2), added onto a sum that starts at 0.0f -- the exact path's bits
+__global__ void mv_rescore_kernel(const float *__restrict__ Q, const uint32_t *__restrict__ q_off, uint32_t qa,
+                                  const float *__restrict__ xnorm, const float *__restrict__ V,
+                                  const float *__restrict__ ysqrt, const uint64_t *__restrict__ offsets,
+                                  const uint64_t *__restrict__ row_ids, uint32_t d, uint32_t B,
+                                  const uint32_t *__restrict__ cand, const uint32_t *__restrict__ count, uint32_t cap,
+                                  float *__restrict__ out, uint64_t *__restrict__ ids)
+{
+    pdl_entry();
+    const uint64_t pair = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 4;
+    const int lane = threadIdx.x & 31, hl = lane & 15, hbase = lane & 16;
+    const unsigned hmask = 0xffffu << hbase;
+    if (pair >= (uint64_t)B * cap) return;                  // whole half-warp exits together
+    const uint32_t b = (uint32_t)(pair / cap), slot = (uint32_t)(pair % cap);
+    if (slot >= min(count[b], cap)) {
+        if (hl == 0) { out[pair] = CUDART_NAN_F; ids[pair] = UINT64_MAX; }
+        return;
+    }
+    const uint32_t r = cand[pair];
+    const uint64_t j0 = offsets[r], j1 = offsets[r + 1];
+    float s = 0.f;
+    for (uint32_t i = q_off[qa + b]; i < q_off[qa + b + 1]; i++) {
+        const float *x = Q + (size_t)i * d;
+        float m = CUDART_NAN_F;
+        for (uint64_t j = j0; j < j1; j++) {
+            const float xy = halfwarp_dot(x, V + j * d, d, hl, hmask, hbase);
+            const float c = __fsub_rn(1.0f, __fdiv_rn(__fdiv_rn(xy, xnorm[i]), ysqrt[j]));
+            if (c < m || m != m) m = c;
+        }
+        s = __fadd_rn(s, m);
+    }
+    if (hl == 0) { out[pair] = s; ids[pair] = row_ids ? row_ids[r] : r; }
+}
+
 // ---- the coarse step after the tensor-core GEMM, in one kernel (one CTA per query):
 // S[q][x] = |x|^2 - 2 bf16(q).bf16(x) differs from |q - x|^2 - |q|^2 by at most E_q (gemm.cu's band).  (1) an upper
 // bound tau of the k-th smallest S of the row by counting bisection; (2) every column with S <= tau + 2 E_q -- a
@@ -467,6 +503,18 @@ void launch_pair_distance(const float *Q, const float *V, const uint64_t *pos, u
     if (B == 0 || nc == 0) return;
     uint64_t threads = (uint64_t)B * nc * 16;
     launch_k(pair_distance_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, V, pos, B, nc, d, metric, out); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+                       const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
+                       const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
+                       cudaStream_t st)
+{
+    if (B == 0 || cap == 0) return;
+    const uint64_t threads = (uint64_t)B * cap * 16;
+    launch_k(mv_rescore_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, q_off, qa, xnorm, V, ysqrt,
+             offsets, row_ids, d, B, cand, count, cap, out, ids); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

@@ -109,6 +109,30 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
+// the same with fp16 operands (the multivector MaxSim score, F16MaxSim)
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
 // D[64 x 128] (+)= popc(A[64 x 256] AND B[128 x 256]^T), both b1 K-major in shared memory (32 bytes of K per row, the
 // same bytes as one k16 bf16 slice, so the descriptors and the fragment layout are those of wgmma_m64n128k16)
 __device__ __forceinline__ void wgmma_m64n128k256_b1(int (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
@@ -151,7 +175,7 @@ __device__ __forceinline__ void fence_acc(int (&d)[64])
 // term popc(x) (s32), S = popc(q) + popc(x) - 2 popc(q AND x) = popc(q XOR x) exactly: every term is an integer
 // below 2^24, so S is the final Hamming distance and needs no re-score.
 struct Bf16Dist {
-    static constexpr bool BIN = false;
+    static constexpr bool BIN = false, MAXSIM = false;
     static constexpr int K_BOX = GK;          // tensor-map elements per stage row (128 bytes)
     using Acc = float; using Row = float; using Row2 = float2; using Filter = GemmFilter;
     __device__ static __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k16(d, a, b, acc); }
@@ -159,12 +183,23 @@ struct Bf16Dist {
     __device__ static __forceinline__ float score(float xn, float acc, int) { return xn - 2.0f * acc; }
 };
 struct B1Hamming {
-    static constexpr bool BIN = true;
+    static constexpr bool BIN = true, MAXSIM = false;
     static constexpr int K_BOX = 2 * GK;      // the map is over bytes
     using Acc = int; using Row = int; using Row2 = int2; using Filter = HamFilter;
     __device__ static __forceinline__ void mma(int (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k256_b1(d, a, b, acc); }
     __device__ static __forceinline__ int qterm(const HamFilter &f, uint32_t q) { return __ldg(f.qpop + q); }
     __device__ static __forceinline__ float score(int xn, int acc, int pq) { return (float)(pq + xn - 2 * acc); }
+};
+// F16MaxSim: fp16 copies of the NORMALISED query and stored vectors of a multivector column, acc = the approximate
+// cosine similarity.  Its epilogue writes nothing dense: per (query vector, document) it keeps the largest similarity
+// over the document's run of columns (MaxSimOut, kernels.cuh), one atomicMax per run of a thread's columns.
+struct F16MaxSim {
+    static constexpr bool BIN = false, MAXSIM = true;
+    static constexpr int K_BOX = GK;
+    using Acc = float; using Row = float; using Row2 = float2; using Filter = MaxSimOut;
+    __device__ static __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k16_f16(d, a, b, acc); }
+    __device__ static __forceinline__ int qterm(const MaxSimOut &, uint32_t) { return 0; }
+    __device__ static __forceinline__ float score(float, float acc, int) { return acc; }
 };
 
 // LIST: the filtering epilogue for DENSE hit rates (coarse step at many lists), see the epilogue; a separate
@@ -261,6 +296,36 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         fence_acc(acc);
         if (leader) mbar_arrive(empty_bar + 8 * prev);
 
+        if constexpr (Pol::MAXSIM) {
+            // MaxSim epilogue: the thread's 32 columns of row q ascend (c0 + 8 j + e), so the columns of one document
+            // form one run; the run's largest similarity goes to M[q][doc - row_base] by an ordered-key atomicMax
+            // (M zeroed by the caller: key 0 = no column seen)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const uint32_t q = r0 + 8 * h;
+                if (q >= B) continue;
+                uint32_t cur = 0xffffffffu;
+                float best = 0.f;
+#pragma unroll
+                for (int j = 0; j < 16; j++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const uint64_t x = c0 + 8 * j + e;
+                        if (x < N) {
+                            const uint32_t doc = __ldg(flt.col_row + x);
+                            const float v = acc[4 * j + 2 * h + e];
+                            if (doc != cur) {
+                                if (cur != 0xffffffffu) atomicMax(flt.M + (size_t)q * flt.ldM + (cur - flt.row_base), f32_key(best));
+                                cur = doc; best = v;
+                            } else {
+                                best = fmaxf(best, v);
+                            }
+                        }
+                    }
+                if (cur != 0xffffffffu) atomicMax(flt.M + (size_t)q * flt.ldM + (cur - flt.row_base), f32_key(best));
+            }
+            continue;
+        }
         if constexpr (LIST) {
             // Filtering epilogue for DENSE hit rates (the coarse step's lists: ~1.5 % of the columns pass).  One returning
             // atomic per hit, as in the sparse form below, would serialise on the query's counter; instead the 4 lanes
@@ -412,15 +477,16 @@ EncodeTiledFn get_encode_fn()
     return fn;
 }
 
-// bf16 row-major [rows][d] matrix (bytes: u8 [rows][d]), box = box_rows x 128 bytes, 128-byte swizzle, OOB = zeros
-CUtensorMap make_map(const void *ptr, uint64_t rows, uint32_t d, uint32_t box_rows, bool bytes = false)
+// bf16 (f16: fp16) row-major [rows][d] matrix (bytes: u8 [rows][d]), box = box_rows x 128 bytes, 128-byte swizzle,
+// OOB = zeros
+CUtensorMap make_map(const void *ptr, uint64_t rows, uint32_t d, uint32_t box_rows, bool bytes = false, bool f16 = false)
 {
     CUtensorMap m;
     cuuint64_t dims[2] = {d, rows};
     cuuint64_t strides[1] = {(cuuint64_t)d * (bytes ? 1 : 2)};
     cuuint32_t box[2] = {(cuuint32_t)(bytes ? 2 * GK : GK), box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = get_encode_fn()(&m, bytes ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+    CUresult r = get_encode_fn()(&m, bytes ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : (f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16), 2,
                                  const_cast<void *>(ptr), dims, strides, box, estr,
                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -635,6 +701,22 @@ void launch_ham_gemm(const void *Qp, const void *Xp, const uint32_t *xpop, const
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, reinterpret_cast<const int *>(xpop), out, ld_out,
              B, N, (uint32_t)((nbytes_pad + 2 * GK - 1) / (2 * GK)), flt); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_maxsim_gemm(const void *Qh, const void *Xh, uint32_t B, uint64_t N, uint32_t d, const MaxSimOut &out,
+                        int num_sms, cudaStream_t st)
+{
+    if (B == 0 || N == 0) return;
+    LGPU_REQUIRE(gemm_shape_supported(d), "tensor-core path needs a dimension that is a multiple of 8");
+    CUtensorMap mq = make_map(Qh, B, d, GM, false, true);
+    CUtensorMap mx = make_map(Xh, N, d, GN, false, true);
+    const uint64_t tiles = (uint64_t)((B + GM - 1) / GM) * ((N + GN - 1) / GN);
+    const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)num_sms);
+    auto kern = gemm_dist_kernel<false, F16MaxSim>;
+    LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
+    launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, out.xdummy, nullptr, (uint64_t)0, B, N,
+             (uint32_t)((d + GK - 1) / GK), out); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

@@ -270,6 +270,55 @@ void launch_ham_flag_list(const uint32_t *flags, uint32_t B, uint32_t chunk, uin
 // thr[q] = dist[q][k-1] when cnt[q] >= k, else +inf (the sample's k-th smallest distance, an upper bound of the k-th
 // smallest over all rows)
 void launch_ham_threshold(const float *dist, const uint32_t *cnt, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
+
+// ---------------- multivector (MaxSim) columns, tensor-core score (gemm.cu F16MaxSim) -----------
+// M[q][col_row[x] - row_base] = f32_key(max over the columns x of that document of fp16(Q[q]) . fp16(X[x])) by
+// atomicMax (M zeroed by the caller); Q [B][d], X [N][d] fp16 of the normalised vectors, d a multiple of 8.
+struct MaxSimOut : GemmFilter {   // (GemmFilter's fields stay unset)
+    const uint32_t *col_row;      // [N] document (row) of each column
+    uint32_t *M;                  // [B][ldM]
+    uint64_t ldM;
+    uint32_t row_base;
+    const float *xdummy;          // any [N] f32 array (the kernel's per-column term is unused by this policy)
+};
+void launch_maxsim_gemm(const void *Qh, const void *Xh, uint32_t B, uint64_t N, uint32_t d, const MaxSimOut &out,
+                        int num_sms, cudaStream_t st);
+// out[n][d] = fp16(x / |x|) (|x| = sqrt(lance dot)); bad[n] = 1 (and the row zeroed) when |x| is 0 or not finite or
+// a component is not finite
+void launch_mv_normalize_f16(const float *X, uint64_t n, uint32_t d, void *out, uint32_t *bad, cudaStream_t st);
+// the per-query error band of the approximate MaxSim distance: |approx - exact| <= mv_band(nq, d) (multivec.cu)
+float mv_band_host(uint32_t nq, uint32_t d);
+// A[b - qa][r] = sum over query b's vectors i of (1 - key_f32(M[i - i_base][r])), NaN when some M entry is 0 (empty row)
+void launch_mv_approx_sum(const uint32_t *M, uint64_t ldM, const uint32_t *q_off, uint32_t qa, uint32_t qb,
+                          uint32_t i_base, uint64_t N, float *A, uint64_t ldA, int num_sms, cudaStream_t st);
+// thr[b] = dist[b][k-1] + 2 E_b when cnt[b] >= k, else +inf; E_b = mv_band(nq_b, d)
+void launch_mv_threshold(const float *dist, const uint32_t *cnt, const uint32_t *q_off, uint32_t qa, uint32_t B,
+                         uint32_t k, uint32_t d, float *thr, cudaStream_t st);
+// every row r with A[b][r] <= thr[b] is appended to cand[b][.] (count[b] zeroed by the caller, may exceed cap)
+void launch_mv_admit(const float *A, uint64_t ldA, uint32_t B, uint64_t N, const float *thr, uint32_t cap,
+                     uint32_t *count, uint32_t *cand, cudaStream_t st);
+// flags[b] = count[b] > cap or a vector of query b is bad; vflags[i] = flags of the query of vector i; *gate = any flag
+void launch_mv_flags(const uint32_t *count, uint32_t cap, const uint32_t *qbad, const uint32_t *q_off, uint32_t qa,
+                     uint32_t B, uint32_t *flags, uint32_t *vflags, uint32_t *gate, cudaStream_t st);
+// exact re-score (dist.cu): for slot s < min(count[b], cap): out[b][s] = MaxSim distance of query b and row cand[b][s]
+// in the oracle's arithmetic, ids[b][s] = its id; other slots NaN / UINT64_MAX
+void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+                       const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
+                       const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
+                       cudaStream_t st);
+
+// ---------------- multivector (MaxSim) columns, exact path (multivec.cu) ----------------------
+// M[i][r] = min over row r0 + r's stored vectors j of P[i][j - offsets[r0]] (NaN skipped; NaN if none), for the nqv
+// query vectors of P [nqv][ldP] and the nr rows r0..r0+nr-1 (offsets: device [nrows+1])
+// gate (optional, device): 0 = nothing to do (the fix-up pass with no flagged query)
+void launch_mv_rowmin(const float *P, uint64_t ldP, uint32_t nqv, const uint64_t *offsets, uint64_t r0, uint32_t nr,
+                      float *M, uint64_t ldM, int num_sms, cudaStream_t st, const uint32_t *gate = nullptr);
+// for queries b in [b_lo, b_hi) (q_off: device [B+1] vector offsets): D[b - qa][col0 + r] = running sum over the
+// query's vectors i in [i0, i1) of M[i - i0][r], in order of i, started at 0.0f at the query's first vector
+void launch_mv_rowsum(const float *M, uint64_t ldM, const uint32_t *q_off, uint32_t b_lo, uint32_t b_hi, uint32_t qa,
+                      uint32_t i0, uint32_t i1, uint32_t nr, float *D, uint64_t ldD, uint64_t col0, int num_sms,
+                      cudaStream_t st, const uint32_t *only = nullptr, const uint32_t *gate = nullptr);
+// (only: optional [B] per-query flags indexed like q_off, queries whose flag is 0 are skipped)
 // filtering epilogue on an existing dense score matrix D[B][ld] (see gemm.cu)
 void launch_filter_dense(const float *D, uint64_t ld, uint32_t B, uint64_t N, const GemmFilter &flt, cudaStream_t st);
 void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,

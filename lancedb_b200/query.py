@@ -30,11 +30,15 @@ class LanceVectorQueryBuilder:
         if isinstance(query, (list, tuple)) and (len(query) == 0 or (isinstance(query[0], (list, tuple)) and len(query[0]) == 0)):
             raise ValueError("Vector query must be a non-empty list")      # ensure_vector_query, query.py:332-350
         q = np.asarray(query, dtype=np.float32)      # every query vector is cast to Float32 (query.rs:1013)
+        # on a multivector column a 2-D query is ONE query of several vectors, with no query_index column
+        # (rust/lancedb/src/table/query.rs:180-199; python/python/lancedb/query.py:3376-3382)
+        is_mv = getattr(table, "_is_multivec", None)
+        self._multivector = bool(is_mv(vector_column)) if is_mv is not None else False
         if q.ndim == 1:
             q = q[None, :]
             self._multi = False
         elif q.ndim == 2:
-            self._multi = q.shape[0] > 1
+            self._multi = q.shape[0] > 1 and not self._multivector
         else:
             raise ValueError("query must be a vector or a list of vectors")
         self._query = np.ascontiguousarray(q)
@@ -184,7 +188,7 @@ class LanceVectorQueryBuilder:
             allow_mask=None if (mask is None or self._postfilter) else mask,
             max_nprobes=max_nprobes, timeout_ms=timeout_ms)
         out = []
-        for qi in range(self._query.shape[0]):
+        for qi in range(len(cnt)):                         # one result list per query (a multivector query is one)
             n = int(cnt[qi])
             row_ids, row_dist = ids[qi, :n], dist[qi, :n]
             if mask is not None and self._postfilter:              # filter the vector search's results

@@ -57,8 +57,16 @@ def _to_arrow_table(data, schema: Optional[pa.Schema] = None) -> pa.Table:
 
 
 def _vector_columns(schema: pa.Schema) -> List[str]:
-    return [f.name for f in schema if pa.types.is_fixed_size_list(f.type) and
-            (pa.types.is_floating(f.type.value_type) or pa.types.is_uint8(f.type.value_type))]
+    return [f.name for f in schema if (pa.types.is_fixed_size_list(f.type) and
+            (pa.types.is_floating(f.type.value_type) or pa.types.is_uint8(f.type.value_type))) or
+            _is_multivec_type(f.type)]
+
+
+def _is_multivec_type(t: pa.DataType) -> bool:
+    """list<fixed_size_list<f16|f32|f64, dim>> (or large_list): a multivector column, searched by late interaction
+    (rust/lancedb/src/table/query.rs:180-199, the `DataType::List` branch)."""
+    return ((pa.types.is_list(t) or pa.types.is_large_list(t)) and pa.types.is_fixed_size_list(t.value_type) and
+            pa.types.is_floating(t.value_type.value_type))
 
 
 def _is_binary_type(t: pa.DataType) -> bool:
@@ -83,6 +91,7 @@ class Table:
         self._device = device
         self._flat: Dict[str, _native.GpuFlat] = {}
         self._binary: Dict[str, _native.GpuBinary] = {}
+        self._multivec: Dict[str, _native.GpuMultivec] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
         self._index_data: Dict[str, IvfPqIndexData] = {}
 
@@ -121,10 +130,26 @@ class Table:
         return np.asarray(col.flatten().to_numpy(zero_copy_only=False), np.float32).reshape(-1, dim)
 
     def _dim(self, column: str) -> int:
-        return self._data.schema.field(column).type.list_size
+        t = self._data.schema.field(column).type
+        return t.value_type.list_size if _is_multivec_type(t) else t.list_size
 
     def _is_binary(self, column: str) -> bool:
         return _is_binary_type(self._data.schema.field(column).type)
+
+    def _is_multivec(self, column: str) -> bool:
+        return _is_multivec_type(self._data.schema.field(column).type)
+
+    def _multivec_rows(self, column: str):
+        """(values [T, dim] f32, offsets [N+1] u64) of a multivector column; a null row holds no vectors.  Stored
+        float16 / float64 elements are upcast to f32."""
+        col = self._data.column(column).combine_chunks()
+        lens = col.value_lengths().fill_null(0).to_numpy(zero_copy_only=False).astype(np.int64)
+        inner = col.flatten()                               # skips the values behind null rows
+        if inner.null_count:
+            raise ValueError(f"multivector column {column!r} holds a null vector inside a row")
+        dim = col.type.value_type.list_size
+        vals = np.asarray(inner.flatten().to_numpy(zero_copy_only=False), np.float32).reshape(-1, dim)
+        return vals, _native.multivec_offsets(lens)
 
     def _binary_vectors(self, column: str) -> np.ndarray:
         col = self._data.column(column).combine_chunks()
@@ -142,6 +167,8 @@ class Table:
         column = vector_column_name or self._infer_vector_column(None)
         if self._is_binary(column):
             raise NotImplementedError("no index over binary vectors on the GPU path: search them flat (hamming)")
+        if self._is_multivec(column):
+            raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
         if column in self._index and not replace:
             raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")   # python/python/tests/test_index.py:357
         dev = None
@@ -221,6 +248,16 @@ class Table:
             if bx is None:
                 bx = self._binary[column] = _native.GpuBinary(self._binary_vectors(column), device=self._device)
             return bx.search(q, k=k, lower=lower, upper=upper, allow=allow, allow_bits=allow_bits, timeout_ms=timeout_ms)
+        if self._is_multivec(column):              # rust/lancedb/src/table/query.rs:180-199: ONE query of nq vectors
+            if distance_type is not None and distance_type != "cosine":
+                raise ValueError(f"distance type {distance_type!r} is not supported on multivector column {column!r}: "
+                                 "only cosine is")
+            mv = self._multivec.get(column)
+            if mv is None:
+                vals, off = self._multivec_rows(column)
+                mv = self._multivec[column] = _native.GpuMultivec(vals, off, device=self._device)
+            return mv.search([np.asarray(queries, np.float32)], k=k, lower=lower, upper=upper, allow=allow,
+                             allow_bits=allow_bits, timeout_ms=timeout_ms)
         if distance_type == "hamming":
             raise ValueError(f"distance type 'hamming' needs a binary (fixed_size_list<uint8>) column; {column!r} "
                              "holds floats")
