@@ -172,6 +172,37 @@ int lgpu_merge_topk_device(int device, uint32_t nlists, uint32_t B, uint32_t k,
                            uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count,
                            void *cuda_stream);
 
+/* ---- IVF_SQ (lance `IvfSq`, rust/lancedb/src/index/vector.rs:216-256): the same IVF partitions, each row stored as
+ * dim 8-bit scalar codes instead of PQ codes.  One global range [lo, hi] (f64) quantises every component:
+ *     code(v) = sat_u8(((double)v - lo) * 255.0 / (hi - lo))
+ * evaluated left to right in f64, truncated toward zero, below 0 -> 0, above 255 -> 255, NaN -> 0, and 0 when lo == hi
+ * (lance's scale_to_u8 [lance, recalled]).  Rows are encoded by the builder (normalised first for cosine); queries are
+ * encoded on the device with the same f64 operations (after normalisation for cosine).
+ *     _distance = (float) sum_i (k_i - q_i)^2
+ * summed exactly in integers, then rounded to nearest f32, for l2 and cosine alike (not halved for cosine), in code
+ * units; refine_factor re-ranks with exact f32 distances on desc.vectors.  dot is not supported (LGPU_INVALID_INPUT).
+ * Partition assignment is find_partitions (lgpu_ivf_assign), there are no residuals.  The handle is an ordinary
+ * lgpu_index: lgpu_search, _filtered, _device, _async and _coalesced serve it with the IVF_PQ semantics of k, nprobes,
+ * maximum_nprobes, prefilter, distance_range (on the SQ distance, before refine), refine_factor and timeout_ms.
+ * lgpu_search_sharded*, lgpu_debug_filter_bounds and lgpu_debug_partition_distances reject it. */
+#define LGPU_SQ_MAX_DIM 65536     /* the exact sum stays below 2^32 */
+typedef struct {
+    uint32_t abi_version;         /* LGPU_ABI_VERSION */
+    uint32_t dim;                 /* 1 .. LGPU_SQ_MAX_DIM */
+    uint32_t nlist;
+    int32_t  metric;              /* LGPU_L2 or LGPU_COSINE */
+    int32_t  device;
+    uint32_t reserved;            /* 0 */
+    uint64_t nrows;
+    double   lo, hi;              /* quantiser bounds, finite, lo <= hi */
+    const float    *centroids;    /* [nlist][dim] */
+    const uint64_t *part_offsets; /* [nlist+1] */
+    const uint8_t  *codes;        /* [nrows][dim] row codes in partition order */
+    const uint64_t *row_ids;      /* [nrows] */
+    const float    *vectors;      /* optional [nrows][dim] raw vectors (refine_factor); NULL if absent */
+} lgpu_ivf_sq_desc;
+int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *desc, lgpu_index **out);
+
 /* ---- partition-sharded search across GPUs (SURVEY.md 8e; the reference is single-process, so there is no
  * reference interface to replace -- this is what north_star adds for an index larger than one GPU's HBM).
  * One process (or thread) per GPU.  Centroids and codebook are replicated, every partition's codes and row ids
@@ -321,6 +352,11 @@ int lgpu_debug_gemm(const float *queries, const float *vectors, uint32_t B, uint
 /* the binary tensor-core kernel alone: out[q][x] = Hamming distance of queries[q] and vectors[x] (host buffers,
  * queries [B][nbytes], vectors [N][nbytes], out [B][N] u32) */
 int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint32_t B, uint64_t N, uint32_t nbytes,
+                            int device, uint32_t *out);
+/* the IVF_SQ scan kernel alone, on one partition of the N rows that every query probes: out[q][x] = sum_i
+ * (x_codes[x][i] - q_codes[q][i])^2, the exact u32 sum (host buffers: q_codes [B][dim], x_codes [N][dim], out [B][N];
+ * dim <= 65536, B x N < 2^32) */
+int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x_codes, uint64_t N, uint32_t dim,
                             int device, uint32_t *out);
 /* the multivector tensor-core score alone: out[i][r] = the largest fp16(q_i / |q_i|) . fp16(v / |v|) (f32 accumulation)
  * over row r's vectors v, NaN for an empty row (host buffers: queries [nqv][dim], values [offsets[nrows]][dim],

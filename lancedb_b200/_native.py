@@ -36,6 +36,7 @@ EXPORTS = [
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
     "lgpu_multivec_open", "lgpu_multivec_close", "lgpu_multivec_search", "lgpu_multivec_search_filtered",
     "lgpu_multivec_search_device", "lgpu_debug_maxsim_gemm",
+    "lgpu_ivf_sq_open", "lgpu_debug_sq_distances",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -49,6 +50,16 @@ class IndexDesc(C.Structure):
         ("nrows", C.c_uint64),
         ("centroids", C.c_void_p), ("codebook", C.c_void_p), ("part_offsets", C.c_void_p),
         ("codes", C.c_void_p), ("row_ids", C.c_void_p), ("vectors", C.c_void_p),
+    ]
+
+
+class SqDesc(C.Structure):
+    """lgpu_ivf_sq_desc"""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("dim", C.c_uint32), ("nlist", C.c_uint32), ("metric", C.c_int32),
+        ("device", C.c_int32), ("reserved", C.c_uint32), ("nrows", C.c_uint64), ("lo", C.c_double), ("hi", C.c_double),
+        ("centroids", C.c_void_p), ("part_offsets", C.c_void_p), ("codes", C.c_void_p), ("row_ids", C.c_void_p),
+        ("vectors", C.c_void_p),
     ]
 
 
@@ -135,6 +146,8 @@ def load():
     lib.lgpu_multivec_search_filtered.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
     lib.lgpu_multivec_search_device.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
+    lib.lgpu_ivf_sq_open.argtypes = [C.POINTER(SqDesc), C.POINTER(vp)]
+    lib.lgpu_debug_sq_distances.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -277,6 +290,30 @@ class GpuIvfPq:
         out = np.empty(n_p, np.float32)
         check(load().lgpu_debug_partition_distances(self._h, _ptr(q), int(part), _ptr(out)))
         return out
+
+
+class GpuIvfSq(GpuIvfPq):
+    """An IVF_SQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_sq_open, so every search entry point of GpuIvfPq
+    serves it.  _distance is the exact integer sum of squared code differences as f32 (l2 and cosine alike)."""
+
+    def __init__(self, data, device: int = 0, with_vectors: bool = True):
+        lib = load()
+        if data.metric not in ("l2", "cosine"):
+            raise ValueError(f"IVF_SQ supports the l2 and cosine distance types, not {data.metric!r}")
+        data.validate()
+        self.dim, self.nlist, self.metric = data.dim, data.nlist, data.metric
+        self.lo, self.hi = float(data.lo), float(data.hi)
+        self.device = device
+        vec = data.vectors if with_vectors else None
+        keep = [np.ascontiguousarray(data.centroids, np.float32), np.ascontiguousarray(data.part_offsets, np.uint64),
+                np.ascontiguousarray(data.codes, np.uint8), np.ascontiguousarray(data.row_ids, np.uint64),
+                None if vec is None else np.ascontiguousarray(vec, np.float32)]
+        desc = SqDesc(ABI_VERSION, data.dim, data.nlist, METRICS[data.metric], device, 0, data.nrows, self.lo, self.hi,
+                      _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]))
+        h = C.c_void_p()
+        check(lib.lgpu_ivf_sq_open(C.byref(desc), C.byref(h)))
+        self._h = h
+        self.has_vectors = vec is not None
 
 
 class GpuFlat:
@@ -621,6 +658,16 @@ def debug_hamming_gemm(queries, vectors, device: int = 0) -> np.ndarray:
         raise ValueError("queries and vectors must be [rows, bytes] arrays with the same bytes per row")
     out = np.empty((q.shape[0], x.shape[0]), np.uint32)
     check(load().lgpu_debug_hamming_gemm(_ptr(q), _ptr(x), q.shape[0], x.shape[0], q.shape[1], device, _ptr(out)))
+    return out
+
+
+def debug_sq_distances(q_codes, x_codes, device: int = 0) -> np.ndarray:
+    """The IVF_SQ scan kernel alone: [B, N] u32 exact sums of squared code differences."""
+    q = np.ascontiguousarray(q_codes, np.uint8); x = np.ascontiguousarray(x_codes, np.uint8)
+    if q.ndim != 2 or x.ndim != 2 or q.shape[1] != x.shape[1]:
+        raise ValueError("q_codes and x_codes must be [rows, dim] uint8 arrays with the same dim")
+    out = np.empty((q.shape[0], x.shape[0]), np.uint32)
+    check(load().lgpu_debug_sq_distances(_ptr(q), q.shape[0], _ptr(x), x.shape[0], q.shape[1], device, _ptr(out)))
     return out
 
 

@@ -127,6 +127,7 @@ struct Workspace {
     DevBuf mv_qoff, mv_P, mv_M;         // multivector search: query vector offsets, pairwise cosd block, per-row minima
     DevBuf mv_qh, mv_qbad, mv_Mk, mv_A; // ... tensor-core path: fp16 queries, bad vectors, max-similarity keys, approx dist
     DevBuf mv_kd, mv_ki, mv_kc, mv_thr, mv_cnt, mv_cand, mv_flags, mv_vflags, mv_gate, mv_ex, mv_exid;   // shortlist
+    DevBuf sq_q, sq_qq;                 // IVF_SQ search: query codes [B][dim_pad], their squared sums
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -261,6 +262,11 @@ struct lgpu_index {
     float cent_max = 0.f, cent_err = 0.f;   // max |c|, max |bf16(c) - c| (the error band, kernels.cuh tc_band)
     bool has_tc = false;
     bool has_vectors = false;
+    // IVF_SQ (lgpu_ivf_sq_open): `codes` holds [nrows][dim_pad] u8 row codes, `sq_xx` the sum of each row's squared codes
+    bool is_sq = false;
+    uint32_t dim_pad = 0;
+    double sq_lo = 0.0, sq_hi = 0.0;
+    DevBuf sq_xx;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
     WorkspacePool pool;
@@ -628,7 +634,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
     // tiny batches (a single query, a micro-batch): one CTA per (query, probe) pair with the exact table in shared
     // memory (small.cu) -- 4 launches instead of ~25; LGPU_SMALL_SLOTS = 0 disables
     const ScanModes modes = scan_modes();
-    const bool small_path = d_ids && !forced_probes && !only && slots <= modes.small_slots &&
+    const bool sq = ix->is_sq;                           // IVF_SQ: no tables, no filter; the SQ scan is exact
+    const bool small_path = !sq && d_ids && !forced_probes && !only && slots <= modes.small_slots &&
                             small_scan_smem(ix->m, dim) <= 200 * 1024 &&
                             (size_t)slots * ix->pad_prefix[1] * 4 <= workspace_budget();
     const bool filter_scan = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && !forced_probes &&
@@ -742,6 +749,11 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         }
     }
     launch_tables();
+    if (sq) {
+        ws->sq_q.ensure((size_t)B * ix->dim_pad); ws->sq_qq.ensure((size_t)B * 4);
+        launch_sq_encode(qsearch, B, dim, ix->dim_pad, ix->sq_lo, ix->sq_hi, ws->sq_q.as<uint8_t>(),
+                         ws->sq_qq.as<uint32_t>(), st);
+    }
     mark();
     if (small_path) {
         mark();                                          // (no regrouping)
@@ -813,7 +825,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         ga.tile_desc = ws->tile_desc.as<TileDesc>(); ga.max_tiles = (uint32_t)max_tiles;
     }
     ga.only = only;
-    ga.rows_tile = filter_scan ? SCAN3_ROWS_TILE : SCAN_ROWS_TILE_MID;
+    ga.rows_tile = filter_scan ? SCAN3_ROWS_TILE : (sq ? SQ_ROWS_TILE : SCAN_ROWS_TILE_MID);
     launch_group(ga, cs);
     mark();
     if (filter_scan) {
@@ -998,7 +1010,16 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         launch_select(sf, st);
         mark();
     } else {
-        launch_scan2(sc, ix->dsub, ix->num_sms, st);
+        if (sq) {
+            SqScanArgs qa{};
+            qa.codes = ix->codes.as<uint8_t>(); qa.xx = ix->sq_xx.as<uint32_t>();
+            qa.qcodes = ws->sq_q.as<uint8_t>(); qa.qq = ws->sq_qq.as<uint32_t>(); qa.dim_pad = ix->dim_pad;
+            qa.total_tiles = ga.total_tiles; qa.tile_counter = ga.tile_counter; qa.tile_desc = ga.tile_desc;
+            qa.dist_out = ws->dist_out.as<float>();
+            launch_sq_scan(qa, 2 * ix->num_sms, st);
+        } else {
+            launch_scan2(sc, ix->dsub, ix->num_sms, st);
+        }
         mark();
         if (!d_ids) { mark(); mark(); return; }     // debug: distances only
         sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
@@ -1060,7 +1081,7 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
         cudaEventElapsedTime(&g_stage_ms[6], ws->ev[0], ws->ev[6]);
         unsigned long long rows = 0;
         LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
-        g_scanned_bytes = (uint64_t)rows * ix->m;
+        g_scanned_bytes = (uint64_t)rows * (ix->is_sq ? ix->dim : ix->m);   // code bytes per row
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
         if (ws->stats_mode == 1) LGPU_CUDA(cudaMemcpy(g_filter_stats, ws->c_stats.p, 32, cudaMemcpyDeviceToHost));
         else if (ws->stats_mode == 2) {                       // dense filter: queries the band check could not prove
@@ -1621,6 +1642,100 @@ static inline void make_key(uint64_t (&key)[4], uint64_t tag, uint32_t B, const 
     key[3] = ((uint64_t)lo | ((uint64_t)hi << 32)) ^ scan_modes().signature();
 }
 
+// the partition layout every IVF index shares (lgpu_index_open, lgpu_ivf_sq_open): checked before any device work
+static void check_ivf_layout(uint32_t dim, uint32_t nlist, int metric, uint64_t nrows, const float *centroids,
+                             const uint64_t *part_offsets, const void *codes, const uint64_t *row_ids)
+{
+    LGPU_REQUIRE(dim > 0 && nlist > 0, "dim and nlist must be positive");
+    LGPU_REQUIRE(metric == LGPU_L2 || metric == LGPU_COSINE || metric == LGPU_DOT, "unknown distance type");
+    LGPU_REQUIRE(centroids && part_offsets, "null index array");
+    LGPU_REQUIRE(nrows == 0 || (codes && row_ids), "null codes / row_ids");
+    LGPU_REQUIRE(nrows < (1ull << 32), "more than 2^32 rows in one GPU shard are not supported (shard the index)");
+    LGPU_REQUIRE(part_offsets[0] == 0 && part_offsets[nlist] == nrows, "part_offsets must start at 0 and end at nrows");
+    for (uint32_t p = 0; p < nlist; p++) {
+        LGPU_REQUIRE(part_offsets[p + 1] >= part_offsets[p], "part_offsets must be non-decreasing");
+        LGPU_REQUIRE(part_offsets[p + 1] - part_offsets[p] < (1ull << 31), "partition too large");
+    }
+}
+
+// The arrays every IVF index holds in HBM, uploaded on the legacy stream: centroids (and their bf16 copy for the
+// tensor-core coarse step), partition sizes and offsets, row ids, optional raw vectors.  `rows_tile` is the scan's
+// tile height, which bounds the tile count of a search (max_nrb).
+static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t nlist, int metric, uint64_t nrows,
+                            const float *centroids, const uint64_t *part_offsets, const uint64_t *row_ids,
+                            const float *vectors, uint32_t rows_tile)
+{
+    ix->device = device;
+    cudaDeviceProp prop;
+    LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+    ix->num_sms = prop.multiProcessorCount;
+    ix->dim = dim; ix->nlist = nlist; ix->metric = metric; ix->nrows = nrows;
+    std::vector<uint32_t> part_n(nlist), part_npad(nlist);
+    std::vector<uint64_t> pads(nlist);
+    for (uint32_t p = 0; p < nlist; p++) {
+        const uint32_t n = (uint32_t)(part_offsets[p + 1] - part_offsets[p]);
+        part_n[p] = n; part_npad[p] = (n + 31u) & ~31u;
+        pads[p] = (n + 3ull) & ~3ull;
+        ix->max_nrb = std::max(ix->max_nrb, scan_nrb(n, rows_tile));
+    }
+    ix->h_part_n = part_n;
+    std::sort(pads.begin(), pads.end(), std::greater<uint64_t>());
+    ix->pad_prefix.assign(nlist + 1, 0);
+    for (uint32_t p = 0; p < nlist; p++) ix->pad_prefix[p + 1] = ix->pad_prefix[p] + pads[p];
+
+    cudaStream_t st = nullptr;
+    auto up = [&](DevBuf &b, const void *src, size_t bytes) {
+        b.ensure(std::max<size_t>(bytes, 16));
+        if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, st));
+        ix->device_bytes += b.bytes;
+    };
+    up(ix->centroids, centroids, (size_t)nlist * dim * 4);
+    up(ix->part_n, part_n.data(), (size_t)nlist * 4);
+    up(ix->part_npad, part_npad.data(), (size_t)nlist * 4);
+    up(ix->part_off, part_offsets, (size_t)(nlist + 1) * 8);
+    up(ix->row_ids, row_ids, (size_t)nrows * 8);
+    if (vectors) { up(ix->vectors, vectors, (size_t)nrows * dim * 4); ix->has_vectors = true; }
+    if (gemm_shape_supported(dim) && metric != LGPU_DOT) {
+        LGPU_CUDA(cudaStreamSynchronize(st));
+        prepare_tc_operand(ix->centroids.as<float>(), nlist, dim, ix->cent_b, ix->cent_n2, ix->cent_max, ix->cent_err, st);
+        ix->device_bytes += ix->cent_b.bytes + ix->cent_n2.bytes;
+        if (nlist >= 1024) {
+            // every 8th centroid, for the sampled threshold of the coarse step (strided: whatever order the
+            // trainer left the lists in -- hierarchical k-means groups neighbours -- the sample spans all of them)
+            constexpr uint32_t COARSE_SAMPLE_STRIDE = 8;
+            const uint32_t ns = nlist / COARSE_SAMPLE_STRIDE;
+            ix->cent_sb.ensure((size_t)ns * dim * 2); ix->cent_sn2.ensure((size_t)ns * 4);
+            LGPU_CUDA(cudaMemcpy2DAsync(ix->cent_sb.p, (size_t)dim * 2, ix->cent_b.p, (size_t)COARSE_SAMPLE_STRIDE * dim * 2,
+                                        (size_t)dim * 2, ns, cudaMemcpyDeviceToDevice, st));
+            LGPU_CUDA(cudaMemcpy2DAsync(ix->cent_sn2.p, 4, ix->cent_n2.p, (size_t)COARSE_SAMPLE_STRIDE * 4, 4, ns,
+                                        cudaMemcpyDeviceToDevice, st));
+            LGPU_CUDA(cudaStreamSynchronize(st));
+            ix->cent_ns = ns;
+            ix->device_bytes += ix->cent_sb.bytes + ix->cent_sn2.bytes;
+        }
+        ix->has_tc = true;
+    }
+    LGPU_CUDA(cudaStreamSynchronize(st));
+}
+
+// IVF_SQ stored rows: dim zero-padded to the scan's K step
+static uint32_t sq_dim_pad(uint32_t dim) { return (uint32_t)round_up64(dim, SQ_K_CHUNK); }
+
+// codes [n][dim] (host) -> dst [n][dim_pad] (device, zero padding) and xx[r] = sum of row r's squared codes
+static void upload_sq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBuf &dst, DevBuf &xx)
+{
+    const uint32_t dim_pad = sq_dim_pad(dim);
+    dst.ensure(std::max<size_t>((size_t)n * dim_pad, 16));
+    xx.ensure(std::max<size_t>((size_t)n * 4, 16));
+    cudaStream_t st = nullptr;
+    LGPU_CUDA(cudaMemsetAsync(dst.p, 0, dst.bytes, st));
+    if (n) {
+        LGPU_CUDA(cudaMemcpy2DAsync(dst.p, dim_pad, codes, dim, dim, n, cudaMemcpyHostToDevice, st));
+        launch_sq_row_norms(dst.as<uint8_t>(), n, dim_pad, xx.as<uint32_t>(), st);
+    }
+    LGPU_CUDA(cudaStreamSynchronize(st));
+}
+
 }  // namespace
 
 extern "C" {
@@ -1647,81 +1762,32 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
         LGPU_REQUIRE(d->dim > 0 && d->nlist > 0 && d->m > 0, "dim, nlist and m must be positive");
         LGPU_REQUIRE(d->dim % d->m == 0, "num_sub_vectors must divide the vector dimension");
         LGPU_REQUIRE(d->nbits == 8, "only 8-bit PQ codes are supported");
-        LGPU_REQUIRE(d->metric == LGPU_L2 || d->metric == LGPU_COSINE || d->metric == LGPU_DOT, "unknown distance type");
         LGPU_REQUIRE(d->codes_layout == LGPU_CODES_ROW_MAJOR || d->codes_layout == LGPU_CODES_PARTITION_TRANSPOSED,
                      "unknown codes layout");
         LGPU_REQUIRE(scan_dsub_supported(d->dim / d->m),
                      "unsupported PQ sub-vector length (dim/num_sub_vectors must be 1,2,4,8,16 or 32)");
-        LGPU_REQUIRE(d->centroids && d->codebook && d->part_offsets, "null index array");
-        LGPU_REQUIRE(d->nrows == 0 || (d->codes && d->row_ids), "null codes / row_ids");
-        LGPU_REQUIRE(d->nrows < (1ull << 32), "more than 2^32 rows in one GPU shard are not supported (shard the index)");
-        LGPU_REQUIRE(d->part_offsets[0] == 0 && d->part_offsets[d->nlist] == d->nrows,
-                     "part_offsets must start at 0 and end at nrows");
-        for (uint32_t p = 0; p < d->nlist; p++) {
-            LGPU_REQUIRE(d->part_offsets[p + 1] >= d->part_offsets[p], "part_offsets must be non-decreasing");
-            LGPU_REQUIRE(d->part_offsets[p + 1] - d->part_offsets[p] < (1ull << 31), "partition too large");
+        LGPU_REQUIRE(d->codebook, "null index array");
+        check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
+        const uint32_t nlist = d->nlist, nch = (d->m + 7) / 8;
+        std::vector<uint64_t> code_base(nlist);
+        uint64_t cb = 0;
+        for (uint32_t p = 0; p < nlist; p++) {
+            code_base[p] = cb;
+            cb += (uint64_t)(nch + 1) * (((d->part_offsets[p + 1] - d->part_offsets[p]) + 31u) & ~31ull) * 8;
+            LGPU_REQUIRE((cb >> 3) < (1ull << 32), "index too large for one GPU shard (re-laid-out codes above 32 GiB)");
         }
         require_device(d->device);
         ix = new lgpu_index();
-        ix->device = d->device;
-        cudaDeviceProp prop;
-        LGPU_CUDA(cudaGetDeviceProperties(&prop, d->device));
-        ix->num_sms = prop.multiProcessorCount;
-        ix->dim = d->dim; ix->nlist = d->nlist; ix->m = d->m; ix->dsub = d->dim / d->m;
-        ix->nch = (d->m + 7) / 8; ix->metric = d->metric; ix->nrows = d->nrows;
-
-        const uint32_t nlist = d->nlist;
-        std::vector<uint32_t> part_n(nlist), part_npad(nlist);
-        std::vector<uint64_t> code_base(nlist), pads(nlist);
-        uint64_t cb = 0;
-        for (uint32_t p = 0; p < nlist; p++) {
-            uint32_t n = (uint32_t)(d->part_offsets[p + 1] - d->part_offsets[p]);
-            part_n[p] = n; part_npad[p] = (n + 31u) & ~31u;
-            code_base[p] = cb;
-            cb += (uint64_t)(ix->nch + 1) * part_npad[p] * 8;
-            LGPU_REQUIRE((cb >> 3) < (1ull << 32), "index too large for one GPU shard (re-laid-out codes above 32 GiB)");
-            pads[p] = (n + 3ull) & ~3ull;
-        }
-        ix->h_part_n = part_n;
-        for (uint32_t p = 0; p < nlist; p++) ix->max_nrb = std::max(ix->max_nrb, scan_nrb(part_n[p], SCAN_ROWS_TILE_MID));
-        std::sort(pads.begin(), pads.end(), std::greater<uint64_t>());
-        ix->pad_prefix.assign(nlist + 1, 0);
-        for (uint32_t p = 0; p < nlist; p++) ix->pad_prefix[p + 1] = ix->pad_prefix[p] + pads[p];
-
+        ix->m = d->m; ix->dsub = d->dim / d->m; ix->nch = nch;
+        open_ivf_common(ix, d->device, d->dim, nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
+                        d->vectors, SCAN_ROWS_TILE_MID);
         cudaStream_t st = nullptr;
         auto up = [&](DevBuf &b, const void *src, size_t bytes) {
             b.ensure(std::max<size_t>(bytes, 16));
             if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, st));
             ix->device_bytes += b.bytes;
         };
-        up(ix->centroids, d->centroids, (size_t)nlist * d->dim * 4);
-        up(ix->part_n, part_n.data(), (size_t)nlist * 4);
-        up(ix->part_npad, part_npad.data(), (size_t)nlist * 4);
         up(ix->code_base, code_base.data(), (size_t)nlist * 8);
-        up(ix->part_off, d->part_offsets, (size_t)(nlist + 1) * 8);
-        up(ix->row_ids, d->row_ids, (size_t)d->nrows * 8);
-        if (d->vectors) { up(ix->vectors, d->vectors, (size_t)d->nrows * d->dim * 4); ix->has_vectors = true; }
-        if (gemm_shape_supported(d->dim) && d->metric != LGPU_DOT) {
-            LGPU_CUDA(cudaStreamSynchronize(st));
-            prepare_tc_operand(ix->centroids.as<float>(), nlist, d->dim, ix->cent_b, ix->cent_n2, ix->cent_max, ix->cent_err,
-                               st);
-            ix->device_bytes += ix->cent_b.bytes + ix->cent_n2.bytes;
-            if (nlist >= 1024) {
-                // every 8th centroid, for the sampled threshold of the coarse step (strided: whatever order the
-                // trainer left the lists in -- hierarchical k-means groups neighbours -- the sample spans all of them)
-                constexpr uint32_t COARSE_SAMPLE_STRIDE = 8;
-                const uint32_t ns = nlist / COARSE_SAMPLE_STRIDE;
-                ix->cent_sb.ensure((size_t)ns * d->dim * 2); ix->cent_sn2.ensure((size_t)ns * 4);
-                LGPU_CUDA(cudaMemcpy2DAsync(ix->cent_sb.p, (size_t)d->dim * 2, ix->cent_b.p, (size_t)COARSE_SAMPLE_STRIDE * d->dim * 2,
-                                            (size_t)d->dim * 2, ns, cudaMemcpyDeviceToDevice, st));
-                LGPU_CUDA(cudaMemcpy2DAsync(ix->cent_sn2.p, 4, ix->cent_n2.p, (size_t)COARSE_SAMPLE_STRIDE * 4, 4, ns,
-                                            cudaMemcpyDeviceToDevice, st));
-                LGPU_CUDA(cudaStreamSynchronize(st));
-                ix->cent_ns = ns;
-                ix->device_bytes += ix->cent_sb.bytes + ix->cent_sn2.bytes;
-            }
-            ix->has_tc = true;
-        }
         // codebook -> [nch][256][8][dsub]
         {
             DevBuf tmp;
@@ -1783,6 +1849,78 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
     });
     if (rc != LGPU_OK && ix) delete ix;
     return rc;
+}
+
+int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
+{
+    lgpu_index *ix = nullptr;
+    int rc = guarded([&] {
+        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+        LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
+        LGPU_REQUIRE(d->metric != LGPU_DOT, "IVF_SQ supports the l2 and cosine distance types, not dot");
+        LGPU_REQUIRE(d->dim <= LGPU_SQ_MAX_DIM, "IVF_SQ supports dimensions up to 65536");
+        LGPU_REQUIRE(std::isfinite(d->lo) && std::isfinite(d->hi) && d->lo <= d->hi,
+                     "IVF_SQ bounds must be finite with lo <= hi");
+        check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
+        require_device(d->device);
+        ix = new lgpu_index();
+        ix->is_sq = true;
+        ix->dim_pad = sq_dim_pad(d->dim);
+        ix->sq_lo = d->lo; ix->sq_hi = d->hi;
+        open_ivf_common(ix, d->device, d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
+                        d->vectors, SQ_ROWS_TILE);
+        // byte offset of each partition's codes (the tile descriptors carry it; the SQ scan addresses rows by part_off)
+        std::vector<uint64_t> code_base(d->nlist);
+        for (uint32_t p = 0; p < d->nlist; p++) code_base[p] = d->part_offsets[p] * ix->dim_pad;
+        ix->code_base.ensure((size_t)d->nlist * 8);
+        LGPU_CUDA(cudaMemcpy(ix->code_base.p, code_base.data(), (size_t)d->nlist * 8, cudaMemcpyHostToDevice));
+        upload_sq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->sq_xx);
+        ix->device_bytes += ix->code_base.bytes + ix->codes.bytes + ix->sq_xx.bytes;
+        register_handle(ix);
+        *out = ix;
+    });
+    if (rc != LGPU_OK && ix) delete ix;
+    return rc;
+}
+
+int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x_codes, uint64_t N, uint32_t dim,
+                            int device, uint32_t *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(dim >= 1 && dim <= LGPU_SQ_MAX_DIM, "dim must be in [1, 65536]");
+        LGPU_REQUIRE(B == 0 || N == 0 || (q_codes && x_codes && out), "null buffer");
+        LGPU_REQUIRE(N < (1ull << 31) && (uint64_t)B * N < (1ull << 32), "B x N must stay below 2^32");
+        if (B == 0 || N == 0) return;
+        require_device(device);
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        DevBuf X, xx, Q, qq, D, tiles, ctr;
+        upload_sq_rows(x_codes, N, dim, X, xx);
+        upload_sq_rows(q_codes, B, dim, Q, qq);
+        // one partition of N rows that every query probes: tiles of SQ_ROWS_TILE rows x 8 queries, query b's
+        // distances at out + b N
+        std::vector<TileDesc> h;
+        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
+            for (uint64_t r0 = 0; r0 < N; r0 += SQ_ROWS_TILE) {
+                TileDesc t{};
+                t.row0 = (uint32_t)r0; t.nrows = (uint32_t)std::min<uint64_t>(SQ_ROWS_TILE, N - r0);
+                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N;
+                for (uint32_t g = 0; g < t.ng; g++) { t.q[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * N); }
+                h.push_back(t);
+            }
+        const uint32_t total = (uint32_t)h.size(), zero[2] = {total, 0u};
+        tiles.ensure(h.size() * sizeof(TileDesc));
+        ctr.ensure(8);
+        D.ensure((size_t)B * N * 4);
+        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(ctr.p, zero, 8, cudaMemcpyHostToDevice));
+        SqScanArgs a{};
+        a.codes = X.as<uint8_t>(); a.xx = xx.as<uint32_t>(); a.qcodes = Q.as<uint8_t>(); a.qq = qq.as<uint32_t>();
+        a.dim_pad = sq_dim_pad(dim); a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1;
+        a.tile_desc = tiles.as<TileDesc>(); a.dist_out = D.as<float>(); a.out_u32 = 1;
+        launch_sq_scan(a, 2 * prop.multiProcessorCount, nullptr);
+        LGPU_CUDA(cudaMemcpy(out, D.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
+    });
 }
 
 void lgpu_index_close(lgpu_index *ix)
@@ -2538,6 +2676,7 @@ int lgpu_search_sharded(lgpu_index *ixh, lgpu_comm *ch, const float *queries, ui
     return guarded([&] {
         HandleRef<lgpu_index> ix(ixh, "index");
         HandleRef<lgpu_comm> c(ch, "communicator");
+        LGPU_REQUIRE(!ix->is_sq, "sharded search serves IVF_PQ indexes only");
         check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -2557,6 +2696,7 @@ int lgpu_search_sharded_device(lgpu_index *ixh, lgpu_comm *ch, const float *d_qu
     return guarded([&] {
         HandleRef<lgpu_index> ix(ixh, "index");
         HandleRef<lgpu_comm> c(ch, "communicator");
+        LGPU_REQUIRE(!ix->is_sq, "sharded search serves IVF_PQ indexes only");
         check_ivf_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -2638,6 +2778,7 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
     return guarded([&] {
         LGPU_REQUIRE(query && out, "null argument");
         HandleRef<lgpu_index> ix(ixh, "index");
+        LGPU_REQUIRE(!ix->is_sq, "lgpu_debug_partition_distances serves IVF_PQ indexes only");
         LGPU_REQUIRE(part < ix->nlist, "partition out of range");
         require_device(ix->device);
         WsLease lease(ix->pool, nullptr, false);
@@ -2660,6 +2801,7 @@ int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, 
     return guarded([&] {
         LGPU_REQUIRE(queries && out_parts && out_L && out_W && out_E && out_bad && B > 0 && nprobes > 0, "bad argument");
         HandleRef<lgpu_index> ix(ixh, "index");
+        LGPU_REQUIRE(!ix->is_sq, "lgpu_debug_filter_bounds serves IVF_PQ indexes only");
         require_device(ix->device);
         nprobes = std::min(nprobes, ix->nlist);
         LGPU_REQUIRE(ivf_sub_batch_size(ix.h, B, nprobes) == B, "batch too large for one filter-scan launch");

@@ -91,6 +91,28 @@ void launch_scan2(const ScanArgs &a, uint32_t dsub, int grid, cudaStream_t st);
 // filter kernel (scan3.cu): lower bounds from 16-bit per-query tables; rows_tile == SCAN3_ROWS_TILE
 void launch_scan3(const ScanArgs &a, int grid, cudaStream_t st);
 
+// ---------------- IVF_SQ scan (sq_scan.cu) ----------------------------------------------
+constexpr uint32_t SQ_ROWS_TILE = 256;            // rows per tile: 8 warps x 32 rows
+constexpr uint32_t SQ_K_CHUNK = 64;               // code bytes per K step of a warp; stored rows are padded to it
+struct SqScanArgs {
+    const uint8_t *codes;         // [nrows][dim_pad] row codes, partitions contiguous, zero padding
+    const uint32_t *xx;           // [nrows] sum of the squared codes of each row
+    const uint8_t *qcodes;        // [B][dim_pad] query codes (launch_sq_encode)
+    const uint32_t *qq;           // [B]
+    uint32_t dim_pad;
+    const uint32_t *total_tiles;  // [1]
+    uint32_t *tile_counter;       // [1], zeroed before launch
+    const TileDesc *tile_desc;    // built with rows_tile == SQ_ROWS_TILE
+    float *dist_out;              // segment of slot e at out[e]: (float) sum_i (k_i - q_i)^2 of row r at out[e] + r
+    int out_u32;                  // 1: write the exact u32 sums instead (lgpu_debug_sq_distances)
+};
+// qc[b] = the codes of query b (sat_u8(((double)q - lo) * 255 / (hi - lo)), zero-padded to dim_pad), qq[b] = |qc[b]|^2
+void launch_sq_encode(const float *Q, uint32_t B, uint32_t dim, uint32_t dim_pad, double lo, double hi, uint8_t *qc,
+                      uint32_t *qq, cudaStream_t st);
+// xx[r] = sum of the squared codes of row r of codes [n][dim_pad]
+void launch_sq_row_norms(const uint8_t *codes, uint64_t n, uint32_t dim_pad, uint32_t *xx, cudaStream_t st);
+void launch_sq_scan(const SqScanArgs &a, int grid, cudaStream_t st);
+
 // ---------------- tiny batches: one CTA per (query, probed partition) pair (small.cu) ----------------
 struct SmallScanArgs {
     const float *centroids; const float *cb_tiled; const unsigned char *codes; const uint64_t *code_base;

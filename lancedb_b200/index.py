@@ -1,4 +1,4 @@
-"""IVF_PQ index container and trainer.
+"""IVF_PQ and IVF_SQ index containers and trainers.
 
 `IvfPqIndexData` is the plain-array form of a Lance IVF_PQ index: exactly the arrays
 the reference's search path consumes after `prewarm_index`
@@ -179,6 +179,35 @@ def _batched_kmeans(x, k, iters, gen):
     return c
 
 
+def _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes):
+    """The IVF half of an index build: rows normalised for cosine (the index stores normalised vectors; search is L2 on
+    them), a training sample of sample_rate rows per partition, k-means centroids and every row's partition.
+    native_passes: the Lloyd loops and the assignment run in the library's kernels (lgpu_kmeans_train /
+    lgpu_ivf_assign), so a row lands in the partition its own vector probes first.
+    Returns (x normalised for cosine, sample, centroids, assign, device ordinal)."""
+    import torch
+    n = x.shape[0]
+    raw = x
+    if metric == "cosine":
+        x = x / x.norm(dim=1, keepdim=True).clamp(min=1e-30)
+    ns = min(n, sample_rate * nlist)
+    samp = x[torch.randperm(n, generator=gen, device="cpu")[:ns].to(x.device)] if ns < n else x
+    dev_index = x.device.index or 0 if x.device.type == "cuda" else 0
+    if native_passes:
+        # accelerator path: the Lloyd loops run in the library's own kernels (csrc/kmeans.cu through
+        # lgpu_kmeans_train): no torch op inside the loop, only the random initial sample is drawn here
+        from . import _native
+        samp_np = samp.detach().cpu().numpy()
+        init = _init_rows(samp, nlist, gen).cpu().numpy()
+        centroids = torch.as_tensor(_native.kmeans_train(samp_np, init, max_iterations, dev_index), device=x.device)
+        assign = torch.as_tensor(_native.ivf_assign(centroids.cpu().numpy(), raw.detach().cpu().numpy(), metric,
+                                                    dev_index).astype(np.int64), device=x.device)
+    else:
+        centroids = _kmeans(samp, nlist, max_iterations, gen)
+        assign = _assign(x, centroids, metric=metric)
+    return x, samp, centroids, assign, dev_index
+
+
 def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vectors: Optional[int] = None,
                  distance_type: str = "l2", sample_rate: int = 256, max_iterations: int = 50,
                  row_ids: Optional[np.ndarray] = None, keep_vectors: bool = False, seed: int = 45,
@@ -219,27 +248,10 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
     dsub = dim // m
     gen = torch.Generator(device="cpu").manual_seed(seed)
     raw = x
-    if metric == "cosine":       # index stores normalised vectors; search is L2 on them
-        x = x / x.norm(dim=1, keepdim=True).clamp(min=1e-30)
-
-    ns = min(n, sample_rate * nlist)
-    samp = x[torch.randperm(n, generator=gen, device="cpu")[:ns].to(x.device)] if ns < n else x
-    dev_index = x.device.index or 0 if x.device.type == "cuda" else 0
+    x, samp, centroids, assign, dev_index = _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes)
     if native_passes:
-        # accelerator path: the Lloyd loops run in the library's own kernels (csrc/kmeans.cu through
-        # lgpu_kmeans_train): no torch op inside the loop, only the random initial sample is drawn here
         from . import _native
-        samp_np = samp.detach().cpu().numpy()
-        init = _init_rows(samp, nlist, gen).cpu().numpy()
-        centroids = torch.as_tensor(_native.kmeans_train(samp_np, init, max_iterations, dev_index), device=x.device)
-    else:
-        centroids = _kmeans(samp, nlist, max_iterations, gen)
-    if native_passes:
         raw_np = raw.detach().cpu().numpy()
-        assign = torch.as_tensor(_native.ivf_assign(centroids.cpu().numpy(), raw_np, metric, dev_index).astype(np.int64),
-                                 device=x.device)
-    else:
-        assign = _assign(x, centroids, metric=metric)
 
     # PQ codebooks: residuals for l2/cosine, raw vectors for dot
     nps = min(n, max(256, sample_rate) * 256)
@@ -286,5 +298,90 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
         codebook=codebook.cpu().numpy().astype(np.float32),
         part_offsets=part_offsets, codes_t=codes_t, row_ids=rid[order_np],
         vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
+    data.validate()
+    return data
+
+
+# --------------------------------------------------------------------------------------
+SQ_METRICS = ("l2", "cosine")
+SQ_MAX_DIM = 65536          # LGPU_SQ_MAX_DIM: the exact integer distance stays below 2^32
+
+
+@dataclass
+class IvfSqIndexData:
+    """The plain-array form of an IVF_SQ index (lance `IvfSq`, rust/lancedb/src/index/vector.rs:216-256): IVF centroids,
+    one global quantiser range [lo, hi] and one 8-bit code per dimension of every row, grouped by partition.  The same
+    arrays go to `lgpu_ivf_sq_open` and to the CPU oracle (tests/sq_oracle.c)."""
+    dim: int
+    nlist: int
+    metric: str
+    centroids: np.ndarray      # f32 [nlist, dim]
+    part_offsets: np.ndarray   # u64 [nlist+1]
+    codes: np.ndarray          # u8 [n, dim] partition order
+    row_ids: np.ndarray        # u64 [n] in partition order
+    lo: float                  # quantiser bounds (f64)
+    hi: float
+    vectors: Optional[np.ndarray] = None   # f32 [n, dim] partition order (refine), optional
+
+    @property
+    def nrows(self) -> int:
+        return int(self.row_ids.size)
+
+    def validate(self) -> None:
+        assert self.metric in SQ_METRICS
+        assert 1 <= self.dim <= SQ_MAX_DIM
+        assert self.centroids.shape == (self.nlist, self.dim) and self.centroids.dtype == np.float32
+        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
+        assert int(self.part_offsets[-1]) == self.nrows
+        assert self.codes.shape == (self.nrows, self.dim) and self.codes.dtype == np.uint8
+        assert self.row_ids.dtype == np.uint64
+        assert np.isfinite(self.lo) and np.isfinite(self.hi) and self.lo <= self.hi
+
+
+def sq_encode(x, lo: float, hi: float) -> np.ndarray:
+    """lance's scale_to_u8 [lance, recalled]: sat_u8(((double)v - lo) * 255 / (hi - lo)), left to right in f64,
+    truncated toward zero; below 0 -> 0, above 255 -> 255, NaN -> 0; every code 0 when lo == hi.  The clipping is
+    explicit: a float -> uint8 cast is undefined outside [0, 256) and for NaN."""
+    v = np.asarray(x, np.float32).astype(np.float64)
+    lo, hi = float(lo), float(hi)
+    if hi == lo:
+        return np.zeros(v.shape, np.uint8)
+    with np.errstate(invalid="ignore", over="ignore"):
+        t = ((v - lo) * 255.0) / (hi - lo)
+    t = np.where(np.isnan(t), 0.0, t)
+    return np.trunc(np.clip(t, 0.0, 255.0)).astype(np.uint8)
+
+
+def train_ivf_sq(vectors, *, num_partitions: Optional[int] = None, distance_type: str = "l2", sample_rate: int = 256,
+                 max_iterations: int = 50, row_ids: Optional[np.ndarray] = None, keep_vectors: bool = False,
+                 seed: int = 45, device: Optional[str] = None, native_passes: bool = False) -> IvfSqIndexData:
+    """Train IVF centroids (the IVF half of train_ivf_pq), take [lo, hi] = the min and max over every component of the
+    training sample (normalised for cosine), and encode every row (normalised for cosine) with sq_encode."""
+    import torch
+    metric = distance_type.lower()
+    if metric not in SQ_METRICS:
+        raise ValueError(f"IVF_SQ supports the l2 and cosine distance types, not {distance_type!r}")
+    x = torch.as_tensor(vectors, dtype=torch.float32)
+    if device is not None:
+        x = x.to(device)
+    n, dim = x.shape
+    if not 1 <= dim <= SQ_MAX_DIM:
+        raise ValueError(f"IVF_SQ supports dimensions 1..{SQ_MAX_DIM}, got {dim}")
+    nlist = int(num_partitions or suggested_num_partitions(n))
+    gen = torch.Generator(device="cpu").manual_seed(seed)
+    raw = x
+    x, samp, centroids, assign, _ = _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes)
+    s = samp.detach().cpu().numpy()
+    lo, hi = (float(np.min(s)), float(np.max(s))) if s.size else (0.0, 0.0)
+    order = torch.argsort(assign, stable=True)                            # ascending row id per partition
+    sizes = torch.bincount(assign, minlength=nlist).cpu().numpy().astype(np.int64)
+    part_offsets = np.zeros(nlist + 1, np.uint64)
+    part_offsets[1:] = np.cumsum(sizes)
+    order_np = order.cpu().numpy()
+    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
+    data = IvfSqIndexData(
+        dim=dim, nlist=nlist, metric=metric, centroids=centroids.cpu().numpy().astype(np.float32),
+        part_offsets=part_offsets, codes=sq_encode(x[order].cpu().numpy(), lo, hi), row_ids=rid[order_np],
+        lo=lo, hi=hi, vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
     data.validate()
     return data

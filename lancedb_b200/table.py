@@ -16,7 +16,7 @@ import numpy as np
 import pyarrow as pa
 
 from . import _native
-from .index import IvfPqIndexData, train_ivf_pq
+from .index import IvfPqIndexData, IvfSqIndexData, train_ivf_pq, train_ivf_sq
 from .query import LanceVectorQueryBuilder
 
 
@@ -93,7 +93,7 @@ class Table:
         self._binary: Dict[str, _native.GpuBinary] = {}
         self._multivec: Dict[str, _native.GpuMultivec] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
-        self._index_data: Dict[str, IvfPqIndexData] = {}
+        self._index_data: Dict[str, Union[IvfPqIndexData, IvfSqIndexData]] = {}
 
     # ---- introspection ----
     @property
@@ -112,8 +112,11 @@ class Table:
     def to_pandas(self):
         return self._data.to_pandas()
 
+    def _index_type(self, column: str) -> str:
+        return "IVF_SQ" if isinstance(self._index_data[column], IvfSqIndexData) else "IVF_PQ"
+
     def list_indices(self):
-        return [{"name": f"{c}_idx", "index_type": "IVF_PQ", "columns": [c]} for c in self._index]
+        return [{"name": f"{c}_idx", "index_type": self._index_type(c), "columns": [c]} for c in self._index]
 
     def index_stats(self, index_name: str):
         """python/python/tests/test_index.py:366-372: every row is indexed (there is no append path here)."""
@@ -121,7 +124,7 @@ class Table:
         if col not in self._index_data:
             return None
         d = self._index_data[col]
-        return {"index_type": "IVF_PQ", "distance_type": d.metric, "num_indexed_rows": d.nrows,
+        return {"index_type": self._index_type(col), "distance_type": d.metric, "num_indexed_rows": d.nrows,
                 "num_unindexed_rows": self.count_rows() - d.nrows, "num_indices": 1}
 
     def _vectors(self, column: str) -> np.ndarray:
@@ -160,8 +163,9 @@ class Table:
                      num_sub_vectors: Optional[int] = None, vector_column_name: Optional[str] = None,
                      replace: bool = True, accelerator: Optional[str] = None, index_type: str = "IVF_PQ",
                      num_bits: int = 8, max_iterations: int = 50, sample_rate: int = 256, **_ignored):
-        if index_type.upper() != "IVF_PQ":
-            raise NotImplementedError("only IVF_PQ is on the GPU hot path")
+        kind = index_type.upper()
+        if kind not in ("IVF_PQ", "IVF_SQ"):
+            raise NotImplementedError("only IVF_PQ and IVF_SQ are on the GPU hot path")
         if num_bits != 8:
             raise ValueError("only num_bits=8 is supported")
         column = vector_column_name or self._infer_vector_column(None)
@@ -169,11 +173,19 @@ class Table:
             raise NotImplementedError("no index over binary vectors on the GPU path: search them flat (hamming)")
         if self._is_multivec(column):
             raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
+        if kind == "IVF_SQ" and metric.lower() not in ("l2", "cosine"):
+            raise ValueError(f"IVF_SQ supports the l2 and cosine distance types, not {metric!r}")
         if column in self._index and not replace:
             raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")   # python/python/tests/test_index.py:357
         dev = None
         if accelerator in ("cuda", "gpu"):
             dev = f"cuda:{self._device}"
+        if kind == "IVF_SQ":               # IvfSqIndexBuilder: distance_type, num_partitions, max_iterations, sample_rate
+            self._attach_index(column, train_ivf_sq(self._vectors(column), num_partitions=num_partitions,
+                                                    distance_type=metric, max_iterations=max_iterations,
+                                                    sample_rate=sample_rate, keep_vectors=True, device=dev,
+                                                    native_passes=dev is not None))
+            return
         data = train_ivf_pq(self._vectors(column), num_partitions=num_partitions,
                             num_sub_vectors=num_sub_vectors, distance_type=metric,
                             max_iterations=max_iterations, sample_rate=sample_rate,
@@ -181,11 +193,12 @@ class Table:
                             native_passes=dev is not None)      # accelerator: row passes through the C ABI (build.cu)
         self._attach_index(column, data)
 
-    def _attach_index(self, column: str, data: IvfPqIndexData):
+    def _attach_index(self, column: str, data: Union[IvfPqIndexData, IvfSqIndexData]):
         if column in self._index:
             self._index[column].close()
         self._index_data[column] = data
-        self._index[column] = _native.GpuIvfPq(data, device=self._device)
+        cls = _native.GpuIvfSq if isinstance(data, IvfSqIndexData) else _native.GpuIvfPq
+        self._index[column] = cls(data, device=self._device)
 
     # ---- on-disk Lance index (SURVEY.md 8f-3; layout [lance, recalled], see lance_index.py) ----
     def load_lance_index(self, index_dir: str, vector_column_name: Optional[str] = None) -> None:
@@ -205,6 +218,8 @@ class Table:
     def save_lance_index(self, index_dir: str, vector_column_name: Optional[str] = None, transposed: bool = True) -> None:
         from .lance_index import write_ivf_pq_index
         column = vector_column_name or self._infer_vector_column(None)
+        if self._index_type(column) != "IVF_PQ":
+            raise NotImplementedError("only IVF_PQ indexes are written as Lance index files")
         write_ivf_pq_index(index_dir, self._index_data[column], transposed=transposed)
 
     def prewarm_index(self, name: str):           # rust/lancedb/src/table.rs:3283-3286
