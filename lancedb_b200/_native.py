@@ -188,8 +188,63 @@ def make_params(k=10, nprobes=20, refine_factor=0, lower=None, upper=None, max_n
                         int(max_nprobes or 0), int(timeout_ms or 0))
 
 
-class GpuIvfPq:
+class _Handle:
+    """A library handle (`_h`) that `_close`, the name of its C close function, releases."""
+    _close = ""
+
+    def close(self):
+        if getattr(self, "_h", None) and _lib is not None:
+            getattr(_lib, self._close)(self._h)
+            self._h = None
+
+    __del__ = close
+
+
+def _host_search(fn: str, head, B: int, k: int, p: SearchParams, allow, allow_bits):
+    """Host-buffer search through `fn`, or through `fn`_filtered with `allow` (u32 bitmap over row ids, `allow_bits`
+    bits); `head` are the arguments before the params.  Returns (ids [B,k] u64, dist [B,k] f32, count [B] u32)."""
+    ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
+    if allow is None:
+        check(getattr(load(), fn)(*head, C.byref(p), _ptr(ids), _ptr(dist), _ptr(cnt)))
+    else:
+        bm = np.ascontiguousarray(allow, np.uint32)
+        if bm.size * 32 < allow_bits:
+            raise ValueError("allow bitmap shorter than allow_bits")
+        check(getattr(load(), fn + "_filtered")(*head, C.byref(p), _ptr(bm), int(allow_bits), _ptr(ids), _ptr(dist),
+                                                _ptr(cnt)))
+    return ids, dist, cnt
+
+
+def binary_components(queries) -> np.ndarray:
+    """Query components for a binary vector column: integers in [0, 255] (checked, not wrapped as a cast would) ->
+    uint8."""
+    a = np.asarray(queries)
+    if a.dtype != np.uint8:
+        if not (np.issubdtype(a.dtype, np.integer) or np.issubdtype(a.dtype, np.floating)) or (
+                a.size and not (np.all(np.isfinite(a)) and np.all(a == np.round(a)) and a.min() >= 0 and
+                                a.max() <= 255)):
+            raise ValueError("binary query components must be integers in [0, 255]")
+    return np.ascontiguousarray(a, np.uint8)
+
+
+def _query_offsets(q_offsets) -> np.ndarray:
+    """Multivector query offsets [B+1] -> u32, checked: they start at 0 and give every query 1..4096 vectors."""
+    off = np.asarray(q_offsets, np.int64).reshape(-1)
+    if off.size < 1 or off[0] != 0:
+        raise ValueError("query offsets must be [B + 1] and start at 0")
+    n = np.diff(off)
+    if np.any(n < 1):
+        raise ValueError("every multivector query needs at least one vector")
+    if n.size and int(n.max()) > MULTIVEC_MAX_NQ:
+        raise ValueError(f"a multivector query holds at most {MULTIVEC_MAX_NQ} vectors")
+    if int(off[-1]) >= 1 << 32:
+        raise ValueError("too many query vectors in one call")
+    return np.ascontiguousarray(off, np.uint32)
+
+
+class GpuIvfPq(_Handle):
     """An IVF_PQ index pinned in HBM (lgpu_index)."""
+    _close = "lgpu_index_close"
 
     def __init__(self, data, device: int = 0, with_vectors: bool = True):
         lib = load()
@@ -209,13 +264,6 @@ class GpuIvfPq:
         self._h = h
         self.has_vectors = vec is not None
 
-    def close(self):
-        if getattr(self, "_h", None) and _lib is not None:
-            _lib.lgpu_index_close(self._h)
-            self._h = None
-
-    __del__ = close
-
     def device_bytes(self) -> int:
         b = C.c_uint64(0)
         check(load().lgpu_index_device_bytes(self._h, C.byref(b)))
@@ -226,18 +274,8 @@ class GpuIvfPq:
         """Host-buffer search: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32).
         `allow` (u32 bitmap over row ids, `allow_bits` bits) = prefilter allow-list."""
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
-        B = q.shape[0]
-        ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
         p = make_params(k, nprobes, refine_factor, lower, upper, max_nprobes, timeout_ms)
-        if allow is None:
-            check(load().lgpu_search(self._h, _ptr(q), B, C.byref(p), _ptr(ids), _ptr(dist), _ptr(cnt)))
-        else:
-            bm = np.ascontiguousarray(allow, np.uint32)
-            if bm.size * 32 < allow_bits:
-                raise ValueError("allow bitmap shorter than allow_bits")
-            check(load().lgpu_search_filtered(self._h, _ptr(q), B, C.byref(p), _ptr(bm), int(allow_bits), _ptr(ids),
-                                              _ptr(dist), _ptr(cnt)))
-        return ids, dist, cnt
+        return _host_search("lgpu_search", (self._h, _ptr(q), q.shape[0]), q.shape[0], k, p, allow, allow_bits)
 
     def search_into(self, q: np.ndarray, p: SearchParams, ids: np.ndarray, dist: np.ndarray, cnt: np.ndarray):
         """Host-buffer search into caller-owned (e.g. pinned) arrays; no allocation."""
@@ -316,8 +354,9 @@ class GpuIvfSq(GpuIvfPq):
         self.has_vectors = vec is not None
 
 
-class GpuFlat:
+class GpuFlat(_Handle):
     """A raw vector column pinned in HBM (lgpu_flat)."""
+    _close = "lgpu_flat_close"
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
         v = np.ascontiguousarray(vectors, np.float32)
@@ -328,28 +367,11 @@ class GpuFlat:
         self._h = h
         self.device = device
 
-    def close(self):
-        if getattr(self, "_h", None) and _lib is not None:
-            _lib.lgpu_flat_close(self._h)
-            self._h = None
-
-    __del__ = close
-
     def search(self, queries, k=10, metric="l2", lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
-        B = q.shape[0]
-        ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
         p = make_params(k, 0, 0, lower, upper, 0, timeout_ms)
-        if allow is None:
-            check(load().lgpu_flat_search(self._h, METRICS[metric], _ptr(q), B, C.byref(p), _ptr(ids), _ptr(dist),
-                                          _ptr(cnt)))
-        else:
-            bm = np.ascontiguousarray(allow, np.uint32)
-            if bm.size * 32 < allow_bits:
-                raise ValueError("allow bitmap shorter than allow_bits")
-            check(load().lgpu_flat_search_filtered(self._h, METRICS[metric], _ptr(q), B, C.byref(p), _ptr(bm),
-                                                   int(allow_bits), _ptr(ids), _ptr(dist), _ptr(cnt)))
-        return ids, dist, cnt
+        return _host_search("lgpu_flat_search", (self._h, METRICS[metric], _ptr(q), q.shape[0]), q.shape[0], k, p,
+                            allow, allow_bits)
 
     def search_into(self, metric: str, q: np.ndarray, p: SearchParams, ids: np.ndarray, dist: np.ndarray,
                     cnt: np.ndarray):
@@ -364,9 +386,10 @@ class GpuFlat:
                                              stream))
 
 
-class GpuBinary:
+class GpuBinary(_Handle):
     """A packed binary vector column (fixed_size_list<uint8, nbytes>) pinned in HBM (lgpu_binary), searched by
     Hamming distance."""
+    _close = "lgpu_binary_close"
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
         v = np.ascontiguousarray(vectors, np.uint8)
@@ -379,40 +402,18 @@ class GpuBinary:
         self._h = h
         self.device = device
 
-    def close(self):
-        if getattr(self, "_h", None) and _lib is not None:
-            _lib.lgpu_binary_close(self._h)
-            self._h = None
-
-    __del__ = close
-
     def search(self, queries, k=10, lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         """Host-buffer search of queries [B, nbytes] (or one [nbytes] query) whose components are integers in
         [0, 255]: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32)."""
         q = self._queries(queries)
-        B = q.shape[0]
-        ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
         p = make_params(k, 0, 0, lower, upper, 0, timeout_ms)
-        if allow is None:
-            check(load().lgpu_binary_search(self._h, _ptr(q), B, C.byref(p), _ptr(ids), _ptr(dist), _ptr(cnt)))
-        else:
-            bm = np.ascontiguousarray(allow, np.uint32)
-            if bm.size * 32 < allow_bits:
-                raise ValueError("allow bitmap shorter than allow_bits")
-            check(load().lgpu_binary_search_filtered(self._h, _ptr(q), B, C.byref(p), _ptr(bm), int(allow_bits),
-                                                     _ptr(ids), _ptr(dist), _ptr(cnt)))
-        return ids, dist, cnt
+        return _host_search("lgpu_binary_search", (self._h, _ptr(q), q.shape[0]), q.shape[0], k, p, allow, allow_bits)
 
     def _queries(self, queries) -> np.ndarray:
         a = np.asarray(queries)
         if a.ndim not in (1, 2) or a.shape[-1] != self.nbytes:
             raise ValueError(f"binary queries must be [B, {self.nbytes}] or [{self.nbytes}], got shape {a.shape}")
-        if a.dtype != np.uint8:
-            if not (np.issubdtype(a.dtype, np.integer) or np.issubdtype(a.dtype, np.floating)) or (
-                    a.size and not (np.all(np.isfinite(a)) and np.all(a == np.round(a)) and a.min() >= 0 and
-                                    a.max() <= 255)):
-                raise ValueError("binary query components must be integers in [0, 255]")
-        return np.ascontiguousarray(a, np.uint8).reshape(-1, self.nbytes)
+        return binary_components(a).reshape(-1, self.nbytes)
 
     def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search (raw addresses; queries [B][nbytes] u8), enqueued on `stream`, not synchronised."""
@@ -427,9 +428,10 @@ def multivec_offsets(lengths) -> np.ndarray:
     return np.concatenate([[0], np.cumsum(n)]).astype(np.uint64)
 
 
-class GpuMultivec:
+class GpuMultivec(_Handle):
     """A multivector column (list<fixed_size_list<float, dim>>) pinned in HBM (lgpu_multivec), searched by late
     interaction: _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors."""
+    _close = "lgpu_multivec_close"
 
     def __init__(self, values, offsets, row_ids=None, device: int = 0):
         v = np.ascontiguousarray(values, np.float32)
@@ -453,13 +455,6 @@ class GpuMultivec:
         self._h = h
         self.device = device
 
-    def close(self):
-        if getattr(self, "_h", None) and _lib is not None:
-            _lib.lgpu_multivec_close(self._h)
-            self._h = None
-
-    __del__ = close
-
     def _queries(self, queries, q_offsets):
         """(values [Tq, dim] f32, offsets [B+1] u32).  queries: a list with one [nq_b, dim] (or [dim]) array per
         query, or [Tq, dim] values with q_offsets; a single numpy array is ONE query."""
@@ -481,46 +476,24 @@ class GpuMultivec:
             off = np.asarray(q_offsets, np.int64).reshape(-1)
         if vals.ndim != 2 or vals.shape[1] != self.dim:
             raise ValueError(f"multivector query vectors must have dimension {self.dim}, got shape {vals.shape}")
-        if off.size < 1 or off[0] != 0 or int(off[-1]) != vals.shape[0]:
-            raise ValueError("query offsets must be [B + 1], start at 0 and end at the number of query vectors")
-        n = np.diff(off)
-        if np.any(n < 1):
-            raise ValueError("every multivector query needs at least one vector")
-        if n.size and int(n.max()) > MULTIVEC_MAX_NQ:
-            raise ValueError(f"a multivector query holds at most {MULTIVEC_MAX_NQ} vectors")
-        if int(off[-1]) >= 1 << 32:
-            raise ValueError("too many query vectors in one call")
-        return np.ascontiguousarray(vals), np.ascontiguousarray(off, np.uint32)
+        off = _query_offsets(off)
+        if int(off[-1]) != vals.shape[0]:
+            raise ValueError("query offsets must end at the number of query vectors")
+        return np.ascontiguousarray(vals), off
 
     def search(self, queries, k=10, q_offsets=None, lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         """Host-buffer search of B multivector queries: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32).
         `queries`: a list with one [nq_b, dim] array per query, or [Tq, dim] values with `q_offsets` [B+1]; a single
         numpy array is ONE query.  Shapes are checked before any device call."""
         q, off = self._queries(queries, q_offsets)
-        B = off.size - 1
-        ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
         p = make_params(k, 0, 0, lower, upper, 0, timeout_ms)
-        if allow is None:
-            check(load().lgpu_multivec_search(self._h, _ptr(q), _ptr(off), B, C.byref(p), _ptr(ids), _ptr(dist),
-                                              _ptr(cnt)))
-        else:
-            bm = np.ascontiguousarray(allow, np.uint32)
-            if bm.size * 32 < allow_bits:
-                raise ValueError("allow bitmap shorter than allow_bits")
-            check(load().lgpu_multivec_search_filtered(self._h, _ptr(q), _ptr(off), B, C.byref(p), _ptr(bm),
-                                                       int(allow_bits), _ptr(ids), _ptr(dist), _ptr(cnt)))
-        return ids, dist, cnt
+        return _host_search("lgpu_multivec_search", (self._h, _ptr(q), _ptr(off), off.size - 1), off.size - 1, k, p,
+                            allow, allow_bits)
 
     def search_device(self, d_q: int, q_offsets, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search: d_q [Tq][dim] f32 and the outputs are raw device addresses, q_offsets [B+1] a host
         array (checked here); enqueued on `stream`, not synchronised."""
-        off = np.asarray(q_offsets, np.int64).reshape(-1)
-        n = np.diff(off)
-        if off.size < 1 or off[0] != 0 or np.any(n < 1) or (n.size and int(n.max()) > MULTIVEC_MAX_NQ):
-            raise ValueError("query offsets must start at 0 and give every query 1..4096 vectors")
-        if int(off[-1]) >= 1 << 32:
-            raise ValueError("too many query vectors in one call")
-        off = np.ascontiguousarray(off, np.uint32)
+        off = _query_offsets(q_offsets)
         check(load().lgpu_multivec_search_device(self._h, d_q, _ptr(off), off.size - 1, C.byref(p), d_ids, d_dist,
                                                  d_cnt, stream))
 
@@ -591,8 +564,9 @@ def comm_unique_id() -> bytes:
     return bytes(buf)
 
 
-class Comm:
+class Comm(_Handle):
     """One rank of a partition-sharded search group (lgpu_comm): collective constructor."""
+    _close = "lgpu_comm_destroy"
 
     def __init__(self, unique_id: bytes, rank: int, world: int, device: int = 0):
         if len(unique_id) != COMM_ID_BYTES:
@@ -601,13 +575,6 @@ class Comm:
         h = C.c_void_p()
         check(load().lgpu_comm_init(buf, COMM_ID_BYTES, rank, world, device, C.byref(h)))
         self._h, self.rank, self.world, self.device = h, rank, world, device
-
-    def close(self):
-        if getattr(self, "_h", None) and _lib is not None:
-            _lib.lgpu_comm_destroy(self._h)
-            self._h = None
-
-    __del__ = close
 
     def search(self, shard: "GpuIvfPq", queries, k=10, nprobes=20, lower=None, upper=None):
         """Collective host-buffer search: same queries on every rank, global top-k on every rank."""

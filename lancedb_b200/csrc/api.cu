@@ -223,6 +223,15 @@ template <class H> static bool retire_handle(H *p)
     g_live_cv.wait(g, [&] { return p->refs.load() == 0; });
     return true;
 }
+// every *_close: unregister, drain the handle's device, free it.  A null or closed handle, or a parent-process
+// handle in a fork child, is left alone.
+template <class H> static void close_handle(H *p)
+{
+    if (!retire_handle(p)) return;
+    cudaSetDevice(p->device);
+    cudaDeviceSynchronize();
+    delete p;
+}
 }  // namespace lgpu
 
 // micro-batcher of concurrent single-vector calls (SURVEY.md 8b "Threading": many tokio workers each with one query
@@ -369,6 +378,11 @@ struct lgpu_comm {
     DevBuf l_ids, l_dist, l_cnt;         // the local (per-shard) top-k before the exchange
     cudaEvent_t ev[3] = {};              // local search done / all-gather done / merge done (stage timing)
     float last_ms[3] = {0, 0, 0};        // local search, all-gather, merge of the most recent profiled call
+    ~lgpu_comm()
+    {
+        try { if (comm) nccl_api().CommDestroy(comm); } catch (const Failure &) {}
+        for (auto &e : ev) if (e) cudaEventDestroy(e);
+    }
 };
 
 namespace {
@@ -491,6 +505,27 @@ static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &X
     xerr = me;
 }
 
+// The tail of tc_topk_l2 and tc_topk_l2_filtered: exact re-score of the [B][cap] candidate slots (ws->t_pos, t_ids;
+// one pair per slot, empty slots included), their top-k into the outputs, then the dense fix-up of the queries
+// flagged in ws->flags (no-ops when none is).
+static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, const float *X, uint64_t N,
+                             uint32_t d, const uint64_t *col_ids, uint32_t k, uint32_t cap, uint64_t *out_ids,
+                             float *out_dist, uint32_t *out_cnt, float *Dbuf, uint64_t ld)
+{
+    launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, cap, d, LGPU_L2, ws->t_exact.as<float>(), st);
+    SelectArgs sb{};
+    sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
+    sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0;
+    sb.B = B; sb.k = k; sb.out_ids = out_ids; sb.out_dist = out_dist; sb.out_count = out_cnt;
+    launch_select(sb, st);
+    launch_dist_matrix(Q, X, B, N, d, 0, nullptr, nullptr, Dbuf, ld, st, ws->flags.as<uint32_t>());
+    SelectArgs sc{};
+    sc.mode = 1; sc.dense = Dbuf; sc.ncols = N; sc.row_stride = ld; sc.col_ids = col_ids;
+    sc.B = B; sc.k = k; sc.out_ids = out_ids; sc.out_dist = out_dist; sc.out_count = out_cnt;
+    sc.only = ws->flags.as<uint32_t>();
+    launch_select(sc, st);
+}
+
 // Tensor-core shortlist + exact re-score (squared L2 only): the k best of the N rows of X for each
 // of B queries by exact lance-order distance, ids from col_ids (or the row index), ascending by
 // (distance, id).  Dbuf: [B][ld] f32 scratch.  Queries whose shortlist cannot be proven complete
@@ -515,19 +550,7 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
     if (kp >= N) LGPU_CUDA(cudaMemsetAsync(ws->flags.p, 0, (size_t)B * 4, st));   // every row is a candidate
     else launch_band_check(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                            xmax, xerr, d, B, k, kp, ws->flags.as<uint32_t>(), st);
-    launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, kp, d, LGPU_L2, ws->t_exact.as<float>(), st);
-    SelectArgs sb{};
-    sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
-    sb.ncols = kp; sb.inner = kp; sb.row_stride = kp; sb.outer_stride = 0;
-    sb.B = B; sb.k = k; sb.out_ids = out_ids; sb.out_dist = out_dist; sb.out_count = out_cnt;
-    launch_select(sb, st);
-    // fix-up pass (no-ops unless a query was flagged)
-    launch_dist_matrix(Q, X, B, N, d, 0, nullptr, nullptr, Dbuf, ld, st, ws->flags.as<uint32_t>());
-    SelectArgs sc{};
-    sc.mode = 1; sc.dense = Dbuf; sc.ncols = N; sc.row_stride = ld; sc.col_ids = col_ids;
-    sc.B = B; sc.k = k; sc.out_ids = out_ids; sc.out_dist = out_dist; sc.out_count = out_cnt;
-    sc.only = ws->flags.as<uint32_t>();
-    launch_select(sc, st);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, kp, out_ids, out_dist, out_cnt, Dbuf, ld);
 }
 
 // Large-N variant of tc_topk_l2 (flat search): a tensor-core pass over a row sample fixes, per query, a
@@ -568,29 +591,35 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     if (Ns == N) launch_filter_dense(Dbuf, lds, B, N, flt, st);      // the sample pass already scored every row
     else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
-    // 3. exact re-score of the admitted rows, final top-k (one pair per slot, empty slots included)
-    launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, cap, d, LGPU_L2, ws->t_exact.as<float>(), st);
-    SelectArgs sb{};
-    sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
-    sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0;
-    sb.B = B; sb.k = k; sb.out_ids = out_ids; sb.out_dist = out_dist; sb.out_count = out_cnt;
-    launch_select(sb, st);
-    // 4. fix-up of overflowed queries (no-ops otherwise)
-    launch_dist_matrix(Q, X, B, N, d, 0, nullptr, nullptr, Dbuf, ld, st, ws->flags.as<uint32_t>());
-    SelectArgs sc{};
-    sc.mode = 1; sc.dense = Dbuf; sc.ncols = N; sc.row_stride = ld; sc.col_ids = col_ids;
-    sc.B = B; sc.k = k; sc.out_ids = out_ids; sc.out_dist = out_dist; sc.out_count = out_cnt;
-    sc.only = ws->flags.as<uint32_t>();
-    launch_select(sc, st);
+    // 3. exact re-score of the admitted rows, final top-k; 4. fix-up of overflowed queries
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out_ids, out_dist, out_cnt, Dbuf, ld);
 }
 
-void check_params(const lgpu_search_params *p)
+// top-k by (distance, id) of the dense scores D [b][ld] over N columns, with the request's distance range and
+// prefilter, into the outputs of queries q0 .. q0 + b
+static void select_dense(const float *D, uint64_t N, uint64_t ld, const uint64_t *col_ids, uint32_t b,
+                         const lgpu_search_params &sp, RowFilter rf, uint32_t q0, uint64_t *d_ids, float *d_dist,
+                         uint32_t *d_cnt, cudaStream_t st)
+{
+    SelectArgs sa{};
+    sa.mode = 1; sa.dense = D; sa.ncols = N; sa.row_stride = ld; sa.col_ids = col_ids;
+    sa.B = b; sa.k = sp.k;
+    sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
+    sa.out_ids = d_ids + (size_t)q0 * sp.k; sa.out_dist = d_dist + (size_t)q0 * sp.k; sa.out_count = d_cnt + q0;
+    sa.allow = rf.bits; sa.allow_bits = rf.nbits;
+    launch_select(sa, st);
+}
+
+// the arguments every search call takes: the parameters, then the query and output buffers of a call with queries
+static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, const void *ids, const void *dist,
+                       const void *cnt)
 {
     LGPU_REQUIRE(p != nullptr, "search params are null");
     LGPU_REQUIRE(p->k >= 1, "limit must be greater than 0");
     LGPU_REQUIRE(p->k <= SELECT_KMAX, "limit+offset above 2048 is not supported on the GPU path");
     if (p->refine_factor)
         LGPU_REQUIRE((uint64_t)p->k * p->refine_factor <= SELECT_KMAX, "limit*refine_factor above 2048 is not supported");
+    LGPU_REQUIRE(B == 0 || (q && ids && dist && cnt), "null buffer");
 }
 
 // lgpu_debug_filter_bounds: the dense filter scan's own lower bounds and band, copied out instead of a result
@@ -1139,14 +1168,8 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
         }
         launch_dist_matrix(q, fl->vectors.as<float>(), b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
                            xn, fl->ysqrt.as<float>(), ws->D.as<float>(), ld, st);
-        SelectArgs sa{};
-        sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = N; sa.row_stride = ld;
-        sa.col_ids = fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr;
-        sa.B = b; sa.k = sp.k;
-        sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
-        sa.out_ids = d_ids + (size_t)q0 * sp.k; sa.out_dist = d_dist + (size_t)q0 * sp.k; sa.out_count = d_cnt + q0;
-        sa.allow = rf.bits; sa.allow_bits = rf.nbits;
-        launch_select(sa, st);
+        select_dense(ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf, q0, d_ids,
+                     d_dist, d_cnt, st);
     }
 }
 
@@ -1279,13 +1302,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
             else
                 launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld,
                                  bx->num_sms, st);
-            SelectArgs sa{};
-            sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = N; sa.row_stride = ld; sa.col_ids = col_ids;
-            sa.B = b; sa.k = k;
-            sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
-            sa.out_ids = d_ids + (size_t)q0 * k; sa.out_dist = d_dist + (size_t)q0 * k; sa.out_count = d_cnt + q0;
-            sa.allow = rf.bits; sa.allow_bits = rf.nbits;
-            launch_select(sa, st);
+            select_dense(ws->D.as<float>(), N, ld, col_ids, b, sp, rf, q0, d_ids, d_dist, d_cnt, st);
         }
     }
     if (prof) {                     // [1] distances computed on the tensor cores, [3] queries
@@ -1451,14 +1468,8 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
             mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld);
-            SelectArgs sa{};
-            sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = N; sa.row_stride = ld;
-            sa.col_ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
-            sa.B = b; sa.k = k;
-            sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
-            sa.out_ids = d_ids + (size_t)qa * k; sa.out_dist = d_dist + (size_t)qa * k; sa.out_count = d_cnt + qa;
-            sa.allow = rf.bits; sa.allow_bits = rf.nbits;
-            launch_select(sa, st);
+            select_dense(ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf, qa,
+                         d_ids, d_dist, d_cnt, st);
         }
     }
     if (prof) {                     // exact path: [1] rows scored exactly; both: [3] queries
@@ -1477,31 +1488,6 @@ static void check_multivec_offsets(const uint32_t *q_off, uint32_t B)
         LGPU_REQUIRE(q_off[b + 1] > q_off[b], "every multivector query needs at least one vector (offsets must increase)");
         LGPU_REQUIRE(q_off[b + 1] - q_off[b] <= MV_MAX_NQ, "a multivector query holds at most 4096 vectors");
     }
-}
-
-// host-buffer multivector call: stage the query vectors in, run, stage the results out.  Not captured into a CUDA
-// graph: the launch sequence depends on every query's vector count, not only on B.
-template <class Run>
-void multivec_host_call(lgpu_multivec *mv, const float *queries, const uint32_t *q_off, uint32_t B,
-                        const lgpu_search_params &sp, uint64_t *out_ids, float *out_dist, uint32_t *out_count, Run &&run)
-{
-    const Deadline deadline(sp.timeout_ms);
-    WsLease lease(mv->pool, nullptr, false);
-    Workspace *ws = lease.ws;
-    cudaStream_t st = lease.st;
-    const size_t tq = q_off[B], k = sp.k;
-    ws->q.ensure(std::max<size_t>(tq * mv->dim, 1) * 4);
-    ws->out_ids.ensure((size_t)B * k * 8);
-    ws->out_dist.ensure((size_t)B * k * 4);
-    ws->out_count.ensure((size_t)B * 4);
-    LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, tq * mv->dim * 4, cudaMemcpyHostToDevice, st));
-    run(ws, st, ws->q.as<float>(), ws->out_ids.as<uint64_t>(), ws->out_dist.as<float>(), ws->out_count.as<uint32_t>(),
-        deadline);
-    deadline.wait(st, ws->ev[7]);
-    LGPU_CUDA(cudaMemcpyAsync(out_ids, ws->out_ids.p, (size_t)B * k * 8, cudaMemcpyDeviceToHost, st));
-    LGPU_CUDA(cudaMemcpyAsync(out_dist, ws->out_dist.p, (size_t)B * k * 4, cudaMemcpyDeviceToHost, st));
-    LGPU_CUDA(cudaMemcpyAsync(out_count, ws->out_count.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-    LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
 template <class F> int guarded(F &&f)
@@ -1539,34 +1525,32 @@ static bool graphs_enabled()
     return v == 1;
 }
 
-// host-buffer wrapper: stage in, run, stage out, synchronise.  Queries are [B][dim] elements of T (f32 vectors, or the
-// bytes of packed binary vectors).  `key` identifies the launch sequence
+// host-buffer wrapper: stage in, run, stage out, synchronise.  The queries are `q_elems` elements of T (f32 vectors,
+// or the bytes of packed binary vectors).  `key` (nullptr: always eager) identifies the launch sequence
 // (shapes + parameters): the second call with the same key is captured into a CUDA graph and later calls
 // replay it, which removes ~15 launch latencies from the synchronous end-to-end path.  Any device
 // (re)allocation anywhere in the process since the capture, profiling mode, or a failed capture falls back to
 // eager launches.
 template <class T, class Run>
-void host_submit(WsLease &lease, const Deadline &deadline, const T *queries, uint32_t B, uint32_t dim, uint32_t k,
-                 uint64_t *out_ids, float *out_dist, uint32_t *out_count, const uint64_t (&key)[4], Run &&run,
-                 bool allow_graph, bool sync)
+void host_submit(WsLease &lease, const Deadline &deadline, const T *queries, size_t q_elems, uint32_t B, uint32_t k,
+                 uint64_t *out_ids, float *out_dist, uint32_t *out_count, const uint64_t *key, Run &&run, bool sync)
 {
     Workspace *ws = lease.ws;
     cudaStream_t st = lease.st;
-    ws->q.ensure(std::max<size_t>((size_t)B * dim, 1) * sizeof(T));
+    ws->q.ensure(std::max<size_t>(q_elems, 1) * sizeof(T));
     ws->out_ids.ensure(std::max<size_t>((size_t)B * k, 1) * 8);
     ws->out_dist.ensure(std::max<size_t>((size_t)B * k, 1) * 4);
     ws->out_count.ensure(std::max<size_t>(B, 1) * 4);
-    LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * sizeof(T), cudaMemcpyHostToDevice, st));
+    LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, q_elems * sizeof(T), cudaMemcpyHostToDevice, st));
     auto eager = [&] {
         run(ws, st, ws->q.as<T>(), ws->out_ids.as<uint64_t>(), ws->out_dist.as<float>(), ws->out_count.as<uint32_t>(),
             deadline);
     };
-    const bool same = memcmp(key, ws->graph_key, sizeof(key)) == 0;
-    if (!allow_graph || !graphs_enabled() || profiling_enabled() || ws->graph_state < 0 || deadline.armed) {
+    if (!key || !graphs_enabled() || profiling_enabled() || ws->graph_state < 0 || deadline.armed) {
         eager();
-    } else if (!same) {                                     // new shape: warm up (allocations), capture next time
+    } else if (memcmp(key, ws->graph_key, sizeof(ws->graph_key)) != 0) {   // new shape: warm up (allocations), capture next time
         if (ws->graph) { cudaGraphExecDestroy(ws->graph); ws->graph = nullptr; }
-        memcpy(ws->graph_key, key, sizeof(key));
+        memcpy(ws->graph_key, key, sizeof(ws->graph_key));
         ws->graph_state = 0;
         eager();
         ws->graph_state = 1;
@@ -1599,14 +1583,14 @@ void host_submit(WsLease &lease, const Deadline &deadline, const T *queries, uin
             if (g) cudaGraphDestroy(g);
             cudaGetLastError();
             ws->graph = nullptr;
-            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * sizeof(T), cudaMemcpyHostToDevice, st));
+            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, q_elems * sizeof(T), cudaMemcpyHostToDevice, st));
             eager();
         } else {                                            // never try again with this workspace
             if (g) cudaGraphDestroy(g);
             cudaGetLastError();
             ws->graph = nullptr;
             ws->graph_state = -1;
-            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * dim * sizeof(T), cudaMemcpyHostToDevice, st));
+            LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, q_elems * sizeof(T), cudaMemcpyHostToDevice, st));
             eager();
         }
     } else {                                                // captured, but a buffer moved since: capture again
@@ -1622,13 +1606,12 @@ void host_submit(WsLease &lease, const Deadline &deadline, const T *queries, uin
 }
 
 template <class T, class Run>
-void host_call(WorkspacePool &pool, const T *queries, uint32_t B, uint32_t dim, uint32_t k, uint64_t *out_ids,
-               float *out_dist, uint32_t *out_count, const uint64_t (&key)[4], uint32_t timeout_ms, Run &&run,
-               bool allow_graph = true)
+void host_call(WorkspacePool &pool, const T *queries, size_t q_elems, uint32_t B, uint32_t k, uint64_t *out_ids,
+               float *out_dist, uint32_t *out_count, const uint64_t *key, uint32_t timeout_ms, Run &&run)
 {
     const Deadline deadline(timeout_ms);
     WsLease lease(pool, nullptr, false);
-    host_submit(lease, deadline, queries, B, dim, k, out_ids, out_dist, out_count, key, run, allow_graph, true);
+    host_submit(lease, deadline, queries, q_elems, B, k, out_ids, out_dist, out_count, key, run, true);
 }
 
 static inline void make_key(uint64_t (&key)[4], uint64_t tag, uint32_t B, const lgpu_search_params &p)
@@ -1640,6 +1623,75 @@ static inline void make_key(uint64_t (&key)[4], uint64_t tag, uint32_t B, const 
     key[2] = (uint64_t)p.refine_factor | ((uint64_t)(p.has_lower ? 1 : 0) << 32) | ((uint64_t)(p.has_upper ? 1 : 0) << 33) |
              ((uint64_t)(p.max_nprobes & 0x3fffffu) << 34);
     key[3] = ((uint64_t)lo | ((uint64_t)hi << 32)) ^ scan_modes().signature();
+}
+
+// the host bitmap over row ids of a filtered call, staged into the workspace on `st`
+static RowFilter upload_allow(Workspace *ws, cudaStream_t st, const uint32_t *allow, uint64_t allow_bits)
+{
+    const size_t words = (size_t)((allow_bits + 31) / 32);
+    ws->allow.ensure(std::max<size_t>(words, 1) * 4);
+    if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
+    RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
+    return rf;
+}
+
+// where a search call's buffers live
+struct Route {
+    enum Via { HOST, FILTERED, DEVICE } via;
+    uint64_t graph_tag;                 // HOST: tag of the CUDA-graph key (0: never captured)
+    const uint32_t *allow;              // FILTERED: host bitmap over row ids
+    uint64_t allow_bits;
+    void *stream;                       // DEVICE: the caller's stream
+};
+static Route host_route(uint64_t graph_tag) { return {Route::HOST, graph_tag, nullptr, 0, nullptr}; }
+static Route filtered_route(const uint32_t *allow, uint64_t allow_bits)
+{
+    return {Route::FILTERED, 0, allow, allow_bits, nullptr};
+}
+static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, stream}; }
+
+// The sequence of every search entry point: resolve the handle; the kind's own checks, `check(h)`, which return how
+// many query elements (T) the call reads; the bitmap of a filtered call; nothing more for B == 0; the device; then
+// the kind's `search(h, ws, st, d_q, B, params, d_ids, d_dist, d_cnt, rf, deadline)` on a workspace leased for the
+// caller's stream, or staged through host_submit.
+template <class H, class T, class Check, class Search>
+int search_call(H *hp, const char *what, const Route &r, const T *queries, uint32_t B, const lgpu_search_params *p,
+                uint64_t *ids, float *dist, uint32_t *cnt, Check &&check, Search &&search)
+{
+    return guarded([&] {
+        HandleRef<H> h(hp, what);
+        const size_t q_elems = check(h.h);
+        if (r.via == Route::FILTERED) LGPU_REQUIRE(r.allow != nullptr || r.allow_bits == 0, "allow bitmap is null");
+        if (B == 0) return;
+        require_device(h->device);
+        if (r.via == Route::DEVICE) {
+            WsLease lease(h->pool, (cudaStream_t)r.stream, true);
+            search(h.h, lease.ws, lease.st, queries, B, *p, ids, dist, cnt, RowFilter(), nullptr);
+            return;
+        }
+        uint64_t key[4];
+        if (r.graph_tag) make_key(key, r.graph_tag, B, *p);
+        host_call(h->pool, queries, q_elems, B, p->k, ids, dist, cnt, r.graph_tag ? key : nullptr, p->timeout_ms,
+                  [&](Workspace *ws, cudaStream_t st, const T *dq, uint64_t *di, float *dd, uint32_t *dc,
+                      const Deadline &dl) {
+                      const RowFilter rf = r.via == Route::FILTERED ? upload_allow(ws, st, r.allow, r.allow_bits)
+                                                                    : RowFilter();
+                      search(h.h, ws, st, dq, B, *p, di, dd, dc, rf, &dl);
+                  });
+    });
+}
+
+// what the flat, binary and multivector opens share: the device's SM count and the optional row ids
+template <class H> static void open_rows(H *h, const uint64_t *row_ids, uint64_t nrows)
+{
+    cudaDeviceProp prop;
+    LGPU_CUDA(cudaGetDeviceProperties(&prop, h->device));
+    h->num_sms = prop.multiProcessorCount;
+    if (row_ids && nrows) {
+        h->row_ids.ensure((size_t)nrows * 8);
+        LGPU_CUDA(cudaMemcpy(h->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
+        h->has_ids = true;
+    }
 }
 
 // the partition layout every IVF index shares (lgpu_index_open, lgpu_ivf_sq_open): checked before any device work
@@ -1923,13 +1975,7 @@ int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x
     });
 }
 
-void lgpu_index_close(lgpu_index *ix)
-{
-    if (!retire_handle(ix)) return;          // null, already closed, or a parent-process handle in a fork child
-    cudaSetDevice(ix->device);
-    cudaDeviceSynchronize();
-    delete ix;
-}
+void lgpu_index_close(lgpu_index *ix) { close_handle(ix); }
 
 int lgpu_index_device_bytes(const lgpu_index *ixh, uint64_t *bytes)
 {
@@ -1969,53 +2015,32 @@ int lgpu_last_stage_ms(float *times)
 static void check_ivf_call(lgpu_index *ix, const void *q, uint32_t B, const lgpu_search_params *p,
                            const void *a, const void *b, const void *c)
 {
-    check_params(p);
+    check_call(p, B, q, a, b, c);
     LGPU_REQUIRE(p->nprobes >= 1, "minimum_nprobes must be greater than 0");
     LGPU_REQUIRE(p->nprobes <= SELECT_KMAX || p->nprobes >= ix->nlist, "nprobes above 2048 is not supported");
-    LGPU_REQUIRE(B == 0 || (q && a && b && c), "null buffer");
     LGPU_REQUIRE(p->refine_factor == 0 || ix->has_vectors,
                  "refine_factor needs the raw vectors: open the index with desc.vectors");
+}
+
+static int ivf_call(lgpu_index *ixh, const Route &r, const float *q, uint32_t B, const lgpu_search_params *p,
+                    uint64_t *ids, float *dist, uint32_t *cnt)
+{
+    return search_call(ixh, "index", r, q, B, p, ids, dist, cnt,
+                       [&](lgpu_index *ix) { check_ivf_call(ix, q, B, p, ids, dist, cnt); return (size_t)B * ix->dim; },
+                       ivf_search_device);
 }
 
 int lgpu_search(lgpu_index *ixh, const float *queries, uint32_t B, const lgpu_search_params *params,
                 uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_index> ix(ixh, "index");
-        check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
-        if (B == 0) return;
-        require_device(ix->device);
-        uint64_t key[4];
-        make_key(key, 0x1f5ull, B, *params);
-        host_call(ix->pool, queries, B, ix->dim, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
-                  [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) { ivf_search_device(ix.h, ws, st, dq, B, *params, di, dd, dc, RowFilter(), &dl); });
-    });
+    return ivf_call(ixh, host_route(0x1f5ull), queries, B, params, out_ids, out_dist, out_count);
 }
 
 int lgpu_search_filtered(lgpu_index *ixh, const float *queries, uint32_t B, const lgpu_search_params *params,
                          const uint32_t *allow, uint64_t allow_bits, uint64_t *out_ids, float *out_dist,
                          uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_index> ix(ixh, "index");
-        check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
-        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
-        if (B == 0) return;
-        require_device(ix->device);
-        uint64_t key[4];
-        make_key(key, 0x1f6ull, B, *params);
-        key[0] ^= allow_bits << 8;
-        host_call(ix->pool, queries, B, ix->dim, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
-                  [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) {
-                      const size_t words = (size_t)((allow_bits + 31) / 32);
-                      ws->allow.ensure(std::max<size_t>(words, 1) * 4);
-                      if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
-                      RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
-                      ivf_search_device(ix.h, ws, st, dq, B, *params, di, dd, dc, rf, &dl);
-                  }, false);
-    });
+    return ivf_call(ixh, filtered_route(allow, allow_bits), queries, B, params, out_ids, out_dist, out_count);
 }
 
 int lgpu_search_coalesced(lgpu_index *ixh, const float *query, const lgpu_search_params *params, uint64_t *out_ids,
@@ -2077,14 +2102,7 @@ int lgpu_search_coalesced(lgpu_index *ixh, const float *query, const lgpu_search
 int lgpu_search_device(lgpu_index *ixh, const float *d_queries, uint32_t B, const lgpu_search_params *params,
                        uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream)
 {
-    return guarded([&] {
-        HandleRef<lgpu_index> ix(ixh, "index");
-        check_ivf_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
-        if (B == 0) return;
-        require_device(ix->device);
-        WsLease lease(ix->pool, (cudaStream_t)cuda_stream, true);
-        ivf_search_device(ix.h, lease.ws, lease.st, d_queries, B, *params, d_out_ids, d_out_dist, d_out_count);
-    });
+    return ivf_call(ixh, device_route(cuda_stream), d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
 }
 
 // ---- asynchronous completion (SURVEY.md 8b "Threading": a tokio worker must not be blocked for the length of a
@@ -2121,10 +2139,10 @@ int lgpu_search_async(lgpu_index *ixh, const float *queries, uint32_t B, const l
             make_key(key, 0x1f5ull, B, *params);
             lgpu_index *ix = t->ix.h;
             const lgpu_search_params sp = *params;
-            host_submit(t->lease, t->deadline, queries, B, ix->dim, sp.k, out_ids, out_dist, out_count, key,
+            host_submit(t->lease, t->deadline, queries, (size_t)B * ix->dim, B, sp.k, out_ids, out_dist, out_count, key,
                         [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
                             const Deadline &) { ivf_search_device(ix, ws, st, dq, B, sp, di, dd, dc); },
-                        true, false);
+                        false);
         }
         LGPU_CUDA(cudaEventRecord(t->done, t->lease.st));
         *ticket = t;
@@ -2196,18 +2214,11 @@ int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uin
         fl->device = device; fl->nrows = nrows; fl->dim = dim;
         fl->vectors.ensure(std::max<size_t>((size_t)nrows * dim * 4, 16));
         if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, (size_t)nrows * dim * 4, cudaMemcpyHostToDevice));
-        cudaDeviceProp prop;
-        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-        fl->num_sms = prop.multiProcessorCount;
         if (gemm_shape_supported(dim) && nrows >= 4096) {
             prepare_tc_operand(fl->vectors.as<float>(), nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max, fl->vec_err, nullptr);
             fl->has_tc = true;
         }
-        if (row_ids && nrows) {
-            fl->row_ids.ensure((size_t)nrows * 8);
-            LGPU_CUDA(cudaMemcpy(fl->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
-            fl->has_ids = true;
-        }
+        open_rows(fl, row_ids, nrows);
         register_handle(fl);
         *out = fl;
     });
@@ -2215,74 +2226,43 @@ int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uin
     return rc;
 }
 
-void lgpu_flat_close(lgpu_flat *fl)
-{
-    if (!retire_handle(fl)) return;
-    cudaSetDevice(fl->device);
-    cudaDeviceSynchronize();
-    delete fl;
-}
+void lgpu_flat_close(lgpu_flat *fl) { close_handle(fl); }
 
-static void check_flat_call(lgpu_flat *fl, int metric, const void *q, uint32_t B, const lgpu_search_params *p,
-                            const void *a, const void *b, const void *c)
+static int flat_call(lgpu_flat *flh, int metric, const Route &r, const float *q, uint32_t B,
+                     const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    LGPU_REQUIRE(metric == LGPU_L2 || metric == LGPU_COSINE || metric == LGPU_DOT, "unknown distance type");
-    check_params(p);
-    LGPU_REQUIRE(B == 0 || (q && a && b && c), "null buffer");
+    return search_call(flh, "flat", r, q, B, p, ids, dist, cnt,
+                       [&](lgpu_flat *fl) {
+                           LGPU_REQUIRE(metric == LGPU_L2 || metric == LGPU_COSINE || metric == LGPU_DOT,
+                                        "unknown distance type");
+                           check_call(p, B, q, ids, dist, cnt);
+                           return (size_t)B * fl->dim;
+                       },
+                       [&](lgpu_flat *fl, Workspace *ws, cudaStream_t st, auto &&...a) {
+                           flat_search_device(fl, ws, st, metric, a...);
+                       });
 }
 
 int lgpu_flat_search(lgpu_flat *flh, int metric, const float *queries, uint32_t B, const lgpu_search_params *params,
                      uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_flat> fl(flh, "flat");
-        check_flat_call(fl.h, metric, queries, B, params, out_ids, out_dist, out_count);
-        if (B == 0) return;
-        require_device(fl->device);
-        uint64_t key[4];
-        make_key(key, 0xf1a7ull + (uint64_t)metric, B, *params);
-        host_call(fl->pool, queries, B, fl->dim, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
-                  [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) { flat_search_device(fl.h, ws, st, metric, dq, B, *params, di, dd, dc, RowFilter(), &dl); });
-    });
+    return flat_call(flh, metric, host_route(0xf1a7ull + (uint64_t)metric), queries, B, params, out_ids, out_dist,
+                     out_count);
 }
 
 int lgpu_flat_search_filtered(lgpu_flat *flh, int metric, const float *queries, uint32_t B,
                               const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
                               uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_flat> fl(flh, "flat");
-        check_flat_call(fl.h, metric, queries, B, params, out_ids, out_dist, out_count);
-        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
-        if (B == 0) return;
-        require_device(fl->device);
-        uint64_t key[4];
-        make_key(key, 0xf1b7ull + (uint64_t)metric, B, *params);
-        host_call(fl->pool, queries, B, fl->dim, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
-                  [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) {
-                      const size_t words = (size_t)((allow_bits + 31) / 32);
-                      ws->allow.ensure(std::max<size_t>(words, 1) * 4);
-                      if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
-                      RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
-                      flat_search_device(fl.h, ws, st, metric, dq, B, *params, di, dd, dc, rf, &dl);
-                  }, false);
-    });
+    return flat_call(flh, metric, filtered_route(allow, allow_bits), queries, B, params, out_ids, out_dist, out_count);
 }
 
 int lgpu_flat_search_device(lgpu_flat *flh, int metric, const float *d_queries, uint32_t B,
                             const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
                             uint32_t *d_out_count, void *cuda_stream)
 {
-    return guarded([&] {
-        HandleRef<lgpu_flat> fl(flh, "flat");
-        check_flat_call(fl.h, metric, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
-        if (B == 0) return;
-        require_device(fl->device);
-        WsLease lease(fl->pool, (cudaStream_t)cuda_stream, true);
-        flat_search_device(fl.h, lease.ws, lease.st, metric, d_queries, B, *params, d_out_ids, d_out_dist, d_out_count);
-    });
+    return flat_call(flh, metric, device_route(cuda_stream), d_queries, B, params, d_out_ids, d_out_dist,
+                     d_out_count);
 }
 
 int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, const uint64_t *row_ids, int device,
@@ -2296,9 +2276,6 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
         require_device(device);
         bx = new lgpu_binary();
         bx->device = device; bx->nrows = nrows; bx->nbytes = nbytes; bx->nbytes_pad = (nbytes + 31) & ~31u;
-        cudaDeviceProp prop;
-        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-        bx->num_sms = prop.multiProcessorCount;
         const uint32_t nbp = bx->nbytes_pad;
         bx->vectors.ensure(std::max<size_t>((size_t)nrows * nbp, 16));
         bx->pop.ensure(std::max<size_t>((size_t)nrows * 4, 16));
@@ -2318,11 +2295,7 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
                             bx->sample_pop.as<uint32_t>(), nullptr);
         }
         LGPU_CUDA(cudaDeviceSynchronize());
-        if (row_ids && nrows) {
-            bx->row_ids.ensure((size_t)nrows * 8);
-            LGPU_CUDA(cudaMemcpy(bx->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
-            bx->has_ids = true;
-        }
+        open_rows(bx, row_ids, nrows);
         register_handle(bx);
         *out = bx;
     });
@@ -2330,72 +2303,33 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
     return rc;
 }
 
-void lgpu_binary_close(lgpu_binary *bx)
-{
-    if (!retire_handle(bx)) return;
-    cudaSetDevice(bx->device);
-    cudaDeviceSynchronize();
-    delete bx;
-}
+void lgpu_binary_close(lgpu_binary *bx) { close_handle(bx); }
 
-static void check_binary_call(const void *q, uint32_t B, const lgpu_search_params *p, const void *a, const void *b,
-                              const void *c)
+static int binary_call(lgpu_binary *bxh, const Route &r, const uint8_t *q, uint32_t B, const lgpu_search_params *p,
+                       uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    check_params(p);
-    LGPU_REQUIRE(B == 0 || (q && a && b && c), "null buffer");
+    return search_call(bxh, "binary", r, q, B, p, ids, dist, cnt,
+                       [&](lgpu_binary *bx) { check_call(p, B, q, ids, dist, cnt); return (size_t)B * bx->nbytes; },
+                       binary_search_device);
 }
 
 int lgpu_binary_search(lgpu_binary *bxh, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
                        uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_binary> bx(bxh, "binary");
-        check_binary_call(queries, B, params, out_ids, out_dist, out_count);
-        if (B == 0) return;
-        require_device(bx->device);
-        uint64_t key[4];
-        make_key(key, 0xb1a7ull, B, *params);
-        host_call(bx->pool, queries, B, bx->nbytes, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
-                  [&](Workspace *ws, cudaStream_t st, const uint8_t *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) { binary_search_device(bx.h, ws, st, dq, B, *params, di, dd, dc, RowFilter(), &dl); });
-    });
+    return binary_call(bxh, host_route(0xb1a7ull), queries, B, params, out_ids, out_dist, out_count);
 }
 
 int lgpu_binary_search_filtered(lgpu_binary *bxh, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
                                 const uint32_t *allow, uint64_t allow_bits, uint64_t *out_ids, float *out_dist,
                                 uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_binary> bx(bxh, "binary");
-        check_binary_call(queries, B, params, out_ids, out_dist, out_count);
-        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
-        if (B == 0) return;
-        require_device(bx->device);
-        uint64_t key[4];
-        make_key(key, 0xb1b7ull, B, *params);
-        host_call(bx->pool, queries, B, bx->nbytes, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
-                  [&](Workspace *ws, cudaStream_t st, const uint8_t *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) {
-                      const size_t words = (size_t)((allow_bits + 31) / 32);
-                      ws->allow.ensure(std::max<size_t>(words, 1) * 4);
-                      if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
-                      RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
-                      binary_search_device(bx.h, ws, st, dq, B, *params, di, dd, dc, rf, &dl);
-                  }, false);
-    });
+    return binary_call(bxh, filtered_route(allow, allow_bits), queries, B, params, out_ids, out_dist, out_count);
 }
 
 int lgpu_binary_search_device(lgpu_binary *bxh, const uint8_t *d_queries, uint32_t B, const lgpu_search_params *params,
                               uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream)
 {
-    return guarded([&] {
-        HandleRef<lgpu_binary> bx(bxh, "binary");
-        check_binary_call(d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
-        if (B == 0) return;
-        require_device(bx->device);
-        WsLease lease(bx->pool, (cudaStream_t)cuda_stream, true);
-        binary_search_device(bx.h, lease.ws, lease.st, d_queries, B, *params, d_out_ids, d_out_dist, d_out_count);
-    });
+    return binary_call(bxh, device_route(cuda_stream), d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
 }
 
 int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
@@ -2418,9 +2352,6 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
         require_device(device);
         mv = new lgpu_multivec();
         mv->device = device; mv->nrows = nrows; mv->total = T; mv->dim = dim; mv->max_row = max_row;
-        cudaDeviceProp prop;
-        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-        mv->num_sms = prop.multiProcessorCount;
         mv->h_offsets.assign(offsets, offsets + nrows + 1);
         mv->vectors.ensure(std::max<size_t>((size_t)T * dim * 4, 16));
         mv->ysqrt.ensure(std::max<size_t>((size_t)T * 4, 16));
@@ -2448,11 +2379,7 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
             mv->tc_ok = ok;
         }
         LGPU_CUDA(cudaDeviceSynchronize());
-        if (row_ids && nrows) {
-            mv->row_ids.ensure((size_t)nrows * 8);
-            LGPU_CUDA(cudaMemcpy(mv->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
-            mv->has_ids = true;
-        }
+        open_rows(mv, row_ids, nrows);
         register_handle(mv);
         *out = mv;
     });
@@ -2460,73 +2387,45 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
     return rc;
 }
 
-void lgpu_multivec_close(lgpu_multivec *mv)
-{
-    if (!retire_handle(mv)) return;
-    cudaSetDevice(mv->device);
-    cudaDeviceSynchronize();
-    delete mv;
-}
+void lgpu_multivec_close(lgpu_multivec *mv) { close_handle(mv); }
 
-static void check_multivec_call(const void *q, const uint32_t *q_off, uint32_t B, const lgpu_search_params *p,
-                                const void *a, const void *b, const void *c)
+// Host calls are never captured into a CUDA graph: the launch sequence depends on every query's vector count, not
+// only on B.
+static int multivec_call(lgpu_multivec *mvh, const Route &r, const float *q, const uint32_t *q_off, uint32_t B,
+                         const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    check_params(p);
-    LGPU_REQUIRE(B == 0 || (q && a && b && c), "null buffer");
-    if (B) check_multivec_offsets(q_off, B);
+    return search_call(mvh, "multivector", r, q, B, p, ids, dist, cnt,
+                       [&](lgpu_multivec *mv) {
+                           check_call(p, B, q, ids, dist, cnt);
+                           if (B == 0) return (size_t)0;
+                           check_multivec_offsets(q_off, B);
+                           return (size_t)q_off[B] * mv->dim;
+                       },
+                       [&](lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *dq, auto &&...a) {
+                           multivec_search_device(mv, ws, st, dq, q_off, a...);
+                       });
 }
 
 int lgpu_multivec_search(lgpu_multivec *mvh, const float *queries, const uint32_t *q_offsets, uint32_t B,
                          const lgpu_search_params *params, uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_multivec> mv(mvh, "multivector");
-        check_multivec_call(queries, q_offsets, B, params, out_ids, out_dist, out_count);
-        if (B == 0) return;
-        require_device(mv->device);
-        multivec_host_call(mv.h, queries, q_offsets, B, *params, out_ids, out_dist, out_count,
-                           [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                               const Deadline &dl) {
-                               multivec_search_device(mv.h, ws, st, dq, q_offsets, B, *params, di, dd, dc, RowFilter(), &dl);
-                           });
-    });
+    return multivec_call(mvh, host_route(0), queries, q_offsets, B, params, out_ids, out_dist, out_count);
 }
 
 int lgpu_multivec_search_filtered(lgpu_multivec *mvh, const float *queries, const uint32_t *q_offsets, uint32_t B,
                                   const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
                                   uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
-    return guarded([&] {
-        HandleRef<lgpu_multivec> mv(mvh, "multivector");
-        check_multivec_call(queries, q_offsets, B, params, out_ids, out_dist, out_count);
-        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
-        if (B == 0) return;
-        require_device(mv->device);
-        multivec_host_call(mv.h, queries, q_offsets, B, *params, out_ids, out_dist, out_count,
-                           [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                               const Deadline &dl) {
-                               const size_t words = (size_t)((allow_bits + 31) / 32);
-                               ws->allow.ensure(std::max<size_t>(words, 1) * 4);
-                               if (words) LGPU_CUDA(cudaMemcpyAsync(ws->allow.p, allow, words * 4, cudaMemcpyHostToDevice, st));
-                               RowFilter rf; rf.bits = ws->allow.as<uint32_t>(); rf.nbits = allow_bits;
-                               multivec_search_device(mv.h, ws, st, dq, q_offsets, B, *params, di, dd, dc, rf, &dl);
-                           });
-    });
+    return multivec_call(mvh, filtered_route(allow, allow_bits), queries, q_offsets, B, params, out_ids, out_dist,
+                         out_count);
 }
 
 int lgpu_multivec_search_device(lgpu_multivec *mvh, const float *d_queries, const uint32_t *q_offsets, uint32_t B,
                                 const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
                                 uint32_t *d_out_count, void *cuda_stream)
 {
-    return guarded([&] {
-        HandleRef<lgpu_multivec> mv(mvh, "multivector");
-        check_multivec_call(d_queries, q_offsets, B, params, d_out_ids, d_out_dist, d_out_count);
-        if (B == 0) return;
-        require_device(mv->device);
-        WsLease lease(mv->pool, (cudaStream_t)cuda_stream, true);
-        multivec_search_device(mv.h, lease.ws, lease.st, d_queries, q_offsets, B, *params, d_out_ids, d_out_dist,
-                               d_out_count);
-    });
+    return multivec_call(mvh, device_route(cuda_stream), d_queries, q_offsets, B, params, d_out_ids, d_out_dist,
+                         d_out_count);
 }
 
 int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
@@ -2624,19 +2523,11 @@ int lgpu_comm_init(const void *unique_id, size_t id_bytes, int rank, int world, 
         register_handle(c);
         *out = c;
     });
-    if (rc != LGPU_OK && c) { if (c->comm) nccl_api().CommDestroy(c->comm); delete c; }
+    if (rc != LGPU_OK && c) delete c;
     return rc;
 }
 
-void lgpu_comm_destroy(lgpu_comm *c)
-{
-    if (!retire_handle(c)) return;
-    cudaSetDevice(c->device);
-    cudaDeviceSynchronize();
-    try { if (c->comm) nccl_api().CommDestroy(c->comm); } catch (const Failure &) {}
-    for (auto &e : c->ev) if (e) cudaEventDestroy(e);
-    delete c;
-}
+void lgpu_comm_destroy(lgpu_comm *c) { close_handle(c); }
 
 // local top-k on this rank's shard -> pack -> ONE all-gather of [B][k] 16-byte records -> merge, all on `st`
 static void sharded_search_device(lgpu_index *ix, lgpu_comm *c, Workspace *ws, cudaStream_t st, const float *d_q,
@@ -2680,12 +2571,10 @@ int lgpu_search_sharded(lgpu_index *ixh, lgpu_comm *ch, const float *queries, ui
         check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
         if (B == 0) return;
         require_device(ix->device);
-        uint64_t key[4];
-        make_key(key, 0x5a4dull, B, *params);
-        host_call(ix->pool, queries, B, ix->dim, params->k, out_ids, out_dist, out_count, key, params->timeout_ms,
+        host_call(ix->pool, queries, (size_t)B * ix->dim, B, params->k, out_ids, out_dist, out_count, nullptr,
+                  params->timeout_ms,
                   [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                      const Deadline &dl) { sharded_search_device(ix.h, c.h, ws, st, dq, B, *params, di, dd, dc, &dl); },
-                  false);
+                      const Deadline &dl) { sharded_search_device(ix.h, c.h, ws, st, dq, B, *params, di, dd, dc, &dl); });
     });
 }
 

@@ -74,16 +74,6 @@ def _is_binary_type(t: pa.DataType) -> bool:
     return pa.types.is_fixed_size_list(t) and pa.types.is_uint8(t.value_type)
 
 
-def binary_query(query) -> np.ndarray:
-    """Query components for a binary column: integers in [0, 255] (checked, not wrapped as a cast would) -> uint8."""
-    a = np.asarray(query)
-    if a.dtype == object or not (np.issubdtype(a.dtype, np.integer) or np.issubdtype(a.dtype, np.floating)):
-        raise ValueError("a query on a binary vector column must hold integers in [0, 255]")
-    if a.size and not (np.all(np.isfinite(a)) and np.all(a == np.round(a)) and a.min() >= 0 and a.max() <= 255):
-        raise ValueError("a query on a binary vector column must hold integers in [0, 255]")
-    return a.astype(np.uint8)
-
-
 class Table:
     def __init__(self, name: str, data: pa.Table, device: int = 0):
         self.name = name
@@ -258,7 +248,7 @@ class Table:
             if distance_type is not None and distance_type != "hamming":
                 raise ValueError(f"distance type {distance_type!r} is not supported on binary column {column!r}: "
                                  "use 'hamming'")
-            q = binary_query(queries)             # the builder's f32 copy: integers are exact up to 2^24
+            q = _native.binary_components(queries)   # the builder's f32 copy: integers are exact up to 2^24
             bx = self._binary.get(column)
             if bx is None:
                 bx = self._binary[column] = _native.GpuBinary(self._binary_vectors(column), device=self._device)
