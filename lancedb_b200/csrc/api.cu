@@ -102,6 +102,7 @@ struct Workspace {
     cudaStream_t front = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     int stats_mode = 0;                 // profiling: 1 = the last sub-batch ran the candidate mode, 2 = the dense filter
+    uint32_t stages_marked = 0;         // profiling: bit s = ev[s] was recorded by the profiled sub-batch (IvfStage)
     bool front_open = false;            // an EAGER fork onto `front` has not been joined yet (a call failed half-way)
     cudaEvent_t done = nullptr;        // last use, for cross-stream reuse
     cudaEvent_t ev[8] = {};
@@ -457,12 +458,13 @@ static bool exact_scan_forced()
 // Mode switches of the IVF path, re-read on every call (tests flip them between calls; getenv is ~100 ns) and folded
 // into the CUDA-graph key so a captured launch sequence is never replayed under a different mode.
 struct ScanModes {
-    bool exact, dense_forced;
+    bool exact, dense_forced, force_tc_coarse;
     uint32_t cand_kmax, cap_env, small_slots, coarse_list_min;
     uint64_t signature() const
     {
-        return ((uint64_t)exact | (uint64_t)dense_forced << 1 | (uint64_t)cand_kmax << 8 | (uint64_t)cap_env << 20 |
-                (uint64_t)small_slots << 36 | (uint64_t)(coarse_list_min & 0xffffu) << 48) * 0x9e3779b97f4a7c15ull;
+        return ((uint64_t)exact | (uint64_t)dense_forced << 1 | (uint64_t)force_tc_coarse << 2 | (uint64_t)cand_kmax << 8 |
+                (uint64_t)cap_env << 20 | (uint64_t)small_slots << 36 | (uint64_t)(coarse_list_min & 0xffffu) << 48) *
+               0x9e3779b97f4a7c15ull;
     }
 };
 static ScanModes scan_modes()
@@ -471,6 +473,7 @@ static ScanModes scan_modes()
     ScanModes m;
     m.exact = exact_scan_forced();
     m.dense_forced = getenv("LGPU_DENSE_FILTER") != nullptr;
+    m.force_tc_coarse = getenv("LGPU_FORCE_TC_COARSE") != nullptr;   // the tensor-core coarse step at any B x nlist
     m.cand_kmax = std::min<uint32_t>(CAND_TOPK_MAX, num("LGPU_CAND_KMAX", CAND_TOPK_MAX));
     m.cap_env = num("LGPU_CAND_CAP", 0u);
     m.small_slots = num("LGPU_SMALL_SLOTS", 1024u);
@@ -505,24 +508,55 @@ static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &X
     xerr = me;
 }
 
+// where a top-k goes: [B][k] ids and distances, [B] counts and, optionally, [B][k] storage positions
+struct TopkOut {
+    uint64_t *ids;
+    float *dist;
+    uint32_t *cnt;
+    uint64_t *pos = nullptr;
+    // the rows of queries q0, q0 + 1, ... of a [B][k] output
+    TopkOut at(uint32_t q0, uint32_t k) const { return {ids + (size_t)q0 * k, dist + (size_t)q0 * k, cnt + q0}; }
+};
+
+// SelectArgs with the fields every mode needs; callers add the optional ones (only, gate, col_ids, range, allow, ...)
+static SelectArgs select_args(int mode, uint32_t B, uint32_t k, TopkOut out)
+{
+    SelectArgs s{};
+    s.mode = mode; s.B = B; s.k = k;
+    s.out_ids = out.ids; s.out_dist = out.dist; s.out_count = out.cnt; s.out_pos = out.pos;
+    return s;
+}
+// mode 1: the k best of the first ncols columns of every row of the dense block D [B][ld]
+static SelectArgs select_rows(const float *D, uint64_t ncols, uint64_t ld, uint32_t B, uint32_t k, TopkOut out)
+{
+    SelectArgs s = select_args(1, B, k, out);
+    s.dense = D; s.ncols = ncols; s.row_stride = ld;
+    return s;
+}
+// mode 2: the k best of every query's n candidates, values and ids [B][n]
+static SelectArgs select_cands(const float *vals, const uint64_t *ids, uint64_t n, uint32_t B, uint32_t k, TopkOut out)
+{
+    SelectArgs s = select_args(2, B, k, out);
+    s.dense = vals; s.cand_ids = ids; s.ncols = n; s.inner = n; s.row_stride = n; s.outer_stride = 0;
+    return s;
+}
+static void with_range(SelectArgs &s, const lgpu_search_params &sp)
+{
+    s.has_lower = sp.has_lower; s.has_upper = sp.has_upper; s.lower = sp.lower; s.upper = sp.upper;
+}
+
 // The tail of tc_topk_l2 and tc_topk_l2_filtered: exact re-score of the [B][cap] candidate slots (ws->t_pos, t_ids;
 // one pair per slot, empty slots included), their top-k into the outputs, then the dense fix-up of the queries
 // flagged in ws->flags (no-ops when none is).
 static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, const float *X, uint64_t N,
-                             uint32_t d, const uint64_t *col_ids, uint32_t k, uint32_t cap, uint64_t *out_ids,
-                             float *out_dist, uint32_t *out_cnt, float *Dbuf, uint64_t ld)
+                             uint32_t d, const uint64_t *col_ids, uint32_t k, uint32_t cap, TopkOut out, float *Dbuf,
+                             uint64_t ld)
 {
     launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, cap, d, LGPU_L2, ws->t_exact.as<float>(), st);
-    SelectArgs sb{};
-    sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
-    sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0;
-    sb.B = B; sb.k = k; sb.out_ids = out_ids; sb.out_dist = out_dist; sb.out_count = out_cnt;
-    launch_select(sb, st);
+    launch_select(select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), cap, B, k, out), st);
     launch_dist_matrix(Q, X, B, N, d, 0, nullptr, nullptr, Dbuf, ld, st, ws->flags.as<uint32_t>());
-    SelectArgs sc{};
-    sc.mode = 1; sc.dense = Dbuf; sc.ncols = N; sc.row_stride = ld; sc.col_ids = col_ids;
-    sc.B = B; sc.k = k; sc.out_ids = out_ids; sc.out_dist = out_dist; sc.out_count = out_cnt;
-    sc.only = ws->flags.as<uint32_t>();
+    SelectArgs sc = select_rows(Dbuf, N, ld, B, k, out);
+    sc.col_ids = col_ids; sc.only = ws->flags.as<uint32_t>();
     launch_select(sc, st);
 }
 
@@ -532,8 +566,7 @@ static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uin
 // (band_check) are redone by the exact kernels in the same stream, without a host round trip.
 static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
                        const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
-                       const uint64_t *col_ids, uint32_t k, uint32_t kp, uint64_t *out_ids, float *out_dist,
-                       uint32_t *out_cnt, float *Dbuf, uint64_t ld)
+                       const uint64_t *col_ids, uint32_t k, uint32_t kp, TopkOut out, float *Dbuf, uint64_t ld)
 {
     ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
     ws->flags.ensure((size_t)B * 4);
@@ -541,16 +574,14 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
     ws->t_pos.ensure((size_t)B * kp * 8); ws->t_cnt.ensure((size_t)B * 4); ws->t_exact.ensure((size_t)B * kp * 4);
     launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, Dbuf, ld, num_sms, st);
-    SelectArgs sa{};
-    sa.mode = 1; sa.dense = Dbuf; sa.ncols = N; sa.row_stride = ld; sa.col_ids = col_ids;
-    sa.B = B; sa.k = kp;
-    sa.out_ids = ws->t_ids.as<uint64_t>(); sa.out_dist = ws->t_dist.as<float>();
-    sa.out_count = ws->t_cnt.as<uint32_t>(); sa.out_pos = ws->t_pos.as<uint64_t>();
+    SelectArgs sa = select_rows(Dbuf, N, ld, B, kp, {ws->t_ids.as<uint64_t>(), ws->t_dist.as<float>(),
+                                                     ws->t_cnt.as<uint32_t>(), ws->t_pos.as<uint64_t>()});
+    sa.col_ids = col_ids;
     launch_select(sa, st);
     if (kp >= N) LGPU_CUDA(cudaMemsetAsync(ws->flags.p, 0, (size_t)B * 4, st));   // every row is a candidate
     else launch_band_check(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                            xmax, xerr, d, B, k, kp, ws->flags.as<uint32_t>(), st);
-    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, kp, out_ids, out_dist, out_cnt, Dbuf, ld);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, kp, out, Dbuf, ld);
 }
 
 // Large-N variant of tc_topk_l2 (flat search): a tensor-core pass over a row sample fixes, per query, a
@@ -559,9 +590,8 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
 // candidate list overflowed are redone by the exact kernels.
 static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
                                 const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
-                                const uint64_t *col_ids, uint32_t k, uint64_t *out_ids, float *out_dist,
-                                uint32_t *out_cnt, float *Dbuf, uint64_t ld, uint64_t min_sample = 65536,
-                                uint32_t cap = 1024)
+                                const uint64_t *col_ids, uint32_t k, TopkOut out, float *Dbuf, uint64_t ld,
+                                uint64_t min_sample = 65536, uint32_t cap = 1024)
 {
     const uint64_t Ns = std::min<uint64_t>(N, std::max<uint64_t>(min_sample, N / 8));
     const uint64_t lds = (Ns + 3) & ~3ull;               // Dbuf is [B][ld >= lds]
@@ -575,10 +605,8 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
     // 1. sample pass: dense scores of the first Ns rows, k-th best per query -> threshold
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, Ns, d, Dbuf, lds, num_sms, st);
-    SelectArgs sa{};
-    sa.mode = 1; sa.dense = Dbuf; sa.ncols = Ns; sa.row_stride = lds; sa.B = B; sa.k = k;
-    sa.out_ids = ws->sbound.as<uint64_t>(); sa.out_dist = ws->t_dist.as<float>(); sa.out_count = ws->t_cnt.as<uint32_t>();
-    launch_select(sa, st);
+    launch_select(select_rows(Dbuf, Ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
+                                                    ws->t_cnt.as<uint32_t>()}), st);
     launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                             xmax, xerr, d, B, k, ws->probe_A.as<float>(), st);
     // 2. full pass with the filtering epilogue
@@ -592,20 +620,17 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
     // 3. exact re-score of the admitted rows, final top-k; 4. fix-up of overflowed queries
-    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out_ids, out_dist, out_cnt, Dbuf, ld);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out, Dbuf, ld);
 }
 
 // top-k by (distance, id) of the dense scores D [b][ld] over N columns, with the request's distance range and
-// prefilter, into the outputs of queries q0 .. q0 + b
+// prefilter, into `out`
 static void select_dense(const float *D, uint64_t N, uint64_t ld, const uint64_t *col_ids, uint32_t b,
-                         const lgpu_search_params &sp, RowFilter rf, uint32_t q0, uint64_t *d_ids, float *d_dist,
-                         uint32_t *d_cnt, cudaStream_t st)
+                         const lgpu_search_params &sp, RowFilter rf, TopkOut out, cudaStream_t st)
 {
-    SelectArgs sa{};
-    sa.mode = 1; sa.dense = D; sa.ncols = N; sa.row_stride = ld; sa.col_ids = col_ids;
-    sa.B = b; sa.k = sp.k;
-    sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
-    sa.out_ids = d_ids + (size_t)q0 * sp.k; sa.out_dist = d_dist + (size_t)q0 * sp.k; sa.out_count = d_cnt + q0;
+    SelectArgs sa = select_rows(D, N, ld, b, sp.k, out);
+    sa.col_ids = col_ids;
+    with_range(sa, sp);
     sa.allow = rf.bits; sa.allow_bits = rf.nbits;
     launch_select(sa, st);
 }
@@ -622,210 +647,258 @@ static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, c
     LGPU_REQUIRE(B == 0 || (q && ids && dist && cnt), "null buffer");
 }
 
-// lgpu_debug_filter_bounds: the dense filter scan's own lower bounds and band, copied out instead of a result
-struct FilterDebug {
-    float *L;                     // host [B][nprobes][ld]: L of row r of the slot's partition at r < n_p
-    uint64_t ld;
-    uint32_t *parts;              // host [B][nprobes]
-    float *W, *E;                 // host [B]: scan_band, unscaled
-    uint32_t *bad;                // host [B]
-    bool ran = false;             // the filter scan ran (false: the index or the request cannot use it)
+// ---- IVF search (IVF_PQ and IVF_SQ).  One sub-batch runs [cosine: normalise] -> coarse step (probes) -> small scan |
+// regroup -> filter scan + fix-up | exact scan + select -> [refine], on the paths ivf_plan picks before any launch ----
+enum class Coarse { exact, tc_dense, tc_list };   // see ivf_coarse
+enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq };
+
+struct IvfPlan {
+    uint32_t B, nprobes, slots;
+    uint32_t np_eff;          // probes that can hold rows: min(nprobes, nlist)
+    uint32_t k, kk;           // the request's k; the PQ top-kk (k, or k * refine_factor candidates for the re-rank)
+    uint32_t lb_short;        // dense filter scan: the rows of the lb_short smallest lower bounds are re-scored
+    bool refine;
+    Coarse coarse;
+    IvfScan scan;
+    uint32_t cand_cap;        // candidate mode: candidates per query (power of two >= kk)
+    bool filter() const { return scan == IvfScan::filter_cand || scan == IvfScan::filter_dense; }
+    uint32_t rows_tile() const { return filter() ? SCAN3_ROWS_TILE : (scan == IvfScan::sq ? SQ_ROWS_TILE : SCAN_ROWS_TILE_MID); }
 };
 
-// one sub-batch of an IVF_PQ search, everything device-side on `st`
-void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
-                   const lgpu_search_params &sp, uint32_t nprobes, uint64_t *d_ids, float *d_dist,
-                   uint32_t *d_cnt, bool prof, const uint64_t *forced_probes = nullptr, RowFilter rf = RowFilter(),
-                   const uint32_t *only = nullptr, FilterDebug *dbg = nullptr)
+// prefilter: the request carries an allow bitmap; widening: the sub-batch redoes the queries flagged by the
+// maximum_nprobes widening (exact kernels only)
+static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, const lgpu_search_params &sp, bool prefilter,
+                        bool widening, const ScanModes &modes)
 {
-    // `only` (device, [B]): redo just the flagged queries (maximum_nprobes widening) -- exact kernels, outputs of
-    // the other queries are left untouched
-    const uint32_t dim = ix->dim, nlist = ix->nlist;
-    const uint32_t slots = B * nprobes;
-    int evi = 0;
-    cudaStream_t cs = st;                                // the stream of the coarse step and the regrouping
-    auto mark = [&]() { if (prof) cudaEventRecord(ws->ev[evi++], cs); };
-    mark();
-    ws->stats_mode = 0;
-    // ---- queries (normalised copy for cosine) ----
-    const float *qsearch = d_q;
-    if (ix->metric == LGPU_COSINE) {
-        ws->qn.ensure((size_t)B * dim * 4);
-        launch_normalize(d_q, B, dim, ws->qn.as<float>(), st);
-        qsearch = ws->qn.as<float>();
+    IvfPlan p{};
+    const uint32_t nlist = ix->nlist;
+    p.B = B; p.nprobes = nprobes; p.slots = B * nprobes; p.np_eff = std::min(nprobes, nlist);
+    p.k = sp.k; p.kk = sp.refine_factor ? sp.k * sp.refine_factor : sp.k; p.refine = sp.refine_factor != 0;
+    p.lb_short = p.kk <= 16 ? 32u : std::min<uint32_t>(SELECT_KMAX, 2 * p.kk + 32);
+    // the bf16 error band around the nprobes-th centroid has to fit in the tensor-core shortlist: 3x nprobes (>= 64)
+    // candidates (dense variant) or admission by threshold (list variant).  The tensor-core shortlist wins at every
+    // shape measured on 1 x H100 (400 W), down to 64 queries x 1024 lists (coarse step 0.052 vs 0.063 ms; 512 x 1024:
+    // 0.082 vs 0.160 ms); smaller problems were not measured and keep the exact kernels.  Many lists (C5: 16384): a
+    // dense [B][nlist] score matrix is 537 MB written and read back, so from coarse_list_min lists the list variant.
+    const uint32_t coarse_short = std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(64, 3 * nprobes));
+    const bool big = (uint64_t)B * nlist >= ((uint64_t)1 << 16) || modes.force_tc_coarse;
+    p.coarse = Coarse::exact;
+    if (ix->has_tc && tc_enabled() && ix->metric != LGPU_DOT && B >= 8 && nlist >= 256 && coarse_short > nprobes && big)
+        p.coarse = modes.coarse_list_min && nlist >= modes.coarse_list_min && ix->cent_ns >= 4 * nprobes && nprobes <= 64
+                       ? Coarse::tc_list : Coarse::tc_dense;
+    // tiny batches (a single query, a micro-batch): the small path, 4 launches instead of ~25; LGPU_SMALL_SLOTS = 0
+    // disables it.  Otherwise filter + verify (scan3.cu) unless the request needs every exact distance.
+    const bool small = !ix->is_sq && !widening && p.slots <= modes.small_slots &&
+                       small_scan_smem(ix->m, ix->dim) <= 200 * 1024 &&
+                       (size_t)p.slots * ix->pad_prefix[1] * 4 <= workspace_budget();
+    const bool filter = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && p.lb_short > p.kk &&
+                        ix->m <= 512 && !widening && !small;
+    if (small) p.scan = IvfScan::small;
+    else if (!filter) p.scan = ix->is_sq ? IvfScan::sq : IvfScan::exact_pq;
+    if (!filter) return p;
+    // candidate mode (no prefilter, kk <= LGPU_CAND_KMAX): the scanners threshold the rows themselves, nothing dense is
+    // written.  LGPU_CAND_CAP shrinks the capacity to exercise the overflow path.
+    const uint32_t kk = p.kk, np_eff = p.np_eff;
+    uint32_t cap = kk <= 32 ? 512 : (kk <= 64 ? 1024 : CAND_CAP_MAX);
+    // long partitions put more rows inside the band around the k-th distance (clustered data: a query near a big blob
+    // sees thousands of nearly equidistant rows): give them longer lists rather than the exact fix-up
+    const uint64_t rows_probe = std::max<uint64_t>(1, ix->pad_prefix[np_eff] / np_eff);   // mean of the np largest
+    if (rows_probe > 16384) cap = std::max<uint32_t>(cap, CAND_CAP_MAX);
+    else if (rows_probe > 4096) cap = std::max<uint32_t>(cap, 1024);
+    const uint32_t cap_env = modes.cap_env;
+    const bool cap_forced = cap_env >= 32 && cap_env <= CAND_CAP_MAX && !(cap_env & (cap_env - 1)) && cap_env >= kk;
+    if (cap_forced) cap = cap_env;
+    // A tile whose query has no threshold yet appends about k rows.  With few queries fanned out over many tiles
+    // (small B, many probes, long partitions) most of a query's tiles run at the same moment on the 2 x SMs CTAs,
+    // before any of them has published a threshold, and the list overflows whatever the scanners tighten later:
+    // estimate that concurrency from the averages and take the dense mode (cheap at such B) when it is too high.
+    bool cand_fits = true;
+    if (!cap_forced) {
+        const uint64_t tiles_part = (rows_probe + SCAN3_ROWS_TILE - 1) / SCAN3_ROWS_TILE;
+        const uint64_t parts = std::min<uint64_t>(nlist, p.slots);
+        const uint64_t groups_part = std::max<uint64_t>(1, (p.slots / parts + SCAN_G - 1) / SCAN_G);
+        const double total = (double)parts * groups_part * tiles_part;
+        const double conc = (double)np_eff * tiles_part * std::min(1.0, 2.0 * ix->num_sms / total);
+        cand_fits = conc * kk <= 2.0 * cap;
     }
-    // ---- which scan: filter + verify (scan3.cu) unless the request needs every exact distance.  The filter's
-    // per-query tables depend on the queries alone, so they are built on this stream while the coarse step and the
-    // regrouping (a latency chain of small kernels) run on the high-priority side stream `front` ----
-    // the PQ top-`kk` of every query (kk = k, or k * refine_factor candidates for the exact re-rank)
-    const uint32_t kk = sp.refine_factor ? sp.k * sp.refine_factor : sp.k;
-    const uint32_t kp = kk <= 16 ? 32u : std::min<uint32_t>(SELECT_KMAX, 2 * kk + 32);
-    // tiny batches (a single query, a micro-batch): one CTA per (query, probe) pair with the exact table in shared
-    // memory (small.cu) -- 4 launches instead of ~25; LGPU_SMALL_SLOTS = 0 disables
-    const ScanModes modes = scan_modes();
-    const bool sq = ix->is_sq;                           // IVF_SQ: no tables, no filter; the SQ scan is exact
-    const bool small_path = !sq && d_ids && !forced_probes && !only && slots <= modes.small_slots &&
-                            small_scan_smem(ix->m, dim) <= 200 * 1024 &&
-                            (size_t)slots * ix->pad_prefix[1] * 4 <= workspace_budget();
-    const bool filter_scan = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && !forced_probes &&
-                             (d_ids || dbg) && kp > kk && ix->m <= 512 && !only && !small_path;
-    bool tables_pending = false;
-    if (filter_scan) {
-        ws->qt.ensure((size_t)B * ix->nch * 256 * 16); ws->qt_mm.ensure((size_t)B * ix->nch * 8 * 8);
-        ws->qt_step.ensure((size_t)B * 4); ws->qt_base.ensure((size_t)B * 4); ws->qt_bad.ensure((size_t)B * 4);
-        ws->sbound.ensure((size_t)B * 4);
-        LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
-        LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
-        ws->front_open = !g_capturing;
-        cs = ws->front;
-        tables_pending = true;
+    p.cand_cap = cap;
+    p.scan = !prefilter && kk <= modes.cand_kmax && !modes.dense_forced && cand_fits ? IvfScan::filter_cand
+                                                                                     : IvfScan::filter_dense;
+    return p;
+}
+
+// Profiling (lgpu_last_stage_ms): ws->ev[s] is recorded where stage s ends (IVF_START: where the sub-batch starts).
+// A stage the path does not run is read back as ending where the stage before it ended.
+enum IvfStage { IVF_START, IVF_COARSE, IVF_PROBES, IVF_REGROUP, IVF_SCAN, IVF_TOPK, IVF_REFINE };
+struct StageMarks {
+    Workspace *ws;
+    bool on;
+    void operator()(IvfStage s, cudaStream_t stream) const
+    {
+        if (on) { cudaEventRecord(ws->ev[s], stream); ws->stages_marked = (s ? ws->stages_marked : 0u) | 1u << s; }
     }
-    // enqueued after the coarse GEMM, so that the GEMM's CTAs (each needs most of an SM's shared memory) are not queued
-    // behind the table grids; as SMs free up, the probe selection after it is dispatched ahead of the waiting table
-    // CTAs by the priority of `front`.  (Making the tables wait for the GEMM to finish was measured slower: the tables
-    // are then the longer branch.)
-    auto launch_tables = [&]() {
-        if (!tables_pending) return;
-        tables_pending = false;
-        launch_query_tables_q16(qsearch, ix->cb_tiled.as<float>(), ix->cb_n2.as<float>(), B, dim, ix->m, ix->nch, ix->dsub,
-                                ix->metric, ws->qt_mm.as<float>(), ws->qt.as<uint4>(), ws->qt_step.as<float>(),
-                                ws->qt_base.as<float>(), ws->sbound.as<float>(), ws->qt_bad.as<uint32_t>(), st);
-    };
-    // ---- K1: exact centroid distances + nprobes nearest ----
-    ws->probes.ensure((size_t)slots * 8);
-    ws->probe_dist.ensure((size_t)slots * 4);
+};
+
+// the queries the search runs on: a normalised copy for cosine
+static const float *ivf_queries(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B)
+{
+    if (ix->metric != LGPU_COSINE) return d_q;
+    ws->qn.ensure((size_t)B * ix->dim * 4);
+    launch_normalize(d_q, B, ix->dim, ws->qn.as<float>(), st);
+    return ws->qn.as<float>();
+}
+
+// The filter scan's per-query tables depend on the queries alone, so they are built on `st` while the coarse step and
+// the regroup (a latency chain of small kernels) run on the high-priority side stream `front`, returned here.  The
+// search stream joins it (ev_join) before the per-probe terms.
+static cudaStream_t fork_front(lgpu_index *ix, Workspace *ws, cudaStream_t st, uint32_t B)
+{
+    ws->qt.ensure((size_t)B * ix->nch * 256 * 16); ws->qt_mm.ensure((size_t)B * ix->nch * 8 * 8);
+    ws->qt_step.ensure((size_t)B * 4); ws->qt_base.ensure((size_t)B * 4); ws->qt_bad.ensure((size_t)B * 4);
+    ws->sbound.ensure((size_t)B * 4);
+    LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
+    LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
+    ws->front_open = !g_capturing;
+    return ws->front;
+}
+
+static void query_tables(lgpu_index *ix, Workspace *ws, const float *qs, uint32_t B, cudaStream_t st)
+{
+    launch_query_tables_q16(qs, ix->cb_tiled.as<float>(), ix->cb_n2.as<float>(), B, ix->dim, ix->m, ix->nch, ix->dsub,
+                            ix->metric, ws->qt_mm.as<float>(), ws->qt.as<uint4>(), ws->qt_step.as<float>(),
+                            ws->qt_base.as<float>(), ws->sbound.as<float>(), ws->qt_bad.as<uint32_t>(), st);
+}
+
+// Coarse::tc_list up to the finishing kernel: (1) dense scores of a strided SAMPLE of the centroids; their nprobes-th
+// smallest + 2 E_q bounds, per query, the scores of every true probe; (2) the full GEMM runs with the filtering epilogue
+// and appends (column, score) of the few columns under that bound to the query's list; (3) the finishing kernel works
+// on the list (second-level threshold from the list's own nprobes-th smallest, exact re-score, sort).
+static void coarse_list(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, uint32_t *cgate,
+                        cudaStream_t cs, cudaStream_t st)
+{
+    const uint32_t B = p.B, nprobes = p.nprobes, dim = ix->dim;
+    const uint32_t ns = ix->cent_ns, lds = (ns + 3u) & ~3u, lcap = 1024;
+    ws->t_dist.ensure((size_t)B * nprobes * 4); ws->t_ids.ensure((size_t)B * nprobes * 8);
+    ws->t_cnt.ensure((size_t)B * 4); ws->probe_A.ensure((size_t)B * 4); ws->amax.ensure((size_t)B * 4);
+    ws->t_pos.ensure((size_t)B * lcap * 8); ws->t_exact.ensure((size_t)B * lcap * 4);
+    launch_gemm_dist(ws->qb.p, ix->cent_sb.p, ix->cent_sn2.as<float>(), B, ns, dim, ws->D.as<float>(), lds, ix->num_sms, cs);
+    if (!launch_sample_kth_threshold(ws->D.as<float>(), lds, ns, ws->qn2.as<float>(), ws->qerr.as<float>(), ix->cent_max,
+                                     ix->cent_err, dim, B, nprobes, ws->probe_A.as<float>(), cs)) {
+        launch_select(select_rows(ws->D.as<float>(), ns, lds, B, nprobes, {ws->t_ids.as<uint64_t>(),
+                                  ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>()}), cs);
+        launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(),
+                                ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, B, nprobes, ws->probe_A.as<float>(),
+                                cs);
+    }
+    LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, cs));
+    GemmFilter flt{};
+    flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
+    flt.cand_ids = nullptr; flt.col_ids = nullptr; flt.cap = lcap; flt.cand_s = ws->t_exact.as<float>();
+    launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, ix->nlist, dim, nullptr, 0, ix->num_sms, cs, &flt);
+    if (p.filter()) query_tables(ix, ws, qs, B, st);
+    launch_coarse_finish(ws->t_exact.as<float>(), lcap, B, lcap, qs, ix->centroids.as<float>(), ws->qn2.as<float>(),
+                         ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes, ws->probes.as<uint64_t>(),
+                         ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate, cs,
+                         ws->t_pos.as<uint64_t>(), ws->amax.as<uint32_t>());
+}
+
+// The nprobes nearest partitions of every query into ws->probes / probe_dist / probe_cnt, on `cs`.  With the filter
+// scan the query tables go on `st`: right after the coarse GEMM (tensor-core variants), so that the GEMM's CTAs (each
+// needs most of an SM's shared memory) are not queued behind the table grids and, as SMs free up, the probe selection
+// after it is dispatched ahead of the waiting table CTAs by the priority of `front` (making the tables wait for the GEMM
+// to finish was measured slower: the tables are then the longer branch); after the probe select (exact variant).
+static void ivf_coarse(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, cudaStream_t cs,
+                       cudaStream_t st, const StageMarks &mark)
+{
+    const uint32_t B = p.B, nprobes = p.nprobes, nlist = ix->nlist, dim = ix->dim;
+    ws->probes.ensure((size_t)p.slots * 8);
+    ws->probe_dist.ensure((size_t)p.slots * 4);
     ws->probe_cnt.ensure((size_t)B * 4);
-    if (forced_probes) {
-        LGPU_CUDA(cudaMemcpyAsync(ws->probes.p, forced_probes, (size_t)slots * 8, cudaMemcpyHostToDevice, cs));
-        mark();
-    } else {
-        const uint64_t ldc = (nlist + 3u) & ~3u;
-        ws->D.ensure((size_t)B * ldc * 4);
-        // the bf16 error band around the nprobes-th centroid has to fit in the shortlist, so take 3x
-        // nprobes (>= 64) candidates (dense variant) or admit by threshold (filtered variant)
-        const uint32_t kp = std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(64, 3 * nprobes));
-        // the tensor-core shortlist wins at every shape measured on 1 x H100 (400 W), down to 64 queries x 1024 lists
-        // (coarse step 0.052 vs 0.063 ms; 512 x 1024: 0.082 vs 0.160 ms); smaller problems were not measured and
-        // keep the exact kernels
-        const bool big = (uint64_t)B * nlist >= ((uint64_t)1 << 16) || getenv("LGPU_FORCE_TC_COARSE");
-        if (ix->has_tc && tc_enabled() && ix->metric != LGPU_DOT && B >= 8 && nlist >= 256 && kp > nprobes && big) {
-            // tensor-core GEMM scores + one finishing kernel per query (threshold, exact re-score in lance order, top
-            // nprobes): bit-identical probe sets; queries whose candidate band overflowed are redone exactly
-            mark();
-            ws->qb.ensure((size_t)B * dim * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
-            ws->flags.ensure((size_t)B * 4);
-            ws->c_wcnt.ensure(16);
-            uint32_t *cgate = ws->c_wcnt.as<uint32_t>() + 2;    // 0 = no query overflowed: the exact fix-up returns at once
-            launch_to_bf16(qsearch, B, dim, ws->qb.p, ws->qn2.as<float>(), cs, ws->qerr.as<float>());
-            if (modes.coarse_list_min && nlist >= modes.coarse_list_min && ix->cent_ns >= 4 * nprobes && nprobes <= 64) {
-                // Many lists (C5: 16384): a dense [B][nlist] score matrix is 537 MB written and read back.  Instead: (1) dense scores of a strided SAMPLE of the centroids; their
-                // nprobes-th smallest + 2 E_q bounds, per query, the scores of every true probe; (2) the full GEMM runs
-                // with the filtering epilogue and appends (column, score) of the few columns under that bound to the
-                // query's list; (3) the finishing kernel works on the list (second-level threshold from the list's own
-                // nprobes-th smallest, exact re-score, sort).  Overflowing lists are redone by the exact kernels.
-                const uint32_t ns = ix->cent_ns, lds = (ns + 3u) & ~3u, lcap = 1024;
-                ws->t_dist.ensure((size_t)B * nprobes * 4); ws->t_ids.ensure((size_t)B * nprobes * 8);
-                ws->t_cnt.ensure((size_t)B * 4); ws->probe_A.ensure((size_t)B * 4); ws->amax.ensure((size_t)B * 4);
-                ws->t_pos.ensure((size_t)B * lcap * 8); ws->t_exact.ensure((size_t)B * lcap * 4);
-                launch_gemm_dist(ws->qb.p, ix->cent_sb.p, ix->cent_sn2.as<float>(), B, ns, dim, ws->D.as<float>(), lds,
-                                 ix->num_sms, cs);
-                if (!launch_sample_kth_threshold(ws->D.as<float>(), lds, ns, ws->qn2.as<float>(), ws->qerr.as<float>(),
-                                                 ix->cent_max, ix->cent_err, dim, B, nprobes, ws->probe_A.as<float>(), cs)) {
-                    SelectArgs ss{};
-                    ss.mode = 1; ss.dense = ws->D.as<float>(); ss.ncols = ns; ss.row_stride = lds; ss.B = B; ss.k = nprobes;
-                    ss.out_ids = ws->t_ids.as<uint64_t>(); ss.out_dist = ws->t_dist.as<float>(); ss.out_count = ws->t_cnt.as<uint32_t>();
-                    launch_select(ss, cs);
-                    launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(),
-                                            ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, B, nprobes,
-                                            ws->probe_A.as<float>(), cs);
-                }
-                LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, cs));
-                GemmFilter flt{};
-                flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
-                flt.cand_ids = nullptr; flt.col_ids = nullptr; flt.cap = lcap; flt.cand_s = ws->t_exact.as<float>();
-                launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, nullptr, 0, ix->num_sms, cs, &flt);
-                launch_tables();
-                launch_coarse_finish(ws->t_exact.as<float>(), lcap, B, lcap, qsearch, ix->centroids.as<float>(),
-                                     ws->qn2.as<float>(), ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes,
-                                     ws->probes.as<uint64_t>(),
-                                     ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate,
-                                     cs, ws->t_pos.as<uint64_t>(), ws->amax.as<uint32_t>());
-            } else {
-                launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, ws->D.as<float>(), ldc,
-                                 ix->num_sms, cs);
-                launch_tables();
-                launch_coarse_finish(ws->D.as<float>(), ldc, B, nlist, qsearch, ix->centroids.as<float>(), ws->qn2.as<float>(),
-                                     ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes, ws->probes.as<uint64_t>(), ws->probe_dist.as<float>(),
-                                     ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate, cs);
-            }
-            launch_dist_matrix(qsearch, ix->centroids.as<float>(), B, nlist, dim, 0, nullptr, nullptr, ws->D.as<float>(), ldc,
-                               cs, ws->flags.as<uint32_t>(), cgate);
-            SelectArgs sc{};
-            sc.mode = 1; sc.dense = ws->D.as<float>(); sc.ncols = nlist; sc.row_stride = ldc;
-            sc.B = B; sc.k = nprobes; sc.out_ids = ws->probes.as<uint64_t>(); sc.out_dist = ws->probe_dist.as<float>();
-            sc.out_count = ws->probe_cnt.as<uint32_t>(); sc.only = ws->flags.as<uint32_t>(); sc.gate = cgate;
-            launch_select(sc, cs);
-        } else {
-            launch_dist_matrix(qsearch, ix->centroids.as<float>(), B, nlist, dim, ix->metric == LGPU_DOT ? 1 : 0,
-                               nullptr, nullptr, ws->D.as<float>(), ldc, cs);
-            mark();
-            SelectArgs sa{};
-            sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = nlist; sa.row_stride = ldc;
-            sa.B = B; sa.k = nprobes;
-            sa.out_ids = ws->probes.as<uint64_t>(); sa.out_dist = ws->probe_dist.as<float>();
-            sa.out_count = ws->probe_cnt.as<uint32_t>();
-            launch_select(sa, cs);
-        }
-    }
-    launch_tables();
-    if (sq) {
-        ws->sq_q.ensure((size_t)B * ix->dim_pad); ws->sq_qq.ensure((size_t)B * 4);
-        launch_sq_encode(qsearch, B, dim, ix->dim_pad, ix->sq_lo, ix->sq_hi, ws->sq_q.as<uint8_t>(),
-                         ws->sq_qq.as<uint32_t>(), st);
-    }
-    mark();
-    if (small_path) {
-        mark();                                          // (no regrouping)
-        const uint64_t stride = std::max<uint64_t>(ix->pad_prefix[1], 4);
-        ws->seg_off.ensure((size_t)slots * 8);
-        ws->dist_out.ensure((size_t)slots * stride * 4);
-        SmallScanArgs ss{};
-        ss.centroids = ix->centroids.as<float>(); ss.cb_tiled = ix->cb_tiled.as<float>();
-        ss.codes = ix->codes.as<unsigned char>(); ss.code_base = ix->code_base.as<uint64_t>();
-        ss.part_n = ix->part_n.as<uint32_t>(); ss.part_npad = ix->part_npad.as<uint32_t>();
-        ss.dim = dim; ss.m = ix->m; ss.nch = ix->nch; ss.metric = (uint32_t)ix->metric; ss.nlist = nlist; ss.nprobes = nprobes;
-        ss.queries = qsearch; ss.probes = ws->probes.as<uint64_t>(); ss.seg_stride = stride;
-        ss.seg_off = ws->seg_off.as<uint64_t>(); ss.dist_out = ws->dist_out.as<float>();
-        launch_small_scan(ss, ix->dsub, slots, st);
-        mark();
-        SelectArgs sa{};
-        sa.mode = 0; sa.dist = ws->dist_out.as<float>(); sa.seg_off = ws->seg_off.as<uint64_t>();
-        sa.probes = ws->probes.as<uint64_t>(); sa.nprobes = nprobes; sa.nlist = nlist;
-        sa.part_n = ix->part_n.as<uint32_t>(); sa.part_off = ix->part_off.as<uint64_t>();
-        sa.row_ids = ix->row_ids.as<uint64_t>(); sa.B = B;
-        sa.allow = rf.bits; sa.allow_bits = rf.nbits;
-        sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
-        sa.k = kk; sa.out_ids = d_ids; sa.out_dist = d_dist; sa.out_count = d_cnt;
-        if (sp.refine_factor) {
-            ws->t_ids.ensure((size_t)B * kk * 8); ws->t_dist.ensure((size_t)B * kk * 4);
-            ws->t_pos.ensure((size_t)B * kk * 8); ws->t_cnt.ensure((size_t)B * 4); ws->t_exact.ensure((size_t)B * kk * 4);
-            sa.out_ids = ws->t_ids.as<uint64_t>(); sa.out_dist = ws->t_dist.as<float>();
-            sa.out_count = ws->t_cnt.as<uint32_t>(); sa.out_pos = ws->t_pos.as<uint64_t>();
-        }
-        launch_select(sa, st);
-        mark();
-        if (sp.refine_factor == 0) { mark(); return; }
-        launch_pair_distance(d_q, ix->vectors.as<float>(), ws->t_pos.as<uint64_t>(), B, kk, dim, ix->metric,
-                             ws->t_exact.as<float>(), st);
-        SelectArgs sr{};
-        sr.mode = 2; sr.dense = ws->t_exact.as<float>(); sr.cand_ids = ws->t_ids.as<uint64_t>();
-        sr.ncols = kk; sr.inner = kk; sr.row_stride = kk; sr.outer_stride = 0;
-        sr.B = B; sr.k = sp.k; sr.out_ids = d_ids; sr.out_dist = d_dist; sr.out_count = d_cnt;
-        launch_select(sr, st);
-        mark();
+    const uint64_t ldc = (nlist + 3u) & ~3u;
+    ws->D.ensure((size_t)B * ldc * 4);
+    const TopkOut probes{ws->probes.as<uint64_t>(), ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>()};
+    if (p.coarse == Coarse::exact) {
+        launch_dist_matrix(qs, ix->centroids.as<float>(), B, nlist, dim, ix->metric == LGPU_DOT ? 1 : 0, nullptr, nullptr,
+                           ws->D.as<float>(), ldc, cs);
+        mark(IVF_COARSE, cs);
+        launch_select(select_rows(ws->D.as<float>(), nlist, ldc, B, nprobes, probes), cs);
+        if (p.filter()) query_tables(ix, ws, qs, B, st);
         return;
     }
-    // ---- regroup probe slots by partition ----
+    // tensor-core GEMM scores + one finishing kernel per query (threshold, exact re-score in lance order, top nprobes):
+    // bit-identical probe sets; queries whose candidate band overflowed are redone exactly
+    mark(IVF_COARSE, cs);
+    ws->qb.ensure((size_t)B * dim * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
+    ws->flags.ensure((size_t)B * 4);
+    ws->c_wcnt.ensure(16);
+    uint32_t *cgate = ws->c_wcnt.as<uint32_t>() + 2;    // 0 = no query overflowed: the exact fix-up returns at once
+    launch_to_bf16(qs, B, dim, ws->qb.p, ws->qn2.as<float>(), cs, ws->qerr.as<float>());
+    if (p.coarse == Coarse::tc_list) {
+        coarse_list(ix, ws, p, qs, cgate, cs, st);
+    } else {
+        launch_gemm_dist(ws->qb.p, ix->cent_b.p, ix->cent_n2.as<float>(), B, nlist, dim, ws->D.as<float>(), ldc,
+                         ix->num_sms, cs);
+        if (p.filter()) query_tables(ix, ws, qs, B, st);
+        launch_coarse_finish(ws->D.as<float>(), ldc, B, nlist, qs, ix->centroids.as<float>(), ws->qn2.as<float>(),
+                             ws->qerr.as<float>(), ix->cent_max, ix->cent_err, dim, nprobes, ws->probes.as<uint64_t>(),
+                             ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>(), ws->flags.as<uint32_t>(), cgate, cs);
+    }
+    launch_dist_matrix(qs, ix->centroids.as<float>(), B, nlist, dim, 0, nullptr, nullptr, ws->D.as<float>(), ldc, cs,
+                       ws->flags.as<uint32_t>(), cgate);
+    SelectArgs sc = select_rows(ws->D.as<float>(), nlist, ldc, B, nprobes, probes);
+    sc.only = ws->flags.as<uint32_t>(); sc.gate = cgate;
+    launch_select(sc, cs);
+}
+
+// mode 0: the k best rows of every query's probed segments of ws->dist_out, prefilter applied before the top-k
+static SelectArgs select_segments(lgpu_index *ix, Workspace *ws, const IvfPlan &p, uint32_t k, TopkOut out, RowFilter rf)
+{
+    SelectArgs s = select_args(0, p.B, k, out);
+    s.dist = ws->dist_out.as<float>(); s.seg_off = ws->seg_off.as<uint64_t>(); s.probes = ws->probes.as<uint64_t>();
+    s.nprobes = p.nprobes; s.nlist = ix->nlist; s.part_n = ix->part_n.as<uint32_t>();
+    s.part_off = ix->part_off.as<uint64_t>(); s.row_ids = ix->row_ids.as<uint64_t>();
+    s.allow = rf.bits; s.allow_bits = rf.nbits;
+    return s;
+}
+
+// where the PQ top-kk goes: straight to the caller, or to the refine stage's candidate lists
+static TopkOut pq_out(Workspace *ws, const IvfPlan &p, TopkOut out)
+{
+    if (!p.refine) return out;
+    const size_t n = (size_t)p.B * p.kk;
+    ws->t_ids.ensure(n * 8); ws->t_dist.ensure(n * 4); ws->t_pos.ensure(n * 8); ws->t_cnt.ensure((size_t)p.B * 4);
+    ws->t_exact.ensure(n * 4);
+    return {ws->t_ids.as<uint64_t>(), ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->t_pos.as<uint64_t>()};
+}
+
+// IvfScan::small: small_scan into one segment per probe slot, then the PQ top-kk
+static void ivf_small(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp, const float *qs,
+                      RowFilter rf, TopkOut out, cudaStream_t st, const StageMarks &mark)
+{
+    const uint64_t stride = std::max<uint64_t>(ix->pad_prefix[1], 4);
+    ws->seg_off.ensure((size_t)p.slots * 8);
+    ws->dist_out.ensure((size_t)p.slots * stride * 4);
+    SmallScanArgs ss{};
+    ss.centroids = ix->centroids.as<float>(); ss.cb_tiled = ix->cb_tiled.as<float>();
+    ss.codes = ix->codes.as<unsigned char>(); ss.code_base = ix->code_base.as<uint64_t>();
+    ss.part_n = ix->part_n.as<uint32_t>(); ss.part_npad = ix->part_npad.as<uint32_t>();
+    ss.dim = ix->dim; ss.m = ix->m; ss.nch = ix->nch; ss.metric = (uint32_t)ix->metric; ss.nlist = ix->nlist;
+    ss.nprobes = p.nprobes;
+    ss.queries = qs; ss.probes = ws->probes.as<uint64_t>(); ss.seg_stride = stride;
+    ss.seg_off = ws->seg_off.as<uint64_t>(); ss.dist_out = ws->dist_out.as<float>();
+    launch_small_scan(ss, ix->dsub, p.slots, st);
+    mark(IVF_SCAN, st);
+    SelectArgs sa = select_segments(ix, ws, p, p.kk, pq_out(ws, p, out), rf);
+    with_range(sa, sp);
+    launch_select(sa, st);
+    mark(IVF_TOPK, st);
+}
+
+// regroup the probe slots by partition into tiles of p.rows_tile() rows (group.cu) on `cs`, and size ws->dist_out for
+// the distance segments.  only (device, [B]): just the flagged queries.
+static GroupArgs ivf_regroup(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const uint32_t *only, cudaStream_t cs)
+{
+    const uint32_t B = p.B, slots = p.slots, nlist = ix->nlist;
     ws->part_cnt.ensure((size_t)nlist * 4);
     ws->slot_pos.ensure((size_t)slots * 4);
     ws->seg_local.ensure((size_t)slots * 8);
@@ -836,7 +909,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
     ws->qlist.ensure((size_t)slots * 4);
     ws->scalars.ensure(64);
     GroupArgs ga{};
-    ga.probes = ws->probes.as<uint64_t>(); ga.B = B; ga.nprobes = nprobes; ga.nlist = nlist;
+    ga.probes = ws->probes.as<uint64_t>(); ga.B = B; ga.nprobes = p.nprobes; ga.nlist = nlist;
     ga.part_n = ix->part_n.as<uint32_t>(); ga.part_cnt = ws->part_cnt.as<uint32_t>();
     ga.part_npad = ix->part_npad.as<uint32_t>(); ga.code_base = ix->code_base.as<uint64_t>(); ga.part_off = ix->part_off.as<uint64_t>();
     ga.slot_pos = ws->slot_pos.as<uint32_t>(); ga.seg_local = ws->seg_local.as<uint64_t>();
@@ -847,226 +920,218 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
     ga.scanned_rows = reinterpret_cast<unsigned long long *>(ws->scalars.as<char>() + 16);
     // tile descriptors, sized by a host bound on the tile count (for 1536-row tiles; 3072-row tiles need fewer)
     // sum_p ceil(cnt_p / 8) * nrb_p <= (slots / 8 + #probed partitions) * max_p nrb_p
-    {
-        uint64_t max_tiles = ((uint64_t)slots / SCAN_G + std::min<uint64_t>(nlist, slots) + 1) * ix->max_nrb;
-        LGPU_REQUIRE(max_tiles < (1ull << 31), "batch too large for one scan launch");
-        ws->tile_desc.ensure((size_t)max_tiles * sizeof(TileDesc));
-        ga.tile_desc = ws->tile_desc.as<TileDesc>(); ga.max_tiles = (uint32_t)max_tiles;
-    }
+    const uint64_t max_tiles = ((uint64_t)slots / SCAN_G + std::min<uint64_t>(nlist, slots) + 1) * ix->max_nrb;
+    LGPU_REQUIRE(max_tiles < (1ull << 31), "batch too large for one scan launch");
+    ws->tile_desc.ensure((size_t)max_tiles * sizeof(TileDesc));
+    ga.tile_desc = ws->tile_desc.as<TileDesc>(); ga.max_tiles = (uint32_t)max_tiles;
     ga.only = only;
-    ga.rows_tile = filter_scan ? SCAN3_ROWS_TILE : (sq ? SQ_ROWS_TILE : SCAN_ROWS_TILE_MID);
+    ga.rows_tile = p.rows_tile();
     launch_group(ga, cs);
-    mark();
-    if (filter_scan) {
-        LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
-        cs = st;
-    }
-    // ---- K2+K3 ----
-    uint32_t np_eff = std::min<uint32_t>(nprobes, nlist);
-    size_t cap_floats = (size_t)B * ix->pad_prefix[np_eff];
-    ws->dist_out.ensure(std::max<size_t>(cap_floats, 4) * 4);
+    ws->dist_out.ensure(std::max<size_t>((size_t)B * ix->pad_prefix[p.np_eff], 4) * 4);
+    return ga;
+}
+
+// the arguments scan2 and scan3 share: the regrouped tiles, the distance segments
+static ScanArgs scan_args(lgpu_index *ix, Workspace *ws, const float *qs, const GroupArgs &ga)
+{
     ScanArgs sc{};
     sc.centroids = ix->centroids.as<float>(); sc.cb_tiled = ix->cb_tiled.as<float>();
     sc.codes = ix->codes.as<unsigned char>(); sc.code_base = ix->code_base.as<uint64_t>();
     sc.part_n = ix->part_n.as<uint32_t>(); sc.part_npad = ix->part_npad.as<uint32_t>();
-    sc.dim = dim; sc.m = ix->m; sc.nch = ix->nch; sc.metric = (uint32_t)ix->metric; sc.nlist = nlist;
+    sc.dim = ix->dim; sc.m = ix->m; sc.nch = ix->nch; sc.metric = (uint32_t)ix->metric; sc.nlist = ix->nlist;
     sc.rows_tile = ga.rows_tile; sc.fzero2 = 0ull;
-    sc.queries = qsearch;
+    sc.queries = qs;
     sc.total_tiles = ga.total_tiles; sc.tile_counter = ga.tile_counter;
     sc.dist_out = ws->dist_out.as<float>();
     sc.tile_desc = ga.tile_desc;
     sc.part_off = ix->part_off.as<uint64_t>();
+    return sc;
+}
 
-    // K4 over the distance segments: the kk best by (_distance, _rowid), prefilter applied before the top-k
-    SelectArgs sa{};
-    sa.mode = 0; sa.dist = ws->dist_out.as<float>(); sa.seg_off = ga.seg_off; sa.probes = ga.probes;
-    sa.nprobes = nprobes; sa.nlist = nlist; sa.part_n = ix->part_n.as<uint32_t>(); sa.part_off = ix->part_off.as<uint64_t>();
-    sa.row_ids = ix->row_ids.as<uint64_t>(); sa.B = B;
-    sa.allow = rf.bits; sa.allow_bits = rf.nbits;
-    sa.only = only;
-    // where the PQ top-kk goes: straight to the caller, or to the refine stage's candidate lists
-    uint64_t *pq_ids = d_ids; float *pq_dist = d_dist; uint32_t *pq_cnt = d_cnt; uint64_t *pq_pos = nullptr;
-    if (sp.refine_factor) {
-        ws->t_ids.ensure((size_t)B * kk * 8); ws->t_dist.ensure((size_t)B * kk * 4);
-        ws->t_pos.ensure((size_t)B * kk * 8); ws->t_cnt.ensure((size_t)B * 4);
-        ws->t_exact.ensure((size_t)B * kk * 4);
-        pq_ids = ws->t_ids.as<uint64_t>(); pq_dist = ws->t_dist.as<float>(); pq_cnt = ws->t_cnt.as<uint32_t>();
-        pq_pos = ws->t_pos.as<uint64_t>();
+// The filter scan's prologue on `st`: its buffers, the join with `front` (probes and regroup), the per-probe terms and
+// the 16-bit per-query tables in `sc`
+static void filter_terms(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, ScanArgs &sc, cudaStream_t st)
+{
+    const uint32_t B = p.B, kp = p.lb_short;
+    const bool dot = ix->metric == LGPU_DOT;
+    ws->flags.ensure((size_t)B * 4); ws->c_wcnt.ensure(16); ws->c_surv.ensure((size_t)B * 4);
+    ws->s_ids.ensure((size_t)B * kp * 8); ws->s_lb.ensure((size_t)B * kp * 4); ws->s_pos.ensure((size_t)B * kp * 8);
+    ws->s_cnt.ensure((size_t)B * 4); ws->s_exact.ensure((size_t)B * kp * 4);
+    LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));
+    ws->front_open = false;
+    ws->qn2.ensure((size_t)B * 4);
+    if (!dot) {
+        ws->probe_A.ensure((size_t)p.slots * 4); ws->amax.ensure((size_t)B * 4);
+        sc.probe_A = ws->probe_A.as<float>(); sc.row_R = ix->row_R.as<float>();
     }
+    launch_probe_terms(ws->probe_dist.as<float>(), qs, B, p.nprobes, ix->dim, dot ? nullptr : ws->probe_A.as<float>(),
+                       dot ? nullptr : ws->amax.as<float>(), ws->qn2.as<float>(), ws->qt_base.as<float>(),
+                       ws->qt_bad.as<uint32_t>(), st);
+    sc.qt = ws->qt.as<uint4>(); sc.qt_step = ws->qt_step.as<float>(); sc.qt_base = ws->qt_base.as<float>();
+}
 
-    if (filter_scan) {
-        // per-query 16-bit tables, per-probe scalars
-        const bool dot = ix->metric == LGPU_DOT;
-        ws->flags.ensure((size_t)B * 4); ws->c_wcnt.ensure(16); ws->c_surv.ensure((size_t)B * 4);
-        ws->s_ids.ensure((size_t)B * kp * 8); ws->s_lb.ensure((size_t)B * kp * 4); ws->s_pos.ensure((size_t)B * kp * 8);
-        ws->s_cnt.ensure((size_t)B * 4); ws->s_exact.ensure((size_t)B * kp * 4);
-        LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));        // the probes and the regrouping, from `front`
-        ws->front_open = false;
-        ws->qn2.ensure((size_t)B * 4);
-        if (!dot) {
-            ws->probe_A.ensure((size_t)slots * 4); ws->amax.ensure((size_t)B * 4);
-            sc.probe_A = ws->probe_A.as<float>(); sc.row_R = ix->row_R.as<float>();
-        }
-        launch_probe_terms(ws->probe_dist.as<float>(), qsearch, B, nprobes, dim, dot ? nullptr : ws->probe_A.as<float>(),
-                           dot ? nullptr : ws->amax.as<float>(), ws->qn2.as<float>(), ws->qt_base.as<float>(),
-                           ws->qt_bad.as<uint32_t>(), st);
-        sc.qt = ws->qt.as<uint4>(); sc.qt_step = ws->qt_step.as<float>(); sc.qt_base = ws->qt_base.as<float>();
-        const float mscale = ix->metric == LGPU_COSINE ? 0.5f : 1.0f;
-        // candidate mode (no prefilter, k <= 32): the scanners threshold the rows themselves, nothing dense is written
-        // candidate capacity per query (power of two >= k); LGPU_CAND_CAP shrinks it to exercise the overflow path
-        const uint32_t cap_env = modes.cap_env;
-        uint32_t cap = kk <= 32 ? 512 : (kk <= 64 ? 1024 : CAND_CAP_MAX);
-        {
-            // long partitions put more rows inside the band around the k-th distance (clustered data: a query near a
-            // big blob sees thousands of nearly equidistant rows): give them longer lists rather than the exact fix-up
-            const uint64_t rows_probe = std::max<uint64_t>(1, ix->pad_prefix[np_eff] / np_eff);   // mean of the np largest
-            if (rows_probe > 16384) cap = std::max<uint32_t>(cap, CAND_CAP_MAX);
-            else if (rows_probe > 4096) cap = std::max<uint32_t>(cap, 1024);
-        }
-        bool cap_forced = false;
-        if (cap_env >= 32 && cap_env <= CAND_CAP_MAX && !(cap_env & (cap_env - 1)) && cap_env >= kk) { cap = cap_env; cap_forced = true; }
-        // A tile whose query has no threshold yet appends about k rows.  With few queries fanned out over many tiles
-        // (small B, many probes, long partitions) most of a query's tiles run at the same moment on the 2 x SMs CTAs,
-        // before any of them has published a threshold, and the list overflows whatever the scanners tighten later:
-        // estimate that concurrency from the averages and take the dense mode (cheap at such B) when it is too high.
-        bool cand_fits = true;
-        if (!cap_forced) {
-            const uint64_t rows_part = std::max<uint64_t>(1, ix->pad_prefix[np_eff] / np_eff);
-            const uint64_t tiles_part = (rows_part + SCAN3_ROWS_TILE - 1) / SCAN3_ROWS_TILE;
-            const uint64_t parts = std::min<uint64_t>(nlist, slots);
-            const uint64_t groups_part = std::max<uint64_t>(1, (slots / parts + SCAN_G - 1) / SCAN_G);
-            const double total = (double)parts * groups_part * tiles_part;
-            const double conc = (double)np_eff * tiles_part * std::min(1.0, 2.0 * ix->num_sms / total);
-            cand_fits = conc * kk <= 2.0 * cap;
-        }
-        const bool cand_mode = !rf.bits && kk <= modes.cand_kmax && !modes.dense_forced && cand_fits && !dbg;
-        if (cand_mode) {
-            ws->c_thr.ensure((size_t)B * 4); ws->c_slack.ensure((size_t)B * 4); ws->c_cnt.ensure((size_t)B * 4);
-            ws->c_rec.ensure((size_t)B * cap * sizeof(CandRec));
-            ws->c_key.ensure((size_t)B * cap * 4); ws->c_last.ensure((size_t)B * 4);
-            launch_cand_prepare(ws->qt_step.as<float>(), ws->sbound.as<float>(), dot ? nullptr : ws->amax.as<float>(),
-                                dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B,
-                                ws->c_slack.as<float>(), ws->c_thr.as<uint32_t>(), ws->c_cnt.as<uint32_t>(),
-                                ws->c_last.as<uint32_t>(), ws->c_key.as<uint32_t>(), cap, st);
-            sc.cand_key = ws->c_key.as<uint32_t>(); sc.cand_last = ws->c_last.as<uint32_t>();
-            sc.nprobes = nprobes; sc.topk = kk; sc.thr = ws->c_thr.as<uint32_t>(); sc.slack = ws->c_slack.as<float>();
-            sc.cand_cnt = ws->c_cnt.as<uint32_t>(); sc.cand = ws->c_rec.as<CandRec>(); sc.cand_cap = cap;
-            launch_scan3(sc, ix->num_sms, st);
-            mark();
-            FinalizeArgs fa{};
-            fa.Q = qsearch; fa.cand = sc.cand; fa.cand_cnt = sc.cand_cnt; fa.cand_cap = cap; fa.cand_key = sc.cand_key; fa.thr = sc.thr;
-            fa.slack = sc.slack; fa.bad = ws->qt_bad.as<uint32_t>();
-            fa.codes = ix->codes.as<unsigned char>(); fa.code_base = ix->code_base.as<uint64_t>();
-            fa.part_npad = ix->part_npad.as<uint32_t>(); fa.part_off = ix->part_off.as<uint64_t>();
-            fa.row_ids = ix->row_ids.as<uint64_t>(); fa.centroids = ix->centroids.as<float>();
-            fa.cb_tiled = ix->cb_tiled.as<float>();
-            fa.B = B; fa.dim = dim; fa.m = ix->m; fa.dsub = ix->dsub; fa.k = kk; fa.metric = ix->metric;
-            fa.out_ids = pq_ids; fa.out_dist = pq_dist; fa.out_count = pq_cnt; fa.out_pos = pq_pos;
-            fa.flags = ws->flags.as<uint32_t>();
-            ws->c_work.ensure((size_t)B * cap * 8); ws->c_wcnt.ensure(16); ws->c_surv.ensure((size_t)B * 4);
-            ws->c_exd.ensure((size_t)B * cap * 4); ws->c_exi.ensure((size_t)B * cap * 8); ws->c_exp.ensure((size_t)B * cap * 8);
-            fa.work = ws->c_work.as<uint2>(); fa.work_cnt = ws->c_wcnt.as<uint32_t>(); fa.surv_cnt = ws->c_surv.as<uint32_t>();
-            fa.ex_dist = ws->c_exd.as<float>(); fa.ex_id = ws->c_exi.as<uint64_t>(); fa.ex_pos = ws->c_exp.as<uint64_t>();
-            fa.num_sms = ix->num_sms;
-            if (prof) {
-                ws->c_stats.ensure(32);
-                LGPU_CUDA(cudaMemsetAsync(ws->c_stats.p, 0, 32, st));
-                fa.stats = ws->c_stats.as<unsigned long long>();
-                ws->stats_mode = 1;
-            }
-            launch_cand_finalize(fa, st);
-            sc.cand = nullptr;                      // (the fix-up pass below is the exact kernel)
-        } else {
-        launch_scan3(sc, ix->num_sms, st);
-        mark();
-        if (dbg) {
-            // W, E of every query (the band the consumers use) and the scan's own L, per probe slot
-            ws->s_exact.ensure((size_t)B * 8);
-            float *dW = ws->s_exact.as<float>(), *dE = dW + B;
-            launch_scan_band(ws->qt_step.as<float>(), ws->sbound.as<float>(), dot ? nullptr : ws->amax.as<float>(),
-                             dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, ix->m, dot, B, dW, dE, st);
-            std::vector<uint64_t> probes(slots), seg(slots);
-            std::vector<float> L(cap_floats);
-            LGPU_CUDA(cudaMemcpyAsync(probes.data(), ws->probes.p, (size_t)slots * 8, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaMemcpyAsync(seg.data(), ga.seg_off, (size_t)slots * 8, cudaMemcpyDeviceToHost, st));
-            if (cap_floats) LGPU_CUDA(cudaMemcpyAsync(L.data(), ws->dist_out.p, cap_floats * 4, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaMemcpyAsync(dbg->W, dW, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaMemcpyAsync(dbg->E, dE, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaMemcpyAsync(dbg->bad, ws->qt_bad.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaStreamSynchronize(st));
-            for (uint32_t sl = 0; sl < slots; sl++) {
-                const uint64_t p = probes[sl];
-                dbg->parts[sl] = p < nlist ? (uint32_t)p : UINT32_MAX;
-                const uint64_t n = p < nlist ? std::min<uint64_t>(ix->h_part_n[p], dbg->ld) : 0;
-                if (n) memcpy(dbg->L + (size_t)sl * dbg->ld, L.data() + seg[sl], n * 4);
-            }
-            dbg->ran = true;
-            return;
-        }
-        // shortlist: the kp smallest lower bounds (with their storage positions)
-        SelectArgs ss = sa;
-        ss.k = kp; ss.out_ids = ws->s_ids.as<uint64_t>(); ss.out_dist = ws->s_lb.as<float>();
-        ss.out_count = ws->s_cnt.as<uint32_t>(); ss.out_pos = ws->s_pos.as<uint64_t>();
-        launch_select(ss, st);
-        ws->stats_mode = 2;
-        launch_band_check3(ws->s_lb.as<float>(), ws->s_cnt.as<uint32_t>(), ws->qt_step.as<float>(), ws->sbound.as<float>(),
-                           dot ? nullptr : ws->amax.as<float>(), dot ? nullptr : ix->rmax_bits.as<int>(),
-                           ws->qt_bad.as<uint32_t>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B, kk, kp,
-                           ws->flags.as<uint32_t>(), ws->c_wcnt.as<uint32_t>() + 1, ws->c_surv.as<uint32_t>(), st);
-        // exact PQ distances of the shortlist (oracle arithmetic), then the kk best of those
-        launch_pq_rescore(qsearch, ws->s_pos.as<uint64_t>(), B, kp, ix->codes.as<unsigned char>(),
-                          ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(), ix->part_off.as<uint64_t>(), nlist,
-                          ix->centroids.as<float>(), ix->cb_tiled.as<float>(), dim, ix->m, ix->dsub, ix->metric,
-                          ws->c_surv.as<uint32_t>(), ws->s_exact.as<float>(), st);
-        SelectArgs sb{};
-        sb.mode = 2; sb.dense = ws->s_exact.as<float>(); sb.cand_ids = ws->s_ids.as<uint64_t>();
-        sb.cand_pos = ws->s_pos.as<uint64_t>(); sb.ncols_q = ws->c_surv.as<uint32_t>();
-        sb.ncols = kp; sb.inner = kp; sb.row_stride = kp; sb.outer_stride = 0;
-        sb.B = B; sb.k = kk; sb.out_ids = pq_ids; sb.out_dist = pq_dist; sb.out_count = pq_cnt; sb.out_pos = pq_pos;
-        launch_select(sb, st);
-        }
-        // fix-up of the queries whose shortlist could not be proven (no tiles, hence no work, unless one is
-        // flagged): regroup them alone, exact scan, exact top-kk over their segments
-        const uint32_t *gate = ws->c_wcnt.as<uint32_t>() + 1;   // 0 = nothing flagged: every kernel below returns at once
-        ga.only = ws->flags.as<uint32_t>(); ga.gate = gate;
-        ga.rows_tile = SCAN_ROWS_TILE_MID;
-        launch_group(ga, st);
-        sc.rows_tile = SCAN_ROWS_TILE_MID; sc.gate = gate;
-        launch_scan2(sc, ix->dsub, ix->num_sms, st);
-        SelectArgs sf = sa;
-        sf.k = kk; sf.out_ids = pq_ids; sf.out_dist = pq_dist; sf.out_count = pq_cnt; sf.out_pos = pq_pos;
-        sf.only = ws->flags.as<uint32_t>(); sf.gate = gate;
-        launch_select(sf, st);
-        mark();
+// IvfScan::filter_cand: scan3 appends the rows under each query's threshold to its candidate list, the finalize kernel
+// re-scores them exactly into the PQ top-kk and flags the queries it cannot prove
+static void filter_candidates(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, ScanArgs &sc,
+                              TopkOut pq, bool prof, cudaStream_t st, const StageMarks &mark)
+{
+    const uint32_t B = p.B, cap = p.cand_cap;
+    const bool dot = ix->metric == LGPU_DOT;
+    const float mscale = ix->metric == LGPU_COSINE ? 0.5f : 1.0f;
+    ws->c_thr.ensure((size_t)B * 4); ws->c_slack.ensure((size_t)B * 4); ws->c_cnt.ensure((size_t)B * 4);
+    ws->c_rec.ensure((size_t)B * cap * sizeof(CandRec));
+    ws->c_key.ensure((size_t)B * cap * 4); ws->c_last.ensure((size_t)B * 4);
+    launch_cand_prepare(ws->qt_step.as<float>(), ws->sbound.as<float>(), dot ? nullptr : ws->amax.as<float>(),
+                        dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B,
+                        ws->c_slack.as<float>(), ws->c_thr.as<uint32_t>(), ws->c_cnt.as<uint32_t>(),
+                        ws->c_last.as<uint32_t>(), ws->c_key.as<uint32_t>(), cap, st);
+    sc.cand_key = ws->c_key.as<uint32_t>(); sc.cand_last = ws->c_last.as<uint32_t>();
+    sc.nprobes = p.nprobes; sc.topk = p.kk; sc.thr = ws->c_thr.as<uint32_t>(); sc.slack = ws->c_slack.as<float>();
+    sc.cand_cnt = ws->c_cnt.as<uint32_t>(); sc.cand = ws->c_rec.as<CandRec>(); sc.cand_cap = cap;
+    launch_scan3(sc, ix->num_sms, st);
+    mark(IVF_SCAN, st);
+    FinalizeArgs fa{};
+    fa.Q = qs; fa.cand = sc.cand; fa.cand_cnt = sc.cand_cnt; fa.cand_cap = cap; fa.cand_key = sc.cand_key; fa.thr = sc.thr;
+    fa.slack = sc.slack; fa.bad = ws->qt_bad.as<uint32_t>();
+    fa.codes = ix->codes.as<unsigned char>(); fa.code_base = ix->code_base.as<uint64_t>();
+    fa.part_npad = ix->part_npad.as<uint32_t>(); fa.part_off = ix->part_off.as<uint64_t>();
+    fa.row_ids = ix->row_ids.as<uint64_t>(); fa.centroids = ix->centroids.as<float>();
+    fa.cb_tiled = ix->cb_tiled.as<float>();
+    fa.B = B; fa.dim = ix->dim; fa.m = ix->m; fa.dsub = ix->dsub; fa.k = p.kk; fa.metric = ix->metric;
+    fa.out_ids = pq.ids; fa.out_dist = pq.dist; fa.out_count = pq.cnt; fa.out_pos = pq.pos;
+    fa.flags = ws->flags.as<uint32_t>();
+    ws->c_work.ensure((size_t)B * cap * 8); ws->c_wcnt.ensure(16); ws->c_surv.ensure((size_t)B * 4);
+    ws->c_exd.ensure((size_t)B * cap * 4); ws->c_exi.ensure((size_t)B * cap * 8); ws->c_exp.ensure((size_t)B * cap * 8);
+    fa.work = ws->c_work.as<uint2>(); fa.work_cnt = ws->c_wcnt.as<uint32_t>(); fa.surv_cnt = ws->c_surv.as<uint32_t>();
+    fa.ex_dist = ws->c_exd.as<float>(); fa.ex_id = ws->c_exi.as<uint64_t>(); fa.ex_pos = ws->c_exp.as<uint64_t>();
+    fa.num_sms = ix->num_sms;
+    if (prof) {
+        ws->c_stats.ensure(32);
+        LGPU_CUDA(cudaMemsetAsync(ws->c_stats.p, 0, 32, st));
+        fa.stats = ws->c_stats.as<unsigned long long>();
+        ws->stats_mode = 1;
+    }
+    launch_cand_finalize(fa, st);
+    sc.cand = nullptr;                      // (the fix-up pass is the exact kernel)
+}
+
+// IvfScan::filter_dense: scan3 writes a lower bound per row; the lb_short smallest are re-scored exactly (oracle
+// arithmetic) into the PQ top-kk, and the queries the band check cannot prove are flagged
+static void filter_dense(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, const ScanArgs &sc,
+                         RowFilter rf, TopkOut pq, cudaStream_t st, const StageMarks &mark)
+{
+    const uint32_t B = p.B, kp = p.lb_short;
+    const bool dot = ix->metric == LGPU_DOT;
+    const float mscale = ix->metric == LGPU_COSINE ? 0.5f : 1.0f;
+    launch_scan3(sc, ix->num_sms, st);
+    mark(IVF_SCAN, st);
+    launch_select(select_segments(ix, ws, p, kp, {ws->s_ids.as<uint64_t>(), ws->s_lb.as<float>(),
+                                  ws->s_cnt.as<uint32_t>(), ws->s_pos.as<uint64_t>()}, rf), st);
+    ws->stats_mode = 2;
+    launch_band_check3(ws->s_lb.as<float>(), ws->s_cnt.as<uint32_t>(), ws->qt_step.as<float>(), ws->sbound.as<float>(),
+                       dot ? nullptr : ws->amax.as<float>(), dot ? nullptr : ix->rmax_bits.as<int>(),
+                       ws->qt_bad.as<uint32_t>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B, p.kk, kp,
+                       ws->flags.as<uint32_t>(), ws->c_wcnt.as<uint32_t>() + 1, ws->c_surv.as<uint32_t>(), st);
+    launch_pq_rescore(qs, ws->s_pos.as<uint64_t>(), B, kp, ix->codes.as<unsigned char>(), ix->code_base.as<uint64_t>(),
+                      ix->part_npad.as<uint32_t>(), ix->part_off.as<uint64_t>(), ix->nlist, ix->centroids.as<float>(),
+                      ix->cb_tiled.as<float>(), ix->dim, ix->m, ix->dsub, ix->metric, ws->c_surv.as<uint32_t>(),
+                      ws->s_exact.as<float>(), st);
+    SelectArgs sb = select_cands(ws->s_exact.as<float>(), ws->s_ids.as<uint64_t>(), kp, B, p.kk, pq);
+    sb.cand_pos = ws->s_pos.as<uint64_t>(); sb.ncols_q = ws->c_surv.as<uint32_t>();
+    launch_select(sb, st);
+}
+
+// fix-up of the queries the filter scan could not prove (ws->flags): regroup them alone, exact scan, exact top-kk over
+// their segments.  Always issued: with nothing flagged the gate is 0 and every kernel returns at once.
+static void filter_fixup(lgpu_index *ix, Workspace *ws, const IvfPlan &p, GroupArgs ga, ScanArgs sc, RowFilter rf,
+                         TopkOut pq, cudaStream_t st)
+{
+    const uint32_t *gate = ws->c_wcnt.as<uint32_t>() + 1;
+    ga.only = ws->flags.as<uint32_t>(); ga.gate = gate;
+    ga.rows_tile = SCAN_ROWS_TILE_MID;
+    launch_group(ga, st);
+    sc.rows_tile = SCAN_ROWS_TILE_MID; sc.gate = gate;
+    launch_scan2(sc, ix->dsub, ix->num_sms, st);
+    SelectArgs sf = select_segments(ix, ws, p, p.kk, pq, rf);
+    sf.only = ws->flags.as<uint32_t>(); sf.gate = gate;
+    launch_select(sf, st);
+}
+
+// IvfScan::exact_pq / sq: the exact scan of every regrouped tile, then the PQ top-kk
+static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp, const float *qs,
+                      const GroupArgs &ga, RowFilter rf, const uint32_t *only, TopkOut pq, cudaStream_t st,
+                      const StageMarks &mark)
+{
+    if (p.scan == IvfScan::sq) {
+        SqScanArgs qa{};
+        qa.codes = ix->codes.as<uint8_t>(); qa.xx = ix->sq_xx.as<uint32_t>();
+        qa.qcodes = ws->sq_q.as<uint8_t>(); qa.qq = ws->sq_qq.as<uint32_t>(); qa.dim_pad = ix->dim_pad;
+        qa.total_tiles = ga.total_tiles; qa.tile_counter = ga.tile_counter; qa.tile_desc = ga.tile_desc;
+        qa.dist_out = ws->dist_out.as<float>();
+        launch_sq_scan(qa, 2 * ix->num_sms, st);
     } else {
-        if (sq) {
-            SqScanArgs qa{};
-            qa.codes = ix->codes.as<uint8_t>(); qa.xx = ix->sq_xx.as<uint32_t>();
-            qa.qcodes = ws->sq_q.as<uint8_t>(); qa.qq = ws->sq_qq.as<uint32_t>(); qa.dim_pad = ix->dim_pad;
-            qa.total_tiles = ga.total_tiles; qa.tile_counter = ga.tile_counter; qa.tile_desc = ga.tile_desc;
-            qa.dist_out = ws->dist_out.as<float>();
-            launch_sq_scan(qa, 2 * ix->num_sms, st);
-        } else {
-            launch_scan2(sc, ix->dsub, ix->num_sms, st);
-        }
-        mark();
-        if (!d_ids) { mark(); mark(); return; }     // debug: distances only
-        sa.has_lower = sp.has_lower; sa.has_upper = sp.has_upper; sa.lower = sp.lower; sa.upper = sp.upper;
-        sa.k = kk; sa.out_ids = pq_ids; sa.out_dist = pq_dist; sa.out_count = pq_cnt; sa.out_pos = pq_pos;
-        launch_select(sa, st);
-        mark();
+        launch_scan2(scan_args(ix, ws, qs, ga), ix->dsub, ix->num_sms, st);
     }
-    if (sp.refine_factor == 0) { mark(); return; }
-    // ---- refine (query.rs:1302-1332): exact distance of the k*rf candidates, re-sort ----
-    launch_pair_distance(d_q, ix->vectors.as<float>(), ws->t_pos.as<uint64_t>(), B, kk, dim, ix->metric,
+    mark(IVF_SCAN, st);
+    SelectArgs sa = select_segments(ix, ws, p, p.kk, pq, rf);
+    sa.only = only;
+    with_range(sa, sp);
+    launch_select(sa, st);
+    mark(IVF_TOPK, st);
+}
+
+// refine (query.rs:1302-1332): exact distance of the k * refine_factor candidates (ws->t_*), re-sort into `out`
+static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *d_q, TopkOut out,
+                       const uint32_t *only, cudaStream_t st)
+{
+    launch_pair_distance(d_q, ix->vectors.as<float>(), ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric,
                          ws->t_exact.as<float>(), st);
-    SelectArgs sr{};
-    sr.mode = 2; sr.dense = ws->t_exact.as<float>(); sr.cand_ids = ws->t_ids.as<uint64_t>();
-    sr.ncols = kk; sr.inner = kk; sr.row_stride = kk; sr.outer_stride = 0;
-    sr.B = B; sr.k = sp.k; sr.out_ids = d_ids; sr.out_dist = d_dist; sr.out_count = d_cnt;
+    SelectArgs sr = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), p.kk, p.B, p.k, out);
     sr.only = only;
     launch_select(sr, st);
-    mark();
+}
+
+// one sub-batch of an IVF_PQ / IVF_SQ search, everything device-side on `st` (and `front`, joined).  only (device,
+// [B]): redo just the flagged queries (maximum_nprobes widening) -- exact kernels, the other queries' outputs are left
+// untouched.
+void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
+                   const lgpu_search_params &sp, uint32_t nprobes, TopkOut out, bool prof, RowFilter rf,
+                   const uint32_t *only = nullptr)
+{
+    const IvfPlan p = ivf_plan(ix, B, nprobes, sp, rf.bits != nullptr, only != nullptr, scan_modes());
+    const StageMarks mark{ws, prof};
+    mark(IVF_START, st);
+    ws->stats_mode = 0;
+    const float *qs = ivf_queries(ix, ws, st, d_q, B);
+    const cudaStream_t cs = p.filter() ? fork_front(ix, ws, st, B) : st;   // the coarse step's and the regroup's
+    ivf_coarse(ix, ws, p, qs, cs, st, mark);
+    if (p.scan == IvfScan::sq) {
+        ws->sq_q.ensure((size_t)B * ix->dim_pad); ws->sq_qq.ensure((size_t)B * 4);
+        launch_sq_encode(qs, B, ix->dim, ix->dim_pad, ix->sq_lo, ix->sq_hi, ws->sq_q.as<uint8_t>(),
+                         ws->sq_qq.as<uint32_t>(), st);
+    }
+    mark(IVF_PROBES, cs);
+    if (p.scan == IvfScan::small) {
+        ivf_small(ix, ws, p, sp, qs, rf, out, st, mark);
+    } else {
+        const GroupArgs ga = ivf_regroup(ix, ws, p, only, cs);
+        mark(IVF_REGROUP, cs);
+        const TopkOut pq = pq_out(ws, p, out);
+        if (p.filter()) {
+            LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
+            ScanArgs sc = scan_args(ix, ws, qs, ga);
+            filter_terms(ix, ws, p, qs, sc, st);
+            if (p.scan == IvfScan::filter_cand) filter_candidates(ix, ws, p, qs, sc, pq, prof, st, mark);
+            else filter_dense(ix, ws, p, qs, sc, rf, pq, st, mark);
+            filter_fixup(ix, ws, p, ga, sc, rf, pq, st);
+            mark(IVF_TOPK, st);
+        } else {
+            ivf_exact(ix, ws, p, sp, qs, ga, rf, only, pq, st, mark);
+        }
+    }
+    if (!p.refine) return;
+    ivf_refine(ix, ws, p, d_q, out, only, st);
+    mark(IVF_REFINE, st);
 }
 
 uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
@@ -1088,28 +1153,32 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
     const uint32_t np_widest = rf.bits ? std::max(nprobes, std::min<uint32_t>(sp.max_nprobes, ix->nlist)) : nprobes;
     const uint32_t bs = ivf_sub_batch_size(ix, B, np_widest);
     const bool prof = profiling_enabled();
+    const TopkOut out{d_ids, d_dist, d_cnt};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
-        ivf_sub_batch(ix, ws, st, d_q + (size_t)q0 * ix->dim, b, sp, nprobes, d_ids + (size_t)q0 * sp.k,
-                      d_dist + (size_t)q0 * sp.k, d_cnt + q0, prof && q0 == 0, nullptr, rf);
+        const float *q = d_q + (size_t)q0 * ix->dim;
+        ivf_sub_batch(ix, ws, st, q, b, sp, nprobes, out.at(q0, sp.k), prof && q0 == 0, rf);
         // maximum_nprobes (query.rs:1250-1275): under a prefilter, the queries that found fewer than k rows in their
         // minimum_nprobes partitions are searched again over their maximum_nprobes nearest (no work if none is)
         const uint32_t np_max = std::min<uint32_t>(sp.max_nprobes, ix->nlist);
         if (rf.bits && np_max > nprobes) {
             LGPU_REQUIRE(np_max <= SELECT_KMAX || np_max >= ix->nlist, "maximum_nprobes above 2048 is not supported");
             ws->widen.ensure((size_t)b * 4);
-            launch_count_below(d_cnt + q0, b, sp.k, ws->widen.as<uint32_t>(), st);
-            ivf_sub_batch(ix, ws, st, d_q + (size_t)q0 * ix->dim, b, sp, np_max, d_ids + (size_t)q0 * sp.k,
-                          d_dist + (size_t)q0 * sp.k, d_cnt + q0, false, nullptr, rf, ws->widen.as<uint32_t>());
+            launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
+            ivf_sub_batch(ix, ws, st, q, b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
         }
     }
     if (prof) {
         LGPU_CUDA(cudaStreamSynchronize(st));
-        for (int i = 0; i < 6; i++) cudaEventElapsedTime(&g_stage_ms[i], ws->ev[i], ws->ev[i + 1]);
-        cudaEventElapsedTime(&g_stage_ms[6], ws->ev[0], ws->ev[6]);
+        cudaEvent_t end[7];
+        for (int i = 0; i < 7; i++) end[i] = i == 0 || (ws->stages_marked >> i & 1) ? ws->ev[i] : end[i - 1];
+        for (int i = 0; i < 6; i++) cudaEventElapsedTime(&g_stage_ms[i], end[i], end[i + 1]);
+        cudaEventElapsedTime(&g_stage_ms[6], end[0], end[6]);
+        // the regroup counts the rows it hands to the scan (the small path has no regroup and counts none)
         unsigned long long rows = 0;
-        LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
+        if (ws->stages_marked >> IVF_REGROUP & 1)
+            LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
         g_scanned_bytes = (uint64_t)rows * (ix->is_sq ? ix->dim : ix->m);   // code bytes per row
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
         if (ws->stats_mode == 1) LGPU_CUDA(cudaMemcpy(g_filter_stats, ws->c_stats.p, 32, cudaMemcpyDeviceToHost));
@@ -1139,6 +1208,7 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
     }
     size_t per_q = std::max<size_t>(ld * 4, 4);
     uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(workspace_budget() / per_q, B));
+    const TopkOut out{d_ids, d_dist, d_cnt};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
@@ -1157,19 +1227,18 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
             if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
                 tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p,
                                     fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
-                                    fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k,
-                                    d_ids + (size_t)q0 * sp.k, d_dist + (size_t)q0 * sp.k, d_cnt + q0,
+                                    fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, out.at(q0, sp.k),
                                     ws->D.as<float>(), ld);
             else
                 tc_topk_l2(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p, fl->vec_n2.as<float>(),
                            fl->vec_max, fl->vec_err, N, fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp,
-                           d_ids + (size_t)q0 * sp.k, d_dist + (size_t)q0 * sp.k, d_cnt + q0, ws->D.as<float>(), ld);
+                           out.at(q0, sp.k), ws->D.as<float>(), ld);
             continue;
         }
         launch_dist_matrix(q, fl->vectors.as<float>(), b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
                            xn, fl->ysqrt.as<float>(), ws->D.as<float>(), ld, st);
-        select_dense(ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf, q0, d_ids,
-                     d_dist, d_cnt, st);
+        select_dense(ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
+                     out.at(q0, sp.k), st);
     }
 }
 
@@ -1202,8 +1271,7 @@ static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
 // overflowed queries runs in chunks of `bf` queries over a [bf][N] matrix: one launch lists each chunk's flagged
 // queries, and each chunk's two launches return at once when its list is empty.
 static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
-                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, uint64_t *out_ids, float *out_dist,
-                          uint32_t *out_cnt)
+                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, TopkOut out)
 {
     const uint64_t N = bx->nrows, ns = bx->nsample, lds = (ns + 3) & ~3ull, ld = (N + 3) & ~3ull;
     const uint32_t nbp = bx->nbytes_pad;
@@ -1211,10 +1279,8 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     // 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest (an upper bound of the true k-th)
     launch_ham_gemm(Q, bx->sample.p, bx->sample_pop.as<uint32_t>(), qpop, B, ns, nbp, ws->h_sample.as<float>(), lds,
                     bx->num_sms, st);
-    SelectArgs sa{};
-    sa.mode = 1; sa.dense = ws->h_sample.as<float>(); sa.ncols = ns; sa.row_stride = lds; sa.B = B; sa.k = k;
-    sa.out_ids = ws->sbound.as<uint64_t>(); sa.out_dist = ws->t_dist.as<float>(); sa.out_count = ws->t_cnt.as<uint32_t>();
-    launch_select(sa, st);
+    launch_select(select_rows(ws->h_sample.as<float>(), ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
+                                                                        ws->t_cnt.as<uint32_t>()}), st);
     launch_ham_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), B, k, ws->probe_A.as<float>(), st);
     // 2. full pass: every row with d <= tau_q is appended as (position, id, distance); the distance is final
     LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
@@ -1224,10 +1290,8 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
     // 3. top-k by (distance, id) of each list (an overflowed list is complete up to cap; its query is redone below)
-    SelectArgs sb{};
-    sb.mode = 2; sb.dense = ws->t_exact.as<float>(); sb.cand_ids = ws->t_ids.as<uint64_t>();
-    sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0; sb.ncols_q = ws->amax.as<uint32_t>();
-    sb.B = B; sb.k = k; sb.out_ids = out_ids; sb.out_dist = out_dist; sb.out_count = out_cnt;
+    SelectArgs sb = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), cap, B, k, out);
+    sb.ncols_q = ws->amax.as<uint32_t>();
     launch_select(sb, st);
     // 4. dense fix-up of the overflowed queries only
     launch_ham_flag_list(ws->flags.as<uint32_t>(), B, bf, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
@@ -1235,10 +1299,8 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         const uint32_t b = std::min(bf, B - q0);
         launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld, bx->num_sms, st,
                          ws->h_list.as<uint32_t>() + q0, ws->h_cnt.as<uint32_t>() + c);
-        SelectArgs sc{};
-        sc.mode = 1; sc.dense = ws->D.as<float>(); sc.ncols = N; sc.row_stride = ld; sc.col_ids = col_ids;
-        sc.B = b; sc.k = k; sc.out_ids = out_ids + (size_t)q0 * k; sc.out_dist = out_dist + (size_t)q0 * k;
-        sc.out_count = out_cnt + q0; sc.only = ws->flags.as<uint32_t>() + q0; sc.gate = ws->h_cnt.as<uint32_t>() + c;
+        SelectArgs sc = select_rows(ws->D.as<float>(), N, ld, b, k, out.at(q0, k));
+        sc.col_ids = col_ids; sc.only = ws->flags.as<uint32_t>() + q0; sc.gate = ws->h_cnt.as<uint32_t>() + c;
         launch_select(sc, st);
     }
 }
@@ -1251,6 +1313,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     const uint64_t N = bx->nrows, ld = (N + 3) & ~3ull;
     const uint32_t nbp = bx->nbytes_pad, k = sp.k;
     const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));
     ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
@@ -1280,8 +1343,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         for (uint32_t q0 = 0; q0 < B; q0 += bs) {
             const uint32_t b = std::min(bs, B - q0);
             if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, ws->hq_pop.as<uint32_t>() + q0, b, k, cap, bf,
-                          d_ids + (size_t)q0 * k, d_dist + (size_t)q0 * k, d_cnt + q0);
+            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, ws->hq_pop.as<uint32_t>() + q0, b, k, cap, bf, out.at(q0, k));
             if (prof) {             // [0] list appends, [2] queries redone densely (over every sub-batch)
                 std::vector<uint32_t> cnt(b), fl(b);
                 LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->amax.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
@@ -1302,7 +1364,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
             else
                 launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld,
                                  bx->num_sms, st);
-            select_dense(ws->D.as<float>(), N, ld, col_ids, b, sp, rf, q0, d_ids, d_dist, d_cnt, st);
+            select_dense(ws->D.as<float>(), N, ld, col_ids, b, sp, rf, out.at(q0, k), st);
         }
     }
     if (prof) {                     // [1] distances computed on the tensor cores, [3] queries
@@ -1379,6 +1441,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
 {
     const uint64_t N = mv->nrows, ld = (N + 3) & ~3ull;
     const uint32_t dim = mv->dim, k = sp.k, Tq = h_qoff[B];
+    const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));
     ws->mv_qoff.ensure((size_t)(B + 1) * 4);
@@ -1419,10 +1482,9 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
                                mv->num_sms, st);
             launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ld, ws->mv_qoff.as<uint32_t>(), qa, qb, va, N,
                                  ws->mv_A.as<float>(), ld, mv->num_sms, st);
-            SelectArgs sa{};                                   // the k-th smallest approximate distance of each query
-            sa.mode = 1; sa.dense = ws->mv_A.as<float>(); sa.ncols = N; sa.row_stride = ld; sa.B = b; sa.k = k;
-            sa.out_ids = ws->mv_ki.as<uint64_t>(); sa.out_dist = ws->mv_kd.as<float>(); sa.out_count = ws->mv_kc.as<uint32_t>();
-            launch_select(sa, st);
+            // the k-th smallest approximate distance of each query
+            launch_select(select_rows(ws->mv_A.as<float>(), N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
+                                                                          ws->mv_kc.as<uint32_t>()}), st);
             launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
                                 ws->mv_thr.as<float>(), st);
             LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
@@ -1434,20 +1496,13 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
                               mv->ysqrt.as<float>(), mv->offsets.as<uint64_t>(),
                               mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, dim, b, ws->mv_cand.as<uint32_t>(),
                               ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), st);
-            SelectArgs sb{};
-            sb.mode = 2; sb.dense = ws->mv_ex.as<float>(); sb.cand_ids = ws->mv_exid.as<uint64_t>();
-            sb.ncols = cap; sb.inner = cap; sb.row_stride = cap; sb.outer_stride = 0;
-            sb.B = b; sb.k = k; sb.out_ids = d_ids + (size_t)qa * k; sb.out_dist = d_dist + (size_t)qa * k;
-            sb.out_count = d_cnt + qa;
-            launch_select(sb, st);
+            launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
             // exact fix-up of the flagged queries (A is free again: it holds their exact distances)
             mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->mv_A.as<float>(), ld, ws->mv_flags.as<uint32_t>(),
                            ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>());
-            SelectArgs sc{};
-            sc.mode = 1; sc.dense = ws->mv_A.as<float>(); sc.ncols = N; sc.row_stride = ld;
+            SelectArgs sc = select_rows(ws->mv_A.as<float>(), N, ld, b, k, out.at(qa, k));
             sc.col_ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
-            sc.B = b; sc.k = k; sc.out_ids = d_ids + (size_t)qa * k; sc.out_dist = d_dist + (size_t)qa * k;
-            sc.out_count = d_cnt + qa; sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = ws->mv_gate.as<uint32_t>();
+            sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = ws->mv_gate.as<uint32_t>();
             launch_select(sc, st);
             if (prof) {             // [0] rows admitted, [1] rows re-scored exactly, [2] queries redone densely
                 std::vector<uint32_t> cnt(b), fl(b);
@@ -1468,8 +1523,8 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
             mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld);
-            select_dense(ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf, qa,
-                         d_ids, d_dist, d_cnt, st);
+            select_dense(ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
+                         out.at(qa, k), st);
         }
     }
     if (prof) {                     // exact path: [1] rows scored exactly; both: [3] queries
@@ -2194,10 +2249,9 @@ int lgpu_merge_topk_device(int device, uint32_t nlists, uint32_t B, uint32_t k, 
         LGPU_REQUIRE(B == 0 || (d_ids && d_dist && d_out_ids && d_out_dist && d_out_count), "null buffer");
         if (B == 0) return;
         require_device(device);
-        SelectArgs sb{};
-        sb.mode = 2; sb.dense = d_dist; sb.cand_ids = d_ids;
-        sb.ncols = (uint64_t)nlists * k; sb.inner = k; sb.row_stride = k; sb.outer_stride = (uint64_t)B * k;
-        sb.B = B; sb.k = k; sb.out_ids = d_out_ids; sb.out_dist = d_out_dist; sb.out_count = d_out_count;
+        // list l of query q at l * B * k + q * k
+        SelectArgs sb = select_cands(d_dist, d_ids, k, B, k, {d_out_ids, d_out_dist, d_out_count});
+        sb.ncols = (uint64_t)nlists * k; sb.outer_stride = (uint64_t)B * k;
         launch_select(sb, (cudaStream_t)cuda_stream);
     });
 }
@@ -2547,10 +2601,9 @@ static void sharded_search_device(lgpu_index *ix, lgpu_comm *c, Workspace *ws, c
     if (prof) cudaEventRecord(c->ev[0], st);
     LGPU_NCCL(nccl_api().AllGather(c->send.p, c->recv.p, n * sizeof(TopkRecord), ncclUint8, c->comm, st));
     if (prof) cudaEventRecord(c->ev[1], st);
-    SelectArgs sb{};
-    sb.mode = 2; sb.cand_rec = c->recv.as<TopkRecord>();
-    sb.ncols = (uint64_t)c->world * sp.k; sb.inner = sp.k; sb.row_stride = sp.k; sb.outer_stride = (uint64_t)B * sp.k;
-    sb.B = B; sb.k = sp.k; sb.out_ids = d_ids; sb.out_dist = d_dist; sb.out_count = d_cnt;
+    // rank r's list of query q at r * B * k + q * k
+    SelectArgs sb = select_cands(nullptr, nullptr, sp.k, B, sp.k, {d_ids, d_dist, d_cnt});
+    sb.cand_rec = c->recv.as<TopkRecord>(); sb.ncols = (uint64_t)c->world * sp.k; sb.outer_stride = (uint64_t)B * sp.k;
     launch_select(sb, st);
     if (prof) {
         cudaEventRecord(c->ev[2], st);
@@ -2616,22 +2669,13 @@ int lgpu_debug_coarse(lgpu_index *ixh, const float *queries, uint32_t B, uint32_
         Workspace *ws = lease.ws; cudaStream_t st = lease.st;
         ws->q.ensure((size_t)B * ix->dim * 4);
         LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * ix->dim * 4, cudaMemcpyHostToDevice, st));
-        const float *qs = ws->q.as<float>();
-        if (ix->metric == LGPU_COSINE) {
-            ws->qn.ensure((size_t)B * ix->dim * 4);
-            launch_normalize(qs, B, ix->dim, ws->qn.as<float>(), st);
-            qs = ws->qn.as<float>();
-        }
-        ws->D.ensure((size_t)B * ix->nlist * 4);
-        ws->probes.ensure((size_t)B * nprobes * 8); ws->probe_dist.ensure((size_t)B * nprobes * 4);
-        ws->probe_cnt.ensure((size_t)B * 4);
-        launch_dist_matrix(qs, ix->centroids.as<float>(), B, ix->nlist, ix->dim, ix->metric == LGPU_DOT ? 1 : 0,
-                           nullptr, nullptr, ws->D.as<float>(), ix->nlist, st);
-        SelectArgs sa{};
-        sa.mode = 1; sa.dense = ws->D.as<float>(); sa.ncols = ix->nlist; sa.row_stride = ix->nlist;
-        sa.B = B; sa.k = nprobes; sa.out_ids = ws->probes.as<uint64_t>(); sa.out_dist = ws->probe_dist.as<float>();
-        sa.out_count = ws->probe_cnt.as<uint32_t>();
-        launch_select(sa, st);
+        lgpu_search_params sp{};
+        sp.k = 1; sp.nprobes = nprobes;
+        ScanModes modes = scan_modes();
+        modes.exact = true;                               // (no filter scan: no query tables)
+        IvfPlan p = ivf_plan(ix.h, B, nprobes, sp, false, false, modes);
+        p.coarse = Coarse::exact;                         // the exact kernels' probes and distances
+        ivf_coarse(ix.h, ws, p, ivf_queries(ix.h, ws, st, ws->q.as<float>(), B), st, st, StageMarks{ws, false});
         std::vector<uint64_t> tmp((size_t)B * nprobes);
         LGPU_CUDA(cudaMemcpyAsync(tmp.data(), ws->probes.p, tmp.size() * 8, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaMemcpyAsync(out_dists, ws->probe_dist.p, tmp.size() * 4, cudaMemcpyDeviceToHost, st));
@@ -2674,10 +2718,18 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
         Workspace *ws = lease.ws; cudaStream_t st = lease.st;
         ws->q.ensure((size_t)ix->dim * 4);
         LGPU_CUDA(cudaMemcpyAsync(ws->q.p, query, (size_t)ix->dim * 4, cudaMemcpyHostToDevice, st));
-        uint64_t forced = part;
+        // the one probe slot is `part`, regrouped for the exact scan (scan2.cu)
         lgpu_search_params sp{};
         sp.k = 1; sp.nprobes = 1;
-        ivf_sub_batch(ix.h, ws, st, ws->q.as<float>(), 1, sp, 1, nullptr, nullptr, nullptr, false, &forced);
+        ScanModes modes = scan_modes();
+        modes.exact = true; modes.small_slots = 0;
+        const IvfPlan p = ivf_plan(ix.h, 1, 1, sp, false, false, modes);
+        const float *qs = ivf_queries(ix.h, ws, st, ws->q.as<float>(), 1);
+        const uint64_t forced = part;
+        ws->probes.ensure(8);
+        LGPU_CUDA(cudaMemcpyAsync(ws->probes.p, &forced, 8, cudaMemcpyHostToDevice, st));
+        const GroupArgs ga = ivf_regroup(ix.h, ws, p, nullptr, st);
+        launch_scan2(scan_args(ix.h, ws, qs, ga), ix->dsub, ix->num_sms, st);
         uint32_t n = ix->h_part_n[part];
         if (n) LGPU_CUDA(cudaMemcpyAsync(out, ws->dist_out.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaStreamSynchronize(st));
@@ -2700,11 +2752,42 @@ int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, 
         LGPU_CUDA(cudaMemcpyAsync(ws->q.p, queries, (size_t)B * ix->dim * 4, cudaMemcpyHostToDevice, st));
         lgpu_search_params sp{};
         sp.k = 10; sp.nprobes = nprobes;
-        FilterDebug dbg{out_L, ld, out_parts, out_W, out_E, out_bad};
-        ivf_sub_batch(ix.h, ws, st, ws->q.as<float>(), B, sp, nprobes, nullptr, nullptr, nullptr, false, nullptr,
-                      RowFilter(), nullptr, &dbg);
+        ScanModes modes = scan_modes();
+        modes.small_slots = 0;
+        const IvfPlan p = ivf_plan(ix.h, B, nprobes, sp, false, false, modes);
+        LGPU_REQUIRE(p.filter(), "this index or configuration does not use the filter scan");
+        // the search's front, then the dense mode's scan: one lower bound L per row
+        const float *qs = ivf_queries(ix.h, ws, st, ws->q.as<float>(), B);
+        const cudaStream_t cs = fork_front(ix.h, ws, st, B);
+        ivf_coarse(ix.h, ws, p, qs, cs, st, StageMarks{ws, false});
+        const GroupArgs ga = ivf_regroup(ix.h, ws, p, nullptr, cs);
+        LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
+        ScanArgs sc = scan_args(ix.h, ws, qs, ga);
+        filter_terms(ix.h, ws, p, qs, sc, st);
+        launch_scan3(sc, ix->num_sms, st);
+        // W, E of every query (the band the consumers use) and the scan's own L, per probe slot
+        const bool dot = ix->metric == LGPU_DOT;
+        const uint32_t slots = p.slots, nlist = ix->nlist;
+        const size_t nL = (size_t)B * ix->pad_prefix[p.np_eff];
+        ws->s_exact.ensure((size_t)B * 8);
+        float *dW = ws->s_exact.as<float>(), *dE = dW + B;
+        launch_scan_band(ws->qt_step.as<float>(), ws->sbound.as<float>(), dot ? nullptr : ws->amax.as<float>(),
+                         dot ? nullptr : ix->rmax_bits.as<int>(), ws->qn2.as<float>(), ix->cb2, ix->m, dot, B, dW, dE, st);
+        std::vector<uint64_t> probes(slots), seg(slots);
+        std::vector<float> L(nL);
+        LGPU_CUDA(cudaMemcpyAsync(probes.data(), ws->probes.p, (size_t)slots * 8, cudaMemcpyDeviceToHost, st));
+        LGPU_CUDA(cudaMemcpyAsync(seg.data(), ga.seg_off, (size_t)slots * 8, cudaMemcpyDeviceToHost, st));
+        if (nL) LGPU_CUDA(cudaMemcpyAsync(L.data(), ws->dist_out.p, nL * 4, cudaMemcpyDeviceToHost, st));
+        LGPU_CUDA(cudaMemcpyAsync(out_W, dW, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+        LGPU_CUDA(cudaMemcpyAsync(out_E, dE, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+        LGPU_CUDA(cudaMemcpyAsync(out_bad, ws->qt_bad.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaStreamSynchronize(st));
-        LGPU_REQUIRE(dbg.ran, "this index or configuration does not use the filter scan");
+        for (uint32_t sl = 0; sl < slots; sl++) {
+            const uint64_t pr = probes[sl];
+            out_parts[sl] = pr < nlist ? (uint32_t)pr : UINT32_MAX;
+            const uint64_t n = pr < nlist ? std::min<uint64_t>(ix->h_part_n[pr], ld) : 0;
+            if (n) memcpy(out_L + (size_t)sl * ld, L.data() + seg[sl], n * 4);
+        }
     });
 }
 
@@ -2736,10 +2819,8 @@ int lgpu_ivf_assign(const float *centroids, uint32_t nlist, uint32_t dim, int me
             // the search path's own coarse step (find_partitions with nprobes = 1)
             launch_dist_matrix(q, cent.as<float>(), b, nlist, dim, metric == LGPU_DOT ? 1 : 0, nullptr, nullptr,
                                D.as<float>(), ld, st);
-            SelectArgs sa{};
-            sa.mode = 1; sa.dense = D.as<float>(); sa.ncols = nlist; sa.row_stride = ld; sa.B = b; sa.k = 1;
-            sa.out_ids = ids.as<uint64_t>(); sa.out_dist = dist.as<float>(); sa.out_count = cnt.as<uint32_t>();
-            launch_select(sa, st);
+            launch_select(select_rows(D.as<float>(), nlist, ld, b, 1, {ids.as<uint64_t>(), dist.as<float>(),
+                                      cnt.as<uint32_t>()}), st);
             LGPU_CUDA(cudaMemcpyAsync(h_ids.data(), ids.p, (size_t)b * 8, cudaMemcpyDeviceToHost, st));
             LGPU_CUDA(cudaStreamSynchronize(st));
             for (uint32_t i = 0; i < b; i++) {
@@ -2769,9 +2850,7 @@ static void assign_nearest(const float *d_x, uint64_t n, uint32_t dim, const flo
     for (uint64_t r0 = 0; r0 < n; r0 += CH) {
         const uint32_t b = (uint32_t)std::min<uint64_t>(CH, n - r0);
         const float *q = d_x + r0 * dim;
-        SelectArgs sa{};
-        sa.mode = 1; sa.dense = D.as<float>(); sa.ncols = k; sa.row_stride = ld; sa.B = b; sa.k = 1;
-        sa.out_ids = d_ids + r0; sa.out_dist = d_dist + r0; sa.out_count = cnt.as<uint32_t>();
+        SelectArgs sa = select_rows(D.as<float>(), k, ld, b, 1, {d_ids + r0, d_dist + r0, cnt.as<uint32_t>()});
         if (tc) {
             launch_to_bf16(q, b, dim, xb.p, xn2.as<float>(), st, xerr.as<float>());
             launch_gemm_dist(xb.p, cb.p, cn2.as<float>(), b, k, dim, D.as<float>(), ld, num_sms, st);
