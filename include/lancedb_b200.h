@@ -203,6 +203,41 @@ typedef struct {
 } lgpu_ivf_sq_desc;
 int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *desc, lgpu_index **out);
 
+/* ---- IVF_RQ (lance `IvfRq`, RaBitQ with num_bits = 1; rust/lancedb/src/index/vector.rs:321-369): the same IVF
+ * partitions, each row stored as one sign bit per dimension of its rotated residual plus two f32 factors.  With P the
+ * f32 [dim][dim] orthogonal rotation and o = P (x - c_p) (f64, at build time): bit i = [o_i > 0] (bit i & 7 of byte
+ * i >> 3, padding bits 0), add = (float) sum o_i^2, scale = (float) (-2 sum o_i^2 / sum |o_i|), both 0 when o = 0.
+ * Search (every operation rounded to f32 on its own, no FMA): rq_i = dot(P row i, q) and rc_{p,i} = dot(P row i, c_p)
+ * in lance's lane order (q normalised first for cosine); per probe slot q'_i = rq_i - rc_{p,i}, lo = min q',
+ * delta = (max q' - lo) / 15, u_i = min(15, trunc((q'_i - lo) / delta + 0.5)) (0 when delta is 0), S = sum u_i,
+ * qq = l2(rq, rc_p); per row ip = sum_i b_i u_i (exact), pc = popcount(b),
+ *     y = delta * (float)(2 ip - S) + lo * (float)(2 pc - dim),   est = (add + qq) + scale * y
+ * and _distance = est (l2) or 0.5 est (cosine, the scale of the exact cosine distance refine_factor reports).  The
+ * estimate may be negative.  A slot with a NaN component in q' or a non-finite delta contributes no rows, and a NaN
+ * estimate is never returned.  dot and num_bits != 1 are not supported (LGPU_INVALID_INPUT).  The handle is an
+ * ordinary lgpu_index: lgpu_search, _filtered, _device, _async and _coalesced serve it with the IVF_PQ semantics of k,
+ * nprobes, maximum_nprobes, prefilter, distance_range (on the estimate, before refine), refine_factor and timeout_ms.
+ * lgpu_search_sharded*, lgpu_debug_filter_bounds and lgpu_debug_partition_distances reject it. */
+#define LGPU_RQ_MAX_DIM 4096      /* P at most 64 MB; every integer above stays exact in f32 */
+typedef struct {
+    uint32_t abi_version;         /* LGPU_ABI_VERSION */
+    uint32_t dim;                 /* 1 .. LGPU_RQ_MAX_DIM */
+    uint32_t nlist;
+    int32_t  metric;              /* LGPU_L2 or LGPU_COSINE */
+    int32_t  device;
+    uint32_t num_bits;            /* 1 */
+    uint64_t nrows;
+    const float    *centroids;    /* [nlist][dim] */
+    const float    *rotation;     /* [dim][dim] P, row-major */
+    const uint64_t *part_offsets; /* [nlist+1] */
+    const uint8_t  *codes;        /* [nrows][ceil(dim / 8)] sign bits in partition order */
+    const float    *add_factors;  /* [nrows] */
+    const float    *scale_factors;/* [nrows] */
+    const uint64_t *row_ids;      /* [nrows] */
+    const float    *vectors;      /* optional [nrows][dim] raw vectors (refine_factor); NULL if absent */
+} lgpu_ivf_rq_desc;
+int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *desc, lgpu_index **out);
+
 /* ---- partition-sharded search across GPUs (SURVEY.md 8e; the reference is single-process, so there is no
  * reference interface to replace -- this is what north_star adds for an index larger than one GPU's HBM).
  * One process (or thread) per GPU.  Centroids and codebook are replicated, every partition's codes and row ids
@@ -358,6 +393,13 @@ int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint
  * dim <= 65536, B x N < 2^32) */
 int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x_codes, uint64_t N, uint32_t dim,
                             int device, uint32_t *out);
+/* the IVF_RQ planes and scan kernels alone, every query one probe slot over one partition of N rows: q_res [B][dim] the
+ * rotated residuals q', codes [N][ceil(dim / 8)], add / scale [N]; out_est [B][N] the reported estimates (NaN where the
+ * slot has no rows), out_ip [B][N] the exact ip = sum_i b_i u_i (either may be NULL; host buffers; dim <= 4096,
+ * B x N < 2^32) */
+int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes, const float *add_factors,
+                            const float *scale_factors, uint64_t N, uint32_t dim, int metric, int device,
+                            float *out_est, uint32_t *out_ip);
 /* the multivector tensor-core score alone: out[i][r] = the largest fp16(q_i / |q_i|) . fp16(v / |v|) (f32 accumulation)
  * over row r's vectors v, NaN for an empty row (host buffers: queries [nqv][dim], values [offsets[nrows]][dim],
  * out [nqv][nrows] f32); dim must be a multiple of 8 */

@@ -37,6 +37,7 @@ EXPORTS = [
     "lgpu_multivec_open", "lgpu_multivec_close", "lgpu_multivec_search", "lgpu_multivec_search_filtered",
     "lgpu_multivec_search_device", "lgpu_debug_maxsim_gemm",
     "lgpu_ivf_sq_open", "lgpu_debug_sq_distances",
+    "lgpu_ivf_rq_open", "lgpu_debug_rq_distances",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -60,6 +61,16 @@ class SqDesc(C.Structure):
         ("device", C.c_int32), ("reserved", C.c_uint32), ("nrows", C.c_uint64), ("lo", C.c_double), ("hi", C.c_double),
         ("centroids", C.c_void_p), ("part_offsets", C.c_void_p), ("codes", C.c_void_p), ("row_ids", C.c_void_p),
         ("vectors", C.c_void_p),
+    ]
+
+
+class RqDesc(C.Structure):
+    """lgpu_ivf_rq_desc"""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("dim", C.c_uint32), ("nlist", C.c_uint32), ("metric", C.c_int32),
+        ("device", C.c_int32), ("num_bits", C.c_uint32), ("nrows", C.c_uint64),
+        ("centroids", C.c_void_p), ("rotation", C.c_void_p), ("part_offsets", C.c_void_p), ("codes", C.c_void_p),
+        ("add_factors", C.c_void_p), ("scale_factors", C.c_void_p), ("row_ids", C.c_void_p), ("vectors", C.c_void_p),
     ]
 
 
@@ -148,6 +159,8 @@ def load():
     lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_sq_open.argtypes = [C.POINTER(SqDesc), C.POINTER(vp)]
     lib.lgpu_debug_sq_distances.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
+    lib.lgpu_ivf_rq_open.argtypes = [C.POINTER(RqDesc), C.POINTER(vp)]
+    lib.lgpu_debug_rq_distances.argtypes = [vp, u32, vp, vp, vp, C.c_uint64, u32, i32, i32, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -350,6 +363,32 @@ class GpuIvfSq(GpuIvfPq):
                       _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]))
         h = C.c_void_p()
         check(lib.lgpu_ivf_sq_open(C.byref(desc), C.byref(h)))
+        self._h = h
+        self.has_vectors = vec is not None
+
+
+class GpuIvfRq(GpuIvfPq):
+    """An IVF_RQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_rq_open, so every search entry point of GpuIvfPq
+    serves it.  _distance is the RaBitQ estimate of the squared L2 distance (half of it for cosine); refine_factor
+    re-ranks by the exact distance."""
+
+    def __init__(self, data, device: int = 0, with_vectors: bool = True):
+        lib = load()
+        if data.metric not in ("l2", "cosine"):
+            raise ValueError(f"IVF_RQ supports the l2 and cosine distance types, not {data.metric!r}")
+        data.validate()
+        self.dim, self.nlist, self.metric = data.dim, data.nlist, data.metric
+        self.device = device
+        vec = data.vectors if with_vectors else None
+        keep = [np.ascontiguousarray(data.centroids, np.float32), np.ascontiguousarray(data.rotation, np.float32),
+                np.ascontiguousarray(data.part_offsets, np.uint64), np.ascontiguousarray(data.codes, np.uint8),
+                np.ascontiguousarray(data.add_factors, np.float32), np.ascontiguousarray(data.scale_factors, np.float32),
+                np.ascontiguousarray(data.row_ids, np.uint64),
+                None if vec is None else np.ascontiguousarray(vec, np.float32)]
+        desc = RqDesc(ABI_VERSION, data.dim, data.nlist, METRICS[data.metric], device, data.num_bits, data.nrows,
+                      *[_ptr(a) for a in keep])
+        h = C.c_void_p()
+        check(lib.lgpu_ivf_rq_open(C.byref(desc), C.byref(h)))
         self._h = h
         self.has_vectors = vec is not None
 
@@ -636,6 +675,21 @@ def debug_sq_distances(q_codes, x_codes, device: int = 0) -> np.ndarray:
     out = np.empty((q.shape[0], x.shape[0]), np.uint32)
     check(load().lgpu_debug_sq_distances(_ptr(q), q.shape[0], _ptr(x), x.shape[0], q.shape[1], device, _ptr(out)))
     return out
+
+
+def debug_rq_distances(q_res, codes, add_factors, scale_factors, metric: str = "l2", device: int = 0):
+    """The IVF_RQ planes and scan kernels alone, each query one probe slot of rotated residual q_res[b] over the N rows:
+    (est [B, N] f32, ip [B, N] u32) -- the reported estimates and the exact sum_i b_i u_i."""
+    q = np.ascontiguousarray(q_res, np.float32); x = np.ascontiguousarray(codes, np.uint8)
+    if q.ndim != 2 or x.ndim != 2 or x.shape[1] != (q.shape[1] + 7) // 8:
+        raise ValueError("q_res must be [B, dim] and codes [N, ceil(dim / 8)]")
+    add = np.ascontiguousarray(add_factors, np.float32); sc = np.ascontiguousarray(scale_factors, np.float32)
+    if add.shape != (x.shape[0],) or sc.shape != (x.shape[0],):
+        raise ValueError("add_factors and scale_factors must be [N]")
+    est = np.empty((q.shape[0], x.shape[0]), np.float32); ip = np.empty((q.shape[0], x.shape[0]), np.uint32)
+    check(load().lgpu_debug_rq_distances(_ptr(q), q.shape[0], _ptr(x), _ptr(add), _ptr(sc), x.shape[0], q.shape[1],
+                                         METRICS[metric], device, _ptr(est), _ptr(ip)))
+    return est, ip
 
 
 def debug_maxsim_gemm(queries, values, offsets, device: int = 0) -> np.ndarray:

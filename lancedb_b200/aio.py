@@ -34,6 +34,17 @@ class IvfPq:
     sample_rate: int = 256
 
 
+@dataclass
+class IvfRq:
+    """Index.IvfRq parameters (python/python/lancedb/index.py:803-856, rust/lancedb/src/index/vector.rs:321-369):
+    RaBitQ with num_bits = 1 (the only width served)."""
+    distance_type: str = "l2"
+    num_partitions: Optional[int] = None
+    num_bits: int = 1
+    max_iterations: int = 50
+    sample_rate: int = 256
+
+
 class AsyncRecordBatchReader:
     """What `to_batches` resolves to: `async for batch in reader`, `await reader.read_all()`."""
 
@@ -249,13 +260,15 @@ class AsyncTable:
     async def list_indices(self):
         return self._table.list_indices()
 
-    async def create_index(self, column: str, *, config: Optional[IvfPq] = None, replace: bool = True,
+    async def create_index(self, column: str, *, config: Optional[Union[IvfPq, IvfRq]] = None, replace: bool = True,
                            accelerator: Optional[str] = "cuda"):
         cfg = config or IvfPq()
+        kind = "IVF_RQ" if isinstance(cfg, IvfRq) else "IVF_PQ"
         await asyncio.to_thread(
             self._table.create_index, metric=cfg.distance_type, num_partitions=cfg.num_partitions,
-            num_sub_vectors=cfg.num_sub_vectors, vector_column_name=column, replace=replace, accelerator=accelerator,
-            num_bits=cfg.num_bits, max_iterations=cfg.max_iterations, sample_rate=cfg.sample_rate)
+            num_sub_vectors=getattr(cfg, "num_sub_vectors", None), vector_column_name=column, replace=replace,
+            accelerator=accelerator, index_type=kind, num_bits=cfg.num_bits, max_iterations=cfg.max_iterations,
+            sample_rate=cfg.sample_rate)
 
     async def prewarm_index(self, name: str):
         return self._table.prewarm_index(name)

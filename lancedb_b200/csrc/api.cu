@@ -129,6 +129,7 @@ struct Workspace {
     DevBuf mv_qh, mv_qbad, mv_Mk, mv_A; // ... tensor-core path: fp16 queries, bad vectors, max-similarity keys, approx dist
     DevBuf mv_kd, mv_ki, mv_kc, mv_thr, mv_cnt, mv_cand, mv_flags, mv_vflags, mv_gate, mv_ex, mv_exid;   // shortlist
     DevBuf sq_q, sq_qq;                 // IVF_SQ search: query codes [B][dim_pad], their squared sums
+    DevBuf rq_q, rq_planes, rq_slots;   // IVF_RQ search: rotated queries [B][dim], per-slot bit-planes and grids
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -277,6 +278,11 @@ struct lgpu_index {
     uint32_t dim_pad = 0;
     double sq_lo = 0.0, sq_hi = 0.0;
     DevBuf sq_xx;
+    // IVF_RQ (lgpu_ivf_rq_open): `codes` holds [nrows][rq_wpr] u32 sign bits; the rotation, the rotated centroids and
+    // the per-row factors and popcounts
+    bool is_rq = false;
+    uint32_t rq_wpr = 0;
+    DevBuf rq_rot, rq_rc, rq_add, rq_scale, rq_popc;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
     WorkspacePool pool;
@@ -647,10 +653,11 @@ static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, c
     LGPU_REQUIRE(B == 0 || (q && ids && dist && cnt), "null buffer");
 }
 
-// ---- IVF search (IVF_PQ and IVF_SQ).  One sub-batch runs [cosine: normalise] -> coarse step (probes) -> small scan |
-// regroup -> filter scan + fix-up | exact scan + select -> [refine], on the paths ivf_plan picks before any launch ----
+// ---- IVF search (IVF_PQ, IVF_SQ and IVF_RQ).  One sub-batch runs [cosine: normalise] -> coarse step (probes) ->
+// small scan | regroup -> filter scan + fix-up | exact scan + select -> [refine], on the paths ivf_plan picks before
+// any launch ----
 enum class Coarse { exact, tc_dense, tc_list };   // see ivf_coarse
-enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq };
+enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq };
 
 struct IvfPlan {
     uint32_t B, nprobes, slots;
@@ -662,7 +669,11 @@ struct IvfPlan {
     IvfScan scan;
     uint32_t cand_cap;        // candidate mode: candidates per query (power of two >= kk)
     bool filter() const { return scan == IvfScan::filter_cand || scan == IvfScan::filter_dense; }
-    uint32_t rows_tile() const { return filter() ? SCAN3_ROWS_TILE : (scan == IvfScan::sq ? SQ_ROWS_TILE : SCAN_ROWS_TILE_MID); }
+    uint32_t rows_tile() const
+    {
+        if (filter()) return SCAN3_ROWS_TILE;
+        return scan == IvfScan::sq ? SQ_ROWS_TILE : (scan == IvfScan::rq ? RQ_ROWS_TILE : SCAN_ROWS_TILE_MID);
+    }
 };
 
 // prefilter: the request carries an allow bitmap; widening: the sub-batch redoes the queries flagged by the
@@ -688,13 +699,13 @@ static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, cons
                        ? Coarse::tc_list : Coarse::tc_dense;
     // tiny batches (a single query, a micro-batch): the small path, 4 launches instead of ~25; LGPU_SMALL_SLOTS = 0
     // disables it.  Otherwise filter + verify (scan3.cu) unless the request needs every exact distance.
-    const bool small = !ix->is_sq && !widening && p.slots <= modes.small_slots &&
+    const bool small = !ix->is_sq && !ix->is_rq && !widening && p.slots <= modes.small_slots &&
                        small_scan_smem(ix->m, ix->dim) <= 200 * 1024 &&
                        (size_t)p.slots * ix->pad_prefix[1] * 4 <= workspace_budget();
     const bool filter = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && p.lb_short > p.kk &&
                         ix->m <= 512 && !widening && !small;
     if (small) p.scan = IvfScan::small;
-    else if (!filter) p.scan = ix->is_sq ? IvfScan::sq : IvfScan::exact_pq;
+    else if (!filter) p.scan = ix->is_sq ? IvfScan::sq : (ix->is_rq ? IvfScan::rq : IvfScan::exact_pq);
     if (!filter) return p;
     // candidate mode (no prefilter, kk <= LGPU_CAND_KMAX): the scanners threshold the rows themselves, nothing dense is
     // written.  LGPU_CAND_CAP shrinks the capacity to exercise the overflow path.
@@ -1057,7 +1068,7 @@ static void filter_fixup(lgpu_index *ix, Workspace *ws, const IvfPlan &p, GroupA
     launch_select(sf, st);
 }
 
-// IvfScan::exact_pq / sq: the exact scan of every regrouped tile, then the PQ top-kk
+// IvfScan::exact_pq / sq / rq: the exact scan of every regrouped tile, then the PQ top-kk
 static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp, const float *qs,
                       const GroupArgs &ga, RowFilter rf, const uint32_t *only, TopkOut pq, cudaStream_t st,
                       const StageMarks &mark)
@@ -1069,6 +1080,15 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
         qa.total_tiles = ga.total_tiles; qa.tile_counter = ga.tile_counter; qa.tile_desc = ga.tile_desc;
         qa.dist_out = ws->dist_out.as<float>();
         launch_sq_scan(qa, 2 * ix->num_sms, st);
+    } else if (p.scan == IvfScan::rq) {
+        RqScanArgs ra{};
+        ra.codes = ix->codes.as<uint32_t>(); ra.add = ix->rq_add.as<float>(); ra.scale = ix->rq_scale.as<float>();
+        ra.popc = ix->rq_popc.as<uint32_t>();
+        ra.planes = ws->rq_planes.as<uint32_t>(); ra.slots = ws->rq_slots.as<RqSlot>();
+        ra.dim = ix->dim; ra.wpr = ix->rq_wpr; ra.cosine = ix->metric == LGPU_COSINE;
+        ra.total_tiles = ga.total_tiles; ra.tile_counter = ga.tile_counter; ra.tile_desc = ga.tile_desc;
+        ra.dist_out = ws->dist_out.as<float>();
+        launch_rq_scan(ra, 2 * ix->num_sms, st);
     } else {
         launch_scan2(scan_args(ix, ws, qs, ga), ix->dsub, ix->num_sms, st);
     }
@@ -1091,9 +1111,9 @@ static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const fl
     launch_select(sr, st);
 }
 
-// one sub-batch of an IVF_PQ / IVF_SQ search, everything device-side on `st` (and `front`, joined).  only (device,
-// [B]): redo just the flagged queries (maximum_nprobes widening) -- exact kernels, the other queries' outputs are left
-// untouched.
+// one sub-batch of an IVF_PQ / IVF_SQ / IVF_RQ search, everything device-side on `st` (and `front`, joined).  only
+// (device, [B]): redo just the flagged queries (maximum_nprobes widening) -- exact kernels, the other queries' outputs
+// are left untouched.
 void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
                    const lgpu_search_params &sp, uint32_t nprobes, TopkOut out, bool prof, RowFilter rf,
                    const uint32_t *only = nullptr)
@@ -1109,6 +1129,13 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         ws->sq_q.ensure((size_t)B * ix->dim_pad); ws->sq_qq.ensure((size_t)B * 4);
         launch_sq_encode(qs, B, ix->dim, ix->dim_pad, ix->sq_lo, ix->sq_hi, ws->sq_q.as<uint8_t>(),
                          ws->sq_qq.as<uint32_t>(), st);
+    } else if (p.scan == IvfScan::rq) {        // rotate the queries, then each probe slot's 4-bit grid of q - c_p
+        ws->rq_q.ensure((size_t)B * ix->dim * 4);
+        ws->rq_planes.ensure((size_t)p.slots * 4 * ix->rq_wpr * 4);
+        ws->rq_slots.ensure((size_t)p.slots * sizeof(RqSlot));
+        launch_rq_rotate(ix->rq_rot.as<float>(), qs, B, ix->dim, ws->rq_q.as<float>(), st);
+        launch_rq_planes(ws->rq_q.as<float>(), ix->rq_rc.as<float>(), ws->probes.as<uint64_t>(), p.slots, nprobes,
+                         ix->nlist, ix->dim, ix->rq_wpr, ws->rq_planes.as<uint32_t>(), ws->rq_slots.as<RqSlot>(), st);
     }
     mark(IVF_PROBES, cs);
     if (p.scan == IvfScan::small) {
@@ -1138,6 +1165,7 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
 {
     uint32_t np_eff = std::min<uint32_t>(nprobes, ix->nlist);
     size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4);
+    if (ix->is_rq) per_q += (size_t)nprobes * (16 * ix->rq_wpr + sizeof(RqSlot)) + (size_t)ix->dim * 4;  // planes, rq
     size_t bs = workspace_budget() / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
     bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
@@ -1179,7 +1207,8 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
         unsigned long long rows = 0;
         if (ws->stages_marked >> IVF_REGROUP & 1)
             LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
-        g_scanned_bytes = (uint64_t)rows * (ix->is_sq ? ix->dim : ix->m);   // code bytes per row
+        const uint32_t row_bytes = ix->is_sq ? ix->dim : (ix->is_rq ? ix->rq_wpr * 4 : ix->m);   // code bytes per row
+        g_scanned_bytes = (uint64_t)rows * row_bytes;
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
         if (ws->stats_mode == 1) LGPU_CUDA(cudaMemcpy(g_filter_stats, ws->c_stats.p, 32, cudaMemcpyDeviceToHost));
         else if (ws->stats_mode == 2) {                       // dense filter: queries the band check could not prove
@@ -1843,6 +1872,24 @@ static void upload_sq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBu
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
+// IVF_RQ stored rows: dim zero-padded to the scan's K step, in 32-bit words
+static uint32_t rq_wpr(uint32_t dim) { return (uint32_t)round_up64(dim, RQ_K_BITS) / 32; }
+
+// codes [n][ceil(dim / 8)] (host) -> dst [n][wpr] u32 (device, zero padding, bits past dim cleared) and popc[r]
+static void upload_rq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBuf &dst, DevBuf &popc)
+{
+    const uint32_t wpr = rq_wpr(dim), nb = (dim + 7) / 8;
+    dst.ensure(std::max<size_t>((size_t)n * wpr * 4, 16));
+    popc.ensure(std::max<size_t>((size_t)n * 4, 16));
+    cudaStream_t st = nullptr;
+    LGPU_CUDA(cudaMemsetAsync(dst.p, 0, dst.bytes, st));
+    if (n) {
+        LGPU_CUDA(cudaMemcpy2DAsync(dst.p, (size_t)wpr * 4, codes, nb, nb, n, cudaMemcpyHostToDevice, st));
+        launch_rq_row_prep(dst.as<uint32_t>(), n, dim, wpr, popc.as<uint32_t>(), st);
+    }
+    LGPU_CUDA(cudaStreamSynchronize(st));
+}
+
 }  // namespace
 
 extern "C" {
@@ -2027,6 +2074,114 @@ int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x
         a.tile_desc = tiles.as<TileDesc>(); a.dist_out = D.as<float>(); a.out_u32 = 1;
         launch_sq_scan(a, 2 * prop.multiProcessorCount, nullptr);
         LGPU_CUDA(cudaMemcpy(out, D.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
+{
+    lgpu_index *ix = nullptr;
+    int rc = guarded([&] {
+        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+        LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
+        LGPU_REQUIRE(d->metric != LGPU_DOT, "IVF_RQ supports the l2 and cosine distance types, not dot");
+        LGPU_REQUIRE(d->num_bits == 1, "IVF_RQ supports num_bits = 1 only");
+        LGPU_REQUIRE(d->dim <= LGPU_RQ_MAX_DIM, "IVF_RQ supports dimensions up to 4096");
+        LGPU_REQUIRE(d->rotation != nullptr, "null index array");
+        LGPU_REQUIRE(d->nrows == 0 || (d->add_factors && d->scale_factors), "null index array");
+        check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
+        require_device(d->device);
+        ix = new lgpu_index();
+        ix->is_rq = true;
+        ix->rq_wpr = rq_wpr(d->dim);
+        open_ivf_common(ix, d->device, d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
+                        d->vectors, RQ_ROWS_TILE);
+        // byte offset of each partition's codes (the tile descriptors carry it; the RQ scan addresses rows by part_off)
+        std::vector<uint64_t> code_base(d->nlist);
+        for (uint32_t p = 0; p < d->nlist; p++) code_base[p] = d->part_offsets[p] * ix->rq_wpr * 4;
+        ix->code_base.ensure((size_t)d->nlist * 8);
+        LGPU_CUDA(cudaMemcpy(ix->code_base.p, code_base.data(), (size_t)d->nlist * 8, cudaMemcpyHostToDevice));
+        upload_rq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->rq_popc);
+        const size_t rows = std::max<size_t>((size_t)d->nrows * 4, 16), rot = (size_t)d->dim * d->dim * 4;
+        ix->rq_add.ensure(rows); ix->rq_scale.ensure(rows); ix->rq_rot.ensure(rot);
+        ix->rq_rc.ensure((size_t)d->nlist * d->dim * 4);
+        if (d->nrows) {
+            LGPU_CUDA(cudaMemcpy(ix->rq_add.p, d->add_factors, (size_t)d->nrows * 4, cudaMemcpyHostToDevice));
+            LGPU_CUDA(cudaMemcpy(ix->rq_scale.p, d->scale_factors, (size_t)d->nrows * 4, cudaMemcpyHostToDevice));
+        }
+        LGPU_CUDA(cudaMemcpy(ix->rq_rot.p, d->rotation, rot, cudaMemcpyHostToDevice));
+        // rc_p = P c_p, once: each probe slot's residual is then one subtraction per dimension
+        launch_rq_rotate(ix->rq_rot.as<float>(), ix->centroids.as<float>(), d->nlist, d->dim, ix->rq_rc.as<float>(),
+                         nullptr);
+        LGPU_CUDA(cudaStreamSynchronize(nullptr));
+        ix->device_bytes += ix->code_base.bytes + ix->codes.bytes + ix->rq_popc.bytes + ix->rq_add.bytes +
+                            ix->rq_scale.bytes + ix->rq_rot.bytes + ix->rq_rc.bytes;
+        register_handle(ix);
+        *out = ix;
+    });
+    if (rc != LGPU_OK && ix) delete ix;
+    return rc;
+}
+
+int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes, const float *add_factors,
+                            const float *scale_factors, uint64_t N, uint32_t dim, int metric, int device,
+                            float *out_est, uint32_t *out_ip)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(dim >= 1 && dim <= LGPU_RQ_MAX_DIM, "dim must be in [1, 4096]");
+        LGPU_REQUIRE(metric == LGPU_L2 || metric == LGPU_COSINE, "IVF_RQ supports the l2 and cosine distance types");
+        LGPU_REQUIRE(B == 0 || N == 0 || (q_res && codes && add_factors && scale_factors && (out_est || out_ip)),
+                     "null buffer");
+        LGPU_REQUIRE(N < (1ull << 31) && (uint64_t)B * N < (1ull << 32), "B x N must stay below 2^32");
+        if (B == 0 || N == 0) return;
+        require_device(device);
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        const uint32_t wpr = rq_wpr(dim);
+        DevBuf X, popc, add, scale, Q, zero, probes, planes, slots, D, tiles, ctr;
+        upload_rq_rows(codes, N, dim, X, popc);
+        add.ensure((size_t)N * 4); scale.ensure((size_t)N * 4);
+        Q.ensure((size_t)B * dim * 4); zero.ensure((size_t)dim * 4); probes.ensure((size_t)B * 8);
+        planes.ensure((size_t)B * 4 * wpr * 4); slots.ensure((size_t)B * sizeof(RqSlot));
+        LGPU_CUDA(cudaMemcpy(add.p, add_factors, (size_t)N * 4, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(scale.p, scale_factors, (size_t)N * 4, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(Q.p, q_res, (size_t)B * dim * 4, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemset(zero.p, 0, (size_t)dim * 4));
+        LGPU_CUDA(cudaMemset(probes.p, 0, (size_t)B * 8));
+        // query b is one probe slot of partition 0 whose rotated centroid is 0: q' = the given residual
+        launch_rq_planes(Q.as<float>(), zero.as<float>(), probes.as<uint64_t>(), B, 1, 1, dim, wpr,
+                         planes.as<uint32_t>(), slots.as<RqSlot>(), nullptr);
+        // one partition of N rows that every slot probes: tiles of RQ_ROWS_TILE rows x 8 slots, slot b's row r at
+        // out + b N + r
+        std::vector<TileDesc> h;
+        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
+            for (uint64_t r0 = 0; r0 < N; r0 += RQ_ROWS_TILE) {
+                TileDesc t{};
+                t.row0 = (uint32_t)r0; t.nrows = (uint32_t)std::min<uint64_t>(RQ_ROWS_TILE, N - r0);
+                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N;
+                for (uint32_t g = 0; g < t.ng; g++) {
+                    t.q[g] = q0 + g; t.slot[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * N);
+                }
+                h.push_back(t);
+            }
+        tiles.ensure(h.size() * sizeof(TileDesc));
+        ctr.ensure(8);
+        D.ensure((size_t)B * N * 4);
+        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
+        RqScanArgs a{};
+        a.codes = X.as<uint32_t>(); a.add = add.as<float>(); a.scale = scale.as<float>(); a.popc = popc.as<uint32_t>();
+        a.planes = planes.as<uint32_t>(); a.slots = slots.as<RqSlot>(); a.dim = dim; a.wpr = wpr;
+        a.cosine = metric == LGPU_COSINE;
+        a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1;
+        a.tile_desc = tiles.as<TileDesc>(); a.dist_out = D.as<float>();
+        const uint32_t total = (uint32_t)h.size(), zero2[2] = {total, 0u};
+        for (int mode = 0; mode < 2; mode++) {
+            void *dst = mode ? (void *)out_ip : (void *)out_est;
+            if (!dst) continue;
+            LGPU_CUDA(cudaMemcpy(ctr.p, zero2, 8, cudaMemcpyHostToDevice));
+            a.out_ip = mode;
+            launch_rq_scan(a, 2 * prop.multiProcessorCount, nullptr);
+            LGPU_CUDA(cudaMemcpy(dst, D.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
+        }
     });
 }
 
@@ -2620,7 +2775,7 @@ int lgpu_search_sharded(lgpu_index *ixh, lgpu_comm *ch, const float *queries, ui
     return guarded([&] {
         HandleRef<lgpu_index> ix(ixh, "index");
         HandleRef<lgpu_comm> c(ch, "communicator");
-        LGPU_REQUIRE(!ix->is_sq, "sharded search serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "sharded search serves IVF_PQ indexes only");
         check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -2638,7 +2793,7 @@ int lgpu_search_sharded_device(lgpu_index *ixh, lgpu_comm *ch, const float *d_qu
     return guarded([&] {
         HandleRef<lgpu_index> ix(ixh, "index");
         HandleRef<lgpu_comm> c(ch, "communicator");
-        LGPU_REQUIRE(!ix->is_sq, "sharded search serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "sharded search serves IVF_PQ indexes only");
         check_ivf_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -2711,7 +2866,7 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
     return guarded([&] {
         LGPU_REQUIRE(query && out, "null argument");
         HandleRef<lgpu_index> ix(ixh, "index");
-        LGPU_REQUIRE(!ix->is_sq, "lgpu_debug_partition_distances serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "lgpu_debug_partition_distances serves IVF_PQ indexes only");
         LGPU_REQUIRE(part < ix->nlist, "partition out of range");
         require_device(ix->device);
         WsLease lease(ix->pool, nullptr, false);
@@ -2742,7 +2897,7 @@ int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, 
     return guarded([&] {
         LGPU_REQUIRE(queries && out_parts && out_L && out_W && out_E && out_bad && B > 0 && nprobes > 0, "bad argument");
         HandleRef<lgpu_index> ix(ixh, "index");
-        LGPU_REQUIRE(!ix->is_sq, "lgpu_debug_filter_bounds serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "lgpu_debug_filter_bounds serves IVF_PQ indexes only");
         require_device(ix->device);
         nprobes = std::min(nprobes, ix->nlist);
         LGPU_REQUIRE(ivf_sub_batch_size(ix.h, B, nprobes) == B, "batch too large for one filter-scan launch");

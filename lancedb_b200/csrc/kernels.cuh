@@ -113,6 +113,38 @@ void launch_sq_encode(const float *Q, uint32_t B, uint32_t dim, uint32_t dim_pad
 void launch_sq_row_norms(const uint8_t *codes, uint64_t n, uint32_t dim_pad, uint32_t *xx, cudaStream_t st);
 void launch_sq_scan(const SqScanArgs &a, int grid, cudaStream_t st);
 
+// ---------------- IVF_RQ scan (rq_scan.cu) ----------------------------------------------
+constexpr uint32_t RQ_ROWS_TILE = 256;            // rows per tile: 8 warps x 32 rows
+constexpr uint32_t RQ_K_BITS = 256;               // code bits per K step (one b1 MMA); stored rows are padded to it
+struct alignas(16) RqSlot {                       // one probe slot's 4-bit query grid
+    float lo, delta;                              // min q', fl(fl(max q' - lo) / 15)
+    uint32_t S;                                   // sum of the 4-bit codes u
+    float qq;                                     // lance_l2(rq, rc_p)
+};
+struct RqScanArgs {
+    const uint32_t *codes;        // [nrows][wpr] sign bits, partitions contiguous, zero padding
+    const float *add, *scale;     // [nrows] |o|^2, -2 |o|^2 / sum |o_i|
+    const uint32_t *popc;         // [nrows] set bits of each row
+    const uint32_t *planes;       // [slots][4][wpr] bit-planes of u (launch_rq_planes)
+    const RqSlot *slots;          // [slots]
+    uint32_t dim, wpr;            // wpr = 32-bit words per row (dim_pad / 32, a multiple of 8)
+    int cosine;                   // report fl(0.5 est)
+    const uint32_t *total_tiles;  // [1]
+    uint32_t *tile_counter;       // [1], zeroed before launch
+    const TileDesc *tile_desc;    // built with rows_tile == RQ_ROWS_TILE; slot[] addresses planes / slots
+    float *dist_out;              // segment of slot e at out[e]: the estimate of row r at out[e] + r
+    int out_ip;                   // 1: write the exact u32 ip = sum_i b_i u_i instead (lgpu_debug_rq_distances)
+};
+// out[v][i] = lance_dot(P row i, x[v]): the rotation of n vectors by P [dim][dim]
+void launch_rq_rotate(const float *P, const float *x, uint32_t n, uint32_t dim, float *out, cudaStream_t st);
+// per probe slot e (query e / nprobes, partition probes[e]; slots without a partition are skipped): the 4-bit grid of
+// q' = rq - rc_p as planes [e][4][wpr] and slot_out[e]
+void launch_rq_planes(const float *rq, const float *rc, const uint64_t *probes, uint32_t slots, uint32_t nprobes,
+                      uint32_t nlist, uint32_t dim, uint32_t wpr, uint32_t *planes, RqSlot *slot_out, cudaStream_t st);
+// clear the padding bits of codes [n][wpr] and count each row's set bits
+void launch_rq_row_prep(uint32_t *codes, uint64_t n, uint32_t dim, uint32_t wpr, uint32_t *popc, cudaStream_t st);
+void launch_rq_scan(const RqScanArgs &a, int grid, cudaStream_t st);
+
 // ---------------- tiny batches: one CTA per (query, probed partition) pair (small.cu) ----------------
 struct SmallScanArgs {
     const float *centroids; const float *cb_tiled; const unsigned char *codes; const uint64_t *code_base;

@@ -1,4 +1,4 @@
-"""IVF_PQ and IVF_SQ index containers and trainers.
+"""IVF_PQ, IVF_SQ and IVF_RQ index containers and trainers.
 
 `IvfPqIndexData` is the plain-array form of a Lance IVF_PQ index: exactly the arrays
 the reference's search path consumes after `prewarm_index`
@@ -383,5 +383,128 @@ def train_ivf_sq(vectors, *, num_partitions: Optional[int] = None, distance_type
         dim=dim, nlist=nlist, metric=metric, centroids=centroids.cpu().numpy().astype(np.float32),
         part_offsets=part_offsets, codes=sq_encode(x[order].cpu().numpy(), lo, hi), row_ids=rid[order_np],
         lo=lo, hi=hi, vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
+    data.validate()
+    return data
+
+
+# --------------------------------------------------------------------------------------
+RQ_METRICS = ("l2", "cosine")
+RQ_MAX_DIM = 4096           # LGPU_RQ_MAX_DIM: P is at most 64 MB, the scan's integers stay exact in f32
+
+
+@dataclass
+class IvfRqIndexData:
+    """The plain-array form of an IVF_RQ index (lance `IvfRq`, RaBitQ with num_bits = 1; rust/lancedb/src/index/
+    vector.rs:321-369): IVF centroids, one f32 orthogonal rotation P and, for every row of partition p with
+    o = P (x - c_p), one sign bit per dimension (LSB first) and the factors add = |o|^2, scale = -2 |o|^2 / sum |o_i|,
+    grouped by partition.  The same arrays go to `lgpu_ivf_rq_open` and to the CPU oracle (tests/rq_oracle.c)."""
+    dim: int
+    nlist: int
+    metric: str
+    centroids: np.ndarray      # f32 [nlist, dim]
+    rotation: np.ndarray       # f32 [dim, dim]
+    part_offsets: np.ndarray   # u64 [nlist+1]
+    codes: np.ndarray          # u8 [n, ceil(dim / 8)] partition order
+    add_factors: np.ndarray    # f32 [n]
+    scale_factors: np.ndarray  # f32 [n]
+    row_ids: np.ndarray        # u64 [n] in partition order
+    vectors: Optional[np.ndarray] = None   # f32 [n, dim] partition order (refine), optional
+    num_bits: int = 1
+
+    @property
+    def nrows(self) -> int:
+        return int(self.row_ids.size)
+
+    def validate(self) -> None:
+        assert self.metric in RQ_METRICS and self.num_bits == 1
+        assert 1 <= self.dim <= RQ_MAX_DIM
+        assert self.centroids.shape == (self.nlist, self.dim) and self.centroids.dtype == np.float32
+        assert self.rotation.shape == (self.dim, self.dim) and self.rotation.dtype == np.float32
+        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
+        assert int(self.part_offsets[-1]) == self.nrows
+        assert self.codes.shape == (self.nrows, (self.dim + 7) // 8) and self.codes.dtype == np.uint8
+        assert self.add_factors.shape == (self.nrows,) and self.add_factors.dtype == np.float32
+        assert self.scale_factors.shape == (self.nrows,) and self.scale_factors.dtype == np.float32
+        assert self.row_ids.dtype == np.uint64
+
+
+def rq_rotation(dim: int, seed: int = 45, device=None) -> np.ndarray:
+    """P: the Q of the QR of a seeded standard-normal f64 [dim, dim] matrix, its columns multiplied by sign(diag(R))
+    (so P is Haar-distributed), cast to f32."""
+    import torch
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    a = torch.randn((dim, dim), generator=g, dtype=torch.float64).to(device or "cpu")
+    q, r = torch.linalg.qr(a)
+    s = torch.sign(torch.diagonal(r))
+    s = torch.where(s == 0, torch.ones_like(s), s)
+    return (q * s[None, :]).to(torch.float32).cpu().numpy()
+
+
+def rq_encode(x, centroids, assign, rotation, chunk: int = 1 << 16):
+    """(codes [n, ceil(dim / 8)] u8, add [n] f32, scale [n] f32) of rows x (already normalised for cosine) in partitions
+    `assign`: o = P (x - c_p) in f64 (from the f32 values), bit i = [o_i > 0] (bit i & 7 of byte i >> 3),
+    add = f32(sum o_i^2), scale = f32(-2 sum o_i^2 / sum |o_i|), both 0 when sum |o_i| = 0.  torch ops on x's device."""
+    import torch
+    x = torch.as_tensor(x)
+    dev = x.device
+    c = torch.as_tensor(centroids, device=dev).to(torch.float64)
+    P = torch.as_tensor(rotation, device=dev).to(torch.float64)
+    a = torch.as_tensor(assign, device=dev).long()
+    n, dim = x.shape
+    nb = (dim + 7) // 8
+    codes = np.zeros((n, nb), np.uint8)
+    add = np.zeros(n, np.float32)
+    scale = np.zeros(n, np.float32)
+    w = (2 ** torch.arange(8, device=dev, dtype=torch.int64))
+    for s in range(0, n, chunk):
+        o = (x[s:s + chunk].to(torch.float64) - c[a[s:s + chunk]]) @ P.T
+        bits = (o > 0).to(torch.int64)
+        pad = nb * 8 - dim
+        if pad:
+            bits = torch.nn.functional.pad(bits, (0, pad))
+        codes[s:s + chunk] = (bits.reshape(-1, nb, 8) * w).sum(2).to(torch.uint8).cpu().numpy()
+        n2 = (o * o).sum(1)
+        l1 = o.abs().sum(1)
+        sc = torch.where(l1 > 0, -2.0 * n2 / torch.where(l1 > 0, l1, torch.ones_like(l1)), torch.zeros_like(l1))
+        add[s:s + chunk] = torch.where(l1 > 0, n2, torch.zeros_like(n2)).to(torch.float32).cpu().numpy()
+        scale[s:s + chunk] = sc.to(torch.float32).cpu().numpy()
+    return codes, add, scale
+
+
+def train_ivf_rq(vectors, *, num_partitions: Optional[int] = None, distance_type: str = "l2", num_bits: int = 1,
+                 sample_rate: int = 256, max_iterations: int = 50, row_ids: Optional[np.ndarray] = None,
+                 keep_vectors: bool = False, seed: int = 45, device: Optional[str] = None,
+                 native_passes: bool = False) -> IvfRqIndexData:
+    """Train IVF centroids (the IVF half of train_ivf_pq), draw the rotation P (rq_rotation) and encode every row
+    (normalised for cosine) with rq_encode, in torch f64 on the given device."""
+    import torch
+    metric = distance_type.lower()
+    if metric not in RQ_METRICS:
+        raise ValueError(f"IVF_RQ supports the l2 and cosine distance types, not {distance_type!r}")
+    if num_bits != 1:
+        raise ValueError(f"IVF_RQ supports num_bits=1 only, got num_bits={num_bits}")
+    x = torch.as_tensor(vectors, dtype=torch.float32)
+    if device is not None:
+        x = x.to(device)
+    n, dim = x.shape
+    if not 1 <= dim <= RQ_MAX_DIM:
+        raise ValueError(f"IVF_RQ supports dimensions 1..{RQ_MAX_DIM}, got {dim}")
+    nlist = int(num_partitions or suggested_num_partitions(n))
+    gen = torch.Generator(device="cpu").manual_seed(seed)
+    raw = x
+    x, _, centroids, assign, _ = _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes)
+    cent = centroids.cpu().numpy().astype(np.float32)
+    P = rq_rotation(dim, seed, x.device)
+    order = torch.argsort(assign, stable=True)                            # ascending row id per partition
+    sizes = torch.bincount(assign, minlength=nlist).cpu().numpy().astype(np.int64)
+    part_offsets = np.zeros(nlist + 1, np.uint64)
+    part_offsets[1:] = np.cumsum(sizes)
+    codes, add, scale = rq_encode(x[order], cent, assign[order], P)
+    order_np = order.cpu().numpy()
+    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
+    data = IvfRqIndexData(
+        dim=dim, nlist=nlist, metric=metric, centroids=cent, rotation=P, part_offsets=part_offsets, codes=codes,
+        add_factors=add, scale_factors=scale, row_ids=rid[order_np],
+        vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
     data.validate()
     return data

@@ -16,7 +16,8 @@ import numpy as np
 import pyarrow as pa
 
 from . import _native
-from .index import IvfPqIndexData, IvfSqIndexData, train_ivf_pq, train_ivf_sq
+from .index import (RQ_MAX_DIM, IvfPqIndexData, IvfRqIndexData, IvfSqIndexData, train_ivf_pq, train_ivf_rq,
+                    train_ivf_sq)
 from .query import LanceVectorQueryBuilder
 
 
@@ -83,7 +84,7 @@ class Table:
         self._binary: Dict[str, _native.GpuBinary] = {}
         self._multivec: Dict[str, _native.GpuMultivec] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
-        self._index_data: Dict[str, Union[IvfPqIndexData, IvfSqIndexData]] = {}
+        self._index_data: Dict[str, Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData]] = {}
 
     # ---- introspection ----
     @property
@@ -103,7 +104,8 @@ class Table:
         return self._data.to_pandas()
 
     def _index_type(self, column: str) -> str:
-        return "IVF_SQ" if isinstance(self._index_data[column], IvfSqIndexData) else "IVF_PQ"
+        d = self._index_data[column]
+        return "IVF_SQ" if isinstance(d, IvfSqIndexData) else ("IVF_RQ" if isinstance(d, IvfRqIndexData) else "IVF_PQ")
 
     def list_indices(self):
         return [{"name": f"{c}_idx", "index_type": self._index_type(c), "columns": [c]} for c in self._index]
@@ -154,17 +156,23 @@ class Table:
                      replace: bool = True, accelerator: Optional[str] = None, index_type: str = "IVF_PQ",
                      num_bits: int = 8, max_iterations: int = 50, sample_rate: int = 256, **_ignored):
         kind = index_type.upper()
-        if kind not in ("IVF_PQ", "IVF_SQ"):
-            raise NotImplementedError("only IVF_PQ and IVF_SQ are on the GPU hot path")
-        if num_bits != 8:
+        if kind not in ("IVF_PQ", "IVF_SQ", "IVF_RQ"):
+            raise NotImplementedError("only IVF_PQ, IVF_SQ and IVF_RQ are on the GPU hot path")
+        if kind == "IVF_RQ" and num_bits != 1:
+            # RaBitQ with 1 bit per dimension only (extended RaBitQ is not served); the legacy default of 8 is refused
+            # rather than quietly building a 1-bit index
+            raise ValueError(f"IVF_RQ supports num_bits=1 only, got num_bits={num_bits}")
+        if kind != "IVF_RQ" and num_bits != 8:
             raise ValueError("only num_bits=8 is supported")
         column = vector_column_name or self._infer_vector_column(None)
         if self._is_binary(column):
             raise NotImplementedError("no index over binary vectors on the GPU path: search them flat (hamming)")
         if self._is_multivec(column):
             raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
-        if kind == "IVF_SQ" and metric.lower() not in ("l2", "cosine"):
-            raise ValueError(f"IVF_SQ supports the l2 and cosine distance types, not {metric!r}")
+        if kind in ("IVF_SQ", "IVF_RQ") and metric.lower() not in ("l2", "cosine"):
+            raise ValueError(f"{kind} supports the l2 and cosine distance types, not {metric!r}")
+        if kind == "IVF_RQ" and self._dim(column) > RQ_MAX_DIM:
+            raise ValueError(f"IVF_RQ supports dimensions up to {RQ_MAX_DIM}, got {self._dim(column)}")
         if column in self._index and not replace:
             raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")   # python/python/tests/test_index.py:357
         dev = None
@@ -176,6 +184,12 @@ class Table:
                                                     sample_rate=sample_rate, keep_vectors=True, device=dev,
                                                     native_passes=dev is not None))
             return
+        if kind == "IVF_RQ":               # IvfRqIndexBuilder: distance_type, num_partitions, num_bits, max_iterations, sample_rate
+            self._attach_index(column, train_ivf_rq(self._vectors(column), num_partitions=num_partitions,
+                                                    distance_type=metric, num_bits=num_bits,
+                                                    max_iterations=max_iterations, sample_rate=sample_rate,
+                                                    keep_vectors=True, device=dev, native_passes=dev is not None))
+            return
         data = train_ivf_pq(self._vectors(column), num_partitions=num_partitions,
                             num_sub_vectors=num_sub_vectors, distance_type=metric,
                             max_iterations=max_iterations, sample_rate=sample_rate,
@@ -183,11 +197,12 @@ class Table:
                             native_passes=dev is not None)      # accelerator: row passes through the C ABI (build.cu)
         self._attach_index(column, data)
 
-    def _attach_index(self, column: str, data: Union[IvfPqIndexData, IvfSqIndexData]):
+    def _attach_index(self, column: str, data: Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData]):
         if column in self._index:
             self._index[column].close()
         self._index_data[column] = data
-        cls = _native.GpuIvfSq if isinstance(data, IvfSqIndexData) else _native.GpuIvfPq
+        cls = (_native.GpuIvfSq if isinstance(data, IvfSqIndexData) else
+               _native.GpuIvfRq if isinstance(data, IvfRqIndexData) else _native.GpuIvfPq)
         self._index[column] = cls(data, device=self._device)
 
     # ---- on-disk Lance index (SURVEY.md 8f-3; layout [lance, recalled], see lance_index.py) ----
