@@ -71,7 +71,7 @@ typedef struct {
     uint32_t dim;
     uint32_t nlist;              /* IVF partitions */
     uint32_t m;                  /* PQ sub-vectors; dim % m == 0 */
-    uint32_t nbits;              /* must be 8 */
+    uint32_t nbits;              /* 8, or 4 (packed nibble codes, see "4-bit IVF_PQ" below) */
     int32_t  metric;             /* lgpu_metric the index was trained with */
     int32_t  codes_layout;       /* lgpu_codes_layout */
     int32_t  device;             /* CUDA device ordinal */
@@ -171,6 +171,25 @@ int lgpu_merge_topk_device(int device, uint32_t nlists, uint32_t B, uint32_t k,
                            const uint64_t *d_ids, const float *d_dist,
                            uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count,
                            void *cuda_stream);
+
+/* ---- 4-bit IVF_PQ (lance `IvfPq` with num_bits = 4, rust/lancedb/src/table/create_index.rs:86-102, 283-303): an
+ * ordinary lgpu_index_desc with nbits = 4.  m is even, dim % m == 0, dim / m is 1, 2, 4, 8, 16 or 32 and
+ * m <= LGPU_PQ4_MAX_M; codebook is [m][16][dim/m]; codes are nrows * m / 2 bytes, byte j of a row holding sub-vector
+ * 2j's code in bits 0-3 and sub-vector 2j+1's in bits 4-7 [lance, recalled]; LGPU_CODES_ROW_MAJOR is [nrows][m/2],
+ * LGPU_CODES_PARTITION_TRANSPOSED is [m/2][n_p] per partition.  Any nbits other than 4 or 8 is LGPU_INVALID_INPUT.
+ * Per query (normalised first for cosine) and probed partition p, with r = q - c_p (l2, cosine) or q (dot):
+ *   1. T[i][j] (i < m, j < 16) = the 8-bit path's table entry on the 16 codewords (sub-vector L2, or 1 - dot).
+ *   2. qmin = min over every T; qmax = max over i = 0 .. m-2 of (max_j T[i][j] + max_j T[i+1][j]); both folds skip
+ *      NaN (an all-NaN fold is +inf / -inf) [lance, recalled].
+ *   3. Q[i][j] = sat_u8(round(((T[i][j] - qmin) * 255) / (qmax - qmin))): each f32 op rounded to nearest, left to
+ *      right, round half away from zero, NaN and below 0 -> 0, above 255 -> 255 [lance, recalled].
+ *   4. S = sum_i Q[i][code_i], an exact integer.
+ *   5. d = ((float) S * (qmax - qmin)) / 255 + qmin * (float) m, each op in f32 without FMA, in this order
+ *      [lance, recalled]; cosine reports 0.5 d, dot d - (m - 1).
+ * A row whose d is NaN is never returned.  Everything else -- k, nprobes, maximum_nprobes, prefilter, distance_range
+ * (on d, before refine), refine_factor, timeout_ms and every search entry point -- is IVF_PQ's.
+ * lgpu_debug_partition_distances serves the index; lgpu_search_sharded* and lgpu_debug_filter_bounds reject it. */
+#define LGPU_PQ4_MAX_M 256        /* a slot's sum stays below 2^16 (255 x 256) */
 
 /* ---- IVF_SQ (lance `IvfSq`, rust/lancedb/src/index/vector.rs:216-256): the same IVF partitions, each row stored as
  * dim 8-bit scalar codes instead of PQ codes.  One global range [lo, hi] (f64) quantises every component:
@@ -393,6 +412,11 @@ int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint
  * dim <= 65536, B x N < 2^32) */
 int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x_codes, uint64_t N, uint32_t dim,
                             int device, uint32_t *out);
+/* the 4-bit IVF_PQ scan kernel alone, every query one probe slot over one partition of N rows: out[q][x] = sum_i
+ * tables[q][i][code_i(x)], the exact u32 sum (host buffers: tables [B][m][16] u8, codes [N][m/2] packed as in the
+ * index, out [B][N]; m even, 2 <= m <= LGPU_PQ4_MAX_M, B x N < 2^32) */
+int lgpu_debug_pq4_sums(const uint8_t *tables, uint32_t B, const uint8_t *codes, uint64_t N, uint32_t m, int device,
+                        uint32_t *out);
 /* the IVF_RQ planes and scan kernels alone, every query one probe slot over one partition of N rows: q_res [B][dim] the
  * rotated residuals q', codes [N][ceil(dim / 8)], add / scale [N]; out_est [B][N] the reported estimates (NaN where the
  * slot has no rows), out_ip [B][N] the exact ip = sum_i b_i u_i (either may be NULL; host buffers; dim <= 4096,

@@ -38,6 +38,7 @@ EXPORTS = [
     "lgpu_multivec_search_device", "lgpu_debug_maxsim_gemm",
     "lgpu_ivf_sq_open", "lgpu_debug_sq_distances",
     "lgpu_ivf_rq_open", "lgpu_debug_rq_distances",
+    "lgpu_debug_pq4_sums",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -161,6 +162,7 @@ def load():
     lib.lgpu_debug_sq_distances.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_rq_open.argtypes = [C.POINTER(RqDesc), C.POINTER(vp)]
     lib.lgpu_debug_rq_distances.argtypes = [vp, u32, vp, vp, vp, C.c_uint64, u32, i32, i32, vp, vp]
+    lib.lgpu_debug_pq4_sums.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -256,7 +258,7 @@ def _query_offsets(q_offsets) -> np.ndarray:
 
 
 class GpuIvfPq(_Handle):
-    """An IVF_PQ index pinned in HBM (lgpu_index)."""
+    """An IVF_PQ index pinned in HBM (lgpu_index), 8-bit or 4-bit codes (data.num_bits)."""
     _close = "lgpu_index_close"
 
     def __init__(self, data, device: int = 0, with_vectors: bool = True):
@@ -269,7 +271,8 @@ class GpuIvfPq(_Handle):
                 np.ascontiguousarray(data.part_offsets, np.uint64), np.ascontiguousarray(data.codes_t, np.uint8),
                 np.ascontiguousarray(data.row_ids, np.uint64),
                 None if vec is None else np.ascontiguousarray(vec, np.float32)]
-        desc = IndexDesc(ABI_VERSION, data.dim, data.nlist, data.m, 8, METRICS[data.metric], 1, device,
+        self.num_bits = data.num_bits
+        desc = IndexDesc(ABI_VERSION, data.dim, data.nlist, data.m, data.num_bits, METRICS[data.metric], 1, device,
                          data.nrows, _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]),
                          _ptr(keep[5]))
         h = C.c_void_p()
@@ -664,6 +667,19 @@ def debug_hamming_gemm(queries, vectors, device: int = 0) -> np.ndarray:
         raise ValueError("queries and vectors must be [rows, bytes] arrays with the same bytes per row")
     out = np.empty((q.shape[0], x.shape[0]), np.uint32)
     check(load().lgpu_debug_hamming_gemm(_ptr(q), _ptr(x), q.shape[0], x.shape[0], q.shape[1], device, _ptr(out)))
+    return out
+
+
+def debug_pq4_sums(tables, codes, device: int = 0) -> np.ndarray:
+    """The 4-bit IVF_PQ scan kernel alone (lgpu_debug_pq4_sums): tables [B, m, 16] u8, codes [N, m/2] packed bytes ->
+    [B, N] u32 sums of tables[b][i][code_i]."""
+    t = np.ascontiguousarray(tables, np.uint8)
+    x = np.ascontiguousarray(codes, np.uint8)
+    B, m = t.shape[0], t.shape[1]
+    if t.shape[2:] != (16,) or x.ndim != 2 or 2 * x.shape[1] != m:
+        raise ValueError("tables must be [B, m, 16] and codes [N, m / 2]")
+    out = np.empty((B, x.shape[0]), np.uint32)
+    check(load().lgpu_debug_pq4_sums(_ptr(t), B, _ptr(x), x.shape[0], m, device, _ptr(out)))
     return out
 
 

@@ -130,6 +130,7 @@ struct Workspace {
     DevBuf mv_kd, mv_ki, mv_kc, mv_thr, mv_cnt, mv_cand, mv_flags, mv_vflags, mv_gate, mv_ex, mv_exid;   // shortlist
     DevBuf sq_q, sq_qq;                 // IVF_SQ search: query codes [B][dim_pad], their squared sums
     DevBuf rq_q, rq_planes, rq_slots;   // IVF_RQ search: rotated queries [B][dim], per-slot bit-planes and grids
+    DevBuf pq4_tab, pq4_slots;          // 4-bit IVF_PQ search: per-slot u8 tables [slots][m][16] and quantisers
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -283,6 +284,10 @@ struct lgpu_index {
     bool is_rq = false;
     uint32_t rq_wpr = 0;
     DevBuf rq_rot, rq_rc, rq_add, rq_scale, rq_popc;
+    // 4-bit IVF_PQ (lgpu_index_open with nbits = 4): `codes` holds per partition [m/2][npad] packed bytes, `pq4_cb` the
+    // codebook [m][dsub][16] (element-major); no filter tables
+    bool is_pq4 = false;
+    DevBuf pq4_cb;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
     WorkspacePool pool;
@@ -657,7 +662,7 @@ static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, c
 // small scan | regroup -> filter scan + fix-up | exact scan + select -> [refine], on the paths ivf_plan picks before
 // any launch ----
 enum class Coarse { exact, tc_dense, tc_list };   // see ivf_coarse
-enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq };
+enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq, pq4 };
 
 struct IvfPlan {
     uint32_t B, nprobes, slots;
@@ -672,6 +677,7 @@ struct IvfPlan {
     uint32_t rows_tile() const
     {
         if (filter()) return SCAN3_ROWS_TILE;
+        if (scan == IvfScan::pq4) return PQ4_ROWS_TILE;
         return scan == IvfScan::sq ? SQ_ROWS_TILE : (scan == IvfScan::rq ? RQ_ROWS_TILE : SCAN_ROWS_TILE_MID);
     }
 };
@@ -699,6 +705,10 @@ static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, cons
                        ? Coarse::tc_list : Coarse::tc_dense;
     // tiny batches (a single query, a micro-batch): the small path, 4 launches instead of ~25; LGPU_SMALL_SLOTS = 0
     // disables it.  Otherwise filter + verify (scan3.cu) unless the request needs every exact distance.
+    if (ix->is_pq4) {                  // 4-bit codes: one exact integer scan, never the small or the filter path
+        p.scan = IvfScan::pq4;
+        return p;
+    }
     const bool small = !ix->is_sq && !ix->is_rq && !widening && p.slots <= modes.small_slots &&
                        small_scan_smem(ix->m, ix->dim) <= 200 * 1024 &&
                        (size_t)p.slots * ix->pad_prefix[1] * 4 <= workspace_budget();
@@ -959,6 +969,26 @@ static ScanArgs scan_args(lgpu_index *ix, Workspace *ws, const float *qs, const 
     return sc;
 }
 
+// IvfScan::pq4: the per-slot u8 tables of every probe slot (after the coarse step), then the scan's arguments
+static void pq4_tables(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, cudaStream_t st)
+{
+    ws->pq4_tab.ensure((size_t)p.slots * ix->m * 16);
+    ws->pq4_slots.ensure((size_t)p.slots * sizeof(Pq4Slot));
+    launch_pq4_tables(qs, ix->centroids.as<float>(), ix->pq4_cb.as<float>(), ws->probes.as<uint64_t>(), p.slots,
+                      p.nprobes, ix->nlist, ix->m, ix->dsub, ix->metric, ws->pq4_tab.as<uint8_t>(),
+                      ws->pq4_slots.as<Pq4Slot>(), st);
+}
+
+static Pq4ScanArgs pq4_args(lgpu_index *ix, Workspace *ws, const GroupArgs &ga)
+{
+    Pq4ScanArgs a{};
+    a.codes = ix->codes.as<uint32_t>(); a.tables = ws->pq4_tab.as<uint8_t>(); a.slots = ws->pq4_slots.as<Pq4Slot>();
+    a.m = ix->m; a.metric = (uint32_t)ix->metric;
+    a.total_tiles = ga.total_tiles; a.tile_counter = ga.tile_counter; a.tile_desc = ga.tile_desc;
+    a.dist_out = ws->dist_out.as<float>();
+    return a;
+}
+
 // The filter scan's prologue on `st`: its buffers, the join with `front` (probes and regroup), the per-probe terms and
 // the 16-bit per-query tables in `sc`
 static void filter_terms(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, ScanArgs &sc, cudaStream_t st)
@@ -1089,6 +1119,8 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
         ra.total_tiles = ga.total_tiles; ra.tile_counter = ga.tile_counter; ra.tile_desc = ga.tile_desc;
         ra.dist_out = ws->dist_out.as<float>();
         launch_rq_scan(ra, 2 * ix->num_sms, st);
+    } else if (p.scan == IvfScan::pq4) {
+        launch_pq4_scan(pq4_args(ix, ws, ga), 2 * ix->num_sms, st);
     } else {
         launch_scan2(scan_args(ix, ws, qs, ga), ix->dsub, ix->num_sms, st);
     }
@@ -1136,6 +1168,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
         launch_rq_rotate(ix->rq_rot.as<float>(), qs, B, ix->dim, ws->rq_q.as<float>(), st);
         launch_rq_planes(ws->rq_q.as<float>(), ix->rq_rc.as<float>(), ws->probes.as<uint64_t>(), p.slots, nprobes,
                          ix->nlist, ix->dim, ix->rq_wpr, ws->rq_planes.as<uint32_t>(), ws->rq_slots.as<RqSlot>(), st);
+    } else if (p.scan == IvfScan::pq4) {
+        pq4_tables(ix, ws, p, qs, st);
     }
     mark(IVF_PROBES, cs);
     if (p.scan == IvfScan::small) {
@@ -1166,6 +1200,7 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
     uint32_t np_eff = std::min<uint32_t>(nprobes, ix->nlist);
     size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4);
     if (ix->is_rq) per_q += (size_t)nprobes * (16 * ix->rq_wpr + sizeof(RqSlot)) + (size_t)ix->dim * 4;  // planes, rq
+    if (ix->is_pq4) per_q += (size_t)nprobes * (16 * ix->m + sizeof(Pq4Slot));                        // u8 tables
     size_t bs = workspace_budget() / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
     bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
@@ -1207,7 +1242,7 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
         unsigned long long rows = 0;
         if (ws->stages_marked >> IVF_REGROUP & 1)
             LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
-        const uint32_t row_bytes = ix->is_sq ? ix->dim : (ix->is_rq ? ix->rq_wpr * 4 : ix->m);   // code bytes per row
+        const uint32_t row_bytes = ix->is_sq ? ix->dim : ix->is_rq ? ix->rq_wpr * 4 : ix->is_pq4 ? ix->m / 2 : ix->m;
         g_scanned_bytes = (uint64_t)rows * row_bytes;
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
         if (ws->stats_mode == 1) LGPU_CUDA(cudaMemcpy(g_filter_stats, ws->c_stats.p, 32, cudaMemcpyDeviceToHost));
@@ -1890,6 +1925,70 @@ static void upload_rq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBu
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
+// 4-bit IVF_PQ codes: per partition [m/2][npad] bytes (zero padding rows) at code_base[p] = m/2 x the npad of the
+// partitions before it.  Returns the total bytes.
+static uint64_t pq4_code_base(const uint64_t *part_offsets, uint32_t nlist, uint32_t m, std::vector<uint64_t> &code_base)
+{
+    code_base.resize(nlist);
+    uint64_t cb = 0;
+    for (uint32_t p = 0; p < nlist; p++) {
+        code_base[p] = cb;
+        cb += (uint64_t)(m / 2) * (((part_offsets[p + 1] - part_offsets[p]) + 31u) & ~31ull);
+        LGPU_REQUIRE((cb >> 3) < (1ull << 32), "index too large for one GPU shard (re-laid-out codes above 32 GiB)");
+    }
+    return cb;
+}
+
+// host codes (m/2 bytes per row, `layout`) -> dst laid out for the 4-bit scan, on the legacy stream
+static void upload_pq4_codes(const uint8_t *codes, int layout, uint64_t nrows, uint32_t m, uint32_t nlist,
+                             const uint64_t *d_part_off, const uint64_t *d_code_base, const uint32_t *d_part_npad,
+                             uint64_t total, DevBuf &dst)
+{
+    cudaStream_t st = nullptr;
+    dst.ensure(std::max<uint64_t>(total, 16));
+    LGPU_CUDA(cudaMemsetAsync(dst.p, 0, dst.bytes, st));
+    if (nrows) {
+        DevBuf tmp;
+        const size_t bytes = (size_t)nrows * (m / 2);
+        tmp.ensure(bytes);
+        LGPU_CUDA(cudaMemcpyAsync(tmp.p, codes, bytes, cudaMemcpyHostToDevice, st));
+        launch_pq4_relayout(tmp.as<uint8_t>(), layout, d_part_off, nlist, nrows, m, d_code_base, d_part_npad,
+                            dst.as<uint8_t>(), st);
+        LGPU_CUDA(cudaStreamSynchronize(st));
+    }
+    LGPU_CUDA(cudaStreamSynchronize(st));
+}
+
+// lgpu_index_open with nbits = 4 (the desc's common fields are checked): the IVF arrays, the codebook and the codes
+// re-laid out for pq4_tables / pq4_scan.  No filter tables: the scan is exact.
+static void open_pq4(const lgpu_index_desc *d, lgpu_index *&ix)
+{
+    LGPU_REQUIRE(d->m % 2 == 0, "num_sub_vectors must be even for 4-bit PQ codes");
+    LGPU_REQUIRE(d->m <= LGPU_PQ4_MAX_M, "4-bit PQ codes support num_sub_vectors up to 256");
+    std::vector<uint64_t> code_base;
+    const uint64_t total = pq4_code_base(d->part_offsets, d->nlist, d->m, code_base);
+    require_device(d->device);
+    ix = new lgpu_index();
+    ix->is_pq4 = true;
+    ix->m = d->m; ix->dsub = d->dim / d->m; ix->nch = (d->m + 7) / 8;
+    open_ivf_common(ix, d->device, d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
+                    d->vectors, PQ4_ROWS_TILE);
+    ix->code_base.ensure((size_t)d->nlist * 8);
+    LGPU_CUDA(cudaMemcpy(ix->code_base.p, code_base.data(), (size_t)d->nlist * 8, cudaMemcpyHostToDevice));
+    // codebook [m][16][dsub] -> [m][dsub][16], the layout the table kernel reads
+    const uint32_t m = d->m, dsub = ix->dsub;
+    std::vector<float> cbt((size_t)m * 16 * dsub);
+    for (uint32_t i = 0; i < m; i++)
+        for (uint32_t j = 0; j < 16; j++)
+            for (uint32_t t = 0; t < dsub; t++)
+                cbt[((size_t)i * dsub + t) * 16 + j] = d->codebook[((size_t)i * 16 + j) * dsub + t];
+    ix->pq4_cb.ensure(cbt.size() * 4);
+    LGPU_CUDA(cudaMemcpy(ix->pq4_cb.p, cbt.data(), cbt.size() * 4, cudaMemcpyHostToDevice));
+    upload_pq4_codes(d->codes, d->codes_layout, d->nrows, d->m, d->nlist, ix->part_off.as<uint64_t>(),
+                     ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(), total, ix->codes);
+    ix->device_bytes += ix->code_base.bytes + ix->pq4_cb.bytes + ix->codes.bytes;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1915,13 +2014,19 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->dim > 0 && d->nlist > 0 && d->m > 0, "dim, nlist and m must be positive");
         LGPU_REQUIRE(d->dim % d->m == 0, "num_sub_vectors must divide the vector dimension");
-        LGPU_REQUIRE(d->nbits == 8, "only 8-bit PQ codes are supported");
+        LGPU_REQUIRE(d->nbits == 8 || d->nbits == 4, "num_bits must be 4 or 8");
         LGPU_REQUIRE(d->codes_layout == LGPU_CODES_ROW_MAJOR || d->codes_layout == LGPU_CODES_PARTITION_TRANSPOSED,
                      "unknown codes layout");
         LGPU_REQUIRE(scan_dsub_supported(d->dim / d->m),
                      "unsupported PQ sub-vector length (dim/num_sub_vectors must be 1,2,4,8,16 or 32)");
         LGPU_REQUIRE(d->codebook, "null index array");
         check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
+        if (d->nbits == 4) {
+            open_pq4(d, ix);
+            register_handle(ix);
+            *out = ix;
+            return;
+        }
         const uint32_t nlist = d->nlist, nch = (d->m + 7) / 8;
         std::vector<uint64_t> code_base(nlist);
         uint64_t cb = 0;
@@ -2074,6 +2179,57 @@ int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x
         a.tile_desc = tiles.as<TileDesc>(); a.dist_out = D.as<float>(); a.out_u32 = 1;
         launch_sq_scan(a, 2 * prop.multiProcessorCount, nullptr);
         LGPU_CUDA(cudaMemcpy(out, D.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int lgpu_debug_pq4_sums(const uint8_t *tables, uint32_t B, const uint8_t *codes, uint64_t N, uint32_t m, int device,
+                        uint32_t *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(m >= 2 && m % 2 == 0 && m <= LGPU_PQ4_MAX_M, "m must be even and in [2, 256]");
+        LGPU_REQUIRE(B == 0 || N == 0 || (tables && codes && out), "null buffer");
+        LGPU_REQUIRE(N < (1ull << 31) && (uint64_t)B * ((N + 3) & ~3ull) < (1ull << 32), "B x N must stay below 2^32");
+        if (B == 0 || N == 0) return;
+        require_device(device);
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        // one partition of N rows that every query probes as its own slot: tiles of PQ4_ROWS_TILE rows x 8 slots,
+        // query b's sums at b * ld (segments padded to 4, as in a search)
+        const uint64_t off[2] = {0, N}, ld = (N + 3) & ~3ull;
+        const uint32_t npad = (uint32_t)((N + 31) & ~31ull);
+        std::vector<uint64_t> code_base;
+        const uint64_t total_bytes = pq4_code_base(off, 1, m, code_base);
+        DevBuf d_off, d_cb, d_npad, X, tab, sl, D, tiles, ctr;
+        d_off.ensure(16); d_cb.ensure(8); d_npad.ensure(4);
+        LGPU_CUDA(cudaMemcpy(d_off.p, off, 16, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(d_cb.p, code_base.data(), 8, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(d_npad.p, &npad, 4, cudaMemcpyHostToDevice));
+        upload_pq4_codes(codes, LGPU_CODES_ROW_MAJOR, N, m, 1, d_off.as<uint64_t>(), d_cb.as<uint64_t>(),
+                         d_npad.as<uint32_t>(), total_bytes, X);
+        tab.ensure((size_t)B * m * 16); sl.ensure((size_t)B * sizeof(Pq4Slot));
+        LGPU_CUDA(cudaMemcpy(tab.p, tables, (size_t)B * m * 16, cudaMemcpyHostToDevice));
+        std::vector<TileDesc> h;
+        const uint32_t nrb = scan_nrb((uint32_t)N, PQ4_ROWS_TILE), rbr = scan_rb_rows((uint32_t)N, nrb);
+        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
+            for (uint32_t rb = 0; rb < nrb; rb++) {
+                TileDesc t{};
+                t.row0 = rb * rbr; t.nrows = std::min<uint32_t>(rbr, (uint32_t)N - t.row0);
+                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N; t.npad = npad;
+                for (uint32_t g = 0; g < t.ng; g++) { t.slot[g] = q0 + g; t.q[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * ld); }
+                h.push_back(t);
+            }
+        const uint32_t total = (uint32_t)h.size(), zero[2] = {total, 0u};
+        tiles.ensure(h.size() * sizeof(TileDesc));
+        ctr.ensure(8);
+        D.ensure((size_t)B * ld * 4);
+        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(ctr.p, zero, 8, cudaMemcpyHostToDevice));
+        Pq4ScanArgs a{};
+        a.codes = X.as<uint32_t>(); a.tables = tab.as<uint8_t>(); a.slots = sl.as<Pq4Slot>(); a.m = m; a.metric = LGPU_L2;
+        a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1; a.tile_desc = tiles.as<TileDesc>();
+        a.dist_out = D.as<float>(); a.out_u32 = 1;
+        launch_pq4_scan(a, 2 * prop.multiProcessorCount, nullptr);
+        LGPU_CUDA(cudaMemcpy2D(out, (size_t)N * 4, D.p, (size_t)ld * 4, (size_t)N * 4, B, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -2775,7 +2931,7 @@ int lgpu_search_sharded(lgpu_index *ixh, lgpu_comm *ch, const float *queries, ui
     return guarded([&] {
         HandleRef<lgpu_index> ix(ixh, "index");
         HandleRef<lgpu_comm> c(ch, "communicator");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "sharded search serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq && !ix->is_pq4, "sharded search serves 8-bit IVF_PQ indexes only");
         check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -2793,7 +2949,7 @@ int lgpu_search_sharded_device(lgpu_index *ixh, lgpu_comm *ch, const float *d_qu
     return guarded([&] {
         HandleRef<lgpu_index> ix(ixh, "index");
         HandleRef<lgpu_comm> c(ch, "communicator");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "sharded search serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq && !ix->is_pq4, "sharded search serves 8-bit IVF_PQ indexes only");
         check_ivf_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -2873,7 +3029,7 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
         Workspace *ws = lease.ws; cudaStream_t st = lease.st;
         ws->q.ensure((size_t)ix->dim * 4);
         LGPU_CUDA(cudaMemcpyAsync(ws->q.p, query, (size_t)ix->dim * 4, cudaMemcpyHostToDevice, st));
-        // the one probe slot is `part`, regrouped for the exact scan (scan2.cu)
+        // the one probe slot is `part`, regrouped for the exact scan (scan2.cu, or pq4_scan.cu for 4-bit codes)
         lgpu_search_params sp{};
         sp.k = 1; sp.nprobes = 1;
         ScanModes modes = scan_modes();
@@ -2883,8 +3039,10 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
         const uint64_t forced = part;
         ws->probes.ensure(8);
         LGPU_CUDA(cudaMemcpyAsync(ws->probes.p, &forced, 8, cudaMemcpyHostToDevice, st));
+        if (p.scan == IvfScan::pq4) pq4_tables(ix.h, ws, p, qs, st);
         const GroupArgs ga = ivf_regroup(ix.h, ws, p, nullptr, st);
-        launch_scan2(scan_args(ix.h, ws, qs, ga), ix->dsub, ix->num_sms, st);
+        if (p.scan == IvfScan::pq4) launch_pq4_scan(pq4_args(ix.h, ws, ga), 2 * ix->num_sms, st);
+        else launch_scan2(scan_args(ix.h, ws, qs, ga), ix->dsub, ix->num_sms, st);
         uint32_t n = ix->h_part_n[part];
         if (n) LGPU_CUDA(cudaMemcpyAsync(out, ws->dist_out.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaStreamSynchronize(st));
@@ -2897,7 +3055,7 @@ int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, 
     return guarded([&] {
         LGPU_REQUIRE(queries && out_parts && out_L && out_W && out_E && out_bad && B > 0 && nprobes > 0, "bad argument");
         HandleRef<lgpu_index> ix(ixh, "index");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "lgpu_debug_filter_bounds serves IVF_PQ indexes only");
+        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq && !ix->is_pq4, "lgpu_debug_filter_bounds serves 8-bit IVF_PQ indexes only");
         require_device(ix->device);
         nprobes = std::min(nprobes, ix->nlist);
         LGPU_REQUIRE(ivf_sub_batch_size(ix.h, B, nprobes) == B, "batch too large for one filter-scan launch");

@@ -145,6 +145,35 @@ void launch_rq_planes(const float *rq, const float *rc, const uint64_t *probes, 
 void launch_rq_row_prep(uint32_t *codes, uint64_t n, uint32_t dim, uint32_t wpr, uint32_t *popc, cudaStream_t st);
 void launch_rq_scan(const RqScanArgs &a, int grid, cudaStream_t st);
 
+// ---------------- 4-bit IVF_PQ scan (pq4_scan.cu) ----------------------------------------
+constexpr uint32_t PQ4_ROWS_TILE = 2048;          // rows per tile: 256 threads x 2 groups of 4 rows
+struct alignas(8) Pq4Slot {                       // one probe slot's table quantiser
+    float qmin, qmax;
+};
+struct Pq4ScanArgs {
+    const uint32_t *codes;        // per partition [m/2][npad] packed code bytes at byte code_base[p] (launch_pq4_relayout)
+    const uint8_t *tables;        // [slots][m][16] u8 tables (launch_pq4_tables)
+    const Pq4Slot *slots;         // [slots]
+    uint32_t m, metric;
+    const uint32_t *total_tiles;  // [1]
+    uint32_t *tile_counter;       // [1], zeroed before launch
+    const TileDesc *tile_desc;    // built with rows_tile == PQ4_ROWS_TILE; slot[] addresses tables / slots
+    float *dist_out;              // segment of slot e at out[e]: the distance of row r at out[e] + r (padded to 4 floats)
+    int out_u32;                  // 1: write the exact u32 sums S instead (lgpu_debug_pq4_sums)
+};
+// dynamic shared memory of the scan kernel for m sub-vectors
+size_t pq4_scan_smem(uint32_t m);
+// per probe slot e (query e / nprobes, partition probes[e]; slots without a partition are skipped): the u8 tables
+// [e][m][16] and slot_out[e]; codebook [m][dsub][16] (element-major: element t of codeword j of sub-space i at
+// (i dsub + t) 16 + j)
+void launch_pq4_tables(const float *Q, const float *centroids, const float *codebook, const uint64_t *probes,
+                       uint32_t slots, uint32_t nprobes, uint32_t nlist, uint32_t m, uint32_t dsub, int metric,
+                       uint8_t *tables, Pq4Slot *slot_out, cudaStream_t st);
+void launch_pq4_scan(const Pq4ScanArgs &a, int grid, cudaStream_t st);
+// codes (layout: lgpu_codes_layout, m/2 bytes per row) -> out, per partition [m/2][part_npad[p]] at code_base[p]
+void launch_pq4_relayout(const uint8_t *codes, int layout, const uint64_t *part_off, uint32_t nlist, uint64_t nrows,
+                         uint32_t m, const uint64_t *code_base, const uint32_t *part_npad, uint8_t *out, cudaStream_t st);
+
 // ---------------- tiny batches: one CTA per (query, probed partition) pair (small.cu) ----------------
 struct SmallScanArgs {
     const float *centroids; const float *cb_tiled; const unsigned char *codes; const uint64_t *code_base;

@@ -8,8 +8,8 @@ transposed PQ codes and row ids.  The same arrays are handed to the C-ABI
 
 `train_ivf_pq` mirrors the *parameters* of `Index::IvfPq`
 (rust/lancedb/src/index/vector.rs:266-319, rust/lancedb/src/table/create_index.rs:68-102,
-283-303): num_partitions, num_sub_vectors (default dim/16, else dim/8, else 1),
-num_bits = 8, sample_rate = 256, max_iterations = 50, distance_type.  Training itself
+283-303): num_partitions, num_sub_vectors (default dim/16, else dim/8, else 1; rounded up to
+even for 4 bits), num_bits = 8 or 4, sample_rate = 256, max_iterations = 50, distance_type.  Training itself
 lives in the un-vendored lance crate; this is a plain k-means / PQ trainer written with
 torch ops (CPU or CUDA), or, with `native_passes` (the `accelerator="cuda"` build), the library's own
 training kernels (csrc/kmeans.cu) -- index *quality* is not on the hot path, and both the CUDA
@@ -34,6 +34,18 @@ def suggested_num_sub_vectors(dim: int) -> int:
     return 1
 
 
+def get_num_sub_vectors(provided: Optional[int], dim: int, num_bits: Optional[int]) -> int:
+    """rust/lancedb/src/table/create_index.rs:86-102: the explicit value, else suggested_num_sub_vectors(dim) rounded up
+    to an even number for 4-bit codes (two codes share a byte)."""
+    if provided is not None:
+        return int(provided)
+    s = suggested_num_sub_vectors(dim)
+    return s + 1 if num_bits == 4 and s % 2 else s
+
+
+PQ4_MAX_M = 256             # LGPU_PQ4_MAX_M: a probe slot's quantised sum stays below 2^16
+
+
 def suggested_num_partitions(num_rows: int, target_partition_size: int = 8192) -> int:
     """Default IVF sizing: 16384 rows => 2 partitions
     (rust/lancedb/src/table/create_index.rs:734-795)."""
@@ -47,11 +59,12 @@ class IvfPqIndexData:
     m: int
     metric: str
     centroids: np.ndarray      # f32 [nlist, dim]
-    codebook: np.ndarray       # f32 [m, 256, dim/m]
+    codebook: np.ndarray       # f32 [m, 2**num_bits, dim/m]
     part_offsets: np.ndarray   # u64 [nlist+1]
-    codes_t: np.ndarray        # u8 flat; partition p at [off[p]*m, off[p+1]*m) as [m][n_p]
+    codes_t: np.ndarray        # u8 flat; partition p at [off[p]*w, off[p+1]*w) as [w][n_p], w = code_bytes
     row_ids: np.ndarray        # u64 [n] in partition order
     vectors: Optional[np.ndarray] = None   # f32 [n, dim] partition order (refine), optional
+    num_bits: int = 8          # 8: one code per byte; 4: byte j holds sub-vector 2j (bits 0-3) and 2j+1 (bits 4-7)
 
     @property
     def nrows(self) -> int:
@@ -61,19 +74,29 @@ class IvfPqIndexData:
     def dsub(self) -> int:
         return self.dim // self.m
 
+    @property
+    def code_bytes(self) -> int:
+        """Bytes of one row's codes: m (8-bit) or m / 2 (4-bit)."""
+        return self.m if self.num_bits == 8 else self.m // 2
+
     def validate(self) -> None:
         assert self.metric in METRICS
+        assert self.num_bits in (4, 8)
         assert self.dim % self.m == 0
+        if self.num_bits == 4:
+            assert self.m % 2 == 0 and self.m <= PQ4_MAX_M
         assert self.centroids.shape == (self.nlist, self.dim) and self.centroids.dtype == np.float32
-        assert self.codebook.shape == (self.m, 256, self.dsub) and self.codebook.dtype == np.float32
+        assert self.codebook.shape == (self.m, 1 << self.num_bits, self.dsub) and self.codebook.dtype == np.float32
         assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
         assert int(self.part_offsets[-1]) == self.nrows
-        assert self.codes_t.dtype == np.uint8 and self.codes_t.size == self.nrows * self.m
+        assert self.codes_t.dtype == np.uint8 and self.codes_t.size == self.nrows * self.code_bytes
         assert self.row_ids.dtype == np.uint64
 
     def partition_codes(self, p: int) -> np.ndarray:
+        """[code_bytes, n_p] code bytes of partition p."""
         a, b = int(self.part_offsets[p]), int(self.part_offsets[p + 1])
-        return self.codes_t[a * self.m:b * self.m].reshape(self.m, b - a)
+        w = self.code_bytes
+        return self.codes_t[a * w:b * w].reshape(w, b - a)
 
     def shard(self, rank: int, world: int) -> "IvfPqIndexData":
         """Partition-sharded view for multi-GPU search (SURVEY.md 8e): centroids and
@@ -88,7 +111,7 @@ class IvfPqIndexData:
         codes, rids, vecs = [], [], []
         for p in np.nonzero(keep)[0]:
             a, b = int(self.part_offsets[p]), int(self.part_offsets[p + 1])
-            codes.append(self.codes_t[a * self.m:b * self.m])
+            codes.append(self.codes_t[a * self.code_bytes:b * self.code_bytes])
             rids.append(self.row_ids[a:b])
             if self.vectors is not None:
                 vecs.append(self.vectors[a:b])
@@ -96,7 +119,7 @@ class IvfPqIndexData:
         return IvfPqIndexData(
             self.dim, self.nlist, self.m, self.metric, self.centroids, self.codebook, new_off,
             cat(codes, np.uint8, (0,)), cat(rids, np.uint64, (0,)),
-            cat(vecs, np.float32, (0, self.dim)) if self.vectors is not None else None)
+            cat(vecs, np.float32, (0, self.dim)) if self.vectors is not None else None, self.num_bits)
 
 
 def assign_partitions(sizes: np.ndarray, world: int) -> np.ndarray:
@@ -212,7 +235,7 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
                  distance_type: str = "l2", sample_rate: int = 256, max_iterations: int = 50,
                  row_ids: Optional[np.ndarray] = None, keep_vectors: bool = False, seed: int = 45,
                  device: Optional[str] = None, encode_chunk: int = 1 << 16,
-                 native_passes: bool = False) -> IvfPqIndexData:
+                 native_passes: bool = False, num_bits: int = 8) -> IvfPqIndexData:
     """Train IVF centroids + residual PQ codebooks and encode every row.
 
     vectors: [n, dim] float32 (numpy or torch).  Returns the plain-array index.
@@ -221,11 +244,17 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
     always lands in the partition its own vector probes first -- instead of torch's GEMM-form argmin.
     With native_passes the k-means training loops run in the library too (`lgpu_kmeans_train` / `lgpu_pq_train`,
     csrc/kmeans.cu); otherwise they are torch ops.
+    num_bits = 4: 16-codeword codebooks and packed codes (byte j = code 2j | code 2j+1 << 4).  num_sub_vectors defaults
+    to get_num_sub_vectors (even) and must be even.  The IVF passes follow native_passes as above; the PQ passes are
+    torch ops on the training device either way (`lgpu_pq_train` / `lgpu_pq_encode` are 256-codeword kernels): k-means
+    codebooks, and each code the argmin of |c|^2 - 2 r.c, ties to the lowest code.
     """
     import torch
     metric = distance_type.lower()
     if metric not in METRICS:
         raise ValueError(f"unknown distance_type {distance_type!r}")
+    if num_bits not in (4, 8):
+        raise ValueError(f"IVF_PQ supports num_bits 4 or 8, got num_bits={num_bits}")
     x = torch.as_tensor(vectors, dtype=torch.float32)
     if device is not None:
         x = x.to(device)
@@ -237,19 +266,22 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
             return train_ivf_pq(x, num_partitions=num_partitions, num_sub_vectors=num_sub_vectors,
                                 distance_type=distance_type, sample_rate=sample_rate, max_iterations=max_iterations,
                                 row_ids=row_ids, keep_vectors=keep_vectors, seed=seed, device=None,
-                                encode_chunk=encode_chunk, native_passes=native_passes)
+                                encode_chunk=encode_chunk, native_passes=native_passes, num_bits=num_bits)
         finally:
             torch.set_num_threads(prev)
     n, dim = x.shape
     nlist = int(num_partitions or suggested_num_partitions(n))
-    m = int(num_sub_vectors or suggested_num_sub_vectors(dim))
+    m = get_num_sub_vectors(num_sub_vectors or None, dim, num_bits)
     if dim % m:
         raise ValueError(f"num_sub_vectors {m} does not divide dimension {dim}")
+    if num_bits == 4 and (m % 2 or m > PQ4_MAX_M):
+        raise ValueError(f"4-bit PQ needs an even num_sub_vectors <= {PQ4_MAX_M}, got {m}")
     dsub = dim // m
     gen = torch.Generator(device="cpu").manual_seed(seed)
     raw = x
     x, samp, centroids, assign, dev_index = _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes)
-    if native_passes:
+    pq_native = native_passes and num_bits == 8       # the library's PQ kernels are 256-codeword
+    if pq_native:
         from . import _native
         raw_np = raw.detach().cpu().numpy()
 
@@ -257,7 +289,7 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
     nps = min(n, max(256, sample_rate) * 256)
     pidx = torch.randperm(n, generator=gen, device="cpu")[:nps].to(x.device)
     ps = x[pidx] - centroids[assign[pidx]] if metric != "dot" else x[pidx]
-    if native_passes:
+    if pq_native:
         init_cb = torch.stack([ps[torch.randperm(nps, generator=gen, device="cpu")[:256].to(x.device) if nps >= 256
                                   else torch.randint(0, nps, (256,), generator=gen, device="cpu").to(x.device)]
                                .reshape(256, m, dsub)[:, i, :] for i in range(m)])              # [m, 256, dsub]
@@ -265,15 +297,15 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
                                                     dev_index), device=x.device)
     else:
         ps3 = ps.reshape(nps, m, dsub).transpose(0, 1).contiguous()      # [m, nps, dsub]
-        codebook = _batched_kmeans(ps3, 256, max_iterations, gen)        # [m, 256, dsub]
+        codebook = _batched_kmeans(ps3, 1 << num_bits, max_iterations, gen)   # [m, 2**num_bits, dsub]
 
     cbn = (codebook * codebook).sum(2)                                     # [m, 256]
     codes = torch.empty((n, m), dtype=torch.uint8, device=x.device)
-    if native_passes:
+    if pq_native:
         codes = torch.as_tensor(_native.pq_encode(centroids.cpu().numpy(), codebook.cpu().numpy(), raw_np,
                                                   assign.cpu().numpy().astype(np.uint32), metric, dev_index),
                                 device=x.device)
-    for s in range(0, n if not native_passes else 0, encode_chunk):
+    for s in range(0, n if not pq_native else 0, encode_chunk):
         xs = x[s:s + encode_chunk]
         r = xs - centroids[assign[s:s + encode_chunk]] if metric != "dot" else xs
         r = r.reshape(-1, m, dsub).transpose(0, 1)                         # [m, c, dsub]
@@ -285,11 +317,14 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
     part_offsets = np.zeros(nlist + 1, np.uint64)
     part_offsets[1:] = np.cumsum(sizes)
     codes_sorted = codes[order].cpu().numpy()                              # [n, m] partition order
-    codes_t = np.empty(n * m, np.uint8)
+    if num_bits == 4:
+        codes_sorted = pack_pq4(codes_sorted)                              # [n, m/2]
+    w = codes_sorted.shape[1]
+    codes_t = np.empty(n * w, np.uint8)
     for p in range(nlist):
         a, b = int(part_offsets[p]), int(part_offsets[p + 1])
         if b > a:
-            codes_t[a * m:b * m] = codes_sorted[a:b].T.reshape(-1)
+            codes_t[a * w:b * w] = codes_sorted[a:b].T.reshape(-1)
     order_np = order.cpu().numpy()
     rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
     data = IvfPqIndexData(
@@ -297,9 +332,26 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
         centroids=centroids.cpu().numpy().astype(np.float32),
         codebook=codebook.cpu().numpy().astype(np.float32),
         part_offsets=part_offsets, codes_t=codes_t, row_ids=rid[order_np],
-        vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
+        vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None), num_bits=num_bits)
     data.validate()
     return data
+
+
+def pack_pq4(codes) -> np.ndarray:
+    """[n, m] 4-bit codes (m even) -> [n, m/2] bytes, byte j = code 2j | code 2j+1 << 4 (lance's packing, recalled)."""
+    c = np.asarray(codes, np.uint8)
+    if c.shape[-1] % 2 or (c.size and int(c.max()) > 15):
+        raise ValueError("4-bit codes need an even number of sub-vectors and values below 16")
+    return (c[..., 0::2] | (c[..., 1::2] << 4)).astype(np.uint8)
+
+
+def unpack_pq4(packed) -> np.ndarray:
+    """The inverse of pack_pq4: [n, m/2] bytes -> [n, m] codes."""
+    b = np.asarray(packed, np.uint8)
+    out = np.empty(b.shape[:-1] + (2 * b.shape[-1],), np.uint8)
+    out[..., 0::2] = b & 15
+    out[..., 1::2] = b >> 4
+    return out
 
 
 # --------------------------------------------------------------------------------------

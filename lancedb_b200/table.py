@@ -162,7 +162,9 @@ class Table:
             # RaBitQ with 1 bit per dimension only (extended RaBitQ is not served); the legacy default of 8 is refused
             # rather than quietly building a 1-bit index
             raise ValueError(f"IVF_RQ supports num_bits=1 only, got num_bits={num_bits}")
-        if kind != "IVF_RQ" and num_bits != 8:
+        if kind == "IVF_PQ" and num_bits not in (4, 8):
+            raise ValueError(f"IVF_PQ supports num_bits 4 or 8, got num_bits={num_bits}")
+        if kind == "IVF_SQ" and num_bits != 8:
             raise ValueError("only num_bits=8 is supported")
         column = vector_column_name or self._infer_vector_column(None)
         if self._is_binary(column):
@@ -193,7 +195,7 @@ class Table:
         data = train_ivf_pq(self._vectors(column), num_partitions=num_partitions,
                             num_sub_vectors=num_sub_vectors, distance_type=metric,
                             max_iterations=max_iterations, sample_rate=sample_rate,
-                            keep_vectors=True, device=dev,
+                            keep_vectors=True, device=dev, num_bits=num_bits,
                             native_passes=dev is not None)      # accelerator: row passes through the C ABI (build.cu)
         self._attach_index(column, data)
 
@@ -225,6 +227,8 @@ class Table:
         column = vector_column_name or self._infer_vector_column(None)
         if self._index_type(column) != "IVF_PQ":
             raise NotImplementedError("only IVF_PQ indexes are written as Lance index files")
+        if self._index_data[column].num_bits != 8:
+            raise NotImplementedError("only 8-bit IVF_PQ indexes are written as Lance index files")
         write_ivf_pq_index(index_dir, self._index_data[column], transposed=transposed)
 
     def prewarm_index(self, name: str):           # rust/lancedb/src/table.rs:3283-3286
