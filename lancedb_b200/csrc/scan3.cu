@@ -53,7 +53,8 @@ constexpr int S3_BUF = 32768;                       // one chunk buffer
 constexpr int S3_SLOTS = 4, S3_SLOT_BYTES = 128;    // tile-descriptor ring
 constexpr size_t S3_TILES = 3 * (size_t)S3_BUF;
 constexpr int S3_SCR = 32;                          // words per bank of threshold scratch
-constexpr size_t S3_SMEM = S3_TILES + S3_SLOTS * S3_SLOT_BYTES + 2 * S3_SCR * 4 + 32;   // + two banks of threshold scratch + mbarriers
+// + two banks of threshold scratch + mbarriers + the candidate epilogue's per-query scalars
+constexpr size_t S3_SMEM = S3_TILES + S3_SLOTS * S3_SLOT_BYTES + 2 * S3_SCR * 4 + 32 + SCAN_G * 16;
 constexpr int S3_LIST_PER = CAND_CAP_MAX / S3_CT;  // list keys per scanner thread in a list-based tightening
 constexpr int S3_LIST_STEPS = 10;
 constexpr int BAR_SCAN = 8;                         // named barrier of the 256 scanner threads (candidate mode)
@@ -66,6 +67,8 @@ constexpr int BAR_SCAN = 8;                         // named barrier of the 256 
 #define LGPU_S3_NAMED_FULL 0
 #endif
 constexpr size_t S3_MBAR_OFF = S3_TILES + S3_SLOTS * S3_SLOT_BYTES + 2 * S3_SCR * 4;   // 3 x 8 bytes, 8-byte aligned
+constexpr size_t S3_QS_OFF = S3_MBAR_OFF + 32;     // [SCAN_G][step, cst, slack, -] f32
+static_assert(S3_QS_OFF + SCAN_G * 16 == S3_SMEM, "shared-memory layout");
 static_assert(SCAN3_ROWS_TILE == S3_CT * S3_RMAX, "rows_tile");
 static_assert(S3_PT == 256, "one stager thread per code");
 
@@ -343,6 +346,20 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
     // every warp then appends the rows under the threshold.
     const int lane = ct & 31;
     const uint32_t k = a.topk;
+    // The queries' scalars (step, base + A, slack) are loaded here for all of the tile's queries at once, beside the
+    // row terms above, and read back from shared memory after each query's first barrier.  The epilogue runs its queries
+    // one after the other behind scanner barriers, so a load inside the query loop would add one L2 round trip per
+    // query that every scanner warp waits for, after the one for the threshold.  The slots are rewritten by the next tile's
+    // epilogue only: every read of query g is before the second barrier of iteration g, and no thread passes the
+    // last such barrier before all have read.
+    float *const qsc = reinterpret_cast<float *>(smem + S3_QS_OFF);
+    if (ct >= 32 && ct < 32 + ng) {
+        const int g = ct - 32;
+        const uint32_t q = T->q[g];
+        qsc[4 * g + 0] = __ldg(a.qt_step + q);
+        qsc[4 * g + 1] = __ldg(a.qt_base + q) + (a.probe_A ? __ldg(a.probe_A + T->slot[g]) : 0.f);
+        qsc[4 * g + 2] = __ldg(a.slack + q);
+    }
     // scratch, two banks alternating by query so that the reset for query g+1 cannot overtake a slow warp still
     // reading query g's counters: [0] threshold key, [1] min key, [2] max key, [3] valid rows, [4..12] counters of the
     // tile bisection; [13] list length, [14] list length at the last list tightening, [15] smallest list key,
@@ -372,9 +389,7 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
             if (tkey != CAND_NO_THR && ln >= 2u * k && ln >= last + k)
                 tkey = tighten_from_list(a.cand_key + (size_t)q * a.cand_cap, a.thr + q, a.cand_last + q, sh, ln, tkey, k, ct);
         }
-        const float step = __ldg(a.qt_step + q);
-        const float cst = __ldg(a.qt_base + q) + (a.probe_A ? __ldg(a.probe_A + slot) : 0.f);
-        const float slack = __ldg(a.slack + q);
+        const float step = qsc[4 * g + 0], cst = qsc[4 * g + 1], slack = qsc[4 * g + 2];
         float L[R];
         uint32_t nvalid = 0, kmin = 0xffffffffu, kmax = 0u;
 #pragma unroll
