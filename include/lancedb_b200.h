@@ -62,6 +62,7 @@ typedef struct lgpu_index lgpu_index;   /* an IVF_PQ index resident in HBM */
 typedef struct lgpu_flat lgpu_flat;     /* a raw vector column resident in HBM */
 typedef struct lgpu_binary lgpu_binary; /* a packed binary (uint8) vector column in HBM, searched by Hamming distance */
 typedef struct lgpu_multivec lgpu_multivec; /* a multivector column in HBM, searched by late interaction (MaxSim) */
+typedef struct lgpu_ivf_binary lgpu_ivf_binary; /* a binary IVF_FLAT index in HBM, searched by Hamming distance */
 
 /* The arrays of one IVF_PQ index (lance v2 `IvfPq`,
  * rust/lancedb/src/table/create_index.rs:283-303, :772): IVF centroids, PQ codebook
@@ -348,6 +349,37 @@ int  lgpu_binary_search_filtered(lgpu_binary *bx, const uint8_t *queries, uint32
 int  lgpu_binary_search_device(lgpu_binary *bx, const uint8_t *d_queries, uint32_t B, const lgpu_search_params *params,
                                uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
 
+/* ---- binary IVF_FLAT (lance `IvfFlat` with distance_type("hamming"), the index LanceDB builds over
+ * fixed_size_list<uint8, nbytes> columns; rust/lancedb/src/index/vector.rs:169-209): packed binary centroids and the
+ * rows grouped by partition.  Search, per query: the nprobes partitions whose centroids are nearest by Hamming distance
+ * (ties to the lower partition id; every partition when nprobes >= nlist), then every row of those partitions scored
+ * exactly, _distance = popcount(q XOR x) as f32, ascending by (_distance, _rowid).  k, nprobes, maximum_nprobes (under
+ * a prefilter), prefilter, distance_range (before the top-k) and timeout_ms behave as on lgpu_index; refine_factor is
+ * accepted and changes nothing (the distances are exact; k x refine_factor is not limited).  With nprobes >= nlist the
+ * result is lgpu_binary_search's.  nprobes above 2048 must cover every partition, and so must maximum_nprobes above
+ * 2048 when it widens (under a prefilter).  queries: [B][nbytes]. */
+typedef struct {
+    uint32_t abi_version;         /* LGPU_ABI_VERSION */
+    uint32_t nbytes;              /* bytes per vector, 8 nbytes <= 2^24 */
+    uint32_t nlist;
+    int32_t  device;
+    uint64_t nrows;
+    const uint8_t  *centroids;    /* [nlist][nbytes] packed bits */
+    const uint64_t *part_offsets; /* [nlist+1] */
+    const uint8_t  *vectors;      /* [nrows][nbytes] in partition order */
+    const uint64_t *row_ids;      /* [nrows] */
+} lgpu_ivf_binary_desc;
+int  lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *desc, lgpu_ivf_binary **out);
+void lgpu_ivf_binary_close(lgpu_ivf_binary *ix);
+int  lgpu_ivf_binary_search(lgpu_ivf_binary *ix, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
+                            uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+int  lgpu_ivf_binary_search_filtered(lgpu_ivf_binary *ix, const uint8_t *queries, uint32_t B,
+                                     const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                                     uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+int  lgpu_ivf_binary_search_device(lgpu_ivf_binary *ix, const uint8_t *d_queries, uint32_t B,
+                                   const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
+                                   uint32_t *d_out_count, void *cuda_stream);
+
 /* ---- multivector columns: exact late-interaction (MaxSim) flat search (the `DataType::List` branch of
  * rust/lancedb/src/table/query.rs:180-199: list<fixed_size_list<float, dim>> columns; the query's vectors are packed
  * into ONE query, python/python/lancedb/query.py:3376-3382) ----
@@ -407,6 +439,11 @@ int lgpu_debug_gemm(const float *queries, const float *vectors, uint32_t B, uint
  * queries [B][nbytes], vectors [N][nbytes], out [B][N] u32) */
 int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint32_t B, uint64_t N, uint32_t nbytes,
                             int device, uint32_t *out);
+/* the binary IVF_FLAT scan kernel alone, every query one probe slot over one partition of N rows: out[q][x] = Hamming
+ * distance of queries[q] and vectors[x] (host buffers: queries [B][nbytes], vectors [N][nbytes], out [B][N] u32;
+ * B x N < 2^32) */
+int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_t *vectors, uint64_t N, uint32_t nbytes,
+                                int device, uint32_t *out);
 /* the IVF_SQ scan kernel alone, on one partition of the N rows that every query probes: out[q][x] = sum_i
  * (x_codes[x][i] - q_codes[q][i])^2, the exact u32 sum (host buffers: q_codes [B][dim], x_codes [N][dim], out [B][N];
  * dim <= 65536, B x N < 2^32) */

@@ -39,6 +39,8 @@ EXPORTS = [
     "lgpu_ivf_sq_open", "lgpu_debug_sq_distances",
     "lgpu_ivf_rq_open", "lgpu_debug_rq_distances",
     "lgpu_debug_pq4_sums",
+    "lgpu_ivf_binary_open", "lgpu_ivf_binary_close", "lgpu_ivf_binary_search", "lgpu_ivf_binary_search_filtered",
+    "lgpu_ivf_binary_search_device", "lgpu_debug_ivf_hamming_scan",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -72,6 +74,15 @@ class RqDesc(C.Structure):
         ("device", C.c_int32), ("num_bits", C.c_uint32), ("nrows", C.c_uint64),
         ("centroids", C.c_void_p), ("rotation", C.c_void_p), ("part_offsets", C.c_void_p), ("codes", C.c_void_p),
         ("add_factors", C.c_void_p), ("scale_factors", C.c_void_p), ("row_ids", C.c_void_p), ("vectors", C.c_void_p),
+    ]
+
+
+class IvfBinaryDesc(C.Structure):
+    """lgpu_ivf_binary_desc"""
+    _fields_ = [
+        ("abi_version", C.c_uint32), ("nbytes", C.c_uint32), ("nlist", C.c_uint32), ("device", C.c_int32),
+        ("nrows", C.c_uint64), ("centroids", C.c_void_p), ("part_offsets", C.c_void_p), ("vectors", C.c_void_p),
+        ("row_ids", C.c_void_p),
     ]
 
 
@@ -163,6 +174,13 @@ def load():
     lib.lgpu_ivf_rq_open.argtypes = [C.POINTER(RqDesc), C.POINTER(vp)]
     lib.lgpu_debug_rq_distances.argtypes = [vp, u32, vp, vp, vp, C.c_uint64, u32, i32, i32, vp, vp]
     lib.lgpu_debug_pq4_sums.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
+    lib.lgpu_ivf_binary_open.argtypes = [C.POINTER(IvfBinaryDesc), C.POINTER(vp)]
+    lib.lgpu_ivf_binary_close.argtypes = [vp]
+    lib.lgpu_ivf_binary_close.restype = None
+    lib.lgpu_ivf_binary_search.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
+    lib.lgpu_ivf_binary_search_filtered.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
+    lib.lgpu_ivf_binary_search_device.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
+    lib.lgpu_debug_ivf_hamming_scan.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -462,6 +480,44 @@ class GpuBinary(_Handle):
         check(load().lgpu_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
 
 
+class GpuIvfBinary(_Handle):
+    """A binary IVF_FLAT index (IvfBinaryIndexData) pinned in HBM (lgpu_ivf_binary): the probed partitions of packed
+    binary rows scored exactly by Hamming distance."""
+    _close = "lgpu_ivf_binary_close"
+
+    def __init__(self, data, device: int = 0):
+        lib = load()
+        data.validate()
+        self.nbytes, self.nlist, self.metric = data.nbytes, data.nlist, data.metric
+        self.device = device
+        self._keep = [np.ascontiguousarray(data.centroids, np.uint8), np.ascontiguousarray(data.part_offsets, np.uint64),
+                      np.ascontiguousarray(data.vectors, np.uint8), np.ascontiguousarray(data.row_ids, np.uint64)]
+        desc = IvfBinaryDesc(ABI_VERSION, data.nbytes, data.nlist, device, data.nrows, *[_ptr(a) for a in self._keep])
+        h = C.c_void_p()
+        check(lib.lgpu_ivf_binary_open(C.byref(desc), C.byref(h)))
+        self._h = h
+        self._keep = None
+
+    def _queries(self, queries) -> np.ndarray:
+        a = np.asarray(queries)
+        if a.ndim not in (1, 2) or a.shape[-1] != self.nbytes:
+            raise ValueError(f"binary queries must be [B, {self.nbytes}] or [{self.nbytes}], got shape {a.shape}")
+        return binary_components(a).reshape(-1, self.nbytes)
+
+    def search(self, queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None, allow=None, allow_bits=0,
+               max_nprobes=0, timeout_ms=0):
+        """Host-buffer search of queries [B, nbytes] (or one [nbytes] query): returns (ids [B,k] u64, dist [B,k] f32,
+        count [B] u32).  refine_factor is accepted and changes nothing: the distances are exact."""
+        q = self._queries(queries)
+        p = make_params(k, nprobes, refine_factor, lower, upper, max_nprobes, timeout_ms)
+        return _host_search("lgpu_ivf_binary_search", (self._h, _ptr(q), q.shape[0]), q.shape[0], k, p, allow,
+                            allow_bits)
+
+    def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
+        """Device-pointer search (raw addresses; queries [B][nbytes] u8), enqueued on `stream`, not synchronised."""
+        check(load().lgpu_ivf_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
+
+
 def multivec_offsets(lengths) -> np.ndarray:
     """Vector counts per row (or per query) -> the [n+1] offsets the multivector entry points take."""
     n = np.asarray(lengths, np.int64).reshape(-1)
@@ -667,6 +723,17 @@ def debug_hamming_gemm(queries, vectors, device: int = 0) -> np.ndarray:
         raise ValueError("queries and vectors must be [rows, bytes] arrays with the same bytes per row")
     out = np.empty((q.shape[0], x.shape[0]), np.uint32)
     check(load().lgpu_debug_hamming_gemm(_ptr(q), _ptr(x), q.shape[0], x.shape[0], q.shape[1], device, _ptr(out)))
+    return out
+
+
+def debug_ivf_hamming_scan(queries, vectors, device: int = 0) -> np.ndarray:
+    """The binary IVF_FLAT scan kernel alone (lgpu_debug_ivf_hamming_scan), every query one probe slot over one partition
+    holding the N rows: [B, N] u32 Hamming distances."""
+    q = np.ascontiguousarray(queries, np.uint8); x = np.ascontiguousarray(vectors, np.uint8)
+    if q.ndim != 2 or x.ndim != 2 or q.shape[1] != x.shape[1]:
+        raise ValueError("queries and vectors must be [rows, bytes] arrays with the same bytes per row")
+    out = np.empty((q.shape[0], x.shape[0]), np.uint32)
+    check(load().lgpu_debug_ivf_hamming_scan(_ptr(q), q.shape[0], _ptr(x), x.shape[0], q.shape[1], device, _ptr(out)))
     return out
 
 

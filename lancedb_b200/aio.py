@@ -45,6 +45,17 @@ class IvfRq:
     sample_rate: int = 256
 
 
+@dataclass
+class IvfFlat:
+    """Index.IvfFlat parameters (rust/lancedb/src/index/vector.rs:169-209): served over binary (fixed_size_list<uint8>)
+    columns with distance_type="hamming"; the default "l2", like any other metric there, is refused (ValueError), and a
+    float column raises NotImplementedError."""
+    distance_type: str = "l2"
+    num_partitions: Optional[int] = None
+    max_iterations: int = 50
+    sample_rate: int = 256
+
+
 class AsyncRecordBatchReader:
     """What `to_batches` resolves to: `async for batch in reader`, `await reader.read_all()`."""
 
@@ -260,15 +271,15 @@ class AsyncTable:
     async def list_indices(self):
         return self._table.list_indices()
 
-    async def create_index(self, column: str, *, config: Optional[Union[IvfPq, IvfRq]] = None, replace: bool = True,
-                           accelerator: Optional[str] = "cuda"):
+    async def create_index(self, column: str, *, config: Optional[Union[IvfPq, IvfRq, IvfFlat]] = None,
+                           replace: bool = True, accelerator: Optional[str] = "cuda"):
         cfg = config or IvfPq()
-        kind = "IVF_RQ" if isinstance(cfg, IvfRq) else "IVF_PQ"
+        kind = "IVF_RQ" if isinstance(cfg, IvfRq) else ("IVF_FLAT" if isinstance(cfg, IvfFlat) else "IVF_PQ")
         await asyncio.to_thread(
             self._table.create_index, metric=cfg.distance_type, num_partitions=cfg.num_partitions,
             num_sub_vectors=getattr(cfg, "num_sub_vectors", None), vector_column_name=column, replace=replace,
-            accelerator=accelerator, index_type=kind, num_bits=cfg.num_bits, max_iterations=cfg.max_iterations,
-            sample_rate=cfg.sample_rate)
+            accelerator=accelerator, index_type=kind, num_bits=getattr(cfg, "num_bits", 8),
+            max_iterations=cfg.max_iterations, sample_rate=cfg.sample_rate)
 
     async def prewarm_index(self, name: str):
         return self._table.prewarm_index(name)

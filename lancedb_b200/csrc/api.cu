@@ -293,6 +293,14 @@ struct lgpu_index {
     WorkspacePool pool;
 };
 
+// a binary IVF_FLAT index (lgpu_ivf_binary_open): the IVF partition arrays of lgpu_index (part_n, part_off, row_ids,
+// pad_prefix, ...; `dim` = nbytes), with `centroids` holding the packed centroids [nlist][nbytes_pad] and `codes` the
+// packed rows [nrows][nbytes_pad] in partition order, both zero-padded, and their popcounts
+struct lgpu_ivf_binary : lgpu_index {
+    uint32_t nbytes = 0, nbytes_pad = 0;
+    DevBuf cent_pop, row_pop;
+};
+
 struct lgpu_flat {
     std::atomic<int> refs{0};
     int device = 0;
@@ -646,14 +654,15 @@ static void select_dense(const float *D, uint64_t N, uint64_t ld, const uint64_t
     launch_select(sa, st);
 }
 
-// the arguments every search call takes: the parameters, then the query and output buffers of a call with queries
+// the arguments every search call takes: the parameters, then the query and output buffers of a call with queries.
+// refine: the kind selects k * refine_factor candidates (a kind whose distances are exact ignores refine_factor)
 static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, const void *ids, const void *dist,
-                       const void *cnt)
+                       const void *cnt, bool refine = true)
 {
     LGPU_REQUIRE(p != nullptr, "search params are null");
     LGPU_REQUIRE(p->k >= 1, "limit must be greater than 0");
     LGPU_REQUIRE(p->k <= SELECT_KMAX, "limit+offset above 2048 is not supported on the GPU path");
-    if (p->refine_factor)
+    if (refine && p->refine_factor)
         LGPU_REQUIRE((uint64_t)p->k * p->refine_factor <= SELECT_KMAX, "limit*refine_factor above 2048 is not supported");
     LGPU_REQUIRE(B == 0 || (q && ids && dist && cnt), "null buffer");
 }
@@ -662,7 +671,7 @@ static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, c
 // small scan | regroup -> filter scan + fix-up | exact scan + select -> [refine], on the paths ivf_plan picks before
 // any launch ----
 enum class Coarse { exact, tc_dense, tc_list };   // see ivf_coarse
-enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq, pq4 };
+enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq, pq4, ham };
 
 struct IvfPlan {
     uint32_t B, nprobes, slots;
@@ -678,6 +687,7 @@ struct IvfPlan {
     {
         if (filter()) return SCAN3_ROWS_TILE;
         if (scan == IvfScan::pq4) return PQ4_ROWS_TILE;
+        if (scan == IvfScan::ham) return HAM_ROWS_TILE;
         return scan == IvfScan::sq ? SQ_ROWS_TILE : (scan == IvfScan::rq ? RQ_ROWS_TILE : SCAN_ROWS_TILE_MID);
     }
 };
@@ -1208,6 +1218,21 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
     return (uint32_t)std::min<size_t>(bs, B);
 }
 
+// After a profiled IVF call (first sub-batch marked): the stage times into g_stage_ms, and the rows the regroup handed
+// to the scan (the small path has no regroup and counts none)
+static uint64_t read_stage_marks(Workspace *ws, cudaStream_t st)
+{
+    LGPU_CUDA(cudaStreamSynchronize(st));
+    cudaEvent_t end[7];
+    for (int i = 0; i < 7; i++) end[i] = i == 0 || (ws->stages_marked >> i & 1) ? ws->ev[i] : end[i - 1];
+    for (int i = 0; i < 6; i++) cudaEventElapsedTime(&g_stage_ms[i], end[i], end[i + 1]);
+    cudaEventElapsedTime(&g_stage_ms[6], end[0], end[6]);
+    unsigned long long rows = 0;
+    if (ws->stages_marked >> IVF_REGROUP & 1)
+        LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
+    return rows;
+}
+
 void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
                        const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                        RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
@@ -1233,15 +1258,7 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
         }
     }
     if (prof) {
-        LGPU_CUDA(cudaStreamSynchronize(st));
-        cudaEvent_t end[7];
-        for (int i = 0; i < 7; i++) end[i] = i == 0 || (ws->stages_marked >> i & 1) ? ws->ev[i] : end[i - 1];
-        for (int i = 0; i < 6; i++) cudaEventElapsedTime(&g_stage_ms[i], end[i], end[i + 1]);
-        cudaEventElapsedTime(&g_stage_ms[6], end[0], end[6]);
-        // the regroup counts the rows it hands to the scan (the small path has no regroup and counts none)
-        unsigned long long rows = 0;
-        if (ws->stages_marked >> IVF_REGROUP & 1)
-            LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
+        const uint64_t rows = read_stage_marks(ws, st);
         const uint32_t row_bytes = ix->is_sq ? ix->dim : ix->is_rq ? ix->rq_wpr * 4 : ix->is_pq4 ? ix->m / 2 : ix->m;
         g_scanned_bytes = (uint64_t)rows * row_bytes;
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
@@ -1435,6 +1452,110 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         LGPU_CUDA(cudaStreamSynchronize(st));
         g_filter_stats[1] = tc ? (uint64_t)B * (N + (list ? bx->nsample : 0)) : 0;
         g_filter_stats[3] = B;
+    }
+}
+
+// ---- binary IVF_FLAT (lgpu_ivf_binary): Hamming coarse step -> regroup (group.cu) -> b1 MMA scan of the probed rows
+// (ivf_ham_scan.cu) -> top-k over the distance segments (select mode 0), the IVF stages of lgpu_index ----
+
+// One sub-batch, everything on `st`.  Q / qpop: the sub-batch's packed queries [B][nbytes_pad] and their popcounts.
+// nprobes <= nlist.  only (device, [B]): redo just the flagged queries (maximum_nprobes widening).
+static void ham_ivf_sub_batch(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
+                              uint32_t B, const lgpu_search_params &sp, uint32_t nprobes, TopkOut out, bool prof,
+                              RowFilter rf, const uint32_t *only = nullptr)
+{
+    IvfPlan p{};
+    p.B = B; p.nprobes = nprobes; p.slots = B * nprobes; p.np_eff = nprobes;
+    p.k = p.kk = sp.k; p.coarse = Coarse::exact; p.scan = IvfScan::ham;
+    const uint32_t nlist = ix->nlist, nbp = ix->nbytes_pad;
+    const StageMarks mark{ws, prof};
+    mark(IVF_START, st);
+    ws->stats_mode = 0;
+    ws->probes.ensure((size_t)p.slots * 8);
+    if (nprobes >= nlist) {                       // every partition: no coarse step, no top-nprobes select
+        launch_ham_all_probes(ws->probes.as<uint64_t>(), B, nlist, st);
+        mark(IVF_COARSE, st);
+    } else {
+        // Hamming distances to the packed centroids, then the nprobes nearest by (distance, partition id).  The b1
+        // wgmma kernel from the flat path's crossover (HAM_TC_MIN_B x HAM_TC_MIN_N); for the coarse step's shapes the
+        // crossover is not measured.
+        const uint64_t ldc = (nlist + 3u) & ~3u;
+        ws->probe_dist.ensure((size_t)p.slots * 4); ws->probe_cnt.ensure((size_t)B * 4);
+        ws->D.ensure((size_t)B * ldc * 4);
+        if (tc_enabled() && B >= HAM_TC_MIN_B && nlist >= HAM_TC_MIN_N)
+            launch_ham_gemm(Q, ix->centroids.p, ix->cent_pop.as<uint32_t>(), qpop, B, nlist, nbp, ws->D.as<float>(), ldc,
+                            ix->num_sms, st);
+        else
+            launch_ham_dense(Q, ix->centroids.as<uint8_t>(), B, nlist, nbp, ws->D.as<float>(), ldc, ix->num_sms, st);
+        mark(IVF_COARSE, st);
+        launch_select(select_rows(ws->D.as<float>(), nlist, ldc, B, nprobes, {ws->probes.as<uint64_t>(),
+                                  ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>()}), st);
+    }
+    mark(IVF_PROBES, st);
+    const GroupArgs ga = ivf_regroup(ix, ws, p, only, st);
+    mark(IVF_REGROUP, st);
+    HamScanArgs ha{};
+    ha.rows = ix->codes.as<uint8_t>(); ha.row_pop = ix->row_pop.as<uint32_t>(); ha.queries = Q; ha.qpop = qpop;
+    ha.nbytes_pad = nbp;
+    ha.total_tiles = ga.total_tiles; ha.tile_counter = ga.tile_counter; ha.tile_desc = ga.tile_desc;
+    ha.dist_out = ws->dist_out.as<float>();
+    launch_ivf_ham_scan(ha, 2 * ix->num_sms, st);
+    mark(IVF_SCAN, st);
+    // distances are exact: refine_factor has nothing to re-rank, the top-k is taken directly
+    SelectArgs sa = select_segments(ix, ws, p, sp.k, out, rf);
+    sa.only = only;
+    with_range(sa, sp);
+    launch_select(sa, st);
+    mark(IVF_TOPK, st);
+}
+
+static uint32_t ham_ivf_sub_batch_size(lgpu_ivf_binary *ix, uint32_t B, uint32_t nprobes)
+{
+    const uint32_t np_eff = std::min<uint32_t>(nprobes, ix->nlist);
+    // distance segments, coarse scores, probe slots (ids, distances, regroup) and their tile descriptors
+    const size_t per_q = ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)np_eff * 36 +
+                         (size_t)np_eff * ix->max_nrb * (sizeof(TileDesc) / SCAN_G + 1) + 64;
+    size_t bs = workspace_budget() / per_q;
+    bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
+    bs = std::max<size_t>(1, std::min<size_t>(bs, 65535));
+    return (uint32_t)std::min<size_t>(bs, B);
+}
+
+// d_q: raw queries [B][nbytes] in device memory
+void ivf_binary_search_device(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t st, const uint8_t *d_q, uint32_t B,
+                              const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
+                              RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
+{
+    const uint32_t nbp = ix->nbytes_pad;
+    const uint32_t nprobes = std::min<uint32_t>(std::max<uint32_t>(sp.nprobes, 1), ix->nlist);
+    const uint32_t np_max = std::min<uint32_t>(sp.max_nprobes, ix->nlist);
+    const bool widen = rf.bits && np_max > nprobes;
+    // maximum_nprobes is only read when it widens (under a prefilter), as on lgpu_index
+    if (widen)
+        LGPU_REQUIRE(np_max <= SELECT_KMAX || np_max >= ix->nlist,
+                     "maximum_nprobes above 2048 is not supported unless it covers every partition");
+    const uint32_t bs = ham_ivf_sub_batch_size(ix, B, widen ? np_max : nprobes);
+    const bool prof = profiling_enabled();
+    const TopkOut out{d_ids, d_dist, d_cnt};
+    ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
+    launch_ham_pack(d_q, ix->nbytes, ix->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
+    for (uint32_t q0 = 0; q0 < B; q0 += bs) {
+        const uint32_t b = std::min(bs, B - q0);
+        if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
+        const uint8_t *Q = ws->hq.as<uint8_t>() + (size_t)q0 * nbp;
+        const uint32_t *qpop = ws->hq_pop.as<uint32_t>() + q0;
+        ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, nprobes, out.at(q0, sp.k), prof && q0 == 0, rf);
+        // maximum_nprobes under a prefilter, as on lgpu_index: the queries that found fewer than k rows are searched
+        // again over their np_max nearest partitions
+        if (widen) {
+            ws->widen.ensure((size_t)b * 4);
+            launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
+            ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
+        }
+    }
+    if (prof) {
+        g_scanned_bytes = read_stage_marks(ws, st) * nbp;
+        memset(g_filter_stats, 0, sizeof(g_filter_stats));
     }
 }
 
@@ -1814,7 +1935,7 @@ template <class H> static void open_rows(H *h, const uint64_t *row_ids, uint64_t
 }
 
 // the partition layout every IVF index shares (lgpu_index_open, lgpu_ivf_sq_open): checked before any device work
-static void check_ivf_layout(uint32_t dim, uint32_t nlist, int metric, uint64_t nrows, const float *centroids,
+static void check_ivf_layout(uint32_t dim, uint32_t nlist, int metric, uint64_t nrows, const void *centroids,
                              const uint64_t *part_offsets, const void *codes, const uint64_t *row_ids)
 {
     LGPU_REQUIRE(dim > 0 && nlist > 0, "dim and nlist must be positive");
@@ -1832,28 +1953,14 @@ static void check_ivf_layout(uint32_t dim, uint32_t nlist, int metric, uint64_t 
 // The arrays every IVF index holds in HBM, uploaded on the legacy stream: centroids (and their bf16 copy for the
 // tensor-core coarse step), partition sizes and offsets, row ids, optional raw vectors.  `rows_tile` is the scan's
 // tile height, which bounds the tile count of a search (max_nrb).
+static void open_ivf_partitions(lgpu_index *ix, int device, uint32_t nlist, uint64_t nrows,
+                                const uint64_t *part_offsets, const uint64_t *row_ids, uint32_t rows_tile);
+
 static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t nlist, int metric, uint64_t nrows,
                             const float *centroids, const uint64_t *part_offsets, const uint64_t *row_ids,
                             const float *vectors, uint32_t rows_tile)
 {
-    ix->device = device;
-    cudaDeviceProp prop;
-    LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-    ix->num_sms = prop.multiProcessorCount;
-    ix->dim = dim; ix->nlist = nlist; ix->metric = metric; ix->nrows = nrows;
-    std::vector<uint32_t> part_n(nlist), part_npad(nlist);
-    std::vector<uint64_t> pads(nlist);
-    for (uint32_t p = 0; p < nlist; p++) {
-        const uint32_t n = (uint32_t)(part_offsets[p + 1] - part_offsets[p]);
-        part_n[p] = n; part_npad[p] = (n + 31u) & ~31u;
-        pads[p] = (n + 3ull) & ~3ull;
-        ix->max_nrb = std::max(ix->max_nrb, scan_nrb(n, rows_tile));
-    }
-    ix->h_part_n = part_n;
-    std::sort(pads.begin(), pads.end(), std::greater<uint64_t>());
-    ix->pad_prefix.assign(nlist + 1, 0);
-    for (uint32_t p = 0; p < nlist; p++) ix->pad_prefix[p + 1] = ix->pad_prefix[p] + pads[p];
-
+    ix->dim = dim; ix->metric = metric;
     cudaStream_t st = nullptr;
     auto up = [&](DevBuf &b, const void *src, size_t bytes) {
         b.ensure(std::max<size_t>(bytes, 16));
@@ -1861,10 +1968,7 @@ static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t n
         ix->device_bytes += b.bytes;
     };
     up(ix->centroids, centroids, (size_t)nlist * dim * 4);
-    up(ix->part_n, part_n.data(), (size_t)nlist * 4);
-    up(ix->part_npad, part_npad.data(), (size_t)nlist * 4);
-    up(ix->part_off, part_offsets, (size_t)(nlist + 1) * 8);
-    up(ix->row_ids, row_ids, (size_t)nrows * 8);
+    open_ivf_partitions(ix, device, nlist, nrows, part_offsets, row_ids, rows_tile);
     if (vectors) { up(ix->vectors, vectors, (size_t)nrows * dim * 4); ix->has_vectors = true; }
     if (gemm_shape_supported(dim) && metric != LGPU_DOT) {
         LGPU_CUDA(cudaStreamSynchronize(st));
@@ -1886,6 +1990,42 @@ static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t n
         }
         ix->has_tc = true;
     }
+    LGPU_CUDA(cudaStreamSynchronize(st));
+}
+
+// The partition arrays every IVF index holds (part_n, part_npad, part_off, row_ids, the host-side tile bound max_nrb and
+// pad_prefix), uploaded on the legacy stream; `rows_tile` is the scan's tile height
+static void open_ivf_partitions(lgpu_index *ix, int device, uint32_t nlist, uint64_t nrows,
+                                const uint64_t *part_offsets, const uint64_t *row_ids, uint32_t rows_tile)
+{
+    ix->device = device;
+    cudaDeviceProp prop;
+    LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+    ix->num_sms = prop.multiProcessorCount;
+    ix->nlist = nlist; ix->nrows = nrows;
+    std::vector<uint32_t> part_n(nlist), part_npad(nlist);
+    std::vector<uint64_t> pads(nlist);
+    for (uint32_t p = 0; p < nlist; p++) {
+        const uint32_t n = (uint32_t)(part_offsets[p + 1] - part_offsets[p]);
+        part_n[p] = n; part_npad[p] = (n + 31u) & ~31u;
+        pads[p] = (n + 3ull) & ~3ull;
+        ix->max_nrb = std::max(ix->max_nrb, scan_nrb(n, rows_tile));
+    }
+    ix->h_part_n = part_n;
+    std::sort(pads.begin(), pads.end(), std::greater<uint64_t>());
+    ix->pad_prefix.assign(nlist + 1, 0);
+    for (uint32_t p = 0; p < nlist; p++) ix->pad_prefix[p + 1] = ix->pad_prefix[p] + pads[p];
+
+    cudaStream_t st = nullptr;
+    auto up = [&](DevBuf &b, const void *src, size_t bytes) {
+        b.ensure(std::max<size_t>(bytes, 16));
+        if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, st));
+        ix->device_bytes += b.bytes;
+    };
+    up(ix->part_n, part_n.data(), (size_t)nlist * 4);
+    up(ix->part_npad, part_npad.data(), (size_t)nlist * 4);
+    up(ix->part_off, part_offsets, (size_t)(nlist + 1) * 8);
+    up(ix->row_ids, row_ids, (size_t)nrows * 8);
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
@@ -2695,6 +2835,131 @@ int lgpu_binary_search_device(lgpu_binary *bxh, const uint8_t *d_queries, uint32
                               uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream)
 {
     return binary_call(bxh, device_route(cuda_stream), d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
+}
+
+int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
+{
+    lgpu_ivf_binary *ix = nullptr;
+    int rc = guarded([&] {
+        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+        LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
+        LGPU_REQUIRE(d->nbytes > 0, "zero bytes per vector");
+        LGPU_REQUIRE((uint64_t)d->nbytes * 8 <= ((uint64_t)1 << 24), "binary vectors above 2^24 bits are not supported");
+        check_ivf_layout(d->nbytes, d->nlist, LGPU_L2, d->nrows, d->centroids, d->part_offsets, d->vectors, d->row_ids);
+        require_device(d->device);
+        ix = new lgpu_ivf_binary();
+        ix->nbytes = d->nbytes; ix->nbytes_pad = (d->nbytes + 31) & ~31u;
+        ix->dim = d->nbytes;
+        open_ivf_partitions(ix, d->device, d->nlist, d->nrows, d->part_offsets, d->row_ids, HAM_ROWS_TILE);
+        // centroids and rows zero-padded to nbytes_pad, with their popcounts (ham_pack)
+        const uint32_t nb = d->nbytes, nbp = ix->nbytes_pad;
+        auto pack = [&](const uint8_t *src, uint64_t n, DevBuf &dst, DevBuf &pop) {
+            dst.ensure(std::max<size_t>((size_t)n * nbp, 16));
+            pop.ensure(std::max<size_t>((size_t)n * 4, 16));
+            if (n) {
+                DevBuf raw;
+                raw.ensure((size_t)n * nb);
+                LGPU_CUDA(cudaMemcpy(raw.p, src, (size_t)n * nb, cudaMemcpyHostToDevice));
+                launch_ham_pack(raw.as<uint8_t>(), nb, nb, n, dst.as<uint8_t>(), nbp, pop.as<uint32_t>(), nullptr);
+                LGPU_CUDA(cudaStreamSynchronize(nullptr));
+            }
+            ix->device_bytes += dst.bytes + pop.bytes;
+        };
+        pack(d->centroids, d->nlist, ix->centroids, ix->cent_pop);
+        pack(d->vectors, d->nrows, ix->codes, ix->row_pop);
+        // the tile descriptors' code offset is unused (the scan addresses rows by part_off)
+        ix->code_base.ensure((size_t)d->nlist * 8);
+        LGPU_CUDA(cudaMemset(ix->code_base.p, 0, (size_t)d->nlist * 8));
+        ix->device_bytes += ix->code_base.bytes;
+        register_handle(ix);
+        *out = ix;
+    });
+    if (rc != LGPU_OK && ix) delete ix;
+    return rc;
+}
+
+void lgpu_ivf_binary_close(lgpu_ivf_binary *ix) { close_handle(ix); }
+
+static int ivf_binary_call(lgpu_ivf_binary *ixh, const Route &r, const uint8_t *q, uint32_t B,
+                           const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)
+{
+    return search_call(ixh, "binary IVF index", r, q, B, p, ids, dist, cnt,
+                       [&](lgpu_ivf_binary *ix) {
+                           check_call(p, B, q, ids, dist, cnt, false);   // refine_factor: exact distances
+                           LGPU_REQUIRE(p->nprobes >= 1, "minimum_nprobes must be greater than 0");
+                           LGPU_REQUIRE(p->nprobes <= SELECT_KMAX || p->nprobes >= ix->nlist,
+                                        "nprobes above 2048 is not supported unless it covers every partition");
+                           return (size_t)B * ix->nbytes;
+                       },
+                       ivf_binary_search_device);
+}
+
+int lgpu_ivf_binary_search(lgpu_ivf_binary *ixh, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
+                           uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return ivf_binary_call(ixh, host_route(0x1fb1ull), queries, B, params, out_ids, out_dist, out_count);
+}
+
+int lgpu_ivf_binary_search_filtered(lgpu_ivf_binary *ixh, const uint8_t *queries, uint32_t B,
+                                    const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                                    uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return ivf_binary_call(ixh, filtered_route(allow, allow_bits), queries, B, params, out_ids, out_dist, out_count);
+}
+
+int lgpu_ivf_binary_search_device(lgpu_ivf_binary *ixh, const uint8_t *d_queries, uint32_t B,
+                                  const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
+                                  uint32_t *d_out_count, void *cuda_stream)
+{
+    return ivf_binary_call(ixh, device_route(cuda_stream), d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
+}
+
+int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_t *vectors, uint64_t N, uint32_t nbytes,
+                                int device, uint32_t *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(nbytes > 0 && (uint64_t)nbytes * 8 <= ((uint64_t)1 << 24), "bytes per vector out of range");
+        LGPU_REQUIRE(B == 0 || N == 0 || (queries && vectors && out), "null buffer");
+        LGPU_REQUIRE(N < (1ull << 31) && (uint64_t)B * N < (1ull << 32), "B x N must stay below 2^32");
+        if (B == 0 || N == 0) return;
+        require_device(device);
+        cudaDeviceProp prop;
+        LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
+        const uint32_t nbp = (nbytes + 31) & ~31u;
+        DevBuf rq, rx, q, x, qp, xp, D, tiles, ctr;
+        rq.ensure((size_t)B * nbytes); rx.ensure((size_t)N * nbytes);
+        q.ensure((size_t)B * nbp); x.ensure((size_t)N * nbp); qp.ensure((size_t)B * 4); xp.ensure((size_t)N * 4);
+        LGPU_CUDA(cudaMemcpy(rq.p, queries, (size_t)B * nbytes, cudaMemcpyHostToDevice));
+        LGPU_CUDA(cudaMemcpy(rx.p, vectors, (size_t)N * nbytes, cudaMemcpyHostToDevice));
+        launch_ham_pack(rq.as<uint8_t>(), nbytes, nbytes, B, q.as<uint8_t>(), nbp, qp.as<uint32_t>(), nullptr);
+        launch_ham_pack(rx.as<uint8_t>(), nbytes, nbytes, N, x.as<uint8_t>(), nbp, xp.as<uint32_t>(), nullptr);
+        // one partition of N rows that every query probes: tiles of HAM_ROWS_TILE rows x 8 queries, query b's row r at
+        // out + b N + r
+        std::vector<TileDesc> h;
+        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
+            for (uint64_t r0 = 0; r0 < N; r0 += HAM_ROWS_TILE) {
+                TileDesc t{};
+                t.row0 = (uint32_t)r0; t.nrows = (uint32_t)std::min<uint64_t>(HAM_ROWS_TILE, N - r0);
+                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N;
+                for (uint32_t g = 0; g < t.ng; g++) {
+                    t.q[g] = q0 + g; t.slot[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * N);
+                }
+                h.push_back(t);
+            }
+        tiles.ensure(h.size() * sizeof(TileDesc));
+        ctr.ensure(8);
+        D.ensure((size_t)B * N * 4);
+        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
+        const uint32_t zero2[2] = {(uint32_t)h.size(), 0u};
+        LGPU_CUDA(cudaMemcpy(ctr.p, zero2, 8, cudaMemcpyHostToDevice));
+        HamScanArgs a{};
+        a.rows = x.as<uint8_t>(); a.row_pop = xp.as<uint32_t>(); a.queries = q.as<uint8_t>(); a.qpop = qp.as<uint32_t>();
+        a.nbytes_pad = nbp;
+        a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1;
+        a.tile_desc = tiles.as<TileDesc>(); a.dist_out = D.as<float>(); a.out_u32 = 1;
+        launch_ivf_ham_scan(a, 2 * prop.multiProcessorCount, nullptr);
+        LGPU_CUDA(cudaMemcpy(out, D.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
+    });
 }
 
 int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,

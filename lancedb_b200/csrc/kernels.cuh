@@ -145,6 +145,24 @@ void launch_rq_planes(const float *rq, const float *rc, const uint64_t *probes, 
 void launch_rq_row_prep(uint32_t *codes, uint64_t n, uint32_t dim, uint32_t wpr, uint32_t *popc, cudaStream_t st);
 void launch_rq_scan(const RqScanArgs &a, int grid, cudaStream_t st);
 
+// ---------------- binary IVF_FLAT scan (ivf_ham_scan.cu) --------------------------------
+constexpr uint32_t HAM_ROWS_TILE = 512;           // rows per tile: 8 warps x 32 rows x 2 passes (not tuned)
+struct HamScanArgs {
+    const uint8_t *rows;          // [nrows][nbytes_pad] packed rows, partitions contiguous, zero padding
+    const uint32_t *row_pop;      // [nrows] popc of each row
+    const uint8_t *queries;       // [B][nbytes_pad] packed queries of the sub-batch (launch_ham_pack)
+    const uint32_t *qpop;         // [B]
+    uint32_t nbytes_pad;          // a multiple of 32
+    const uint32_t *total_tiles;  // [1]
+    uint32_t *tile_counter;       // [1], zeroed before launch
+    const TileDesc *tile_desc;    // built with rows_tile == HAM_ROWS_TILE; q[] addresses queries / qpop
+    float *dist_out;              // segment of slot e at out[e]: popc(q XOR x) of row r at out[e] + r, as f32
+    int out_u32;                  // 1: write the u32 distances instead (lgpu_debug_ivf_hamming_scan)
+};
+void launch_ivf_ham_scan(const HamScanArgs &a, int grid, cudaStream_t st);
+// probes[q][j] = j for q < B, j < nlist: every partition, for nprobes >= nlist (no coarse step, no top-nprobes select)
+void launch_ham_all_probes(uint64_t *probes, uint32_t B, uint32_t nlist, cudaStream_t st);
+
 // ---------------- 4-bit IVF_PQ scan (pq4_scan.cu) ----------------------------------------
 constexpr uint32_t PQ4_ROWS_TILE = 2048;          // rows per tile: 256 threads x 2 groups of 4 rows
 struct alignas(8) Pq4Slot {                       // one probe slot's table quantiser

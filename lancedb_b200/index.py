@@ -1,4 +1,4 @@
-"""IVF_PQ, IVF_SQ and IVF_RQ index containers and trainers.
+"""IVF_PQ, IVF_SQ, IVF_RQ and binary IVF_FLAT index containers and trainers.
 
 `IvfPqIndexData` is the plain-array form of a Lance IVF_PQ index: exactly the arrays
 the reference's search path consumes after `prewarm_index`
@@ -558,5 +558,124 @@ def train_ivf_rq(vectors, *, num_partitions: Optional[int] = None, distance_type
         dim=dim, nlist=nlist, metric=metric, centroids=cent, rotation=P, part_offsets=part_offsets, codes=codes,
         add_factors=add, scale_factors=scale, row_ids=rid[order_np],
         vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
+    data.validate()
+    return data
+
+
+# --------------------------------------------------------------------------------------
+HAMMING_MAX_BITS = 1 << 24  # binary vectors above 2^24 bits are rejected, as on the flat binary path
+
+
+@dataclass
+class IvfBinaryIndexData:
+    """The plain-array form of a binary IVF_FLAT index (lance `IvfFlat` with distance_type "hamming",
+    rust/lancedb/src/index/vector.rs:169-209): packed bit-vector centroids and the packed rows grouped by partition.  The
+    same arrays go to `lgpu_ivf_binary_open` and to the CPU oracle (tests/ivf_binary_oracle.c)."""
+    nbytes: int
+    nlist: int
+    centroids: np.ndarray      # u8 [nlist, nbytes] packed bits
+    part_offsets: np.ndarray   # u64 [nlist+1]
+    vectors: np.ndarray        # u8 [n, nbytes] partition order
+    row_ids: np.ndarray        # u64 [n] in partition order
+    metric: str = "hamming"
+
+    @property
+    def nrows(self) -> int:
+        return int(self.row_ids.size)
+
+    def validate(self) -> None:
+        assert self.metric == "hamming"
+        assert 1 <= self.nbytes and 8 * self.nbytes <= HAMMING_MAX_BITS
+        assert self.centroids.shape == (self.nlist, self.nbytes) and self.centroids.dtype == np.uint8
+        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
+        assert int(self.part_offsets[0]) == 0 and int(self.part_offsets[-1]) == self.nrows
+        assert self.vectors.shape == (self.nrows, self.nbytes) and self.vectors.dtype == np.uint8
+        assert self.row_ids.dtype == np.uint64
+
+
+def _unpack_bits(x, device, dtype):
+    """packed u8 rows [n, nbytes] -> 0/1 tensor [n, 8 nbytes] (bit i & 7 of byte i >> 3, the packing order)"""
+    import torch
+    t = torch.as_tensor(np.require(x, np.uint8, ["C", "W"]), device=device)
+    shifts = torch.arange(8, device=device, dtype=torch.uint8)
+    return ((t[:, :, None] >> shifts) & 1).reshape(t.shape[0], -1).to(dtype)
+
+
+def kmodes_assign(x, centroids, device=None, chunk: int = 1 << 15) -> np.ndarray:
+    """Index of the nearest centroid of every packed row by Hamming distance, ties to the lowest index:
+    popc(x XOR c) = popc(x) + popc(c) - 2 x.c over the unpacked bits.  Operands and result are f32 on every device: 0
+    and 1 are exact (also when TF32 rounds the operands), every product is exact, and the f32 sums stay exact integers
+    below 2^24 bits per row.  (A bf16 result would round x.c above 256.)  The tie rule does not lean on argmin's
+    choice among equal values: the key is d * nlist + index, an exact int64."""
+    import torch
+    dev = torch.device(device or "cpu")
+    c = _unpack_bits(centroids, dev, torch.float32)
+    k = c.shape[0]
+    cpop = c.sum(1)
+    idx = torch.arange(k, device=dev, dtype=torch.int64)
+    x = np.ascontiguousarray(x, np.uint8)
+    out = np.empty(x.shape[0], np.int64)
+    chunk = max(1, min(chunk, (1 << 27) // max(8 * x.shape[1], k)))    # unpacked rows and keys: ~1 GB at most
+    for s in range(0, x.shape[0], chunk):
+        b = _unpack_bits(x[s:s + chunk], dev, torch.float32)
+        d = b.sum(1)[:, None] + cpop[None, :] - 2.0 * (b @ c.T)
+        key = d.to(torch.int64) * k + idx[None, :]
+        out[s:s + chunk] = torch.argmin(key, dim=1).cpu().numpy()
+    return out
+
+
+def kmodes_update(x, assign, centroids, device=None) -> np.ndarray:
+    """One k-modes centroid update [lance, recalled: KModeAlgo]: bit j of centroid c is set when 2 ones > members over
+    the rows assigned to c (an exact half keeps 0, a project decision); a cluster with no rows keeps its previous
+    centroid (a project decision)."""
+    import torch
+    dev = torch.device(device or "cpu")
+    k = centroids.shape[0]
+    a = torch.as_tensor(np.asarray(assign, np.int64), device=dev)
+    ones = torch.zeros((k, 8 * centroids.shape[1]), dtype=torch.float32, device=dev)
+    ones.index_add_(0, a, _unpack_bits(x, dev, torch.float32))
+    members = torch.bincount(a, minlength=k).to(torch.float32)
+    bits = (2.0 * ones > members[:, None]).to(torch.uint8).cpu().numpy()
+    new = np.packbits(bits, axis=1, bitorder="little")
+    empty = members.cpu().numpy() == 0
+    new[empty] = np.asarray(centroids, np.uint8)[empty]
+    return new
+
+
+def train_ivf_binary(vectors, *, num_partitions: Optional[int] = None, distance_type: str = "hamming",
+                     sample_rate: int = 256, max_iterations: int = 50, row_ids: Optional[np.ndarray] = None,
+                     seed: int = 45, device: Optional[str] = None) -> IvfBinaryIndexData:
+    """Binary IVF_FLAT (IvfFlat with distance_type "hamming"): k-modes over packed bit vectors [n, nbytes].  On a sample
+    of min(n, sample_rate nlist) rows (seeded), the initial centroids are nlist distinct sample rows; each of
+    max_iterations rounds assigns every sample row to its nearest centroid (kmodes_assign) and updates the centroids
+    (kmodes_update).  Every row then lands in its nearest centroid.  All of it is integer work: the result does not
+    depend on the device."""
+    if distance_type.lower() != "hamming":
+        raise ValueError(f"IVF_FLAT over binary vectors supports the hamming distance type only, not {distance_type!r}")
+    x = np.ascontiguousarray(vectors, np.uint8)
+    if x.ndim != 2 or x.shape[1] < 1:
+        raise ValueError("binary vectors must be a [rows, bytes] uint8 array")
+    n, nbytes = x.shape
+    if 8 * nbytes > HAMMING_MAX_BITS:
+        raise ValueError("binary vectors above 2^24 bits are not supported")
+    nlist = int(num_partitions or suggested_num_partitions(n))
+    if nlist < 1 or nlist > max(n, 1):
+        raise ValueError(f"num_partitions must be in [1, {max(n, 1)}] for {n} rows, got {nlist}")
+    rng = np.random.default_rng(seed)
+    ns = min(n, int(sample_rate) * nlist)
+    samp = x[np.sort(rng.choice(n, ns, replace=False))] if ns < n else x
+    cent = samp[rng.choice(samp.shape[0], nlist, replace=False)] if n else np.zeros((nlist, nbytes), np.uint8)
+    for _ in range(int(max_iterations) if n else 0):
+        new = kmodes_update(samp, kmodes_assign(samp, cent, device), cent, device)
+        if np.array_equal(new, cent):
+            break
+        cent = new
+    assign = kmodes_assign(x, cent, device) if n else np.zeros(0, np.int64)
+    order = np.argsort(assign, kind="stable")                         # ascending row id per partition
+    part_offsets = np.zeros(nlist + 1, np.uint64)
+    part_offsets[1:] = np.cumsum(np.bincount(assign, minlength=nlist))
+    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
+    data = IvfBinaryIndexData(nbytes=nbytes, nlist=nlist, centroids=np.ascontiguousarray(cent, np.uint8),
+                              part_offsets=part_offsets, vectors=np.ascontiguousarray(x[order]), row_ids=rid[order])
     data.validate()
     return data

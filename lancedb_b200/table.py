@@ -16,8 +16,8 @@ import numpy as np
 import pyarrow as pa
 
 from . import _native
-from .index import (RQ_MAX_DIM, IvfPqIndexData, IvfRqIndexData, IvfSqIndexData, train_ivf_pq, train_ivf_rq,
-                    train_ivf_sq)
+from .index import (RQ_MAX_DIM, IvfBinaryIndexData, IvfPqIndexData, IvfRqIndexData, IvfSqIndexData,
+                    train_ivf_binary, train_ivf_pq, train_ivf_rq, train_ivf_sq)
 from .query import LanceVectorQueryBuilder
 
 
@@ -84,7 +84,7 @@ class Table:
         self._binary: Dict[str, _native.GpuBinary] = {}
         self._multivec: Dict[str, _native.GpuMultivec] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
-        self._index_data: Dict[str, Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData]] = {}
+        self._index_data: Dict[str, Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData, IvfBinaryIndexData]] = {}
 
     # ---- introspection ----
     @property
@@ -105,6 +105,8 @@ class Table:
 
     def _index_type(self, column: str) -> str:
         d = self._index_data[column]
+        if isinstance(d, IvfBinaryIndexData):
+            return "IVF_FLAT"
         return "IVF_SQ" if isinstance(d, IvfSqIndexData) else ("IVF_RQ" if isinstance(d, IvfRqIndexData) else "IVF_PQ")
 
     def list_indices(self):
@@ -156,6 +158,22 @@ class Table:
                      replace: bool = True, accelerator: Optional[str] = None, index_type: str = "IVF_PQ",
                      num_bits: int = 8, max_iterations: int = 50, sample_rate: int = 256, **_ignored):
         kind = index_type.upper()
+        if kind == "IVF_FLAT":             # binary columns only: IvfFlat(distance_type="hamming")
+            column = vector_column_name or self._infer_vector_column(None)
+            if self._is_multivec(column):
+                raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
+            if not self._is_binary(column):
+                raise NotImplementedError("IVF_FLAT is served over binary (fixed_size_list<uint8>) columns only; index "
+                                          "float columns with IVF_PQ, IVF_SQ or IVF_RQ")
+            if metric.lower() != "hamming":
+                raise ValueError(f"IVF_FLAT over binary vectors supports the hamming distance type only, not {metric!r}")
+            if column in self._index and not replace:
+                raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")
+            dev = f"cuda:{self._device}" if accelerator in ("cuda", "gpu") else None
+            self._attach_index(column, train_ivf_binary(self._binary_vectors(column), num_partitions=num_partitions,
+                                                        max_iterations=max_iterations, sample_rate=sample_rate,
+                                                        device=dev))
+            return
         if kind not in ("IVF_PQ", "IVF_SQ", "IVF_RQ"):
             raise NotImplementedError("only IVF_PQ, IVF_SQ and IVF_RQ are on the GPU hot path")
         if kind == "IVF_RQ" and num_bits != 1:
@@ -199,11 +217,13 @@ class Table:
                             native_passes=dev is not None)      # accelerator: row passes through the C ABI (build.cu)
         self._attach_index(column, data)
 
-    def _attach_index(self, column: str, data: Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData]):
+    def _attach_index(self, column: str,
+                      data: Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData, IvfBinaryIndexData]):
         if column in self._index:
             self._index[column].close()
         self._index_data[column] = data
-        cls = (_native.GpuIvfSq if isinstance(data, IvfSqIndexData) else
+        cls = (_native.GpuIvfBinary if isinstance(data, IvfBinaryIndexData) else
+               _native.GpuIvfSq if isinstance(data, IvfSqIndexData) else
                _native.GpuIvfRq if isinstance(data, IvfRqIndexData) else _native.GpuIvfPq)
         self._index[column] = cls(data, device=self._device)
 
@@ -268,6 +288,11 @@ class Table:
                 raise ValueError(f"distance type {distance_type!r} is not supported on binary column {column!r}: "
                                  "use 'hamming'")
             q = _native.binary_components(queries)   # the builder's f32 copy: integers are exact up to 2^24
+            idx = self._index.get(column) if use_index else None
+            if idx is not None:                    # IVF_FLAT (hamming); bypass_vector_index() searches flat below
+                return idx.search(q, k=k, nprobes=nprobes, refine_factor=refine_factor or 0, lower=lower, upper=upper,
+                                  allow=allow, allow_bits=allow_bits,
+                                  max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms)
             bx = self._binary.get(column)
             if bx is None:
                 bx = self._binary[column] = _native.GpuBinary(self._binary_vectors(column), device=self._device)
