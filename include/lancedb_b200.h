@@ -466,12 +466,19 @@ int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes
  * out [nqv][nrows] f32); dim must be a multiple of 8 */
 int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
                            uint64_t nrows, uint32_t dim, int device, float *out);
-/* per-kernel device time (ms) of the most recent lgpu_search* call made with
- * LGPU_PROFILE=1 in the environment: coarse, select-probes, group, scan, top-k,
- * refine, total.  times: [7] */
+/* the number of queries per sub-batch an lgpu_search* call of B queries and `nprobes` probes (the widest the call uses:
+ * maximum_nprobes under a prefilter) on `ix` runs in under the process's LGPU_WS_BYTES: B when the batch is not split */
+int lgpu_debug_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32_t *out);
+/* per-stage device time (ms) of the most recent profiled lgpu_search* / lgpu_ivf_binary_search* call on this thread:
+ * coarse, select-probes, group, scan, top-k, refine, total.  times: [7].  A call the workspace budget splits into
+ * sub-batches reports, per stage, the sum over its sub-batches (profiling synchronises after each one); the
+ * maximum_nprobes widening passes are not timed.  lgpu_last_scanned_code_bytes covers the same: the code bytes every
+ * sub-batch's first pass handed to the scan (0 for a sub-batch on the small path, which has no regroup). */
 int lgpu_last_stage_ms(float *times);
-/* filter-scan counters of the most recent profiled lgpu_search* call on this thread (first sub-batch): candidates the
- * scanners appended, survivors re-scored exactly, queries sent to the exact fix-up pass, queries.  stats: [4]
+/* filter-scan counters of the most recent profiled lgpu_search* call on this thread, summed over the call's sub-batches
+ * (each sub-batch picks its own filter mode): candidates the scanners appended and survivors re-scored exactly
+ * (candidate mode only), queries sent to the exact fix-up pass, queries that went through the filter scan (a
+ * sub-batch on the exact or the small path adds none).  stats: [4]
  * After lgpu_binary_search* (whole batch): [0] candidates the tensor-core list pass appended (0 on the dense paths),
  * [1] distances computed on the tensor cores (0 on the SIMT path), [2] queries redone densely after a list overflow,
  * [3] queries.  After lgpu_multivec_search*: see the multivector section above. */

@@ -30,7 +30,8 @@ EXPORTS = [
     "lgpu_comm_last_stage_ms",
     "lgpu_flat_open", "lgpu_flat_close", "lgpu_flat_search", "lgpu_flat_search_filtered", "lgpu_flat_search_device",
     "lgpu_ivf_assign", "lgpu_pq_encode", "lgpu_kmeans_train", "lgpu_pq_train",
-    "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_filter_bounds", "lgpu_debug_gemm", "lgpu_last_stage_ms", "lgpu_set_profiling",
+    "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_filter_bounds", "lgpu_debug_gemm",
+    "lgpu_debug_sub_batch_size", "lgpu_last_stage_ms", "lgpu_set_profiling",
     "lgpu_kernel_launch_count", "lgpu_last_filter_stats",
     "lgpu_binary_open", "lgpu_binary_close", "lgpu_binary_search", "lgpu_binary_search_filtered",
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
@@ -152,6 +153,7 @@ def load():
     lib.lgpu_debug_partition_distances.argtypes = [vp, vp, u32, vp]
     lib.lgpu_debug_filter_bounds.argtypes = [vp, vp, u32, u32, C.c_uint64, vp, vp, vp, vp, vp]
     lib.lgpu_debug_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
+    lib.lgpu_debug_sub_batch_size.argtypes = [vp, u32, u32, C.POINTER(u32)]
     lib.lgpu_last_stage_ms.argtypes = [vp]
     lib.lgpu_set_profiling.argtypes = [i32]
     lib.lgpu_kernel_launch_count.argtypes = [C.POINTER(C.c_uint64)]
@@ -335,6 +337,12 @@ class GpuIvfPq(_Handle):
     def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search (raw addresses), enqueued on `stream`, not synchronised."""
         check(load().lgpu_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
+
+    def debug_sub_batch_size(self, B: int, nprobes: int) -> int:
+        """Queries per sub-batch of a search of B queries over `nprobes` probes under this process's LGPU_WS_BYTES."""
+        n = C.c_uint32(0)
+        check(load().lgpu_debug_sub_batch_size(self._h, int(B), int(nprobes), C.byref(n)))
+        return n.value
 
     def debug_coarse(self, queries, nprobes):
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)

@@ -1218,18 +1218,40 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
     return (uint32_t)std::min<size_t>(bs, B);
 }
 
-// After a profiled IVF call (first sub-batch marked): the stage times into g_stage_ms, and the rows the regroup handed
-// to the scan (the small path has no regroup and counts none)
-static uint64_t read_stage_marks(Workspace *ws, cudaStream_t st)
+// After a profiled IVF sub-batch: its stage times are added to g_stage_ms; returns the rows its regroup handed to the
+// scan (the small path has no regroup and counts none).  Synchronises `st`.
+static uint64_t add_stage_marks(Workspace *ws, cudaStream_t st)
 {
     LGPU_CUDA(cudaStreamSynchronize(st));
     cudaEvent_t end[7];
     for (int i = 0; i < 7; i++) end[i] = i == 0 || (ws->stages_marked >> i & 1) ? ws->ev[i] : end[i - 1];
-    for (int i = 0; i < 6; i++) cudaEventElapsedTime(&g_stage_ms[i], end[i], end[i + 1]);
-    cudaEventElapsedTime(&g_stage_ms[6], end[0], end[6]);
+    for (int i = 0; i < 7; i++) {
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, i < 6 ? end[i] : end[0], i < 6 ? end[i + 1] : end[6]);
+        g_stage_ms[i] += ms;
+    }
     unsigned long long rows = 0;
     if (ws->stages_marked >> IVF_REGROUP & 1)
         LGPU_CUDA(cudaMemcpy(&rows, ws->scalars.as<char>() + 16, 8, cudaMemcpyDeviceToHost));
+    return rows;
+}
+
+// Profiling covers the whole call: every sub-batch's first pass is marked and read back here (a synchronisation per
+// sub-batch, which profiling accepts), its stage times, scanned rows and filter counters added to the call's.  The
+// maximum_nprobes widening pass is not part of any of them.  b: the sub-batch's queries (ws->flags holds b flags).
+static uint64_t add_ivf_profile(Workspace *ws, cudaStream_t st, uint32_t b)
+{
+    const uint64_t rows = add_stage_marks(ws, st);
+    if (ws->stats_mode == 1) {
+        uint64_t s[4];
+        LGPU_CUDA(cudaMemcpy(s, ws->c_stats.p, 32, cudaMemcpyDeviceToHost));
+        for (int i = 0; i < 4; i++) g_filter_stats[i] += s[i];
+    } else if (ws->stats_mode == 2) {                       // dense filter: queries the band check could not prove
+        std::vector<uint32_t> fl(b);
+        LGPU_CUDA(cudaMemcpy(fl.data(), ws->flags.p, (size_t)b * 4, cudaMemcpyDeviceToHost));
+        for (uint32_t f : fl) g_filter_stats[2] += f ? 1 : 0;
+        g_filter_stats[3] += b;
+    }
     return rows;
 }
 
@@ -1241,12 +1263,19 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
     const uint32_t np_widest = rf.bits ? std::max(nprobes, std::min<uint32_t>(sp.max_nprobes, ix->nlist)) : nprobes;
     const uint32_t bs = ivf_sub_batch_size(ix, B, np_widest);
     const bool prof = profiling_enabled();
+    const uint32_t row_bytes = ix->is_sq ? ix->dim : ix->is_rq ? ix->rq_wpr * 4 : ix->is_pq4 ? ix->m / 2 : ix->m;
+    if (prof) {
+        memset(g_stage_ms, 0, sizeof(g_stage_ms));
+        memset(g_filter_stats, 0, sizeof(g_filter_stats));
+        g_scanned_bytes = 0;
+    }
     const TopkOut out{d_ids, d_dist, d_cnt};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
         const float *q = d_q + (size_t)q0 * ix->dim;
-        ivf_sub_batch(ix, ws, st, q, b, sp, nprobes, out.at(q0, sp.k), prof && q0 == 0, rf);
+        ivf_sub_batch(ix, ws, st, q, b, sp, nprobes, out.at(q0, sp.k), prof, rf);
+        if (prof) g_scanned_bytes += add_ivf_profile(ws, st, b) * row_bytes;
         // maximum_nprobes (query.rs:1250-1275): under a prefilter, the queries that found fewer than k rows in their
         // minimum_nprobes partitions are searched again over their maximum_nprobes nearest (no work if none is)
         const uint32_t np_max = std::min<uint32_t>(sp.max_nprobes, ix->nlist);
@@ -1255,19 +1284,6 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const flo
             ws->widen.ensure((size_t)b * 4);
             launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
             ivf_sub_batch(ix, ws, st, q, b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
-        }
-    }
-    if (prof) {
-        const uint64_t rows = read_stage_marks(ws, st);
-        const uint32_t row_bytes = ix->is_sq ? ix->dim : ix->is_rq ? ix->rq_wpr * 4 : ix->is_pq4 ? ix->m / 2 : ix->m;
-        g_scanned_bytes = (uint64_t)rows * row_bytes;
-        memset(g_filter_stats, 0, sizeof(g_filter_stats));
-        if (ws->stats_mode == 1) LGPU_CUDA(cudaMemcpy(g_filter_stats, ws->c_stats.p, 32, cudaMemcpyDeviceToHost));
-        else if (ws->stats_mode == 2) {                       // dense filter: queries the band check could not prove
-            std::vector<uint32_t> fl(B);
-            LGPU_CUDA(cudaMemcpy(fl.data(), ws->flags.p, (size_t)B * 4, cudaMemcpyDeviceToHost));
-            for (uint32_t f : fl) g_filter_stats[2] += f ? 1 : 0;
-            g_filter_stats[3] = B;
         }
     }
 }
@@ -1537,6 +1553,11 @@ void ivf_binary_search_device(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t s
     const uint32_t bs = ham_ivf_sub_batch_size(ix, B, widen ? np_max : nprobes);
     const bool prof = profiling_enabled();
     const TopkOut out{d_ids, d_dist, d_cnt};
+    if (prof) {
+        memset(g_stage_ms, 0, sizeof(g_stage_ms));
+        memset(g_filter_stats, 0, sizeof(g_filter_stats));
+        g_scanned_bytes = 0;
+    }
     ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
     launch_ham_pack(d_q, ix->nbytes, ix->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
@@ -1544,7 +1565,8 @@ void ivf_binary_search_device(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t s
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
         const uint8_t *Q = ws->hq.as<uint8_t>() + (size_t)q0 * nbp;
         const uint32_t *qpop = ws->hq_pop.as<uint32_t>() + q0;
-        ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, nprobes, out.at(q0, sp.k), prof && q0 == 0, rf);
+        ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, nprobes, out.at(q0, sp.k), prof, rf);
+        if (prof) g_scanned_bytes += add_stage_marks(ws, st) * nbp;      // the whole call, as on lgpu_index
         // maximum_nprobes under a prefilter, as on lgpu_index: the queries that found fewer than k rows are searched
         // again over their np_max nearest partitions
         if (widen) {
@@ -1552,10 +1574,6 @@ void ivf_binary_search_device(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t s
             launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
             ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
         }
-    }
-    if (prof) {
-        g_scanned_bytes = read_stage_marks(ws, st) * nbp;
-        memset(g_filter_stats, 0, sizeof(g_filter_stats));
     }
 }
 
@@ -2516,6 +2534,15 @@ int lgpu_set_profiling(int enabled)
 int lgpu_last_stage_ms(float *times)
 {
     return guarded([&] { LGPU_REQUIRE(times, "null argument"); memcpy(times, g_stage_ms, sizeof(g_stage_ms)); });
+}
+
+int lgpu_debug_sub_batch_size(lgpu_index *ixh, uint32_t B, uint32_t nprobes, uint32_t *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(out && B > 0 && nprobes > 0, "bad argument");
+        HandleRef<lgpu_index> ix(ixh, "index");
+        *out = ivf_sub_batch_size(ix.h, B, nprobes);
+    });
 }
 
 static void check_ivf_call(lgpu_index *ix, const void *q, uint32_t B, const lgpu_search_params *p,

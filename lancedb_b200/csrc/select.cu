@@ -96,7 +96,12 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
         if (a.has_upper && !(v < a.upper)) return false;
         return true;
     };
-    // sort what is staged, keep the k best, tighten the threshold
+    // sort what is staged, keep the k best, tighten the threshold.  Whether to compact is decided inside the barrier that
+    // ends an iteration (__syncthreads_or: the last thread to arrive sees every append of the iteration), so the whole
+    // CTA takes the same branch.  Reading s_cnt after a plain barrier does not: a warp that skips the compaction goes on
+    // appending for the next iteration, a slower warp then reads a count at or above `trigger` and enters compact()
+    // alone, and the CTA's barriers no longer pair up -- seen as wrong rows, now and then, when the staged count lands
+    // right at the trigger (k = 432: 432 kept + about 432 of the next 1024 rows = 2 k)
     auto compact = [&]() {
         uint32_t cnt = s_cnt;
         uint32_t n2 = 2;
@@ -161,8 +166,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
 #pragma unroll
                 for (int u = 0; u < 4; u++) ok[u] = r + u < n;
                 offer4(v, ok, rowbase + r, a.row_ids, rowbase + r);
-                __syncthreads();
-                if (s_cnt >= trigger) compact();
+                if (__syncthreads_or(s_cnt >= trigger)) compact();
             }
         }
     } else if (a.mode == 1) {
@@ -182,8 +186,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
 #pragma unroll
             for (int u = 0; u < 4; u++) ok[u] = c + u < a.ncols;
             offer4(v, ok, c, a.col_ids, c);
-            __syncthreads();
-            if (s_cnt >= trigger) compact();
+            if (__syncthreads_or(s_cnt >= trigger)) compact();
         }
     } else {
         const uint64_t ncols = a.ncols_q ? min((uint64_t)a.ncols_q[q], a.ncols) : a.ncols;
@@ -229,8 +232,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
                     }
                 }
             }
-            __syncthreads();
-            if (s_cnt >= trigger) compact();
+            if (__syncthreads_or(s_cnt >= trigger)) compact();
         }
     }
     __syncthreads();

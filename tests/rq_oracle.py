@@ -121,13 +121,17 @@ def search(data, queries, k: int, nprobes: int, refine_factor: int = 0, lower=No
     return ids, dist, cnt
 
 
-def random_rq_index(rng, n=600, dim=24, nlist=6, metric="l2", with_vectors=True, empty=(1,), seed=7):
-    """A small IVF_RQ index with empty partitions `empty`, a few duplicate rows and non-contiguous row ids."""
+def random_rq_index(rng, n=600, dim=24, nlist=6, metric="l2", with_vectors=True, empty=(1,), seed=7,
+                    unit_centroids=False):
+    """A small IVF_RQ index with empty partitions `empty`, a few duplicate rows and non-contiguous row ids.
+    unit_centroids: centroids of length 1, so that a cosine index (rows normalised) fills every partition."""
     from lancedb_b200.index import IvfRqIndexData, rq_encode, rq_rotation
     x = rng.standard_normal((n, dim)).astype(f32)
     if n > 8:
         x[5:9] = x[4]                                    # duplicates: equal estimates, ordered by row id
     c = rng.standard_normal((nlist, dim)).astype(f32)
+    if unit_centroids:
+        c /= np.linalg.norm(c, axis=1, keepdims=True).astype(f32)
     for p in empty:
         c[p] += 100.0                                    # nothing lands here
     xs = x / np.linalg.norm(x, axis=1, keepdims=True).astype(f32) if metric == "cosine" else x

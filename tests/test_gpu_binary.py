@@ -74,7 +74,8 @@ def test_every_path_matches_the_oracle(nbytes):
 
 def test_list_path_sub_batches_inside_a_small_workspace_budget():
     """LGPU_WS_BYTES (read once per process, hence the subprocess) bounds the list path's workspace: at 1 MiB a batch
-    of 16 runs as sub-batches of 2 queries with a one-query fix-up matrix, and still returns the oracle's rows."""
+    of 16 runs as sub-batches of 2 queries with a one-query fix-up matrix, and still returns the oracle's rows.  (The
+    dense branch and the other search kinds under a small budget: tests/test_gpu_sub_batches.py.)"""
     import os
     import subprocess
     import sys

@@ -293,7 +293,8 @@ np.savez({dst!r}, i=i, d=d, c=c)
 
 def test_default_no_tensor_core_and_small_workspace_agree(tmp_path):
     """LGPU_WS_BYTES (read once per process, hence the subprocesses): at 1 MiB the batch runs as sub-batches of
-    queries, blocks of query vectors and many row chunks, and must return the same bits as the default run."""
+    queries, blocks of query vectors and many row chunks, and must return the same bits as the default run.  (The
+    other search kinds under a small budget: tests/test_gpu_sub_batches.py.)"""
     from tests.multivec_oracle import flat_search_mv as ref
     res = {}
     for name, extra in (("default", {}), ("notc", {"LGPU_NO_TENSOR_CORE": "1"}), ("ws", {"LGPU_WS_BYTES": str(1 << 20)})):
