@@ -123,7 +123,11 @@ int  lgpu_last_scanned_code_bytes(uint64_t *bytes);
 /* Search a batch of B queries held in HOST memory.  queries: [B][dim] f32.
  * out_ids/out_dist: [B][k] (`_rowid` / `_distance`, ascending by
  * (_distance,_rowid)); out_count: [B] valid entries per query; unused slots are
- * UINT64_MAX / +inf.  H2D and D2H copies happen inside the call. */
+ * UINT64_MAX / +inf.  H2D and D2H copies happen inside the call.
+ * Non-finite values (DESIGN.md section 0): a NaN _distance is never returned (refine included); +-inf distances are
+ * returned and ordered like any other; a partition whose coarse distance is NaN is never probed, so a query may have
+ * fewer than nprobes probes.  A NaN / inf centroid, or one whose |c|^2 overflows, keeps the coarse step on the exact
+ * kernels; a query whose tensor-core error band is not finite is redone by them. */
 int lgpu_search(lgpu_index *ix, const float *queries, uint32_t B,
                 const lgpu_search_params *params,
                 uint64_t *out_ids, float *out_dist, uint32_t *out_count);
@@ -312,7 +316,11 @@ int lgpu_kmeans_train(const float *x, uint64_t n, uint32_t dim, float *centroids
  * for dot); codebook [m][256][dim/m] in = initial codewords, out = trained */
 int lgpu_pq_train(const float *x, uint64_t n, uint32_t dim, uint32_t m, float *codebook, uint32_t iters, int device);
 
-/* ---- flat / brute force (LanceRead -> KNNVectorDistance -> TopK) --------- */
+/* ---- flat / brute force (LanceRead -> KNNVectorDistance -> TopK) ---------
+ * A column of at least 4096 rows with dim a multiple of 8 is scored on the tensor cores (l2, no prefilter or
+ * distance_range, B >= 8) with an exact re-score of every row inside the bf16 error band; a column holding a NaN or inf,
+ * or a row whose |x|^2 overflows, has no finite band and is always served by the exact kernels, and so is any query
+ * whose band is not finite.  NaN distances are never returned, +-inf ones are ordered like any other. */
 int  lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim,
                     const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device,
                     lgpu_flat **out);

@@ -91,7 +91,8 @@ struct DevBuf {
         bytes = want;
     }
     template <class T> T *as() { return reinterpret_cast<T *>(p); }
-    ~DevBuf() { if (p) cudaFree(p); }
+    void reset() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
+    ~DevBuf() { reset(); }
 };
 
 struct Workspace {
@@ -507,8 +508,10 @@ static bool tc_enabled()
     return v == 1;
 }
 
-// bf16 copy + squared norms + max norm and max bf16 rounding error |bf16(x) - x| of a row-major f32 matrix (open time)
-static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
+// bf16 copy + squared norms + max norm and max bf16 rounding error |bf16(x) - x| of a row-major f32 matrix (open time).
+// Returns false when a row holds a NaN or inf, or its |x|^2 or rounding error overflows: the error band (tc_band) is
+// then not finite for any query, and the caller leaves the operand to the exact kernels.
+static bool prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
                                cudaStream_t st)
 {
     Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
@@ -521,10 +524,12 @@ static void prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &X
     LGPU_CUDA(cudaMemcpyAsync(he.data(), err.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     LGPU_CUDA(cudaStreamSynchronize(st));
     float m = 0.f, me = 0.f;
-    for (float v : h) m = std::max(m, v);
-    for (float v : he) me = std::max(me, v);
+    bool finite = true;                        // (std::max skips a NaN: look at every value)
+    for (float v : h) { m = std::max(m, v); finite &= std::isfinite(v); }
+    for (float v : he) { me = std::max(me, v); finite &= std::isfinite(v); }
     xmax = std::sqrt(m) * 1.0001f;
     xerr = me;
+    return finite && std::isfinite(xmax);
 }
 
 // where a top-k goes: [B][k] ids and distances, [B] counts and, optionally, [B][k] storage positions
@@ -637,7 +642,7 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap;
     if (Ns == N) launch_filter_dense(Dbuf, lds, B, N, flt, st);      // the sample pass already scored every row
     else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt);
-    launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
+    launch_overflow_flags(ws->amax.as<uint32_t>(), cap, ws->probe_A.as<float>(), B, ws->flags.as<uint32_t>(), st);
     // 3. exact re-score of the admitted rows, final top-k; 4. fix-up of overflowed queries
     tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out, Dbuf, ld);
 }
@@ -1385,7 +1390,7 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
     flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap; flt.cand_s = ws->t_exact.as<float>();
     launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
-    launch_overflow_flags(ws->amax.as<uint32_t>(), cap, B, ws->flags.as<uint32_t>(), st);
+    launch_overflow_flags(ws->amax.as<uint32_t>(), cap, nullptr, B, ws->flags.as<uint32_t>(), st);
     // 3. top-k by (distance, id) of each list (an overflowed list is complete up to cap; its query is redone below)
     SelectArgs sb = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), cap, B, k, out);
     sb.ncols_q = ws->amax.as<uint32_t>();
@@ -1990,9 +1995,11 @@ static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t n
     if (vectors) { up(ix->vectors, vectors, (size_t)nrows * dim * 4); ix->has_vectors = true; }
     if (gemm_shape_supported(dim) && metric != LGPU_DOT) {
         LGPU_CUDA(cudaStreamSynchronize(st));
-        prepare_tc_operand(ix->centroids.as<float>(), nlist, dim, ix->cent_b, ix->cent_n2, ix->cent_max, ix->cent_err, st);
+        const bool finite =
+            prepare_tc_operand(ix->centroids.as<float>(), nlist, dim, ix->cent_b, ix->cent_n2, ix->cent_max, ix->cent_err, st);
+        if (!finite) { ix->cent_b.reset(); ix->cent_n2.reset(); }     // never read: the exact coarse kernels serve it
         ix->device_bytes += ix->cent_b.bytes + ix->cent_n2.bytes;
-        if (nlist >= 1024) {
+        if (finite && nlist >= 1024) {
             // every 8th centroid, for the sampled threshold of the coarse step (strided: whatever order the
             // trainer left the lists in -- hierarchical k-means groups neighbours -- the sample spans all of them)
             constexpr uint32_t COARSE_SAMPLE_STRIDE = 8;
@@ -2006,7 +2013,7 @@ static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t n
             ix->cent_ns = ns;
             ix->device_bytes += ix->cent_sb.bytes + ix->cent_sn2.bytes;
         }
-        ix->has_tc = true;
+        ix->has_tc = finite;                   // a non-finite centroid: the exact coarse kernels
     }
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
@@ -2250,6 +2257,7 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
             }
             ix->cb2 = (float)(cb2 * 1.000001);
         }
+        float rmax = 0.f;
         if (d->metric != LGPU_DOT) {   // per-row constants of the filter scan (tables.cu)
             ix->row_R.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));
             ix->rmax_bits.ensure(16);
@@ -2259,8 +2267,13 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
                              ix->cb_tiled.as<float>(), d->dim, d->m, ix->dsub, ix->row_R.as<float>(),
                              ix->rmax_bits.as<int>(), st);
             LGPU_CUDA(cudaStreamSynchronize(st));
+            int bits = 0;
+            LGPU_CUDA(cudaMemcpy(&bits, ix->rmax_bits.p, 4, cudaMemcpyDeviceToHost));
+            rmax = __builtin_bit_cast(float, bits);
         }
-        ix->has_tables = true;
+        // the filter scan's error band (kernels.cuh scan_band) is finite only with a finite CB2 and max |R|: a NaN / inf
+        // centroid or codeword leaves the index on the exact scan
+        ix->has_tables = std::isfinite(ix->cb2) && std::isfinite(rmax);
         register_handle(ix);
         *out = ix;
     });
@@ -2747,8 +2760,10 @@ int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uin
         fl->vectors.ensure(std::max<size_t>((size_t)nrows * dim * 4, 16));
         if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, (size_t)nrows * dim * 4, cudaMemcpyHostToDevice));
         if (gemm_shape_supported(dim) && nrows >= 4096) {
-            prepare_tc_operand(fl->vectors.as<float>(), nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max, fl->vec_err, nullptr);
-            fl->has_tc = true;
+            // a non-finite or overflowing row: the exact kernels serve the column
+            fl->has_tc = prepare_tc_operand(fl->vectors.as<float>(), nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
+                                            fl->vec_err, nullptr);
+            if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
         }
         open_rows(fl, row_ids, nrows);
         register_handle(fl);
@@ -3445,12 +3460,12 @@ static void assign_nearest(const float *d_x, uint64_t n, uint32_t dim, const flo
     const uint64_t CH = std::max<uint64_t>(256, std::min<uint64_t>(65536, ((uint64_t)1 << 28) / (ld * 4)));
     DevBuf D, cnt, flags, gate, xb, xn2, xerr, cb, cn2;
     D.ensure((size_t)CH * ld * 4); cnt.ensure((size_t)CH * 4);
-    const bool tc = gemm_shape_supported(dim) && k >= 256 && tc_enabled();
+    bool tc = gemm_shape_supported(dim) && k >= 256 && tc_enabled();
     float cmax = 0.f, cerr = 0.f;
     if (tc) {
         flags.ensure((size_t)CH * 4); gate.ensure(16);
         xb.ensure((size_t)CH * dim * 2); xn2.ensure((size_t)CH * 4); xerr.ensure((size_t)CH * 4);
-        prepare_tc_operand(d_cent, k, dim, cb, cn2, cmax, cerr, st);
+        tc = prepare_tc_operand(d_cent, k, dim, cb, cn2, cmax, cerr, st);
     }
     for (uint64_t r0 = 0; r0 < n; r0 += CH) {
         const uint32_t b = (uint32_t)std::min<uint64_t>(CH, n - r0);

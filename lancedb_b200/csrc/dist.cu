@@ -349,10 +349,12 @@ __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *
     if (lane == 0) { atomicMin(&s_lo, kmin); atomicMax(&s_hi, kmax); atomicAdd(&s_valid, nv); }
     __syncthreads();
     const uint32_t kk = min(k, s_valid);
+    // a non-finite query (inf, NaN, |q|^2 overflowing) has no finite band: its scores prove nothing, the caller redoes it
+    const float E = tc_band(qn2[q], qerr[q], xmax, xerr, d);
+    const bool band_ok = isfinite(E);
     float thr = -CUDART_INF_F;
-    if (kk > 0) {
+    if (kk > 0 && band_ok) {
         float lo = key_f32(s_lo), hi = key_f32(s_hi);               // invariant: count(S <= hi) >= kk
-        const float E = tc_band(qn2[q], qerr[q], xmax, xerr, d);
         if (hi < CUDART_INF_F && lo > -CUDART_INF_F) {
             for (int it = 0; it < 20 && hi - lo > 0.25f * E; it++) {    // the band is 2E wide anyway
                 const float mid = 0.5f * lo + 0.5f * hi;
@@ -393,7 +395,7 @@ __global__ void __launch_bounds__(CF_THREADS) coarse_finish_kernel(const float *
     __syncthreads();
     const uint32_t total = s_n, n = min(total, cap);
     if (tid == 0) {
-        const bool redo = total > cap || listed > ld;               // (a list that overflowed is not a superset)
+        const bool redo = total > cap || listed > ld || !band_ok;   // (a list that overflowed is not a superset)
         flags[q] = redo ? 1u : 0u;
         if (redo && gate) *gate = 1u;                               // opens the gate of the caller's exact fix-up
     }

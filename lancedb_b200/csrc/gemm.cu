@@ -504,8 +504,10 @@ __global__ void band_check_kernel(const float *__restrict__ approx, const uint32
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
     uint32_t f = 0;
-    if (cnt[q] >= kp && kp > 0) {              // list is full: columns beyond it may exist
-        const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
+    const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
+    if (!isfinite(E)) {                        // a non-finite query: its NaN scores never reached the list
+        f = 1u;
+    } else if (cnt[q] >= kp && kp > 0) {       // list is full: columns beyond it may exist
         const float kth = approx[(size_t)q * kp + (k - 1 < kp ? k - 1 : kp - 1)];
         const float last = approx[(size_t)q * kp + kp - 1];
         f = (k >= kp || !(last > kth + 2.0f * E)) ? 1u : 0u;
@@ -514,18 +516,19 @@ __global__ void band_check_kernel(const float *__restrict__ approx, const uint32
 }
 
 // thr[q] = (k-th smallest approximate score of the sample) + 2 E_q, or +inf when the sample holds < k rows;
-// every true top-k row of the full set has a score <= thr[q] (E_q: tc_band)
+// every true top-k row of the full set has a score <= thr[q] (E_q: tc_band).  A query whose E_q is not finite gets
+// thr[q] = NaN: the filtering epilogue admits nothing for it and the consumer flags it for the exact fix-up
+// (overflow_flags_kernel, coarse_finish_kernel)
 __global__ void sample_threshold_kernel(const float *__restrict__ approx, const uint32_t *__restrict__ cnt,
                                         const float *__restrict__ qnorm2, const float *__restrict__ qerr, float xmax,
                                         float xerr, uint32_t d, uint32_t B, uint32_t k, float *__restrict__ thr)
 {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
+    const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
     float t = __int_as_float(0x7f800000);
-    if (cnt[q] >= k) {
-        const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
-        t = approx[(size_t)q * k + k - 1] + 2.0f * E;
-    }
+    if (!isfinite(E)) t = __int_as_float(0x7fc00000);
+    else if (cnt[q] >= k) t = approx[(size_t)q * k + k - 1] + 2.0f * E;
     thr[q] = t;
 }
 // The same threshold straight from the dense sample scores D[B][ld] (ns columns), one warp per query: the k-th smallest
@@ -570,9 +573,11 @@ __global__ void __launch_bounds__(128) sample_kth_threshold_kernel(const float *
         lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o)); hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
     }
     nv = __reduce_add_sync(0xffffffffu, nv);
+    const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
     float t = __int_as_float(0x7f800000);
-    if (nv >= k && hi < __int_as_float(0x7f800000) && lo > -__int_as_float(0x7f800000)) {
-        const float E = tc_band(qnorm2[q], qerr[q], xmax, xerr, d);
+    if (!isfinite(E)) {
+        t = __int_as_float(0x7fc00000);                                 // NaN: as sample_threshold_kernel
+    } else if (nv >= k && hi < __int_as_float(0x7f800000) && lo > -__int_as_float(0x7f800000)) {
         for (int it = 0; it < 24 && hi - lo > 0.25f * E; it++) {        // invariant: count(S <= hi) >= k
             const float mid = 0.5f * lo + 0.5f * hi;
             uint32_t c = 0;
@@ -586,10 +591,12 @@ __global__ void __launch_bounds__(128) sample_kth_threshold_kernel(const float *
     if (lane == 0) thr[q] = t;
 }
 
-__global__ void overflow_flags_kernel(const uint32_t *__restrict__ count, uint32_t cap, uint32_t B, uint32_t *__restrict__ flags)
+// flags[q]: the query's list overflowed, or its threshold is NaN (the band was not finite: nothing was admitted)
+__global__ void overflow_flags_kernel(const uint32_t *__restrict__ count, uint32_t cap, const float *__restrict__ thr,
+                                      uint32_t B, uint32_t *__restrict__ flags)
 {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q < B) flags[q] = count[q] > cap ? 1u : 0u;
+    if (q < B) flags[q] = count[q] > cap || (thr && thr[q] != thr[q]) ? 1u : 0u;
 }
 
 }  // namespace
@@ -615,10 +622,11 @@ bool launch_sample_kth_threshold(const float *D, uint64_t ld, uint32_t ns, const
     return true;
 }
 
-void launch_overflow_flags(const uint32_t *count, uint32_t cap, uint32_t B, uint32_t *flags, cudaStream_t st)
+void launch_overflow_flags(const uint32_t *count, uint32_t cap, const float *thr, uint32_t B, uint32_t *flags,
+                           cudaStream_t st)
 {
     if (B == 0) return;
-    overflow_flags_kernel<<<(B + 127) / 128, 128, 0, st>>>(count, cap, B, flags); LGPU_COUNT_LAUNCH();
+    overflow_flags_kernel<<<(B + 127) / 128, 128, 0, st>>>(count, cap, thr, B, flags); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

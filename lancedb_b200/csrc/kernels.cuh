@@ -323,7 +323,9 @@ void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *nor
 // bf16(q).bf16(x) - q.x = bf16(q).(bf16(x) - x) + (bf16(q) - q).x and |bf16(q)| <= |q| + r_q; 2^-10 covers the f32
 // arithmetic of the r's and of E_q itself, the last term the f32 sums (|x|^2, the accumulation, the exact re-score).
 // Both operands round: r can reach 2^-8 of the norm each, so E_q reaches ~2^-6 |q| xmax on adversarial data.  Every
-// consumer (band check, sample thresholds, coarse finishing kernel) takes its band from here.
+// consumer (band check, sample thresholds, coarse finishing kernel) takes its band from here.  A non-finite query (or
+// one whose |q|^2 overflows) makes E_q inf or NaN: every consumer then hands the query to the exact kernels.  The
+// operand's xmax and xerr are finite by construction: an operand without a finite bound gets no tensor-core copy.
 __device__ __forceinline__ float tc_band(float qnorm2, float qerr, float xmax, float xerr, uint32_t d)
 {
     const float qn = sqrtf(qnorm2), s = qn + xmax;
@@ -422,14 +424,18 @@ void launch_mv_rowsum(const float *M, uint64_t ldM, const uint32_t *q_off, uint3
 // (only: optional [B] per-query flags indexed like q_off, queries whose flag is 0 are skipped)
 // filtering epilogue on an existing dense score matrix D[B][ld] (see gemm.cu)
 void launch_filter_dense(const float *D, uint64_t ld, uint32_t B, uint64_t N, const GemmFilter &flt, cudaStream_t st);
+// thr[q] = k-th smallest sample score + 2 E_q (+inf: fewer than k scores; NaN: E_q is not finite, see tc_band)
 void launch_sample_threshold(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,
                              float xerr, uint32_t d, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
 // the same threshold straight from dense sample scores D[B][ld] (ns <= 4096 columns; false = shape not handled)
 bool launch_sample_kth_threshold(const float *D, uint64_t ld, uint32_t ns, const float *qnorm2, const float *qerr, float xmax,
                                  float xerr, uint32_t d, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
-void launch_overflow_flags(const uint32_t *count, uint32_t cap, uint32_t B, uint32_t *flags, cudaStream_t st);
+// flags[q] = count[q] > cap, or thr[q] is NaN (thr optional)
+void launch_overflow_flags(const uint32_t *count, uint32_t cap, const float *thr, uint32_t B, uint32_t *flags,
+                           cudaStream_t st);
 // flags[q] = 1 when the approximate shortlist of query q cannot be proven to contain the exact top-k:
-// approx[q][0..kp) ascending, cnt[q] entries valid; proven iff cnt < kp or approx[kp-1] > approx[k-1] + 2E_q (tc_band)
+// approx[q][0..kp) ascending, cnt[q] entries valid; proven iff E_q is finite and cnt < kp or
+// approx[kp-1] > approx[k-1] + 2E_q (tc_band)
 void launch_band_check(const float *approx, const uint32_t *cnt, const float *qnorm2, const float *qerr, float xmax,
                        float xerr, uint32_t d, uint32_t B, uint32_t k, uint32_t kp, uint32_t *flags, cudaStream_t st);
 

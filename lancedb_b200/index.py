@@ -207,8 +207,14 @@ def _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes
     them), a training sample of sample_rate rows per partition, k-means centroids and every row's partition.
     native_passes: the Lloyd loops and the assignment run in the library's kernels (lgpu_kmeans_train /
     lgpu_ivf_assign), so a row lands in the partition its own vector probes first.
-    Returns (x normalised for cosine, sample, centroids, assign, device ordinal)."""
+    Returns (x normalised for cosine, sample, centroids, assign, device ordinal).
+    A NaN or infinite component anywhere is refused: k-means would spread it into a centroid, and a row with no finite
+    centroid distance has no partition."""
     import torch
+    bad = ~torch.isfinite(x).all(dim=1)
+    if bool(bad.any()):
+        raise ValueError(f"vector {int(bad.nonzero()[0, 0])} holds a NaN or infinite value; IVF training needs finite "
+                         f"vectors")
     n = x.shape[0]
     raw = x
     if metric == "cosine":

@@ -134,11 +134,15 @@ float orc_l2_subvec(const float *x, const float *y, size_t dsub)
 
 /* ------------------------------------------------------------------------ */
 /* (distance, id) ordering: `_distance ASC, _rowid ASC`, the tie-break the
- * reference pins for TopK at python/python/lancedb/query.py:1366-1368.      */
+ * reference pins for TopK at python/python/lancedb/query.py:1366-1368.
+ * A NaN distance sorts after every number (ties by id), so the order stays a
+ * strict weak order whatever the data holds; +-inf are ordinary values.     */
 typedef struct { float d; uint64_t id; uint64_t pos; } cand_t;
 
 static inline int cand_less(const cand_t *a, const cand_t *b)
 {
+    const int an = a->d != a->d, bn = b->d != b->d;
+    if (an != bn) return bn;
     if (a->d < b->d) return 1;
     if (a->d > b->d) return 0;
     return a->id < b->id;
@@ -223,7 +227,8 @@ void orc_find_partitions(const orc_index *ix, const float *q, uint32_t nprobes,
         c[p].id = p; c[p].pos = p;
         if (all_dists) all_dists[p] = c[p].d;
     }
-    /* sort_to_indices(dists, limit = nprobes): ascending; ties by partition id */
+    /* sort_to_indices(dists, limit = nprobes): ascending; ties by partition id; NaN distances last (the
+     * search loops never probe them: DESIGN.md section 0, rule c) */
     qsort(c, nlist, sizeof(cand_t), cand_cmp);
     for (uint32_t j = 0; j < nprobes; j++) {
         out_parts[j] = (uint32_t)c[j].id;
@@ -309,9 +314,15 @@ typedef struct {
     size_t max_part;
 } ivf_job;
 
+/* a NaN distance is never returned (FilterExec: _distance IS NOT NULL); only the
+ * refine's exact distances can still be NaN here */
 static void emit(const orc_params *p, heap_t *h, uint64_t *ids, float *dist,
                  uint32_t *count)
 {
+    uint32_t kept = 0;
+    for (uint32_t j = 0; j < h->n; j++)
+        if (h->a[j].d == h->a[j].d) h->a[kept++] = h->a[j];
+    h->n = kept;
     qsort(h->a, h->n, sizeof(cand_t), cand_cmp);
     uint32_t n = h->n < p->k ? h->n : p->k;
     for (uint32_t j = 0; j < p->k; j++) {
@@ -339,6 +350,7 @@ static void *ivf_worker(void *arg)
     float *lut = (float *)malloc(sizeof(float) * ix->m * 256);
     float *dists = (float *)malloc(sizeof(float) * (job->max_part ? job->max_part : 1));
     uint32_t *parts = (uint32_t *)malloc(sizeof(uint32_t) * (nprobes_max ? nprobes_max : 1));
+    float *pd = (float *)malloc(sizeof(float) * (nprobes_max ? nprobes_max : 1));
     heap_t h; h.a = (cand_t *)malloc(sizeof(cand_t) * (kk ? kk : 1)); h.cap = kk;
 
     for (uint32_t qi = job->q0; qi < job->q1; qi++) {
@@ -346,9 +358,10 @@ static void *ivf_worker(void *arg)
         if (ix->metric == ORC_COSINE) orc_normalize_f32(q, dim, qn);
         else memcpy(qn, q, sizeof(float) * dim);
         for (uint32_t np_use = nprobes;;) {
-            orc_find_partitions(ix, qn, np_use, parts, NULL, NULL);
+            orc_find_partitions(ix, qn, np_use, parts, pd, NULL);
             h.n = 0;
             for (uint32_t j = 0; j < np_use; j++) {
+                if (pd[j] != pd[j]) continue;              /* a NaN coarse distance is never probed */
                 uint32_t part = parts[j];
                 size_t off = ix->part_offsets[part], n = ix->part_offsets[part + 1] - off;
                 if (n == 0) continue;
@@ -369,7 +382,7 @@ static void *ivf_worker(void *arg)
         emit(p, &h, job->out_ids + (size_t)qi * p->k, job->out_dist + (size_t)qi * p->k,
              job->out_count + qi);
     }
-    free(qn); free(lut); free(dists); free(parts); free(h.a);
+    free(qn); free(lut); free(dists); free(parts); free(pd); free(h.a);
     return NULL;
 }
 

@@ -125,9 +125,11 @@ def ivfpq_search_one(ix, q, k, nprobes, lower=None, upper=None, allowed=None):
         cd = np.array([f32(f32(1) - dot(qn, c)) for c in ix.centroids], f32)
     else:
         cd = np.array([l2(qn, c) for c in ix.centroids], f32)
-    order = np.lexsort((np.arange(ix.nlist), cd))[:min(nprobes, ix.nlist)]
+    order = np.lexsort((np.arange(ix.nlist), cd))[:min(nprobes, ix.nlist)]     # NaN last
     cands = []
     for p in order:
+        if np.isnan(cd[p]):                 # a NaN coarse distance is never probed
+            continue
         a, b = int(ix.part_offsets[p]), int(ix.part_offsets[p + 1])
         if a == b:
             continue
@@ -140,6 +142,8 @@ def ivfpq_search_one(ix, q, k, nprobes, lower=None, upper=None, allowed=None):
         elif ix.metric == "dot":
             d = (d - f32(ix.m - 1)).astype(f32)
         for r in range(b - a):
+            if np.isnan(d[r]):                  # _distance IS NOT NULL
+                continue
             if lower is not None and not d[r] >= f32(lower):
                 continue
             if upper is not None and not d[r] < f32(upper):

@@ -314,7 +314,8 @@ def pq4_search_np(data, queries, k: int, nprobes: int, refine_factor: int = 0, l
         cands = cands[:kk]
         if refine_factor and data.vectors is not None:
             dfun = {"cosine": onp.cosine, "l2": onp.l2, "dot": lambda x, y: f32(f32(1) - onp.dot(x, y))}[data.metric]
-            cands = sorted((dfun(q[b], data.vectors[pos]), rid, pos) for _, rid, pos in cands)
+            cands = [(dfun(q[b], data.vectors[pos]), rid, pos) for _, rid, pos in cands]
+            cands = sorted(c for c in cands if not np.isnan(c[0]))     # a NaN distance is never returned
         n = min(k, len(cands))
         ids[b, :n] = [c[1] for c in cands[:n]]
         dist[b, :n] = [c[0] for c in cands[:n]]

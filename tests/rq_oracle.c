@@ -86,6 +86,8 @@ typedef struct { float d; uint64_t id, pos; } cand;
 static int cand_cmp(const void *a, const void *b)
 {
     const cand *x = (const cand *)a, *y = (const cand *)b;
+    const int xn = x->d != x->d, yn = y->d != y->d;   /* NaN after every number: a strict weak order */
+    if (xn != yn) return xn ? 1 : -1;
     if (x->d < y->d) return -1;
     if (x->d > y->d) return 1;
     return x->id < y->id ? -1 : (x->id > y->id ? 1 : 0);
@@ -158,7 +160,13 @@ static void *worker(void *arg)
         qsort(c, nc, sizeof(cand), cand_cmp);
         if (nc > kk) nc = kk;
         if (p->refine_factor && ix->vectors) {
-            for (uint64_t i = 0; i < nc; i++) c[i].d = orc_distance_f32(ix->metric, q, ix->vectors + c[i].pos * dim, dim);
+            uint64_t kept = 0;                     /* a NaN exact distance is never returned */
+            for (uint64_t i = 0; i < nc; i++) {
+                c[kept] = c[i];
+                c[kept].d = orc_distance_f32(ix->metric, q, ix->vectors + c[i].pos * dim, dim);
+                if (c[kept].d == c[kept].d) kept++;
+            }
+            nc = kept;
             qsort(c, nc, sizeof(cand), cand_cmp);
         }
         const uint32_t cnt = (uint32_t)(nc < p->k ? nc : p->k);

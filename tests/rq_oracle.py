@@ -261,7 +261,8 @@ def rq_search_np(data, queries, k: int, nprobes: int, refine_factor: int = 0, lo
         cands = cands[:kk]
         if refine_factor and data.vectors is not None:
             dfun = onp.cosine if data.metric == "cosine" else onp.l2
-            cands = sorted((dfun(q[b], data.vectors[pos]), rid, pos) for _, rid, pos in cands)
+            cands = [(dfun(q[b], data.vectors[pos]), rid, pos) for _, rid, pos in cands]
+            cands = sorted(c for c in cands if not np.isnan(c[0]))     # a NaN distance is never returned
         n = min(k, len(cands))
         ids[b, :n] = [c[1] for c in cands[:n]]
         dist[b, :n] = [c[0] for c in cands[:n]]
