@@ -1,4 +1,4 @@
-"""ctypes loader for the CPU oracle (oracle/oracle.c).
+"""ctypes loader for the CPU oracle (oracle/oracle.c and the index kinds' oracles, tests/*_oracle.c).
 
 TEST INFRASTRUCTURE ONLY.  May be imported by tests/, __graft_entry__.smoke()
 and bench.py's cpu_baseline / ``--impl reference`` legs -- never by
@@ -56,13 +56,49 @@ def _params(k, nprobes, refine_factor, lower, upper, allow=None, allow_bits=0, m
 
 
 def build(force: bool = False) -> str:
-    """Compile oracle.c with gcc (flags in oracle/Makefile)."""
-    src = os.path.join(_HERE, "oracle.c")
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(
-        os.path.getmtime(src), os.path.getmtime(os.path.join(_HERE, "oracle.h"))
-    ):
-        subprocess.run(["make", "-C", _HERE, "-s"], check=True)
+    """Compile oracle.c and the index kinds' oracles under tests/ into one library with gcc (flags and sources in
+    oracle/Makefile; make rebuilds it when a source is newer)."""
+    subprocess.run(["make", "-C", _HERE, "-s"] + (["-B"] if force else []), check=True)
     return _LIB_PATH
+
+
+_IX, _P = C.POINTER(_Index), C.POINTER(_Params)
+_vp, _u8, _u32, _u64, _int, _f, _d, _sz = (C.c_void_p, C.c_uint8, C.c_uint32, C.c_uint64, C.c_int, C.c_float,
+                                           C.c_double, C.c_size_t)
+# name: (restype, argtypes); every search ends in (queries, B, &params, ids, dist, count, nthreads)
+_SIGNATURES = {
+    "orc_l2_f32": (_f, [_vp, _vp, _sz]),
+    "orc_dot_f32": (_f, [_vp, _vp, _sz]),
+    "orc_cosine_f32": (_f, [_vp, _vp, _sz]),
+    "orc_distance_f32": (_f, [_int, _vp, _vp, _sz]),
+    "orc_l2_subvec": (_f, [_vp, _vp, _sz]),
+    "orc_normalize_f32": (None, [_vp, _sz, _vp]),
+    "orc_find_partitions": (None, [_IX, _vp, _u32, _vp, _vp, _vp]),
+    "orc_build_lut": (None, [_IX, _vp, _vp]),
+    "orc_pq_scan": (None, [_vp, _vp, _sz, _u32, _vp]),
+    "orc_partition_distances": (None, [_IX, _vp, _u32, _vp]),
+    "orc_ivf_assign": (None, [_IX, _vp, _u64, _vp]),
+    "orc_pq_encode": (None, [_IX, _vp, _vp, _u64, _vp]),
+    "orc_ivfpq_search": (_int, [_IX, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_flat_search": (_int, [_vp, _u64, _u32, _vp, _int, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_sq_encode": (None, [_vp, _u64, _d, _d, _vp]),
+    "orc_sq_distance": (_f, [_vp, _vp, _u32]),
+    "orc_sq_search": (_int, [_IX, _vp, _d, _d, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_rq_rotate": (None, [_vp, _vp, _u64, _u32, _vp]),
+    "orc_rq_slot": (None, [_vp, _vp, _u32, _vp, _vp, _vp, _vp]),
+    "orc_rq_estimate": (_f, [_vp, _f, _f, _vp, _vp, _u32, _u32, _int]),
+    "orc_rq_search": (_int, [_IX, _vp, _vp, _vp, _vp, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_pq4_quant": (_u8, [_f, _f, _f]),
+    "orc_pq4_distance": (_f, [_u32, _f, _f, _u32, _int]),
+    "orc_pq4_tables": (None, [_IX, _vp, _u32, _vp, _vp]),
+    "orc_pq4_partition_distances": (None, [_IX, _vp, _u32, _vp]),
+    "orc_pq4_search": (_int, [_IX, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_ivf_binary_search": (_int, [_vp, _u32, _vp, _vp, _vp, _u32, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_hamming_u8": (_int, [_vp, _u32, _vp, _u64, _u32, _vp, _int]),
+    "orc_flat_search_u8": (_int, [_vp, _u64, _u32, _vp, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+    "orc_multivec_distances": (_int, [_vp, _vp, _u64, _u32, _vp, _vp, _u32, _vp, _int]),
+    "orc_multivec_search": (_int, [_vp, _vp, _u64, _u32, _vp, _vp, _vp, _u32, _P, _vp, _vp, _vp, _int]),
+}
 
 
 def load():
@@ -71,39 +107,34 @@ def load():
         return _lib
     build()
     lib = C.CDLL(_LIB_PATH)
-    f32p, vp = C.POINTER(C.c_float), C.c_void_p
-    lib.orc_l2_f32.restype = C.c_float
-    lib.orc_l2_f32.argtypes = [vp, vp, C.c_size_t]
-    lib.orc_dot_f32.restype = C.c_float
-    lib.orc_dot_f32.argtypes = [vp, vp, C.c_size_t]
-    lib.orc_cosine_f32.restype = C.c_float
-    lib.orc_cosine_f32.argtypes = [vp, vp, C.c_size_t]
-    lib.orc_distance_f32.restype = C.c_float
-    lib.orc_distance_f32.argtypes = [C.c_int, vp, vp, C.c_size_t]
-    lib.orc_l2_subvec.restype = C.c_float
-    lib.orc_l2_subvec.argtypes = [vp, vp, C.c_size_t]
-    lib.orc_normalize_f32.restype = None
-    lib.orc_normalize_f32.argtypes = [vp, C.c_size_t, vp]
-    lib.orc_find_partitions.restype = None
-    lib.orc_find_partitions.argtypes = [C.POINTER(_Index), vp, C.c_uint32, vp, vp, vp]
-    lib.orc_build_lut.restype = None
-    lib.orc_build_lut.argtypes = [C.POINTER(_Index), vp, vp]
-    lib.orc_pq_scan.restype = None
-    lib.orc_pq_scan.argtypes = [vp, vp, C.c_size_t, C.c_uint32, vp]
-    lib.orc_partition_distances.restype = None
-    lib.orc_partition_distances.argtypes = [C.POINTER(_Index), vp, C.c_uint32, vp]
-    lib.orc_ivf_assign.argtypes = [C.POINTER(_Index), vp, C.c_uint64, vp]
-    lib.orc_ivf_assign.restype = None
-    lib.orc_pq_encode.argtypes = [C.POINTER(_Index), vp, vp, C.c_uint64, vp]
-    lib.orc_pq_encode.restype = None
-    lib.orc_ivfpq_search.restype = C.c_int
-    lib.orc_ivfpq_search.argtypes = [C.POINTER(_Index), vp, C.c_uint32, C.POINTER(_Params), vp, vp, vp, C.c_int]
-    lib.orc_flat_search.restype = C.c_int
-    lib.orc_flat_search.argtypes = [vp, C.c_uint64, C.c_uint32, vp, C.c_int, vp, C.c_uint32,
-                                    C.POINTER(_Params), vp, vp, vp, C.c_int]
-    del f32p
+    for name, (res, args) in _SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = res, args
     _lib = lib
     return lib
+
+
+def threads(nthreads) -> int:
+    """nthreads, or every host core for 0"""
+    return int(nthreads) if nthreads else (os.cpu_count() or 1)
+
+
+def search_call(name, args, B, k, nthreads=0, nprobes=0, refine_factor=0, lower=None, upper=None, allow=None,
+                allow_bits=0, max_nprobes=0):
+    """Runs the C search `name`(*args, B, &orc_params, ids, dist, count, nthreads) and returns (ids [B, k] u64,
+    dist [B, k] f32, count [B] u32).  allow: a u32 bitmap of allow_bits bits, or a bool mask over row ids."""
+    if allow is not None:
+        allow = np.asarray(allow)
+        if allow.dtype == bool:
+            allow, allow_bits = allow_bitmap(np.nonzero(allow)[0], allow.size), allow.size
+        allow = np.ascontiguousarray(allow, np.uint32)
+    p = _params(k, nprobes, refine_factor, lower, upper, allow, allow_bits, max_nprobes)
+    ids = np.empty((B, k), np.uint64)
+    dist = np.empty((B, k), np.float32)
+    cnt = np.empty(B, np.uint32)
+    if B and getattr(load(), name)(*args, B, C.byref(p), _ptr(ids), _ptr(dist), _ptr(cnt), threads(nthreads)):
+        raise RuntimeError(f"{name} failed")
+    return ids, dist, cnt
 
 
 def _f32(a):
@@ -202,17 +233,8 @@ class OracleIndex:
     def search(self, queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None, nthreads=1,
                allow=None, allow_bits=0, max_nprobes=0):
         q = _f32(queries).reshape(-1, self.dim)
-        B = q.shape[0]
-        allow = None if allow is None else np.ascontiguousarray(allow, np.uint32)
-        p = _params(k, nprobes, refine_factor, lower, upper, allow, allow_bits, max_nprobes)
-        ids = np.empty((B, k), np.uint64)
-        dist = np.empty((B, k), np.float32)
-        cnt = np.empty(B, np.uint32)
-        rc = load().orc_ivfpq_search(C.byref(self.c), _ptr(q), B, C.byref(p), _ptr(ids), _ptr(dist),
-                                     _ptr(cnt), nthreads)
-        if rc:
-            raise RuntimeError(f"orc_ivfpq_search rc={rc}")
-        return ids, dist, cnt
+        return search_call("orc_ivfpq_search", (C.byref(self.c), _ptr(q)), q.shape[0], k, nthreads, nprobes,
+                           refine_factor, lower, upper, allow, allow_bits, max_nprobes)
 
 
 def flat_search(vectors, queries, k=10, metric="l2", row_ids=None, lower=None, upper=None, nthreads=1,
@@ -220,18 +242,9 @@ def flat_search(vectors, queries, k=10, metric="l2", row_ids=None, lower=None, u
     v = _f32(vectors)
     n, dim = v.shape
     q = _f32(queries).reshape(-1, dim)
-    B = q.shape[0]
     rid = np.ascontiguousarray(row_ids, dtype=np.uint64) if row_ids is not None else None
-    allow = None if allow is None else np.ascontiguousarray(allow, np.uint32)
-    p = _params(k, 0, 0, lower, upper, allow, allow_bits)
-    ids = np.empty((B, k), np.uint64)
-    dist = np.empty((B, k), np.float32)
-    cnt = np.empty(B, np.uint32)
-    rc = load().orc_flat_search(_ptr(v), n, dim, _ptr(rid), METRICS[metric], _ptr(q), B, C.byref(p),
-                                _ptr(ids), _ptr(dist), _ptr(cnt), nthreads)
-    if rc:
-        raise RuntimeError(f"orc_flat_search rc={rc}")
-    return ids, dist, cnt
+    return search_call("orc_flat_search", (_ptr(v), n, dim, _ptr(rid), METRICS[metric], _ptr(q)), q.shape[0], k,
+                       nthreads, lower=lower, upper=upper, allow=allow, allow_bits=allow_bits)
 
 
 def pq_scan(lut, codes_t, n, m):

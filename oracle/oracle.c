@@ -137,9 +137,7 @@ float orc_l2_subvec(const float *x, const float *y, size_t dsub)
  * reference pins for TopK at python/python/lancedb/query.py:1366-1368.
  * A NaN distance sorts after every number (ties by id), so the order stays a
  * strict weak order whatever the data holds; +-inf are ordinary values.     */
-typedef struct { float d; uint64_t id; uint64_t pos; } cand_t;
-
-static inline int cand_less(const cand_t *a, const cand_t *b)
+static inline int cand_less(const orc_cand *a, const orc_cand *b)
 {
     const int an = a->d != a->d, bn = b->d != b->d;
     if (an != bn) return bn;
@@ -148,36 +146,42 @@ static inline int cand_less(const cand_t *a, const cand_t *b)
     return a->id < b->id;
 }
 
+static int cand_cmp(const void *pa, const void *pb)
+{
+    const orc_cand *a = (const orc_cand *)pa, *b = (const orc_cand *)pb;
+    if (cand_less(a, b)) return -1;
+    if (cand_less(b, a)) return 1;
+    return 0;
+}
+
 /* bounded max-heap of the k smallest (lance-index flat/index.rs keeps a
  * BinaryHeap of k with strict `<` [lance, recalled]; partitions here are in
  * ascending row-id scan order, so "first seen wins a tie" == smaller row id) */
-typedef struct { cand_t *a; uint32_t n, cap; } heap_t;
-
-static void heap_sift_up(heap_t *h, uint32_t i)
+static void heap_sift_up(orc_topk *h, uint32_t i)
 {
     while (i > 0) {
         uint32_t p = (i - 1) / 2;
         if (cand_less(&h->a[p], &h->a[i])) {
-            cand_t t = h->a[p]; h->a[p] = h->a[i]; h->a[i] = t; i = p;
+            orc_cand t = h->a[p]; h->a[p] = h->a[i]; h->a[i] = t; i = p;
         } else break;
     }
 }
 
-static void heap_sift_down(heap_t *h, uint32_t i)
+static void heap_sift_down(orc_topk *h, uint32_t i)
 {
     for (;;) {
         uint32_t l = 2 * i + 1, r = l + 1, m = i;
         if (l < h->n && cand_less(&h->a[m], &h->a[l])) m = l;
         if (r < h->n && cand_less(&h->a[m], &h->a[r])) m = r;
         if (m == i) break;
-        cand_t t = h->a[m]; h->a[m] = h->a[i]; h->a[i] = t; i = m;
+        orc_cand t = h->a[m]; h->a[m] = h->a[i]; h->a[i] = t; i = m;
     }
 }
 
-static inline void heap_offer(heap_t *h, float d, uint64_t id, uint64_t pos)
+void orc_topk_offer(orc_topk *h, float d, uint64_t id, uint64_t pos)
 {
     if (h->cap == 0) return;
-    cand_t c = { d, id, pos };
+    orc_cand c = { d, id, pos };
     if (h->n < h->cap) {
         h->a[h->n] = c; heap_sift_up(h, h->n); h->n++;
     } else if (cand_less(&c, &h->a[0])) {
@@ -185,26 +189,75 @@ static inline void heap_offer(heap_t *h, float d, uint64_t id, uint64_t pos)
     }
 }
 
-static int cand_cmp(const void *pa, const void *pb)
+/* a NaN distance is never returned (FilterExec: _distance IS NOT NULL); the
+ * row filter has dropped them already, only refine's exact distances can
+ * still be NaN here */
+void orc_topk_emit(const orc_params *p, orc_topk *h, uint64_t *ids, float *dist, uint32_t *count)
 {
-    const cand_t *a = (const cand_t *)pa, *b = (const cand_t *)pb;
-    if (cand_less(a, b)) return -1;
-    if (cand_less(b, a)) return 1;
-    return 0;
+    uint32_t kept = 0;
+    for (uint32_t j = 0; j < h->n; j++)
+        if (h->a[j].d == h->a[j].d) h->a[kept++] = h->a[j];
+    h->n = kept;
+    qsort(h->a, h->n, sizeof(orc_cand), cand_cmp);
+    uint32_t n = h->n < p->k ? h->n : p->k;
+    for (uint32_t j = 0; j < p->k; j++) {
+        ids[j] = j < n ? h->a[j].id : UINT64_MAX;
+        dist[j] = j < n ? h->a[j].d : INFINITY;
+    }
+    *count = n;
 }
 
-static inline int allowed(const orc_params *p, uint64_t id)
+void orc_nearest(const float *d, uint32_t n, uint32_t nprobes, uint32_t *out_idx, float *out_d)
 {
-    if (!p->allow) return 1;
-    return id < p->allow_bits && ((p->allow[id >> 5] >> (id & 31)) & 1u);
+    if (nprobes > n) nprobes = n;
+    orc_cand *c = (orc_cand *)malloc(sizeof(orc_cand) * (n ? n : 1));
+    if (!c) return;
+    for (uint32_t i = 0; i < n; i++) { c[i].d = d[i]; c[i].id = i; c[i].pos = i; }
+    qsort(c, n, sizeof(orc_cand), cand_cmp);
+    for (uint32_t j = 0; j < nprobes; j++) {
+        out_idx[j] = (uint32_t)c[j].id;
+        if (out_d) out_d[j] = c[j].d;
+    }
+    free(c);
 }
 
-static inline int in_range(const orc_params *p, float d)
+typedef struct {
+    int (*fn)(void *, uint64_t, uint64_t);
+    void *ctx;
+    uint64_t lo, hi;
+    int rc, threaded;
+} span_t;
+
+static void *span_run(void *arg)
 {
-    if (d != d) return 0;                      /* FilterExec: _distance IS NOT NULL */
-    if (p->has_lower && !(d >= p->lower)) return 0;
-    if (p->has_upper && !(d < p->upper)) return 0;
-    return 1;
+    span_t *s = (span_t *)arg;
+    s->rc = s->fn(s->ctx, s->lo, s->hi);
+    return NULL;
+}
+
+int orc_parallel(uint64_t n, int nthreads, int (*fn)(void *ctx, uint64_t lo, uint64_t hi), void *ctx)
+{
+    if (nthreads < 1) nthreads = 1;
+    if ((uint64_t)nthreads > n) nthreads = n ? (int)n : 1;
+    span_t *s = (span_t *)calloc((size_t)nthreads, sizeof(span_t));
+    pthread_t *th = (pthread_t *)calloc((size_t)nthreads, sizeof(pthread_t));
+    if (!s || !th) { free(s); free(th); return 1; }
+    for (int t = 0; t < nthreads; t++) {
+        span_t x = { fn, ctx, n * t / nthreads, n * (t + 1) / nthreads, 0, 0 };
+        s[t] = x;
+    }
+    for (int t = 1; t < nthreads; t++) {
+        s[t].threaded = pthread_create(&th[t], NULL, span_run, &s[t]) == 0;
+        if (!s[t].threaded) span_run(&s[t]);
+    }
+    span_run(&s[0]);
+    int rc = 0;
+    for (int t = 0; t < nthreads; t++) {
+        if (s[t].threaded) pthread_join(th[t], NULL);
+        rc |= s[t].rc;
+    }
+    free(s); free(th);
+    return rc;
 }
 
 /* ------------------------------------------------------------------------ */
@@ -220,23 +273,16 @@ void orc_find_partitions(const orc_index *ix, const float *q, uint32_t nprobes,
                          uint32_t *out_parts, float *out_dists, float *all_dists)
 {
     uint32_t nlist = ix->nlist;
-    if (nprobes > nlist) nprobes = nlist;
-    cand_t *c = (cand_t *)malloc(sizeof(cand_t) * (nlist ? nlist : 1));
-    for (uint32_t p = 0; p < nlist; p++) {
-        c[p].d = coarse_distance(ix, q, ix->centroids + (size_t)p * ix->dim);
-        c[p].id = p; c[p].pos = p;
-        if (all_dists) all_dists[p] = c[p].d;
-    }
+    if (nlist == 0) return;
+    float *d = all_dists ? all_dists : (float *)malloc(sizeof(float) * nlist);
+    if (!d) return;
+    for (uint32_t p = 0; p < nlist; p++)
+        d[p] = coarse_distance(ix, q, ix->centroids + (size_t)p * ix->dim);
     /* sort_to_indices(dists, limit = nprobes): ascending; ties by partition id; NaN distances last (the
-     * search loops never probe them: DESIGN.md section 0, rule c) */
-    qsort(c, nlist, sizeof(cand_t), cand_cmp);
-    for (uint32_t j = 0; j < nprobes; j++) {
-        out_parts[j] = (uint32_t)c[j].id;
-        if (out_dists) out_dists[j] = c[j].d;
-    }
-    free(c);
+     * search never probes them: DESIGN.md section 0, rule c) */
+    orc_nearest(d, nlist, nprobes, out_parts, out_dists);
+    if (!all_dists) free(d);
 }
-
 void orc_build_lut(const orc_index *ix, const float *rq, float *lut)
 {
     uint32_t m = ix->m, dsub = ix->dim / m;
@@ -305,39 +351,33 @@ void orc_partition_distances(const orc_index *ix, const float *q, uint32_t part,
 }
 
 /* ------------------------------------------------------------------------ */
+void orc_ivf_query_f32(const orc_ivf_kind *k, const void *q, void *state)
+{
+    const orc_index *ix = k->ix;
+    if (ix->metric == ORC_COSINE) orc_normalize_f32((const float *)q, ix->dim, (float *)state);
+    else memcpy(state, q, sizeof(float) * ix->dim);
+}
+
+void orc_ivf_coarse_f32(const orc_ivf_kind *k, const void *state, uint32_t nprobes, uint32_t *parts, float *dists)
+{
+    orc_find_partitions(k->ix, (const float *)state, nprobes, parts, dists, NULL);
+}
+
 typedef struct {
-    const orc_index *ix;
-    const float *queries;
-    uint32_t B, q0, q1;
+    const orc_ivf_kind *k;
+    const uint8_t *queries;
     const orc_params *p;
     uint64_t *out_ids; float *out_dist; uint32_t *out_count;
     size_t max_part;
-} ivf_job;
+} ivf_run;
 
-/* a NaN distance is never returned (FilterExec: _distance IS NOT NULL); only the
- * refine's exact distances can still be NaN here */
-static void emit(const orc_params *p, heap_t *h, uint64_t *ids, float *dist,
-                 uint32_t *count)
+static int ivf_range(void *arg, uint64_t q0, uint64_t q1)
 {
-    uint32_t kept = 0;
-    for (uint32_t j = 0; j < h->n; j++)
-        if (h->a[j].d == h->a[j].d) h->a[kept++] = h->a[j];
-    h->n = kept;
-    qsort(h->a, h->n, sizeof(cand_t), cand_cmp);
-    uint32_t n = h->n < p->k ? h->n : p->k;
-    for (uint32_t j = 0; j < p->k; j++) {
-        ids[j] = j < n ? h->a[j].id : UINT64_MAX;
-        dist[j] = j < n ? h->a[j].d : INFINITY;
-    }
-    *count = n;
-}
-
-static void *ivf_worker(void *arg)
-{
-    ivf_job *job = (ivf_job *)arg;
-    const orc_index *ix = job->ix;
-    const orc_params *p = job->p;
-    uint32_t dim = ix->dim, nprobes = p->nprobes < ix->nlist ? p->nprobes : ix->nlist;
+    const ivf_run *run = (const ivf_run *)arg;
+    const orc_ivf_kind *k = run->k;
+    const orc_index *ix = k->ix;
+    const orc_params *p = run->p;
+    uint32_t nprobes = p->nprobes < ix->nlist ? p->nprobes : ix->nlist;
     /* maximum_nprobes (rust/lancedb/src/query.rs:1250-1275): "the excess partitions will only be searched if
      * the initial search does not return enough results ... useful when there is a narrow filter".  Restated as:
      * under a prefilter, a query whose minimum_nprobes partitions yield fewer than k rows is searched again
@@ -345,30 +385,28 @@ static void *ivf_worker(void *arg)
     uint32_t nprobes_max = nprobes;
     if (p->allow && p->max_nprobes > nprobes) nprobes_max = p->max_nprobes < ix->nlist ? p->max_nprobes : ix->nlist;
     uint32_t kk = p->refine_factor ? p->k * p->refine_factor : p->k;
-    float *qn = (float *)malloc(sizeof(float) * dim * 2);
-    float *resid = qn + dim;
-    float *lut = (float *)malloc(sizeof(float) * ix->m * 256);
-    float *dists = (float *)malloc(sizeof(float) * (job->max_part ? job->max_part : 1));
+    void *state = malloc(k->state_bytes ? k->state_bytes : 1);
+    float *dists = (float *)malloc(sizeof(float) * (run->max_part ? run->max_part : 1));
     uint32_t *parts = (uint32_t *)malloc(sizeof(uint32_t) * (nprobes_max ? nprobes_max : 1));
     float *pd = (float *)malloc(sizeof(float) * (nprobes_max ? nprobes_max : 1));
-    heap_t h; h.a = (cand_t *)malloc(sizeof(cand_t) * (kk ? kk : 1)); h.cap = kk;
+    orc_topk h = { (orc_cand *)malloc(sizeof(orc_cand) * (kk ? kk : 1)), 0, kk };
+    const int err = !state || !dists || !parts || !pd || !h.a;
 
-    for (uint32_t qi = job->q0; qi < job->q1; qi++) {
-        const float *q = job->queries + (size_t)qi * dim;
-        if (ix->metric == ORC_COSINE) orc_normalize_f32(q, dim, qn);
-        else memcpy(qn, q, sizeof(float) * dim);
+    for (uint64_t qi = q0; qi < q1 && !err; qi++) {
+        const void *q = run->queries + qi * k->query_bytes;
+        k->prepare(k, q, state);
+        k->coarse(k, state, nprobes_max, parts, pd);
         for (uint32_t np_use = nprobes;;) {
-            orc_find_partitions(ix, qn, np_use, parts, pd, NULL);
             h.n = 0;
             for (uint32_t j = 0; j < np_use; j++) {
                 if (pd[j] != pd[j]) continue;              /* a NaN coarse distance is never probed */
                 uint32_t part = parts[j];
                 size_t off = ix->part_offsets[part], n = ix->part_offsets[part + 1] - off;
                 if (n == 0) continue;
-                partition_distances(ix, qn, part, resid, lut, dists);
+                k->partition(k, state, part, dists);
                 for (size_t r = 0; r < n; r++)
-                    if (in_range(p, dists[r]) && allowed(p, ix->row_ids[off + r]))
-                        heap_offer(&h, dists[r], ix->row_ids[off + r], off + r);
+                    if (orc_keep(p, ix->row_ids[off + r], dists[r]))
+                        orc_topk_offer(&h, dists[r], ix->row_ids[off + r], off + r);
             }
             if (np_use >= nprobes_max || h.n >= p->k) break;
             np_use = nprobes_max;
@@ -377,13 +415,31 @@ static void *ivf_worker(void *arg)
             /* refine (rust/lancedb/src/query.rs:1302-1332): exact distance of the
              * k*refine_factor ANN candidates on the raw vectors, re-sort, keep k */
             for (uint32_t c = 0; c < h.n; c++)
-                h.a[c].d = orc_distance_f32(ix->metric, q, ix->vectors + h.a[c].pos * dim, dim);
+                h.a[c].d = orc_distance_f32(ix->metric, (const float *)q, ix->vectors + h.a[c].pos * ix->dim, ix->dim);
         }
-        emit(p, &h, job->out_ids + (size_t)qi * p->k, job->out_dist + (size_t)qi * p->k,
-             job->out_count + qi);
+        orc_topk_emit(p, &h, run->out_ids + qi * p->k, run->out_dist + qi * p->k, run->out_count + qi);
     }
-    free(qn); free(lut); free(dists); free(parts); free(pd); free(h.a);
-    return NULL;
+    free(state); free(dists); free(parts); free(pd); free(h.a);
+    return err;
+}
+
+int orc_ivf_search(const orc_ivf_kind *k, const void *queries, uint32_t B, const orc_params *p, uint64_t *out_ids,
+                   float *out_dist, uint32_t *out_count, int nthreads)
+{
+    size_t max_part = 0;
+    for (uint32_t i = 0; i < k->ix->nlist; i++) {
+        size_t n = k->ix->part_offsets[i + 1] - k->ix->part_offsets[i];
+        if (n > max_part) max_part = n;
+    }
+    ivf_run run = { k, (const uint8_t *)queries, p, out_ids, out_dist, out_count, max_part };
+    return orc_parallel(B, nthreads, ivf_range, &run);
+}
+
+/* IVF_PQ, 8-bit: state = the query (normalised for cosine), the residual, the table */
+static void pq_partition(const orc_ivf_kind *k, void *state, uint32_t part, float *dists)
+{
+    float *qn = (float *)state;
+    partition_distances(k->ix, qn, part, qn + k->ix->dim, qn + 2 * k->ix->dim, dists);
 }
 
 int orc_ivfpq_search(const orc_index *ix, const float *queries, uint32_t B,
@@ -391,26 +447,9 @@ int orc_ivfpq_search(const orc_index *ix, const float *queries, uint32_t B,
                      uint32_t *out_count, int nthreads)
 {
     if (!ix || !p || ix->m == 0 || ix->dim % ix->m) return -1;
-    if (nthreads < 1) nthreads = 1;
-    if ((uint32_t)nthreads > B) nthreads = B ? (int)B : 1;
-    size_t max_part = 0;
-    for (uint32_t i = 0; i < ix->nlist; i++) {
-        size_t n = ix->part_offsets[i + 1] - ix->part_offsets[i];
-        if (n > max_part) max_part = n;
-    }
-    pthread_t *th = (pthread_t *)malloc(sizeof(pthread_t) * nthreads);
-    ivf_job *jobs = (ivf_job *)malloc(sizeof(ivf_job) * nthreads);
-    for (int t = 0; t < nthreads; t++) {
-        ivf_job j = { ix, queries, B, (uint32_t)((uint64_t)B * t / nthreads),
-                      (uint32_t)((uint64_t)B * (t + 1) / nthreads), p,
-                      out_ids, out_dist, out_count, max_part };
-        jobs[t] = j;
-        if (nthreads == 1) ivf_worker(&jobs[t]);
-        else pthread_create(&th[t], NULL, ivf_worker, &jobs[t]);
-    }
-    if (nthreads > 1) for (int t = 0; t < nthreads; t++) pthread_join(th[t], NULL);
-    free(th); free(jobs);
-    return 0;
+    const orc_ivf_kind k = { ix, sizeof(float) * ix->dim, sizeof(float) * (2 * ix->dim + (size_t)ix->m * 256),
+                             orc_ivf_query_f32, orc_ivf_coarse_f32, pq_partition };
+    return orc_ivf_search(&k, queries, B, p, out_ids, out_dist, out_count, nthreads);
 }
 
 /* ------------------------------------------------------------------------ */
@@ -460,30 +499,30 @@ void orc_pq_encode(const orc_index *ix, const float *vectors, const uint32_t *pa
 /* ------------------------------------------------------------------------ */
 typedef struct {
     const float *vectors; uint64_t n; uint32_t dim; const uint64_t *row_ids; int metric;
-    const float *queries; uint32_t q0, q1; const orc_params *p;
+    const float *queries; const orc_params *p;
     uint64_t *out_ids; float *out_dist; uint32_t *out_count;
-} flat_job;
+} flat_run;
 
 /* KNNVectorDistance + SortExec TopK(_distance ASC, _rowid ASC) + FilterExec
  * (_distance IS NOT NULL): python/python/lancedb/query.py:1364-1370           */
-static void *flat_worker(void *arg)
+static int flat_range(void *arg, uint64_t q0, uint64_t q1)
 {
-    flat_job *job = (flat_job *)arg;
-    const orc_params *p = job->p;
-    heap_t h; h.a = (cand_t *)malloc(sizeof(cand_t) * (p->k ? p->k : 1)); h.cap = p->k;
-    for (uint32_t qi = job->q0; qi < job->q1; qi++) {
-        const float *q = job->queries + (size_t)qi * job->dim;
+    const flat_run *run = (const flat_run *)arg;
+    const orc_params *p = run->p;
+    orc_topk h = { (orc_cand *)malloc(sizeof(orc_cand) * (p->k ? p->k : 1)), 0, p->k };
+    if (!h.a) return 1;
+    for (uint64_t qi = q0; qi < q1; qi++) {
+        const float *q = run->queries + qi * run->dim;
         h.n = 0;
-        for (uint64_t r = 0; r < job->n; r++) {
-            float d = orc_distance_f32(job->metric, q, job->vectors + r * job->dim, job->dim);
-            uint64_t id = job->row_ids ? job->row_ids[r] : r;
-            if (in_range(p, d) && allowed(p, id)) heap_offer(&h, d, id, r);
+        for (uint64_t r = 0; r < run->n; r++) {
+            float d = orc_distance_f32(run->metric, q, run->vectors + r * run->dim, run->dim);
+            uint64_t id = run->row_ids ? run->row_ids[r] : r;
+            if (orc_keep(p, id, d)) orc_topk_offer(&h, d, id, r);
         }
-        emit(p, &h, job->out_ids + (size_t)qi * p->k, job->out_dist + (size_t)qi * p->k,
-             job->out_count + qi);
+        orc_topk_emit(p, &h, run->out_ids + qi * p->k, run->out_dist + qi * p->k, run->out_count + qi);
     }
     free(h.a);
-    return NULL;
+    return 0;
 }
 
 int orc_flat_search(const float *vectors, uint64_t n, uint32_t dim,
@@ -492,20 +531,6 @@ int orc_flat_search(const float *vectors, uint64_t n, uint32_t dim,
                     float *out_dist, uint32_t *out_count, int nthreads)
 {
     if (!p) return -1;
-    if (nthreads < 1) nthreads = 1;
-    if ((uint32_t)nthreads > B) nthreads = B ? (int)B : 1;
-    pthread_t *th = (pthread_t *)malloc(sizeof(pthread_t) * nthreads);
-    flat_job *jobs = (flat_job *)malloc(sizeof(flat_job) * nthreads);
-    for (int t = 0; t < nthreads; t++) {
-        flat_job j = { vectors, n, dim, row_ids, metric, queries,
-                       (uint32_t)((uint64_t)B * t / nthreads),
-                       (uint32_t)((uint64_t)B * (t + 1) / nthreads), p,
-                       out_ids, out_dist, out_count };
-        jobs[t] = j;
-        if (nthreads == 1) flat_worker(&jobs[t]);
-        else pthread_create(&th[t], NULL, flat_worker, &jobs[t]);
-    }
-    if (nthreads > 1) for (int t = 0; t < nthreads; t++) pthread_join(th[t], NULL);
-    free(th); free(jobs);
-    return 0;
+    flat_run run = { vectors, n, dim, row_ids, metric, queries, p, out_ids, out_dist, out_count };
+    return orc_parallel(B, nthreads, flat_range, &run);
 }

@@ -94,7 +94,8 @@ void orc_pq_scan(const float *lut, const uint8_t *codes_t, size_t n, uint32_t m,
 
 /* Whole path for a batch; nthreads worker threads over queries.
  * out_ids/out_dist: [B][k], out_count: [B].  Unused slots: id = UINT64_MAX,
- * dist = +inf.  Returns 0 or a negative error. */
+ * dist = +inf.  Returns 0, a negative error for invalid arguments, or 1 when
+ * allocation fails. */
 int orc_ivfpq_search(const orc_index *ix, const float *queries, uint32_t B,
                      const orc_params *p, uint64_t *out_ids, float *out_dist,
                      uint32_t *out_count, int nthreads);
@@ -118,6 +119,57 @@ int orc_flat_search(const float *vectors, uint64_t n, uint32_t dim,
                     const uint64_t *row_ids, int metric, const float *queries,
                     uint32_t B, const orc_params *p, uint64_t *out_ids,
                     float *out_dist, uint32_t *out_count, int nthreads);
+
+/* ---- the result contract every oracle shares (DESIGN.md section 0) ----- */
+/* The row filter: a NaN distance is dropped (FilterExec: _distance IS NOT NULL), then distance_range [lower, upper)
+ * and the allow bitmap. */
+static inline int orc_keep(const orc_params *p, uint64_t id, float d)
+{
+    if (d != d) return 0;
+    if (p->has_lower && !(d >= p->lower)) return 0;
+    if (p->has_upper && !(d < p->upper)) return 0;
+    return !p->allow || (id < p->allow_bits && ((p->allow[id >> 5] >> (id & 31)) & 1u));
+}
+
+/* A candidate row; pos is its index in the row order (refine reads the raw vector there). */
+typedef struct { float d; uint64_t id; uint64_t pos; } orc_cand;
+
+/* The cap best candidates by (distance ASC, row id ASC), a NaN distance after every number. */
+typedef struct { orc_cand *a; uint32_t n, cap; } orc_topk;
+void orc_topk_offer(orc_topk *h, float d, uint64_t id, uint64_t pos);
+/* Drops NaN distances, sorts, and writes p->k slots (unused: UINT64_MAX / +inf) and the count. */
+void orc_topk_emit(const orc_params *p, orc_topk *h, uint64_t *ids, float *dist, uint32_t *count);
+
+/* The indices of the nprobes smallest of d[0..n) by (distance, index), NaN last, and their distances (out_d may be
+ * NULL). */
+void orc_nearest(const float *d, uint32_t n, uint32_t nprobes, uint32_t *out_idx, float *out_d);
+
+/* Runs fn(ctx, lo, hi) over min(nthreads, n) contiguous ranges of [0, n) on worker threads (inline when a thread
+ * cannot be started).  Nonzero when allocation fails or a range returns nonzero. */
+int orc_parallel(uint64_t n, int nthreads, int (*fn)(void *ctx, uint64_t lo, uint64_t hi), void *ctx);
+
+/* ---- one IVF search for every index kind --------------------------------
+ * Per query: prepare, the coarse order, widening, top-k, refine and emit are the driver's (orc_ivf_search); a kind
+ * supplies its query preparation, its coarse step and the distances of one partition's rows. */
+typedef struct orc_ivf_kind orc_ivf_kind;
+struct orc_ivf_kind {
+    const orc_index *ix;     /* nlist, part_offsets, row_ids; metric, dim and vectors (NULL: no refine) for refine */
+    size_t query_bytes;      /* one raw query */
+    size_t state_bytes;      /* one prepared query; a float kind's starts with the query the coarse step takes */
+    void (*prepare)(const orc_ivf_kind *k, const void *q, void *state);
+    /* the nprobes nearest partitions by (coarse distance, partition id) and their coarse distances */
+    void (*coarse)(const orc_ivf_kind *k, const void *state, uint32_t nprobes, uint32_t *parts, float *dists);
+    /* the distances of partition part's rows, in row order */
+    void (*partition)(const orc_ivf_kind *k, void *state, uint32_t part, float *dists);
+};
+int orc_ivf_search(const orc_ivf_kind *k, const void *queries, uint32_t B, const orc_params *p, uint64_t *out_ids,
+                   float *out_dist, uint32_t *out_count, int nthreads);
+/* The float kinds' prepare prefix (the query, normalised for cosine) and their coarse step (orc_find_partitions). */
+void orc_ivf_query_f32(const orc_ivf_kind *k, const void *q, void *state);
+void orc_ivf_coarse_f32(const orc_ivf_kind *k, const void *state, uint32_t nprobes, uint32_t *parts, float *dists);
+
+/* popcount(q XOR x) over nbytes bytes (tests/hamming_oracle.c) */
+uint32_t orc_hamming_row(const uint8_t *q, const uint8_t *x, uint32_t nbytes);
 
 #ifdef __cplusplus
 }

@@ -116,41 +116,98 @@ def pq_encode(ix, v, parts):
     return out
 
 
+def distance(metric, x, y):
+    """orc_distance_f32: the exact distance refine re-ranks by"""
+    if metric == "cosine":
+        return cosine(x, y)
+    return f32(f32(1) - dot(x, y)) if metric == "dot" else l2(x, y)
+
+
+def query(metric, q):
+    """the query the coarse step and the tables see: normalised for cosine"""
+    q = np.asarray(q, f32)
+    return normalize(q) if metric == "cosine" else q
+
+
+def coarse(metric, qn, centroids):
+    """find_partitions' distances: 1 - x.y for dot, l2 otherwise (cosine: on the normalised query)"""
+    if metric == "dot":
+        return np.array([f32(f32(1) - dot(qn, c)) for c in centroids], f32)
+    return np.array([l2(qn, c) for c in centroids], f32)
+
+
+def ivf_search_np(B, data, k, nprobes, coarse_of, partition_of, refine_of=None, refine_factor=0, lower=None,
+                  upper=None, allow=None, max_nprobes=0):
+    """The IVF search every index kind shares (DESIGN.md section 0), the mirror of orc_ivf_search.  data: nlist,
+    part_offsets, row_ids.  Per query b: coarse_of(b) -> the [nlist] coarse distances (a NaN one is never probed);
+    partition_of(b, p) -> the distances of partition p's rows; refine_of(b, pos) -> the exact distance of row pos
+    (None: no refine).  allow: bool mask over row ids.  Returns (ids [B, k] u64, dist [B, k] f32, count [B] u32)."""
+    nlist = data.nlist
+    off = np.asarray(data.part_offsets, np.int64)
+    rid = np.asarray(data.row_ids, np.uint64)
+    keep = np.ones(rid.size, bool)
+    if allow is not None:                               # ids beyond the mask are excluded
+        a = np.asarray(allow, bool)
+        inside = rid < a.size
+        keep = np.zeros(rid.size, bool)
+        keep[inside] = a[rid[inside].astype(np.int64)]
+    nprobes = min(nprobes, nlist)
+    np_max = max(nprobes, min(max_nprobes, nlist)) if allow is not None else nprobes
+    kk = k * refine_factor if refine_factor else k
+    ids = np.full((B, k), np.iinfo(np.uint64).max, np.uint64)
+    dist = np.full((B, k), np.inf, f32)
+    cnt = np.zeros(B, np.uint32)
+    for b in range(B):
+        cd = np.asarray(coarse_of(b))
+        order = np.lexsort((np.arange(nlist), cd))     # ties by partition id, NaN last
+        for np_use in (nprobes, np_max):                # maximum_nprobes: again, wider, when fewer than k rows remain
+            pos, ds = [np.zeros(0, np.int64)], [np.zeros(0, f32)]
+            for p in order[:np_use]:
+                if np.isnan(cd[p]) or off[p] == off[p + 1]:
+                    continue
+                d = np.asarray(partition_of(b, p), f32)
+                m = keep[off[p]:off[p + 1]] & ~np.isnan(d)            # _distance IS NOT NULL
+                if lower is not None:
+                    m &= d >= f32(lower)
+                if upper is not None:
+                    m &= d < f32(upper)
+                pos.append(np.arange(off[p], off[p + 1])[m])
+                ds.append(d[m])
+            pos, d = np.concatenate(pos), np.concatenate(ds)
+            if len(pos) >= k:
+                break
+        o = np.lexsort((rid[pos], d))[:kk]              # (_distance, _rowid)
+        pos, d = pos[o], d[o]
+        if refine_factor and refine_of is not None:
+            d = np.array([refine_of(b, r) for r in pos], f32)
+            pos, d = pos[~np.isnan(d)], d[~np.isnan(d)]               # a NaN distance is never returned
+            o = np.lexsort((rid[pos], d))
+            pos, d = pos[o], d[o]
+        n = min(k, len(pos))
+        ids[b, :n] = rid[pos[:n]]
+        dist[b, :n] = d[:n]
+        cnt[b] = n
+    return ids, dist, cnt
+
+
+def partition_distances(ix, qn, p):
+    """the 8-bit IVF_PQ distances of partition p's rows: table sums, then cosine L2^2 / 2 or dot sum - (m - 1)"""
+    a, b = int(ix.part_offsets[p]), int(ix.part_offsets[p + 1])
+    rq = qn if ix.metric == "dot" else (qn - ix.centroids[p]).astype(f32)
+    d = pq_scan(build_lut(ix.codebook, rq, ix.metric), ix.codes_t[a * ix.m:b * ix.m].reshape(ix.m, b - a))
+    if ix.metric == "cosine":
+        return (d * f32(0.5)).astype(f32)
+    return (d - f32(ix.m - 1)).astype(f32) if ix.metric == "dot" else d
+
+
 def ivfpq_search_one(ix, q, k, nprobes, lower=None, upper=None, allowed=None):
     """ix: lancedb_b200.index.IvfPqIndexData; returns (ids, dists) sorted by (dist, id).
     allowed: optional set of row ids (prefilter: other rows are dropped before the top-k)"""
-    q = np.asarray(q, f32)
-    qn = normalize(q) if ix.metric == "cosine" else q
-    if ix.metric == "dot":
-        cd = np.array([f32(f32(1) - dot(qn, c)) for c in ix.centroids], f32)
-    else:
-        cd = np.array([l2(qn, c) for c in ix.centroids], f32)
-    order = np.lexsort((np.arange(ix.nlist), cd))[:min(nprobes, ix.nlist)]     # NaN last
-    cands = []
-    for p in order:
-        if np.isnan(cd[p]):                 # a NaN coarse distance is never probed
-            continue
-        a, b = int(ix.part_offsets[p]), int(ix.part_offsets[p + 1])
-        if a == b:
-            continue
-        rq = qn if ix.metric == "dot" else (qn - ix.centroids[p]).astype(f32)
-        lut = build_lut(ix.codebook, rq, ix.metric)
-        codes_t = ix.codes_t[a * ix.m:b * ix.m].reshape(ix.m, b - a)
-        d = pq_scan(lut, codes_t)
-        if ix.metric == "cosine":
-            d = (d * f32(0.5)).astype(f32)
-        elif ix.metric == "dot":
-            d = (d - f32(ix.m - 1)).astype(f32)
-        for r in range(b - a):
-            if np.isnan(d[r]):                  # _distance IS NOT NULL
-                continue
-            if lower is not None and not d[r] >= f32(lower):
-                continue
-            if upper is not None and not d[r] < f32(upper):
-                continue
-            if allowed is not None and int(ix.row_ids[a + r]) not in allowed:
-                continue
-            cands.append((d[r], int(ix.row_ids[a + r])))
-    cands.sort()
-    cands = cands[:k]
-    return np.array([c[1] for c in cands], np.uint64), np.array([c[0] for c in cands], f32)
+    qn = query(ix.metric, q)
+    allow = None
+    if allowed is not None:
+        allow = np.zeros(int(ix.row_ids.max(initial=0)) + 1, bool)
+        allow[[r for r in allowed if r < allow.size]] = True
+    ids, dist, cnt = ivf_search_np(1, ix, k, nprobes, lambda b: coarse(ix.metric, qn, ix.centroids),
+                                   lambda b, p: partition_distances(ix, qn, p), lower=lower, upper=upper, allow=allow)
+    return ids[0, :cnt[0]], dist[0, :cnt[0]]

@@ -13,71 +13,24 @@ orc_params), which the GPU tests, smoke() and scripts/bench_ivf_binary.py compar
 """
 from __future__ import annotations
 
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_SRC = os.path.join(_HERE, "ivf_binary_oracle.c")
-_LIB_PATH = os.path.join(_HERE, "_build", "libivf_binary_oracle.so")
-_lib = None
+import oracle
+
 U64_MAX = np.iinfo(np.uint64).max
-
-
-def build(force: bool = False) -> str:
-    """gcc -> tests/_build/libivf_binary_oracle.so (rebuilt when the source or oracle/oracle.h is newer)."""
-    deps = [_SRC, os.path.join(_ROOT, "oracle", "oracle.h")]
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(map(os.path.getmtime, deps)):
-        os.makedirs(os.path.dirname(_LIB_PATH), exist_ok=True)
-        subprocess.run(["gcc", "-O3", "-mpopcnt", "-fPIC", "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared",
-                        "-o", _LIB_PATH, _SRC, "-lm"], check=True)
-    return _LIB_PATH
-
-
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        lib = C.CDLL(_LIB_PATH)
-        vp = C.c_void_p
-        lib.orc_ivf_binary_search.argtypes = [vp, C.c_uint32, vp, vp, vp, C.c_uint32, vp, C.c_uint32, vp, vp, vp, vp,
-                                              C.c_int]
-        _lib = lib
-    return _lib
-
-
-def _allow_bits(allow):
-    """bool mask over row ids -> (u32 bitmap, bits)"""
-    import oracle
-    a = np.asarray(allow, bool)
-    return oracle.allow_bitmap(np.nonzero(a)[0], a.size), a.size
 
 
 def search(data, queries, k: int, nprobes: int, lower=None, upper=None, allow=None, max_nprobes: int = 0,
            nthreads: int = 0):
     """(ids [B, k] u64, dist [B, k] f32, count [B] u32) from the C oracle; allow: optional bool mask over row ids."""
-    import oracle
     q = np.ascontiguousarray(queries, np.uint8).reshape(-1, data.nbytes)
-    B = q.shape[0]
-    bm, nbits = (None, 0) if allow is None else _allow_bits(allow)
-    p = oracle._params(k, nprobes, 0, lower, upper, bm, nbits, max_nprobes)
-    ids = np.empty((B, k), np.uint64)
-    dist = np.empty((B, k), np.float32)
-    cnt = np.empty(B, np.uint32)
     cent = np.ascontiguousarray(data.centroids, np.uint8)
     off = np.ascontiguousarray(data.part_offsets, np.uint64)
     x = np.ascontiguousarray(data.vectors, np.uint8)
     rid = np.ascontiguousarray(data.row_ids, np.uint64)
-    if B and load().orc_ivf_binary_search(cent.ctypes.data, data.nlist, off.ctypes.data, x.ctypes.data,
-                                          rid.ctypes.data, data.nbytes, q.ctypes.data, B, C.addressof(p),
-                                          ids.ctypes.data, dist.ctypes.data, cnt.ctypes.data,
-                                          int(nthreads) if nthreads else (os.cpu_count() or 1)) != 0:
-        raise RuntimeError("orc_ivf_binary_search failed")
-    return ids, dist, cnt
+    return oracle.search_call("orc_ivf_binary_search", (cent.ctypes.data, data.nlist, off.ctypes.data, x.ctypes.data,
+                                                        rid.ctypes.data, data.nbytes, q.ctypes.data), q.shape[0], k,
+                              nthreads, nprobes, 0, lower, upper, allow, max_nprobes=max_nprobes)
 
 
 # ---- NumPy mirror ----
@@ -95,43 +48,14 @@ def hamming_np(q, x) -> np.ndarray:
 
 
 def search_np(data, queries, k: int, nprobes: int, lower=None, upper=None, allow=None, max_nprobes: int = 0):
-    """The same search, spelled with NumPy one query at a time."""
+    """The same search, spelled with NumPy one query at a time (the search loop from oracle/oracle_np.py)."""
+    from oracle import oracle_np as onp
     q = np.asarray(queries, np.uint8).reshape(-1, data.nbytes)
-    B, nlist = q.shape[0], data.nlist
     off = data.part_offsets.astype(np.int64)
-    rid = data.row_ids.astype(np.uint64)
-    keep = np.ones(data.nrows, bool)
-    if allow is not None:
-        a = np.asarray(allow, bool)
-        inside = rid < a.size
-        keep = np.zeros(data.nrows, bool)
-        keep[inside] = a[rid[inside].astype(np.int64)]
-    D = hamming_np(q, data.vectors) if data.nrows else np.zeros((B, 0), np.int64)
-    C_ = hamming_np(q, data.centroids)
-    np0 = min(nprobes, nlist)
-    npm = min(max_nprobes, nlist) if allow is not None and max_nprobes > np0 else np0
-    ids = np.full((B, k), U64_MAX, np.uint64)
-    dist = np.full((B, k), np.inf, np.float32)
-    cnt = np.zeros(B, np.uint32)
-    for b in range(B):
-        order = np.lexsort((np.arange(nlist), C_[b]))
-        for npu in (np0, npm):
-            rows = np.concatenate([np.arange(off[p], off[p + 1]) for p in order[:npu]]).astype(np.int64)
-            m = keep[rows].copy()
-            d = D[b, rows].astype(np.float32)
-            if lower is not None:
-                m &= d >= np.float32(lower)
-            if upper is not None:
-                m &= d < np.float32(upper)
-            rows, d = rows[m], d[m]
-            if len(rows) >= k or npu == npm:
-                break
-        o = np.lexsort((rid[rows], d))[:k]
-        n = len(o)
-        ids[b, :n] = rid[rows[o]]
-        dist[b, :n] = d[o]
-        cnt[b] = n
-    return ids, dist, cnt
+    C_ = hamming_np(q, data.centroids).astype(np.float32)
+    return onp.ivf_search_np(len(q), data, k, nprobes, lambda b: C_[b],
+                             lambda b, p: hamming_np(q[b:b + 1], data.vectors[off[p]:off[p + 1]])[0].astype(np.float32),
+                             lower=lower, upper=upper, allow=allow, max_nprobes=max_nprobes)
 
 
 def kmodes_np(x, centroids, iters: int):

@@ -9,10 +9,8 @@
  * (_distance, _rowid); unused slots are UINT64_MAX / +inf.  Worker threads split the rows.  The NumPy mirror is
  * tests/multivec_oracle.py. */
 #include <math.h>
-#include <pthread.h>
 #include <stdint.h>
 #include <stdlib.h>
-#include <string.h>
 
 #include "../oracle/oracle.h"
 
@@ -36,61 +34,29 @@ typedef struct {
     const uint64_t *offsets;
     const uint32_t *q_off;
     uint32_t dim, B;
-    uint64_t r0, r1, nrows;
+    uint64_t nrows;
     float *out;                 /* [B][nrows] */
 } job;
 
-static void *dist_worker(void *arg)
+static int dist_range(void *arg, uint64_t r0, uint64_t r1)
 {
-    job *j = (job *)arg;
-    for (uint64_t r = j->r0; r < j->r1; r++) {
+    const job *j = (const job *)arg;
+    for (uint64_t r = r0; r < r1; r++) {
         const float *v = j->values + j->offsets[r] * j->dim;
         const uint64_t nr = j->offsets[r + 1] - j->offsets[r];
         for (uint32_t b = 0; b < j->B; b++)
             j->out[(size_t)b * j->nrows + r] =
                 maxsim_distance(j->queries + (size_t)j->q_off[b] * j->dim, j->q_off[b + 1] - j->q_off[b], v, nr, j->dim);
     }
-    return NULL;
+    return 0;
 }
 
 /* out[b][r] = _distance(query b, row r).  values [offsets[nrows]][dim], queries [q_off[B]][dim]. */
 int orc_multivec_distances(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
                            const float *queries, const uint32_t *q_off, uint32_t B, float *out, int nthreads)
 {
-    if (nthreads < 1) nthreads = 1;
-    if ((uint64_t)nthreads > nrows) nthreads = nrows ? (int)nrows : 1;
-    job *js = (job *)calloc((size_t)nthreads, sizeof(job));
-    pthread_t *th = (pthread_t *)calloc((size_t)nthreads, sizeof(pthread_t));
-    if (!js || !th) { free(js); free(th); return 1; }
-    for (int t = 0; t < nthreads; t++) {
-        job p = { values, queries, offsets, q_off, dim, B, nrows * t / nthreads, nrows * (t + 1) / nthreads, nrows, out };
-        js[t] = p;
-        if (pthread_create(&th[t], NULL, dist_worker, &js[t]) != 0) { dist_worker(&js[t]); th[t] = 0; }
-    }
-    for (int t = 0; t < nthreads; t++)
-        if (th[t]) pthread_join(th[t], NULL);
-    free(js);
-    free(th);
-    return 0;
-}
-
-typedef struct { float d; uint64_t id; } cand;
-
-static int cand_cmp(const void *a, const void *b)
-{
-    const cand *x = (const cand *)a, *y = (const cand *)b;
-    if (x->d < y->d) return -1;
-    if (x->d > y->d) return 1;
-    return x->id < y->id ? -1 : (x->id > y->id ? 1 : 0);
-}
-
-static int keep_row(const orc_params *p, uint64_t id, float d)
-{
-    if (d != d) return 0;
-    if (p->allow && (id >= p->allow_bits || !((p->allow[id >> 5] >> (id & 31)) & 1u))) return 0;
-    if (p->has_lower && !(d >= p->lower)) return 0;
-    if (p->has_upper && !(d < p->upper)) return 0;
-    return 1;
+    job j = { values, queries, offsets, q_off, dim, B, nrows, out };
+    return orc_parallel(nrows, nthreads, dist_range, &j);
 }
 
 /* flat MaxSim search: p->k results per query (k, has_lower/has_upper, allow/allow_bits are used) */
@@ -101,25 +67,19 @@ int orc_multivec_search(const float *values, const uint64_t *offsets, uint64_t n
     if (!p || p->k == 0 || dim == 0) return 1;
     const size_t nd = (size_t)B * nrows;
     float *d = (float *)malloc((nd ? nd : 1) * sizeof(float));
-    cand *c = (cand *)malloc((nrows ? nrows : 1) * sizeof(cand));
-    if (!d || !c) { free(d); free(c); return 1; }
-    int rc = orc_multivec_distances(values, offsets, nrows, dim, queries, q_off, B, d, nthreads);
+    orc_topk h = { (orc_cand *)malloc(sizeof(orc_cand) * p->k), 0, p->k };
+    int rc = !d || !h.a;
+    if (!rc) rc = orc_multivec_distances(values, offsets, nrows, dim, queries, q_off, B, d, nthreads);
     for (uint32_t b = 0; b < B && rc == 0; b++) {
-        uint64_t nc = 0;
+        h.n = 0;
         for (uint64_t r = 0; r < nrows; r++) {
             const uint64_t id = row_ids ? row_ids[r] : r;
             const float x = d[(size_t)b * nrows + r];
-            if (keep_row(p, id, x)) { c[nc].d = x; c[nc].id = id; nc++; }
+            if (orc_keep(p, id, x)) orc_topk_offer(&h, x, id, r);
         }
-        qsort(c, nc, sizeof(cand), cand_cmp);
-        const uint32_t cnt = (uint32_t)(nc < p->k ? nc : p->k);
-        for (uint32_t i = 0; i < p->k; i++) {
-            out_ids[(size_t)b * p->k + i] = i < cnt ? c[i].id : UINT64_MAX;
-            out_dist[(size_t)b * p->k + i] = i < cnt ? c[i].d : INFINITY;
-        }
-        out_count[b] = cnt;
+        orc_topk_emit(p, &h, out_ids + (size_t)b * p->k, out_dist + (size_t)b * p->k, out_count + b);
     }
     free(d);
-    free(c);
+    free(h.a);
     return rc;
 }

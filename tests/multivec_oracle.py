@@ -7,7 +7,7 @@ row's distance NaN, and NaN distances are never returned.  Results ascend by (_d
 [lower, upper) applies to the summed distance; an allow mask over row ids drops rows before the top-k; unused slots are
 UINT64_MAX / +inf.
 
-Two statements of it: the threaded C oracle (multivec_oracle.c, built together with oracle/oracle.c so that it calls
+Two statements of it: the threaded C oracle (multivec_oracle.c, built into oracle/'s library, so that it calls
 orc_cosine_f32 itself), which the GPU tests, smoke() and scripts/bench_multivector.py compare against and time, and
 the NumPy mirror below (cosine_matrix_np, distances_np, flat_search_mv_np), which the CPU tests check the C oracle
 against.
@@ -16,48 +16,11 @@ Rows are given as (values [T, dim], offsets [N+1]); queries as (values [Tq, dim]
 """
 from __future__ import annotations
 
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_SRC = os.path.join(_HERE, "multivec_oracle.c")
-_ORACLE_SRC = os.path.join(_ROOT, "oracle", "oracle.c")
-_LIB_PATH = os.path.join(_HERE, "_build", "libmultivec_oracle.so")
-_lib = None
+import oracle
+
 f32 = np.float32
-
-
-def build(force: bool = False) -> str:
-    """gcc -> tests/_build/libmultivec_oracle.so with oracle/oracle.c's flags (rebuilt when a source is newer)."""
-    deps = [_SRC, _ORACLE_SRC, os.path.join(_ROOT, "oracle", "oracle.h")]
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(map(os.path.getmtime, deps)):
-        os.makedirs(os.path.dirname(_LIB_PATH), exist_ok=True)
-        subprocess.run(["gcc", "-O3", "-mavx2", "-mfma", "-mf16c", "-ffp-contract=off", "-fno-fast-math", "-fPIC",
-                        "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", _LIB_PATH, _SRC, _ORACLE_SRC,
-                        "-lm"], check=True)
-    return _LIB_PATH
-
-
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        lib = C.CDLL(_LIB_PATH)
-        vp = C.c_void_p
-        lib.orc_multivec_distances.argtypes = [vp, vp, C.c_uint64, C.c_uint32, vp, vp, C.c_uint32, vp, C.c_int]
-        lib.orc_multivec_search.argtypes = [vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, C.c_uint32, vp, vp, vp, vp,
-                                            C.c_int]
-        _lib = lib
-    return _lib
-
-
-def _threads(nthreads):
-    return int(nthreads) if nthreads else (os.cpu_count() or 1)
 
 
 def offsets_of(lengths) -> np.ndarray:
@@ -82,8 +45,9 @@ def distances(values, offsets, queries, q_offsets, nthreads: int = 0) -> np.ndar
     q, qo = _queries(queries, q_offsets)
     N, B = off.size - 1, qo.size - 1
     out = np.empty((B, N), np.float32)
-    if out.size and load().orc_multivec_distances(v.ctypes.data, off.ctypes.data, N, v.shape[1], q.ctypes.data,
-                                                  qo.ctypes.data, B, out.ctypes.data, _threads(nthreads)) != 0:
+    if out.size and oracle.load().orc_multivec_distances(v.ctypes.data, off.ctypes.data, N, v.shape[1], q.ctypes.data,
+                                                         qo.ctypes.data, B, out.ctypes.data,
+                                                         oracle.threads(nthreads)) != 0:
         raise MemoryError("orc_multivec_distances failed")
     return out
 
@@ -91,25 +55,14 @@ def distances(values, offsets, queries, q_offsets, nthreads: int = 0) -> np.ndar
 def flat_search_mv(values, offsets, queries, q_offsets, k: int, row_ids=None, lower=None, upper=None, allow=None,
                    nthreads: int = 0):
     """(ids [B, k] u64, dist [B, k] f32, count [B] u32) from the C oracle; allow: optional bool mask over row ids."""
-    import oracle
     v, off = _rows(values, offsets)
     q, qo = _queries(queries, q_offsets)
-    N, B = off.size - 1, qo.size - 1
     rid = None if row_ids is None else np.ascontiguousarray(row_ids, np.uint64)
-    bm = None
-    if allow is not None:
-        a = np.asarray(allow, bool)
-        bm = oracle.allow_bitmap(np.nonzero(a)[0], a.size)
-    p = oracle._params(k, 0, 0, lower, upper, bm, 0 if allow is None else np.asarray(allow).size)
-    ids = np.empty((B, k), np.uint64)
-    dist = np.empty((B, k), np.float32)
-    cnt = np.empty(B, np.uint32)
-    if B and load().orc_multivec_search(v.ctypes.data, off.ctypes.data, N, v.shape[1] if v.ndim == 2 else 1,
-                                        None if rid is None else rid.ctypes.data, q.ctypes.data, qo.ctypes.data, B,
-                                        C.addressof(p), ids.ctypes.data, dist.ctypes.data, cnt.ctypes.data,
-                                        _threads(nthreads)) != 0:
-        raise MemoryError("orc_multivec_search failed")
-    return ids, dist, cnt
+    return oracle.search_call("orc_multivec_search", (v.ctypes.data, off.ctypes.data, off.size - 1,
+                                                      v.shape[1] if v.ndim == 2 else 1,
+                                                      None if rid is None else rid.ctypes.data, q.ctypes.data,
+                                                      qo.ctypes.data), qo.size - 1, k, nthreads, lower=lower,
+                              upper=upper, allow=allow)
 
 
 # ---- NumPy mirror ----

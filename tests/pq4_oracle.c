@@ -11,13 +11,9 @@
  *   Q[i][j]  = pq4_quant(T[i][j])                                                                 [lance, recalled]
  *   d        = pq4_distance(S = sum_i Q[i][code_i])                                               [lance, recalled]
  * The three recalled steps are one function each here (pq4_fold, orc_pq4_quant, orc_pq4_distance) and in
- * lancedb_b200/csrc/pq4_scan.cu.  A NaN d is never returned; distance_range [lower, upper) on d and the row-id allow
- * bitmap drop rows before the top-k; maximum_nprobes (under a prefilter) searches a query again over its max_nprobes
- * nearest partitions when it found fewer than k rows; refine_factor keeps the k * refine_factor best and re-ranks them by
- * orc_distance_f32 on the raw query and vectors.  Results ascend by (_distance, _rowid); unused slots are
- * UINT64_MAX / +inf.  Worker threads split the queries.  The NumPy mirror is tests/pq4_oracle.py. */
+ * lancedb_b200/csrc/pq4_scan.cu.  orc_ivf_search (oracle/oracle.c) runs the search around them.  The NumPy mirror is
+ * tests/pq4_oracle.py. */
 #include <math.h>
-#include <pthread.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -123,124 +119,18 @@ void orc_pq4_partition_distances(const orc_index *ix, const float *q, uint32_t p
     free(qn); free(Q);
 }
 
-typedef struct { float d; uint64_t id, pos; } cand;
-
-static int cand_cmp(const void *a, const void *b)
+/* state: the query (normalised for cosine), then the slot's u8 table */
+static void pq4_kind_partition(const orc_ivf_kind *k, void *state, uint32_t part, float *dists)
 {
-    const cand *x = (const cand *)a, *y = (const cand *)b;
-    const int xn = x->d != x->d, yn = y->d != y->d;   /* NaN after every number: a strict weak order */
-    if (xn != yn) return xn ? 1 : -1;
-    if (x->d < y->d) return -1;
-    if (x->d > y->d) return 1;
-    return x->id < y->id ? -1 : (x->id > y->id ? 1 : 0);
-}
-
-static int keep_row(const orc_params *p, uint64_t id, float d)
-{
-    if (d != d) return 0;
-    if (p->allow && (id >= p->allow_bits || !((p->allow[id >> 5] >> (id & 31)) & 1u))) return 0;
-    if (p->has_lower && !(d >= p->lower)) return 0;
-    if (p->has_upper && !(d < p->upper)) return 0;
-    return 1;
-}
-
-typedef struct {
-    const orc_index *ix;
-    const float *queries;
-    uint32_t q0, q1;
-    const orc_params *p;
-    uint64_t *out_ids; float *out_dist; uint32_t *out_count;
-    int err;
-} job;
-
-static void *worker(void *arg)
-{
-    job *j = (job *)arg;
-    const orc_index *ix = j->ix;
-    const orc_params *p = j->p;
-    const uint32_t dim = ix->dim, nlist = ix->nlist;
-    const uint32_t nprobes = p->nprobes < nlist ? p->nprobes : nlist;
-    uint32_t nprobes_max = nprobes;
-    if (p->allow && p->max_nprobes > nprobes) nprobes_max = p->max_nprobes < nlist ? p->max_nprobes : nlist;
-    const uint32_t kk = p->refine_factor ? p->k * p->refine_factor : p->k;
-    size_t max_part = 1;
-    for (uint32_t q = 0; q < nlist; q++) {
-        const size_t n = ix->part_offsets[q + 1] - ix->part_offsets[q];
-        if (n > max_part) max_part = n;
-    }
-    float *qn = (float *)malloc(sizeof(float) * (dim ? dim : 1));
-    uint8_t *Q = (uint8_t *)malloc((size_t)ix->m * 16);
-    float *dists = (float *)malloc(sizeof(float) * max_part);
-    uint32_t *parts = (uint32_t *)malloc(sizeof(uint32_t) * (nlist ? nlist : 1));
-    float *pd = (float *)malloc(sizeof(float) * (nlist ? nlist : 1));
-    cand *c = (cand *)malloc(sizeof(cand) * (ix->nrows ? ix->nrows : 1));
-    if (!qn || !Q || !dists || !parts || !pd || !c) { j->err = 1; goto done; }
-    for (uint32_t qi = j->q0; qi < j->q1; qi++) {
-        const float *q = j->queries + (size_t)qi * dim;
-        if (ix->metric == ORC_COSINE) orc_normalize_f32(q, dim, qn);
-        else memcpy(qn, q, sizeof(float) * dim);
-        uint64_t nc = 0;
-        for (uint32_t np_use = nprobes;;) {
-            orc_find_partitions(ix, qn, np_use, parts, pd, NULL);
-            nc = 0;
-            for (uint32_t s = 0; s < np_use; s++) {
-                if (pd[s] != pd[s]) continue;
-                const uint64_t a = ix->part_offsets[parts[s]], b = ix->part_offsets[parts[s] + 1];
-                if (a == b) continue;
-                pq4_partition(ix, qn, parts[s], Q, dists);
-                for (uint64_t r = a; r < b; r++) {
-                    const float d = dists[r - a];
-                    if (keep_row(p, ix->row_ids[r], d)) { c[nc].d = d; c[nc].id = ix->row_ids[r]; c[nc].pos = r; nc++; }
-                }
-            }
-            if (np_use >= nprobes_max || nc >= p->k) break;
-            np_use = nprobes_max;
-        }
-        qsort(c, nc, sizeof(cand), cand_cmp);
-        if (nc > kk) nc = kk;
-        if (p->refine_factor && ix->vectors) {
-            uint64_t kept = 0;                     /* a NaN exact distance is never returned */
-            for (uint64_t i = 0; i < nc; i++) {
-                c[kept] = c[i];
-                c[kept].d = orc_distance_f32(ix->metric, q, ix->vectors + c[i].pos * dim, dim);
-                if (c[kept].d == c[kept].d) kept++;
-            }
-            nc = kept;
-            qsort(c, nc, sizeof(cand), cand_cmp);
-        }
-        const uint32_t cnt = (uint32_t)(nc < p->k ? nc : p->k);
-        for (uint32_t i = 0; i < p->k; i++) {
-            j->out_ids[(size_t)qi * p->k + i] = i < cnt ? c[i].id : UINT64_MAX;
-            j->out_dist[(size_t)qi * p->k + i] = i < cnt ? c[i].d : INFINITY;
-        }
-        j->out_count[qi] = cnt;
-    }
-done:
-    free(qn); free(Q); free(dists); free(parts); free(pd); free(c);
-    return NULL;
+    const float *qn = (const float *)state;
+    pq4_partition(k->ix, qn, part, (uint8_t *)(qn + k->ix->dim), dists);
 }
 
 int orc_pq4_search(const orc_index *ix, const float *queries, uint32_t B, const orc_params *p, uint64_t *out_ids,
                    float *out_dist, uint32_t *out_count, int nthreads)
 {
     if (!ix || !p || p->k == 0 || ix->dim == 0 || ix->m < 2 || ix->m % 2) return 1;
-    if (nthreads < 1) nthreads = 1;
-    if ((uint32_t)nthreads > B) nthreads = B ? (int)B : 1;
-    job *js = (job *)calloc((size_t)nthreads, sizeof(job));
-    pthread_t *th = (pthread_t *)calloc((size_t)nthreads, sizeof(pthread_t));
-    if (!js || !th) { free(js); free(th); return 1; }
-    for (int t = 0; t < nthreads; t++) {
-        job x = { ix, queries, (uint32_t)((uint64_t)B * t / nthreads), (uint32_t)((uint64_t)B * (t + 1) / nthreads), p,
-                  out_ids, out_dist, out_count, 0 };
-        js[t] = x;
-        if (pthread_create(&th[t], NULL, worker, &js[t]) != 0) { worker(&js[t]); th[t] = 0; }
-    }
-    int rc = 0;
-    for (int t = 0; t < nthreads; t++) {
-        if (th[t]) pthread_join(th[t], NULL);
-        rc |= js[t].err;
-    }
-    free(js);
-    free(th);
-    return rc;
+    const orc_ivf_kind k = { ix, sizeof(float) * ix->dim, sizeof(float) * ix->dim + (size_t)ix->m * 16,
+                             orc_ivf_query_f32, orc_ivf_coarse_f32, pq4_kind_partition };
+    return orc_ivf_search(&k, queries, B, p, out_ids, out_dist, out_count, nthreads);
 }

@@ -9,8 +9,8 @@ A NaN d is never returned; distance_range [lower, upper) and the allow mask drop
 maximum_nprobes widens under a prefilter; refine_factor re-ranks the k * refine_factor best by the exact f32 distance on
 the raw vectors.  Results ascend by (_distance, _rowid); unused slots are UINT64_MAX / +inf.
 
-Two statements of it: the threaded C oracle (pq4_oracle.c, built together with oracle/oracle.c so that it calls
-orc_find_partitions / orc_normalize_f32 / orc_l2_subvec / orc_dot_f32 itself), which the GPU tests and
+Two statements of it: the threaded C oracle (pq4_oracle.c, built into oracle/'s library and run by its IVF search
+driver), which the GPU tests and
 scripts/bench_ivf_pq4.py compare against and time, and the NumPy mirror below (quant_np, distance_np, tables_np,
 pq4_search_np), which the CPU tests check the C oracle against.  `data` is a lancedb_b200.index.IvfPqIndexData with
 num_bits = 4.
@@ -18,57 +18,16 @@ num_bits = 4.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_SRC = os.path.join(_HERE, "pq4_oracle.c")
-_ORACLE_SRC = os.path.join(_ROOT, "oracle", "oracle.c")
-_LIB_PATH = os.path.join(_HERE, "_build", "libpq4_oracle.so")
-_lib = None
+import oracle
+
 f32 = np.float32
-
-
-def build(force: bool = False) -> str:
-    """gcc -> tests/_build/libpq4_oracle.so with oracle/oracle.c's flags (rebuilt when a source is newer)."""
-    deps = [_SRC, _ORACLE_SRC, os.path.join(_ROOT, "oracle", "oracle.h")]
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(map(os.path.getmtime, deps)):
-        os.makedirs(os.path.dirname(_LIB_PATH), exist_ok=True)
-        subprocess.run(["gcc", "-O3", "-mavx2", "-mfma", "-mf16c", "-ffp-contract=off", "-fno-fast-math", "-fPIC",
-                        "-Wall", "-Wextra", "-std=c11", "-pthread", "-shared", "-o", _LIB_PATH, _SRC, _ORACLE_SRC,
-                        "-lm"], check=True)
-    return _LIB_PATH
-
-
-def load():
-    global _lib
-    if _lib is None:
-        import oracle
-        if not os.path.exists(_LIB_PATH):
-            build()
-        lib = C.CDLL(_LIB_PATH)
-        vp, u32 = C.c_void_p, C.c_uint32
-        lib.orc_pq4_quant.argtypes = [C.c_float, C.c_float, C.c_float]
-        lib.orc_pq4_quant.restype = C.c_uint8
-        lib.orc_pq4_distance.argtypes = [u32, C.c_float, C.c_float, u32, C.c_int]
-        lib.orc_pq4_distance.restype = C.c_float
-        lib.orc_pq4_tables.argtypes = [C.POINTER(oracle._Index), vp, u32, vp, vp]
-        lib.orc_pq4_tables.restype = None
-        lib.orc_pq4_partition_distances.argtypes = [C.POINTER(oracle._Index), vp, u32, vp]
-        lib.orc_pq4_partition_distances.restype = None
-        lib.orc_pq4_search.argtypes = [C.POINTER(oracle._Index), vp, u32, C.POINTER(oracle._Params), vp, vp, vp,
-                                       C.c_int]
-        lib.orc_pq4_search.restype = C.c_int
-        _lib = lib
-    return _lib
 
 
 def _index(data):
     """(orc_index, arrays it points into)"""
-    import oracle
     assert data.num_bits == 4
     keep = [np.ascontiguousarray(data.centroids, f32), np.ascontiguousarray(data.codebook, f32),
             np.ascontiguousarray(data.part_offsets, np.uint64), np.ascontiguousarray(data.codes_t, np.uint8),
@@ -81,7 +40,7 @@ def _index(data):
 
 def quant(t, qmin, qmax) -> np.ndarray:
     """The C oracle's orc_pq4_quant, element-wise."""
-    lib = load()
+    lib = oracle.load()
     t = np.asarray(t, f32)
     return np.array([lib.orc_pq4_quant(float(v), float(qmin), float(qmax)) for v in t.ravel()],
                     np.uint8).reshape(t.shape)
@@ -89,8 +48,7 @@ def quant(t, qmin, qmax) -> np.ndarray:
 
 def distance(S, qmin, qmax, m, metric) -> np.ndarray:
     """The C oracle's orc_pq4_distance, element-wise."""
-    import oracle
-    lib = load()
+    lib = oracle.load()
     S = np.asarray(S, np.uint32)
     return np.array([lib.orc_pq4_distance(int(s), float(qmin), float(qmax), int(m), oracle.METRICS[metric])
                      for s in S.ravel()], f32).reshape(S.shape)
@@ -102,7 +60,7 @@ def tables(data, qn, part):
     q = np.ascontiguousarray(qn, f32)
     Q = np.empty((data.m, 16), np.uint8)
     qmm = np.empty(2, f32)
-    load().orc_pq4_tables(C.byref(ix), q.ctypes.data, int(part), Q.ctypes.data, qmm.ctypes.data)
+    oracle.load().orc_pq4_tables(C.byref(ix), q.ctypes.data, int(part), Q.ctypes.data, qmm.ctypes.data)
     return Q, qmm[0], qmm[1]
 
 
@@ -112,28 +70,17 @@ def partition_distances(data, q, part) -> np.ndarray:
     q = np.ascontiguousarray(q, f32)
     n = int(data.part_offsets[part + 1] - data.part_offsets[part])
     out = np.empty(max(n, 1), f32)
-    load().orc_pq4_partition_distances(C.byref(ix), q.ctypes.data, int(part), out.ctypes.data)
+    oracle.load().orc_pq4_partition_distances(C.byref(ix), q.ctypes.data, int(part), out.ctypes.data)
     return out[:n]
 
 
 def search(data, queries, k: int, nprobes: int, refine_factor: int = 0, lower=None, upper=None, allow=None,
            max_nprobes: int = 0, nthreads: int = 0):
     """(ids [B, k] u64, dist [B, k] f32, count [B] u32) from the C oracle; allow: optional bool mask over row ids."""
-    import oracle
     q = np.ascontiguousarray(queries, f32).reshape(-1, data.dim)
-    B = q.shape[0]
     ix, keep = _index(data)
-    bm = None
-    if allow is not None:
-        a = np.asarray(allow, bool)
-        bm = oracle.allow_bitmap(np.nonzero(a)[0], a.size)
-    p = oracle._params(k, nprobes, refine_factor, lower, upper, bm, 0 if allow is None else np.asarray(allow).size,
-                       max_nprobes)
-    ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), f32); cnt = np.empty(B, np.uint32)
-    if B and load().orc_pq4_search(C.byref(ix), q.ctypes.data, B, C.byref(p), ids.ctypes.data, dist.ctypes.data,
-                                   cnt.ctypes.data, int(nthreads) if nthreads else (os.cpu_count() or 1)) != 0:
-        raise MemoryError("orc_pq4_search failed")
-    return ids, dist, cnt
+    return oracle.search_call("orc_pq4_search", (C.byref(ix), q.ctypes.data), q.shape[0], k, nthreads, nprobes,
+                              refine_factor, lower, upper, allow, max_nprobes=max_nprobes)
 
 
 def random_pq4_index(rng, n=600, dim=32, nlist=6, m=8, metric="l2", with_vectors=True, empty=(1,), sizes=None,
@@ -270,54 +217,13 @@ def partition_distances_np(data, qn, part) -> np.ndarray:
 
 def pq4_search_np(data, queries, k: int, nprobes: int, refine_factor: int = 0, lower=None, upper=None, allow=None,
                   max_nprobes: int = 0):
-    """The mirror of orc_pq4_search (find_partitions and the refine distances from oracle/oracle_np.py)."""
+    """The mirror of orc_pq4_search (the search loop, find_partitions and the refine distances from
+    oracle/oracle_np.py)."""
     from oracle import oracle_np as onp
     q = np.asarray(queries, f32).reshape(-1, data.dim)
-    B = q.shape[0]
-    nprobes = min(nprobes, data.nlist)
-    np_max = max(nprobes, min(max_nprobes, data.nlist)) if allow is not None else nprobes
-    kk = k * refine_factor if refine_factor else k
-    ids = np.full((B, k), np.iinfo(np.uint64).max, np.uint64)
-    dist = np.full((B, k), np.inf, f32)
-    cnt = np.zeros(B, np.uint32)
-    a = None if allow is None else np.asarray(allow, bool)
-    for b in range(B):
-        qn = onp.normalize(q[b]) if data.metric == "cosine" else q[b]
-        if data.metric == "dot":
-            cd = np.array([f32(f32(1) - onp.dot(qn, c)) for c in data.centroids], f32)
-        else:
-            cd = np.array([onp.l2(qn, c) for c in data.centroids], f32)
-        order = np.lexsort((np.arange(data.nlist), cd))
-        for np_use in (nprobes, np_max):
-            cands = []
-            for p in order[:np_use]:
-                if np.isnan(cd[p]):
-                    continue
-                s, e = int(data.part_offsets[p]), int(data.part_offsets[p + 1])
-                if s == e:
-                    continue
-                d = partition_distances_np(data, qn, p)
-                for r in range(e - s):
-                    rid = int(data.row_ids[s + r])
-                    if np.isnan(d[r]):
-                        continue
-                    if lower is not None and not d[r] >= f32(lower):
-                        continue
-                    if upper is not None and not d[r] < f32(upper):
-                        continue
-                    if a is not None and not (rid < a.size and a[rid]):
-                        continue
-                    cands.append((d[r], rid, s + r))
-            if len(cands) >= k:
-                break
-        cands.sort()
-        cands = cands[:kk]
-        if refine_factor and data.vectors is not None:
-            dfun = {"cosine": onp.cosine, "l2": onp.l2, "dot": lambda x, y: f32(f32(1) - onp.dot(x, y))}[data.metric]
-            cands = [(dfun(q[b], data.vectors[pos]), rid, pos) for _, rid, pos in cands]
-            cands = sorted(c for c in cands if not np.isnan(c[0]))     # a NaN distance is never returned
-        n = min(k, len(cands))
-        ids[b, :n] = [c[1] for c in cands[:n]]
-        dist[b, :n] = [c[0] for c in cands[:n]]
-        cnt[b] = n
-    return ids, dist, cnt
+    qn = [onp.query(data.metric, x) for x in q]
+    return onp.ivf_search_np(len(q), data, k, nprobes, lambda b: onp.coarse(data.metric, qn[b], data.centroids),
+                             lambda b, p: partition_distances_np(data, qn[b], p),
+                             None if data.vectors is None else lambda b, r: onp.distance(data.metric, q[b],
+                                                                                         data.vectors[r]),
+                             refine_factor, lower, upper, allow, max_nprobes)
