@@ -17,7 +17,7 @@
 #include <cstring>
 #include <mutex>
 #include <thread>
-#include <unordered_set>
+#include <unordered_map>
 #include <vector>
 
 #include <dlfcn.h>
@@ -175,13 +175,27 @@ struct WorkspacePool {
 using namespace lgpu;
 
 // ---- live-handle registry: every entry point resolves its handle through it, so a handle that was closed (or
-// that belongs to the parent of a fork()) is rejected instead of dereferenced, and close waits for the calls
-// still inside the handle (BaseTable is Send + Sync: rust/lancedb/src/table.rs:549; queries are re-executable
-// from any tokio worker: rust/lancedb/src/query.rs:954-955).
+// that belongs to the parent of a fork()), or a live handle of another kind, is rejected instead of dereferenced, and
+// close waits for the calls still inside the handle (BaseTable is Send + Sync: rust/lancedb/src/table.rs:549; queries
+// are re-executable from any tokio worker: rust/lancedb/src/query.rs:954-955).
 namespace lgpu {
+enum class HandleKind { index, ivf_binary, flat, binary, multivec, comm };
+static const char *handle_name(HandleKind k)
+{
+    static const char *const names[] = {"index", "binary IVF index", "flat", "binary", "multivector", "communicator"};
+    return names[(int)k];
+}
+template <class H> constexpr HandleKind handle_kind();
+template <> constexpr HandleKind handle_kind<lgpu_index>() { return HandleKind::index; }
+template <> constexpr HandleKind handle_kind<lgpu_ivf_binary>() { return HandleKind::ivf_binary; }
+template <> constexpr HandleKind handle_kind<lgpu_flat>() { return HandleKind::flat; }
+template <> constexpr HandleKind handle_kind<lgpu_binary>() { return HandleKind::binary; }
+template <> constexpr HandleKind handle_kind<lgpu_multivec>() { return HandleKind::multivec; }
+template <> constexpr HandleKind handle_kind<lgpu_comm>() { return HandleKind::comm; }
+
 static std::mutex g_live_mu;
 static std::condition_variable g_live_cv;
-static std::unordered_set<const void *> g_live;
+static std::unordered_map<const void *, HandleKind> g_live;
 static std::atomic<bool> g_cuda_touched{false};   // this process has created a CUDA context through the library
 static std::atomic<bool> g_fork_poisoned{false};  // we are the child of a fork() taken after that
 // fork(): the reference rebuilds its tokio runtime in the child (python/src/runtime.rs:68-81); a CUDA context has
@@ -194,22 +208,32 @@ static void atfork_child()
     if (g_cuda_touched.load()) g_fork_poisoned.store(true);
     g_live_mu.unlock();
 }
-static void register_handle(const void *h)
+template <class H> static void register_handle(const H *h)
 {
     static std::once_flag once;
     std::call_once(once, [] { pthread_atfork(atfork_prepare, atfork_parent, atfork_child); });
     std::lock_guard<std::mutex> g(g_live_mu);
-    g_live.insert(h);
+    g_live[h] = handle_kind<H>();
+}
+// throws unless p is a live handle of kind `want` (g_live_mu held)
+static void require_live(const void *p, HandleKind want)
+{
+    const auto it = p ? g_live.find(p) : g_live.end();
+    if (it == g_live.end())
+        set_error(std::string(handle_name(want)) + " handle is null, closed, or was opened in another process (fork)");
+    else if (it->second != want)
+        set_error(std::string(handle_name(want)) + " handle expected, got " +
+                  (it->second == HandleKind::index ? "an " : "a ") + handle_name(it->second) + " handle");
+    else
+        return;
+    throw Failure{LGPU_INVALID_INPUT};
 }
 template <class H> struct HandleRef {
     H *h;
-    HandleRef(H *p, const char *what) : h(nullptr)
+    explicit HandleRef(H *p) : h(nullptr)
     {
         std::lock_guard<std::mutex> g(g_live_mu);
-        if (!p || !g_live.count(p)) {
-            set_error(std::string(what) + " handle is null, closed, or was opened in another process (fork)");
-            throw Failure{LGPU_INVALID_INPUT};
-        }
+        require_live(p, handle_kind<H>());
         p->refs.fetch_add(1);
         h = p;
     }
@@ -219,16 +243,18 @@ template <class H> struct HandleRef {
     }
     H *operator->() const { return h; }
 };
-// unregister and wait until no call is inside the handle any more; false = it was not a live handle
+// unregister and wait until no call is inside the handle any more; false = it was not a live handle of kind H
 template <class H> static bool retire_handle(H *p)
 {
     std::unique_lock<std::mutex> g(g_live_mu);
-    if (!p || !g_live.erase(p)) return false;
+    const auto it = p ? g_live.find(p) : g_live.end();
+    if (it == g_live.end() || it->second != handle_kind<H>()) return false;
+    g_live.erase(it);
     g_live_cv.wait(g, [&] { return p->refs.load() == 0; });
     return true;
 }
-// every *_close: unregister, drain the handle's device, free it.  A null or closed handle, or a parent-process
-// handle in a fork child, is left alone.
+// every *_close: unregister, drain the handle's device, free it.  A null or closed handle, a handle of another kind,
+// or a parent-process handle in a fork child, is left alone.
 template <class H> static void close_handle(H *p)
 {
     if (!retire_handle(p)) return;
@@ -256,9 +282,15 @@ struct Coalescer {
 };
 }  // namespace lgpu
 
+namespace lgpu {
+// the kinds of IVF index: 8-bit and 4-bit PQ codes, 8-bit scalar codes, 1-bit RaBitQ codes, packed binary rows
+enum class IvfKind { pq8, pq4, sq, rq, ham };
+}  // namespace lgpu
+
 struct lgpu_index {
     std::atomic<int> refs{0};
     Coalescer coalescer;
+    IvfKind kind = IvfKind::pq8;
     int device = 0, num_sms = 0;
     uint32_t dim = 0, nlist = 0, m = 0, dsub = 0, nch = 0;
     uint32_t max_nrb = 1;          // row blocks (of 1536 rows) of the largest partition: bounds the tile count
@@ -276,31 +308,27 @@ struct lgpu_index {
     bool has_tc = false;
     bool has_vectors = false;
     // IVF_SQ (lgpu_ivf_sq_open): `codes` holds [nrows][dim_pad] u8 row codes, `sq_xx` the sum of each row's squared codes
-    bool is_sq = false;
     uint32_t dim_pad = 0;
     double sq_lo = 0.0, sq_hi = 0.0;
     DevBuf sq_xx;
     // IVF_RQ (lgpu_ivf_rq_open): `codes` holds [nrows][rq_wpr] u32 sign bits; the rotation, the rotated centroids and
     // the per-row factors and popcounts
-    bool is_rq = false;
     uint32_t rq_wpr = 0;
     DevBuf rq_rot, rq_rc, rq_add, rq_scale, rq_popc;
     // 4-bit IVF_PQ (lgpu_index_open with nbits = 4): `codes` holds per partition [m/2][npad] packed bytes, `pq4_cb` the
     // codebook [m][dsub][16] (element-major); no filter tables
-    bool is_pq4 = false;
     DevBuf pq4_cb;
+    // binary IVF_FLAT (lgpu_ivf_binary_open; `dim` = nbytes): `centroids` holds the packed centroids [nlist][nbytes_pad]
+    // and `codes` the packed rows [nrows][nbytes_pad] in partition order, both zero-padded, and their popcounts
+    uint32_t nbytes = 0, nbytes_pad = 0;
+    DevBuf cent_pop, row_pop;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
     WorkspacePool pool;
 };
 
-// a binary IVF_FLAT index (lgpu_ivf_binary_open): the IVF partition arrays of lgpu_index (part_n, part_off, row_ids,
-// pad_prefix, ...; `dim` = nbytes), with `centroids` holding the packed centroids [nlist][nbytes_pad] and `codes` the
-// packed rows [nrows][nbytes_pad] in partition order, both zero-padded, and their popcounts
-struct lgpu_ivf_binary : lgpu_index {
-    uint32_t nbytes = 0, nbytes_pad = 0;
-    DevBuf cent_pop, row_pop;
-};
+// the C header's handle type of a binary IVF_FLAT index (an lgpu_index of kind IvfKind::ham)
+struct lgpu_ivf_binary : lgpu_index {};
 
 struct lgpu_flat {
     std::atomic<int> refs{0};
@@ -672,11 +700,56 @@ static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, c
     LGPU_REQUIRE(B == 0 || (q && ids && dist && cnt), "null buffer");
 }
 
-// ---- IVF search (IVF_PQ, IVF_SQ and IVF_RQ).  One sub-batch runs [cosine: normalise] -> coarse step (probes) ->
-// small scan | regroup -> filter scan + fix-up | exact scan + select -> [refine], on the paths ivf_plan picks before
-// any launch ----
+// binary vectors (Hamming distance): the crossovers of the flat search (DESIGN.md section 6) and of the binary IVF
+// coarse step
+constexpr uint64_t HAM_SAMPLE = 65536;     // rows of the threshold sample
+constexpr uint32_t HAM_TC_MIN_B = 128;     // dense tensor-core path from this many queries (measured: SIMT faster at
+                                           // 64 queries x 60000 rows, wgmma at 256) ...
+constexpr uint64_t HAM_TC_MIN_N = 4096;    // ... and this many rows (not measured)
+
+// ---- IVF search (IVF_PQ 8-bit and 4-bit, IVF_SQ, IVF_RQ and binary IVF_FLAT).  One sub-batch runs [cosine:
+// normalise] -> coarse step (probes) -> small scan | regroup -> filter scan + fix-up | exact scan + select -> [refine],
+// on the paths ivf_plan picks before any launch ----
 enum class Coarse { exact, tc_dense, tc_list };   // see ivf_coarse
 enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq, pq4, ham };
+
+// bytes of one stored row, as the scan reads them (profiling: lgpu_last_scanned_code_bytes)
+static uint32_t ivf_row_bytes(const lgpu_index *ix)
+{
+    switch (ix->kind) {
+    case IvfKind::pq8: return ix->m;
+    case IvfKind::pq4: return ix->m / 2;
+    case IvfKind::sq: return ix->dim;
+    case IvfKind::rq: return ix->rq_wpr * 4;
+    case IvfKind::ham: return ix->nbytes_pad;
+    }
+    return 0;
+}
+
+// workspace bytes per query of a sub-batch that only the kind uses: the per-slot u8 tables (pq4), the per-slot
+// bit-planes and the rotated query (rq), the probe slots' ids, distances, regroup and tile descriptors (ham)
+static size_t ivf_kind_query_bytes(const lgpu_index *ix, uint32_t nprobes, uint32_t np_eff)
+{
+    switch (ix->kind) {
+    case IvfKind::pq4: return (size_t)nprobes * (16 * ix->m + sizeof(Pq4Slot));
+    case IvfKind::rq: return (size_t)nprobes * (16 * ix->rq_wpr + sizeof(RqSlot)) + (size_t)ix->dim * 4;
+    case IvfKind::ham: return (size_t)np_eff * 36 + (size_t)np_eff * ix->max_nrb * (sizeof(TileDesc) / SCAN_G + 1) + 64;
+    default: return 0;
+    }
+}
+
+// the queries of an IVF sub-batch in the kind's format: f32 rows [B][dim], or (ham) rows packed to [B][nbytes_pad]
+// bytes and their popcounts
+struct IvfQueries {
+    const float *f;
+    const uint8_t *h;
+    const uint32_t *pop;
+    size_t ld;                // elements of one row
+    IvfQueries at(uint32_t q0) const
+    {
+        return {f ? f + q0 * ld : nullptr, h ? h + q0 * ld : nullptr, pop ? pop + q0 : nullptr, ld};
+    }
+};
 
 struct IvfPlan {
     uint32_t B, nprobes, slots;
@@ -718,19 +791,23 @@ static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, cons
     if (ix->has_tc && tc_enabled() && ix->metric != LGPU_DOT && B >= 8 && nlist >= 256 && coarse_short > nprobes && big)
         p.coarse = modes.coarse_list_min && nlist >= modes.coarse_list_min && ix->cent_ns >= 4 * nprobes && nprobes <= 64
                        ? Coarse::tc_list : Coarse::tc_dense;
+    // every kind but 8-bit PQ: one exact scan, never the small or the filter path.  Hamming distances are exact:
+    // no refine.
+    switch (ix->kind) {
+    case IvfKind::pq4: p.scan = IvfScan::pq4; return p;
+    case IvfKind::sq: p.scan = IvfScan::sq; return p;
+    case IvfKind::rq: p.scan = IvfScan::rq; return p;
+    case IvfKind::ham: p.scan = IvfScan::ham; p.kk = p.k; p.refine = false; return p;
+    case IvfKind::pq8: break;
+    }
     // tiny batches (a single query, a micro-batch): the small path, 4 launches instead of ~25; LGPU_SMALL_SLOTS = 0
     // disables it.  Otherwise filter + verify (scan3.cu) unless the request needs every exact distance.
-    if (ix->is_pq4) {                  // 4-bit codes: one exact integer scan, never the small or the filter path
-        p.scan = IvfScan::pq4;
-        return p;
-    }
-    const bool small = !ix->is_sq && !ix->is_rq && !widening && p.slots <= modes.small_slots &&
-                       small_scan_smem(ix->m, ix->dim) <= 200 * 1024 &&
+    const bool small = !widening && p.slots <= modes.small_slots && small_scan_smem(ix->m, ix->dim) <= 200 * 1024 &&
                        (size_t)p.slots * ix->pad_prefix[1] * 4 <= workspace_budget();
     const bool filter = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && p.lb_short > p.kk &&
                         ix->m <= 512 && !widening && !small;
     if (small) p.scan = IvfScan::small;
-    else if (!filter) p.scan = ix->is_sq ? IvfScan::sq : (ix->is_rq ? IvfScan::rq : IvfScan::exact_pq);
+    else if (!filter) p.scan = IvfScan::exact_pq;
     if (!filter) return p;
     // candidate mode (no prefilter, kk <= LGPU_CAND_KMAX): the scanners threshold the rows themselves, nothing dense is
     // written.  LGPU_CAND_CAP shrinks the capacity to exercise the overflow path.
@@ -843,19 +920,35 @@ static void coarse_list(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const f
 // needs most of an SM's shared memory) are not queued behind the table grids and, as SMs free up, the probe selection
 // after it is dispatched ahead of the waiting table CTAs by the priority of `front` (making the tables wait for the GEMM
 // to finish was measured slower: the tables are then the longer branch); after the probe select (exact variant).
-static void ivf_coarse(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *qs, cudaStream_t cs,
+// Binary IVF_FLAT: Hamming distances to the packed centroids, or every partition when nprobes covers them all.
+static void ivf_coarse(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const IvfQueries &q, cudaStream_t cs,
                        cudaStream_t st, const StageMarks &mark)
 {
     const uint32_t B = p.B, nprobes = p.nprobes, nlist = ix->nlist, dim = ix->dim;
+    const float *qs = q.f;
     ws->probes.ensure((size_t)p.slots * 8);
+    if (p.scan == IvfScan::ham && nprobes >= nlist) {   // every partition: no coarse step, no top-nprobes select
+        launch_ham_all_probes(ws->probes.as<uint64_t>(), B, nlist, cs);
+        mark(IVF_COARSE, cs);
+        return;
+    }
     ws->probe_dist.ensure((size_t)p.slots * 4);
     ws->probe_cnt.ensure((size_t)B * 4);
     const uint64_t ldc = (nlist + 3u) & ~3u;
     ws->D.ensure((size_t)B * ldc * 4);
     const TopkOut probes{ws->probes.as<uint64_t>(), ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>()};
     if (p.coarse == Coarse::exact) {
-        launch_dist_matrix(qs, ix->centroids.as<float>(), B, nlist, dim, ix->metric == LGPU_DOT ? 1 : 0, nullptr, nullptr,
-                           ws->D.as<float>(), ldc, cs);
+        // binary: the b1 wgmma kernel from the flat path's crossover (HAM_TC_MIN_B x HAM_TC_MIN_N); for the coarse
+        // step's shapes the crossover is not measured
+        if (p.scan != IvfScan::ham)
+            launch_dist_matrix(qs, ix->centroids.as<float>(), B, nlist, dim, ix->metric == LGPU_DOT ? 1 : 0, nullptr,
+                               nullptr, ws->D.as<float>(), ldc, cs);
+        else if (tc_enabled() && B >= HAM_TC_MIN_B && nlist >= HAM_TC_MIN_N)
+            launch_ham_gemm(q.h, ix->centroids.p, ix->cent_pop.as<uint32_t>(), q.pop, B, nlist, ix->nbytes_pad,
+                            ws->D.as<float>(), ldc, ix->num_sms, cs);
+        else
+            launch_ham_dense(q.h, ix->centroids.as<uint8_t>(), B, nlist, ix->nbytes_pad, ws->D.as<float>(), ldc,
+                             ix->num_sms, cs);
         mark(IVF_COARSE, cs);
         launch_select(select_rows(ws->D.as<float>(), nlist, ldc, B, nprobes, probes), cs);
         if (p.filter()) query_tables(ix, ws, qs, B, st);
@@ -1113,10 +1206,10 @@ static void filter_fixup(lgpu_index *ix, Workspace *ws, const IvfPlan &p, GroupA
     launch_select(sf, st);
 }
 
-// IvfScan::exact_pq / sq / rq: the exact scan of every regrouped tile, then the PQ top-kk
-static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp, const float *qs,
-                      const GroupArgs &ga, RowFilter rf, const uint32_t *only, TopkOut pq, cudaStream_t st,
-                      const StageMarks &mark)
+// IvfScan::exact_pq / sq / rq / pq4 / ham: the exact scan of every regrouped tile, then the PQ top-kk
+static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp,
+                      const IvfQueries &q, const GroupArgs &ga, RowFilter rf, const uint32_t *only, TopkOut pq,
+                      cudaStream_t st, const StageMarks &mark)
 {
     if (p.scan == IvfScan::sq) {
         SqScanArgs qa{};
@@ -1136,8 +1229,15 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
         launch_rq_scan(ra, 2 * ix->num_sms, st);
     } else if (p.scan == IvfScan::pq4) {
         launch_pq4_scan(pq4_args(ix, ws, ga), 2 * ix->num_sms, st);
+    } else if (p.scan == IvfScan::ham) {
+        HamScanArgs ha{};
+        ha.rows = ix->codes.as<uint8_t>(); ha.row_pop = ix->row_pop.as<uint32_t>(); ha.queries = q.h; ha.qpop = q.pop;
+        ha.nbytes_pad = ix->nbytes_pad;
+        ha.total_tiles = ga.total_tiles; ha.tile_counter = ga.tile_counter; ha.tile_desc = ga.tile_desc;
+        ha.dist_out = ws->dist_out.as<float>();
+        launch_ivf_ham_scan(ha, 2 * ix->num_sms, st);
     } else {
-        launch_scan2(scan_args(ix, ws, qs, ga), ix->dsub, ix->num_sms, st);
+        launch_scan2(scan_args(ix, ws, q.f, ga), ix->dsub, ix->num_sms, st);
     }
     mark(IVF_SCAN, st);
     SelectArgs sa = select_segments(ix, ws, p, p.kk, pq, rf);
@@ -1158,10 +1258,9 @@ static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const fl
     launch_select(sr, st);
 }
 
-// one sub-batch of an IVF_PQ / IVF_SQ / IVF_RQ search, everything device-side on `st` (and `front`, joined).  only
-// (device, [B]): redo just the flagged queries (maximum_nprobes widening) -- exact kernels, the other queries' outputs
-// are left untouched.
-void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
+// one sub-batch of an IVF search, everything device-side on `st` (and `front`, joined).  only (device, [B]): redo just
+// the flagged queries (maximum_nprobes widening) -- exact kernels, the other queries' outputs are left untouched.
+void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const IvfQueries &q, uint32_t B,
                    const lgpu_search_params &sp, uint32_t nprobes, TopkOut out, bool prof, RowFilter rf,
                    const uint32_t *only = nullptr)
 {
@@ -1169,9 +1268,11 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
     const StageMarks mark{ws, prof};
     mark(IVF_START, st);
     ws->stats_mode = 0;
-    const float *qs = ivf_queries(ix, ws, st, d_q, B);
+    IvfQueries prep = q;
+    prep.f = ivf_queries(ix, ws, st, q.f, B);
+    const float *qs = prep.f;
     const cudaStream_t cs = p.filter() ? fork_front(ix, ws, st, B) : st;   // the coarse step's and the regroup's
-    ivf_coarse(ix, ws, p, qs, cs, st, mark);
+    ivf_coarse(ix, ws, p, prep, cs, st, mark);
     if (p.scan == IvfScan::sq) {
         ws->sq_q.ensure((size_t)B * ix->dim_pad); ws->sq_qq.ensure((size_t)B * 4);
         launch_sq_encode(qs, B, ix->dim, ix->dim_pad, ix->sq_lo, ix->sq_hi, ws->sq_q.as<uint8_t>(),
@@ -1202,20 +1303,20 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *
             filter_fixup(ix, ws, p, ga, sc, rf, pq, st);
             mark(IVF_TOPK, st);
         } else {
-            ivf_exact(ix, ws, p, sp, qs, ga, rf, only, pq, st, mark);
+            ivf_exact(ix, ws, p, sp, prep, ga, rf, only, pq, st, mark);
         }
     }
     if (!p.refine) return;
-    ivf_refine(ix, ws, p, d_q, out, only, st);
+    ivf_refine(ix, ws, p, q.f, out, only, st);
     mark(IVF_REFINE, st);
 }
 
 uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
 {
     uint32_t np_eff = std::min<uint32_t>(nprobes, ix->nlist);
-    size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4);
-    if (ix->is_rq) per_q += (size_t)nprobes * (16 * ix->rq_wpr + sizeof(RqSlot)) + (size_t)ix->dim * 4;  // planes, rq
-    if (ix->is_pq4) per_q += (size_t)nprobes * (16 * ix->m + sizeof(Pq4Slot));                        // u8 tables
+    // distance segments, coarse scores, the filter scan's per-query tables, then the kind's own buffers
+    size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4) +
+                   ivf_kind_query_bytes(ix, nprobes, np_eff);
     size_t bs = workspace_budget() / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
     bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
@@ -1260,35 +1361,49 @@ static uint64_t add_ivf_profile(Workspace *ws, cudaStream_t st, uint32_t b)
     return rows;
 }
 
-void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
+// the queries of an IVF call in the kind's format: the caller's f32 rows, or (ham) the caller's bytes [B][nbytes]
+// packed once per call into ws->hq / hq_pop
+static IvfQueries ivf_call_queries(lgpu_index *ix, Workspace *ws, cudaStream_t st, const void *d_q, uint32_t B)
+{
+    if (ix->kind != IvfKind::ham) return {static_cast<const float *>(d_q), nullptr, nullptr, ix->dim};
+    const uint32_t nbp = ix->nbytes_pad;
+    ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
+    launch_ham_pack(static_cast<const uint8_t *>(d_q), ix->nbytes, ix->nbytes, B, ws->hq.as<uint8_t>(), nbp,
+                    ws->hq_pop.as<uint32_t>(), st);
+    return {nullptr, ws->hq.as<uint8_t>(), ws->hq_pop.as<uint32_t>(), nbp};
+}
+
+// d_q: the caller's queries in device memory, [B][dim] f32 or (binary IVF_FLAT) [B][nbytes] bytes
+void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const void *d_q, uint32_t B,
                        const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                        RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
 {
     const uint32_t nprobes = std::min<uint32_t>(std::max<uint32_t>(sp.nprobes, 1), ix->nlist);
-    const uint32_t np_widest = rf.bits ? std::max(nprobes, std::min<uint32_t>(sp.max_nprobes, ix->nlist)) : nprobes;
-    const uint32_t bs = ivf_sub_batch_size(ix, B, np_widest);
+    // maximum_nprobes (query.rs:1250-1275): under a prefilter, the queries that found fewer than k rows in their
+    // minimum_nprobes partitions are searched again over their maximum_nprobes nearest (no work if none is)
+    const uint32_t np_max = std::min<uint32_t>(sp.max_nprobes, ix->nlist);
+    const bool widen = rf.bits && np_max > nprobes;
+    if (widen)
+        LGPU_REQUIRE(np_max <= SELECT_KMAX || np_max >= ix->nlist,
+                     "maximum_nprobes above 2048 is not supported unless it covers every partition");
+    const uint32_t bs = ivf_sub_batch_size(ix, B, widen ? np_max : nprobes);
     const bool prof = profiling_enabled();
-    const uint32_t row_bytes = ix->is_sq ? ix->dim : ix->is_rq ? ix->rq_wpr * 4 : ix->is_pq4 ? ix->m / 2 : ix->m;
     if (prof) {
         memset(g_stage_ms, 0, sizeof(g_stage_ms));
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
         g_scanned_bytes = 0;
     }
+    const IvfQueries qs = ivf_call_queries(ix, ws, st, d_q, B);
     const TopkOut out{d_ids, d_dist, d_cnt};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
-        const float *q = d_q + (size_t)q0 * ix->dim;
-        ivf_sub_batch(ix, ws, st, q, b, sp, nprobes, out.at(q0, sp.k), prof, rf);
-        if (prof) g_scanned_bytes += add_ivf_profile(ws, st, b) * row_bytes;
-        // maximum_nprobes (query.rs:1250-1275): under a prefilter, the queries that found fewer than k rows in their
-        // minimum_nprobes partitions are searched again over their maximum_nprobes nearest (no work if none is)
-        const uint32_t np_max = std::min<uint32_t>(sp.max_nprobes, ix->nlist);
-        if (rf.bits && np_max > nprobes) {
-            LGPU_REQUIRE(np_max <= SELECT_KMAX || np_max >= ix->nlist, "maximum_nprobes above 2048 is not supported");
+        ivf_sub_batch(ix, ws, st, qs.at(q0), b, sp, nprobes, out.at(q0, sp.k), prof, rf);
+        if (prof) g_scanned_bytes += add_ivf_profile(ws, st, b) * ivf_row_bytes(ix);
+        if (widen) {
             ws->widen.ensure((size_t)b * 4);
             launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
-            ivf_sub_batch(ix, ws, st, q, b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
+            ivf_sub_batch(ix, ws, st, qs.at(q0), b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
         }
     }
 }
@@ -1354,11 +1469,6 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
 //                 every batch size measured, one query included: a single query's select over a dense row of N
 //                 columns runs on one SM.
 // Every path computes exact integer distances, so all three return the same rows.
-constexpr uint64_t HAM_SAMPLE = 65536;     // rows of the threshold sample
-constexpr uint32_t HAM_TC_MIN_B = 128;     // dense tensor-core path from this many queries (measured: SIMT faster at
-                                           // 64 queries x 60000 rows, wgmma at 256) ...
-constexpr uint64_t HAM_TC_MIN_N = 4096;    // ... and this many rows (not measured)
-
 // Candidate-list capacity of the list path.  Rows with d <= tau_q, tau_q the k-th smallest distance among the sample's
 // rows, number about k N / ns (more under ties): 4x that, at least 1024, at most 16384.
 static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
@@ -1473,112 +1583,6 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         LGPU_CUDA(cudaStreamSynchronize(st));
         g_filter_stats[1] = tc ? (uint64_t)B * (N + (list ? bx->nsample : 0)) : 0;
         g_filter_stats[3] = B;
-    }
-}
-
-// ---- binary IVF_FLAT (lgpu_ivf_binary): Hamming coarse step -> regroup (group.cu) -> b1 MMA scan of the probed rows
-// (ivf_ham_scan.cu) -> top-k over the distance segments (select mode 0), the IVF stages of lgpu_index ----
-
-// One sub-batch, everything on `st`.  Q / qpop: the sub-batch's packed queries [B][nbytes_pad] and their popcounts.
-// nprobes <= nlist.  only (device, [B]): redo just the flagged queries (maximum_nprobes widening).
-static void ham_ivf_sub_batch(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
-                              uint32_t B, const lgpu_search_params &sp, uint32_t nprobes, TopkOut out, bool prof,
-                              RowFilter rf, const uint32_t *only = nullptr)
-{
-    IvfPlan p{};
-    p.B = B; p.nprobes = nprobes; p.slots = B * nprobes; p.np_eff = nprobes;
-    p.k = p.kk = sp.k; p.coarse = Coarse::exact; p.scan = IvfScan::ham;
-    const uint32_t nlist = ix->nlist, nbp = ix->nbytes_pad;
-    const StageMarks mark{ws, prof};
-    mark(IVF_START, st);
-    ws->stats_mode = 0;
-    ws->probes.ensure((size_t)p.slots * 8);
-    if (nprobes >= nlist) {                       // every partition: no coarse step, no top-nprobes select
-        launch_ham_all_probes(ws->probes.as<uint64_t>(), B, nlist, st);
-        mark(IVF_COARSE, st);
-    } else {
-        // Hamming distances to the packed centroids, then the nprobes nearest by (distance, partition id).  The b1
-        // wgmma kernel from the flat path's crossover (HAM_TC_MIN_B x HAM_TC_MIN_N); for the coarse step's shapes the
-        // crossover is not measured.
-        const uint64_t ldc = (nlist + 3u) & ~3u;
-        ws->probe_dist.ensure((size_t)p.slots * 4); ws->probe_cnt.ensure((size_t)B * 4);
-        ws->D.ensure((size_t)B * ldc * 4);
-        if (tc_enabled() && B >= HAM_TC_MIN_B && nlist >= HAM_TC_MIN_N)
-            launch_ham_gemm(Q, ix->centroids.p, ix->cent_pop.as<uint32_t>(), qpop, B, nlist, nbp, ws->D.as<float>(), ldc,
-                            ix->num_sms, st);
-        else
-            launch_ham_dense(Q, ix->centroids.as<uint8_t>(), B, nlist, nbp, ws->D.as<float>(), ldc, ix->num_sms, st);
-        mark(IVF_COARSE, st);
-        launch_select(select_rows(ws->D.as<float>(), nlist, ldc, B, nprobes, {ws->probes.as<uint64_t>(),
-                                  ws->probe_dist.as<float>(), ws->probe_cnt.as<uint32_t>()}), st);
-    }
-    mark(IVF_PROBES, st);
-    const GroupArgs ga = ivf_regroup(ix, ws, p, only, st);
-    mark(IVF_REGROUP, st);
-    HamScanArgs ha{};
-    ha.rows = ix->codes.as<uint8_t>(); ha.row_pop = ix->row_pop.as<uint32_t>(); ha.queries = Q; ha.qpop = qpop;
-    ha.nbytes_pad = nbp;
-    ha.total_tiles = ga.total_tiles; ha.tile_counter = ga.tile_counter; ha.tile_desc = ga.tile_desc;
-    ha.dist_out = ws->dist_out.as<float>();
-    launch_ivf_ham_scan(ha, 2 * ix->num_sms, st);
-    mark(IVF_SCAN, st);
-    // distances are exact: refine_factor has nothing to re-rank, the top-k is taken directly
-    SelectArgs sa = select_segments(ix, ws, p, sp.k, out, rf);
-    sa.only = only;
-    with_range(sa, sp);
-    launch_select(sa, st);
-    mark(IVF_TOPK, st);
-}
-
-static uint32_t ham_ivf_sub_batch_size(lgpu_ivf_binary *ix, uint32_t B, uint32_t nprobes)
-{
-    const uint32_t np_eff = std::min<uint32_t>(nprobes, ix->nlist);
-    // distance segments, coarse scores, probe slots (ids, distances, regroup) and their tile descriptors
-    const size_t per_q = ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)np_eff * 36 +
-                         (size_t)np_eff * ix->max_nrb * (sizeof(TileDesc) / SCAN_G + 1) + 64;
-    size_t bs = workspace_budget() / per_q;
-    bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
-    bs = std::max<size_t>(1, std::min<size_t>(bs, 65535));
-    return (uint32_t)std::min<size_t>(bs, B);
-}
-
-// d_q: raw queries [B][nbytes] in device memory
-void ivf_binary_search_device(lgpu_ivf_binary *ix, Workspace *ws, cudaStream_t st, const uint8_t *d_q, uint32_t B,
-                              const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
-                              RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
-{
-    const uint32_t nbp = ix->nbytes_pad;
-    const uint32_t nprobes = std::min<uint32_t>(std::max<uint32_t>(sp.nprobes, 1), ix->nlist);
-    const uint32_t np_max = std::min<uint32_t>(sp.max_nprobes, ix->nlist);
-    const bool widen = rf.bits && np_max > nprobes;
-    // maximum_nprobes is only read when it widens (under a prefilter), as on lgpu_index
-    if (widen)
-        LGPU_REQUIRE(np_max <= SELECT_KMAX || np_max >= ix->nlist,
-                     "maximum_nprobes above 2048 is not supported unless it covers every partition");
-    const uint32_t bs = ham_ivf_sub_batch_size(ix, B, widen ? np_max : nprobes);
-    const bool prof = profiling_enabled();
-    const TopkOut out{d_ids, d_dist, d_cnt};
-    if (prof) {
-        memset(g_stage_ms, 0, sizeof(g_stage_ms));
-        memset(g_filter_stats, 0, sizeof(g_filter_stats));
-        g_scanned_bytes = 0;
-    }
-    ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
-    launch_ham_pack(d_q, ix->nbytes, ix->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
-    for (uint32_t q0 = 0; q0 < B; q0 += bs) {
-        const uint32_t b = std::min(bs, B - q0);
-        if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
-        const uint8_t *Q = ws->hq.as<uint8_t>() + (size_t)q0 * nbp;
-        const uint32_t *qpop = ws->hq_pop.as<uint32_t>() + q0;
-        ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, nprobes, out.at(q0, sp.k), prof, rf);
-        if (prof) g_scanned_bytes += add_stage_marks(ws, st) * nbp;      // the whole call, as on lgpu_index
-        // maximum_nprobes under a prefilter, as on lgpu_index: the queries that found fewer than k rows are searched
-        // again over their np_max nearest partitions
-        if (widen) {
-            ws->widen.ensure((size_t)b * 4);
-            launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
-            ham_ivf_sub_batch(ix, ws, st, Q, qpop, b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
-        }
     }
 }
 
@@ -1918,11 +1922,11 @@ static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, 
 // the kind's `search(h, ws, st, d_q, B, params, d_ids, d_dist, d_cnt, rf, deadline)` on a workspace leased for the
 // caller's stream, or staged through host_submit.
 template <class H, class T, class Check, class Search>
-int search_call(H *hp, const char *what, const Route &r, const T *queries, uint32_t B, const lgpu_search_params *p,
+int search_call(H *hp, const Route &r, const T *queries, uint32_t B, const lgpu_search_params *p,
                 uint64_t *ids, float *dist, uint32_t *cnt, Check &&check, Search &&search)
 {
     return guarded([&] {
-        HandleRef<H> h(hp, what);
+        HandleRef<H> h(hp);
         const size_t q_elems = check(h.h);
         if (r.via == Route::FILTERED) LGPU_REQUIRE(r.allow != nullptr || r.allow_bits == 0, "allow bitmap is null");
         if (B == 0) return;
@@ -1973,32 +1977,62 @@ static void check_ivf_layout(uint32_t dim, uint32_t nlist, int metric, uint64_t 
     }
 }
 
-// The arrays every IVF index holds in HBM, uploaded on the legacy stream: centroids (and their bf16 copy for the
-// tensor-core coarse step), partition sizes and offsets, row ids, optional raw vectors.  `rows_tile` is the scan's
-// tile height, which bounds the tile count of a search (max_nrb).
-static void open_ivf_partitions(lgpu_index *ix, int device, uint32_t nlist, uint64_t nrows,
-                                const uint64_t *part_offsets, const uint64_t *row_ids, uint32_t rows_tile);
-
-static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t nlist, int metric, uint64_t nrows,
-                            const float *centroids, const uint64_t *part_offsets, const uint64_t *row_ids,
-                            const float *vectors, uint32_t rows_tile)
+// copy a host array into a device buffer of at least 16 bytes, on the legacy stream
+static void upload(DevBuf &b, const void *src, size_t bytes)
 {
-    ix->dim = dim; ix->metric = metric;
+    b.ensure(std::max<size_t>(bytes, 16));
+    if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, nullptr));
+}
+
+// The partition arrays every IVF index holds (part_n, part_npad, part_off, row_ids, code_base, the host-side tile bound
+// max_nrb and pad_prefix), uploaded on the legacy stream; `rows_tile` is the scan's tile height.  code_base: the byte
+// offset of each partition's codes, which the regroup copies into the tile descriptors -- padded_code_base for the PQ
+// layouts, zeros for the row-major kinds (sq, rq, ham), whose scans address rows by part_off.
+template <class Desc>
+static void open_ivf_partitions(lgpu_index *ix, const Desc *d, uint32_t rows_tile, const std::vector<uint64_t> &code_base)
+{
+    const uint32_t nlist = d->nlist;
+    ix->device = d->device;
+    cudaDeviceProp prop;
+    LGPU_CUDA(cudaGetDeviceProperties(&prop, ix->device));
+    ix->num_sms = prop.multiProcessorCount;
+    ix->nlist = nlist; ix->nrows = d->nrows;
+    std::vector<uint32_t> part_n(nlist), part_npad(nlist);
+    std::vector<uint64_t> pads(nlist);
+    for (uint32_t p = 0; p < nlist; p++) {
+        const uint32_t n = (uint32_t)(d->part_offsets[p + 1] - d->part_offsets[p]);
+        part_n[p] = n; part_npad[p] = (n + 31u) & ~31u;
+        pads[p] = (n + 3ull) & ~3ull;
+        ix->max_nrb = std::max(ix->max_nrb, scan_nrb(n, rows_tile));
+    }
+    ix->h_part_n = part_n;
+    std::sort(pads.begin(), pads.end(), std::greater<uint64_t>());
+    ix->pad_prefix.assign(nlist + 1, 0);
+    for (uint32_t p = 0; p < nlist; p++) ix->pad_prefix[p + 1] = ix->pad_prefix[p] + pads[p];
+    upload(ix->part_n, part_n.data(), (size_t)nlist * 4);
+    upload(ix->part_npad, part_npad.data(), (size_t)nlist * 4);
+    upload(ix->part_off, d->part_offsets, (size_t)(nlist + 1) * 8);
+    upload(ix->row_ids, d->row_ids, (size_t)d->nrows * 8);
+    upload(ix->code_base, code_base.data(), (size_t)nlist * 8);
+    LGPU_CUDA(cudaStreamSynchronize(nullptr));
+}
+
+// What the float IVF indexes add, uploaded on the legacy stream: centroids (and their bf16 copy for the tensor-core
+// coarse step) and the optional raw vectors
+template <class Desc>
+static void open_ivf_common(lgpu_index *ix, const Desc *d, uint32_t rows_tile, const std::vector<uint64_t> &code_base)
+{
+    const uint32_t dim = d->dim, nlist = d->nlist;
+    ix->dim = dim; ix->metric = d->metric;
     cudaStream_t st = nullptr;
-    auto up = [&](DevBuf &b, const void *src, size_t bytes) {
-        b.ensure(std::max<size_t>(bytes, 16));
-        if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, st));
-        ix->device_bytes += b.bytes;
-    };
-    up(ix->centroids, centroids, (size_t)nlist * dim * 4);
-    open_ivf_partitions(ix, device, nlist, nrows, part_offsets, row_ids, rows_tile);
-    if (vectors) { up(ix->vectors, vectors, (size_t)nrows * dim * 4); ix->has_vectors = true; }
-    if (gemm_shape_supported(dim) && metric != LGPU_DOT) {
+    upload(ix->centroids, d->centroids, (size_t)nlist * dim * 4);
+    open_ivf_partitions(ix, d, rows_tile, code_base);
+    if (d->vectors) { upload(ix->vectors, d->vectors, (size_t)d->nrows * dim * 4); ix->has_vectors = true; }
+    if (gemm_shape_supported(dim) && d->metric != LGPU_DOT) {
         LGPU_CUDA(cudaStreamSynchronize(st));
         const bool finite =
             prepare_tc_operand(ix->centroids.as<float>(), nlist, dim, ix->cent_b, ix->cent_n2, ix->cent_max, ix->cent_err, st);
         if (!finite) { ix->cent_b.reset(); ix->cent_n2.reset(); }     // never read: the exact coarse kernels serve it
-        ix->device_bytes += ix->cent_b.bytes + ix->cent_n2.bytes;
         if (finite && nlist >= 1024) {
             // every 8th centroid, for the sampled threshold of the coarse step (strided: whatever order the
             // trainer left the lists in -- hierarchical k-means groups neighbours -- the sample spans all of them)
@@ -2011,46 +2045,9 @@ static void open_ivf_common(lgpu_index *ix, int device, uint32_t dim, uint32_t n
                                         cudaMemcpyDeviceToDevice, st));
             LGPU_CUDA(cudaStreamSynchronize(st));
             ix->cent_ns = ns;
-            ix->device_bytes += ix->cent_sb.bytes + ix->cent_sn2.bytes;
         }
         ix->has_tc = finite;                   // a non-finite centroid: the exact coarse kernels
     }
-    LGPU_CUDA(cudaStreamSynchronize(st));
-}
-
-// The partition arrays every IVF index holds (part_n, part_npad, part_off, row_ids, the host-side tile bound max_nrb and
-// pad_prefix), uploaded on the legacy stream; `rows_tile` is the scan's tile height
-static void open_ivf_partitions(lgpu_index *ix, int device, uint32_t nlist, uint64_t nrows,
-                                const uint64_t *part_offsets, const uint64_t *row_ids, uint32_t rows_tile)
-{
-    ix->device = device;
-    cudaDeviceProp prop;
-    LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-    ix->num_sms = prop.multiProcessorCount;
-    ix->nlist = nlist; ix->nrows = nrows;
-    std::vector<uint32_t> part_n(nlist), part_npad(nlist);
-    std::vector<uint64_t> pads(nlist);
-    for (uint32_t p = 0; p < nlist; p++) {
-        const uint32_t n = (uint32_t)(part_offsets[p + 1] - part_offsets[p]);
-        part_n[p] = n; part_npad[p] = (n + 31u) & ~31u;
-        pads[p] = (n + 3ull) & ~3ull;
-        ix->max_nrb = std::max(ix->max_nrb, scan_nrb(n, rows_tile));
-    }
-    ix->h_part_n = part_n;
-    std::sort(pads.begin(), pads.end(), std::greater<uint64_t>());
-    ix->pad_prefix.assign(nlist + 1, 0);
-    for (uint32_t p = 0; p < nlist; p++) ix->pad_prefix[p + 1] = ix->pad_prefix[p] + pads[p];
-
-    cudaStream_t st = nullptr;
-    auto up = [&](DevBuf &b, const void *src, size_t bytes) {
-        b.ensure(std::max<size_t>(bytes, 16));
-        if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, st));
-        ix->device_bytes += b.bytes;
-    };
-    up(ix->part_n, part_n.data(), (size_t)nlist * 4);
-    up(ix->part_npad, part_npad.data(), (size_t)nlist * 4);
-    up(ix->part_off, part_offsets, (size_t)(nlist + 1) * 8);
-    up(ix->row_ids, row_ids, (size_t)nrows * 8);
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
@@ -2090,15 +2087,16 @@ static void upload_rq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBu
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
-// 4-bit IVF_PQ codes: per partition [m/2][npad] bytes (zero padding rows) at code_base[p] = m/2 x the npad of the
-// partitions before it.  Returns the total bytes.
-static uint64_t pq4_code_base(const uint64_t *part_offsets, uint32_t nlist, uint32_t m, std::vector<uint64_t> &code_base)
+// The padded PQ layouts: partition p's codes at code_base[p] = row_bytes x the 32-row padded heights of the partitions
+// before it ((nch + 1) x 8 bytes per row for the 8-bit streams, m/2 for 4-bit codes).  Returns the total bytes.
+static uint64_t padded_code_base(const uint64_t *part_offsets, uint32_t nlist, uint64_t row_bytes,
+                                 std::vector<uint64_t> &code_base)
 {
     code_base.resize(nlist);
     uint64_t cb = 0;
     for (uint32_t p = 0; p < nlist; p++) {
         code_base[p] = cb;
-        cb += (uint64_t)(m / 2) * (((part_offsets[p + 1] - part_offsets[p]) + 31u) & ~31ull);
+        cb += row_bytes * (((part_offsets[p + 1] - part_offsets[p]) + 31u) & ~31ull);
         LGPU_REQUIRE((cb >> 3) < (1ull << 32), "index too large for one GPU shard (re-laid-out codes above 32 GiB)");
     }
     return cb;
@@ -2124,6 +2122,79 @@ static void upload_pq4_codes(const uint8_t *codes, int layout, uint64_t nrows, u
     LGPU_CUDA(cudaStreamSynchronize(st));
 }
 
+// after the desc's checks: the device, then a new index of `kind`
+template <class H = lgpu_index> static H *new_ivf(int device, IvfKind kind)
+{
+    require_device(device);
+    H *ix = new H();
+    ix->kind = kind;
+    return ix;
+}
+
+// lgpu_index_open with nbits = 8 (the desc's common fields are checked): the IVF arrays, the codebook tiled for the
+// scans, the codes re-laid out as skewed streams (retile.cu) and the filter scan's tables (tables.cu)
+static void open_pq8(const lgpu_index_desc *d, lgpu_index *&ix)
+{
+    const uint32_t nlist = d->nlist, nch = (d->m + 7) / 8;
+    std::vector<uint64_t> code_base;
+    const uint64_t cb = padded_code_base(d->part_offsets, nlist, (uint64_t)(nch + 1) * 8, code_base);
+    ix = new_ivf(d->device, IvfKind::pq8);
+    ix->m = d->m; ix->dsub = d->dim / d->m; ix->nch = nch;
+    open_ivf_common(ix, d, SCAN_ROWS_TILE_MID, code_base);
+    cudaStream_t st = nullptr;
+    {   // codebook -> [nch][256][8][dsub]
+        DevBuf tmp;
+        upload(tmp, d->codebook, (size_t)d->m * 256 * ix->dsub * 4);
+        ix->cb_tiled.ensure((size_t)ix->nch * 256 * 8 * ix->dsub * 4);
+        launch_retile_codebook(tmp.as<float>(), d->m, ix->dsub, ix->nch, ix->cb_tiled.as<float>(), st);
+        LGPU_CUDA(cudaStreamSynchronize(st));
+    }
+    {   // codes -> skewed streams
+        ix->codes.ensure(std::max<uint64_t>(cb, 16));
+        LGPU_CUDA(cudaMemsetAsync(ix->codes.p, 0, ix->codes.bytes, st));
+        DevBuf tmp;
+        if (d->nrows) {
+            upload(tmp, d->codes, (size_t)d->nrows * d->m);
+            launch_retile_codes(tmp.as<unsigned char>(), d->codes_layout, ix->part_off.as<uint64_t>(), nlist, d->nrows,
+                                d->m, ix->nch, ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(),
+                                ix->codes.as<unsigned char>(), st);
+        }
+        LGPU_CUDA(cudaStreamSynchronize(st));
+    }
+    {   // |b|^2 of the tiled codebook entries and CB2 = sum_i max_c |b|^2 (filter scan, tables.cu)
+        ix->cb_n2.ensure((size_t)ix->nch * 256 * 8 * 4);
+        launch_cb_norms(ix->cb_tiled.as<float>(), ix->nch, ix->dsub, ix->cb_n2.as<float>(), st);
+        double cb2 = 0.0;
+        for (uint32_t i = 0; i < d->m; i++) {
+            double mx = 0.0;
+            for (uint32_t c = 0; c < 256; c++) {
+                double n2 = 0.0;
+                const float *e = d->codebook + ((size_t)i * 256 + c) * ix->dsub;
+                for (uint32_t t = 0; t < ix->dsub; t++) n2 += (double)e[t] * e[t];
+                mx = std::max(mx, n2);
+            }
+            cb2 += mx;
+        }
+        ix->cb2 = (float)(cb2 * 1.000001);
+    }
+    float rmax = 0.f;
+    if (d->metric != LGPU_DOT) {   // per-row constants of the filter scan (tables.cu)
+        ix->row_R.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));
+        ix->rmax_bits.ensure(16);
+        launch_row_const(ix->codes.as<unsigned char>(), ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(),
+                         ix->part_off.as<uint64_t>(), nlist, d->nrows, ix->centroids.as<float>(),
+                         ix->cb_tiled.as<float>(), d->dim, d->m, ix->dsub, ix->row_R.as<float>(),
+                         ix->rmax_bits.as<int>(), st);
+        LGPU_CUDA(cudaStreamSynchronize(st));
+        int bits = 0;
+        LGPU_CUDA(cudaMemcpy(&bits, ix->rmax_bits.p, 4, cudaMemcpyDeviceToHost));
+        rmax = __builtin_bit_cast(float, bits);
+    }
+    // the filter scan's error band (kernels.cuh scan_band) is finite only with a finite CB2 and max |R|: a NaN / inf
+    // centroid or codeword leaves the index on the exact scan
+    ix->has_tables = std::isfinite(ix->cb2) && std::isfinite(rmax);
+}
+
 // lgpu_index_open with nbits = 4 (the desc's common fields are checked): the IVF arrays, the codebook and the codes
 // re-laid out for pq4_tables / pq4_scan.  No filter tables: the scan is exact.
 static void open_pq4(const lgpu_index_desc *d, lgpu_index *&ix)
@@ -2131,15 +2202,10 @@ static void open_pq4(const lgpu_index_desc *d, lgpu_index *&ix)
     LGPU_REQUIRE(d->m % 2 == 0, "num_sub_vectors must be even for 4-bit PQ codes");
     LGPU_REQUIRE(d->m <= LGPU_PQ4_MAX_M, "4-bit PQ codes support num_sub_vectors up to 256");
     std::vector<uint64_t> code_base;
-    const uint64_t total = pq4_code_base(d->part_offsets, d->nlist, d->m, code_base);
-    require_device(d->device);
-    ix = new lgpu_index();
-    ix->is_pq4 = true;
+    const uint64_t total = padded_code_base(d->part_offsets, d->nlist, d->m / 2, code_base);
+    ix = new_ivf(d->device, IvfKind::pq4);
     ix->m = d->m; ix->dsub = d->dim / d->m; ix->nch = (d->m + 7) / 8;
-    open_ivf_common(ix, d->device, d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
-                    d->vectors, PQ4_ROWS_TILE);
-    ix->code_base.ensure((size_t)d->nlist * 8);
-    LGPU_CUDA(cudaMemcpy(ix->code_base.p, code_base.data(), (size_t)d->nlist * 8, cudaMemcpyHostToDevice));
+    open_ivf_common(ix, d, PQ4_ROWS_TILE, code_base);
     // codebook [m][16][dsub] -> [m][dsub][16], the layout the table kernel reads
     const uint32_t m = d->m, dsub = ix->dsub;
     std::vector<float> cbt((size_t)m * 16 * dsub);
@@ -2147,11 +2213,60 @@ static void open_pq4(const lgpu_index_desc *d, lgpu_index *&ix)
         for (uint32_t j = 0; j < 16; j++)
             for (uint32_t t = 0; t < dsub; t++)
                 cbt[((size_t)i * dsub + t) * 16 + j] = d->codebook[((size_t)i * 16 + j) * dsub + t];
-    ix->pq4_cb.ensure(cbt.size() * 4);
-    LGPU_CUDA(cudaMemcpy(ix->pq4_cb.p, cbt.data(), cbt.size() * 4, cudaMemcpyHostToDevice));
+    upload(ix->pq4_cb, cbt.data(), cbt.size() * 4);
     upload_pq4_codes(d->codes, d->codes_layout, d->nrows, d->m, d->nlist, ix->part_off.as<uint64_t>(),
                      ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(), total, ix->codes);
-    ix->device_bytes += ix->code_base.bytes + ix->pq4_cb.bytes + ix->codes.bytes;
+}
+
+// the HBM an index holds: every buffer its open allocated
+static uint64_t index_device_bytes(const lgpu_index *ix)
+{
+    uint64_t n = 0;
+    for (const DevBuf *b : {&ix->centroids, &ix->cb_tiled, &ix->codes, &ix->code_base, &ix->part_n, &ix->part_npad,
+                            &ix->part_off, &ix->row_ids, &ix->vectors, &ix->row_R, &ix->rmax_bits, &ix->cb_n2,
+                            &ix->cent_b, &ix->cent_n2, &ix->cent_sb, &ix->cent_sn2, &ix->sq_xx, &ix->rq_rot, &ix->rq_rc,
+                            &ix->rq_add, &ix->rq_scale, &ix->rq_popc, &ix->pq4_cb, &ix->cent_pop, &ix->row_pop})
+        n += b->bytes;
+    return n;
+}
+
+// The sequence of every IVF open: `open(ix)` checks the desc, then creates the index (new_ivf) and fills it; the index
+// is then registered and returned, or deleted if any step failed.
+template <class H, class Open> static int open_ivf(H **out, Open &&open)
+{
+    H *ix = nullptr;
+    const int rc = guarded([&] {
+        LGPU_REQUIRE(out != nullptr, "null argument");
+        open(ix);
+        LGPU_CUDA(cudaStreamSynchronize(nullptr));
+        ix->device_bytes = index_device_bytes(ix);
+        register_handle(ix);
+        *out = ix;
+    });
+    if (rc != LGPU_OK) delete ix;
+    return rc;
+}
+
+// The tile queue of a kernel-alone debug entry: B queries, query b alone in probe slot b of one partition of N rows
+// (at row 0, padded to 32 rows), cut into the regroup's row blocks for `rows_tile`; query b's output at b * stride.
+// The descriptors go to `tiles`, the {total, 0} counter to `ctr`.  Returns the tile count.
+static uint32_t debug_tiles(uint32_t B, uint32_t N, uint32_t rows_tile, uint64_t stride, DevBuf &tiles, DevBuf &ctr)
+{
+    const uint32_t nrb = scan_nrb(N, rows_tile), rbr = scan_rb_rows(N, nrb);
+    std::vector<TileDesc> h;
+    for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
+        for (uint32_t rb = 0; rb < nrb; rb++) {
+            TileDesc t{};
+            t.row0 = rb * rbr; t.nrows = std::min(rbr, N - t.row0);
+            t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = N; t.npad = (N + 31u) & ~31u;
+            for (uint32_t g = 0; g < t.ng; g++) { t.q[g] = t.slot[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * stride); }
+            h.push_back(t);
+        }
+    const uint32_t total = (uint32_t)h.size(), counter[2] = {total, 0u};
+    upload(tiles, h.data(), h.size() * sizeof(TileDesc));
+    upload(ctr, counter, 8);
+    LGPU_CUDA(cudaStreamSynchronize(nullptr));
+    return total;
 }
 
 }  // namespace
@@ -2173,9 +2288,8 @@ int lgpu_device_count(int *count)
 
 int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
 {
-    lgpu_index *ix = nullptr;
-    int rc = guarded([&] {
-        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+    return open_ivf(out, [&](lgpu_index *&ix) {
+        LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->dim > 0 && d->nlist > 0 && d->m > 0, "dim, nlist and m must be positive");
         LGPU_REQUIRE(d->dim % d->m == 0, "num_sub_vectors must divide the vector dimension");
@@ -2186,131 +2300,27 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
                      "unsupported PQ sub-vector length (dim/num_sub_vectors must be 1,2,4,8,16 or 32)");
         LGPU_REQUIRE(d->codebook, "null index array");
         check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
-        if (d->nbits == 4) {
-            open_pq4(d, ix);
-            register_handle(ix);
-            *out = ix;
-            return;
-        }
-        const uint32_t nlist = d->nlist, nch = (d->m + 7) / 8;
-        std::vector<uint64_t> code_base(nlist);
-        uint64_t cb = 0;
-        for (uint32_t p = 0; p < nlist; p++) {
-            code_base[p] = cb;
-            cb += (uint64_t)(nch + 1) * (((d->part_offsets[p + 1] - d->part_offsets[p]) + 31u) & ~31ull) * 8;
-            LGPU_REQUIRE((cb >> 3) < (1ull << 32), "index too large for one GPU shard (re-laid-out codes above 32 GiB)");
-        }
-        require_device(d->device);
-        ix = new lgpu_index();
-        ix->m = d->m; ix->dsub = d->dim / d->m; ix->nch = nch;
-        open_ivf_common(ix, d->device, d->dim, nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
-                        d->vectors, SCAN_ROWS_TILE_MID);
-        cudaStream_t st = nullptr;
-        auto up = [&](DevBuf &b, const void *src, size_t bytes) {
-            b.ensure(std::max<size_t>(bytes, 16));
-            if (bytes) LGPU_CUDA(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, st));
-            ix->device_bytes += b.bytes;
-        };
-        up(ix->code_base, code_base.data(), (size_t)nlist * 8);
-        // codebook -> [nch][256][8][dsub]
-        {
-            DevBuf tmp;
-            size_t bytes = (size_t)d->m * 256 * ix->dsub * 4;
-            tmp.ensure(bytes);
-            LGPU_CUDA(cudaMemcpyAsync(tmp.p, d->codebook, bytes, cudaMemcpyHostToDevice, st));
-            ix->cb_tiled.ensure((size_t)ix->nch * 256 * 8 * ix->dsub * 4);
-            ix->device_bytes += ix->cb_tiled.bytes;
-            launch_retile_codebook(tmp.as<float>(), d->m, ix->dsub, ix->nch, ix->cb_tiled.as<float>(), st);
-            LGPU_CUDA(cudaStreamSynchronize(st));
-        }
-        // codes -> skewed streams
-        {
-            ix->codes.ensure(std::max<uint64_t>(cb, 16));
-            ix->device_bytes += ix->codes.bytes;
-            LGPU_CUDA(cudaMemsetAsync(ix->codes.p, 0, ix->codes.bytes, st));
-            DevBuf tmp;
-            size_t bytes = (size_t)d->nrows * d->m;
-            if (bytes) {
-                tmp.ensure(bytes);
-                LGPU_CUDA(cudaMemcpyAsync(tmp.p, d->codes, bytes, cudaMemcpyHostToDevice, st));
-                launch_retile_codes(tmp.as<unsigned char>(), d->codes_layout, ix->part_off.as<uint64_t>(), nlist,
-                                    d->nrows, d->m, ix->nch, ix->code_base.as<uint64_t>(),
-                                    ix->part_npad.as<uint32_t>(), ix->codes.as<unsigned char>(), st);
-            }
-            LGPU_CUDA(cudaStreamSynchronize(st));
-        }
-        {   // |b|^2 of the tiled codebook entries and CB2 = sum_i max_c |b|^2 (filter scan, tables.cu)
-            const size_t ne = (size_t)ix->nch * 256 * 8;
-            ix->cb_n2.ensure(ne * 4);
-            ix->device_bytes += ix->cb_n2.bytes;
-            launch_cb_norms(ix->cb_tiled.as<float>(), ix->nch, ix->dsub, ix->cb_n2.as<float>(), st);
-            double cb2 = 0.0;
-            for (uint32_t i = 0; i < d->m; i++) {
-                double mx = 0.0;
-                for (uint32_t c = 0; c < 256; c++) {
-                    double n2 = 0.0;
-                    const float *e = d->codebook + ((size_t)i * 256 + c) * ix->dsub;
-                    for (uint32_t t = 0; t < ix->dsub; t++) n2 += (double)e[t] * e[t];
-                    mx = std::max(mx, n2);
-                }
-                cb2 += mx;
-            }
-            ix->cb2 = (float)(cb2 * 1.000001);
-        }
-        float rmax = 0.f;
-        if (d->metric != LGPU_DOT) {   // per-row constants of the filter scan (tables.cu)
-            ix->row_R.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));
-            ix->rmax_bits.ensure(16);
-            ix->device_bytes += ix->row_R.bytes;
-            launch_row_const(ix->codes.as<unsigned char>(), ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(),
-                             ix->part_off.as<uint64_t>(), nlist, d->nrows, ix->centroids.as<float>(),
-                             ix->cb_tiled.as<float>(), d->dim, d->m, ix->dsub, ix->row_R.as<float>(),
-                             ix->rmax_bits.as<int>(), st);
-            LGPU_CUDA(cudaStreamSynchronize(st));
-            int bits = 0;
-            LGPU_CUDA(cudaMemcpy(&bits, ix->rmax_bits.p, 4, cudaMemcpyDeviceToHost));
-            rmax = __builtin_bit_cast(float, bits);
-        }
-        // the filter scan's error band (kernels.cuh scan_band) is finite only with a finite CB2 and max |R|: a NaN / inf
-        // centroid or codeword leaves the index on the exact scan
-        ix->has_tables = std::isfinite(ix->cb2) && std::isfinite(rmax);
-        register_handle(ix);
-        *out = ix;
+        if (d->nbits == 4) open_pq4(d, ix);
+        else open_pq8(d, ix);
     });
-    if (rc != LGPU_OK && ix) delete ix;
-    return rc;
 }
 
 int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
 {
-    lgpu_index *ix = nullptr;
-    int rc = guarded([&] {
-        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+    return open_ivf(out, [&](lgpu_index *&ix) {
+        LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->metric != LGPU_DOT, "IVF_SQ supports the l2 and cosine distance types, not dot");
         LGPU_REQUIRE(d->dim <= LGPU_SQ_MAX_DIM, "IVF_SQ supports dimensions up to 65536");
         LGPU_REQUIRE(std::isfinite(d->lo) && std::isfinite(d->hi) && d->lo <= d->hi,
                      "IVF_SQ bounds must be finite with lo <= hi");
         check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
-        require_device(d->device);
-        ix = new lgpu_index();
-        ix->is_sq = true;
+        ix = new_ivf(d->device, IvfKind::sq);
         ix->dim_pad = sq_dim_pad(d->dim);
         ix->sq_lo = d->lo; ix->sq_hi = d->hi;
-        open_ivf_common(ix, d->device, d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
-                        d->vectors, SQ_ROWS_TILE);
-        // byte offset of each partition's codes (the tile descriptors carry it; the SQ scan addresses rows by part_off)
-        std::vector<uint64_t> code_base(d->nlist);
-        for (uint32_t p = 0; p < d->nlist; p++) code_base[p] = d->part_offsets[p] * ix->dim_pad;
-        ix->code_base.ensure((size_t)d->nlist * 8);
-        LGPU_CUDA(cudaMemcpy(ix->code_base.p, code_base.data(), (size_t)d->nlist * 8, cudaMemcpyHostToDevice));
+        open_ivf_common(ix, d, SQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
         upload_sq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->sq_xx);
-        ix->device_bytes += ix->code_base.bytes + ix->codes.bytes + ix->sq_xx.bytes;
-        register_handle(ix);
-        *out = ix;
     });
-    if (rc != LGPU_OK && ix) delete ix;
-    return rc;
 }
 
 int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x_codes, uint64_t N, uint32_t dim,
@@ -2327,23 +2337,8 @@ int lgpu_debug_sq_distances(const uint8_t *q_codes, uint32_t B, const uint8_t *x
         DevBuf X, xx, Q, qq, D, tiles, ctr;
         upload_sq_rows(x_codes, N, dim, X, xx);
         upload_sq_rows(q_codes, B, dim, Q, qq);
-        // one partition of N rows that every query probes: tiles of SQ_ROWS_TILE rows x 8 queries, query b's
-        // distances at out + b N
-        std::vector<TileDesc> h;
-        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
-            for (uint64_t r0 = 0; r0 < N; r0 += SQ_ROWS_TILE) {
-                TileDesc t{};
-                t.row0 = (uint32_t)r0; t.nrows = (uint32_t)std::min<uint64_t>(SQ_ROWS_TILE, N - r0);
-                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N;
-                for (uint32_t g = 0; g < t.ng; g++) { t.q[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * N); }
-                h.push_back(t);
-            }
-        const uint32_t total = (uint32_t)h.size(), zero[2] = {total, 0u};
-        tiles.ensure(h.size() * sizeof(TileDesc));
-        ctr.ensure(8);
+        debug_tiles(B, (uint32_t)N, SQ_ROWS_TILE, N, tiles, ctr);
         D.ensure((size_t)B * N * 4);
-        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(ctr.p, zero, 8, cudaMemcpyHostToDevice));
         SqScanArgs a{};
         a.codes = X.as<uint8_t>(); a.xx = xx.as<uint32_t>(); a.qcodes = Q.as<uint8_t>(); a.qq = qq.as<uint32_t>();
         a.dim_pad = sq_dim_pad(dim); a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1;
@@ -2364,37 +2359,20 @@ int lgpu_debug_pq4_sums(const uint8_t *tables, uint32_t B, const uint8_t *codes,
         require_device(device);
         cudaDeviceProp prop;
         LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-        // one partition of N rows that every query probes as its own slot: tiles of PQ4_ROWS_TILE rows x 8 slots,
-        // query b's sums at b * ld (segments padded to 4, as in a search)
+        // the one partition's codes laid out as in an index; query b's sums at b * ld (segments padded to 4, as in a
+        // search)
         const uint64_t off[2] = {0, N}, ld = (N + 3) & ~3ull;
         const uint32_t npad = (uint32_t)((N + 31) & ~31ull);
         std::vector<uint64_t> code_base;
-        const uint64_t total_bytes = pq4_code_base(off, 1, m, code_base);
+        const uint64_t total_bytes = padded_code_base(off, 1, m / 2, code_base);
         DevBuf d_off, d_cb, d_npad, X, tab, sl, D, tiles, ctr;
-        d_off.ensure(16); d_cb.ensure(8); d_npad.ensure(4);
-        LGPU_CUDA(cudaMemcpy(d_off.p, off, 16, cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(d_cb.p, code_base.data(), 8, cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(d_npad.p, &npad, 4, cudaMemcpyHostToDevice));
+        upload(d_off, off, 16); upload(d_cb, code_base.data(), 8); upload(d_npad, &npad, 4);
         upload_pq4_codes(codes, LGPU_CODES_ROW_MAJOR, N, m, 1, d_off.as<uint64_t>(), d_cb.as<uint64_t>(),
                          d_npad.as<uint32_t>(), total_bytes, X);
-        tab.ensure((size_t)B * m * 16); sl.ensure((size_t)B * sizeof(Pq4Slot));
-        LGPU_CUDA(cudaMemcpy(tab.p, tables, (size_t)B * m * 16, cudaMemcpyHostToDevice));
-        std::vector<TileDesc> h;
-        const uint32_t nrb = scan_nrb((uint32_t)N, PQ4_ROWS_TILE), rbr = scan_rb_rows((uint32_t)N, nrb);
-        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
-            for (uint32_t rb = 0; rb < nrb; rb++) {
-                TileDesc t{};
-                t.row0 = rb * rbr; t.nrows = std::min<uint32_t>(rbr, (uint32_t)N - t.row0);
-                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N; t.npad = npad;
-                for (uint32_t g = 0; g < t.ng; g++) { t.slot[g] = q0 + g; t.q[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * ld); }
-                h.push_back(t);
-            }
-        const uint32_t total = (uint32_t)h.size(), zero[2] = {total, 0u};
-        tiles.ensure(h.size() * sizeof(TileDesc));
-        ctr.ensure(8);
+        upload(tab, tables, (size_t)B * m * 16);
+        sl.ensure((size_t)B * sizeof(Pq4Slot));
+        debug_tiles(B, (uint32_t)N, PQ4_ROWS_TILE, ld, tiles, ctr);
         D.ensure((size_t)B * ld * 4);
-        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(ctr.p, zero, 8, cudaMemcpyHostToDevice));
         Pq4ScanArgs a{};
         a.codes = X.as<uint32_t>(); a.tables = tab.as<uint8_t>(); a.slots = sl.as<Pq4Slot>(); a.m = m; a.metric = LGPU_L2;
         a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1; a.tile_desc = tiles.as<TileDesc>();
@@ -2406,9 +2384,8 @@ int lgpu_debug_pq4_sums(const uint8_t *tables, uint32_t B, const uint8_t *codes,
 
 int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
 {
-    lgpu_index *ix = nullptr;
-    int rc = guarded([&] {
-        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+    return open_ivf(out, [&](lgpu_index *&ix) {
+        LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->metric != LGPU_DOT, "IVF_RQ supports the l2 and cosine distance types, not dot");
         LGPU_REQUIRE(d->num_bits == 1, "IVF_RQ supports num_bits = 1 only");
@@ -2416,37 +2393,18 @@ int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
         LGPU_REQUIRE(d->rotation != nullptr, "null index array");
         LGPU_REQUIRE(d->nrows == 0 || (d->add_factors && d->scale_factors), "null index array");
         check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
-        require_device(d->device);
-        ix = new lgpu_index();
-        ix->is_rq = true;
+        ix = new_ivf(d->device, IvfKind::rq);
         ix->rq_wpr = rq_wpr(d->dim);
-        open_ivf_common(ix, d->device, d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->row_ids,
-                        d->vectors, RQ_ROWS_TILE);
-        // byte offset of each partition's codes (the tile descriptors carry it; the RQ scan addresses rows by part_off)
-        std::vector<uint64_t> code_base(d->nlist);
-        for (uint32_t p = 0; p < d->nlist; p++) code_base[p] = d->part_offsets[p] * ix->rq_wpr * 4;
-        ix->code_base.ensure((size_t)d->nlist * 8);
-        LGPU_CUDA(cudaMemcpy(ix->code_base.p, code_base.data(), (size_t)d->nlist * 8, cudaMemcpyHostToDevice));
+        open_ivf_common(ix, d, RQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
         upload_rq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->rq_popc);
-        const size_t rows = std::max<size_t>((size_t)d->nrows * 4, 16), rot = (size_t)d->dim * d->dim * 4;
-        ix->rq_add.ensure(rows); ix->rq_scale.ensure(rows); ix->rq_rot.ensure(rot);
+        upload(ix->rq_add, d->add_factors, (size_t)d->nrows * 4);
+        upload(ix->rq_scale, d->scale_factors, (size_t)d->nrows * 4);
+        upload(ix->rq_rot, d->rotation, (size_t)d->dim * d->dim * 4);
         ix->rq_rc.ensure((size_t)d->nlist * d->dim * 4);
-        if (d->nrows) {
-            LGPU_CUDA(cudaMemcpy(ix->rq_add.p, d->add_factors, (size_t)d->nrows * 4, cudaMemcpyHostToDevice));
-            LGPU_CUDA(cudaMemcpy(ix->rq_scale.p, d->scale_factors, (size_t)d->nrows * 4, cudaMemcpyHostToDevice));
-        }
-        LGPU_CUDA(cudaMemcpy(ix->rq_rot.p, d->rotation, rot, cudaMemcpyHostToDevice));
         // rc_p = P c_p, once: each probe slot's residual is then one subtraction per dimension
         launch_rq_rotate(ix->rq_rot.as<float>(), ix->centroids.as<float>(), d->nlist, d->dim, ix->rq_rc.as<float>(),
                          nullptr);
-        LGPU_CUDA(cudaStreamSynchronize(nullptr));
-        ix->device_bytes += ix->code_base.bytes + ix->codes.bytes + ix->rq_popc.bytes + ix->rq_add.bytes +
-                            ix->rq_scale.bytes + ix->rq_rot.bytes + ix->rq_rc.bytes;
-        register_handle(ix);
-        *out = ix;
     });
-    if (rc != LGPU_OK && ix) delete ix;
-    return rc;
 }
 
 int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes, const float *add_factors,
@@ -2466,45 +2424,27 @@ int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes
         const uint32_t wpr = rq_wpr(dim);
         DevBuf X, popc, add, scale, Q, zero, probes, planes, slots, D, tiles, ctr;
         upload_rq_rows(codes, N, dim, X, popc);
-        add.ensure((size_t)N * 4); scale.ensure((size_t)N * 4);
-        Q.ensure((size_t)B * dim * 4); zero.ensure((size_t)dim * 4); probes.ensure((size_t)B * 8);
+        upload(add, add_factors, (size_t)N * 4); upload(scale, scale_factors, (size_t)N * 4);
+        upload(Q, q_res, (size_t)B * dim * 4);
+        zero.ensure((size_t)dim * 4); probes.ensure((size_t)B * 8);
         planes.ensure((size_t)B * 4 * wpr * 4); slots.ensure((size_t)B * sizeof(RqSlot));
-        LGPU_CUDA(cudaMemcpy(add.p, add_factors, (size_t)N * 4, cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(scale.p, scale_factors, (size_t)N * 4, cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(Q.p, q_res, (size_t)B * dim * 4, cudaMemcpyHostToDevice));
         LGPU_CUDA(cudaMemset(zero.p, 0, (size_t)dim * 4));
         LGPU_CUDA(cudaMemset(probes.p, 0, (size_t)B * 8));
         // query b is one probe slot of partition 0 whose rotated centroid is 0: q' = the given residual
         launch_rq_planes(Q.as<float>(), zero.as<float>(), probes.as<uint64_t>(), B, 1, 1, dim, wpr,
                          planes.as<uint32_t>(), slots.as<RqSlot>(), nullptr);
-        // one partition of N rows that every slot probes: tiles of RQ_ROWS_TILE rows x 8 slots, slot b's row r at
-        // out + b N + r
-        std::vector<TileDesc> h;
-        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
-            for (uint64_t r0 = 0; r0 < N; r0 += RQ_ROWS_TILE) {
-                TileDesc t{};
-                t.row0 = (uint32_t)r0; t.nrows = (uint32_t)std::min<uint64_t>(RQ_ROWS_TILE, N - r0);
-                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N;
-                for (uint32_t g = 0; g < t.ng; g++) {
-                    t.q[g] = q0 + g; t.slot[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * N);
-                }
-                h.push_back(t);
-            }
-        tiles.ensure(h.size() * sizeof(TileDesc));
-        ctr.ensure(8);
+        const uint32_t total = debug_tiles(B, (uint32_t)N, RQ_ROWS_TILE, N, tiles, ctr), counter[2] = {total, 0u};
         D.ensure((size_t)B * N * 4);
-        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
         RqScanArgs a{};
         a.codes = X.as<uint32_t>(); a.add = add.as<float>(); a.scale = scale.as<float>(); a.popc = popc.as<uint32_t>();
         a.planes = planes.as<uint32_t>(); a.slots = slots.as<RqSlot>(); a.dim = dim; a.wpr = wpr;
         a.cosine = metric == LGPU_COSINE;
         a.total_tiles = ctr.as<uint32_t>(); a.tile_counter = ctr.as<uint32_t>() + 1;
         a.tile_desc = tiles.as<TileDesc>(); a.dist_out = D.as<float>();
-        const uint32_t total = (uint32_t)h.size(), zero2[2] = {total, 0u};
         for (int mode = 0; mode < 2; mode++) {
             void *dst = mode ? (void *)out_ip : (void *)out_est;
             if (!dst) continue;
-            LGPU_CUDA(cudaMemcpy(ctr.p, zero2, 8, cudaMemcpyHostToDevice));
+            LGPU_CUDA(cudaMemcpy(ctr.p, counter, 8, cudaMemcpyHostToDevice));
             a.out_ip = mode;
             launch_rq_scan(a, 2 * prop.multiProcessorCount, nullptr);
             LGPU_CUDA(cudaMemcpy(dst, D.p, (size_t)B * N * 4, cudaMemcpyDeviceToHost));
@@ -2518,7 +2458,7 @@ int lgpu_index_device_bytes(const lgpu_index *ixh, uint64_t *bytes)
 {
     return guarded([&] {
         LGPU_REQUIRE(bytes, "null argument");
-        HandleRef<lgpu_index> ix(const_cast<lgpu_index *>(ixh), "index");
+        HandleRef<lgpu_index> ix(const_cast<lgpu_index *>(ixh));
         *bytes = ix->device_bytes;
     });
 }
@@ -2553,7 +2493,7 @@ int lgpu_debug_sub_batch_size(lgpu_index *ixh, uint32_t B, uint32_t nprobes, uin
 {
     return guarded([&] {
         LGPU_REQUIRE(out && B > 0 && nprobes > 0, "bad argument");
-        HandleRef<lgpu_index> ix(ixh, "index");
+        HandleRef<lgpu_index> ix(ixh);
         *out = ivf_sub_batch_size(ix.h, B, nprobes);
     });
 }
@@ -2561,17 +2501,19 @@ int lgpu_debug_sub_batch_size(lgpu_index *ixh, uint32_t B, uint32_t nprobes, uin
 static void check_ivf_call(lgpu_index *ix, const void *q, uint32_t B, const lgpu_search_params *p,
                            const void *a, const void *b, const void *c)
 {
-    check_call(p, B, q, a, b, c);
+    const bool refine = ix->kind != IvfKind::ham;     // Hamming distances are exact: refine_factor is ignored
+    check_call(p, B, q, a, b, c, refine);
     LGPU_REQUIRE(p->nprobes >= 1, "minimum_nprobes must be greater than 0");
-    LGPU_REQUIRE(p->nprobes <= SELECT_KMAX || p->nprobes >= ix->nlist, "nprobes above 2048 is not supported");
-    LGPU_REQUIRE(p->refine_factor == 0 || ix->has_vectors,
+    LGPU_REQUIRE(p->nprobes <= SELECT_KMAX || p->nprobes >= ix->nlist,
+                 "nprobes above 2048 is not supported unless it covers every partition");
+    LGPU_REQUIRE(!refine || p->refine_factor == 0 || ix->has_vectors,
                  "refine_factor needs the raw vectors: open the index with desc.vectors");
 }
 
 static int ivf_call(lgpu_index *ixh, const Route &r, const float *q, uint32_t B, const lgpu_search_params *p,
                     uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    return search_call(ixh, "index", r, q, B, p, ids, dist, cnt,
+    return search_call(ixh, r, q, B, p, ids, dist, cnt,
                        [&](lgpu_index *ix) { check_ivf_call(ix, q, B, p, ids, dist, cnt); return (size_t)B * ix->dim; },
                        ivf_search_device);
 }
@@ -2598,7 +2540,7 @@ int lgpu_search_coalesced(lgpu_index *ixh, const float *query, const lgpu_search
     std::vector<PendingQuery *> batch;
     lgpu_search_params p{};
     int rc = guarded([&] {
-        HandleRef<lgpu_index> ix(ixh, "index");
+        HandleRef<lgpu_index> ix(ixh);
         check_ivf_call(ix.h, query, 1, params, out_ids, out_dist, out_count);
         p = *params;
         Coalescer &co = ix->coalescer;
@@ -2662,7 +2604,7 @@ struct lgpu_ticket {
     Deadline deadline;
     cudaEvent_t done = nullptr;
     lgpu_ticket(lgpu_index *h, uint32_t timeout_ms)
-        : ix(h, "index"), lease(ix->pool, nullptr, false), deadline(timeout_ms) {}
+        : ix(h), lease(ix->pool, nullptr, false), deadline(timeout_ms) {}
     ~lgpu_ticket() { if (done) cudaEventDestroy(done); }
 };
 
@@ -2674,7 +2616,7 @@ int lgpu_search_async(lgpu_index *ixh, const float *queries, uint32_t B, const l
         LGPU_REQUIRE(ticket != nullptr, "ticket is null");
         LGPU_REQUIRE(params != nullptr, "search params are null");
         {   // validate before taking a workspace
-            HandleRef<lgpu_index> ix(ixh, "index");
+            HandleRef<lgpu_index> ix(ixh);
             check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
             require_device(ix->device);
         }
@@ -2778,7 +2720,7 @@ void lgpu_flat_close(lgpu_flat *fl) { close_handle(fl); }
 static int flat_call(lgpu_flat *flh, int metric, const Route &r, const float *q, uint32_t B,
                      const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    return search_call(flh, "flat", r, q, B, p, ids, dist, cnt,
+    return search_call(flh, r, q, B, p, ids, dist, cnt,
                        [&](lgpu_flat *fl) {
                            LGPU_REQUIRE(metric == LGPU_L2 || metric == LGPU_COSINE || metric == LGPU_DOT,
                                         "unknown distance type");
@@ -2855,7 +2797,7 @@ void lgpu_binary_close(lgpu_binary *bx) { close_handle(bx); }
 static int binary_call(lgpu_binary *bxh, const Route &r, const uint8_t *q, uint32_t B, const lgpu_search_params *p,
                        uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    return search_call(bxh, "binary", r, q, B, p, ids, dist, cnt,
+    return search_call(bxh, r, q, B, p, ids, dist, cnt,
                        [&](lgpu_binary *bx) { check_call(p, B, q, ids, dist, cnt); return (size_t)B * bx->nbytes; },
                        binary_search_device);
 }
@@ -2881,18 +2823,16 @@ int lgpu_binary_search_device(lgpu_binary *bxh, const uint8_t *d_queries, uint32
 
 int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
 {
-    lgpu_ivf_binary *ix = nullptr;
-    int rc = guarded([&] {
-        LGPU_REQUIRE(d != nullptr && out != nullptr, "null argument");
+    return open_ivf(out, [&](lgpu_ivf_binary *&ix) {
+        LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->nbytes > 0, "zero bytes per vector");
         LGPU_REQUIRE((uint64_t)d->nbytes * 8 <= ((uint64_t)1 << 24), "binary vectors above 2^24 bits are not supported");
         check_ivf_layout(d->nbytes, d->nlist, LGPU_L2, d->nrows, d->centroids, d->part_offsets, d->vectors, d->row_ids);
-        require_device(d->device);
-        ix = new lgpu_ivf_binary();
+        ix = new_ivf<lgpu_ivf_binary>(d->device, IvfKind::ham);
         ix->nbytes = d->nbytes; ix->nbytes_pad = (d->nbytes + 31) & ~31u;
         ix->dim = d->nbytes;
-        open_ivf_partitions(ix, d->device, d->nlist, d->nrows, d->part_offsets, d->row_ids, HAM_ROWS_TILE);
+        open_ivf_partitions(ix, d, HAM_ROWS_TILE, std::vector<uint64_t>(d->nlist));
         // centroids and rows zero-padded to nbytes_pad, with their popcounts (ham_pack)
         const uint32_t nb = d->nbytes, nbp = ix->nbytes_pad;
         auto pack = [&](const uint8_t *src, uint64_t n, DevBuf &dst, DevBuf &pop) {
@@ -2900,24 +2840,14 @@ int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
             pop.ensure(std::max<size_t>((size_t)n * 4, 16));
             if (n) {
                 DevBuf raw;
-                raw.ensure((size_t)n * nb);
-                LGPU_CUDA(cudaMemcpy(raw.p, src, (size_t)n * nb, cudaMemcpyHostToDevice));
+                upload(raw, src, (size_t)n * nb);
                 launch_ham_pack(raw.as<uint8_t>(), nb, nb, n, dst.as<uint8_t>(), nbp, pop.as<uint32_t>(), nullptr);
                 LGPU_CUDA(cudaStreamSynchronize(nullptr));
             }
-            ix->device_bytes += dst.bytes + pop.bytes;
         };
         pack(d->centroids, d->nlist, ix->centroids, ix->cent_pop);
         pack(d->vectors, d->nrows, ix->codes, ix->row_pop);
-        // the tile descriptors' code offset is unused (the scan addresses rows by part_off)
-        ix->code_base.ensure((size_t)d->nlist * 8);
-        LGPU_CUDA(cudaMemset(ix->code_base.p, 0, (size_t)d->nlist * 8));
-        ix->device_bytes += ix->code_base.bytes;
-        register_handle(ix);
-        *out = ix;
     });
-    if (rc != LGPU_OK && ix) delete ix;
-    return rc;
 }
 
 void lgpu_ivf_binary_close(lgpu_ivf_binary *ix) { close_handle(ix); }
@@ -2925,15 +2855,9 @@ void lgpu_ivf_binary_close(lgpu_ivf_binary *ix) { close_handle(ix); }
 static int ivf_binary_call(lgpu_ivf_binary *ixh, const Route &r, const uint8_t *q, uint32_t B,
                            const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    return search_call(ixh, "binary IVF index", r, q, B, p, ids, dist, cnt,
-                       [&](lgpu_ivf_binary *ix) {
-                           check_call(p, B, q, ids, dist, cnt, false);   // refine_factor: exact distances
-                           LGPU_REQUIRE(p->nprobes >= 1, "minimum_nprobes must be greater than 0");
-                           LGPU_REQUIRE(p->nprobes <= SELECT_KMAX || p->nprobes >= ix->nlist,
-                                        "nprobes above 2048 is not supported unless it covers every partition");
-                           return (size_t)B * ix->nbytes;
-                       },
-                       ivf_binary_search_device);
+    return search_call(ixh, r, q, B, p, ids, dist, cnt,
+                       [&](lgpu_ivf_binary *ix) { check_ivf_call(ix, q, B, p, ids, dist, cnt); return (size_t)B * ix->nbytes; },
+                       ivf_search_device);
 }
 
 int lgpu_ivf_binary_search(lgpu_ivf_binary *ixh, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
@@ -2969,31 +2893,12 @@ int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_
         LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
         const uint32_t nbp = (nbytes + 31) & ~31u;
         DevBuf rq, rx, q, x, qp, xp, D, tiles, ctr;
-        rq.ensure((size_t)B * nbytes); rx.ensure((size_t)N * nbytes);
         q.ensure((size_t)B * nbp); x.ensure((size_t)N * nbp); qp.ensure((size_t)B * 4); xp.ensure((size_t)N * 4);
-        LGPU_CUDA(cudaMemcpy(rq.p, queries, (size_t)B * nbytes, cudaMemcpyHostToDevice));
-        LGPU_CUDA(cudaMemcpy(rx.p, vectors, (size_t)N * nbytes, cudaMemcpyHostToDevice));
+        upload(rq, queries, (size_t)B * nbytes); upload(rx, vectors, (size_t)N * nbytes);
         launch_ham_pack(rq.as<uint8_t>(), nbytes, nbytes, B, q.as<uint8_t>(), nbp, qp.as<uint32_t>(), nullptr);
         launch_ham_pack(rx.as<uint8_t>(), nbytes, nbytes, N, x.as<uint8_t>(), nbp, xp.as<uint32_t>(), nullptr);
-        // one partition of N rows that every query probes: tiles of HAM_ROWS_TILE rows x 8 queries, query b's row r at
-        // out + b N + r
-        std::vector<TileDesc> h;
-        for (uint32_t q0 = 0; q0 < B; q0 += SCAN_G)
-            for (uint64_t r0 = 0; r0 < N; r0 += HAM_ROWS_TILE) {
-                TileDesc t{};
-                t.row0 = (uint32_t)r0; t.nrows = (uint32_t)std::min<uint64_t>(HAM_ROWS_TILE, N - r0);
-                t.ng = std::min<uint32_t>(SCAN_G, B - q0); t.n_p = (uint32_t)N;
-                for (uint32_t g = 0; g < t.ng; g++) {
-                    t.q[g] = q0 + g; t.slot[g] = q0 + g; t.out[g] = (uint32_t)((q0 + g) * N);
-                }
-                h.push_back(t);
-            }
-        tiles.ensure(h.size() * sizeof(TileDesc));
-        ctr.ensure(8);
+        debug_tiles(B, (uint32_t)N, HAM_ROWS_TILE, N, tiles, ctr);
         D.ensure((size_t)B * N * 4);
-        LGPU_CUDA(cudaMemcpy(tiles.p, h.data(), h.size() * sizeof(TileDesc), cudaMemcpyHostToDevice));
-        const uint32_t zero2[2] = {(uint32_t)h.size(), 0u};
-        LGPU_CUDA(cudaMemcpy(ctr.p, zero2, 8, cudaMemcpyHostToDevice));
         HamScanArgs a{};
         a.rows = x.as<uint8_t>(); a.row_pop = xp.as<uint32_t>(); a.queries = q.as<uint8_t>(); a.qpop = qp.as<uint32_t>();
         a.nbytes_pad = nbp;
@@ -3066,7 +2971,7 @@ void lgpu_multivec_close(lgpu_multivec *mv) { close_handle(mv); }
 static int multivec_call(lgpu_multivec *mvh, const Route &r, const float *q, const uint32_t *q_off, uint32_t B,
                          const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)
 {
-    return search_call(mvh, "multivector", r, q, B, p, ids, dist, cnt,
+    return search_call(mvh, r, q, B, p, ids, dist, cnt,
                        [&](lgpu_multivec *mv) {
                            check_call(p, B, q, ids, dist, cnt);
                            if (B == 0) return (size_t)0;
@@ -3236,9 +3141,9 @@ int lgpu_search_sharded(lgpu_index *ixh, lgpu_comm *ch, const float *queries, ui
                         const lgpu_search_params *params, uint64_t *out_ids, float *out_dist, uint32_t *out_count)
 {
     return guarded([&] {
-        HandleRef<lgpu_index> ix(ixh, "index");
-        HandleRef<lgpu_comm> c(ch, "communicator");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq && !ix->is_pq4, "sharded search serves 8-bit IVF_PQ indexes only");
+        HandleRef<lgpu_index> ix(ixh);
+        HandleRef<lgpu_comm> c(ch);
+        LGPU_REQUIRE(ix->kind == IvfKind::pq8, "sharded search serves 8-bit IVF_PQ indexes only");
         check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -3254,9 +3159,9 @@ int lgpu_search_sharded_device(lgpu_index *ixh, lgpu_comm *ch, const float *d_qu
                                uint32_t *d_out_count, void *cuda_stream)
 {
     return guarded([&] {
-        HandleRef<lgpu_index> ix(ixh, "index");
-        HandleRef<lgpu_comm> c(ch, "communicator");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq && !ix->is_pq4, "sharded search serves 8-bit IVF_PQ indexes only");
+        HandleRef<lgpu_index> ix(ixh);
+        HandleRef<lgpu_comm> c(ch);
+        LGPU_REQUIRE(ix->kind == IvfKind::pq8, "sharded search serves 8-bit IVF_PQ indexes only");
         check_ivf_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
         if (B == 0) return;
         require_device(ix->device);
@@ -3270,7 +3175,7 @@ int lgpu_comm_last_stage_ms(lgpu_comm *ch, float *times)
 {
     return guarded([&] {
         LGPU_REQUIRE(times, "null argument");
-        HandleRef<lgpu_comm> c(ch, "communicator");
+        HandleRef<lgpu_comm> c(ch);
         memcpy(times, c->last_ms, sizeof(c->last_ms));
     });
 }
@@ -3280,7 +3185,7 @@ int lgpu_debug_coarse(lgpu_index *ixh, const float *queries, uint32_t B, uint32_
 {
     return guarded([&] {
         LGPU_REQUIRE(queries && out_parts && out_dists && B > 0 && nprobes > 0, "bad argument");
-        HandleRef<lgpu_index> ix(ixh, "index");
+        HandleRef<lgpu_index> ix(ixh);
         require_device(ix->device);
         nprobes = std::min(nprobes, ix->nlist);
         WsLease lease(ix->pool, nullptr, false);
@@ -3293,7 +3198,8 @@ int lgpu_debug_coarse(lgpu_index *ixh, const float *queries, uint32_t B, uint32_
         modes.exact = true;                               // (no filter scan: no query tables)
         IvfPlan p = ivf_plan(ix.h, B, nprobes, sp, false, false, modes);
         p.coarse = Coarse::exact;                         // the exact kernels' probes and distances
-        ivf_coarse(ix.h, ws, p, ivf_queries(ix.h, ws, st, ws->q.as<float>(), B), st, st, StageMarks{ws, false});
+        const IvfQueries q{ivf_queries(ix.h, ws, st, ws->q.as<float>(), B), nullptr, nullptr, ix->dim};
+        ivf_coarse(ix.h, ws, p, q, st, st, StageMarks{ws, false});
         std::vector<uint64_t> tmp((size_t)B * nprobes);
         LGPU_CUDA(cudaMemcpyAsync(tmp.data(), ws->probes.p, tmp.size() * 8, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaMemcpyAsync(out_dists, ws->probe_dist.p, tmp.size() * 4, cudaMemcpyDeviceToHost, st));
@@ -3328,8 +3234,9 @@ int lgpu_debug_partition_distances(lgpu_index *ixh, const float *query, uint32_t
 {
     return guarded([&] {
         LGPU_REQUIRE(query && out, "null argument");
-        HandleRef<lgpu_index> ix(ixh, "index");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq, "lgpu_debug_partition_distances serves IVF_PQ indexes only");
+        HandleRef<lgpu_index> ix(ixh);
+        LGPU_REQUIRE(ix->kind == IvfKind::pq8 || ix->kind == IvfKind::pq4,
+                     "lgpu_debug_partition_distances serves IVF_PQ indexes only");
         LGPU_REQUIRE(part < ix->nlist, "partition out of range");
         require_device(ix->device);
         WsLease lease(ix->pool, nullptr, false);
@@ -3361,8 +3268,8 @@ int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, 
 {
     return guarded([&] {
         LGPU_REQUIRE(queries && out_parts && out_L && out_W && out_E && out_bad && B > 0 && nprobes > 0, "bad argument");
-        HandleRef<lgpu_index> ix(ixh, "index");
-        LGPU_REQUIRE(!ix->is_sq && !ix->is_rq && !ix->is_pq4, "lgpu_debug_filter_bounds serves 8-bit IVF_PQ indexes only");
+        HandleRef<lgpu_index> ix(ixh);
+        LGPU_REQUIRE(ix->kind == IvfKind::pq8, "lgpu_debug_filter_bounds serves 8-bit IVF_PQ indexes only");
         require_device(ix->device);
         nprobes = std::min(nprobes, ix->nlist);
         LGPU_REQUIRE(ivf_sub_batch_size(ix.h, B, nprobes) == B, "batch too large for one filter-scan launch");
@@ -3379,7 +3286,7 @@ int lgpu_debug_filter_bounds(lgpu_index *ixh, const float *queries, uint32_t B, 
         // the search's front, then the dense mode's scan: one lower bound L per row
         const float *qs = ivf_queries(ix.h, ws, st, ws->q.as<float>(), B);
         const cudaStream_t cs = fork_front(ix.h, ws, st, B);
-        ivf_coarse(ix.h, ws, p, qs, cs, st, StageMarks{ws, false});
+        ivf_coarse(ix.h, ws, p, IvfQueries{qs, nullptr, nullptr, ix->dim}, cs, st, StageMarks{ws, false});
         const GroupArgs ga = ivf_regroup(ix.h, ws, p, nullptr, cs);
         LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
         ScanArgs sc = scan_args(ix.h, ws, qs, ga);

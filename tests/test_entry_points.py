@@ -41,6 +41,9 @@ def _searches(h, comm):
         ("binary", "lgpu_binary_search", (h, qp, 1, pp) + out),
         ("binary", "lgpu_binary_search_filtered", (h, qp, 1, pp, bm.ctypes.data, 32) + out),
         ("binary", "lgpu_binary_search_device", (h, qp, 1, pp) + out + (None,)),
+        ("binary IVF index", "lgpu_ivf_binary_search", (h, qp, 1, pp) + out),
+        ("binary IVF index", "lgpu_ivf_binary_search_filtered", (h, qp, 1, pp, bm.ctypes.data, 32) + out),
+        ("binary IVF index", "lgpu_ivf_binary_search_device", (h, qp, 1, pp) + out + (None,)),
         ("multivector", "lgpu_multivec_search", (h, qp, off.ctypes.data, 1, pp) + out),
         ("multivector", "lgpu_multivec_search_filtered", (h, qp, off.ctypes.data, 1, pp, bm.ctypes.data, 32) + out),
         ("multivector", "lgpu_multivec_search_device", (h, qp, off.ctypes.data, 1, pp) + out + (None,)),
@@ -57,7 +60,7 @@ def _refused(rc, kind):
 def test_every_search_entry_point_refuses_a_dead_handle(handle):
     lib = _lib()
     calls, keep = _searches(handle, STALE)
-    assert len(calls) == 15
+    assert len(calls) == 18
     for kind, name, args in calls:
         _refused(getattr(lib, name)(*args), kind)
 
@@ -98,7 +101,7 @@ def test_other_handle_entry_points_name_their_kind():
 def test_close_accepts_null_and_stale_handles():
     lib = _lib()
     for name in ("lgpu_index_close", "lgpu_flat_close", "lgpu_binary_close", "lgpu_multivec_close",
-                 "lgpu_comm_destroy"):
+                 "lgpu_ivf_binary_close", "lgpu_comm_destroy"):
         getattr(lib, name)(None)
         getattr(lib, name)(STALE)
 

@@ -1,13 +1,15 @@
-"""The search entry points of every column kind (IVF_PQ, IVF_SQ, flat under each metric, binary, multivector) on each
-route (host buffers, host buffers with a prefilter, device pointers) behave alike: B = 0 is a no-op, a closed handle,
-a null output buffer and a null bitmap are refused, the routes return the same bits, and repeated host calls (eager,
-CUDA-graph capture, replay) return the same bits with the same launch count."""
+"""The search entry points of every column kind (IVF_PQ, IVF_SQ, flat under each metric, binary, binary IVF_FLAT,
+multivector) on each route (host buffers, host buffers with a prefilter, device pointers) behave alike: B = 0 is a
+no-op, a closed handle, a live handle of another kind, a null output buffer and a null bitmap are refused, the routes
+return the same bits, and repeated host calls (eager, CUDA-graph capture, replay) return the same bits with the same
+launch count."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
 from lancedb_b200 import _native
+from tests import ivf_binary_oracle
 from tests.multivec_oracle import offsets_of
 from tests.sq_oracle import random_sq_index
 from tests.util import queries, random_index
@@ -15,10 +17,14 @@ from tests.util import queries, random_index
 pytestmark = pytest.mark.gpu
 
 K = 5
-KINDS = ["ivf_pq", "ivf_sq", "flat_l2", "flat_cosine", "flat_dot", "binary", "multivec"]
+KINDS = ["ivf_pq", "ivf_sq", "flat_l2", "flat_cosine", "flat_dot", "binary", "ivf_binary", "multivec"]
 ROUTES = ["host", "filtered", "device"]
 SYMBOL = {"ivf": "lgpu_search", "flat": "lgpu_flat_search", "binary": "lgpu_binary_search",
-          "multivec": "lgpu_multivec_search"}
+          "ivf_binary": "lgpu_ivf_binary_search", "multivec": "lgpu_multivec_search"}
+# the handle kind of each family, as the library's messages name it, and its close function
+NAME = {"ivf": "index", "flat": "flat", "binary": "binary", "ivf_binary": "binary IVF index", "multivec": "multivector"}
+CLOSE = {"ivf": "lgpu_index_close", "flat": "lgpu_flat_close", "binary": "lgpu_binary_close",
+         "ivf_binary": "lgpu_ivf_binary_close", "multivec": "lgpu_multivec_close", "comm": "lgpu_comm_destroy"}
 
 
 class Case:
@@ -26,7 +32,7 @@ class Case:
 
     def __init__(self, kind, B=6):
         rng = np.random.default_rng(7)
-        self.kind, self.family = kind, kind.split("_")[0]
+        self.kind, self.family = kind, kind if kind == "ivf_binary" else kind.split("_")[0]
         self.metric = _native.METRICS[kind.split("_")[1]] if self.family == "flat" else None
         self.off = None
         if kind == "ivf_pq":
@@ -37,6 +43,9 @@ class Case:
             self.obj, self.q = _native.GpuFlat(queries(rng, 5000, 32)), queries(rng, B, 32)
         elif kind == "binary":
             self.obj = _native.GpuBinary(rng.integers(0, 256, (5000, 16), dtype=np.uint8))
+            self.q = rng.integers(0, 256, (B, 16), dtype=np.uint8)
+        elif kind == "ivf_binary":
+            self.obj = _native.GpuIvfBinary(ivf_binary_oracle.random_index(rng, 3000, 16, 8))
             self.q = rng.integers(0, 256, (B, 16), dtype=np.uint8)
         else:
             lens = rng.integers(0, 5, 2000)
@@ -163,10 +172,61 @@ def test_repeated_host_calls_return_the_same_bits_and_launches(case):
 
 @pytest.mark.parametrize("route", ROUTES)
 def test_closed_handle_is_refused(route):
-    for k in (Case(kind, B=2) for kind in ("ivf_pq", "flat_l2", "binary", "multivec")):
+    for k in (Case(kind, B=2) for kind in ("ivf_pq", "flat_l2", "binary", "ivf_binary", "multivec")):
         h = C.c_void_p(k.obj._h.value)
         k.obj.close()
         outs = [np.zeros(2 * K, np.uint64), np.zeros(2 * K, np.float32), np.zeros(2, np.uint32)]
         rc = k.call(route, h, k.q.ctypes.data, 2, [o.ctypes.data for o in outs], k.bitmap().ctypes.data, 32)
         assert rc == _native.LGPU_INVALID_INPUT
         assert b"closed" in _native.load().lgpu_last_error()
+
+
+def test_a_live_handle_of_another_kind_is_refused():
+    """Every live handle, passed to every other kind's search on every route, to the index-only entry points and as a
+    communicator, is refused on the host before it is read; a close of another kind leaves it open and unchanged."""
+    lib = _native.load()
+    cases = [Case(kind) for kind in KINDS]
+    before = [c.host("host") for c in cases]
+    ids, dist, cnt = np.zeros(64, np.uint64), np.zeros(64, np.float32), np.zeros(8, np.uint32)
+    outs = (ids.ctypes.data, dist.ctypes.data, cnt.ctypes.data)
+
+    def refused(rc, want, got):
+        assert rc == _native.LGPU_INVALID_INPUT
+        article = "an" if got == "index" else "a"
+        assert lib.lgpu_last_error().decode() == f"{want} handle expected, got {article} {got} handle"
+
+    for h in cases:
+        got = NAME[h.family]
+        for c in cases:
+            if c.family == h.family:
+                continue
+            for route in ROUTES:
+                bm = c.bitmap()
+                refused(c.call(route, h.obj._h, c.q.ctypes.data, c.B, outs, bm.ctypes.data, 32), NAME[c.family], got)
+        if h.family != "ivf":
+            refused(lib.lgpu_index_device_bytes(h.obj._h, C.byref(C.c_uint64())), "index", got)
+        t = (C.c_float * 3)()
+        refused(lib.lgpu_comm_last_stage_ms(h.obj._h, t), "communicator", got)
+    ix, q = cases[KINDS.index("ivf_pq")], cases[KINDS.index("ivf_pq")].q
+    p = C.byref(ix.params)
+    refused(lib.lgpu_search_sharded(ix.obj._h, ix.obj._h, q.ctypes.data, 1, p, *outs), "communicator", "index")
+    refused(lib.lgpu_search_sharded_device(ix.obj._h, ix.obj._h, q.ctypes.data, 1, p, *outs, None), "communicator",
+            "index")
+    ivb = cases[KINDS.index("ivf_binary")].obj._h
+    refused(lib.lgpu_search_sharded_device(ivb, ix.obj._h, q.ctypes.data, 1, p, *outs, None), "index",
+            "binary IVF index")
+    parts, L = np.zeros(64, np.uint32), np.zeros(64 * 64, np.float32)
+    refused(lib.lgpu_debug_filter_bounds(ivb, q.ctypes.data, 1, 4, 64, parts.ctypes.data, L.ctypes.data,
+                                         dist.ctypes.data, dist.ctypes.data, cnt.ctypes.data), "index", "binary IVF index")
+    refused(lib.lgpu_debug_partition_distances(ivb, q.ctypes.data, 0, L.ctypes.data), "index", "binary IVF index")
+
+    for h in cases:
+        for family, close in CLOSE.items():
+            if family != h.family:
+                getattr(lib, close)(h.obj._h)
+    try:
+        for c, b in zip(cases, before):
+            assert _equal(c.host("host"), b), c.kind
+    finally:
+        for c in cases:
+            c.obj.close()
