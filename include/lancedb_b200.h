@@ -477,6 +477,55 @@ int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *valu
 /* the number of queries per sub-batch an lgpu_search* call of B queries and `nprobes` probes (the widest the call uses:
  * maximum_nprobes under a prefilter) on `ix` runs in under the process's LGPU_WS_BYTES: B when the batch is not split */
 int lgpu_debug_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32_t *out);
+/* the top-k selection every search ends in, run as given: per query q < B, the k entries with the smallest
+ * (_distance, id) among its candidates, ascending, into out_ids / out_dist (or out_rec), out_count[q] of them, the rest
+ * padded with id UINT64_MAX and +inf.  A candidate is dropped when its distance is NaN or outside [lower, upper) (each
+ * bound only when has_lower / has_upper is set), or when allow is set and its id is >= allow_bits or has bit 0 there;
+ * -0 is reported as +0.  The candidates of query q:
+ *   mode 0 (IVF distance segments): for each probe slot s = q * nprobes + j whose probes[s] = p < nlist, the part_n[p]
+ *     values at dist + seg_off[s], row r with id row_ids[part_off[p] + r] (part_off[p] + r when row_ids is NULL) and
+ *     pos part_off[p] + r.  Every such segment starts at a multiple of 4 floats and, padded to 4, lies in dist_len;
+ *   mode 1 (dense rows): dense[q * row_stride + c] for c < ncols, id col_ids[c] (c when NULL), pos c;
+ *   mode 2 (strided lists): c < ncols (< ncols_q[q] too when ncols_q is set) at
+ *     addr = (c / inner) * outer_stride + q * row_stride + c % inner: id cand_ids[addr], value dense[addr] (or both from
+ *     the 16-byte record cand_rec[addr] = {u64 id, f32 dist, u32 pad}), pos cand_pos[addr] (c when NULL); an entry with
+ *     id UINT64_MAX is an unused slot.
+ * out_pos (optional) receives each entry's pos (UINT64_MAX when padded), out_rec (optional) the entries as 16-byte
+ * records instead of out_ids / out_dist.  A query with only[q] == 0, or every query when *gate == 0, is left untouched.
+ * Every pointer is a device pointer on `device`; dist, cand_rec and out_rec are 16-byte aligned.  Enqueued on
+ * cuda_stream, not synchronised (mode 0 synchronises the stream once to check the segments). */
+typedef struct {
+    int32_t mode;                 /* 0, 1 or 2 */
+    const float *dist;            /* mode 0 */
+    const uint64_t *seg_off;      /* mode 0: [B * nprobes] */
+    const uint64_t *probes;       /* mode 0: [B * nprobes] */
+    uint32_t nprobes, nlist;
+    const uint32_t *part_n;       /* mode 0: [nlist] */
+    const uint64_t *part_off;     /* mode 0: [nlist] */
+    const uint64_t *row_ids;      /* mode 0: optional */
+    const float *dense;           /* mode 1, mode 2 without cand_rec */
+    uint64_t ncols, row_stride;
+    uint64_t inner, outer_stride; /* mode 2: inner >= 1 */
+    const uint64_t *col_ids;      /* mode 1: optional [ncols] */
+    const uint64_t *cand_ids;     /* mode 2 without cand_rec */
+    const uint64_t *cand_pos;     /* mode 2: optional */
+    const uint32_t *ncols_q;      /* mode 2: optional [B] */
+    const void *cand_rec;         /* mode 2: optional */
+    uint32_t B, k;                /* 1 <= k <= 2048 */
+    int32_t has_lower, has_upper;
+    float lower, upper;
+    uint64_t *out_ids;            /* [B][k] */
+    float *out_dist;              /* [B][k] */
+    uint32_t *out_count;          /* [B] */
+    void *out_rec;                /* optional [B][k] */
+    uint64_t *out_pos;            /* optional [B][k] */
+    const uint32_t *only;         /* optional [B] */
+    const uint32_t *gate;         /* optional [1] */
+    const uint32_t *allow;        /* optional bitmap: bit i & 31 of word i >> 5 */
+    uint64_t allow_bits;
+    uint64_t dist_len;            /* mode 0: floats in dist */
+} lgpu_debug_select_args;
+int lgpu_debug_select(const lgpu_debug_select_args *a, int device, void *cuda_stream);
 /* per-stage device time (ms) of the most recent profiled lgpu_search* / lgpu_ivf_binary_search* call on this thread:
  * coarse, select-probes, group, scan, top-k, refine, total.  times: [7].  A call the workspace budget splits into
  * sub-batches reports, per stage, the sum over its sub-batches (profiling synchronises after each one); the

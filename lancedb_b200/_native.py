@@ -31,7 +31,7 @@ EXPORTS = [
     "lgpu_flat_open", "lgpu_flat_close", "lgpu_flat_search", "lgpu_flat_search_filtered", "lgpu_flat_search_device",
     "lgpu_ivf_assign", "lgpu_pq_encode", "lgpu_kmeans_train", "lgpu_pq_train",
     "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_filter_bounds", "lgpu_debug_gemm",
-    "lgpu_debug_sub_batch_size", "lgpu_last_stage_ms", "lgpu_set_profiling",
+    "lgpu_debug_sub_batch_size", "lgpu_debug_select", "lgpu_last_stage_ms", "lgpu_set_profiling",
     "lgpu_kernel_launch_count", "lgpu_last_filter_stats",
     "lgpu_binary_open", "lgpu_binary_close", "lgpu_binary_search", "lgpu_binary_search_filtered",
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
@@ -84,6 +84,21 @@ class IvfBinaryDesc(C.Structure):
         ("abi_version", C.c_uint32), ("nbytes", C.c_uint32), ("nlist", C.c_uint32), ("device", C.c_int32),
         ("nrows", C.c_uint64), ("centroids", C.c_void_p), ("part_offsets", C.c_void_p), ("vectors", C.c_void_p),
         ("row_ids", C.c_void_p),
+    ]
+
+
+class DebugSelectArgs(C.Structure):
+    """lgpu_debug_select_args: the top-k selection's arguments, every pointer a device address"""
+    _fields_ = [
+        ("mode", C.c_int32), ("dist", C.c_void_p), ("seg_off", C.c_void_p), ("probes", C.c_void_p),
+        ("nprobes", C.c_uint32), ("nlist", C.c_uint32), ("part_n", C.c_void_p), ("part_off", C.c_void_p),
+        ("row_ids", C.c_void_p), ("dense", C.c_void_p), ("ncols", C.c_uint64), ("row_stride", C.c_uint64),
+        ("inner", C.c_uint64), ("outer_stride", C.c_uint64), ("col_ids", C.c_void_p), ("cand_ids", C.c_void_p),
+        ("cand_pos", C.c_void_p), ("ncols_q", C.c_void_p), ("cand_rec", C.c_void_p), ("B", C.c_uint32),
+        ("k", C.c_uint32), ("has_lower", C.c_int32), ("has_upper", C.c_int32), ("lower", C.c_float),
+        ("upper", C.c_float), ("out_ids", C.c_void_p), ("out_dist", C.c_void_p), ("out_count", C.c_void_p),
+        ("out_rec", C.c_void_p), ("out_pos", C.c_void_p), ("only", C.c_void_p), ("gate", C.c_void_p),
+        ("allow", C.c_void_p), ("allow_bits", C.c_uint64), ("dist_len", C.c_uint64),
     ]
 
 
@@ -154,6 +169,7 @@ def load():
     lib.lgpu_debug_filter_bounds.argtypes = [vp, vp, u32, u32, C.c_uint64, vp, vp, vp, vp, vp]
     lib.lgpu_debug_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
     lib.lgpu_debug_sub_batch_size.argtypes = [vp, u32, u32, C.POINTER(u32)]
+    lib.lgpu_debug_select.argtypes = [C.POINTER(DebugSelectArgs), i32, vp]
     lib.lgpu_last_stage_ms.argtypes = [vp]
     lib.lgpu_set_profiling.argtypes = [i32]
     lib.lgpu_kernel_launch_count.argtypes = [C.POINTER(C.c_uint64)]
@@ -715,6 +731,12 @@ def merge_topk_device(device: int, nlists: int, B: int, k: int, d_ids: int, d_di
                       d_out_dist: int, d_out_cnt: int, stream: int = 0):
     check(load().lgpu_merge_topk_device(device, nlists, B, k, d_ids, d_dist, d_out_ids, d_out_dist, d_out_cnt,
                                         stream))
+
+
+def debug_select(device: int = 0, stream: int = 0, **args) -> None:
+    """The top-k selection alone (lgpu_debug_select): `args` are lgpu_debug_select_args fields, device addresses as
+    ints; enqueued on `stream`, not synchronised."""
+    check(load().lgpu_debug_select(C.byref(DebugSelectArgs(**args)), device, stream))
 
 
 def debug_gemm(queries, vectors, device: int = 0) -> np.ndarray:

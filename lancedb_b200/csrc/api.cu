@@ -2498,6 +2498,60 @@ int lgpu_debug_sub_batch_size(lgpu_index *ixh, uint32_t B, uint32_t nprobes, uin
     });
 }
 
+int lgpu_debug_select(const lgpu_debug_select_args *a, int device, void *cuda_stream)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(a != nullptr, "null argument");
+        LGPU_REQUIRE(a->mode >= 0 && a->mode <= 2, "select mode must be 0, 1 or 2");
+        LGPU_REQUIRE(a->k >= 1 && a->k <= SELECT_KMAX, "k must be in [1, 2048]");
+        auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+        LGPU_REQUIRE(a->out_count && (a->out_rec || (a->out_ids && a->out_dist)), "null output buffer");
+        LGPU_REQUIRE(a16(a->out_rec), "out_rec must be 16-byte aligned");
+        if (a->mode == 0) {
+            LGPU_REQUIRE(a->dist && a->seg_off && a->probes && a->part_n && a->part_off, "null mode-0 buffer");
+            LGPU_REQUIRE(a16(a->dist), "mode 0: dist must be 16-byte aligned");   // float4 loads
+        } else if (a->mode == 1) {
+            LGPU_REQUIRE(a->dense, "null mode-1 buffer");
+        } else {
+            LGPU_REQUIRE(a->cand_rec || (a->dense && a->cand_ids), "null mode-2 buffer");
+            LGPU_REQUIRE(a16(a->cand_rec), "cand_rec must be 16-byte aligned");
+            LGPU_REQUIRE(a->inner >= 1, "mode 2: inner must be at least 1");
+        }
+        require_device(device);
+        cudaStream_t st = (cudaStream_t)cuda_stream;
+        if (a->mode == 0 && a->B > 0 && a->nprobes > 0) {
+            // the kernels load every probed segment as float4 up to its length rounded up to 4
+            const size_t ns = (size_t)a->B * a->nprobes;
+            std::vector<uint64_t> probes(ns), seg(ns);
+            std::vector<uint32_t> part_n(a->nlist);
+            LGPU_CUDA(cudaStreamSynchronize(st));
+            LGPU_CUDA(cudaMemcpy(probes.data(), a->probes, ns * 8, cudaMemcpyDeviceToHost));
+            LGPU_CUDA(cudaMemcpy(seg.data(), a->seg_off, ns * 8, cudaMemcpyDeviceToHost));
+            if (a->nlist) LGPU_CUDA(cudaMemcpy(part_n.data(), a->part_n, (size_t)a->nlist * 4, cudaMemcpyDeviceToHost));
+            for (size_t s = 0; s < ns; s++) {
+                if (probes[s] >= a->nlist) continue;
+                LGPU_REQUIRE(seg[s] % 4 == 0, "mode 0: seg_off must be a multiple of 4");
+                LGPU_REQUIRE(seg[s] <= a->dist_len && round_up64(part_n[probes[s]], 4) <= a->dist_len - seg[s],
+                             "mode 0: a segment padded to 4 floats runs past dist_len");
+            }
+        }
+        SelectArgs s{};
+        s.mode = a->mode;
+        s.dist = a->dist; s.seg_off = a->seg_off; s.probes = a->probes; s.nprobes = a->nprobes; s.nlist = a->nlist;
+        s.part_n = a->part_n; s.part_off = a->part_off; s.row_ids = a->row_ids;
+        s.dense = a->dense; s.ncols = a->ncols; s.row_stride = a->row_stride;
+        s.inner = a->inner; s.outer_stride = a->outer_stride;
+        s.col_ids = a->col_ids; s.cand_ids = a->cand_ids; s.cand_pos = a->cand_pos; s.ncols_q = a->ncols_q;
+        s.cand_rec = static_cast<const TopkRecord *>(a->cand_rec);
+        s.B = a->B; s.k = a->k;
+        s.has_lower = a->has_lower; s.has_upper = a->has_upper; s.lower = a->lower; s.upper = a->upper;
+        s.out_ids = a->out_ids; s.out_dist = a->out_dist; s.out_count = a->out_count;
+        s.out_rec = static_cast<TopkRecord *>(a->out_rec); s.out_pos = a->out_pos;
+        s.only = a->only; s.gate = a->gate; s.allow = a->allow; s.allow_bits = a->allow_bits;
+        launch_select(s, st);
+    });
+}
+
 static void check_ivf_call(lgpu_index *ix, const void *q, uint32_t B, const lgpu_search_params *p,
                            const void *a, const void *b, const void *c)
 {

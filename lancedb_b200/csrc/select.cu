@@ -247,36 +247,32 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
 }
 
 // ---------------------------------------------------------------------------------
-// k <= 128: four warps per query; every warp keeps the k best of its share in registers
-// (NQ = 1, 2 or 4 sorted entries per lane).  Candidates stream through 8 per lane per
-// iteration (two float4 loads in flight) and only the ones not worse than the warp's
-// current k-th best are inserted (ballot loop).  After warm-up almost nothing passes, so
-// a query costs ~1 compare per candidate.  The four queues are merged through shared memory.
+// k <= 32: four warps per query; every warp keeps the k best of its share in registers, lane i holding its i-th best.
+// Candidates stream through 8 per lane per iteration (two float4 loads in flight) and only the ones not worse than the
+// warp's current k-th best are inserted (ballot loop).  After warm-up almost nothing passes, so a query costs ~1 compare
+// per candidate.  The four queues are merged through shared memory.
 #ifndef SELW_WARPS_V
 #define SELW_WARPS_V 4
 #endif
 constexpr int SELW_WARPS = SELW_WARPS_V;       // power of two
 
-template <bool POS, int NQ>
+template <bool POS>
 __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs a)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
-    // NQ queue entries per lane: slot (i, lane) = i * 32 + lane, sorted ascending over slots; k <= 32 * NQ
-    __shared__ uint32_t m_key[SELW_WARPS - 1][32 * NQ];
-    __shared__ uint64_t m_id[SELW_WARPS - 1][32 * NQ];
-    __shared__ uint64_t m_pos[SELW_WARPS - 1][POS ? 32 * NQ : 1];
+    __shared__ uint32_t m_key[SELW_WARPS - 1][32];
+    __shared__ uint64_t m_id[SELW_WARPS - 1][32];
+    __shared__ uint64_t m_pos[SELW_WARPS - 1][POS ? 32 : 1];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const uint32_t q = blockIdx.x;
     if (a.gate && *a.gate == 0) return;
     if (a.only && !a.only[q]) return;                       // fix-up pass: untouched query
     const uint32_t k = a.k;
-    uint32_t qk[NQ];
-    uint64_t qid[NQ], qpos[NQ];
-#pragma unroll
-    for (int i = 0; i < NQ; i++) { qk[i] = 0xffffffffu; qid[i] = UINT64_MAX; qpos[i] = UINT64_MAX; }
+    uint32_t qk = 0xffffffffu;                              // the warp's queue, sorted ascending over the lanes
+    uint64_t qid = UINT64_MAX, qpos = UINT64_MAX;
     uint32_t tau_k = 0xffffffffu;                           // (key, id) of the k-th best so far
     uint64_t tau_id = UINT64_MAX;
-    const int tau_row = (int)((k - 1) >> 5), tau_lane = (int)((k - 1) & 31);
+    const int tau_lane = (int)k - 1;
 
     auto in_range = [&](float v) -> bool {
         if (v != v) return false;
@@ -294,32 +290,16 @@ __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs
             const uint64_t cid = __shfl_sync(0xffffffffu, id, src);
             if (!key_less(ck, cid, tau_k, tau_id)) continue;          // threshold moved meanwhile
             const uint64_t cpos = POS ? __shfl_sync(0xffffffffu, pos, src) : 0;
-            int at = 0;                                     // queue is sorted: `at` entries are smaller
-#pragma unroll
-            for (int i = 0; i < NQ; i++) at += __popc(__ballot_sync(0xffffffffu, key_less(qk[i], qid[i], ck, cid)));
-#pragma unroll
-            for (int i = NQ - 1; i >= 0; i--) {             // shift slots >= at up by one (rows high to low)
-                uint32_t uk = __shfl_up_sync(0xffffffffu, qk[i], 1);
-                uint64_t uid = __shfl_up_sync(0xffffffffu, qid[i], 1);
-                uint64_t upos = POS ? __shfl_up_sync(0xffffffffu, qpos[i], 1) : 0;
-                if (i > 0) {                                // lane 0 takes the last entry of the row below
-                    const uint32_t pk = __shfl_sync(0xffffffffu, qk[i - 1], 31);
-                    const uint64_t pid = __shfl_sync(0xffffffffu, qid[i - 1], 31);
-                    const uint64_t ppos = POS ? __shfl_sync(0xffffffffu, qpos[i - 1], 31) : 0;
-                    if (lane == 0) { uk = pk; uid = pid; upos = ppos; }
-                }
-                const int slot = i * 32 + lane;
-                if (slot == at) { qk[i] = ck; qid[i] = cid; if (POS) qpos[i] = cpos; }
-                else if (slot > at) { qk[i] = uk; qid[i] = uid; if (POS) qpos[i] = upos; }
-                if (slot >= (int)k) { qk[i] = 0xffffffffu; qid[i] = UINT64_MAX; }
-            }
-#pragma unroll
-            for (int i = 0; i < NQ; i++) {
-                if (i == tau_row) {
-                    tau_k = __shfl_sync(0xffffffffu, qk[i], tau_lane);
-                    tau_id = __shfl_sync(0xffffffffu, qid[i], tau_lane);
-                }
-            }
+            // the queue is sorted: `at` entries are smaller; lanes >= at shift up by one
+            const int at = __popc(__ballot_sync(0xffffffffu, key_less(qk, qid, ck, cid)));
+            const uint32_t uk = __shfl_up_sync(0xffffffffu, qk, 1);
+            const uint64_t uid = __shfl_up_sync(0xffffffffu, qid, 1);
+            const uint64_t upos = POS ? __shfl_up_sync(0xffffffffu, qpos, 1) : 0;
+            if (lane == at) { qk = ck; qid = cid; if (POS) qpos = cpos; }
+            else if (lane > at) { qk = uk; qid = uid; if (POS) qpos = upos; }
+            if (lane >= (int)k) { qk = 0xffffffffu; qid = UINT64_MAX; }
+            tau_k = __shfl_sync(0xffffffffu, qk, tau_lane);
+            tau_id = __shfl_sync(0xffffffffu, qid, tau_lane);
         }
     };
     auto offer4 = [&](const float4 t, uint64_t n_left, uint64_t idbase, const uint64_t *idsrc, uint64_t posbase) {
@@ -400,33 +380,22 @@ __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs
     }
     // merge the four queues: warps 1..3 publish, warp 0 inserts
     if (w > 0) {
-#pragma unroll
-        for (int i = 0; i < NQ; i++) {
-            m_key[w - 1][i * 32 + lane] = qk[i]; m_id[w - 1][i * 32 + lane] = qid[i];
-            if (POS) m_pos[w - 1][i * 32 + lane] = qpos[i];
-        }
+        m_key[w - 1][lane] = qk; m_id[w - 1][lane] = qid;
+        if (POS) m_pos[w - 1][lane] = qpos;
     }
     __syncthreads();
     if (w > 0) return;
 #pragma unroll
     for (int o = 0; o < SELW_WARPS - 1; o++) {
-#pragma unroll
-        for (int i = 0; i < NQ; i++) {
-            const uint32_t ck = m_key[o][i * 32 + lane];
-            const uint64_t cid = m_id[o][i * 32 + lane];
-            offer(cid != UINT64_MAX || ck != 0xffffffffu, ck, cid, POS ? m_pos[o][i * 32 + lane] : 0);
-        }
+        const uint32_t ck = m_key[o][lane];
+        const uint64_t cid = m_id[o][lane];
+        offer(cid != UINT64_MAX || ck != 0xffffffffu, ck, cid, POS ? m_pos[o][lane] : 0);
     }
-    uint32_t total = 0;
-#pragma unroll
-    for (int i = 0; i < NQ; i++) {
-        const bool have = qid[i] != UINT64_MAX || qk[i] != 0xffffffffu;
-        total += __popc(__ballot_sync(0xffffffffu, have));
-        const uint32_t slot = i * 32 + lane;
-        if (slot < k) {
-            write_entry(a, (size_t)q * k + slot, have, qid[i], qk[i]);
-            if (POS) a.out_pos[(size_t)q * k + slot] = have ? qpos[i] : UINT64_MAX;
-        }
+    const bool have = qid != UINT64_MAX || qk != 0xffffffffu;
+    const uint32_t total = __popc(__ballot_sync(0xffffffffu, have));
+    if (lane < (int)k) {
+        write_entry(a, (size_t)q * k + lane, have, qid, qk);
+        if (POS) a.out_pos[(size_t)q * k + lane] = have ? qpos : UINT64_MAX;
     }
     if (lane == 0) a.out_count[q] = min(total, k);
 }
@@ -466,15 +435,12 @@ void launch_select(const SelectArgs &a, cudaStream_t st)
 {
     if (a.B == 0) return;
     LGPU_REQUIRE(a.k >= 1 && a.k <= SELECT_KMAX, "limit+offset (k) must be in [1, 2048] on the GPU path");
-    // with 2 / 4 entries per lane the insert path dominates (k ln(n/k) serial inserts per warp): above k = 32 the
-    // shared-memory stage + bitonic kernel is the faster one
+    // above k = 32 the warp queues' serial inserts (k ln(n/k) per warp) dominate: the shared-memory stage + bitonic
+    // kernel is the faster one there
     if (a.k <= 32) {
-        const unsigned grid = a.B;
-        const int nq = a.k <= 32 ? 1 : (a.k <= 64 ? 2 : 4);
-#define LGPU_SELW(P, N) launch_k(select_warp_kernel<P, N>, dim3(grid), dim3(SELW_WARPS * 32), 0, st, a), LGPU_COUNT_LAUNCH()
-        if (a.out_pos) { if (nq == 1) LGPU_SELW(true, 1); else if (nq == 2) LGPU_SELW(true, 2); else LGPU_SELW(true, 4); }
-        else { if (nq == 1) LGPU_SELW(false, 1); else if (nq == 2) LGPU_SELW(false, 2); else LGPU_SELW(false, 4); }
-#undef LGPU_SELW
+        if (a.out_pos) launch_k(select_warp_kernel<true>, dim3(a.B), dim3(SELW_WARPS * 32), 0, st, a);
+        else launch_k(select_warp_kernel<false>, dim3(a.B), dim3(SELW_WARPS * 32), 0, st, a);
+        LGPU_COUNT_LAUNCH();
         LGPU_CUDA(cudaGetLastError());
         return;
     }

@@ -40,17 +40,18 @@ def pack_records(ids: np.ndarray, dist: np.ndarray) -> np.ndarray:
 
 def merge_records(gathered: np.ndarray, k: int):
     """Host restatement of the merge kernel: gathered [world][B][k] records -> global top-k per query by
-    (_distance, _rowid); unused slots carry id UINT64_MAX.  Used by the CPU (gloo) test of the exchange."""
+    (_distance, _rowid); unused slots carry id UINT64_MAX.  Like the kernel it drops NaN distances and reports -0 as
+    +0 (the two tie).  Used by the CPU (gloo) test of the exchange."""
     world, B, kk = gathered.shape
     ids = np.full((B, k), np.iinfo(np.uint64).max, np.uint64)
     dist = np.full((B, k), np.inf, np.float32)
     cnt = np.zeros(B, np.uint32)
     for b in range(B):
         c = gathered[:, b, :].reshape(-1)
-        c = c[c["id"] != np.iinfo(np.uint64).max]
+        c = c[(c["id"] != np.iinfo(np.uint64).max) & ~np.isnan(c["dist"])]
         order = np.lexsort((c["id"], c["dist"]))[:k]
         n = len(order)
-        ids[b, :n] = c["id"][order]; dist[b, :n] = c["dist"][order]; cnt[b] = n
+        ids[b, :n] = c["id"][order]; dist[b, :n] = c["dist"][order] + np.float32(0); cnt[b] = n     # -0 + 0 = +0
     return ids, dist, cnt
 
 
