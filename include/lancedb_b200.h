@@ -41,6 +41,11 @@ extern "C" {
 
 #define LGPU_ABI_VERSION 2
 
+/* Largest k (limit + offset) and k x refine_factor every single-GPU search serves (rust/lancedb/src/table/query.rs:231
+ * passes limit + offset to the scanner unbounded).  k up to 2048 runs the shared-memory selects, above that the
+ * global-memory radix select (DESIGN.md section 3).  The sharded search and lgpu_merge_topk_device keep k <= 2048. */
+#define LGPU_K_MAX 65536
+
 typedef enum {
     LGPU_OK = 0,
     LGPU_INVALID_INPUT = 1,  /* lancedb::Error::InvalidInput */
@@ -89,7 +94,8 @@ typedef struct {
 /* One vector query request = lancedb::query::VectorQueryRequest
  * (rust/lancedb/src/query.rs:1066-1114) reduced to what reaches the kernels. */
 typedef struct {
-    uint32_t k;              /* limit + offset (table/query.rs:231); default 10 */
+    uint32_t k;              /* limit + offset (table/query.rs:231); default 10; k and k x refine_factor at most
+                                LGPU_K_MAX */
     uint32_t nprobes;        /* maximum_nprobes (== minimum_nprobes == 20 by default) */
     uint32_t refine_factor;  /* 0 = no refine (query.rs:1302-1332) */
     int32_t  has_lower;      /* distance_range lower bound, inclusive */
@@ -278,7 +284,7 @@ int  lgpu_comm_unique_id(void *id_out, size_t id_bytes);
 int  lgpu_comm_init(const void *unique_id, size_t id_bytes, int rank, int world, int device, lgpu_comm **out);
 void lgpu_comm_destroy(lgpu_comm *comm);
 /* collective: every rank passes the same B queries (host buffers) and its own shard; every rank receives the
- * global top-k.  refine_factor must be 0. */
+ * global top-k.  refine_factor must be 0 and k at most 2048. */
 int  lgpu_search_sharded(lgpu_index *shard, lgpu_comm *comm, const float *queries, uint32_t B,
                          const lgpu_search_params *params,
                          uint64_t *out_ids, float *out_dist, uint32_t *out_count);
@@ -511,7 +517,7 @@ typedef struct {
     const uint64_t *cand_pos;     /* mode 2: optional */
     const uint32_t *ncols_q;      /* mode 2: optional [B] */
     const void *cand_rec;         /* mode 2: optional */
-    uint32_t B, k;                /* 1 <= k <= 2048 */
+    uint32_t B, k;                /* 1 <= k <= 2048 (lgpu_debug_select_large: 2048 < k <= LGPU_K_MAX) */
     int32_t has_lower, has_upper;
     float lower, upper;
     uint64_t *out_ids;            /* [B][k] */
@@ -526,6 +532,9 @@ typedef struct {
     uint64_t dist_len;            /* mode 0: floats in dist */
 } lgpu_debug_select_args;
 int lgpu_debug_select(const lgpu_debug_select_args *a, int device, void *cuda_stream);
+/* the same selection for 2048 < k <= LGPU_K_MAX (the global-memory radix select the searches run above k = 2048), same
+ * arguments and results.  Allocates its scratch and synchronises cuda_stream before returning. */
+int lgpu_debug_select_large(const lgpu_debug_select_args *a, int device, void *cuda_stream);
 /* per-stage device time (ms) of the most recent profiled lgpu_search* / lgpu_ivf_binary_search* call on this thread:
  * coarse, select-probes, group, scan, top-k, refine, total.  times: [7].  A call the workspace budget splits into
  * sub-batches reports, per stage, the sum over its sub-batches (profiling synchronises after each one); the

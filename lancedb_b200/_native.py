@@ -20,6 +20,8 @@ _lib = None
 LGPU_OK, LGPU_INVALID_INPUT, LGPU_RUNTIME, LGPU_TIMEOUT, LGPU_OOM = 0, 1, 2, 3, 4
 METRICS = {"l2": 0, "euclidean": 0, "cosine": 1, "dot": 2}
 ABI_VERSION = 2
+K_MAX = 65536                   # LGPU_K_MAX: largest k and k x refine_factor of a single-GPU search
+SHARDED_K_MAX = 2048            # the sharded search's bound on k
 
 EXPORTS = [
     "lgpu_last_error", "lgpu_abi_version", "lgpu_device_count",
@@ -31,7 +33,8 @@ EXPORTS = [
     "lgpu_flat_open", "lgpu_flat_close", "lgpu_flat_search", "lgpu_flat_search_filtered", "lgpu_flat_search_device",
     "lgpu_ivf_assign", "lgpu_pq_encode", "lgpu_kmeans_train", "lgpu_pq_train",
     "lgpu_debug_coarse", "lgpu_debug_partition_distances", "lgpu_debug_filter_bounds", "lgpu_debug_gemm",
-    "lgpu_debug_sub_batch_size", "lgpu_debug_select", "lgpu_last_stage_ms", "lgpu_set_profiling",
+    "lgpu_debug_sub_batch_size", "lgpu_debug_select", "lgpu_debug_select_large", "lgpu_last_stage_ms",
+    "lgpu_set_profiling",
     "lgpu_kernel_launch_count", "lgpu_last_filter_stats",
     "lgpu_binary_open", "lgpu_binary_close", "lgpu_binary_search", "lgpu_binary_search_filtered",
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
@@ -170,6 +173,7 @@ def load():
     lib.lgpu_debug_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
     lib.lgpu_debug_sub_batch_size.argtypes = [vp, u32, u32, C.POINTER(u32)]
     lib.lgpu_debug_select.argtypes = [C.POINTER(DebugSelectArgs), i32, vp]
+    lib.lgpu_debug_select_large.argtypes = [C.POINTER(DebugSelectArgs), i32, vp]
     lib.lgpu_last_stage_ms.argtypes = [vp]
     lib.lgpu_set_profiling.argtypes = [i32]
     lib.lgpu_kernel_launch_count.argtypes = [C.POINTER(C.c_uint64)]
@@ -737,6 +741,12 @@ def debug_select(device: int = 0, stream: int = 0, **args) -> None:
     """The top-k selection alone (lgpu_debug_select): `args` are lgpu_debug_select_args fields, device addresses as
     ints; enqueued on `stream`, not synchronised."""
     check(load().lgpu_debug_select(C.byref(DebugSelectArgs(**args)), device, stream))
+
+
+def debug_select_large(device: int = 0, stream: int = 0, **args) -> None:
+    """The large top-k selection alone (lgpu_debug_select_large, 2048 < k <= K_MAX): the arguments of debug_select;
+    synchronises `stream` before returning."""
+    check(load().lgpu_debug_select_large(C.byref(DebugSelectArgs(**args)), device, stream))
 
 
 def debug_gemm(queries, vectors, device: int = 0) -> np.ndarray:

@@ -132,6 +132,7 @@ struct Workspace {
     DevBuf sq_q, sq_qq;                 // IVF_SQ search: query codes [B][dim_pad], their squared sums
     DevBuf rq_q, rq_planes, rq_slots;   // IVF_RQ search: rotated queries [B][dim], per-slot bit-planes and grids
     DevBuf pq4_tab, pq4_slots;          // 4-bit IVF_PQ search: per-slot u8 tables [slots][m][16] and quantisers
+    DevBuf sel_large;                   // the large select's scratch (k > SELECT_KMAX, select_large.cu)
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -596,6 +597,22 @@ static void with_range(SelectArgs &s, const lgpu_search_params &sp)
 {
     s.has_lower = sp.has_lower; s.has_upper = sp.has_upper; s.lower = sp.lower; s.upper = sp.upper;
 }
+// k > SELECT_KMAX: the large select's scratch, from the workspace (nothing for k <= SELECT_KMAX)
+static SelectArgs &with_scratch(Workspace *ws, SelectArgs &s)
+{
+    if (s.k > SELECT_KMAX) {
+        s.scratch_bytes = select_large_scratch_bytes(s.B, s.k, s.out_pos != nullptr);
+        ws->sel_large.ensure(s.scratch_bytes);
+        s.scratch = ws->sel_large.p;
+    }
+    return s;
+}
+// workspace bytes per query that grow with k: the large select's scratch above SELECT_KMAX (below it, every per-query
+// buffer is bounded by SELECT_KMAX entries and stays outside the sub-batch budget, DESIGN.md section 2)
+static size_t large_k_query_bytes(uint32_t k)
+{
+    return k > SELECT_KMAX ? select_large_scratch_bytes(1, k, true) : 0;
+}
 
 // The tail of tc_topk_l2 and tc_topk_l2_filtered: exact re-score of the [B][cap] candidate slots (ws->t_pos, t_ids;
 // one pair per slot, empty slots included), their top-k into the outputs, then the dense fix-up of the queries
@@ -677,26 +694,30 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
 
 // top-k by (distance, id) of the dense scores D [b][ld] over N columns, with the request's distance range and
 // prefilter, into `out`
-static void select_dense(const float *D, uint64_t N, uint64_t ld, const uint64_t *col_ids, uint32_t b,
+static void select_dense(Workspace *ws, const float *D, uint64_t N, uint64_t ld, const uint64_t *col_ids, uint32_t b,
                          const lgpu_search_params &sp, RowFilter rf, TopkOut out, cudaStream_t st)
 {
     SelectArgs sa = select_rows(D, N, ld, b, sp.k, out);
     sa.col_ids = col_ids;
     with_range(sa, sp);
     sa.allow = rf.bits; sa.allow_bits = rf.nbits;
-    launch_select(sa, st);
+    launch_select(with_scratch(ws, sa), st);
 }
 
 // the arguments every search call takes: the parameters, then the query and output buffers of a call with queries.
-// refine: the kind selects k * refine_factor candidates (a kind whose distances are exact ignores refine_factor)
+// k = limit + offset, and k * refine_factor when the kind re-ranks, go up to LGPU_K_MAX on every single-GPU search:
+// up to SELECT_KMAX on the shared-memory selects, above it on the large select (select_large.cu) over the kind's exact
+// route.  refine: the kind selects k * refine_factor candidates (a kind whose distances are exact ignores
+// refine_factor).  The sharded search adds its own bound (SELECT_KMAX, check_sharded_call).
 static void check_call(const lgpu_search_params *p, uint32_t B, const void *q, const void *ids, const void *dist,
                        const void *cnt, bool refine = true)
 {
     LGPU_REQUIRE(p != nullptr, "search params are null");
     LGPU_REQUIRE(p->k >= 1, "limit must be greater than 0");
-    LGPU_REQUIRE(p->k <= SELECT_KMAX, "limit+offset above 2048 is not supported on the GPU path");
+    LGPU_REQUIRE(p->k <= LGPU_K_MAX, "limit+offset above 65536 (LGPU_K_MAX) is not supported");
     if (refine && p->refine_factor)
-        LGPU_REQUIRE((uint64_t)p->k * p->refine_factor <= SELECT_KMAX, "limit*refine_factor above 2048 is not supported");
+        LGPU_REQUIRE((uint64_t)p->k * p->refine_factor <= LGPU_K_MAX,
+                     "limit*refine_factor above 65536 (LGPU_K_MAX) is not supported");
     LGPU_REQUIRE(B == 0 || (q && ids && dist && cnt), "null buffer");
 }
 
@@ -779,6 +800,9 @@ static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, cons
     const uint32_t nlist = ix->nlist;
     p.B = B; p.nprobes = nprobes; p.slots = B * nprobes; p.np_eff = std::min(nprobes, nlist);
     p.k = sp.k; p.kk = sp.refine_factor ? sp.k * sp.refine_factor : sp.k; p.refine = sp.refine_factor != 0;
+    // kk above SELECT_KMAX: the exact scan (or the small path) feeds every row to the large select; the filter scan's
+    // shortlists are sized to SELECT_KMAX (lb_short) and its candidate mode to CAND_TOPK_MAX
+    const bool large_k = p.kk > SELECT_KMAX;
     p.lb_short = p.kk <= 16 ? 32u : std::min<uint32_t>(SELECT_KMAX, 2 * p.kk + 32);
     // the bf16 error band around the nprobes-th centroid has to fit in the tensor-core shortlist: 3x nprobes (>= 64)
     // candidates (dense variant) or admission by threshold (list variant).  The tensor-core shortlist wins at every
@@ -805,7 +829,7 @@ static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, cons
     const bool small = !widening && p.slots <= modes.small_slots && small_scan_smem(ix->m, ix->dim) <= 200 * 1024 &&
                        (size_t)p.slots * ix->pad_prefix[1] * 4 <= workspace_budget();
     const bool filter = ix->has_tables && !modes.exact && !sp.has_lower && !sp.has_upper && p.lb_short > p.kk &&
-                        ix->m <= 512 && !widening && !small;
+                        ix->m <= 512 && !widening && !small && !large_k;
     if (small) p.scan = IvfScan::small;
     else if (!filter) p.scan = IvfScan::exact_pq;
     if (!filter) return p;
@@ -1019,7 +1043,7 @@ static void ivf_small(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
     mark(IVF_SCAN, st);
     SelectArgs sa = select_segments(ix, ws, p, p.kk, pq_out(ws, p, out), rf);
     with_range(sa, sp);
-    launch_select(sa, st);
+    launch_select(with_scratch(ws, sa), st);
     mark(IVF_TOPK, st);
 }
 
@@ -1243,7 +1267,7 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
     SelectArgs sa = select_segments(ix, ws, p, p.kk, pq, rf);
     sa.only = only;
     with_range(sa, sp);
-    launch_select(sa, st);
+    launch_select(with_scratch(ws, sa), st);
     mark(IVF_TOPK, st);
 }
 
@@ -1255,7 +1279,7 @@ static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const fl
                          ws->t_exact.as<float>(), st);
     SelectArgs sr = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), p.kk, p.B, p.k, out);
     sr.only = only;
-    launch_select(sr, st);
+    launch_select(with_scratch(ws, sr), st);
 }
 
 // one sub-batch of an IVF search, everything device-side on `st` (and `front`, joined).  only (device, [B]): redo just
@@ -1311,12 +1335,16 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const IvfQuer
     mark(IVF_REFINE, st);
 }
 
-uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes)
+// kk: the PQ top-kk of the request (0: not known, lgpu_debug_sub_batch_size)
+uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32_t kk = 0)
 {
     uint32_t np_eff = std::min<uint32_t>(nprobes, ix->nlist);
-    // distance segments, coarse scores, the filter scan's per-query tables, then the kind's own buffers
+    // distance segments, coarse scores, the filter scan's per-query tables, then the kind's own buffers; above
+    // SELECT_KMAX the large select's scratch and the refine stage's [kk] candidates (ids, distances, positions, exact
+    // distances) grow with kk and count too
     size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4) +
-                   ivf_kind_query_bytes(ix, nprobes, np_eff);
+                   ivf_kind_query_bytes(ix, nprobes, np_eff) + large_k_query_bytes(kk) +
+                   (kk > SELECT_KMAX ? (size_t)kk * 28 : 0);
     size_t bs = workspace_budget() / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
     bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
@@ -1386,7 +1414,8 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const voi
     if (widen)
         LGPU_REQUIRE(np_max <= SELECT_KMAX || np_max >= ix->nlist,
                      "maximum_nprobes above 2048 is not supported unless it covers every partition");
-    const uint32_t bs = ivf_sub_batch_size(ix, B, widen ? np_max : nprobes);
+    const uint32_t kk = sp.refine_factor && ix->kind != IvfKind::ham ? sp.k * sp.refine_factor : sp.k;
+    const uint32_t bs = ivf_sub_batch_size(ix, B, widen ? np_max : nprobes, kk);
     const bool prof = profiling_enabled();
     if (prof) {
         memset(g_stage_ms, 0, sizeof(g_stage_ms));
@@ -1423,7 +1452,7 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
             fl->has_norms = true;
         }
     }
-    size_t per_q = std::max<size_t>(ld * 4, 4);
+    size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(sp.k);
     uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(workspace_budget() / per_q, B));
     const TopkOut out{d_ids, d_dist, d_cnt};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
@@ -1438,9 +1467,10 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
             xn = ws->xnorm.as<float>();
         }
         const uint32_t kp = (uint32_t)std::min<uint64_t>(N, std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(8 * sp.k, 256)));
-        // (a prefilter goes through the exact kernels: the shortlist thresholds are fixed on unfiltered rows)
+        // (a prefilter goes through the exact kernels: the shortlist thresholds are fixed on unfiltered rows, and so
+        // does k above SELECT_KMAX: the shortlists are sized to SELECT_KMAX)
         if (fl->has_tc && tc_enabled() && metric == LGPU_L2 && !sp.has_lower && !sp.has_upper && b >= 8 && N >= 4096 &&
-            !rf.bits) {
+            !rf.bits && sp.k <= SELECT_KMAX) {
             if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
                 tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p,
                                     fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
@@ -1454,7 +1484,7 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
         }
         launch_dist_matrix(q, fl->vectors.as<float>(), b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
                            xn, fl->ysqrt.as<float>(), ws->D.as<float>(), ld, st);
-        select_dense(ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
+        select_dense(ws, ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
                      out.at(q0, sp.k), st);
     }
 }
@@ -1532,7 +1562,8 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     launch_ham_pack(d_q, bx->nbytes, bx->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
     const uint8_t *Q = ws->hq.as<uint8_t>();
     const bool tc_ok = tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper;
-    const bool list = tc_ok && bx->nsample > 0;
+    // k above SELECT_KMAX: a dense path (the list path's capacity stops at 16384 rows)
+    const bool list = tc_ok && bx->nsample > 0 && k <= SELECT_KMAX;
     const bool tc = list || (tc_ok && B >= HAM_TC_MIN_B && N >= HAM_TC_MIN_N);
     const size_t budget = workspace_budget();
     if (list) {
@@ -1565,7 +1596,8 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
             }
         }
     } else {
-        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / std::max<size_t>(ld * 4, 4), B));
+        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
+        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / per_q, B));
         for (uint32_t q0 = 0; q0 < B; q0 += bs) {
             const uint32_t b = std::min(bs, B - q0);
             if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
@@ -1576,7 +1608,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
             else
                 launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld,
                                  bx->num_sms, st);
-            select_dense(ws->D.as<float>(), N, ld, col_ids, b, sp, rf, out.at(q0, k), st);
+            select_dense(ws, ws->D.as<float>(), N, ld, col_ids, b, sp, rf, out.at(q0, k), st);
         }
     }
     if (prof) {                     // [1] distances computed on the tensor cores, [3] queries
@@ -1664,7 +1696,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
     uint32_t max_nq = 0;
     for (uint32_t b = 0; b < B; b++) max_nq = std::max(max_nq, h_qoff[b + 1] - h_qoff[b]);
     const size_t quarter = budget / 4;
-    const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper &&
+    const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper && k <= SELECT_KMAX &&
                     (size_t)(max_nq + 1) * ld * 4 <= quarter;
     if (tc) {
         // fp16 normalised queries (and the queries holding a bad vector), then sub-batches of whole queries whose scores
@@ -1729,13 +1761,15 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             qa = qb;
         }
     } else {
-        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / 2 / std::max<size_t>(ld * 4, 4), B));
+        // (half the budget goes to the distance blocks of mv_exact_dense)
+        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
+        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / 2 / per_q, B));
         for (uint32_t qa = 0; qa < B; qa += bs) {
             const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
             mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld);
-            select_dense(ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
+            select_dense(ws, ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
                          out.at(qa, k), st);
         }
     }
@@ -2498,57 +2532,79 @@ int lgpu_debug_sub_batch_size(lgpu_index *ixh, uint32_t B, uint32_t nprobes, uin
     });
 }
 
+// lgpu_debug_select(_large): the checks of the arguments (k_lo <= k <= k_hi) and the SelectArgs they describe
+static SelectArgs debug_select_args(const lgpu_debug_select_args *a, int device, cudaStream_t st, uint32_t k_lo,
+                                    uint32_t k_hi, const char *k_msg)
+{
+    LGPU_REQUIRE(a != nullptr, "null argument");
+    LGPU_REQUIRE(a->mode >= 0 && a->mode <= 2, "select mode must be 0, 1 or 2");
+    LGPU_REQUIRE(a->k >= k_lo && a->k <= k_hi, k_msg);
+    auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    LGPU_REQUIRE(a->out_count && (a->out_rec || (a->out_ids && a->out_dist)), "null output buffer");
+    LGPU_REQUIRE(a16(a->out_rec), "out_rec must be 16-byte aligned");
+    if (a->mode == 0) {
+        LGPU_REQUIRE(a->dist && a->seg_off && a->probes && a->part_n && a->part_off, "null mode-0 buffer");
+        LGPU_REQUIRE(a16(a->dist), "mode 0: dist must be 16-byte aligned");   // float4 loads
+    } else if (a->mode == 1) {
+        LGPU_REQUIRE(a->dense, "null mode-1 buffer");
+    } else {
+        LGPU_REQUIRE(a->cand_rec || (a->dense && a->cand_ids), "null mode-2 buffer");
+        LGPU_REQUIRE(a16(a->cand_rec), "cand_rec must be 16-byte aligned");
+        LGPU_REQUIRE(a->inner >= 1, "mode 2: inner must be at least 1");
+    }
+    require_device(device);
+    if (a->mode == 0 && a->B > 0 && a->nprobes > 0) {
+        // the kernels load every probed segment as float4 up to its length rounded up to 4
+        const size_t ns = (size_t)a->B * a->nprobes;
+        std::vector<uint64_t> probes(ns), seg(ns);
+        std::vector<uint32_t> part_n(a->nlist);
+        LGPU_CUDA(cudaStreamSynchronize(st));
+        LGPU_CUDA(cudaMemcpy(probes.data(), a->probes, ns * 8, cudaMemcpyDeviceToHost));
+        LGPU_CUDA(cudaMemcpy(seg.data(), a->seg_off, ns * 8, cudaMemcpyDeviceToHost));
+        if (a->nlist) LGPU_CUDA(cudaMemcpy(part_n.data(), a->part_n, (size_t)a->nlist * 4, cudaMemcpyDeviceToHost));
+        for (size_t s = 0; s < ns; s++) {
+            if (probes[s] >= a->nlist) continue;
+            LGPU_REQUIRE(seg[s] % 4 == 0, "mode 0: seg_off must be a multiple of 4");
+            LGPU_REQUIRE(seg[s] <= a->dist_len && round_up64(part_n[probes[s]], 4) <= a->dist_len - seg[s],
+                         "mode 0: a segment padded to 4 floats runs past dist_len");
+        }
+    }
+    SelectArgs s{};
+    s.mode = a->mode;
+    s.dist = a->dist; s.seg_off = a->seg_off; s.probes = a->probes; s.nprobes = a->nprobes; s.nlist = a->nlist;
+    s.part_n = a->part_n; s.part_off = a->part_off; s.row_ids = a->row_ids;
+    s.dense = a->dense; s.ncols = a->ncols; s.row_stride = a->row_stride;
+    s.inner = a->inner; s.outer_stride = a->outer_stride;
+    s.col_ids = a->col_ids; s.cand_ids = a->cand_ids; s.cand_pos = a->cand_pos; s.ncols_q = a->ncols_q;
+    s.cand_rec = static_cast<const TopkRecord *>(a->cand_rec);
+    s.B = a->B; s.k = a->k;
+    s.has_lower = a->has_lower; s.has_upper = a->has_upper; s.lower = a->lower; s.upper = a->upper;
+    s.out_ids = a->out_ids; s.out_dist = a->out_dist; s.out_count = a->out_count;
+    s.out_rec = static_cast<TopkRecord *>(a->out_rec); s.out_pos = a->out_pos;
+    s.only = a->only; s.gate = a->gate; s.allow = a->allow; s.allow_bits = a->allow_bits;
+    return s;
+}
+
 int lgpu_debug_select(const lgpu_debug_select_args *a, int device, void *cuda_stream)
 {
     return guarded([&] {
-        LGPU_REQUIRE(a != nullptr, "null argument");
-        LGPU_REQUIRE(a->mode >= 0 && a->mode <= 2, "select mode must be 0, 1 or 2");
-        LGPU_REQUIRE(a->k >= 1 && a->k <= SELECT_KMAX, "k must be in [1, 2048]");
-        auto a16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-        LGPU_REQUIRE(a->out_count && (a->out_rec || (a->out_ids && a->out_dist)), "null output buffer");
-        LGPU_REQUIRE(a16(a->out_rec), "out_rec must be 16-byte aligned");
-        if (a->mode == 0) {
-            LGPU_REQUIRE(a->dist && a->seg_off && a->probes && a->part_n && a->part_off, "null mode-0 buffer");
-            LGPU_REQUIRE(a16(a->dist), "mode 0: dist must be 16-byte aligned");   // float4 loads
-        } else if (a->mode == 1) {
-            LGPU_REQUIRE(a->dense, "null mode-1 buffer");
-        } else {
-            LGPU_REQUIRE(a->cand_rec || (a->dense && a->cand_ids), "null mode-2 buffer");
-            LGPU_REQUIRE(a16(a->cand_rec), "cand_rec must be 16-byte aligned");
-            LGPU_REQUIRE(a->inner >= 1, "mode 2: inner must be at least 1");
-        }
-        require_device(device);
         cudaStream_t st = (cudaStream_t)cuda_stream;
-        if (a->mode == 0 && a->B > 0 && a->nprobes > 0) {
-            // the kernels load every probed segment as float4 up to its length rounded up to 4
-            const size_t ns = (size_t)a->B * a->nprobes;
-            std::vector<uint64_t> probes(ns), seg(ns);
-            std::vector<uint32_t> part_n(a->nlist);
-            LGPU_CUDA(cudaStreamSynchronize(st));
-            LGPU_CUDA(cudaMemcpy(probes.data(), a->probes, ns * 8, cudaMemcpyDeviceToHost));
-            LGPU_CUDA(cudaMemcpy(seg.data(), a->seg_off, ns * 8, cudaMemcpyDeviceToHost));
-            if (a->nlist) LGPU_CUDA(cudaMemcpy(part_n.data(), a->part_n, (size_t)a->nlist * 4, cudaMemcpyDeviceToHost));
-            for (size_t s = 0; s < ns; s++) {
-                if (probes[s] >= a->nlist) continue;
-                LGPU_REQUIRE(seg[s] % 4 == 0, "mode 0: seg_off must be a multiple of 4");
-                LGPU_REQUIRE(seg[s] <= a->dist_len && round_up64(part_n[probes[s]], 4) <= a->dist_len - seg[s],
-                             "mode 0: a segment padded to 4 floats runs past dist_len");
-            }
-        }
-        SelectArgs s{};
-        s.mode = a->mode;
-        s.dist = a->dist; s.seg_off = a->seg_off; s.probes = a->probes; s.nprobes = a->nprobes; s.nlist = a->nlist;
-        s.part_n = a->part_n; s.part_off = a->part_off; s.row_ids = a->row_ids;
-        s.dense = a->dense; s.ncols = a->ncols; s.row_stride = a->row_stride;
-        s.inner = a->inner; s.outer_stride = a->outer_stride;
-        s.col_ids = a->col_ids; s.cand_ids = a->cand_ids; s.cand_pos = a->cand_pos; s.ncols_q = a->ncols_q;
-        s.cand_rec = static_cast<const TopkRecord *>(a->cand_rec);
-        s.B = a->B; s.k = a->k;
-        s.has_lower = a->has_lower; s.has_upper = a->has_upper; s.lower = a->lower; s.upper = a->upper;
-        s.out_ids = a->out_ids; s.out_dist = a->out_dist; s.out_count = a->out_count;
-        s.out_rec = static_cast<TopkRecord *>(a->out_rec); s.out_pos = a->out_pos;
-        s.only = a->only; s.gate = a->gate; s.allow = a->allow; s.allow_bits = a->allow_bits;
-        launch_select(s, st);
+        launch_select(debug_select_args(a, device, st, 1, SELECT_KMAX, "k must be in [1, 2048]"), st);
+    });
+}
+
+int lgpu_debug_select_large(const lgpu_debug_select_args *a, int device, void *cuda_stream)
+{
+    return guarded([&] {
+        cudaStream_t st = (cudaStream_t)cuda_stream;
+        SelectArgs s = debug_select_args(a, device, st, SELECT_KMAX + 1, LGPU_K_MAX,
+                                         "k must be in [2049, 65536] (above 2048, at most LGPU_K_MAX)");
+        DevBuf scratch;
+        s.scratch_bytes = select_large_scratch_bytes(s.B, s.k, s.out_pos != nullptr);
+        scratch.ensure(s.scratch_bytes);
+        s.scratch = scratch.p;
+        launch_select_large(s, st);
+        LGPU_CUDA(cudaStreamSynchronize(st));                // before the scratch is freed
     });
 }
 
@@ -3160,6 +3216,15 @@ int lgpu_comm_init(const void *unique_id, size_t id_bytes, int rank, int world, 
 
 void lgpu_comm_destroy(lgpu_comm *c) { close_handle(c); }
 
+// the sharded search's own bound on k: its merge (select mode 2 over world * k records) stays on the shared-memory
+// selects, k <= SELECT_KMAX
+static void check_sharded_call(lgpu_index *ix, const void *q, uint32_t B, const lgpu_search_params *p, const void *a,
+                               const void *b, const void *c)
+{
+    check_ivf_call(ix, q, B, p, a, b, c);
+    LGPU_REQUIRE(p->k <= SELECT_KMAX, "limit+offset above 2048 is not supported on the sharded path");
+}
+
 // local top-k on this rank's shard -> pack -> ONE all-gather of [B][k] 16-byte records -> merge, all on `st`
 static void sharded_search_device(lgpu_index *ix, lgpu_comm *c, Workspace *ws, cudaStream_t st, const float *d_q,
                                   uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist,
@@ -3198,7 +3263,7 @@ int lgpu_search_sharded(lgpu_index *ixh, lgpu_comm *ch, const float *queries, ui
         HandleRef<lgpu_index> ix(ixh);
         HandleRef<lgpu_comm> c(ch);
         LGPU_REQUIRE(ix->kind == IvfKind::pq8, "sharded search serves 8-bit IVF_PQ indexes only");
-        check_ivf_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
+        check_sharded_call(ix.h, queries, B, params, out_ids, out_dist, out_count);
         if (B == 0) return;
         require_device(ix->device);
         host_call(ix->pool, queries, (size_t)B * ix->dim, B, params->k, out_ids, out_dist, out_count, nullptr,
@@ -3216,7 +3281,7 @@ int lgpu_search_sharded_device(lgpu_index *ixh, lgpu_comm *ch, const float *d_qu
         HandleRef<lgpu_index> ix(ixh);
         HandleRef<lgpu_comm> c(ch);
         LGPU_REQUIRE(ix->kind == IvfKind::pq8, "sharded search serves 8-bit IVF_PQ indexes only");
-        check_ivf_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
+        check_sharded_call(ix.h, d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
         if (B == 0) return;
         require_device(ix->device);
         WsLease lease(ix->pool, (cudaStream_t)cuda_stream, true);

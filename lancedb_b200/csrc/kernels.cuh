@@ -305,8 +305,15 @@ struct SelectArgs {
     // >= allow_bits) is dropped before it can enter the top-k
     const uint32_t *allow;
     uint64_t allow_bits;
+    // k > SELECT_KMAX (select_large.cu): device scratch of at least select_large_scratch_bytes(B, k, out_pos != NULL)
+    void *scratch;
+    size_t scratch_bytes;
 };
+// k <= SELECT_KMAX: select.cu; SELECT_KMAX < k <= LGPU_K_MAX: launch_select_large
 void launch_select(const SelectArgs &a, cudaStream_t st);
+// the global-memory radix top-k (select_large.cu): same contract as the small selects, any k in (SELECT_KMAX, LGPU_K_MAX]
+void launch_select_large(const SelectArgs &a, cudaStream_t st);
+size_t select_large_scratch_bytes(uint32_t B, uint32_t k, bool pos);
 // flags[q] = cnt[q] < k (maximum_nprobes widening: the queries that did not find k rows)
 void launch_count_below(const uint32_t *cnt, uint32_t B, uint32_t k, uint32_t *flags, cudaStream_t st);
 // rec[i] = (ids[i], dist[i]) for i < n

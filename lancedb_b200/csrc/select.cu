@@ -434,7 +434,8 @@ void launch_pack_records(const uint64_t *ids, const float *dist, uint64_t n, Top
 void launch_select(const SelectArgs &a, cudaStream_t st)
 {
     if (a.B == 0) return;
-    LGPU_REQUIRE(a.k >= 1 && a.k <= SELECT_KMAX, "limit+offset (k) must be in [1, 2048] on the GPU path");
+    if (a.k > SELECT_KMAX) { launch_select_large(a, st); return; }   // select_large.cu
+    LGPU_REQUIRE(a.k >= 1, "limit+offset (k) must be at least 1");
     // above k = 32 the warp queues' serial inserts (k ln(n/k) per warp) dominate: the shared-memory stage + bitonic
     // kernel is the faster one there
     if (a.k <= 32) {

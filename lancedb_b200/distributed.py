@@ -63,6 +63,14 @@ def exchange_unique_id(group=None) -> bytes:
     return box[0]
 
 
+def check_k(k: int) -> None:
+    """The sharded search serves k (limit + offset) up to SHARDED_K_MAX = 2048: its merge of world x k records per
+    query stays on the shared-memory selects.  Refused here, before any device work."""
+    if k > _native.SHARDED_K_MAX:
+        raise ValueError(f"limit + offset = {k} is above {_native.SHARDED_K_MAX}, the largest k the sharded search "
+                         "serves")
+
+
 class ShardedIvfPq:
     def __init__(self, data: IvfPqIndexData, *, group=None, device: Optional[int] = None, presharded: bool = False):
         import torch
@@ -85,6 +93,7 @@ class ShardedIvfPq:
     def search_device(self, d_q, k: int = 10, nprobes: int = 20, lower=None, upper=None):
         """d_q: [B, dim] float32 CUDA tensor (identical on every rank).  Returns CUDA tensors
         (ids int64 holding the u64 row ids, dist float32, count int32), identical on every rank."""
+        check_k(k)
         import torch
         B = d_q.shape[0]
         dev = d_q.device
@@ -98,4 +107,5 @@ class ShardedIvfPq:
 
     def search(self, queries, k: int = 10, nprobes: int = 20, lower=None, upper=None):
         """Host-buffer collective search through lgpu_search_sharded."""
+        check_k(k)
         return self.comm.search(self.local, queries, k=k, nprobes=nprobes, lower=lower, upper=upper)

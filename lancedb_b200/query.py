@@ -19,6 +19,7 @@ import numpy as np
 import pyarrow as pa
 
 from . import filter as _filter
+from ._native import K_MAX
 
 DEFAULT_TOP_K = 10          # rust/lancedb/src/query.rs:36
 DEFAULT_NPROBES = 20        # rust/lancedb/src/query.rs:1097-1113
@@ -134,6 +135,8 @@ class LanceVectorQueryBuilder:
     def _resolve(self):
         lim = self._limit if self._limit is not None else DEFAULT_TOP_K
         k = lim + self._offset                          # table/query.rs:231
+        if k > K_MAX:                                   # (k x refine_factor is checked by the kinds that re-rank)
+            raise ValueError(f"limit + offset = {k} is above {K_MAX} (LGPU_K_MAX), the largest k the GPU search serves")
         # The request starts at minimum_nprobes = 20, maximum_nprobes = Some(20) (query.rs:1097-1113) and the sync builder
         # is lowered onto it as python/python/lancedb/table.py:5777-5787 does: both set -> nprobes(min) then
         # maximum_nprobes(max); one set -> that setter alone, validated against the OTHER one's default of 20
