@@ -102,7 +102,8 @@ typedef struct {
     int32_t  has_upper;      /* distance_range upper bound, exclusive */
     float    lower;
     float    upper;
-    uint32_t flags;          /* reserved, 0 */
+    uint32_t ef;             /* IVF_HNSW_SQ: the search beam (query.rs:1290-1300); 0 = ceil(1.5 k).  Every other kind
+                                ignores it */
     uint32_t max_nprobes;    /* maximum_nprobes (query.rs:1250-1275): under a prefilter, queries that found fewer
                                 than k rows in their `nprobes` nearest partitions are searched again over their
                                 max_nprobes nearest; 0 or <= nprobes = no widening */
@@ -232,6 +233,39 @@ typedef struct {
     const float    *vectors;      /* optional [nrows][dim] raw vectors (refine_factor); NULL if absent */
 } lgpu_ivf_sq_desc;
 int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *desc, lgpu_index **out);
+
+/* ---- IVF_HNSW_SQ (lance `HnswSq`, python/python/tests/test_table.py:1565-1590): IVF_SQ's partitions, codes and
+ * distance, plus one HNSW graph per partition over its rows.  Positions are row indices within the partition.
+ * Search, per query [lance, recalled]: IVF_SQ's normalisation, coarse step and query codes; then in each probed
+ * partition, with rows ordered by (d, position) and d IVF_SQ's f32 distance:
+ *   - upper levels: from the partition's entry row on its top level, at each level >= 1 move to the best neighbour
+ *     while it is better than the current row; the row reached starts level 0;
+ *   - level 0: W = the ef' best rows seen (ef' = max(ef, kk), kk = k or k x refine_factor, ef = 0 meaning
+ *     ceil(1.5 k)), W = {start}; while W holds an unexpanded row, expand the best one: evaluate each of its level-0
+ *     neighbours and offer it to W;
+ *   - the partition contributes R, the kk best evaluated rows (the start row included) that pass the row filter
+ *     (distance_range, prefilter); traversal ignores the filter.
+ * The R lists are merged by (_distance, _rowid); refine_factor, maximum_nprobes, timeout_ms and every entry point are
+ * IVF_SQ's.  ef' above LGPU_HNSW_EF_MAX is LGPU_INVALID_INPUT.  lgpu_search_sharded*, lgpu_debug_filter_bounds and
+ * lgpu_debug_partition_distances reject the handle. */
+#define LGPU_HNSW_MAX_M 64        /* a level-0 list has at most 128 entries */
+#define LGPU_HNSW_MAX_LEVEL 15
+#define LGPU_HNSW_EF_MAX 2048     /* W lives in shared memory */
+#define LGPU_HNSW_NONE 0xFFFFFFFFu
+/* Positions are below 2^31: every IVF open refuses a partition of 2^31 rows or more. */
+typedef struct {
+    lgpu_ivf_sq_desc sq;          /* the IVF_SQ arrays */
+    uint32_t m;                   /* 1 .. LGPU_HNSW_MAX_M: level-0 lists hold 2m entries, upper lists m */
+    uint32_t reserved;            /* 0 */
+    uint64_t upper_blocks;        /* rows of upper_adj */
+    const uint8_t  *levels;       /* [nrows] level of each row, <= its partition's top_level */
+    const uint32_t *adj0;         /* [nrows][2m] level-0 neighbour positions, LGPU_HNSW_NONE padded */
+    const uint32_t *upper_index;  /* [nrows] first upper_adj block of a row with level >= 1 (level L at + L - 1) */
+    const uint32_t *upper_adj;    /* [upper_blocks][m] neighbours at level L, each of level >= L, LGPU_HNSW_NONE padded */
+    const uint32_t *entry;        /* [nlist] entry row of each non-empty partition; its level is top_level */
+    const uint8_t  *top_level;    /* [nlist] <= LGPU_HNSW_MAX_LEVEL */
+} lgpu_ivf_hnsw_sq_desc;
+int lgpu_ivf_hnsw_sq_open(const lgpu_ivf_hnsw_sq_desc *desc, lgpu_index **out);
 
 /* ---- IVF_RQ (lance `IvfRq`, RaBitQ with num_bits = 1; rust/lancedb/src/index/vector.rs:321-369): the same IVF
  * partitions, each row stored as one sign bit per dimension of its rotated residual plus two f32 factors.  With P the

@@ -40,7 +40,7 @@ EXPORTS = [
     "lgpu_binary_search_device", "lgpu_debug_hamming_gemm",
     "lgpu_multivec_open", "lgpu_multivec_close", "lgpu_multivec_search", "lgpu_multivec_search_filtered",
     "lgpu_multivec_search_device", "lgpu_debug_maxsim_gemm",
-    "lgpu_ivf_sq_open", "lgpu_debug_sq_distances",
+    "lgpu_ivf_sq_open", "lgpu_debug_sq_distances", "lgpu_ivf_hnsw_sq_open",
     "lgpu_ivf_rq_open", "lgpu_debug_rq_distances",
     "lgpu_debug_pq4_sums",
     "lgpu_ivf_binary_open", "lgpu_ivf_binary_close", "lgpu_ivf_binary_search", "lgpu_ivf_binary_search_filtered",
@@ -69,6 +69,18 @@ class SqDesc(C.Structure):
         ("centroids", C.c_void_p), ("part_offsets", C.c_void_p), ("codes", C.c_void_p), ("row_ids", C.c_void_p),
         ("vectors", C.c_void_p),
     ]
+
+
+class HnswSqDesc(C.Structure):
+    """lgpu_ivf_hnsw_sq_desc"""
+    _fields_ = [
+        ("sq", SqDesc), ("m", C.c_uint32), ("reserved", C.c_uint32), ("upper_blocks", C.c_uint64),
+        ("levels", C.c_void_p), ("adj0", C.c_void_p), ("upper_index", C.c_void_p), ("upper_adj", C.c_void_p),
+        ("entry", C.c_void_p), ("top_level", C.c_void_p),
+    ]
+
+
+HNSW_EF_MAX = 2048              # LGPU_HNSW_EF_MAX: largest ef' = max(ef, k x refine_factor) of an IVF_HNSW_SQ search
 
 
 class RqDesc(C.Structure):
@@ -109,7 +121,7 @@ class SearchParams(C.Structure):
     _fields_ = [
         ("k", C.c_uint32), ("nprobes", C.c_uint32), ("refine_factor", C.c_uint32),
         ("has_lower", C.c_int32), ("has_upper", C.c_int32), ("lower", C.c_float), ("upper", C.c_float),
-        ("flags", C.c_uint32), ("max_nprobes", C.c_uint32), ("timeout_ms", C.c_uint32),
+        ("ef", C.c_uint32), ("max_nprobes", C.c_uint32), ("timeout_ms", C.c_uint32),
     ]
 
 
@@ -193,6 +205,7 @@ def load():
     lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_sq_open.argtypes = [C.POINTER(SqDesc), C.POINTER(vp)]
     lib.lgpu_debug_sq_distances.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
+    lib.lgpu_ivf_hnsw_sq_open.argtypes = [C.POINTER(HnswSqDesc), C.POINTER(vp)]
     lib.lgpu_ivf_rq_open.argtypes = [C.POINTER(RqDesc), C.POINTER(vp)]
     lib.lgpu_debug_rq_distances.argtypes = [vp, u32, vp, vp, vp, C.c_uint64, u32, i32, i32, vp, vp]
     lib.lgpu_debug_pq4_sums.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
@@ -237,9 +250,10 @@ def _ptr(a: Optional[np.ndarray]):
 
 
 def make_params(k=10, nprobes=20, refine_factor=0, lower=None, upper=None, max_nprobes=0,
-                timeout_ms=0) -> SearchParams:
+                timeout_ms=0, ef=0) -> SearchParams:
+    """ef: IVF_HNSW_SQ's search beam (0 = ceil(1.5 k)); every other kind ignores it."""
     return SearchParams(int(k), int(nprobes), int(refine_factor or 0), lower is not None, upper is not None,
-                        0.0 if lower is None else float(lower), 0.0 if upper is None else float(upper), 0,
+                        0.0 if lower is None else float(lower), 0.0 if upper is None else float(upper), int(ef or 0),
                         int(max_nprobes or 0), int(timeout_ms or 0))
 
 
@@ -326,11 +340,11 @@ class GpuIvfPq(_Handle):
         return b.value
 
     def search(self, queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None, allow=None, allow_bits=0,
-               max_nprobes=0, timeout_ms=0):
+               max_nprobes=0, timeout_ms=0, ef=0):
         """Host-buffer search: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32).
-        `allow` (u32 bitmap over row ids, `allow_bits` bits) = prefilter allow-list."""
+        `allow` (u32 bitmap over row ids, `allow_bits` bits) = prefilter allow-list.  ef: IVF_HNSW_SQ only."""
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
-        p = make_params(k, nprobes, refine_factor, lower, upper, max_nprobes, timeout_ms)
+        p = make_params(k, nprobes, refine_factor, lower, upper, max_nprobes, timeout_ms, ef)
         return _host_search("lgpu_search", (self._h, _ptr(q), q.shape[0]), q.shape[0], k, p, allow, allow_bits)
 
     def search_into(self, q: np.ndarray, p: SearchParams, ids: np.ndarray, dist: np.ndarray, cnt: np.ndarray):
@@ -338,12 +352,12 @@ class GpuIvfPq(_Handle):
         check(load().lgpu_search(self._h, q.ctypes.data, q.shape[0], C.byref(p), ids.ctypes.data,
                                  dist.ctypes.data, cnt.ctypes.data))
 
-    def search_one(self, query, k=10, nprobes=20, refine_factor=0):
+    def search_one(self, query, k=10, nprobes=20, refine_factor=0, ef=0):
         """One query vector through the micro-batcher (lgpu_search_coalesced): concurrent callers share a batch.
         ctypes releases the GIL for the duration of the call, so Python threads do coalesce."""
         q = np.ascontiguousarray(query, np.float32).reshape(self.dim)
         ids = np.empty(k, np.uint64); dist = np.empty(k, np.float32); cnt = np.zeros(1, np.uint32)
-        p = make_params(k, nprobes, refine_factor)
+        p = make_params(k, nprobes, refine_factor, ef=ef)
         check(load().lgpu_search_coalesced(self._h, _ptr(q), C.byref(p), _ptr(ids), _ptr(dist), _ptr(cnt)))
         return ids, dist, int(cnt[0])
 
@@ -412,6 +426,35 @@ class GpuIvfSq(GpuIvfPq):
                       _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]))
         h = C.c_void_p()
         check(lib.lgpu_ivf_sq_open(C.byref(desc), C.byref(h)))
+        self._h = h
+        self.has_vectors = vec is not None
+
+
+class GpuIvfHnswSq(GpuIvfPq):
+    """An IVF_HNSW_SQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_hnsw_sq_open (IVF_SQ's arrays plus the
+    per-partition HNSW graphs), so every search entry point of GpuIvfPq serves it; `ef` sets the search beam."""
+
+    def __init__(self, data, device: int = 0, with_vectors: bool = True):
+        lib = load()
+        sq = data.sq
+        if sq.metric not in ("l2", "cosine"):
+            raise ValueError(f"IVF_HNSW_SQ supports the l2 and cosine distance types, not {sq.metric!r}")
+        sq.validate()
+        self.dim, self.nlist, self.metric, self.m = sq.dim, sq.nlist, sq.metric, int(data.m)
+        self.lo, self.hi = float(sq.lo), float(sq.hi)
+        self.device = device
+        vec = sq.vectors if with_vectors else None
+        keep = [np.ascontiguousarray(sq.centroids, np.float32), np.ascontiguousarray(sq.part_offsets, np.uint64),
+                np.ascontiguousarray(sq.codes, np.uint8), np.ascontiguousarray(sq.row_ids, np.uint64),
+                None if vec is None else np.ascontiguousarray(vec, np.float32),
+                np.ascontiguousarray(data.levels, np.uint8), np.ascontiguousarray(data.adj0, np.uint32),
+                np.ascontiguousarray(data.upper_index, np.uint32), np.ascontiguousarray(data.upper_adj, np.uint32),
+                np.ascontiguousarray(data.entry, np.uint32), np.ascontiguousarray(data.top_level, np.uint8)]
+        desc = HnswSqDesc(SqDesc(ABI_VERSION, sq.dim, sq.nlist, METRICS[sq.metric], device, 0, sq.nrows, self.lo,
+                                 self.hi, *[_ptr(a) for a in keep[:5]]),
+                          self.m, 0, keep[8].shape[0], *[_ptr(a) for a in keep[5:]])
+        h = C.c_void_p()
+        check(lib.lgpu_ivf_hnsw_sq_open(C.byref(desc), C.byref(h)))
         self._h = h
         self.has_vectors = vec is not None
 

@@ -46,6 +46,18 @@ class IvfRq:
 
 
 @dataclass
+class HnswSq:
+    """Index.HnswSq parameters (python/python/lancedb/index.py, python/python/tests/test_table.py:1565-1590): IVF
+    partitions of 8-bit scalar codes with an HNSW graph in each; builds an IVF_HNSW_SQ index."""
+    distance_type: str = "l2"
+    num_partitions: Optional[int] = None
+    m: int = 20
+    ef_construction: int = 300
+    max_iterations: int = 50
+    sample_rate: int = 256
+
+
+@dataclass
 class IvfFlat:
     """Index.IvfFlat parameters (rust/lancedb/src/index/vector.rs:169-209): served over binary (fixed_size_list<uint8>)
     columns with distance_type="hamming"; the default "l2", like any other metric there, is refused (ValueError), and a
@@ -167,6 +179,7 @@ class AsyncVectorQuery(_AsyncQueryBase):
         self._lower: Optional[float] = None
         self._upper: Optional[float] = None
         self._refine_factor: Optional[int] = None
+        self._ef: Optional[int] = None
         self._use_index = True
 
     def add_query_vector(self, vector):
@@ -204,7 +217,8 @@ class AsyncVectorQuery(_AsyncQueryBase):
         self._lower, self._upper = lower_bound, upper_bound
         return self
 
-    def ef(self, ef: int):                       # HNSW only: no effect on IVF_PQ (query.py:3642-3655)
+    def ef(self, ef: int):                       # HNSW only: no effect on the other kinds (query.py:3642-3655)
+        self._ef = ef
         return self
 
     def refine_factor(self, refine_factor: int):
@@ -232,6 +246,8 @@ class AsyncVectorQuery(_AsyncQueryBase):
             b.distance_range(self._lower, self._upper)
         if self._refine_factor is not None:
             b.refine_factor(self._refine_factor)
+        if self._ef is not None:
+            b.ef(self._ef)
         if self._limit is not None:
             b.limit(self._limit)
         if self._offset:
@@ -271,15 +287,17 @@ class AsyncTable:
     async def list_indices(self):
         return self._table.list_indices()
 
-    async def create_index(self, column: str, *, config: Optional[Union[IvfPq, IvfRq, IvfFlat]] = None,
+    async def create_index(self, column: str, *, config: Optional[Union[IvfPq, IvfRq, HnswSq, IvfFlat]] = None,
                            replace: bool = True, accelerator: Optional[str] = "cuda"):
         cfg = config or IvfPq()
-        kind = "IVF_RQ" if isinstance(cfg, IvfRq) else ("IVF_FLAT" if isinstance(cfg, IvfFlat) else "IVF_PQ")
+        kind = ("IVF_RQ" if isinstance(cfg, IvfRq) else "IVF_FLAT" if isinstance(cfg, IvfFlat) else
+                "IVF_HNSW_SQ" if isinstance(cfg, HnswSq) else "IVF_PQ")
+        hnsw = {"m": cfg.m, "ef_construction": cfg.ef_construction} if isinstance(cfg, HnswSq) else {}
         await asyncio.to_thread(
             self._table.create_index, metric=cfg.distance_type, num_partitions=cfg.num_partitions,
             num_sub_vectors=getattr(cfg, "num_sub_vectors", None), vector_column_name=column, replace=replace,
             accelerator=accelerator, index_type=kind, num_bits=getattr(cfg, "num_bits", 8),
-            max_iterations=cfg.max_iterations, sample_rate=cfg.sample_rate)
+            max_iterations=cfg.max_iterations, sample_rate=cfg.sample_rate, **hnsw)
 
     async def prewarm_index(self, name: str):
         return self._table.prewarm_index(name)

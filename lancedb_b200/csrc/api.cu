@@ -130,6 +130,7 @@ struct Workspace {
     DevBuf mv_qh, mv_qbad, mv_Mk, mv_A; // ... tensor-core path: fp16 queries, bad vectors, max-similarity keys, approx dist
     DevBuf mv_kd, mv_ki, mv_kc, mv_thr, mv_cnt, mv_cand, mv_flags, mv_vflags, mv_gate, mv_ex, mv_exid;   // shortlist
     DevBuf sq_q, sq_qq;                 // IVF_SQ search: query codes [B][dim_pad], their squared sums
+    DevBuf hn_ids, hn_dist, hn_pos, hn_ctr;   // IVF_HNSW_SQ search: each probe slot's R [slots][kk], the slot counter
     DevBuf rq_q, rq_planes, rq_slots;   // IVF_RQ search: rotated queries [B][dim], per-slot bit-planes and grids
     DevBuf pq4_tab, pq4_slots;          // 4-bit IVF_PQ search: per-slot u8 tables [slots][m][16] and quantisers
     DevBuf sel_large;                   // the large select's scratch (k > SELECT_KMAX, select_large.cu)
@@ -284,8 +285,9 @@ struct Coalescer {
 }  // namespace lgpu
 
 namespace lgpu {
-// the kinds of IVF index: 8-bit and 4-bit PQ codes, 8-bit scalar codes, 1-bit RaBitQ codes, packed binary rows
-enum class IvfKind { pq8, pq4, sq, rq, ham };
+// the kinds of IVF index: 8-bit and 4-bit PQ codes, 8-bit scalar codes (scanned, or searched by per-partition HNSW
+// graphs), 1-bit RaBitQ codes, packed binary rows
+enum class IvfKind { pq8, pq4, sq, hnsw_sq, rq, ham };
 }  // namespace lgpu
 
 struct lgpu_index {
@@ -312,6 +314,9 @@ struct lgpu_index {
     uint32_t dim_pad = 0;
     double sq_lo = 0.0, sq_hi = 0.0;
     DevBuf sq_xx;
+    // IVF_HNSW_SQ (lgpu_ivf_hnsw_sq_open): IVF_SQ's arrays plus the graph, lgpu_ivf_hnsw_sq_desc's layout
+    uint32_t hnsw_m = 0;
+    DevBuf hn_levels, hn_adj0, hn_upper_index, hn_upper_adj, hn_entry, hn_top;
     // IVF_RQ (lgpu_ivf_rq_open): `codes` holds [nrows][rq_wpr] u32 sign bits; the rotation, the rotated centroids and
     // the per-row factors and popcounts
     uint32_t rq_wpr = 0;
@@ -732,7 +737,7 @@ constexpr uint64_t HAM_TC_MIN_N = 4096;    // ... and this many rows (not measur
 // normalise] -> coarse step (probes) -> small scan | regroup -> filter scan + fix-up | exact scan + select -> [refine],
 // on the paths ivf_plan picks before any launch ----
 enum class Coarse { exact, tc_dense, tc_list };   // see ivf_coarse
-enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq, pq4, ham };
+enum class IvfScan { small, filter_cand, filter_dense, exact_pq, sq, rq, pq4, ham, hnsw };
 
 // bytes of one stored row, as the scan reads them (profiling: lgpu_last_scanned_code_bytes)
 static uint32_t ivf_row_bytes(const lgpu_index *ix)
@@ -740,7 +745,7 @@ static uint32_t ivf_row_bytes(const lgpu_index *ix)
     switch (ix->kind) {
     case IvfKind::pq8: return ix->m;
     case IvfKind::pq4: return ix->m / 2;
-    case IvfKind::sq: return ix->dim;
+    case IvfKind::sq: case IvfKind::hnsw_sq: return ix->dim;
     case IvfKind::rq: return ix->rq_wpr * 4;
     case IvfKind::ham: return ix->nbytes_pad;
     }
@@ -748,10 +753,12 @@ static uint32_t ivf_row_bytes(const lgpu_index *ix)
 }
 
 // workspace bytes per query of a sub-batch that only the kind uses: the per-slot u8 tables (pq4), the per-slot
-// bit-planes and the rotated query (rq), the probe slots' ids, distances, regroup and tile descriptors (ham)
-static size_t ivf_kind_query_bytes(const lgpu_index *ix, uint32_t nprobes, uint32_t np_eff)
+// bit-planes and the rotated query (rq), the probe slots' ids, distances, regroup and tile descriptors (ham), the probe
+// slots' [kk] result lists (hnsw_sq; kk = 0: not known, the largest)
+static size_t ivf_kind_query_bytes(const lgpu_index *ix, uint32_t nprobes, uint32_t np_eff, uint32_t kk)
 {
     switch (ix->kind) {
+    case IvfKind::hnsw_sq: return (size_t)nprobes * (kk ? kk : LGPU_HNSW_EF_MAX) * 20;
     case IvfKind::pq4: return (size_t)nprobes * (16 * ix->m + sizeof(Pq4Slot));
     case IvfKind::rq: return (size_t)nprobes * (16 * ix->rq_wpr + sizeof(RqSlot)) + (size_t)ix->dim * 4;
     case IvfKind::ham: return (size_t)np_eff * 36 + (size_t)np_eff * ix->max_nrb * (sizeof(TileDesc) / SCAN_G + 1) + 64;
@@ -781,6 +788,7 @@ struct IvfPlan {
     Coarse coarse;
     IvfScan scan;
     uint32_t cand_cap;        // candidate mode: candidates per query (power of two >= kk)
+    uint32_t efp;             // hnsw: W's capacity, ef' = max(ef, kk)
     bool filter() const { return scan == IvfScan::filter_cand || scan == IvfScan::filter_dense; }
     uint32_t rows_tile() const
     {
@@ -790,6 +798,13 @@ struct IvfPlan {
         return scan == IvfScan::sq ? SQ_ROWS_TILE : (scan == IvfScan::rq ? RQ_ROWS_TILE : SCAN_ROWS_TILE_MID);
     }
 };
+
+// IVF_HNSW_SQ's ef' = max(ef, kk), ef = 0 meaning ceil(1.5 k) (query.rs:1290-1300)
+static uint64_t hnsw_efp(const lgpu_search_params &sp)
+{
+    const uint64_t kk = sp.refine_factor ? (uint64_t)sp.k * sp.refine_factor : sp.k;
+    return std::max<uint64_t>(sp.ef ? sp.ef : (3ull * sp.k + 1) / 2, kk);
+}
 
 // prefilter: the request carries an allow bitmap; widening: the sub-batch redoes the queries flagged by the
 // maximum_nprobes widening (exact kernels only)
@@ -820,6 +835,7 @@ static IvfPlan ivf_plan(const lgpu_index *ix, uint32_t B, uint32_t nprobes, cons
     switch (ix->kind) {
     case IvfKind::pq4: p.scan = IvfScan::pq4; return p;
     case IvfKind::sq: p.scan = IvfScan::sq; return p;
+    case IvfKind::hnsw_sq: p.scan = IvfScan::hnsw; p.efp = hnsw_efp(sp); return p;
     case IvfKind::rq: p.scan = IvfScan::rq; return p;
     case IvfKind::ham: p.scan = IvfScan::ham; p.kk = p.k; p.refine = false; return p;
     case IvfKind::pq8: break;
@@ -1271,6 +1287,34 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
     mark(IVF_TOPK, st);
 }
 
+// IvfScan::hnsw: the graph search of every probe slot into its [kk] list (hnsw_scan.cu), then the top-kk over a query's
+// nprobes lists.  Each list already holds only rows that pass the row filter.
+static void ivf_hnsw(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp, RowFilter rf,
+                     const uint32_t *only, TopkOut pq, cudaStream_t st, const StageMarks &mark)
+{
+    const size_t n = (size_t)p.slots * p.kk;
+    ws->hn_ids.ensure(n * 8); ws->hn_dist.ensure(n * 4); ws->hn_pos.ensure(n * 8); ws->hn_ctr.ensure(16);
+    LGPU_CUDA(cudaMemsetAsync(ws->hn_ctr.p, 0, 4, st));
+    HnswArgs a{};
+    a.codes = ix->codes.as<uint8_t>(); a.qcodes = ws->sq_q.as<uint8_t>(); a.dim_pad = ix->dim_pad;
+    a.probes = ws->probes.as<uint64_t>(); a.slots = p.slots; a.nprobes = p.nprobes; a.nlist = ix->nlist;
+    a.part_off = ix->part_off.as<uint64_t>(); a.row_ids = ix->row_ids.as<uint64_t>();
+    a.levels = ix->hn_levels.as<uint8_t>(); a.adj0 = ix->hn_adj0.as<uint32_t>();
+    a.upper_index = ix->hn_upper_index.as<uint32_t>(); a.upper_adj = ix->hn_upper_adj.as<uint32_t>();
+    a.entry = ix->hn_entry.as<uint32_t>(); a.top_level = ix->hn_top.as<uint8_t>();
+    a.m = ix->hnsw_m; a.efp = p.efp; a.kk = p.kk;
+    a.has_lower = sp.has_lower; a.has_upper = sp.has_upper; a.lower = sp.lower; a.upper = sp.upper;
+    a.allow = rf.bits; a.allow_bits = rf.nbits; a.only = only;
+    a.counter = ws->hn_ctr.as<uint32_t>();
+    a.out_ids = ws->hn_ids.as<uint64_t>(); a.out_dist = ws->hn_dist.as<float>(); a.out_pos = ws->hn_pos.as<uint64_t>();
+    launch_hnsw_search(a, ix->num_sms, st);
+    mark(IVF_SCAN, st);
+    SelectArgs sa = select_cands(a.out_dist, a.out_ids, (uint64_t)p.nprobes * p.kk, p.B, p.kk, pq);
+    sa.cand_pos = a.out_pos; sa.only = only;
+    launch_select(sa, st);
+    mark(IVF_TOPK, st);
+}
+
 // refine (query.rs:1302-1332): exact distance of the k * refine_factor candidates (ws->t_*), re-sort into `out`
 static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *d_q, TopkOut out,
                        const uint32_t *only, cudaStream_t st)
@@ -1297,7 +1341,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const IvfQuer
     const float *qs = prep.f;
     const cudaStream_t cs = p.filter() ? fork_front(ix, ws, st, B) : st;   // the coarse step's and the regroup's
     ivf_coarse(ix, ws, p, prep, cs, st, mark);
-    if (p.scan == IvfScan::sq) {
+    if (p.scan == IvfScan::sq || p.scan == IvfScan::hnsw) {
         ws->sq_q.ensure((size_t)B * ix->dim_pad); ws->sq_qq.ensure((size_t)B * 4);
         launch_sq_encode(qs, B, ix->dim, ix->dim_pad, ix->sq_lo, ix->sq_hi, ws->sq_q.as<uint8_t>(),
                          ws->sq_qq.as<uint32_t>(), st);
@@ -1314,6 +1358,8 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const IvfQuer
     mark(IVF_PROBES, cs);
     if (p.scan == IvfScan::small) {
         ivf_small(ix, ws, p, sp, qs, rf, out, st, mark);
+    } else if (p.scan == IvfScan::hnsw) {
+        ivf_hnsw(ix, ws, p, sp, rf, only, pq_out(ws, p, out), st, mark);
     } else {
         const GroupArgs ga = ivf_regroup(ix, ws, p, only, cs);
         mark(IVF_REGROUP, cs);
@@ -1343,7 +1389,7 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32
     // SELECT_KMAX the large select's scratch and the refine stage's [kk] candidates (ids, distances, positions, exact
     // distances) grow with kk and count too
     size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4) +
-                   ivf_kind_query_bytes(ix, nprobes, np_eff) + large_k_query_bytes(kk) +
+                   ivf_kind_query_bytes(ix, nprobes, np_eff, kk) + large_k_query_bytes(kk) +
                    (kk > SELECT_KMAX ? (size_t)kk * 28 : 0);
     size_t bs = workspace_budget() / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
@@ -1919,7 +1965,9 @@ static inline void make_key(uint64_t (&key)[4], uint64_t tag, uint32_t B, const 
 {
     uint32_t lo, hi;
     memcpy(&lo, &p.lower, 4); memcpy(&hi, &p.upper, 4);
-    key[0] = tag ^ ((uint64_t)B << 32);
+    // tags are below 2^16; ef in bits 16..31 (values above 0xffff share a key: IVF_HNSW_SQ refuses ef above
+    // LGPU_HNSW_EF_MAX and every other kind ignores ef)
+    key[0] = tag ^ ((uint64_t)std::min<uint32_t>(p.ef, 0xffffu) << 16) ^ ((uint64_t)B << 32);
     key[1] = (uint64_t)p.k | ((uint64_t)p.nprobes << 32);
     key[2] = (uint64_t)p.refine_factor | ((uint64_t)(p.has_lower ? 1 : 0) << 32) | ((uint64_t)(p.has_upper ? 1 : 0) << 33) |
              ((uint64_t)(p.max_nprobes & 0x3fffffu) << 34);
@@ -2259,7 +2307,9 @@ static uint64_t index_device_bytes(const lgpu_index *ix)
     for (const DevBuf *b : {&ix->centroids, &ix->cb_tiled, &ix->codes, &ix->code_base, &ix->part_n, &ix->part_npad,
                             &ix->part_off, &ix->row_ids, &ix->vectors, &ix->row_R, &ix->rmax_bits, &ix->cb_n2,
                             &ix->cent_b, &ix->cent_n2, &ix->cent_sb, &ix->cent_sn2, &ix->sq_xx, &ix->rq_rot, &ix->rq_rc,
-                            &ix->rq_add, &ix->rq_scale, &ix->rq_popc, &ix->pq4_cb, &ix->cent_pop, &ix->row_pop})
+                            &ix->rq_add, &ix->rq_scale, &ix->rq_popc, &ix->pq4_cb, &ix->cent_pop, &ix->row_pop,
+                            &ix->hn_levels, &ix->hn_adj0, &ix->hn_upper_index, &ix->hn_upper_adj, &ix->hn_entry,
+                            &ix->hn_top})
         n += b->bytes;
     return n;
 }
@@ -2354,6 +2404,72 @@ int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
         ix->sq_lo = d->lo; ix->sq_hi = d->hi;
         open_ivf_common(ix, d, SQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
         upload_sq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->sq_xx);
+    });
+}
+
+// IVF_HNSW_SQ's graph, checked on the host before any device work: every position in its partition, every upper-level
+// block inside upper_adj, every upper-level neighbour at least on the level it is listed at, every entry row on its
+// partition's top level
+static void check_hnsw_graph(const lgpu_ivf_hnsw_sq_desc *d)
+{
+    const uint32_t m = d->m, nlist = d->sq.nlist;
+    LGPU_REQUIRE(m >= 1 && m <= LGPU_HNSW_MAX_M, "IVF_HNSW_SQ: m must be in [1, 64]");
+    LGPU_REQUIRE(d->sq.nrows == 0 || (d->levels && d->adj0 && d->upper_index), "null graph array");
+    LGPU_REQUIRE(d->entry && d->top_level, "null graph array");
+    LGPU_REQUIRE(d->upper_blocks == 0 || d->upper_adj, "null graph array");
+    LGPU_REQUIRE(d->upper_blocks < (1ull << 32), "IVF_HNSW_SQ: more than 2^32 upper-level blocks");
+    for (uint32_t p = 0; p < nlist; p++) {
+        const uint64_t off = d->sq.part_offsets[p], n = d->sq.part_offsets[p + 1] - off;
+        if (n == 0) continue;
+        const uint32_t top = d->top_level[p];
+        LGPU_REQUIRE(top <= LGPU_HNSW_MAX_LEVEL, "IVF_HNSW_SQ: a top level above 15");
+        LGPU_REQUIRE(d->entry[p] < n && d->levels[off + d->entry[p]] == top,
+                     "IVF_HNSW_SQ: an entry row outside its partition or not on the top level");
+        for (uint64_t r = off; r < off + n; r++) {
+            const uint32_t lv = d->levels[r];
+            LGPU_REQUIRE(lv <= top, "IVF_HNSW_SQ: a row above its partition's top level");
+            for (uint32_t j = 0; j < 2 * m; j++) {
+                const uint32_t v = d->adj0[r * 2 * m + j];
+                LGPU_REQUIRE(v == LGPU_HNSW_NONE || v < n, "IVF_HNSW_SQ: a level-0 neighbour outside its partition");
+            }
+            if (lv == 0) continue;
+            const uint64_t u = d->upper_index[r];
+            LGPU_REQUIRE(u + lv <= d->upper_blocks, "IVF_HNSW_SQ: an upper_index outside upper_adj");
+            for (uint32_t L = 1; L <= lv; L++)
+                for (uint32_t j = 0; j < m; j++) {
+                    const uint32_t v = d->upper_adj[(u + L - 1) * m + j];
+                    LGPU_REQUIRE(v == LGPU_HNSW_NONE || (v < n && d->levels[off + v] >= L),
+                                 "IVF_HNSW_SQ: an upper-level neighbour outside its partition or below its level");
+                }
+        }
+    }
+}
+
+int lgpu_ivf_hnsw_sq_open(const lgpu_ivf_hnsw_sq_desc *d, lgpu_index **out)
+{
+    return open_ivf(out, [&](lgpu_index *&ix) {
+        LGPU_REQUIRE(d != nullptr, "null argument");
+        const lgpu_ivf_sq_desc *s = &d->sq;
+        LGPU_REQUIRE(s->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
+        LGPU_REQUIRE(s->metric != LGPU_DOT, "IVF_HNSW_SQ supports the l2 and cosine distance types, not dot");
+        LGPU_REQUIRE(s->dim <= LGPU_SQ_MAX_DIM, "IVF_HNSW_SQ supports dimensions up to 65536");
+        LGPU_REQUIRE(std::isfinite(s->lo) && std::isfinite(s->hi) && s->lo <= s->hi,
+                     "IVF_HNSW_SQ bounds must be finite with lo <= hi");
+        check_ivf_layout(s->dim, s->nlist, s->metric, s->nrows, s->centroids, s->part_offsets, s->codes, s->row_ids);
+        check_hnsw_graph(d);
+        ix = new_ivf(s->device, IvfKind::hnsw_sq);
+        ix->dim_pad = sq_dim_pad(s->dim);
+        ix->sq_lo = s->lo; ix->sq_hi = s->hi;
+        ix->hnsw_m = d->m;
+        open_ivf_common(ix, s, SQ_ROWS_TILE, std::vector<uint64_t>(s->nlist));
+        upload_sq_rows(s->codes, s->nrows, s->dim, ix->codes, ix->sq_xx);
+        upload(ix->hn_levels, d->levels, (size_t)s->nrows);
+        upload(ix->hn_adj0, d->adj0, (size_t)s->nrows * 2 * d->m * 4);
+        upload(ix->hn_upper_index, d->upper_index, (size_t)s->nrows * 4);
+        upload(ix->hn_upper_adj, d->upper_adj, (size_t)d->upper_blocks * d->m * 4);
+        upload(ix->hn_entry, d->entry, (size_t)s->nlist * 4);
+        upload(ix->hn_top, d->top_level, (size_t)s->nlist);
+        LGPU_CUDA(cudaStreamSynchronize(nullptr));
     });
 }
 
@@ -2618,6 +2734,10 @@ static void check_ivf_call(lgpu_index *ix, const void *q, uint32_t B, const lgpu
                  "nprobes above 2048 is not supported unless it covers every partition");
     LGPU_REQUIRE(!refine || p->refine_factor == 0 || ix->has_vectors,
                  "refine_factor needs the raw vectors: open the index with desc.vectors");
+    if (ix->kind == IvfKind::hnsw_sq)
+        LGPU_REQUIRE(hnsw_efp(*p) <= LGPU_HNSW_EF_MAX,
+                     "IVF_HNSW_SQ: ef and limit*refine_factor (or limit+offset) above 2048 (LGPU_HNSW_EF_MAX) are not "
+                     "supported");
 }
 
 static int ivf_call(lgpu_index *ixh, const Route &r, const float *q, uint32_t B, const lgpu_search_params *p,

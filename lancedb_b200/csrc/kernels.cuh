@@ -113,6 +113,31 @@ void launch_sq_encode(const float *Q, uint32_t B, uint32_t dim, uint32_t dim_pad
 void launch_sq_row_norms(const uint8_t *codes, uint64_t n, uint32_t dim_pad, uint32_t *xx, cudaStream_t st);
 void launch_sq_scan(const SqScanArgs &a, int grid, cudaStream_t st);
 
+// ---------------- IVF_HNSW_SQ graph search (hnsw_scan.cu) ---------------------------------
+struct HnswArgs {
+    const uint8_t *codes;         // IVF_SQ's [nrows][dim_pad] row codes
+    const uint8_t *qcodes;        // [B][dim_pad] query codes (launch_sq_encode)
+    uint32_t dim_pad;
+    const uint64_t *probes;       // [slots] partition of each probe slot (>= nlist: unused)
+    uint32_t slots, nprobes, nlist;
+    const uint64_t *part_off;     // [nlist + 1]
+    const uint64_t *row_ids;
+    const uint8_t *levels;        // the graph, lgpu_ivf_hnsw_sq_desc's layout
+    const uint32_t *adj0, *upper_index, *upper_adj, *entry;
+    const uint8_t *top_level;
+    uint32_t m, efp, kk;          // efp: W's capacity, kk: R's (kk <= efp <= LGPU_HNSW_EF_MAX)
+    int has_lower, has_upper;     // the row filter R applies
+    float lower, upper;
+    const uint32_t *allow;
+    uint64_t allow_bits;
+    const uint32_t *only;         // optional [B]: slots of other queries are skipped
+    uint32_t *counter;            // [1], zeroed before launch
+    uint64_t *out_ids;            // [slots][kk]: R of each slot, ascending by (d, position), padded with UINT64_MAX
+    float *out_dist;              //   and +inf
+    uint64_t *out_pos;            //   (the rows' global positions, for refine)
+};
+void launch_hnsw_search(const HnswArgs &a, int num_sms, cudaStream_t st);
+
 // ---------------- IVF_RQ scan (rq_scan.cu) ----------------------------------------------
 constexpr uint32_t RQ_ROWS_TILE = 256;            // rows per tile: 8 warps x 32 rows
 constexpr uint32_t RQ_K_BITS = 256;               // code bits per K step (one b1 MMA); stored rows are padded to it

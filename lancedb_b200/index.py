@@ -1,4 +1,4 @@
-"""IVF_PQ, IVF_SQ, IVF_RQ and binary IVF_FLAT index containers and trainers.
+"""IVF_PQ, IVF_SQ, IVF_HNSW_SQ, IVF_RQ and binary IVF_FLAT index containers and trainers.
 
 `IvfPqIndexData` is the plain-array form of a Lance IVF_PQ index: exactly the arrays
 the reference's search path consumes after `prewarm_index`
@@ -683,5 +683,202 @@ def train_ivf_binary(vectors, *, num_partitions: Optional[int] = None, distance_
     rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
     data = IvfBinaryIndexData(nbytes=nbytes, nlist=nlist, centroids=np.ascontiguousarray(cent, np.uint8),
                               part_offsets=part_offsets, vectors=np.ascontiguousarray(x[order]), row_ids=rid[order])
+    data.validate()
+    return data
+
+
+# --------------------------------------------------------------------------------------
+HNSW_MAX_M = 64             # LGPU_HNSW_MAX_M: a level-0 list (2m entries) is at most 4 per lane of a warp
+HNSW_MAX_LEVEL = 15         # LGPU_HNSW_MAX_LEVEL
+HNSW_NONE = 0xFFFFFFFF      # an unused adjacency slot, an empty partition's entry, a level-0 row's upper_index
+HNSW_BUILD_CAND_CAP = 128   # candidates the neighbour heuristic looks at, at most (ef_construction above it is capped)
+
+
+@dataclass
+class IvfHnswSqIndexData:
+    """The plain-array form of an IVF_HNSW_SQ index (lance `HnswSq`, python/python/lancedb/index.py): an IVF_SQ index
+    (`sq`) plus, in every partition, an HNSW graph over its rows.  Positions are row indices within the partition.
+      levels       u8  [n]         the level of each row
+      adj0         u32 [n, 2m]     level-0 neighbours, padded with HNSW_NONE
+      upper_index  u32 [n]         first block of the row's upper adjacency (level L at upper_index + L - 1); HNSW_NONE
+                                   for a level-0 row
+      upper_adj    u32 [blocks, m] neighbours at levels >= 1, padded with HNSW_NONE
+      entry        u32 [nlist]     the entry row of each partition (HNSW_NONE when empty); its level is top_level
+      top_level    u8  [nlist]
+    The same arrays go to `lgpu_ivf_hnsw_sq_open` and to the CPU oracle (tests/hnsw_sq_oracle.c)."""
+    sq: IvfSqIndexData
+    m: int
+    levels: np.ndarray
+    adj0: np.ndarray
+    upper_index: np.ndarray
+    upper_adj: np.ndarray
+    entry: np.ndarray
+    top_level: np.ndarray
+
+    dim = property(lambda self: self.sq.dim)
+    nlist = property(lambda self: self.sq.nlist)
+    metric = property(lambda self: self.sq.metric)
+    nrows = property(lambda self: self.sq.nrows)
+    part_offsets = property(lambda self: self.sq.part_offsets)
+    row_ids = property(lambda self: self.sq.row_ids)
+    vectors = property(lambda self: self.sq.vectors)
+
+    def validate(self) -> None:
+        """Every index in range and every degree bound held: what lgpu_ivf_hnsw_sq_open checks."""
+        self.sq.validate()
+        n, m = self.nrows, self.m
+        assert 1 <= m <= HNSW_MAX_M
+        assert self.levels.shape == (n,) and self.levels.dtype == np.uint8
+        assert self.adj0.shape == (n, 2 * m) and self.adj0.dtype == np.uint32
+        assert self.upper_index.shape == (n,) and self.upper_index.dtype == np.uint32
+        assert self.upper_adj.ndim == 2 and self.upper_adj.shape[1] == m and self.upper_adj.dtype == np.uint32
+        assert self.entry.shape == (self.nlist,) and self.entry.dtype == np.uint32
+        assert self.top_level.shape == (self.nlist,) and self.top_level.dtype == np.uint8
+        off = self.part_offsets.astype(np.int64)
+        nb = self.upper_adj.shape[0]
+        for p in range(self.nlist):
+            a, b = off[p], off[p + 1]
+            if a == b:
+                continue
+            lv = self.levels[a:b].astype(np.int64)
+            top = int(self.top_level[p])
+            assert top <= HNSW_MAX_LEVEL and int(self.entry[p]) < b - a and lv[self.entry[p]] == top
+            assert lv.max() <= top
+            adj = self.adj0[a:b]
+            assert ((adj == HNSW_NONE) | (adj < b - a)).all()
+            for r in np.nonzero(lv)[0]:
+                u = int(self.upper_index[a + r])
+                assert u != HNSW_NONE and u + lv[r] <= nb
+                for L in range(1, lv[r] + 1):
+                    blk = self.upper_adj[u + L - 1]
+                    ok = blk == HNSW_NONE
+                    ok[~ok] = (blk[~ok] < b - a)
+                    assert ok.all() and (lv[blk[blk != HNSW_NONE].astype(np.int64)] >= L).all()
+
+
+def _hnsw_candidates(xc, ncand, chunk):
+    """The ncand nearest other rows of every row of xc [s, dim] (codes as floats), nearest first, ties to the lower
+    position: ([s, C] positions, [s, C] f32 distances), C = min(ncand, s - 1)."""
+    import torch
+    s = xc.shape[0]
+    c = min(ncand, s - 1)
+    nx = (xc.float() * xc.float()).sum(1)
+    pos = torch.arange(s, device=xc.device, dtype=torch.float64)
+    out_i = torch.empty((s, c), dtype=torch.long, device=xc.device)
+    out_d = torch.empty((s, c), dtype=torch.float32, device=xc.device)
+    for a in range(0, s, chunk):
+        b = min(s, a + chunk)
+        d = (nx[a:b, None] + nx[None, :] - 2.0 * (xc[a:b] @ xc.T).float()).clamp(min=0)
+        key = d.double() * s + pos                       # exact: ties fall to the lower position
+        key[torch.arange(b - a, device=xc.device), torch.arange(a, b, device=xc.device)] = float("inf")
+        _, idx = torch.topk(key, c, dim=1, largest=False, sorted=True)
+        out_i[a:b] = idx
+        out_d[a:b] = torch.gather(d, 1, idx)
+    return out_i, out_d
+
+
+def _hnsw_level_graph(xc, deg, ncand, chunk=1024):
+    """Neighbour lists [s, deg] (local positions, -1 padded) of the rows xc [s, dim] at one level: the HNSW heuristic
+    over each row's nearest candidates (a candidate is kept while fewer than deg are, unless a kept one is nearer to it
+    than the row is), then reverse edges, every list pruned to its deg nearest (ties to the lower position)."""
+    import torch
+    s, dev = xc.shape[0], xc.device
+    adj = torch.full((s, deg), -1, dtype=torch.long, device=dev)
+    if s <= 1:
+        return adj
+    cand, cd = _hnsw_candidates(xc, min(ncand, HNSW_BUILD_CAND_CAP), chunk)
+    c = cand.shape[1]
+    nx = (xc.float() * xc.float()).sum(1)
+    srcs, dsts, ds = [], [], []
+    hb = max(1, (1 << 27) // max(1, c * xc.shape[1]))   # rows per heuristic batch (bounds the gathered codes)
+    for a in range(0, s, hb):
+        b = min(s, a + hb)
+        ci, dv = cand[a:b], cd[a:b]
+        g = xc[ci]                                                           # [b, c, dim]
+        pair = (nx[ci][:, :, None] + nx[ci][:, None, :] - 2.0 * torch.bmm(g, g.transpose(1, 2)).float())
+        sel = torch.zeros((b - a, c), dtype=torch.bool, device=dev)
+        cnt = torch.zeros(b - a, dtype=torch.long, device=dev)
+        for j in range(c):
+            closer = ((pair[:, j, :] < dv[:, j:j + 1]) & sel).any(1)
+            ok = ~closer & (cnt < deg)
+            sel[:, j] = ok
+            cnt += ok
+        r, j = sel.nonzero(as_tuple=True)
+        srcs.append(r + a); dsts.append(ci[r, j]); ds.append(dv[r, j])
+    src, dst, d = torch.cat(srcs), torch.cat(dsts), torch.cat(ds)
+    src, dst, d = torch.cat([src, dst]), torch.cat([dst, src]), torch.cat([d, d])     # reverse edges
+    for i in (1, 2, 0):                                                               # sort by (src, d, dst)
+        o = torch.sort((src, dst, d)[i], stable=True).indices
+        src, dst, d = src[o], dst[o], d[o]
+    keep = torch.ones_like(src, dtype=torch.bool)
+    keep[1:] = (src[1:] != src[:-1]) | (dst[1:] != dst[:-1])
+    src, dst = src[keep], dst[keep]
+    first = torch.zeros(s + 1, dtype=torch.long, device=dev)
+    first[1:] = torch.cumsum(torch.bincount(src, minlength=s), 0)
+    rank = torch.arange(src.numel(), device=dev) - first[src]
+    m = rank < deg
+    adj[src[m], rank[m]] = dst[m]
+    return adj
+
+
+def build_hnsw_graph(codes, part_offsets, m: int = 20, ef_construction: int = 300, seed: int = 45, device=None):
+    """The HNSW graphs of every partition of an IVF_SQ index over its codes [n, dim] (u8, partition order), in the
+    IvfHnswSqIndexData layout: (levels, adj0, upper_index, upper_adj, entry, top_level).  Levels are a seeded geometric
+    draw, floor(-ln(U) / ln m) capped at HNSW_MAX_LEVEL; each level's lists come from _hnsw_level_graph over the rows of
+    that level in the partition (degree 2m at level 0, m above).  Deterministic for a seed on a given device."""
+    import math
+    import torch
+    if not 1 <= m <= HNSW_MAX_M:
+        raise ValueError(f"m must be in [1, {HNSW_MAX_M}], got {m}")
+    if ef_construction < 1:
+        raise ValueError(f"ef_construction must be positive, got {ef_construction}")
+    codes = np.ascontiguousarray(codes, np.uint8)
+    n = codes.shape[0]
+    off = np.asarray(part_offsets, np.int64)
+    nlist = off.size - 1
+    gen = torch.Generator(device="cpu").manual_seed(seed)
+    u = torch.rand(n, generator=gen, dtype=torch.float64).clamp(min=1e-300)
+    lv = (-torch.log(u) / math.log(max(m, 2))).floor().clamp(max=HNSW_MAX_LEVEL).to(torch.uint8).numpy()
+    dev = torch.device(device) if device is not None else torch.device("cpu")
+    ftype = torch.float32          # codes are exact in f32 (and TF32); products and sums accumulate in f32
+    adj0 = np.full((n, 2 * m), HNSW_NONE, np.uint32)
+    upper_index = np.full(n, HNSW_NONE, np.uint32)
+    up = np.nonzero(lv)[0]
+    upper_index[up] = (np.cumsum(lv[up].astype(np.int64)) - lv[up]).astype(np.uint32)
+    upper_adj = np.full((int(lv.astype(np.int64).sum()), m), HNSW_NONE, np.uint32)
+    entry = np.full(nlist, HNSW_NONE, np.uint32)
+    top = np.zeros(nlist, np.uint8)
+    for p in range(nlist):
+        a, b = int(off[p]), int(off[p + 1])
+        if a == b:
+            continue
+        plv = lv[a:b]
+        top[p] = plv.max()
+        entry[p] = int(np.argmax(plv))                       # the first row of the top level
+        xc = torch.as_tensor(codes[a:b], device=dev).to(ftype)
+        for L in range(int(top[p]) + 1):
+            rows = np.nonzero(plv >= L)[0]
+            sub = _hnsw_level_graph(xc[torch.as_tensor(rows, device=dev)], 2 * m if L == 0 else m,
+                                    ef_construction).cpu().numpy()
+            g = np.where(sub >= 0, rows[np.maximum(sub, 0)], HNSW_NONE).astype(np.uint32)
+            if L == 0:
+                adj0[a:b] = g
+            else:
+                upper_adj[upper_index[a + rows].astype(np.int64) + L - 1] = g
+    return lv, adj0, upper_index, upper_adj, entry, top
+
+
+def train_ivf_hnsw_sq(vectors, *, num_partitions: Optional[int] = None, distance_type: str = "l2", m: int = 20,
+                      ef_construction: int = 300, sample_rate: int = 256, max_iterations: int = 50,
+                      row_ids: Optional[np.ndarray] = None, keep_vectors: bool = False, seed: int = 45,
+                      device: Optional[str] = None, native_passes: bool = False) -> IvfHnswSqIndexData:
+    """train_ivf_sq, then build_hnsw_graph over its codes (on `device`: torch on the GPU for "cuda", else the CPU)."""
+    if not 1 <= m <= HNSW_MAX_M:
+        raise ValueError(f"m must be in [1, {HNSW_MAX_M}], got {m}")
+    sq = train_ivf_sq(vectors, num_partitions=num_partitions, distance_type=distance_type, sample_rate=sample_rate,
+                      max_iterations=max_iterations, row_ids=row_ids, keep_vectors=keep_vectors, seed=seed,
+                      device=device, native_passes=native_passes)
+    g = build_hnsw_graph(sq.codes, sq.part_offsets, m, ef_construction, seed, device)
+    data = IvfHnswSqIndexData(sq, m, *g)
     data.validate()
     return data

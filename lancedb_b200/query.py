@@ -50,6 +50,7 @@ class LanceVectorQueryBuilder:
         self._lower_bound: Optional[float] = None
         self._upper_bound: Optional[float] = None
         self._refine_factor: Optional[int] = None
+        self._ef: Optional[int] = None
         self._limit: Optional[int] = None
         self._offset: int = 0
         self._columns: Optional[List[str]] = None
@@ -87,6 +88,15 @@ class LanceVectorQueryBuilder:
 
     def refine_factor(self, refine_factor: int) -> "LanceVectorQueryBuilder":
         self._refine_factor = refine_factor
+        return self
+
+    def ef(self, ef: int) -> "LanceVectorQueryBuilder":
+        """The HNSW search beam (python/python/lancedb/query.py:1719, rust/lancedb/src/query.rs:1290-1300): IVF_HNSW_SQ
+        keeps the max(ef, limit x refine_factor) best rows seen per probed partition; unset means 1.5 x limit.  Other
+        index kinds ignore it."""
+        if int(ef) <= 0:
+            raise ValueError("ef must be greater than 0")
+        self._ef = int(ef)
         return self
 
     def limit(self, limit: Optional[int]) -> "LanceVectorQueryBuilder":
@@ -189,7 +199,7 @@ class LanceVectorQueryBuilder:
             refine_factor=self._refine_factor, distance_type=self._distance_type,
             lower=self._lower_bound, upper=self._upper_bound, use_index=self._use_index,
             allow_mask=None if (mask is None or self._postfilter) else mask,
-            max_nprobes=max_nprobes, timeout_ms=timeout_ms)
+            max_nprobes=max_nprobes, timeout_ms=timeout_ms, **({"ef": self._ef} if self._ef else {}))
         out = []
         for qi in range(len(cnt)):                         # one result list per query (a multivector query is one)
             n = int(cnt[qi])

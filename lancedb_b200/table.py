@@ -16,8 +16,8 @@ import numpy as np
 import pyarrow as pa
 
 from . import _native
-from .index import (RQ_MAX_DIM, IvfBinaryIndexData, IvfPqIndexData, IvfRqIndexData, IvfSqIndexData,
-                    train_ivf_binary, train_ivf_pq, train_ivf_rq, train_ivf_sq)
+from .index import (RQ_MAX_DIM, IvfBinaryIndexData, IvfHnswSqIndexData, IvfPqIndexData, IvfRqIndexData,
+                    IvfSqIndexData, train_ivf_binary, train_ivf_hnsw_sq, train_ivf_pq, train_ivf_rq, train_ivf_sq)
 from .query import LanceVectorQueryBuilder
 
 
@@ -107,6 +107,8 @@ class Table:
         d = self._index_data[column]
         if isinstance(d, IvfBinaryIndexData):
             return "IVF_FLAT"
+        if isinstance(d, IvfHnswSqIndexData):
+            return "IVF_HNSW_SQ"
         return "IVF_SQ" if isinstance(d, IvfSqIndexData) else ("IVF_RQ" if isinstance(d, IvfRqIndexData) else "IVF_PQ")
 
     def list_indices(self):
@@ -156,7 +158,8 @@ class Table:
     def create_index(self, metric: str = "l2", num_partitions: Optional[int] = None,
                      num_sub_vectors: Optional[int] = None, vector_column_name: Optional[str] = None,
                      replace: bool = True, accelerator: Optional[str] = None, index_type: str = "IVF_PQ",
-                     num_bits: int = 8, max_iterations: int = 50, sample_rate: int = 256, **_ignored):
+                     num_bits: int = 8, max_iterations: int = 50, sample_rate: int = 256, m: int = 20,
+                     ef_construction: int = 300, **_ignored):
         kind = index_type.upper()
         if kind == "IVF_FLAT":             # binary columns only: IvfFlat(distance_type="hamming")
             column = vector_column_name or self._infer_vector_column(None)
@@ -174,22 +177,22 @@ class Table:
                                                         max_iterations=max_iterations, sample_rate=sample_rate,
                                                         device=dev))
             return
-        if kind not in ("IVF_PQ", "IVF_SQ", "IVF_RQ"):
-            raise NotImplementedError("only IVF_PQ, IVF_SQ and IVF_RQ are on the GPU hot path")
+        if kind not in ("IVF_PQ", "IVF_SQ", "IVF_RQ", "IVF_HNSW_SQ"):
+            raise NotImplementedError("only IVF_PQ, IVF_SQ, IVF_HNSW_SQ and IVF_RQ are on the GPU hot path")
         if kind == "IVF_RQ" and num_bits != 1:
             # RaBitQ with 1 bit per dimension only (extended RaBitQ is not served); the legacy default of 8 is refused
             # rather than quietly building a 1-bit index
             raise ValueError(f"IVF_RQ supports num_bits=1 only, got num_bits={num_bits}")
         if kind == "IVF_PQ" and num_bits not in (4, 8):
             raise ValueError(f"IVF_PQ supports num_bits 4 or 8, got num_bits={num_bits}")
-        if kind == "IVF_SQ" and num_bits != 8:
+        if kind in ("IVF_SQ", "IVF_HNSW_SQ") and num_bits != 8:
             raise ValueError("only num_bits=8 is supported")
         column = vector_column_name or self._infer_vector_column(None)
         if self._is_binary(column):
             raise NotImplementedError("no index over binary vectors on the GPU path: search them flat (hamming)")
         if self._is_multivec(column):
             raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
-        if kind in ("IVF_SQ", "IVF_RQ") and metric.lower() not in ("l2", "cosine"):
+        if kind in ("IVF_SQ", "IVF_HNSW_SQ", "IVF_RQ") and metric.lower() not in ("l2", "cosine"):
             raise ValueError(f"{kind} supports the l2 and cosine distance types, not {metric!r}")
         if kind == "IVF_RQ" and self._dim(column) > RQ_MAX_DIM:
             raise ValueError(f"IVF_RQ supports dimensions up to {RQ_MAX_DIM}, got {self._dim(column)}")
@@ -203,6 +206,12 @@ class Table:
                                                     distance_type=metric, max_iterations=max_iterations,
                                                     sample_rate=sample_rate, keep_vectors=True, device=dev,
                                                     native_passes=dev is not None))
+            return
+        if kind == "IVF_HNSW_SQ":          # HnswSq: distance_type, num_partitions, m, ef_construction, max_iterations, sample_rate
+            self._attach_index(column, train_ivf_hnsw_sq(self._vectors(column), num_partitions=num_partitions,
+                                                         distance_type=metric, m=m, ef_construction=ef_construction,
+                                                         max_iterations=max_iterations, sample_rate=sample_rate,
+                                                         keep_vectors=True, device=dev, native_passes=dev is not None))
             return
         if kind == "IVF_RQ":               # IvfRqIndexBuilder: distance_type, num_partitions, num_bits, max_iterations, sample_rate
             self._attach_index(column, train_ivf_rq(self._vectors(column), num_partitions=num_partitions,
@@ -218,11 +227,13 @@ class Table:
         self._attach_index(column, data)
 
     def _attach_index(self, column: str,
-                      data: Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData, IvfBinaryIndexData]):
+                      data: Union[IvfPqIndexData, IvfSqIndexData, IvfHnswSqIndexData, IvfRqIndexData,
+                                  IvfBinaryIndexData]):
         if column in self._index:
             self._index[column].close()
         self._index_data[column] = data
         cls = (_native.GpuIvfBinary if isinstance(data, IvfBinaryIndexData) else
+               _native.GpuIvfHnswSq if isinstance(data, IvfHnswSqIndexData) else
                _native.GpuIvfSq if isinstance(data, IvfSqIndexData) else
                _native.GpuIvfRq if isinstance(data, IvfRqIndexData) else _native.GpuIvfPq)
         self._index[column] = cls(data, device=self._device)
@@ -279,7 +290,7 @@ class Table:
         return LanceVectorQueryBuilder(self, query, column)
 
     def _vector_search(self, queries: np.ndarray, *, column, k, nprobes, refine_factor, distance_type,
-                       lower, upper, use_index, allow_mask=None, max_nprobes=0, timeout_ms=0):
+                       lower, upper, use_index, allow_mask=None, max_nprobes=0, timeout_ms=0, ef=0):
         allow, allow_bits = None, 0
         if allow_mask is not None:                 # prefilter: row-id allow-list as the C ABI's bitmap
             allow, allow_bits = _native.mask_bitmap(allow_mask), int(len(allow_mask))
@@ -317,7 +328,7 @@ class Table:
                 raise ValueError(f"distance_type {distance_type!r} does not match the index's {idx.metric!r}")
             return idx.search(queries, k=k, nprobes=nprobes, refine_factor=refine_factor or 0,
                               lower=lower, upper=upper, allow=allow, allow_bits=allow_bits,
-                              max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms)
+                              max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms, ef=ef)
         fl = self._flat.get(column)
         if fl is None:
             fl = self._flat[column] = _native.GpuFlat(self._vectors(column), device=self._device)
