@@ -296,6 +296,15 @@ def binary_components(queries) -> np.ndarray:
     return np.ascontiguousarray(a, np.uint8)
 
 
+def _binary_queries(handle, queries) -> np.ndarray:
+    """The `_queries` method of GpuBinary and GpuIvfBinary: queries [B, nbytes] (or one [nbytes] query) with
+    nbytes = handle.nbytes, checked by binary_components -> u8 [B, nbytes]."""
+    a = np.asarray(queries)
+    if a.ndim not in (1, 2) or a.shape[-1] != handle.nbytes:
+        raise ValueError(f"binary queries must be [B, {handle.nbytes}] or [{handle.nbytes}], got shape {a.shape}")
+    return binary_components(a).reshape(-1, handle.nbytes)
+
+
 def _query_offsets(q_offsets) -> np.ndarray:
     """Multivector query offsets [B+1] -> u32, checked: they start at 0 and give every query 1..4096 vectors."""
     off = np.asarray(q_offsets, np.int64).reshape(-1)
@@ -312,27 +321,30 @@ def _query_offsets(q_offsets) -> np.ndarray:
 
 
 class GpuIvfPq(_Handle):
-    """An IVF_PQ index pinned in HBM (lgpu_index), 8-bit or 4-bit codes (data.num_bits)."""
-    _close = "lgpu_index_close"
+    """An IVF_PQ index pinned in HBM (lgpu_index), 8-bit or 4-bit codes (data.num_bits).  The other float IVF kinds
+    open an lgpu_index through their own C function, `_open`, so they subclass this and supply only `_desc`."""
+    _open, _close = "lgpu_index_open", "lgpu_index_close"
 
     def __init__(self, data, device: int = 0, with_vectors: bool = True):
         lib = load()
-        data.validate()
-        self.dim, self.nlist, self.m, self.metric = data.dim, data.nlist, data.m, data.metric
-        self.device = device
+        self.dim, self.nlist, self.metric, self.device = data.dim, data.nlist, data.metric, device
         vec = data.vectors if with_vectors else None
-        keep = [np.ascontiguousarray(data.centroids, np.float32), np.ascontiguousarray(data.codebook, np.float32),
-                np.ascontiguousarray(data.part_offsets, np.uint64), np.ascontiguousarray(data.codes_t, np.uint8),
-                np.ascontiguousarray(data.row_ids, np.uint64),
-                None if vec is None else np.ascontiguousarray(vec, np.float32)]
-        self.num_bits = data.num_bits
-        desc = IndexDesc(ABI_VERSION, data.dim, data.nlist, data.m, data.num_bits, METRICS[data.metric], 1, device,
-                         data.nrows, _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]),
-                         _ptr(keep[5]))
+        desc, keep = self._desc(data, device, None if vec is None else np.ascontiguousarray(vec, np.float32))
         h = C.c_void_p()
-        check(lib.lgpu_index_open(C.byref(desc), C.byref(h)))
+        check(getattr(lib, self._open)(C.byref(desc), C.byref(h)))
         self._h = h
         self.has_vectors = vec is not None
+
+    def _desc(self, data, device: int, vec: Optional[np.ndarray]):
+        """(desc, keep): the C desc of `data` once data.validate() passes, and the arrays it points into, which must
+        outlive the open call.  Also sets the kind's own attributes."""
+        data.validate()
+        self.m, self.num_bits = data.m, data.num_bits
+        keep = [np.ascontiguousarray(data.centroids, np.float32), np.ascontiguousarray(data.codebook, np.float32),
+                np.ascontiguousarray(data.part_offsets, np.uint64), np.ascontiguousarray(data.codes_t, np.uint8),
+                np.ascontiguousarray(data.row_ids, np.uint64), vec]
+        return IndexDesc(ABI_VERSION, data.dim, data.nlist, data.m, data.num_bits, METRICS[data.metric], 1, device,
+                         data.nrows, *[_ptr(a) for a in keep]), keep
 
     def device_bytes(self) -> int:
         b = C.c_uint64(0)
@@ -409,80 +421,46 @@ class GpuIvfPq(_Handle):
 class GpuIvfSq(GpuIvfPq):
     """An IVF_SQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_sq_open, so every search entry point of GpuIvfPq
     serves it.  _distance is the exact integer sum of squared code differences as f32 (l2 and cosine alike)."""
+    _open = "lgpu_ivf_sq_open"
 
-    def __init__(self, data, device: int = 0, with_vectors: bool = True):
-        lib = load()
-        if data.metric not in ("l2", "cosine"):
-            raise ValueError(f"IVF_SQ supports the l2 and cosine distance types, not {data.metric!r}")
+    def _desc(self, data, device, vec):
         data.validate()
-        self.dim, self.nlist, self.metric = data.dim, data.nlist, data.metric
         self.lo, self.hi = float(data.lo), float(data.hi)
-        self.device = device
-        vec = data.vectors if with_vectors else None
         keep = [np.ascontiguousarray(data.centroids, np.float32), np.ascontiguousarray(data.part_offsets, np.uint64),
-                np.ascontiguousarray(data.codes, np.uint8), np.ascontiguousarray(data.row_ids, np.uint64),
-                None if vec is None else np.ascontiguousarray(vec, np.float32)]
-        desc = SqDesc(ABI_VERSION, data.dim, data.nlist, METRICS[data.metric], device, 0, data.nrows, self.lo, self.hi,
-                      _ptr(keep[0]), _ptr(keep[1]), _ptr(keep[2]), _ptr(keep[3]), _ptr(keep[4]))
-        h = C.c_void_p()
-        check(lib.lgpu_ivf_sq_open(C.byref(desc), C.byref(h)))
-        self._h = h
-        self.has_vectors = vec is not None
+                np.ascontiguousarray(data.codes, np.uint8), np.ascontiguousarray(data.row_ids, np.uint64), vec]
+        return SqDesc(ABI_VERSION, data.dim, data.nlist, METRICS[data.metric], device, 0, data.nrows, self.lo, self.hi,
+                      *[_ptr(a) for a in keep]), keep
 
 
-class GpuIvfHnswSq(GpuIvfPq):
+class GpuIvfHnswSq(GpuIvfSq):
     """An IVF_HNSW_SQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_hnsw_sq_open (IVF_SQ's arrays plus the
-    per-partition HNSW graphs), so every search entry point of GpuIvfPq serves it; `ef` sets the search beam."""
+    per-partition HNSW graphs), so every search entry point of GpuIvfPq serves it; `ef` sets the search beam.  The
+    graphs are checked by lgpu_ivf_hnsw_sq_open, not by data.validate()."""
+    _open = "lgpu_ivf_hnsw_sq_open"
 
-    def __init__(self, data, device: int = 0, with_vectors: bool = True):
-        lib = load()
-        sq = data.sq
-        if sq.metric not in ("l2", "cosine"):
-            raise ValueError(f"IVF_HNSW_SQ supports the l2 and cosine distance types, not {sq.metric!r}")
-        sq.validate()
-        self.dim, self.nlist, self.metric, self.m = sq.dim, sq.nlist, sq.metric, int(data.m)
-        self.lo, self.hi = float(sq.lo), float(sq.hi)
-        self.device = device
-        vec = sq.vectors if with_vectors else None
-        keep = [np.ascontiguousarray(sq.centroids, np.float32), np.ascontiguousarray(sq.part_offsets, np.uint64),
-                np.ascontiguousarray(sq.codes, np.uint8), np.ascontiguousarray(sq.row_ids, np.uint64),
-                None if vec is None else np.ascontiguousarray(vec, np.float32),
-                np.ascontiguousarray(data.levels, np.uint8), np.ascontiguousarray(data.adj0, np.uint32),
-                np.ascontiguousarray(data.upper_index, np.uint32), np.ascontiguousarray(data.upper_adj, np.uint32),
-                np.ascontiguousarray(data.entry, np.uint32), np.ascontiguousarray(data.top_level, np.uint8)]
-        desc = HnswSqDesc(SqDesc(ABI_VERSION, sq.dim, sq.nlist, METRICS[sq.metric], device, 0, sq.nrows, self.lo,
-                                 self.hi, *[_ptr(a) for a in keep[:5]]),
-                          self.m, 0, keep[8].shape[0], *[_ptr(a) for a in keep[5:]])
-        h = C.c_void_p()
-        check(lib.lgpu_ivf_hnsw_sq_open(C.byref(desc), C.byref(h)))
-        self._h = h
-        self.has_vectors = vec is not None
+    def _desc(self, data, device, vec):
+        sq, keep = super()._desc(data.sq, device, vec)
+        self.m = int(data.m)
+        graph = [np.ascontiguousarray(data.levels, np.uint8), np.ascontiguousarray(data.adj0, np.uint32),
+                 np.ascontiguousarray(data.upper_index, np.uint32), np.ascontiguousarray(data.upper_adj, np.uint32),
+                 np.ascontiguousarray(data.entry, np.uint32), np.ascontiguousarray(data.top_level, np.uint8)]
+        return HnswSqDesc(sq, self.m, 0, graph[3].shape[0], *[_ptr(a) for a in graph]), keep + graph
 
 
 class GpuIvfRq(GpuIvfPq):
     """An IVF_RQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_rq_open, so every search entry point of GpuIvfPq
     serves it.  _distance is the RaBitQ estimate of the squared L2 distance (half of it for cosine); refine_factor
     re-ranks by the exact distance."""
+    _open = "lgpu_ivf_rq_open"
 
-    def __init__(self, data, device: int = 0, with_vectors: bool = True):
-        lib = load()
-        if data.metric not in ("l2", "cosine"):
-            raise ValueError(f"IVF_RQ supports the l2 and cosine distance types, not {data.metric!r}")
+    def _desc(self, data, device, vec):
         data.validate()
-        self.dim, self.nlist, self.metric = data.dim, data.nlist, data.metric
-        self.device = device
-        vec = data.vectors if with_vectors else None
         keep = [np.ascontiguousarray(data.centroids, np.float32), np.ascontiguousarray(data.rotation, np.float32),
                 np.ascontiguousarray(data.part_offsets, np.uint64), np.ascontiguousarray(data.codes, np.uint8),
                 np.ascontiguousarray(data.add_factors, np.float32), np.ascontiguousarray(data.scale_factors, np.float32),
-                np.ascontiguousarray(data.row_ids, np.uint64),
-                None if vec is None else np.ascontiguousarray(vec, np.float32)]
-        desc = RqDesc(ABI_VERSION, data.dim, data.nlist, METRICS[data.metric], device, data.num_bits, data.nrows,
-                      *[_ptr(a) for a in keep])
-        h = C.c_void_p()
-        check(lib.lgpu_ivf_rq_open(C.byref(desc), C.byref(h)))
-        self._h = h
-        self.has_vectors = vec is not None
+                np.ascontiguousarray(data.row_ids, np.uint64), vec]
+        return RqDesc(ABI_VERSION, data.dim, data.nlist, METRICS[data.metric], device, data.num_bits, data.nrows,
+                      *[_ptr(a) for a in keep]), keep
 
 
 class GpuFlat(_Handle):
@@ -521,6 +499,7 @@ class GpuBinary(_Handle):
     """A packed binary vector column (fixed_size_list<uint8, nbytes>) pinned in HBM (lgpu_binary), searched by
     Hamming distance."""
     _close = "lgpu_binary_close"
+    _queries = _binary_queries
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
         v = np.ascontiguousarray(vectors, np.uint8)
@@ -540,12 +519,6 @@ class GpuBinary(_Handle):
         p = make_params(k, 0, 0, lower, upper, 0, timeout_ms)
         return _host_search("lgpu_binary_search", (self._h, _ptr(q), q.shape[0]), q.shape[0], k, p, allow, allow_bits)
 
-    def _queries(self, queries) -> np.ndarray:
-        a = np.asarray(queries)
-        if a.ndim not in (1, 2) or a.shape[-1] != self.nbytes:
-            raise ValueError(f"binary queries must be [B, {self.nbytes}] or [{self.nbytes}], got shape {a.shape}")
-        return binary_components(a).reshape(-1, self.nbytes)
-
     def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search (raw addresses; queries [B][nbytes] u8), enqueued on `stream`, not synchronised."""
         check(load().lgpu_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
@@ -555,25 +528,19 @@ class GpuIvfBinary(_Handle):
     """A binary IVF_FLAT index (IvfBinaryIndexData) pinned in HBM (lgpu_ivf_binary): the probed partitions of packed
     binary rows scored exactly by Hamming distance."""
     _close = "lgpu_ivf_binary_close"
+    _queries = _binary_queries
 
     def __init__(self, data, device: int = 0):
         lib = load()
         data.validate()
         self.nbytes, self.nlist, self.metric = data.nbytes, data.nlist, data.metric
         self.device = device
-        self._keep = [np.ascontiguousarray(data.centroids, np.uint8), np.ascontiguousarray(data.part_offsets, np.uint64),
-                      np.ascontiguousarray(data.vectors, np.uint8), np.ascontiguousarray(data.row_ids, np.uint64)]
-        desc = IvfBinaryDesc(ABI_VERSION, data.nbytes, data.nlist, device, data.nrows, *[_ptr(a) for a in self._keep])
+        keep = [np.ascontiguousarray(data.centroids, np.uint8), np.ascontiguousarray(data.part_offsets, np.uint64),
+                np.ascontiguousarray(data.vectors, np.uint8), np.ascontiguousarray(data.row_ids, np.uint64)]
+        desc = IvfBinaryDesc(ABI_VERSION, data.nbytes, data.nlist, device, data.nrows, *[_ptr(a) for a in keep])
         h = C.c_void_p()
         check(lib.lgpu_ivf_binary_open(C.byref(desc), C.byref(h)))
         self._h = h
-        self._keep = None
-
-    def _queries(self, queries) -> np.ndarray:
-        a = np.asarray(queries)
-        if a.ndim not in (1, 2) or a.shape[-1] != self.nbytes:
-            raise ValueError(f"binary queries must be [B, {self.nbytes}] or [{self.nbytes}], got shape {a.shape}")
-        return binary_components(a).reshape(-1, self.nbytes)
 
     def search(self, queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None, allow=None, allow_bits=0,
                max_nprobes=0, timeout_ms=0):

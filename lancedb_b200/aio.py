@@ -13,7 +13,7 @@ Plain scans (`query()` without `nearest_to`) are served from the host table: the
 from __future__ import annotations
 
 import asyncio
-from dataclasses import dataclass
+from dataclasses import asdict, dataclass
 from typing import Dict, Iterable, List, Optional, Union
 
 import numpy as np
@@ -26,6 +26,7 @@ from .table import DBConnection, Table
 @dataclass
 class IvfPq:
     """Index.IvfPq parameters (python/python/lancedb/index.py:670-800, rust/lancedb/src/index/vector.rs:246-319)."""
+    index_type = "IVF_PQ"
     distance_type: str = "l2"
     num_partitions: Optional[int] = None
     num_sub_vectors: Optional[int] = None
@@ -38,6 +39,7 @@ class IvfPq:
 class IvfRq:
     """Index.IvfRq parameters (python/python/lancedb/index.py:803-856, rust/lancedb/src/index/vector.rs:321-369):
     RaBitQ with num_bits = 1 (the only width served)."""
+    index_type = "IVF_RQ"
     distance_type: str = "l2"
     num_partitions: Optional[int] = None
     num_bits: int = 1
@@ -49,6 +51,7 @@ class IvfRq:
 class HnswSq:
     """Index.HnswSq parameters (python/python/lancedb/index.py, python/python/tests/test_table.py:1565-1590): IVF
     partitions of 8-bit scalar codes with an HNSW graph in each; builds an IVF_HNSW_SQ index."""
+    index_type = "IVF_HNSW_SQ"
     distance_type: str = "l2"
     num_partitions: Optional[int] = None
     m: int = 20
@@ -62,6 +65,7 @@ class IvfFlat:
     """Index.IvfFlat parameters (rust/lancedb/src/index/vector.rs:169-209): served over binary (fixed_size_list<uint8>)
     columns with distance_type="hamming"; the default "l2", like any other metric there, is refused (ValueError), and a
     float column raises NotImplementedError."""
+    index_type = "IVF_FLAT"
     distance_type: str = "l2"
     num_partitions: Optional[int] = None
     max_iterations: int = 50
@@ -290,14 +294,9 @@ class AsyncTable:
     async def create_index(self, column: str, *, config: Optional[Union[IvfPq, IvfRq, HnswSq, IvfFlat]] = None,
                            replace: bool = True, accelerator: Optional[str] = "cuda"):
         cfg = config or IvfPq()
-        kind = ("IVF_RQ" if isinstance(cfg, IvfRq) else "IVF_FLAT" if isinstance(cfg, IvfFlat) else
-                "IVF_HNSW_SQ" if isinstance(cfg, HnswSq) else "IVF_PQ")
-        hnsw = {"m": cfg.m, "ef_construction": cfg.ef_construction} if isinstance(cfg, HnswSq) else {}
-        await asyncio.to_thread(
-            self._table.create_index, metric=cfg.distance_type, num_partitions=cfg.num_partitions,
-            num_sub_vectors=getattr(cfg, "num_sub_vectors", None), vector_column_name=column, replace=replace,
-            accelerator=accelerator, index_type=kind, num_bits=getattr(cfg, "num_bits", 8),
-            max_iterations=cfg.max_iterations, sample_rate=cfg.sample_rate, **hnsw)
+        kw = asdict(cfg)            # Table.create_index takes every field under its own name but distance_type
+        await asyncio.to_thread(self._table.create_index, index_type=cfg.index_type, metric=kw.pop("distance_type"),
+                                vector_column_name=column, replace=replace, accelerator=accelerator, **kw)
 
     async def prewarm_index(self, name: str):
         return self._table.prewarm_index(name)

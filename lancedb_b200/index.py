@@ -18,7 +18,7 @@ path and the oracle consume the identical arrays it produces.
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Optional
+from typing import Callable, Optional, Tuple
 
 import numpy as np
 
@@ -52,8 +52,30 @@ def suggested_num_partitions(num_rows: int, target_partition_size: int = 8192) -
     return max(1, num_rows // target_partition_size)
 
 
+def _check_ivf_layout(d, width: int, dtype) -> None:
+    """The layout every IVF index shares: centroids [nlist, width] of `dtype`, u64 part_offsets [nlist+1] running from
+    0 to nrows, u64 row ids."""
+    assert d.centroids.shape == (d.nlist, width) and d.centroids.dtype == dtype
+    assert d.part_offsets.shape == (d.nlist + 1,) and d.part_offsets.dtype == np.uint64
+    assert int(d.part_offsets[0]) == 0 and int(d.part_offsets[-1]) == d.nrows
+    assert d.row_ids.dtype == np.uint64
+
+
+def _partition_order(assign, nlist: int, row_ids):
+    """Rows grouped by partition, ascending row id within each: (order, a torch tensor of row positions;
+    part_offsets u64 [nlist+1]; the row ids (0..n-1 when row_ids is None) as u64 in that order)."""
+    import torch
+    assign = torch.as_tensor(assign)
+    order = torch.argsort(assign, stable=True)
+    part_offsets = np.zeros(nlist + 1, np.uint64)
+    part_offsets[1:] = np.cumsum(torch.bincount(assign, minlength=nlist).cpu().numpy())
+    rid = np.arange(assign.shape[0], dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
+    return order, part_offsets, rid[order.cpu().numpy()]
+
+
 @dataclass
 class IvfPqIndexData:
+    index_type = "IVF_PQ"
     dim: int
     nlist: int
     m: int
@@ -85,12 +107,9 @@ class IvfPqIndexData:
         assert self.dim % self.m == 0
         if self.num_bits == 4:
             assert self.m % 2 == 0 and self.m <= PQ4_MAX_M
-        assert self.centroids.shape == (self.nlist, self.dim) and self.centroids.dtype == np.float32
+        _check_ivf_layout(self, self.dim, np.float32)
         assert self.codebook.shape == (self.m, 1 << self.num_bits, self.dsub) and self.codebook.dtype == np.float32
-        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
-        assert int(self.part_offsets[-1]) == self.nrows
         assert self.codes_t.dtype == np.uint8 and self.codes_t.size == self.nrows * self.code_bytes
-        assert self.row_ids.dtype == np.uint64
 
     def partition_codes(self, p: int) -> np.ndarray:
         """[code_bytes, n_p] code bytes of partition p."""
@@ -318,10 +337,7 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
         d = cbn[:, None, :] - 2.0 * torch.bmm(r, codebook.transpose(1, 2))
         codes[s:s + encode_chunk] = d.argmin(2).transpose(0, 1).to(torch.uint8)
 
-    order = torch.argsort(assign, stable=True)                            # ascending row id per partition
-    sizes = torch.bincount(assign, minlength=nlist).cpu().numpy().astype(np.int64)
-    part_offsets = np.zeros(nlist + 1, np.uint64)
-    part_offsets[1:] = np.cumsum(sizes)
+    order, part_offsets, rid = _partition_order(assign, nlist, row_ids)
     codes_sorted = codes[order].cpu().numpy()                              # [n, m] partition order
     if num_bits == 4:
         codes_sorted = pack_pq4(codes_sorted)                              # [n, m/2]
@@ -331,13 +347,11 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
         a, b = int(part_offsets[p]), int(part_offsets[p + 1])
         if b > a:
             codes_t[a * w:b * w] = codes_sorted[a:b].T.reshape(-1)
-    order_np = order.cpu().numpy()
-    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
     data = IvfPqIndexData(
         dim=dim, nlist=nlist, m=m, metric=metric,
         centroids=centroids.cpu().numpy().astype(np.float32),
         codebook=codebook.cpu().numpy().astype(np.float32),
-        part_offsets=part_offsets, codes_t=codes_t, row_ids=rid[order_np],
+        part_offsets=part_offsets, codes_t=codes_t, row_ids=rid,
         vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None), num_bits=num_bits)
     data.validate()
     return data
@@ -370,6 +384,7 @@ class IvfSqIndexData:
     """The plain-array form of an IVF_SQ index (lance `IvfSq`, rust/lancedb/src/index/vector.rs:216-256): IVF centroids,
     one global quantiser range [lo, hi] and one 8-bit code per dimension of every row, grouped by partition.  The same
     arrays go to `lgpu_ivf_sq_open` and to the CPU oracle (tests/sq_oracle.c)."""
+    index_type = "IVF_SQ"
     dim: int
     nlist: int
     metric: str
@@ -388,11 +403,8 @@ class IvfSqIndexData:
     def validate(self) -> None:
         assert self.metric in SQ_METRICS
         assert 1 <= self.dim <= SQ_MAX_DIM
-        assert self.centroids.shape == (self.nlist, self.dim) and self.centroids.dtype == np.float32
-        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
-        assert int(self.part_offsets[-1]) == self.nrows
+        _check_ivf_layout(self, self.dim, np.float32)
         assert self.codes.shape == (self.nrows, self.dim) and self.codes.dtype == np.uint8
-        assert self.row_ids.dtype == np.uint64
         assert np.isfinite(self.lo) and np.isfinite(self.hi) and self.lo <= self.hi
 
 
@@ -431,15 +443,10 @@ def train_ivf_sq(vectors, *, num_partitions: Optional[int] = None, distance_type
     x, samp, centroids, assign, _ = _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes)
     s = samp.detach().cpu().numpy()
     lo, hi = (float(np.min(s)), float(np.max(s))) if s.size else (0.0, 0.0)
-    order = torch.argsort(assign, stable=True)                            # ascending row id per partition
-    sizes = torch.bincount(assign, minlength=nlist).cpu().numpy().astype(np.int64)
-    part_offsets = np.zeros(nlist + 1, np.uint64)
-    part_offsets[1:] = np.cumsum(sizes)
-    order_np = order.cpu().numpy()
-    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
+    order, part_offsets, rid = _partition_order(assign, nlist, row_ids)
     data = IvfSqIndexData(
         dim=dim, nlist=nlist, metric=metric, centroids=centroids.cpu().numpy().astype(np.float32),
-        part_offsets=part_offsets, codes=sq_encode(x[order].cpu().numpy(), lo, hi), row_ids=rid[order_np],
+        part_offsets=part_offsets, codes=sq_encode(x[order].cpu().numpy(), lo, hi), row_ids=rid,
         lo=lo, hi=hi, vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
     data.validate()
     return data
@@ -456,6 +463,7 @@ class IvfRqIndexData:
     vector.rs:321-369): IVF centroids, one f32 orthogonal rotation P and, for every row of partition p with
     o = P (x - c_p), one sign bit per dimension (LSB first) and the factors add = |o|^2, scale = -2 |o|^2 / sum |o_i|,
     grouped by partition.  The same arrays go to `lgpu_ivf_rq_open` and to the CPU oracle (tests/rq_oracle.c)."""
+    index_type = "IVF_RQ"
     dim: int
     nlist: int
     metric: str
@@ -476,14 +484,11 @@ class IvfRqIndexData:
     def validate(self) -> None:
         assert self.metric in RQ_METRICS and self.num_bits == 1
         assert 1 <= self.dim <= RQ_MAX_DIM
-        assert self.centroids.shape == (self.nlist, self.dim) and self.centroids.dtype == np.float32
+        _check_ivf_layout(self, self.dim, np.float32)
         assert self.rotation.shape == (self.dim, self.dim) and self.rotation.dtype == np.float32
-        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
-        assert int(self.part_offsets[-1]) == self.nrows
         assert self.codes.shape == (self.nrows, (self.dim + 7) // 8) and self.codes.dtype == np.uint8
         assert self.add_factors.shape == (self.nrows,) and self.add_factors.dtype == np.float32
         assert self.scale_factors.shape == (self.nrows,) and self.scale_factors.dtype == np.float32
-        assert self.row_ids.dtype == np.uint64
 
 
 def rq_rotation(dim: int, seed: int = 45, device=None) -> np.ndarray:
@@ -553,16 +558,11 @@ def train_ivf_rq(vectors, *, num_partitions: Optional[int] = None, distance_type
     x, _, centroids, assign, _ = _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes)
     cent = centroids.cpu().numpy().astype(np.float32)
     P = rq_rotation(dim, seed, x.device)
-    order = torch.argsort(assign, stable=True)                            # ascending row id per partition
-    sizes = torch.bincount(assign, minlength=nlist).cpu().numpy().astype(np.int64)
-    part_offsets = np.zeros(nlist + 1, np.uint64)
-    part_offsets[1:] = np.cumsum(sizes)
+    order, part_offsets, rid = _partition_order(assign, nlist, row_ids)
     codes, add, scale = rq_encode(x[order], cent, assign[order], P)
-    order_np = order.cpu().numpy()
-    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
     data = IvfRqIndexData(
         dim=dim, nlist=nlist, metric=metric, centroids=cent, rotation=P, part_offsets=part_offsets, codes=codes,
-        add_factors=add, scale_factors=scale, row_ids=rid[order_np],
+        add_factors=add, scale_factors=scale, row_ids=rid,
         vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None))
     data.validate()
     return data
@@ -577,6 +577,7 @@ class IvfBinaryIndexData:
     """The plain-array form of a binary IVF_FLAT index (lance `IvfFlat` with distance_type "hamming",
     rust/lancedb/src/index/vector.rs:169-209): packed bit-vector centroids and the packed rows grouped by partition.  The
     same arrays go to `lgpu_ivf_binary_open` and to the CPU oracle (tests/ivf_binary_oracle.c)."""
+    index_type = "IVF_FLAT"
     nbytes: int
     nlist: int
     centroids: np.ndarray      # u8 [nlist, nbytes] packed bits
@@ -592,11 +593,8 @@ class IvfBinaryIndexData:
     def validate(self) -> None:
         assert self.metric == "hamming"
         assert 1 <= self.nbytes and 8 * self.nbytes <= HAMMING_MAX_BITS
-        assert self.centroids.shape == (self.nlist, self.nbytes) and self.centroids.dtype == np.uint8
-        assert self.part_offsets.shape == (self.nlist + 1,) and self.part_offsets.dtype == np.uint64
-        assert int(self.part_offsets[0]) == 0 and int(self.part_offsets[-1]) == self.nrows
+        _check_ivf_layout(self, self.nbytes, np.uint8)
         assert self.vectors.shape == (self.nrows, self.nbytes) and self.vectors.dtype == np.uint8
-        assert self.row_ids.dtype == np.uint64
 
 
 def _unpack_bits(x, device, dtype):
@@ -677,12 +675,9 @@ def train_ivf_binary(vectors, *, num_partitions: Optional[int] = None, distance_
             break
         cent = new
     assign = kmodes_assign(x, cent, device) if n else np.zeros(0, np.int64)
-    order = np.argsort(assign, kind="stable")                         # ascending row id per partition
-    part_offsets = np.zeros(nlist + 1, np.uint64)
-    part_offsets[1:] = np.cumsum(np.bincount(assign, minlength=nlist))
-    rid = np.arange(n, dtype=np.uint64) if row_ids is None else np.asarray(row_ids, np.uint64)
+    order, part_offsets, rid = _partition_order(assign, nlist, row_ids)
     data = IvfBinaryIndexData(nbytes=nbytes, nlist=nlist, centroids=np.ascontiguousarray(cent, np.uint8),
-                              part_offsets=part_offsets, vectors=np.ascontiguousarray(x[order]), row_ids=rid[order])
+                              part_offsets=part_offsets, vectors=np.ascontiguousarray(x[order.numpy()]), row_ids=rid)
     data.validate()
     return data
 
@@ -706,6 +701,7 @@ class IvfHnswSqIndexData:
       entry        u32 [nlist]     the entry row of each partition (HNSW_NONE when empty); its level is top_level
       top_level    u8  [nlist]
     The same arrays go to `lgpu_ivf_hnsw_sq_open` and to the CPU oracle (tests/hnsw_sq_oracle.c)."""
+    index_type = "IVF_HNSW_SQ"
     sq: IvfSqIndexData
     m: int
     levels: np.ndarray
@@ -882,3 +878,38 @@ def train_ivf_hnsw_sq(vectors, *, num_partitions: Optional[int] = None, distance
     data = IvfHnswSqIndexData(sq, m, *g)
     data.validate()
     return data
+
+
+# --------------------------------------------------------------------------------------
+@dataclass(frozen=True)
+class IvfKind:
+    """One IVF index kind as `Table.create_index` builds it: what it accepts, how it is trained and which `_native`
+    handle class opens its data.  The refusals are formatted with the value given (`kind`, `metric`, `num_bits`)."""
+    index_type: str
+    data: type                       # its IndexData class
+    train: Callable
+    handle: str
+    metrics: Tuple[str, ...]
+    metric_error: str
+    num_bits: Tuple[int, ...] = ()   # () = any: the kind has no num_bits and create_index's is ignored
+    num_bits_error: str = ""
+    max_dim: Optional[int] = None    # a dimension bound checked before training
+    params: Tuple[str, ...] = ()     # create_index arguments passed on to `train` besides the ones every kind takes
+    column: str = "float"            # the vector column it indexes: "float" or "binary"
+
+
+_L2_COSINE = "{kind} supports the l2 and cosine distance types, not {metric!r}"
+IVF_KINDS = {k.index_type: k for k in (
+    IvfKind("IVF_PQ", IvfPqIndexData, train_ivf_pq, "GpuIvfPq", METRICS, "unknown distance_type {metric!r}", (4, 8),
+            "IVF_PQ supports num_bits 4 or 8, got num_bits={num_bits}", params=("num_sub_vectors", "num_bits")),
+    IvfKind("IVF_SQ", IvfSqIndexData, train_ivf_sq, "GpuIvfSq", SQ_METRICS, _L2_COSINE, (8,),
+            "only num_bits=8 is supported"),
+    IvfKind("IVF_HNSW_SQ", IvfHnswSqIndexData, train_ivf_hnsw_sq, "GpuIvfHnswSq", SQ_METRICS, _L2_COSINE, (8,),
+            "only num_bits=8 is supported", params=("m", "ef_construction")),
+    # RaBitQ with 1 bit per dimension only (extended RaBitQ is not served): the legacy default of 8 is refused rather
+    # than quietly building a 1-bit index
+    IvfKind("IVF_RQ", IvfRqIndexData, train_ivf_rq, "GpuIvfRq", RQ_METRICS, _L2_COSINE, (1,),
+            "IVF_RQ supports num_bits=1 only, got num_bits={num_bits}", max_dim=RQ_MAX_DIM, params=("num_bits",)),
+    IvfKind("IVF_FLAT", IvfBinaryIndexData, train_ivf_binary, "GpuIvfBinary", ("hamming",),
+            "IVF_FLAT over binary vectors supports the hamming distance type only, not {metric!r}", column="binary"),
+)}

@@ -10,14 +10,13 @@ row positions, like a single-fragment Lance dataset.
 """
 from __future__ import annotations
 
-from typing import Dict, Iterable, List, Optional, Union
+from typing import Dict, Iterable, List, Optional
 
 import numpy as np
 import pyarrow as pa
 
 from . import _native
-from .index import (RQ_MAX_DIM, IvfBinaryIndexData, IvfHnswSqIndexData, IvfPqIndexData, IvfRqIndexData,
-                    IvfSqIndexData, train_ivf_binary, train_ivf_hnsw_sq, train_ivf_pq, train_ivf_rq, train_ivf_sq)
+from .index import IVF_KINDS
 from .query import LanceVectorQueryBuilder
 
 
@@ -75,6 +74,14 @@ def _is_binary_type(t: pa.DataType) -> bool:
     return pa.types.is_fixed_size_list(t) and pa.types.is_uint8(t.value_type)
 
 
+# create_index's refusal of a column of the other kind, by the column an index kind needs
+_WRONG_COLUMN = {
+    "float": "no index over binary vectors on the GPU path: search them flat (hamming)",
+    "binary": "IVF_FLAT is served over binary (fixed_size_list<uint8>) columns only; index float columns with IVF_PQ, "
+              "IVF_SQ or IVF_RQ",
+}
+
+
 class Table:
     def __init__(self, name: str, data: pa.Table, device: int = 0):
         self.name = name
@@ -84,7 +91,7 @@ class Table:
         self._binary: Dict[str, _native.GpuBinary] = {}
         self._multivec: Dict[str, _native.GpuMultivec] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
-        self._index_data: Dict[str, Union[IvfPqIndexData, IvfSqIndexData, IvfRqIndexData, IvfBinaryIndexData]] = {}
+        self._index_data: Dict[str, object] = {}      # the IndexData of one of IVF_KINDS
 
     # ---- introspection ----
     @property
@@ -104,12 +111,7 @@ class Table:
         return self._data.to_pandas()
 
     def _index_type(self, column: str) -> str:
-        d = self._index_data[column]
-        if isinstance(d, IvfBinaryIndexData):
-            return "IVF_FLAT"
-        if isinstance(d, IvfHnswSqIndexData):
-            return "IVF_HNSW_SQ"
-        return "IVF_SQ" if isinstance(d, IvfSqIndexData) else ("IVF_RQ" if isinstance(d, IvfRqIndexData) else "IVF_PQ")
+        return self._index_data[column].index_type
 
     def list_indices(self):
         return [{"name": f"{c}_idx", "index_type": self._index_type(c), "columns": [c]} for c in self._index]
@@ -160,82 +162,38 @@ class Table:
                      replace: bool = True, accelerator: Optional[str] = None, index_type: str = "IVF_PQ",
                      num_bits: int = 8, max_iterations: int = 50, sample_rate: int = 256, m: int = 20,
                      ef_construction: int = 300, **_ignored):
-        kind = index_type.upper()
-        if kind == "IVF_FLAT":             # binary columns only: IvfFlat(distance_type="hamming")
-            column = vector_column_name or self._infer_vector_column(None)
-            if self._is_multivec(column):
-                raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
-            if not self._is_binary(column):
-                raise NotImplementedError("IVF_FLAT is served over binary (fixed_size_list<uint8>) columns only; index "
-                                          "float columns with IVF_PQ, IVF_SQ or IVF_RQ")
-            if metric.lower() != "hamming":
-                raise ValueError(f"IVF_FLAT over binary vectors supports the hamming distance type only, not {metric!r}")
-            if column in self._index and not replace:
-                raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")
-            dev = f"cuda:{self._device}" if accelerator in ("cuda", "gpu") else None
-            self._attach_index(column, train_ivf_binary(self._binary_vectors(column), num_partitions=num_partitions,
-                                                        max_iterations=max_iterations, sample_rate=sample_rate,
-                                                        device=dev))
-            return
-        if kind not in ("IVF_PQ", "IVF_SQ", "IVF_RQ", "IVF_HNSW_SQ"):
+        kind = IVF_KINDS.get(index_type.upper())
+        if kind is None:
             raise NotImplementedError("only IVF_PQ, IVF_SQ, IVF_HNSW_SQ and IVF_RQ are on the GPU hot path")
-        if kind == "IVF_RQ" and num_bits != 1:
-            # RaBitQ with 1 bit per dimension only (extended RaBitQ is not served); the legacy default of 8 is refused
-            # rather than quietly building a 1-bit index
-            raise ValueError(f"IVF_RQ supports num_bits=1 only, got num_bits={num_bits}")
-        if kind == "IVF_PQ" and num_bits not in (4, 8):
-            raise ValueError(f"IVF_PQ supports num_bits 4 or 8, got num_bits={num_bits}")
-        if kind in ("IVF_SQ", "IVF_HNSW_SQ") and num_bits != 8:
-            raise ValueError("only num_bits=8 is supported")
+        if kind.num_bits and num_bits not in kind.num_bits:
+            raise ValueError(kind.num_bits_error.format(num_bits=num_bits))
         column = vector_column_name or self._infer_vector_column(None)
-        if self._is_binary(column):
-            raise NotImplementedError("no index over binary vectors on the GPU path: search them flat (hamming)")
         if self._is_multivec(column):
             raise NotImplementedError("no index over multivector columns on the GPU path: they are searched flat")
-        if kind in ("IVF_SQ", "IVF_HNSW_SQ", "IVF_RQ") and metric.lower() not in ("l2", "cosine"):
-            raise ValueError(f"{kind} supports the l2 and cosine distance types, not {metric!r}")
-        if kind == "IVF_RQ" and self._dim(column) > RQ_MAX_DIM:
-            raise ValueError(f"IVF_RQ supports dimensions up to {RQ_MAX_DIM}, got {self._dim(column)}")
+        if self._is_binary(column) != (kind.column == "binary"):
+            raise NotImplementedError(_WRONG_COLUMN[kind.column])
+        if metric.lower() not in kind.metrics:
+            raise ValueError(kind.metric_error.format(kind=kind.index_type, metric=metric))
+        if kind.max_dim is not None and self._dim(column) > kind.max_dim:
+            raise ValueError(f"{kind.index_type} supports dimensions up to {kind.max_dim}, got {self._dim(column)}")
         if column in self._index and not replace:
             raise RuntimeError(f"index {column}_idx already exists (pass replace=True)")   # python/python/tests/test_index.py:357
-        dev = None
-        if accelerator in ("cuda", "gpu"):
-            dev = f"cuda:{self._device}"
-        if kind == "IVF_SQ":               # IvfSqIndexBuilder: distance_type, num_partitions, max_iterations, sample_rate
-            self._attach_index(column, train_ivf_sq(self._vectors(column), num_partitions=num_partitions,
-                                                    distance_type=metric, max_iterations=max_iterations,
-                                                    sample_rate=sample_rate, keep_vectors=True, device=dev,
-                                                    native_passes=dev is not None))
-            return
-        if kind == "IVF_HNSW_SQ":          # HnswSq: distance_type, num_partitions, m, ef_construction, max_iterations, sample_rate
-            self._attach_index(column, train_ivf_hnsw_sq(self._vectors(column), num_partitions=num_partitions,
-                                                         distance_type=metric, m=m, ef_construction=ef_construction,
-                                                         max_iterations=max_iterations, sample_rate=sample_rate,
-                                                         keep_vectors=True, device=dev, native_passes=dev is not None))
-            return
-        if kind == "IVF_RQ":               # IvfRqIndexBuilder: distance_type, num_partitions, num_bits, max_iterations, sample_rate
-            self._attach_index(column, train_ivf_rq(self._vectors(column), num_partitions=num_partitions,
-                                                    distance_type=metric, num_bits=num_bits,
-                                                    max_iterations=max_iterations, sample_rate=sample_rate,
-                                                    keep_vectors=True, device=dev, native_passes=dev is not None))
-            return
-        data = train_ivf_pq(self._vectors(column), num_partitions=num_partitions,
-                            num_sub_vectors=num_sub_vectors, distance_type=metric,
-                            max_iterations=max_iterations, sample_rate=sample_rate,
-                            keep_vectors=True, device=dev, num_bits=num_bits,
-                            native_passes=dev is not None)      # accelerator: row passes through the C ABI (build.cu)
-        self._attach_index(column, data)
+        dev = f"cuda:{self._device}" if accelerator in ("cuda", "gpu") else None
+        args = {"num_sub_vectors": num_sub_vectors, "num_bits": num_bits, "m": m, "ef_construction": ef_construction}
+        kw = {p: args[p] for p in kind.params}
+        if kind.column == "binary":
+            vectors = self._binary_vectors(column)
+        else:       # accelerator: the row passes run through the C ABI (build.cu); keep the raw vectors for refine
+            vectors = self._vectors(column)
+            kw.update(keep_vectors=True, native_passes=dev is not None)
+        self._attach_index(column, kind.train(vectors, num_partitions=num_partitions, distance_type=metric,
+                                              max_iterations=max_iterations, sample_rate=sample_rate, device=dev, **kw))
 
-    def _attach_index(self, column: str,
-                      data: Union[IvfPqIndexData, IvfSqIndexData, IvfHnswSqIndexData, IvfRqIndexData,
-                                  IvfBinaryIndexData]):
+    def _attach_index(self, column: str, data):
         if column in self._index:
             self._index[column].close()
         self._index_data[column] = data
-        cls = (_native.GpuIvfBinary if isinstance(data, IvfBinaryIndexData) else
-               _native.GpuIvfHnswSq if isinstance(data, IvfHnswSqIndexData) else
-               _native.GpuIvfSq if isinstance(data, IvfSqIndexData) else
-               _native.GpuIvfRq if isinstance(data, IvfRqIndexData) else _native.GpuIvfPq)
+        cls = getattr(_native, IVF_KINDS[data.index_type].handle)     # looked up now, so a replaced class is used
         self._index[column] = cls(data, device=self._device)
 
     # ---- on-disk Lance index (SURVEY.md 8f-3; layout [lance, recalled], see lance_index.py) ----
