@@ -336,7 +336,9 @@ int  lgpu_comm_last_stage_ms(lgpu_comm *comm, float *times);
  * building vector index", python/python/lancedb/table.py:2883-2937).  k-means training stays with the caller;
  * these are the two passes over every row, bit-consistent with the search kernels.  All pointers are HOST
  * memory; vectors are raw rows (normalised internally for LGPU_COSINE). ------------------------------- */
-/* out_parts[r] = the partition find_partitions(vectors[r], nprobes = 1) returns */
+/* out_parts[r] = the partition find_partitions(vectors[r], nprobes = 1) returns.  A row whose distance to every centroid
+ * is NaN has no partition, and the call fails with LGPU_INVALID_INPUT: a row holding a NaN, and under LGPU_COSINE an
+ * all-zero row (it has no direction: normalising it divides 0 by 0). */
 int lgpu_ivf_assign(const float *centroids, uint32_t nlist, uint32_t dim, int metric,
                     const float *vectors, uint64_t n, int device, uint32_t *out_parts);
 /* out_codes[r][i] (row-major [n][m]) = the codeword of sub-space i with the smallest distance-table entry
@@ -349,11 +351,13 @@ int lgpu_pq_encode(const float *centroids, const float *codebook, uint32_t nlist
  * rust/lancedb/src/index/vector.rs:286-297).  x: HOST [n][dim] training rows (already sampled, normalised for cosine).
  * centroids: in = initial centres (e.g. k sampled rows), out = trained centres.  Assignment is the search's own coarse
  * step (exact nearest centre), empty clusters keep their previous centre.  *inertia_out (optional) = sum of squared
- * distances of the rows to their nearest trained centre. */
+ * distances of the rows to their nearest trained centre.  iters = 0 runs one iteration.  Every row must be finite: a row
+ * holding a NaN or an infinity fails the call with LGPU_INVALID_INPUT before any device work. */
 int lgpu_kmeans_train(const float *x, uint64_t n, uint32_t dim, float *centroids, uint32_t k, uint32_t iters, int device,
                       double *inertia_out);
 /* the 256-entry PQ codebooks of all m sub-spaces: x = HOST [n][dim] rows to quantise (residuals for l2 / cosine, raw rows
- * for dot); codebook [m][256][dim/m] in = initial codewords, out = trained */
+ * for dot); codebook [m][256][dim/m] in = initial codewords, out = trained.  A codeword no row encodes to keeps its value;
+ * iters = 0 runs one iteration; a row holding a NaN or an infinity fails the call with LGPU_INVALID_INPUT. */
 int lgpu_pq_train(const float *x, uint64_t n, uint32_t dim, uint32_t m, float *codebook, uint32_t iters, int device);
 
 /* ---- flat / brute force (LanceRead -> KNNVectorDistance -> TopK) ---------

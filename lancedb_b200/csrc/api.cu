@@ -3635,12 +3635,25 @@ static void assign_nearest(const float *d_x, uint64_t n, uint32_t dim, const flo
     LGPU_CUDA(cudaStreamSynchronize(st));                            // the scratch buffers die with this scope
 }
 
+// a training row holding a NaN or an infinity would be summed into the centre (or codeword) it lands in and poison it:
+// an inf row has distance inf to every centre and goes to centre 0, a NaN row encodes to code 0 in every sub-space
+static void require_finite_rows(const float *x, uint64_t n, uint32_t dim)
+{
+    for (uint64_t r = 0; r < n; r++)
+        for (uint32_t t = 0; t < dim; t++)
+            if (!std::isfinite(x[r * dim + t])) {
+                set_error("training row " + std::to_string(r) + " holds a NaN or infinite value; training needs finite rows");
+                throw Failure{LGPU_INVALID_INPUT};
+            }
+}
+
 int lgpu_kmeans_train(const float *x, uint64_t n, uint32_t dim, float *centroids, uint32_t k, uint32_t iters, int device,
                       double *inertia_out)
 {
     return guarded([&] {
         LGPU_REQUIRE(x && centroids && n > 0 && dim > 0 && k > 0, "null argument / empty shape");
         LGPU_REQUIRE(n < (1ull << 32), "too many training rows (sample them: sample_rate * num_partitions)");
+        require_finite_rows(x, n, dim);
         require_device(device);
         cudaDeviceProp prop;
         LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
@@ -3675,6 +3688,7 @@ int lgpu_pq_train(const float *x, uint64_t n, uint32_t dim, uint32_t m, float *c
         LGPU_REQUIRE(x && codebook && n > 0 && dim > 0 && m > 0, "null argument / empty shape");
         LGPU_REQUIRE(dim % m == 0 && scan_dsub_supported(dim / m),
                      "unsupported PQ sub-vector length (dim/num_sub_vectors must be 1,2,4,8,16 or 32)");
+        require_finite_rows(x, n, dim);
         require_device(device);
         cudaStream_t st = nullptr;
         const uint32_t dsub = dim / m;

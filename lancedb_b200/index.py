@@ -228,12 +228,18 @@ def _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes
     lgpu_ivf_assign), so a row lands in the partition its own vector probes first.
     Returns (x normalised for cosine, sample, centroids, assign, device ordinal).
     A NaN or infinite component anywhere is refused: k-means would spread it into a centroid, and a row with no finite
-    centroid distance has no partition."""
+    centroid distance has no partition.  So is an all-zero row under cosine (any row whose squared norm is 0 in f32): it
+    has no direction, and its distance to every centroid is NaN."""
     import torch
     bad = ~torch.isfinite(x).all(dim=1)
     if bool(bad.any()):
         raise ValueError(f"vector {int(bad.nonzero()[0, 0])} holds a NaN or infinite value; IVF training needs finite "
                          f"vectors")
+    if metric == "cosine":
+        zero = (x * x).sum(dim=1) == 0
+        if bool(zero.any()):
+            raise ValueError(f"vector {int(zero.nonzero()[0, 0])} has norm 0; a cosine index needs vectors with a "
+                             f"direction")
     n = x.shape[0]
     raw = x
     if metric == "cosine":
