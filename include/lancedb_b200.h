@@ -381,6 +381,29 @@ int  lgpu_flat_search_device(lgpu_flat *fl, int metric, const float *d_queries, 
                              const lgpu_search_params *params,
                              uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count,
                              void *cuda_stream);
+/* Append n rows (HOST [n][dim]) to the column; row_ids NULL => the positions that follow (nrows, nrows + 1, ...).
+ * Afterwards the handle returns, on every entry point, exactly what lgpu_flat_open on the concatenated rows (and
+ * ids) returns.  The call takes the handle alone: it waits for the calls inside it, keeps new ones out, and drains the
+ * device before it moves or rewrites a buffer, so a device-route search enqueued earlier still reads what it was given.
+ * Storage grows geometrically; the derived data (bf16 copy, |x|^2, norms) is computed for the new rows only. */
+int  lgpu_flat_append(lgpu_flat *fl, const float *rows, uint64_t n, const uint64_t *row_ids);
+
+/* ---- rows added after an index was built (the reference's unindexed fragments, searched unless fast_search is set;
+ * rust/lancedb/src/table/query.rs:289-290).  `tail` holds them.  The result is the top-k by (_distance, _rowid) of
+ * the union of
+ *   - lgpu_search_filtered's result on the index (k x refine_factor candidates refined to k, maximum_nprobes widening
+ *     under a prefilter), and
+ *   - the exact flat top-k of the tail under the index's metric (lgpu_flat_search_filtered with the same k),
+ * with distance_range and the allow bitmap (over row ids, NULL = no prefilter) applied to both.  k up to LGPU_K_MAX;
+ * the tail must have the index's dimension and device.  The host entry point honours timeout_ms; the device entry point
+ * takes every buffer, `allow` included, in DEVICE memory and is enqueued on `cuda_stream`, not synchronised.  The call
+ * uses a workspace of each handle, each within LGPU_WS_BYTES, plus the two [B][k] lists it merges (DESIGN.md section 2). */
+int  lgpu_search_unindexed(lgpu_index *ix, lgpu_flat *tail, const float *queries, uint32_t B,
+                           const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                           uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+int  lgpu_search_unindexed_device(lgpu_index *ix, lgpu_flat *tail, const float *d_queries, uint32_t B,
+                                  const lgpu_search_params *params, const uint32_t *d_allow, uint64_t allow_bits,
+                                  uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
 
 /* ---- binary vectors: flat search by Hamming distance (the `is_binary` branch of
  * rust/lancedb/src/table/query.rs:229-236: fixed_size_list<uint8, nbytes> columns, distance_type("hamming")) ----
@@ -400,6 +423,8 @@ int  lgpu_binary_search_filtered(lgpu_binary *bx, const uint8_t *queries, uint32
 /* all five buffers in DEVICE memory, enqueued on `cuda_stream`, not synchronised */
 int  lgpu_binary_search_device(lgpu_binary *bx, const uint8_t *d_queries, uint32_t B, const lgpu_search_params *params,
                                uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
+/* Append n rows (HOST [n][nbytes]); everything else as lgpu_flat_append. */
+int  lgpu_binary_append(lgpu_binary *bx, const uint8_t *rows, uint64_t n, const uint64_t *row_ids);
 
 /* ---- binary IVF_FLAT (lance `IvfFlat` with distance_type("hamming"), the index LanceDB builds over
  * fixed_size_list<uint8, nbytes> columns; rust/lancedb/src/index/vector.rs:169-209): packed binary centroids and the
@@ -431,6 +456,14 @@ int  lgpu_ivf_binary_search_filtered(lgpu_ivf_binary *ix, const uint8_t *queries
 int  lgpu_ivf_binary_search_device(lgpu_ivf_binary *ix, const uint8_t *d_queries, uint32_t B,
                                    const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
                                    uint32_t *d_out_count, void *cuda_stream);
+/* lgpu_search_unindexed[_device] for a binary IVF_FLAT index and a binary tail (Hamming distance on both lists) */
+int  lgpu_ivf_binary_search_unindexed(lgpu_ivf_binary *ix, lgpu_binary *tail, const uint8_t *queries, uint32_t B,
+                                      const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                                      uint64_t *out_ids, float *out_dist, uint32_t *out_count);
+int  lgpu_ivf_binary_search_unindexed_device(lgpu_ivf_binary *ix, lgpu_binary *tail, const uint8_t *d_queries,
+                                             uint32_t B, const lgpu_search_params *params, const uint32_t *d_allow,
+                                             uint64_t allow_bits, uint64_t *d_out_ids, float *d_out_dist,
+                                             uint32_t *d_out_count, void *cuda_stream);
 
 /* ---- multivector columns: exact late-interaction (MaxSim) flat search (the `DataType::List` branch of
  * rust/lancedb/src/table/query.rs:180-199: list<fixed_size_list<float, dim>> columns; the query's vectors are packed

@@ -45,6 +45,8 @@ EXPORTS = [
     "lgpu_debug_pq4_sums",
     "lgpu_ivf_binary_open", "lgpu_ivf_binary_close", "lgpu_ivf_binary_search", "lgpu_ivf_binary_search_filtered",
     "lgpu_ivf_binary_search_device", "lgpu_debug_ivf_hamming_scan",
+    "lgpu_flat_append", "lgpu_binary_append", "lgpu_search_unindexed", "lgpu_search_unindexed_device",
+    "lgpu_ivf_binary_search_unindexed", "lgpu_ivf_binary_search_unindexed_device",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -216,6 +218,12 @@ def load():
     lib.lgpu_ivf_binary_search_filtered.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
     lib.lgpu_ivf_binary_search_device.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_debug_ivf_hamming_scan.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
+    lib.lgpu_flat_append.argtypes = [vp, vp, C.c_uint64, vp]
+    lib.lgpu_binary_append.argtypes = [vp, vp, C.c_uint64, vp]
+    for fn in ("lgpu_search_unindexed", "lgpu_ivf_binary_search_unindexed"):
+        getattr(lib, fn).argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
+        getattr(lib, fn + "_device").argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp,
+                                                 vp]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -282,6 +290,31 @@ def _host_search(fn: str, head, B: int, k: int, p: SearchParams, allow, allow_bi
         check(getattr(load(), fn + "_filtered")(*head, C.byref(p), _ptr(bm), int(allow_bits), _ptr(ids), _ptr(dist),
                                                 _ptr(cnt)))
     return ids, dist, cnt
+
+
+def _union_search(fn: str, ix, tail, q: np.ndarray, k: int, p: SearchParams, allow, allow_bits):
+    """Host-buffer union search through `fn` (lgpu_search_unindexed or its binary twin) of the index `ix` and the
+    tail handle `tail`: returns (ids [B,k] u64, dist [B,k] f32, count [B] u32)."""
+    B = q.shape[0]
+    ids = np.empty((B, k), np.uint64); dist = np.empty((B, k), np.float32); cnt = np.empty(B, np.uint32)
+    bm = None
+    if allow is not None:
+        bm = np.ascontiguousarray(allow, np.uint32)
+        if bm.size * 32 < allow_bits:
+            raise ValueError("allow bitmap shorter than allow_bits")
+    check(getattr(load(), fn)(ix._h, tail._h, _ptr(q), B, C.byref(p), _ptr(bm), int(allow_bits) if bm is not None else 0,
+                              _ptr(ids), _ptr(dist), _ptr(cnt)))
+    return ids, dist, cnt
+
+
+def _rows_ids(rows: np.ndarray, row_ids):
+    """The row ids an append passes: None, or one u64 per row."""
+    if row_ids is None:
+        return None
+    rid = np.ascontiguousarray(row_ids, np.uint64).reshape(-1)
+    if rid.size != rows.shape[0]:
+        raise ValueError("row_ids must hold one id per appended row")
+    return rid
 
 
 def binary_components(queries) -> np.ndarray:
@@ -383,6 +416,20 @@ class GpuIvfPq(_Handle):
     def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search (raw addresses), enqueued on `stream`, not synchronised."""
         check(load().lgpu_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
+
+    def search_unindexed(self, tail: "GpuFlat", queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None,
+                         allow=None, allow_bits=0, max_nprobes=0, timeout_ms=0, ef=0):
+        """search() over the index together with `tail`, the rows added after it was built (lgpu_search_unindexed):
+        the top-k of the union of the index's result and the tail's exact top-k under the index's metric."""
+        q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
+        p = make_params(k, nprobes, refine_factor, lower, upper, max_nprobes, timeout_ms, ef)
+        return _union_search("lgpu_search_unindexed", self, tail, q, k, p, allow, allow_bits)
+
+    def search_unindexed_device(self, tail: "GpuFlat", d_q: int, B: int, p: SearchParams, d_allow: int, allow_bits: int,
+                                d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
+        """Device-pointer union search (raw addresses; d_allow = 0: no prefilter), enqueued on `stream`."""
+        check(load().lgpu_search_unindexed_device(self._h, tail._h, d_q, B, C.byref(p), d_allow or None,
+                                                  int(allow_bits), d_ids, d_dist, d_cnt, stream))
 
     def debug_sub_batch_size(self, B: int, nprobes: int) -> int:
         """Queries per sub-batch of a search of B queries over `nprobes` probes under this process's LGPU_WS_BYTES."""
@@ -494,6 +541,13 @@ class GpuFlat(_Handle):
         check(load().lgpu_flat_search_device(self._h, METRICS[metric], d_q, B, C.byref(p), d_ids, d_dist, d_cnt,
                                              stream))
 
+    def append(self, rows, row_ids=None):
+        """Append rows [n, dim] in place (lgpu_flat_append); row_ids None = the positions that follow."""
+        v = np.ascontiguousarray(rows, np.float32).reshape(-1, self.dim)
+        rid = _rows_ids(v, row_ids)
+        check(load().lgpu_flat_append(self._h, _ptr(v), v.shape[0], _ptr(rid)))
+        self.nrows += v.shape[0]
+
 
 class GpuBinary(_Handle):
     """A packed binary vector column (fixed_size_list<uint8, nbytes>) pinned in HBM (lgpu_binary), searched by
@@ -522,6 +576,15 @@ class GpuBinary(_Handle):
     def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search (raw addresses; queries [B][nbytes] u8), enqueued on `stream`, not synchronised."""
         check(load().lgpu_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
+
+    def append(self, rows, row_ids=None):
+        """Append packed rows [n, nbytes] in place (lgpu_binary_append); row_ids None = the positions that follow."""
+        v = np.ascontiguousarray(rows, np.uint8)
+        if v.ndim != 2 or v.shape[1] != self.nbytes:
+            raise ValueError(f"binary rows must be [n, {self.nbytes}] uint8")
+        rid = _rows_ids(v, row_ids)
+        check(load().lgpu_binary_append(self._h, _ptr(v), v.shape[0], _ptr(rid)))
+        self.nrows += v.shape[0]
 
 
 class GpuIvfBinary(_Handle):
@@ -554,6 +617,19 @@ class GpuIvfBinary(_Handle):
     def search_device(self, d_q: int, B: int, p: SearchParams, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
         """Device-pointer search (raw addresses; queries [B][nbytes] u8), enqueued on `stream`, not synchronised."""
         check(load().lgpu_ivf_binary_search_device(self._h, d_q, B, C.byref(p), d_ids, d_dist, d_cnt, stream))
+
+    def search_unindexed(self, tail: "GpuBinary", queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None,
+                         allow=None, allow_bits=0, max_nprobes=0, timeout_ms=0):
+        """search() over the index together with `tail` (lgpu_ivf_binary_search_unindexed), Hamming on both."""
+        q = self._queries(queries)
+        p = make_params(k, nprobes, refine_factor, lower, upper, max_nprobes, timeout_ms)
+        return _union_search("lgpu_ivf_binary_search_unindexed", self, tail, q, k, p, allow, allow_bits)
+
+    def search_unindexed_device(self, tail: "GpuBinary", d_q: int, B: int, p: SearchParams, d_allow: int,
+                                allow_bits: int, d_ids: int, d_dist: int, d_cnt: int, stream: int = 0):
+        """Device-pointer union search (raw addresses; d_allow = 0: no prefilter), enqueued on `stream`."""
+        check(load().lgpu_ivf_binary_search_unindexed_device(self._h, tail._h, d_q, B, C.byref(p), d_allow or None,
+                                                             int(allow_bits), d_ids, d_dist, d_cnt, stream))
 
 
 def multivec_offsets(lengths) -> np.ndarray:

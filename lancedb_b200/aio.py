@@ -185,6 +185,7 @@ class AsyncVectorQuery(_AsyncQueryBase):
         self._refine_factor: Optional[int] = None
         self._ef: Optional[int] = None
         self._use_index = True
+        self._fast_search = False
 
     def add_query_vector(self, vector):
         self._vectors.append(np.asarray(vector, np.float32))
@@ -237,6 +238,10 @@ class AsyncVectorQuery(_AsyncQueryBase):
         self._use_index = False
         return self
 
+    def fast_search(self):                       # skip the rows the index does not hold yet (query.py:3250)
+        self._fast_search = True
+        return self
+
     def _builder(self):
         dims = {v.shape[-1] for v in self._vectors}
         if len(dims) != 1 or any(v.ndim != 1 for v in self._vectors):
@@ -262,6 +267,8 @@ class AsyncVectorQuery(_AsyncQueryBase):
             b.with_row_id(True)
         if not self._use_index:
             b.bypass_vector_index()
+        if self._fast_search:
+            b.fast_search()
         if self._where is not None:
             b.where(self._where, prefilter=not self._postfilter)
         return b
@@ -300,6 +307,13 @@ class AsyncTable:
 
     async def prewarm_index(self, name: str):
         return self._table.prewarm_index(name)
+
+    async def add(self, data, mode: str = "append") -> None:
+        await asyncio.to_thread(self._table.add, data, mode=mode)
+
+    async def optimize(self, *, cleanup_older_than=None, delete_unverified: bool = False, retrain: bool = False) -> None:
+        await asyncio.to_thread(self._table.optimize, cleanup_older_than=cleanup_older_than,
+                                delete_unverified=delete_unverified, retrain=retrain)
 
     def query(self) -> AsyncQuery:
         return AsyncQuery(self._table)

@@ -18,6 +18,7 @@
 #include <mutex>
 #include <thread>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include <dlfcn.h>
@@ -134,6 +135,7 @@ struct Workspace {
     DevBuf rq_q, rq_planes, rq_slots;   // IVF_RQ search: rotated queries [B][dim], per-slot bit-planes and grids
     DevBuf pq4_tab, pq4_slots;          // 4-bit IVF_PQ search: per-slot u8 tables [slots][m][16] and quantisers
     DevBuf sel_large;                   // the large select's scratch (k > SELECT_KMAX, select_large.cu)
+    DevBuf u_ids, u_dist, u_cnt;        // union search: the index's and the tail's top-k, [2][B][k] and [2][B]
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -198,6 +200,9 @@ template <> constexpr HandleKind handle_kind<lgpu_comm>() { return HandleKind::c
 static std::mutex g_live_mu;
 static std::condition_variable g_live_cv;
 static std::unordered_map<const void *, HandleKind> g_live;
+// handles an append holds exclusively (HandleExcl): a call that would enter one waits until the append is done, and so
+// does the close of one (retire_handle)
+static std::unordered_set<const void *> g_excl;
 static std::atomic<bool> g_cuda_touched{false};   // this process has created a CUDA context through the library
 static std::atomic<bool> g_fork_poisoned{false};  // we are the child of a fork() taken after that
 // fork(): the reference rebuilds its tokio runtime in the child (python/src/runtime.rs:68-81); a CUDA context has
@@ -234,7 +239,8 @@ template <class H> struct HandleRef {
     H *h;
     explicit HandleRef(H *p) : h(nullptr)
     {
-        std::lock_guard<std::mutex> g(g_live_mu);
+        std::unique_lock<std::mutex> g(g_live_mu);
+        g_live_cv.wait(g, [&] { return g_excl.empty() || !g_excl.count(p); });
         require_live(p, handle_kind<H>());
         p->refs.fetch_add(1);
         h = p;
@@ -245,6 +251,35 @@ template <class H> struct HandleRef {
     }
     H *operator->() const { return h; }
 };
+// the handle alone: waits for the calls inside it to finish and keeps new ones out until released (close waits too)
+template <class H> struct HandleExcl {
+    H *h;
+    explicit HandleExcl(H *p) : h(nullptr)
+    {
+        std::unique_lock<std::mutex> g(g_live_mu);
+        g_live_cv.wait(g, [&] { return !g_excl.count(p); });
+        require_live(p, handle_kind<H>());
+        g_excl.insert(p);
+        g_live_cv.wait(g, [&] { return p->refs.load() == 0; });   // p stays allocated: close waits for g_excl
+        if (!g_live.count(p)) {                                    // closed meanwhile: let the close go on
+            g_excl.erase(p);
+            g_live_cv.notify_all();
+            set_error(std::string(handle_name(handle_kind<H>())) + " handle was closed during the append");
+            throw Failure{LGPU_INVALID_INPUT};
+        }
+        p->refs.fetch_add(1);
+        h = p;
+    }
+    ~HandleExcl()
+    {
+        if (!h) return;
+        std::lock_guard<std::mutex> g(g_live_mu);
+        h->refs.fetch_sub(1);
+        g_excl.erase(h);
+        g_live_cv.notify_all();
+    }
+    H *operator->() const { return h; }
+};
 // unregister and wait until no call is inside the handle any more; false = it was not a live handle of kind H
 template <class H> static bool retire_handle(H *p)
 {
@@ -252,7 +287,9 @@ template <class H> static bool retire_handle(H *p)
     const auto it = p ? g_live.find(p) : g_live.end();
     if (it == g_live.end() || it->second != handle_kind<H>()) return false;
     g_live.erase(it);
-    g_live_cv.wait(g, [&] { return p->refs.load() == 0; });
+    // an append that claimed the handle (HandleExcl) before it was retired is let out first: it sees the handle gone
+    // and backs off, or it finishes, before p can be freed
+    g_live_cv.wait(g, [&] { return p->refs.load() == 0 && !g_excl.count(p); });
     return true;
 }
 // every *_close: unregister, drain the handle's device, free it.  A null or closed handle, a handle of another kind,
@@ -545,16 +582,15 @@ static bool tc_enabled()
 // bf16 copy + squared norms + max norm and max bf16 rounding error |bf16(x) - x| of a row-major f32 matrix (open time).
 // Returns false when a row holds a NaN or inf, or its |x|^2 or rounding error overflows: the error band (tc_band) is
 // then not finite for any query, and the caller leaves the operand to the exact kernels.
-static bool prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
-                               cudaStream_t st)
+// The rows' part: Xb and n2 point at room for n rows (an append prepares its new rows only).
+static bool tc_operand_rows(const float *X, uint64_t n, uint32_t d, void *Xb, float *n2, float &xmax, float &xerr,
+                            cudaStream_t st)
 {
-    Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
-    n2.ensure(std::max<size_t>((size_t)n * 4, 16));
     DevBuf err;
     err.ensure(std::max<size_t>((size_t)n * 4, 16));
-    launch_to_bf16(X, n, d, Xb.p, n2.as<float>(), st, err.as<float>());
+    launch_to_bf16(X, n, d, Xb, n2, st, err.as<float>());
     std::vector<float> h(n), he(n);
-    LGPU_CUDA(cudaMemcpyAsync(h.data(), n2.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    LGPU_CUDA(cudaMemcpyAsync(h.data(), n2, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     LGPU_CUDA(cudaMemcpyAsync(he.data(), err.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     LGPU_CUDA(cudaStreamSynchronize(st));
     float m = 0.f, me = 0.f;
@@ -564,6 +600,13 @@ static bool prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &X
     xmax = std::sqrt(m) * 1.0001f;
     xerr = me;
     return finite && std::isfinite(xmax);
+}
+static bool prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
+                               cudaStream_t st)
+{
+    Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
+    n2.ensure(std::max<size_t>((size_t)n * 4, 16));
+    return tc_operand_rows(X, n, d, Xb.p, n2.as<float>(), xmax, xerr, st);
 }
 
 // where a top-k goes: [B][k] ids and distances, [B] counts and, optionally, [B][k] storage positions
@@ -3108,6 +3151,260 @@ int lgpu_ivf_binary_search_device(lgpu_ivf_binary *ixh, const uint8_t *d_queries
                                   uint32_t *d_out_count, void *cuda_stream)
 {
     return ivf_binary_call(ixh, device_route(cuda_stream), d_queries, B, params, d_out_ids, d_out_dist, d_out_count);
+}
+
+}  // extern "C"
+
+// ---- appends to a flat handle (the unindexed rows of a table, DESIGN.md section 3) ----
+// `b` holds `used` bytes; make room for `need`: capacity at least doubles, the contents move by a device-to-device
+// copy.  The caller has drained the device, so nothing still reads the old buffer when it is released.
+static void grow_keep(DevBuf &b, size_t used, size_t need)
+{
+    if (need <= b.bytes) return;
+    DevBuf nb;
+    nb.ensure(std::max(need, 2 * b.bytes));                    // bumps g_alloc_epoch
+    if (used) LGPU_CUDA(cudaMemcpy(nb.p, b.p, used, cudaMemcpyDeviceToDevice));
+    std::swap(b.p, nb.p);
+    std::swap(b.bytes, nb.bytes);
+}
+
+// The row ids after an append of n rows to n0: explicit ids stay explicit (positions n0.. when none are given), and
+// ids given to a handle that had none make the old rows' positions explicit.
+template <class H> static void append_ids(H *h, uint64_t n0, uint64_t n, const uint64_t *row_ids)
+{
+    if (!row_ids && !h->has_ids) return;
+    grow_keep(h->row_ids, h->has_ids ? n0 * 8 : 0, (n0 + n) * 8);
+    std::vector<uint64_t> ids;
+    if (!h->has_ids && n0) {
+        ids.resize(n0);
+        for (uint64_t i = 0; i < n0; i++) ids[i] = i;
+        LGPU_CUDA(cudaMemcpy(h->row_ids.p, ids.data(), n0 * 8, cudaMemcpyHostToDevice));
+    }
+    if (!row_ids) {
+        ids.resize(n);
+        for (uint64_t i = 0; i < n; i++) ids[i] = n0 + i;
+        row_ids = ids.data();
+    }
+    LGPU_CUDA(cudaMemcpy(static_cast<uint64_t *>(h->row_ids.p) + n0, row_ids, n * 8, cudaMemcpyHostToDevice));
+    h->has_ids = true;
+}
+
+// What every append does first, with the handle held exclusively: drain the device (a search enqueued earlier on a
+// caller's stream may still read the buffers that move or the sample that is rewritten), and invalidate every captured
+// graph, which bakes the row count in even when no buffer moves.
+static void begin_append(int device)
+{
+    require_device(device);
+    LGPU_CUDA(cudaDeviceSynchronize());
+    g_alloc_epoch++;
+}
+
+extern "C" {
+
+int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64_t *row_ids)
+{
+    return guarded([&] {
+        HandleExcl<lgpu_flat> h(flh);
+        lgpu_flat *fl = h.h;
+        LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
+        if (n == 0) return;
+        begin_append(fl->device);
+        const uint64_t n0 = fl->nrows, n1 = n0 + n;
+        const uint32_t d = fl->dim;
+        grow_keep(fl->vectors, (size_t)n0 * d * 4, (size_t)n1 * d * 4);
+        float *x = fl->vectors.as<float>() + (size_t)n0 * d;
+        LGPU_CUDA(cudaMemcpy(x, rows, (size_t)n * d * 4, cudaMemcpyHostToDevice));
+        append_ids(fl, n0, n, row_ids);
+        if (fl->has_norms) {
+            grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
+            launch_row_norms(x, n, d, fl->ysqrt.as<float>() + n0, nullptr);
+        }
+        // the tensor-core operand, as lgpu_flat_open builds it for n1 rows: the whole column when it first reaches 4096
+        // rows, else the new rows only, the band constants the max over both parts
+        if (gemm_shape_supported(d) && n1 >= 4096) {
+            if (n0 < 4096) {
+                fl->has_tc = prepare_tc_operand(fl->vectors.as<float>(), n1, d, fl->vec_b, fl->vec_n2, fl->vec_max,
+                                                fl->vec_err, nullptr);
+            } else if (fl->has_tc) {
+                grow_keep(fl->vec_b, (size_t)n0 * d * 2, (size_t)n1 * d * 2);
+                grow_keep(fl->vec_n2, (size_t)n0 * 4, (size_t)n1 * 4);
+                float xmax = 0.f, xerr = 0.f;
+                fl->has_tc = tc_operand_rows(x, n, d, fl->vec_b.as<char>() + (size_t)n0 * d * 2,
+                                             fl->vec_n2.as<float>() + n0, xmax, xerr, nullptr);
+                fl->vec_max = std::max(fl->vec_max, xmax);
+                fl->vec_err = std::max(fl->vec_err, xerr);
+            }
+            if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
+        }
+        LGPU_CUDA(cudaDeviceSynchronize());
+        fl->nrows = n1;
+    });
+}
+
+int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const uint64_t *row_ids)
+{
+    return guarded([&] {
+        HandleExcl<lgpu_binary> h(bxh);
+        lgpu_binary *bx = h.h;
+        LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
+        if (n == 0) return;
+        begin_append(bx->device);
+        const uint64_t n0 = bx->nrows, n1 = n0 + n;
+        const uint32_t nbp = bx->nbytes_pad;
+        grow_keep(bx->vectors, (size_t)n0 * nbp, (size_t)n1 * nbp);
+        grow_keep(bx->pop, (size_t)n0 * 4, (size_t)n1 * 4);
+        DevBuf raw;
+        upload(raw, rows, (size_t)n * bx->nbytes);
+        launch_ham_pack(raw.as<uint8_t>(), bx->nbytes, bx->nbytes, n, bx->vectors.as<uint8_t>() + (size_t)n0 * nbp, nbp,
+                        bx->pop.as<uint32_t>() + n0, nullptr);
+        append_ids(bx, n0, n, row_ids);
+        if (n1 > HAM_SAMPLE) {             // the threshold sample lgpu_binary_open takes from n1 rows
+            const uint64_t stride = n1 / HAM_SAMPLE;
+            bx->nsample = HAM_SAMPLE;
+            bx->sample.ensure((size_t)HAM_SAMPLE * nbp);
+            bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
+            launch_ham_pack(bx->vectors.as<uint8_t>(), stride * nbp, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp,
+                            bx->sample_pop.as<uint32_t>(), nullptr);
+        }
+        LGPU_CUDA(cudaDeviceSynchronize());
+        bx->nrows = n1;
+    });
+}
+
+}  // extern "C"
+
+// ---- union search: an IVF index and a flat tail holding the rows added after it was built ([unindexed fragments &
+// !fast_search] flat KNN over them, union, TopK again; SURVEY.md section 3.1).  The tail's exact scan runs on the tail
+// workspace's stream, forked from the caller's, while the IVF step runs on the caller's; both write into the index
+// workspace's [2][B][k] lists, and one select by (_distance, _rowid) merges them by their counts. ----
+// the tail's row width and its exact scan: a float tail under the index's metric, a binary tail by Hamming distance
+static uint32_t row_elems(const lgpu_flat *fl) { return fl->dim; }
+static uint32_t row_elems(const lgpu_binary *bx) { return bx->nbytes; }
+static void tail_search(lgpu_index *ix, lgpu_flat *fl, Workspace *ws, cudaStream_t st, const float *d_q, uint32_t B,
+                        const lgpu_search_params &sp, uint64_t *ids, float *dist, uint32_t *cnt, RowFilter rf,
+                        const Deadline *dl)
+{
+    flat_search_device(fl, ws, st, ix->metric, d_q, B, sp, ids, dist, cnt, rf, dl);
+}
+static void tail_search(lgpu_ivf_binary *, lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *d_q,
+                        uint32_t B, const lgpu_search_params &sp, uint64_t *ids, float *dist, uint32_t *cnt,
+                        RowFilter rf, const Deadline *dl)
+{
+    binary_search_device(bx, ws, st, d_q, B, sp, ids, dist, cnt, rf, dl);
+}
+
+template <class IX, class TL, class T>
+static void union_search_device(IX *ix, Workspace *ws, cudaStream_t st, TL *tl, Workspace *wt, const T *d_q, uint32_t B,
+                                const lgpu_search_params &sp, RowFilter rf, uint64_t *d_ids, float *d_dist,
+                                uint32_t *d_cnt, const Deadline *dl)
+{
+    const uint32_t k = sp.k;
+    const size_t bk = (size_t)B * k;
+    ws->u_ids.ensure(2 * bk * 8); ws->u_dist.ensure(2 * bk * 4); ws->u_cnt.ensure((size_t)2 * B * 4);
+    uint64_t *ids = ws->u_ids.as<uint64_t>();
+    float *dist = ws->u_dist.as<float>();
+    uint32_t *cnt = ws->u_cnt.as<uint32_t>();
+    // ivf_search_device's own refusal, checked before the fork (no tail work is left behind by it)
+    if (rf.bits && std::min<uint32_t>(sp.max_nprobes, ix->nlist) > std::min<uint32_t>(std::max<uint32_t>(sp.nprobes, 1), ix->nlist))
+        LGPU_REQUIRE(std::min<uint32_t>(sp.max_nprobes, ix->nlist) <= SELECT_KMAX || sp.max_nprobes >= ix->nlist,
+                     "maximum_nprobes above 2048 is not supported unless it covers every partition");
+    // joins the tail's stream back into st on every exit, a throw included (a timeout between sub-batches, a CUDA
+    // error): the index workspace's `done` event, recorded on st, then fences the tail's writes into u_ids / u_dist
+    struct Join {
+        Workspace *wt;
+        cudaStream_t st;
+        bool forked = false;
+        ~Join()
+        {
+            if (forked && (cudaEventRecord(wt->ev_join, wt->stream) != cudaSuccess ||
+                           cudaStreamWaitEvent(st, wt->ev_join, 0) != cudaSuccess))
+                cudaGetLastError();
+        }
+    } join{wt, st};
+    if (tl->nrows) {
+        LGPU_CUDA(cudaEventRecord(wt->ev_fork, st));
+        LGPU_CUDA(cudaStreamWaitEvent(wt->stream, wt->ev_fork, 0));
+        join.forked = true;
+        tail_search(ix, tl, wt, wt->stream, d_q, B, sp, ids + bk, dist + bk, cnt + B, rf, dl);
+    } else {                                    // an empty tail contributes an empty list
+        LGPU_CUDA(cudaMemsetAsync(cnt + B, 0, (size_t)B * 4, st));
+    }
+    ivf_search_device(ix, ws, st, d_q, B, sp, ids, dist, cnt, rf, dl);
+    if (join.forked) {
+        join.forked = false;
+        LGPU_CUDA(cudaEventRecord(wt->ev_join, wt->stream));
+        LGPU_CUDA(cudaStreamWaitEvent(st, wt->ev_join, 0));
+    }
+    SelectArgs s = select_cands(dist, ids, k, B, k, {d_ids, d_dist, d_cnt});
+    s.ncols = 2 * (uint64_t)k; s.outer_stride = bk; s.list_cnt = cnt;
+    launch_select(with_scratch(ws, s), st);
+}
+
+// The entry sequence of the four union entry points: resolve both handles, check the call, then run
+// union_search_device on workspaces leased from both handles' pools, on the caller's stream (device route; `allow` is
+// then a device bitmap) or staged through host_call (host route: eager, honours timeout_ms).
+template <class IX, class TL, class T>
+static int union_call(IX *ixh, TL *tlh, bool device, const T *q, uint32_t B, const lgpu_search_params *p,
+                      const uint32_t *allow, uint64_t allow_bits, uint64_t *ids, float *dist, uint32_t *cnt,
+                      void *stream)
+{
+    return guarded([&] {
+        HandleRef<IX> ix(ixh);
+        HandleRef<TL> tl(tlh);
+        check_ivf_call(ix.h, q, B, p, ids, dist, cnt);
+        LGPU_REQUIRE(row_elems(tl.h) == ix->dim, "the tail's vectors do not have the index's dimension");
+        LGPU_REQUIRE(tl->device == ix->device, "the tail and the index are on different devices");
+        LGPU_REQUIRE(allow != nullptr || allow_bits == 0, "allow bitmap is null");
+        if (B == 0) return;
+        require_device(ix->device);
+        if (device) {
+            WsLease li(ix->pool, (cudaStream_t)stream, true);
+            WsLease lt(tl->pool, nullptr, false);
+            const RowFilter rf{allow, allow ? allow_bits : 0};
+            union_search_device(ix.h, li.ws, li.st, tl.h, lt.ws, q, B, *p, rf, ids, dist, cnt, nullptr);
+            return;
+        }
+        host_call(ix->pool, q, (size_t)B * ix->dim, B, p->k, ids, dist, cnt, nullptr, p->timeout_ms,
+                  [&](Workspace *ws, cudaStream_t st, const T *dq, uint64_t *di, float *dd, uint32_t *dc,
+                      const Deadline &dl) {
+                      const RowFilter rf = allow ? upload_allow(ws, st, allow, allow_bits) : RowFilter();
+                      WsLease lt(tl->pool, nullptr, false);
+                      union_search_device(ix.h, ws, st, tl.h, lt.ws, dq, B, *p, rf, di, dd, dc, &dl);
+                  });
+    });
+}
+
+extern "C" {
+
+int lgpu_search_unindexed(lgpu_index *ixh, lgpu_flat *tail, const float *queries, uint32_t B,
+                          const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                          uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return union_call(ixh, tail, false, queries, B, params, allow, allow_bits, out_ids, out_dist, out_count, nullptr);
+}
+
+int lgpu_search_unindexed_device(lgpu_index *ixh, lgpu_flat *tail, const float *d_queries, uint32_t B,
+                                 const lgpu_search_params *params, const uint32_t *d_allow, uint64_t allow_bits,
+                                 uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream)
+{
+    return union_call(ixh, tail, true, d_queries, B, params, d_allow, allow_bits, d_out_ids, d_out_dist, d_out_count,
+                      cuda_stream);
+}
+
+int lgpu_ivf_binary_search_unindexed(lgpu_ivf_binary *ixh, lgpu_binary *tail, const uint8_t *queries, uint32_t B,
+                                     const lgpu_search_params *params, const uint32_t *allow, uint64_t allow_bits,
+                                     uint64_t *out_ids, float *out_dist, uint32_t *out_count)
+{
+    return union_call(ixh, tail, false, queries, B, params, allow, allow_bits, out_ids, out_dist, out_count, nullptr);
+}
+
+int lgpu_ivf_binary_search_unindexed_device(lgpu_ivf_binary *ixh, lgpu_binary *tail, const uint8_t *d_queries,
+                                            uint32_t B, const lgpu_search_params *params, const uint32_t *d_allow,
+                                            uint64_t allow_bits, uint64_t *d_out_ids, float *d_out_dist,
+                                            uint32_t *d_out_count, void *cuda_stream)
+{
+    return union_call(ixh, tail, true, d_queries, B, params, d_allow, allow_bits, d_out_ids, d_out_dist, d_out_count,
+                      cuda_stream);
 }
 
 int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_t *vectors, uint64_t N, uint32_t nbytes,

@@ -314,6 +314,8 @@ struct SelectArgs {
     const uint64_t *cand_ids;     // mode 2: id per entry (same addressing as dense)
     const uint64_t *cand_pos;     // mode 2: optional pos per entry
     const uint32_t *ncols_q;      // mode 2: optional [B] candidates of each query (<= ncols)
+    const uint32_t *list_cnt;     // mode 2: optional [ncols / inner][B] valid entries of list l (columns l * inner ..)
+                                  // of query q at l * B + q; the entries of a list past its count are not read
     const TopkRecord *cand_rec;   // mode 2: optional packed (id, dist) entries instead of dense + cand_ids
     // common
     uint32_t B, k;

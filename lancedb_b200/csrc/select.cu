@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
 #pragma unroll
             for (int u = 0; u < 4; u++) {
                 ok[u] = false; idv[u] = UINT64_MAX;
-                if (c + u < ncols) {
+                if (c + u < ncols && (!a.list_cnt || (c + u) % a.inner < a.list_cnt[(c + u) / a.inner * a.B + q])) {
                     uint64_t cc = c + u;
                     uint64_t addr = (cc / a.inner) * a.outer_stride + (uint64_t)q * a.row_stride + cc % a.inner;
                     if (a.cand_rec) { const TopkRecord r = a.cand_rec[addr]; idv[u] = r.id; v[u] = r.dist; }
@@ -364,8 +364,9 @@ __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs
             bool pass = false;
             uint32_t key = 0;
             uint64_t id = UINT64_MAX, pos = cc;
-            if (cc < ncols) {
-                const uint64_t addr = (cc / a.inner) * a.outer_stride + (uint64_t)q * a.row_stride + cc % a.inner;
+            const uint64_t l = cc / a.inner, e = cc - l * a.inner;     // list, entry
+            if (cc < ncols && (!a.list_cnt || e < a.list_cnt[l * a.B + q])) {
+                const uint64_t addr = l * a.outer_stride + (uint64_t)q * a.row_stride + e;
                 float f;
                 if (a.cand_rec) { const TopkRecord r = a.cand_rec[addr]; id = r.id; f = r.dist; }
                 else { id = a.cand_ids[addr]; f = a.dense[addr]; }

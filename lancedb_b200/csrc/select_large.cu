@@ -122,6 +122,7 @@ __device__ __forceinline__ void for_each_candidate(const SelectArgs &a, uint32_t
     } else {
         const uint64_t ncols = a.ncols_q ? min((uint64_t)a.ncols_q[q], a.ncols) : a.ncols;
         for (uint64_t c = first; c < ncols; c += step) {
+            if (a.list_cnt && c % a.inner >= a.list_cnt[c / a.inner * a.B + q]) continue;
             const uint64_t addr = (c / a.inner) * a.outer_stride + (uint64_t)q * a.row_stride + c % a.inner;
             uint64_t id;
             float v;

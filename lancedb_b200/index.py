@@ -73,6 +73,61 @@ def _partition_order(assign, nlist: int, row_ids):
     return order, part_offsets, rid[order.cpu().numpy()]
 
 
+def _normalise(x):
+    """Rows scaled to unit length, as a cosine index stores and encodes them (torch, any device)."""
+    return x / x.norm(dim=1, keepdim=True).clamp(min=1e-30)
+
+
+def _extend_order(part_offsets, assign, row_ids):
+    """Where appended rows go: every partition keeps its rows in their order and takes its new rows after them, in
+    row-id order.  Returns (order over [old rows, new rows] giving the extended partition order, the new part_offsets
+    u64 [nlist+1], the new rows' ids u64)."""
+    off = np.asarray(part_offsets, np.int64)
+    nlist, n0 = off.size - 1, int(off[-1])
+    rid = np.asarray(row_ids, np.uint64).reshape(-1)
+    a = np.asarray(assign, np.int64).reshape(-1)
+    by_id = np.argsort(rid, kind="stable")
+    label = np.concatenate([np.repeat(np.arange(nlist), np.diff(off)), a[by_id]])
+    order = np.argsort(label, kind="stable")
+    order = np.where(order < n0, order, n0 + by_id[np.maximum(order - n0, 0)])
+    new_off = np.zeros(nlist + 1, np.uint64)
+    new_off[1:] = np.cumsum(np.bincount(label, minlength=nlist))
+    return order, new_off, rid
+
+
+def _cat_rows(old, new, order):
+    """Per-row arrays in the extended partition order (None stays None)."""
+    if old is None:
+        return None
+    return np.ascontiguousarray(np.concatenate([np.asarray(old), np.asarray(new, old.dtype)])[order])
+
+
+def _float_rows(d, vectors, row_ids, device: int):
+    """(raw f32 rows [n, dim], rows as the index encodes them -- normalised for cosine --, partitions u32 [n] by the
+    search's own coarse kernels on CUDA device `device`) of rows appended to the float IVF index `d`."""
+    import torch
+    from . import _native
+    raw = np.ascontiguousarray(vectors, np.float32).reshape(-1, d.dim)
+    if np.asarray(row_ids).size != raw.shape[0]:
+        raise ValueError("row_ids must hold one id per appended row")
+    x = torch.as_tensor(raw)
+    if d.metric == "cosine":
+        x = _normalise(x)
+    parts = _native.ivf_assign(d.centroids, raw, d.metric, device) if raw.shape[0] else np.zeros(0, np.uint32)
+    return raw, x, parts
+
+
+def _transpose_codes(codes_sorted: np.ndarray, part_offsets) -> np.ndarray:
+    """Row-major codes [n, w] in partition order -> the flat per-partition transposed layout ([w][n_p] each)."""
+    n, w = codes_sorted.shape
+    codes_t = np.empty(n * w, np.uint8)
+    for p in range(len(part_offsets) - 1):
+        a, b = int(part_offsets[p]), int(part_offsets[p + 1])
+        if b > a:
+            codes_t[a * w:b * w] = codes_sorted[a:b].T.reshape(-1)
+    return codes_t
+
+
 @dataclass
 class IvfPqIndexData:
     index_type = "IVF_PQ"
@@ -116,6 +171,31 @@ class IvfPqIndexData:
         a, b = int(self.part_offsets[p]), int(self.part_offsets[p + 1])
         w = self.code_bytes
         return self.codes_t[a * w:b * w].reshape(w, b - a)
+
+    def row_codes(self) -> np.ndarray:
+        """[n, code_bytes] code bytes of every row, row-major in partition order."""
+        return np.concatenate([self.partition_codes(p).T for p in range(self.nlist)]) if self.nrows else \
+            np.zeros((0, self.code_bytes), np.uint8)
+
+    def extend(self, vectors, row_ids, device: int = 0) -> "IvfPqIndexData":
+        """The index with rows appended, without retraining: each row goes to the partition the search's coarse step
+        ranks first (lgpu_ivf_assign) and is encoded against its centroid with the index's codebook -- lgpu_pq_encode
+        for 8-bit codes, pq_codes for 4-bit ones -- and lands after the partition's rows (_extend_order)."""
+        import torch
+        from . import _native
+        raw, x, parts = _float_rows(self, vectors, row_ids, device)
+        if self.num_bits == 8:
+            codes = (_native.pq_encode(self.centroids, self.codebook, raw, parts, self.metric, device) if raw.shape[0]
+                     else np.zeros((0, self.m), np.uint8))
+        else:
+            codes = pack_pq4(pq_codes(x, torch.as_tensor(self.centroids), torch.as_tensor(parts.astype(np.int64)),
+                                      torch.as_tensor(self.codebook), self.metric).numpy())
+        order, off, rid = _extend_order(self.part_offsets, parts, row_ids)
+        data = IvfPqIndexData(self.dim, self.nlist, self.m, self.metric, self.centroids, self.codebook, off,
+                              _transpose_codes(_cat_rows(self.row_codes(), codes, order), off),
+                              _cat_rows(self.row_ids, rid, order), _cat_rows(self.vectors, raw, order), self.num_bits)
+        data.validate()
+        return data
 
     def shard(self, rank: int, world: int) -> "IvfPqIndexData":
         """Partition-sharded view for multi-GPU search (SURVEY.md 8e): centroids and
@@ -243,7 +323,7 @@ def _train_ivf(x, nlist, metric, sample_rate, max_iterations, gen, native_passes
     n = x.shape[0]
     raw = x
     if metric == "cosine":
-        x = x / x.norm(dim=1, keepdim=True).clamp(min=1e-30)
+        x = _normalise(x)
     ns = min(n, sample_rate * nlist)
     samp = x[torch.randperm(n, generator=gen, device="cpu")[:ns].to(x.device)] if ns < n else x
     dev_index = x.device.index or 0 if x.device.type == "cuda" else 0
@@ -330,29 +410,18 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
         ps3 = ps.reshape(nps, m, dsub).transpose(0, 1).contiguous()      # [m, nps, dsub]
         codebook = _batched_kmeans(ps3, 1 << num_bits, max_iterations, gen)   # [m, 2**num_bits, dsub]
 
-    cbn = (codebook * codebook).sum(2)                                     # [m, 256]
-    codes = torch.empty((n, m), dtype=torch.uint8, device=x.device)
     if pq_native:
         codes = torch.as_tensor(_native.pq_encode(centroids.cpu().numpy(), codebook.cpu().numpy(), raw_np,
                                                   assign.cpu().numpy().astype(np.uint32), metric, dev_index),
                                 device=x.device)
-    for s in range(0, n if not pq_native else 0, encode_chunk):
-        xs = x[s:s + encode_chunk]
-        r = xs - centroids[assign[s:s + encode_chunk]] if metric != "dot" else xs
-        r = r.reshape(-1, m, dsub).transpose(0, 1)                         # [m, c, dsub]
-        d = cbn[:, None, :] - 2.0 * torch.bmm(r, codebook.transpose(1, 2))
-        codes[s:s + encode_chunk] = d.argmin(2).transpose(0, 1).to(torch.uint8)
+    else:
+        codes = pq_codes(x, centroids, assign, codebook, metric, encode_chunk)
 
     order, part_offsets, rid = _partition_order(assign, nlist, row_ids)
     codes_sorted = codes[order].cpu().numpy()                              # [n, m] partition order
     if num_bits == 4:
         codes_sorted = pack_pq4(codes_sorted)                              # [n, m/2]
-    w = codes_sorted.shape[1]
-    codes_t = np.empty(n * w, np.uint8)
-    for p in range(nlist):
-        a, b = int(part_offsets[p]), int(part_offsets[p + 1])
-        if b > a:
-            codes_t[a * w:b * w] = codes_sorted[a:b].T.reshape(-1)
+    codes_t = _transpose_codes(codes_sorted, part_offsets)
     data = IvfPqIndexData(
         dim=dim, nlist=nlist, m=m, metric=metric,
         centroids=centroids.cpu().numpy().astype(np.float32),
@@ -361,6 +430,22 @@ def train_ivf_pq(vectors, *, num_partitions: Optional[int] = None, num_sub_vecto
         vectors=(raw[order].cpu().numpy().astype(np.float32) if keep_vectors else None), num_bits=num_bits)
     data.validate()
     return data
+
+
+def pq_codes(x, centroids, assign, codebook, metric: str, chunk: int = 1 << 16):
+    """Codes [n, m] (torch u8) of rows x (normalised for cosine) in partitions `assign`: per sub-space the argmin over
+    the codewords of |c|^2 - 2 r.c, r the residual (the row itself for dot), ties to the lowest code."""
+    import torch
+    m, _, dsub = codebook.shape
+    cbn = (codebook * codebook).sum(2)                                     # [m, 2**num_bits]
+    codes = torch.empty((x.shape[0], m), dtype=torch.uint8, device=x.device)
+    for s in range(0, x.shape[0], chunk):
+        xs = x[s:s + chunk]
+        r = xs - centroids[assign[s:s + chunk]] if metric != "dot" else xs
+        r = r.reshape(-1, m, dsub).transpose(0, 1)                         # [m, c, dsub]
+        d = cbn[:, None, :] - 2.0 * torch.bmm(r, codebook.transpose(1, 2))
+        codes[s:s + chunk] = d.argmin(2).transpose(0, 1).to(torch.uint8)
+    return codes
 
 
 def pack_pq4(codes) -> np.ndarray:
@@ -412,6 +497,18 @@ class IvfSqIndexData:
         _check_ivf_layout(self, self.dim, np.float32)
         assert self.codes.shape == (self.nrows, self.dim) and self.codes.dtype == np.uint8
         assert np.isfinite(self.lo) and np.isfinite(self.hi) and self.lo <= self.hi
+
+    def extend(self, vectors, row_ids, device: int = 0) -> "IvfSqIndexData":
+        """The index with rows appended, without retraining: partitions from lgpu_ivf_assign, codes from sq_encode
+        with the index's [lo, hi] (rows normalised for cosine); each partition's new rows follow its old ones."""
+        raw, x, parts = _float_rows(self, vectors, row_ids, device)
+        order, off, rid = _extend_order(self.part_offsets, parts, row_ids)
+        data = IvfSqIndexData(self.dim, self.nlist, self.metric, self.centroids, off,
+                              _cat_rows(self.codes, sq_encode(x.numpy(), self.lo, self.hi), order),
+                              _cat_rows(self.row_ids, rid, order), self.lo, self.hi,
+                              _cat_rows(self.vectors, raw, order))
+        data.validate()
+        return data
 
 
 def sq_encode(x, lo: float, hi: float) -> np.ndarray:
@@ -495,6 +592,20 @@ class IvfRqIndexData:
         assert self.codes.shape == (self.nrows, (self.dim + 7) // 8) and self.codes.dtype == np.uint8
         assert self.add_factors.shape == (self.nrows,) and self.add_factors.dtype == np.float32
         assert self.scale_factors.shape == (self.nrows,) and self.scale_factors.dtype == np.float32
+
+    def extend(self, vectors, row_ids, device: int = 0) -> "IvfRqIndexData":
+        """The index with rows appended, without retraining: partitions from lgpu_ivf_assign, sign bits and factors from
+        rq_encode against the assigned centroid with the index's rotation; each partition's new rows follow its old
+        ones."""
+        raw, x, parts = _float_rows(self, vectors, row_ids, device)
+        codes, add, scale = rq_encode(x, self.centroids, parts.astype(np.int64), self.rotation)
+        order, off, rid = _extend_order(self.part_offsets, parts, row_ids)
+        data = IvfRqIndexData(self.dim, self.nlist, self.metric, self.centroids, self.rotation, off,
+                              _cat_rows(self.codes, codes, order), _cat_rows(self.add_factors, add, order),
+                              _cat_rows(self.scale_factors, scale, order), _cat_rows(self.row_ids, rid, order),
+                              _cat_rows(self.vectors, raw, order), self.num_bits)
+        data.validate()
+        return data
 
 
 def rq_rotation(dim: int, seed: int = 45, device=None) -> np.ndarray:
@@ -601,6 +712,20 @@ class IvfBinaryIndexData:
         assert 1 <= self.nbytes and 8 * self.nbytes <= HAMMING_MAX_BITS
         _check_ivf_layout(self, self.nbytes, np.uint8)
         assert self.vectors.shape == (self.nrows, self.nbytes) and self.vectors.dtype == np.uint8
+
+    def extend(self, vectors, row_ids, device: int = 0) -> "IvfBinaryIndexData":
+        """The index with rows appended, without retraining: each row goes to its nearest centroid by Hamming distance
+        (kmodes_assign, ties to the lower partition) after the partition's rows.  The assignment is exact integer work,
+        so it runs on the host whatever `device` is."""
+        x = np.ascontiguousarray(vectors, np.uint8).reshape(-1, self.nbytes)
+        if np.asarray(row_ids).size != x.shape[0]:
+            raise ValueError("row_ids must hold one id per appended row")
+        parts = kmodes_assign(x, self.centroids) if x.shape[0] else np.zeros(0, np.int64)
+        order, off, rid = _extend_order(self.part_offsets, parts, row_ids)
+        data = IvfBinaryIndexData(self.nbytes, self.nlist, self.centroids, off, _cat_rows(self.vectors, x, order),
+                                  _cat_rows(self.row_ids, rid, order))
+        data.validate()
+        return data
 
 
 def _unpack_bits(x, device, dtype):
@@ -716,6 +841,8 @@ class IvfHnswSqIndexData:
     upper_adj: np.ndarray
     entry: np.ndarray
     top_level: np.ndarray
+    ef_construction: int = 300       # how the graphs were built: extend rebuilds a partition's graph the same way
+    graph_device: Optional[str] = None
 
     dim = property(lambda self: self.sq.dim)
     nlist = property(lambda self: self.sq.nlist)
@@ -756,6 +883,37 @@ class IvfHnswSqIndexData:
                     ok = blk == HNSW_NONE
                     ok[~ok] = (blk[~ok] < b - a)
                     assert ok.all() and (lv[blk[blk != HNSW_NONE].astype(np.int64)] >= L).all()
+
+
+    def extend(self, vectors, row_ids, device: int = 0, seed: int = 45) -> "IvfHnswSqIndexData":
+        """IvfSqIndexData.extend, then the graph of every partition that received rows is built again over all of its
+        rows (build_hnsw_graph with the index's m, ef_construction and graph device); the other partitions keep their
+        graphs."""
+        sq = self.sq.extend(vectors, row_ids, device)
+        old, new = self.part_offsets.astype(np.int64), sq.part_offsets.astype(np.int64)
+        entry, top = self.entry.copy(), self.top_level.copy()
+        lvs, adjs, uas = [], [], []
+        for p in range(self.nlist):
+            a, b, a2, b2 = old[p], old[p + 1], new[p], new[p + 1]
+            if b2 - a2 == b - a:
+                lv, adj = self.levels[a:b], self.adj0[a:b]
+                up = np.nonzero(lv)[0]
+                first = int(self.upper_index[a + up[0]]) if up.size else 0
+                ua = self.upper_adj[first:first + int(lv.astype(np.int64).sum())]
+            else:
+                lv, adj, _, ua, e, t = build_hnsw_graph(sq.codes[a2:b2], np.array([0, b2 - a2]), self.m,
+                                                        self.ef_construction, seed, self.graph_device)
+                entry[p], top[p] = e[0], t[0]
+            lvs.append(lv); adjs.append(adj); uas.append(ua)
+        levels = np.concatenate(lvs).astype(np.uint8)
+        upper_index = np.full(levels.size, HNSW_NONE, np.uint32)
+        up = np.nonzero(levels)[0]
+        upper_index[up] = (np.cumsum(levels[up].astype(np.int64)) - levels[up]).astype(np.uint32)
+        data = IvfHnswSqIndexData(sq, self.m, levels, np.concatenate(adjs).astype(np.uint32), upper_index,
+                                  np.concatenate(uas).astype(np.uint32).reshape(-1, self.m), entry, top,
+                                  self.ef_construction, self.graph_device)
+        data.validate()
+        return data
 
 
 def _hnsw_candidates(xc, ncand, chunk):
@@ -881,7 +1039,7 @@ def train_ivf_hnsw_sq(vectors, *, num_partitions: Optional[int] = None, distance
                       max_iterations=max_iterations, row_ids=row_ids, keep_vectors=keep_vectors, seed=seed,
                       device=device, native_passes=native_passes)
     g = build_hnsw_graph(sq.codes, sq.part_offsets, m, ef_construction, seed, device)
-    data = IvfHnswSqIndexData(sq, m, *g)
+    data = IvfHnswSqIndexData(sq, m, *g, ef_construction=ef_construction, graph_device=device)
     data.validate()
     return data
 

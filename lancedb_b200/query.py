@@ -56,6 +56,7 @@ class LanceVectorQueryBuilder:
         self._columns: Optional[List[str]] = None
         self._with_row_id = False
         self._use_index = True
+        self._fast_search = False
         self._where: Optional[str] = None
         self._postfilter = False
 
@@ -120,6 +121,12 @@ class LanceVectorQueryBuilder:
     def bypass_vector_index(self) -> "LanceVectorQueryBuilder":
         """Exhaustive flat search even when an index exists (use_index = false)."""
         self._use_index = False
+        return self
+
+    def fast_search(self) -> "LanceVectorQueryBuilder":
+        """Search the index alone: rows added since it was built (Table.add) are skipped until optimize() folds them
+        in (python/python/lancedb/query.py:1950-1961).  Without an index it changes nothing."""
+        self._fast_search = True
         return self
 
     def where(self, where: str, prefilter: Optional[bool] = None) -> "LanceVectorQueryBuilder":
@@ -199,7 +206,8 @@ class LanceVectorQueryBuilder:
             refine_factor=self._refine_factor, distance_type=self._distance_type,
             lower=self._lower_bound, upper=self._upper_bound, use_index=self._use_index,
             allow_mask=None if (mask is None or self._postfilter) else mask,
-            max_nprobes=max_nprobes, timeout_ms=timeout_ms, **({"ef": self._ef} if self._ef else {}))
+            max_nprobes=max_nprobes, timeout_ms=timeout_ms, **({"ef": self._ef} if self._ef else {}),
+            **({"fast_search": True} if self._fast_search else {}))
         out = []
         for qi in range(len(cnt)):                         # one result list per query (a multivector query is one)
             n = int(cnt[qi])

@@ -116,6 +116,8 @@ def handle_query(table, body: Union[str, bytes, Dict[str, Any]]) -> bytes:
         q = q.refine_factor(int(body["refine_factor"]))
     if body.get("bypass_vector_index"):
         q = q.bypass_vector_index()
+    if body.get("fast_search"):
+        q = q.fast_search()
     if body.get("filter"):
         q = q.where(str(body["filter"]), prefilter=bool(body.get("prefilter", True)))
     cols = body.get("columns")

@@ -92,6 +92,10 @@ class Table:
         self._multivec: Dict[str, _native.GpuMultivec] = {}
         self._index: Dict[str, _native.GpuIvfPq] = {}
         self._index_data: Dict[str, object] = {}      # the IndexData of one of IVF_KINDS
+        # rows added after an indexed column's index was built: a flat handle over them (GpuFlat / GpuBinary, row ids =
+        # table positions) and the position of the first
+        self._tail: Dict[str, object] = {}
+        self._tail_from: Dict[str, int] = {}
 
     # ---- introspection ----
     @property
@@ -117,7 +121,8 @@ class Table:
         return [{"name": f"{c}_idx", "index_type": self._index_type(c), "columns": [c]} for c in self._index]
 
     def index_stats(self, index_name: str):
-        """python/python/tests/test_index.py:366-372: every row is indexed (there is no append path here)."""
+        """python/python/tests/test_index.py:366-372: rows added after the index was built count as unindexed until
+        optimize() folds them in."""
         col = index_name[:-4] if index_name.endswith("_idx") else index_name
         if col not in self._index_data:
             return None
@@ -192,6 +197,7 @@ class Table:
     def _attach_index(self, column: str, data):
         if column in self._index:
             self._index[column].close()
+        self._drop_tail(column)                 # the new index holds every row the table has
         self._index_data[column] = data
         cls = getattr(_native, IVF_KINDS[data.index_type].handle)     # looked up now, so a replaced class is used
         self._index[column] = cls(data, device=self._device)
@@ -219,6 +225,109 @@ class Table:
         if self._index_data[column].num_bits != 8:
             raise NotImplementedError("only 8-bit IVF_PQ indexes are written as Lance index files")
         write_ivf_pq_index(index_dir, self._index_data[column], transposed=transposed)
+
+    # ---- appends and index maintenance (python/python/lancedb/table.py:3393, 3970) ----
+    def add(self, data, mode: str = "append", on_bad_vectors: str = "error", **_ignored) -> None:
+        """Append rows with the table's schema.  Row ids are table positions.  An indexed column's new rows are not
+        indexed: they go to its tail, which every vector search scans exactly and merges with the index's result
+        (unless fast_search()), until optimize() folds them into the index.
+        on_bad_vectors="error" (the reference's default, and the only policy served): a float vector holding a NaN is
+        refused (python/python/lancedb/table.py:4429-4445), and so is a row the column's index could not take at
+        optimize(): an infinite component, or a zero vector under a cosine index.  A refused call changes nothing."""
+        if mode == "overwrite":
+            raise NotImplementedError("add(mode='overwrite') is not supported: only appends are")
+        if mode != "append":
+            raise ValueError(f"mode must be 'append' or 'overwrite', got {mode!r}")
+        if on_bad_vectors != "error":
+            raise NotImplementedError(f"on_bad_vectors={on_bad_vectors!r} is not supported: only 'error' is")
+        new = _to_arrow_table(data)
+        if sorted(new.column_names) != sorted(self.schema.names):
+            raise ValueError(f"the data's columns {new.column_names} do not match the table's schema "
+                             f"{self.schema.names}")
+        try:
+            new = new.select(self.schema.names).cast(self.schema)
+        except (pa.ArrowInvalid, pa.ArrowNotImplementedError, pa.ArrowTypeError, ValueError) as e:
+            raise ValueError(f"the data does not match the table's schema: {e}") from None
+        n0, n = self.count_rows(), new.num_rows
+        if n == 0:
+            return
+        rows = {c: self._rows_of(new, c) for c in _vector_columns(self.schema) if not self._is_multivec(c)}
+        for c, x in rows.items():
+            self._check_new_rows(c, x)
+        ids = np.arange(n0, n0 + n, dtype=np.uint64)
+        done = []                   # the tails grow before the table does: a failure leaves the table as it was
+        try:
+            for column in self._index:
+                if column in self._tail:
+                    self._tail[column].append(rows[column], ids)
+                else:
+                    cls = _native.GpuBinary if self._is_binary(column) else _native.GpuFlat
+                    self._tail[column] = cls(rows[column], row_ids=ids, device=self._device)
+                    self._tail_from[column] = n0
+                done.append(column)
+        except BaseException:
+            for column in done:    # back to the rows the table holds
+                start = self._tail_from[column]
+                self._drop_tail(column)
+                if start < n0:
+                    cls = _native.GpuBinary if self._is_binary(column) else _native.GpuFlat
+                    self._tail[column] = cls(self._new_rows(column, start), device=self._device,
+                                             row_ids=np.arange(start, n0, dtype=np.uint64))
+                    self._tail_from[column] = start
+            raise
+        self._data = pa.concat_tables([self._data, new]).combine_chunks()
+        for cache in (self._flat, self._binary):         # full-column caches grow in place (ids = positions)
+            for column in list(cache):
+                try:
+                    cache[column].append(rows[column])
+                except BaseException:
+                    cache.pop(column).close()             # reopened from the table on the next search
+                    raise
+        for mv in self._multivec.values():               # reopened on the next search
+            mv.close()
+        self._multivec.clear()
+
+    def _check_new_rows(self, column: str, x: np.ndarray) -> None:
+        if self._is_binary(column):
+            return
+        bad = np.isnan(x).any(axis=1)
+        if bad.any():
+            raise ValueError(f"Vector column '{column}' has NaNs (row {int(np.nonzero(bad)[0][0])} of the data)")
+        if column in self._index:
+            bad = np.isinf(x).any(axis=1)
+            if self._index_data[column].metric == "cosine":
+                bad |= ~(np.square(x.astype(np.float32)).sum(axis=1) > 0)
+            if bad.any():
+                raise ValueError(f"row {int(np.nonzero(bad)[0][0])} of the data cannot join column '{column}''s "
+                                 "index: an infinite component, or a zero vector under cosine")
+
+    @staticmethod
+    def _rows_of(table: pa.Table, column: str) -> np.ndarray:
+        """The vectors of a float (f32) or binary (u8) column of `table`."""
+        col = table.column(column).combine_chunks()
+        dt = np.uint8 if pa.types.is_uint8(col.type.value_type) else np.float32
+        return np.asarray(col.flatten().to_numpy(zero_copy_only=False), dt).reshape(-1, col.type.list_size)
+
+    def _new_rows(self, column: str, start: int) -> np.ndarray:
+        """The vectors of rows start.. of a float (f32) or binary (u8) column."""
+        return self._rows_of(self._data.slice(start), column)
+
+    def _drop_tail(self, column: str) -> None:
+        tail = self._tail.pop(column, None)
+        if tail is not None:
+            tail.close()
+        self._tail_from.pop(column, None)
+
+    def optimize(self, *, cleanup_older_than=None, delete_unverified: bool = False, retrain: bool = False) -> None:
+        """Fold every indexed column's unindexed rows into its index without retraining (IndexData.extend: the fitted
+        centroids and quantiser), then reopen it.  Compaction and version cleanup have nothing to do here."""
+        if retrain:
+            raise NotImplementedError("optimize(retrain=True) is not supported: rows are added with the index's model")
+        for column in list(self._tail):
+            start = self._tail_from[column]
+            rows = self._new_rows(column, start)
+            ids = np.arange(start, start + rows.shape[0], dtype=np.uint64)
+            self._attach_index(column, self._index_data[column].extend(rows, ids, device=self._device))
 
     def prewarm_index(self, name: str):           # rust/lancedb/src/table.rs:3283-3286
         return None                                # indexes are pinned in HBM at create/open time
@@ -248,7 +357,8 @@ class Table:
         return LanceVectorQueryBuilder(self, query, column)
 
     def _vector_search(self, queries: np.ndarray, *, column, k, nprobes, refine_factor, distance_type,
-                       lower, upper, use_index, allow_mask=None, max_nprobes=0, timeout_ms=0, ef=0):
+                       lower, upper, use_index, allow_mask=None, max_nprobes=0, timeout_ms=0, ef=0,
+                       fast_search=False):
         allow, allow_bits = None, 0
         if allow_mask is not None:                 # prefilter: row-id allow-list as the C ABI's bitmap
             allow, allow_bits = _native.mask_bitmap(allow_mask), int(len(allow_mask))
@@ -259,9 +369,11 @@ class Table:
             q = _native.binary_components(queries)   # the builder's f32 copy: integers are exact up to 2^24
             idx = self._index.get(column) if use_index else None
             if idx is not None:                    # IVF_FLAT (hamming); bypass_vector_index() searches flat below
-                return idx.search(q, k=k, nprobes=nprobes, refine_factor=refine_factor or 0, lower=lower, upper=upper,
-                                  allow=allow, allow_bits=allow_bits,
-                                  max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms)
+                kw = dict(k=k, nprobes=nprobes, refine_factor=refine_factor or 0, lower=lower, upper=upper, allow=allow,
+                          allow_bits=allow_bits, max_nprobes=max_nprobes if allow is not None else 0,
+                          timeout_ms=timeout_ms)
+                tail = None if fast_search else self._tail.get(column)
+                return idx.search(q, **kw) if tail is None else idx.search_unindexed(tail, q, **kw)
             bx = self._binary.get(column)
             if bx is None:
                 bx = self._binary[column] = _native.GpuBinary(self._binary_vectors(column), device=self._device)
@@ -284,9 +396,11 @@ class Table:
             if distance_type is not None and distance_type != idx.metric:
                 # the reference documents this as invalid results; be explicit instead
                 raise ValueError(f"distance_type {distance_type!r} does not match the index's {idx.metric!r}")
-            return idx.search(queries, k=k, nprobes=nprobes, refine_factor=refine_factor or 0,
-                              lower=lower, upper=upper, allow=allow, allow_bits=allow_bits,
-                              max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms, ef=ef)
+            kw = dict(k=k, nprobes=nprobes, refine_factor=refine_factor or 0, lower=lower, upper=upper, allow=allow,
+                      allow_bits=allow_bits, max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms,
+                      ef=ef)
+            tail = None if fast_search else self._tail.get(column)   # rows added since the index was built
+            return idx.search(queries, **kw) if tail is None else idx.search_unindexed(tail, queries, **kw)
         fl = self._flat.get(column)
         if fl is None:
             fl = self._flat[column] = _native.GpuFlat(self._vectors(column), device=self._device)
