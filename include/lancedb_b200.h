@@ -361,8 +361,9 @@ int lgpu_kmeans_train(const float *x, uint64_t n, uint32_t dim, float *centroids
 int lgpu_pq_train(const float *x, uint64_t n, uint32_t dim, uint32_t m, float *codebook, uint32_t iters, int device);
 
 /* ---- flat / brute force (LanceRead -> KNNVectorDistance -> TopK) ---------
- * A column of at least 4096 rows with dim a multiple of 8 is scored on the tensor cores (l2, no prefilter or
- * distance_range, B >= 8) with an exact re-score of every row inside the bf16 error band; a column holding a NaN or inf,
+ * A column of at least 4096 rows with dim a multiple of 8 is scored on the tensor cores (l2, no distance_range,
+ * B >= 8, k <= 2048; a prefilter or deleted rows keep that path) with an exact re-score of every row inside the bf16
+ * error band; a column holding a NaN or inf,
  * or a row whose |x|^2 overflows, has no finite band and is always served by the exact kernels, and so is any query
  * whose band is not finite.  NaN distances are never returned, +-inf ones are ordered like any other. */
 int  lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim,
@@ -425,6 +426,26 @@ int  lgpu_binary_search_device(lgpu_binary *bx, const uint8_t *d_queries, uint32
                                uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
 /* Append n rows (HOST [n][nbytes]); everything else as lgpu_flat_append. */
 int  lgpu_binary_append(lgpu_binary *bx, const uint8_t *rows, uint64_t n, const uint64_t *row_ids);
+
+/* ---- deleted rows (the reference's Table::delete; Lance keeps them per dataset in deletion files).  Delete the rows
+ * whose ids are among row_ids (HOST [n]); *n_deleted (may be NULL) = how many of those ids were live and are now
+ * deleted.  An id the handle does not hold, or already deleted, changes nothing.  Nothing is undeleted: rows appended
+ * later (lgpu_*_append) are live, and an append that would give a row the id of a deleted row the handle still holds
+ * fails with LGPU_INVALID_INPUT and changes nothing.
+ * Every later search on the handle, on every entry point (host, _filtered, _device, _async, _coalesced, _sharded, and
+ * each side of an _unindexed union), returns exactly what it would return with the allow bitmap
+ * allow AND NOT deleted (with no allow bitmap: every id not deleted), so maximum_nprobes widening applies as under a
+ * prefilter.  The handle keeps a device bitmap of its live row ids, one bit per id below id_bound = the largest row
+ * id + 1, built by the first delete: a handle never deleted from holds none and searches as before.  Every row id of
+ * the handle must be below LGPU_DELETE_ID_BOUND for a delete (and for an append after one), else LGPU_INVALID_INPUT.
+ * The call takes the handle alone, as an append does, and invalidates captured CUDA graphs.  lgpu_index_delete serves
+ * every float IVF kind; each function refuses a handle of another kind. */
+#define LGPU_DELETE_ID_BOUND (1ull << 32)   /* the live bitmap takes at most 512 MiB */
+int  lgpu_index_delete(lgpu_index *ix, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted);
+int  lgpu_ivf_binary_delete(lgpu_ivf_binary *ix, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted);
+int  lgpu_flat_delete(lgpu_flat *fl, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted);
+int  lgpu_binary_delete(lgpu_binary *bx, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted);
+int  lgpu_multivec_delete(lgpu_multivec *mv, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted);
 
 /* ---- binary IVF_FLAT (lance `IvfFlat` with distance_type("hamming"), the index LanceDB builds over
  * fixed_size_list<uint8, nbytes> columns; rust/lancedb/src/index/vector.rs:169-209): packed binary centroids and the
@@ -618,7 +639,8 @@ int lgpu_last_stage_ms(float *times);
  * sub-batch on the exact or the small path adds none).  stats: [4]
  * After lgpu_binary_search* (whole batch): [0] candidates the tensor-core list pass appended (0 on the dense paths),
  * [1] distances computed on the tensor cores (0 on the SIMT path), [2] queries redone densely after a list overflow,
- * [3] queries.  After lgpu_multivec_search*: see the multivector section above. */
+ * [3] queries.  After lgpu_flat_search* (whole batch): [1] distances computed on the tensor cores (0 on the exact
+ * path), [3] queries, [0] = [2] = 0.  After lgpu_multivec_search*: see the multivector section above. */
 int lgpu_last_filter_stats(uint64_t *stats);
 /* kernels this process has launched through the library so far (eager launches and graph replays alike) */
 int lgpu_kernel_launch_count(uint64_t *count);

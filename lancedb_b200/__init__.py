@@ -8,11 +8,11 @@ the reference's builder surface plus a ctypes binding.  There is no CPU fallback
 from .index import (IvfPqIndexData, IvfSqIndexData, IvfHnswSqIndexData, IvfRqIndexData, IvfBinaryIndexData,
                     train_ivf_pq, train_ivf_sq, train_ivf_hnsw_sq, train_ivf_rq, train_ivf_binary, suggested_num_sub_vectors, suggested_num_partitions)
 from .query import LanceVectorQueryBuilder, DEFAULT_TOP_K, DEFAULT_NPROBES
-from .table import DBConnection, Table, connect
+from .table import DBConnection, DeleteResult, Table, connect
 from .aio import AsyncConnection, AsyncTable, HnswSq, IvfFlat, IvfRq, connect_async
 
 __all__ = [
-    "connect", "connect_async", "DBConnection", "AsyncConnection", "Table", "AsyncTable", "LanceVectorQueryBuilder", "IvfPqIndexData", "train_ivf_pq",
+    "connect", "connect_async", "DBConnection", "AsyncConnection", "Table", "AsyncTable", "DeleteResult", "LanceVectorQueryBuilder", "IvfPqIndexData", "train_ivf_pq",
     "IvfSqIndexData", "train_ivf_sq", "IvfHnswSqIndexData", "train_ivf_hnsw_sq", "HnswSq", "IvfRqIndexData", "train_ivf_rq", "IvfRq",
     "IvfBinaryIndexData", "train_ivf_binary", "IvfFlat",
     "suggested_num_sub_vectors", "suggested_num_partitions", "DEFAULT_TOP_K", "DEFAULT_NPROBES",

@@ -47,6 +47,7 @@ EXPORTS = [
     "lgpu_ivf_binary_search_device", "lgpu_debug_ivf_hamming_scan",
     "lgpu_flat_append", "lgpu_binary_append", "lgpu_search_unindexed", "lgpu_search_unindexed_device",
     "lgpu_ivf_binary_search_unindexed", "lgpu_ivf_binary_search_unindexed_device",
+    "lgpu_index_delete", "lgpu_ivf_binary_delete", "lgpu_flat_delete", "lgpu_binary_delete", "lgpu_multivec_delete",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -224,6 +225,9 @@ def load():
         getattr(lib, fn).argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
         getattr(lib, fn + "_device").argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp,
                                                  vp]
+    for fn in ("lgpu_index_delete", "lgpu_ivf_binary_delete", "lgpu_flat_delete", "lgpu_binary_delete",
+               "lgpu_multivec_delete"):
+        getattr(lib, fn).argtypes = [vp, vp, C.c_uint64, C.POINTER(C.c_uint64)]
     for name in EXPORTS:
         getattr(lib, name)          # every declared symbol must be exported
     if lib.lgpu_abi_version() != ABI_VERSION:
@@ -275,6 +279,19 @@ class _Handle:
             self._h = None
 
     __del__ = close
+
+
+class _RowsHandle(_Handle):
+    """A handle over rows, which `_delete`, the name of its lgpu_*_delete, deletes rows from."""
+    _delete = ""
+
+    def delete(self, row_ids) -> int:
+        """Delete the rows whose ids are in `row_ids` (lgpu_*_delete): every later search on this handle leaves them
+        out.  Returns how many of the ids were live and are now deleted."""
+        ids = np.ascontiguousarray(row_ids, np.uint64).reshape(-1)
+        n = C.c_uint64(0)
+        check(getattr(load(), self._delete)(self._h, _ptr(ids), ids.size, C.byref(n)))
+        return n.value
 
 
 def _host_search(fn: str, head, B: int, k: int, p: SearchParams, allow, allow_bits):
@@ -353,10 +370,11 @@ def _query_offsets(q_offsets) -> np.ndarray:
     return np.ascontiguousarray(off, np.uint32)
 
 
-class GpuIvfPq(_Handle):
+class GpuIvfPq(_RowsHandle):
     """An IVF_PQ index pinned in HBM (lgpu_index), 8-bit or 4-bit codes (data.num_bits).  The other float IVF kinds
     open an lgpu_index through their own C function, `_open`, so they subclass this and supply only `_desc`."""
     _open, _close = "lgpu_index_open", "lgpu_index_close"
+    _delete = "lgpu_index_delete"
 
     def __init__(self, data, device: int = 0, with_vectors: bool = True):
         lib = load()
@@ -510,9 +528,10 @@ class GpuIvfRq(GpuIvfPq):
                       *[_ptr(a) for a in keep]), keep
 
 
-class GpuFlat(_Handle):
+class GpuFlat(_RowsHandle):
     """A raw vector column pinned in HBM (lgpu_flat)."""
     _close = "lgpu_flat_close"
+    _delete = "lgpu_flat_delete"
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
         v = np.ascontiguousarray(vectors, np.float32)
@@ -549,10 +568,11 @@ class GpuFlat(_Handle):
         self.nrows += v.shape[0]
 
 
-class GpuBinary(_Handle):
+class GpuBinary(_RowsHandle):
     """A packed binary vector column (fixed_size_list<uint8, nbytes>) pinned in HBM (lgpu_binary), searched by
     Hamming distance."""
     _close = "lgpu_binary_close"
+    _delete = "lgpu_binary_delete"
     _queries = _binary_queries
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
@@ -587,10 +607,11 @@ class GpuBinary(_Handle):
         self.nrows += v.shape[0]
 
 
-class GpuIvfBinary(_Handle):
+class GpuIvfBinary(_RowsHandle):
     """A binary IVF_FLAT index (IvfBinaryIndexData) pinned in HBM (lgpu_ivf_binary): the probed partitions of packed
     binary rows scored exactly by Hamming distance."""
     _close = "lgpu_ivf_binary_close"
+    _delete = "lgpu_ivf_binary_delete"
     _queries = _binary_queries
 
     def __init__(self, data, device: int = 0):
@@ -640,10 +661,11 @@ def multivec_offsets(lengths) -> np.ndarray:
     return np.concatenate([[0], np.cumsum(n)]).astype(np.uint64)
 
 
-class GpuMultivec(_Handle):
+class GpuMultivec(_RowsHandle):
     """A multivector column (list<fixed_size_list<float, dim>>) pinned in HBM (lgpu_multivec), searched by late
     interaction: _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors."""
     _close = "lgpu_multivec_close"
+    _delete = "lgpu_multivec_delete"
 
     def __init__(self, values, offsets, row_ids=None, device: int = 0):
         v = np.ascontiguousarray(values, np.float32)

@@ -19,8 +19,7 @@ from typing import Dict, Iterable, List, Optional, Union
 import numpy as np
 import pyarrow as pa
 
-from . import filter as _filter
-from .table import DBConnection, Table
+from .table import DBConnection, DeleteResult, Table
 
 
 @dataclass
@@ -160,7 +159,9 @@ class AsyncQuery(_AsyncQueryBase):
         if self._with_row_id:
             t = t.append_column("_rowid", pa.array(np.arange(t.num_rows, dtype=np.uint64)))
         if self._where is not None:
-            t = t.filter(pa.array(_filter.evaluate(self._table._data, self._where)))
+            t = t.filter(pa.array(self._table._where_mask(self._where)))
+        elif self._table._live is not None:         # deleted rows are left out; the others keep their _rowid
+            t = t.filter(pa.array(self._table._live))
         if self._columns is not None:
             t = t.select(self._columns + (["_rowid"] if self._with_row_id else []))
         t = t.slice(self._offset)
@@ -290,7 +291,7 @@ class AsyncTable:
     async def count_rows(self, filter: Optional[str] = None) -> int:
         if filter is None:
             return self._table.count_rows()
-        return int(_filter.evaluate(self._table._data, filter).sum())
+        return int(self._table._where_mask(filter).sum())
 
     async def to_arrow(self) -> pa.Table:
         return self._table.to_arrow()
@@ -310,6 +311,9 @@ class AsyncTable:
 
     async def add(self, data, mode: str = "append") -> None:
         await asyncio.to_thread(self._table.add, data, mode=mode)
+
+    async def delete(self, where: str) -> DeleteResult:
+        return await asyncio.to_thread(self._table.delete, where)
 
     async def optimize(self, *, cleanup_older_than=None, delete_unverified: bool = False, retrain: bool = False) -> None:
         await asyncio.to_thread(self._table.optimize, cleanup_older_than=cleanup_older_than,

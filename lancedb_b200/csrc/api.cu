@@ -17,6 +17,7 @@
 #include <cstring>
 #include <mutex>
 #include <thread>
+#include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -63,15 +64,23 @@ static bool profiling_enabled()
     }
     return v == 1;
 }
+// bytes of the calling thread's current call held in a workspace outside its sub-batches: the AND of the call's bitmap
+// with a handle's live rows (with_live), charged to LGPU_WS_BYTES once per call and released when the call ends
+// (WsCharge).  The sub-batches share what is left, at least the 1 MiB floor.
+static thread_local size_t g_ws_charged = 0;
+struct WsCharge {
+    ~WsCharge() { g_ws_charged = 0; }
+};
 static size_t workspace_budget()
 {
     static size_t v = 0;
+    constexpr size_t floor = (size_t)1 << 20;
     if (!v) {
         const char *e = getenv("LGPU_WS_BYTES");
         v = e ? (size_t)strtoull(e, nullptr, 10) : ((size_t)8 << 30);
-        if (v < ((size_t)1 << 20)) v = (size_t)1 << 20;
+        if (v < floor) v = floor;
     }
-    return v;
+    return v > g_ws_charged + floor ? v - g_ws_charged : floor;
 }
 
 // bumped by every device (re)allocation in the process.  A captured CUDA graph bakes workspace pointers in, so a
@@ -136,6 +145,7 @@ struct Workspace {
     DevBuf pq4_tab, pq4_slots;          // 4-bit IVF_PQ search: per-slot u8 tables [slots][m][16] and quantisers
     DevBuf sel_large;                   // the large select's scratch (k > SELECT_KMAX, select_large.cu)
     DevBuf u_ids, u_dist, u_cnt;        // union search: the index's and the tail's top-k, [2][B][k] and [2][B]
+    DevBuf live_and;                    // a filtered call on a handle with deleted rows: its bitmap AND the live rows
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -172,6 +182,15 @@ struct WorkspacePool {
     }
     void give(Workspace *w) { std::lock_guard<std::mutex> g(mu); free_list.push_back(w); }
     ~WorkspacePool() { for (auto *w : free_list) delete w; }
+};
+
+// The rows of a handle that were not deleted (lgpu_*_delete): a device bitmap over row ids [0, id_bound), id_bound the
+// largest row id + 1, with the bit of every row id the handle holds set until that id is deleted (rowmask.cu).  The
+// first delete builds it; a handle never deleted from holds none (active false) and searches as before.
+struct RowLive {
+    DevBuf bits;
+    uint64_t id_bound = 0;
+    bool active = false;
 };
 
 }  // namespace lgpu
@@ -367,6 +386,7 @@ struct lgpu_index {
     DevBuf cent_pop, row_pop;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
+    RowLive live;
     WorkspacePool pool;
 };
 
@@ -385,6 +405,7 @@ struct lgpu_flat {
     bool has_tc = false;
     bool has_ids = false, has_norms = false;
     std::mutex mu;
+    RowLive live;
     WorkspacePool pool;
 };
 
@@ -397,7 +418,9 @@ struct lgpu_binary {
     DevBuf vectors, pop, row_ids;          // [nrows][nbytes_pad] zero-padded rows, popc of each row, optional ids
     DevBuf sample, sample_pop;             // every (nrows / nsample)-th row: the threshold sample of the list path
     uint64_t nsample = 0;                  // 0: no sample (nrows <= HAM_SAMPLE)
+    DevBuf sample_ids;                     // the sample rows' ids (a row filter tests them in the sample's select)
     bool has_ids = false;
+    RowLive live;
     WorkspacePool pool;
 };
 
@@ -413,6 +436,7 @@ struct lgpu_multivec {
     bool tc_ok = false;                    // the tensor-core path may run (see multivec_search_device)
     std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
     bool has_ids = false;
+    RowLive live;
     WorkspacePool pool;
 };
 
@@ -663,27 +687,30 @@ static size_t large_k_query_bytes(uint32_t k)
 }
 
 // The tail of tc_topk_l2 and tc_topk_l2_filtered: exact re-score of the [B][cap] candidate slots (ws->t_pos, t_ids;
-// one pair per slot, empty slots included), their top-k into the outputs, then the dense fix-up of the queries
-// flagged in ws->flags (no-ops when none is).
+// one pair per slot, empty slots included; every candidate passed the row filter), their top-k into the outputs, then
+// the dense fix-up of the queries flagged in ws->flags under the row filter (no-ops when none is).
 static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, const float *X, uint64_t N,
                              uint32_t d, const uint64_t *col_ids, uint32_t k, uint32_t cap, TopkOut out, float *Dbuf,
-                             uint64_t ld)
+                             uint64_t ld, RowFilter rf)
 {
     launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, cap, d, LGPU_L2, ws->t_exact.as<float>(), st);
     launch_select(select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), cap, B, k, out), st);
     launch_dist_matrix(Q, X, B, N, d, 0, nullptr, nullptr, Dbuf, ld, st, ws->flags.as<uint32_t>());
     SelectArgs sc = select_rows(Dbuf, N, ld, B, k, out);
     sc.col_ids = col_ids; sc.only = ws->flags.as<uint32_t>();
+    sc.allow = rf.bits; sc.allow_bits = rf.nbits;
     launch_select(sc, st);
 }
 
-// Tensor-core shortlist + exact re-score (squared L2 only): the k best of the N rows of X for each
-// of B queries by exact lance-order distance, ids from col_ids (or the row index), ascending by
-// (distance, id).  Dbuf: [B][ld] f32 scratch.  Queries whose shortlist cannot be proven complete
-// (band_check) are redone by the exact kernels in the same stream, without a host round trip.
+// Tensor-core shortlist + exact re-score (squared L2 only): the k best of the N rows of X that pass the row filter rf
+// (none: every row) for each of B queries by exact lance-order distance, ids from col_ids (or the row index),
+// ascending by (distance, id).  Dbuf: [B][ld] f32 scratch.  The shortlist holds the kp best allowed rows by approximate
+// score; queries whose shortlist cannot be proven complete (band_check: it is full and its last score is within the
+// band of the k-th) are redone by the exact kernels in the same stream, without a host round trip.
 static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
                        const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
-                       const uint64_t *col_ids, uint32_t k, uint32_t kp, TopkOut out, float *Dbuf, uint64_t ld)
+                       const uint64_t *col_ids, uint32_t k, uint32_t kp, TopkOut out, float *Dbuf, uint64_t ld,
+                       RowFilter rf)
 {
     ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
     ws->flags.ensure((size_t)B * 4);
@@ -694,21 +721,23 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
     SelectArgs sa = select_rows(Dbuf, N, ld, B, kp, {ws->t_ids.as<uint64_t>(), ws->t_dist.as<float>(),
                                                      ws->t_cnt.as<uint32_t>(), ws->t_pos.as<uint64_t>()});
     sa.col_ids = col_ids;
+    sa.allow = rf.bits; sa.allow_bits = rf.nbits;
     launch_select(sa, st);
     if (kp >= N) LGPU_CUDA(cudaMemsetAsync(ws->flags.p, 0, (size_t)B * 4, st));   // every row is a candidate
     else launch_band_check(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                            xmax, xerr, d, B, k, kp, ws->flags.as<uint32_t>(), st);
-    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, kp, out, Dbuf, ld);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, kp, out, Dbuf, ld, rf);
 }
 
 // Large-N variant of tc_topk_l2 (flat search): a tensor-core pass over a row sample fixes, per query, a
-// score threshold that provably admits every true top-k row; the pass over all rows then runs with the
-// filtering epilogue (no dense score matrix), the few admitted rows are re-scored exactly, and queries whose
-// candidate list overflowed are redone by the exact kernels.
+// score threshold that provably admits every true top-k row (from the k best sample rows that pass the row filter rf:
+// with fewer, +inf); the pass over all rows then runs with the filtering epilogue (no dense score matrix), admitting
+// the rows under the threshold that pass rf, the few admitted rows are re-scored exactly, and queries whose candidate
+// list overflowed are redone by the exact kernels.
 static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
                                 const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
                                 const uint64_t *col_ids, uint32_t k, TopkOut out, float *Dbuf, uint64_t ld,
-                                uint64_t min_sample = 65536, uint32_t cap = 1024)
+                                RowFilter rf, uint64_t min_sample = 65536, uint32_t cap = 1024)
 {
     const uint64_t Ns = std::min<uint64_t>(N, std::max<uint64_t>(min_sample, N / 8));
     const uint64_t lds = (Ns + 3) & ~3ull;               // Dbuf is [B][ld >= lds]
@@ -722,8 +751,10 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
     // 1. sample pass: dense scores of the first Ns rows, k-th best per query -> threshold
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, Ns, d, Dbuf, lds, num_sms, st);
-    launch_select(select_rows(Dbuf, Ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
-                                                    ws->t_cnt.as<uint32_t>()}), st);
+    SelectArgs ss = select_rows(Dbuf, Ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
+                                                      ws->t_cnt.as<uint32_t>()});
+    if (rf.bits) { ss.col_ids = col_ids; ss.allow = rf.bits; ss.allow_bits = rf.nbits; }
+    launch_select(ss, st);
     launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                             xmax, xerr, d, B, k, ws->probe_A.as<float>(), st);
     // 2. full pass with the filtering epilogue
@@ -733,11 +764,12 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     GemmFilter flt{};
     flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
     flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap;
+    flt.allow = rf.bits; flt.allow_bits = rf.nbits;
     if (Ns == N) launch_filter_dense(Dbuf, lds, B, N, flt, st);      // the sample pass already scored every row
     else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, ws->probe_A.as<float>(), B, ws->flags.as<uint32_t>(), st);
     // 3. exact re-score of the admitted rows, final top-k; 4. fix-up of overflowed queries
-    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out, Dbuf, ld);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out, Dbuf, ld, rf);
 }
 
 // top-k by (distance, id) of the dense scores D [b][ld] over N columns, with the request's distance range and
@@ -1544,6 +1576,8 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
     size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(sp.k);
     uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(workspace_budget() / per_q, B));
     const TopkOut out{d_ids, d_dist, d_cnt};
+    const bool prof = profiling_enabled();
+    if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));      // [1] tensor-core distances, [3] queries
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
@@ -1556,19 +1590,21 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
             xn = ws->xnorm.as<float>();
         }
         const uint32_t kp = (uint32_t)std::min<uint64_t>(N, std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(8 * sp.k, 256)));
-        // (a prefilter goes through the exact kernels: the shortlist thresholds are fixed on unfiltered rows, and so
-        // does k above SELECT_KMAX: the shortlists are sized to SELECT_KMAX)
+        // (a row filter -- a prefilter, deleted rows -- stays on the tensor cores: the shortlists and thresholds are
+        // taken over the allowed rows, DESIGN.md section 3; k above SELECT_KMAX goes through the exact kernels: the
+        // shortlists are sized to SELECT_KMAX)
         if (fl->has_tc && tc_enabled() && metric == LGPU_L2 && !sp.has_lower && !sp.has_upper && b >= 8 && N >= 4096 &&
-            !rf.bits && sp.k <= SELECT_KMAX) {
+            sp.k <= SELECT_KMAX) {
             if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
                 tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p,
                                     fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
                                     fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, out.at(q0, sp.k),
-                                    ws->D.as<float>(), ld);
+                                    ws->D.as<float>(), ld, rf);
             else
                 tc_topk_l2(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p, fl->vec_n2.as<float>(),
                            fl->vec_max, fl->vec_err, N, fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp,
-                           out.at(q0, sp.k), ws->D.as<float>(), ld);
+                           out.at(q0, sp.k), ws->D.as<float>(), ld, rf);
+            if (prof) g_filter_stats[1] += (uint64_t)b * N;
             continue;
         }
         launch_dist_matrix(q, fl->vectors.as<float>(), b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
@@ -1576,18 +1612,20 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
         select_dense(ws, ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
                      out.at(q0, sp.k), st);
     }
+    if (prof) g_filter_stats[3] = B;
 }
 
 // ---- binary vectors (Hamming distance) ----
 // Paths, chosen from shape and request (DESIGN.md section 6):
 //   SIMT dense    ham_dense_kernel -> D[b][N] -> select mode 1.  N < HAM_TC_MIN_N, or fewer than HAM_TC_MIN_B queries
-//                 with N <= HAM_SAMPLE, prefilter or distance_range, LGPU_NO_TENSOR_CORE=1.
+//                 with N <= HAM_SAMPLE, distance_range, LGPU_NO_TENSOR_CORE=1.
 //   wgmma dense   the b1 gemm_dist_kernel writes D[b][N] -> select mode 1 (N <= HAM_SAMPLE).
 //   wgmma list    N > HAM_SAMPLE, any batch size: sample pass -> threshold -> filtering pass -> select mode 2 -> dense
 //                 fix-up of the queries whose list overflowed (ham_topk_list).  On the H100 it beat the SIMT kernel at
 //                 every batch size measured, one query included: a single query's select over a dense row of N
 //                 columns runs on one SM.
-// Every path computes exact integer distances, so all three return the same rows.
+// Every path computes exact integer distances, so all three return the same rows.  A row filter (prefilter, deleted
+// rows) keeps the path: the selects, the sample's threshold and the filtering pass all skip the rows it leaves out.
 // Candidate-list capacity of the list path.  Rows with d <= tau_q, tau_q the k-th smallest distance among the sample's
 // rows, number about k N / ns (more under ties): 4x that, at least 1024, at most 16384.
 static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
@@ -1598,26 +1636,55 @@ static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
     return cap;
 }
 
-// One sub-batch through the tensor-core list path (Q: padded queries [B][nbytes_pad], qpop [B]).  The dense fix-up of
-// overflowed queries runs in chunks of `bf` queries over a [bf][N] matrix: one launch lists each chunk's flagged
-// queries, and each chunk's two launches return at once when its list is empty.
+// The threshold sample of the list path, taken from the handle's rows at open and after every append (which hold the
+// handle alone): every (nrows / HAM_SAMPLE)-th row, packed, with its popcount and its id.  Enqueued on the legacy
+// stream; the caller synchronises.
+static void ham_sample(lgpu_binary *bx, uint64_t nrows)
+{
+    if (nrows <= HAM_SAMPLE) return;
+    const uint64_t stride = nrows / HAM_SAMPLE;
+    const uint32_t nbp = bx->nbytes_pad;
+    bx->nsample = HAM_SAMPLE;
+    bx->sample.ensure((size_t)HAM_SAMPLE * nbp);
+    bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
+    bx->sample_ids.ensure((size_t)HAM_SAMPLE * 8);
+    launch_ham_pack(bx->vectors.as<uint8_t>(), stride * nbp, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp,
+                    bx->sample_pop.as<uint32_t>(), nullptr);
+    if (bx->has_ids) {
+        LGPU_CUDA(cudaMemcpy2DAsync(bx->sample_ids.p, 8, bx->row_ids.p, stride * 8, 8, HAM_SAMPLE,
+                                    cudaMemcpyDeviceToDevice, nullptr));
+    } else {
+        std::vector<uint64_t> ids(HAM_SAMPLE);
+        for (uint64_t s = 0; s < HAM_SAMPLE; s++) ids[s] = s * stride;
+        LGPU_CUDA(cudaMemcpy(bx->sample_ids.p, ids.data(), ids.size() * 8, cudaMemcpyHostToDevice));
+    }
+}
+
+// One sub-batch through the tensor-core list path (Q: padded queries [B][nbytes_pad], qpop [B]) over the rows that pass
+// the row filter rf (none: every row).  The dense fix-up of overflowed queries runs in chunks of `bf` queries over a
+// [bf][N] matrix: one launch lists each chunk's flagged queries, and each chunk's two launches return at once when its
+// list is empty.
 static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
-                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, TopkOut out)
+                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, TopkOut out, RowFilter rf)
 {
     const uint64_t N = bx->nrows, ns = bx->nsample, lds = (ns + 3) & ~3ull, ld = (N + 3) & ~3ull;
     const uint32_t nbp = bx->nbytes_pad;
     const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
-    // 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest (an upper bound of the true k-th)
+    // 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest over the allowed ones (an upper
+    // bound of the true k-th; +inf with fewer than k)
     launch_ham_gemm(Q, bx->sample.p, bx->sample_pop.as<uint32_t>(), qpop, B, ns, nbp, ws->h_sample.as<float>(), lds,
                     bx->num_sms, st);
-    launch_select(select_rows(ws->h_sample.as<float>(), ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
-                                                                        ws->t_cnt.as<uint32_t>()}), st);
+    SelectArgs ss = select_rows(ws->h_sample.as<float>(), ns, lds, B, k, {ws->sbound.as<uint64_t>(),
+                                                                          ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>()});
+    if (rf.bits) { ss.col_ids = bx->sample_ids.as<uint64_t>(); ss.allow = rf.bits; ss.allow_bits = rf.nbits; }
+    launch_select(ss, st);
     launch_ham_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), B, k, ws->probe_A.as<float>(), st);
-    // 2. full pass: every row with d <= tau_q is appended as (position, id, distance); the distance is final
+    // 2. full pass: every allowed row with d <= tau_q is appended as (position, id, distance); the distance is final
     LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
     GemmFilter flt{};
     flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
     flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap; flt.cand_s = ws->t_exact.as<float>();
+    flt.allow = rf.bits; flt.allow_bits = rf.nbits;
     launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, nullptr, B, ws->flags.as<uint32_t>(), st);
     // 3. top-k by (distance, id) of each list (an overflowed list is complete up to cap; its query is redone below)
@@ -1632,6 +1699,7 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
                          ws->h_list.as<uint32_t>() + q0, ws->h_cnt.as<uint32_t>() + c);
         SelectArgs sc = select_rows(ws->D.as<float>(), N, ld, b, k, out.at(q0, k));
         sc.col_ids = col_ids; sc.only = ws->flags.as<uint32_t>() + q0; sc.gate = ws->h_cnt.as<uint32_t>() + c;
+        sc.allow = rf.bits; sc.allow_bits = rf.nbits;
         launch_select(sc, st);
     }
 }
@@ -1650,7 +1718,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
     launch_ham_pack(d_q, bx->nbytes, bx->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
     const uint8_t *Q = ws->hq.as<uint8_t>();
-    const bool tc_ok = tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper;
+    const bool tc_ok = tc_enabled() && !sp.has_lower && !sp.has_upper;
     // k above SELECT_KMAX: a dense path (the list path's capacity stops at 16384 rows)
     const bool list = tc_ok && bx->nsample > 0 && k <= SELECT_KMAX;
     const bool tc = list || (tc_ok && B >= HAM_TC_MIN_B && N >= HAM_TC_MIN_N);
@@ -1675,7 +1743,8 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         for (uint32_t q0 = 0; q0 < B; q0 += bs) {
             const uint32_t b = std::min(bs, B - q0);
             if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, ws->hq_pop.as<uint32_t>() + q0, b, k, cap, bf, out.at(q0, k));
+            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, ws->hq_pop.as<uint32_t>() + q0, b, k, cap, bf, out.at(q0, k),
+                          rf);
             if (prof) {             // [0] list appends, [2] queries redone densely (over every sub-batch)
                 std::vector<uint32_t> cnt(b), fl(b);
                 LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->amax.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
@@ -2027,6 +2096,22 @@ static RowFilter upload_allow(Workspace *ws, cudaStream_t st, const uint32_t *al
     return rf;
 }
 
+// The row filter of a call on a handle, given the call's own (rf, none when rf.bits is null): rf itself when nothing
+// was deleted; the handle's live bitmap when the call has none (no copy, no launch); else their AND, made on `st` into
+// the workspace once per call and charged to the call's workspace budget (WsCharge).  A row passes the result exactly
+// when it passes rf and was not deleted.
+static RowFilter with_live(Workspace *ws, cudaStream_t st, RowFilter rf, const RowLive &live)
+{
+    if (!live.active) return rf;
+    const uint32_t *lb = static_cast<const uint32_t *>(live.bits.p);
+    if (!rf.bits) return {lb, live.id_bound};
+    const uint64_t nbits = std::min(rf.nbits, live.id_bound), words = (nbits + 31) / 32;
+    ws->live_and.ensure(std::max<size_t>(words, 1) * 4);
+    g_ws_charged += std::max<size_t>(words, 1) * 4;
+    launch_rowmask_and(rf.bits, lb, words, ws->live_and.as<uint32_t>(), st);
+    return {ws->live_and.as<uint32_t>(), nbits};
+}
+
 // where a search call's buffers live
 struct Route {
     enum Via { HOST, FILTERED, DEVICE } via;
@@ -2051,6 +2136,7 @@ int search_call(H *hp, const Route &r, const T *queries, uint32_t B, const lgpu_
                 uint64_t *ids, float *dist, uint32_t *cnt, Check &&check, Search &&search)
 {
     return guarded([&] {
+        const WsCharge charge;
         HandleRef<H> h(hp);
         const size_t q_elems = check(h.h);
         if (r.via == Route::FILTERED) LGPU_REQUIRE(r.allow != nullptr || r.allow_bits == 0, "allow bitmap is null");
@@ -2058,7 +2144,8 @@ int search_call(H *hp, const Route &r, const T *queries, uint32_t B, const lgpu_
         require_device(h->device);
         if (r.via == Route::DEVICE) {
             WsLease lease(h->pool, (cudaStream_t)r.stream, true);
-            search(h.h, lease.ws, lease.st, queries, B, *p, ids, dist, cnt, RowFilter(), nullptr);
+            search(h.h, lease.ws, lease.st, queries, B, *p, ids, dist, cnt,
+                   with_live(lease.ws, lease.st, RowFilter(), h->live), nullptr);
             return;
         }
         uint64_t key[4];
@@ -2068,7 +2155,7 @@ int search_call(H *hp, const Route &r, const T *queries, uint32_t B, const lgpu_
                       const Deadline &dl) {
                       const RowFilter rf = r.via == Route::FILTERED ? upload_allow(ws, st, r.allow, r.allow_bits)
                                                                     : RowFilter();
-                      search(h.h, ws, st, dq, B, *p, di, dd, dc, rf, &dl);
+                      search(h.h, ws, st, dq, B, *p, di, dd, dc, with_live(ws, st, rf, h->live), &dl);
                   });
     });
 }
@@ -2902,7 +2989,9 @@ int lgpu_search_async(lgpu_index *ixh, const float *queries, uint32_t B, const l
             const lgpu_search_params sp = *params;
             host_submit(t->lease, t->deadline, queries, (size_t)B * ix->dim, B, sp.k, out_ids, out_dist, out_count, key,
                         [&](Workspace *ws, cudaStream_t st, const float *dq, uint64_t *di, float *dd, uint32_t *dc,
-                            const Deadline &) { ivf_search_device(ix, ws, st, dq, B, sp, di, dd, dc); },
+                            const Deadline &) {
+                            ivf_search_device(ix, ws, st, dq, B, sp, di, dd, dc, with_live(ws, st, RowFilter(), ix->live));
+                        },
                         false);
         }
         LGPU_CUDA(cudaEventRecord(t->done, t->lease.st));
@@ -3048,16 +3137,9 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
             launch_ham_pack(raw.as<uint8_t>(), nbytes, nbytes, nrows, bx->vectors.as<uint8_t>(), nbp, bx->pop.as<uint32_t>(),
                             nullptr);
         }
-        if (nrows > HAM_SAMPLE) {
-            const uint64_t stride = nrows / HAM_SAMPLE;
-            bx->nsample = HAM_SAMPLE;
-            bx->sample.ensure((size_t)HAM_SAMPLE * nbp);
-            bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
-            launch_ham_pack(bx->vectors.as<uint8_t>(), stride * nbp, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp,
-                            bx->sample_pop.as<uint32_t>(), nullptr);
-        }
-        LGPU_CUDA(cudaDeviceSynchronize());
         open_rows(bx, row_ids, nrows);
+        ham_sample(bx, nrows);
+        LGPU_CUDA(cudaDeviceSynchronize());
         register_handle(bx);
         *out = bx;
     });
@@ -3189,14 +3271,122 @@ template <class H> static void append_ids(H *h, uint64_t n0, uint64_t n, const u
     h->has_ids = true;
 }
 
-// What every append does first, with the handle held exclusively: drain the device (a search enqueued earlier on a
-// caller's stream may still read the buffers that move or the sample that is rewritten), and invalidate every captured
-// graph, which bakes the row count in even when no buffer moves.
+// What every append and delete does first, with the handle held exclusively: drain the device (a search enqueued
+// earlier on a caller's stream may still read the buffers that move, the sample that is rewritten or the live bitmap
+// that changes), and invalidate every captured graph, which bakes the row count and the row filter in even when no
+// buffer moves.
 static void begin_append(int device)
 {
     require_device(device);
     LGPU_CUDA(cudaDeviceSynchronize());
     g_alloc_epoch++;
+}
+
+// ---- deleted rows (lgpu_*_delete): the live bitmap of a handle (RowLive) ----
+// the row ids of a handle in device memory, or null when they are the positions 0 .. nrows - 1
+template <class H> static const uint64_t *device_row_ids(H *h)
+{
+    if constexpr (std::is_base_of_v<lgpu_index, H>) return h->row_ids.template as<uint64_t>();
+    else return h->has_ids ? h->row_ids.template as<uint64_t>() : nullptr;
+}
+
+static void require_id_bound(uint64_t max_id)
+{
+    LGPU_REQUIRE(max_id < LGPU_DELETE_ID_BOUND, "deleting rows needs every row id of the handle below "
+                                                "LGPU_DELETE_ID_BOUND (2^32): the live bitmap holds one bit per id");
+}
+
+// the first delete: id_bound, and a bitmap with the bit of every row id the handle holds
+template <class H> static void build_live(H *h)
+{
+    if (h->live.active) return;
+    const uint64_t *ids = device_row_ids(h);
+    uint64_t bound = h->nrows;
+    if (ids && h->nrows) {
+        DevBuf m;
+        m.ensure(8);
+        LGPU_CUDA(cudaMemset(m.p, 0, 8));
+        launch_rowmask_max(ids, h->nrows, m.as<unsigned long long>(), nullptr);
+        uint64_t mx = 0;
+        LGPU_CUDA(cudaMemcpy(&mx, m.p, 8, cudaMemcpyDeviceToHost));
+        require_id_bound(mx);
+        bound = mx + 1;
+    } else if (bound) {
+        require_id_bound(bound - 1);
+    }
+    h->live.bits.ensure(std::max<size_t>((bound + 31) / 32, 1) * 4);
+    LGPU_CUDA(cudaMemset(h->live.bits.p, 0, h->live.bits.bytes));
+    launch_rowmask_set(h->live.bits.template as<uint32_t>(), bound, ids, 0, h->nrows, nullptr);
+    LGPU_CUDA(cudaDeviceSynchronize());
+    h->live.id_bound = bound;
+    h->live.active = true;
+}
+
+// An append to a handle with deleted rows, checked before anything changes: the id_bound after the n rows (row_ids:
+// host, null = the positions that follow).  An appended row may not take the id of a deleted row the handle still
+// holds: the id's bit would make that row live again, and nothing is undeleted.  (Ids at or above id_bound name no
+// row, so the usual append -- ids above every held one -- needs no device work for this.)
+template <class H> static uint64_t live_bound_after(H *h, uint64_t n, const uint64_t *row_ids)
+{
+    if (!h->live.active) return 0;
+    uint64_t mn = h->nrows, mx = h->nrows + n - 1;
+    if (row_ids) {
+        mn = UINT64_MAX; mx = 0;
+        for (uint64_t i = 0; i < n; i++) { mn = std::min(mn, row_ids[i]); mx = std::max(mx, row_ids[i]); }
+    }
+    require_id_bound(mx);
+    const uint64_t nbits = h->live.id_bound;
+    if (mn < nbits) {
+        DevBuf mark, ids, cnt;
+        mark.ensure(std::max<size_t>((nbits + 31) / 32, 1) * 4);
+        LGPU_CUDA(cudaMemset(mark.p, 0, mark.bytes));
+        if (row_ids) upload(ids, row_ids, (size_t)n * 8);
+        launch_rowmask_set(mark.as<uint32_t>(), nbits, row_ids ? ids.as<uint64_t>() : nullptr, h->nrows, n, nullptr);
+        cnt.ensure(8);
+        LGPU_CUDA(cudaMemsetAsync(cnt.p, 0, 8, nullptr));
+        launch_rowmask_revived(mark.as<uint32_t>(), static_cast<const uint32_t *>(h->live.bits.p), nbits,
+                               device_row_ids(h), h->nrows, cnt.as<unsigned long long>(), nullptr);
+        uint64_t revived = 0;
+        LGPU_CUDA(cudaMemcpy(&revived, cnt.p, 8, cudaMemcpyDeviceToHost));
+        LGPU_REQUIRE(revived == 0, "an appended row takes the id of a deleted row of the handle: appending it would "
+                                   "undelete that row");
+    }
+    return std::max(nbits, mx + 1);
+}
+
+// ... and the appended rows marked live, once their ids are in place
+template <class H> static void grow_live(H *h, uint64_t n0, uint64_t n, uint64_t bound)
+{
+    if (!h->live.active) return;
+    const size_t w0 = (h->live.id_bound + 31) / 32, w1 = (bound + 31) / 32;
+    if (w1 > w0) {
+        grow_keep(h->live.bits, w0 * 4, w1 * 4);
+        LGPU_CUDA(cudaMemset(h->live.bits.template as<uint32_t>() + w0, 0, (w1 - w0) * 4));
+    }
+    launch_rowmask_set(h->live.bits.template as<uint32_t>(), bound,
+                       h->has_ids ? h->row_ids.template as<uint64_t>() + n0 : nullptr, n0, n, nullptr);
+    h->live.id_bound = bound;
+}
+
+template <class H> static int delete_rows(H *hp, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
+{
+    return guarded([&] {
+        HandleExcl<H> h(hp);
+        LGPU_REQUIRE(n == 0 || row_ids != nullptr, "null row ids");
+        if (n_deleted) *n_deleted = 0;
+        if (n == 0) return;
+        begin_append(h->device);
+        build_live(h.h);
+        DevBuf ids, cnt;
+        upload(ids, row_ids, (size_t)n * 8);
+        cnt.ensure(8);
+        LGPU_CUDA(cudaMemsetAsync(cnt.p, 0, 8, nullptr));
+        launch_rowmask_clear(h->live.bits.template as<uint32_t>(), h->live.id_bound, ids.as<uint64_t>(), n,
+                             cnt.as<unsigned long long>(), nullptr);
+        uint64_t c = 0;
+        LGPU_CUDA(cudaMemcpy(&c, cnt.p, 8, cudaMemcpyDeviceToHost));
+        if (n_deleted) *n_deleted = c;
+    });
 }
 
 extern "C" {
@@ -3208,6 +3398,7 @@ int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64
         lgpu_flat *fl = h.h;
         LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
         if (n == 0) return;
+        const uint64_t bound = live_bound_after(fl, n, row_ids);
         begin_append(fl->device);
         const uint64_t n0 = fl->nrows, n1 = n0 + n;
         const uint32_t d = fl->dim;
@@ -3215,6 +3406,7 @@ int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64
         float *x = fl->vectors.as<float>() + (size_t)n0 * d;
         LGPU_CUDA(cudaMemcpy(x, rows, (size_t)n * d * 4, cudaMemcpyHostToDevice));
         append_ids(fl, n0, n, row_ids);
+        grow_live(fl, n0, n, bound);
         if (fl->has_norms) {
             grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
             launch_row_norms(x, n, d, fl->ysqrt.as<float>() + n0, nullptr);
@@ -3248,6 +3440,7 @@ int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const 
         lgpu_binary *bx = h.h;
         LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
         if (n == 0) return;
+        const uint64_t bound = live_bound_after(bx, n, row_ids);
         begin_append(bx->device);
         const uint64_t n0 = bx->nrows, n1 = n0 + n;
         const uint32_t nbp = bx->nbytes_pad;
@@ -3258,17 +3451,36 @@ int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const 
         launch_ham_pack(raw.as<uint8_t>(), bx->nbytes, bx->nbytes, n, bx->vectors.as<uint8_t>() + (size_t)n0 * nbp, nbp,
                         bx->pop.as<uint32_t>() + n0, nullptr);
         append_ids(bx, n0, n, row_ids);
-        if (n1 > HAM_SAMPLE) {             // the threshold sample lgpu_binary_open takes from n1 rows
-            const uint64_t stride = n1 / HAM_SAMPLE;
-            bx->nsample = HAM_SAMPLE;
-            bx->sample.ensure((size_t)HAM_SAMPLE * nbp);
-            bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
-            launch_ham_pack(bx->vectors.as<uint8_t>(), stride * nbp, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp,
-                            bx->sample_pop.as<uint32_t>(), nullptr);
-        }
+        grow_live(bx, n0, n, bound);
+        ham_sample(bx, n1);                // the threshold sample lgpu_binary_open takes from n1 rows
         LGPU_CUDA(cudaDeviceSynchronize());
         bx->nrows = n1;
     });
+}
+
+int lgpu_index_delete(lgpu_index *ix, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
+{
+    return delete_rows(ix, row_ids, n, n_deleted);
+}
+
+int lgpu_ivf_binary_delete(lgpu_ivf_binary *ix, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
+{
+    return delete_rows(ix, row_ids, n, n_deleted);
+}
+
+int lgpu_flat_delete(lgpu_flat *fl, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
+{
+    return delete_rows(fl, row_ids, n, n_deleted);
+}
+
+int lgpu_binary_delete(lgpu_binary *bx, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
+{
+    return delete_rows(bx, row_ids, n, n_deleted);
+}
+
+int lgpu_multivec_delete(lgpu_multivec *mv, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
+{
+    return delete_rows(mv, row_ids, n, n_deleted);
 }
 
 }  // extern "C"
@@ -3304,8 +3516,10 @@ static void union_search_device(IX *ix, Workspace *ws, cudaStream_t st, TL *tl, 
     uint64_t *ids = ws->u_ids.as<uint64_t>();
     float *dist = ws->u_dist.as<float>();
     uint32_t *cnt = ws->u_cnt.as<uint32_t>();
+    // each handle's own deleted rows (rf: the call's filter)
+    const RowFilter rf_ix = with_live(ws, st, rf, ix->live);
     // ivf_search_device's own refusal, checked before the fork (no tail work is left behind by it)
-    if (rf.bits && std::min<uint32_t>(sp.max_nprobes, ix->nlist) > std::min<uint32_t>(std::max<uint32_t>(sp.nprobes, 1), ix->nlist))
+    if (rf_ix.bits && std::min<uint32_t>(sp.max_nprobes, ix->nlist) > std::min<uint32_t>(std::max<uint32_t>(sp.nprobes, 1), ix->nlist))
         LGPU_REQUIRE(std::min<uint32_t>(sp.max_nprobes, ix->nlist) <= SELECT_KMAX || sp.max_nprobes >= ix->nlist,
                      "maximum_nprobes above 2048 is not supported unless it covers every partition");
     // joins the tail's stream back into st on every exit, a throw included (a timeout between sub-batches, a CUDA
@@ -3325,11 +3539,12 @@ static void union_search_device(IX *ix, Workspace *ws, cudaStream_t st, TL *tl, 
         LGPU_CUDA(cudaEventRecord(wt->ev_fork, st));
         LGPU_CUDA(cudaStreamWaitEvent(wt->stream, wt->ev_fork, 0));
         join.forked = true;
-        tail_search(ix, tl, wt, wt->stream, d_q, B, sp, ids + bk, dist + bk, cnt + B, rf, dl);
+        tail_search(ix, tl, wt, wt->stream, d_q, B, sp, ids + bk, dist + bk, cnt + B,
+                    with_live(wt, wt->stream, rf, tl->live), dl);
     } else {                                    // an empty tail contributes an empty list
         LGPU_CUDA(cudaMemsetAsync(cnt + B, 0, (size_t)B * 4, st));
     }
-    ivf_search_device(ix, ws, st, d_q, B, sp, ids, dist, cnt, rf, dl);
+    ivf_search_device(ix, ws, st, d_q, B, sp, ids, dist, cnt, rf_ix, dl);
     if (join.forked) {
         join.forked = false;
         LGPU_CUDA(cudaEventRecord(wt->ev_join, wt->stream));
@@ -3349,6 +3564,7 @@ static int union_call(IX *ixh, TL *tlh, bool device, const T *q, uint32_t B, con
                       void *stream)
 {
     return guarded([&] {
+        const WsCharge charge;
         HandleRef<IX> ix(ixh);
         HandleRef<TL> tl(tlh);
         check_ivf_call(ix.h, q, B, p, ids, dist, cnt);
@@ -3655,7 +3871,7 @@ static void sharded_search_device(lgpu_index *ix, lgpu_comm *c, Workspace *ws, c
     c->send.ensure(n * sizeof(TopkRecord)); c->recv.ensure(n * sizeof(TopkRecord) * c->world);
     const bool prof = profiling_enabled();
     ivf_search_device(ix, ws, st, d_q, B, sp, c->l_ids.as<uint64_t>(), c->l_dist.as<float>(), c->l_cnt.as<uint32_t>(),
-                      RowFilter(), deadline);
+                      with_live(ws, st, RowFilter(), ix->live), deadline);
     launch_pack_records(c->l_ids.as<uint64_t>(), c->l_dist.as<float>(), n, c->send.as<TopkRecord>(), st);
     if (prof) cudaEventRecord(c->ev[0], st);
     LGPU_NCCL(nccl_api().AllGather(c->send.p, c->recv.p, n * sizeof(TopkRecord), ncclUint8, c->comm, st));

@@ -204,8 +204,10 @@ struct F16MaxSim {
 
 // LIST: the filtering epilogue for DENSE hit rates (coarse step at many lists), see the epilogue; a separate
 // instantiation so that the dense / sparse-filter kernel of the flat path and of the small coarse problems carries
-// none of its code.  Pol: Bf16Dist or B1Hamming (above).
-template <bool LIST, class Pol>
+// none of its code.  ROWF: the filtering epilogues admit only columns that pass the filter's row filter (flt.allow);
+// also a separate instantiation, so the kernels of unfiltered calls are the ones they were without it.
+// Pol: Bf16Dist or B1Hamming (above).
+template <bool LIST, class Pol, bool ROWF = false>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
                  const typename Pol::Row *__restrict__ xnorm2, float *__restrict__ out, uint64_t ld_out, uint32_t B,
@@ -344,6 +346,12 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                     for (int e = 0; e < 2; e++)
                         if (live && c0 + 8 * j + e < N && Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], pq) <= thr)
                             hit |= 1u << (2 * j + e);
+                if (ROWF && hit) {                                       // the row filter, on the passing columns only
+                    for (uint32_t m = hit; m; m &= m - 1) {
+                        const int b = __ffs(m) - 1;
+                        if (!gemm_filter_admits(flt, c0 + 8 * (b >> 1) + (b & 1))) hit &= ~(1u << b);
+                    }
+                }
                 const uint32_t n = __popc(hit);
                 uint32_t incl = n, v;                                    // inclusive prefix over the row's 4 lanes
                 v = __shfl_up_sync(0xffffffffu, incl, 1, 4); if (lane & 3) incl += v;
@@ -383,7 +391,8 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
                         const uint64_t x = c0 + 8 * j + e;
-                        if (x < N && Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], 0) <= thr) {
+                        if (x < N && Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], 0) <= thr &&
+                            (!ROWF || gemm_filter_admits(flt, x))) {
                             const uint32_t slot = atomicAdd(flt.count + q, 1u);
                             if (slot < flt.cap) {
                                 flt.cand_pos[(size_t)q * flt.cap + slot] = x;
@@ -657,7 +666,7 @@ __global__ void filter_dense_kernel(const float *__restrict__ D, uint64_t ld, ui
     const float thr = flt.thr[q];
     const float *row = D + (size_t)q * ld;
     for (uint64_t x = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; x < N; x += (uint64_t)gridDim.x * blockDim.x) {
-        if (row[x] <= thr) {
+        if (row[x] <= thr && (!flt.allow || gemm_filter_admits(flt, x))) {
             const uint32_t slot = atomicAdd(flt.count + q, 1u);
             if (slot < flt.cap) {
                 flt.cand_pos[(size_t)q * flt.cap + slot] = x;
@@ -687,7 +696,9 @@ void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint3
     GemmFilter flt{};
     if (filter) flt = *filter;
     const bool list = flt.thr && flt.cand_s;                  // dense hit rates: one reservation per row and tile
-    auto kern = list ? gemm_dist_kernel<true, Bf16Dist> : gemm_dist_kernel<false, Bf16Dist>;
+    LGPU_REQUIRE(!(list && flt.allow), "the dense-rate filtering epilogue of float scores takes no row filter");
+    auto kern = list ? gemm_dist_kernel<true, Bf16Dist>
+                     : (flt.thr && flt.allow ? gemm_dist_kernel<false, Bf16Dist, true> : gemm_dist_kernel<false, Bf16Dist>);
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, xnorm2, out, ld_out, B, N, (uint32_t)((d + GK - 1) / GK), flt); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
@@ -705,7 +716,8 @@ void launch_ham_gemm(const void *Qp, const void *Xp, const uint32_t *xpop, const
     HamFilter flt{};
     if (filter) static_cast<GemmFilter &>(flt) = *filter;
     flt.qpop = reinterpret_cast<const int *>(qpop);
-    auto kern = flt.thr ? gemm_dist_kernel<true, B1Hamming> : gemm_dist_kernel<false, B1Hamming>;
+    auto kern = !flt.thr ? gemm_dist_kernel<false, B1Hamming>
+                         : (flt.allow ? gemm_dist_kernel<true, B1Hamming, true> : gemm_dist_kernel<true, B1Hamming>);
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, reinterpret_cast<const int *>(xpop), out, ld_out,
              B, N, (uint32_t)((nbytes_pad + 2 * GK - 1) / (2 * GK)), flt); LGPU_COUNT_LAUNCH();

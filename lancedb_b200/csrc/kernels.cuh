@@ -346,6 +346,20 @@ void launch_count_below(const uint32_t *cnt, uint32_t B, uint32_t k, uint32_t *f
 // rec[i] = (ids[i], dist[i]) for i < n
 void launch_pack_records(const uint64_t *ids, const float *dist, uint64_t n, TopkRecord *out, cudaStream_t st);
 
+// ---------------- live-row bitmaps of handles with deleted rows (rowmask.cu) ----------------
+// *out = max(*out, ids[0..n))
+void launch_rowmask_max(const uint64_t *ids, uint64_t n, unsigned long long *out, cudaStream_t st);
+// set the bits of ids[0..n) (ids null: of first .. first + n - 1) below nbits
+void launch_rowmask_set(uint32_t *bits, uint64_t nbits, const uint64_t *ids, uint64_t first, uint64_t n, cudaStream_t st);
+// *count += the rows i < n whose id (ids[i], ids null: i) is below nbits, set in mark and clear in live
+void launch_rowmask_revived(const uint32_t *mark, const uint32_t *live, uint64_t nbits, const uint64_t *ids, uint64_t n,
+                            unsigned long long *count, cudaStream_t st);
+// clear the bits of ids[0..n) below nbits; *count += the bits this call found set
+void launch_rowmask_clear(uint32_t *bits, uint64_t nbits, const uint64_t *ids, uint64_t n, unsigned long long *count,
+                          cudaStream_t st);
+// out[i] = a[i] & b[i] for i < words
+void launch_rowmask_and(const uint32_t *a, const uint32_t *b, uint64_t words, uint32_t *out, cudaStream_t st);
+
 // ---------------- tensor-core shortlist (gemm.cu) ------------------------------------
 bool gemm_shape_supported(uint32_t d);
 // X f32 [n][d] -> bf16 [n][d]; norm2[n] = |x|^2 (f32) if norm2 != nullptr; err[n] = |bf16(x) - x| if err != nullptr
@@ -376,7 +390,17 @@ struct GemmFilter {
     const uint64_t *col_ids;      // optional
     uint32_t cap;
     float *cand_s;                // optional [B][cap]: the admitted score itself (coarse step: second-level threshold)
+    // optional row filter: a column passing the threshold is admitted only if the bit of its id (col_ids[x] or x) is
+    // set, id < allow_bits (a prefilter, deleted rows)
+    const uint32_t *allow;
+    uint64_t allow_bits;
 };
+// whether column x passes the row filter of a filter that has one (tested only for columns under the threshold)
+__device__ __forceinline__ bool gemm_filter_admits(const GemmFilter &f, uint64_t x)
+{
+    const uint64_t id = f.col_ids ? f.col_ids[x] : x;
+    return id < f.allow_bits && ((__ldg(f.allow + (id >> 5)) >> (id & 31)) & 1u);
+}
 void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint32_t B, uint64_t N, uint32_t d,
                       float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter = nullptr);
 // the binary (Hamming) form of the same kernel: the GemmFilter fields plus popc(q) of every query

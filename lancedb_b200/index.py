@@ -95,6 +95,24 @@ def _extend_order(part_offsets, assign, row_ids):
     return order, new_off, rid
 
 
+def _compact_offsets(d, keep):
+    """The rows `keep` (bool [n], True = kept) selects from an IVF index `d`, checked, and the part_offsets u64
+    [nlist+1] once the others are dropped: every partition keeps its remaining rows in their order."""
+    keep = np.asarray(keep, bool).reshape(-1)
+    if keep.size != d.nrows:
+        raise ValueError("keep must hold one flag per row of the index")
+    off = np.asarray(d.part_offsets, np.int64)
+    label = np.repeat(np.arange(off.size - 1), np.diff(off))
+    new_off = np.zeros(off.size, np.uint64)
+    new_off[1:] = np.cumsum(np.bincount(label[keep], minlength=off.size - 1))
+    return keep, new_off
+
+
+def _kept(a, keep):
+    """Per-row array `a` (partition order) without the dropped rows (None stays None)."""
+    return None if a is None else np.ascontiguousarray(np.asarray(a)[keep])
+
+
 def _cat_rows(old, new, order):
     """Per-row arrays in the extended partition order (None stays None)."""
     if old is None:
@@ -194,6 +212,17 @@ class IvfPqIndexData:
         data = IvfPqIndexData(self.dim, self.nlist, self.m, self.metric, self.centroids, self.codebook, off,
                               _transpose_codes(_cat_rows(self.row_codes(), codes, order), off),
                               _cat_rows(self.row_ids, rid, order), _cat_rows(self.vectors, raw, order), self.num_bits)
+        data.validate()
+        return data
+
+    def compact(self, keep) -> "IvfPqIndexData":
+        """The index without the rows whose `keep` flag (bool [n], partition order) is False, without retraining: the
+        other rows keep their partitions, order and ids; each partition's codes are transposed again (4-bit rows keep
+        their packed bytes)."""
+        keep, off = _compact_offsets(self, keep)
+        data = IvfPqIndexData(self.dim, self.nlist, self.m, self.metric, self.centroids, self.codebook, off,
+                              _transpose_codes(_kept(self.row_codes(), keep), off), _kept(self.row_ids, keep),
+                              _kept(self.vectors, keep), self.num_bits)
         data.validate()
         return data
 
@@ -510,6 +539,14 @@ class IvfSqIndexData:
         data.validate()
         return data
 
+    def compact(self, keep) -> "IvfSqIndexData":
+        """The index without the rows whose `keep` flag is False (IvfPqIndexData.compact)."""
+        keep, off = _compact_offsets(self, keep)
+        data = IvfSqIndexData(self.dim, self.nlist, self.metric, self.centroids, off, _kept(self.codes, keep),
+                              _kept(self.row_ids, keep), self.lo, self.hi, _kept(self.vectors, keep))
+        data.validate()
+        return data
+
 
 def sq_encode(x, lo: float, hi: float) -> np.ndarray:
     """lance's scale_to_u8 [lance, recalled]: sat_u8(((double)v - lo) * 255 / (hi - lo)), left to right in f64,
@@ -604,6 +641,15 @@ class IvfRqIndexData:
                               _cat_rows(self.codes, codes, order), _cat_rows(self.add_factors, add, order),
                               _cat_rows(self.scale_factors, scale, order), _cat_rows(self.row_ids, rid, order),
                               _cat_rows(self.vectors, raw, order), self.num_bits)
+        data.validate()
+        return data
+
+    def compact(self, keep) -> "IvfRqIndexData":
+        """The index without the rows whose `keep` flag is False (IvfPqIndexData.compact)."""
+        keep, off = _compact_offsets(self, keep)
+        data = IvfRqIndexData(self.dim, self.nlist, self.metric, self.centroids, self.rotation, off,
+                              _kept(self.codes, keep), _kept(self.add_factors, keep), _kept(self.scale_factors, keep),
+                              _kept(self.row_ids, keep), _kept(self.vectors, keep), self.num_bits)
         data.validate()
         return data
 
@@ -724,6 +770,14 @@ class IvfBinaryIndexData:
         order, off, rid = _extend_order(self.part_offsets, parts, row_ids)
         data = IvfBinaryIndexData(self.nbytes, self.nlist, self.centroids, off, _cat_rows(self.vectors, x, order),
                                   _cat_rows(self.row_ids, rid, order))
+        data.validate()
+        return data
+
+    def compact(self, keep) -> "IvfBinaryIndexData":
+        """The index without the rows whose `keep` flag is False (IvfPqIndexData.compact)."""
+        keep, off = _compact_offsets(self, keep)
+        data = IvfBinaryIndexData(self.nbytes, self.nlist, self.centroids, off, _kept(self.vectors, keep),
+                                  _kept(self.row_ids, keep))
         data.validate()
         return data
 
@@ -889,7 +943,16 @@ class IvfHnswSqIndexData:
         """IvfSqIndexData.extend, then the graph of every partition that received rows is built again over all of its
         rows (build_hnsw_graph with the index's m, ef_construction and graph device); the other partitions keep their
         graphs."""
-        sq = self.sq.extend(vectors, row_ids, device)
+        return self._with_rows(self.sq.extend(vectors, row_ids, device), seed)
+
+    def compact(self, keep, seed: int = 45) -> "IvfHnswSqIndexData":
+        """IvfSqIndexData.compact, then the graph of every partition that lost rows is built again over the rows it
+        keeps, as extend does; the other partitions keep their graphs."""
+        return self._with_rows(self.sq.compact(keep), seed)
+
+    def _with_rows(self, sq: IvfSqIndexData, seed: int) -> "IvfHnswSqIndexData":
+        """This index's graphs over `sq`, whose partitions hold either this index's rows or a different number of
+        rows: the graph of a partition whose row count changed is built again."""
         old, new = self.part_offsets.astype(np.int64), sq.part_offsets.astype(np.int64)
         entry, top = self.entry.copy(), self.top_level.copy()
         lvs, adjs, uas = [], [], []

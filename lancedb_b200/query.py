@@ -200,7 +200,7 @@ class LanceVectorQueryBuilder:
             return tbl
         mask = None
         if self._where is not None:
-            mask = _filter.evaluate(t._data, self._where)          # row id == row position
+            mask = t._where_mask(self._where)                      # row id == row position; live rows only
         ids, dist, cnt = t._vector_search(
             self._query, column=self._vector_column, k=k, nprobes=nprobes,
             refine_factor=self._refine_factor, distance_type=self._distance_type,

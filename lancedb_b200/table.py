@@ -10,12 +10,15 @@ row positions, like a single-fragment Lance dataset.
 """
 from __future__ import annotations
 
+import threading
+from dataclasses import dataclass
 from typing import Dict, Iterable, List, Optional
 
 import numpy as np
 import pyarrow as pa
 
 from . import _native
+from . import filter as _filter
 from .index import IVF_KINDS
 from .query import LanceVectorQueryBuilder
 
@@ -82,11 +85,24 @@ _WRONG_COLUMN = {
 }
 
 
+@dataclass
+class DeleteResult:
+    """What Table.delete returns (python/python/lancedb/table.py:1672-1720)."""
+    num_deleted_rows: int
+    version: int
+
+
 class Table:
     def __init__(self, name: str, data: pa.Table, device: int = 0):
         self.name = name
         self._data = data
         self._device = device
+        # deleted rows stay in _data as tombstones, so a row's id (its position) never changes: _live is the mask of
+        # the rows not deleted (None: nothing was deleted).  Every GPU handle holding a deleted row has been told so
+        # (its .delete), and so leaves it out of every search.
+        self._live: Optional[np.ndarray] = None
+        self.version = 1                              # +1 for every add or delete that changes rows
+        self._lock = threading.RLock()                # serialises add, delete and optimize
         self._flat: Dict[str, _native.GpuFlat] = {}
         self._binary: Dict[str, _native.GpuBinary] = {}
         self._multivec: Dict[str, _native.GpuMultivec] = {}
@@ -103,16 +119,29 @@ class Table:
         return self._data.schema
 
     def count_rows(self) -> int:
-        return self._data.num_rows
+        return self._data.num_rows if self._live is None else int(self._live.sum())
 
     def __len__(self) -> int:
-        return self._data.num_rows
+        return self.count_rows()
 
     def to_arrow(self) -> pa.Table:
-        return self._data
+        return self._data if self._live is None else self._data.filter(pa.array(self._live))
 
     def to_pandas(self):
-        return self._data.to_pandas()
+        return self.to_arrow().to_pandas()
+
+    def _deleted(self) -> np.ndarray:
+        """The ids (positions) of the deleted rows, u64."""
+        return np.zeros(0, np.uint64) if self._live is None else np.nonzero(~self._live)[0].astype(np.uint64)
+
+    def _live_positions(self) -> Optional[np.ndarray]:
+        """The ids of the live rows, u64, or None when nothing was deleted."""
+        return None if self._live is None else np.nonzero(self._live)[0].astype(np.uint64)
+
+    def _where_mask(self, where: str) -> np.ndarray:
+        """The rows (by position) that are live and satisfy the SQL predicate `where`."""
+        mask = _filter.evaluate(self._data, where)
+        return mask if self._live is None else mask & self._live
 
     def _index_type(self, column: str) -> str:
         return self._index_data[column].index_type
@@ -127,8 +156,9 @@ class Table:
         if col not in self._index_data:
             return None
         d = self._index_data[col]
-        return {"index_type": self._index_type(col), "distance_type": d.metric, "num_indexed_rows": d.nrows,
-                "num_unindexed_rows": self.count_rows() - d.nrows, "num_indices": 1}
+        indexed = d.nrows if self._live is None else int(self._live[d.row_ids.astype(np.int64)].sum())
+        return {"index_type": self._index_type(col), "distance_type": d.metric, "num_indexed_rows": indexed,
+                "num_unindexed_rows": self.count_rows() - indexed, "num_indices": 1}
 
     def _vectors(self, column: str) -> np.ndarray:
         col = self._data.column(column).combine_chunks()
@@ -191,6 +221,10 @@ class Table:
         else:       # accelerator: the row passes run through the C ABI (build.cu); keep the raw vectors for refine
             vectors = self._vectors(column)
             kw.update(keep_vectors=True, native_passes=dev is not None)
+        live = self._live_positions()
+        if live is not None:        # trained on the live rows, which keep their positions as row ids
+            vectors = vectors[live.astype(np.int64)]
+            kw.update(row_ids=live)
         self._attach_index(column, kind.train(vectors, num_partitions=num_partitions, distance_type=metric,
                                               max_iterations=max_iterations, sample_rate=sample_rate, device=dev, **kw))
 
@@ -199,8 +233,7 @@ class Table:
             self._index[column].close()
         self._drop_tail(column)                 # the new index holds every row the table has
         self._index_data[column] = data
-        cls = getattr(_native, IVF_KINDS[data.index_type].handle)     # looked up now, so a replaced class is used
-        self._index[column] = cls(data, device=self._device)
+        self._index[column] = self._open_index(column)
 
     # ---- on-disk Lance index (SURVEY.md 8f-3; layout [lance, recalled], see lance_index.py) ----
     def load_lance_index(self, index_dir: str, vector_column_name: Optional[str] = None) -> None:
@@ -228,6 +261,10 @@ class Table:
 
     # ---- appends and index maintenance (python/python/lancedb/table.py:3393, 3970) ----
     def add(self, data, mode: str = "append", on_bad_vectors: str = "error", **_ignored) -> None:
+        with self._lock:
+            self._add(data, mode, on_bad_vectors)
+
+    def _add(self, data, mode: str, on_bad_vectors: str) -> None:
         """Append rows with the table's schema.  Row ids are table positions.  An indexed column's new rows are not
         indexed: they go to its tail, which every vector search scans exactly and merges with the index's result
         (unless fast_search()), until optimize() folds them into the index.
@@ -248,7 +285,7 @@ class Table:
             new = new.select(self.schema.names).cast(self.schema)
         except (pa.ArrowInvalid, pa.ArrowNotImplementedError, pa.ArrowTypeError, ValueError) as e:
             raise ValueError(f"the data does not match the table's schema: {e}") from None
-        n0, n = self.count_rows(), new.num_rows
+        n0, n = self._data.num_rows, new.num_rows          # positions, tombstones included: the new ids
         if n == 0:
             return
         rows = {c: self._rows_of(new, c) for c in _vector_columns(self.schema) if not self._is_multivec(c)}
@@ -270,22 +307,22 @@ class Table:
                 start = self._tail_from[column]
                 self._drop_tail(column)
                 if start < n0:
-                    cls = _native.GpuBinary if self._is_binary(column) else _native.GpuFlat
-                    self._tail[column] = cls(self._new_rows(column, start), device=self._device,
-                                             row_ids=np.arange(start, n0, dtype=np.uint64))
-                    self._tail_from[column] = start
+                    self._open_tail(column, start)
             raise
         self._data = pa.concat_tables([self._data, new]).combine_chunks()
+        if self._live is not None:
+            self._live = np.concatenate([self._live, np.ones(n, bool)])
         for cache in (self._flat, self._binary):         # full-column caches grow in place (ids = positions)
             for column in list(cache):
-                try:
-                    cache[column].append(rows[column])
+                try:   # (a cache opened over the live rows holds explicit ids: the new ones are passed)
+                    cache[column].append(rows[column], None if self._live is None else ids)
                 except BaseException:
                     cache.pop(column).close()             # reopened from the table on the next search
                     raise
         for mv in self._multivec.values():               # reopened on the next search
             mv.close()
         self._multivec.clear()
+        self.version += 1
 
     def _check_new_rows(self, column: str, x: np.ndarray) -> None:
         if self._is_binary(column):
@@ -318,16 +355,98 @@ class Table:
             tail.close()
         self._tail_from.pop(column, None)
 
+    def _open_tail(self, column: str, start: int) -> None:
+        """The tail of `column` from the table's rows start.. (ids = positions), told of the deleted ones."""
+        cls = _native.GpuBinary if self._is_binary(column) else _native.GpuFlat
+        rows = self._new_rows(column, start)
+        tail = cls(rows, device=self._device, row_ids=np.arange(start, start + rows.shape[0], dtype=np.uint64))
+        dead = self._deleted()
+        dead = dead[dead >= start]
+        if dead.size:
+            tail.delete(dead)
+        self._tail[column], self._tail_from[column] = tail, start
+
+    def _open_index(self, column: str):
+        """The handle of `column`'s IndexData, told of the deleted rows it holds."""
+        data = self._index_data[column]
+        h = getattr(_native, IVF_KINDS[data.index_type].handle)(data, device=self._device)
+        dead = self._deleted()
+        if dead.size:
+            held = np.zeros(self._data.num_rows, bool)
+            held[data.row_ids.astype(np.int64)] = True
+            dead = dead[held[dead.astype(np.int64)]]
+            if dead.size:
+                h.delete(dead)
+        return h
+
+    # ---- deletes (python/python/lancedb/table.py:1672-1720) ----
+    def delete(self, where: str) -> DeleteResult:
+        """Delete the rows that satisfy the SQL predicate `where`; returns DeleteResult(num_deleted_rows, version).
+        The rows stay in place as tombstones, so every other row keeps its _rowid; each GPU handle holding one is told
+        (lgpu_*_delete) and leaves it out of every later search, exactly as a prefilter would.  optimize() drops them
+        from the handles.  A failed delete leaves the table and every handle as they were."""
+        if not isinstance(where, str) or not where.strip():
+            raise ValueError("delete needs a non-empty SQL predicate")
+        with self._lock:
+            ids = np.nonzero(self._where_mask(where))[0].astype(np.uint64)
+            if ids.size == 0:
+                return DeleteResult(0, self.version)
+            # (handle, the ids it holds, how to open it again from the table's rows and tombstones)
+            todo = []
+            for column, idx in self._index.items():
+                start = self._tail_from.get(column)
+                held = ids if start is None else ids[ids < start]
+                todo.append((idx, held, lambda c=column: self._reopen_index(c)))
+            for column, tail in self._tail.items():
+                start = self._tail_from[column]
+                todo.append((tail, ids[ids >= start], lambda c=column, s=start: self._open_tail(c, s)))
+            for cache in (self._flat, self._binary, self._multivec):
+                for column, h in cache.items():
+                    todo.append((h, ids, lambda c=cache, col=column: c.pop(col).close()))   # reopened lazily
+            done = []
+            try:
+                for h, held, reopen in todo:
+                    if held.size:
+                        done.append(reopen)
+                        h.delete(held)
+            except BaseException:
+                for reopen in done:
+                    reopen()
+                raise
+            live = np.ones(self._data.num_rows, bool) if self._live is None else self._live.copy()
+            live[ids.astype(np.int64)] = False
+            self._live = live
+            self.version += 1
+            return DeleteResult(int(ids.size), self.version)
+
+    def _reopen_index(self, column: str) -> None:
+        self._index[column].close()
+        self._index[column] = self._open_index(column)
+
     def optimize(self, *, cleanup_older_than=None, delete_unverified: bool = False, retrain: bool = False) -> None:
         """Fold every indexed column's unindexed rows into its index without retraining (IndexData.extend: the fitted
         centroids and quantiser), then reopen it.  Compaction and version cleanup have nothing to do here."""
         if retrain:
             raise NotImplementedError("optimize(retrain=True) is not supported: rows are added with the index's model")
-        for column in list(self._tail):
-            start = self._tail_from[column]
-            rows = self._new_rows(column, start)
-            ids = np.arange(start, start + rows.shape[0], dtype=np.uint64)
-            self._attach_index(column, self._index_data[column].extend(rows, ids, device=self._device))
+        with self._lock:
+            for column in list(self._tail):
+                start = self._tail_from[column]
+                rows = self._new_rows(column, start)
+                ids = np.arange(start, start + rows.shape[0], dtype=np.uint64)
+                self._attach_index(column, self._index_data[column].extend(rows, ids, device=self._device))
+            if self._live is None:
+                return
+            # deleted rows leave every handle (IndexData.compact: no retraining).  The host rows stay, so row ids do
+            # not change: unlike a Lance compaction, which renumbers row addresses unless stable row ids are on.
+            for column in list(self._index):
+                data = self._index_data[column]
+                keep = self._live[data.row_ids.astype(np.int64)]
+                if not keep.all():
+                    self._attach_index(column, data.compact(keep))
+            for cache in (self._flat, self._binary, self._multivec):    # reopened over the live rows
+                for h in cache.values():
+                    h.close()
+                cache.clear()
 
     def prewarm_index(self, name: str):           # rust/lancedb/src/table.rs:3283-3286
         return None                                # indexes are pinned in HBM at create/open time
@@ -362,6 +481,8 @@ class Table:
         allow, allow_bits = None, 0
         if allow_mask is not None:                 # prefilter: row-id allow-list as the C ABI's bitmap
             allow, allow_bits = _native.mask_bitmap(allow_mask), int(len(allow_mask))
+        # deleted rows make every request prefiltered (the handles filter them out): maximum_nprobes applies
+        widen = max_nprobes if (allow is not None or self._live is not None) else 0
         if self._is_binary(column):                # rust/lancedb/src/table/query.rs:229-236 (is_binary)
             if distance_type is not None and distance_type != "hamming":
                 raise ValueError(f"distance type {distance_type!r} is not supported on binary column {column!r}: "
@@ -370,13 +491,12 @@ class Table:
             idx = self._index.get(column) if use_index else None
             if idx is not None:                    # IVF_FLAT (hamming); bypass_vector_index() searches flat below
                 kw = dict(k=k, nprobes=nprobes, refine_factor=refine_factor or 0, lower=lower, upper=upper, allow=allow,
-                          allow_bits=allow_bits, max_nprobes=max_nprobes if allow is not None else 0,
-                          timeout_ms=timeout_ms)
+                          allow_bits=allow_bits, max_nprobes=widen, timeout_ms=timeout_ms)
                 tail = None if fast_search else self._tail.get(column)
                 return idx.search(q, **kw) if tail is None else idx.search_unindexed(tail, q, **kw)
             bx = self._binary.get(column)
             if bx is None:
-                bx = self._binary[column] = _native.GpuBinary(self._binary_vectors(column), device=self._device)
+                bx = self._binary[column] = self._open_cache(_native.GpuBinary, self._binary_vectors(column))
             return bx.search(q, k=k, lower=lower, upper=upper, allow=allow, allow_bits=allow_bits, timeout_ms=timeout_ms)
         if self._is_multivec(column):              # rust/lancedb/src/table/query.rs:180-199: ONE query of nq vectors
             if distance_type is not None and distance_type != "cosine":
@@ -385,7 +505,12 @@ class Table:
             mv = self._multivec.get(column)
             if mv is None:
                 vals, off = self._multivec_rows(column)
-                mv = self._multivec[column] = _native.GpuMultivec(vals, off, device=self._device)
+                rid = self._live_positions()
+                if rid is not None:                # the live rows' vectors, with their positions as row ids
+                    lens = np.diff(off.astype(np.int64))[rid.astype(np.int64)]
+                    vals = vals[np.repeat(self._live, np.diff(off.astype(np.int64)))]
+                    off = _native.multivec_offsets(lens)
+                mv = self._multivec[column] = _native.GpuMultivec(vals, off, row_ids=rid, device=self._device)
             return mv.search([np.asarray(queries, np.float32)], k=k, lower=lower, upper=upper, allow=allow,
                              allow_bits=allow_bits, timeout_ms=timeout_ms)
         if distance_type == "hamming":
@@ -397,18 +522,25 @@ class Table:
                 # the reference documents this as invalid results; be explicit instead
                 raise ValueError(f"distance_type {distance_type!r} does not match the index's {idx.metric!r}")
             kw = dict(k=k, nprobes=nprobes, refine_factor=refine_factor or 0, lower=lower, upper=upper, allow=allow,
-                      allow_bits=allow_bits, max_nprobes=max_nprobes if allow is not None else 0, timeout_ms=timeout_ms,
-                      ef=ef)
+                      allow_bits=allow_bits, max_nprobes=widen, timeout_ms=timeout_ms, ef=ef)
             tail = None if fast_search else self._tail.get(column)   # rows added since the index was built
             return idx.search(queries, **kw) if tail is None else idx.search_unindexed(tail, queries, **kw)
         fl = self._flat.get(column)
         if fl is None:
-            fl = self._flat[column] = _native.GpuFlat(self._vectors(column), device=self._device)
+            fl = self._flat[column] = self._open_cache(_native.GpuFlat, self._vectors(column))
         metric = distance_type or "l2"
         if metric not in ("l2", "cosine", "dot"):
             raise ValueError(f"unsupported distance type {metric!r}")
         return fl.search(queries, k=k, metric=metric, lower=lower, upper=upper, allow=allow, allow_bits=allow_bits,
                          timeout_ms=timeout_ms)
+
+    def _open_cache(self, cls, x: np.ndarray):
+        """A full-column cache (GpuFlat / GpuBinary) over the column's rows x: every row (ids = positions), or the live
+        rows with their positions as ids."""
+        rid = self._live_positions()
+        if rid is None:
+            return cls(x, device=self._device)
+        return cls(np.ascontiguousarray(x[rid.astype(np.int64)]), row_ids=rid, device=self._device)
 
     def _take(self, row_ids: np.ndarray, columns: Optional[List[str]]) -> pa.Table:
         t = self._data if columns is None else self._data.select(columns)
