@@ -389,6 +389,25 @@ int  lgpu_flat_search_device(lgpu_flat *fl, int metric, const float *d_queries, 
  * Storage grows geometrically; the derived data (bf16 copy, |x|^2, norms) is computed for the new rows only. */
 int  lgpu_flat_append(lgpu_flat *fl, const float *rows, uint64_t n, const uint64_t *row_ids);
 
+/* ---- float16 columns (fixed_size_list<float16, dim>) kept as float16 in HBM: 2 bytes per element instead of the 6 an
+ * f32 handle holds (f32 rows + their bf16 tensor-core copy).  Queries stay f32.  _distance is the f32 distance of the
+ * query and the row's exact f32 upcast, so an fp16 handle opened on rows x16 returns exactly -- same ids, counts and
+ * distance bits -- what lgpu_flat_open on x16 converted to f32 returns, on every entry point (host, _filtered,
+ * _device, and as the tail of lgpu_search_unindexed[_device]), for every metric, k, distance_range, prefilter,
+ * deleted rows, appends and sub-batch split.  The paths are chosen as for f32 rows; the l2 tensor-core path multiplies
+ * fp16(q) by the stored rows themselves (fp16 wgmma, f32 accumulation) and re-scores its shortlist exactly, and a query
+ * with a component beyond fp16's range (|q_i| >= 65520) is served by the exact kernels.
+ * vectors / rows: IEEE binary16 bits, [nrows][dim] / [n][dim].  lgpu_flat_append on an fp16 handle, or
+ * lgpu_flat_append_f16 on an f32 handle, fails with LGPU_INVALID_INPUT and changes nothing; every other lgpu_flat_*
+ * function takes both row types. */
+int  lgpu_flat_open_f16(const uint16_t *vectors, uint64_t nrows, uint32_t dim,
+                        const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device, lgpu_flat **out);
+int  lgpu_flat_append_f16(lgpu_flat *fl, const uint16_t *rows, uint64_t n, const uint64_t *row_ids);
+/* *bytes = the device memory the handle holds for its rows and their per-row data (rows, tensor-core operand, |x|^2,
+ * row norms once a cosine search computed them, row ids, the live bitmap), capacity kept for appends included; the
+ * per-call search workspaces (each within LGPU_WS_BYTES) are not counted.  Both row types. */
+int  lgpu_flat_device_bytes(const lgpu_flat *fl, uint64_t *bytes);
+
 /* ---- rows added after an index was built (the reference's unindexed fragments, searched unless fast_search is set;
  * rust/lancedb/src/table/query.rs:289-290).  `tail` holds them.  The result is the top-k by (_distance, _rowid) of
  * the union of

@@ -48,6 +48,7 @@ EXPORTS = [
     "lgpu_flat_append", "lgpu_binary_append", "lgpu_search_unindexed", "lgpu_search_unindexed_device",
     "lgpu_ivf_binary_search_unindexed", "lgpu_ivf_binary_search_unindexed_device",
     "lgpu_index_delete", "lgpu_ivf_binary_delete", "lgpu_flat_delete", "lgpu_binary_delete", "lgpu_multivec_delete",
+    "lgpu_flat_open_f16", "lgpu_flat_append_f16", "lgpu_flat_device_bytes",
 ]
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
@@ -173,6 +174,8 @@ def load():
     lib.lgpu_search_sharded_device.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_comm_last_stage_ms.argtypes = [vp, vp]
     lib.lgpu_flat_open.argtypes = [vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
+    lib.lgpu_flat_open_f16.argtypes = [vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
+    lib.lgpu_flat_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.lgpu_flat_close.argtypes = [vp]
     lib.lgpu_flat_close.restype = None
     lib.lgpu_ivf_assign.argtypes = [vp, u32, u32, i32, vp, C.c_uint64, i32, vp]
@@ -220,6 +223,7 @@ def load():
     lib.lgpu_ivf_binary_search_device.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_debug_ivf_hamming_scan.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_flat_append.argtypes = [vp, vp, C.c_uint64, vp]
+    lib.lgpu_flat_append_f16.argtypes = [vp, vp, C.c_uint64, vp]
     lib.lgpu_binary_append.argtypes = [vp, vp, C.c_uint64, vp]
     for fn in ("lgpu_search_unindexed", "lgpu_ivf_binary_search_unindexed"):
         getattr(lib, fn).argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
@@ -529,18 +533,29 @@ class GpuIvfRq(GpuIvfPq):
 
 
 class GpuFlat(_RowsHandle):
-    """A raw vector column pinned in HBM (lgpu_flat)."""
+    """A raw vector column pinned in HBM (lgpu_flat).  A float16 array opens an fp16 handle (lgpu_flat_open_f16: the
+    rows stay float16 on the device, results are those of their exact f32 upcast); anything else is converted to f32.
+    `dtype` is the handle's row type."""
     _close = "lgpu_flat_close"
     _delete = "lgpu_flat_delete"
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
-        v = np.ascontiguousarray(vectors, np.float32)
+        self.dtype = np.dtype(np.float16 if getattr(vectors, "dtype", None) == np.float16 else np.float32)
+        v = np.ascontiguousarray(vectors, self.dtype)
         self.nrows, self.dim = v.shape
         rid = None if row_ids is None else np.ascontiguousarray(row_ids, np.uint64)
         h = C.c_void_p()
-        check(load().lgpu_flat_open(_ptr(v), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
+        opener = "lgpu_flat_open_f16" if self.dtype == np.float16 else "lgpu_flat_open"
+        check(getattr(load(), opener)(_ptr(v), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
+
+    @property
+    def device_bytes(self) -> int:
+        """The HBM the handle holds for its rows and per-row data (lgpu_flat_device_bytes)."""
+        n = C.c_uint64(0)
+        check(load().lgpu_flat_device_bytes(self._h, C.byref(n)))
+        return n.value
 
     def search(self, queries, k=10, metric="l2", lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
@@ -561,10 +576,15 @@ class GpuFlat(_RowsHandle):
                                              stream))
 
     def append(self, rows, row_ids=None):
-        """Append rows [n, dim] in place (lgpu_flat_append); row_ids None = the positions that follow."""
-        v = np.ascontiguousarray(rows, np.float32).reshape(-1, self.dim)
+        """Append rows [n, dim] in place (lgpu_flat_append[_f16]); row_ids None = the positions that follow.  An fp16
+        handle takes float16 rows only, and an f32 handle no float16 rows: a row is never rounded to fit the handle."""
+        if (getattr(rows, "dtype", None) == np.float16) != (self.dtype == np.float16):
+            raise ValueError(f"append to a {self.dtype.name} flat handle needs rows of that type, not "
+                             f"{getattr(rows, 'dtype', type(rows).__name__)}")
+        v = np.ascontiguousarray(rows, self.dtype).reshape(-1, self.dim)
         rid = _rows_ids(v, row_ids)
-        check(load().lgpu_flat_append(self._h, _ptr(v), v.shape[0], _ptr(rid)))
+        appender = "lgpu_flat_append_f16" if self.dtype == np.float16 else "lgpu_flat_append"
+        check(getattr(load(), appender)(self._h, _ptr(v), v.shape[0], _ptr(rid)))
         self.nrows += v.shape[0]
 
 

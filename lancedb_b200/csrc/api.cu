@@ -91,12 +91,13 @@ static std::atomic<uint64_t> g_alloc_epoch{0};
 struct DevBuf {
     void *p = nullptr;
     size_t bytes = 0;
-    void ensure(size_t n)
+    // exact: no headroom (per-row storage of a handle, whose growth goes through grow_keep)
+    void ensure(size_t n, bool exact = false)
     {
         if (n <= bytes) return;
         g_alloc_epoch++;
         if (p) { cudaFree(p); p = nullptr; bytes = 0; }
-        size_t want = n + n / 8;
+        size_t want = exact ? n : n + n / 8;
         LGPU_CUDA(cudaMalloc(&p, want));
         bytes = want;
     }
@@ -398,9 +399,11 @@ struct lgpu_flat {
     int device = 0;
     uint64_t nrows = 0;
     uint32_t dim = 0;
+    bool f16 = false;                   // row type: `vectors` holds [nrows][dim] f32, or fp16 (lgpu_flat_open_f16)
     DevBuf vectors, row_ids, ysqrt;
-    DevBuf vec_b, vec_n2;               // bf16 rows + |x|^2 for the tensor-core path
-    float vec_max = 0.f, vec_err = 0.f;     // max |x|, max |bf16(x) - x|
+    // the tensor-core path: bf16 rows (f32 handles; an fp16 handle's rows are their own operand) + |x|^2
+    DevBuf vec_b, vec_n2;
+    float vec_max = 0.f, vec_err = 0.f;     // max |x|, max |h(x) - x| (h: bf16 or fp16 rounding, gemm.cu)
     int num_sms = 0;
     bool has_tc = false;
     bool has_ids = false, has_norms = false;
@@ -604,15 +607,17 @@ static bool tc_enabled()
 }
 
 // bf16 copy + squared norms + max norm and max bf16 rounding error |bf16(x) - x| of a row-major f32 matrix (open time).
+// Fp16 rows (f16) are their own operand: no copy (Xb unused), and the error is |h(x) - x| of the fp16 MMA's operand.
 // Returns false when a row holds a NaN or inf, or its |x|^2 or rounding error overflows: the error band (tc_band) is
 // then not finite for any query, and the caller leaves the operand to the exact kernels.
 // The rows' part: Xb and n2 point at room for n rows (an append prepares its new rows only).
-static bool tc_operand_rows(const float *X, uint64_t n, uint32_t d, void *Xb, float *n2, float &xmax, float &xerr,
-                            cudaStream_t st)
+static bool tc_operand_rows(const void *X, bool f16, uint64_t n, uint32_t d, void *Xb, float *n2, float &xmax,
+                            float &xerr, cudaStream_t st)
 {
     DevBuf err;
     err.ensure(std::max<size_t>((size_t)n * 4, 16));
-    launch_to_bf16(X, n, d, Xb, n2, st, err.as<float>());
+    if (f16) launch_f16_row_terms(X, n, d, n2, err.as<float>(), st);
+    else launch_to_bf16(static_cast<const float *>(X), n, d, Xb, n2, st, err.as<float>());
     std::vector<float> h(n), he(n);
     LGPU_CUDA(cudaMemcpyAsync(h.data(), n2, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     LGPU_CUDA(cudaMemcpyAsync(he.data(), err.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
@@ -625,12 +630,17 @@ static bool tc_operand_rows(const float *X, uint64_t n, uint32_t d, void *Xb, fl
     xerr = me;
     return finite && std::isfinite(xmax);
 }
+static bool prepare_tc_operand(const void *X, bool f16, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax,
+                               float &xerr, cudaStream_t st)
+{
+    if (!f16) Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
+    n2.ensure(std::max<size_t>((size_t)n * 4, 16), f16);
+    return tc_operand_rows(X, f16, n, d, Xb.p, n2.as<float>(), xmax, xerr, st);
+}
 static bool prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
                                cudaStream_t st)
 {
-    Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
-    n2.ensure(std::max<size_t>((size_t)n * 4, 16));
-    return tc_operand_rows(X, n, d, Xb.p, n2.as<float>(), xmax, xerr, st);
+    return prepare_tc_operand(X, false, n, d, Xb, n2, xmax, xerr, st);
 }
 
 // where a top-k goes: [B][k] ids and distances, [B] counts and, optionally, [B][k] storage positions
@@ -688,8 +698,10 @@ static size_t large_k_query_bytes(uint32_t k)
 
 // The tail of tc_topk_l2 and tc_topk_l2_filtered: exact re-score of the [B][cap] candidate slots (ws->t_pos, t_ids;
 // one pair per slot, empty slots included; every candidate passed the row filter), their top-k into the outputs, then
-// the dense fix-up of the queries flagged in ws->flags under the row filter (no-ops when none is).
-static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, const float *X, uint64_t N,
+// the dense fix-up of the queries flagged in ws->flags under the row filter (no-ops when none is).  T: the stored row
+// type (float, or __half for an fp16 flat handle, whose rows X are also the GEMM operand Xb).
+template <class T>
+static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, const T *X, uint64_t N,
                              uint32_t d, const uint64_t *col_ids, uint32_t k, uint32_t cap, TopkOut out, float *Dbuf,
                              uint64_t ld, RowFilter rf)
 {
@@ -707,17 +719,26 @@ static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uin
 // ascending by (distance, id).  Dbuf: [B][ld] f32 scratch.  The shortlist holds the kp best allowed rows by approximate
 // score; queries whose shortlist cannot be proven complete (band_check: it is full and its last score is within the
 // band of the k-th) are redone by the exact kernels in the same stream, without a host round trip.
-static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
+// the 16-bit query operand of the tensor-core paths (bf16, or fp16 for fp16 rows), |q|^2 and |h(q) - q|
+template <class T> static void tc_queries(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, uint32_t d)
+{
+    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
+    if (std::is_same<T, __half>::value) launch_to_f16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), ws->qerr.as<float>(), st);
+    else launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
+}
+
+template <class T>
+static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const T *X,
                        const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
                        const uint64_t *col_ids, uint32_t k, uint32_t kp, TopkOut out, float *Dbuf, uint64_t ld,
                        RowFilter rf)
 {
-    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
+    constexpr bool f16 = std::is_same<T, __half>::value;
     ws->flags.ensure((size_t)B * 4);
     ws->t_ids.ensure((size_t)B * kp * 8); ws->t_dist.ensure((size_t)B * kp * 4);
     ws->t_pos.ensure((size_t)B * kp * 8); ws->t_cnt.ensure((size_t)B * 4); ws->t_exact.ensure((size_t)B * kp * 4);
-    launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
-    launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, Dbuf, ld, num_sms, st);
+    tc_queries<T>(ws, st, Q, B, d);
+    launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, Dbuf, ld, num_sms, st, nullptr, f16);
     SelectArgs sa = select_rows(Dbuf, N, ld, B, kp, {ws->t_ids.as<uint64_t>(), ws->t_dist.as<float>(),
                                                      ws->t_cnt.as<uint32_t>(), ws->t_pos.as<uint64_t>()});
     sa.col_ids = col_ids;
@@ -734,23 +755,24 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
 // with fewer, +inf); the pass over all rows then runs with the filtering epilogue (no dense score matrix), admitting
 // the rows under the threshold that pass rf, the few admitted rows are re-scored exactly, and queries whose candidate
 // list overflowed are redone by the exact kernels.
-static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const float *X,
+template <class T>
+static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const T *X,
                                 const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
                                 const uint64_t *col_ids, uint32_t k, TopkOut out, float *Dbuf, uint64_t ld,
                                 RowFilter rf, uint64_t min_sample = 65536, uint32_t cap = 1024)
 {
+    constexpr bool f16 = std::is_same<T, __half>::value;
     const uint64_t Ns = std::min<uint64_t>(N, std::max<uint64_t>(min_sample, N / 8));
     const uint64_t lds = (Ns + 3) & ~3ull;               // Dbuf is [B][ld >= lds]
-    ws->qb.ensure((size_t)B * d * 2); ws->qn2.ensure((size_t)B * 4); ws->qerr.ensure((size_t)B * 4);
     ws->flags.ensure((size_t)B * 4);
     ws->t_ids.ensure((size_t)B * cap * 8); ws->t_dist.ensure((size_t)B * std::max<uint32_t>(k, 32) * 4);
     ws->t_pos.ensure((size_t)B * cap * 8); ws->t_cnt.ensure((size_t)B * 4); ws->t_exact.ensure((size_t)B * cap * 4);
     ws->probe_A.ensure((size_t)B * 4);                   // thr[q]
     ws->amax.ensure((size_t)B * 4);                      // candidate counters
     ws->sbound.ensure((size_t)B * std::max<uint32_t>(k, 32) * 8);   // sample ids (unused)
-    launch_to_bf16(Q, B, d, ws->qb.p, ws->qn2.as<float>(), st, ws->qerr.as<float>());
+    tc_queries<T>(ws, st, Q, B, d);
     // 1. sample pass: dense scores of the first Ns rows, k-th best per query -> threshold
-    launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, Ns, d, Dbuf, lds, num_sms, st);
+    launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, Ns, d, Dbuf, lds, num_sms, st, nullptr, f16);
     SelectArgs ss = select_rows(Dbuf, Ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
                                                       ws->t_cnt.as<uint32_t>()});
     if (rf.bits) { ss.col_ids = col_ids; ss.allow = rf.bits; ss.allow_bits = rf.nbits; }
@@ -766,7 +788,7 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap;
     flt.allow = rf.bits; flt.allow_bits = rf.nbits;
     if (Ns == N) launch_filter_dense(Dbuf, lds, B, N, flt, st);      // the sample pass already scored every row
-    else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt);
+    else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt, f16);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, ws->probe_A.as<float>(), B, ws->flags.as<uint32_t>(), st);
     // 3. exact re-score of the admitted rows, final top-k; 4. fix-up of overflowed queries
     tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out, Dbuf, ld, rf);
@@ -1558,17 +1580,19 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const voi
     }
 }
 
-void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *d_q, uint32_t B,
-                        const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
-                        RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
+// X: the handle's rows, as stored (T = float, or __half for an fp16 handle); every path reads them as they are
+template <class T>
+static void flat_search_rows(lgpu_flat *fl, const T *X, Workspace *ws, cudaStream_t st, int metric, const float *d_q,
+                             uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
+                             RowFilter rf, const Deadline *deadline)
 {
     const uint64_t N = fl->nrows;
     const uint64_t ld = (N + 3) & ~3ull;
     if (metric == LGPU_COSINE) {
         std::lock_guard<std::mutex> g(fl->mu);
         if (!fl->has_norms) {
-            fl->ysqrt.ensure(std::max<size_t>(N, 1) * 4);
-            launch_row_norms(fl->vectors.as<float>(), N, fl->dim, fl->ysqrt.as<float>(), st);
+            fl->ysqrt.ensure(std::max<size_t>(N, 1) * 4, true);
+            launch_row_norms(X, N, fl->dim, fl->ysqrt.as<float>(), st);
             LGPU_CUDA(cudaStreamSynchronize(st));
             fl->has_norms = true;
         }
@@ -1595,24 +1619,32 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
         // shortlists are sized to SELECT_KMAX)
         if (fl->has_tc && tc_enabled() && metric == LGPU_L2 && !sp.has_lower && !sp.has_upper && b >= 8 && N >= 4096 &&
             sp.k <= SELECT_KMAX) {
+            const void *Xop = fl->f16 ? static_cast<const void *>(X) : fl->vec_b.p;   // the GEMM operand
             if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
-                tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p,
-                                    fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
-                                    fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, out.at(q0, sp.k),
+                tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, X, Xop, fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N,
+                                    fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, out.at(q0, sp.k),
                                     ws->D.as<float>(), ld, rf);
             else
-                tc_topk_l2(ws, st, fl->num_sms, q, b, fl->vectors.as<float>(), fl->vec_b.p, fl->vec_n2.as<float>(),
-                           fl->vec_max, fl->vec_err, N, fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp,
-                           out.at(q0, sp.k), ws->D.as<float>(), ld, rf);
+                tc_topk_l2(ws, st, fl->num_sms, q, b, X, Xop, fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
+                           fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp, out.at(q0, sp.k),
+                           ws->D.as<float>(), ld, rf);
             if (prof) g_filter_stats[1] += (uint64_t)b * N;
             continue;
         }
-        launch_dist_matrix(q, fl->vectors.as<float>(), b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
+        launch_dist_matrix(q, X, b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
                            xn, fl->ysqrt.as<float>(), ws->D.as<float>(), ld, st);
         select_dense(ws, ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
                      out.at(q0, sp.k), st);
     }
     if (prof) g_filter_stats[3] = B;
+}
+
+void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *d_q, uint32_t B,
+                        const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
+                        RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
+{
+    if (fl->f16) flat_search_rows(fl, fl->vectors.as<__half>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    else flat_search_rows(fl, fl->vectors.as<float>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
 }
 
 // ---- binary vectors (Hamming distance) ----
@@ -2167,7 +2199,7 @@ template <class H> static void open_rows(H *h, const uint64_t *row_ids, uint64_t
     LGPU_CUDA(cudaGetDeviceProperties(&prop, h->device));
     h->num_sms = prop.multiProcessorCount;
     if (row_ids && nrows) {
-        h->row_ids.ensure((size_t)nrows * 8);
+        h->row_ids.ensure((size_t)nrows * 8, true);
         LGPU_CUDA(cudaMemcpy(h->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
         h->has_ids = true;
     }
@@ -3051,8 +3083,9 @@ int lgpu_merge_topk_device(int device, uint32_t nlists, uint32_t B, uint32_t k, 
     });
 }
 
-int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uint64_t *row_ids, int device,
-                   lgpu_flat **out)
+// lgpu_flat_open and lgpu_flat_open_f16: rows f32 or fp16 (f16), kept on the device as given
+static int flat_open(const void *vectors, bool f16, uint64_t nrows, uint32_t dim, const uint64_t *row_ids, int device,
+                     lgpu_flat **out)
 {
     lgpu_flat *fl = nullptr;
     int rc = guarded([&] {
@@ -3060,12 +3093,13 @@ int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uin
         LGPU_REQUIRE(nrows == 0 || vectors != nullptr, "null vectors");
         require_device(device);
         fl = new lgpu_flat();
-        fl->device = device; fl->nrows = nrows; fl->dim = dim;
-        fl->vectors.ensure(std::max<size_t>((size_t)nrows * dim * 4, 16));
-        if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, (size_t)nrows * dim * 4, cudaMemcpyHostToDevice));
+        fl->device = device; fl->nrows = nrows; fl->dim = dim; fl->f16 = f16;
+        const size_t es = f16 ? 2 : 4;
+        fl->vectors.ensure(std::max<size_t>((size_t)nrows * dim * es, 16), f16);
+        if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, (size_t)nrows * dim * es, cudaMemcpyHostToDevice));
         if (gemm_shape_supported(dim) && nrows >= 4096) {
             // a non-finite or overflowing row: the exact kernels serve the column
-            fl->has_tc = prepare_tc_operand(fl->vectors.as<float>(), nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
+            fl->has_tc = prepare_tc_operand(fl->vectors.p, f16, nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
                                             fl->vec_err, nullptr);
             if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
         }
@@ -3075,6 +3109,29 @@ int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uin
     });
     if (rc != LGPU_OK && fl) delete fl;
     return rc;
+}
+
+int lgpu_flat_open(const float *vectors, uint64_t nrows, uint32_t dim, const uint64_t *row_ids, int device,
+                   lgpu_flat **out)
+{
+    return flat_open(vectors, false, nrows, dim, row_ids, device, out);
+}
+
+int lgpu_flat_open_f16(const uint16_t *vectors, uint64_t nrows, uint32_t dim, const uint64_t *row_ids, int device,
+                       lgpu_flat **out)
+{
+    return flat_open(vectors, true, nrows, dim, row_ids, device, out);
+}
+
+int lgpu_flat_device_bytes(const lgpu_flat *flh, uint64_t *bytes)
+{
+    return guarded([&] {
+        HandleRef<lgpu_flat> h(const_cast<lgpu_flat *>(flh));
+        LGPU_REQUIRE(bytes != nullptr, "null argument");
+        const lgpu_flat *fl = h.h;
+        *bytes = fl->vectors.bytes + fl->row_ids.bytes + fl->ysqrt.bytes + fl->vec_b.bytes + fl->vec_n2.bytes +
+                 fl->live.bits.bytes;
+    });
 }
 
 void lgpu_flat_close(lgpu_flat *fl) { close_handle(fl); }
@@ -3391,37 +3448,42 @@ template <class H> static int delete_rows(H *hp, const uint64_t *row_ids, uint64
 
 extern "C" {
 
-int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64_t *row_ids)
+// lgpu_flat_append and lgpu_flat_append_f16: the rows must have the handle's row type (f16)
+static int flat_append(lgpu_flat *flh, const void *rows, bool f16, uint64_t n, const uint64_t *row_ids)
 {
     return guarded([&] {
         HandleExcl<lgpu_flat> h(flh);
         lgpu_flat *fl = h.h;
+        LGPU_REQUIRE(fl->f16 == f16, fl->f16 ? "the handle holds fp16 rows: append them with lgpu_flat_append_f16"
+                                             : "the handle holds f32 rows: append them with lgpu_flat_append");
         LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
         if (n == 0) return;
         const uint64_t bound = live_bound_after(fl, n, row_ids);
         begin_append(fl->device);
         const uint64_t n0 = fl->nrows, n1 = n0 + n;
         const uint32_t d = fl->dim;
-        grow_keep(fl->vectors, (size_t)n0 * d * 4, (size_t)n1 * d * 4);
-        float *x = fl->vectors.as<float>() + (size_t)n0 * d;
-        LGPU_CUDA(cudaMemcpy(x, rows, (size_t)n * d * 4, cudaMemcpyHostToDevice));
+        const size_t es = f16 ? 2 : 4;
+        grow_keep(fl->vectors, (size_t)n0 * d * es, (size_t)n1 * d * es);
+        char *x = fl->vectors.as<char>() + (size_t)n0 * d * es;
+        LGPU_CUDA(cudaMemcpy(x, rows, (size_t)n * d * es, cudaMemcpyHostToDevice));
         append_ids(fl, n0, n, row_ids);
         grow_live(fl, n0, n, bound);
         if (fl->has_norms) {
             grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
-            launch_row_norms(x, n, d, fl->ysqrt.as<float>() + n0, nullptr);
+            if (f16) launch_row_norms(reinterpret_cast<const __half *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
+            else launch_row_norms(reinterpret_cast<const float *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
         }
         // the tensor-core operand, as lgpu_flat_open builds it for n1 rows: the whole column when it first reaches 4096
         // rows, else the new rows only, the band constants the max over both parts
         if (gemm_shape_supported(d) && n1 >= 4096) {
             if (n0 < 4096) {
-                fl->has_tc = prepare_tc_operand(fl->vectors.as<float>(), n1, d, fl->vec_b, fl->vec_n2, fl->vec_max,
+                fl->has_tc = prepare_tc_operand(fl->vectors.p, f16, n1, d, fl->vec_b, fl->vec_n2, fl->vec_max,
                                                 fl->vec_err, nullptr);
             } else if (fl->has_tc) {
-                grow_keep(fl->vec_b, (size_t)n0 * d * 2, (size_t)n1 * d * 2);
+                if (!f16) grow_keep(fl->vec_b, (size_t)n0 * d * 2, (size_t)n1 * d * 2);
                 grow_keep(fl->vec_n2, (size_t)n0 * 4, (size_t)n1 * 4);
                 float xmax = 0.f, xerr = 0.f;
-                fl->has_tc = tc_operand_rows(x, n, d, fl->vec_b.as<char>() + (size_t)n0 * d * 2,
+                fl->has_tc = tc_operand_rows(x, f16, n, d, f16 ? nullptr : fl->vec_b.as<char>() + (size_t)n0 * d * 2,
                                              fl->vec_n2.as<float>() + n0, xmax, xerr, nullptr);
                 fl->vec_max = std::max(fl->vec_max, xmax);
                 fl->vec_err = std::max(fl->vec_err, xerr);
@@ -3431,6 +3493,16 @@ int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64
         LGPU_CUDA(cudaDeviceSynchronize());
         fl->nrows = n1;
     });
+}
+
+int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64_t *row_ids)
+{
+    return flat_append(flh, rows, false, n, row_ids);
+}
+
+int lgpu_flat_append_f16(lgpu_flat *flh, const uint16_t *rows, uint64_t n, const uint64_t *row_ids)
+{
+    return flat_append(flh, rows, true, n, row_ids);
 }
 
 int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const uint64_t *row_ids)

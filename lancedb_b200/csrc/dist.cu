@@ -10,6 +10,7 @@
 // `launch_pair_distance` is the exact re-rank used by refine_factor (row a10).
 #include "kernels.cuh"
 
+#include <cuda_fp16.h>
 #include <math_constants.h>
 
 #include <algorithm>
@@ -20,8 +21,14 @@ namespace {
 
 constexpr int DM_Q = 16, DM_C = 32, DM_KT = 32, DM_STR = 36, DM_THREADS = 256;
 
+// A stored row element as f32: an fp16 row converts exactly in registers, so every kernel below runs the same f32
+// arithmetic, in the same lane order, on either row type (the stored-row type T is float or __half)
+__device__ __forceinline__ float ldf(float v) { return v; }
+__device__ __forceinline__ float ldf(__half v) { return __half2float(v); }
+
+template <class T>
 __global__ void __launch_bounds__(DM_THREADS) dist_matrix_kernel(
-    const float *__restrict__ Q, const float *__restrict__ C, uint32_t B, uint64_t N, uint32_t d, int mode,
+    const float *__restrict__ Q, const T *__restrict__ C, uint32_t B, uint64_t N, uint32_t d, int mode,
     const float *__restrict__ xnorm, const float *__restrict__ ysqrt, float *__restrict__ D, uint64_t ldD,
     const uint32_t *__restrict__ only, const uint32_t *__restrict__ gate)
 {
@@ -66,7 +73,7 @@ __global__ void __launch_bounds__(DM_THREADS) dist_matrix_kernel(
         for (int u = 0; u < 4; u++) {
             int idx = tid + DM_THREADS * u, row = idx >> 5, col = idx & 31;
             uint64_t gc = c0 + row; uint32_t gk = k0 + col;
-            cs[row][col] = (gc < N && gk < d16) ? C[(size_t)gc * d + gk] : 0.f;
+            cs[row][col] = (gc < N && gk < d16) ? ldf(C[(size_t)gc * d + gk]) : 0.f;
         }
         __syncthreads();
 #pragma unroll
@@ -109,10 +116,11 @@ __global__ void __launch_bounds__(DM_THREADS) dist_matrix_kernel(
 #pragma unroll
         for (int l = 0; l < 16; l++) t = __fadd_rn(t, red[pair][l]);
         float s = 0.f;                                   // remainder dims, sequential
-        const float *x = Q + (size_t)gq * d, *y = C + (size_t)gc * d;
+        const float *x = Q + (size_t)gq * d;
+        const T *y = C + (size_t)gc * d;
         for (uint32_t i = d16; i < d; i++) {
-            if (mode == 0) { float df = __fsub_rn(x[i], y[i]); s = __fadd_rn(s, __fmul_rn(df, df)); }
-            else s = __fadd_rn(s, __fmul_rn(x[i], y[i]));
+            if (mode == 0) { float df = __fsub_rn(x[i], ldf(y[i])); s = __fadd_rn(s, __fmul_rn(df, df)); }
+            else s = __fadd_rn(s, __fmul_rn(x[i], ldf(y[i])));
         }
         float v = __fadd_rn(s, t);
         if (mode == 1) v = __fsub_rn(1.0f, v);
@@ -123,20 +131,22 @@ __global__ void __launch_bounds__(DM_THREADS) dist_matrix_kernel(
 }
 
 // half-warp per row: lane l (< 16) is lance's accumulator lane l
-__device__ __forceinline__ float halfwarp_dot(const float *__restrict__ x, const float *__restrict__ y,
+template <class TX, class TY>
+__device__ __forceinline__ float halfwarp_dot(const TX *__restrict__ x, const TY *__restrict__ y,
                                                uint32_t d, int hl, unsigned hmask, int hbase)
 {
     const uint32_t d16 = d & ~15u;
     float a = 0.f;
-    for (uint32_t k = hl; k < d16; k += 16) a = __fadd_rn(a, __fmul_rn(x[k], y[k]));
+    for (uint32_t k = hl; k < d16; k += 16) a = __fadd_rn(a, __fmul_rn(ldf(x[k]), ldf(y[k])));
     float t = 0.f;
 #pragma unroll
     for (int l = 0; l < 16; l++) t = __fadd_rn(t, __shfl_sync(hmask, a, hbase + l));
     float s = 0.f;
-    for (uint32_t i = d16; i < d; i++) s = __fadd_rn(s, __fmul_rn(x[i], y[i]));
+    for (uint32_t i = d16; i < d; i++) s = __fadd_rn(s, __fmul_rn(ldf(x[i]), ldf(y[i])));
     return __fadd_rn(s, t);
 }
-__device__ __forceinline__ float halfwarp_l2(const float *__restrict__ x, const float *__restrict__ y,
+template <class TY>
+__device__ __forceinline__ float halfwarp_l2(const float *__restrict__ x, const TY *__restrict__ y,
                                               uint32_t d, int hl, unsigned hmask, int hbase)
 {
     const uint32_t d16 = d & ~15u;
@@ -145,16 +155,16 @@ __device__ __forceinline__ float halfwarp_l2(const float *__restrict__ x, const 
     for (; k + 7 * 16 < d16; k += 8 * 16) {             // eight independent loads of each operand in flight
         float xv[8], yv[8];
 #pragma unroll
-        for (int u = 0; u < 8; u++) { xv[u] = x[k + 16 * u]; yv[u] = y[k + 16 * u]; }
+        for (int u = 0; u < 8; u++) { xv[u] = x[k + 16 * u]; yv[u] = ldf(y[k + 16 * u]); }
 #pragma unroll
         for (int u = 0; u < 8; u++) { const float df = __fsub_rn(xv[u], yv[u]); a = __fadd_rn(a, __fmul_rn(df, df)); }
     }
-    for (; k < d16; k += 16) { float df = __fsub_rn(x[k], y[k]); a = __fadd_rn(a, __fmul_rn(df, df)); }
+    for (; k < d16; k += 16) { float df = __fsub_rn(x[k], ldf(y[k])); a = __fadd_rn(a, __fmul_rn(df, df)); }
     float t = 0.f;
 #pragma unroll
     for (int l = 0; l < 16; l++) t = __fadd_rn(t, __shfl_sync(hmask, a, hbase + l));
     float s = 0.f;
-    for (uint32_t i = d16; i < d; i++) { float df = __fsub_rn(x[i], y[i]); s = __fadd_rn(s, __fmul_rn(df, df)); }
+    for (uint32_t i = d16; i < d; i++) { float df = __fsub_rn(x[i], ldf(y[i])); s = __fadd_rn(s, __fmul_rn(df, df)); }
     return __fadd_rn(s, t);
 }
 
@@ -183,13 +193,14 @@ __device__ __forceinline__ float halfwarp_l2_sx(const float *sx, const float *__
     return __fadd_rn(s, t);
 }
 
-__global__ void row_norms_kernel(const float *__restrict__ X, uint64_t n, uint32_t d, float *__restrict__ out)
+template <class T>
+__global__ void row_norms_kernel(const T *__restrict__ X, uint64_t n, uint32_t d, float *__restrict__ out)
 {
     const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 4;
     const int lane = threadIdx.x & 31, hl = lane & 15, hbase = lane & 16;
     const unsigned hmask = 0xffffu << hbase;
     if (row >= n) return;                               // whole half-warp exits together
-    const float *x = X + row * d;
+    const T *x = X + row * d;
     float v = sqrtf(halfwarp_dot(x, x, d, hl, hmask, hbase));
     if (hl == 0) out[row] = v;
 }
@@ -206,7 +217,8 @@ __global__ void normalize_kernel(const float *__restrict__ X, uint32_t B, uint32
     for (uint32_t k = hl; k < d; k += 16) out[(size_t)row * d + k] = __fdiv_rn(x[k], nrm);
 }
 
-__global__ void pair_distance_kernel(const float *__restrict__ Q, const float *__restrict__ V,
+template <class T>
+__global__ void pair_distance_kernel(const float *__restrict__ Q, const T *__restrict__ V,
                                      const uint64_t *__restrict__ pos, uint32_t B, uint32_t nc, uint32_t d,
                                      int metric, float *__restrict__ out)
 {
@@ -218,7 +230,8 @@ __global__ void pair_distance_kernel(const float *__restrict__ Q, const float *_
     const uint32_t q = (uint32_t)(pair / nc);
     const uint64_t ps = pos[pair];
     if (ps == UINT64_MAX) { if (hl == 0) out[pair] = CUDART_INF_F; return; }
-    const float *x = Q + (size_t)q * d, *y = V + ps * d;
+    const float *x = Q + (size_t)q * d;
+    const T *y = V + ps * d;
     float v;
     if (metric == LGPU_L2) v = halfwarp_l2(x, y, d, hl, hmask, hbase);
     else if (metric == LGPU_DOT) v = __fsub_rn(1.0f, halfwarp_dot(x, y, d, hl, hmask, hbase));
@@ -471,7 +484,8 @@ void launch_coarse_finish(const float *S, uint64_t ld, uint32_t B, uint32_t N, c
     LGPU_CUDA(cudaGetLastError());
 }
 
-void launch_dist_matrix(const float *Q, const float *C, uint32_t B, uint64_t N, uint32_t d, int mode,
+template <class T>
+void launch_dist_matrix(const float *Q, const T *C, uint32_t B, uint64_t N, uint32_t d, int mode,
                         const float *xnorm, const float *ysqrt, float *D, uint64_t ldD, cudaStream_t st,
                         const uint32_t *only, const uint32_t *gate)
 {
@@ -479,15 +493,16 @@ void launch_dist_matrix(const float *Q, const float *C, uint32_t B, uint64_t N, 
     // the fix-up pass (`only`) is almost always a no-op: keep its CTA count small
     const uint64_t ct = (N + DM_C - 1) / DM_C;
     dim3 grid((unsigned)std::min<uint64_t>(ct, only ? 16 : ((uint64_t)1 << 30)), (B + DM_Q - 1) / DM_Q);
-    launch_k(dist_matrix_kernel, grid, dim3(DM_THREADS), 0, st, Q, C, B, N, d, mode, xnorm, ysqrt, D, ldD, only, gate); LGPU_COUNT_LAUNCH();
+    launch_k(dist_matrix_kernel<T>, grid, dim3(DM_THREADS), 0, st, Q, C, B, N, d, mode, xnorm, ysqrt, D, ldD, only, gate); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
-void launch_row_norms(const float *X, uint64_t n, uint32_t d, float *out, cudaStream_t st)
+template <class T>
+void launch_row_norms(const T *X, uint64_t n, uint32_t d, float *out, cudaStream_t st)
 {
     if (n == 0) return;
     uint64_t threads = n * 16;
-    row_norms_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(X, n, d, out); LGPU_COUNT_LAUNCH();
+    row_norms_kernel<T><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(X, n, d, out); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
@@ -499,14 +514,26 @@ void launch_normalize(const float *X, uint32_t B, uint32_t d, float *out, cudaSt
     LGPU_CUDA(cudaGetLastError());
 }
 
-void launch_pair_distance(const float *Q, const float *V, const uint64_t *pos, uint32_t B, uint32_t nc,
+template <class T>
+void launch_pair_distance(const float *Q, const T *V, const uint64_t *pos, uint32_t B, uint32_t nc,
                           uint32_t d, int metric, float *out, cudaStream_t st)
 {
     if (B == 0 || nc == 0) return;
     uint64_t threads = (uint64_t)B * nc * 16;
-    launch_k(pair_distance_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, V, pos, B, nc, d, metric, out); LGPU_COUNT_LAUNCH();
+    launch_k(pair_distance_kernel<T>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, V, pos, B, nc, d, metric, out); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
+
+#define LGPU_ROW_TYPE(T)                                                                                                 \
+    template void launch_dist_matrix<T>(const float *, const T *, uint32_t, uint64_t, uint32_t, int, const float *,     \
+                                        const float *, float *, uint64_t, cudaStream_t, const uint32_t *,               \
+                                        const uint32_t *);                                                              \
+    template void launch_row_norms<T>(const T *, uint64_t, uint32_t, float *, cudaStream_t);                            \
+    template void launch_pair_distance<T>(const float *, const T *, const uint64_t *, uint32_t, uint32_t, uint32_t, int, \
+                                          float *, cudaStream_t);
+LGPU_ROW_TYPE(float)
+LGPU_ROW_TYPE(__half)
+#undef LGPU_ROW_TYPE
 
 void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
                        const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,

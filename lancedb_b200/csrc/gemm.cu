@@ -26,6 +26,9 @@
 
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include <type_traits>
 
 namespace lgpu {
 
@@ -190,6 +193,26 @@ struct B1Hamming {
     __device__ static __forceinline__ int qterm(const HamFilter &f, uint32_t q) { return __ldg(f.qpop + q); }
     __device__ static __forceinline__ float score(int xn, int acc, int pq) { return (float)(pq + xn - 2 * acc); }
 };
+// F16Dist: the Bf16Dist score on fp16 operands, the stored rows of an fp16 flat handle read by TMA as they are (no
+// operand copy) and the query rounded to fp16 (launch_to_f16).  Its band is tc_band's, with
+//   r_X = max_x |h(x) - x| (xerr) and r_q = |h(q) - q| (qerr),
+// h(v) the value the MMA consumes for v.  Every product of two fp16 values is exact in f32 (11 + 11 significant bits,
+// exponents within f32's range, subnormal fp16 included), so the derivation above tc_band carries over term by term:
+// S - (|x|^2 - 2 q.x) = -2 (h(q).h(x) - q.x) + (the f32 sums), h(q).h(x) - q.x = h(q).(h(x) - x) + (h(q) - q).x.
+// A stored row IS fp16, so h(x) = x and r_X = 0 provided the MMA consumes fp16 subnormals as they are; Hopper's does
+// (tests/test_gpu_flat_f16.py measures it through the same instruction), and r_X is still computed at open and append
+// by the same conversion the query takes, so the band stays right if h ever differs from the identity.  The query term
+// shrinks from bf16's 2^-8 |q| to fp16's 2^-11 |q| (normal range) plus 2^-25 per subnormal component.  A query
+// component beyond fp16's range (|q_i| >= 65520) converts to inf: r_q and E_q are then inf and the query goes to the
+// exact kernels, as every query with a non-finite band does.
+struct F16Dist {
+    static constexpr bool BIN = false, MAXSIM = false;
+    static constexpr int K_BOX = GK;
+    using Acc = float; using Row = float; using Row2 = float2; using Filter = GemmFilter;
+    __device__ static __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k16_f16(d, a, b, acc); }
+    __device__ static __forceinline__ int qterm(const GemmFilter &, uint32_t) { return 0; }
+    __device__ static __forceinline__ float score(float xn, float acc, int) { return xn - 2.0f * acc; }
+};
 // F16MaxSim: fp16 copies of the NORMALISED query and stored vectors of a multivector column, acc = the approximate
 // cosine similarity.  Its epilogue writes nothing dense: per (query vector, document) it keeps the largest similarity
 // over the document's run of columns (MaxSimOut, kernels.cuh), one atomicMax per run of a thread's columns.
@@ -206,7 +229,7 @@ struct F16MaxSim {
 // instantiation so that the dense / sparse-filter kernel of the flat path and of the small coarse problems carries
 // none of its code.  ROWF: the filtering epilogues admit only columns that pass the filter's row filter (flt.allow);
 // also a separate instantiation, so the kernels of unfiltered calls are the ones they were without it.
-// Pol: Bf16Dist or B1Hamming (above).
+// Pol: Bf16Dist, F16Dist, B1Hamming or F16MaxSim (above).
 template <bool LIST, class Pol, bool ROWF = false>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
@@ -427,17 +450,26 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     }
 }
 
-// X f32 [n][d] -> bf16 [n][d] (round to nearest even), |x|^2 and the rounding error |bf16(x) - x| in f32; one warp
-// per row
-__global__ void to_bf16_norm_kernel(const float *__restrict__ X, uint64_t n, uint32_t d, __nv_bfloat16 *__restrict__ Xb,
+// the 16-bit operand value h(v) the MMA consumes for v (round to nearest even), and back to f32 (exact)
+template <class H> __device__ __forceinline__ H round_to(float v);
+template <> __device__ __forceinline__ __nv_bfloat16 round_to<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half round_to<__half>(float v) { return __float2half_rn(v); }
+__device__ __forceinline__ float widen(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
+
+// X [n][d] (TI: f32, or fp16 rows that are their own operand) -> H [n][d] (bf16 or fp16; written only for f32 X),
+// |x|^2 and the rounding error |h(x) - x| in f32; one warp per row
+template <class TI, class H>
+__global__ void to_half_norm_kernel(const TI *__restrict__ X, uint64_t n, uint32_t d, H *__restrict__ Xb,
                                     float *__restrict__ norm2, float *__restrict__ err)
 {
+    constexpr bool COPY = std::is_same<TI, float>::value;
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (row >= n) return;
-    const float *x = X + row * d;
-    __nv_bfloat16 *xb = Xb + row * d;
+    const TI *x = X + row * d;
+    H *xb = Xb + row * d;
     float s = 0.f, se = 0.f;
     // U loads of the lane in flight at once (a rolled loop waited for one DRAM round trip per element: 13 us for
     // 1024 x 768 on an H100); the sums still run over k = lane, lane + 32, ... in order
@@ -445,14 +477,16 @@ __global__ void to_bf16_norm_kernel(const float *__restrict__ X, uint64_t n, uin
     for (uint32_t k0 = lane; k0 < d; k0 += 32 * U) {
         float v[U];
 #pragma unroll
-        for (uint32_t u = 0; u < U; u++) v[u] = k0 + 32 * u < d ? x[k0 + 32 * u] : 0.f;
+        for (uint32_t u = 0; u < U; u++) v[u] = k0 + 32 * u < d ? (float)x[k0 + 32 * u] : 0.f;
 #pragma unroll
         for (uint32_t u = 0; u < U; u++) {
             if (k0 + 32 * u < d) {
-                const __nv_bfloat16 b = __float2bfloat16_rn(v[u]);
-                xb[k0 + 32 * u] = b;
+                const H b = round_to<H>(v[u]);
+                if constexpr (COPY) xb[k0 + 32 * u] = b;
                 s = fmaf(v[u], v[u], s);
-                const float e = __bfloat162float(b) - v[u];         // exact: b and v are within a factor of 2
+                // exact: b and v are within a factor of 2, or (fp16 subnormal range) both on the grid of v's ulp; inf
+                // when v overflows fp16
+                const float e = widen(b) - v[u];
                 se = fmaf(e, e, se);
             }
         }
@@ -653,7 +687,23 @@ void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *nor
 {
     if (n == 0) return;
     uint64_t threads = n * 32;
-    launch_k(to_bf16_norm_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, X, n, d, reinterpret_cast<__nv_bfloat16 *>(Xb), norm2, err); LGPU_COUNT_LAUNCH();
+    launch_k(to_half_norm_kernel<float, __nv_bfloat16>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, X, n, d, reinterpret_cast<__nv_bfloat16 *>(Xb), norm2, err); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_to_f16(const float *Q, uint32_t B, uint32_t d, void *Qh, float *qn2, float *qerr, cudaStream_t st)
+{
+    if (B == 0) return;
+    uint64_t threads = (uint64_t)B * 32;
+    launch_k(to_half_norm_kernel<float, __half>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, (uint64_t)B, d, reinterpret_cast<__half *>(Qh), qn2, qerr); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_f16_row_terms(const void *X, uint64_t n, uint32_t d, float *norm2, float *err, cudaStream_t st)
+{
+    if (n == 0) return;
+    uint64_t threads = n * 32;
+    launch_k(to_half_norm_kernel<__half, __half>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, reinterpret_cast<const __half *>(X), n, d, static_cast<__half *>(nullptr), norm2, err); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
@@ -685,20 +735,23 @@ void launch_filter_dense(const float *D, uint64_t ld, uint32_t B, uint64_t N, co
 }
 
 void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint32_t B, uint64_t N, uint32_t d,
-                      float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter)
+                      float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter, bool f16)
 {
     if (B == 0 || N == 0) return;
     LGPU_REQUIRE(gemm_shape_supported(d), "tensor-core path needs a dimension that is a multiple of 8");
-    CUtensorMap mq = make_map(Qb, B, d, GM);
-    CUtensorMap mx = make_map(Xb, N, d, GN);
+    CUtensorMap mq = make_map(Qb, B, d, GM, false, f16);
+    CUtensorMap mx = make_map(Xb, N, d, GN, false, f16);
     const uint64_t tiles = (uint64_t)((B + GM - 1) / GM) * ((N + GN - 1) / GN);
     const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)num_sms);
     GemmFilter flt{};
     if (filter) flt = *filter;
     const bool list = flt.thr && flt.cand_s;                  // dense hit rates: one reservation per row and tile
     LGPU_REQUIRE(!(list && flt.allow), "the dense-rate filtering epilogue of float scores takes no row filter");
-    auto kern = list ? gemm_dist_kernel<true, Bf16Dist>
-                     : (flt.thr && flt.allow ? gemm_dist_kernel<false, Bf16Dist, true> : gemm_dist_kernel<false, Bf16Dist>);
+    LGPU_REQUIRE(!(list && f16), "the dense-rate filtering epilogue takes bf16 operands");
+    const bool rowf = flt.thr && flt.allow;
+    auto kern = f16    ? (rowf ? gemm_dist_kernel<false, F16Dist, true> : gemm_dist_kernel<false, F16Dist>)
+                : list ? gemm_dist_kernel<true, Bf16Dist>
+                       : (rowf ? gemm_dist_kernel<false, Bf16Dist, true> : gemm_dist_kernel<false, Bf16Dist>);
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
     launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, xnorm2, out, ld_out, B, N, (uint32_t)((d + GK - 1) / GK), flt); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());

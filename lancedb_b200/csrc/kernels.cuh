@@ -3,6 +3,8 @@
 
 #include "common.cuh"
 
+#include <cuda_fp16.h>
+
 namespace lgpu {
 
 // ---------------- scan (K2+K3) geometry ------------------------------------------
@@ -261,8 +263,11 @@ void launch_group(const GroupArgs &a, cudaStream_t st);
 // ---------------- exact distance matrix (K1 coarse, flat v1) ----------------------
 // D[q][c] for q < B, c < N.  mode 0: L2 (squared), 1: dot distance 1 - x.y,
 // 2: cosine 1 - x.y/|x|/|y| (xnorm[B] = |x|, ysqrt[N] = |y| required).
-// `only` (optional, [B]): rows whose flag is 0 are skipped (used by the tensor-core paths' fix-up pass)
-void launch_dist_matrix(const float *Q, const float *C, uint32_t B, uint64_t N, uint32_t d, int mode,
+// `only` (optional, [B]): rows whose flag is 0 are skipped (used by the tensor-core paths' fix-up pass).
+// The stored rows C (and V, X below) are float or __half: fp16 rows are converted to f32 in registers, so the distances
+// are those of the rows' exact f32 upcast, bit for bit.
+template <class T>
+void launch_dist_matrix(const float *Q, const T *C, uint32_t B, uint64_t N, uint32_t d, int mode,
                         const float *xnorm, const float *ysqrt, float *D, uint64_t ldD, cudaStream_t st,
                         const uint32_t *only = nullptr, const uint32_t *gate = nullptr);
 // coarse step after the tensor-core GEMM, one kernel: from S[B][ld] = |x|^2 - 2 bf16(q).bf16(x) (N columns) to the k
@@ -276,12 +281,14 @@ void launch_coarse_finish(const float *S, uint64_t ld, uint32_t B, uint32_t N, c
 // list mode (list_pos / list_cnt given, N == ld == the list capacity): S[q] holds the list_cnt[q] scores the GEMM's
 // filtering epilogue admitted for query q and list_pos[q] their columns; a list longer than its capacity flags the query
 // row norms |x| = sqrt(dot(x,x)) in lance order; out[n]
-void launch_row_norms(const float *X, uint64_t n, uint32_t d, float *out, cudaStream_t st);
+template <class T>
+void launch_row_norms(const T *X, uint64_t n, uint32_t d, float *out, cudaStream_t st);
 // out[q] = x[q] / |x[q]|
 void launch_normalize(const float *X, uint32_t B, uint32_t d, float *out, cudaStream_t st);
 // exact distances of (query, stored row) pairs: out[q][c] = dist(Q[q], V[pos[q][c]]),
 // pos == UINT64_MAX => +inf
-void launch_pair_distance(const float *Q, const float *V, const uint64_t *pos, uint32_t B, uint32_t nc,
+template <class T>
+void launch_pair_distance(const float *Q, const T *V, const uint64_t *pos, uint32_t B, uint32_t nc,
                           uint32_t d, int metric, float *out, cudaStream_t st);
 
 // ---------------- top-k select (K4) ------------------------------------------------
@@ -364,6 +371,11 @@ void launch_rowmask_and(const uint32_t *a, const uint32_t *b, uint64_t words, ui
 bool gemm_shape_supported(uint32_t d);
 // X f32 [n][d] -> bf16 [n][d]; norm2[n] = |x|^2 (f32) if norm2 != nullptr; err[n] = |bf16(x) - x| if err != nullptr
 void launch_to_bf16(const float *X, uint64_t n, uint32_t d, void *Xb, float *norm2, cudaStream_t st, float *err = nullptr);
+// the operands of the fp16 form (F16Dist): queries Q f32 [B][d] -> Qh fp16 [B][d], qn2[q] = |q|^2 (f32),
+// qerr[q] = |h(q) - q| (inf when a component overflows fp16); stored fp16 rows X [n][d] -> norm2[n] = |x|^2 (f32),
+// err[n] = |h(x) - x| (h: the value the MMA consumes)
+void launch_to_f16(const float *Q, uint32_t B, uint32_t d, void *Qh, float *qn2, float *qerr, cudaStream_t st);
+void launch_f16_row_terms(const void *X, uint64_t n, uint32_t d, float *norm2, float *err, cudaStream_t st);
 // E_q, the error band of the tensor-core scores: |S[q][x] - (|q - x|^2 - |q|^2)| <= E_q for every row x of the operand,
 // S[q][x] = |x|^2 - 2 bf16(q).bf16(x) (f32 accumulation), with r_q = |bf16(q) - q| (qerr), r_X = max_x |bf16(x) - x|
 // (xerr) and xmax >= max_x |x|:
@@ -379,7 +391,8 @@ __device__ __forceinline__ float tc_band(float qnorm2, float qerr, float xmax, f
     const float qn = sqrtf(qnorm2), s = qn + xmax;
     return 2.0f * 1.0009765625f * ((qn + qerr) * xerr + qerr * xmax) + 4.0f * (float)d * 5.9604645e-8f * s * s;
 }
-// out[q][x] = xnorm2[x] - 2 * bf16(Q[q]) . bf16(X[x])   (wgmma + TMA), q < B, x < N
+// out[q][x] = xnorm2[x] - 2 * bf16(Q[q]) . bf16(X[x])   (wgmma + TMA), q < B, x < N; f16: Qb and Xb are fp16
+// (F16Dist, gemm.cu)
 // optional filtering epilogue: instead of writing the dense score matrix, append the columns whose score
 // is <= thr[q] to the query's candidate list (count may exceed cap: those appends are dropped)
 struct GemmFilter {
@@ -402,7 +415,8 @@ __device__ __forceinline__ bool gemm_filter_admits(const GemmFilter &f, uint64_t
     return id < f.allow_bits && ((__ldg(f.allow + (id >> 5)) >> (id & 31)) & 1u);
 }
 void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint32_t B, uint64_t N, uint32_t d,
-                      float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter = nullptr);
+                      float *out, uint64_t ld_out, int num_sms, cudaStream_t st, const GemmFilter *filter = nullptr,
+                      bool f16 = false);
 // the binary (Hamming) form of the same kernel: the GemmFilter fields plus popc(q) of every query
 struct HamFilter : GemmFilter {
     const int *qpop;              // [B]

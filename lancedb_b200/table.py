@@ -340,13 +340,15 @@ class Table:
 
     @staticmethod
     def _rows_of(table: pa.Table, column: str) -> np.ndarray:
-        """The vectors of a float (f32) or binary (u8) column of `table`."""
+        """The vectors of a float or binary (u8) column of `table`, as the flat handles keep them: float16 columns as
+        float16 (GpuFlat keeps them so in HBM, with the results of their exact f32 upcast), other floats as f32."""
         col = table.column(column).combine_chunks()
-        dt = np.uint8 if pa.types.is_uint8(col.type.value_type) else np.float32
+        vt = col.type.value_type
+        dt = np.uint8 if pa.types.is_uint8(vt) else (np.float16 if pa.types.is_float16(vt) else np.float32)
         return np.asarray(col.flatten().to_numpy(zero_copy_only=False), dt).reshape(-1, col.type.list_size)
 
     def _new_rows(self, column: str, start: int) -> np.ndarray:
-        """The vectors of rows start.. of a float (f32) or binary (u8) column."""
+        """The vectors of rows start.. of a float or binary (u8) column (_rows_of)."""
         return self._rows_of(self._data.slice(start), column)
 
     def _drop_tail(self, column: str) -> None:
@@ -432,6 +434,8 @@ class Table:
             for column in list(self._tail):
                 start = self._tail_from[column]
                 rows = self._new_rows(column, start)
+                if rows.dtype == np.float16:      # an index holds the f32 upcast of a float16 column
+                    rows = rows.astype(np.float32)
                 ids = np.arange(start, start + rows.shape[0], dtype=np.uint64)
                 self._attach_index(column, self._index_data[column].extend(rows, ids, device=self._device))
             if self._live is None:
@@ -527,7 +531,7 @@ class Table:
             return idx.search(queries, **kw) if tail is None else idx.search_unindexed(tail, queries, **kw)
         fl = self._flat.get(column)
         if fl is None:
-            fl = self._flat[column] = self._open_cache(_native.GpuFlat, self._vectors(column))
+            fl = self._flat[column] = self._open_cache(_native.GpuFlat, self._rows_of(self._data, column))
         metric = distance_type or "l2"
         if metric not in ("l2", "cosine", "dot"):
             raise ValueError(f"unsupported distance type {metric!r}")
