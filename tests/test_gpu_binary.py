@@ -9,6 +9,7 @@ import pytest
 import lancedb_b200 as lancedb
 from lancedb_b200 import _native
 from tests.hamming_oracle import flat_search_u8, hamming_u8
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
 
@@ -24,14 +25,6 @@ def _stats(fn):
         _native.set_profiling(False)
 
 
-def _same(got, want):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc)
-    assert np.array_equal(gi, oi)
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32))
-
-
 def _check(x, q, k, row_ids=None, **kw):
     bx = _native.GpuBinary(x, row_ids=row_ids)
     got, st = _stats(lambda: bx.search(q, k=k, **kw))
@@ -40,7 +33,7 @@ def _check(x, q, k, row_ids=None, **kw):
     if allow is not None:
         bits = np.unpackbits(np.asarray(allow, np.uint32).view(np.uint8), bitorder="little")
         mask = bits[:kw.pop("allow_bits")].astype(bool)
-    _same(got, flat_search_u8(x, q, k, row_ids=row_ids, allow=mask, **kw))
+    assert_same(got, flat_search_u8(x, q, k, row_ids=row_ids, allow=mask, **kw))
     bx.close()
     return st
 
@@ -169,7 +162,7 @@ def test_device_entry_point_and_graph_replay_match_the_host_call(N):
     bx = _native.GpuBinary(x)
     want = flat_search_u8(x, q, 10)
     for _ in range(3):                          # warm-up, capture, replay
-        _same(bx.search(q, k=10), want)
+        assert_same(bx.search(q, k=10), want)
     dq = torch.from_numpy(q).cuda()
     oi = torch.empty(32, 10, dtype=torch.int64, device="cuda"); od = torch.empty(32, 10, device="cuda")
     oc = torch.empty(32, dtype=torch.int32, device="cuda")
@@ -177,7 +170,7 @@ def test_device_entry_point_and_graph_replay_match_the_host_call(N):
         bx.search_device(dq.data_ptr(), 32, _native.make_params(k=10, nprobes=0), oi.data_ptr(), od.data_ptr(),
                          oc.data_ptr(), torch.cuda.current_stream().cuda_stream)
         torch.cuda.synchronize()
-        _same((oi.cpu().numpy().view(np.uint64), od.cpu().numpy(), oc.cpu().numpy().view(np.uint32)), want)
+        assert_same((oi.cpu().numpy().view(np.uint64), od.cpu().numpy(), oc.cpu().numpy().view(np.uint32)), want)
     bx.close()
 
 

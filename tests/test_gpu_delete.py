@@ -25,6 +25,7 @@ import oracle
 from lancedb_b200 import _native
 from lancedb_b200.index import IVF_KINDS
 from tests import hamming_oracle, multivec_oracle, unindexed_oracle as U
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -40,16 +41,6 @@ KINDS = [
     ("IVF_RQ", dict(num_bits=1), "cosine"),
     ("IVF_FLAT", dict(), "hamming"),
 ]
-
-
-def _same(got, want, what=""):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(np.asarray(gc, np.uint32), np.asarray(oc, np.uint32)), f"{what}: counts differ"
-    for i in range(len(gc)):
-        n = int(gc[i])
-        assert np.array_equal(gi[i, :n], oi[i, :n]), f"{what}: ids differ (query {i})"
-        assert np.array_equal(gd[i, :n].view(np.uint32), od[i, :n].view(np.uint32)), f"{what}: distances differ ({i})"
 
 
 def _live(nbits, dead, allow=None):
@@ -114,29 +105,32 @@ def test_ivf_deletes_on_every_route(kind, params, metric):
         live = _live(N + NT, dead)
         for nprobes, max_np in ((4, 0), (2, NLIST)):
             what = f"step {step} nprobes {nprobes}/{max_np}"
-            _same(h.search(q, k=K, nprobes=nprobes, max_nprobes=max_np),
-                  U.index_search(d, q, K, nprobes, allow=live[:N], max_nprobes=max_np), what + " host")
-            _same(h.search(q, k=K, nprobes=nprobes, max_nprobes=max_np, allow=call_bm, allow_bits=N + NT),
-                  U.index_search(d, q, K, nprobes, allow=live & call, max_nprobes=max_np), what + " filtered")
-            _same(h.search_unindexed(th, q, k=K, nprobes=nprobes, max_nprobes=max_np),
-                  U.union_search(d, tail, tail_ids, q, K, nprobes, allow=live, max_nprobes=max_np), what + " union")
-            _same(h.search_unindexed(th, q, k=K, nprobes=nprobes, max_nprobes=max_np, allow=call_bm,
-                                     allow_bits=N + NT),
-                  U.union_search(d, tail, tail_ids, q, K, nprobes, allow=live & call, max_nprobes=max_np),
-                  what + " union filtered")
+            assert_same(h.search(q, k=K, nprobes=nprobes, max_nprobes=max_np),
+                        U.index_search(d, q, K, nprobes, allow=live[:N], max_nprobes=max_np),
+                        what + " host", prefix=True)
+            assert_same(h.search(q, k=K, nprobes=nprobes, max_nprobes=max_np, allow=call_bm, allow_bits=N + NT),
+                        U.index_search(d, q, K, nprobes, allow=live & call, max_nprobes=max_np),
+                        what + " filtered", prefix=True)
+            assert_same(h.search_unindexed(th, q, k=K, nprobes=nprobes, max_nprobes=max_np),
+                        U.union_search(d, tail, tail_ids, q, K, nprobes, allow=live, max_nprobes=max_np),
+                        what + " union", prefix=True)
+            assert_same(h.search_unindexed(th, q, k=K, nprobes=nprobes, max_nprobes=max_np, allow=call_bm,
+                                           allow_bits=N + NT),
+                        U.union_search(d, tail, tail_ids, q, K, nprobes, allow=live & call, max_nprobes=max_np),
+                        what + " union filtered", prefix=True)
         p = _native.make_params(K, 4, max_nprobes=NLIST)
         want = U.index_search(d, q, K, 4, allow=live[:N], max_nprobes=NLIST)
-        _same(_device_search(h, q, p, B, K, binary), want, f"step {step} device")
+        assert_same(_device_search(h, q, p, B, K, binary), want, f"step {step} device", prefix=True)
         if binary:
             continue
         ids, dist, cnt = (np.empty((B, K), np.uint64), np.empty((B, K), f32), np.empty(B, np.uint32))
         _native.ticket_wait(h.search_async(q, p, ids, dist, cnt))
-        _same((ids, dist, cnt), want, f"step {step} async")
+        assert_same((ids, dist, cnt), want, f"step {step} async", prefix=True)
         want = U.index_search(d, q[:3], K, 20, allow=live[:N])
         for i in range(3):
             gi, gd, gc = h.search_one(q[i], k=K, nprobes=20)
-            _same((gi[None], gd[None], np.array([gc], np.uint32)),
-                  (want[0][i:i + 1], want[1][i:i + 1], want[2][i:i + 1]), f"step {step} coalesced")
+            assert_same((gi[None], gd[None], np.array([gc], np.uint32)),
+                        (want[0][i:i + 1], want[1][i:i + 1], want[2][i:i + 1]), f"step {step} coalesced", prefix=True)
     assert dead == set(range(N + NT))
     h.close(); th.close()
 
@@ -148,7 +142,7 @@ def test_widening_matches_the_oracle_with_deletions():
     h.delete(gone)
     live = _live(N, set(int(i) for i in gone))
     want = U.index_search(d, q, K, 1, allow=live, max_nprobes=NLIST)
-    _same(h.search(q, k=K, nprobes=1, max_nprobes=NLIST), want, "widened")
+    assert_same(h.search(q, k=K, nprobes=1, max_nprobes=NLIST), want, "widened", prefix=True)
     narrow = U.index_search(d, q, K, 1, allow=live)
     assert (want[2] > narrow[2]).any()
     h.close(); th.close()
@@ -173,10 +167,10 @@ def test_flat_float_deletes(metric):
         live = _live(nbits, dead)
         for k in ((K, 2100) if step == 1 else (K,)):
             want = oracle.flat_search(x, q, k, metric=metric, row_ids=ids, nthreads=0, allow=live)
-            _same(fl.search(q, k=k, metric=metric), want, f"{metric} step {step} k {k}")
-        _same(fl.search(q, k=K, metric=metric, allow=call_bm, allow_bits=nbits),
-              oracle.flat_search(x, q, K, metric=metric, row_ids=ids, nthreads=0, allow=live & call),
-              f"{metric} step {step} filtered")
+            assert_same(fl.search(q, k=k, metric=metric), want, f"{metric} step {step} k {k}", prefix=True)
+        assert_same(fl.search(q, k=K, metric=metric, allow=call_bm, allow_bits=nbits),
+                    oracle.flat_search(x, q, K, metric=metric, row_ids=ids, nthreads=0, allow=live & call),
+                    f"{metric} step {step} filtered", prefix=True)
         p = _native.make_params(K, 0)
         import torch
         dq = torch.from_numpy(q).cuda()
@@ -185,8 +179,9 @@ def test_flat_float_deletes(metric):
         fl.search_device(metric, dq.data_ptr(), 32, p, o[0].data_ptr(), o[1].data_ptr(), c.data_ptr(),
                          torch.cuda.current_stream().cuda_stream)
         torch.cuda.synchronize()
-        _same((o[0].cpu().numpy().view(np.uint64), o[1].cpu().numpy(), c.cpu().numpy().view(np.uint32)),
-              oracle.flat_search(x, q, K, metric=metric, row_ids=ids, nthreads=0, allow=live), f"{metric} device")
+        assert_same((o[0].cpu().numpy().view(np.uint64), o[1].cpu().numpy(), c.cpu().numpy().view(np.uint32)),
+                    oracle.flat_search(x, q, K, metric=metric, row_ids=ids, nthreads=0, allow=live),
+                    f"{metric} device", prefix=True)
     fl.close()
 
 
@@ -201,7 +196,7 @@ def test_flat_l2_above_the_large_shortlist_threshold():
     gone = np.concatenate([gone, rng.permutation(n)[:n // 3]])
     fl.delete(gone)
     live = _live(n, set(int(i) for i in gone))
-    _same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0, allow=live), "large N")
+    assert_same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0, allow=live), "large N", prefix=True)
     fl.close()
 
 
@@ -218,11 +213,13 @@ def test_flat_binary_deletes(n):
         assert bx.delete(di) == len(new)
         dead |= new
         live = _live(n, dead)
-        _same(bx.search(q, k=K), hamming_oracle.flat_search_u8(x, q, K, allow=live), f"binary {n} step {step}")
-        _same(bx.search(q, k=K, allow=_native.mask_bitmap(call), allow_bits=n),
-              hamming_oracle.flat_search_u8(x, q, K, allow=live & call), f"binary {n} step {step} filtered")
-        _same(_device_search(bx, q, _native.make_params(K, 0), 24, K, True),
-              hamming_oracle.flat_search_u8(x, q, K, allow=live), f"binary {n} step {step} device")
+        assert_same(bx.search(q, k=K), hamming_oracle.flat_search_u8(x, q, K, allow=live),
+                    f"binary {n} step {step}", prefix=True)
+        assert_same(bx.search(q, k=K, allow=_native.mask_bitmap(call), allow_bits=n),
+                    hamming_oracle.flat_search_u8(x, q, K, allow=live & call),
+                    f"binary {n} step {step} filtered", prefix=True)
+        assert_same(_device_search(bx, q, _native.make_params(K, 0), 24, K, True),
+                    hamming_oracle.flat_search_u8(x, q, K, allow=live), f"binary {n} step {step} device", prefix=True)
     bx.close()
 
 
@@ -239,8 +236,9 @@ def test_multivector_deletes():
         dead |= set(int(i) for i in di)
         mv.delete(di)
         live = _live(3000, dead)
-        _same(mv.search(q, k=K, q_offsets=qoff),
-              multivec_oracle.flat_search_mv(x, off, q, qoff, K, allow=live), f"multivector step {step}")
+        assert_same(mv.search(q, k=K, q_offsets=qoff),
+                    multivec_oracle.flat_search_mv(x, off, q, qoff, K, allow=live),
+                    f"multivector step {step}", prefix=True)
     mv.close()
 
 
@@ -263,7 +261,7 @@ def test_delete_append_delete(binary):
     else:
         want = oracle.flat_search(allx, q, K, nthreads=0, allow=live)
     assert live[7500]
-    _same(h.search(q, k=K), want, "after delete / append / delete")
+    assert_same(h.search(q, k=K), want, "after delete / append / delete", prefix=True)
     h.close()
 
 
@@ -273,21 +271,21 @@ def test_graph_replay_after_delete():
     q = rng.standard_normal((16, 64)).astype(f32)
     fl = _native.GpuFlat(x)
     for _ in range(3):                                      # eager, capture, replay
-        _same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0), "before")
+        assert_same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0), "before", prefix=True)
     gone = np.unique(oracle.flat_search(x, q, 3, nthreads=0)[0].astype(np.int64))
     fl.delete(gone)
     live = _live(5000, set(int(i) for i in gone))
     for _ in range(3):                                      # the graph captured without a filter is not replayed
-        _same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0, allow=live), "after")
+        assert_same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0, allow=live), "after", prefix=True)
     fl.close()
     d, h, q, _, th = _train("IVF_PQ", dict(num_sub_vectors=8), "l2", rng)
     for _ in range(3):
-        _same(h.search(q, k=K, nprobes=4), U.index_search(d, q, K, 4), "ivf before")
+        assert_same(h.search(q, k=K, nprobes=4), U.index_search(d, q, K, 4), "ivf before", prefix=True)
     gone = np.unique(h.search(q, k=2, nprobes=4)[0].astype(np.int64))
     h.delete(gone)
     live = _live(N, set(int(i) for i in gone))
     for _ in range(3):
-        _same(h.search(q, k=K, nprobes=4), U.index_search(d, q, K, 4, allow=live), "ivf after")
+        assert_same(h.search(q, k=K, nprobes=4), U.index_search(d, q, K, 4, allow=live), "ivf after", prefix=True)
     h.close(); th.close()
 
 
@@ -352,7 +350,7 @@ def _tc_flat_case(x, q, gone, call=None, ids=None):
         _native.set_profiling(False)
     fl.close()
     want = oracle.flat_search(x, q, K, row_ids=ids, nthreads=0, allow=live if call is None else live & call)
-    _same(got, want, "tensor-core flat under a filter")
+    assert_same(got, want, "tensor-core flat under a filter", prefix=True)
     # [1]: distances the tensor cores computed, every row for every query on the tensor-core route, none on the exact one
     assert st["rescored"] == len(q) * len(x) and st["queries"] == len(q), f"the exact route ran: {st}"
     return got
@@ -420,7 +418,7 @@ def test_tensor_core_binary_under_a_filter(n, B, with_ids):
             st = _native.last_filter_stats()
         finally:
             _native.set_profiling(False)
-        _same(got, hamming_oracle.flat_search_u8(x, q, K, row_ids=ids, allow=allow), f"binary {n}")
+        assert_same(got, hamming_oracle.flat_search_u8(x, q, K, row_ids=ids, allow=allow), f"binary {n}", prefix=True)
         assert st["rescored"] > 0, "the binary search did not run on the tensor cores"
     bx.close()
 
@@ -467,11 +465,12 @@ def test_append_may_not_undelete():
         q = x[rng.integers(0, 5000, 16)]
         search = (lambda xx, qq, k, **kw: hamming_oracle.flat_search_u8(xx, qq, k, **kw)) if binary else \
             (lambda xx, qq, k, **kw: oracle.flat_search(xx, qq, k, nthreads=0, **kw))
-        _same(h.search(q, k=K), search(x, q, K, row_ids=ids), "after a refused append")
+        assert_same(h.search(q, k=K), search(x, q, K, row_ids=ids), "after a refused append", prefix=True)
         h.append(extra, np.array([11, 20001], np.uint64))               # a gap below id_bound, and a new id above it
         allx, allid = np.concatenate([x, extra]), np.concatenate([ids, [11, 20001]]).astype(np.uint64)
         keep = ~np.isin(allid, [10, 12])
-        _same(h.search(q, k=K), search(allx[keep], q, K, row_ids=allid[keep]), "after an allowed append")
+        assert_same(h.search(q, k=K), search(allx[keep], q, K, row_ids=allid[keep]),
+                    "after an allowed append", prefix=True)
         h.close()
 
 
@@ -486,19 +485,21 @@ def _sub_batch_child():
     fl.delete(gone)
     live = _live(6000, set(int(i) for i in gone))
     call = rng.random(6000) < 0.5
-    _same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0, allow=live), "flat split")
-    _same(fl.search(q, k=K, allow=_native.mask_bitmap(call), allow_bits=6000),
-          oracle.flat_search(x, q, K, nthreads=0, allow=live & call), "flat split filtered")
+    assert_same(fl.search(q, k=K), oracle.flat_search(x, q, K, nthreads=0, allow=live), "flat split", prefix=True)
+    assert_same(fl.search(q, k=K, allow=_native.mask_bitmap(call), allow_bits=6000),
+                oracle.flat_search(x, q, K, nthreads=0, allow=live & call), "flat split filtered", prefix=True)
     d, h, _, tail, th = _train("IVF_PQ", dict(num_sub_vectors=8), "l2", rng)
     qi = rng.standard_normal((1024, DIM)).astype(f32)
     gone = np.concatenate([rng.permutation(N)[:N // 2], np.arange(N, N + NT, 2)])
     h.delete(gone[gone < N]); th.delete(gone[gone >= N])
     live = _live(N + NT, set(int(i) for i in gone))
     assert h.debug_sub_batch_size(1024, 4) < 1024
-    _same(h.search(qi, k=K, nprobes=4, max_nprobes=NLIST),
-          U.index_search(d, qi, K, 4, allow=live[:N], max_nprobes=NLIST), "ivf split")
-    _same(h.search_unindexed(th, qi, k=K, nprobes=4), U.union_search(d, tail, np.arange(N, N + NT, dtype=np.uint64),
-                                                                      qi, K, 4, allow=live), "union split")
+    assert_same(h.search(qi, k=K, nprobes=4, max_nprobes=NLIST),
+                U.index_search(d, qi, K, 4, allow=live[:N], max_nprobes=NLIST), "ivf split", prefix=True)
+    assert_same(h.search_unindexed(th, qi, k=K, nprobes=4),
+                U.union_search(d, tail, np.arange(N, N + NT, dtype=np.uint64),
+                                                                            qi, K, 4, allow=live),
+                "union split", prefix=True)
     print("ok")
 
 
@@ -521,11 +522,12 @@ def _charge_child():
     n0 = _native.kernel_launch_count()
     got = fl.search(q, k=K, timeout_ms=60000)          # (a deadline keeps the call eager: every launch is counted)
     plain = _native.kernel_launch_count() - n0
-    _same(got, oracle.flat_search(x, q, K, row_ids=ids, nthreads=0, allow=live), "live bitmap only")
+    assert_same(got, oracle.flat_search(x, q, K, row_ids=ids, nthreads=0, allow=live), "live bitmap only", prefix=True)
     n0 = _native.kernel_launch_count()
     got = fl.search(q, k=K, allow=_native.mask_bitmap(call), allow_bits=nbits)
     filtered = _native.kernel_launch_count() - n0
-    _same(got, oracle.flat_search(x, q, K, row_ids=ids, nthreads=0, allow=live & call), "with a call bitmap")
+    assert_same(got, oracle.flat_search(x, q, K, row_ids=ids, nthreads=0, allow=live & call),
+                "with a call bitmap", prefix=True)
     # 24 000 bytes per query: 2 sub-batches in 8 MiB, 3 once the 3.7 MiB bitmap is charged (plus the AND launch)
     assert filtered > plain + 1, (plain, filtered)
     print("ok")

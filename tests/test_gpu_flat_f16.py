@@ -17,7 +17,7 @@ import pytest
 import oracle
 import lancedb_b200 as lancedb
 from lancedb_b200 import _native
-from tests.util import random_index, same_result
+from tests.util import assert_same, random_index
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -34,10 +34,6 @@ def _rows(rng, n, d, scale=1.0):
 
 def _pair(x16, row_ids=None):
     return _native.GpuFlat(x16, row_ids=row_ids), _native.GpuFlat(x16.astype(F32), row_ids=row_ids)
-
-
-def _same(a, b, what):
-    assert same_result(a, b), what
 
 
 @pytest.fixture(scope="module", params=SHAPES, ids=[s[3] + f"-{s[0]}x{s[2]}" for s in SHAPES])
@@ -63,21 +59,23 @@ def test_parity_on_every_path(shape, metric):
         got = h16.search(q, **kw)
         st = _native.last_filter_stats()
         _native.set_profiling(False)
-        _same(got, h32.search(q, **kw), (metric, k))
+        assert_same(got, h32.search(q, **kw), (metric, k))
         tc = metric == "l2" and path != "exact" and k <= 2048
         assert st["rescored"] == (B * N if tc else 0), (path, metric, k, st)   # [1]: tensor-core distances
         if k in (10, 2049) or (k == 65536 and N <= 20000):
-            _same(got, oracle.flat_search(x32, q, k=k, metric=metric, nthreads=16), ("oracle", metric, k))
+            assert_same(got, oracle.flat_search(x32, q, k=k, metric=metric, nthreads=16), ("oracle", metric, k))
     lo, hi = (0.5, 1.5) if metric != "l2" else (float(d) * 1.5, float(d) * 2.5)
     for k in (10, 2049):
         kw = dict(k=k, metric=metric, lower=lo, upper=hi)
         got = h16.search(q, **kw)
-        _same(got, h32.search(q, **kw), ("range", metric, k))
-        _same(got, oracle.flat_search(x32, q, k=k, metric=metric, lower=lo, upper=hi, nthreads=16), ("range oracle", k))
+        assert_same(got, h32.search(q, **kw), ("range", metric, k))
+        assert_same(got, oracle.flat_search(x32, q, k=k, metric=metric, lower=lo, upper=hi, nthreads=16),
+                    ("range oracle", k))
         kw = dict(k=k, metric=metric, allow=_native.mask_bitmap(mask), allow_bits=N)
         got = h16.search(q, **kw)
-        _same(got, h32.search(q, **kw), ("prefilter", metric, k))
-        _same(got, oracle.flat_search(x32, q, k=k, metric=metric, allow=mask, nthreads=16), ("prefilter oracle", k))
+        assert_same(got, h32.search(q, **kw), ("prefilter", metric, k))
+        assert_same(got, oracle.flat_search(x32, q, k=k, metric=metric, allow=mask, nthreads=16),
+                    ("prefilter oracle", k))
 
 
 def test_deleted_rows_on_every_path(shape):
@@ -90,8 +88,9 @@ def test_deleted_rows_on_every_path(shape):
     for metric in ("l2", "cosine"):
         for k in (10, 2049):
             got = h16.search(q, k=k, metric=metric)
-            _same(got, h32.search(q, k=k, metric=metric), ("deleted", metric, k))
-            _same(got, oracle.flat_search(x16.astype(F32), q, k=k, metric=metric, allow=live, nthreads=16), "oracle")
+            assert_same(got, h32.search(q, k=k, metric=metric), ("deleted", metric, k))
+            assert_same(got, oracle.flat_search(x16.astype(F32), q, k=k, metric=metric, allow=live, nthreads=16),
+                        "oracle")
     h16.close(); h32.close()
 
 
@@ -128,8 +127,8 @@ def test_band_on_adversarial_queries(N):
     h16, h32 = _pair(x16)
     for k in (1, 10, 100):
         got = h16.search(q, k=k)
-        _same(got, h32.search(q, k=k), ("band", k))
-        _same(got, oracle.flat_search(x16.astype(F32), q, k=k, nthreads=16), ("band oracle", k))
+        assert_same(got, h32.search(q, k=k), ("band", k))
+        assert_same(got, oracle.flat_search(x16.astype(F32), q, k=k, nthreads=16), ("band oracle", k))
     h16.close(); h32.close()
 
 
@@ -158,8 +157,8 @@ def test_fp16_mma_consumes_subnormal_operands_exactly():
     st = _native.last_filter_stats()
     _native.set_profiling(False)
     assert st["rescored"] == 16 * 8192                     # the tensor cores scored every row
-    _same(got, h32.search(q, k=10), "subnormal rows")
-    _same(got, oracle.flat_search(x16.astype(F32), q, k=10, nthreads=16), "subnormal rows oracle")
+    assert_same(got, h32.search(q, k=10), "subnormal rows")
+    assert_same(got, oracle.flat_search(x16.astype(F32), q, k=10, nthreads=16), "subnormal rows oracle")
     h16.close(); h32.close()
 
 
@@ -175,7 +174,7 @@ def test_appends_across_both_thresholds_and_after_deletes():
         ref = _native.GpuFlat(x16[:n1])
         for metric in ("l2", "cosine"):
             for k in (10, 2049):
-                _same(h.search(q, k=k, metric=metric), ref.search(q, k=k, metric=metric), (n1, metric, k))
+                assert_same(h.search(q, k=k, metric=metric), ref.search(q, k=k, metric=metric), (n1, metric, k))
         ref.close()
     h.close()
     h16, h32 = _pair(x16[:200000])
@@ -183,7 +182,7 @@ def test_appends_across_both_thresholds_and_after_deletes():
     h16.delete(gone); h32.delete(gone)
     h16.append(x16[200000:]); h32.append(x16[200000:].astype(F32))
     for k in (10, 2049):
-        _same(h16.search(q, k=k), h32.search(q, k=k), ("delete then append", k))
+        assert_same(h16.search(q, k=k), h32.search(q, k=k), ("delete then append", k))
     with pytest.raises(ValueError):
         h16.append(x16[:2].astype(F32))
     with pytest.raises(ValueError):
@@ -202,7 +201,8 @@ def test_fp16_tail_of_an_unindexed_union():
     q = rng.standard_normal((16, d)).astype(F32)
     allow = _native.mask_bitmap(rng.random(10000) < 0.8)
     for kw in (dict(k=10), dict(k=2049), dict(k=10, refine_factor=2), dict(k=10, allow=allow, allow_bits=10000)):
-        _same(gi.search_unindexed(t16, q, nprobes=4, **kw), gi.search_unindexed(t32, q, nprobes=4, **kw), kw.keys())
+        assert_same(gi.search_unindexed(t16, q, nprobes=4, **kw), gi.search_unindexed(t32, q, nprobes=4, **kw),
+                    kw.keys())
     t16.close(); t32.close(); gi.close()
 
 
@@ -217,7 +217,7 @@ def test_non_finite_rows_give_the_f32_handles_results():
         h16, h32 = _pair(x16)
         for metric in ("l2", "cosine", "dot"):
             for k in (10, 2049):
-                _same(h16.search(q, k=k, metric=metric), h32.search(q, k=k, metric=metric), (N, metric, k))
+                assert_same(h16.search(q, k=k, metric=metric), h32.search(q, k=k, metric=metric), (N, metric, k))
         h16.close(); h32.close()
 
 

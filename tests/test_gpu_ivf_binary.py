@@ -9,16 +9,9 @@ import lancedb_b200 as lancedb
 import pyarrow as pa
 from lancedb_b200 import _native
 from tests import ivf_binary_oracle as O
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
-
-
-def _same(got, want, what=""):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distance bits differ"
 
 
 @pytest.mark.parametrize("B,N,nbytes", [(1, 1, 1), (7, 300, 3), (8, 257, 32), (9, 33, 33), (13, 1000, 128),
@@ -47,7 +40,7 @@ def test_gpu_ivf_binary_equals_oracle(n, nbytes, nlist, B, k, nprobes, patterns,
     ix = O.random_index(rng, n, nbytes, nlist, empty=empty, patterns=patterns)
     q = ix.vectors[rng.integers(0, n, B)] ^ (rng.random((B, nbytes)) < 0.1).astype(np.uint8)
     gpu = _native.GpuIvfBinary(ix)
-    _same(gpu.search(q, k=k, nprobes=nprobes), O.search(ix, q, k=k, nprobes=nprobes), "search")
+    assert_same(gpu.search(q, k=k, nprobes=nprobes), O.search(ix, q, k=k, nprobes=nprobes), "search")
     gpu.close()
 
 
@@ -59,14 +52,14 @@ def test_all_probes_equal_flat_binary_search(nlist, nbytes):
     gpu = _native.GpuIvfBinary(ix)
     got = gpu.search(q, k=20, nprobes=nlist)
     if nlist > 2048:                                     # above the select's k limit nprobes must cover every partition
-        _same(gpu.search(q, k=20, nprobes=nlist + 5), got, "nprobes > nlist")
+        assert_same(gpu.search(q, k=20, nprobes=nlist + 5), got, "nprobes > nlist")
         with pytest.raises(ValueError, match="2048"):
             gpu.search(q, k=20, nprobes=3000)
     gpu.close()
     flat = _native.GpuBinary(ix.vectors, row_ids=ix.row_ids)
     want = flat.search(q, k=20)
     flat.close()
-    _same(got, want, "nprobes = nlist vs flat")
+    assert_same(got, want, "nprobes = nlist vs flat")
 
 
 def test_prefilter_range_refine_timeout_and_entry_points():
@@ -80,13 +73,14 @@ def test_prefilter_range_refine_timeout_and_entry_points():
     bm = _native.mask_bitmap(mask)
     for mx in (0, 50, nlist):
         got = gpu.search(q, k=10, nprobes=2, allow=bm, allow_bits=n, max_nprobes=mx)
-        _same(got, O.search(ix, q, k=10, nprobes=2, allow=mask, max_nprobes=mx), f"prefilter max_nprobes={mx}")
+        assert_same(got, O.search(ix, q, k=10, nprobes=2, allow=mask, max_nprobes=mx), f"prefilter max_nprobes={mx}")
     d = O.search(ix, q[:1], k=60, nprobes=6)[1][0]
     lo, hi = float(d[5]), float(d[40])
-    _same(gpu.search(q, k=20, nprobes=6, lower=lo, upper=hi), O.search(ix, q, k=20, nprobes=6, lower=lo, upper=hi),
-          "distance_range")
-    _same(gpu.search(q, k=7, nprobes=6, refine_factor=5), O.search(ix, q, k=7, nprobes=6), "refine_factor")
-    _same(gpu.search(q, k=7, nprobes=6, timeout_ms=60000), O.search(ix, q, k=7, nprobes=6), "generous timeout")
+    assert_same(gpu.search(q, k=20, nprobes=6, lower=lo, upper=hi),
+                O.search(ix, q, k=20, nprobes=6, lower=lo, upper=hi),
+                "distance_range")
+    assert_same(gpu.search(q, k=7, nprobes=6, refine_factor=5), O.search(ix, q, k=7, nprobes=6), "refine_factor")
+    assert_same(gpu.search(q, k=7, nprobes=6, timeout_ms=60000), O.search(ix, q, k=7, nprobes=6), "generous timeout")
     want = O.search(ix, q, k=9, nprobes=6)
     p = _native.make_params(9, 6)
     dq = torch.from_numpy(np.ascontiguousarray(q)).cuda()
@@ -95,7 +89,7 @@ def test_prefilter_range_refine_timeout_and_entry_points():
     dc = torch.empty(33, dtype=torch.int32, device="cuda")
     gpu.search_device(dq.data_ptr(), 33, p, di.data_ptr(), dd.data_ptr(), dc.data_ptr(), 0)
     torch.cuda.synchronize()
-    _same((di.cpu().numpy().view(np.uint64), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32)), want, "device")
+    assert_same((di.cpu().numpy().view(np.uint64), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32)), want, "device")
     _native.set_profiling(True)
     gpu.search(q, k=9, nprobes=6)
     stages = _native.last_stage_ms()
@@ -112,7 +106,7 @@ def test_multi_sub_batch_and_timeout():
     ix = O.random_index(rng, n, nbytes, nlist, patterns=3000)
     q = rng.integers(0, 256, (9000, nbytes), dtype=np.uint8)
     gpu = _native.GpuIvfBinary(ix)
-    _same(gpu.search(q, k=5, nprobes=2), O.search(ix, q, k=5, nprobes=2), "two sub-batches")
+    assert_same(gpu.search(q, k=5, nprobes=2), O.search(ix, q, k=5, nprobes=2), "two sub-batches")
     with pytest.raises(TimeoutError, match="timeout"):
         gpu.search(q, k=5, nprobes=2, timeout_ms=1)
     gpu.close()
@@ -142,8 +136,8 @@ def test_unused_refine_factor_and_maximum_nprobes_are_not_limited():
     q = ix.vectors[rng.integers(0, n, 40)]
     gpu = _native.GpuIvfBinary(ix)
     want = O.search(ix, q, k=300, nprobes=8)
-    _same(gpu.search(q, k=300, nprobes=8, refine_factor=10), want, "k x refine_factor above 2048")
-    _same(gpu.search(q, k=300, nprobes=8, max_nprobes=3000), want, "maximum_nprobes without a prefilter")
+    assert_same(gpu.search(q, k=300, nprobes=8, refine_factor=10), want, "k x refine_factor above 2048")
+    assert_same(gpu.search(q, k=300, nprobes=8, max_nprobes=3000), want, "maximum_nprobes without a prefilter")
     mask = rng.random(n) < 0.01
     with pytest.raises(ValueError, match="maximum_nprobes"):
         gpu.search(q, k=20, nprobes=8, allow=_native.mask_bitmap(mask), allow_bits=n, max_nprobes=3000)

@@ -12,18 +12,11 @@ import pytest
 
 from lancedb_b200 import _native
 from tests import hnsw_sq_oracle as H
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
 f32 = np.float32
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _same(got, want, what=""):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distance bits differ"
 
 
 _IX = {}
@@ -58,7 +51,7 @@ def test_search_equals_the_c_oracle(dim, metric, case):
     data, g = _index(dim, metric)
     q = _queries(np.random.default_rng(case), data, 37)
     kw = CASES[case]
-    _same(g.search(q, **kw), H.search(data, q, **kw), f"{dim} {metric} {kw}")
+    assert_same(g.search(q, **kw), H.search(data, q, **kw), f"{dim} {metric} {kw}")
 
 
 @pytest.mark.parametrize("dim", [24, 100])
@@ -71,7 +64,7 @@ def test_prefilter_with_widening_equals_the_c_oracle(dim):
     bm = _native_bitmap(mask)
     for kw in (dict(k=10, nprobes=1, max_nprobes=5), dict(k=10, nprobes=2, max_nprobes=5, ef=30, refine_factor=2)):
         got = g.search(q, allow=bm, allow_bits=nbits, **kw)
-        _same(got, H.search(data, q, allow=mask, **kw), str(kw))
+        assert_same(got, H.search(data, q, allow=mask, **kw), str(kw))
 
 
 def _native_bitmap(mask):
@@ -88,7 +81,7 @@ def test_complete_graph_equals_the_gpu_ivf_sq_search():
     g, s = _native.GpuIvfHnswSq(full), _native.GpuIvfSq(sq)
     q = _queries(np.random.default_rng(5), full, 16)
     for kw in (dict(k=10, nprobes=5), dict(k=10, nprobes=2, refine_factor=3)):
-        _same(g.search(q, ef=2048, **kw), s.search(q, **kw), str(kw))
+        assert_same(g.search(q, ef=2048, **kw), s.search(q, **kw), str(kw))
 
 
 def test_every_entry_point_returns_the_host_result():
@@ -97,7 +90,7 @@ def test_every_entry_point_returns_the_host_result():
     q = _queries(np.random.default_rng(9), data, 12)
     kw = dict(k=10, nprobes=3, ef=40)
     want = g.search(q, **kw)
-    _same(want, H.search(data, q, **kw), "host")
+    assert_same(want, H.search(data, q, **kw), "host")
     p = _native.make_params(10, 3, ef=40)
     dq = torch.as_tensor(q, device="cuda")
     di = torch.empty((12, 10), dtype=torch.int64, device="cuda")
@@ -105,11 +98,11 @@ def test_every_entry_point_returns_the_host_result():
     dc = torch.empty(12, dtype=torch.int32, device="cuda")
     g.search_device(dq.data_ptr(), 12, p, di.data_ptr(), dd.data_ptr(), dc.data_ptr(), 0)
     torch.cuda.synchronize()
-    _same((di.cpu().numpy().view(np.uint64), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32)), want, "device")
+    assert_same((di.cpu().numpy().view(np.uint64), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32)), want, "device")
     ids, dist, cnt = np.empty((12, 10), np.uint64), np.empty((12, 10), f32), np.empty(12, np.uint32)
     t = g.search_async(q, p, ids, dist, cnt)
     _native.ticket_wait(t)
-    _same((ids, dist, cnt), want, "async")
+    assert_same((ids, dist, cnt), want, "async")
     out = [None] * 12
 
     def one(i):
@@ -118,7 +111,7 @@ def test_every_entry_point_returns_the_host_result():
     [x.start() for x in th]
     [x.join() for x in th]
     for i, (oi, od, oc) in enumerate(out):
-        _same((oi[None], od[None], np.array([oc], np.uint32)), tuple(a[i:i + 1] for a in want), f"coalesced {i}")
+        assert_same((oi[None], od[None], np.array([oc], np.uint32)), tuple(a[i:i + 1] for a in want), f"coalesced {i}")
 
 
 _CHILD = r"""
@@ -168,9 +161,9 @@ def test_ef_sweep_with_one_shape_equals_the_c_oracle_on_every_call():
     ids, dist, cnt = np.empty((16, 10), np.uint64), np.empty((16, 10), f32), np.empty(16, np.uint32)
     for ef in (16, 16, 16, 40, 11, 200, 16, 40):
         want = H.search(data, q, k=10, nprobes=3, ef=ef)
-        _same(g.search(q, k=10, nprobes=3, ef=ef), want, f"sync ef {ef}")
+        assert_same(g.search(q, k=10, nprobes=3, ef=ef), want, f"sync ef {ef}")
         _native.ticket_wait(g.search_async(q, _native.make_params(10, 3, ef=ef), ids, dist, cnt))
-        _same((ids, dist, cnt), want, f"async ef {ef}")
+        assert_same((ids, dist, cnt), want, f"async ef {ef}")
 
 
 def test_wide_lists_duplicate_neighbours_and_a_single_row_partition():
@@ -203,7 +196,7 @@ def test_wide_lists_duplicate_neighbours_and_a_single_row_partition():
     g = _native.GpuIvfHnswSq(data)
     q = _queries(np.random.default_rng(13), data, 40)
     for kw in (dict(k=10, nprobes=5), dict(k=10, nprobes=5, ef=150), dict(k=3, nprobes=2, ef=3)):
-        _same(g.search(q, **kw), H.search(data, q, **kw), str(kw))
+        assert_same(g.search(q, **kw), H.search(data, q, **kw), str(kw))
 
 
 # recall@10 of a CUDA-built graph against IVF_SQ over the same probes; the CPU build of this fixture reaches 0.974
@@ -220,7 +213,7 @@ def test_cuda_built_index_validates_and_meets_the_recall_floor():
     assert (data.adj0 != H.NONE).sum(1).mean() > 4       # the lists are not collapsed
     q = (centres[rng.integers(0, 12, 50)] + rng.standard_normal((50, 32))).astype(f32)
     gi, gd, gc = _native.GpuIvfHnswSq(data).search(q, k=10, nprobes=2)
-    _same((gi, gd, gc), H.search(data, q, k=10, nprobes=2), "cuda-built")
+    assert_same((gi, gd, gc), H.search(data, q, k=10, nprobes=2), "cuda-built")
     si, _, _ = sq_oracle.search(data.sq, q, k=10, nprobes=2)
     assert np.mean([len(set(a) & set(b)) / 10 for a, b in zip(gi.tolist(), si.tolist())]) >= RECALL_FLOOR
 

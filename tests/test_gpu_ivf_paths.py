@@ -14,7 +14,7 @@ import oracle
 from lancedb_b200 import _native
 from tests import sq_oracle
 from tests.sq_oracle import random_sq_index
-from tests.util import queries, random_index
+from tests.util import assert_same, queries, random_index
 
 pytestmark = pytest.mark.gpu
 
@@ -103,21 +103,13 @@ def _run(name):
     return got, [again, profiled], want(), launches, stage_ms
 
 
-def _same(got, want, what):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distance bits differ"
-
-
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_ivf_path(name, monkeypatch):
     for var, value in CASES[name][3].items():
         monkeypatch.setenv(var, value)
     got, repeats, want, launches, stage_ms = _run(name)
-    _same(got, want, name)
+    assert_same(got, want, name)
     for r in repeats:
-        _same(r, got, f"{name} (repeated)")
+        assert_same(r, got, f"{name} (repeated)")
     assert launches == LAUNCHES[name], (name, launches)
     assert len(stage_ms) == 7 and all(math.isfinite(t) and t >= 0 for t in stage_ms), stage_ms

@@ -26,6 +26,7 @@ if ROOT not in sys.path:
 
 from lancedb_b200 import _native  # noqa: E402
 from tests import select_oracle as so  # noqa: E402
+from tests.util import assert_same  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 NTH = min(16, os.cpu_count() or 1)
@@ -203,15 +204,6 @@ def test_searches_refuse_k_above_k_max_before_device_work():
 
 
 # ---------------------------------------------------------------- 2. every search kind against its oracle
-def _same(what, got, exp):
-    gi, gd, gc = got
-    oi, od, oc = exp
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: ids differ"
-    assert np.array_equal(np.asarray(gd, np.float32).view(np.uint32), np.asarray(od, np.float32).view(np.uint32)), \
-        f"{what}: distance bits differ"
-
-
 @pytest.fixture(scope="module")
 def pq8():
     import oracle
@@ -228,7 +220,7 @@ def test_ivf_pq(pq8, k):
     """k = 2049 and 10000 over 8 of 16 partitions, and k = 50000 above the 40000 rows of the index"""
     ix, gpu, orc, q = pq8
     np_ = 16 if k > 40000 else 8
-    _same(f"pq8 k={k}", gpu.search(q, k=k, nprobes=np_), orc.search(q, k=k, nprobes=np_, nthreads=NTH))
+    assert_same(gpu.search(q, k=k, nprobes=np_), orc.search(q, k=k, nprobes=np_, nthreads=NTH), f"pq8 k={k}")
 
 
 def test_ivf_pq_refine_range_prefilter(pq8):
@@ -236,24 +228,24 @@ def test_ivf_pq_refine_range_prefilter(pq8):
     with a limit above the rows inside it); a prefilter whose starved queries widen to maximum_nprobes"""
     import oracle
     ix, gpu, orc, q = pq8
-    _same("pq8 refine 100x30", gpu.search(q, k=100, nprobes=8, refine_factor=30),
-          orc.search(q, k=100, nprobes=8, refine_factor=30, nthreads=NTH))
-    _same("pq8 refine 3000x2", gpu.search(q, k=3000, nprobes=8, refine_factor=2),
-          orc.search(q, k=3000, nprobes=8, refine_factor=2, nthreads=NTH))
+    assert_same(gpu.search(q, k=100, nprobes=8, refine_factor=30),
+                orc.search(q, k=100, nprobes=8, refine_factor=30, nthreads=NTH), "pq8 refine 100x30")
+    assert_same(gpu.search(q, k=3000, nprobes=8, refine_factor=2),
+                orc.search(q, k=3000, nprobes=8, refine_factor=2, nthreads=NTH), "pq8 refine 3000x2")
     d = orc.search(q[:1], k=5000, nprobes=8, nthreads=NTH)[1][0]
     lo, hi = float(d[100]), float(d[4000])
     got = gpu.search(q, k=20000, nprobes=8, lower=lo, upper=hi)
-    _same("pq8 range", got, orc.search(q, k=20000, nprobes=8, lower=lo, upper=hi, nthreads=NTH))
+    assert_same(got, orc.search(q, k=20000, nprobes=8, lower=lo, upper=hi, nthreads=NTH), "pq8 range")
     assert (got[2] < 20000).all() and got[2][0] > 3000                    # everything inside the range came back
     ids = np.asarray(ix.row_ids, np.int64)
     off = np.asarray(ix.part_offsets, np.int64)
     mask = np.zeros(int(ids.max()) + 1, bool)
     mask[ids[:off[4]]] = True                                             # the rows of partitions 0..3
     bm = _native.mask_bitmap(mask)
-    _same("pq8 prefilter + widening",
-          gpu.search(q, k=3000, nprobes=1, max_nprobes=8, allow=bm, allow_bits=mask.size),
-          orc.search(q, k=3000, nprobes=1, max_nprobes=8, allow=oracle.allow_bitmap(np.nonzero(mask)[0], mask.size),
-                     allow_bits=mask.size, nthreads=NTH))
+    assert_same(gpu.search(q, k=3000, nprobes=1, max_nprobes=8, allow=bm, allow_bits=mask.size),
+                orc.search(q, k=3000, nprobes=1, max_nprobes=8,
+                           allow=oracle.allow_bitmap(np.nonzero(mask)[0], mask.size), allow_bits=mask.size,
+                           nthreads=NTH), "pq8 prefilter + widening")
 
 
 @pytest.mark.parametrize("kind", ["pq4", "sq", "rq"])
@@ -275,8 +267,9 @@ def test_other_ivf_kinds(kind):
     q = queries(rng, 8, 32)
     try:
         for k, np_, rf in ((2049, 8, 0), (10000, 8, 0), (25000, 16, 0), (100, 8, 30)):
-            _same(f"{kind} k={k} refine={rf}", gpu.search(q, k=k, nprobes=np_, refine_factor=rf),
-                  mod.search(data, q, k=k, nprobes=np_, refine_factor=rf, nthreads=NTH))
+            assert_same(gpu.search(q, k=k, nprobes=np_, refine_factor=rf),
+                        mod.search(data, q, k=k, nprobes=np_, refine_factor=rf, nthreads=NTH),
+                        f"{kind} k={k} refine={rf}")
     finally:
         gpu.close()
 
@@ -296,8 +289,8 @@ def test_flat(metric):
     fl = _native.GpuFlat(v)
     try:
         for k in (2049, 10000, 40000):
-            _same(f"flat {metric} k={k}", fl.search(q, k=k, metric=metric),
-                  oracle.flat_search(v, q, k=k, metric=metric, nthreads=NTH))
+            assert_same(fl.search(q, k=k, metric=metric),
+                        oracle.flat_search(v, q, k=k, metric=metric, nthreads=NTH), f"flat {metric} k={k}")
     finally:
         fl.close()
 
@@ -316,7 +309,7 @@ def test_binary_flat_and_ivf():
     try:
         for k, B in ((2049, 3), (10000, 130), (65536, 2)):
             q = x[rng.integers(0, 60000, B)]
-            _same(f"binary k={k} B={B}", bx.search(q, k=k), flat_search_u8(x, q, k=k, nthreads=NTH))
+            assert_same(bx.search(q, k=k), flat_search_u8(x, q, k=k, nthreads=NTH), f"binary k={k} B={B}")
     finally:
         bx.close()
     bix = ivf_binary_oracle.random_index(rng, 30000, 32, 64, patterns=50)
@@ -324,8 +317,8 @@ def test_binary_flat_and_ivf():
     q = bix.vectors[rng.integers(0, 30000, 16)]
     try:
         for k, np_, rf in ((4097, 8, 0), (4097, 8, 30)):          # refine_factor is ignored: k x 30 is not limited
-            _same(f"ivf binary k={k}", ib.search(q, k=k, nprobes=np_, refine_factor=rf),
-                  ivf_binary_oracle.search(bix, q, k=k, nprobes=np_, nthreads=NTH))
+            assert_same(ib.search(q, k=k, nprobes=np_, refine_factor=rf),
+                        ivf_binary_oracle.search(bix, q, k=k, nprobes=np_, nthreads=NTH), f"ivf binary k={k}")
     finally:
         ib.close()
 
@@ -341,8 +334,8 @@ def test_multivector():
     mv = _native.GpuMultivec(x, off)
     try:
         for k in (2049, 6000):
-            _same(f"multivector k={k}", mv.search(q, k=k, q_offsets=qoff),
-                  flat_search_mv(x, off, q, qoff, k=k, nthreads=NTH))
+            assert_same(mv.search(q, k=k, q_offsets=qoff),
+                        flat_search_mv(x, off, q, qoff, k=k, nthreads=NTH), f"multivector k={k}")
     finally:
         mv.close()
 
@@ -403,7 +396,7 @@ def test_entry_points_agree():
             co = (np.stack([o[0] for o in one]), np.stack([o[1] for o in one]),
                   np.array([o[2] for o in one], np.uint32))
             for name, got in (("filtered", filt), ("device", dev), ("async", (ai, ad, ac)), ("coalesced", co)):
-                _same(f"{name} k={k} refine={rf}", got, host)
+                assert_same(got, host, f"{name} k={k} refine={rf}")
     finally:
         gpu.close()
 

@@ -14,18 +14,11 @@ import lancedb_b200 as lancedb
 from lancedb_b200 import _native, remote
 from lancedb_b200.aio import AsyncTable
 from tests.multivec_oracle import flat_search_mv, offsets_of
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _same(got, want):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc)
-    assert np.array_equal(gi, oi)
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32))
 
 
 def _data(rng, lens, dim, qlens):
@@ -42,7 +35,7 @@ def _check(x, off, q, qoff, k, row_ids=None, allow=None, **kw):
     got = mv.search(q, k=k, q_offsets=qoff, allow=bm, allow_bits=bits, **kw)
     mv.close()
     want = flat_search_mv(x, off, q, qoff, k, row_ids=row_ids, allow=allow, nthreads=8, **kw)
-    _same(got, want)
+    assert_same(got, want)
     return got
 
 
@@ -90,7 +83,7 @@ def test_many_rows_take_the_tensor_core_path(B):
     mv = _native.GpuMultivec(x, off)
     got, st = _stats(lambda: mv.search(q, k=25, q_offsets=qoff))
     mv.close()
-    _same(got, flat_search_mv(x, off, q, qoff, 25, nthreads=8))
+    assert_same(got, flat_search_mv(x, off, q, qoff, 25, nthreads=8))
     assert st["queries"] == B and st["rescored"] < B * 100_000          # a shortlist, not every row
     assert st["candidates"] >= 25 * B and st["flagged_queries"] < B
 
@@ -104,7 +97,7 @@ def test_tensor_core_path_colbert_shape():
     mv = _native.GpuMultivec(x, off)
     got, st = _stats(lambda: mv.search(q, k=10, q_offsets=qoff))
     mv.close()
-    _same(got, flat_search_mv(x, off, q, qoff, 10, nthreads=8))
+    assert_same(got, flat_search_mv(x, off, q, qoff, 10, nthreads=8))
     assert st["rescored"] < 3 * 2000 and st["flagged_queries"] == 0
 
 
@@ -121,7 +114,7 @@ def test_near_duplicate_rows_take_the_fix_up():
     mv = _native.GpuMultivec(x, off)
     got, st = _stats(lambda: mv.search(q, k=40, q_offsets=qoff))
     mv.close()
-    _same(got, flat_search_mv(x, off, q, qoff, 40, nthreads=8))
+    assert_same(got, flat_search_mv(x, off, q, qoff, 40, nthreads=8))
     assert st["flagged_queries"] == 2 and st["candidates"] > 2 * 1024
 
 
@@ -134,10 +127,10 @@ def test_tensor_core_path_with_bad_query_vectors_and_next_call():
     q[3] = 0.0                                               # query 1: a zero vector -> no rows, via the fix-up
     mv = _native.GpuMultivec(x, off)
     got, st = _stats(lambda: mv.search(q, k=12, q_offsets=qoff))
-    _same(got, flat_search_mv(x, off, q, qoff, 12, nthreads=8))
+    assert_same(got, flat_search_mv(x, off, q, qoff, 12, nthreads=8))
     assert got[2][1] == 0 and st["flagged_queries"] == 1
     q2 = q[:3]
-    _same(mv.search(q2, k=12), flat_search_mv(x, off, q2, [0, 3], 12, nthreads=8))
+    assert_same(mv.search(q2, k=12), flat_search_mv(x, off, q2, [0, 3], 12, nthreads=8))
     mv.close()
 
 
@@ -172,7 +165,7 @@ def test_timeout_is_reported_and_the_handle_still_works():
         mv.search(q, k=10, q_offsets=qoff, timeout_ms=1, allow=_native.mask_bitmap(np.ones(20_000, bool)),
                   allow_bits=20_000)
     small = q[:2]
-    _same(mv.search(small, k=5), flat_search_mv(x, off, small, [0, 2], 5, nthreads=8))
+    assert_same(mv.search(small, k=5), flat_search_mv(x, off, small, [0, 2], 5, nthreads=8))
     mv.close()
 
 
@@ -197,11 +190,11 @@ def test_empty_null_zero_and_nan_behave_as_the_contract_says():
     q[7, 3] = np.nan                                         # query 3 holds a NaN component: no rows
     mv = _native.GpuMultivec(x, off)
     got = mv.search(q, k=30, q_offsets=qoff)
-    _same(got, flat_search_mv(x, off, q, qoff, 30))
+    assert_same(got, flat_search_mv(x, off, q, qoff, 30))
     assert got[2][1] == 0 and got[2][3] == 0 and got[2][0] == 30
     assert not np.isin(got[0][0], np.nonzero(lens == 0)[0]).any()
     nxt = mv.search(q[:1], k=30)                             # the next call still works
-    _same(nxt, flat_search_mv(x, off, q[:1], [0, 1], 30))
+    assert_same(nxt, flat_search_mv(x, off, q[:1], [0, 1], 30))
     mv.close()
 
 
@@ -237,12 +230,12 @@ def test_device_entry_point_consecutive_shapes_and_closed_handle():
     mv.search_device(dq.data_ptr(), qoff, _native.make_params(16), di.data_ptr(), dd.data_ptr(), dc.data_ptr(),
                      torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
-    _same((di.cpu().numpy().view(np.uint64), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32)), want)
+    assert_same((di.cpu().numpy().view(np.uint64), dd.cpu().numpy(), dc.cpu().numpy().view(np.uint32)), want)
     # same B, different per-query vector counts, back to back (host calls are never replayed from a graph)
     for lens in ([5, 1, 17], [1, 17, 5], [5, 1, 17], [2, 2, 2], [5, 1, 17]):
         qo = offsets_of(lens)
         qq = q[:int(qo[-1])]
-        _same(mv.search(qq, k=16, q_offsets=qo), flat_search_mv(x, off, qq, qo, 16, nthreads=8))
+        assert_same(mv.search(qq, k=16, q_offsets=qo), flat_search_mv(x, off, qq, qo, 16, nthreads=8))
     h = mv._h
     mv.close()
     qo = np.ascontiguousarray(qoff, np.uint32)
@@ -312,7 +305,7 @@ def test_default_no_tensor_core_and_small_workspace_agree(tmp_path):
     x = rng.standard_normal((int(off[-1]), 32)).astype(np.float32)
     qoff = offsets_of(rng.integers(1, 50, 12))
     q = rng.standard_normal((int(qoff[-1]), 32)).astype(np.float32)
-    _same((res["default"]["i"], res["default"]["d"], res["default"]["c"]), ref(x, off, q, qoff, 40, nthreads=8))
+    assert_same((res["default"]["i"], res["default"]["d"], res["default"]["c"]), ref(x, off, q, qoff, 40, nthreads=8))
 
 
 def test_profiling_stats():

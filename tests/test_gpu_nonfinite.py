@@ -14,7 +14,7 @@ from tests import pq4_oracle, rq_oracle, sq_oracle
 from tests.pq4_oracle import random_pq4_index
 from tests.rq_oracle import random_rq_index
 from tests.sq_oracle import random_sq_index
-from tests.util import queries, random_index
+from tests.util import assert_same, queries, random_index
 
 pytestmark = pytest.mark.gpu
 
@@ -23,14 +23,6 @@ INF = float("inf")
 # stored-row components: NaN, +inf, -inf, 2e19 (|x|^2 overflows, the row stays finite), +-FLT_MAX (bf16 rounds it to
 # inf)
 ROW_VALUES = [np.nan, INF, -INF, 2e19, FMAX, -FMAX]
-
-
-def _same(got, want, what):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ {gc} vs {oc}"
-    assert np.array_equal(gi, oi), f"{what}: ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distance bits differ"
 
 
 def _launches(fn):
@@ -84,7 +76,7 @@ def test_flat_simt_nonfinite_rows_and_queries(metric):
     X = _plant_rows(queries(rng, 3000, 12), [0, 17, 18, 400, 1999, 2998, 2999])
     X[100:140] = X[17]                                     # ties at +inf: ordered by row id
     got, want, launches, simt = _flat(X, _queries(rng, 16, 12), metric)
-    _same(got, want, f"flat simt {metric}")
+    assert_same(got, want, f"flat simt {metric}")
     assert launches == simt
 
 
@@ -96,13 +88,13 @@ def test_flat_tc_dense_nonfinite_rows_take_the_exact_kernels(metric):
     X = queries(rng, 8192, 64)
     q = _queries(rng, 16, 64)
     got, want, tc, simt = _flat(X, q, metric)
-    _same(got, want, f"flat tc dense finite {metric}")
+    assert_same(got, want, f"flat tc dense finite {metric}")
     assert (tc != simt) == (metric == "l2"), (tc, simt)         # finite l2: the tensor-core route ran
     for value in ROW_VALUES:
         Xp = X.copy()
         Xp[[5, 4000], 9] = value
         got, want, launches, simt = _flat(Xp, q, metric)
-        _same(got, want, f"flat tc dense {metric} row value {value}")
+        assert_same(got, want, f"flat tc dense {metric} row value {value}")
         assert launches == simt, (value, launches, simt)
 
 
@@ -115,7 +107,7 @@ def test_flat_tc_dense_mostly_nonfinite_column():
     q = _queries(rng, 16, 64)
     q[:, 0] = 0.0                                          # 0 * inf = NaN scores, exact distance +inf
     got, want, launches, simt = _flat(X, q, "l2", k=100)   # 92 finite rows, then the inf rows by id
-    _same(got, want, "flat tc dense, 8100 inf rows")
+    assert_same(got, want, "flat tc dense, 8100 inf rows")
     assert launches == simt
 
 
@@ -126,7 +118,7 @@ def test_flat_tc_nonfinite_queries_take_the_fixup():
         X = queries(rng, N, d)
         q = _queries(rng, 16, d)
         got, want, launches, simt = _flat(X, q, "l2")
-        _same(got, want, f"flat tc N={N} non-finite queries")
+        assert_same(got, want, f"flat tc N={N} non-finite queries")
         finite = _flat(X, queries(rng, 16, d), "l2")
         assert launches == finite[2] != simt
 
@@ -144,7 +136,7 @@ def test_flat_tc_filtered_one_inf_row(where):
     q[10] = 0.0
     q[11] = 2.0
     got, want, launches, simt = _flat(X, q, "l2")
-    _same(got, want, f"flat tc filtered, non-finite rows in {where}")
+    assert_same(got, want, f"flat tc filtered, non-finite rows in {where}")
     assert launches == simt
 
 
@@ -156,7 +148,7 @@ def test_flat_distance_range_with_infinite_bounds():
     q = _queries(rng, 16, 12)
     for lower, upper in ((-INF, INF), (-INF, None), (None, INF), (0.5, INF), (INF, None), (-INF, -INF)):
         got, want, _, _ = _flat(X, q, "l2", k=20, lower=lower, upper=upper)
-        _same(got, want, f"flat range [{lower}, {upper})")
+        assert_same(got, want, f"flat range [{lower}, {upper})")
 
 
 def test_flat_finite_launch_counts_are_unchanged():
@@ -166,7 +158,7 @@ def test_flat_finite_launch_counts_are_unchanged():
     for N, d in ((8192, 64), (262144, 16)):
         X = queries(rng, N, d)
         got, want, tc, simt = _flat(X, queries(rng, 16, d), "l2")
-        _same(got, want, f"flat finite N={N}")
+        assert_same(got, want, f"flat finite N={N}")
         counts += [tc, simt]
     assert counts == FLAT_LAUNCHES, counts
 
@@ -227,7 +219,7 @@ def _pq_case(ix, q, scan, route, monkeypatch, what, **kw):
     exact scan's on the same request), "exact" (the exact scan's count) or "small" (at most SMALL_MAX_LAUNCHES)"""
     B, env = SCANS[scan]
     got, want, launches = _pq_search(ix, q, env, monkeypatch, **kw)
-    _same(got, want, what)
+    assert_same(got, want, what)
     exact = _pq_search(ix, q, SCANS["exact"][1], monkeypatch, **kw)[2]
     if route == "small":
         assert launches <= SMALL_MAX_LAUNCHES, (what, launches)
@@ -307,7 +299,7 @@ def test_ivf_pq4_nonfinite_centroids_and_queries(metric, monkeypatch):
     _plant_centroids(ix)
     for kw, n in zip(KWS, finite):
         got, want, launches = _pq_search(ix, q, {}, monkeypatch, **kw)
-        _same(got, want, f"4-bit IVF_PQ {metric} {kw}")
+        assert_same(got, want, f"4-bit IVF_PQ {metric} {kw}")
         assert launches == n, (kw, launches, n)
 
 
@@ -326,10 +318,10 @@ def test_ivf_tc_coarse_nonfinite(metric, variant, monkeypatch):
     kw = dict(k=10, nprobes=20)
     q = _queries(rng, B, 64)
     got, want, launches = _pq_search(ix, q, env, monkeypatch, **kw)
-    _same(got, want, f"tc coarse {variant} {metric}, non-finite queries")
+    assert_same(got, want, f"tc coarse {variant} {metric}, non-finite queries")
     finite = _pq_search(ix, queries(rng, B, 64), env, monkeypatch, **kw)
     exact = _pq_search(ix, queries(rng, B, 64), {}, monkeypatch, **kw)
-    _same(*finite[:2], "finite control")
+    assert_same(*finite[:2], "finite control")
     assert launches == finite[2] != exact[2], (launches, finite[2], exact[2])     # the tensor-core coarse step ran
     base = ix.centroids.copy()
     for plant in ("nonfinite", "overflow"):
@@ -339,7 +331,7 @@ def test_ivf_tc_coarse_nonfinite(metric, variant, monkeypatch):
         else:
             ix.centroids[11, 7] = 2e19
         got, want, launches = _pq_search(ix, q, env, monkeypatch, **kw)
-        _same(got, want, f"tc coarse {variant} {metric}, {plant} centroids")
+        assert_same(got, want, f"tc coarse {variant} {metric}, {plant} centroids")
         assert launches == _pq_search(ix, q, {}, monkeypatch, **kw)[2], plant     # the exact coarse kernels
 
 
@@ -376,7 +368,7 @@ def test_ivf_pq_widening_after_nan_probes(monkeypatch):
     for name, kw in (("narrow", dict(nprobes=2)), ("widened", dict(nprobes=2, max_nprobes=32)),
                      ("all", dict(nprobes=32))):
         got, want, launches[name] = _pq_search(ix, q, {}, monkeypatch, k=10, allow=allow, allow_bits=n, **kw)
-        _same(got, want, f"widening {kw}")
+        assert_same(got, want, f"widening {kw}")
     assert launches["widened"] > launches["narrow"], launches
 
 
@@ -390,7 +382,7 @@ def test_inf_query_is_answered_as_the_oracle_answers_it(metric, monkeypatch):
     q[4, :] = INF
     q[5, :] = -INF
     got, want, _ = _pq_search(ix, q, {}, monkeypatch, k=5, nprobes=4)
-    _same(got, want, f"inf query {metric}")
+    assert_same(got, want, f"inf query {metric}")
     if metric == "l2":
         assert got[2][4] == 5 and np.all(np.isposinf(got[1][4]))
 
@@ -399,11 +391,11 @@ def test_ivf_finite_launch_counts_are_unchanged(monkeypatch):
     rng = np.random.default_rng(515)
     ix = _pq_index("l2", rng)
     got, want, launches = _pq_search(ix, queries(rng, 64, ix.dim), {}, monkeypatch, k=10, nprobes=8)
-    _same(got, want, "finite IVF_PQ")
+    assert_same(got, want, "finite IVF_PQ")
     assert launches == IVF_PQ_LAUNCHES, launches
     six = random_sq_index(rng, n=8000, dim=48, nlist=32)
     got, want, launches = _sq_search(six, queries(rng, 40, 48), k=10, nprobes=4)
-    _same(got, want, "finite IVF_SQ")
+    assert_same(got, want, "finite IVF_SQ")
     assert launches == IVF_SQ_LAUNCHES, launches
 
 
@@ -441,7 +433,7 @@ def test_ivf_sq_rq_nonfinite(kind, metric):
         ix.vectors[r, i % ix.dim] = ROW_VALUES[i % len(ROW_VALUES)]
     for kw, n in zip(kws, finite):                         # the kind's scan, as on the finite index
         got, want, launches = search(ix, q, **kw)
-        _same(got, want, f"IVF_{kind.upper()} {metric} {kw}")
+        assert_same(got, want, f"IVF_{kind.upper()} {metric} {kw}")
         assert launches == n, (kw, launches, n)
 
 
@@ -475,14 +467,14 @@ def test_multivector_nonfinite_stored_vectors():
     q = rng.standard_normal((int(qoff[-1]), 48)).astype(np.float32)
     rows = lens.size
     got, want, st = _mv(x, off, q, qoff)
-    _same(got, want, "multivector, finite")
+    assert_same(got, want, "multivector, finite")
     assert st["rescored"] < 3 * rows, st                    # the tensor-core shortlist ran
     near = int(off[int(np.argmax(lens > 0))])               # a vector of the first non-empty row, and one far on
     for value in [INF, -INF, FMAX, -FMAX, 2e19]:
         xp = x.copy()
         xp[[near, x.shape[0] - 3], 5] = value
         got, want, st = _mv(xp, off, q, qoff, k=30)
-        _same(got, want, f"multivector, stored component {value}")
+        assert_same(got, want, f"multivector, stored component {value}")
         assert st["rescored"] == 3 * rows, (value, st)      # the exact kernels scored every row
 
 

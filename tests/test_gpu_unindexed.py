@@ -13,6 +13,7 @@ import pytest
 import lancedb_b200 as lancedb
 from lancedb_b200 import _native
 from tests import hamming_oracle, unindexed_oracle as U
+from tests.util import assert_same
 
 pytestmark = pytest.mark.gpu
 f32 = np.float32
@@ -28,16 +29,6 @@ KINDS = [
     ("IVF_RQ", dict(num_bits=1), "cosine"),
     ("IVF_FLAT", dict(), "hamming"),
 ]
-
-
-def _same(got, want, what=""):
-    gi, gd, gc = got
-    oi, od, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    for i in range(len(gc)):
-        n = int(gc[i])
-        assert np.array_equal(gi[i, :n], oi[i, :n]), f"{what}: ids differ (query {i})"
-        assert np.array_equal(gd[i, :n].view(np.uint32), od[i, :n].view(np.uint32)), f"{what}: distances differ ({i})"
 
 
 def _rows(rng, kind, n):
@@ -75,7 +66,7 @@ def _check(t, q, what, k=10, nprobes=3, refine_factor=0, lower=None, upper=None,
                   allow_mask=mask, max_nprobes=max_nprobes)
     want = U.union_search(t._index_data["vector"], tail, tid, q, k, nprobes, refine_factor, lower, upper, mask,
                           max_nprobes if mask is not None else 0)
-    _same(got, want, what)
+    assert_same(got, want, what, prefix=True)
 
 
 @pytest.mark.parametrize("kind,params,metric", KINDS, ids=[f"{k}-{m}-{p.get('num_bits', '')}" for k, p, m in KINDS])
@@ -86,14 +77,14 @@ def test_union_search_matches_the_oracle_as_the_tail_grows(kind, params, metric)
     index_only = _search(t, q)
     t.add({"vector": _rows(rng, kind, 0)})                # nothing added: no tail, today's call
     assert "vector" not in t._tail
-    _same(_search(t, q), index_only, "empty add")
+    assert_same(_search(t, q), index_only, "empty add", prefix=True)
     for n, what in ((1, "1"), (4094, "4095"), (1, "4096"), (15904, "20000")):
         t.add({"vector": _rows(rng, kind, n)})
         _check(t, q, f"tail {what}")
     assert t.index_stats("vector_idx")["num_unindexed_rows"] == 20000
     # fast_search: the index alone, exactly today's call
     data = t._index_data["vector"]
-    _same(_search(t, q, fast_search=True), U.index_search(data, q, 10, 3), "fast_search")
+    assert_same(_search(t, q, fast_search=True), U.index_search(data, q, 10, 3), "fast_search", prefix=True)
     big_k = kind != "IVF_HNSW_SQ"                         # IVF_HNSW_SQ keeps k x refine_factor <= 2048
     if big_k:
         _check(t, q, "k 2049", k=2049)
@@ -123,16 +114,17 @@ def test_union_search_matches_the_oracle_as_the_tail_grows(kind, params, metric)
     torch.cuda.synchronize()
     got = (ids.cpu().numpy().view(np.uint64), dist.cpu().numpy(), cnt.cpu().numpy().view(np.uint32))
     tail, tid = _tail(t)
-    _same(got, U.union_search(data, tail, tid, q, 10, 3, allow=mask), "device route")
+    assert_same(got, U.union_search(data, tail, tid, q, 10, 3, allow=mask), "device route", prefix=True)
     # optimize: the tail is folded into the index without retraining
     t.optimize()
     st = t.index_stats("vector_idx")
     assert (st["num_indexed_rows"], st["num_unindexed_rows"]) == (n, 0) and "vector" not in t._tail
     ext = t._index_data["vector"]
     assert np.array_equal(np.sort(ext.row_ids), np.arange(n, dtype=np.uint64))
-    _same(_search(t, q), U.index_search(ext, q, 10, 3), "after optimize")
+    assert_same(_search(t, q), U.index_search(ext, q, 10, 3), "after optimize", prefix=True)
     if big_k:
-        _same(_search(t, q, k=2049, nprobes=5), U.index_search(ext, q, 2049, 5), "after optimize, k 2049")
+        assert_same(_search(t, q, k=2049, nprobes=5), U.index_search(ext, q, 2049, 5),
+                    "after optimize, k 2049", prefix=True)
 
 
 def test_union_with_non_finite_tail_rows():
@@ -153,8 +145,8 @@ def test_union_with_non_finite_tail_rows():
     q[0] = tail[12]
     data, ix = t._index_data["vector"], t._index["vector"]
     for k in (10, 2049):
-        _same(ix.search_unindexed(fl, q, k=k, nprobes=3), U.union_search(data, tail, ids, q, k, 3),
-              f"non-finite tail, k {k}")
+        assert_same(ix.search_unindexed(fl, q, k=k, nprobes=3), U.union_search(data, tail, ids, q, k, 3),
+                    f"non-finite tail, k {k}", prefix=True)
     fl.close()
 
 
@@ -167,11 +159,12 @@ def test_host_union_honours_timeout_ms():
     bm = _native.mask_bitmap(np.ones(N0 + n, bool))
     q = _rows(rng, "IVF_PQ", 4096)
     want = ix.search_unindexed(fl, q[:256], k=10, nprobes=3, allow=bm, allow_bits=N0 + n)
-    _same(ix.search_unindexed(fl, q[:256], k=10, nprobes=3, allow=bm, allow_bits=N0 + n, timeout_ms=60000), want,
-          "generous timeout")
+    assert_same(ix.search_unindexed(fl, q[:256], k=10, nprobes=3, allow=bm, allow_bits=N0 + n, timeout_ms=60000), want,
+                "generous timeout", prefix=True)
     with pytest.raises(TimeoutError, match="timeout"):       # 4096 x 300k exact distances cannot finish in 1 ms
         ix.search_unindexed(fl, q, k=10, nprobes=3, allow=bm, allow_bits=N0 + n, timeout_ms=1)
-    _same(ix.search_unindexed(fl, q[:256], k=10, nprobes=3, allow=bm, allow_bits=N0 + n), want, "after the timeout")
+    assert_same(ix.search_unindexed(fl, q[:256], k=10, nprobes=3, allow=bm, allow_bits=N0 + n), want,
+                "after the timeout", prefix=True)
     fl.close()
 
 
@@ -242,14 +235,17 @@ def test_appended_flat_equals_flat_opened_on_the_concatenation(cuts, nan):
     bm = _native.mask_bitmap(mask)
     for metric in ("l2", "cosine", "dot"):
         for k in (10, 2049):
-            _same(grown.search(q, k=k, metric=metric), whole.search(q, k=k, metric=metric), f"{metric} k {k}")
-        _same(grown.search(q, k=10, metric=metric, allow=bm, allow_bits=mask.size),
-              whole.search(q, k=10, metric=metric, allow=bm, allow_bits=mask.size), f"{metric} filtered")
-    _same(grown.search(q, k=10), oracle.flat_search(x, q, k=10, row_ids=ids, nthreads=0), "l2 oracle")
+            assert_same(grown.search(q, k=k, metric=metric), whole.search(q, k=k, metric=metric),
+                        f"{metric} k {k}", prefix=True)
+        assert_same(grown.search(q, k=10, metric=metric, allow=bm, allow_bits=mask.size),
+                    whole.search(q, k=10, metric=metric, allow=bm, allow_bits=mask.size),
+                    f"{metric} filtered", prefix=True)
+    assert_same(grown.search(q, k=10), oracle.flat_search(x, q, k=10, row_ids=ids, nthreads=0),
+                "l2 oracle", prefix=True)
     # positions continue when no ids are given
     pos = _native.GpuFlat(x[:7])
     pos.append(x[7:n])
-    _same(pos.search(q, k=10), _native.GpuFlat(x).search(q, k=10), "positions")
+    assert_same(pos.search(q, k=10), _native.GpuFlat(x).search(q, k=10), "positions", prefix=True)
 
 
 @pytest.mark.parametrize("cuts", [(100, 65436, 5000), (70000, 3)])
@@ -269,8 +265,8 @@ def test_appended_binary_equals_binary_opened_on_the_concatenation(cuts):
         a += c
     for k in (10, 2049):
         got = grown.search(q, k=k)
-        _same(got, whole.search(q, k=k), f"k {k}")
-        _same(got, hamming_oracle.flat_search_u8(x, q, k, row_ids=ids), f"oracle k {k}")
+        assert_same(got, whole.search(q, k=k), f"k {k}", prefix=True)
+        assert_same(got, hamming_oracle.flat_search_u8(x, q, k, row_ids=ids), f"oracle k {k}", prefix=True)
 
 
 if __name__ == "__main__" and sys.argv[1:] == ["sub_batches"]:

@@ -7,14 +7,9 @@ import pytest
 from lancedb_b200.index import HNSW_NONE, IvfHnswSqIndexData, build_hnsw_graph
 from tests import hnsw_sq_oracle as H
 from tests import sq_oracle
+from tests.util import assert_same
 
 f32 = np.float32
-
-
-def _same(a, b, what=""):
-    assert np.array_equal(a[2], b[2]), f"{what}: counts differ"
-    assert np.array_equal(a[0], b[0]), f"{what}: ids differ"
-    assert np.array_equal(a[1].view(np.uint32), b[1].view(np.uint32)), f"{what}: distance bits differ"
 
 
 _IX = {}
@@ -39,7 +34,7 @@ def test_c_oracle_equals_the_numpy_mirror(metric, case):
     q = np.random.default_rng(case).standard_normal((9, data.dim)).astype(f32)
     q[1] = data.vectors[5]                                   # a row with duplicates: ties by position, then row id
     kw = CASES[case]
-    _same(H.search(data, q, nthreads=2, **kw), H.search_np(data, q, **kw), str(kw))
+    assert_same(H.search(data, q, nthreads=2, **kw), H.search_np(data, q, **kw), str(kw))
 
 
 def test_prefilter_with_widening_c_equals_numpy():
@@ -48,7 +43,7 @@ def test_prefilter_with_widening_c_equals_numpy():
     q = rng.standard_normal((8, data.dim)).astype(f32)
     mask = rng.random(int(data.row_ids.max()) + 1) < 0.04
     for kw in (dict(k=10, nprobes=1, max_nprobes=6), dict(k=10, nprobes=2, max_nprobes=4, ef=25)):
-        _same(H.search(data, q, allow=mask, **kw), H.search_np(data, q, allow=mask, **kw), str(kw))
+        assert_same(H.search(data, q, allow=mask, **kw), H.search_np(data, q, allow=mask, **kw), str(kw))
 
 
 def test_empty_and_single_row_partitions():
@@ -63,7 +58,7 @@ def test_empty_and_single_row_partitions():
     data.validate()
     q = rng.standard_normal((5, 8)).astype(f32)
     for kw in (dict(k=3, nprobes=4), dict(k=10, nprobes=4, ef=2)):
-        _same(H.search(data, q, **kw), H.search_np(data, q, **kw), str(kw))
+        assert_same(H.search(data, q, **kw), H.search_np(data, q, **kw), str(kw))
 
 
 def _random_graph(rng, n, deg):
@@ -96,7 +91,7 @@ def test_complete_graph_returns_ivf_sq_results():
     q = np.random.default_rng(6).standard_normal((10, data.dim)).astype(f32)
     big = int(np.diff(data.part_offsets.astype(np.int64)).max())
     for kw in (dict(k=10, nprobes=6), dict(k=5, nprobes=3, refine_factor=2)):
-        _same(H.search(full, q, ef=big, **kw), sq_oracle.search(data.sq, q, **kw), str(kw))
+        assert_same(H.search(full, q, ef=big, **kw), sq_oracle.search(data.sq, q, **kw), str(kw))
 
 
 def test_ef_prime_above_2048_is_refused_by_the_oracle():

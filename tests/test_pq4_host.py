@@ -5,12 +5,12 @@ import numpy as np
 import pytest
 
 import lancedb_b200 as lancedb
-from lancedb_b200 import _native
 from oracle import oracle_np as onp
 from lancedb_b200.index import (IvfPqIndexData, get_num_sub_vectors, pack_pq4, suggested_num_sub_vectors,
                                 train_ivf_pq, unpack_pq4)
 from tests import pq4_oracle
 from tests.pq4_oracle import random_pq4_index
+from tests.util import record_opens
 
 f32 = np.float32
 
@@ -217,32 +217,15 @@ def test_shard_and_partition_codes_use_the_row_byte_width():
     assert sum(s.nrows for s in parts) == 300
 
 
-class _StubPq:
-    """Stands in for _native.GpuIvfPq: records the arrays it was opened with."""
-    opened = []
-
-    def __init__(self, data, device=0):
-        self.data, self.metric = data, data.metric
-        _StubPq.opened.append(data)
-
-    def close(self):
-        pass
-
-
-@pytest.fixture
-def stub(monkeypatch):
-    _StubPq.opened = []
-    monkeypatch.setattr(_native, "GpuIvfPq", _StubPq)
-    return _StubPq
-
-
-def test_create_index_num_bits_4_builds_and_rejections(stub):
+def test_create_index_num_bits_4_builds_and_rejections(monkeypatch):
+    opened = record_opens(monkeypatch)
     rng = np.random.default_rng(12)
     db = lancedb.connect("memory://")
     t = db.create_table("t", {"vector": rng.standard_normal((400, 24)).astype(f32), "id": np.arange(400)})
     t.create_index(metric="l2", num_partitions=4, num_bits=4, max_iterations=2)
-    assert len(stub.opened) == 1 and isinstance(stub.opened[0], IvfPqIndexData)
-    assert stub.opened[0].num_bits == 4 and stub.opened[0].m == 4 and stub.opened[0].vectors is not None
+    assert [name for name, _ in opened] == ["GpuIvfPq"]
+    data = opened[0][1]
+    assert isinstance(data, IvfPqIndexData) and data.num_bits == 4 and data.m == 4 and data.vectors is not None
     assert t.list_indices() == [{"name": "vector_idx", "index_type": "IVF_PQ", "columns": ["vector"]}]
     with pytest.raises(NotImplementedError, match="8-bit"):
         t.save_lance_index("/nonexistent")
@@ -251,4 +234,4 @@ def test_create_index_num_bits_4_builds_and_rejections(stub):
             t.create_index(num_bits=nb)
     with pytest.raises(ValueError, match="even"):
         t.create_index(num_bits=4, num_sub_vectors=3, num_partitions=4)
-    assert len(stub.opened) == 1
+    assert len(opened) == 1

@@ -1,6 +1,7 @@
 """IVF_RQ without a GPU: the C oracle against its NumPy mirror (rotation, slot grid, estimates, whole searches), edge
-cases of the grid, the estimator's algebra and bias, the trainer's invariants, and the Python surface of
-create_index(index_type="IVF_RQ") against a stubbed native layer."""
+cases of the grid, the estimator's algebra and bias, the trainer's invariants, and the refusals of
+create_index(index_type="IVF_RQ") and its aio config against a stubbed native layer.  The build through create_index
+is in test_ivf_kinds_host.py."""
 import asyncio
 
 import numpy as np
@@ -8,10 +9,10 @@ import pyarrow as pa
 import pytest
 
 import lancedb_b200 as lancedb
-from lancedb_b200 import _native
-from lancedb_b200.index import IvfRqIndexData, rq_encode, rq_rotation, train_ivf_rq
+from lancedb_b200.index import rq_encode, rq_rotation, train_ivf_rq
 from tests import rq_oracle
 from tests.rq_oracle import random_rq_index, rq_estimates_np, rq_rotate_np, rq_slot_np
+from tests.util import record_opens
 
 f32 = np.float32
 
@@ -187,40 +188,8 @@ def test_trainer_invariants(metric):
         train_ivf_rq(x, num_partitions=4, num_bits=2)
 
 
-class _StubRq:
-    """Stands in for _native.GpuIvfRq: records the arrays it was opened with."""
-    opened = []
-
-    def __init__(self, data, device=0):
-        self.data, self.metric = data, data.metric
-        _StubRq.opened.append(data)
-
-    def close(self):
-        pass
-
-
-@pytest.fixture
-def stub(monkeypatch):
-    _StubRq.opened = []
-    monkeypatch.setattr(_native, "GpuIvfRq", _StubRq)
-    return _StubRq
-
-
-def test_create_index_ivf_rq_builds_and_lists(stub):
-    rng = np.random.default_rng(15)
-    db = lancedb.connect("memory://")
-    t = db.create_table("t", {"vector": rng.standard_normal((400, 16)).astype(f32), "id": np.arange(400)})
-    t.create_index(metric="cosine", num_partitions=4, index_type="IVF_RQ", num_bits=1, max_iterations=2)
-    assert len(stub.opened) == 1 and isinstance(stub.opened[0], IvfRqIndexData)
-    assert stub.opened[0].metric == "cosine" and stub.opened[0].vectors is not None
-    assert t.list_indices() == [{"name": "vector_idx", "index_type": "IVF_RQ", "columns": ["vector"]}]
-    st = t.index_stats("vector_idx")
-    assert st["index_type"] == "IVF_RQ" and st["distance_type"] == "cosine" and st["num_indexed_rows"] == 400
-    with pytest.raises(NotImplementedError, match="IVF_PQ"):
-        t.save_lance_index("/nonexistent")
-
-
-def test_create_index_ivf_rq_rejections(stub):
+def test_create_index_ivf_rq_rejections(monkeypatch):
+    opened = record_opens(monkeypatch)
     rng = np.random.default_rng(16)
     db = lancedb.connect("memory://")
     t = db.create_table("t", {"vector": rng.standard_normal((300, 8)).astype(f32)})
@@ -244,10 +213,11 @@ def test_create_index_ivf_rq_rejections(stub):
     tm = db.create_table("m", pa.table({"mv": mv}))
     with pytest.raises(NotImplementedError, match="multivector"):
         tm.create_index(index_type="IVF_RQ", num_bits=1)
-    assert stub.opened == []
+    assert opened == []
 
 
-def test_async_create_index_with_ivf_rq_config(stub):
+def test_async_create_index_with_ivf_rq_config(monkeypatch):
+    opened = record_opens(monkeypatch)
     rng = np.random.default_rng(17)
 
     async def run():
@@ -261,4 +231,5 @@ def test_async_create_index_with_ivf_rq_config(stub):
         return await t.list_indices()
 
     assert asyncio.run(run())[0]["index_type"] == "IVF_RQ"
-    assert len(stub.opened) == 1 and stub.opened[0].metric == "cosine" and stub.opened[0].nlist == 3
+    assert [name for name, _ in opened] == ["GpuIvfRq"]
+    assert opened[0][1].metric == "cosine" and opened[0][1].nlist == 3

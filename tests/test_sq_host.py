@@ -1,15 +1,15 @@
 """IVF_SQ without a GPU: the C oracle against its NumPy mirror, the quantiser at and around its code boundaries, the
-integer distance above 2^24, ties, the trainer, and the Python surface of create_index(index_type="IVF_SQ") against a
-stubbed native layer."""
+integer distance above 2^24, ties, the trainer, and the refusals of create_index(index_type="IVF_SQ") against a stubbed
+native layer.  The build through create_index is in test_ivf_kinds_host.py."""
 import numpy as np
 import pyarrow as pa
 import pytest
 
 import lancedb_b200 as lancedb
-from lancedb_b200 import _native
-from lancedb_b200.index import IvfSqIndexData, sq_encode, train_ivf_sq
+from lancedb_b200.index import sq_encode, train_ivf_sq
 from tests import sq_oracle
 from tests.sq_oracle import random_sq_index
+from tests.util import record_opens
 
 f32 = np.float32
 
@@ -112,40 +112,8 @@ def test_trainer_encodes_rows_with_the_sample_bounds(metric):
         train_ivf_sq(x, num_partitions=4, distance_type="dot")
 
 
-class _StubSq:
-    """Stands in for _native.GpuIvfSq: records the arrays it was opened with."""
-    opened = []
-
-    def __init__(self, data, device=0):
-        self.data, self.metric = data, data.metric
-        _StubSq.opened.append(data)
-
-    def close(self):
-        pass
-
-
-@pytest.fixture
-def stub(monkeypatch):
-    _StubSq.opened = []
-    monkeypatch.setattr(_native, "GpuIvfSq", _StubSq)
-    return _StubSq
-
-
-def test_create_index_ivf_sq_builds_and_lists(stub):
-    rng = np.random.default_rng(6)
-    db = lancedb.connect("memory://")
-    t = db.create_table("t", {"vector": rng.standard_normal((400, 16)).astype(f32), "id": np.arange(400)})
-    t.create_index(metric="cosine", num_partitions=4, index_type="IVF_SQ", max_iterations=2)
-    assert len(stub.opened) == 1 and isinstance(stub.opened[0], IvfSqIndexData)
-    assert stub.opened[0].metric == "cosine" and stub.opened[0].vectors is not None
-    assert t.list_indices() == [{"name": "vector_idx", "index_type": "IVF_SQ", "columns": ["vector"]}]
-    st = t.index_stats("vector_idx")
-    assert st["index_type"] == "IVF_SQ" and st["distance_type"] == "cosine" and st["num_indexed_rows"] == 400
-    with pytest.raises(NotImplementedError, match="IVF_PQ"):
-        t.save_lance_index("/nonexistent")
-
-
-def test_create_index_ivf_sq_rejections(stub):
+def test_create_index_ivf_sq_rejections(monkeypatch):
+    opened = record_opens(monkeypatch)
     rng = np.random.default_rng(7)
     db = lancedb.connect("memory://")
     t = db.create_table("t", {"vector": rng.standard_normal((300, 8)).astype(f32)})
@@ -164,4 +132,4 @@ def test_create_index_ivf_sq_rejections(stub):
     tm = db.create_table("m", pa.table({"mv": mv}))
     with pytest.raises(NotImplementedError, match="multivector"):
         tm.create_index(index_type="IVF_SQ")
-    assert stub.opened == []
+    assert opened == []

@@ -5,7 +5,8 @@ tests shape edge cases (empty, tiny and multi-tile partitions)."""
 import numpy as np
 
 import oracle
-from lancedb_b200.index import IvfPqIndexData
+from lancedb_b200 import _native
+from lancedb_b200.index import IVF_KINDS, IvfPqIndexData
 
 
 def random_index(rng, *, dim, nlist, m, metric="l2", sizes=None, n=None, with_vectors=False, scale=1.0,
@@ -142,6 +143,46 @@ def same_result(got, want):
     return (np.array_equal(gc, wc) and np.array_equal(gi, wi)
             and np.array_equal(np.asarray(gd, np.float32).view(np.uint32), np.asarray(wd, np.float32).view(np.uint32)))
 
+
+def assert_same(got, want, what="", prefix=False):
+    """Asserts that two search results (ids, dist, count) have equal counts, then equal ids, then equal f32 distance
+    bits, naming the field that differs.  prefix: compare only the first count[i] entries of each row i."""
+    gi, gd, gc = got
+    wi, wd, wc = want
+    assert np.array_equal(gc, wc), f"{what}: counts differ"
+    gd, wd = np.asarray(gd, np.float32).view(np.uint32), np.asarray(wd, np.float32).view(np.uint32)
+    if not prefix:
+        assert np.array_equal(gi, wi), f"{what}: ids differ"
+        assert np.array_equal(gd, wd), f"{what}: distance bits differ"
+        return
+    for i, n in enumerate(np.asarray(gc, np.int64)):
+        assert np.array_equal(gi[i, :n], wi[i, :n]), f"{what}: ids differ (query {i})"
+        assert np.array_equal(gd[i, :n], wd[i, :n]), f"{what}: distance bits differ (query {i})"
+
+
+
+def ivf_queries(rng, ix, B, far):
+    """B normal queries for the index ix; from B = 4 on, awkward ones: query 1 scaled by `far`, query 2 with a NaN (no
+    finite centroid distance: no rows) and, when ix keeps its vectors, query 3 equal to stored row 7 (and its
+    duplicates)"""
+    q = rng.standard_normal((B, ix.dim)).astype(np.float32)
+    if B > 3:
+        q[1] *= far
+        q[2, 0] = np.nan
+        if ix.vectors is not None:
+            q[3] = ix.vectors[7]
+    return q
+
+
+def record_opens(monkeypatch):
+    """Replaces every IVF handle class of _native with a stub that records (its class name, the data it was opened
+    with).  Returns the record."""
+    log = []
+    for name in sorted({kind.handle for kind in IVF_KINDS.values()}):
+        def init(self, data, device=0, _name=name):
+            log.append((_name, data))
+        monkeypatch.setattr(_native, name, type(name, (), {"__init__": init, "close": lambda self: None}))
+    return log
 
 # ---- the filter scan's arithmetic (tables.cu + scan3.cu), restated bit for bit for CPU checks of its band ----
 def fmaf(a, b, c):
