@@ -31,6 +31,11 @@
 //   scanners: thread = rows row0 + ct + 256 r (r < 6); the skewed code stream (retile.cu) makes the eight lanes of
 //             a quarter-warp read eight different sub-space slots, so every LDS.128 is conflict-free whatever the
 //             codes are; accumulators are 4 x u32 per row (8 queries x u16).
+//   candidate epilogue (k <= 32): the scanners keep the tile's last data buffer after the zero stage, park the sums
+//             in it ([8 queries][1536 rows] u16 + the row terms) behind two scanner barriers, and warp g then runs
+//             query g alone with warp reductions; each warp hands the buffer back when its query is done.  The
+//             stagers need it for the next tile's chunk 1 only (tests/test_scan3_epilogue_protocol.py).  k > 32 keeps
+//             the block-wide epilogue, one query after the other, because of its list tightening.
 // Algorithmic bytes per tile row and query: m code bytes (SURVEY.md 8d), as for the exact kernel.
 #include "kernels.cuh"
 #include "scan_common.cuh"
@@ -69,6 +74,10 @@ constexpr int BAR_SCAN = 8;                         // named barrier of the 256 
 constexpr size_t S3_MBAR_OFF = S3_TILES + S3_SLOTS * S3_SLOT_BYTES + 2 * S3_SCR * 4;   // 3 x 8 bytes, 8-byte aligned
 constexpr size_t S3_QS_OFF = S3_MBAR_OFF + 32;     // [SCAN_G][step, cst, slack, -] f32
 static_assert(S3_QS_OFF + SCAN_G * 16 == S3_SMEM, "shared-memory layout");
+// The k <= 32 candidate epilogue parks the tile's sums in the chunk buffer its last data stage used:
+// [SCAN_G queries][SCAN3_ROWS_TILE rows] u16, then the row terms R(row) as [SCAN3_ROWS_TILE] f32.
+constexpr int S3_SUMS_BYTES = SCAN_G * SCAN3_ROWS_TILE * 2;
+static_assert(S3_SUMS_BYTES + SCAN3_ROWS_TILE * 4 <= S3_BUF, "sum area inside one chunk buffer");
 static_assert(SCAN3_ROWS_TILE == S3_CT * S3_RMAX, "rows_tile");
 static_assert(S3_PT == 256, "one stager thread per code");
 
@@ -107,6 +116,21 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
         "DONE_%=:\n\t"
         "}" ::"r"(bar), "r"(parity) : "memory");
 }
+__device__ __forceinline__ uint2 lds64u(uint32_t addr)
+{
+    uint2 v;
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ float4 lds128f(uint32_t addr)
+{
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+    return v;
+}
+// (float) of the low / high u16 of w: 2^23 + s built by one PRMT, minus 2^23 -- exact, and full-rate unlike I2F
+__device__ __forceinline__ float u16lo_f32(uint32_t w) { return __uint_as_float(__byte_perm(w, 0x4b00u, 0x5410)) - 8388608.f; }
+__device__ __forceinline__ float u16hi_f32(uint32_t w) { return __uint_as_float(__byte_perm(w, 0x4b00u, 0x5432)) - 8388608.f; }
 __device__ __forceinline__ uint32_t word_of(const uint4 &v, int w)
 {
     return w == 0 ? v.x : (w == 1 ? v.y : (w == 2 ? v.z : v.w));
@@ -252,6 +276,179 @@ __device__ __noinline__ uint32_t tighten_from_list(const uint32_t *keys, uint32_
     return tkey;
 }
 
+// ---- candidate epilogue for k <= 32: one warp per query, on sums parked in the last data buffer.
+// tau_q (global, atomicMin) is any value such that at least k rows of the query have L <= tau_q: then the k-th
+// smallest exact distance is <= tau_q + W + E and every row of the exact top-k has L <= tau_q + W + 2E =
+// tau_q + slack_q.  A tile tightens tau_q from its own rows (an upper bound of their k-th smallest L, by 8 counting
+// bisections) when the query has no threshold yet or when this is one of its three nearest partitions -- that is where
+// the small distances are -- and otherwise only when the tile alone holds 2k or more rows under the current threshold
+// (without that a loose early threshold, set by whichever far partition happened to finish first, would let whole
+// near partitions through); then it appends the rows under the threshold.
+// The scanners hold the sums in registers, one row per thread and eight queries per row.  They write them to the sum
+// area behind one scanner barrier (every warp has read the buffer) and read them back behind a second one, so that
+// warp g handles query g alone: its counts are warp reductions, and the only block barriers of the epilogue are those
+// two.  The buffer goes back to the stagers when every warp is done with its query; the stagers need it for the next
+// tile's chunk 1 only, which no scanner can use before then.  tests/test_scan3_epilogue_protocol.py models the hold.
+// One query of a tile (query g), by one warp, over the sums and row terms parked in ring buffer bp.  Out of line, like
+// tighten_from_list, with only pointers and two indices as arguments: of the forms tried (inlined into the three gather
+// variants, out of line with the query's values as arguments) this one adds the fewest spill reloads to the gather
+// loops, though still 1-2 per stage (DESIGN.md §3).  `a` is the kernel's __grid_constant__ parameter, read in place.
+__device__ __noinline__ void cand_query_warp(const ScanArgs *ap, const TileDesc *T, int g, int bp)
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const ScanArgs &a = *ap;
+    const int lane = threadIdx.x & 31;
+    const uint32_t q = T->q[g], slot = T->slot[g], row0 = T->row0, nrows = T->nrows, n_p = T->n_p, p = T->p;
+    uint32_t *const thr_q = a.thr + q;
+    uint32_t tkey = __ldcg(thr_q);
+    const float step = __ldg(a.qt_step + q), cst = __ldg(a.qt_base + q) + (a.probe_A ? __ldg(a.probe_A + slot) : 0.f);
+    const float slack = __ldg(a.slack + q), scale = a.metric == LGPU_COSINE ? 0.5f : 1.0f;
+    const uint32_t k = a.topk, rank = slot - q * a.nprobes, cap = a.cand_cap;
+    const uint32_t nv = n_p > row0 ? min(nrows, n_p - row0) : 0u;         // valid rows: a prefix of the tile
+    const int nm = (int)((nrows + 127) / 128);
+    // lane's rows: 128 m + 4 lane + (0..3); sums by LDS.64, row terms by LDS.128, both conflict-free
+    const uint32_t base = (uint32_t)__cvta_generic_to_shared(smem + bp * S3_BUF);
+    const uint32_t sa = base + (uint32_t)(g * SCAN3_ROWS_TILE * 2 + lane * 8), ra = base + (uint32_t)(S3_SUMS_BYTES + lane * 16);
+    auto rows4 = [&](int m, float (&L)[4]) {
+        const uint2 s = lds64u(sa + (uint32_t)m * 256u);
+        const float4 v = lds128f(ra + (uint32_t)m * 512u);
+        L[0] = (fmaf(step, u16lo_f32(s.x), cst) + v.x) * scale;
+        L[1] = (fmaf(step, u16hi_f32(s.x), cst) + v.y) * scale;
+        L[2] = (fmaf(step, u16lo_f32(s.y), cst) + v.z) * scale;
+        L[3] = (fmaf(step, u16hi_f32(s.y), cst) + v.w) * scale;
+    };
+    const bool had = tkey != CAND_NO_THR;
+    const float cur = had ? key_f32(tkey) : CUDART_INF_F;
+    const float lim0 = had ? cur + slack : CUDART_INF_F;
+    uint32_t kmin = 0xffffffffu, kmax = 0u, under = 0, npass = 0;
+#pragma unroll 2
+    for (int m = 0; m < nm; m++) {
+        float L[4];
+        rows4(m, L);
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            if ((uint32_t)(128 * m + 4 * lane + j) < nv) {
+                const uint32_t kk = f32_key(L[j]);
+                kmin = min(kmin, kk); kmax = max(kmax, kk);
+            }
+            under += L[j] <= cur ? 1u : 0u;
+            npass += L[j] <= lim0 ? 1u : 0u;
+        }
+    }
+    kmin = __reduce_min_sync(0xffffffffu, kmin); kmax = __reduce_max_sync(0xffffffffu, kmax);
+    under = __reduce_add_sync(0xffffffffu, under);
+
+    bool bisect = !had || rank < 3u;
+    float lo = key_f32(kmin), hi = key_f32(kmax);
+    if (had) { bisect = bisect ? under >= k : under >= 2u * k; if (cur < hi) hi = cur; }
+    if (bisect && nv >= k && hi < CUDART_INF_F && lo == lo && hi == hi) {
+        // invariant: count(L <= hi) >= k
+#pragma unroll 1
+        for (int it = 0; it < 8; it++) {
+            const float mid = 0.5f * lo + 0.5f * hi;
+            uint32_t c = 0;
+#pragma unroll 2
+            for (int m = 0; m < nm; m++) {
+                float L[4];
+                rows4(m, L);
+#pragma unroll
+                for (int j = 0; j < 4; j++) c += L[j] <= mid ? 1u : 0u;
+            }
+            c = __reduce_add_sync(0xffffffffu, c);
+            if (c >= k) hi = mid; else lo = mid;
+        }
+        const uint32_t nk = f32_key(hi);
+        if (nk < tkey) {
+            if (lane == 0) atomicMin(thr_q, nk);
+            tkey = nk;
+            const float lim = key_f32(tkey) + slack;
+            npass = 0;
+#pragma unroll 2
+            for (int m = 0; m < nm; m++) {
+                float L[4];
+                rows4(m, L);
+#pragma unroll
+                for (int j = 0; j < 4; j++) npass += L[j] <= lim ? 1u : 0u;
+            }
+        }
+    }
+    // The tile's queries run at once, so each read its threshold before any of them tightened it.  Read it again before
+    // the append: other CTAs may have tightened it meanwhile, and the rows that pass are fewer.
+    {
+        const uint32_t fresh = __shfl_sync(0xffffffffu, __ldcg(thr_q), 0);
+        if (fresh < tkey) {
+            tkey = fresh;
+            const float lim = key_f32(tkey) + slack;
+            npass = 0;
+#pragma unroll 2
+            for (int m = 0; m < nm; m++) {
+                float L[4];
+                rows4(m, L);
+#pragma unroll
+                for (int j = 0; j < 4; j++) npass += L[j] <= lim ? 1u : 0u;
+            }
+        }
+    }
+    const float lim = tkey == CAND_NO_THR ? CUDART_INF_F : key_f32(tkey) + slack;
+    const uint32_t wpass = __reduce_add_sync(0xffffffffu, npass);
+    if (wpass == 0) return;
+    uint32_t pre = npass;                                 // inclusive scan over lanes
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, pre, o);
+        if (lane >= o) pre += t;
+    }
+    uint32_t at = 0;
+    if (lane == 31) at = atomicAdd(a.cand_cnt + q, wpass);
+    at = __shfl_sync(0xffffffffu, at, 31) + pre - npass;
+#pragma unroll 1
+    for (int m = 0; m < nm; m++) {
+        float L[4];
+        rows4(m, L);
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            if (L[j] <= lim) {
+                if (at < cap) {
+                    CandRec rec; rec.lb = L[j]; rec.p = p; rec.row = row0 + 128 * m + 4 * lane + j; rec.pad = 0u;
+                    a.cand[(size_t)q * cap + at] = rec;
+                    a.cand_key[(size_t)q * cap + at] = f32_key(L[j]);
+                }
+                at++;
+            }
+        }
+    }
+}
+
+template <int R>
+__device__ __forceinline__ void cand_epilogue_warp(const ScanArgs &a, const TileDesc *T, bool next_exists, int bp, int ct,
+                                                   const uint32_t (&acc)[R][4], const bool (&valid)[R], const float (&rr)[R])
+{
+    extern __shared__ __align__(1024) unsigned char smem[];
+    const int ng = (int)T->ng, lane = ct & 31, g = ct >> 5;
+    unsigned char *const area = smem + bp * S3_BUF;
+    bar_sync(BAR_SCAN, S3_CT);                            // every warp has read the last data buffer
+    {
+        unsigned short *const sums = reinterpret_cast<unsigned short *>(area);
+        float *const rrs = reinterpret_cast<float *>(area + S3_SUMS_BYTES);
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+            const int i = ct + r * S3_CT;
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                if (2 * j < ng) sums[(2 * j) * SCAN3_ROWS_TILE + i] = (unsigned short)(acc[r][j] & 0xffffu);
+                if (2 * j + 1 < ng) sums[(2 * j + 1) * SCAN3_ROWS_TILE + i] = (unsigned short)(acc[r][j] >> 16);
+            }
+            rrs[i] = valid[r] ? rr[r] : CUDART_NAN_F;       // a NaN row term: the row never counts and never passes
+        }
+    }
+    bar_sync(BAR_SCAN, S3_CT);
+    if (g < ng) cand_query_warp(&a, T, g, bp);
+    if (next_exists) {                                    // hand the buffer back for the next tile's chunk 1
+        __syncwarp();
+        bar_arrive(BAR_EMPTY + bp, S3_NT);
+    }
+}
+
 template <int R, bool LIST>
 __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, bool next_exists, int b, int ct, uint32_t &ph)
 {
@@ -307,7 +504,8 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
                 acc[r][0] += v.x; acc[r][1] += v.y; acc[r][2] += v.z; acc[r][3] += v.w;
             }
         }
-        if (it + 2 <= nch || next_exists) bar_arrive(BAR_EMPTY + bp, S3_NT);
+        // the k <= 32 candidate epilogue keeps the last data buffer (the zero stage's bp) and hands it back itself
+        if (it + 2 <= nch || (next_exists && (it < nch || a.cand == nullptr || LIST))) bar_arrive(BAR_EMPTY + bp, S3_NT);
         b = ring_next3(b);
     }
 
@@ -338,12 +536,14 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
         }
         return b;
     }
-    // candidate mode.  tau_q (global, atomicMin) is any value such that at least k rows of the query have L <= tau_q:
-    // then the k-th smallest exact distance is <= tau_q + W + E and every row of the exact top-k has
-    // L <= tau_q + W + 2E = tau_q + slack_q.  The CTA's 256 scanner threads tighten tau_q from the tile's own rows (an
-    // upper bound of their k-th smallest L, by 8 counting bisections through shared counters) when the query has no
-    // threshold yet or when this is one of its three nearest partitions -- that is where the small distances are;
-    // every warp then appends the rows under the threshold.
+    if constexpr (!LIST) {
+        // the zero stage's previous buffer: two stages before the next tile's, i.e. b + 1 in the ring of three
+        cand_epilogue_warp<R>(a, T, next_exists, ring_next3(b), ct, acc, valid, rr);
+        return b;
+    }
+    // candidate mode with the list tightening (k > 32), the same threshold policy as cand_epilogue_warp, run by the
+    // CTA's 256 scanner threads together: the tile's own bisection counts through shared counters, every warp then
+    // appends the rows under the threshold.
     const int lane = ct & 31;
     const uint32_t k = a.topk;
     // The queries' scalars (step, base + A, slack) are loaded here for all of the tile's queries at once, beside the
@@ -504,7 +704,7 @@ __device__ __forceinline__ void scanner_loop(const ScanArgs &a, int tid)
 // overflow the lists).  A separate instantiation, so that the list keys held in registers there do not cost the
 // k <= 32 kernel (BASELINE config 2) spills inside its gather loop.
 template <bool LIST>
-__global__ void __launch_bounds__(S3_NT, 2) scan3_kernel(ScanArgs a)
+__global__ void __launch_bounds__(S3_NT, 2) scan3_kernel(const __grid_constant__ ScanArgs a)
 {
     pdl_entry();                                       // PDL: let the next grid in, wait for the previous one
     extern __shared__ __align__(1024) unsigned char smem[];
