@@ -120,8 +120,19 @@ int         lgpu_device_count(int *count);
 /* ---- IVF_PQ (ANNIvfPartitionExec -> ANNIvfSubIndexExec -> TopK) ---------- */
 int  lgpu_index_open(const lgpu_index_desc *desc, lgpu_index **out);
 void lgpu_index_close(lgpu_index *ix);
-/* bytes of HBM held by the index (codes + ids + centroids + codebook + vectors) */
+/* bytes of HBM held by the index (codes + ids + centroids + codebook, and the raw vectors when they are in HBM) */
 int  lgpu_index_device_bytes(const lgpu_index *ix, uint64_t *bytes);
+/* Where an index keeps the raw vectors desc.vectors gave it (refine_factor).  Every float IVF open (lgpu_index_open,
+ * lgpu_ivf_sq_open, lgpu_ivf_hnsw_sq_open, lgpu_ivf_rq_open) copies them into HBM when they fit with room to spare: the
+ * device's free memory, once the rest of the index is in place, covers them plus the workspace budget (LGPU_WS_BYTES,
+ * default 8 GiB), and they are at most LGPU_VECTORS_HBM_BYTES (read at every open; unset = no cap, 0 = never in HBM).
+ * Otherwise the index copies them into pinned, mapped host memory that it owns (rows padded to a multiple of 4 floats,
+ * freed by lgpu_index_close) and refine reads the k x refine_factor candidates over PCIe; results are identical.  A
+ * pinned allocation that fails is LGPU_OOM.  The caller's buffer is borrowed for the open call only, either way. */
+typedef enum { LGPU_VECTORS_NONE = 0, LGPU_VECTORS_HBM = 1, LGPU_VECTORS_HOST = 2 } lgpu_vectors_placement;
+/* bytes of pinned host memory held by the index (nrows x round_up(dim, 4) x 4 when the raw vectors are on the host,
+ * else 0) and where the raw vectors are (lgpu_vectors_placement); either output may be NULL */
+int  lgpu_index_host_bytes(const lgpu_index *ix, uint64_t *bytes, int *placement);
 /* sum over a batch of the PQ code bytes its probes must scan (the roofline's
  * algorithmic bytes, SURVEY.md 8d); valid for the most recent search on the
  * calling thread */
@@ -591,6 +602,12 @@ int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes
  * out [nqv][nrows] f32); dim must be a multiple of 8 */
 int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
                            uint64_t nrows, uint32_t dim, int device, float *out);
+/* the refine kernel of an index whose raw vectors are on the host, alone: out[q][c] = the exact distance (lgpu_metric)
+ * of queries[q] and rows[pos[q][c]], +inf where pos is UINT64_MAX -- the value refine_factor re-ranks by.  The rows are
+ * copied into pinned, mapped host memory and read from there (host buffers: queries [B][dim], rows [N][dim],
+ * pos [B][nc], out [B][nc]) */
+int lgpu_debug_refine_host(const float *queries, uint32_t B, const float *rows, uint64_t N, uint32_t dim,
+                           const uint64_t *pos, uint32_t nc, int metric, int device, float *out);
 /* the number of queries per sub-batch an lgpu_search* call of B queries and `nprobes` probes (the widest the call uses:
  * maximum_nprobes under a prefilter) on `ix` runs in under the process's LGPU_WS_BYTES: B when the batch is not split */
 int lgpu_debug_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32_t *out);

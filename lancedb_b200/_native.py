@@ -49,7 +49,9 @@ EXPORTS = [
     "lgpu_ivf_binary_search_unindexed", "lgpu_ivf_binary_search_unindexed_device",
     "lgpu_index_delete", "lgpu_ivf_binary_delete", "lgpu_flat_delete", "lgpu_binary_delete", "lgpu_multivec_delete",
     "lgpu_flat_open_f16", "lgpu_flat_append_f16", "lgpu_flat_device_bytes",
+    "lgpu_index_host_bytes", "lgpu_debug_refine_host",
 ]
+VECTORS_NONE, VECTORS_HBM, VECTORS_HOST = 0, 1, 2     # lgpu_vectors_placement
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
 MULTIVEC_MAX_ROW = 1 << 20      # vectors per multivector row
 MULTIVEC_MAX_DIM = 65536
@@ -157,6 +159,8 @@ def load():
     lib.lgpu_index_close.argtypes = [vp]
     lib.lgpu_index_close.restype = None
     lib.lgpu_index_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.lgpu_index_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+    lib.lgpu_debug_refine_host.argtypes = [vp, u32, vp, C.c_uint64, u32, vp, u32, i32, i32, vp]
     lib.lgpu_last_scanned_code_bytes.argtypes = [C.POINTER(C.c_uint64)]
     lib.lgpu_search.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
     lib.lgpu_search_async.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, C.POINTER(vp)]
@@ -402,9 +406,25 @@ class GpuIvfPq(_RowsHandle):
                          data.nrows, *[_ptr(a) for a in keep]), keep
 
     def device_bytes(self) -> int:
+        """The HBM the index holds; its raw vectors count only when they are in HBM."""
         b = C.c_uint64(0)
         check(load().lgpu_index_device_bytes(self._h, C.byref(b)))
         return b.value
+
+    def _host(self):
+        b, where = C.c_uint64(0), C.c_int(0)
+        check(load().lgpu_index_host_bytes(self._h, C.byref(b), C.byref(where)))
+        return b.value, where.value
+
+    def host_bytes(self) -> int:
+        """The pinned host memory the index holds: its raw vectors (rows padded to 4 floats) when they did not fit in
+        HBM at open, else 0 (lgpu_index_host_bytes)."""
+        return self._host()[0]
+
+    @property
+    def vectors_on_host(self) -> bool:
+        """True when the raw vectors (refine_factor) are kept in pinned host memory and refine reads them over PCIe."""
+        return self._host()[1] == VECTORS_HOST
 
     def search(self, queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None, allow=None, allow_bits=0,
                max_nprobes=0, timeout_ms=0, ef=0):
@@ -787,6 +807,21 @@ def pq_train(vectors, init_codebook, iters: int, device: int = 0) -> np.ndarray:
     cb = np.array(init_codebook, np.float32, order="C", copy=True)
     check(load().lgpu_pq_train(_ptr(v), v.shape[0], v.shape[1], cb.shape[0], _ptr(cb), int(iters), device))
     return cb
+
+
+def debug_refine_host(queries, rows, pos, metric: str = "l2", device: int = 0) -> np.ndarray:
+    """The host-rows refine kernel alone (lgpu_debug_refine_host): out [B, nc] f32, the exact distance of queries[q]
+    and rows[pos[q, c]] (+inf where pos is UINT64_MAX), with the rows read from pinned host memory."""
+    q = np.ascontiguousarray(queries, np.float32)
+    x = np.ascontiguousarray(rows, np.float32)
+    p = np.ascontiguousarray(pos, np.uint64)
+    B, nc = p.shape
+    if x.ndim != 2 or q.shape != (B, x.shape[1]):
+        raise ValueError("queries must be [B, dim] and rows [N, dim], with B the rows of pos")
+    out = np.empty((B, nc), np.float32)
+    check(load().lgpu_debug_refine_host(_ptr(q), B, _ptr(x), x.shape[0], x.shape[1], _ptr(p), nc, METRICS[metric],
+                                        device, _ptr(out)))
+    return out
 
 
 def allow_bitmap(row_ids, nbits: int) -> np.ndarray:

@@ -106,6 +106,22 @@ struct DevBuf {
     ~DevBuf() { reset(); }
 };
 
+// pinned host memory mapped into the device's address space (cudaHostAllocMapped): `dev` is the alias kernels read
+// over PCIe
+struct PinnedBuf {
+    void *p = nullptr, *dev = nullptr;
+    size_t bytes = 0;
+    void alloc(size_t n)
+    {
+        reset();
+        LGPU_CUDA(cudaHostAlloc(&p, std::max<size_t>(n, 16), cudaHostAllocMapped));
+        bytes = n;
+        LGPU_CUDA(cudaHostGetDevicePointer(&dev, p, 0));
+    }
+    void reset() { if (p) cudaFreeHost(p); p = dev = nullptr; bytes = 0; }
+    ~PinnedBuf() { reset(); }
+};
+
 struct Workspace {
     cudaStream_t stream = nullptr;     // private stream (host-buffer entry points)
     // side stream of the filter scan's front: the coarse step and the regrouping run here while the per-query tables
@@ -367,6 +383,10 @@ struct lgpu_index {
     float cent_max = 0.f, cent_err = 0.f;   // max |c|, max |bf16(c) - c| (the error band, kernels.cuh tc_band)
     bool has_tc = false;
     bool has_vectors = false;
+    // the raw vectors (refine_factor) live in `vectors` (HBM, [nrows][dim]) or, when they do not fit there
+    // (place_vectors), in `vectors_host`: [nrows][vec_stride] f32, vec_stride = dim rounded up to 4, padding zero
+    PinnedBuf vectors_host;
+    uint32_t vec_stride = 0;
     // IVF_SQ (lgpu_ivf_sq_open): `codes` holds [nrows][dim_pad] u8 row codes, `sq_xx` the sum of each row's squared codes
     uint32_t dim_pad = 0;
     double sq_lo = 0.0, sq_hi = 0.0;
@@ -1416,8 +1436,13 @@ static void ivf_hnsw(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu
 static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *d_q, TopkOut out,
                        const uint32_t *only, cudaStream_t st)
 {
-    launch_pair_distance(d_q, ix->vectors.as<float>(), ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric,
-                         ws->t_exact.as<float>(), st);
+    if (ix->vectors_host.p)
+        launch_refine_host(d_q, static_cast<const float *>(ix->vectors_host.dev), ix->vec_stride,
+                           ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric, ws->t_exact.as<float>(),
+                           ix->num_sms, st);
+    else
+        launch_pair_distance(d_q, ix->vectors.as<float>(), ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric,
+                             ws->t_exact.as<float>(), st);
     SelectArgs sr = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), p.kk, p.B, p.k, out);
     sr.only = only;
     launch_select(with_scratch(ws, sr), st);
@@ -2262,7 +2287,7 @@ static void open_ivf_partitions(lgpu_index *ix, const Desc *d, uint32_t rows_til
 }
 
 // What the float IVF indexes add, uploaded on the legacy stream: centroids (and their bf16 copy for the tensor-core
-// coarse step) and the optional raw vectors
+// coarse step).  The optional raw vectors are placed last, by place_vectors, once the rest of the index is in HBM.
 template <class Desc>
 static void open_ivf_common(lgpu_index *ix, const Desc *d, uint32_t rows_tile, const std::vector<uint64_t> &code_base)
 {
@@ -2271,7 +2296,6 @@ static void open_ivf_common(lgpu_index *ix, const Desc *d, uint32_t rows_tile, c
     cudaStream_t st = nullptr;
     upload(ix->centroids, d->centroids, (size_t)nlist * dim * 4);
     open_ivf_partitions(ix, d, rows_tile, code_base);
-    if (d->vectors) { upload(ix->vectors, d->vectors, (size_t)d->nrows * dim * 4); ix->has_vectors = true; }
     if (gemm_shape_supported(dim) && d->metric != LGPU_DOT) {
         LGPU_CUDA(cudaStreamSynchronize(st));
         const bool finite =
@@ -2476,14 +2500,51 @@ static uint64_t index_device_bytes(const lgpu_index *ix)
     return n;
 }
 
-// The sequence of every IVF open: `open(ix)` checks the desc, then creates the index (new_ivf) and fills it; the index
-// is then registered and returned, or deleted if any step failed.
+// Where an index keeps its raw vectors ([nrows][dim] f32 on the host, borrowed for the open call), decided after
+// everything else the index holds is in HBM.  HBM when they fit with room to spare: at most LGPU_VECTORS_HBM_BYTES of
+// them (read at every open; unset = no cap, 0 = never HBM), and the device's free memory covers them plus the
+// workspace budget (LGPU_WS_BYTES) its searches may lease.  HBM rows are allocated exactly, so that device bytes of the
+// two placements differ by nrows x dim x 4.  Otherwise a pinned, mapped host copy that the index owns,
+// rows padded to a multiple of 4 floats, which refine reads over PCIe (launch_refine_host).
+static void place_vectors(lgpu_index *ix, const float *vectors)
+{
+    if (!vectors) return;
+    ix->has_vectors = true;
+    const uint64_t n = ix->nrows, dim = ix->dim, bytes = n * dim * 4;
+    const char *e = getenv("LGPU_VECTORS_HBM_BYTES");
+    const uint64_t cap = (e && *e) ? strtoull(e, nullptr, 10) : UINT64_MAX;
+    size_t free_b = 0, total_b = 0;
+    LGPU_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    if (cap > 0 && bytes <= cap && (uint64_t)free_b >= bytes + workspace_budget()) {
+        ix->vectors.ensure(std::max<size_t>(bytes, 16), true);
+        if (bytes) LGPU_CUDA(cudaMemcpy(ix->vectors.p, vectors, bytes, cudaMemcpyHostToDevice));
+        return;
+    }
+    const uint32_t stride = (uint32_t)round_up64(dim, 4);
+    ix->vectors_host.alloc((size_t)n * stride * 4);
+    float *dst = static_cast<float *>(ix->vectors_host.p);
+    if (stride == dim) {
+        memcpy(dst, vectors, bytes);
+    } else {
+        for (uint64_t r = 0; r < n; r++) {
+            memcpy(dst + r * stride, vectors + r * dim, dim * 4);
+            memset(dst + r * stride + dim, 0, (stride - dim) * 4);
+        }
+    }
+    ix->vec_stride = stride;
+}
+
+// The sequence of every IVF open: `open(ix)` checks the desc, then creates the index (new_ivf) and fills it, and returns
+// the raw vectors it keeps for refine_factor (or null), which place_vectors places last; the index is then registered
+// and returned, or deleted if any step failed.
 template <class H, class Open> static int open_ivf(H **out, Open &&open)
 {
     H *ix = nullptr;
     const int rc = guarded([&] {
         LGPU_REQUIRE(out != nullptr, "null argument");
-        open(ix);
+        const float *vectors = open(ix);
+        LGPU_CUDA(cudaStreamSynchronize(nullptr));
+        place_vectors(ix, vectors);
         LGPU_CUDA(cudaStreamSynchronize(nullptr));
         ix->device_bytes = index_device_bytes(ix);
         register_handle(ix);
@@ -2534,7 +2595,7 @@ int lgpu_device_count(int *count)
 
 int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
 {
-    return open_ivf(out, [&](lgpu_index *&ix) {
+    return open_ivf(out, [&](lgpu_index *&ix) -> const float * {
         LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->dim > 0 && d->nlist > 0 && d->m > 0, "dim, nlist and m must be positive");
@@ -2548,12 +2609,13 @@ int lgpu_index_open(const lgpu_index_desc *d, lgpu_index **out)
         check_ivf_layout(d->dim, d->nlist, d->metric, d->nrows, d->centroids, d->part_offsets, d->codes, d->row_ids);
         if (d->nbits == 4) open_pq4(d, ix);
         else open_pq8(d, ix);
+        return d->vectors;
     });
 }
 
 int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
 {
-    return open_ivf(out, [&](lgpu_index *&ix) {
+    return open_ivf(out, [&](lgpu_index *&ix) -> const float * {
         LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->metric != LGPU_DOT, "IVF_SQ supports the l2 and cosine distance types, not dot");
@@ -2566,6 +2628,7 @@ int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
         ix->sq_lo = d->lo; ix->sq_hi = d->hi;
         open_ivf_common(ix, d, SQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
         upload_sq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->sq_xx);
+        return d->vectors;
     });
 }
 
@@ -2609,7 +2672,7 @@ static void check_hnsw_graph(const lgpu_ivf_hnsw_sq_desc *d)
 
 int lgpu_ivf_hnsw_sq_open(const lgpu_ivf_hnsw_sq_desc *d, lgpu_index **out)
 {
-    return open_ivf(out, [&](lgpu_index *&ix) {
+    return open_ivf(out, [&](lgpu_index *&ix) -> const float * {
         LGPU_REQUIRE(d != nullptr, "null argument");
         const lgpu_ivf_sq_desc *s = &d->sq;
         LGPU_REQUIRE(s->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
@@ -2632,6 +2695,7 @@ int lgpu_ivf_hnsw_sq_open(const lgpu_ivf_hnsw_sq_desc *d, lgpu_index **out)
         upload(ix->hn_entry, d->entry, (size_t)s->nlist * 4);
         upload(ix->hn_top, d->top_level, (size_t)s->nlist);
         LGPU_CUDA(cudaStreamSynchronize(nullptr));
+        return s->vectors;
     });
 }
 
@@ -2696,7 +2760,7 @@ int lgpu_debug_pq4_sums(const uint8_t *tables, uint32_t B, const uint8_t *codes,
 
 int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
 {
-    return open_ivf(out, [&](lgpu_index *&ix) {
+    return open_ivf(out, [&](lgpu_index *&ix) -> const float * {
         LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->metric != LGPU_DOT, "IVF_RQ supports the l2 and cosine distance types, not dot");
@@ -2716,6 +2780,7 @@ int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
         // rc_p = P c_p, once: each probe slot's residual is then one subtraction per dimension
         launch_rq_rotate(ix->rq_rot.as<float>(), ix->centroids.as<float>(), d->nlist, d->dim, ix->rq_rc.as<float>(),
                          nullptr);
+        return d->vectors;
     });
 }
 
@@ -2772,6 +2837,45 @@ int lgpu_index_device_bytes(const lgpu_index *ixh, uint64_t *bytes)
         LGPU_REQUIRE(bytes, "null argument");
         HandleRef<lgpu_index> ix(const_cast<lgpu_index *>(ixh));
         *bytes = ix->device_bytes;
+    });
+}
+
+int lgpu_index_host_bytes(const lgpu_index *ixh, uint64_t *bytes, int *placement)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(bytes || placement, "null argument");
+        HandleRef<lgpu_index> ix(const_cast<lgpu_index *>(ixh));
+        if (bytes) *bytes = ix->vectors_host.bytes;
+        if (placement)
+            *placement = !ix->has_vectors ? LGPU_VECTORS_NONE : ix->vectors_host.p ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+    });
+}
+
+int lgpu_debug_refine_host(const float *queries, uint32_t B, const float *rows, uint64_t N, uint32_t dim,
+                           const uint64_t *pos, uint32_t nc, int metric, int device, float *out)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(dim >= 1, "dim must be positive");
+        LGPU_REQUIRE(metric == LGPU_L2 || metric == LGPU_COSINE || metric == LGPU_DOT, "unknown distance type");
+        LGPU_REQUIRE(B == 0 || nc == 0 || (queries && pos && out && (N == 0 || rows)), "null buffer");
+        for (uint64_t i = 0; i < (uint64_t)B * nc; i++)
+            LGPU_REQUIRE(pos[i] < N || pos[i] == UINT64_MAX, "a position outside the rows");
+        if (B == 0 || nc == 0) return;
+        require_device(device);
+        int sms = 0;
+        LGPU_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+        const uint32_t stride = (uint32_t)round_up64(dim, 4);
+        PinnedBuf h;
+        h.alloc((size_t)N * stride * 4);
+        memset(h.p, 0, h.bytes);
+        for (uint64_t r = 0; r < N; r++) memcpy(static_cast<float *>(h.p) + r * stride, rows + r * dim, (size_t)dim * 4);
+        DevBuf q, p, o;
+        upload(q, queries, (size_t)B * dim * 4);
+        upload(p, pos, (size_t)B * nc * 8);
+        o.ensure((size_t)B * nc * 4);
+        launch_refine_host(q.as<float>(), static_cast<const float *>(h.dev), stride, p.as<uint64_t>(), B, nc, dim, metric,
+                           o.as<float>(), sms, nullptr);
+        LGPU_CUDA(cudaMemcpy(out, o.p, (size_t)B * nc * 4, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -3235,7 +3339,7 @@ int lgpu_binary_search_device(lgpu_binary *bxh, const uint8_t *d_queries, uint32
 
 int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
 {
-    return open_ivf(out, [&](lgpu_ivf_binary *&ix) {
+    return open_ivf(out, [&](lgpu_ivf_binary *&ix) -> const float * {
         LGPU_REQUIRE(d != nullptr, "null argument");
         LGPU_REQUIRE(d->abi_version == LGPU_ABI_VERSION, "ABI version mismatch");
         LGPU_REQUIRE(d->nbytes > 0, "zero bytes per vector");
@@ -3259,6 +3363,7 @@ int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
         };
         pack(d->centroids, d->nlist, ix->centroids, ix->cent_pop);
         pack(d->vectors, d->nrows, ix->codes, ix->row_pop);
+        return nullptr;             // the packed rows are the index: no separate raw vectors
     });
 }
 

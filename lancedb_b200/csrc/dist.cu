@@ -244,6 +244,99 @@ __global__ void pair_distance_kernel(const float *__restrict__ Q, const T *__res
     if (hl == 0) out[pair] = v;
 }
 
+// pair_distance_kernel's values when the stored rows are in pinned host memory, read through their mapped device alias
+// over PCIe.  Each warp owns a run of consecutive (query, candidate) pairs and walks it in steps: step s is one chunk of
+// the rows of two pairs, copied by the whole warp into a shared-memory ring slot with cp.async 16-byte requests (one
+// instruction = 512 contiguous bytes of a row, where halfwarp_l2's reads would be 64-byte pieces), RH_STAGES - 1 steps
+// in flight while the next one is reduced (RH_STAGES 2, 4 and 8 all read at 88-94 % of the pinned memcpy rate on an
+// H100 80GB HBM3, 2 the fastest: DESIGN.md section 7).  Half-warp h then reduces pair 2j + h from shared memory with the
+// same lane accumulators, lane sum, remainder and roundings as pair_distance_kernel.  Rows are `stride` floats apart (dim rounded up
+// to 4, so every row starts 16-byte aligned); a chunk is a multiple of 16 floats, so each lane's accumulator sees its
+// dims in lance's order across chunks and the remainder dims [d16, d) all lie in the last chunk.
+constexpr int RH_WARPS = 4, RH_STAGES = 2;
+constexpr uint32_t RH_CHUNK_MAX = 1024;             // floats of a row per step: at most 64 KB of ring per CTA
+
+__global__ void __launch_bounds__(RH_WARPS * 32) refine_host_kernel(
+    const float *__restrict__ Q, const float *V, uint32_t stride, const uint64_t *__restrict__ pos, uint64_t npairs,
+    uint32_t nc, uint32_t d, int metric, uint32_t chunk, uint32_t nchunks, uint32_t per_warp, float *__restrict__ out)
+{
+    pdl_entry();
+    extern __shared__ __align__(16) float rh_ring[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, h = lane >> 4, hl = lane & 15, hbase = lane & 16;
+    const unsigned hmask = 0xffffu << hbase;
+    const uint64_t p0 = ((uint64_t)blockIdx.x * RH_WARPS + warp) * per_warp;
+    if (p0 >= npairs) return;                                    // the whole warp
+    const uint64_t p1 = min(p0 + per_warp, npairs);
+    const uint32_t nsteps = (uint32_t)((p1 - p0 + 1) / 2) * nchunks, d16 = d & ~15u;
+    float *ring = rh_ring + (size_t)warp * RH_STAGES * 2 * chunk;
+    const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(ring);
+    // step s -> slot s % RH_STAGES: chunk s % nchunks of the rows of pairs p0 + 2 (s / nchunks) + {0, 1}.  Every lane
+    // commits one group per step, empty or not, so that wait_group counts steps.
+    auto issue = [&](uint32_t s) {
+        if (s < nsteps) {
+            const uint32_t j = s / nchunks, k0 = (s % nchunks) * chunk, len = min(chunk, stride - k0);
+            for (int r = 0; r < 2; r++) {
+                const uint64_t pr = p0 + 2 * j + r;
+                const uint64_t ps = pr < p1 ? pos[pr] : UINT64_MAX;
+                if (ps == UINT64_MAX) continue;
+                const float *src = V + ps * stride + k0;
+                const uint32_t dst = ring_s + ((s % RH_STAGES) * 2 + r) * chunk * 4;
+                for (uint32_t o = (uint32_t)lane * 4; o < len; o += 128)
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + o * 4), "l"(src + o) : "memory");
+            }
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    for (uint32_t s = 0; s < RH_STAGES - 1; s++) issue(s);
+    float a0 = 0.f, a1 = 0.f;                    // lane accumulators: l2 / dot in a0; cosine yy in a0, xy in a1
+    for (uint32_t s = 0; s < nsteps; s++) {
+        issue(s + RH_STAGES - 1);                // into the slot step s - 1 used, released by the last __syncwarp
+        asm volatile("cp.async.wait_group %0;" ::"n"(RH_STAGES - 1) : "memory");
+        __syncwarp();                            // every lane's copies of step s are in place
+        const uint32_t c = s % nchunks, k0 = c * chunk;
+        const uint64_t pr = p0 + 2 * (s / nchunks) + h;
+        const uint64_t ps = pr < p1 ? pos[pr] : UINT64_MAX;      // uniform over the half-warp
+        const float *y = ring + ((s % RH_STAGES) * 2 + h) * chunk;        // y[k - k0]: dim k of the row
+        const float *x = Q + (size_t)(pr / nc) * d;
+        if (ps != UINT64_MAX) {
+            for (uint32_t k = k0 + hl; k < min(k0 + chunk, d16); k += 16) {
+                const float xv = x[k], yv = y[k - k0];
+                if (metric == LGPU_L2) { const float df = __fsub_rn(xv, yv); a0 = __fadd_rn(a0, __fmul_rn(df, df)); }
+                else if (metric == LGPU_DOT) a0 = __fadd_rn(a0, __fmul_rn(xv, yv));
+                else { a0 = __fadd_rn(a0, __fmul_rn(yv, yv)); a1 = __fadd_rn(a1, __fmul_rn(xv, yv)); }
+            }
+        }
+        if (c == nchunks - 1 && ps != UINT64_MAX) {              // the row's last chunk: lane sum, remainder, metric
+            float t0 = 0.f, t1 = 0.f;
+#pragma unroll
+            for (int l = 0; l < 16; l++) {
+                t0 = __fadd_rn(t0, __shfl_sync(hmask, a0, hbase + l));
+                t1 = __fadd_rn(t1, __shfl_sync(hmask, a1, hbase + l));
+            }
+            float s0 = 0.f, s1 = 0.f;
+            for (uint32_t i = d16; i < d; i++) {
+                const float xv = x[i], yv = y[i - k0];
+                if (metric == LGPU_L2) { const float df = __fsub_rn(xv, yv); s0 = __fadd_rn(s0, __fmul_rn(df, df)); }
+                else if (metric == LGPU_DOT) s0 = __fadd_rn(s0, __fmul_rn(xv, yv));
+                else { s0 = __fadd_rn(s0, __fmul_rn(yv, yv)); s1 = __fadd_rn(s1, __fmul_rn(xv, yv)); }
+            }
+            float v;
+            if (metric == LGPU_L2) v = __fadd_rn(s0, t0);
+            else if (metric == LGPU_DOT) v = __fsub_rn(1.0f, __fadd_rn(s0, t0));
+            else {   // cosine_scalar: 1 - xy / |x| / sqrt(yy)
+                const float xn = sqrtf(halfwarp_dot(x, x, d, hl, hmask, hbase));
+                v = __fsub_rn(1.0f, __fdiv_rn(__fdiv_rn(__fadd_rn(s1, t1), xn), sqrtf(__fadd_rn(s0, t0))));
+            }
+            if (hl == 0) out[pr] = v;
+        } else if (c == nchunks - 1 && pr < p1 && hl == 0) {
+            out[pr] = CUDART_INF_F;
+        }
+        if (c == nchunks - 1) { a0 = 0.f; a1 = 0.f; }
+        __syncwarp();                            // slot s % RH_STAGES is read: step s + RH_STAGES may overwrite it
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+}
+
 // exact MaxSim re-score of the multivector shortlist, half a warp per (query, candidate row): for each query vector i
 // in order, the NaN-skipping min over the row's vectors j of 1 - xy / |q_i| / |v_j| (xy in lance's lane order: the
 // same roundings as dist_matrix_kernel mode 2), added onto a sum that starts at 0.0f -- the exact path's bits
@@ -521,6 +614,24 @@ void launch_pair_distance(const float *Q, const T *V, const uint64_t *pos, uint3
     if (B == 0 || nc == 0) return;
     uint64_t threads = (uint64_t)B * nc * 16;
     launch_k(pair_distance_kernel<T>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, V, pos, B, nc, d, metric, out); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_refine_host(const float *Q, const float *V, uint32_t stride, const uint64_t *pos, uint32_t B, uint32_t nc,
+                        uint32_t d, int metric, float *out, int num_sms, cudaStream_t st)
+{
+    const uint64_t npairs = (uint64_t)B * nc;
+    if (npairs == 0) return;
+    const uint32_t chunk = std::min<uint32_t>((d + 15) & ~15u, RH_CHUNK_MAX), nchunks = (d + chunk - 1) / chunk;
+    // an even run of pairs per warp, sized so that the grid is about 16 warps per SM (a few waves at most)
+    const uint64_t want = (uint64_t)std::max(num_sms, 1) * 16;
+    const uint32_t per_warp = (uint32_t)std::max<uint64_t>(2, ((npairs + want - 1) / want + 1) & ~1ull);
+    const uint64_t warps = (npairs + per_warp - 1) / per_warp;
+    const size_t smem = (size_t)RH_WARPS * RH_STAGES * 2 * chunk * 4;
+    if (smem > 48 * 1024)
+        LGPU_CUDA(cudaFuncSetAttribute(refine_host_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    launch_k(refine_host_kernel, dim3((unsigned)((warps + RH_WARPS - 1) / RH_WARPS)), dim3(RH_WARPS * 32), smem, st, Q,
+             V, stride, pos, npairs, nc, d, metric, chunk, nchunks, per_warp, out); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

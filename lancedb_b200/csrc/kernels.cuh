@@ -290,6 +290,10 @@ void launch_normalize(const float *X, uint32_t B, uint32_t d, float *out, cudaSt
 template <class T>
 void launch_pair_distance(const float *Q, const T *V, const uint64_t *pos, uint32_t B, uint32_t nc,
                           uint32_t d, int metric, float *out, cudaStream_t st);
+// the same out[q][c], bit for bit, with the rows in pinned host memory: V is their mapped device alias, rows `stride`
+// floats apart (a multiple of 4, 16-byte aligned).  Reads whole rows over PCIe into shared memory (dist.cu)
+void launch_refine_host(const float *Q, const float *V, uint32_t stride, const uint64_t *pos, uint32_t B, uint32_t nc,
+                        uint32_t d, int metric, float *out, int num_sms, cudaStream_t st);
 
 // ---------------- top-k select (K4) ------------------------------------------------
 constexpr uint32_t SELECT_KMAX = 2048;
