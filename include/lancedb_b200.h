@@ -416,8 +416,24 @@ int  lgpu_flat_open_f16(const uint16_t *vectors, uint64_t nrows, uint32_t dim,
 int  lgpu_flat_append_f16(lgpu_flat *fl, const uint16_t *rows, uint64_t n, const uint64_t *row_ids);
 /* *bytes = the device memory the handle holds for its rows and their per-row data (rows, tensor-core operand, |x|^2,
  * row norms once a cosine search computed them, row ids, the live bitmap), capacity kept for appends included; the
- * per-call search workspaces (each within LGPU_WS_BYTES) are not counted.  Both row types. */
+ * per-call search workspaces (each within LGPU_WS_BYTES) are not counted.  Both row types.  A handle whose rows are in
+ * host memory (lgpu_flat_host_bytes) holds only its row ids and live bitmap here. */
 int  lgpu_flat_device_bytes(const lgpu_flat *fl, uint64_t *bytes);
+/* Where a flat handle keeps its rows.  lgpu_flat_open and lgpu_flat_open_f16 copy them into HBM, as above, when their
+ * row data -- the rows, plus the tensor-core operand and |x|^2 of a column of at least 4096 rows with dim a multiple of
+ * 8 (a bf16 copy for f32 rows; fp16 rows are their own) -- is at most LGPU_FLAT_HBM_BYTES (read at every open; unset =
+ * no cap, 0 = never in HBM) and the device's free memory covers it plus the workspace budget (LGPU_WS_BYTES, default
+ * 8 GiB).  Otherwise the handle copies the rows into pinned host memory that it owns, [nrows][dim] in the row type
+ * (freed by lgpu_flat_close), and keeps only the row ids and the live bitmap in HBM.  Every search of such a handle
+ * (host, _filtered, _device, and as the tail of lgpu_search_unindexed[_device]) streams the rows through two staging
+ * buffers of its workspace, within LGPU_WS_BYTES: each row crosses PCIe once per call when the workspace holds the
+ * running top-k of all B queries, else once per group of queries it holds.  Results are identical to an HBM handle's
+ * on the same rows -- same ids, counts and distance bits -- for every metric, k, distance_range, prefilter, deleted
+ * rows and append.  A handle keeps its placement for life; lgpu_flat_append grows the pinned rows geometrically.  A
+ * pinned allocation that fails is LGPU_OOM.  The caller's buffer is borrowed for the open call only, either way.
+ * *bytes = the pinned host memory the handle holds (nrows x dim x the element size at open, capacity kept for appends
+ * included; 0 for an HBM handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output may be NULL. */
+int  lgpu_flat_host_bytes(const lgpu_flat *fl, uint64_t *bytes, int *placement);
 
 /* ---- rows added after an index was built (the reference's unindexed fragments, searched unless fast_search is set;
  * rust/lancedb/src/table/query.rs:289-290).  `tail` holds them.  The result is the top-k by (_distance, _rowid) of

@@ -49,7 +49,7 @@ EXPORTS = [
     "lgpu_ivf_binary_search_unindexed", "lgpu_ivf_binary_search_unindexed_device",
     "lgpu_index_delete", "lgpu_ivf_binary_delete", "lgpu_flat_delete", "lgpu_binary_delete", "lgpu_multivec_delete",
     "lgpu_flat_open_f16", "lgpu_flat_append_f16", "lgpu_flat_device_bytes",
-    "lgpu_index_host_bytes", "lgpu_debug_refine_host",
+    "lgpu_index_host_bytes", "lgpu_debug_refine_host", "lgpu_flat_host_bytes",
 ]
 VECTORS_NONE, VECTORS_HBM, VECTORS_HOST = 0, 1, 2     # lgpu_vectors_placement
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
@@ -180,6 +180,7 @@ def load():
     lib.lgpu_flat_open.argtypes = [vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
     lib.lgpu_flat_open_f16.argtypes = [vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
     lib.lgpu_flat_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.lgpu_flat_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
     lib.lgpu_flat_close.argtypes = [vp]
     lib.lgpu_flat_close.restype = None
     lib.lgpu_ivf_assign.argtypes = [vp, u32, u32, i32, vp, C.c_uint64, i32, vp]
@@ -553,9 +554,10 @@ class GpuIvfRq(GpuIvfPq):
 
 
 class GpuFlat(_RowsHandle):
-    """A raw vector column pinned in HBM (lgpu_flat).  A float16 array opens an fp16 handle (lgpu_flat_open_f16: the
-    rows stay float16 on the device, results are those of their exact f32 upcast); anything else is converted to f32.
-    `dtype` is the handle's row type."""
+    """A raw vector column searched on the GPU (lgpu_flat).  A float16 array opens an fp16 handle (lgpu_flat_open_f16:
+    the rows stay float16, results are those of their exact f32 upcast); anything else is converted to f32.  `dtype` is
+    the handle's row type.  The rows are kept in HBM when they fit there (LGPU_FLAT_HBM_BYTES), else in pinned host
+    memory and streamed through the GPU once per search, with the same results (`rows_on_host`)."""
     _close = "lgpu_flat_close"
     _delete = "lgpu_flat_delete"
 
@@ -576,6 +578,21 @@ class GpuFlat(_RowsHandle):
         n = C.c_uint64(0)
         check(load().lgpu_flat_device_bytes(self._h, C.byref(n)))
         return n.value
+
+    def _host(self):
+        b, where = C.c_uint64(0), C.c_int(0)
+        check(load().lgpu_flat_host_bytes(self._h, C.byref(b), C.byref(where)))
+        return b.value, where.value
+
+    def host_bytes(self) -> int:
+        """The pinned host memory the handle holds: its rows when they did not fit in HBM at open, else 0
+        (lgpu_flat_host_bytes)."""
+        return self._host()[0]
+
+    @property
+    def rows_on_host(self) -> bool:
+        """True when the rows are kept in pinned host memory and every search streams them through the GPU."""
+        return self._host()[1] == VECTORS_HOST
 
     def search(self, queries, k=10, metric="l2", lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)

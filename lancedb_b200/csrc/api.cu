@@ -163,6 +163,11 @@ struct Workspace {
     DevBuf sel_large;                   // the large select's scratch (k > SELECT_KMAX, select_large.cu)
     DevBuf u_ids, u_dist, u_cnt;        // union search: the index's and the tail's top-k, [2][B][k] and [2][B]
     DevBuf live_and;                    // a filtered call on a handle with deleted rows: its bitmap AND the live rows
+    // a flat handle whose rows are in pinned host memory (flat_search_streamed): two staging buffers of rows, the
+    // staged chunk's tensor-core operand, |x|^2 and |x|, and the running top-k, [2 buffers][2 lists][P][k] / [..][P];
+    // hf_copied[i]: staging buffer i holds its chunk (side stream), hf_free[i]: its chunk was scored (call's stream)
+    DevBuf hf_stage[2], hf_xb, hf_n2, hf_ysqrt, hf_ids, hf_dist, hf_cnt;
+    cudaEvent_t hf_copied[2] = {}, hf_free[2] = {};
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -173,6 +178,10 @@ struct Workspace {
         LGPU_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
         LGPU_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
         for (auto &e : ev) LGPU_CUDA(cudaEventCreate(&e));
+        for (int i = 0; i < 2; i++) {
+            LGPU_CUDA(cudaEventCreateWithFlags(&hf_copied[i], cudaEventDisableTiming));
+            LGPU_CUDA(cudaEventCreateWithFlags(&hf_free[i], cudaEventDisableTiming));
+        }
     }
     ~Workspace()
     {
@@ -183,6 +192,10 @@ struct Workspace {
         if (ev_join) cudaEventDestroy(ev_join);
         if (done) cudaEventDestroy(done);
         for (auto &e : ev) if (e) cudaEventDestroy(e);
+        for (int i = 0; i < 2; i++) {
+            if (hf_copied[i]) cudaEventDestroy(hf_copied[i]);
+            if (hf_free[i]) cudaEventDestroy(hf_free[i]);
+        }
     }
 };
 
@@ -421,6 +434,10 @@ struct lgpu_flat {
     uint32_t dim = 0;
     bool f16 = false;                   // row type: `vectors` holds [nrows][dim] f32, or fp16 (lgpu_flat_open_f16)
     DevBuf vectors, row_ids, ysqrt;
+    // rows that did not fit in HBM at open (flat_open): `rows_host` holds them, [nrows][dim] in the row type, and
+    // `vectors`, `ysqrt`, `vec_b` and `vec_n2` stay empty; searches stream the rows through HBM (flat_search_streamed)
+    bool on_host = false;
+    PinnedBuf rows_host;
     // the tensor-core path: bf16 rows (f32 handles; an fp16 handle's rows are their own operand) + |x|^2
     DevBuf vec_b, vec_n2;
     float vec_max = 0.f, vec_err = 0.f;     // max |x|, max |h(x) - x| (h: bf16 or fp16 rounding, gemm.cu)
@@ -673,6 +690,14 @@ struct TopkOut {
     TopkOut at(uint32_t q0, uint32_t k) const { return {ids + (size_t)q0 * k, dist + (size_t)q0 * k, cnt + q0}; }
 };
 
+// the ids of the columns of a block of scores: ids[c], or base + c without ids (base: the position of the block's first
+// row in its column, nonzero for a chunk of a streamed flat column)
+struct Cols {
+    const uint64_t *ids;
+    uint64_t base;
+    Cols(const uint64_t *i = nullptr, uint64_t b = 0) : ids(i), base(b) {}
+};
+
 // SelectArgs with the fields every mode needs; callers add the optional ones (only, gate, col_ids, range, allow, ...)
 static SelectArgs select_args(int mode, uint32_t B, uint32_t k, TopkOut out)
 {
@@ -694,6 +719,10 @@ static SelectArgs select_cands(const float *vals, const uint64_t *ids, uint64_t 
     SelectArgs s = select_args(2, B, k, out);
     s.dense = vals; s.cand_ids = ids; s.ncols = n; s.inner = n; s.row_stride = n; s.outer_stride = 0;
     return s;
+}
+static void with_cols(SelectArgs &s, Cols c)
+{
+    s.col_ids = c.ids; s.col_base = c.base;
 }
 static void with_range(SelectArgs &s, const lgpu_search_params &sp)
 {
@@ -722,20 +751,20 @@ static size_t large_k_query_bytes(uint32_t k)
 // type (float, or __half for an fp16 flat handle, whose rows X are also the GEMM operand Xb).
 template <class T>
 static void tc_rescore_fixup(Workspace *ws, cudaStream_t st, const float *Q, uint32_t B, const T *X, uint64_t N,
-                             uint32_t d, const uint64_t *col_ids, uint32_t k, uint32_t cap, TopkOut out, float *Dbuf,
-                             uint64_t ld, RowFilter rf)
+                             uint32_t d, Cols cols, uint32_t k, uint32_t cap, TopkOut out, float *Dbuf, uint64_t ld,
+                             RowFilter rf)
 {
     launch_pair_distance(Q, X, ws->t_pos.as<uint64_t>(), B, cap, d, LGPU_L2, ws->t_exact.as<float>(), st);
     launch_select(select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), cap, B, k, out), st);
     launch_dist_matrix(Q, X, B, N, d, 0, nullptr, nullptr, Dbuf, ld, st, ws->flags.as<uint32_t>());
     SelectArgs sc = select_rows(Dbuf, N, ld, B, k, out);
-    sc.col_ids = col_ids; sc.only = ws->flags.as<uint32_t>();
+    with_cols(sc, cols); sc.only = ws->flags.as<uint32_t>();
     sc.allow = rf.bits; sc.allow_bits = rf.nbits;
     launch_select(sc, st);
 }
 
 // Tensor-core shortlist + exact re-score (squared L2 only): the k best of the N rows of X that pass the row filter rf
-// (none: every row) for each of B queries by exact lance-order distance, ids from col_ids (or the row index),
+// (none: every row) for each of B queries by exact lance-order distance, ids from cols,
 // ascending by (distance, id).  Dbuf: [B][ld] f32 scratch.  The shortlist holds the kp best allowed rows by approximate
 // score; queries whose shortlist cannot be proven complete (band_check: it is full and its last score is within the
 // band of the k-th) are redone by the exact kernels in the same stream, without a host round trip.
@@ -750,8 +779,7 @@ template <class T> static void tc_queries(Workspace *ws, cudaStream_t st, const 
 template <class T>
 static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const T *X,
                        const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
-                       const uint64_t *col_ids, uint32_t k, uint32_t kp, TopkOut out, float *Dbuf, uint64_t ld,
-                       RowFilter rf)
+                       Cols cols, uint32_t k, uint32_t kp, TopkOut out, float *Dbuf, uint64_t ld, RowFilter rf)
 {
     constexpr bool f16 = std::is_same<T, __half>::value;
     ws->flags.ensure((size_t)B * 4);
@@ -761,13 +789,13 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, Dbuf, ld, num_sms, st, nullptr, f16);
     SelectArgs sa = select_rows(Dbuf, N, ld, B, kp, {ws->t_ids.as<uint64_t>(), ws->t_dist.as<float>(),
                                                      ws->t_cnt.as<uint32_t>(), ws->t_pos.as<uint64_t>()});
-    sa.col_ids = col_ids;
+    with_cols(sa, cols);
     sa.allow = rf.bits; sa.allow_bits = rf.nbits;
     launch_select(sa, st);
     if (kp >= N) LGPU_CUDA(cudaMemsetAsync(ws->flags.p, 0, (size_t)B * 4, st));   // every row is a candidate
     else launch_band_check(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                            xmax, xerr, d, B, k, kp, ws->flags.as<uint32_t>(), st);
-    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, kp, out, Dbuf, ld, rf);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, cols, k, kp, out, Dbuf, ld, rf);
 }
 
 // Large-N variant of tc_topk_l2 (flat search): a tensor-core pass over a row sample fixes, per query, a
@@ -778,8 +806,8 @@ static void tc_topk_l2(Workspace *ws, cudaStream_t st, int num_sms, const float 
 template <class T>
 static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, const float *Q, uint32_t B, const T *X,
                                 const void *Xb, const float *xnorm2, float xmax, float xerr, uint64_t N, uint32_t d,
-                                const uint64_t *col_ids, uint32_t k, TopkOut out, float *Dbuf, uint64_t ld,
-                                RowFilter rf, uint64_t min_sample = 65536, uint32_t cap = 1024)
+                                Cols cols, uint32_t k, TopkOut out, float *Dbuf, uint64_t ld, RowFilter rf,
+                                uint64_t min_sample = 65536, uint32_t cap = 1024)
 {
     constexpr bool f16 = std::is_same<T, __half>::value;
     const uint64_t Ns = std::min<uint64_t>(N, std::max<uint64_t>(min_sample, N / 8));
@@ -795,7 +823,7 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, Ns, d, Dbuf, lds, num_sms, st, nullptr, f16);
     SelectArgs ss = select_rows(Dbuf, Ns, lds, B, k, {ws->sbound.as<uint64_t>(), ws->t_dist.as<float>(),
                                                       ws->t_cnt.as<uint32_t>()});
-    if (rf.bits) { ss.col_ids = col_ids; ss.allow = rf.bits; ss.allow_bits = rf.nbits; }
+    if (rf.bits) { with_cols(ss, cols); ss.allow = rf.bits; ss.allow_bits = rf.nbits; }
     launch_select(ss, st);
     launch_sample_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), ws->qn2.as<float>(), ws->qerr.as<float>(),
                             xmax, xerr, d, B, k, ws->probe_A.as<float>(), st);
@@ -805,22 +833,22 @@ static void tc_topk_l2_filtered(Workspace *ws, cudaStream_t st, int num_sms, con
     LGPU_CUDA(cudaMemsetAsync(ws->t_ids.p, 0xff, (size_t)B * cap * 8, st));
     GemmFilter flt{};
     flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
-    flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap;
+    flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = cols.ids; flt.col_base = cols.base; flt.cap = cap;
     flt.allow = rf.bits; flt.allow_bits = rf.nbits;
     if (Ns == N) launch_filter_dense(Dbuf, lds, B, N, flt, st);      // the sample pass already scored every row
     else launch_gemm_dist(ws->qb.p, Xb, xnorm2, B, N, d, nullptr, 0, num_sms, st, &flt, f16);
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, ws->probe_A.as<float>(), B, ws->flags.as<uint32_t>(), st);
     // 3. exact re-score of the admitted rows, final top-k; 4. fix-up of overflowed queries
-    tc_rescore_fixup(ws, st, Q, B, X, N, d, col_ids, k, cap, out, Dbuf, ld, rf);
+    tc_rescore_fixup(ws, st, Q, B, X, N, d, cols, k, cap, out, Dbuf, ld, rf);
 }
 
 // top-k by (distance, id) of the dense scores D [b][ld] over N columns, with the request's distance range and
 // prefilter, into `out`
-static void select_dense(Workspace *ws, const float *D, uint64_t N, uint64_t ld, const uint64_t *col_ids, uint32_t b,
+static void select_dense(Workspace *ws, const float *D, uint64_t N, uint64_t ld, Cols cols, uint32_t b,
                          const lgpu_search_params &sp, RowFilter rf, TopkOut out, cudaStream_t st)
 {
     SelectArgs sa = select_rows(D, N, ld, b, sp.k, out);
-    sa.col_ids = col_ids;
+    with_cols(sa, cols);
     with_range(sa, sp);
     sa.allow = rf.bits; sa.allow_bits = rf.nbits;
     launch_select(with_scratch(ws, sa), st);
@@ -1605,7 +1633,57 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const voi
     }
 }
 
-// X: the handle's rows, as stored (T = float, or __half for an fp16 handle); every path reads them as they are
+// N rows of a flat handle as a search scores them: all the rows of an HBM handle, or one chunk of a host handle's
+// staged in HBM.  X: the rows as stored (T = float, or __half for an fp16 handle; every path reads them as they are);
+// Xop, n2: their tensor-core operand and |x|^2 (tc: present, and the handle's band is finite); ysqrt: |x| (cosine)
+template <class T> struct FlatRows {
+    const T *X;
+    const void *Xop;
+    const float *n2, *ysqrt;
+    uint64_t N;
+    Cols cols;
+    bool tc;
+};
+
+// Whether b queries over N rows go to the l2 tensor-core path.  A row filter -- a prefilter, deleted rows -- stays on
+// the tensor cores: the shortlists and thresholds are taken over the allowed rows, DESIGN.md section 3; k above
+// SELECT_KMAX goes through the exact kernels: the shortlists are sized to SELECT_KMAX.
+static bool flat_tc_route(bool tc, int metric, const lgpu_search_params &sp, uint32_t b, uint64_t N)
+{
+    return tc && tc_enabled() && metric == LGPU_L2 && !sp.has_lower && !sp.has_upper && b >= 8 && N >= 4096 &&
+           sp.k <= SELECT_KMAX;
+}
+
+// the k best of the rows r for the b queries q into out (b rows of k)
+template <class T>
+static void flat_score(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *q, uint32_t b,
+                       const lgpu_search_params &sp, const FlatRows<T> &r, TopkOut out, RowFilter rf, bool prof)
+{
+    const uint64_t N = r.N, ld = (N + 3) & ~3ull;
+    ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+    const float *xn = nullptr;
+    if (metric == LGPU_COSINE) {
+        ws->xnorm.ensure((size_t)b * 4);
+        launch_row_norms(q, b, fl->dim, ws->xnorm.as<float>(), st);
+        xn = ws->xnorm.as<float>();
+    }
+    const uint32_t kp = (uint32_t)std::min<uint64_t>(N, std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(8 * sp.k, 256)));
+    if (flat_tc_route(r.tc, metric, sp, b, N)) {
+        if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
+            tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, r.X, r.Xop, r.n2, fl->vec_max, fl->vec_err, N, fl->dim, r.cols,
+                                sp.k, out, ws->D.as<float>(), ld, rf);
+        else
+            tc_topk_l2(ws, st, fl->num_sms, q, b, r.X, r.Xop, r.n2, fl->vec_max, fl->vec_err, N, fl->dim, r.cols, sp.k, kp,
+                       out, ws->D.as<float>(), ld, rf);
+        if (prof) g_filter_stats[1] += (uint64_t)b * N;
+        return;
+    }
+    launch_dist_matrix(q, r.X, b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2), xn, r.ysqrt,
+                       ws->D.as<float>(), ld, st);
+    select_dense(ws, ws->D.as<float>(), N, ld, r.cols, b, sp, rf, out, st);
+}
+
+// an HBM handle: its rows X, the queries in sub-batches that the workspace budget holds the scores of
 template <class T>
 static void flat_search_rows(lgpu_flat *fl, const T *X, Workspace *ws, cudaStream_t st, int metric, const float *d_q,
                              uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
@@ -1627,40 +1705,113 @@ static void flat_search_rows(lgpu_flat *fl, const T *X, Workspace *ws, cudaStrea
     const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));      // [1] tensor-core distances, [3] queries
+    const FlatRows<T> rows{X, fl->f16 ? static_cast<const void *>(X) : fl->vec_b.p, fl->vec_n2.as<float>(),
+                           fl->ysqrt.as<float>(), N, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, fl->has_tc};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-        const float *q = d_q + (size_t)q0 * fl->dim;
-        ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-        const float *xn = nullptr;
-        if (metric == LGPU_COSINE) {
-            ws->xnorm.ensure((size_t)b * 4);
-            launch_row_norms(q, b, fl->dim, ws->xnorm.as<float>(), st);
-            xn = ws->xnorm.as<float>();
-        }
-        const uint32_t kp = (uint32_t)std::min<uint64_t>(N, std::min<uint32_t>(SELECT_KMAX, std::max<uint32_t>(8 * sp.k, 256)));
-        // (a row filter -- a prefilter, deleted rows -- stays on the tensor cores: the shortlists and thresholds are
-        // taken over the allowed rows, DESIGN.md section 3; k above SELECT_KMAX goes through the exact kernels: the
-        // shortlists are sized to SELECT_KMAX)
-        if (fl->has_tc && tc_enabled() && metric == LGPU_L2 && !sp.has_lower && !sp.has_upper && b >= 8 && N >= 4096 &&
-            sp.k <= SELECT_KMAX) {
-            const void *Xop = fl->f16 ? static_cast<const void *>(X) : fl->vec_b.p;   // the GEMM operand
-            if (N >= 262144 && !getenv("LGPU_FLAT_DENSE"))
-                tc_topk_l2_filtered(ws, st, fl->num_sms, q, b, X, Xop, fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N,
-                                    fl->dim, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, out.at(q0, sp.k),
-                                    ws->D.as<float>(), ld, rf);
-            else
-                tc_topk_l2(ws, st, fl->num_sms, q, b, X, Xop, fl->vec_n2.as<float>(), fl->vec_max, fl->vec_err, N, fl->dim,
-                           fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, sp.k, kp, out.at(q0, sp.k),
-                           ws->D.as<float>(), ld, rf);
-            if (prof) g_filter_stats[1] += (uint64_t)b * N;
-            continue;
-        }
-        launch_dist_matrix(q, X, b, N, fl->dim, metric == LGPU_L2 ? 0 : (metric == LGPU_DOT ? 1 : 2),
-                           xn, fl->ysqrt.as<float>(), ws->D.as<float>(), ld, st);
-        select_dense(ws, ws->D.as<float>(), N, ld, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
-                     out.at(q0, sp.k), st);
+        flat_score(fl, ws, st, metric, d_q + (size_t)q0 * fl->dim, b, sp, rows, out.at(q0, sp.k), rf, prof);
     }
+    if (prof) g_filter_stats[3] = B;
+}
+
+// the most rows of a host handle one staging buffer holds, in bytes: large enough that the copy engine runs at the
+// PCIe rate and a chunk's fixed scoring cost is small, small enough that the unoverlapped first copy is short
+constexpr size_t FLAT_STAGE_BYTES = (size_t)128 << 20;
+
+// A host handle (lgpu_flat::on_host): its rows cross PCIe in chunks of C rows, copied into the workspace's two staging
+// buffers on its side stream (`front`, forked from the call's stream and joined back to it), chunk i + 1 while chunk i
+// is scored on the call's stream by the route an HBM handle of that chunk's rows takes (flat_score).  Each chunk's
+// exact top-k is merged into a running top-k per query by (distance, id).  Chunks are the outer loop: a pass over the
+// column serves P queries, all B unless the budget cannot hold the running top-k of that many, in scoring groups of
+// bs queries whose scores fit.  The staging buffers, the chunk's per-row terms and the running lists all count against
+// the workspace budget.  timeout_ms is checked between chunks.
+template <class T>
+static void flat_search_streamed(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *d_q,
+                                 uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist,
+                                 uint32_t *d_cnt, RowFilter rf, const Deadline *deadline)
+{
+    const uint64_t N = fl->nrows;
+    const uint32_t d = fl->dim, k = sp.k;
+    const size_t es = sizeof(T), budget = workspace_budget();
+    // per row of a chunk: two staging copies, the bf16 operand (f32 rows), |x|^2 and |x|
+    const size_t row_b = 2 * (size_t)d * es + (fl->f16 ? 0 : 2 * (size_t)d) + 8;
+    const uint64_t C = std::max<uint64_t>(1, std::min<uint64_t>(std::max<uint64_t>(N, 1),
+                                                                std::min(budget / 2 / row_b, FLAT_STAGE_BYTES / (d * es))));
+    const uint64_t ldc = (C + 3) & ~3ull, nchunks = N ? (N + C - 1) / C : 1;
+    const size_t rest = budget > C * row_b ? budget - C * row_b : 0;
+    // per query: the running top-k (two buffers of two lists of k ids and distances, and their counts), and the scores
+    // of a chunk
+    const size_t run_q = (size_t)k * 48 + 16, score_q = ldc * 4 + large_k_query_bytes(k);
+    const uint32_t P = (uint32_t)std::max<size_t>(1, std::min<size_t>(B, rest / 2 / run_q));
+    const size_t left = rest > (size_t)P * run_q ? rest - (size_t)P * run_q : 0;
+    const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(P, left / score_q));
+    for (auto &b : ws->hf_stage) b.ensure(std::max<size_t>(C * d * es, 16));
+    if (fl->has_tc && !fl->f16) ws->hf_xb.ensure(C * d * 2);
+    ws->hf_n2.ensure(C * 4);
+    if (metric == LGPU_COSINE) ws->hf_ysqrt.ensure(C * 4);
+    if (nchunks > 1) {
+        ws->hf_ids.ensure((size_t)4 * P * k * 8); ws->hf_dist.ensure((size_t)4 * P * k * 4);
+        ws->hf_cnt.ensure((size_t)4 * P * 4);
+    }
+    const TopkOut out{d_ids, d_dist, d_cnt};
+    const bool prof = profiling_enabled();
+    if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));      // [1] tensor-core distances, [3] queries
+    const char *rows = static_cast<const char *>(fl->rows_host.p);
+    const uint64_t steps = (uint64_t)((B + P - 1) / P) * nchunks;      // step s: pass s / nchunks, chunk s % nchunks
+    auto chunk_rows = [&](uint64_t c) { return N ? std::min<uint64_t>(C, N - c * C) : 0; };
+    // the chunk of step s into staging buffer s & 1, once the chunk it held two steps earlier was scored
+    auto copy = [&](uint64_t s) {
+        const int i = (int)(s & 1);
+        const uint64_t c = s % nchunks;
+        if (s >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->hf_free[i], 0));
+        if (const size_t bytes = chunk_rows(c) * d * es)
+            LGPU_CUDA(cudaMemcpyAsync(ws->hf_stage[i].p, rows + c * C * d * es, bytes, cudaMemcpyHostToDevice, ws->front));
+        LGPU_CUDA(cudaEventRecord(ws->hf_copied[i], ws->front));
+    };
+    LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
+    LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
+    ws->front_open = true;
+    copy(0);
+    for (uint64_t s = 0; s < steps; s++) {
+        const uint32_t p0 = (uint32_t)(s / nchunks) * P, pb = std::min(P, B - p0);
+        const uint64_t c = s % nchunks, n = chunk_rows(c);
+        const int i = (int)(s & 1);
+        if (deadline && s > 0) deadline->wait(st, ws->ev[7]);
+        if (s + 1 < steps) copy(s + 1);
+        LGPU_CUDA(cudaStreamWaitEvent(st, ws->hf_copied[i], 0));
+        const T *X = ws->hf_stage[i].as<T>();
+        // the operand only when a scoring group takes the tensor cores (the first group is the largest)
+        const bool tc = flat_tc_route(fl->has_tc, metric, sp, std::min(bs, pb), n);
+        if (tc && fl->f16) launch_f16_row_terms(X, n, d, ws->hf_n2.as<float>(), nullptr, st);
+        else if (tc) launch_to_bf16(reinterpret_cast<const float *>(X), n, d, ws->hf_xb.p, ws->hf_n2.as<float>(), st);
+        if (metric == LGPU_COSINE) launch_row_norms(X, n, d, ws->hf_ysqrt.as<float>(), st);
+        const FlatRows<T> chunk{X, fl->f16 ? static_cast<const void *>(X) : ws->hf_xb.p, ws->hf_n2.as<float>(),
+                                ws->hf_ysqrt.as<float>(), n,
+                                fl->has_ids ? Cols(fl->row_ids.as<uint64_t>() + c * C) : Cols(nullptr, c * C), tc};
+        // list l of running buffer r: [pb][k] entries and [pb] counts.  Chunk 0 goes to list 0 of buffer 0; chunk
+        // c > 0 to list 1 of buffer (c - 1) & 1, merged with its list 0 into list 0 of the other buffer, or into the
+        // output after the last chunk.  A column of one chunk is scored straight into the output.
+        auto run = [&](uint64_t r, uint32_t l) -> TopkOut {
+            const size_t off = (size_t)(2 * r + l) * pb;
+            return {ws->hf_ids.as<uint64_t>() + off * k, ws->hf_dist.as<float>() + off * k, ws->hf_cnt.as<uint32_t>() + off};
+        };
+        const TopkOut pass_out = out.at(p0, k);
+        const TopkOut dst = nchunks == 1 ? pass_out : c == 0 ? run(0, 0) : run((c - 1) & 1, 1);
+        for (uint32_t g0 = 0; g0 < pb; g0 += bs)
+            flat_score(fl, ws, st, metric, d_q + (size_t)(p0 + g0) * d, std::min(bs, pb - g0), sp, chunk, dst.at(g0, k),
+                       rf, prof);
+        LGPU_CUDA(cudaEventRecord(ws->hf_free[i], st));
+        if (c > 0) {
+            const TopkOut a = run((c - 1) & 1, 0);
+            SelectArgs m = select_cands(a.dist, a.ids, k, pb, k, c + 1 == nchunks ? pass_out : run(c & 1, 0));
+            m.ncols = 2 * (uint64_t)k; m.outer_stride = (uint64_t)pb * k; m.list_cnt = a.cnt;
+            launch_select(with_scratch(ws, m), st);
+        }
+    }
+    LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
+    LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));
+    ws->front_open = false;
     if (prof) g_filter_stats[3] = B;
 }
 
@@ -1668,8 +1819,14 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
                         const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                         RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
 {
-    if (fl->f16) flat_search_rows(fl, fl->vectors.as<__half>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
-    else flat_search_rows(fl, fl->vectors.as<float>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    if (fl->on_host && fl->f16)
+        flat_search_streamed<__half>(fl, ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    else if (fl->on_host)
+        flat_search_streamed<float>(fl, ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    else if (fl->f16)
+        flat_search_rows(fl, fl->vectors.as<__half>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    else
+        flat_search_rows(fl, fl->vectors.as<float>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
 }
 
 // ---- binary vectors (Hamming distance) ----
@@ -2184,6 +2341,11 @@ static Route filtered_route(const uint32_t *allow, uint64_t allow_bits)
 }
 static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, stream}; }
 
+// Whether the host route may capture a handle's calls into a CUDA graph: not a flat handle whose rows are on the host,
+// whose calls stream from pinned memory that an append moves, on a side stream (flat_search_streamed)
+template <class H> static bool graph_capturable(const H *) { return true; }
+static bool graph_capturable(const lgpu_flat *fl) { return !fl->on_host; }
+
 // The sequence of every search entry point: resolve the handle; the kind's own checks, `check(h)`, which return how
 // many query elements (T) the call reads; the bitmap of a filtered call; nothing more for B == 0; the device; then
 // the kind's `search(h, ws, st, d_q, B, params, d_ids, d_dist, d_cnt, rf, deadline)` on a workspace leased for the
@@ -2206,8 +2368,9 @@ int search_call(H *hp, const Route &r, const T *queries, uint32_t B, const lgpu_
             return;
         }
         uint64_t key[4];
-        if (r.graph_tag) make_key(key, r.graph_tag, B, *p);
-        host_call(h->pool, queries, q_elems, B, p->k, ids, dist, cnt, r.graph_tag ? key : nullptr, p->timeout_ms,
+        const bool graph = r.graph_tag && graph_capturable(h.h);
+        if (graph) make_key(key, r.graph_tag, B, *p);
+        host_call(h->pool, queries, q_elems, B, p->k, ids, dist, cnt, graph ? key : nullptr, p->timeout_ms,
                   [&](Workspace *ws, cudaStream_t st, const T *dq, uint64_t *di, float *dd, uint32_t *dc,
                       const Deadline &dl) {
                       const RowFilter rf = r.via == Route::FILTERED ? upload_allow(ws, st, r.allow, r.allow_bits)
@@ -2500,6 +2663,18 @@ static uint64_t index_device_bytes(const lgpu_index *ix)
     return n;
 }
 
+// Whether `bytes` of a handle's rows go to HBM at open: at most the cap the variable `cap_var` sets (read at every open;
+// unset = no cap, 0 = never HBM), and the device's free memory covers them plus the workspace budget (LGPU_WS_BYTES)
+// the handle's searches may lease
+static bool rows_fit_hbm(const char *cap_var, uint64_t bytes)
+{
+    const char *e = getenv(cap_var);
+    const uint64_t cap = (e && *e) ? strtoull(e, nullptr, 10) : UINT64_MAX;
+    size_t free_b = 0, total_b = 0;
+    LGPU_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    return cap > 0 && bytes <= cap && (uint64_t)free_b >= bytes + workspace_budget();
+}
+
 // Where an index keeps its raw vectors ([nrows][dim] f32 on the host, borrowed for the open call), decided after
 // everything else the index holds is in HBM.  HBM when they fit with room to spare: at most LGPU_VECTORS_HBM_BYTES of
 // them (read at every open; unset = no cap, 0 = never HBM), and the device's free memory covers them plus the
@@ -2511,11 +2686,7 @@ static void place_vectors(lgpu_index *ix, const float *vectors)
     if (!vectors) return;
     ix->has_vectors = true;
     const uint64_t n = ix->nrows, dim = ix->dim, bytes = n * dim * 4;
-    const char *e = getenv("LGPU_VECTORS_HBM_BYTES");
-    const uint64_t cap = (e && *e) ? strtoull(e, nullptr, 10) : UINT64_MAX;
-    size_t free_b = 0, total_b = 0;
-    LGPU_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    if (cap > 0 && bytes <= cap && (uint64_t)free_b >= bytes + workspace_budget()) {
+    if (rows_fit_hbm("LGPU_VECTORS_HBM_BYTES", bytes)) {
         ix->vectors.ensure(std::max<size_t>(bytes, 16), true);
         if (bytes) LGPU_CUDA(cudaMemcpy(ix->vectors.p, vectors, bytes, cudaMemcpyHostToDevice));
         return;
@@ -3187,7 +3358,42 @@ int lgpu_merge_topk_device(int device, uint32_t nlists, uint32_t B, uint32_t k, 
     });
 }
 
-// lgpu_flat_open and lgpu_flat_open_f16: rows f32 or fp16 (f16), kept on the device as given
+// The row data of a flat handle of n rows in HBM: the rows, and the tensor-core operand the handle builds for them (a
+// bf16 copy for f32 rows; fp16 rows are their own) and |x|^2
+static uint64_t flat_row_data_bytes(uint64_t n, uint32_t d, bool f16)
+{
+    const uint64_t rows = n * d * (f16 ? 2 : 4);
+    if (!gemm_shape_supported(d) || n < 4096) return rows;
+    return rows + (f16 ? 0 : n * d * 2) + n * 4;
+}
+
+// The tensor-core band of n rows in host memory (a host handle's rows at open or append): tc_operand_rows over chunks
+// staged through HBM, the maxima of their constants, so xmax and xerr are those of the whole rows.  False when a row
+// has no finite band.
+static bool host_rows_band(const void *rows, bool f16, uint64_t n, uint32_t d, float &xmax, float &xerr)
+{
+    const size_t es = f16 ? 2 : 4;
+    const uint64_t C = std::max<uint64_t>(1, std::min<uint64_t>(n, FLAT_STAGE_BYTES / ((size_t)d * es)));
+    DevBuf x, xb, n2;
+    x.ensure(C * d * es);
+    if (!f16) xb.ensure(C * d * 2);
+    n2.ensure(C * 4);
+    bool finite = true;
+    xmax = xerr = 0.f;
+    for (uint64_t r = 0; r < n; r += C) {
+        const uint64_t m = std::min(C, n - r);
+        LGPU_CUDA(cudaMemcpy(x.p, static_cast<const char *>(rows) + r * d * es, m * d * es, cudaMemcpyHostToDevice));
+        float a = 0.f, e = 0.f;
+        finite &= tc_operand_rows(x.p, f16, m, d, xb.p, n2.as<float>(), a, e, nullptr);
+        xmax = std::max(xmax, a);
+        xerr = std::max(xerr, e);
+    }
+    return finite;
+}
+
+// lgpu_flat_open and lgpu_flat_open_f16: rows f32 or fp16 (f16), kept as given in HBM when their row data fits there
+// (LGPU_FLAT_HBM_BYTES, rows_fit_hbm), else in pinned host memory the handle owns.  HBM rows and their operand are
+// allocated exactly, so that device bytes of the two placements differ by the row data.
 static int flat_open(const void *vectors, bool f16, uint64_t nrows, uint32_t dim, const uint64_t *row_ids, int device,
                      lgpu_flat **out)
 {
@@ -3198,14 +3404,25 @@ static int flat_open(const void *vectors, bool f16, uint64_t nrows, uint32_t dim
         require_device(device);
         fl = new lgpu_flat();
         fl->device = device; fl->nrows = nrows; fl->dim = dim; fl->f16 = f16;
-        const size_t es = f16 ? 2 : 4;
-        fl->vectors.ensure(std::max<size_t>((size_t)nrows * dim * es, 16), f16);
-        if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, (size_t)nrows * dim * es, cudaMemcpyHostToDevice));
-        if (gemm_shape_supported(dim) && nrows >= 4096) {
+        const size_t es = f16 ? 2 : 4, bytes = (size_t)nrows * dim * es;
+        const bool tc_shape = gemm_shape_supported(dim) && nrows >= 4096;
+        if (!rows_fit_hbm("LGPU_FLAT_HBM_BYTES", flat_row_data_bytes(nrows, dim, f16))) {
+            fl->on_host = true;
+            fl->rows_host.alloc(bytes);
+            if (bytes) memcpy(fl->rows_host.p, vectors, bytes);
             // a non-finite or overflowing row: the exact kernels serve the column
-            fl->has_tc = prepare_tc_operand(fl->vectors.p, f16, nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
-                                            fl->vec_err, nullptr);
-            if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
+            if (tc_shape) fl->has_tc = host_rows_band(fl->rows_host.p, f16, nrows, dim, fl->vec_max, fl->vec_err);
+        } else {
+            fl->vectors.ensure(std::max<size_t>(bytes, 16), true);
+            if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, bytes, cudaMemcpyHostToDevice));
+            if (tc_shape) {
+                if (!f16) fl->vec_b.ensure((size_t)nrows * dim * 2, true);
+                fl->vec_n2.ensure((size_t)nrows * 4, true);
+                // a non-finite or overflowing row: the exact kernels serve the column
+                fl->has_tc = prepare_tc_operand(fl->vectors.p, f16, nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
+                                                fl->vec_err, nullptr);
+                if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
+            }
         }
         open_rows(fl, row_ids, nrows);
         register_handle(fl);
@@ -3235,6 +3452,16 @@ int lgpu_flat_device_bytes(const lgpu_flat *flh, uint64_t *bytes)
         const lgpu_flat *fl = h.h;
         *bytes = fl->vectors.bytes + fl->row_ids.bytes + fl->ysqrt.bytes + fl->vec_b.bytes + fl->vec_n2.bytes +
                  fl->live.bits.bytes;
+    });
+}
+
+int lgpu_flat_host_bytes(const lgpu_flat *flh, uint64_t *bytes, int *placement)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(bytes || placement, "null argument");
+        HandleRef<lgpu_flat> fl(const_cast<lgpu_flat *>(flh));
+        if (bytes) *bytes = fl->rows_host.bytes;
+        if (placement) *placement = fl->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
     });
 }
 
@@ -3412,6 +3639,18 @@ static void grow_keep(DevBuf &b, size_t used, size_t need)
     std::swap(b.bytes, nb.bytes);
 }
 
+// ... and the pinned rows of a host handle, moved by a host copy
+static void grow_keep(PinnedBuf &b, size_t used, size_t need)
+{
+    if (need <= b.bytes) return;
+    PinnedBuf nb;
+    nb.alloc(std::max(need, 2 * b.bytes));
+    if (used) memcpy(nb.p, b.p, used);
+    std::swap(b.p, nb.p);
+    std::swap(b.dev, nb.dev);
+    std::swap(b.bytes, nb.bytes);
+}
+
 // The row ids after an append of n rows to n0: explicit ids stay explicit (positions n0.. when none are given), and
 // ids given to a handle that had none make the old rows' positions explicit.
 template <class H> static void append_ids(H *h, uint64_t n0, uint64_t n, const uint64_t *row_ids)
@@ -3568,6 +3807,28 @@ static int flat_append(lgpu_flat *flh, const void *rows, bool f16, uint64_t n, c
         const uint64_t n0 = fl->nrows, n1 = n0 + n;
         const uint32_t d = fl->dim;
         const size_t es = f16 ? 2 : 4;
+        if (fl->on_host) {
+            grow_keep(fl->rows_host, (size_t)n0 * d * es, (size_t)n1 * d * es);
+            char *x = static_cast<char *>(fl->rows_host.p) + (size_t)n0 * d * es;
+            memcpy(x, rows, (size_t)n * d * es);
+            append_ids(fl, n0, n, row_ids);
+            grow_live(fl, n0, n, bound);
+            // the band as lgpu_flat_open takes it from n1 rows: the whole column when it first reaches 4096 rows, else
+            // the new rows', the constants the max over both parts
+            if (gemm_shape_supported(d) && n1 >= 4096) {
+                if (n0 < 4096) {
+                    fl->has_tc = host_rows_band(fl->rows_host.p, f16, n1, d, fl->vec_max, fl->vec_err);
+                } else if (fl->has_tc) {
+                    float xmax = 0.f, xerr = 0.f;
+                    fl->has_tc = host_rows_band(x, f16, n, d, xmax, xerr);
+                    fl->vec_max = std::max(fl->vec_max, xmax);
+                    fl->vec_err = std::max(fl->vec_err, xerr);
+                }
+            }
+            LGPU_CUDA(cudaDeviceSynchronize());
+            fl->nrows = n1;
+            return;
+        }
         grow_keep(fl->vectors, (size_t)n0 * d * es, (size_t)n1 * d * es);
         char *x = fl->vectors.as<char>() + (size_t)n0 * d * es;
         LGPU_CUDA(cudaMemcpy(x, rows, (size_t)n * d * es, cudaMemcpyHostToDevice));

@@ -393,7 +393,7 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                                     flt.cand_pos[(size_t)q * flt.cap + slot] = c0 + 8 * j + e;
                                     flt.cand_s[(size_t)q * flt.cap + slot] = Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], pq);
                                     if constexpr (Pol::BIN)
-                                        flt.cand_ids[(size_t)q * flt.cap + slot] = flt.col_ids ? flt.col_ids[c0 + 8 * j + e] : c0 + 8 * j + e;
+                                        flt.cand_ids[(size_t)q * flt.cap + slot] = gemm_filter_id(flt, c0 + 8 * j + e);
                                 }
                                 slot++;
                             }
@@ -419,7 +419,7 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                             const uint32_t slot = atomicAdd(flt.count + q, 1u);
                             if (slot < flt.cap) {
                                 flt.cand_pos[(size_t)q * flt.cap + slot] = x;
-                                if (flt.cand_ids) flt.cand_ids[(size_t)q * flt.cap + slot] = flt.col_ids ? flt.col_ids[x] : x;
+                                if (flt.cand_ids) flt.cand_ids[(size_t)q * flt.cap + slot] = gemm_filter_id(flt, x);
                             }
                         }
                     }
@@ -720,7 +720,7 @@ __global__ void filter_dense_kernel(const float *__restrict__ D, uint64_t ld, ui
             const uint32_t slot = atomicAdd(flt.count + q, 1u);
             if (slot < flt.cap) {
                 flt.cand_pos[(size_t)q * flt.cap + slot] = x;
-                flt.cand_ids[(size_t)q * flt.cap + slot] = flt.col_ids ? flt.col_ids[x] : x;
+                flt.cand_ids[(size_t)q * flt.cap + slot] = gemm_filter_id(flt, x);
             }
         }
     }

@@ -321,7 +321,8 @@ struct SelectArgs {
     uint64_t ncols;               // candidates per query
     uint64_t row_stride;          // mode 1: ld; mode 2: stride between queries
     uint64_t inner, outer_stride; // mode 2: col -> (col/inner)*outer_stride + q*row_stride + col%inner
-    const uint64_t *col_ids;      // mode 1: optional id per column (NULL => column index)
+    const uint64_t *col_ids;      // mode 1: optional id per column (NULL => col_base + column index)
+    uint64_t col_base;            // mode 1: the id of column 0 when col_ids is NULL (a chunk of a streamed column)
     const uint64_t *cand_ids;     // mode 2: id per entry (same addressing as dense)
     const uint64_t *cand_pos;     // mode 2: optional pos per entry
     const uint32_t *ncols_q;      // mode 2: optional [B] candidates of each query (<= ncols)
@@ -403,19 +404,25 @@ struct GemmFilter {
     const float *thr;             // [B]; nullptr = dense output
     uint32_t *count;              // [B], zeroed by the caller
     uint64_t *cand_pos;           // [B][cap] column (storage row) of each candidate
-    uint64_t *cand_ids;           // [B][cap] its id (col_ids[x] or x)
+    uint64_t *cand_ids;           // [B][cap] its id (gemm_filter_id)
     const uint64_t *col_ids;      // optional
+    uint64_t col_base;            // without col_ids, the id of column 0 (a chunk of a streamed column)
     uint32_t cap;
     float *cand_s;                // optional [B][cap]: the admitted score itself (coarse step: second-level threshold)
-    // optional row filter: a column passing the threshold is admitted only if the bit of its id (col_ids[x] or x) is
+    // optional row filter: a column passing the threshold is admitted only if the bit of its id (gemm_filter_id) is
     // set, id < allow_bits (a prefilter, deleted rows)
     const uint32_t *allow;
     uint64_t allow_bits;
 };
+// the id of column x: col_ids[x], or col_base + x
+__device__ __forceinline__ uint64_t gemm_filter_id(const GemmFilter &f, uint64_t x)
+{
+    return f.col_ids ? f.col_ids[x] : f.col_base + x;
+}
 // whether column x passes the row filter of a filter that has one (tested only for columns under the threshold)
 __device__ __forceinline__ bool gemm_filter_admits(const GemmFilter &f, uint64_t x)
 {
-    const uint64_t id = f.col_ids ? f.col_ids[x] : x;
+    const uint64_t id = gemm_filter_id(f, x);
     return id < f.allow_bits && ((__ldg(f.allow + (id >> 5)) >> (id & 31)) & 1u);
 }
 void launch_gemm_dist(const void *Qb, const void *Xb, const float *xnorm2, uint32_t B, uint64_t N, uint32_t d,

@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_kernel(SelectArgs a, uint3
             }
 #pragma unroll
             for (int u = 0; u < 4; u++) ok[u] = c + u < a.ncols;
-            offer4(v, ok, c, a.col_ids, c);
+            offer4(v, ok, a.col_ids ? c : a.col_base + c, a.col_ids, c);
             if (__syncthreads_or(s_cnt >= trigger)) compact();
         }
     } else {
@@ -319,7 +319,9 @@ __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs
         }
     };
     // one warp-iteration = 256 consecutive values of `src` starting at r0 (n values in total)
-    auto scan256 = [&](const float *src, uint64_t r0, uint64_t n, bool vec, uint64_t idbase, const uint64_t *idsrc) {
+    // (ids from idsrc[idbase + r], or idbase + r without idsrc; positions posbase + r)
+    auto scan256 = [&](const float *src, uint64_t r0, uint64_t n, bool vec, uint64_t posbase, uint64_t idbase,
+                       const uint64_t *idsrc) {
         const uint64_t ra = r0 + (uint64_t)lane * 4, rb = ra + 128;
         float4 ta = make_float4(0.f, 0.f, 0.f, 0.f), tb = ta;
         if (vec) {
@@ -333,8 +335,8 @@ __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs
                 if (rb + u < n) pb[u] = src[rb + u];
             }
         }
-        offer4(ta, ra < n ? n - ra : 0, idbase + ra, idsrc, idbase + ra);
-        offer4(tb, rb < n ? n - rb : 0, idbase + rb, idsrc, idbase + rb);
+        offer4(ta, ra < n ? n - ra : 0, idbase + ra, idsrc, posbase + ra);
+        offer4(tb, rb < n ? n - rb : 0, idbase + rb, idsrc, posbase + rb);
     };
 
     if (a.mode == 0) {
@@ -348,14 +350,14 @@ __global__ void __launch_bounds__(SELW_WARPS * 32) select_warp_kernel(SelectArgs
             const float *src = a.dist + a.seg_off[slot];
             const uint64_t rowbase = a.part_off[p];
             for (uint32_t r0 = 0; r0 < n; r0 += 256, itc++)
-                if ((itc & (SELW_WARPS - 1)) == (uint32_t)w) scan256(src, r0, n, true, rowbase, a.row_ids);
+                if ((itc & (SELW_WARPS - 1)) == (uint32_t)w) scan256(src, r0, n, true, rowbase, rowbase, a.row_ids);
         }
     } else if (a.mode == 1) {
         const float *src = a.dense + (size_t)q * a.row_stride;
         const bool aligned = ((a.row_stride & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.dense) & 15) == 0);
         for (uint64_t c0 = (uint64_t)w * 256; c0 < a.ncols; c0 += 256 * SELW_WARPS) {
             const bool vec = aligned && c0 + 256 <= a.ncols;
-            scan256(src, c0, a.ncols, vec, 0, a.col_ids);
+            scan256(src, c0, a.ncols, vec, 0, a.col_ids ? 0 : a.col_base, a.col_ids);
         }
     } else {
         const uint64_t ncols = a.ncols_q ? min((uint64_t)a.ncols_q[q], a.ncols) : a.ncols;

@@ -118,7 +118,7 @@ __device__ __forceinline__ void for_each_candidate(const SelectArgs &a, uint32_t
         }
     } else if (a.mode == 1) {
         const float *src = a.dense + (size_t)q * a.row_stride;
-        for (uint64_t c = first; c < a.ncols; c += step) offer(src[c], c, a.col_ids, c, false);
+        for (uint64_t c = first; c < a.ncols; c += step) offer(src[c], a.col_ids ? c : a.col_base + c, a.col_ids, c, false);
     } else {
         const uint64_t ncols = a.ncols_q ? min((uint64_t)a.ncols_q[q], a.ncols) : a.ncols;
         for (uint64_t c = first; c < ncols; c += step) {
