@@ -66,7 +66,8 @@ typedef enum {
 typedef struct lgpu_index lgpu_index;   /* an IVF_PQ index resident in HBM */
 typedef struct lgpu_flat lgpu_flat;     /* a raw vector column resident in HBM */
 typedef struct lgpu_binary lgpu_binary; /* a packed binary (uint8) vector column in HBM, searched by Hamming distance */
-typedef struct lgpu_multivec lgpu_multivec; /* a multivector column in HBM, searched by late interaction (MaxSim) */
+typedef struct lgpu_multivec lgpu_multivec; /* a multivector column in HBM or pinned host memory, searched by late
+                                             * interaction (MaxSim) */
 typedef struct lgpu_ivf_binary lgpu_ivf_binary; /* a binary IVF_FLAT index in HBM, searched by Hamming distance */
 
 /* The arrays of one IVF_PQ index (lance v2 `IvfPq`,
@@ -566,6 +567,28 @@ int  lgpu_multivec_search_filtered(lgpu_multivec *mv, const float *queries, cons
 int  lgpu_multivec_search_device(lgpu_multivec *mv, const float *d_queries, const uint32_t *q_offsets, uint32_t B,
                                  const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
                                  uint32_t *d_out_count, void *cuda_stream);
+/* *bytes = the device memory the handle holds for its vectors and their per-vector and per-row data (f32 vectors,
+ * tensor-core operand, |v|, the row of each vector, offsets, row ids, the live bitmap); the per-call search workspaces
+ * (each within LGPU_WS_BYTES) are not counted.  A handle whose row data is in host memory (lgpu_multivec_host_bytes)
+ * holds only |v|, the row of each vector, the offsets, row ids and live bitmap here: 8 bytes per vector. */
+int  lgpu_multivec_device_bytes(const lgpu_multivec *mv, uint64_t *bytes);
+/* Where a multivector handle keeps its row data: the f32 vectors, plus the fp16 normalised tensor-core operand of a
+ * column of the tensor-core shape (at least 65536 vectors, fewer than 2^31, dim a multiple of 8).  lgpu_multivec_open
+ * copies it into HBM when it is at most LGPU_MULTIVEC_HBM_BYTES (read at every open; unset = no cap, 0 = never in HBM)
+ * and the device's free memory covers it plus the workspace budget (LGPU_WS_BYTES, default 8 GiB).  Otherwise the
+ * handle copies the vectors into pinned host memory that it owns and builds the operand there, both [T][dim] (freed by
+ * lgpu_multivec_close).  Every search of such a handle (host, _filtered, _device) streams chunks of whole rows through
+ * two staging buffers of its workspace, within LGPU_WS_BYTES: each vector crosses PCIe once per call when the
+ * workspace holds the per-query state of all B queries, else once per group of queries it holds; the tensor-core
+ * route reads the fp16 operand and re-scores its shortlist from the pinned f32 vectors.  A staging buffer holds the
+ * longest row: a search of a handle whose longest row does not fit twice in LGPU_WS_BYTES fails with LGPU_OOM before
+ * any device work.  Results are identical to an HBM handle's on the same rows -- same ids, counts and distance bits --
+ * for every k, distance_range, prefilter and deleted rows, and lgpu_last_filter_stats means the same.  A handle keeps
+ * its placement for life.  A pinned allocation that fails is LGPU_OOM.  The caller's buffers are borrowed for the
+ * open call only, either way.
+ * *bytes = the pinned host memory the handle holds (T x dim x 4, plus T x dim x 2 for the operand; 0 for an HBM
+ * handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output may be NULL. */
+int  lgpu_multivec_host_bytes(const lgpu_multivec *mv, uint64_t *bytes, int *placement);
 
 /* ---- per-stage access (parity localisation and kernel benchmarks) -------- */
 /* coarse stage only: the nprobes nearest partitions of each query and their

@@ -50,6 +50,7 @@ EXPORTS = [
     "lgpu_index_delete", "lgpu_ivf_binary_delete", "lgpu_flat_delete", "lgpu_binary_delete", "lgpu_multivec_delete",
     "lgpu_flat_open_f16", "lgpu_flat_append_f16", "lgpu_flat_device_bytes",
     "lgpu_index_host_bytes", "lgpu_debug_refine_host", "lgpu_flat_host_bytes",
+    "lgpu_multivec_device_bytes", "lgpu_multivec_host_bytes",
 ]
 VECTORS_NONE, VECTORS_HBM, VECTORS_HOST = 0, 1, 2     # lgpu_vectors_placement
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
@@ -213,6 +214,8 @@ def load():
     lib.lgpu_multivec_search.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
     lib.lgpu_multivec_search_filtered.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, C.c_uint64, vp, vp, vp]
     lib.lgpu_multivec_search_device.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
+    lib.lgpu_multivec_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.lgpu_multivec_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
     lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_sq_open.argtypes = [C.POINTER(SqDesc), C.POINTER(vp)]
     lib.lgpu_debug_sq_distances.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
@@ -719,8 +722,10 @@ def multivec_offsets(lengths) -> np.ndarray:
 
 
 class GpuMultivec(_RowsHandle):
-    """A multivector column (list<fixed_size_list<float, dim>>) pinned in HBM (lgpu_multivec), searched by late
-    interaction: _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors."""
+    """A multivector column (list<fixed_size_list<float, dim>>) (lgpu_multivec), searched by late interaction:
+    _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors.  Its vectors are
+    kept in HBM when they fit (LGPU_MULTIVEC_HBM_BYTES), else in pinned host memory and streamed through the GPU once
+    per search, with the same results (`rows_on_host`)."""
     _close = "lgpu_multivec_close"
     _delete = "lgpu_multivec_delete"
 
@@ -745,6 +750,28 @@ class GpuMultivec(_RowsHandle):
         check(load().lgpu_multivec_open(_ptr(v), _ptr(off), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
+
+    @property
+    def device_bytes(self) -> int:
+        """The HBM the handle holds for its vectors and per-vector data (lgpu_multivec_device_bytes)."""
+        n = C.c_uint64(0)
+        check(load().lgpu_multivec_device_bytes(self._h, C.byref(n)))
+        return n.value
+
+    def _host(self):
+        b, where = C.c_uint64(0), C.c_int(0)
+        check(load().lgpu_multivec_host_bytes(self._h, C.byref(b), C.byref(where)))
+        return b.value, where.value
+
+    def host_bytes(self) -> int:
+        """The pinned host memory the handle holds: its vectors (and tensor-core operand) when they did not fit in HBM
+        at open, else 0 (lgpu_multivec_host_bytes)."""
+        return self._host()[0]
+
+    @property
+    def rows_on_host(self) -> bool:
+        """True when the vectors are kept in pinned host memory and every search streams them through the GPU."""
+        return self._host()[1] == VECTORS_HOST
 
     def _queries(self, queries, q_offsets):
         """(values [Tq, dim] f32, offsets [B+1] u32).  queries: a list with one [nq_b, dim] (or [dim]) array per

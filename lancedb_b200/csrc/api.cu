@@ -474,6 +474,11 @@ struct lgpu_multivec {
     DevBuf vectors, ysqrt, offsets, row_ids;   // [T][dim] f32, |v| = sqrt(dot(v, v)) per vector, [nrows+1], optional ids
     DevBuf vec_h, col_row;                 // tensor-core path: fp16 normalised vectors [T][dim], row of each vector [T]
     bool tc_ok = false;                    // the tensor-core path may run (see multivec_search_device)
+    // row data that did not fit in HBM at open (lgpu_multivec_open): `vectors_host` holds the f32 vectors and
+    // `vec_h_host` the fp16 operand (tensor-core shape only), both [T][dim]; `vectors` and `vec_h` stay empty, and
+    // searches stream the rows through HBM (multivec_search_streamed)
+    bool on_host = false;
+    PinnedBuf vectors_host, vec_h_host;
     std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
     bool has_ids = false;
     RowLive live;
@@ -2010,12 +2015,14 @@ constexpr uint32_t MV_MAX_DIM = 65536;
 // Workspace stays inside LGPU_WS_BYTES.
 constexpr uint64_t MV_TC_MIN_T = 65536;   // stored vectors from which the tensor-core path runs (not measured)
 
-// the exact distances of queries [qa, qb) into D[b - qa][N] (only / vflags / gate: the fix-up of flagged queries)
+// the exact distances of queries [qa, qb) to rows [ra, rb) into D[b - qa][ra..rb) (only / vflags / gate: the fix-up of
+// flagged queries).  X holds the vectors of those rows, from the first vector of row ra (a host handle's staged chunk);
+// the order of the additions per row depends only on the blocking of the query vectors, not on [ra, rb).
 static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
-                           uint32_t qa, uint32_t qb, float *D, uint64_t ld, const uint32_t *only = nullptr,
-                           const uint32_t *vflags = nullptr, const uint32_t *gate = nullptr)
+                           uint32_t qa, uint32_t qb, float *D, uint64_t ld, const float *X, uint64_t ra, uint64_t rb,
+                           const uint32_t *only = nullptr, const uint32_t *vflags = nullptr,
+                           const uint32_t *gate = nullptr)
 {
-    const uint64_t N = mv->nrows;
     const uint32_t dim = mv->dim;
     const size_t budget = workspace_budget();
     // a chunk of rows costs (n_r + 1) floats per query vector in the block (P and M); every row fits in half a chunk
@@ -2030,15 +2037,15 @@ static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, co
         uint32_t bhi = blo;
         while (bhi < qb && h_qoff[bhi] < i1) bhi++;                  // one past the last
         const uint64_t cap = std::max<uint64_t>(pair_floats / nqv, 2 * row_cost);
-        for (uint64_t r0 = 0; r0 < N;) {
+        for (uint64_t r0 = ra; r0 < rb;) {
             uint64_t r1 = r0 + 1;
-            while (r1 < N && (off[r1 + 1] - off[r0]) + (r1 + 1 - r0) <= cap) r1++;
+            while (r1 < rb && (off[r1 + 1] - off[r0]) + (r1 + 1 - r0) <= cap) r1++;
             const uint64_t span = off[r1] - off[r0], ldP = (span + 3) & ~3ull;
             const uint32_t nr = (uint32_t)(r1 - r0);
             ws->mv_P.ensure(std::max<size_t>((size_t)nqv * ldP, 4) * 4);
             ws->mv_M.ensure((size_t)nqv * nr * 4);
             if (span)
-                launch_dist_matrix(d_q + (size_t)i0 * dim, mv->vectors.as<float>() + (size_t)off[r0] * dim, nqv, span,
+                launch_dist_matrix(d_q + (size_t)i0 * dim, X + (size_t)(off[r0] - off[ra]) * dim, nqv, span,
                                    dim, 2, ws->xnorm.as<float>() + i0, mv->ysqrt.as<float>() + off[r0],
                                    ws->mv_P.as<float>(), ldP, st, vflags ? vflags + (i0 - h_qoff[qa]) : nullptr, gate);
             launch_mv_rowmin(ws->mv_P.as<float>(), ldP, nqv, mv->offsets.as<uint64_t>(), r0, nr, ws->mv_M.as<float>(),
@@ -2047,6 +2054,191 @@ static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, co
                              mv->num_sms, st, only, gate);
             r0 = r1;
         }
+    }
+}
+
+// ---- a host multivector handle (lgpu_multivec::on_host): its row data crosses PCIe in chunks of whole rows ----
+// The bytes of one staging buffer: FLAT_STAGE_BYTES, or an eighth of the budget when that is smaller, and never less
+// than the longest row's f32 vectors.  Two such buffers must fit the budget (mv_check_stage, before any device work).
+static size_t mv_stage_bytes(const lgpu_multivec *mv)
+{
+    const size_t longest = (size_t)mv->max_row * mv->dim * 4;
+    return std::max<size_t>(std::min(FLAT_STAGE_BYTES, workspace_budget() / 8), std::max<size_t>(longest, 16));
+}
+
+static void mv_check_stage(const lgpu_multivec *mv)
+{
+    const size_t longest = (size_t)mv->max_row * mv->dim * 4;
+    if (mv->on_host && 2 * longest > workspace_budget()) {
+        set_error("a multivector row of " + std::to_string(mv->max_row) + " vectors (" + std::to_string(longest) +
+                  " bytes) does not fit twice in the workspace budget (LGPU_WS_BYTES) that streams a host handle");
+        throw Failure{LGPU_OOM};
+    }
+}
+
+// the rows of each chunk: bounds cut[c]..cut[c + 1], whole rows of at most `cap_vec` vectors in all (a longer row
+// is a chunk of its own)
+static std::vector<uint64_t> mv_chunks(const lgpu_multivec *mv, uint64_t cap_vec)
+{
+    const uint64_t *off = mv->h_offsets.data();
+    std::vector<uint64_t> cut{0};
+    for (uint64_t r = 0; r < mv->nrows;) {
+        uint64_t r1 = r + 1;
+        while (r1 < mv->nrows && off[r1 + 1] - off[r] <= cap_vec) r1++;
+        cut.push_back(r1);
+        r = r1;
+    }
+    return cut;
+}
+
+// Copies chunk c of `src` (pinned, `vb` bytes per stored vector) into staging buffer c & 1 on the side stream (`front`,
+// forked from the call's stream and joined back to it), chunk c + 1 while chunk c is scored on the call's stream by
+// score(c, staged vectors): flat_search_streamed's pipeline, on the same buffers and events.  timeout_ms is checked
+// between chunks.
+template <class F>
+static void mv_stream(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const void *src, size_t vb,
+                      const std::vector<uint64_t> &cut, const Deadline *deadline, F &&score)
+{
+    const uint64_t *off = mv->h_offsets.data();
+    const size_t nch = cut.size() - 1;
+    auto copy = [&](size_t c) {
+        const int i = (int)(c & 1);
+        if (c >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->hf_free[i], 0));
+        if (const size_t bytes = (off[cut[c + 1]] - off[cut[c]]) * vb)
+            LGPU_CUDA(cudaMemcpyAsync(ws->hf_stage[i].p, static_cast<const char *>(src) + off[cut[c]] * vb, bytes,
+                                      cudaMemcpyHostToDevice, ws->front));
+        LGPU_CUDA(cudaEventRecord(ws->hf_copied[i], ws->front));
+    };
+    LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
+    LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
+    ws->front_open = true;
+    if (nch) copy(0);
+    for (size_t c = 0; c < nch; c++) {
+        const int i = (int)(c & 1);
+        if (deadline && c > 0) deadline->wait(st, ws->ev[7]);
+        if (c + 1 < nch) copy(c + 1);
+        LGPU_CUDA(cudaStreamWaitEvent(st, ws->hf_copied[i], 0));
+        score(c, ws->hf_stage[i].p);
+        LGPU_CUDA(cudaEventRecord(ws->hf_free[i], st));
+    }
+    LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
+    LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));
+    ws->front_open = false;
+}
+
+// The routes of multivec_search_device for a host handle, with the same results.  Chunks are the outer loop: one pass
+// over the column serves P queries, all B unless the budget cannot hold their per-query state, so each vector crosses
+// PCIe once per pass.  Half the budget goes to the two staging buffers and the per-query state, the other half to the
+// distance blocks of mv_exact_dense.
+//   tensor cores  stream the fp16 operand; per chunk the F16MaxSim GEMM keeps chunk-local keys (row_base = the chunk's
+//                 first row) and mv_approx_sum fills the chunk's columns of A [P][N]; after the pass the HBM route's
+//                 k-th select, threshold, admission and flags, the exact re-score of the admitted rows from the pinned
+//                 f32 vectors (launch_mv_rescore_host), select mode 2, and the fix-up of flagged queries: the f32 rows,
+//                 chunk by chunk, copied by a kernel that returns at once when the gate is 0, through the exact kernels
+//                 for the flagged queries only.  No host synchronisation decides anything.
+//   exact         stream the f32 vectors; per chunk mv_exact_dense into D [P][N]; then select_dense.
+static void multivec_search_streamed(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q,
+                                     const uint32_t *h_qoff, uint32_t B, const lgpu_search_params &sp, bool tc,
+                                     const TopkOut &out, RowFilter rf, const Deadline *deadline, bool prof)
+{
+    const uint64_t N = mv->nrows, ld = (N + 3) & ~3ull;
+    const uint32_t dim = mv->dim, k = sp.k;
+    const uint64_t *off = mv->h_offsets.data();
+    const size_t budget = workspace_budget(), S = mv_stage_bytes(mv);
+    const size_t left = budget / 2 > 2 * S ? budget / 2 - 2 * S : 0;
+    for (auto &b : ws->hf_stage) b.ensure(S);
+    const std::vector<uint64_t> cut32 = mv_chunks(mv, S / ((size_t)dim * 4));
+    const float *V = static_cast<const float *>(mv->vectors_host.dev);
+    const uint64_t *ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
+    if (!tc) {
+        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
+        const uint32_t P = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
+        for (uint32_t qa = 0; qa < B; qa += P) {
+            const uint32_t qb = std::min(B, qa + P), b = qb - qa;
+            if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
+            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+            mv_stream(mv, ws, st, mv->vectors_host.p, (size_t)dim * 4, cut32, deadline, [&](size_t c, void *X) {
+                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, static_cast<const float *>(X),
+                               cut32[c], cut32[c + 1]);
+            });
+            select_dense(ws, ws->D.as<float>(), N, ld, ids, b, sp, rf, out.at(qa, k), st);
+        }
+        return;
+    }
+    const std::vector<uint64_t> cut16 = mv_chunks(mv, S / ((size_t)dim * 2));
+    uint64_t R = 1;                                   // the most rows of an operand chunk
+    for (size_t c = 0; c + 1 < cut16.size(); c++) R = std::max(R, cut16[c + 1] - cut16[c]);
+    const uint64_t ldR = (R + 3) & ~3ull;
+    uint32_t cap = 1024;
+    while (cap < 8 * k && cap < 16384) cap <<= 1;
+    const size_t Tq = h_qoff[B];
+    ws->mv_qh.ensure(std::max<size_t>(Tq * dim * 2, 16));
+    ws->mv_qbad.ensure(std::max<size_t>(Tq, 1) * 4);
+    launch_mv_normalize_f16(d_q, Tq, dim, ws->mv_qh.p, ws->mv_qbad.as<uint32_t>(), st);
+    // per query: A, the k-th select, threshold, counters, the shortlist and its exact scores; per query vector: the
+    // keys of one chunk
+    const size_t per_q = ld * 4 + (size_t)k * 12 + (size_t)cap * 16 + 32, per_v = ldR * 4 + 4;
+    for (uint32_t qa = 0; qa < B;) {
+        uint32_t qb = qa + 1;
+        while (qb < B && (size_t)(qb + 1 - qa) * per_q + (size_t)(h_qoff[qb + 1] - h_qoff[qa]) * per_v <= left) qb++;
+        if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
+        const uint32_t b = qb - qa, va = h_qoff[qa], nqv = h_qoff[qb] - va;
+        ws->mv_Mk.ensure((size_t)nqv * ldR * 4);
+        ws->mv_A.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+        ws->mv_kd.ensure((size_t)b * k * 4); ws->mv_ki.ensure((size_t)b * k * 8); ws->mv_kc.ensure((size_t)b * 4);
+        ws->mv_thr.ensure((size_t)b * 4); ws->mv_cnt.ensure((size_t)b * 4); ws->mv_cand.ensure((size_t)b * cap * 4);
+        ws->mv_flags.ensure((size_t)b * 4); ws->mv_vflags.ensure((size_t)nqv * 4); ws->mv_gate.ensure(16);
+        ws->mv_ex.ensure((size_t)b * cap * 4); ws->mv_exid.ensure((size_t)b * cap * 8);
+        float *A = ws->mv_A.as<float>();
+        mv_stream(mv, ws, st, mv->vec_h_host.p, (size_t)dim * 2, cut16, deadline, [&](size_t c, void *Xh) {
+            const uint64_t ra = cut16[c], rb = cut16[c + 1], span = off[rb] - off[ra], ldc = (rb - ra + 3) & ~3ull;
+            LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ldc * 4, st));
+            MaxSimOut mo{};
+            mo.col_row = mv->col_row.as<uint32_t>() + off[ra]; mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ldc;
+            mo.row_base = (uint32_t)ra; mo.xdummy = mv->ysqrt.as<float>() + off[ra];
+            launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, Xh, nqv, span, dim, mo, mv->num_sms, st);
+            launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ldc, ws->mv_qoff.as<uint32_t>(), qa, qb, va, rb - ra, A + ra,
+                                 ld, mv->num_sms, st);
+        });
+        launch_select(select_rows(A, N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
+                                                  ws->mv_kc.as<uint32_t>()}), st);
+        launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
+                            ws->mv_thr.as<float>(), st);
+        LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
+        launch_mv_admit(A, ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(), ws->mv_cand.as<uint32_t>(),
+                        st);
+        launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
+                        ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
+        launch_mv_rescore_host(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), V, mv->ysqrt.as<float>(),
+                               mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
+                               ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(),
+                               mv->num_sms, st);
+        launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
+        // the fix-up of the flagged queries into A (free again), the f32 rows through staging buffer 0 on the call's
+        // stream: with no query flagged, every launch returns at once
+        const uint32_t *gate = ws->mv_gate.as<uint32_t>();
+        float *X = ws->hf_stage[0].as<float>();
+        for (size_t c = 0; c + 1 < cut32.size(); c++) {
+            const uint64_t ra = cut32[c], rb = cut32[c + 1];
+            launch_mv_copy_gated(V + off[ra] * dim, X, (off[rb] - off[ra]) * dim, gate, mv->num_sms, st);
+            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, A, ld, X, ra, rb, ws->mv_flags.as<uint32_t>(),
+                           ws->mv_vflags.as<uint32_t>(), gate);
+        }
+        SelectArgs sc = select_rows(A, N, ld, b, k, out.at(qa, k));
+        sc.col_ids = ids;
+        sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = gate;
+        launch_select(sc, st);
+        if (prof) {             // [0] rows admitted, [1] rows re-scored exactly, [2] queries redone densely
+            std::vector<uint32_t> cnt(b), fl(b);
+            LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->mv_cnt.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaMemcpyAsync(fl.data(), ws->mv_flags.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
+            LGPU_CUDA(cudaStreamSynchronize(st));
+            for (uint32_t q = 0; q < b; q++) {
+                g_filter_stats[0] += cnt[q]; g_filter_stats[1] += std::min(cnt[q], cap);
+                g_filter_stats[2] += fl[q] ? 1 : 0;
+            }
+        }
+        qa = qb;
     }
 }
 
@@ -2070,7 +2262,9 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
     const size_t quarter = budget / 4;
     const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper && k <= SELECT_KMAX &&
                     (size_t)(max_nq + 1) * ld * 4 <= quarter;
-    if (tc) {
+    if (mv->on_host) {
+        multivec_search_streamed(mv, ws, st, d_q, h_qoff, B, sp, tc, out, rf, deadline, prof);
+    } else if (tc) {
         // fp16 normalised queries (and the queries holding a bad vector), then sub-batches of whole queries whose scores
         // M [vectors][ld] u32 and approximate distances A [queries][ld] f32 take a quarter of the budget each
         ws->mv_qh.ensure(std::max<size_t>((size_t)Tq * dim * 2, 16));
@@ -2114,8 +2308,8 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
                               ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), st);
             launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
             // exact fix-up of the flagged queries (A is free again: it holds their exact distances)
-            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->mv_A.as<float>(), ld, ws->mv_flags.as<uint32_t>(),
-                           ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>());
+            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->mv_A.as<float>(), ld, mv->vectors.as<float>(), 0, N,
+                           ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>());
             SelectArgs sc = select_rows(ws->mv_A.as<float>(), N, ld, b, k, out.at(qa, k));
             sc.col_ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
             sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = ws->mv_gate.as<uint32_t>();
@@ -2140,7 +2334,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld);
+            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, mv->vectors.as<float>(), 0, N);
             select_dense(ws, ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
                          out.at(qa, k), st);
         }
@@ -4111,25 +4305,57 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
         mv = new lgpu_multivec();
         mv->device = device; mv->nrows = nrows; mv->total = T; mv->dim = dim; mv->max_row = max_row;
         mv->h_offsets.assign(offsets, offsets + nrows + 1);
-        mv->vectors.ensure(std::max<size_t>((size_t)T * dim * 4, 16));
+        // the tensor-core operand: only when every stored vector normalises (a zero or non-finite vector has NaN pairs,
+        // which the approximate score cannot skip as the exact min does) and the shape suits the GEMM
+        const bool tc_shape = T >= MV_TC_MIN_T && T < ((uint64_t)1 << 31) && nrows < 0xffffffffull &&
+                              gemm_shape_supported(dim);
+        const size_t xbytes = (size_t)T * dim * 4, hbytes = tc_shape ? (size_t)T * dim * 2 : 0;
         mv->ysqrt.ensure(std::max<size_t>((size_t)T * 4, 16));
         mv->offsets.ensure((size_t)(nrows + 1) * 8);
         LGPU_CUDA(cudaMemcpy(mv->offsets.p, offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice));
-        if (T) {
-            LGPU_CUDA(cudaMemcpy(mv->vectors.p, values, (size_t)T * dim * 4, cudaMemcpyHostToDevice));
-            launch_row_norms(mv->vectors.as<float>(), T, dim, mv->ysqrt.as<float>(), nullptr);
+        bool ok = true;
+        if (!rows_fit_hbm("LGPU_MULTIVEC_HBM_BYTES", xbytes + hbytes)) {
+            // pinned host memory: the f32 vectors as given, |v| and the fp16 operand computed chunk by chunk of whole
+            // rows staged through HBM (each vector's terms depend on that vector alone)
+            mv->on_host = true;
+            mv->vectors_host.alloc(xbytes);
+            if (xbytes) memcpy(mv->vectors_host.p, values, xbytes);
+            if (tc_shape) mv->vec_h_host.alloc(hbytes);
+            const std::vector<uint64_t> cut = mv_chunks(mv, std::max<uint64_t>(1, FLAT_STAGE_BYTES / ((size_t)dim * 4)));
+            DevBuf xs, hs, bad;
+            std::vector<uint32_t> hb;
+            for (size_t c = 0; c + 1 < cut.size(); c++) {
+                const uint64_t j0 = offsets[cut[c]], n = offsets[cut[c + 1]] - j0;
+                if (!n) continue;
+                xs.ensure(n * dim * 4);
+                LGPU_CUDA(cudaMemcpy(xs.p, values + j0 * dim, n * dim * 4, cudaMemcpyHostToDevice));
+                launch_row_norms(xs.as<float>(), n, dim, mv->ysqrt.as<float>() + j0, nullptr);
+                if (!tc_shape) continue;
+                hs.ensure(n * dim * 2); bad.ensure(n * 4); hb.resize(n);
+                launch_mv_normalize_f16(xs.as<float>(), n, dim, hs.p, bad.as<uint32_t>(), nullptr);
+                LGPU_CUDA(cudaMemcpy(static_cast<char *>(mv->vec_h_host.p) + j0 * dim * 2, hs.p, n * dim * 2,
+                                     cudaMemcpyDeviceToHost));
+                LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, n * 4, cudaMemcpyDeviceToHost));
+                for (uint64_t i = 0; i < n; i++) ok = ok && !hb[i];
+            }
+        } else {
+            mv->vectors.ensure(std::max<size_t>(xbytes, 16), true);
+            if (T) {
+                LGPU_CUDA(cudaMemcpy(mv->vectors.p, values, xbytes, cudaMemcpyHostToDevice));
+                launch_row_norms(mv->vectors.as<float>(), T, dim, mv->ysqrt.as<float>(), nullptr);
+            }
+            if (tc_shape) {
+                mv->vec_h.ensure(hbytes, true);
+                DevBuf bad;
+                bad.ensure((size_t)T * 4);
+                launch_mv_normalize_f16(mv->vectors.as<float>(), T, dim, mv->vec_h.p, bad.as<uint32_t>(), nullptr);
+                std::vector<uint32_t> hb(T);
+                LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, (size_t)T * 4, cudaMemcpyDeviceToHost));
+                for (uint64_t i = 0; i < T; i++) ok = ok && !hb[i];
+            }
         }
-        // the tensor-core operand: only when every stored vector normalises (a zero or non-finite vector has NaN pairs,
-        // which the approximate score cannot skip as the exact min does) and the shape suits the GEMM
-        if (T >= MV_TC_MIN_T && T < ((uint64_t)1 << 31) && nrows < 0xffffffffull && gemm_shape_supported(dim)) {
-            mv->vec_h.ensure((size_t)T * dim * 2);
-            DevBuf bad;
-            bad.ensure((size_t)T * 4);
-            launch_mv_normalize_f16(mv->vectors.as<float>(), T, dim, mv->vec_h.p, bad.as<uint32_t>(), nullptr);
-            std::vector<uint32_t> hb(T), cr(T);
-            LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, (size_t)T * 4, cudaMemcpyDeviceToHost));
-            bool ok = true;
-            for (uint64_t i = 0; i < T; i++) ok = ok && !hb[i];
+        if (tc_shape) {
+            std::vector<uint32_t> cr(T);
             for (uint64_t r = 0; r < nrows; r++)
                 for (uint64_t j = offsets[r]; j < offsets[r + 1]; j++) cr[j] = (uint32_t)r;
             mv->col_row.ensure((size_t)T * 4);
@@ -4145,6 +4371,27 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
     return rc;
 }
 
+int lgpu_multivec_device_bytes(const lgpu_multivec *mvh, uint64_t *bytes)
+{
+    return guarded([&] {
+        HandleRef<lgpu_multivec> h(const_cast<lgpu_multivec *>(mvh));
+        LGPU_REQUIRE(bytes != nullptr, "null argument");
+        const lgpu_multivec *mv = h.h;
+        *bytes = mv->vectors.bytes + mv->ysqrt.bytes + mv->offsets.bytes + mv->row_ids.bytes + mv->vec_h.bytes +
+                 mv->col_row.bytes + mv->live.bits.bytes;
+    });
+}
+
+int lgpu_multivec_host_bytes(const lgpu_multivec *mvh, uint64_t *bytes, int *placement)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(bytes || placement, "null argument");
+        HandleRef<lgpu_multivec> mv(const_cast<lgpu_multivec *>(mvh));
+        if (bytes) *bytes = mv->vectors_host.bytes + mv->vec_h_host.bytes;
+        if (placement) *placement = mv->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+    });
+}
+
 void lgpu_multivec_close(lgpu_multivec *mv) { close_handle(mv); }
 
 // Host calls are never captured into a CUDA graph: the launch sequence depends on every query's vector count, not
@@ -4157,6 +4404,7 @@ static int multivec_call(lgpu_multivec *mvh, const Route &r, const float *q, con
                            check_call(p, B, q, ids, dist, cnt);
                            if (B == 0) return (size_t)0;
                            check_multivec_offsets(q_off, B);
+                           mv_check_stage(mv);
                            return (size_t)q_off[B] * mv->dim;
                        },
                        [&](lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *dq, auto &&...a) {

@@ -337,6 +337,14 @@ __global__ void __launch_bounds__(RH_WARPS * 32) refine_host_kernel(
     asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// one step of the exact MaxSim's min over a row: the running NaN-skipping minimum m after the pair of query vector i and
+// stored vector j, cosd = 1 - xy / |q_i| / |v_j| (dist_matrix_kernel mode 2's roundings; a NaN c never replaces a number)
+__device__ __forceinline__ float mv_min_step(float m, float xy, float xn, float ys)
+{
+    const float c = __fsub_rn(1.0f, __fdiv_rn(__fdiv_rn(xy, xn), ys));
+    return (c < m || m != m) ? c : m;
+}
+
 // exact MaxSim re-score of the multivector shortlist, half a warp per (query, candidate row): for each query vector i
 // in order, the NaN-skipping min over the row's vectors j of 1 - xy / |q_i| / |v_j| (xy in lance's lane order: the
 // same roundings as dist_matrix_kernel mode 2), added onto a sum that starts at 0.0f -- the exact path's bits
@@ -363,14 +371,99 @@ __global__ void mv_rescore_kernel(const float *__restrict__ Q, const uint32_t *_
     for (uint32_t i = q_off[qa + b]; i < q_off[qa + b + 1]; i++) {
         const float *x = Q + (size_t)i * d;
         float m = CUDART_NAN_F;
-        for (uint64_t j = j0; j < j1; j++) {
-            const float xy = halfwarp_dot(x, V + j * d, d, hl, hmask, hbase);
-            const float c = __fsub_rn(1.0f, __fdiv_rn(__fdiv_rn(xy, xnorm[i]), ysqrt[j]));
-            if (c < m || m != m) m = c;
-        }
+        for (uint64_t j = j0; j < j1; j++) m = mv_min_step(m, halfwarp_dot(x, V + j * d, d, hl, hmask, hbase), xnorm[i], ysqrt[j]);
         s = __fadd_rn(s, m);
     }
     if (hl == 0) { out[pair] = s; ids[pair] = row_ids ? row_ids[r] : r; }
+}
+
+// mv_rescore_kernel's values when the stored vectors are in pinned host memory, read through their mapped device alias
+// over PCIe.  One warp per (query, candidate row) pair at a time.  The row is one contiguous run of n_r x d floats;
+// the warp copies it in chunks of whole vectors into a shared-memory ring with cp.async 16-byte requests (one
+// instruction = 512 contiguous bytes, refine_host_kernel's technique), the next chunk in flight while this one is
+// scored.  The query's vectors are taken in blocks of MH_QV: half-warp h keeps the running minima of vectors
+// i0 + 32 h + 16 u + l (u = 0, 1) in lane l, updated in order of j by the same mv_min_step as mv_rescore_kernel, and
+// the block's minima are added onto the sum in order of i once the row was streamed.  A query of more than MH_QV
+// vectors streams the row once per block.  `staged` false (d not a multiple of 4, or a vector longer than a ring slot):
+// the half-warps read the mapped alias directly.
+constexpr int MH_WARPS = 4;
+constexpr uint32_t MH_QV = 64, MH_SLOT = 1024;      // query vectors per block; floats per ring slot (2 slots per warp)
+
+__global__ void __launch_bounds__(MH_WARPS * 32) mv_rescore_host_kernel(
+    const float *__restrict__ Q, const uint32_t *__restrict__ q_off, uint32_t qa, const float *__restrict__ xnorm,
+    const float *V, const float *__restrict__ ysqrt, const uint64_t *__restrict__ offsets,
+    const uint64_t *__restrict__ row_ids, uint32_t d, uint32_t B, const uint32_t *__restrict__ cand,
+    const uint32_t *__restrict__ count, uint32_t cap, bool staged, float *__restrict__ out, uint64_t *__restrict__ ids)
+{
+    pdl_entry();
+    __shared__ __align__(16) float mh_ring[MH_WARPS][2][MH_SLOT];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, h = lane >> 4, hl = lane & 15, hbase = lane & 16;
+    const unsigned hmask = 0xffffu << hbase;
+    const uint32_t vps = staged ? MH_SLOT / d : 1;                 // vectors per chunk
+    const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(&mh_ring[warp][0][0]);
+    const uint64_t npairs = (uint64_t)B * cap, nwarps = (uint64_t)gridDim.x * MH_WARPS;
+    for (uint64_t pair = (uint64_t)blockIdx.x * MH_WARPS + warp; pair < npairs; pair += nwarps) {
+        const uint32_t b = (uint32_t)(pair / cap), slot = (uint32_t)(pair % cap);
+        if (slot >= min(count[b], cap)) {
+            if (lane == 0) { out[pair] = CUDART_NAN_F; ids[pair] = UINT64_MAX; }
+            continue;
+        }
+        const uint32_t r = cand[pair];
+        const uint64_t j0 = offsets[r], n = offsets[r + 1] - j0;
+        const uint32_t nch = staged ? (uint32_t)((n + vps - 1) / vps) : 0;
+        const float *row = V + j0 * d;
+        // chunk c of the row into ring slot c & 1; every lane commits one group per chunk, empty or not
+        auto issue = [&](uint32_t c) {
+            if (c < nch) {
+                const uint32_t len = (uint32_t)(min((uint64_t)vps, n - (uint64_t)c * vps) * d);
+                const float *src = row + (size_t)c * vps * d;
+                const uint32_t dst = ring_s + (c & 1) * MH_SLOT * 4;
+                for (uint32_t o = (uint32_t)lane * 4; o < len; o += 128)
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + o * 4), "l"(src + o) : "memory");
+            }
+            asm volatile("cp.async.commit_group;" ::: "memory");
+        };
+        const uint32_t qs = q_off[qa + b], qe = q_off[qa + b + 1];
+        float s = 0.f;
+        for (uint32_t i0 = qs; i0 < qe; i0 += MH_QV) {
+            float m[2] = {CUDART_NAN_F, CUDART_NAN_F};
+            // the minima of this half-warp's vectors i0 + 32 h + 16 u + t over stored vectors [j, j + nv) at y
+            auto score = [&](const float *y, uint64_t j, uint32_t nv) {
+                for (uint32_t v = 0; v < nv; v++) {
+                    const float ys = ysqrt[j0 + j + v];
+#pragma unroll
+                    for (int u = 0; u < 2; u++)
+                        for (uint32_t t = 0; t < 16; t++) {
+                            const uint32_t i = i0 + 32 * h + 16 * u + t;
+                            if (i >= qe) break;                           // uniform over the half-warp
+                            const float xy = halfwarp_dot(Q + (size_t)i * d, y + (size_t)v * d, d, hl, hmask, hbase);
+                            if ((uint32_t)hl == t) m[u] = mv_min_step(m[u], xy, xnorm[i], ys);
+                        }
+                }
+            };
+            if (staged) {
+                issue(0);
+                for (uint32_t c = 0; c < nch; c++) {
+                    issue(c + 1);                         // into the slot chunk c - 1 used, released by the last __syncwarp
+                    asm volatile("cp.async.wait_group 1;" ::: "memory");
+                    __syncwarp();                         // every lane's copies of chunk c are in place
+                    score(&mh_ring[warp][c & 1][0], (uint64_t)c * vps, (uint32_t)min((uint64_t)vps, n - (uint64_t)c * vps));
+                    __syncwarp();                         // slot c & 1 is read: chunk c + 2 may overwrite it
+                }
+                asm volatile("cp.async.wait_group 0;" ::: "memory");
+            } else {
+                score(row, 0, (uint32_t)n);
+            }
+            __syncwarp();
+#pragma unroll
+            for (int g = 0; g < 4; g++)                   // vectors i0 + 16 g + t: half g >> 1, register g & 1
+                for (uint32_t t = 0; t < 16; t++) {
+                    const float v = __shfl_sync(0xffffffffu, m[g & 1], (g >> 1) * 16 + t);
+                    if (i0 + 16 * g + t < qe) s = __fadd_rn(s, v);
+                }
+        }
+        if (lane == 0) { out[pair] = s; ids[pair] = row_ids ? row_ids[r] : r; }
+    }
 }
 
 // ---- the coarse step after the tensor-core GEMM, in one kernel (one CTA per query):
@@ -632,6 +725,20 @@ void launch_refine_host(const float *Q, const float *V, uint32_t stride, const u
         LGPU_CUDA(cudaFuncSetAttribute(refine_host_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     launch_k(refine_host_kernel, dim3((unsigned)((warps + RH_WARPS - 1) / RH_WARPS)), dim3(RH_WARPS * 32), smem, st, Q,
              V, stride, pos, npairs, nc, d, metric, chunk, nchunks, per_warp, out); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+                            const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
+                            const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
+                            int num_sms, cudaStream_t st)
+{
+    if (B == 0 || cap == 0) return;
+    const bool staged = d % 4 == 0 && d <= MH_SLOT && ((uintptr_t)V & 15) == 0;
+    const uint64_t npairs = (uint64_t)B * cap;
+    const unsigned grid = (unsigned)std::min<uint64_t>((npairs + MH_WARPS - 1) / MH_WARPS, (uint64_t)std::max(num_sms, 1) * 16);
+    launch_k(mv_rescore_host_kernel, dim3(grid), dim3(MH_WARPS * 32), 0, st, Q, q_off, qa, xnorm, V, ysqrt, offsets,
+             row_ids, d, B, cand, count, cap, staged, out, ids); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

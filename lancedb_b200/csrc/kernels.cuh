@@ -492,6 +492,14 @@ void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const
                        const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
                        const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
                        cudaStream_t st);
+// the same values when V is the mapped device alias of pinned host memory: each candidate row is read over PCIe in
+// 16-byte cp.async requests staged in shared memory (dist.cu mv_rescore_host_kernel)
+void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+                            const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
+                            const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
+                            int num_sms, cudaStream_t st);
+// dst[0, n) = src[0, n) floats when *gate (device) != 0; nothing otherwise (multivec.cu)
+void launch_mv_copy_gated(const float *src, float *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st);
 
 // ---------------- multivector (MaxSim) columns, exact path (multivec.cu) ----------------------
 // M[i][r] = min over row r0 + r's stored vectors j of P[i][j - offsets[r0]] (NaN skipped; NaN if none), for the nqv

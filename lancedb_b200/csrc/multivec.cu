@@ -189,6 +189,24 @@ __global__ void __launch_bounds__(MV_THREADS) mv_rowsum_kernel(const float *__re
     }
 }
 
+// dst[0, n) = src[0, n) when *gate != 0, else nothing: the fix-up's chunk copy out of a host handle's mapped rows,
+// which costs one empty launch when no query is flagged.  16-byte requests when both ends allow them.
+__global__ void __launch_bounds__(MV_THREADS) mv_copy_gated_kernel(const float *src, float *__restrict__ dst, uint64_t n,
+                                                                   const uint32_t *__restrict__ gate)
+{
+    pdl_entry();
+    if (*gate == 0) return;
+    const uint64_t t0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, step = (uint64_t)gridDim.x * blockDim.x;
+    uint64_t head = 0;
+    if ((((uintptr_t)src | (uintptr_t)dst) & 15) == 0) {
+        head = n & ~3ull;
+        const uint4 *s4 = reinterpret_cast<const uint4 *>(src);
+        uint4 *d4 = reinterpret_cast<uint4 *>(dst);
+        for (uint64_t w = t0; w < head / 4; w += step) d4[w] = s4[w];
+    }
+    for (uint64_t w = head + t0; w < n; w += step) dst[w] = src[w];
+}
+
 unsigned grid_for(uint64_t items, int num_sms)
 {
     return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((items + MV_THREADS - 1) / MV_THREADS, (uint64_t)num_sms * 16));
@@ -212,6 +230,14 @@ void launch_mv_rowsum(const float *M, uint64_t ldM, const uint32_t *q_off, uint3
     if (b_hi <= b_lo || nr == 0) return;
     launch_k(mv_rowsum_kernel, dim3(grid_for((uint64_t)(b_hi - b_lo) * nr, num_sms)), dim3(MV_THREADS), 0, st, M, ldM,
              q_off, b_lo, b_hi, qa, i0, i1, nr, D, ldD, col0, only, gate); LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
+
+void launch_mv_copy_gated(const float *src, float *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st)
+{
+    if (n == 0) return;
+    launch_k(mv_copy_gated_kernel, dim3(grid_for((n + 3) / 4, num_sms)), dim3(MV_THREADS), 0, st, src, dst, n, gate);
+    LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
