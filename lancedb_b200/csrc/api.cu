@@ -15,6 +15,7 @@
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <thread>
 #include <type_traits>
@@ -122,6 +123,73 @@ struct PinnedBuf {
     ~PinnedBuf() { reset(); }
 };
 
+// Deadline of one call (QueryExecutionOptions::timeout -> TimeoutStream, rust/lancedb/src/utils/mod.rs:328-393,
+// used at rust/lancedb/src/query.rs:1452-1457).  Kernels cannot be cancelled, so the deadline is enforced where
+// the host waits: between sub-batches and before the results are copied back.  On expiry the call returns
+// LGPU_TIMEOUT without touching the caller's output buffers; work already enqueued drains into the workspace,
+// which stays fenced by its `done` event until then.
+struct Deadline {
+    bool armed = false;
+    std::chrono::steady_clock::time_point at;
+    explicit Deadline(uint32_t timeout_ms)
+    {
+        if (timeout_ms) { armed = true; at = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms); }
+    }
+    bool expired() const { return armed && std::chrono::steady_clock::now() >= at; }
+    // wait for everything enqueued on `st` so far, or for the deadline
+    void wait(cudaStream_t st, cudaEvent_t ev) const
+    {
+        if (!armed) return;
+        LGPU_CUDA(cudaEventRecord(ev, st));
+        for (;;) {
+            cudaError_t e = cudaEventQuery(ev);
+            if (e == cudaSuccess) return;
+            if (e != cudaErrorNotReady) LGPU_CUDA(e);
+            if (expired()) { set_error("Query timeout"); throw Failure{LGPU_TIMEOUT}; }
+            std::this_thread::sleep_for(std::chrono::microseconds(50));
+        }
+    }
+};
+
+struct Workspace;
+
+// Rows streamed from pinned host memory through HBM (the search of a host flat or multivector handle).  Between open
+// and close, chunk s of `steps` is copied into buf[s & 1] by cudaMemcpyAsync on the workspace's side stream (`front`,
+// forked from the call's stream and joined back to it), chunk s + 1 while chunk s is used on the call's stream:
+// take(s) hands over chunk s once the copy of chunk s + 1 is issued, release(s) marks every use of it enqueued.
+// copied[i]: buf[i] holds its chunk (side stream); freed[i]: the uses of its chunk are enqueued (call's stream), so the
+// copy two steps later may overwrite it.  timeout_ms is checked between chunks.
+struct Staging {
+    using Source = std::function<std::pair<const void *, size_t>(uint64_t)>;   // chunk s: its pinned rows and bytes
+    DevBuf buf[2];
+    cudaEvent_t copied[2] = {}, freed[2] = {};
+    Staging()
+    {
+        for (int i = 0; i < 2; i++) {
+            LGPU_CUDA(cudaEventCreateWithFlags(&copied[i], cudaEventDisableTiming));
+            LGPU_CUDA(cudaEventCreateWithFlags(&freed[i], cudaEventDisableTiming));
+        }
+    }
+    ~Staging()
+    {
+        for (int i = 0; i < 2; i++) {
+            if (copied[i]) cudaEventDestroy(copied[i]);
+            if (freed[i]) cudaEventDestroy(freed[i]);
+        }
+    }
+    void open(Workspace *ws, cudaStream_t st, uint64_t steps, const Deadline *deadline, Source src);
+    void *take(uint64_t s);
+    void release(uint64_t s) { LGPU_CUDA(cudaEventRecord(freed[s & 1], st)); }
+    void close();
+    void copy(uint64_t s);
+    // the open run
+    Workspace *ws = nullptr;
+    cudaStream_t st = nullptr;
+    uint64_t steps = 0;
+    const Deadline *deadline = nullptr;
+    Source src;
+};
+
 struct Workspace {
     cudaStream_t stream = nullptr;     // private stream (host-buffer entry points)
     // side stream of the filter scan's front: the coarse step and the regrouping run here while the per-query tables
@@ -163,11 +231,10 @@ struct Workspace {
     DevBuf sel_large;                   // the large select's scratch (k > SELECT_KMAX, select_large.cu)
     DevBuf u_ids, u_dist, u_cnt;        // union search: the index's and the tail's top-k, [2][B][k] and [2][B]
     DevBuf live_and;                    // a filtered call on a handle with deleted rows: its bitmap AND the live rows
-    // a flat handle whose rows are in pinned host memory (flat_search_streamed): two staging buffers of rows, the
-    // staged chunk's tensor-core operand, |x|^2 and |x|, and the running top-k, [2 buffers][2 lists][P][k] / [..][P];
-    // hf_copied[i]: staging buffer i holds its chunk (side stream), hf_free[i]: its chunk was scored (call's stream)
-    DevBuf hf_stage[2], hf_xb, hf_n2, hf_ysqrt, hf_ids, hf_dist, hf_cnt;
-    cudaEvent_t hf_copied[2] = {}, hf_free[2] = {};
+    Staging stage;                      // a handle whose rows are in pinned host memory: the rows staged through HBM
+    // a flat handle whose rows are in pinned host memory (flat_search_streamed): the staged chunk's tensor-core
+    // operand, |x|^2 and |x|, and the running top-k, [2 buffers][2 lists][P][k] / [..][P]
+    DevBuf chunk_xb, chunk_n2, chunk_ysqrt, run_ids, run_dist, run_cnt;
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -178,10 +245,6 @@ struct Workspace {
         LGPU_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
         LGPU_CUDA(cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
         for (auto &e : ev) LGPU_CUDA(cudaEventCreate(&e));
-        for (int i = 0; i < 2; i++) {
-            LGPU_CUDA(cudaEventCreateWithFlags(&hf_copied[i], cudaEventDisableTiming));
-            LGPU_CUDA(cudaEventCreateWithFlags(&hf_free[i], cudaEventDisableTiming));
-        }
     }
     ~Workspace()
     {
@@ -192,12 +255,42 @@ struct Workspace {
         if (ev_join) cudaEventDestroy(ev_join);
         if (done) cudaEventDestroy(done);
         for (auto &e : ev) if (e) cudaEventDestroy(e);
-        for (int i = 0; i < 2; i++) {
-            if (hf_copied[i]) cudaEventDestroy(hf_copied[i]);
-            if (hf_free[i]) cudaEventDestroy(hf_free[i]);
-        }
     }
 };
+
+void Staging::open(Workspace *w, cudaStream_t s, uint64_t n, const Deadline *dl, Source source)
+{
+    ws = w; st = s; steps = n; deadline = dl; src = std::move(source);
+    LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
+    LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
+    ws->front_open = true;
+    if (steps) copy(0);
+}
+
+// chunk s into buf[s & 1], once the uses of the chunk it held two steps earlier are enqueued
+void Staging::copy(uint64_t s)
+{
+    const int i = (int)(s & 1);
+    if (s >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, freed[i], 0));
+    const auto [rows, bytes] = src(s);
+    if (bytes) LGPU_CUDA(cudaMemcpyAsync(buf[i].p, rows, bytes, cudaMemcpyHostToDevice, ws->front));
+    LGPU_CUDA(cudaEventRecord(copied[i], ws->front));
+}
+
+void *Staging::take(uint64_t s)
+{
+    if (deadline && s > 0) deadline->wait(st, ws->ev[7]);
+    if (s + 1 < steps) copy(s + 1);
+    LGPU_CUDA(cudaStreamWaitEvent(st, copied[s & 1], 0));
+    return buf[s & 1].p;
+}
+
+void Staging::close()
+{
+    LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
+    LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));
+    ws->front_open = false;
+}
 
 struct WorkspacePool {
     std::mutex mu;
@@ -476,7 +569,7 @@ struct lgpu_multivec {
     bool tc_ok = false;                    // the tensor-core path may run (see multivec_search_device)
     // row data that did not fit in HBM at open (lgpu_multivec_open): `vectors_host` holds the f32 vectors and
     // `vec_h_host` the fp16 operand (tensor-core shape only), both [T][dim]; `vectors` and `vec_h` stay empty, and
-    // searches stream the rows through HBM (multivec_search_streamed)
+    // searches stream the rows through HBM (multivec_search_device)
     bool on_host = false;
     PinnedBuf vectors_host, vec_h_host;
     std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
@@ -570,34 +663,6 @@ struct WsLease {
         }
         if (cudaEventRecord(ws->done, st) != cudaSuccess) cudaGetLastError();
         pool.give(ws);
-    }
-};
-
-// Deadline of one call (QueryExecutionOptions::timeout -> TimeoutStream, rust/lancedb/src/utils/mod.rs:328-393,
-// used at rust/lancedb/src/query.rs:1452-1457).  Kernels cannot be cancelled, so the deadline is enforced where
-// the host waits: between sub-batches and before the results are copied back.  On expiry the call returns
-// LGPU_TIMEOUT without touching the caller's output buffers; work already enqueued drains into the workspace,
-// which stays fenced by its `done` event until then.
-struct Deadline {
-    bool armed = false;
-    std::chrono::steady_clock::time_point at;
-    explicit Deadline(uint32_t timeout_ms)
-    {
-        if (timeout_ms) { armed = true; at = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms); }
-    }
-    bool expired() const { return armed && std::chrono::steady_clock::now() >= at; }
-    // wait for everything enqueued on `st` so far, or for the deadline
-    void wait(cudaStream_t st, cudaEvent_t ev) const
-    {
-        if (!armed) return;
-        LGPU_CUDA(cudaEventRecord(ev, st));
-        for (;;) {
-            cudaError_t e = cudaEventQuery(ev);
-            if (e == cudaSuccess) return;
-            if (e != cudaErrorNotReady) LGPU_CUDA(e);
-            if (expired()) { set_error("Query timeout"); throw Failure{LGPU_TIMEOUT}; }
-            std::this_thread::sleep_for(std::chrono::microseconds(50));
-        }
     }
 };
 
@@ -1751,13 +1816,13 @@ static void flat_search_streamed(lgpu_flat *fl, Workspace *ws, cudaStream_t st, 
     const uint32_t P = (uint32_t)std::max<size_t>(1, std::min<size_t>(B, rest / 2 / run_q));
     const size_t left = rest > (size_t)P * run_q ? rest - (size_t)P * run_q : 0;
     const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(P, left / score_q));
-    for (auto &b : ws->hf_stage) b.ensure(std::max<size_t>(C * d * es, 16));
-    if (fl->has_tc && !fl->f16) ws->hf_xb.ensure(C * d * 2);
-    ws->hf_n2.ensure(C * 4);
-    if (metric == LGPU_COSINE) ws->hf_ysqrt.ensure(C * 4);
+    for (auto &b : ws->stage.buf) b.ensure(std::max<size_t>(C * d * es, 16));
+    if (fl->has_tc && !fl->f16) ws->chunk_xb.ensure(C * d * 2);
+    ws->chunk_n2.ensure(C * 4);
+    if (metric == LGPU_COSINE) ws->chunk_ysqrt.ensure(C * 4);
     if (nchunks > 1) {
-        ws->hf_ids.ensure((size_t)4 * P * k * 8); ws->hf_dist.ensure((size_t)4 * P * k * 4);
-        ws->hf_cnt.ensure((size_t)4 * P * 4);
+        ws->run_ids.ensure((size_t)4 * P * k * 8); ws->run_dist.ensure((size_t)4 * P * k * 4);
+        ws->run_cnt.ensure((size_t)4 * P * 4);
     }
     const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
@@ -1765,48 +1830,36 @@ static void flat_search_streamed(lgpu_flat *fl, Workspace *ws, cudaStream_t st, 
     const char *rows = static_cast<const char *>(fl->rows_host.p);
     const uint64_t steps = (uint64_t)((B + P - 1) / P) * nchunks;      // step s: pass s / nchunks, chunk s % nchunks
     auto chunk_rows = [&](uint64_t c) { return N ? std::min<uint64_t>(C, N - c * C) : 0; };
-    // the chunk of step s into staging buffer s & 1, once the chunk it held two steps earlier was scored
-    auto copy = [&](uint64_t s) {
-        const int i = (int)(s & 1);
+    ws->stage.open(ws, st, steps, deadline, [&](uint64_t s) -> std::pair<const void *, size_t> {
         const uint64_t c = s % nchunks;
-        if (s >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->hf_free[i], 0));
-        if (const size_t bytes = chunk_rows(c) * d * es)
-            LGPU_CUDA(cudaMemcpyAsync(ws->hf_stage[i].p, rows + c * C * d * es, bytes, cudaMemcpyHostToDevice, ws->front));
-        LGPU_CUDA(cudaEventRecord(ws->hf_copied[i], ws->front));
-    };
-    LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
-    LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
-    ws->front_open = true;
-    copy(0);
+        return {rows + c * C * d * es, chunk_rows(c) * d * es};
+    });
     for (uint64_t s = 0; s < steps; s++) {
         const uint32_t p0 = (uint32_t)(s / nchunks) * P, pb = std::min(P, B - p0);
         const uint64_t c = s % nchunks, n = chunk_rows(c);
-        const int i = (int)(s & 1);
-        if (deadline && s > 0) deadline->wait(st, ws->ev[7]);
-        if (s + 1 < steps) copy(s + 1);
-        LGPU_CUDA(cudaStreamWaitEvent(st, ws->hf_copied[i], 0));
-        const T *X = ws->hf_stage[i].as<T>();
+        const T *X = static_cast<const T *>(ws->stage.take(s));
         // the operand only when a scoring group takes the tensor cores (the first group is the largest)
         const bool tc = flat_tc_route(fl->has_tc, metric, sp, std::min(bs, pb), n);
-        if (tc && fl->f16) launch_f16_row_terms(X, n, d, ws->hf_n2.as<float>(), nullptr, st);
-        else if (tc) launch_to_bf16(reinterpret_cast<const float *>(X), n, d, ws->hf_xb.p, ws->hf_n2.as<float>(), st);
-        if (metric == LGPU_COSINE) launch_row_norms(X, n, d, ws->hf_ysqrt.as<float>(), st);
-        const FlatRows<T> chunk{X, fl->f16 ? static_cast<const void *>(X) : ws->hf_xb.p, ws->hf_n2.as<float>(),
-                                ws->hf_ysqrt.as<float>(), n,
+        if (tc && fl->f16) launch_f16_row_terms(X, n, d, ws->chunk_n2.as<float>(), nullptr, st);
+        else if (tc) launch_to_bf16(reinterpret_cast<const float *>(X), n, d, ws->chunk_xb.p, ws->chunk_n2.as<float>(), st);
+        if (metric == LGPU_COSINE) launch_row_norms(X, n, d, ws->chunk_ysqrt.as<float>(), st);
+        const FlatRows<T> chunk{X, fl->f16 ? static_cast<const void *>(X) : ws->chunk_xb.p, ws->chunk_n2.as<float>(),
+                                ws->chunk_ysqrt.as<float>(), n,
                                 fl->has_ids ? Cols(fl->row_ids.as<uint64_t>() + c * C) : Cols(nullptr, c * C), tc};
         // list l of running buffer r: [pb][k] entries and [pb] counts.  Chunk 0 goes to list 0 of buffer 0; chunk
         // c > 0 to list 1 of buffer (c - 1) & 1, merged with its list 0 into list 0 of the other buffer, or into the
         // output after the last chunk.  A column of one chunk is scored straight into the output.
         auto run = [&](uint64_t r, uint32_t l) -> TopkOut {
             const size_t off = (size_t)(2 * r + l) * pb;
-            return {ws->hf_ids.as<uint64_t>() + off * k, ws->hf_dist.as<float>() + off * k, ws->hf_cnt.as<uint32_t>() + off};
+            return {ws->run_ids.as<uint64_t>() + off * k, ws->run_dist.as<float>() + off * k, ws->run_cnt.as<uint32_t>() + off};
         };
         const TopkOut pass_out = out.at(p0, k);
         const TopkOut dst = nchunks == 1 ? pass_out : c == 0 ? run(0, 0) : run((c - 1) & 1, 1);
         for (uint32_t g0 = 0; g0 < pb; g0 += bs)
             flat_score(fl, ws, st, metric, d_q + (size_t)(p0 + g0) * d, std::min(bs, pb - g0), sp, chunk, dst.at(g0, k),
                        rf, prof);
-        LGPU_CUDA(cudaEventRecord(ws->hf_free[i], st));
+        // released before the merge, so that the next copy does not wait for it
+        ws->stage.release(s);
         if (c > 0) {
             const TopkOut a = run((c - 1) & 1, 0);
             SelectArgs m = select_cands(a.dist, a.ids, k, pb, k, c + 1 == nchunks ? pass_out : run(c & 1, 0));
@@ -1814,9 +1867,7 @@ static void flat_search_streamed(lgpu_flat *fl, Workspace *ws, cudaStream_t st, 
             launch_select(with_scratch(ws, m), st);
         }
     }
-    LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
-    LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));
-    ws->front_open = false;
+    ws->stage.close();
     if (prof) g_filter_stats[3] = B;
 }
 
@@ -2091,164 +2142,22 @@ static std::vector<uint64_t> mv_chunks(const lgpu_multivec *mv, uint64_t cap_vec
     return cut;
 }
 
-// Copies chunk c of `src` (pinned, `vb` bytes per stored vector) into staging buffer c & 1 on the side stream (`front`,
-// forked from the call's stream and joined back to it), chunk c + 1 while chunk c is scored on the call's stream by
-// score(c, staged vectors): flat_search_streamed's pipeline, on the same buffers and events.  timeout_ms is checked
-// between chunks.
-template <class F>
-static void mv_stream(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const void *src, size_t vb,
-                      const std::vector<uint64_t> &cut, const Deadline *deadline, F &&score)
-{
-    const uint64_t *off = mv->h_offsets.data();
-    const size_t nch = cut.size() - 1;
-    auto copy = [&](size_t c) {
-        const int i = (int)(c & 1);
-        if (c >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->hf_free[i], 0));
-        if (const size_t bytes = (off[cut[c + 1]] - off[cut[c]]) * vb)
-            LGPU_CUDA(cudaMemcpyAsync(ws->hf_stage[i].p, static_cast<const char *>(src) + off[cut[c]] * vb, bytes,
-                                      cudaMemcpyHostToDevice, ws->front));
-        LGPU_CUDA(cudaEventRecord(ws->hf_copied[i], ws->front));
-    };
-    LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
-    LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
-    ws->front_open = true;
-    if (nch) copy(0);
-    for (size_t c = 0; c < nch; c++) {
-        const int i = (int)(c & 1);
-        if (deadline && c > 0) deadline->wait(st, ws->ev[7]);
-        if (c + 1 < nch) copy(c + 1);
-        LGPU_CUDA(cudaStreamWaitEvent(st, ws->hf_copied[i], 0));
-        score(c, ws->hf_stage[i].p);
-        LGPU_CUDA(cudaEventRecord(ws->hf_free[i], st));
-    }
-    LGPU_CUDA(cudaEventRecord(ws->ev_join, ws->front));
-    LGPU_CUDA(cudaStreamWaitEvent(st, ws->ev_join, 0));
-    ws->front_open = false;
-}
-
-// The routes of multivec_search_device for a host handle, with the same results.  Chunks are the outer loop: one pass
-// over the column serves P queries, all B unless the budget cannot hold their per-query state, so each vector crosses
-// PCIe once per pass.  Half the budget goes to the two staging buffers and the per-query state, the other half to the
-// distance blocks of mv_exact_dense.
-//   tensor cores  stream the fp16 operand; per chunk the F16MaxSim GEMM keeps chunk-local keys (row_base = the chunk's
-//                 first row) and mv_approx_sum fills the chunk's columns of A [P][N]; after the pass the HBM route's
-//                 k-th select, threshold, admission and flags, the exact re-score of the admitted rows from the pinned
-//                 f32 vectors (launch_mv_rescore_host), select mode 2, and the fix-up of flagged queries: the f32 rows,
-//                 chunk by chunk, copied by a kernel that returns at once when the gate is 0, through the exact kernels
-//                 for the flagged queries only.  No host synchronisation decides anything.
-//   exact         stream the f32 vectors; per chunk mv_exact_dense into D [P][N]; then select_dense.
-static void multivec_search_streamed(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q,
-                                     const uint32_t *h_qoff, uint32_t B, const lgpu_search_params &sp, bool tc,
-                                     const TopkOut &out, RowFilter rf, const Deadline *deadline, bool prof)
-{
-    const uint64_t N = mv->nrows, ld = (N + 3) & ~3ull;
-    const uint32_t dim = mv->dim, k = sp.k;
-    const uint64_t *off = mv->h_offsets.data();
-    const size_t budget = workspace_budget(), S = mv_stage_bytes(mv);
-    const size_t left = budget / 2 > 2 * S ? budget / 2 - 2 * S : 0;
-    for (auto &b : ws->hf_stage) b.ensure(S);
-    const std::vector<uint64_t> cut32 = mv_chunks(mv, S / ((size_t)dim * 4));
-    const float *V = static_cast<const float *>(mv->vectors_host.dev);
-    const uint64_t *ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
-    if (!tc) {
-        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
-        const uint32_t P = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
-        for (uint32_t qa = 0; qa < B; qa += P) {
-            const uint32_t qb = std::min(B, qa + P), b = qb - qa;
-            if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
-            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-            mv_stream(mv, ws, st, mv->vectors_host.p, (size_t)dim * 4, cut32, deadline, [&](size_t c, void *X) {
-                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, static_cast<const float *>(X),
-                               cut32[c], cut32[c + 1]);
-            });
-            select_dense(ws, ws->D.as<float>(), N, ld, ids, b, sp, rf, out.at(qa, k), st);
-        }
-        return;
-    }
-    const std::vector<uint64_t> cut16 = mv_chunks(mv, S / ((size_t)dim * 2));
-    uint64_t R = 1;                                   // the most rows of an operand chunk
-    for (size_t c = 0; c + 1 < cut16.size(); c++) R = std::max(R, cut16[c + 1] - cut16[c]);
-    const uint64_t ldR = (R + 3) & ~3ull;
-    uint32_t cap = 1024;
-    while (cap < 8 * k && cap < 16384) cap <<= 1;
-    const size_t Tq = h_qoff[B];
-    ws->mv_qh.ensure(std::max<size_t>(Tq * dim * 2, 16));
-    ws->mv_qbad.ensure(std::max<size_t>(Tq, 1) * 4);
-    launch_mv_normalize_f16(d_q, Tq, dim, ws->mv_qh.p, ws->mv_qbad.as<uint32_t>(), st);
-    // per query: A, the k-th select, threshold, counters, the shortlist and its exact scores; per query vector: the
-    // keys of one chunk
-    const size_t per_q = ld * 4 + (size_t)k * 12 + (size_t)cap * 16 + 32, per_v = ldR * 4 + 4;
-    for (uint32_t qa = 0; qa < B;) {
-        uint32_t qb = qa + 1;
-        while (qb < B && (size_t)(qb + 1 - qa) * per_q + (size_t)(h_qoff[qb + 1] - h_qoff[qa]) * per_v <= left) qb++;
-        if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
-        const uint32_t b = qb - qa, va = h_qoff[qa], nqv = h_qoff[qb] - va;
-        ws->mv_Mk.ensure((size_t)nqv * ldR * 4);
-        ws->mv_A.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-        ws->mv_kd.ensure((size_t)b * k * 4); ws->mv_ki.ensure((size_t)b * k * 8); ws->mv_kc.ensure((size_t)b * 4);
-        ws->mv_thr.ensure((size_t)b * 4); ws->mv_cnt.ensure((size_t)b * 4); ws->mv_cand.ensure((size_t)b * cap * 4);
-        ws->mv_flags.ensure((size_t)b * 4); ws->mv_vflags.ensure((size_t)nqv * 4); ws->mv_gate.ensure(16);
-        ws->mv_ex.ensure((size_t)b * cap * 4); ws->mv_exid.ensure((size_t)b * cap * 8);
-        float *A = ws->mv_A.as<float>();
-        mv_stream(mv, ws, st, mv->vec_h_host.p, (size_t)dim * 2, cut16, deadline, [&](size_t c, void *Xh) {
-            const uint64_t ra = cut16[c], rb = cut16[c + 1], span = off[rb] - off[ra], ldc = (rb - ra + 3) & ~3ull;
-            LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ldc * 4, st));
-            MaxSimOut mo{};
-            mo.col_row = mv->col_row.as<uint32_t>() + off[ra]; mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ldc;
-            mo.row_base = (uint32_t)ra; mo.xdummy = mv->ysqrt.as<float>() + off[ra];
-            launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, Xh, nqv, span, dim, mo, mv->num_sms, st);
-            launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ldc, ws->mv_qoff.as<uint32_t>(), qa, qb, va, rb - ra, A + ra,
-                                 ld, mv->num_sms, st);
-        });
-        launch_select(select_rows(A, N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
-                                                  ws->mv_kc.as<uint32_t>()}), st);
-        launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
-                            ws->mv_thr.as<float>(), st);
-        LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
-        launch_mv_admit(A, ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(), ws->mv_cand.as<uint32_t>(),
-                        st);
-        launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
-                        ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
-        launch_mv_rescore_host(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), V, mv->ysqrt.as<float>(),
-                               mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
-                               ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(),
-                               mv->num_sms, st);
-        launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
-        // the fix-up of the flagged queries into A (free again), the f32 rows through staging buffer 0 on the call's
-        // stream: with no query flagged, every launch returns at once
-        const uint32_t *gate = ws->mv_gate.as<uint32_t>();
-        float *X = ws->hf_stage[0].as<float>();
-        for (size_t c = 0; c + 1 < cut32.size(); c++) {
-            const uint64_t ra = cut32[c], rb = cut32[c + 1];
-            launch_mv_copy_gated(V + off[ra] * dim, X, (off[rb] - off[ra]) * dim, gate, mv->num_sms, st);
-            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, A, ld, X, ra, rb, ws->mv_flags.as<uint32_t>(),
-                           ws->mv_vflags.as<uint32_t>(), gate);
-        }
-        SelectArgs sc = select_rows(A, N, ld, b, k, out.at(qa, k));
-        sc.col_ids = ids;
-        sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = gate;
-        launch_select(sc, st);
-        if (prof) {             // [0] rows admitted, [1] rows re-scored exactly, [2] queries redone densely
-            std::vector<uint32_t> cnt(b), fl(b);
-            LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->mv_cnt.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaMemcpyAsync(fl.data(), ws->mv_flags.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
-            LGPU_CUDA(cudaStreamSynchronize(st));
-            for (uint32_t q = 0; q < b; q++) {
-                g_filter_stats[0] += cnt[q]; g_filter_stats[1] += std::min(cnt[q], cap);
-                g_filter_stats[2] += fl[q] ? 1 : 0;
-            }
-        }
-        qa = qb;
-    }
-}
-
 // h_qoff: HOST [B+1] offsets of each query's vectors in d_q (validated by the caller).
+// Both routes (above) read the row data in chunks of whole rows, bounds cut[c]..cut[c + 1]: an HBM handle's one
+// resident chunk [0, N); a host handle's mv_chunks of one staging buffer each, streamed through Workspace::stage in
+// every sub-batch, so each vector crosses PCIe once per sub-batch.  The tensor-core GEMM keeps chunk-local keys
+// (row_base = the chunk's first row) and fills the chunk's columns of A.  A host handle re-scores the shortlist from the
+// pinned f32 vectors, and its fix-up copies each f32 chunk into staging buffer 0 by a kernel that returns at once when
+// the gate is 0: no host synchronisation decides anything.  Half the budget goes to the distance blocks of
+// mv_exact_dense; the other half, less a host handle's two staging buffers, is `left`.
 void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
                             uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                             RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
 {
     const uint64_t N = mv->nrows, ld = (N + 3) & ~3ull;
     const uint32_t dim = mv->dim, k = sp.k, Tq = h_qoff[B];
+    const uint64_t *off = mv->h_offsets.data();
+    const uint64_t *ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
     const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));
@@ -2262,57 +2171,117 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
     const size_t quarter = budget / 4;
     const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper && k <= SELECT_KMAX &&
                     (size_t)(max_nq + 1) * ld * 4 <= quarter;
-    if (mv->on_host) {
-        multivec_search_streamed(mv, ws, st, d_q, h_qoff, B, sp, tc, out, rf, deadline, prof);
-    } else if (tc) {
-        // fp16 normalised queries (and the queries holding a bad vector), then sub-batches of whole queries whose scores
-        // M [vectors][ld] u32 and approximate distances A [queries][ld] f32 take a quarter of the budget each
+    const size_t S = mv->on_host ? mv_stage_bytes(mv) : 0, left = budget / 2 > 2 * S ? budget / 2 - 2 * S : 0;
+    if (mv->on_host)
+        for (auto &b : ws->stage.buf) b.ensure(S);
+    // the chunks of a copy of the vectors at `vb` bytes each
+    auto chunks = [&](size_t vb) { return mv->on_host ? mv_chunks(mv, S / (dim * vb)) : std::vector<uint64_t>{0, N}; };
+    // use(ra, rb, X) for each chunk of `cut`, X its vectors: in `hbm`, or copied from `host`
+    auto each_chunk = [&](const std::vector<uint64_t> &cut, const void *hbm, const void *host, size_t vb, auto &&use) {
+        if (!mv->on_host) { use(cut[0], cut[1], hbm); return; }
+        ws->stage.open(ws, st, cut.size() - 1, deadline, [&](uint64_t c) -> std::pair<const void *, size_t> {
+            return {static_cast<const char *>(host) + off[cut[c]] * vb, (off[cut[c + 1]] - off[cut[c]]) * vb};
+        });
+        for (size_t c = 0; c + 1 < cut.size(); c++) {
+            use(cut[c], cut[c + 1], ws->stage.take(c));
+            ws->stage.release(c);
+        }
+        ws->stage.close();
+    };
+    const std::vector<uint64_t> cut32 = chunks(4);
+    if (!tc) {
+        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
+        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
+        for (uint32_t qa = 0; qa < B; qa += bs) {
+            const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
+            if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
+            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+            each_chunk(cut32, mv->vectors.p, mv->vectors_host.p, (size_t)dim * 4, [&](uint64_t ra, uint64_t rb, const void *X) {
+                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, static_cast<const float *>(X),
+                               ra, rb);
+            });
+            select_dense(ws, ws->D.as<float>(), N, ld, ids, b, sp, rf, out.at(qa, k), st);
+        }
+    } else {
+        // fp16 normalised queries (and the queries holding a bad vector)
         ws->mv_qh.ensure(std::max<size_t>((size_t)Tq * dim * 2, 16));
         ws->mv_qbad.ensure(std::max<size_t>(Tq, 1) * 4);
         launch_mv_normalize_f16(d_q, Tq, dim, ws->mv_qh.p, ws->mv_qbad.as<uint32_t>(), st);
         uint32_t cap = 1024;
         while (cap < 8 * k && cap < 16384) cap <<= 1;
+        const std::vector<uint64_t> cut16 = chunks(2);
+        uint64_t R = 1;                                   // the most rows of an operand chunk
+        for (size_t c = 0; c + 1 < cut16.size(); c++) R = std::max(R, cut16[c + 1] - cut16[c]);
+        const uint64_t ldR = (R + 3) & ~3ull;
+        // may queries [qa, qb] form one sub-batch?  An HBM handle: if their keys M [vectors][ld] u32 and approximate
+        // distances A [queries][ld] f32 take a quarter of the budget each.  A host handle: if their per-query state
+        // (A, the k-th select, threshold, counters, the shortlist and its exact scores) and per query vector the keys
+        // of one chunk fit `left`.
+        const size_t per_q = ld * 4 + (size_t)k * 12 + (size_t)cap * 16 + 32, per_v = ldR * 4 + 4;
+        auto fits = [&](uint32_t qa, uint32_t qb) {
+            const size_t nq = qb + 1 - qa, nv = h_qoff[qb + 1] - h_qoff[qa];
+            return mv->on_host ? nq * per_q + nv * per_v <= left : nv * ld * 4 <= quarter && nq * ld * 4 <= quarter;
+        };
+        const float *V = mv->on_host ? static_cast<const float *>(mv->vectors_host.dev) : mv->vectors.as<float>();
         for (uint32_t qa = 0; qa < B;) {
             uint32_t qb = qa + 1;
-            while (qb < B && (size_t)(h_qoff[qb + 1] - h_qoff[qa]) * ld * 4 <= quarter && (size_t)(qb + 1 - qa) * ld * 4 <= quarter)
-                qb++;
+            while (qb < B && fits(qa, qb)) qb++;
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             const uint32_t b = qb - qa, va = h_qoff[qa], nqv = h_qoff[qb] - va;
-            ws->mv_Mk.ensure((size_t)nqv * ld * 4);
+            ws->mv_Mk.ensure((size_t)nqv * ldR * 4);
             ws->mv_A.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
             ws->mv_kd.ensure((size_t)b * k * 4); ws->mv_ki.ensure((size_t)b * k * 8); ws->mv_kc.ensure((size_t)b * 4);
             ws->mv_thr.ensure((size_t)b * 4); ws->mv_cnt.ensure((size_t)b * 4); ws->mv_cand.ensure((size_t)b * cap * 4);
             ws->mv_flags.ensure((size_t)b * 4); ws->mv_vflags.ensure((size_t)nqv * 4); ws->mv_gate.ensure(16);
             ws->mv_ex.ensure((size_t)b * cap * 4); ws->mv_exid.ensure((size_t)b * cap * 8);
-            LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ld * 4, st));
-            MaxSimOut mo{};
-            mo.col_row = mv->col_row.as<uint32_t>(); mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ld; mo.row_base = 0;
-            mo.xdummy = mv->ysqrt.as<float>();
-            launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, mv->vec_h.p, nqv, mv->total, dim, mo,
-                               mv->num_sms, st);
-            launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ld, ws->mv_qoff.as<uint32_t>(), qa, qb, va, N,
-                                 ws->mv_A.as<float>(), ld, mv->num_sms, st);
+            float *A = ws->mv_A.as<float>();
+            each_chunk(cut16, mv->vec_h.p, mv->vec_h_host.p, (size_t)dim * 2, [&](uint64_t ra, uint64_t rb, const void *Xh) {
+                const uint64_t span = off[rb] - off[ra], ldc = (rb - ra + 3) & ~3ull;
+                LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ldc * 4, st));
+                MaxSimOut mo{};
+                mo.col_row = mv->col_row.as<uint32_t>() + off[ra]; mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ldc;
+                mo.row_base = (uint32_t)ra; mo.xdummy = mv->ysqrt.as<float>() + off[ra];
+                launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, Xh, nqv, span, dim, mo, mv->num_sms, st);
+                launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ldc, ws->mv_qoff.as<uint32_t>(), qa, qb, va, rb - ra,
+                                     A + ra, ld, mv->num_sms, st);
+            });
             // the k-th smallest approximate distance of each query
-            launch_select(select_rows(ws->mv_A.as<float>(), N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
-                                                                          ws->mv_kc.as<uint32_t>()}), st);
+            launch_select(select_rows(A, N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
+                                                      ws->mv_kc.as<uint32_t>()}), st);
             launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
                                 ws->mv_thr.as<float>(), st);
             LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
-            launch_mv_admit(ws->mv_A.as<float>(), ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(),
+            launch_mv_admit(A, ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(),
                             ws->mv_cand.as<uint32_t>(), st);
             launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
                             ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
-            launch_mv_rescore(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), mv->vectors.as<float>(),
-                              mv->ysqrt.as<float>(), mv->offsets.as<uint64_t>(),
-                              mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, dim, b, ws->mv_cand.as<uint32_t>(),
-                              ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), st);
+            if (mv->on_host)
+                launch_mv_rescore_host(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), V, mv->ysqrt.as<float>(),
+                                       mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
+                                       ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(),
+                                       mv->num_sms, st);
+            else
+                launch_mv_rescore(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), V, mv->ysqrt.as<float>(),
+                                  mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
+                                  ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), st);
             launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
-            // exact fix-up of the flagged queries (A is free again: it holds their exact distances)
-            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->mv_A.as<float>(), ld, mv->vectors.as<float>(), 0, N,
-                           ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>());
-            SelectArgs sc = select_rows(ws->mv_A.as<float>(), N, ld, b, k, out.at(qa, k));
-            sc.col_ids = mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr;
-            sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = ws->mv_gate.as<uint32_t>();
+            // exact fix-up of the flagged queries into A (free again: it holds their exact distances).  A host handle's
+            // f32 rows go through staging buffer 0 on the call's stream; with no query flagged, every launch returns at
+            // once
+            const uint32_t *gate = ws->mv_gate.as<uint32_t>();
+            for (size_t c = 0; c + 1 < cut32.size(); c++) {
+                const uint64_t ra = cut32[c], rb = cut32[c + 1];
+                const float *X = V + off[ra] * dim;
+                if (mv->on_host) {
+                    launch_mv_copy_gated(X, ws->stage.buf[0].as<float>(), (off[rb] - off[ra]) * dim, gate, mv->num_sms, st);
+                    X = ws->stage.buf[0].as<float>();
+                }
+                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, A, ld, X, ra, rb, ws->mv_flags.as<uint32_t>(),
+                               ws->mv_vflags.as<uint32_t>(), gate);
+            }
+            SelectArgs sc = select_rows(A, N, ld, b, k, out.at(qa, k));
+            sc.col_ids = ids;
+            sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = gate;
             launch_select(sc, st);
             if (prof) {             // [0] rows admitted, [1] rows re-scored exactly, [2] queries redone densely
                 std::vector<uint32_t> cnt(b), fl(b);
@@ -2325,18 +2294,6 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
                 }
             }
             qa = qb;
-        }
-    } else {
-        // (half the budget goes to the distance blocks of mv_exact_dense)
-        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
-        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / 2 / per_q, B));
-        for (uint32_t qa = 0; qa < B; qa += bs) {
-            const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
-            if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
-            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-            mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, mv->vectors.as<float>(), 0, N);
-            select_dense(ws, ws->D.as<float>(), N, ld, mv->has_ids ? mv->row_ids.as<uint64_t>() : nullptr, b, sp, rf,
-                         out.at(qa, k), st);
         }
     }
     if (prof) {                     // exact path: [1] rows scored exactly; both: [3] queries
@@ -4284,6 +4241,20 @@ int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_
     });
 }
 
+// |v| of n stored vectors in HBM into ysqrt and, given Xh, their fp16 normalised operand into Xh.  False when one of
+// them is zero or not finite: the tensor-core path may then not run.
+static bool mv_vector_terms(const float *X, uint64_t n, uint32_t dim, float *ysqrt, void *Xh)
+{
+    launch_row_norms(X, n, dim, ysqrt, nullptr);
+    if (!Xh) return true;
+    DevBuf bad;
+    bad.ensure(n * 4);
+    launch_mv_normalize_f16(X, n, dim, Xh, bad.as<uint32_t>(), nullptr);
+    std::vector<uint32_t> hb(n);
+    LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, n * 4, cudaMemcpyDeviceToHost));
+    return std::none_of(hb.begin(), hb.end(), [](uint32_t b) { return b != 0; });
+}
+
 int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
                        const uint64_t *row_ids, int device, lgpu_multivec **out)
 {
@@ -4322,36 +4293,24 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
             if (xbytes) memcpy(mv->vectors_host.p, values, xbytes);
             if (tc_shape) mv->vec_h_host.alloc(hbytes);
             const std::vector<uint64_t> cut = mv_chunks(mv, std::max<uint64_t>(1, FLAT_STAGE_BYTES / ((size_t)dim * 4)));
-            DevBuf xs, hs, bad;
-            std::vector<uint32_t> hb;
+            DevBuf xs, hs;
             for (size_t c = 0; c + 1 < cut.size(); c++) {
                 const uint64_t j0 = offsets[cut[c]], n = offsets[cut[c + 1]] - j0;
                 if (!n) continue;
                 xs.ensure(n * dim * 4);
+                if (tc_shape) hs.ensure(n * dim * 2);
                 LGPU_CUDA(cudaMemcpy(xs.p, values + j0 * dim, n * dim * 4, cudaMemcpyHostToDevice));
-                launch_row_norms(xs.as<float>(), n, dim, mv->ysqrt.as<float>() + j0, nullptr);
-                if (!tc_shape) continue;
-                hs.ensure(n * dim * 2); bad.ensure(n * 4); hb.resize(n);
-                launch_mv_normalize_f16(xs.as<float>(), n, dim, hs.p, bad.as<uint32_t>(), nullptr);
-                LGPU_CUDA(cudaMemcpy(static_cast<char *>(mv->vec_h_host.p) + j0 * dim * 2, hs.p, n * dim * 2,
-                                     cudaMemcpyDeviceToHost));
-                LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, n * 4, cudaMemcpyDeviceToHost));
-                for (uint64_t i = 0; i < n; i++) ok = ok && !hb[i];
+                ok &= mv_vector_terms(xs.as<float>(), n, dim, mv->ysqrt.as<float>() + j0, tc_shape ? hs.p : nullptr);
+                if (tc_shape)
+                    LGPU_CUDA(cudaMemcpy(static_cast<char *>(mv->vec_h_host.p) + j0 * dim * 2, hs.p, n * dim * 2,
+                                         cudaMemcpyDeviceToHost));
             }
         } else {
             mv->vectors.ensure(std::max<size_t>(xbytes, 16), true);
+            if (tc_shape) mv->vec_h.ensure(hbytes, true);
             if (T) {
                 LGPU_CUDA(cudaMemcpy(mv->vectors.p, values, xbytes, cudaMemcpyHostToDevice));
-                launch_row_norms(mv->vectors.as<float>(), T, dim, mv->ysqrt.as<float>(), nullptr);
-            }
-            if (tc_shape) {
-                mv->vec_h.ensure(hbytes, true);
-                DevBuf bad;
-                bad.ensure((size_t)T * 4);
-                launch_mv_normalize_f16(mv->vectors.as<float>(), T, dim, mv->vec_h.p, bad.as<uint32_t>(), nullptr);
-                std::vector<uint32_t> hb(T);
-                LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, (size_t)T * 4, cudaMemcpyDeviceToHost));
-                for (uint64_t i = 0; i < T; i++) ok = ok && !hb[i];
+                ok = mv_vector_terms(mv->vectors.as<float>(), T, dim, mv->ysqrt.as<float>(), tc_shape ? mv->vec_h.p : nullptr);
             }
         }
         if (tc_shape) {
