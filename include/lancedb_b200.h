@@ -555,6 +555,18 @@ int  lgpu_ivf_binary_search_unindexed_device(lgpu_ivf_binary *ix, lgpu_binary *t
  * exactly (on the exact path: B x nrows), [2] queries redone densely after the shortlist, [3] queries. */
 int  lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
                         const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device, lgpu_multivec **out);
+/* float16 multivector columns (list<fixed_size_list<float16, dim>>) kept as float16: 2 bytes per element instead of
+ * the 6 an f32 handle of the tensor-core shape holds (f32 vectors + their fp16 normalised copy), or the 4 it holds
+ * below it.  Queries stay f32.  _distance is the MaxSim distance of the query and the row's exact f32 upcast, so an
+ * fp16 handle opened on values x16 returns exactly -- same ids, counts and distance bits -- what lgpu_multivec_open on
+ * x16 converted to f32 returns, on every entry point (host, _filtered, _device), for every k, distance_range,
+ * prefilter, deleted rows, row ids, sub-batch split and placement (HBM or host), and lgpu_last_filter_stats means the
+ * same.  The paths are chosen as for f32 vectors; the tensor-core path multiplies fp16(q / |q|) by the stored vectors
+ * themselves (fp16 wgmma, f32 accumulation), scales each similarity by 1 / |v|, and re-scores its shortlist exactly.  A
+ * stored inf or NaN component, or a zero vector, sends the column to the exact path, as for f32 vectors.
+ * values: IEEE binary16 bits, [T][dim].  Every other lgpu_multivec_* function takes both row types. */
+int  lgpu_multivec_open_f16(const uint16_t *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
+                            const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device, lgpu_multivec **out);
 void lgpu_multivec_close(lgpu_multivec *mv);
 int  lgpu_multivec_search(lgpu_multivec *mv, const float *queries, const uint32_t *q_offsets, uint32_t B,
                           const lgpu_search_params *params, uint64_t *out_ids, float *out_dist, uint32_t *out_count);
@@ -567,27 +579,29 @@ int  lgpu_multivec_search_filtered(lgpu_multivec *mv, const float *queries, cons
 int  lgpu_multivec_search_device(lgpu_multivec *mv, const float *d_queries, const uint32_t *q_offsets, uint32_t B,
                                  const lgpu_search_params *params, uint64_t *d_out_ids, float *d_out_dist,
                                  uint32_t *d_out_count, void *cuda_stream);
-/* *bytes = the device memory the handle holds for its vectors and their per-vector and per-row data (f32 vectors,
- * tensor-core operand, |v|, the row of each vector, offsets, row ids, the live bitmap); the per-call search workspaces
- * (each within LGPU_WS_BYTES) are not counted.  A handle whose row data is in host memory (lgpu_multivec_host_bytes)
+/* *bytes = the device memory the handle holds for its vectors and their per-vector and per-row data (vectors in the
+ * row type, an f32 handle's tensor-core operand, |v|, the row of each vector, offsets, row ids, the live bitmap); the
+ * per-call search workspaces (each within LGPU_WS_BYTES) are not counted.  A handle whose row data is in host memory (lgpu_multivec_host_bytes)
  * holds only |v|, the row of each vector, the offsets, row ids and live bitmap here: 8 bytes per vector. */
 int  lgpu_multivec_device_bytes(const lgpu_multivec *mv, uint64_t *bytes);
-/* Where a multivector handle keeps its row data: the f32 vectors, plus the fp16 normalised tensor-core operand of a
- * column of the tensor-core shape (at least 65536 vectors, fewer than 2^31, dim a multiple of 8).  lgpu_multivec_open
- * copies it into HBM when it is at most LGPU_MULTIVEC_HBM_BYTES (read at every open; unset = no cap, 0 = never in HBM)
- * and the device's free memory covers it plus the workspace budget (LGPU_WS_BYTES, default 8 GiB).  Otherwise the
- * handle copies the vectors into pinned host memory that it owns and builds the operand there, both [T][dim] (freed by
+/* Where a multivector handle keeps its row data: the vectors in the row type, plus, for an f32 handle, the fp16
+ * normalised tensor-core operand of a column of the tensor-core shape (at least 65536 vectors, fewer than 2^31, dim a
+ * multiple of 8; an fp16 handle's vectors are their own operand).  lgpu_multivec_open[_f16] copies it into HBM when it
+ * is at most LGPU_MULTIVEC_HBM_BYTES (read at every open; unset = no cap, 0 = never in HBM) and the device's free
+ * memory covers it plus the workspace budget (LGPU_WS_BYTES, default 8 GiB).  Otherwise the handle copies the vectors
+ * into pinned host memory that it owns and builds an f32 handle's operand there, both [T][dim] (freed by
  * lgpu_multivec_close).  Every search of such a handle (host, _filtered, _device) streams chunks of whole rows through
- * two staging buffers of its workspace, within LGPU_WS_BYTES: each vector crosses PCIe once per call when the
- * workspace holds the per-query state of all B queries, else once per group of queries it holds; the tensor-core
- * route reads the fp16 operand and re-scores its shortlist from the pinned f32 vectors.  A staging buffer holds the
- * longest row: a search of a handle whose longest row does not fit twice in LGPU_WS_BYTES fails with LGPU_OOM before
- * any device work.  Results are identical to an HBM handle's on the same rows -- same ids, counts and distance bits --
- * for every k, distance_range, prefilter and deleted rows, and lgpu_last_filter_stats means the same.  A handle keeps
- * its placement for life.  A pinned allocation that fails is LGPU_OOM.  The caller's buffers are borrowed for the
- * open call only, either way.
- * *bytes = the pinned host memory the handle holds (T x dim x 4, plus T x dim x 2 for the operand; 0 for an HBM
- * handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output may be NULL. */
+ * two staging buffers of its workspace, within LGPU_WS_BYTES: each vector crosses PCIe once per call when the workspace
+ * holds the per-query state of all B queries, else once per group of queries it holds; the tensor-core route reads the
+ * fp16 operand and re-scores its shortlist from the pinned vectors.  A staging buffer holds the longest row: a search
+ * of a handle whose longest row does not fit twice in LGPU_WS_BYTES fails with LGPU_OOM before any device work.
+ * Results are identical to an HBM handle's on the same rows -- same ids, counts and distance bits -- for every k,
+ * distance_range, prefilter and deleted rows, and lgpu_last_filter_stats means the same.  A handle keeps its placement
+ * for life.  A pinned allocation that fails is LGPU_OOM.  The caller's buffers are borrowed for the open call only,
+ * either way.
+ * *bytes = the pinned host memory the handle holds (T x dim x 4, plus T x dim x 2 for the operand, for an f32 handle; T
+ * x dim x 2 for an fp16 handle; 0 for an HBM handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output
+ * may be NULL. */
 int  lgpu_multivec_host_bytes(const lgpu_multivec *mv, uint64_t *bytes, int *placement);
 
 /* ---- per-stage access (parity localisation and kernel benchmarks) -------- */
@@ -641,6 +655,11 @@ int lgpu_debug_rq_distances(const float *q_res, uint32_t B, const uint8_t *codes
  * out [nqv][nrows] f32); dim must be a multiple of 8 */
 int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
                            uint64_t nrows, uint32_t dim, int device, float *out);
+/* the same for fp16 values (IEEE binary16 bits), scored as an fp16 multivector handle scores them: out[i][r] = the
+ * largest (fp16(q_i / |q_i|) . v) * fl(1 / |v|) (f32 accumulation, f32 reciprocal and product) over row r's
+ * vectors v, NaN for an empty row; dim must be a multiple of 8 */
+int lgpu_debug_maxsim_gemm_f16(const float *queries, uint32_t nqv, const uint16_t *values, const uint64_t *offsets,
+                               uint64_t nrows, uint32_t dim, int device, float *out);
 /* the refine kernel of an index whose raw vectors are on the host, alone: out[q][c] = the exact distance (lgpu_metric)
  * of queries[q] and rows[pos[q][c]], +inf where pos is UINT64_MAX -- the value refine_factor re-ranks by.  The rows are
  * copied into pinned, mapped host memory and read from there (host buffers: queries [B][dim], rows [N][dim],

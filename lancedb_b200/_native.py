@@ -51,6 +51,7 @@ EXPORTS = [
     "lgpu_flat_open_f16", "lgpu_flat_append_f16", "lgpu_flat_device_bytes",
     "lgpu_index_host_bytes", "lgpu_debug_refine_host", "lgpu_flat_host_bytes",
     "lgpu_multivec_device_bytes", "lgpu_multivec_host_bytes",
+    "lgpu_multivec_open_f16", "lgpu_debug_maxsim_gemm_f16",
 ]
 VECTORS_NONE, VECTORS_HBM, VECTORS_HOST = 0, 1, 2     # lgpu_vectors_placement
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
@@ -209,6 +210,7 @@ def load():
     lib.lgpu_binary_search_device.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_debug_hamming_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
     lib.lgpu_multivec_open.argtypes = [vp, vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
+    lib.lgpu_multivec_open_f16.argtypes = [vp, vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
     lib.lgpu_multivec_close.argtypes = [vp]
     lib.lgpu_multivec_close.restype = None
     lib.lgpu_multivec_search.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
@@ -217,6 +219,7 @@ def load():
     lib.lgpu_multivec_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.lgpu_multivec_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
     lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
+    lib.lgpu_debug_maxsim_gemm_f16.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_sq_open.argtypes = [C.POINTER(SqDesc), C.POINTER(vp)]
     lib.lgpu_debug_sq_distances.argtypes = [vp, u32, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_hnsw_sq_open.argtypes = [C.POINTER(HnswSqDesc), C.POINTER(vp)]
@@ -725,12 +728,15 @@ class GpuMultivec(_RowsHandle):
     """A multivector column (list<fixed_size_list<float, dim>>) (lgpu_multivec), searched by late interaction:
     _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors.  Its vectors are
     kept in HBM when they fit (LGPU_MULTIVEC_HBM_BYTES), else in pinned host memory and streamed through the GPU once
-    per search, with the same results (`rows_on_host`)."""
+    per search, with the same results (`rows_on_host`).  A float16 `values` array opens an fp16 handle
+    (lgpu_multivec_open_f16: the vectors stay float16, results are those of their exact f32 upcast); anything else is
+    converted to f32.  `dtype` is the handle's row type."""
     _close = "lgpu_multivec_close"
     _delete = "lgpu_multivec_delete"
 
     def __init__(self, values, offsets, row_ids=None, device: int = 0):
-        v = np.ascontiguousarray(values, np.float32)
+        self.dtype = np.dtype(np.float16 if getattr(values, "dtype", None) == np.float16 else np.float32)
+        v = np.ascontiguousarray(values, self.dtype)
         off = np.ascontiguousarray(offsets, np.uint64)
         if v.ndim != 2:
             raise ValueError("multivector values must be a [vectors, dim] array")
@@ -747,7 +753,8 @@ class GpuMultivec(_RowsHandle):
         if rid is not None and rid.shape != (self.nrows,):
             raise ValueError("row_ids must hold one id per row")
         h = C.c_void_p()
-        check(load().lgpu_multivec_open(_ptr(v), _ptr(off), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
+        opener = "lgpu_multivec_open_f16" if self.dtype == np.float16 else "lgpu_multivec_open"
+        check(getattr(load(), opener)(_ptr(v), _ptr(off), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
 
@@ -764,8 +771,8 @@ class GpuMultivec(_RowsHandle):
         return b.value, where.value
 
     def host_bytes(self) -> int:
-        """The pinned host memory the handle holds: its vectors (and tensor-core operand) when they did not fit in HBM
-        at open, else 0 (lgpu_multivec_host_bytes)."""
+        """The pinned host memory the handle holds: its vectors (and an f32 handle's tensor-core operand) when they did
+        not fit in HBM at open, else 0 (lgpu_multivec_host_bytes)."""
         return self._host()[0]
 
     @property
@@ -1024,14 +1031,17 @@ def debug_rq_distances(q_res, codes, add_factors, scale_factors, metric: str = "
 
 def debug_maxsim_gemm(queries, values, offsets, device: int = 0) -> np.ndarray:
     """The multivector tensor-core score alone: [nqv, nrows] f32, the largest fp16 normalised similarity of each query
-    vector over each row's vectors (NaN for an empty row)."""
-    q = np.ascontiguousarray(queries, np.float32); x = np.ascontiguousarray(values, np.float32)
+    vector over each row's vectors (NaN for an empty row).  float16 values are scored as an fp16 handle scores them
+    (lgpu_debug_maxsim_gemm_f16: the stored vectors as they are, each similarity scaled by 1 / |v|); anything else is
+    converted to f32."""
+    f16 = getattr(values, "dtype", None) == np.float16
+    q = np.ascontiguousarray(queries, np.float32); x = np.ascontiguousarray(values, np.float16 if f16 else np.float32)
     off = np.ascontiguousarray(offsets, np.uint64)
     if q.ndim != 2 or x.ndim != 2 or q.shape[1] != x.shape[1] or int(off[-1]) != x.shape[0]:
         raise ValueError("queries [nqv, dim], values [T, dim] and offsets [nrows + 1] ending at T are required")
     out = np.empty((q.shape[0], off.size - 1), np.float32)
-    check(load().lgpu_debug_maxsim_gemm(_ptr(q), q.shape[0], _ptr(x), _ptr(off), off.size - 1, q.shape[1], device,
-                                        _ptr(out)))
+    fn = load().lgpu_debug_maxsim_gemm_f16 if f16 else load().lgpu_debug_maxsim_gemm
+    check(fn(_ptr(q), q.shape[0], _ptr(x), _ptr(off), off.size - 1, q.shape[1], device, _ptr(out)))
     return out
 
 

@@ -564,12 +564,15 @@ struct lgpu_multivec {
     uint64_t nrows = 0, total = 0;         // rows; stored vectors T = offsets[nrows]
     uint32_t dim = 0;
     uint64_t max_row = 0;                  // largest n_r
-    DevBuf vectors, ysqrt, offsets, row_ids;   // [T][dim] f32, |v| = sqrt(dot(v, v)) per vector, [nrows+1], optional ids
-    DevBuf vec_h, col_row;                 // tensor-core path: fp16 normalised vectors [T][dim], row of each vector [T]
+    bool f16 = false;                      // row type: `vectors` holds f32, or fp16 (lgpu_multivec_open_f16)
+    DevBuf vectors, ysqrt, offsets, row_ids;   // [T][dim] in the row type, |v| = sqrt(dot(v, v)) per vector, [nrows+1], ids
+    // tensor-core path: fp16 normalised vectors [T][dim] (f32 handles; an fp16 handle's vectors are their own operand),
+    // row of each vector [T]
+    DevBuf vec_h, col_row;
     bool tc_ok = false;                    // the tensor-core path may run (see multivec_search_device)
-    // row data that did not fit in HBM at open (lgpu_multivec_open): `vectors_host` holds the f32 vectors and
-    // `vec_h_host` the fp16 operand (tensor-core shape only), both [T][dim]; `vectors` and `vec_h` stay empty, and
-    // searches stream the rows through HBM (multivec_search_device)
+    // row data that did not fit in HBM at open (multivec_open): `vectors_host` holds the vectors in the row type and
+    // `vec_h_host` the fp16 operand (f32 handles of the tensor-core shape only), both [T][dim]; `vectors` and `vec_h`
+    // stay empty, and searches stream the rows through HBM (multivec_search_device)
     bool on_host = false;
     PinnedBuf vectors_host, vec_h_host;
     std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
@@ -2053,13 +2056,15 @@ constexpr uint64_t MV_MAX_ROW = (uint64_t)1 << 20;
 constexpr uint32_t MV_MAX_DIM = 65536;
 
 // Paths (multivec.cu, DESIGN.md section 6), chosen per call:
-//   tensor cores  the F16MaxSim gemm_dist_kernel scores fp16 copies of the normalised vectors and keeps the largest
-//                 similarity per (query vector, row); approximate distances -> the k-th smallest (select mode 1) -> every
-//                 row within 2 E_q of it (mv_band) -> exact re-score of those rows (dist.cu) -> select mode 2; a query
-//                 whose list overflowed or that holds a zero / non-finite vector is redone by the exact path below in
-//                 the same stream (flags / gate: nothing runs when no query is flagged).  Taken when the column holds at
-//                 least MV_TC_MIN_T vectors (all of them finite and non-zero), dim is a multiple of 8, there is no
-//                 prefilter or distance_range, LGPU_NO_TENSOR_CORE is not set and one query's scores fit the workspace.
+//   tensor cores  the F16MaxSim gemm_dist_kernel scores fp16 copies of the normalised vectors (an fp16 handle: the
+//                 F16RowMaxSim policy, fp16 normalised queries against the stored vectors, each similarity scaled by
+//                 1 / |v|) and keeps the largest similarity per (query vector, row); approximate distances -> the k-th
+//                 smallest (select mode 1) -> every row within 2 E_q of it (mv_band, mv_band_f16) -> exact re-score of
+//                 those rows (dist.cu) -> select mode 2; a query whose list overflowed or that holds a zero /
+//                 non-finite vector is redone by the exact path below in the same stream (flags / gate: nothing runs
+//                 when no query is flagged).  Taken when the column holds at least MV_TC_MIN_T vectors (all of them
+//                 finite and non-zero), dim is a multiple of 8, there is no prefilter or distance_range,
+//                 LGPU_NO_TENSOR_CORE is not set and one query's scores fit the workspace.
 //   exact         for every sub-batch of queries, blocks of consecutive query vectors against chunks of whole rows --
 //                 dist_matrix_kernel (cosine, lance order) -> per-row minimum -> in-order running sum into D[b][N] --
 //                 then select mode 1 (distance_range, prefilter, (_distance, _rowid) order, NaN dropped).
@@ -2067,10 +2072,11 @@ constexpr uint32_t MV_MAX_DIM = 65536;
 constexpr uint64_t MV_TC_MIN_T = 65536;   // stored vectors from which the tensor-core path runs (not measured)
 
 // the exact distances of queries [qa, qb) to rows [ra, rb) into D[b - qa][ra..rb) (only / vflags / gate: the fix-up of
-// flagged queries).  X holds the vectors of those rows, from the first vector of row ra (a host handle's staged chunk);
-// the order of the additions per row depends only on the blocking of the query vectors, not on [ra, rb).
+// flagged queries).  X holds the vectors of those rows in the row type, from the first vector of row ra (a host
+// handle's staged chunk); the order of the additions per row depends only on the blocking of the query vectors, not
+// on [ra, rb).
 static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
-                           uint32_t qa, uint32_t qb, float *D, uint64_t ld, const float *X, uint64_t ra, uint64_t rb,
+                           uint32_t qa, uint32_t qb, float *D, uint64_t ld, const void *X, uint64_t ra, uint64_t rb,
                            const uint32_t *only = nullptr, const uint32_t *vflags = nullptr,
                            const uint32_t *gate = nullptr)
 {
@@ -2095,10 +2101,15 @@ static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, co
             const uint32_t nr = (uint32_t)(r1 - r0);
             ws->mv_P.ensure(std::max<size_t>((size_t)nqv * ldP, 4) * 4);
             ws->mv_M.ensure((size_t)nqv * nr * 4);
-            if (span)
-                launch_dist_matrix(d_q + (size_t)i0 * dim, X + (size_t)(off[r0] - off[ra]) * dim, nqv, span,
-                                   dim, 2, ws->xnorm.as<float>() + i0, mv->ysqrt.as<float>() + off[r0],
-                                   ws->mv_P.as<float>(), ldP, st, vflags ? vflags + (i0 - h_qoff[qa]) : nullptr, gate);
+            auto dist = [&](auto *x) {
+                launch_dist_matrix(d_q + (size_t)i0 * dim, x + (size_t)(off[r0] - off[ra]) * dim, nqv, span, dim, 2,
+                                   ws->xnorm.as<float>() + i0, mv->ysqrt.as<float>() + off[r0], ws->mv_P.as<float>(),
+                                   ldP, st, vflags ? vflags + (i0 - h_qoff[qa]) : nullptr, gate);
+            };
+            if (span) {
+                if (mv->f16) dist(static_cast<const __half *>(X));
+                else dist(static_cast<const float *>(X));
+            }
             launch_mv_rowmin(ws->mv_P.as<float>(), ldP, nqv, mv->offsets.as<uint64_t>(), r0, nr, ws->mv_M.as<float>(),
                              nr, mv->num_sms, st, gate);
             launch_mv_rowsum(ws->mv_M.as<float>(), nr, ws->mv_qoff.as<uint32_t>(), blo, bhi, qa, i0, i1, nr, D, ld, r0,
@@ -2110,16 +2121,19 @@ static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, co
 
 // ---- a host multivector handle (lgpu_multivec::on_host): its row data crosses PCIe in chunks of whole rows ----
 // The bytes of one staging buffer: FLAT_STAGE_BYTES, or an eighth of the budget when that is smaller, and never less
-// than the longest row's f32 vectors.  Two such buffers must fit the budget (mv_check_stage, before any device work).
+// than the longest row's vectors in the row type.  Two such buffers must fit the budget (mv_check_stage, before any
+// device work).
+static size_t mv_elem_bytes(const lgpu_multivec *mv) { return mv->f16 ? 2 : 4; }
+
 static size_t mv_stage_bytes(const lgpu_multivec *mv)
 {
-    const size_t longest = (size_t)mv->max_row * mv->dim * 4;
+    const size_t longest = (size_t)mv->max_row * mv->dim * mv_elem_bytes(mv);
     return std::max<size_t>(std::min(FLAT_STAGE_BYTES, workspace_budget() / 8), std::max<size_t>(longest, 16));
 }
 
 static void mv_check_stage(const lgpu_multivec *mv)
 {
-    const size_t longest = (size_t)mv->max_row * mv->dim * 4;
+    const size_t longest = (size_t)mv->max_row * mv->dim * mv_elem_bytes(mv);
     if (mv->on_host && 2 * longest > workspace_budget()) {
         set_error("a multivector row of " + std::to_string(mv->max_row) + " vectors (" + std::to_string(longest) +
                   " bytes) does not fit twice in the workspace budget (LGPU_WS_BYTES) that streams a host handle");
@@ -2147,9 +2161,10 @@ static std::vector<uint64_t> mv_chunks(const lgpu_multivec *mv, uint64_t cap_vec
 // resident chunk [0, N); a host handle's mv_chunks of one staging buffer each, streamed through Workspace::stage in
 // every sub-batch, so each vector crosses PCIe once per sub-batch.  The tensor-core GEMM keeps chunk-local keys
 // (row_base = the chunk's first row) and fills the chunk's columns of A.  A host handle re-scores the shortlist from the
-// pinned f32 vectors, and its fix-up copies each f32 chunk into staging buffer 0 by a kernel that returns at once when
-// the gate is 0: no host synchronisation decides anything.  Half the budget goes to the distance blocks of
-// mv_exact_dense; the other half, less a host handle's two staging buffers, is `left`.
+// pinned vectors, and its fix-up copies each chunk of them into staging buffer 0 by a kernel that returns at once when
+// the gate is 0: no host synchronisation decides anything.  The vectors are in the row type (es bytes per element); an
+// fp16 handle's vectors are also its tensor-core operand, so both routes stream the same 2-byte rows.  Half the budget
+// goes to the distance blocks of mv_exact_dense; the other half, less a host handle's two staging buffers, is `left`.
 void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
                             uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                             RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
@@ -2188,7 +2203,8 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
         }
         ws->stage.close();
     };
-    const std::vector<uint64_t> cut32 = chunks(4);
+    const size_t es = mv_elem_bytes(mv);
+    const std::vector<uint64_t> cutv = chunks(es);                  // chunks of the vectors in the row type
     if (!tc) {
         const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
         const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
@@ -2196,9 +2212,8 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-            each_chunk(cut32, mv->vectors.p, mv->vectors_host.p, (size_t)dim * 4, [&](uint64_t ra, uint64_t rb, const void *X) {
-                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, static_cast<const float *>(X),
-                               ra, rb);
+            each_chunk(cutv, mv->vectors.p, mv->vectors_host.p, (size_t)dim * es, [&](uint64_t ra, uint64_t rb, const void *X) {
+                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, X, ra, rb);
             });
             select_dense(ws, ws->D.as<float>(), N, ld, ids, b, sp, rf, out.at(qa, k), st);
         }
@@ -2222,7 +2237,9 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             const size_t nq = qb + 1 - qa, nv = h_qoff[qb + 1] - h_qoff[qa];
             return mv->on_host ? nq * per_q + nv * per_v <= left : nv * ld * 4 <= quarter && nq * ld * 4 <= quarter;
         };
-        const float *V = mv->on_host ? static_cast<const float *>(mv->vectors_host.dev) : mv->vectors.as<float>();
+        const void *V = mv->on_host ? mv->vectors_host.dev : mv->vectors.p;        // the vectors, for the re-score
+        const void *Xop = mv->f16 ? mv->vectors.p : mv->vec_h.p;                  // the operand, in HBM
+        const void *Xop_host = mv->f16 ? mv->vectors_host.p : mv->vec_h_host.p;   // ... or pinned
         for (uint32_t qa = 0; qa < B;) {
             uint32_t qb = qa + 1;
             while (qb < B && fits(qa, qb)) qb++;
@@ -2235,13 +2252,14 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             ws->mv_flags.ensure((size_t)b * 4); ws->mv_vflags.ensure((size_t)nqv * 4); ws->mv_gate.ensure(16);
             ws->mv_ex.ensure((size_t)b * cap * 4); ws->mv_exid.ensure((size_t)b * cap * 8);
             float *A = ws->mv_A.as<float>();
-            each_chunk(cut16, mv->vec_h.p, mv->vec_h_host.p, (size_t)dim * 2, [&](uint64_t ra, uint64_t rb, const void *Xh) {
+            each_chunk(cut16, Xop, Xop_host, (size_t)dim * 2, [&](uint64_t ra, uint64_t rb, const void *Xh) {
                 const uint64_t span = off[rb] - off[ra], ldc = (rb - ra + 3) & ~3ull;
                 LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ldc * 4, st));
                 MaxSimOut mo{};
                 mo.col_row = mv->col_row.as<uint32_t>() + off[ra]; mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ldc;
-                mo.row_base = (uint32_t)ra; mo.xdummy = mv->ysqrt.as<float>() + off[ra];
-                launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, Xh, nqv, span, dim, mo, mv->num_sms, st);
+                mo.row_base = (uint32_t)ra; mo.vnorm = mv->ysqrt.as<float>() + off[ra];
+                launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, Xh, nqv, span, dim, mo, mv->f16,
+                                   mv->num_sms, st);
                 launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ldc, ws->mv_qoff.as<uint32_t>(), qa, qb, va, rb - ra,
                                      A + ra, ld, mv->num_sms, st);
             });
@@ -2249,32 +2267,43 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             launch_select(select_rows(A, N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
                                                       ws->mv_kc.as<uint32_t>()}), st);
             launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
-                                ws->mv_thr.as<float>(), st);
+                                mv->f16, ws->mv_thr.as<float>(), st);
             LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
             launch_mv_admit(A, ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(),
                             ws->mv_cand.as<uint32_t>(), st);
             launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
                             ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
-            if (mv->on_host)
-                launch_mv_rescore_host(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), V, mv->ysqrt.as<float>(),
-                                       mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
-                                       ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(),
-                                       mv->num_sms, st);
-            else
-                launch_mv_rescore(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), V, mv->ysqrt.as<float>(),
-                                  mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
-                                  ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), st);
+            auto rescore = [&](auto *v) {
+                if (mv->on_host)
+                    launch_mv_rescore_host(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), v,
+                                           mv->ysqrt.as<float>(), mv->offsets.as<uint64_t>(), ids, dim, b,
+                                           ws->mv_cand.as<uint32_t>(), ws->mv_cnt.as<uint32_t>(), cap,
+                                           ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), mv->num_sms, st);
+                else
+                    launch_mv_rescore(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), v, mv->ysqrt.as<float>(),
+                                      mv->offsets.as<uint64_t>(), ids, dim, b, ws->mv_cand.as<uint32_t>(),
+                                      ws->mv_cnt.as<uint32_t>(), cap, ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(),
+                                      st);
+            };
+            if (mv->f16) rescore(static_cast<const __half *>(V));
+            else rescore(static_cast<const float *>(V));
             launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
             // exact fix-up of the flagged queries into A (free again: it holds their exact distances).  A host handle's
-            // f32 rows go through staging buffer 0 on the call's stream; with no query flagged, every launch returns at
+            // rows go through staging buffer 0 on the call's stream; with no query flagged, every launch returns at
             // once
             const uint32_t *gate = ws->mv_gate.as<uint32_t>();
-            for (size_t c = 0; c + 1 < cut32.size(); c++) {
-                const uint64_t ra = cut32[c], rb = cut32[c + 1];
-                const float *X = V + off[ra] * dim;
+            for (size_t c = 0; c + 1 < cutv.size(); c++) {
+                const uint64_t ra = cutv[c], rb = cutv[c + 1];
+                const void *X = static_cast<const char *>(V) + off[ra] * dim * es;
                 if (mv->on_host) {
-                    launch_mv_copy_gated(X, ws->stage.buf[0].as<float>(), (off[rb] - off[ra]) * dim, gate, mv->num_sms, st);
-                    X = ws->stage.buf[0].as<float>();
+                    const uint64_t n = (off[rb] - off[ra]) * dim;
+                    if (mv->f16)
+                        launch_mv_copy_gated(static_cast<const __half *>(X), ws->stage.buf[0].as<__half>(), n, gate,
+                                             mv->num_sms, st);
+                    else
+                        launch_mv_copy_gated(static_cast<const float *>(X), ws->stage.buf[0].as<float>(), n, gate,
+                                             mv->num_sms, st);
+                    X = ws->stage.buf[0].p;
                 }
                 mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, A, ld, X, ra, rb, ws->mv_flags.as<uint32_t>(),
                                ws->mv_vflags.as<uint32_t>(), gate);
@@ -4241,22 +4270,27 @@ int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_
     });
 }
 
-// |v| of n stored vectors in HBM into ysqrt and, given Xh, their fp16 normalised operand into Xh.  False when one of
-// them is zero or not finite: the tensor-core path may then not run.
-static bool mv_vector_terms(const float *X, uint64_t n, uint32_t dim, float *ysqrt, void *Xh)
+// |v| of n stored vectors in HBM (f32, or fp16 when f16) into ysqrt and, when `check`, whether every one of them is
+// finite and non-zero (false: the tensor-core path may not run), with the fp16 normalised operand of f32 vectors into
+// Xh.  fp16 vectors are their own operand: the same kernels read their exact f32 upcast, so |v| and the check are an
+// f32 handle's on those values.
+static bool mv_vector_terms(const void *X, bool f16, uint64_t n, uint32_t dim, float *ysqrt, bool check, void *Xh)
 {
-    launch_row_norms(X, n, dim, ysqrt, nullptr);
-    if (!Xh) return true;
+    if (f16) launch_row_norms(static_cast<const __half *>(X), n, dim, ysqrt, nullptr);
+    else launch_row_norms(static_cast<const float *>(X), n, dim, ysqrt, nullptr);
+    if (!check) return true;
     DevBuf bad;
     bad.ensure(n * 4);
-    launch_mv_normalize_f16(X, n, dim, Xh, bad.as<uint32_t>(), nullptr);
+    if (f16) launch_mv_normalize_f16(static_cast<const __half *>(X), n, dim, nullptr, bad.as<uint32_t>(), nullptr);
+    else launch_mv_normalize_f16(static_cast<const float *>(X), n, dim, Xh, bad.as<uint32_t>(), nullptr);
     std::vector<uint32_t> hb(n);
     LGPU_CUDA(cudaMemcpy(hb.data(), bad.p, n * 4, cudaMemcpyDeviceToHost));
     return std::none_of(hb.begin(), hb.end(), [](uint32_t b) { return b != 0; });
 }
 
-int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
-                       const uint64_t *row_ids, int device, lgpu_multivec **out)
+// lgpu_multivec_open and lgpu_multivec_open_f16: vectors f32 or fp16 (f16), kept as given
+static int multivec_open(const void *values, bool f16, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
+                         const uint64_t *row_ids, int device, lgpu_multivec **out)
 {
     lgpu_multivec *mv = nullptr;
     int rc = guarded([&] {
@@ -4274,43 +4308,47 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
         LGPU_REQUIRE(T == 0 || values != nullptr, "null vectors");
         require_device(device);
         mv = new lgpu_multivec();
-        mv->device = device; mv->nrows = nrows; mv->total = T; mv->dim = dim; mv->max_row = max_row;
+        mv->device = device; mv->nrows = nrows; mv->total = T; mv->dim = dim; mv->max_row = max_row; mv->f16 = f16;
         mv->h_offsets.assign(offsets, offsets + nrows + 1);
         // the tensor-core operand: only when every stored vector normalises (a zero or non-finite vector has NaN pairs,
-        // which the approximate score cannot skip as the exact min does) and the shape suits the GEMM
+        // which the approximate score cannot skip as the exact min does) and the shape suits the GEMM.  An fp16
+        // handle's vectors are their own operand: no copy
         const bool tc_shape = T >= MV_TC_MIN_T && T < ((uint64_t)1 << 31) && nrows < 0xffffffffull &&
                               gemm_shape_supported(dim);
-        const size_t xbytes = (size_t)T * dim * 4, hbytes = tc_shape ? (size_t)T * dim * 2 : 0;
+        const size_t es = f16 ? 2 : 4;
+        const size_t xbytes = (size_t)T * dim * es, hbytes = tc_shape && !f16 ? (size_t)T * dim * 2 : 0;
         mv->ysqrt.ensure(std::max<size_t>((size_t)T * 4, 16));
         mv->offsets.ensure((size_t)(nrows + 1) * 8);
         LGPU_CUDA(cudaMemcpy(mv->offsets.p, offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice));
         bool ok = true;
         if (!rows_fit_hbm("LGPU_MULTIVEC_HBM_BYTES", xbytes + hbytes)) {
-            // pinned host memory: the f32 vectors as given, |v| and the fp16 operand computed chunk by chunk of whole
-            // rows staged through HBM (each vector's terms depend on that vector alone)
+            // pinned host memory: the vectors as given, |v| (and an f32 handle's fp16 operand) computed chunk by chunk
+            // of whole rows staged through HBM (each vector's terms depend on that vector alone)
             mv->on_host = true;
             mv->vectors_host.alloc(xbytes);
             if (xbytes) memcpy(mv->vectors_host.p, values, xbytes);
-            if (tc_shape) mv->vec_h_host.alloc(hbytes);
-            const std::vector<uint64_t> cut = mv_chunks(mv, std::max<uint64_t>(1, FLAT_STAGE_BYTES / ((size_t)dim * 4)));
+            if (hbytes) mv->vec_h_host.alloc(hbytes);
+            const std::vector<uint64_t> cut = mv_chunks(mv, std::max<uint64_t>(1, FLAT_STAGE_BYTES / ((size_t)dim * es)));
             DevBuf xs, hs;
             for (size_t c = 0; c + 1 < cut.size(); c++) {
                 const uint64_t j0 = offsets[cut[c]], n = offsets[cut[c + 1]] - j0;
                 if (!n) continue;
-                xs.ensure(n * dim * 4);
-                if (tc_shape) hs.ensure(n * dim * 2);
-                LGPU_CUDA(cudaMemcpy(xs.p, values + j0 * dim, n * dim * 4, cudaMemcpyHostToDevice));
-                ok &= mv_vector_terms(xs.as<float>(), n, dim, mv->ysqrt.as<float>() + j0, tc_shape ? hs.p : nullptr);
-                if (tc_shape)
+                xs.ensure(n * dim * es);
+                if (hbytes) hs.ensure(n * dim * 2);
+                LGPU_CUDA(cudaMemcpy(xs.p, static_cast<const char *>(values) + j0 * dim * es, n * dim * es,
+                                     cudaMemcpyHostToDevice));
+                ok &= mv_vector_terms(xs.p, f16, n, dim, mv->ysqrt.as<float>() + j0, tc_shape, hbytes ? hs.p : nullptr);
+                if (hbytes)
                     LGPU_CUDA(cudaMemcpy(static_cast<char *>(mv->vec_h_host.p) + j0 * dim * 2, hs.p, n * dim * 2,
                                          cudaMemcpyDeviceToHost));
             }
         } else {
             mv->vectors.ensure(std::max<size_t>(xbytes, 16), true);
-            if (tc_shape) mv->vec_h.ensure(hbytes, true);
+            if (hbytes) mv->vec_h.ensure(hbytes, true);
             if (T) {
                 LGPU_CUDA(cudaMemcpy(mv->vectors.p, values, xbytes, cudaMemcpyHostToDevice));
-                ok = mv_vector_terms(mv->vectors.as<float>(), T, dim, mv->ysqrt.as<float>(), tc_shape ? mv->vec_h.p : nullptr);
+                ok = mv_vector_terms(mv->vectors.p, f16, T, dim, mv->ysqrt.as<float>(), tc_shape,
+                                     hbytes ? mv->vec_h.p : nullptr);
             }
         }
         if (tc_shape) {
@@ -4328,6 +4366,18 @@ int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nr
     });
     if (rc != LGPU_OK && mv) delete mv;
     return rc;
+}
+
+int lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
+                       const uint64_t *row_ids, int device, lgpu_multivec **out)
+{
+    return multivec_open(values, false, offsets, nrows, dim, row_ids, device, out);
+}
+
+int lgpu_multivec_open_f16(const uint16_t *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
+                           const uint64_t *row_ids, int device, lgpu_multivec **out)
+{
+    return multivec_open(values, true, offsets, nrows, dim, row_ids, device, out);
 }
 
 int lgpu_multivec_device_bytes(const lgpu_multivec *mvh, uint64_t *bytes)
@@ -4393,8 +4443,11 @@ int lgpu_multivec_search_device(lgpu_multivec *mvh, const float *d_queries, cons
                          d_out_count);
 }
 
-int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
-                           uint64_t nrows, uint32_t dim, int device, float *out)
+// lgpu_debug_maxsim_gemm (f32 values: the F16MaxSim operand built as an f32 handle builds it) and
+// lgpu_debug_maxsim_gemm_f16 (fp16 values: the F16RowMaxSim score on the values as they are, over |v| as an fp16 handle
+// computes it)
+static int debug_maxsim_gemm(const float *queries, uint32_t nqv, const void *values, bool f16, const uint64_t *offsets,
+                             uint64_t nrows, uint32_t dim, int device, float *out)
 {
     return guarded([&] {
         LGPU_REQUIRE(offsets != nullptr && (nqv == 0 || (queries && out)), "null buffer");
@@ -4407,29 +4460,43 @@ int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *valu
         if (nqv == 0 || nrows == 0) return;
         cudaDeviceProp prop;
         LGPU_CUDA(cudaGetDeviceProperties(&prop, device));
-        DevBuf q, x, qh, xh, bad, cr, M;
-        q.ensure((size_t)nqv * dim * 4); x.ensure(std::max<size_t>((size_t)T * dim * 4, 16));
+        const size_t es = f16 ? 2 : 4;
+        DevBuf q, x, qh, xh, bad, cr, M, vn;
+        q.ensure((size_t)nqv * dim * 4); x.ensure(std::max<size_t>((size_t)T * dim * es, 16));
         qh.ensure((size_t)nqv * dim * 2); xh.ensure(std::max<size_t>((size_t)T * dim * 2, 16));
         bad.ensure(std::max<size_t>(std::max<uint64_t>(T, nqv), 1) * 4); cr.ensure(std::max<size_t>(T, 1) * 4);
-        M.ensure((size_t)nqv * nrows * 4);
+        M.ensure((size_t)nqv * nrows * 4); vn.ensure(std::max<size_t>(T, 1) * 4);
         std::vector<uint32_t> hcr(T);
         for (uint64_t r = 0; r < nrows; r++)
             for (uint64_t j = offsets[r]; j < offsets[r + 1]; j++) hcr[j] = (uint32_t)r;
         LGPU_CUDA(cudaMemcpy(q.p, queries, (size_t)nqv * dim * 4, cudaMemcpyHostToDevice));
         if (T) {
-            LGPU_CUDA(cudaMemcpy(x.p, values, (size_t)T * dim * 4, cudaMemcpyHostToDevice));
+            LGPU_CUDA(cudaMemcpy(x.p, values, (size_t)T * dim * es, cudaMemcpyHostToDevice));
             LGPU_CUDA(cudaMemcpy(cr.p, hcr.data(), (size_t)T * 4, cudaMemcpyHostToDevice));
         }
         LGPU_CUDA(cudaMemset(M.p, 0, (size_t)nqv * nrows * 4));
         launch_mv_normalize_f16(q.as<float>(), nqv, dim, qh.p, bad.as<uint32_t>(), nullptr);
-        launch_mv_normalize_f16(x.as<float>(), T, dim, xh.p, bad.as<uint32_t>(), nullptr);
+        if (f16) launch_row_norms(x.as<__half>(), T, dim, vn.as<float>(), nullptr);
+        else launch_mv_normalize_f16(x.as<float>(), T, dim, xh.p, bad.as<uint32_t>(), nullptr);
         MaxSimOut mo{};
-        mo.col_row = cr.as<uint32_t>(); mo.M = M.as<uint32_t>(); mo.ldM = nrows; mo.row_base = 0; mo.xdummy = x.as<float>();
-        launch_maxsim_gemm(qh.p, xh.p, nqv, T, dim, mo, prop.multiProcessorCount, nullptr);
+        mo.col_row = cr.as<uint32_t>(); mo.M = M.as<uint32_t>(); mo.ldM = nrows; mo.row_base = 0; mo.vnorm = vn.as<float>();
+        launch_maxsim_gemm(qh.p, f16 ? x.p : xh.p, nqv, T, dim, mo, f16, prop.multiProcessorCount, nullptr);
         std::vector<uint32_t> keys((size_t)nqv * nrows);
         LGPU_CUDA(cudaMemcpy(keys.data(), M.p, keys.size() * 4, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < keys.size(); i++) out[i] = keys[i] ? key_f32(keys[i]) : NAN;
     });
+}
+
+int lgpu_debug_maxsim_gemm(const float *queries, uint32_t nqv, const float *values, const uint64_t *offsets,
+                           uint64_t nrows, uint32_t dim, int device, float *out)
+{
+    return debug_maxsim_gemm(queries, nqv, values, false, offsets, nrows, dim, device, out);
+}
+
+int lgpu_debug_maxsim_gemm_f16(const float *queries, uint32_t nqv, const uint16_t *values, const uint64_t *offsets,
+                               uint64_t nrows, uint32_t dim, int device, float *out)
+{
+    return debug_maxsim_gemm(queries, nqv, values, true, offsets, nrows, dim, device, out);
 }
 
 int lgpu_debug_hamming_gemm(const uint8_t *queries, const uint8_t *vectors, uint32_t B, uint64_t N, uint32_t nbytes,

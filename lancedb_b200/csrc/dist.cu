@@ -347,9 +347,11 @@ __device__ __forceinline__ float mv_min_step(float m, float xy, float xn, float 
 
 // exact MaxSim re-score of the multivector shortlist, half a warp per (query, candidate row): for each query vector i
 // in order, the NaN-skipping min over the row's vectors j of 1 - xy / |q_i| / |v_j| (xy in lance's lane order: the
-// same roundings as dist_matrix_kernel mode 2), added onto a sum that starts at 0.0f -- the exact path's bits
+// same roundings as dist_matrix_kernel mode 2), added onto a sum that starts at 0.0f -- the exact path's bits.  V: the
+// stored vectors as kept (T float, or __half converted in registers)
+template <class T>
 __global__ void mv_rescore_kernel(const float *__restrict__ Q, const uint32_t *__restrict__ q_off, uint32_t qa,
-                                  const float *__restrict__ xnorm, const float *__restrict__ V,
+                                  const float *__restrict__ xnorm, const T *__restrict__ V,
                                   const float *__restrict__ ysqrt, const uint64_t *__restrict__ offsets,
                                   const uint64_t *__restrict__ row_ids, uint32_t d, uint32_t B,
                                   const uint32_t *__restrict__ cand, const uint32_t *__restrict__ count, uint32_t cap,
@@ -385,21 +387,24 @@ __global__ void mv_rescore_kernel(const float *__restrict__ Q, const uint32_t *_
 // i0 + 32 h + 16 u + l (u = 0, 1) in lane l, updated in order of j by the same mv_min_step as mv_rescore_kernel, and
 // the block's minima are added onto the sum in order of i once the row was streamed.  A query of more than MH_QV
 // vectors streams the row once per block.  `staged` false (d not a multiple of 4, or a vector longer than a ring slot):
-// the half-warps read the mapped alias directly.
+// the half-warps read the mapped alias directly.  fp16 vectors (T = __half) are staged as they are, twice as many per
+// slot, and converted in registers by halfwarp_dot: the bits of their exact f32 upcast.
 constexpr int MH_WARPS = 4;
-constexpr uint32_t MH_QV = 64, MH_SLOT = 1024;      // query vectors per block; floats per ring slot (2 slots per warp)
+constexpr uint32_t MH_QV = 64, MH_SLOT_BYTES = 4096;  // query vectors per block; bytes per ring slot (2 slots per warp)
 
+template <class T>
 __global__ void __launch_bounds__(MH_WARPS * 32) mv_rescore_host_kernel(
     const float *__restrict__ Q, const uint32_t *__restrict__ q_off, uint32_t qa, const float *__restrict__ xnorm,
-    const float *V, const float *__restrict__ ysqrt, const uint64_t *__restrict__ offsets,
+    const T *V, const float *__restrict__ ysqrt, const uint64_t *__restrict__ offsets,
     const uint64_t *__restrict__ row_ids, uint32_t d, uint32_t B, const uint32_t *__restrict__ cand,
     const uint32_t *__restrict__ count, uint32_t cap, bool staged, float *__restrict__ out, uint64_t *__restrict__ ids)
 {
+    constexpr uint32_t SLOT = MH_SLOT_BYTES / sizeof(T), E16 = 16 / sizeof(T);   // elements per slot, per request
     pdl_entry();
-    __shared__ __align__(16) float mh_ring[MH_WARPS][2][MH_SLOT];
+    __shared__ __align__(16) T mh_ring[MH_WARPS][2][SLOT];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, h = lane >> 4, hl = lane & 15, hbase = lane & 16;
     const unsigned hmask = 0xffffu << hbase;
-    const uint32_t vps = staged ? MH_SLOT / d : 1;                 // vectors per chunk
+    const uint32_t vps = staged ? SLOT / d : 1;                    // vectors per chunk
     const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(&mh_ring[warp][0][0]);
     const uint64_t npairs = (uint64_t)B * cap, nwarps = (uint64_t)gridDim.x * MH_WARPS;
     for (uint64_t pair = (uint64_t)blockIdx.x * MH_WARPS + warp; pair < npairs; pair += nwarps) {
@@ -411,15 +416,16 @@ __global__ void __launch_bounds__(MH_WARPS * 32) mv_rescore_host_kernel(
         const uint32_t r = cand[pair];
         const uint64_t j0 = offsets[r], n = offsets[r + 1] - j0;
         const uint32_t nch = staged ? (uint32_t)((n + vps - 1) / vps) : 0;
-        const float *row = V + j0 * d;
+        const T *row = V + j0 * d;
         // chunk c of the row into ring slot c & 1; every lane commits one group per chunk, empty or not
         auto issue = [&](uint32_t c) {
             if (c < nch) {
                 const uint32_t len = (uint32_t)(min((uint64_t)vps, n - (uint64_t)c * vps) * d);
-                const float *src = row + (size_t)c * vps * d;
-                const uint32_t dst = ring_s + (c & 1) * MH_SLOT * 4;
-                for (uint32_t o = (uint32_t)lane * 4; o < len; o += 128)
-                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + o * 4), "l"(src + o) : "memory");
+                const T *src = row + (size_t)c * vps * d;
+                const uint32_t dst = ring_s + (c & 1) * MH_SLOT_BYTES;
+                for (uint32_t o = (uint32_t)lane * E16; o < len; o += 32 * E16)
+                    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + o * (uint32_t)sizeof(T)),
+                                 "l"(src + o) : "memory");
             }
             asm volatile("cp.async.commit_group;" ::: "memory");
         };
@@ -428,7 +434,7 @@ __global__ void __launch_bounds__(MH_WARPS * 32) mv_rescore_host_kernel(
         for (uint32_t i0 = qs; i0 < qe; i0 += MH_QV) {
             float m[2] = {CUDART_NAN_F, CUDART_NAN_F};
             // the minima of this half-warp's vectors i0 + 32 h + 16 u + t over stored vectors [j, j + nv) at y
-            auto score = [&](const float *y, uint64_t j, uint32_t nv) {
+            auto score = [&](const T *y, uint64_t j, uint32_t nv) {
                 for (uint32_t v = 0; v < nv; v++) {
                     const float ys = ysqrt[j0 + j + v];
 #pragma unroll
@@ -728,16 +734,19 @@ void launch_refine_host(const float *Q, const float *V, uint32_t stride, const u
     LGPU_CUDA(cudaGetLastError());
 }
 
-void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+// staged: every vector a whole number of 16-byte requests (d a multiple of 4 floats or 8 halves) that fits a slot
+template <class T>
+void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const T *V,
                             const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
                             const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
                             int num_sms, cudaStream_t st)
 {
     if (B == 0 || cap == 0) return;
-    const bool staged = d % 4 == 0 && d <= MH_SLOT && ((uintptr_t)V & 15) == 0;
+    const bool staged = ((size_t)d * sizeof(T)) % 16 == 0 && (size_t)d * sizeof(T) <= MH_SLOT_BYTES &&
+                        ((uintptr_t)V & 15) == 0;
     const uint64_t npairs = (uint64_t)B * cap;
     const unsigned grid = (unsigned)std::min<uint64_t>((npairs + MH_WARPS - 1) / MH_WARPS, (uint64_t)std::max(num_sms, 1) * 16);
-    launch_k(mv_rescore_host_kernel, dim3(grid), dim3(MH_WARPS * 32), 0, st, Q, q_off, qa, xnorm, V, ysqrt, offsets,
+    launch_k(mv_rescore_host_kernel<T>, dim3(grid), dim3(MH_WARPS * 32), 0, st, Q, q_off, qa, xnorm, V, ysqrt, offsets,
              row_ids, d, B, cand, count, cap, staged, out, ids); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
@@ -753,16 +762,29 @@ LGPU_ROW_TYPE(float)
 LGPU_ROW_TYPE(__half)
 #undef LGPU_ROW_TYPE
 
-void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+template <class T>
+void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const T *V,
                        const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
                        const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
                        cudaStream_t st)
 {
     if (B == 0 || cap == 0) return;
     const uint64_t threads = (uint64_t)B * cap * 16;
-    launch_k(mv_rescore_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, q_off, qa, xnorm, V, ysqrt,
-             offsets, row_ids, d, B, cand, count, cap, out, ids); LGPU_COUNT_LAUNCH();
+    launch_k(mv_rescore_kernel<T>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, st, Q, q_off, qa, xnorm, V,
+             ysqrt, offsets, row_ids, d, B, cand, count, cap, out, ids); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
+
+#define LGPU_MV_ROW_TYPE(T)                                                                                              \
+    template void launch_mv_rescore<T>(const float *, const uint32_t *, uint32_t, const float *, const T *,             \
+                                       const float *, const uint64_t *, const uint64_t *, uint32_t, uint32_t,           \
+                                       const uint32_t *, const uint32_t *, uint32_t, float *, uint64_t *, cudaStream_t); \
+    template void launch_mv_rescore_host<T>(const float *, const uint32_t *, uint32_t, const float *, const T *,        \
+                                            const float *, const uint64_t *, const uint64_t *, uint32_t, uint32_t,      \
+                                            const uint32_t *, const uint32_t *, uint32_t, float *, uint64_t *, int,     \
+                                            cudaStream_t);
+LGPU_MV_ROW_TYPE(float)
+LGPU_MV_ROW_TYPE(__half)
+#undef LGPU_MV_ROW_TYPE
 
 }  // namespace lgpu

@@ -224,12 +224,24 @@ struct F16MaxSim {
     __device__ static __forceinline__ int qterm(const MaxSimOut &, uint32_t) { return 0; }
     __device__ static __forceinline__ float score(float, float acc, int) { return acc; }
 };
+// F16RowMaxSim: the F16MaxSim score of an fp16 multivector handle, whose stored vectors are their own operand (read by
+// TMA as they are, not normalised): acc = fp16(q / |q|) . v.  The kernel loads |v| (the handle's ysqrt) as the
+// per-column term and takes its f32 reciprocal once per column, so the similarity is acc * fl(1 / |v|), one f32
+// multiplication per score before the running max of the document (multivec.cu mv_band_f16).
+struct F16RowMaxSim {
+    static constexpr bool BIN = false, MAXSIM = true;
+    static constexpr int K_BOX = GK;
+    using Acc = float; using Row = float; using Row2 = float2; using Filter = MaxSimOut;
+    __device__ static __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k16_f16(d, a, b, acc); }
+    __device__ static __forceinline__ int qterm(const MaxSimOut &, uint32_t) { return 0; }
+    __device__ static __forceinline__ float score(float rv, float acc, int) { return __fmul_rn(acc, rv); }
+};
 
 // LIST: the filtering epilogue for DENSE hit rates (coarse step at many lists), see the epilogue; a separate
 // instantiation so that the dense / sparse-filter kernel of the flat path and of the small coarse problems carries
 // none of its code.  ROWF: the filtering epilogues admit only columns that pass the filter's row filter (flt.allow);
 // also a separate instantiation, so the kernels of unfiltered calls are the ones they were without it.
-// Pol: Bf16Dist, F16Dist, B1Hamming or F16MaxSim (above).
+// Pol: Bf16Dist, F16Dist, B1Hamming, F16MaxSim or F16RowMaxSim (above).
 template <bool LIST, class Pol, bool ROWF = false>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_x,
@@ -289,18 +301,25 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         // this thread's rows r0, r0 + 8 and columns c0 + 8 j + {0, 1}
         const uint32_t r0 = m_tile * GM + wg * 64 + (uint32_t)(warp & 3) * 16 + (uint32_t)(lane >> 2);
         const uint64_t c0 = n_tile * GN + 2 * (uint32_t)(lane & 3);
-        // |x|^2 of the thread's 32 columns, requested before the MMAs so that the loads land under them; past N: 0
+        // |x|^2 of the thread's 32 columns, requested before the MMAs so that the loads land under them; past N: 0.
+        // F16RowMaxSim's term (|v| from a chunk's first vector on) may start at an odd column: scalar loads, and the
+        // reciprocals 1 / |v| its score multiplies by
+        constexpr bool odd = std::is_same<Pol, F16RowMaxSim>::value;
         typename Pol::Row xn[32];
 #pragma unroll
         for (int j = 0; j < 16; j++) {
             const uint64_t x = c0 + 8 * j;
-            if (x + 1 < N) {
+            if (!odd && x + 1 < N) {
                 const typename Pol::Row2 v = __ldg(reinterpret_cast<const typename Pol::Row2 *>(xnorm2 + x));
                 xn[2 * j] = v.x; xn[2 * j + 1] = v.y;
             } else {
                 xn[2 * j] = x < N ? __ldg(xnorm2 + x) : 0;
-                xn[2 * j + 1] = 0;
+                xn[2 * j + 1] = odd && x + 1 < N ? __ldg(xnorm2 + x + 1) : 0;
             }
+        }
+        if constexpr (odd) {
+#pragma unroll
+            for (int i = 0; i < 32; i++) xn[i] = __frcp_rn(xn[i]);
         }
         uint32_t prev = 0;
         for (uint32_t kb = 0; kb < num_kb; kb++) {
@@ -323,8 +342,8 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
         if constexpr (Pol::MAXSIM) {
             // MaxSim epilogue: the thread's 32 columns of row q ascend (c0 + 8 j + e), so the columns of one document
-            // form one run; the run's largest similarity goes to M[q][doc - row_base] by an ordered-key atomicMax
-            // (M zeroed by the caller: key 0 = no column seen)
+            // form one run; the run's largest similarity (Pol::score of each column) goes to M[q][doc - row_base] by
+            // an ordered-key atomicMax (M zeroed by the caller: key 0 = no column seen)
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 const uint32_t q = r0 + 8 * h;
@@ -338,7 +357,7 @@ gemm_dist_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                         const uint64_t x = c0 + 8 * j + e;
                         if (x < N) {
                             const uint32_t doc = __ldg(flt.col_row + x);
-                            const float v = acc[4 * j + 2 * h + e];
+                            const float v = Pol::score(xn[2 * j + e], acc[4 * j + 2 * h + e], 0);
                             if (doc != cur) {
                                 if (cur != 0xffffffffu) atomicMax(flt.M + (size_t)q * flt.ldM + (cur - flt.row_base), f32_key(best));
                                 cur = doc; best = v;
@@ -778,7 +797,7 @@ void launch_ham_gemm(const void *Qp, const void *Xp, const uint32_t *xpop, const
 }
 
 void launch_maxsim_gemm(const void *Qh, const void *Xh, uint32_t B, uint64_t N, uint32_t d, const MaxSimOut &out,
-                        int num_sms, cudaStream_t st)
+                        bool rows, int num_sms, cudaStream_t st)
 {
     if (B == 0 || N == 0) return;
     LGPU_REQUIRE(gemm_shape_supported(d), "tensor-core path needs a dimension that is a multiple of 8");
@@ -786,9 +805,9 @@ void launch_maxsim_gemm(const void *Qh, const void *Xh, uint32_t B, uint64_t N, 
     CUtensorMap mx = make_map(Xh, N, d, GN, false, true);
     const uint64_t tiles = (uint64_t)((B + GM - 1) / GM) * ((N + GN - 1) / GN);
     const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)num_sms);
-    auto kern = gemm_dist_kernel<false, F16MaxSim>;
+    auto kern = rows ? gemm_dist_kernel<false, F16RowMaxSim> : gemm_dist_kernel<false, F16MaxSim>;
     LGPU_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM_BYTES));
-    launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, out.xdummy, nullptr, (uint64_t)0, B, N,
+    launch_k(kern, dim3(grid), dim3(G_THREADS), G_SMEM_BYTES, st, mq, mx, out.vnorm, nullptr, (uint64_t)0, B, N,
              (uint32_t)((d + GK - 1) / GK), out); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }

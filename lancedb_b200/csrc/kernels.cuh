@@ -457,29 +457,34 @@ void launch_ham_flag_list(const uint32_t *flags, uint32_t B, uint32_t chunk, uin
 // smallest over all rows)
 void launch_ham_threshold(const float *dist, const uint32_t *cnt, uint32_t B, uint32_t k, float *thr, cudaStream_t st);
 
-// ---------------- multivector (MaxSim) columns, tensor-core score (gemm.cu F16MaxSim) -----------
-// M[q][col_row[x] - row_base] = f32_key(max over the columns x of that document of fp16(Q[q]) . fp16(X[x])) by
-// atomicMax (M zeroed by the caller); Q [B][d], X [N][d] fp16 of the normalised vectors, d a multiple of 8.
+// ---------------- multivector (MaxSim) columns, tensor-core score (gemm.cu F16MaxSim, F16RowMaxSim) -----------
+// M[q][col_row[x] - row_base] = f32_key(max over the columns x of that document of the similarity) by atomicMax (M
+// zeroed by the caller); Q [B][d] fp16 of the normalised query vectors, d a multiple of 8.  rows false (F16MaxSim):
+// X [N][d] fp16 of the normalised stored vectors, similarity fp16(Q[q]) . X[x].  rows true (F16RowMaxSim): X [N][d]
+// the stored fp16 vectors themselves, similarity (fp16(Q[q]) . X[x]) / vnorm[x].
 struct MaxSimOut : GemmFilter {   // (GemmFilter's fields stay unset)
     const uint32_t *col_row;      // [N] document (row) of each column
     uint32_t *M;                  // [B][ldM]
     uint64_t ldM;
     uint32_t row_base;
-    const float *xdummy;          // any [N] f32 array (the kernel's per-column term is unused by this policy)
+    const float *vnorm;           // [N] |v| of each column (the per-column term; F16MaxSim does not use it)
 };
 void launch_maxsim_gemm(const void *Qh, const void *Xh, uint32_t B, uint64_t N, uint32_t d, const MaxSimOut &out,
-                        int num_sms, cudaStream_t st);
-// out[n][d] = fp16(x / |x|) (|x| = sqrt(lance dot)); bad[n] = 1 (and the row zeroed) when |x| is 0 or not finite or
-// a component is not finite
-void launch_mv_normalize_f16(const float *X, uint64_t n, uint32_t d, void *out, uint32_t *bad, cudaStream_t st);
-// the per-query error band of the approximate MaxSim distance: |approx - exact| <= mv_band(nq, d) (multivec.cu)
+                        bool rows, int num_sms, cudaStream_t st);
+// out[n][d] = fp16(x / |x|) (|x| = sqrt(lance dot)) unless out is null; bad[n] = 1 (and the row zeroed) when |x| is 0
+// or not finite or a component is not finite.  X: f32, or fp16 rows (the same arithmetic on their exact f32 upcast)
+template <class T>
+void launch_mv_normalize_f16(const T *X, uint64_t n, uint32_t d, void *out, uint32_t *bad, cudaStream_t st);
+// the per-query error band of the approximate MaxSim distance: |approx - exact| <= mv_band(nq, d), or mv_band_f16(nq, d)
+// for an fp16 handle's F16RowMaxSim score (multivec.cu)
 float mv_band_host(uint32_t nq, uint32_t d);
+float mv_band_f16_host(uint32_t nq, uint32_t d);
 // A[b - qa][r] = sum over query b's vectors i of (1 - key_f32(M[i - i_base][r])), NaN when some M entry is 0 (empty row)
 void launch_mv_approx_sum(const uint32_t *M, uint64_t ldM, const uint32_t *q_off, uint32_t qa, uint32_t qb,
                           uint32_t i_base, uint64_t N, float *A, uint64_t ldA, int num_sms, cudaStream_t st);
-// thr[b] = dist[b][k-1] + 2 E_b when cnt[b] >= k, else +inf; E_b = mv_band(nq_b, d)
+// thr[b] = dist[b][k-1] + 2 E_b when cnt[b] >= k, else +inf; E_b = mv_band(nq_b, d), or mv_band_f16 when f16
 void launch_mv_threshold(const float *dist, const uint32_t *cnt, const uint32_t *q_off, uint32_t qa, uint32_t B,
-                         uint32_t k, uint32_t d, float *thr, cudaStream_t st);
+                         uint32_t k, uint32_t d, bool f16, float *thr, cudaStream_t st);
 // every row r with A[b][r] <= thr[b] is appended to cand[b][.] (count[b] zeroed by the caller, may exceed cap)
 void launch_mv_admit(const float *A, uint64_t ldA, uint32_t B, uint64_t N, const float *thr, uint32_t cap,
                      uint32_t *count, uint32_t *cand, cudaStream_t st);
@@ -487,19 +492,23 @@ void launch_mv_admit(const float *A, uint64_t ldA, uint32_t B, uint64_t N, const
 void launch_mv_flags(const uint32_t *count, uint32_t cap, const uint32_t *qbad, const uint32_t *q_off, uint32_t qa,
                      uint32_t B, uint32_t *flags, uint32_t *vflags, uint32_t *gate, cudaStream_t st);
 // exact re-score (dist.cu): for slot s < min(count[b], cap): out[b][s] = MaxSim distance of query b and row cand[b][s]
-// in the oracle's arithmetic, ids[b][s] = its id; other slots NaN / UINT64_MAX
-void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+// in the oracle's arithmetic, ids[b][s] = its id; other slots NaN / UINT64_MAX.  V: the stored vectors, float or
+// __half (converted in registers: the bits of their exact f32 upcast)
+template <class T>
+void launch_mv_rescore(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const T *V,
                        const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
                        const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
                        cudaStream_t st);
 // the same values when V is the mapped device alias of pinned host memory: each candidate row is read over PCIe in
 // 16-byte cp.async requests staged in shared memory (dist.cu mv_rescore_host_kernel)
-void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const float *V,
+template <class T>
+void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, const float *xnorm, const T *V,
                             const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
                             const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
                             int num_sms, cudaStream_t st);
-// dst[0, n) = src[0, n) floats when *gate (device) != 0; nothing otherwise (multivec.cu)
-void launch_mv_copy_gated(const float *src, float *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st);
+// dst[0, n) = src[0, n) elements (float or __half) when *gate (device) != 0; nothing otherwise (multivec.cu)
+template <class T>
+void launch_mv_copy_gated(const T *src, T *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st);
 
 // ---------------- multivector (MaxSim) columns, exact path (multivec.cu) ----------------------
 // M[i][r] = min over row r0 + r's stored vectors j of P[i][j - offsets[r0]] (NaN skipped; NaN if none), for the nqv

@@ -5,10 +5,12 @@
 // row, or every pair NaN) makes the row's distance NaN, and select drops NaN distances.
 //
 // The tensor-core path (api.cu multivec_search_device) scores fp16 copies of the normalised vectors with the F16MaxSim
-// policy of gemm_dist_kernel, whose epilogue keeps the largest approximate similarity per (query vector, document);
-// mv_approx_sum_kernel turns those into approximate distances, a shortlist admits every row within 2 E of the k-th
-// approximate distance (mv_band below), dist.cu's mv_rescore_kernel re-scores the admitted rows exactly, and a query
-// whose list overflowed (or that holds a zero / non-finite vector) is redone by the exact path.
+// policy of gemm_dist_kernel, whose epilogue keeps the largest approximate similarity per (query vector, document)
+// (an fp16 handle: the F16RowMaxSim policy, fp16 normalised queries against the stored fp16 vectors, each similarity
+// scaled by 1 / |v|); mv_approx_sum_kernel turns those into approximate distances, a shortlist admits every row within
+// 2 E of the k-th approximate distance (mv_band below, mv_band_f16 for an fp16 handle), dist.cu's mv_rescore_kernel
+// re-scores the admitted rows exactly, and a query whose list overflowed (or that holds a zero / non-finite vector)
+// is redone by the exact path.
 //
 // The exact path runs in three steps per (block of query vectors, chunk of whole rows) (api.cu multivec_search_device):
 //   dist_matrix_kernel   P[i][j]  = cosd(q_i, v_j) for the chunk's stored vectors j
@@ -44,12 +46,38 @@ __host__ __device__ __forceinline__ float mv_band(uint32_t nq, uint32_t d)
     return ((float)nq * e + 4.04f * (float)nq * (float)nq * u) * (1.0f + 0x1p-8f);
 }
 
+// The band of an fp16 handle's approximate distance (the F16RowMaxSim score, gemm.cu): the stored fp16 vector v is the
+// operand itself and the similarity is s~ = fl(acc * fl(1 / |v|~)), acc the wgmma sum of h(a) . v, |v|~ = ysqrt
+// (lance's f32 norm, |v| / |v|~ <= 1 + (d + 4) u).  Per query vector and stored vector, against a.v / |v|~:
+//   - the query's fp16 rounding alone: |h(a).v - a.v| / |v|~ <= |h(a) - a| |v| / |v|~
+//     <= (2^-11 (1 + (d + 8) u) + 2^-25 sqrt(d)) (1 + (d + 4) u) < 1.01 * 2^-11 + sqrt(d) u  (2^-25 per subnormal
+//     component of h(a)); the stored side is exact, whatever its magnitude: every product of two fp16 values is exact
+//     in f32 (11 + 11 significant bits, products between 2^-48 and 2^32), subnormal fp16 and +-65504 included;
+//   - wgmma's f32 accumulation: <= 4 d u sum |h(a)_i v_i| / |v|~ <= 4 d u |h(a)| |v| / |v|~ <= 4.1 d u, as above;
+//   - the scaling: the reciprocal and the product round twice, (1 + u)^2 |acc| / |v|~ <= 2.02 u + |acc| / |v|~, and
+//     a.v / |v|~ against the lance formula (the dot's lane sums, the query's norm and normalisation, the divisions,
+//     1 - s~) stays within the (3 d + 30) u + 2 u above;
+// so e = 1.01 * 2^-11 + (8 d + sqrt(d) + 42) u: mv_band's e without the stored-side 2^-11, plus 2 u for the scaling.
+// The sums over i and the f32 arithmetic of E itself are carried as in mv_band.
+__host__ __device__ __forceinline__ float mv_band_f16(uint32_t nq, uint32_t d)
+{
+    const float u = 0x1p-24f;
+    const float e = 1.01f * 0x1p-11f + (8.0f * (float)d + sqrtf((float)d) + 42.0f) * u;
+    return ((float)nq * e + 4.04f * (float)nq * (float)nq * u) * (1.0f + 0x1p-8f);
+}
+
 namespace {
 
 constexpr int MV_THREADS = 256;
 
-// fp16(x / |x|), |x| = sqrt of lance's dot (the normalisation of dist.cu normalize_kernel); half a warp per row
-__global__ void mv_normalize_f16_kernel(const float *__restrict__ X, uint64_t n, uint32_t d, __half *__restrict__ out,
+__device__ __forceinline__ float mv_ld(float v) { return v; }
+__device__ __forceinline__ float mv_ld(__half v) { return __half2float(v); }
+
+// fp16(x / |x|), |x| = sqrt of lance's dot (the normalisation of dist.cu normalize_kernel); half a warp per row.  fp16
+// rows (T = __half) are read as their exact f32 upcast: the same |x| and bad flag as f32 rows of those values.  out
+// null: only the bad flags (an fp16 handle's open, whose rows are their own operand)
+template <class T>
+__global__ void mv_normalize_f16_kernel(const T *__restrict__ X, uint64_t n, uint32_t d, __half *__restrict__ out,
                                         uint32_t *__restrict__ bad)
 {
     pdl_entry();
@@ -57,19 +85,23 @@ __global__ void mv_normalize_f16_kernel(const float *__restrict__ X, uint64_t n,
     const int lane = threadIdx.x & 31, hl = lane & 15, hbase = lane & 16;
     const unsigned hmask = 0xffffu << hbase;
     if (row >= n) return;
-    const float *x = X + row * d;
+    const T *x = X + row * d;
     const uint32_t d16 = d & ~15u;
     float a = 0.f;
     bool fin = true;
-    for (uint32_t k = hl; k < d16; k += 16) { a = __fadd_rn(a, __fmul_rn(x[k], x[k])); fin = fin && isfinite(x[k]); }
+    for (uint32_t k = hl; k < d16; k += 16) {
+        const float v = mv_ld(x[k]);
+        a = __fadd_rn(a, __fmul_rn(v, v)); fin = fin && isfinite(v);
+    }
     float t = 0.f;
 #pragma unroll
     for (int l = 0; l < 16; l++) t = __fadd_rn(t, __shfl_sync(hmask, a, hbase + l));
     float s = 0.f;
-    for (uint32_t i = d16; i < d; i++) { s = __fadd_rn(s, __fmul_rn(x[i], x[i])); fin = fin && isfinite(x[i]); }
+    for (uint32_t i = d16; i < d; i++) { const float v = mv_ld(x[i]); s = __fadd_rn(s, __fmul_rn(v, v)); fin = fin && isfinite(v); }
     const float nrm = sqrtf(__fadd_rn(s, t));
     const bool ok = __all_sync(hmask, fin) && nrm > 0.f && isfinite(nrm);
-    for (uint32_t k = hl; k < d; k += 16) out[row * d + k] = __float2half_rn(ok ? __fdiv_rn(x[k], nrm) : 0.f);
+    if (out)
+        for (uint32_t k = hl; k < d; k += 16) out[row * d + k] = __float2half_rn(ok ? __fdiv_rn(mv_ld(x[k]), nrm) : 0.f);
     if (hl == 0) bad[row] = ok ? 0u : 1u;
 }
 
@@ -96,12 +128,13 @@ __global__ void __launch_bounds__(MV_THREADS) mv_approx_sum_kernel(const uint32_
 
 __global__ void mv_threshold_kernel(const float *__restrict__ dist, const uint32_t *__restrict__ cnt,
                                     const uint32_t *__restrict__ q_off, uint32_t qa, uint32_t B, uint32_t k, uint32_t d,
-                                    float *__restrict__ thr)
+                                    bool f16, float *__restrict__ thr)
 {
     pdl_entry();
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const float E = mv_band(q_off[qa + b + 1] - q_off[qa + b], d);
+    const uint32_t nq = q_off[qa + b + 1] - q_off[qa + b];
+    const float E = f16 ? mv_band_f16(nq, d) : mv_band(nq, d);
     thr[b] = cnt[b] >= k ? __fadd_ru(dist[(size_t)b * k + k - 1], __fmul_ru(2.0f, E)) : CUDART_INF_F;   // rounded up
 }
 
@@ -190,19 +223,21 @@ __global__ void __launch_bounds__(MV_THREADS) mv_rowsum_kernel(const float *__re
 }
 
 // dst[0, n) = src[0, n) when *gate != 0, else nothing: the fix-up's chunk copy out of a host handle's mapped rows,
-// which costs one empty launch when no query is flagged.  16-byte requests when both ends allow them.
-__global__ void __launch_bounds__(MV_THREADS) mv_copy_gated_kernel(const float *src, float *__restrict__ dst, uint64_t n,
+// which costs one empty launch when no query is flagged.  16-byte requests (V elements of T) when both ends allow them.
+template <class T>
+__global__ void __launch_bounds__(MV_THREADS) mv_copy_gated_kernel(const T *src, T *__restrict__ dst, uint64_t n,
                                                                    const uint32_t *__restrict__ gate)
 {
+    constexpr uint64_t V = 16 / sizeof(T);
     pdl_entry();
     if (*gate == 0) return;
     const uint64_t t0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, step = (uint64_t)gridDim.x * blockDim.x;
     uint64_t head = 0;
     if ((((uintptr_t)src | (uintptr_t)dst) & 15) == 0) {
-        head = n & ~3ull;
+        head = n & ~(V - 1);
         const uint4 *s4 = reinterpret_cast<const uint4 *>(src);
         uint4 *d4 = reinterpret_cast<uint4 *>(dst);
-        for (uint64_t w = t0; w < head / 4; w += step) d4[w] = s4[w];
+        for (uint64_t w = t0; w < head / V; w += step) d4[w] = s4[w];
     }
     for (uint64_t w = head + t0; w < n; w += step) dst[w] = src[w];
 }
@@ -233,23 +268,33 @@ void launch_mv_rowsum(const float *M, uint64_t ldM, const uint32_t *q_off, uint3
     LGPU_CUDA(cudaGetLastError());
 }
 
-void launch_mv_copy_gated(const float *src, float *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st)
+template <class T>
+void launch_mv_copy_gated(const T *src, T *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st)
 {
+    constexpr uint64_t V = 16 / sizeof(T);
     if (n == 0) return;
-    launch_k(mv_copy_gated_kernel, dim3(grid_for((n + 3) / 4, num_sms)), dim3(MV_THREADS), 0, st, src, dst, n, gate);
+    launch_k(mv_copy_gated_kernel<T>, dim3(grid_for((n + V - 1) / V, num_sms)), dim3(MV_THREADS), 0, st, src, dst, n,
+             gate);
     LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 
 float mv_band_host(uint32_t nq, uint32_t d) { return mv_band(nq, d); }
+float mv_band_f16_host(uint32_t nq, uint32_t d) { return mv_band_f16(nq, d); }
 
-void launch_mv_normalize_f16(const float *X, uint64_t n, uint32_t d, void *out, uint32_t *bad, cudaStream_t st)
+template <class T>
+void launch_mv_normalize_f16(const T *X, uint64_t n, uint32_t d, void *out, uint32_t *bad, cudaStream_t st)
 {
     if (n == 0) return;
-    launch_k(mv_normalize_f16_kernel, dim3((unsigned)((n * 16 + 255) / 256)), dim3(256), 0, st, X, n, d,
+    launch_k(mv_normalize_f16_kernel<T>, dim3((unsigned)((n * 16 + 255) / 256)), dim3(256), 0, st, X, n, d,
              reinterpret_cast<__half *>(out), bad); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
+
+template void launch_mv_copy_gated<float>(const float *, float *, uint64_t, const uint32_t *, int, cudaStream_t);
+template void launch_mv_copy_gated<__half>(const __half *, __half *, uint64_t, const uint32_t *, int, cudaStream_t);
+template void launch_mv_normalize_f16<float>(const float *, uint64_t, uint32_t, void *, uint32_t *, cudaStream_t);
+template void launch_mv_normalize_f16<__half>(const __half *, uint64_t, uint32_t, void *, uint32_t *, cudaStream_t);
 
 void launch_mv_approx_sum(const uint32_t *M, uint64_t ldM, const uint32_t *q_off, uint32_t qa, uint32_t qb,
                           uint32_t i_base, uint64_t N, float *A, uint64_t ldA, int num_sms, cudaStream_t st)
@@ -261,10 +306,10 @@ void launch_mv_approx_sum(const uint32_t *M, uint64_t ldM, const uint32_t *q_off
 }
 
 void launch_mv_threshold(const float *dist, const uint32_t *cnt, const uint32_t *q_off, uint32_t qa, uint32_t B,
-                         uint32_t k, uint32_t d, float *thr, cudaStream_t st)
+                         uint32_t k, uint32_t d, bool f16, float *thr, cudaStream_t st)
 {
     if (B == 0) return;
-    launch_k(mv_threshold_kernel, dim3((B + 127) / 128), dim3(128), 0, st, dist, cnt, q_off, qa, B, k, d, thr);
+    launch_k(mv_threshold_kernel, dim3((B + 127) / 128), dim3(128), 0, st, dist, cnt, q_off, qa, B, k, d, f16, thr);
     LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }

@@ -176,15 +176,17 @@ class Table:
         return _is_multivec_type(self._data.schema.field(column).type)
 
     def _multivec_rows(self, column: str):
-        """(values [T, dim] f32, offsets [N+1] u64) of a multivector column; a null row holds no vectors.  Stored
-        float16 / float64 elements are upcast to f32."""
+        """(values [T, dim], offsets [N+1] u64) of a multivector column; a null row holds no vectors.  float16 elements
+        stay float16 (GpuMultivec keeps them so, with the results of their exact f32 upcast); float64 elements are
+        converted to f32."""
         col = self._data.column(column).combine_chunks()
         lens = col.value_lengths().fill_null(0).to_numpy(zero_copy_only=False).astype(np.int64)
         inner = col.flatten()                               # skips the values behind null rows
         if inner.null_count:
             raise ValueError(f"multivector column {column!r} holds a null vector inside a row")
         dim = col.type.value_type.list_size
-        vals = np.asarray(inner.flatten().to_numpy(zero_copy_only=False), np.float32).reshape(-1, dim)
+        dt = np.float16 if pa.types.is_float16(col.type.value_type.value_type) else np.float32
+        vals = np.asarray(inner.flatten().to_numpy(zero_copy_only=False), dt).reshape(-1, dim)
         return vals, _native.multivec_offsets(lens)
 
     def _binary_vectors(self, column: str) -> np.ndarray:
