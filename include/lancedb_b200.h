@@ -473,6 +473,24 @@ int  lgpu_binary_search_device(lgpu_binary *bx, const uint8_t *d_queries, uint32
                                uint64_t *d_out_ids, float *d_out_dist, uint32_t *d_out_count, void *cuda_stream);
 /* Append n rows (HOST [n][nbytes]); everything else as lgpu_flat_append. */
 int  lgpu_binary_append(lgpu_binary *bx, const uint8_t *rows, uint64_t n, const uint64_t *row_ids);
+/* *bytes = the device memory the handle holds for its rows and their per-row data (the rows zero-padded to nbytes_pad
+ * = nbytes rounded up to 32, their popcounts, the threshold sample of a handle above 65536 rows, row ids, the live
+ * bitmap), capacity kept for appends included; the per-call search workspaces (each within LGPU_WS_BYTES) are not
+ * counted.  A handle whose rows are in host memory (lgpu_binary_host_bytes) holds no rows or popcounts here. */
+int  lgpu_binary_device_bytes(const lgpu_binary *bx, uint64_t *bytes);
+/* Where a binary handle keeps its rows.  lgpu_binary_open packs them into HBM, as above, when the rows and their
+ * popcounts, nrows x (nbytes_pad + 4) bytes, are at most LGPU_BINARY_HBM_BYTES (read at every open; unset = no cap,
+ * 0 = never in HBM) and the device's free memory covers them plus the workspace budget (LGPU_WS_BYTES, default 8 GiB).
+ * Otherwise the handle packs the rows into pinned host memory that it owns, [nrows][nbytes_pad] zero-padded (freed by
+ * lgpu_binary_close), and keeps the row ids, the live bitmap and the threshold sample in HBM; the open then needs no
+ * HBM that grows with nrows beyond those.  Every search of such a handle (host, _filtered, _device, and as the tail of
+ * lgpu_ivf_binary_search_unindexed[_device]) streams the rows through two staging buffers of its workspace, within
+ * LGPU_WS_BYTES, as lgpu_flat_host_bytes describes.  Results are identical to an HBM handle's on the same rows -- same
+ * ids, counts and distance bits -- for every k, distance_range, prefilter, deleted rows and append.  A handle keeps its
+ * placement for life; lgpu_binary_append grows the pinned rows geometrically.  A pinned allocation that fails is
+ * LGPU_OOM.  *bytes = the pinned host memory the handle holds (nrows x nbytes_pad at open, capacity kept for appends
+ * included; 0 for an HBM handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output may be NULL. */
+int  lgpu_binary_host_bytes(const lgpu_binary *bx, uint64_t *bytes, int *placement);
 
 /* ---- deleted rows (the reference's Table::delete; Lance keeps them per dataset in deletion files).  Delete the rows
  * whose ids are among row_ids (HOST [n]); *n_deleted (may be NULL) = how many of those ids were live and are now

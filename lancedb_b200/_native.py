@@ -52,6 +52,7 @@ EXPORTS = [
     "lgpu_index_host_bytes", "lgpu_debug_refine_host", "lgpu_flat_host_bytes",
     "lgpu_multivec_device_bytes", "lgpu_multivec_host_bytes",
     "lgpu_multivec_open_f16", "lgpu_debug_maxsim_gemm_f16",
+    "lgpu_binary_device_bytes", "lgpu_binary_host_bytes",
 ]
 VECTORS_NONE, VECTORS_HBM, VECTORS_HOST = 0, 1, 2     # lgpu_vectors_placement
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
@@ -218,6 +219,8 @@ def load():
     lib.lgpu_multivec_search_device.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, vp]
     lib.lgpu_multivec_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.lgpu_multivec_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+    lib.lgpu_binary_device_bytes.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.lgpu_binary_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
     lib.lgpu_debug_maxsim_gemm.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_debug_maxsim_gemm_f16.argtypes = [vp, u32, vp, vp, C.c_uint64, u32, i32, vp]
     lib.lgpu_ivf_sq_open.argtypes = [C.POINTER(SqDesc), C.POINTER(vp)]
@@ -632,8 +635,9 @@ class GpuFlat(_RowsHandle):
 
 
 class GpuBinary(_RowsHandle):
-    """A packed binary vector column (fixed_size_list<uint8, nbytes>) pinned in HBM (lgpu_binary), searched by
-    Hamming distance."""
+    """A packed binary vector column (fixed_size_list<uint8, nbytes>) searched by Hamming distance (lgpu_binary).  The
+    packed rows are kept in HBM when they fit there (LGPU_BINARY_HBM_BYTES), else in pinned host memory and streamed
+    through the GPU once per search, with the same results (`rows_on_host`)."""
     _close = "lgpu_binary_close"
     _delete = "lgpu_binary_delete"
     _queries = _binary_queries
@@ -648,6 +652,28 @@ class GpuBinary(_RowsHandle):
         check(load().lgpu_binary_open(_ptr(v), self.nrows, self.nbytes, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
+
+    @property
+    def device_bytes(self) -> int:
+        """The HBM the handle holds for its rows and per-row data (lgpu_binary_device_bytes)."""
+        n = C.c_uint64(0)
+        check(load().lgpu_binary_device_bytes(self._h, C.byref(n)))
+        return n.value
+
+    def _host(self):
+        b, where = C.c_uint64(0), C.c_int(0)
+        check(load().lgpu_binary_host_bytes(self._h, C.byref(b), C.byref(where)))
+        return b.value, where.value
+
+    def host_bytes(self) -> int:
+        """The pinned host memory the handle holds: its packed rows when they did not fit in HBM at open, else 0
+        (lgpu_binary_host_bytes)."""
+        return self._host()[0]
+
+    @property
+    def rows_on_host(self) -> bool:
+        """True when the rows are kept in pinned host memory and every search streams them through the GPU."""
+        return self._host()[1] == VECTORS_HOST
 
     def search(self, queries, k=10, lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         """Host-buffer search of queries [B, nbytes] (or one [nbytes] query) whose components are integers in

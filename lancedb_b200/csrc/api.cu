@@ -153,7 +153,7 @@ struct Deadline {
 
 struct Workspace;
 
-// Rows streamed from pinned host memory through HBM (the search of a host flat or multivector handle).  Between open
+// Rows streamed from pinned host memory through HBM (the search of a host flat, binary or multivector handle).  Between open
 // and close, chunk s of `steps` is copied into buf[s & 1] by cudaMemcpyAsync on the workspace's side stream (`front`,
 // forked from the call's stream and joined back to it), chunk s + 1 while chunk s is used on the call's stream:
 // take(s) hands over chunk s once the copy of chunk s + 1 is issued, release(s) marks every use of it enqueued.
@@ -235,6 +235,7 @@ struct Workspace {
     // a flat handle whose rows are in pinned host memory (flat_search_streamed): the staged chunk's tensor-core
     // operand, |x|^2 and |x|, and the running top-k, [2 buffers][2 lists][P][k] / [..][P]
     DevBuf chunk_xb, chunk_n2, chunk_ysqrt, run_ids, run_dist, run_cnt;
+    DevBuf chunk_pop;                   // ... of a binary handle (binary_search_streamed): popc of each staged row
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -552,6 +553,11 @@ struct lgpu_binary {
     DevBuf sample, sample_pop;             // every (nrows / nsample)-th row: the threshold sample of the list path
     uint64_t nsample = 0;                  // 0: no sample (nrows <= HAM_SAMPLE)
     DevBuf sample_ids;                     // the sample rows' ids (a row filter tests them in the sample's select)
+    // rows that did not fit in HBM at open (lgpu_binary_open): `rows_host` holds them packed as `vectors` would,
+    // [nrows][nbytes_pad] zero-padded, and `vectors` and `pop` stay empty; searches stream the rows through HBM
+    // (binary_search_streamed).  The threshold sample stays in HBM.
+    bool on_host = false;
+    PinnedBuf rows_host;
     bool has_ids = false;
     RowLive live;
     WorkspacePool pool;
@@ -1792,85 +1798,136 @@ static void flat_search_rows(lgpu_flat *fl, const T *X, Workspace *ws, cudaStrea
 // PCIe rate and a chunk's fixed scoring cost is small, small enough that the unoverlapped first copy is short
 constexpr size_t FLAT_STAGE_BYTES = (size_t)128 << 20;
 
-// A host handle (lgpu_flat::on_host): its rows cross PCIe in chunks of C rows, copied into the workspace's two staging
-// buffers on its side stream (`front`, forked from the call's stream and joined back to it), chunk i + 1 while chunk i
-// is scored on the call's stream by the route an HBM handle of that chunk's rows takes (flat_score).  Each chunk's
-// exact top-k is merged into a running top-k per query by (distance, id).  Chunks are the outer loop: a pass over the
-// column serves P queries, all B unless the budget cannot hold the running top-k of that many, in scoring groups of
-// bs queries whose scores fit.  The staging buffers, the chunk's per-row terms and the running lists all count against
-// the workspace budget.  timeout_ms is checked between chunks.
+// A host handle (lgpu_flat::on_host, lgpu_binary::on_host): its rows cross PCIe in chunks of C rows, copied into the
+// workspace's two staging buffers on its side stream (Workspace::stage), chunk i + 1 while chunk i is scored on the
+// call's stream by the route an HBM handle of that chunk's rows takes.  Each chunk's exact top-k is merged into a
+// running top-k per query by (distance, id).  Chunks are the outer loop: a pass over the column serves P queries, all B
+// unless the budget cannot hold the running top-k of that many, in scoring groups of bs queries whose scores fit.  The
+// staging buffers, the chunk's per-row terms and the running lists all count against the workspace budget.  timeout_ms
+// is checked between chunks.
+struct StreamShape {
+    uint64_t C, nchunks;                // rows per chunk, chunks of the column
+    uint32_t P, bs;                     // queries per pass, per scoring group
+};
+// row_b: workspace bytes per row of a chunk (its two staging copies and its per-row terms); row_bytes: the bytes of one
+// stored row (a chunk stages at most FLAT_STAGE_BYTES of them).  A scoring group holds each query's [ldc] f32 scores.
+static StreamShape stream_shape(uint64_t N, size_t row_b, size_t row_bytes, uint32_t B, uint32_t k)
+{
+    const size_t budget = workspace_budget();
+    StreamShape s;
+    s.C = std::max<uint64_t>(1, std::min<uint64_t>(std::max<uint64_t>(N, 1),
+                                                   std::min(budget / 2 / row_b, FLAT_STAGE_BYTES / row_bytes)));
+    const uint64_t ldc = (s.C + 3) & ~3ull;
+    s.nchunks = N ? (N + s.C - 1) / s.C : 1;
+    const size_t rest = budget > s.C * row_b ? budget - s.C * row_b : 0;
+    // per query: the running top-k (two buffers of two lists of k ids and distances, and their counts), and the scores
+    // of a chunk
+    const size_t run_q = (size_t)k * 48 + 16, score_q = ldc * 4 + large_k_query_bytes(k);
+    s.P = (uint32_t)std::max<size_t>(1, std::min<size_t>(B, rest / 2 / run_q));
+    const size_t left = rest > (size_t)s.P * run_q ? rest - (size_t)s.P * run_q : 0;
+    s.bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(s.P, left / score_q));
+    return s;
+}
+
+// The running top-k of pb queries over the chunks of a streamed column, in the workspace's run lists: list l of buffer
+// r holds [pb][k] entries and [pb] counts.  Chunk 0's top-k goes to list 0 of buffer 0, chunk c > 0's to list 1 of
+// buffer (c - 1) & 1, and merge(c) folds it with list 0 of that buffer into list 0 of the other, or into `out` after
+// the last chunk.  A column of one chunk is scored straight into `out`.  only / gate (the fix-up of flagged queries):
+// the merges touch the flagged queries alone, and return at once when none is.
+struct RunningTopk {
+    Workspace *ws;
+    uint64_t nchunks;
+    uint32_t pb, k;
+    TopkOut out;
+    const uint32_t *only = nullptr, *gate = nullptr;
+    // room for passes of P queries
+    static void reserve(Workspace *ws, uint64_t nchunks, uint32_t P, uint32_t k)
+    {
+        if (nchunks < 2) return;
+        ws->run_ids.ensure((size_t)4 * P * k * 8); ws->run_dist.ensure((size_t)4 * P * k * 4);
+        ws->run_cnt.ensure((size_t)4 * P * 4);
+    }
+    TopkOut run(uint64_t r, uint32_t l) const
+    {
+        const size_t off = (size_t)(2 * r + l) * pb;
+        return {ws->run_ids.as<uint64_t>() + off * k, ws->run_dist.as<float>() + off * k, ws->run_cnt.as<uint32_t>() + off};
+    }
+    TopkOut dst(uint64_t c) const { return nchunks == 1 ? out : c == 0 ? run(0, 0) : run((c - 1) & 1, 1); }
+    void merge(uint64_t c, cudaStream_t st) const
+    {
+        if (c == 0) return;
+        const TopkOut a = run((c - 1) & 1, 0);
+        SelectArgs m = select_cands(a.dist, a.ids, k, pb, k, c + 1 == nchunks ? out : run(c & 1, 0));
+        m.ncols = 2 * (uint64_t)k; m.outer_stride = (uint64_t)pb * k; m.list_cnt = a.cnt;
+        m.only = only; m.gate = gate;
+        launch_select(with_scratch(ws, m), st);
+    }
+};
+
+// The chunk loop of a host handle's search: `rows` [N][row_bytes] pinned, in chunks and passes of shape sh.
+// score(X, c, n, p0, pb, dst) enqueues on the call's stream the k best of chunk c -- its n rows staged at X, ids from
+// position c C -- for the pb queries p0, p0 + 1, ... into dst ([pb][k], [pb]).
+template <class Score>
+static void stream_topk(Workspace *ws, cudaStream_t st, const void *rows, size_t row_bytes, uint64_t N,
+                        const StreamShape &sh, uint32_t B, uint32_t k, TopkOut out, const Deadline *deadline,
+                        Score &&score)
+{
+    const uint64_t C = sh.C, nchunks = sh.nchunks;
+    const uint32_t P = sh.P;
+    for (auto &b : ws->stage.buf) b.ensure(std::max<size_t>(C * row_bytes, 16));
+    RunningTopk::reserve(ws, nchunks, P, k);
+    const char *base = static_cast<const char *>(rows);
+    const uint64_t steps = (uint64_t)((B + P - 1) / P) * nchunks;      // step s: pass s / nchunks, chunk s % nchunks
+    auto chunk_rows = [&](uint64_t c) { return N ? std::min<uint64_t>(C, N - c * C) : 0; };
+    ws->stage.open(ws, st, steps, deadline, [&](uint64_t s) -> std::pair<const void *, size_t> {
+        const uint64_t c = s % nchunks;
+        return {base + c * C * row_bytes, chunk_rows(c) * row_bytes};
+    });
+    for (uint64_t s = 0; s < steps; s++) {
+        const uint32_t p0 = (uint32_t)(s / nchunks) * P, pb = std::min(P, B - p0);
+        const uint64_t c = s % nchunks;
+        const void *X = ws->stage.take(s);
+        const RunningTopk run{ws, nchunks, pb, k, out.at(p0, k)};
+        score(X, c, chunk_rows(c), p0, pb, run.dst(c));
+        // released before the merge, so that the next copy does not wait for it
+        ws->stage.release(s);
+        run.merge(c, st);
+    }
+    ws->stage.close();
+}
+
+// a host flat handle through stream_topk, each chunk scored by flat_score
 template <class T>
 static void flat_search_streamed(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *d_q,
                                  uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist,
                                  uint32_t *d_cnt, RowFilter rf, const Deadline *deadline)
 {
-    const uint64_t N = fl->nrows;
     const uint32_t d = fl->dim, k = sp.k;
-    const size_t es = sizeof(T), budget = workspace_budget();
+    const size_t es = sizeof(T);
     // per row of a chunk: two staging copies, the bf16 operand (f32 rows), |x|^2 and |x|
     const size_t row_b = 2 * (size_t)d * es + (fl->f16 ? 0 : 2 * (size_t)d) + 8;
-    const uint64_t C = std::max<uint64_t>(1, std::min<uint64_t>(std::max<uint64_t>(N, 1),
-                                                                std::min(budget / 2 / row_b, FLAT_STAGE_BYTES / (d * es))));
-    const uint64_t ldc = (C + 3) & ~3ull, nchunks = N ? (N + C - 1) / C : 1;
-    const size_t rest = budget > C * row_b ? budget - C * row_b : 0;
-    // per query: the running top-k (two buffers of two lists of k ids and distances, and their counts), and the scores
-    // of a chunk
-    const size_t run_q = (size_t)k * 48 + 16, score_q = ldc * 4 + large_k_query_bytes(k);
-    const uint32_t P = (uint32_t)std::max<size_t>(1, std::min<size_t>(B, rest / 2 / run_q));
-    const size_t left = rest > (size_t)P * run_q ? rest - (size_t)P * run_q : 0;
-    const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(P, left / score_q));
-    for (auto &b : ws->stage.buf) b.ensure(std::max<size_t>(C * d * es, 16));
+    const StreamShape sh = stream_shape(fl->nrows, row_b, (size_t)d * es, B, k);
+    const uint64_t C = sh.C;
     if (fl->has_tc && !fl->f16) ws->chunk_xb.ensure(C * d * 2);
     ws->chunk_n2.ensure(C * 4);
     if (metric == LGPU_COSINE) ws->chunk_ysqrt.ensure(C * 4);
-    if (nchunks > 1) {
-        ws->run_ids.ensure((size_t)4 * P * k * 8); ws->run_dist.ensure((size_t)4 * P * k * 4);
-        ws->run_cnt.ensure((size_t)4 * P * 4);
-    }
-    const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));      // [1] tensor-core distances, [3] queries
-    const char *rows = static_cast<const char *>(fl->rows_host.p);
-    const uint64_t steps = (uint64_t)((B + P - 1) / P) * nchunks;      // step s: pass s / nchunks, chunk s % nchunks
-    auto chunk_rows = [&](uint64_t c) { return N ? std::min<uint64_t>(C, N - c * C) : 0; };
-    ws->stage.open(ws, st, steps, deadline, [&](uint64_t s) -> std::pair<const void *, size_t> {
-        const uint64_t c = s % nchunks;
-        return {rows + c * C * d * es, chunk_rows(c) * d * es};
-    });
-    for (uint64_t s = 0; s < steps; s++) {
-        const uint32_t p0 = (uint32_t)(s / nchunks) * P, pb = std::min(P, B - p0);
-        const uint64_t c = s % nchunks, n = chunk_rows(c);
-        const T *X = static_cast<const T *>(ws->stage.take(s));
+    stream_topk(ws, st, fl->rows_host.p, (size_t)d * es, fl->nrows, sh, B, k, TopkOut{d_ids, d_dist, d_cnt}, deadline,
+                [&](const void *Xv, uint64_t c, uint64_t n, uint32_t p0, uint32_t pb, TopkOut dst) {
+        const T *X = static_cast<const T *>(Xv);
         // the operand only when a scoring group takes the tensor cores (the first group is the largest)
-        const bool tc = flat_tc_route(fl->has_tc, metric, sp, std::min(bs, pb), n);
+        const bool tc = flat_tc_route(fl->has_tc, metric, sp, std::min(sh.bs, pb), n);
         if (tc && fl->f16) launch_f16_row_terms(X, n, d, ws->chunk_n2.as<float>(), nullptr, st);
         else if (tc) launch_to_bf16(reinterpret_cast<const float *>(X), n, d, ws->chunk_xb.p, ws->chunk_n2.as<float>(), st);
         if (metric == LGPU_COSINE) launch_row_norms(X, n, d, ws->chunk_ysqrt.as<float>(), st);
         const FlatRows<T> chunk{X, fl->f16 ? static_cast<const void *>(X) : ws->chunk_xb.p, ws->chunk_n2.as<float>(),
                                 ws->chunk_ysqrt.as<float>(), n,
                                 fl->has_ids ? Cols(fl->row_ids.as<uint64_t>() + c * C) : Cols(nullptr, c * C), tc};
-        // list l of running buffer r: [pb][k] entries and [pb] counts.  Chunk 0 goes to list 0 of buffer 0; chunk
-        // c > 0 to list 1 of buffer (c - 1) & 1, merged with its list 0 into list 0 of the other buffer, or into the
-        // output after the last chunk.  A column of one chunk is scored straight into the output.
-        auto run = [&](uint64_t r, uint32_t l) -> TopkOut {
-            const size_t off = (size_t)(2 * r + l) * pb;
-            return {ws->run_ids.as<uint64_t>() + off * k, ws->run_dist.as<float>() + off * k, ws->run_cnt.as<uint32_t>() + off};
-        };
-        const TopkOut pass_out = out.at(p0, k);
-        const TopkOut dst = nchunks == 1 ? pass_out : c == 0 ? run(0, 0) : run((c - 1) & 1, 1);
-        for (uint32_t g0 = 0; g0 < pb; g0 += bs)
-            flat_score(fl, ws, st, metric, d_q + (size_t)(p0 + g0) * d, std::min(bs, pb - g0), sp, chunk, dst.at(g0, k),
-                       rf, prof);
-        // released before the merge, so that the next copy does not wait for it
-        ws->stage.release(s);
-        if (c > 0) {
-            const TopkOut a = run((c - 1) & 1, 0);
-            SelectArgs m = select_cands(a.dist, a.ids, k, pb, k, c + 1 == nchunks ? pass_out : run(c & 1, 0));
-            m.ncols = 2 * (uint64_t)k; m.outer_stride = (uint64_t)pb * k; m.list_cnt = a.cnt;
-            launch_select(with_scratch(ws, m), st);
-        }
-    }
-    ws->stage.close();
+        for (uint32_t g0 = 0; g0 < pb; g0 += sh.bs)
+            flat_score(fl, ws, st, metric, d_q + (size_t)(p0 + g0) * d, std::min(sh.bs, pb - g0), sp, chunk,
+                       dst.at(g0, k), rf, prof);
+    });
     if (prof) g_filter_stats[3] = B;
 }
 
@@ -1910,8 +1967,9 @@ static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
 }
 
 // The threshold sample of the list path, taken from the handle's rows at open and after every append (which hold the
-// handle alone): every (nrows / HAM_SAMPLE)-th row, packed, with its popcount and its id.  Enqueued on the legacy
-// stream; the caller synchronises.
+// handle alone): every (nrows / HAM_SAMPLE)-th row, packed, with its popcount and its id.  A host handle's sample rows
+// are gathered on the host and uploaded, so the sample is in HBM for both placements.  Enqueued on the legacy stream;
+// the caller synchronises.
 static void ham_sample(lgpu_binary *bx, uint64_t nrows)
 {
     if (nrows <= HAM_SAMPLE) return;
@@ -1921,8 +1979,20 @@ static void ham_sample(lgpu_binary *bx, uint64_t nrows)
     bx->sample.ensure((size_t)HAM_SAMPLE * nbp);
     bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
     bx->sample_ids.ensure((size_t)HAM_SAMPLE * 8);
-    launch_ham_pack(bx->vectors.as<uint8_t>(), stride * nbp, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp,
-                    bx->sample_pop.as<uint32_t>(), nullptr);
+    DevBuf gathered;
+    const uint8_t *src = bx->vectors.as<uint8_t>();
+    uint64_t src_stride = stride * nbp;
+    if (bx->on_host) {
+        std::vector<uint8_t> h((size_t)HAM_SAMPLE * nbp);
+        const uint8_t *rows = static_cast<const uint8_t *>(bx->rows_host.p);
+        for (uint64_t s = 0; s < HAM_SAMPLE; s++) memcpy(h.data() + s * nbp, rows + s * stride * nbp, nbp);
+        gathered.ensure(h.size());
+        LGPU_CUDA(cudaMemcpy(gathered.p, h.data(), h.size(), cudaMemcpyHostToDevice));
+        src = gathered.as<uint8_t>();
+        src_stride = nbp;
+    }
+    launch_ham_pack(src, src_stride, nbp, HAM_SAMPLE, bx->sample.as<uint8_t>(), nbp, bx->sample_pop.as<uint32_t>(),
+                    nullptr);
     if (bx->has_ids) {
         LGPU_CUDA(cudaMemcpy2DAsync(bx->sample_ids.p, 8, bx->row_ids.p, stride * 8, 8, HAM_SAMPLE,
                                     cudaMemcpyDeviceToDevice, nullptr));
@@ -1933,37 +2003,58 @@ static void ham_sample(lgpu_binary *bx, uint64_t nrows)
     }
 }
 
-// One sub-batch through the tensor-core list path (Q: padded queries [B][nbytes_pad], qpop [B]) over the rows that pass
-// the row filter rf (none: every row).  The dense fix-up of overflowed queries runs in chunks of `bf` queries over a
-// [bf][N] matrix: one launch lists each chunk's flagged queries, and each chunk's two launches return at once when its
-// list is empty.
-static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
-                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, TopkOut out, RowFilter rf)
+// The list path of one sub-batch (Q: padded queries [B][nbytes_pad], qpop [B]) over the rows that pass the row filter rf
+// (none: every row), in four steps: the threshold (ham_list_threshold), the filtering pass over every row into the
+// candidate lists, their top-k (ham_list_select), the dense fix-up of the queries whose list overflowed.  An HBM handle
+// runs the filtering pass as one GEMM (ham_topk_list), a host handle as one per staged chunk appending to the same
+// lists (ham_topk_list_streamed).
+// 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest over the allowed ones (an upper bound of
+// the true k-th over all rows; +inf with fewer than k).  Then the candidate counters are zeroed, and the filter of the
+// filtering pass is returned: every allowed row with d <= tau_q is appended as (position, id, distance); the distance
+// is final.
+static GemmFilter ham_list_threshold(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q,
+                                     const uint32_t *qpop, uint32_t B, uint32_t k, uint32_t cap, RowFilter rf)
 {
-    const uint64_t N = bx->nrows, ns = bx->nsample, lds = (ns + 3) & ~3ull, ld = (N + 3) & ~3ull;
-    const uint32_t nbp = bx->nbytes_pad;
-    const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
-    // 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest over the allowed ones (an upper
-    // bound of the true k-th; +inf with fewer than k)
-    launch_ham_gemm(Q, bx->sample.p, bx->sample_pop.as<uint32_t>(), qpop, B, ns, nbp, ws->h_sample.as<float>(), lds,
-                    bx->num_sms, st);
+    const uint64_t ns = bx->nsample, lds = (ns + 3) & ~3ull;
+    launch_ham_gemm(Q, bx->sample.p, bx->sample_pop.as<uint32_t>(), qpop, B, ns, bx->nbytes_pad,
+                    ws->h_sample.as<float>(), lds, bx->num_sms, st);
     SelectArgs ss = select_rows(ws->h_sample.as<float>(), ns, lds, B, k, {ws->sbound.as<uint64_t>(),
                                                                           ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>()});
     if (rf.bits) { ss.col_ids = bx->sample_ids.as<uint64_t>(); ss.allow = rf.bits; ss.allow_bits = rf.nbits; }
     launch_select(ss, st);
     launch_ham_threshold(ws->t_dist.as<float>(), ws->t_cnt.as<uint32_t>(), B, k, ws->probe_A.as<float>(), st);
-    // 2. full pass: every allowed row with d <= tau_q is appended as (position, id, distance); the distance is final
     LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
     GemmFilter flt{};
     flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
-    flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = col_ids; flt.cap = cap; flt.cand_s = ws->t_exact.as<float>();
+    flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    flt.cap = cap; flt.cand_s = ws->t_exact.as<float>();
     flt.allow = rf.bits; flt.allow_bits = rf.nbits;
-    launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
+    return flt;
+}
+
+// 3. the overflow flags, and the top-k by (distance, id) of each list (an overflowed list is complete up to cap; its
+// query is redone by the fix-up)
+static void ham_list_select(Workspace *ws, cudaStream_t st, uint32_t B, uint32_t k, uint32_t cap, TopkOut out)
+{
     launch_overflow_flags(ws->amax.as<uint32_t>(), cap, nullptr, B, ws->flags.as<uint32_t>(), st);
-    // 3. top-k by (distance, id) of each list (an overflowed list is complete up to cap; its query is redone below)
     SelectArgs sb = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), cap, B, k, out);
     sb.ncols_q = ws->amax.as<uint32_t>();
     launch_select(sb, st);
+}
+
+// An HBM handle.  The dense fix-up of overflowed queries runs in chunks of `bf` queries over a [bf][N] matrix: one
+// launch lists each chunk's flagged queries, and each chunk's two launches return at once when its list is empty.
+static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
+                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, TopkOut out, RowFilter rf)
+{
+    const uint64_t N = bx->nrows, ld = (N + 3) & ~3ull;
+    const uint32_t nbp = bx->nbytes_pad;
+    const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    // 1, 2. threshold, filtering pass
+    const GemmFilter flt = ham_list_threshold(bx, ws, st, Q, qpop, B, k, cap, rf);
+    launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
+    // 3. top-k of the lists
+    ham_list_select(ws, st, B, k, cap, out);
     // 4. dense fix-up of the overflowed queries only
     launch_ham_flag_list(ws->flags.as<uint32_t>(), B, bf, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
     for (uint32_t q0 = 0, c = 0; q0 < B; q0 += bf, c++) {
@@ -1977,47 +2068,144 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     }
 }
 
-// d_q: raw queries [B][nbytes] in device memory
+// the ids of rows [r0, ..) of a binary handle: its explicit ids from r0, or the positions from r0
+static Cols ham_cols(lgpu_binary *bx, uint64_t r0)
+{
+    return bx->has_ids ? Cols(bx->row_ids.as<uint64_t>() + r0) : Cols(nullptr, r0);
+}
+
+// A host handle, chunks of C rows.  The one threshold tau_q bounds the k-th distance over every row, so each staged
+// chunk runs the filtering GEMM (its popcounts computed on the device, ids from its first row) into the sub-batch's
+// candidate lists, whose counts add up across chunks: each row crosses PCIe once and the lists need no merge.  The
+// fix-up: one list of all B flagged queries (its count gates every launch below), then per chunk a gated copy of its
+// rows out of the mapped pinned memory into staging buffer 0, the dense Hamming scores of the flagged queries
+// ([B][C] matrix) and their top-k, merged into a running top-k of the flagged queries; with nothing flagged each launch
+// returns at once, and nothing waits on the host.
+static void ham_topk_list_streamed(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q,
+                                   const uint32_t *qpop, uint32_t B, uint32_t k, uint32_t cap, uint64_t C, TopkOut out,
+                                   RowFilter rf, const Deadline *deadline)
+{
+    const uint64_t N = bx->nrows, nchunks = (N + C - 1) / C, ldc = (C + 3) & ~3ull;
+    const uint32_t nbp = bx->nbytes_pad;
+    auto chunk_rows = [&](uint64_t c) { return std::min<uint64_t>(C, N - c * C); };
+    const char *rows = static_cast<const char *>(bx->rows_host.p);
+    // 1, 2. threshold, filtering pass per chunk
+    GemmFilter flt = ham_list_threshold(bx, ws, st, Q, qpop, B, k, cap, rf);
+    ws->stage.open(ws, st, nchunks, deadline, [&](uint64_t c) -> std::pair<const void *, size_t> {
+        return {rows + c * C * nbp, chunk_rows(c) * nbp};
+    });
+    for (uint64_t c = 0; c < nchunks; c++) {
+        const uint64_t n = chunk_rows(c);
+        const void *X = ws->stage.take(c);
+        launch_ham_pack(static_cast<const uint8_t *>(X), nbp, nbp, n, nullptr, nbp, ws->chunk_pop.as<uint32_t>(), st);
+        const Cols cols = ham_cols(bx, c * C);
+        flt.col_ids = cols.ids; flt.col_base = cols.base;
+        launch_ham_gemm(Q, X, ws->chunk_pop.as<uint32_t>(), qpop, B, n, nbp, nullptr, 0, bx->num_sms, st, &flt);
+        ws->stage.release(c);
+    }
+    ws->stage.close();
+    // 3. top-k of the lists
+    ham_list_select(ws, st, B, k, cap, out);
+    // 4. dense fix-up of the overflowed queries only
+    launch_ham_flag_list(ws->flags.as<uint32_t>(), B, B, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
+    const uint32_t *gate = ws->h_cnt.as<uint32_t>();
+    RunningTopk run{ws, nchunks, B, k, out};
+    run.only = ws->flags.as<uint32_t>(); run.gate = gate;
+    const uint8_t *mapped = static_cast<const uint8_t *>(bx->rows_host.dev);
+    for (uint64_t c = 0; c < nchunks; c++) {
+        const uint64_t n = chunk_rows(c);
+        launch_mv_copy_gated(mapped + c * C * nbp, ws->stage.buf[0].as<uint8_t>(), n * nbp, gate, bx->num_sms, st);
+        launch_ham_dense(Q, ws->stage.buf[0].as<uint8_t>(), B, n, nbp, ws->D.as<float>(), ldc, bx->num_sms, st,
+                         ws->h_list.as<uint32_t>(), gate);
+        SelectArgs sc = select_rows(ws->D.as<float>(), n, ldc, B, k, run.dst(c));
+        with_cols(sc, ham_cols(bx, c * C));
+        sc.only = run.only; sc.gate = gate;
+        sc.allow = rf.bits; sc.allow_bits = rf.nbits;
+        launch_select(sc, st);
+        run.merge(c, st);
+    }
+}
+
+// b queries (Q, qpop) against N rows X of a binary handle (ids from cols) by the dense route of an HBM handle of those
+// rows, xpop their popcounts (tc only), into out: the b1 wgmma kernel (tc) or the SIMT kernel writes D [b][ld], then the
+// top-k with the request's range and row filter
+static void ham_dense_topk(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
+                           uint32_t b, const uint8_t *X, const uint32_t *xpop, uint64_t N, Cols cols, bool tc,
+                           const lgpu_search_params &sp, RowFilter rf, TopkOut out)
+{
+    const uint64_t ld = (N + 3) & ~3ull;
+    ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
+    if (tc) launch_ham_gemm(Q, X, xpop, qpop, b, N, bx->nbytes_pad, ws->D.as<float>(), ld, bx->num_sms, st);
+    else launch_ham_dense(Q, X, b, N, bx->nbytes_pad, ws->D.as<float>(), ld, bx->num_sms, st);
+    select_dense(ws, ws->D.as<float>(), N, ld, cols, b, sp, rf, out, st);
+}
+
+// d_q: raw queries [B][nbytes] in device memory.  A host handle (lgpu_binary::on_host) takes the same route as an HBM
+// handle of its rows, its rows streamed: the list route through ham_topk_list_streamed, the dense routes through
+// stream_topk, each chunk scored as an HBM handle of the chunk's rows would score it.
 void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *d_q, uint32_t B,
                           const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                           RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
 {
     const uint64_t N = bx->nrows, ld = (N + 3) & ~3ull;
     const uint32_t nbp = bx->nbytes_pad, k = sp.k;
-    const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
     const TopkOut out{d_ids, d_dist, d_cnt};
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));
     ws->hq.ensure((size_t)B * nbp); ws->hq_pop.ensure((size_t)B * 4);
     launch_ham_pack(d_q, bx->nbytes, bx->nbytes, B, ws->hq.as<uint8_t>(), nbp, ws->hq_pop.as<uint32_t>(), st);
     const uint8_t *Q = ws->hq.as<uint8_t>();
+    const uint32_t *qpop = ws->hq_pop.as<uint32_t>();
     const bool tc_ok = tc_enabled() && !sp.has_lower && !sp.has_upper;
     // k above SELECT_KMAX: a dense path (the list path's capacity stops at 16384 rows)
     const bool list = tc_ok && bx->nsample > 0 && k <= SELECT_KMAX;
     const bool tc = list || (tc_ok && B >= HAM_TC_MIN_B && N >= HAM_TC_MIN_N);
     const size_t budget = workspace_budget();
+    uint64_t tc_dists = 0;          // profiling: distances computed on the tensor cores
     if (list) {
-        // Workspace, all inside LGPU_WS_BYTES: the fix-up matrix [bf][N] gets at most half the budget and 1 GiB (it is
-        // rarely used); the rest is split into sub-batches of bs queries, each holding its sample scores [bs][ns] and
-        // candidate lists [bs][cap] (at the default 8 GiB, 1024 queries x 10M rows run as one sub-batch).
+        // Workspace, all inside LGPU_WS_BYTES.  An HBM handle: the fix-up matrix [bf][N] gets at most half the budget
+        // and 1 GiB (it is rarely used); the rest is split into sub-batches of bs queries, each holding its sample
+        // scores [bs][ns] and candidate lists [bs][cap] (at the default 8 GiB, 1024 queries x 10M rows run as one
+        // sub-batch).  A host handle: chunks of C rows take the two staging copies and popcounts of at most half the
+        // budget; each query of a sub-batch adds to the above its running top-k and its row of the fix-up matrix
+        // [bs][C].
         const uint64_t ns = bx->nsample, lds = (ns + 3) & ~3ull;
         const uint32_t cap = ham_list_cap(k, N, ns);
-        const uint32_t bf = (uint32_t)std::max<size_t>(1, std::min<size_t>(std::min<size_t>(budget / 2, (size_t)1 << 30) / (ld * 4), B));
-        const size_t per_q = lds * 4 + (size_t)cap * 20 + (size_t)k * 12 + 16;
-        const size_t left = budget > (size_t)bf * ld * 4 ? budget - (size_t)bf * ld * 4 : 0;
-        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
+        const size_t per_q0 = lds * 4 + (size_t)cap * 20 + (size_t)k * 12 + 16;
+        uint32_t bf = 0, bs = 0;
+        uint64_t C = 0;
+        if (bx->on_host) {
+            const size_t row_b = 2 * (size_t)nbp + 4;
+            C = std::max<uint64_t>(1, std::min<uint64_t>(N, std::min(budget / 2 / row_b, FLAT_STAGE_BYTES / nbp)));
+            const uint64_t ldc = (C + 3) & ~3ull;
+            const size_t per_q = per_q0 + (size_t)k * 48 + 16 + ldc * 4;
+            const size_t left = budget > C * row_b ? budget - C * row_b : 0;
+            bs = bf = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
+            for (auto &b : ws->stage.buf) b.ensure(C * nbp);
+            ws->chunk_pop.ensure(C * 4);
+            RunningTopk::reserve(ws, (N + C - 1) / C, bs, k);
+            ws->D.ensure((size_t)bs * ldc * 4);
+        } else {
+            bf = (uint32_t)std::max<size_t>(1, std::min<size_t>(std::min<size_t>(budget / 2, (size_t)1 << 30) / (ld * 4), B));
+            const size_t left = budget > (size_t)bf * ld * 4 ? budget - (size_t)bf * ld * 4 : 0;
+            bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q0, B));
+            ws->D.ensure((size_t)bf * ld * 4);
+        }
         ws->h_sample.ensure((size_t)bs * lds * 4);
         ws->t_dist.ensure((size_t)bs * k * 4); ws->sbound.ensure((size_t)bs * k * 8); ws->t_cnt.ensure((size_t)bs * 4);
         ws->probe_A.ensure((size_t)bs * 4); ws->amax.ensure((size_t)bs * 4); ws->flags.ensure((size_t)bs * 4);
         ws->t_pos.ensure((size_t)bs * cap * 8); ws->t_ids.ensure((size_t)bs * cap * 8);
         ws->t_exact.ensure((size_t)bs * cap * 4);
-        ws->D.ensure((size_t)bf * ld * 4); ws->h_list.ensure((size_t)bs * 4);
+        ws->h_list.ensure((size_t)bs * 4);
         ws->h_cnt.ensure((size_t)((bs + bf - 1) / bf) * 4);
         for (uint32_t q0 = 0; q0 < B; q0 += bs) {
             const uint32_t b = std::min(bs, B - q0);
             if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, ws->hq_pop.as<uint32_t>() + q0, b, k, cap, bf, out.at(q0, k),
-                          rf);
+            if (bx->on_host)
+                ham_topk_list_streamed(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, k, cap, C, out.at(q0, k), rf,
+                                       deadline);
+            else
+                ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, k, cap, bf, out.at(q0, k), rf);
             if (prof) {             // [0] list appends, [2] queries redone densely (over every sub-batch)
                 std::vector<uint32_t> cnt(b), fl(b);
                 LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->amax.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
@@ -2026,25 +2214,40 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
                 for (uint32_t q = 0; q < b; q++) { g_filter_stats[0] += cnt[q]; g_filter_stats[2] += fl[q] ? 1 : 0; }
             }
         }
+        tc_dists = (uint64_t)B * (N + ns);
+    } else if (bx->on_host) {
+        // per row of a chunk: two staging copies and its popcount
+        const StreamShape sh = stream_shape(N, 2 * (size_t)nbp + 4, nbp, B, k);
+        ws->chunk_pop.ensure(sh.C * 4);
+        stream_topk(ws, st, bx->rows_host.p, nbp, N, sh, B, k, out, deadline,
+                    [&](const void *Xv, uint64_t c, uint64_t n, uint32_t p0, uint32_t pb, TopkOut dst) {
+            const uint8_t *X = static_cast<const uint8_t *>(Xv);
+            auto group_tc = [&](uint32_t b) { return tc_ok && b >= HAM_TC_MIN_B && n >= HAM_TC_MIN_N; };
+            // the popcounts only when a scoring group takes the tensor cores (the first group is the largest)
+            if (group_tc(std::min(sh.bs, pb)))
+                launch_ham_pack(X, nbp, nbp, n, nullptr, nbp, ws->chunk_pop.as<uint32_t>(), st);
+            for (uint32_t g0 = 0; g0 < pb; g0 += sh.bs) {
+                const uint32_t b = std::min(sh.bs, pb - g0);
+                ham_dense_topk(bx, ws, st, Q + (size_t)(p0 + g0) * nbp, qpop + p0 + g0, b, X,
+                               ws->chunk_pop.as<uint32_t>(), n, ham_cols(bx, c * sh.C), group_tc(b), sp, rf,
+                               dst.at(g0, k));
+                if (group_tc(b)) tc_dists += (uint64_t)b * n;
+            }
+        });
     } else {
         const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
         const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / per_q, B));
         for (uint32_t q0 = 0; q0 < B; q0 += bs) {
             const uint32_t b = std::min(bs, B - q0);
             if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-            ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-            if (tc)
-                launch_ham_gemm(Q + (size_t)q0 * nbp, bx->vectors.p, bx->pop.as<uint32_t>(), ws->hq_pop.as<uint32_t>() + q0, b,
-                                N, nbp, ws->D.as<float>(), ld, bx->num_sms, st);
-            else
-                launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld,
-                                 bx->num_sms, st);
-            select_dense(ws, ws->D.as<float>(), N, ld, col_ids, b, sp, rf, out.at(q0, k), st);
+            ham_dense_topk(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, bx->vectors.as<uint8_t>(),
+                           bx->pop.as<uint32_t>(), N, ham_cols(bx, 0), tc, sp, rf, out.at(q0, k));
         }
+        if (tc) tc_dists = (uint64_t)B * N;
     }
     if (prof) {                     // [1] distances computed on the tensor cores, [3] queries
         LGPU_CUDA(cudaStreamSynchronize(st));
-        g_filter_stats[1] = tc ? (uint64_t)B * (N + (list ? bx->nsample : 0)) : 0;
+        g_filter_stats[1] = tc_dists;
         g_filter_stats[3] = B;
     }
 }
@@ -2521,10 +2724,11 @@ static Route filtered_route(const uint32_t *allow, uint64_t allow_bits)
 }
 static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, stream}; }
 
-// Whether the host route may capture a handle's calls into a CUDA graph: not a flat handle whose rows are on the host,
-// whose calls stream from pinned memory that an append moves, on a side stream (flat_search_streamed)
+// Whether the host route may capture a handle's calls into a CUDA graph: not a flat or binary handle whose rows are on
+// the host, whose calls stream from pinned memory that an append moves, on a side stream (stream_topk)
 template <class H> static bool graph_capturable(const H *) { return true; }
 static bool graph_capturable(const lgpu_flat *fl) { return !fl->on_host; }
+static bool graph_capturable(const lgpu_binary *bx) { return !bx->on_host; }
 
 // The sequence of every search entry point: resolve the handle; the kind's own checks, `check(h)`, which return how
 // many query elements (T) the call reads; the bitmap of a filtered call; nothing more for B == 0; the device; then
@@ -3684,6 +3888,20 @@ int lgpu_flat_search_device(lgpu_flat *flh, int metric, const float *d_queries, 
                      d_out_count);
 }
 
+// n rows [n][nbytes] packed on the host as a binary handle stores them, [n][nbytes_pad] zero-padded: the layout the b1
+// GEMM's TMA reads, so a host handle's staged chunk is the operand as it is
+static void ham_pack_host(const uint8_t *src, uint64_t n, uint32_t nbytes, uint32_t nbytes_pad, uint8_t *dst)
+{
+    if (nbytes == nbytes_pad) { memcpy(dst, src, (size_t)n * nbytes); return; }
+    for (uint64_t r = 0; r < n; r++) {
+        memcpy(dst + r * nbytes_pad, src + r * nbytes, nbytes);
+        memset(dst + r * nbytes_pad + nbytes, 0, nbytes_pad - nbytes);
+    }
+}
+
+// The packed rows and their popcounts go to HBM when they fit there (LGPU_BINARY_HBM_BYTES, rows_fit_hbm), else the
+// rows are packed into pinned host memory the handle owns.  HBM rows and popcounts are allocated exactly, so that
+// device bytes of the two placements differ by nrows x (nbytes_pad + 4).
 int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, const uint64_t *row_ids, int device,
                      lgpu_binary **out)
 {
@@ -3696,14 +3914,21 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
         bx = new lgpu_binary();
         bx->device = device; bx->nrows = nrows; bx->nbytes = nbytes; bx->nbytes_pad = (nbytes + 31) & ~31u;
         const uint32_t nbp = bx->nbytes_pad;
-        bx->vectors.ensure(std::max<size_t>((size_t)nrows * nbp, 16));
-        bx->pop.ensure(std::max<size_t>((size_t)nrows * 4, 16));
-        if (nrows) {
+        if (!rows_fit_hbm("LGPU_BINARY_HBM_BYTES", nrows * (nbp + 4))) {
+            bx->on_host = true;
+            bx->rows_host.alloc((size_t)nrows * nbp);
+            ham_pack_host(vectors, nrows, nbytes, nbp, static_cast<uint8_t *>(bx->rows_host.p));
+        } else if (nrows) {
+            bx->vectors.ensure((size_t)nrows * nbp, true);
+            bx->pop.ensure((size_t)nrows * 4, true);
             DevBuf raw;
             raw.ensure((size_t)nrows * nbytes);
             LGPU_CUDA(cudaMemcpy(raw.p, vectors, (size_t)nrows * nbytes, cudaMemcpyHostToDevice));
             launch_ham_pack(raw.as<uint8_t>(), nbytes, nbytes, nrows, bx->vectors.as<uint8_t>(), nbp, bx->pop.as<uint32_t>(),
                             nullptr);
+        } else {
+            bx->vectors.ensure(16);
+            bx->pop.ensure(16);
         }
         open_rows(bx, row_ids, nrows);
         ham_sample(bx, nrows);
@@ -3713,6 +3938,27 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
     });
     if (rc != LGPU_OK && bx) delete bx;
     return rc;
+}
+
+int lgpu_binary_device_bytes(const lgpu_binary *bxh, uint64_t *bytes)
+{
+    return guarded([&] {
+        HandleRef<lgpu_binary> h(const_cast<lgpu_binary *>(bxh));
+        LGPU_REQUIRE(bytes != nullptr, "null argument");
+        const lgpu_binary *bx = h.h;
+        *bytes = bx->vectors.bytes + bx->pop.bytes + bx->row_ids.bytes + bx->sample.bytes + bx->sample_pop.bytes +
+                 bx->sample_ids.bytes + bx->live.bits.bytes;
+    });
+}
+
+int lgpu_binary_host_bytes(const lgpu_binary *bxh, uint64_t *bytes, int *placement)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(bytes || placement, "null argument");
+        HandleRef<lgpu_binary> bx(const_cast<lgpu_binary *>(bxh));
+        if (bytes) *bytes = bx->rows_host.bytes;
+        if (placement) *placement = bx->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+    });
 }
 
 void lgpu_binary_close(lgpu_binary *bx) { close_handle(bx); }
@@ -4062,6 +4308,16 @@ int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const 
         begin_append(bx->device);
         const uint64_t n0 = bx->nrows, n1 = n0 + n;
         const uint32_t nbp = bx->nbytes_pad;
+        if (bx->on_host) {
+            grow_keep(bx->rows_host, (size_t)n0 * nbp, (size_t)n1 * nbp);
+            ham_pack_host(rows, n, bx->nbytes, nbp, static_cast<uint8_t *>(bx->rows_host.p) + (size_t)n0 * nbp);
+            append_ids(bx, n0, n, row_ids);
+            grow_live(bx, n0, n, bound);
+            ham_sample(bx, n1);
+            LGPU_CUDA(cudaDeviceSynchronize());
+            bx->nrows = n1;
+            return;
+        }
         grow_keep(bx->vectors, (size_t)n0 * nbp, (size_t)n1 * nbp);
         grow_keep(bx->pop, (size_t)n0 * 4, (size_t)n1 * 4);
         DevBuf raw;

@@ -14,7 +14,7 @@ namespace {
 constexpr int HD_THREADS = 256;   // one row per thread
 constexpr int HD_Q = 8;           // queries per work item: each row word loaded once serves 8 queries
 
-// one warp per row
+// one warp per row; dst null: the popcounts alone (rows that are packed already, a host handle's staged chunk)
 __global__ void ham_pack_kernel(const uint8_t *__restrict__ src, uint64_t src_stride, uint32_t nbytes, uint64_t n,
                                 uint8_t *__restrict__ dst, uint32_t nbytes_pad, uint32_t *__restrict__ pop)
 {
@@ -23,11 +23,10 @@ __global__ void ham_pack_kernel(const uint8_t *__restrict__ src, uint64_t src_st
     const uint32_t lane = threadIdx.x & 31;
     if (row >= n) return;
     const uint8_t *s = src + row * src_stride;
-    uint8_t *d = dst + row * nbytes_pad;
     uint32_t p = 0;
     for (uint32_t c = lane; c < nbytes_pad; c += 32) {
         const uint32_t b = c < nbytes ? s[c] : 0u;
-        d[c] = (uint8_t)b;
+        if (dst) dst[row * nbytes_pad + c] = (uint8_t)b;
         p += __popc(b);
     }
     p = __reduce_add_sync(0xffffffffu, p);

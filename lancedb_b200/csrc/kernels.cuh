@@ -441,7 +441,8 @@ void launch_ham_gemm(const void *Qp, const void *Xp, const uint32_t *xpop, const
                      const GemmFilter *filter = nullptr);
 
 // ---------------- binary vectors, SIMT side (hamming.cu) --------------------------------
-// dst[r] = src row r (src rows `src_stride` bytes apart, nbytes used) zero-padded to nbytes_pad; pop[r] = its popcount
+// dst[r] = src row r (src rows `src_stride` bytes apart, nbytes used) zero-padded to nbytes_pad; pop[r] = its popcount.
+// dst null: pop alone (rows already packed: nbytes = nbytes_pad)
 void launch_ham_pack(const uint8_t *src, uint64_t src_stride, uint32_t nbytes, uint64_t n, uint8_t *dst,
                      uint32_t nbytes_pad, uint32_t *pop, cudaStream_t st);
 // D[q][x] = popc(Q[q] XOR X[x]) as f32 for x < N (LOP3 + POPC over 32-bit words; rows padded to a multiple of 32
@@ -506,7 +507,8 @@ void launch_mv_rescore_host(const float *Q, const uint32_t *q_off, uint32_t qa, 
                             const float *ysqrt, const uint64_t *offsets, const uint64_t *row_ids, uint32_t d, uint32_t B,
                             const uint32_t *cand, const uint32_t *count, uint32_t cap, float *out, uint64_t *ids,
                             int num_sms, cudaStream_t st);
-// dst[0, n) = src[0, n) elements (float or __half) when *gate (device) != 0; nothing otherwise (multivec.cu)
+// dst[0, n) = src[0, n) elements (float, __half, or the bytes of packed binary rows) when *gate (device) != 0; nothing
+// otherwise (multivec.cu)
 template <class T>
 void launch_mv_copy_gated(const T *src, T *dst, uint64_t n, const uint32_t *gate, int num_sms, cudaStream_t st);
 

@@ -293,6 +293,7 @@ void launch_mv_normalize_f16(const T *X, uint64_t n, uint32_t d, void *out, uint
 
 template void launch_mv_copy_gated<float>(const float *, float *, uint64_t, const uint32_t *, int, cudaStream_t);
 template void launch_mv_copy_gated<__half>(const __half *, __half *, uint64_t, const uint32_t *, int, cudaStream_t);
+template void launch_mv_copy_gated<uint8_t>(const uint8_t *, uint8_t *, uint64_t, const uint32_t *, int, cudaStream_t);
 template void launch_mv_normalize_f16<float>(const float *, uint64_t, uint32_t, void *, uint32_t *, cudaStream_t);
 template void launch_mv_normalize_f16<__half>(const __half *, uint64_t, uint32_t, void *, uint32_t *, cudaStream_t);
 
