@@ -75,7 +75,9 @@ typedef struct lgpu_ivf_binary lgpu_ivf_binary; /* a binary IVF_FLAT index in HB
  * (8-bit, 256 centroids per sub-vector), PQ codes and row ids grouped by partition. */
 typedef struct {
     uint32_t abi_version;        /* LGPU_ABI_VERSION */
-    uint32_t dim;
+    uint32_t dim;                /* no upper limit is checked.  8-bit codes: the filter scan serves m <= 512, so
+                                    dim <= 16384 (dim / m <= 32), where its band's underflow floor is argued; a wider
+                                    index takes the exact scan, tested bit for bit up to dim 32768 (m 1024 and 2048) */
     uint32_t nlist;              /* IVF partitions */
     uint32_t m;                  /* PQ sub-vectors; dim % m == 0 */
     uint32_t nbits;              /* 8, or 4 (packed nibble codes, see "4-bit IVF_PQ" below) */
