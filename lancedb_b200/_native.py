@@ -299,6 +299,27 @@ class _Handle:
     __del__ = close
 
 
+class _Placed:
+    """A handle that reports where it keeps its rows, through lgpu_*_device_bytes and lgpu_*_host_bytes, `_bytes` the
+    lgpu_* prefix."""
+    _bytes = ""
+
+    def _host(self):
+        b, where = C.c_uint64(0), C.c_int(0)
+        check(getattr(load(), self._bytes + "_host_bytes")(self._h, C.byref(b), C.byref(where)))
+        return b.value, where.value
+
+    def _device_bytes(self) -> int:
+        n = C.c_uint64(0)
+        check(getattr(load(), self._bytes + "_device_bytes")(self._h, C.byref(n)))
+        return n.value
+
+    def host_bytes(self) -> int:
+        """The pinned host memory the handle holds: the row data that did not fit in HBM at open, else 0
+        (lgpu_*_host_bytes)."""
+        return self._host()[0]
+
+
 class _RowsHandle(_Handle):
     """A handle over rows, which `_delete`, the name of its lgpu_*_delete, deletes rows from."""
     _delete = ""
@@ -310,6 +331,21 @@ class _RowsHandle(_Handle):
         n = C.c_uint64(0)
         check(getattr(load(), self._delete)(self._h, _ptr(ids), ids.size, C.byref(n)))
         return n.value
+
+
+class _Column(_Placed, _RowsHandle):
+    """A flat, binary or multivector column: its rows are kept in HBM when they fit there, else in pinned host memory
+    and streamed through the GPU once per search, with the same results (`rows_on_host`)."""
+
+    @property
+    def device_bytes(self) -> int:
+        """The HBM the handle holds for its rows and per-row data (lgpu_*_device_bytes)."""
+        return self._device_bytes()
+
+    @property
+    def rows_on_host(self) -> bool:
+        """True when the rows are kept in pinned host memory and every search streams them through the GPU."""
+        return self._host()[1] == VECTORS_HOST
 
 
 def _host_search(fn: str, head, B: int, k: int, p: SearchParams, allow, allow_bits):
@@ -388,11 +424,11 @@ def _query_offsets(q_offsets) -> np.ndarray:
     return np.ascontiguousarray(off, np.uint32)
 
 
-class GpuIvfPq(_RowsHandle):
+class GpuIvfPq(_Placed, _RowsHandle):
     """An IVF_PQ index pinned in HBM (lgpu_index), 8-bit or 4-bit codes (data.num_bits).  The other float IVF kinds
     open an lgpu_index through their own C function, `_open`, so they subclass this and supply only `_desc`."""
     _open, _close = "lgpu_index_open", "lgpu_index_close"
-    _delete = "lgpu_index_delete"
+    _delete, _bytes = "lgpu_index_delete", "lgpu_index"
 
     def __init__(self, data, device: int = 0, with_vectors: bool = True):
         lib = load()
@@ -417,19 +453,7 @@ class GpuIvfPq(_RowsHandle):
 
     def device_bytes(self) -> int:
         """The HBM the index holds; its raw vectors count only when they are in HBM."""
-        b = C.c_uint64(0)
-        check(load().lgpu_index_device_bytes(self._h, C.byref(b)))
-        return b.value
-
-    def _host(self):
-        b, where = C.c_uint64(0), C.c_int(0)
-        check(load().lgpu_index_host_bytes(self._h, C.byref(b), C.byref(where)))
-        return b.value, where.value
-
-    def host_bytes(self) -> int:
-        """The pinned host memory the index holds: its raw vectors (rows padded to 4 floats) when they did not fit in
-        HBM at open, else 0 (lgpu_index_host_bytes)."""
-        return self._host()[0]
+        return self._device_bytes()
 
     @property
     def vectors_on_host(self) -> bool:
@@ -562,13 +586,14 @@ class GpuIvfRq(GpuIvfPq):
                       *[_ptr(a) for a in keep]), keep
 
 
-class GpuFlat(_RowsHandle):
+class GpuFlat(_Column):
     """A raw vector column searched on the GPU (lgpu_flat).  A float16 array opens an fp16 handle (lgpu_flat_open_f16:
     the rows stay float16, results are those of their exact f32 upcast); anything else is converted to f32.  `dtype` is
     the handle's row type.  The rows are kept in HBM when they fit there (LGPU_FLAT_HBM_BYTES), else in pinned host
     memory and streamed through the GPU once per search, with the same results (`rows_on_host`)."""
     _close = "lgpu_flat_close"
     _delete = "lgpu_flat_delete"
+    _bytes = "lgpu_flat"
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
         self.dtype = np.dtype(np.float16 if getattr(vectors, "dtype", None) == np.float16 else np.float32)
@@ -580,28 +605,6 @@ class GpuFlat(_RowsHandle):
         check(getattr(load(), opener)(_ptr(v), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
-
-    @property
-    def device_bytes(self) -> int:
-        """The HBM the handle holds for its rows and per-row data (lgpu_flat_device_bytes)."""
-        n = C.c_uint64(0)
-        check(load().lgpu_flat_device_bytes(self._h, C.byref(n)))
-        return n.value
-
-    def _host(self):
-        b, where = C.c_uint64(0), C.c_int(0)
-        check(load().lgpu_flat_host_bytes(self._h, C.byref(b), C.byref(where)))
-        return b.value, where.value
-
-    def host_bytes(self) -> int:
-        """The pinned host memory the handle holds: its rows when they did not fit in HBM at open, else 0
-        (lgpu_flat_host_bytes)."""
-        return self._host()[0]
-
-    @property
-    def rows_on_host(self) -> bool:
-        """True when the rows are kept in pinned host memory and every search streams them through the GPU."""
-        return self._host()[1] == VECTORS_HOST
 
     def search(self, queries, k=10, metric="l2", lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         q = np.ascontiguousarray(queries, np.float32).reshape(-1, self.dim)
@@ -634,12 +637,13 @@ class GpuFlat(_RowsHandle):
         self.nrows += v.shape[0]
 
 
-class GpuBinary(_RowsHandle):
+class GpuBinary(_Column):
     """A packed binary vector column (fixed_size_list<uint8, nbytes>) searched by Hamming distance (lgpu_binary).  The
     packed rows are kept in HBM when they fit there (LGPU_BINARY_HBM_BYTES), else in pinned host memory and streamed
     through the GPU once per search, with the same results (`rows_on_host`)."""
     _close = "lgpu_binary_close"
     _delete = "lgpu_binary_delete"
+    _bytes = "lgpu_binary"
     _queries = _binary_queries
 
     def __init__(self, vectors, row_ids=None, device: int = 0):
@@ -652,28 +656,6 @@ class GpuBinary(_RowsHandle):
         check(load().lgpu_binary_open(_ptr(v), self.nrows, self.nbytes, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
-
-    @property
-    def device_bytes(self) -> int:
-        """The HBM the handle holds for its rows and per-row data (lgpu_binary_device_bytes)."""
-        n = C.c_uint64(0)
-        check(load().lgpu_binary_device_bytes(self._h, C.byref(n)))
-        return n.value
-
-    def _host(self):
-        b, where = C.c_uint64(0), C.c_int(0)
-        check(load().lgpu_binary_host_bytes(self._h, C.byref(b), C.byref(where)))
-        return b.value, where.value
-
-    def host_bytes(self) -> int:
-        """The pinned host memory the handle holds: its packed rows when they did not fit in HBM at open, else 0
-        (lgpu_binary_host_bytes)."""
-        return self._host()[0]
-
-    @property
-    def rows_on_host(self) -> bool:
-        """True when the rows are kept in pinned host memory and every search streams them through the GPU."""
-        return self._host()[1] == VECTORS_HOST
 
     def search(self, queries, k=10, lower=None, upper=None, allow=None, allow_bits=0, timeout_ms=0):
         """Host-buffer search of queries [B, nbytes] (or one [nbytes] query) whose components are integers in
@@ -750,7 +732,7 @@ def multivec_offsets(lengths) -> np.ndarray:
     return np.concatenate([[0], np.cumsum(n)]).astype(np.uint64)
 
 
-class GpuMultivec(_RowsHandle):
+class GpuMultivec(_Column):
     """A multivector column (list<fixed_size_list<float, dim>>) (lgpu_multivec), searched by late interaction:
     _distance = sum over the query's vectors of the smallest cosine distance to the row's vectors.  Its vectors are
     kept in HBM when they fit (LGPU_MULTIVEC_HBM_BYTES), else in pinned host memory and streamed through the GPU once
@@ -759,6 +741,7 @@ class GpuMultivec(_RowsHandle):
     converted to f32.  `dtype` is the handle's row type."""
     _close = "lgpu_multivec_close"
     _delete = "lgpu_multivec_delete"
+    _bytes = "lgpu_multivec"
 
     def __init__(self, values, offsets, row_ids=None, device: int = 0):
         self.dtype = np.dtype(np.float16 if getattr(values, "dtype", None) == np.float16 else np.float32)
@@ -783,28 +766,6 @@ class GpuMultivec(_RowsHandle):
         check(getattr(load(), opener)(_ptr(v), _ptr(off), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
-
-    @property
-    def device_bytes(self) -> int:
-        """The HBM the handle holds for its vectors and per-vector data (lgpu_multivec_device_bytes)."""
-        n = C.c_uint64(0)
-        check(load().lgpu_multivec_device_bytes(self._h, C.byref(n)))
-        return n.value
-
-    def _host(self):
-        b, where = C.c_uint64(0), C.c_int(0)
-        check(load().lgpu_multivec_host_bytes(self._h, C.byref(b), C.byref(where)))
-        return b.value, where.value
-
-    def host_bytes(self) -> int:
-        """The pinned host memory the handle holds: its vectors (and an f32 handle's tensor-core operand) when they did
-        not fit in HBM at open, else 0 (lgpu_multivec_host_bytes)."""
-        return self._host()[0]
-
-    @property
-    def rows_on_host(self) -> bool:
-        """True when the vectors are kept in pinned host memory and every search streams them through the GPU."""
-        return self._host()[1] == VECTORS_HOST
 
     def _queries(self, queries, q_offsets):
         """(values [Tq, dim] f32, offsets [B+1] u32).  queries: a list with one [nq_b, dim] (or [dim]) array per

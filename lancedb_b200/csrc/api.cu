@@ -232,10 +232,10 @@ struct Workspace {
     DevBuf u_ids, u_dist, u_cnt;        // union search: the index's and the tail's top-k, [2][B][k] and [2][B]
     DevBuf live_and;                    // a filtered call on a handle with deleted rows: its bitmap AND the live rows
     Staging stage;                      // a handle whose rows are in pinned host memory: the rows staged through HBM
-    // a flat handle whose rows are in pinned host memory (flat_search_streamed): the staged chunk's tensor-core
+    // a flat handle whose rows are in pinned host memory (flat_search): the staged chunk's tensor-core
     // operand, |x|^2 and |x|, and the running top-k, [2 buffers][2 lists][P][k] / [..][P]
     DevBuf chunk_xb, chunk_n2, chunk_ysqrt, run_ids, run_dist, run_cnt;
-    DevBuf chunk_pop;                   // ... of a binary handle (binary_search_streamed): popc of each staged row
+    DevBuf chunk_pop;                   // ... of a binary handle (binary_search_device): popc of each staged row
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -316,6 +316,116 @@ struct RowLive {
     uint64_t id_bound = 0;
     bool active = false;
 };
+
+// `b` holds `used` bytes; make room for `need` (an append): capacity at least doubles, the contents move by a
+// device-to-device copy.  The caller has drained the device, so nothing still reads the old buffer when it is released.
+static void grow_keep(DevBuf &b, size_t used, size_t need)
+{
+    if (need <= b.bytes) return;
+    DevBuf nb;
+    nb.ensure(std::max(need, 2 * b.bytes));                    // bumps g_alloc_epoch
+    if (used) LGPU_CUDA(cudaMemcpy(nb.p, b.p, used, cudaMemcpyDeviceToDevice));
+    std::swap(b.p, nb.p);
+    std::swap(b.bytes, nb.bytes);
+}
+
+// One chunk of a RowStore walk: step s, rows [r0, r1), X the rows as a kernel reads them.  resident: X is the store's
+// own HBM (the handle's per-row terms apply as they are); else a staging buffer (the chunk's terms are built for it).
+struct RowChunk {
+    uint64_t s, r0, r1;
+    const void *X;
+    bool resident;
+};
+
+// The stored rows of a flat, binary or multivector handle, [n][row bytes]: in HBM, or -- when the open found they do
+// not fit there (rows_fit_hbm) -- in pinned host memory mapped into the device's address space, which searches stream
+// through HBM.  The placement is fixed at open.
+struct RowStore {
+    bool on_host = false;
+    DevBuf hbm;
+    PinnedBuf host;
+    // `bytes` of rows, allocated exactly (HBM: at least 16)
+    void open(bool in_host, size_t bytes)
+    {
+        on_host = in_host;
+        if (on_host) host.alloc(bytes);
+        else hbm.ensure(std::max<size_t>(bytes, 16), true);
+    }
+    // the rows as host code addresses them: an HBM pointer, or the pinned host memory
+    char *data() const { return static_cast<char *>(on_host ? host.p : hbm.p); }
+    // the rows as a kernel reads them: an HBM pointer, or the mapped alias of the pinned memory
+    const void *dev() const { return on_host ? host.dev : hbm.p; }
+    // bytes from a host pointer into the rows at byte `at`
+    void fill(size_t at, const void *src, size_t bytes)
+    {
+        if (!bytes) return;
+        if (on_host) memcpy(data() + at, src, bytes);
+        else LGPU_CUDA(cudaMemcpy(data() + at, src, bytes, cudaMemcpyHostToDevice));
+    }
+    // room for `need` bytes of rows, `used` of them kept (an append)
+    void grow(size_t used, size_t need)
+    {
+        if (!on_host) return grow_keep(hbm, used, need);
+        if (need <= host.bytes) return;
+        PinnedBuf nb;
+        nb.alloc(std::max(need, 2 * host.bytes));
+        if (used) memcpy(nb.p, host.p, used);
+        std::swap(host.p, nb.p);
+        std::swap(host.dev, nb.dev);
+        std::swap(host.bytes, nb.bytes);
+    }
+    uint64_t device_bytes() const { return hbm.bytes; }
+    uint64_t host_bytes() const { return host.bytes; }
+    // the two staging buffers of a host store's walk, `bytes` each
+    void reserve_stage(Workspace *ws, size_t bytes) const
+    {
+        if (on_host) for (auto &b : ws->stage.buf) b.ensure(bytes);
+    }
+    // use(RowChunk) for `passes` passes over the chunks cut[c]..cut[c + 1] (row r at byte at(r)), then after(s) once
+    // step s's staging buffer is released.  An HBM store is one resident chunk [cut.front(), cut.back()) per pass, the
+    // deadline checked between passes; a host store streams each chunk through Workspace::stage, which checks it
+    // between steps.
+    template <class At, class Use, class After>
+    void walk(Workspace *ws, cudaStream_t st, const std::vector<uint64_t> &cut, uint64_t passes, At &&at,
+              const Deadline *deadline, Use &&use, After &&after) const
+    {
+        const uint64_t nc = cut.size() - 1;
+        if (!on_host) {
+            for (uint64_t s = 0; s < passes; s++) {
+                if (deadline && s > 0) deadline->wait(st, ws->ev[7]);
+                use(RowChunk{s, cut.front(), cut.back(), hbm.p, true});
+                after(s);
+            }
+            return;
+        }
+        ws->stage.open(ws, st, passes * nc, deadline, [&](uint64_t s) -> std::pair<const void *, size_t> {
+            const uint64_t c = s % nc;
+            return {static_cast<const char *>(host.p) + at(cut[c]), at(cut[c + 1]) - at(cut[c])};
+        });
+        for (uint64_t s = 0; s < passes * nc; s++) {
+            const uint64_t c = s % nc;
+            use(RowChunk{s, cut[c], cut[c + 1], ws->stage.take(s), false});
+            ws->stage.release(s);
+            after(s);
+        }
+        ws->stage.close();
+    }
+    template <class At, class Use>
+    void walk(Workspace *ws, cudaStream_t st, const std::vector<uint64_t> &cut, At &&at, const Deadline *deadline,
+              Use &&use) const
+    {
+        walk(ws, st, cut, 1, at, deadline, use, [](uint64_t) {});
+    }
+};
+
+// the cuts of N rows in chunks of C
+static std::vector<uint64_t> uniform_cuts(uint64_t N, uint64_t C)
+{
+    std::vector<uint64_t> cut{0};
+    for (uint64_t r = 0; r < N; r += C) cut.push_back(std::min(N, r + C));
+    if (cut.size() == 1) cut.push_back(0);
+    return cut;
+}
 
 }  // namespace lgpu
 
@@ -521,71 +631,60 @@ struct lgpu_index {
 // the C header's handle type of a binary IVF_FLAT index (an lgpu_index of kind IvfKind::ham)
 struct lgpu_ivf_binary : lgpu_index {};
 
-struct lgpu_flat {
+// What the flat, binary and multivector handles share: their rows (RowStore, in HBM or pinned host memory), optional
+// row ids (else the positions), the live bitmap and the workspaces of their searches
+struct lgpu_rows {
     std::atomic<int> refs{0};
-    int device = 0;
+    int device = 0, num_sms = 0;
     uint64_t nrows = 0;
+    RowStore rows;
+    DevBuf row_ids;
+    bool has_ids = false;
+    RowLive live;
+    WorkspacePool pool;
+};
+
+// a float vector column.  `rows` holds [nrows][dim] f32, or fp16 (f16, lgpu_flat_open_f16); ysqrt, vec_b and vec_n2
+// stay empty for a host store
+struct lgpu_flat : lgpu_rows {
     uint32_t dim = 0;
-    bool f16 = false;                   // row type: `vectors` holds [nrows][dim] f32, or fp16 (lgpu_flat_open_f16)
-    DevBuf vectors, row_ids, ysqrt;
-    // rows that did not fit in HBM at open (flat_open): `rows_host` holds them, [nrows][dim] in the row type, and
-    // `vectors`, `ysqrt`, `vec_b` and `vec_n2` stay empty; searches stream the rows through HBM (flat_search_streamed)
-    bool on_host = false;
-    PinnedBuf rows_host;
+    bool f16 = false;
+    DevBuf ysqrt;                       // |x| (cosine), built by the first cosine search of an HBM store
     // the tensor-core path: bf16 rows (f32 handles; an fp16 handle's rows are their own operand) + |x|^2
     DevBuf vec_b, vec_n2;
     float vec_max = 0.f, vec_err = 0.f;     // max |x|, max |h(x) - x| (h: bf16 or fp16 rounding, gemm.cu)
-    int num_sms = 0;
     bool has_tc = false;
-    bool has_ids = false, has_norms = false;
+    bool has_norms = false;
     std::mutex mu;
-    RowLive live;
-    WorkspacePool pool;
 };
 
-// a packed binary vector column (fixed_size_list<uint8, nbytes>) searched by Hamming distance
-struct lgpu_binary {
-    std::atomic<int> refs{0};
-    int device = 0, num_sms = 0;
-    uint64_t nrows = 0;
+// a packed binary vector column (fixed_size_list<uint8, nbytes>) searched by Hamming distance.  `rows` holds
+// [nrows][nbytes_pad] zero-padded rows; `pop` (HBM store only) their popcounts
+struct lgpu_binary : lgpu_rows {
     uint32_t nbytes = 0, nbytes_pad = 0;   // caller's row bytes; stored row bytes (multiple of 32)
-    DevBuf vectors, pop, row_ids;          // [nrows][nbytes_pad] zero-padded rows, popc of each row, optional ids
-    DevBuf sample, sample_pop;             // every (nrows / nsample)-th row: the threshold sample of the list path
+    DevBuf pop;
+    // every (nrows / nsample)-th row: the threshold sample of the list path, in HBM for both placements
+    DevBuf sample, sample_pop;
     uint64_t nsample = 0;                  // 0: no sample (nrows <= HAM_SAMPLE)
     DevBuf sample_ids;                     // the sample rows' ids (a row filter tests them in the sample's select)
-    // rows that did not fit in HBM at open (lgpu_binary_open): `rows_host` holds them packed as `vectors` would,
-    // [nrows][nbytes_pad] zero-padded, and `vectors` and `pop` stay empty; searches stream the rows through HBM
-    // (binary_search_streamed).  The threshold sample stays in HBM.
-    bool on_host = false;
-    PinnedBuf rows_host;
-    bool has_ids = false;
-    RowLive live;
-    WorkspacePool pool;
 };
 
-// a multivector column (list<fixed_size_list<float, dim>>) searched by late interaction (MaxSim over cosine)
-struct lgpu_multivec {
-    std::atomic<int> refs{0};
-    int device = 0, num_sms = 0;
-    uint64_t nrows = 0, total = 0;         // rows; stored vectors T = offsets[nrows]
+// a multivector column (list<fixed_size_list<float, dim>>) searched by late interaction (MaxSim over cosine).  `rows`
+// holds the vectors [T][dim] in the row type (f32, or fp16: lgpu_multivec_open_f16), `ops` (same placement) the fp16
+// normalised tensor-core operand [T][dim] of an f32 handle of the tensor-core shape (an fp16 handle's vectors are
+// their own operand)
+struct lgpu_multivec : lgpu_rows {
+    uint64_t total = 0;                    // stored vectors T = offsets[nrows]
     uint32_t dim = 0;
     uint64_t max_row = 0;                  // largest n_r
-    bool f16 = false;                      // row type: `vectors` holds f32, or fp16 (lgpu_multivec_open_f16)
-    DevBuf vectors, ysqrt, offsets, row_ids;   // [T][dim] in the row type, |v| = sqrt(dot(v, v)) per vector, [nrows+1], ids
-    // tensor-core path: fp16 normalised vectors [T][dim] (f32 handles; an fp16 handle's vectors are their own operand),
-    // row of each vector [T]
-    DevBuf vec_h, col_row;
+    bool f16 = false;
+    RowStore ops;
+    DevBuf ysqrt, offsets;                 // |v| = sqrt(dot(v, v)) per vector, [nrows+1]
+    DevBuf col_row;                        // tensor-core path: row of each vector [T]
     bool tc_ok = false;                    // the tensor-core path may run (see multivec_search_device)
-    // row data that did not fit in HBM at open (multivec_open): `vectors_host` holds the vectors in the row type and
-    // `vec_h_host` the fp16 operand (f32 handles of the tensor-core shape only), both [T][dim]; `vectors` and `vec_h`
-    // stay empty, and searches stream the rows through HBM (multivec_search_device)
-    bool on_host = false;
-    PinnedBuf vectors_host, vec_h_host;
     std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
-    bool has_ids = false;
-    RowLive live;
-    WorkspacePool pool;
 };
+
 
 // ---- NCCL, bound at run time (dlopen): single-GPU hosts need no libnccl, and inside a process that already
 // loaded one (torch) the same library instance is used ----
@@ -776,6 +875,12 @@ struct Cols {
     uint64_t base;
     Cols(const uint64_t *i = nullptr, uint64_t b = 0) : ids(i), base(b) {}
 };
+
+// the ids of rows [r0, ..) of a handle: its explicit ids from r0, or the positions from r0
+static Cols row_cols(const lgpu_rows *h, uint64_t r0)
+{
+    return h->has_ids ? Cols(static_cast<const uint64_t *>(h->row_ids.p) + r0) : Cols(nullptr, r0);
+}
 
 // SelectArgs with the fields every mode needs; callers add the optional ones (only, gate, col_ids, range, allow, ...)
 static SelectArgs select_args(int mode, uint32_t B, uint32_t k, TopkOut out)
@@ -1762,59 +1867,38 @@ static void flat_score(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric
     select_dense(ws, ws->D.as<float>(), N, ld, r.cols, b, sp, rf, out, st);
 }
 
-// an HBM handle: its rows X, the queries in sub-batches that the workspace budget holds the scores of
-template <class T>
-static void flat_search_rows(lgpu_flat *fl, const T *X, Workspace *ws, cudaStream_t st, int metric, const float *d_q,
-                             uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
-                             RowFilter rf, const Deadline *deadline)
-{
-    const uint64_t N = fl->nrows;
-    const uint64_t ld = (N + 3) & ~3ull;
-    if (metric == LGPU_COSINE) {
-        std::lock_guard<std::mutex> g(fl->mu);
-        if (!fl->has_norms) {
-            fl->ysqrt.ensure(std::max<size_t>(N, 1) * 4, true);
-            launch_row_norms(X, N, fl->dim, fl->ysqrt.as<float>(), st);
-            LGPU_CUDA(cudaStreamSynchronize(st));
-            fl->has_norms = true;
-        }
-    }
-    size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(sp.k);
-    uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(workspace_budget() / per_q, B));
-    const TopkOut out{d_ids, d_dist, d_cnt};
-    const bool prof = profiling_enabled();
-    if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));      // [1] tensor-core distances, [3] queries
-    const FlatRows<T> rows{X, fl->f16 ? static_cast<const void *>(X) : fl->vec_b.p, fl->vec_n2.as<float>(),
-                           fl->ysqrt.as<float>(), N, fl->has_ids ? fl->row_ids.as<uint64_t>() : nullptr, fl->has_tc};
-    for (uint32_t q0 = 0; q0 < B; q0 += bs) {
-        uint32_t b = std::min(bs, B - q0);
-        if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-        flat_score(fl, ws, st, metric, d_q + (size_t)q0 * fl->dim, b, sp, rows, out.at(q0, sp.k), rf, prof);
-    }
-    if (prof) g_filter_stats[3] = B;
-}
-
 // the most rows of a host handle one staging buffer holds, in bytes: large enough that the copy engine runs at the
 // PCIe rate and a chunk's fixed scoring cost is small, small enough that the unoverlapped first copy is short
 constexpr size_t FLAT_STAGE_BYTES = (size_t)128 << 20;
 
-// A host handle (lgpu_flat::on_host, lgpu_binary::on_host): its rows cross PCIe in chunks of C rows, copied into the
-// workspace's two staging buffers on its side stream (Workspace::stage), chunk i + 1 while chunk i is scored on the
-// call's stream by the route an HBM handle of that chunk's rows takes.  Each chunk's exact top-k is merged into a
-// running top-k per query by (distance, id).  Chunks are the outer loop: a pass over the column serves P queries, all B
-// unless the budget cannot hold the running top-k of that many, in scoring groups of bs queries whose scores fit.  The
-// staging buffers, the chunk's per-row terms and the running lists all count against the workspace budget.  timeout_ms
-// is checked between chunks.
+// The dense search of a flat or binary handle (stream_topk) reads its rows in chunks of C rows.  An HBM store is one
+// resident chunk of all N rows, the queries in passes of P = bs that the budget holds the scores of.  A host store's
+// chunks cross PCIe, copied into the workspace's two staging buffers on its side stream (RowStore::walk), chunk i + 1
+// while chunk i is scored on the call's stream by the route an HBM handle of that chunk's rows takes.  Each chunk's
+// exact top-k is merged into a running top-k per query by (distance, id).  Chunks are the outer loop: a pass over the
+// column serves P queries, all B unless the budget cannot hold the running top-k of that many, in scoring groups of bs
+// queries whose scores fit.  The staging buffers, the chunk's per-row terms and the running lists all count against
+// the workspace budget.  timeout_ms is checked between chunks, and between the passes of an HBM store.
 struct StreamShape {
     uint64_t C, nchunks;                // rows per chunk, chunks of the column
     uint32_t P, bs;                     // queries per pass, per scoring group
 };
-// row_b: workspace bytes per row of a chunk (its two staging copies and its per-row terms); row_bytes: the bytes of one
-// stored row (a chunk stages at most FLAT_STAGE_BYTES of them).  A scoring group holds each query's [ldc] f32 scores.
-static StreamShape stream_shape(uint64_t N, size_t row_b, size_t row_bytes, uint32_t B, uint32_t k)
+// row_b: workspace bytes per row of a staged chunk (its two staging copies and its per-row terms); row_bytes: the bytes
+// of one stored row (a chunk stages at most FLAT_STAGE_BYTES of them).  A scoring group holds each query's [ldc] f32
+// scores.
+static StreamShape stream_shape(const RowStore &rows, uint64_t N, size_t row_b, size_t row_bytes, uint32_t B,
+                                uint32_t k)
 {
     const size_t budget = workspace_budget();
     StreamShape s;
+    if (!rows.on_host) {
+        const uint64_t ld = (N + 3) & ~3ull;
+        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
+        s.C = std::max<uint64_t>(N, 1);
+        s.nchunks = 1;
+        s.P = s.bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / per_q, B));
+        return s;
+    }
     s.C = std::max<uint64_t>(1, std::min<uint64_t>(std::max<uint64_t>(N, 1),
                                                    std::min(budget / 2 / row_b, FLAT_STAGE_BYTES / row_bytes)));
     const uint64_t ldc = (s.C + 3) & ~3ull;
@@ -1864,68 +1948,83 @@ struct RunningTopk {
     }
 };
 
-// The chunk loop of a host handle's search: `rows` [N][row_bytes] pinned, in chunks and passes of shape sh.
-// score(X, c, n, p0, pb, dst) enqueues on the call's stream the k best of chunk c -- its n rows staged at X, ids from
-// position c C -- for the pb queries p0, p0 + 1, ... into dst ([pb][k], [pb]).
+// The dense search of a flat or binary handle: its rows, N of row_bytes each, in chunks and passes of shape sh
+// (stream_shape).  score(ch, p0, pb, dst) enqueues on the call's stream the k best of chunk ch (RowChunk) for the pb
+// queries p0, p0 + 1, ... into dst ([pb][k], [pb]).
 template <class Score>
-static void stream_topk(Workspace *ws, cudaStream_t st, const void *rows, size_t row_bytes, uint64_t N,
+static void stream_topk(const RowStore &rows, Workspace *ws, cudaStream_t st, size_t row_bytes, uint64_t N,
                         const StreamShape &sh, uint32_t B, uint32_t k, TopkOut out, const Deadline *deadline,
                         Score &&score)
 {
-    const uint64_t C = sh.C, nchunks = sh.nchunks;
+    const uint64_t nchunks = sh.nchunks;
     const uint32_t P = sh.P;
-    for (auto &b : ws->stage.buf) b.ensure(std::max<size_t>(C * row_bytes, 16));
+    rows.reserve_stage(ws, std::max<size_t>(sh.C * row_bytes, 16));
     RunningTopk::reserve(ws, nchunks, P, k);
-    const char *base = static_cast<const char *>(rows);
-    const uint64_t steps = (uint64_t)((B + P - 1) / P) * nchunks;      // step s: pass s / nchunks, chunk s % nchunks
-    auto chunk_rows = [&](uint64_t c) { return N ? std::min<uint64_t>(C, N - c * C) : 0; };
-    ws->stage.open(ws, st, steps, deadline, [&](uint64_t s) -> std::pair<const void *, size_t> {
-        const uint64_t c = s % nchunks;
-        return {base + c * C * row_bytes, chunk_rows(c) * row_bytes};
-    });
-    for (uint64_t s = 0; s < steps; s++) {
-        const uint32_t p0 = (uint32_t)(s / nchunks) * P, pb = std::min(P, B - p0);
-        const uint64_t c = s % nchunks;
-        const void *X = ws->stage.take(s);
-        const RunningTopk run{ws, nchunks, pb, k, out.at(p0, k)};
-        score(X, c, chunk_rows(c), p0, pb, run.dst(c));
-        // released before the merge, so that the next copy does not wait for it
-        ws->stage.release(s);
-        run.merge(c, st);
-    }
-    ws->stage.close();
+    // step s: pass s / nchunks, chunk s % nchunks
+    auto run = [&](uint64_t s) {
+        const uint32_t p0 = (uint32_t)(s / nchunks) * P;
+        return RunningTopk{ws, nchunks, std::min(P, B - p0), k, out.at(p0, k)};
+    };
+    rows.walk(ws, st, uniform_cuts(N, sh.C), (B + P - 1) / P, [&](uint64_t r) { return r * row_bytes; }, deadline,
+              [&](const RowChunk &ch) {
+                  const RunningTopk r = run(ch.s);
+                  score(ch, (uint32_t)(ch.s / nchunks) * P, r.pb, r.dst(ch.s % nchunks));
+              },
+              // after the chunk's staging buffer is released, so that the next copy does not wait for the merge
+              [&](uint64_t s) { run(s).merge(s % nchunks, st); });
 }
 
-// a host flat handle through stream_topk, each chunk scored by flat_score
+// |x| of the rows X of an HBM flat handle, built by its first cosine search
+template <class T> static void flat_norms(lgpu_flat *fl, const T *X, cudaStream_t st)
+{
+    std::lock_guard<std::mutex> g(fl->mu);
+    if (fl->has_norms) return;
+    fl->ysqrt.ensure(std::max<size_t>(fl->nrows, 1) * 4, true);
+    launch_row_norms(X, fl->nrows, fl->dim, fl->ysqrt.as<float>(), st);
+    LGPU_CUDA(cudaStreamSynchronize(st));
+    fl->has_norms = true;
+}
+
+// stream_topk, each chunk scored by flat_score: a resident chunk with the handle's per-row terms, a staged chunk with
+// its terms built into the workspace
 template <class T>
-static void flat_search_streamed(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *d_q,
-                                 uint32_t B, const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist,
-                                 uint32_t *d_cnt, RowFilter rf, const Deadline *deadline)
+static void flat_search(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric, const float *d_q, uint32_t B,
+                        const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt, RowFilter rf,
+                        const Deadline *deadline)
 {
     const uint32_t d = fl->dim, k = sp.k;
     const size_t es = sizeof(T);
-    // per row of a chunk: two staging copies, the bf16 operand (f32 rows), |x|^2 and |x|
+    // per row of a staged chunk: two staging copies, the bf16 operand (f32 rows), |x|^2 and |x|
     const size_t row_b = 2 * (size_t)d * es + (fl->f16 ? 0 : 2 * (size_t)d) + 8;
-    const StreamShape sh = stream_shape(fl->nrows, row_b, (size_t)d * es, B, k);
-    const uint64_t C = sh.C;
-    if (fl->has_tc && !fl->f16) ws->chunk_xb.ensure(C * d * 2);
-    ws->chunk_n2.ensure(C * 4);
-    if (metric == LGPU_COSINE) ws->chunk_ysqrt.ensure(C * 4);
+    const StreamShape sh = stream_shape(fl->rows, fl->nrows, row_b, (size_t)d * es, B, k);
+    if (fl->rows.on_host) {
+        if (fl->has_tc && !fl->f16) ws->chunk_xb.ensure(sh.C * d * 2);
+        ws->chunk_n2.ensure(sh.C * 4);
+        if (metric == LGPU_COSINE) ws->chunk_ysqrt.ensure(sh.C * 4);
+    }
     const bool prof = profiling_enabled();
     if (prof) memset(g_filter_stats, 0, sizeof(g_filter_stats));      // [1] tensor-core distances, [3] queries
-    stream_topk(ws, st, fl->rows_host.p, (size_t)d * es, fl->nrows, sh, B, k, TopkOut{d_ids, d_dist, d_cnt}, deadline,
-                [&](const void *Xv, uint64_t c, uint64_t n, uint32_t p0, uint32_t pb, TopkOut dst) {
-        const T *X = static_cast<const T *>(Xv);
-        // the operand only when a scoring group takes the tensor cores (the first group is the largest)
-        const bool tc = flat_tc_route(fl->has_tc, metric, sp, std::min(sh.bs, pb), n);
-        if (tc && fl->f16) launch_f16_row_terms(X, n, d, ws->chunk_n2.as<float>(), nullptr, st);
-        else if (tc) launch_to_bf16(reinterpret_cast<const float *>(X), n, d, ws->chunk_xb.p, ws->chunk_n2.as<float>(), st);
-        if (metric == LGPU_COSINE) launch_row_norms(X, n, d, ws->chunk_ysqrt.as<float>(), st);
-        const FlatRows<T> chunk{X, fl->f16 ? static_cast<const void *>(X) : ws->chunk_xb.p, ws->chunk_n2.as<float>(),
-                                ws->chunk_ysqrt.as<float>(), n,
-                                fl->has_ids ? Cols(fl->row_ids.as<uint64_t>() + c * C) : Cols(nullptr, c * C), tc};
+    stream_topk(fl->rows, ws, st, (size_t)d * es, fl->nrows, sh, B, k, TopkOut{d_ids, d_dist, d_cnt}, deadline,
+                [&](const RowChunk &ch, uint32_t p0, uint32_t pb, TopkOut dst) {
+        const T *X = static_cast<const T *>(ch.X);
+        const uint64_t n = ch.r1 - ch.r0;
+        FlatRows<T> rows{X, fl->f16 ? static_cast<const void *>(X) : fl->vec_b.p, fl->vec_n2.as<float>(), nullptr, n,
+                         row_cols(fl, ch.r0), fl->has_tc};
+        if (ch.resident) {
+            if (metric == LGPU_COSINE) flat_norms(fl, X, st);
+            rows.ysqrt = fl->ysqrt.as<float>();
+        } else {
+            // the operand only when a scoring group takes the tensor cores (the first group is the largest)
+            rows.tc = flat_tc_route(fl->has_tc, metric, sp, std::min(sh.bs, pb), n);
+            if (rows.tc && fl->f16) launch_f16_row_terms(X, n, d, ws->chunk_n2.as<float>(), nullptr, st);
+            else if (rows.tc) launch_to_bf16(reinterpret_cast<const float *>(X), n, d, ws->chunk_xb.p, ws->chunk_n2.as<float>(), st);
+            if (metric == LGPU_COSINE) launch_row_norms(X, n, d, ws->chunk_ysqrt.as<float>(), st);
+            if (!fl->f16) rows.Xop = ws->chunk_xb.p;
+            rows.n2 = ws->chunk_n2.as<float>();
+            rows.ysqrt = ws->chunk_ysqrt.as<float>();
+        }
         for (uint32_t g0 = 0; g0 < pb; g0 += sh.bs)
-            flat_score(fl, ws, st, metric, d_q + (size_t)(p0 + g0) * d, std::min(sh.bs, pb - g0), sp, chunk,
+            flat_score(fl, ws, st, metric, d_q + (size_t)(p0 + g0) * d, std::min(sh.bs, pb - g0), sp, rows,
                        dst.at(g0, k), rf, prof);
     });
     if (prof) g_filter_stats[3] = B;
@@ -1935,14 +2034,8 @@ void flat_search_device(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metri
                         const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                         RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
 {
-    if (fl->on_host && fl->f16)
-        flat_search_streamed<__half>(fl, ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
-    else if (fl->on_host)
-        flat_search_streamed<float>(fl, ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
-    else if (fl->f16)
-        flat_search_rows(fl, fl->vectors.as<__half>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
-    else
-        flat_search_rows(fl, fl->vectors.as<float>(), ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    if (fl->f16) flat_search<__half>(fl, ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
+    else flat_search<float>(fl, ws, st, metric, d_q, B, sp, d_ids, d_dist, d_cnt, rf, deadline);
 }
 
 // ---- binary vectors (Hamming distance) ----
@@ -1980,12 +2073,11 @@ static void ham_sample(lgpu_binary *bx, uint64_t nrows)
     bx->sample_pop.ensure((size_t)HAM_SAMPLE * 4);
     bx->sample_ids.ensure((size_t)HAM_SAMPLE * 8);
     DevBuf gathered;
-    const uint8_t *src = bx->vectors.as<uint8_t>();
+    const uint8_t *src = reinterpret_cast<const uint8_t *>(bx->rows.data());
     uint64_t src_stride = stride * nbp;
-    if (bx->on_host) {
+    if (bx->rows.on_host) {
         std::vector<uint8_t> h((size_t)HAM_SAMPLE * nbp);
-        const uint8_t *rows = static_cast<const uint8_t *>(bx->rows_host.p);
-        for (uint64_t s = 0; s < HAM_SAMPLE; s++) memcpy(h.data() + s * nbp, rows + s * stride * nbp, nbp);
+        for (uint64_t s = 0; s < HAM_SAMPLE; s++) memcpy(h.data() + s * nbp, src + s * stride * nbp, nbp);
         gathered.ensure(h.size());
         LGPU_CUDA(cudaMemcpy(gathered.p, h.data(), h.size(), cudaMemcpyHostToDevice));
         src = gathered.as<uint8_t>();
@@ -2004,10 +2096,8 @@ static void ham_sample(lgpu_binary *bx, uint64_t nrows)
 }
 
 // The list path of one sub-batch (Q: padded queries [B][nbytes_pad], qpop [B]) over the rows that pass the row filter rf
-// (none: every row), in four steps: the threshold (ham_list_threshold), the filtering pass over every row into the
-// candidate lists, their top-k (ham_list_select), the dense fix-up of the queries whose list overflowed.  An HBM handle
-// runs the filtering pass as one GEMM (ham_topk_list), a host handle as one per staged chunk appending to the same
-// lists (ham_topk_list_streamed).
+// (none: every row), in four steps (ham_topk_list): the threshold (ham_list_threshold), the filtering pass over every
+// row into the candidate lists, their top-k (ham_list_select), the dense fix-up of the queries whose list overflowed.
 // 1. sample pass: exact distances to the sample rows, tau_q = the k-th smallest over the allowed ones (an upper bound of
 // the true k-th over all rows; +inf with fewer than k).  Then the candidate counters are zeroed, and the filter of the
 // filtering pass is returned: every allowed row with d <= tau_q is appended as (position, id, distance); the distance
@@ -2026,7 +2116,7 @@ static GemmFilter ham_list_threshold(lgpu_binary *bx, Workspace *ws, cudaStream_
     LGPU_CUDA(cudaMemsetAsync(ws->amax.p, 0, (size_t)B * 4, st));
     GemmFilter flt{};
     flt.thr = ws->probe_A.as<float>(); flt.count = ws->amax.as<uint32_t>(); flt.cand_pos = ws->t_pos.as<uint64_t>();
-    flt.cand_ids = ws->t_ids.as<uint64_t>(); flt.col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    flt.cand_ids = ws->t_ids.as<uint64_t>();
     flt.cap = cap; flt.cand_s = ws->t_exact.as<float>();
     flt.allow = rf.bits; flt.allow_bits = rf.nbits;
     return flt;
@@ -2042,83 +2132,68 @@ static void ham_list_select(Workspace *ws, cudaStream_t st, uint32_t B, uint32_t
     launch_select(sb, st);
 }
 
-// An HBM handle.  The dense fix-up of overflowed queries runs in chunks of `bf` queries over a [bf][N] matrix: one
-// launch lists each chunk's flagged queries, and each chunk's two launches return at once when its list is empty.
+// The list path of one sub-batch (above).  The one threshold tau_q bounds the k-th distance over every row, so the
+// filtering GEMM runs over each chunk of the row store's walk (chunks of C rows: an HBM store's one resident chunk
+// with its stored popcounts, a host store's staged chunks with theirs computed on the device, ids from the chunk's
+// first row) into the sub-batch's candidate lists, whose counts add up across chunks: each row crosses PCIe once and
+// the lists need no merge.  The dense fix-up of the overflowed queries differs by placement.  An HBM store: chunks of
+// `bf` queries over a [bf][N] matrix; one launch lists each chunk's flagged queries, and each chunk's two launches
+// return at once when its list is empty.  A host store: one list of all B flagged queries (its count gates every
+// launch below), then per chunk a gated copy of its rows out of the mapped pinned memory into staging buffer 0, the
+// dense Hamming scores of the flagged queries ([B][C] matrix) and their top-k, merged into a running top-k of the
+// flagged queries; with nothing flagged each launch returns at once, and nothing waits on the host.
 static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
-                          uint32_t B, uint32_t k, uint32_t cap, uint32_t bf, TopkOut out, RowFilter rf)
+                          uint32_t B, uint32_t k, uint32_t cap, uint64_t C, uint32_t bf, TopkOut out, RowFilter rf,
+                          const Deadline *deadline)
 {
-    const uint64_t N = bx->nrows, ld = (N + 3) & ~3ull;
+    const uint64_t N = bx->nrows;
     const uint32_t nbp = bx->nbytes_pad;
-    const uint64_t *col_ids = bx->has_ids ? bx->row_ids.as<uint64_t>() : nullptr;
+    const std::vector<uint64_t> cut = uniform_cuts(N, C);
     // 1, 2. threshold, filtering pass
-    const GemmFilter flt = ham_list_threshold(bx, ws, st, Q, qpop, B, k, cap, rf);
-    launch_ham_gemm(Q, bx->vectors.p, bx->pop.as<uint32_t>(), qpop, B, N, nbp, nullptr, 0, bx->num_sms, st, &flt);
-    // 3. top-k of the lists
-    ham_list_select(ws, st, B, k, cap, out);
-    // 4. dense fix-up of the overflowed queries only
-    launch_ham_flag_list(ws->flags.as<uint32_t>(), B, bf, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
-    for (uint32_t q0 = 0, c = 0; q0 < B; q0 += bf, c++) {
-        const uint32_t b = std::min(bf, B - q0);
-        launch_ham_dense(Q + (size_t)q0 * nbp, bx->vectors.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld, bx->num_sms, st,
-                         ws->h_list.as<uint32_t>() + q0, ws->h_cnt.as<uint32_t>() + c);
-        SelectArgs sc = select_rows(ws->D.as<float>(), N, ld, b, k, out.at(q0, k));
-        sc.col_ids = col_ids; sc.only = ws->flags.as<uint32_t>() + q0; sc.gate = ws->h_cnt.as<uint32_t>() + c;
-        sc.allow = rf.bits; sc.allow_bits = rf.nbits;
-        launch_select(sc, st);
-    }
-}
-
-// the ids of rows [r0, ..) of a binary handle: its explicit ids from r0, or the positions from r0
-static Cols ham_cols(lgpu_binary *bx, uint64_t r0)
-{
-    return bx->has_ids ? Cols(bx->row_ids.as<uint64_t>() + r0) : Cols(nullptr, r0);
-}
-
-// A host handle, chunks of C rows.  The one threshold tau_q bounds the k-th distance over every row, so each staged
-// chunk runs the filtering GEMM (its popcounts computed on the device, ids from its first row) into the sub-batch's
-// candidate lists, whose counts add up across chunks: each row crosses PCIe once and the lists need no merge.  The
-// fix-up: one list of all B flagged queries (its count gates every launch below), then per chunk a gated copy of its
-// rows out of the mapped pinned memory into staging buffer 0, the dense Hamming scores of the flagged queries
-// ([B][C] matrix) and their top-k, merged into a running top-k of the flagged queries; with nothing flagged each launch
-// returns at once, and nothing waits on the host.
-static void ham_topk_list_streamed(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q,
-                                   const uint32_t *qpop, uint32_t B, uint32_t k, uint32_t cap, uint64_t C, TopkOut out,
-                                   RowFilter rf, const Deadline *deadline)
-{
-    const uint64_t N = bx->nrows, nchunks = (N + C - 1) / C, ldc = (C + 3) & ~3ull;
-    const uint32_t nbp = bx->nbytes_pad;
-    auto chunk_rows = [&](uint64_t c) { return std::min<uint64_t>(C, N - c * C); };
-    const char *rows = static_cast<const char *>(bx->rows_host.p);
-    // 1, 2. threshold, filtering pass per chunk
     GemmFilter flt = ham_list_threshold(bx, ws, st, Q, qpop, B, k, cap, rf);
-    ws->stage.open(ws, st, nchunks, deadline, [&](uint64_t c) -> std::pair<const void *, size_t> {
-        return {rows + c * C * nbp, chunk_rows(c) * nbp};
-    });
-    for (uint64_t c = 0; c < nchunks; c++) {
-        const uint64_t n = chunk_rows(c);
-        const void *X = ws->stage.take(c);
-        launch_ham_pack(static_cast<const uint8_t *>(X), nbp, nbp, n, nullptr, nbp, ws->chunk_pop.as<uint32_t>(), st);
-        const Cols cols = ham_cols(bx, c * C);
+    bx->rows.walk(ws, st, cut, [&](uint64_t r) { return r * nbp; }, deadline, [&](const RowChunk &ch) {
+        const uint64_t n = ch.r1 - ch.r0;
+        const uint32_t *xpop = bx->pop.as<uint32_t>();
+        if (!ch.resident) {
+            launch_ham_pack(static_cast<const uint8_t *>(ch.X), nbp, nbp, n, nullptr, nbp, ws->chunk_pop.as<uint32_t>(),
+                            st);
+            xpop = ws->chunk_pop.as<uint32_t>();
+        }
+        const Cols cols = row_cols(bx, ch.r0);
         flt.col_ids = cols.ids; flt.col_base = cols.base;
-        launch_ham_gemm(Q, X, ws->chunk_pop.as<uint32_t>(), qpop, B, n, nbp, nullptr, 0, bx->num_sms, st, &flt);
-        ws->stage.release(c);
-    }
-    ws->stage.close();
+        launch_ham_gemm(Q, ch.X, xpop, qpop, B, n, nbp, nullptr, 0, bx->num_sms, st, &flt);
+    });
     // 3. top-k of the lists
     ham_list_select(ws, st, B, k, cap, out);
     // 4. dense fix-up of the overflowed queries only
+    if (!bx->rows.on_host) {
+        const uint64_t ld = (N + 3) & ~3ull;
+        launch_ham_flag_list(ws->flags.as<uint32_t>(), B, bf, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
+        for (uint32_t q0 = 0, c = 0; q0 < B; q0 += bf, c++) {
+            const uint32_t b = std::min(bf, B - q0);
+            launch_ham_dense(Q + (size_t)q0 * nbp, bx->rows.hbm.as<uint8_t>(), b, N, nbp, ws->D.as<float>(), ld,
+                             bx->num_sms, st, ws->h_list.as<uint32_t>() + q0, ws->h_cnt.as<uint32_t>() + c);
+            SelectArgs sc = select_rows(ws->D.as<float>(), N, ld, b, k, out.at(q0, k));
+            sc.col_ids = row_cols(bx, 0).ids; sc.only = ws->flags.as<uint32_t>() + q0;
+            sc.gate = ws->h_cnt.as<uint32_t>() + c;
+            sc.allow = rf.bits; sc.allow_bits = rf.nbits;
+            launch_select(sc, st);
+        }
+        return;
+    }
+    const uint64_t ldc = (C + 3) & ~3ull;
     launch_ham_flag_list(ws->flags.as<uint32_t>(), B, B, ws->h_list.as<uint32_t>(), ws->h_cnt.as<uint32_t>(), st);
     const uint32_t *gate = ws->h_cnt.as<uint32_t>();
-    RunningTopk run{ws, nchunks, B, k, out};
+    RunningTopk run{ws, cut.size() - 1, B, k, out};
     run.only = ws->flags.as<uint32_t>(); run.gate = gate;
-    const uint8_t *mapped = static_cast<const uint8_t *>(bx->rows_host.dev);
-    for (uint64_t c = 0; c < nchunks; c++) {
-        const uint64_t n = chunk_rows(c);
-        launch_mv_copy_gated(mapped + c * C * nbp, ws->stage.buf[0].as<uint8_t>(), n * nbp, gate, bx->num_sms, st);
+    const uint8_t *mapped = static_cast<const uint8_t *>(bx->rows.dev());
+    for (uint64_t c = 0; c + 1 < cut.size(); c++) {
+        const uint64_t n = cut[c + 1] - cut[c];
+        launch_mv_copy_gated(mapped + cut[c] * nbp, ws->stage.buf[0].as<uint8_t>(), n * nbp, gate, bx->num_sms, st);
         launch_ham_dense(Q, ws->stage.buf[0].as<uint8_t>(), B, n, nbp, ws->D.as<float>(), ldc, bx->num_sms, st,
                          ws->h_list.as<uint32_t>(), gate);
         SelectArgs sc = select_rows(ws->D.as<float>(), n, ldc, B, k, run.dst(c));
-        with_cols(sc, ham_cols(bx, c * C));
+        with_cols(sc, row_cols(bx, cut[c]));
         sc.only = run.only; sc.gate = gate;
         sc.allow = rf.bits; sc.allow_bits = rf.nbits;
         launch_select(sc, st);
@@ -2140,9 +2215,9 @@ static void ham_dense_topk(lgpu_binary *bx, Workspace *ws, cudaStream_t st, cons
     select_dense(ws, ws->D.as<float>(), N, ld, cols, b, sp, rf, out, st);
 }
 
-// d_q: raw queries [B][nbytes] in device memory.  A host handle (lgpu_binary::on_host) takes the same route as an HBM
-// handle of its rows, its rows streamed: the list route through ham_topk_list_streamed, the dense routes through
-// stream_topk, each chunk scored as an HBM handle of the chunk's rows would score it.
+// d_q: raw queries [B][nbytes] in device memory.  Both placements take the same route: the list route through
+// ham_topk_list, the dense routes through stream_topk, each staged chunk scored as an HBM handle of the chunk's rows
+// would score it.
 void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *d_q, uint32_t B,
                           const lgpu_search_params &sp, uint64_t *d_ids, float *d_dist, uint32_t *d_cnt,
                           RowFilter rf = RowFilter(), const Deadline *deadline = nullptr)
@@ -2173,8 +2248,8 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         const uint32_t cap = ham_list_cap(k, N, ns);
         const size_t per_q0 = lds * 4 + (size_t)cap * 20 + (size_t)k * 12 + 16;
         uint32_t bf = 0, bs = 0;
-        uint64_t C = 0;
-        if (bx->on_host) {
+        uint64_t C = N;
+        if (bx->rows.on_host) {
             const size_t row_b = 2 * (size_t)nbp + 4;
             C = std::max<uint64_t>(1, std::min<uint64_t>(N, std::min(budget / 2 / row_b, FLAT_STAGE_BYTES / nbp)));
             const uint64_t ldc = (C + 3) & ~3ull;
@@ -2201,11 +2276,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
         for (uint32_t q0 = 0; q0 < B; q0 += bs) {
             const uint32_t b = std::min(bs, B - q0);
             if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-            if (bx->on_host)
-                ham_topk_list_streamed(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, k, cap, C, out.at(q0, k), rf,
-                                       deadline);
-            else
-                ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, k, cap, bf, out.at(q0, k), rf);
+            ham_topk_list(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, k, cap, C, bf, out.at(q0, k), rf, deadline);
             if (prof) {             // [0] list appends, [2] queries redone densely (over every sub-batch)
                 std::vector<uint32_t> cnt(b), fl(b);
                 LGPU_CUDA(cudaMemcpyAsync(cnt.data(), ws->amax.p, (size_t)b * 4, cudaMemcpyDeviceToHost, st));
@@ -2215,35 +2286,34 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
             }
         }
         tc_dists = (uint64_t)B * (N + ns);
-    } else if (bx->on_host) {
-        // per row of a chunk: two staging copies and its popcount
-        const StreamShape sh = stream_shape(N, 2 * (size_t)nbp + 4, nbp, B, k);
-        ws->chunk_pop.ensure(sh.C * 4);
-        stream_topk(ws, st, bx->rows_host.p, nbp, N, sh, B, k, out, deadline,
-                    [&](const void *Xv, uint64_t c, uint64_t n, uint32_t p0, uint32_t pb, TopkOut dst) {
-            const uint8_t *X = static_cast<const uint8_t *>(Xv);
-            auto group_tc = [&](uint32_t b) { return tc_ok && b >= HAM_TC_MIN_B && n >= HAM_TC_MIN_N; };
-            // the popcounts only when a scoring group takes the tensor cores (the first group is the largest)
-            if (group_tc(std::min(sh.bs, pb)))
-                launch_ham_pack(X, nbp, nbp, n, nullptr, nbp, ws->chunk_pop.as<uint32_t>(), st);
+    } else {
+        // per row of a staged chunk: two staging copies and its popcount
+        const StreamShape sh = stream_shape(bx->rows, N, 2 * (size_t)nbp + 4, nbp, B, k);
+        if (bx->rows.on_host) ws->chunk_pop.ensure(sh.C * 4);
+        stream_topk(bx->rows, ws, st, nbp, N, sh, B, k, out, deadline,
+                    [&](const RowChunk &ch, uint32_t p0, uint32_t pb, TopkOut dst) {
+            const uint8_t *X = static_cast<const uint8_t *>(ch.X);
+            const uint64_t n = ch.r1 - ch.r0;
+            // The two placements choose the tensor cores differently: the resident chunk from the call's B (tc), a
+            // staged chunk per scoring group.  Both choices are kept as they are; making them agree changes which
+            // kernels a call launches.
+            auto group_tc = [&](uint32_t b) {
+                return ch.resident ? tc : tc_ok && b >= HAM_TC_MIN_B && n >= HAM_TC_MIN_N;
+            };
+            const uint32_t *xpop = bx->pop.as<uint32_t>();
+            if (!ch.resident) {
+                // the popcounts only when a scoring group takes the tensor cores (the first group is the largest)
+                if (group_tc(std::min(sh.bs, pb)))
+                    launch_ham_pack(X, nbp, nbp, n, nullptr, nbp, ws->chunk_pop.as<uint32_t>(), st);
+                xpop = ws->chunk_pop.as<uint32_t>();
+            }
             for (uint32_t g0 = 0; g0 < pb; g0 += sh.bs) {
                 const uint32_t b = std::min(sh.bs, pb - g0);
-                ham_dense_topk(bx, ws, st, Q + (size_t)(p0 + g0) * nbp, qpop + p0 + g0, b, X,
-                               ws->chunk_pop.as<uint32_t>(), n, ham_cols(bx, c * sh.C), group_tc(b), sp, rf,
-                               dst.at(g0, k));
+                ham_dense_topk(bx, ws, st, Q + (size_t)(p0 + g0) * nbp, qpop + p0 + g0, b, X, xpop, n,
+                               row_cols(bx, ch.r0), group_tc(b), sp, rf, dst.at(g0, k));
                 if (group_tc(b)) tc_dists += (uint64_t)b * n;
             }
         });
-    } else {
-        const size_t per_q = std::max<size_t>(ld * 4, 4) + large_k_query_bytes(k);
-        const uint32_t bs = (uint32_t)std::max<size_t>(1, std::min<size_t>(budget / per_q, B));
-        for (uint32_t q0 = 0; q0 < B; q0 += bs) {
-            const uint32_t b = std::min(bs, B - q0);
-            if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);
-            ham_dense_topk(bx, ws, st, Q + (size_t)q0 * nbp, qpop + q0, b, bx->vectors.as<uint8_t>(),
-                           bx->pop.as<uint32_t>(), N, ham_cols(bx, 0), tc, sp, rf, out.at(q0, k));
-        }
-        if (tc) tc_dists = (uint64_t)B * N;
     }
     if (prof) {                     // [1] distances computed on the tensor cores, [3] queries
         LGPU_CUDA(cudaStreamSynchronize(st));
@@ -2322,7 +2392,7 @@ static void mv_exact_dense(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, co
     }
 }
 
-// ---- a host multivector handle (lgpu_multivec::on_host): its row data crosses PCIe in chunks of whole rows ----
+// ---- a host multivector handle (RowStore::on_host): its row data crosses PCIe in chunks of whole rows ----
 // The bytes of one staging buffer: FLAT_STAGE_BYTES, or an eighth of the budget when that is smaller, and never less
 // than the longest row's vectors in the row type.  Two such buffers must fit the budget (mv_check_stage, before any
 // device work).
@@ -2337,7 +2407,7 @@ static size_t mv_stage_bytes(const lgpu_multivec *mv)
 static void mv_check_stage(const lgpu_multivec *mv)
 {
     const size_t longest = (size_t)mv->max_row * mv->dim * mv_elem_bytes(mv);
-    if (mv->on_host && 2 * longest > workspace_budget()) {
+    if (mv->rows.on_host && 2 * longest > workspace_budget()) {
         set_error("a multivector row of " + std::to_string(mv->max_row) + " vectors (" + std::to_string(longest) +
                   " bytes) does not fit twice in the workspace budget (LGPU_WS_BYTES) that streams a host handle");
         throw Failure{LGPU_OOM};
@@ -2389,23 +2459,11 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
     const size_t quarter = budget / 4;
     const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper && k <= SELECT_KMAX &&
                     (size_t)(max_nq + 1) * ld * 4 <= quarter;
-    const size_t S = mv->on_host ? mv_stage_bytes(mv) : 0, left = budget / 2 > 2 * S ? budget / 2 - 2 * S : 0;
-    if (mv->on_host)
-        for (auto &b : ws->stage.buf) b.ensure(S);
-    // the chunks of a copy of the vectors at `vb` bytes each
-    auto chunks = [&](size_t vb) { return mv->on_host ? mv_chunks(mv, S / (dim * vb)) : std::vector<uint64_t>{0, N}; };
-    // use(ra, rb, X) for each chunk of `cut`, X its vectors: in `hbm`, or copied from `host`
-    auto each_chunk = [&](const std::vector<uint64_t> &cut, const void *hbm, const void *host, size_t vb, auto &&use) {
-        if (!mv->on_host) { use(cut[0], cut[1], hbm); return; }
-        ws->stage.open(ws, st, cut.size() - 1, deadline, [&](uint64_t c) -> std::pair<const void *, size_t> {
-            return {static_cast<const char *>(host) + off[cut[c]] * vb, (off[cut[c + 1]] - off[cut[c]]) * vb};
-        });
-        for (size_t c = 0; c + 1 < cut.size(); c++) {
-            use(cut[c], cut[c + 1], ws->stage.take(c));
-            ws->stage.release(c);
-        }
-        ws->stage.close();
-    };
+    const size_t S = mv->rows.on_host ? mv_stage_bytes(mv) : 0, left = budget / 2 > 2 * S ? budget / 2 - 2 * S : 0;
+    mv->rows.reserve_stage(ws, S);
+    // the chunks of a copy of the vectors at `vb` bytes each, and the byte of each row's first vector in it
+    auto chunks = [&](size_t vb) { return S ? mv_chunks(mv, S / (dim * vb)) : std::vector<uint64_t>{0, N}; };
+    auto at = [&](size_t vb) { return [&, vb](uint64_t r) { return off[r] * vb; }; };
     const size_t es = mv_elem_bytes(mv);
     const std::vector<uint64_t> cutv = chunks(es);                  // chunks of the vectors in the row type
     if (!tc) {
@@ -2415,8 +2473,8 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             const uint32_t qb = std::min(B, qa + bs), b = qb - qa;
             if (deadline && qa > 0) deadline->wait(st, ws->ev[7]);
             ws->D.ensure(std::max<size_t>((size_t)b * ld, 4) * 4);
-            each_chunk(cutv, mv->vectors.p, mv->vectors_host.p, (size_t)dim * es, [&](uint64_t ra, uint64_t rb, const void *X) {
-                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, X, ra, rb);
+            mv->rows.walk(ws, st, cutv, at((size_t)dim * es), deadline, [&](const RowChunk &ch) {
+                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, ws->D.as<float>(), ld, ch.X, ch.r0, ch.r1);
             });
             select_dense(ws, ws->D.as<float>(), N, ld, ids, b, sp, rf, out.at(qa, k), st);
         }
@@ -2438,11 +2496,10 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
         const size_t per_q = ld * 4 + (size_t)k * 12 + (size_t)cap * 16 + 32, per_v = ldR * 4 + 4;
         auto fits = [&](uint32_t qa, uint32_t qb) {
             const size_t nq = qb + 1 - qa, nv = h_qoff[qb + 1] - h_qoff[qa];
-            return mv->on_host ? nq * per_q + nv * per_v <= left : nv * ld * 4 <= quarter && nq * ld * 4 <= quarter;
+            return mv->rows.on_host ? nq * per_q + nv * per_v <= left : nv * ld * 4 <= quarter && nq * ld * 4 <= quarter;
         };
-        const void *V = mv->on_host ? mv->vectors_host.dev : mv->vectors.p;        // the vectors, for the re-score
-        const void *Xop = mv->f16 ? mv->vectors.p : mv->vec_h.p;                  // the operand, in HBM
-        const void *Xop_host = mv->f16 ? mv->vectors_host.p : mv->vec_h_host.p;   // ... or pinned
+        const void *V = mv->rows.dev();                                 // the vectors, for the re-score
+        const RowStore &op = mv->f16 ? mv->rows : mv->ops;             // the operand
         for (uint32_t qa = 0; qa < B;) {
             uint32_t qb = qa + 1;
             while (qb < B && fits(qa, qb)) qb++;
@@ -2455,13 +2512,13 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             ws->mv_flags.ensure((size_t)b * 4); ws->mv_vflags.ensure((size_t)nqv * 4); ws->mv_gate.ensure(16);
             ws->mv_ex.ensure((size_t)b * cap * 4); ws->mv_exid.ensure((size_t)b * cap * 8);
             float *A = ws->mv_A.as<float>();
-            each_chunk(cut16, Xop, Xop_host, (size_t)dim * 2, [&](uint64_t ra, uint64_t rb, const void *Xh) {
-                const uint64_t span = off[rb] - off[ra], ldc = (rb - ra + 3) & ~3ull;
+            op.walk(ws, st, cut16, at((size_t)dim * 2), deadline, [&](const RowChunk &ch) {
+                const uint64_t ra = ch.r0, rb = ch.r1, span = off[rb] - off[ra], ldc = (rb - ra + 3) & ~3ull;
                 LGPU_CUDA(cudaMemsetAsync(ws->mv_Mk.p, 0, (size_t)nqv * ldc * 4, st));
                 MaxSimOut mo{};
                 mo.col_row = mv->col_row.as<uint32_t>() + off[ra]; mo.M = ws->mv_Mk.as<uint32_t>(); mo.ldM = ldc;
                 mo.row_base = (uint32_t)ra; mo.vnorm = mv->ysqrt.as<float>() + off[ra];
-                launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, Xh, nqv, span, dim, mo, mv->f16,
+                launch_maxsim_gemm(ws->mv_qh.as<char>() + (size_t)va * dim * 2, ch.X, nqv, span, dim, mo, mv->f16,
                                    mv->num_sms, st);
                 launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ldc, ws->mv_qoff.as<uint32_t>(), qa, qb, va, rb - ra,
                                      A + ra, ld, mv->num_sms, st);
@@ -2477,7 +2534,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
                             ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
             auto rescore = [&](auto *v) {
-                if (mv->on_host)
+                if (mv->rows.on_host)
                     launch_mv_rescore_host(d_q, ws->mv_qoff.as<uint32_t>(), qa, ws->xnorm.as<float>(), v,
                                            mv->ysqrt.as<float>(), mv->offsets.as<uint64_t>(), ids, dim, b,
                                            ws->mv_cand.as<uint32_t>(), ws->mv_cnt.as<uint32_t>(), cap,
@@ -2498,7 +2555,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             for (size_t c = 0; c + 1 < cutv.size(); c++) {
                 const uint64_t ra = cutv[c], rb = cutv[c + 1];
                 const void *X = static_cast<const char *>(V) + off[ra] * dim * es;
-                if (mv->on_host) {
+                if (mv->rows.on_host) {
                     const uint64_t n = (off[rb] - off[ra]) * dim;
                     if (mv->f16)
                         launch_mv_copy_gated(static_cast<const __half *>(X), ws->stage.buf[0].as<__half>(), n, gate,
@@ -2724,11 +2781,13 @@ static Route filtered_route(const uint32_t *allow, uint64_t allow_bits)
 }
 static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, stream}; }
 
-// Whether the host route may capture a handle's calls into a CUDA graph: not a flat or binary handle whose rows are on
-// the host, whose calls stream from pinned memory that an append moves, on a side stream (stream_topk)
-template <class H> static bool graph_capturable(const H *) { return true; }
-static bool graph_capturable(const lgpu_flat *fl) { return !fl->on_host; }
-static bool graph_capturable(const lgpu_binary *bx) { return !bx->on_host; }
+// Whether the host route may capture a handle's calls into a CUDA graph: not a handle whose rows are on the host,
+// whose calls stream from pinned memory that an append moves, on a side stream (RowStore::walk)
+template <class H> static bool graph_capturable(const H *h)
+{
+    if constexpr (std::is_base_of_v<lgpu_rows, H>) return !h->rows.on_host;
+    else return true;
+}
 
 // The sequence of every search entry point: resolve the handle; the kind's own checks, `check(h)`, which return how
 // many query elements (T) the call reads; the bitmap of a filtered call; nothing more for B == 0; the device; then
@@ -2765,7 +2824,7 @@ int search_call(H *hp, const Route &r, const T *queries, uint32_t B, const lgpu_
 }
 
 // what the flat, binary and multivector opens share: the device's SM count and the optional row ids
-template <class H> static void open_rows(H *h, const uint64_t *row_ids, uint64_t nrows)
+static void open_rows(lgpu_rows *h, const uint64_t *row_ids, uint64_t nrows)
 {
     cudaDeviceProp prop;
     LGPU_CUDA(cudaGetDeviceProperties(&prop, h->device));
@@ -2775,6 +2834,43 @@ template <class H> static void open_rows(H *h, const uint64_t *row_ids, uint64_t
         LGPU_CUDA(cudaMemcpy(h->row_ids.p, row_ids, (size_t)nrows * 8, cudaMemcpyHostToDevice));
         h->has_ids = true;
     }
+}
+
+// The byte accounting of a flat, binary or multivector handle (lgpu_*_device_bytes, lgpu_*_host_bytes): its row stores,
+// ids and live bitmap, and its kind's per-row buffers in HBM
+static uint64_t sum_bytes(std::initializer_list<const DevBuf *> bufs)
+{
+    uint64_t n = 0;
+    for (const DevBuf *b : bufs) n += b->bytes;
+    return n;
+}
+static uint64_t own_device_bytes(const lgpu_flat *fl) { return sum_bytes({&fl->ysqrt, &fl->vec_b, &fl->vec_n2}); }
+static uint64_t own_device_bytes(const lgpu_binary *bx)
+{
+    return sum_bytes({&bx->pop, &bx->sample, &bx->sample_pop, &bx->sample_ids});
+}
+static uint64_t own_device_bytes(const lgpu_multivec *mv)
+{
+    return sum_bytes({&mv->ysqrt, &mv->offsets, &mv->col_row}) + mv->ops.device_bytes();
+}
+static uint64_t own_host_bytes(const lgpu_rows *) { return 0; }
+static uint64_t own_host_bytes(const lgpu_multivec *mv) { return mv->ops.host_bytes(); }
+template <class H> static int rows_device_bytes(const H *hp, uint64_t *bytes)
+{
+    return guarded([&] {
+        HandleRef<H> h(const_cast<H *>(hp));
+        LGPU_REQUIRE(bytes != nullptr, "null argument");
+        *bytes = h->rows.device_bytes() + h->row_ids.bytes + h->live.bits.bytes + own_device_bytes(h.h);
+    });
+}
+template <class H> static int rows_host_bytes(const H *hp, uint64_t *bytes, int *placement)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(bytes || placement, "null argument");
+        HandleRef<H> h(const_cast<H *>(hp));
+        if (bytes) *bytes = h->rows.host_bytes() + own_host_bytes(h.h);
+        if (placement) *placement = h->rows.on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+    });
 }
 
 // the partition layout every IVF index shares (lgpu_index_open, lgpu_ivf_sq_open): checked before any device work
@@ -3790,23 +3886,17 @@ static int flat_open(const void *vectors, bool f16, uint64_t nrows, uint32_t dim
         fl->device = device; fl->nrows = nrows; fl->dim = dim; fl->f16 = f16;
         const size_t es = f16 ? 2 : 4, bytes = (size_t)nrows * dim * es;
         const bool tc_shape = gemm_shape_supported(dim) && nrows >= 4096;
-        if (!rows_fit_hbm("LGPU_FLAT_HBM_BYTES", flat_row_data_bytes(nrows, dim, f16))) {
-            fl->on_host = true;
-            fl->rows_host.alloc(bytes);
-            if (bytes) memcpy(fl->rows_host.p, vectors, bytes);
-            // a non-finite or overflowing row: the exact kernels serve the column
-            if (tc_shape) fl->has_tc = host_rows_band(fl->rows_host.p, f16, nrows, dim, fl->vec_max, fl->vec_err);
-        } else {
-            fl->vectors.ensure(std::max<size_t>(bytes, 16), true);
-            if (nrows) LGPU_CUDA(cudaMemcpy(fl->vectors.p, vectors, bytes, cudaMemcpyHostToDevice));
-            if (tc_shape) {
-                if (!f16) fl->vec_b.ensure((size_t)nrows * dim * 2, true);
-                fl->vec_n2.ensure((size_t)nrows * 4, true);
-                // a non-finite or overflowing row: the exact kernels serve the column
-                fl->has_tc = prepare_tc_operand(fl->vectors.p, f16, nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
-                                                fl->vec_err, nullptr);
-                if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
-            }
+        fl->rows.open(!rows_fit_hbm("LGPU_FLAT_HBM_BYTES", flat_row_data_bytes(nrows, dim, f16)), bytes);
+        fl->rows.fill(0, vectors, bytes);
+        // the band (a non-finite or overflowing row: the exact kernels serve the column), and in HBM the operand
+        if (tc_shape && fl->rows.on_host) {
+            fl->has_tc = host_rows_band(fl->rows.data(), f16, nrows, dim, fl->vec_max, fl->vec_err);
+        } else if (tc_shape) {
+            if (!f16) fl->vec_b.ensure((size_t)nrows * dim * 2, true);
+            fl->vec_n2.ensure((size_t)nrows * 4, true);
+            fl->has_tc = prepare_tc_operand(fl->rows.data(), f16, nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
+                                            fl->vec_err, nullptr);
+            if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
         }
         open_rows(fl, row_ids, nrows);
         register_handle(fl);
@@ -3828,25 +3918,10 @@ int lgpu_flat_open_f16(const uint16_t *vectors, uint64_t nrows, uint32_t dim, co
     return flat_open(vectors, true, nrows, dim, row_ids, device, out);
 }
 
-int lgpu_flat_device_bytes(const lgpu_flat *flh, uint64_t *bytes)
+int lgpu_flat_device_bytes(const lgpu_flat *fl, uint64_t *bytes) { return rows_device_bytes(fl, bytes); }
+int lgpu_flat_host_bytes(const lgpu_flat *fl, uint64_t *bytes, int *placement)
 {
-    return guarded([&] {
-        HandleRef<lgpu_flat> h(const_cast<lgpu_flat *>(flh));
-        LGPU_REQUIRE(bytes != nullptr, "null argument");
-        const lgpu_flat *fl = h.h;
-        *bytes = fl->vectors.bytes + fl->row_ids.bytes + fl->ysqrt.bytes + fl->vec_b.bytes + fl->vec_n2.bytes +
-                 fl->live.bits.bytes;
-    });
-}
-
-int lgpu_flat_host_bytes(const lgpu_flat *flh, uint64_t *bytes, int *placement)
-{
-    return guarded([&] {
-        LGPU_REQUIRE(bytes || placement, "null argument");
-        HandleRef<lgpu_flat> fl(const_cast<lgpu_flat *>(flh));
-        if (bytes) *bytes = fl->rows_host.bytes;
-        if (placement) *placement = fl->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
-    });
+    return rows_host_bytes(fl, bytes, placement);
 }
 
 void lgpu_flat_close(lgpu_flat *fl) { close_handle(fl); }
@@ -3899,6 +3974,18 @@ static void ham_pack_host(const uint8_t *src, uint64_t n, uint32_t nbytes, uint3
     }
 }
 
+// n of the caller's rows [n][nbytes] into rows n0.. of a binary handle's store, packed: on the host into pinned memory,
+// or in HBM from an upload, with their popcounts into `pop`
+static void ham_store_rows(lgpu_binary *bx, const uint8_t *src, uint64_t n0, uint64_t n)
+{
+    const uint32_t nbytes = bx->nbytes, nbp = bx->nbytes_pad;
+    uint8_t *dst = reinterpret_cast<uint8_t *>(bx->rows.data()) + (size_t)n0 * nbp;
+    if (bx->rows.on_host) return ham_pack_host(src, n, nbytes, nbp, dst);
+    DevBuf raw;
+    upload(raw, src, (size_t)n * nbytes);
+    launch_ham_pack(raw.as<uint8_t>(), nbytes, nbytes, n, dst, nbp, bx->pop.as<uint32_t>() + n0, nullptr);
+}
+
 // The packed rows and their popcounts go to HBM when they fit there (LGPU_BINARY_HBM_BYTES, rows_fit_hbm), else the
 // rows are packed into pinned host memory the handle owns.  HBM rows and popcounts are allocated exactly, so that
 // device bytes of the two placements differ by nrows x (nbytes_pad + 4).
@@ -3914,20 +4001,13 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
         bx = new lgpu_binary();
         bx->device = device; bx->nrows = nrows; bx->nbytes = nbytes; bx->nbytes_pad = (nbytes + 31) & ~31u;
         const uint32_t nbp = bx->nbytes_pad;
-        if (!rows_fit_hbm("LGPU_BINARY_HBM_BYTES", nrows * (nbp + 4))) {
-            bx->on_host = true;
-            bx->rows_host.alloc((size_t)nrows * nbp);
-            ham_pack_host(vectors, nrows, nbytes, nbp, static_cast<uint8_t *>(bx->rows_host.p));
-        } else if (nrows) {
-            bx->vectors.ensure((size_t)nrows * nbp, true);
-            bx->pop.ensure((size_t)nrows * 4, true);
-            DevBuf raw;
-            raw.ensure((size_t)nrows * nbytes);
-            LGPU_CUDA(cudaMemcpy(raw.p, vectors, (size_t)nrows * nbytes, cudaMemcpyHostToDevice));
-            launch_ham_pack(raw.as<uint8_t>(), nbytes, nbytes, nrows, bx->vectors.as<uint8_t>(), nbp, bx->pop.as<uint32_t>(),
-                            nullptr);
+        const bool host = !rows_fit_hbm("LGPU_BINARY_HBM_BYTES", nrows * (nbp + 4));
+        if (host || nrows) {
+            bx->rows.open(host, (size_t)nrows * nbp);
+            if (!host) bx->pop.ensure((size_t)nrows * 4, true);
+            ham_store_rows(bx, vectors, 0, nrows);
         } else {
-            bx->vectors.ensure(16);
+            bx->rows.hbm.ensure(16);
             bx->pop.ensure(16);
         }
         open_rows(bx, row_ids, nrows);
@@ -3940,25 +4020,10 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
     return rc;
 }
 
-int lgpu_binary_device_bytes(const lgpu_binary *bxh, uint64_t *bytes)
+int lgpu_binary_device_bytes(const lgpu_binary *bx, uint64_t *bytes) { return rows_device_bytes(bx, bytes); }
+int lgpu_binary_host_bytes(const lgpu_binary *bx, uint64_t *bytes, int *placement)
 {
-    return guarded([&] {
-        HandleRef<lgpu_binary> h(const_cast<lgpu_binary *>(bxh));
-        LGPU_REQUIRE(bytes != nullptr, "null argument");
-        const lgpu_binary *bx = h.h;
-        *bytes = bx->vectors.bytes + bx->pop.bytes + bx->row_ids.bytes + bx->sample.bytes + bx->sample_pop.bytes +
-                 bx->sample_ids.bytes + bx->live.bits.bytes;
-    });
-}
-
-int lgpu_binary_host_bytes(const lgpu_binary *bxh, uint64_t *bytes, int *placement)
-{
-    return guarded([&] {
-        LGPU_REQUIRE(bytes || placement, "null argument");
-        HandleRef<lgpu_binary> bx(const_cast<lgpu_binary *>(bxh));
-        if (bytes) *bytes = bx->rows_host.bytes;
-        if (placement) *placement = bx->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
-    });
+    return rows_host_bytes(bx, bytes, placement);
 }
 
 void lgpu_binary_close(lgpu_binary *bx) { close_handle(bx); }
@@ -4052,34 +4117,10 @@ int lgpu_ivf_binary_search_device(lgpu_ivf_binary *ixh, const uint8_t *d_queries
 
 }  // extern "C"
 
-// ---- appends to a flat handle (the unindexed rows of a table, DESIGN.md section 3) ----
-// `b` holds `used` bytes; make room for `need`: capacity at least doubles, the contents move by a device-to-device
-// copy.  The caller has drained the device, so nothing still reads the old buffer when it is released.
-static void grow_keep(DevBuf &b, size_t used, size_t need)
-{
-    if (need <= b.bytes) return;
-    DevBuf nb;
-    nb.ensure(std::max(need, 2 * b.bytes));                    // bumps g_alloc_epoch
-    if (used) LGPU_CUDA(cudaMemcpy(nb.p, b.p, used, cudaMemcpyDeviceToDevice));
-    std::swap(b.p, nb.p);
-    std::swap(b.bytes, nb.bytes);
-}
-
-// ... and the pinned rows of a host handle, moved by a host copy
-static void grow_keep(PinnedBuf &b, size_t used, size_t need)
-{
-    if (need <= b.bytes) return;
-    PinnedBuf nb;
-    nb.alloc(std::max(need, 2 * b.bytes));
-    if (used) memcpy(nb.p, b.p, used);
-    std::swap(b.p, nb.p);
-    std::swap(b.dev, nb.dev);
-    std::swap(b.bytes, nb.bytes);
-}
-
+// ---- appends to a flat or binary handle (the unindexed rows of a table, DESIGN.md section 3) ----
 // The row ids after an append of n rows to n0: explicit ids stay explicit (positions n0.. when none are given), and
 // ids given to a handle that had none make the old rows' positions explicit.
-template <class H> static void append_ids(H *h, uint64_t n0, uint64_t n, const uint64_t *row_ids)
+static void append_ids(lgpu_rows *h, uint64_t n0, uint64_t n, const uint64_t *row_ids)
 {
     if (!row_ids && !h->has_ids) return;
     grow_keep(h->row_ids, h->has_ids ? n0 * 8 : 0, (n0 + n) * 8);
@@ -4111,11 +4152,8 @@ static void begin_append(int device)
 
 // ---- deleted rows (lgpu_*_delete): the live bitmap of a handle (RowLive) ----
 // the row ids of a handle in device memory, or null when they are the positions 0 .. nrows - 1
-template <class H> static const uint64_t *device_row_ids(H *h)
-{
-    if constexpr (std::is_base_of_v<lgpu_index, H>) return h->row_ids.template as<uint64_t>();
-    else return h->has_ids ? h->row_ids.template as<uint64_t>() : nullptr;
-}
+static const uint64_t *device_row_ids(lgpu_index *ix) { return ix->row_ids.as<uint64_t>(); }
+static const uint64_t *device_row_ids(const lgpu_rows *h) { return row_cols(h, 0).ids; }
 
 static void require_id_bound(uint64_t max_id)
 {
@@ -4216,60 +4254,73 @@ template <class H> static int delete_rows(H *hp, const uint64_t *row_ids, uint64
     });
 }
 
-extern "C" {
+// the bytes of one stored row
+static size_t stored_row_bytes(const lgpu_flat *fl) { return (size_t)fl->dim * (fl->f16 ? 2 : 4); }
+static size_t stored_row_bytes(const lgpu_binary *bx) { return bx->nbytes_pad; }
 
-// lgpu_flat_append and lgpu_flat_append_f16: the rows must have the handle's row type (f16)
-static int flat_append(lgpu_flat *flh, const void *rows, bool f16, uint64_t n, const uint64_t *row_ids)
+// The sequence of a flat or binary append of n rows (row_ids: host, null = the positions that follow): hold the handle
+// alone, `check(h)`, grow the row store and `store(h, n0, n)` the rows into it, set their ids and live bits, then the
+// kind's per-row terms `terms(h, n0, n)`, drain the device and publish the new row count.
+template <class H, class Check, class Store, class Terms>
+static int append_rows(H *hp, const void *rows, uint64_t n, const uint64_t *row_ids, Check &&check, Store &&store,
+                       Terms &&terms)
 {
     return guarded([&] {
-        HandleExcl<lgpu_flat> h(flh);
-        lgpu_flat *fl = h.h;
-        LGPU_REQUIRE(fl->f16 == f16, fl->f16 ? "the handle holds fp16 rows: append them with lgpu_flat_append_f16"
-                                             : "the handle holds f32 rows: append them with lgpu_flat_append");
+        HandleExcl<H> h(hp);
+        check(h.h);
         LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
         if (n == 0) return;
-        const uint64_t bound = live_bound_after(fl, n, row_ids);
-        begin_append(fl->device);
-        const uint64_t n0 = fl->nrows, n1 = n0 + n;
-        const uint32_t d = fl->dim;
-        const size_t es = f16 ? 2 : 4;
-        if (fl->on_host) {
-            grow_keep(fl->rows_host, (size_t)n0 * d * es, (size_t)n1 * d * es);
-            char *x = static_cast<char *>(fl->rows_host.p) + (size_t)n0 * d * es;
-            memcpy(x, rows, (size_t)n * d * es);
-            append_ids(fl, n0, n, row_ids);
-            grow_live(fl, n0, n, bound);
-            // the band as lgpu_flat_open takes it from n1 rows: the whole column when it first reaches 4096 rows, else
-            // the new rows', the constants the max over both parts
-            if (gemm_shape_supported(d) && n1 >= 4096) {
+        const uint64_t bound = live_bound_after(h.h, n, row_ids);
+        begin_append(h->device);
+        const uint64_t n0 = h->nrows, n1 = n0 + n;
+        h->rows.grow(n0 * stored_row_bytes(h.h), n1 * stored_row_bytes(h.h));
+        store(h.h, n0, n);
+        append_ids(h.h, n0, n, row_ids);
+        grow_live(h.h, n0, n, bound);
+        terms(h.h, n0, n);
+        LGPU_CUDA(cudaDeviceSynchronize());
+        h->nrows = n1;
+    });
+}
+
+extern "C" {
+
+// lgpu_flat_append and lgpu_flat_append_f16: the rows must have the handle's row type (f16).  The terms, as
+// lgpu_flat_open takes them from n1 rows: the whole column's when it first reaches 4096 rows, else the new rows', the
+// band constants the max over both parts.  In HBM: |x| once a cosine search built it, and the tensor-core operand
+static int flat_append(lgpu_flat *flh, const void *rows, bool f16, uint64_t n, const uint64_t *row_ids)
+{
+    const size_t es = f16 ? 2 : 4;
+    return append_rows(flh, rows, n, row_ids,
+        [&](lgpu_flat *fl) {
+            LGPU_REQUIRE(fl->f16 == f16, fl->f16 ? "the handle holds fp16 rows: append them with lgpu_flat_append_f16"
+                                                 : "the handle holds f32 rows: append them with lgpu_flat_append");
+        },
+        [&](lgpu_flat *fl, uint64_t n0, uint64_t n) { fl->rows.fill(n0 * es * fl->dim, rows, n * es * fl->dim); },
+        [&](lgpu_flat *fl, uint64_t n0, uint64_t n) {
+            const uint64_t n1 = n0 + n;
+            const uint32_t d = fl->dim;
+            const char *x = fl->rows.data() + (size_t)n0 * d * es;
+            if (fl->rows.on_host) {
+                if (!gemm_shape_supported(d) || n1 < 4096) return;
                 if (n0 < 4096) {
-                    fl->has_tc = host_rows_band(fl->rows_host.p, f16, n1, d, fl->vec_max, fl->vec_err);
+                    fl->has_tc = host_rows_band(fl->rows.data(), f16, n1, d, fl->vec_max, fl->vec_err);
                 } else if (fl->has_tc) {
                     float xmax = 0.f, xerr = 0.f;
                     fl->has_tc = host_rows_band(x, f16, n, d, xmax, xerr);
                     fl->vec_max = std::max(fl->vec_max, xmax);
                     fl->vec_err = std::max(fl->vec_err, xerr);
                 }
+                return;
             }
-            LGPU_CUDA(cudaDeviceSynchronize());
-            fl->nrows = n1;
-            return;
-        }
-        grow_keep(fl->vectors, (size_t)n0 * d * es, (size_t)n1 * d * es);
-        char *x = fl->vectors.as<char>() + (size_t)n0 * d * es;
-        LGPU_CUDA(cudaMemcpy(x, rows, (size_t)n * d * es, cudaMemcpyHostToDevice));
-        append_ids(fl, n0, n, row_ids);
-        grow_live(fl, n0, n, bound);
-        if (fl->has_norms) {
-            grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
-            if (f16) launch_row_norms(reinterpret_cast<const __half *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
-            else launch_row_norms(reinterpret_cast<const float *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
-        }
-        // the tensor-core operand, as lgpu_flat_open builds it for n1 rows: the whole column when it first reaches 4096
-        // rows, else the new rows only, the band constants the max over both parts
-        if (gemm_shape_supported(d) && n1 >= 4096) {
+            if (fl->has_norms) {
+                grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
+                if (f16) launch_row_norms(reinterpret_cast<const __half *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
+                else launch_row_norms(reinterpret_cast<const float *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
+            }
+            if (!gemm_shape_supported(d) || n1 < 4096) return;
             if (n0 < 4096) {
-                fl->has_tc = prepare_tc_operand(fl->vectors.p, f16, n1, d, fl->vec_b, fl->vec_n2, fl->vec_max,
+                fl->has_tc = prepare_tc_operand(fl->rows.data(), f16, n1, d, fl->vec_b, fl->vec_n2, fl->vec_max,
                                                 fl->vec_err, nullptr);
             } else if (fl->has_tc) {
                 if (!f16) grow_keep(fl->vec_b, (size_t)n0 * d * 2, (size_t)n1 * d * 2);
@@ -4281,10 +4332,7 @@ static int flat_append(lgpu_flat *flh, const void *rows, bool f16, uint64_t n, c
                 fl->vec_err = std::max(fl->vec_err, xerr);
             }
             if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
-        }
-        LGPU_CUDA(cudaDeviceSynchronize());
-        fl->nrows = n1;
-    });
+        });
 }
 
 int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64_t *row_ids)
@@ -4297,39 +4345,16 @@ int lgpu_flat_append_f16(lgpu_flat *flh, const uint16_t *rows, uint64_t n, const
     return flat_append(flh, rows, true, n, row_ids);
 }
 
+// the terms: an HBM store's popcounts (stored with the rows), and the threshold sample lgpu_binary_open takes from n1
+// rows
 int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const uint64_t *row_ids)
 {
-    return guarded([&] {
-        HandleExcl<lgpu_binary> h(bxh);
-        lgpu_binary *bx = h.h;
-        LGPU_REQUIRE(n == 0 || rows != nullptr, "null rows");
-        if (n == 0) return;
-        const uint64_t bound = live_bound_after(bx, n, row_ids);
-        begin_append(bx->device);
-        const uint64_t n0 = bx->nrows, n1 = n0 + n;
-        const uint32_t nbp = bx->nbytes_pad;
-        if (bx->on_host) {
-            grow_keep(bx->rows_host, (size_t)n0 * nbp, (size_t)n1 * nbp);
-            ham_pack_host(rows, n, bx->nbytes, nbp, static_cast<uint8_t *>(bx->rows_host.p) + (size_t)n0 * nbp);
-            append_ids(bx, n0, n, row_ids);
-            grow_live(bx, n0, n, bound);
-            ham_sample(bx, n1);
-            LGPU_CUDA(cudaDeviceSynchronize());
-            bx->nrows = n1;
-            return;
-        }
-        grow_keep(bx->vectors, (size_t)n0 * nbp, (size_t)n1 * nbp);
-        grow_keep(bx->pop, (size_t)n0 * 4, (size_t)n1 * 4);
-        DevBuf raw;
-        upload(raw, rows, (size_t)n * bx->nbytes);
-        launch_ham_pack(raw.as<uint8_t>(), bx->nbytes, bx->nbytes, n, bx->vectors.as<uint8_t>() + (size_t)n0 * nbp, nbp,
-                        bx->pop.as<uint32_t>() + n0, nullptr);
-        append_ids(bx, n0, n, row_ids);
-        grow_live(bx, n0, n, bound);
-        ham_sample(bx, n1);                // the threshold sample lgpu_binary_open takes from n1 rows
-        LGPU_CUDA(cudaDeviceSynchronize());
-        bx->nrows = n1;
-    });
+    return append_rows(bxh, rows, n, row_ids, [](lgpu_binary *) {},
+        [&](lgpu_binary *bx, uint64_t n0, uint64_t n) {
+            if (!bx->rows.on_host) grow_keep(bx->pop, (size_t)n0 * 4, (size_t)(n0 + n) * 4);
+            ham_store_rows(bx, rows, n0, n);
+        },
+        [](lgpu_binary *bx, uint64_t n0, uint64_t n) { ham_sample(bx, n0 + n); });
 }
 
 int lgpu_index_delete(lgpu_index *ix, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
@@ -4577,13 +4602,13 @@ static int multivec_open(const void *values, bool f16, const uint64_t *offsets, 
         mv->offsets.ensure((size_t)(nrows + 1) * 8);
         LGPU_CUDA(cudaMemcpy(mv->offsets.p, offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice));
         bool ok = true;
-        if (!rows_fit_hbm("LGPU_MULTIVEC_HBM_BYTES", xbytes + hbytes)) {
-            // pinned host memory: the vectors as given, |v| (and an f32 handle's fp16 operand) computed chunk by chunk
-            // of whole rows staged through HBM (each vector's terms depend on that vector alone)
-            mv->on_host = true;
-            mv->vectors_host.alloc(xbytes);
-            if (xbytes) memcpy(mv->vectors_host.p, values, xbytes);
-            if (hbytes) mv->vec_h_host.alloc(hbytes);
+        const bool host = !rows_fit_hbm("LGPU_MULTIVEC_HBM_BYTES", xbytes + hbytes);
+        mv->rows.open(host, xbytes);
+        mv->rows.fill(0, values, xbytes);
+        if (hbytes) mv->ops.open(host, hbytes);
+        if (host) {
+            // |v| (and an f32 handle's fp16 operand) computed chunk by chunk of whole rows staged through HBM (each
+            // vector's terms depend on that vector alone)
             const std::vector<uint64_t> cut = mv_chunks(mv, std::max<uint64_t>(1, FLAT_STAGE_BYTES / ((size_t)dim * es)));
             DevBuf xs, hs;
             for (size_t c = 0; c + 1 < cut.size(); c++) {
@@ -4595,17 +4620,11 @@ static int multivec_open(const void *values, bool f16, const uint64_t *offsets, 
                                      cudaMemcpyHostToDevice));
                 ok &= mv_vector_terms(xs.p, f16, n, dim, mv->ysqrt.as<float>() + j0, tc_shape, hbytes ? hs.p : nullptr);
                 if (hbytes)
-                    LGPU_CUDA(cudaMemcpy(static_cast<char *>(mv->vec_h_host.p) + j0 * dim * 2, hs.p, n * dim * 2,
-                                         cudaMemcpyDeviceToHost));
+                    LGPU_CUDA(cudaMemcpy(mv->ops.data() + j0 * dim * 2, hs.p, n * dim * 2, cudaMemcpyDeviceToHost));
             }
-        } else {
-            mv->vectors.ensure(std::max<size_t>(xbytes, 16), true);
-            if (hbytes) mv->vec_h.ensure(hbytes, true);
-            if (T) {
-                LGPU_CUDA(cudaMemcpy(mv->vectors.p, values, xbytes, cudaMemcpyHostToDevice));
-                ok = mv_vector_terms(mv->vectors.p, f16, T, dim, mv->ysqrt.as<float>(), tc_shape,
-                                     hbytes ? mv->vec_h.p : nullptr);
-            }
+        } else if (T) {
+            ok = mv_vector_terms(mv->rows.data(), f16, T, dim, mv->ysqrt.as<float>(), tc_shape,
+                                 hbytes ? mv->ops.data() : nullptr);
         }
         if (tc_shape) {
             std::vector<uint32_t> cr(T);
@@ -4636,25 +4655,10 @@ int lgpu_multivec_open_f16(const uint16_t *values, const uint64_t *offsets, uint
     return multivec_open(values, true, offsets, nrows, dim, row_ids, device, out);
 }
 
-int lgpu_multivec_device_bytes(const lgpu_multivec *mvh, uint64_t *bytes)
+int lgpu_multivec_device_bytes(const lgpu_multivec *mv, uint64_t *bytes) { return rows_device_bytes(mv, bytes); }
+int lgpu_multivec_host_bytes(const lgpu_multivec *mv, uint64_t *bytes, int *placement)
 {
-    return guarded([&] {
-        HandleRef<lgpu_multivec> h(const_cast<lgpu_multivec *>(mvh));
-        LGPU_REQUIRE(bytes != nullptr, "null argument");
-        const lgpu_multivec *mv = h.h;
-        *bytes = mv->vectors.bytes + mv->ysqrt.bytes + mv->offsets.bytes + mv->row_ids.bytes + mv->vec_h.bytes +
-                 mv->col_row.bytes + mv->live.bits.bytes;
-    });
-}
-
-int lgpu_multivec_host_bytes(const lgpu_multivec *mvh, uint64_t *bytes, int *placement)
-{
-    return guarded([&] {
-        LGPU_REQUIRE(bytes || placement, "null argument");
-        HandleRef<lgpu_multivec> mv(const_cast<lgpu_multivec *>(mvh));
-        if (bytes) *bytes = mv->vectors_host.bytes + mv->vec_h_host.bytes;
-        if (placement) *placement = mv->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
-    });
+    return rows_host_bytes(mv, bytes, placement);
 }
 
 void lgpu_multivec_close(lgpu_multivec *mv) { close_handle(mv); }
