@@ -123,7 +123,8 @@ int         lgpu_device_count(int *count);
 /* ---- IVF_PQ (ANNIvfPartitionExec -> ANNIvfSubIndexExec -> TopK) ---------- */
 int  lgpu_index_open(const lgpu_index_desc *desc, lgpu_index **out);
 void lgpu_index_close(lgpu_index *ix);
-/* bytes of HBM held by the index (codes + ids + centroids + codebook, and the raw vectors when they are in HBM) */
+/* bytes of HBM held by the index (codes when they are in HBM + ids + centroids + codebook, and the raw vectors when
+ * they are in HBM) */
 int  lgpu_index_device_bytes(const lgpu_index *ix, uint64_t *bytes);
 /* Where an index keeps the raw vectors desc.vectors gave it (refine_factor).  Every float IVF open (lgpu_index_open,
  * lgpu_ivf_sq_open, lgpu_ivf_hnsw_sq_open, lgpu_ivf_rq_open) copies them into HBM when they fit with room to spare: the
@@ -140,6 +141,25 @@ int  lgpu_index_host_bytes(const lgpu_index *ix, uint64_t *bytes, int *placement
  * algorithmic bytes, SURVEY.md 8d); valid for the most recent search on the
  * calling thread */
 int  lgpu_last_scanned_code_bytes(uint64_t *bytes);
+/* bytes of host-resident codes (lgpu_index_code_bytes) the most recent IVF search on the calling thread copied into HBM,
+ * every sub-batch and maximum_nprobes pass included; counted while profiling (LGPU_PROFILE=1, lgpu_set_profiling),
+ * else 0 */
+int  lgpu_last_streamed_code_bytes(uint64_t *bytes);
+
+/* Where an IVF index keeps its stored codes.  lgpu_ivf_sq_open, lgpu_ivf_rq_open and lgpu_ivf_binary_open put them in
+ * HBM when they fit with room to spare: the device's free memory, once the centroids, partition arrays and per-row terms
+ * are in place, covers them plus the workspace budget (LGPU_WS_BYTES), and they are at most LGPU_CODES_HBM_BYTES (read
+ * at every open; unset = no cap, 0 = never in HBM).  Otherwise the index keeps them in pinned, mapped host memory that
+ * it owns, in the HBM layout (IVF_SQ [nrows][dim_pad] bytes, dim_pad = dim rounded up to 64; IVF_RQ [nrows][wpr] u32,
+ * wpr = dim rounded up to 256 bits; binary IVF_FLAT [nrows][nbytes_pad], nbytes_pad = nbytes rounded up to 32; padding
+ * zero), and each search copies the partitions its queries probe into HBM in chunks of consecutive partitions, double
+ * buffered, scanning one chunk while the next is copied; results are identical.  The per-row terms and row ids stay in
+ * HBM.  Two staging buffers of the largest partition must fit the workspace budget, else the open is LGPU_OOM; a pinned
+ * allocation that fails is LGPU_OOM too.  The codes are placed before the raw vectors (lgpu_index_host_bytes).
+ * IVF_HNSW_SQ (its graph walk reads rows at random) and IVF_PQ (4-bit and 8-bit) keep their codes in HBM whatever the
+ * cap says.  host_bytes: the pinned bytes of codes (0 in HBM); placement: LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either
+ * output may be NULL.  lgpu_ivf_binary_code_bytes is the same for a binary IVF_FLAT handle. */
+int  lgpu_index_code_bytes(const lgpu_index *ix, uint64_t *host_bytes, int *placement);
 
 /* Search a batch of B queries held in HOST memory.  queries: [B][dim] f32.
  * out_ids/out_dist: [B][k] (`_rowid` / `_distance`, ascending by
@@ -229,7 +249,8 @@ int lgpu_merge_topk_device(int device, uint32_t nlists, uint32_t B, uint32_t k,
  * Partition assignment is find_partitions (lgpu_ivf_assign), there are no residuals.  The handle is an ordinary
  * lgpu_index: lgpu_search, _filtered, _device, _async and _coalesced serve it with the IVF_PQ semantics of k, nprobes,
  * maximum_nprobes, prefilter, distance_range (on the SQ distance, before refine), refine_factor and timeout_ms.
- * lgpu_search_sharded*, lgpu_debug_filter_bounds and lgpu_debug_partition_distances reject it. */
+ * lgpu_search_sharded*, lgpu_debug_filter_bounds and lgpu_debug_partition_distances reject it.  The codes go to pinned
+ * host memory when they do not fit in HBM (LGPU_CODES_HBM_BYTES, lgpu_index_code_bytes). */
 #define LGPU_SQ_MAX_DIM 65536     /* the exact sum stays below 2^32 */
 typedef struct {
     uint32_t abi_version;         /* LGPU_ABI_VERSION */
@@ -261,7 +282,7 @@ int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *desc, lgpu_index **out);
  *     (distance_range, prefilter); traversal ignores the filter.
  * The R lists are merged by (_distance, _rowid); refine_factor, maximum_nprobes, timeout_ms and every entry point are
  * IVF_SQ's.  ef' above LGPU_HNSW_EF_MAX is LGPU_INVALID_INPUT.  lgpu_search_sharded*, lgpu_debug_filter_bounds and
- * lgpu_debug_partition_distances reject the handle. */
+ * lgpu_debug_partition_distances reject the handle.  The codes stay in HBM whatever LGPU_CODES_HBM_BYTES says. */
 #define LGPU_HNSW_MAX_M 64        /* a level-0 list has at most 128 entries */
 #define LGPU_HNSW_MAX_LEVEL 15
 #define LGPU_HNSW_EF_MAX 2048     /* W lives in shared memory */
@@ -295,7 +316,8 @@ int lgpu_ivf_hnsw_sq_open(const lgpu_ivf_hnsw_sq_desc *desc, lgpu_index **out);
  * estimate is never returned.  dot and num_bits != 1 are not supported (LGPU_INVALID_INPUT).  The handle is an
  * ordinary lgpu_index: lgpu_search, _filtered, _device, _async and _coalesced serve it with the IVF_PQ semantics of k,
  * nprobes, maximum_nprobes, prefilter, distance_range (on the estimate, before refine), refine_factor and timeout_ms.
- * lgpu_search_sharded*, lgpu_debug_filter_bounds and lgpu_debug_partition_distances reject it. */
+ * lgpu_search_sharded*, lgpu_debug_filter_bounds and lgpu_debug_partition_distances reject it.  The codes go to pinned
+ * host memory when they do not fit in HBM (LGPU_CODES_HBM_BYTES, lgpu_index_code_bytes). */
 #define LGPU_RQ_MAX_DIM 4096      /* P at most 64 MB; every integer above stays exact in f32 */
 typedef struct {
     uint32_t abi_version;         /* LGPU_ABI_VERSION */
@@ -522,7 +544,8 @@ int  lgpu_multivec_delete(lgpu_multivec *mv, const uint64_t *row_ids, uint64_t n
  * a prefilter), prefilter, distance_range (before the top-k) and timeout_ms behave as on lgpu_index; refine_factor is
  * accepted and changes nothing (the distances are exact; k x refine_factor is not limited).  With nprobes >= nlist the
  * result is lgpu_binary_search's.  nprobes above 2048 must cover every partition, and so must maximum_nprobes above
- * 2048 when it widens (under a prefilter).  queries: [B][nbytes]. */
+ * 2048 when it widens (under a prefilter).  queries: [B][nbytes].  The packed rows go to pinned host memory when they do
+ * not fit in HBM (LGPU_CODES_HBM_BYTES, lgpu_ivf_binary_code_bytes). */
 typedef struct {
     uint32_t abi_version;         /* LGPU_ABI_VERSION */
     uint32_t nbytes;              /* bytes per vector, 8 nbytes <= 2^24 */
@@ -536,6 +559,8 @@ typedef struct {
 } lgpu_ivf_binary_desc;
 int  lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *desc, lgpu_ivf_binary **out);
 void lgpu_ivf_binary_close(lgpu_ivf_binary *ix);
+/* where the packed rows are (LGPU_CODES_HBM_BYTES, see lgpu_index_code_bytes) */
+int  lgpu_ivf_binary_code_bytes(const lgpu_ivf_binary *ix, uint64_t *host_bytes, int *placement);
 int  lgpu_ivf_binary_search(lgpu_ivf_binary *ix, const uint8_t *queries, uint32_t B, const lgpu_search_params *params,
                             uint64_t *out_ids, float *out_dist, uint32_t *out_count);
 int  lgpu_ivf_binary_search_filtered(lgpu_ivf_binary *ix, const uint8_t *queries, uint32_t B,

@@ -53,6 +53,7 @@ EXPORTS = [
     "lgpu_multivec_device_bytes", "lgpu_multivec_host_bytes",
     "lgpu_multivec_open_f16", "lgpu_debug_maxsim_gemm_f16",
     "lgpu_binary_device_bytes", "lgpu_binary_host_bytes",
+    "lgpu_index_code_bytes", "lgpu_ivf_binary_code_bytes", "lgpu_last_streamed_code_bytes",
 ]
 VECTORS_NONE, VECTORS_HBM, VECTORS_HOST = 0, 1, 2     # lgpu_vectors_placement
 MULTIVEC_MAX_NQ = 4096          # vectors per multivector query (include/lancedb_b200.h)
@@ -165,6 +166,9 @@ def load():
     lib.lgpu_index_host_bytes.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
     lib.lgpu_debug_refine_host.argtypes = [vp, u32, vp, C.c_uint64, u32, vp, u32, i32, i32, vp]
     lib.lgpu_last_scanned_code_bytes.argtypes = [C.POINTER(C.c_uint64)]
+    lib.lgpu_last_streamed_code_bytes.argtypes = [C.POINTER(C.c_uint64)]
+    for fn in ("lgpu_index_code_bytes", "lgpu_ivf_binary_code_bytes"):
+        getattr(lib, fn).argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
     lib.lgpu_search.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
     lib.lgpu_search_async.argtypes = [vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp, C.POINTER(vp)]
     lib.lgpu_ticket_poll.argtypes = [vp, C.POINTER(C.c_int)]
@@ -320,6 +324,27 @@ class _Placed:
         return self._host()[0]
 
 
+class _Codes:
+    """An IVF index that reports where it keeps its stored codes through `_codes`, its lgpu_*_code_bytes: in HBM, or --
+    IVF_SQ, IVF_RQ and binary IVF_FLAT whose codes did not fit there at open (LGPU_CODES_HBM_BYTES) -- in pinned host
+    memory, the probed partitions streamed through the GPU by every search, with the same results."""
+    _codes = ""
+
+    def _code_placement(self):
+        b, where = C.c_uint64(0), C.c_int(0)
+        check(getattr(load(), self._codes)(self._h, C.byref(b), C.byref(where)))
+        return b.value, where.value
+
+    @property
+    def codes_on_host(self) -> bool:
+        """True when the codes are kept in pinned host memory and every search stages its probed partitions."""
+        return self._code_placement()[1] == VECTORS_HOST
+
+    def code_host_bytes(self) -> int:
+        """The pinned host memory the index holds for its codes (their padded layout), 0 when they are in HBM."""
+        return self._code_placement()[0]
+
+
 class _RowsHandle(_Handle):
     """A handle over rows, which `_delete`, the name of its lgpu_*_delete, deletes rows from."""
     _delete = ""
@@ -424,11 +449,11 @@ def _query_offsets(q_offsets) -> np.ndarray:
     return np.ascontiguousarray(off, np.uint32)
 
 
-class GpuIvfPq(_Placed, _RowsHandle):
+class GpuIvfPq(_Placed, _Codes, _RowsHandle):
     """An IVF_PQ index pinned in HBM (lgpu_index), 8-bit or 4-bit codes (data.num_bits).  The other float IVF kinds
     open an lgpu_index through their own C function, `_open`, so they subclass this and supply only `_desc`."""
     _open, _close = "lgpu_index_open", "lgpu_index_close"
-    _delete, _bytes = "lgpu_index_delete", "lgpu_index"
+    _delete, _bytes, _codes = "lgpu_index_delete", "lgpu_index", "lgpu_index_code_bytes"
 
     def __init__(self, data, device: int = 0, with_vectors: bool = True):
         lib = load()
@@ -542,8 +567,9 @@ class GpuIvfPq(_Placed, _RowsHandle):
 
 
 class GpuIvfSq(GpuIvfPq):
-    """An IVF_SQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_sq_open, so every search entry point of GpuIvfPq
-    serves it.  _distance is the exact integer sum of squared code differences as f32 (l2 and cosine alike)."""
+    """An IVF_SQ index: an lgpu_index opened by lgpu_ivf_sq_open, so every search entry point of GpuIvfPq serves it.
+    _distance is the exact integer sum of squared code differences as f32 (l2 and cosine alike).  The codes are in HBM,
+    or in pinned host memory when they do not fit there (LGPU_CODES_HBM_BYTES, `codes_on_host`)."""
     _open = "lgpu_ivf_sq_open"
 
     def _desc(self, data, device, vec):
@@ -571,9 +597,10 @@ class GpuIvfHnswSq(GpuIvfSq):
 
 
 class GpuIvfRq(GpuIvfPq):
-    """An IVF_RQ index pinned in HBM: an lgpu_index opened by lgpu_ivf_rq_open, so every search entry point of GpuIvfPq
-    serves it.  _distance is the RaBitQ estimate of the squared L2 distance (half of it for cosine); refine_factor
-    re-ranks by the exact distance."""
+    """An IVF_RQ index: an lgpu_index opened by lgpu_ivf_rq_open, so every search entry point of GpuIvfPq serves it.
+    _distance is the RaBitQ estimate of the squared L2 distance (half of it for cosine); refine_factor re-ranks by the
+    exact distance.  The codes are in HBM, or in pinned host memory when they do not fit there (LGPU_CODES_HBM_BYTES,
+    `codes_on_host`)."""
     _open = "lgpu_ivf_rq_open"
 
     def _desc(self, data, device, vec):
@@ -678,11 +705,13 @@ class GpuBinary(_Column):
         self.nrows += v.shape[0]
 
 
-class GpuIvfBinary(_RowsHandle):
-    """A binary IVF_FLAT index (IvfBinaryIndexData) pinned in HBM (lgpu_ivf_binary): the probed partitions of packed
-    binary rows scored exactly by Hamming distance."""
+class GpuIvfBinary(_Codes, _RowsHandle):
+    """A binary IVF_FLAT index (IvfBinaryIndexData, lgpu_ivf_binary): the probed partitions of packed binary rows
+    scored exactly by Hamming distance.  The packed rows are in HBM, or in pinned host memory when they do not fit there
+    (LGPU_CODES_HBM_BYTES, `codes_on_host`)."""
     _close = "lgpu_ivf_binary_close"
     _delete = "lgpu_ivf_binary_delete"
+    _codes = "lgpu_ivf_binary_code_bytes"
     _queries = _binary_queries
 
     def __init__(self, data, device: int = 0):
@@ -1052,6 +1081,13 @@ def last_stage_ms():
     t = (C.c_float * 7)()
     check(load().lgpu_last_stage_ms(t))
     return dict(zip(["coarse", "select_probes", "group", "scan", "topk", "refine", "total"], list(t)))
+
+
+def last_streamed_code_bytes() -> int:
+    """Bytes of host-resident IVF codes the last profiled search on this thread copied into HBM."""
+    b = C.c_uint64(0)
+    check(load().lgpu_last_streamed_code_bytes(C.byref(b)))
+    return b.value
 
 
 def last_scanned_code_bytes() -> int:

@@ -33,6 +33,7 @@ namespace lgpu {
 static thread_local std::string g_err;
 static thread_local float g_stage_ms[7] = {0, 0, 0, 0, 0, 0, 0};
 static thread_local uint64_t g_scanned_bytes = 0;
+static thread_local uint64_t g_streamed_bytes = 0;   // profiling: the host-resident codes the last IVF call copied
 static thread_local uint64_t g_filter_stats[4] = {0, 0, 0, 0};
 void set_error(const std::string &msg) { g_err = msg; }
 
@@ -158,9 +159,12 @@ struct Workspace;
 // forked from the call's stream and joined back to it), chunk s + 1 while chunk s is used on the call's stream:
 // take(s) hands over chunk s once the copy of chunk s + 1 is issued, release(s) marks every use of it enqueued.
 // copied[i]: buf[i] holds its chunk (side stream); freed[i]: the uses of its chunk are enqueued (call's stream), so the
-// copy two steps later may overwrite it.  timeout_ms is checked between chunks.
+// copy two steps later may overwrite it.  timeout_ms is checked between chunks.  A walk that copies by a kernel of its
+// own instead (an IVF index's probed partitions, launch_codes_copy_gated) passes `copier`, which enqueues chunk s into
+// the buffer it is given on the side stream, in place of the cudaMemcpyAsync of src(s).
 struct Staging {
     using Source = std::function<std::pair<const void *, size_t>(uint64_t)>;   // chunk s: its pinned rows and bytes
+    using Copier = std::function<void(uint64_t, void *, cudaStream_t)>;        // chunk s into a buffer, on a stream
     DevBuf buf[2];
     cudaEvent_t copied[2] = {}, freed[2] = {};
     Staging()
@@ -177,7 +181,8 @@ struct Staging {
             if (freed[i]) cudaEventDestroy(freed[i]);
         }
     }
-    void open(Workspace *ws, cudaStream_t st, uint64_t steps, const Deadline *deadline, Source src);
+    void open(Workspace *ws, cudaStream_t st, uint64_t steps, const Deadline *deadline, Source src,
+              Copier copier = nullptr);
     void *take(uint64_t s);
     void release(uint64_t s) { LGPU_CUDA(cudaEventRecord(freed[s & 1], st)); }
     void close();
@@ -188,6 +193,7 @@ struct Staging {
     uint64_t steps = 0;
     const Deadline *deadline = nullptr;
     Source src;
+    Copier copier;
 };
 
 struct Workspace {
@@ -236,6 +242,7 @@ struct Workspace {
     // operand, |x|^2 and |x|, and the running top-k, [2 buffers][2 lists][P][k] / [..][P]
     DevBuf chunk_xb, chunk_n2, chunk_ysqrt, run_ids, run_dist, run_cnt;
     DevBuf chunk_pop;                   // ... of a binary handle (binary_search_device): popc of each staged row
+    DevBuf code_ctr;                    // an IVF index with codes on the host: each chunk's tile counter, the bytes copied
     Workspace()
     {
         LGPU_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -259,9 +266,9 @@ struct Workspace {
     }
 };
 
-void Staging::open(Workspace *w, cudaStream_t s, uint64_t n, const Deadline *dl, Source source)
+void Staging::open(Workspace *w, cudaStream_t s, uint64_t n, const Deadline *dl, Source source, Copier cp)
 {
-    ws = w; st = s; steps = n; deadline = dl; src = std::move(source);
+    ws = w; st = s; steps = n; deadline = dl; src = std::move(source); copier = std::move(cp);
     LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
     LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
     ws->front_open = true;
@@ -273,8 +280,12 @@ void Staging::copy(uint64_t s)
 {
     const int i = (int)(s & 1);
     if (s >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, freed[i], 0));
-    const auto [rows, bytes] = src(s);
-    if (bytes) LGPU_CUDA(cudaMemcpyAsync(buf[i].p, rows, bytes, cudaMemcpyHostToDevice, ws->front));
+    if (copier) {
+        copier(s, buf[i].p, ws->front);
+    } else {
+        const auto [rows, bytes] = src(s);
+        if (bytes) LGPU_CUDA(cudaMemcpyAsync(buf[i].p, rows, bytes, cudaMemcpyHostToDevice, ws->front));
+    }
     LGPU_CUDA(cudaEventRecord(copied[i], ws->front));
 }
 
@@ -622,6 +633,15 @@ struct lgpu_index {
     // and `codes` the packed rows [nrows][nbytes_pad] in partition order, both zero-padded, and their popcounts
     uint32_t nbytes = 0, nbytes_pad = 0;
     DevBuf cent_pop, row_pop;
+    // IVF_SQ, IVF_RQ and binary IVF_FLAT whose codes did not fit in HBM at open (place_codes): `codes_host` holds them,
+    // pinned and mapped, in the layout `codes` would ([nrows][code_row_bytes]), and `codes` stays empty.  A search
+    // stages them through HBM in chunks of consecutive partitions, code_cut[c] .. code_cut[c + 1], at most code_stage
+    // bytes of rows each
+    PinnedBuf codes_host;
+    uint32_t code_row_bytes = 0;
+    size_t code_stage = 0;
+    std::vector<uint32_t> code_cut;
+    std::vector<uint64_t> h_part_off;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
     RowLive live;
@@ -1575,36 +1595,71 @@ static void filter_fixup(lgpu_index *ix, Workspace *ws, const IvfPlan &p, GroupA
     launch_select(sf, st);
 }
 
+// The scan of a row-major kind (sq, rq, ham) with `rows(a, X)` setting its rows to X.  An HBM index: one launch over
+// the whole tile queue of its own rows.  An index whose codes are in pinned host memory: a walk over the chunks of
+// code_cut through Workspace::stage.  Chunk c's probed partitions (part_cnt of the regroup, so the flagged queries'
+// probes in the maximum_nprobes pass) are copied into a staging buffer by launch_codes_copy_gated on the side stream
+// while chunk c - 1 is scanned; then the scan runs over chunk c's tiles alone (TileRange, its own claim counter), its
+// rows read from the buffer.  Nothing waits on the host but the deadline, checked between chunks.
+template <class Args, class Rows, class Launch>
+static void scan_codes(lgpu_index *ix, Workspace *ws, const GroupArgs &ga, Args a, Rows &&rows, Launch &&launch,
+                       const Deadline *deadline, cudaStream_t st)
+{
+    a.total_tiles = ga.total_tiles; a.tile_counter = ga.tile_counter; a.tile_desc = ga.tile_desc;
+    a.dist_out = ws->dist_out.as<float>();
+    if (!ix->codes_host.p) {
+        rows(a, ix->codes.p);
+        launch(a, 2 * ix->num_sms, st);
+        return;
+    }
+    const std::vector<uint32_t> &cut = ix->code_cut;
+    const uint64_t nc = cut.size() - 1, rb = ix->code_row_bytes;
+    unsigned long long *moved = ws->code_ctr.as<unsigned long long>();      // [0]: bytes copied; then the counters
+    uint32_t *ctr = ws->code_ctr.as<uint32_t>() + 2;
+    for (auto &b : ws->stage.buf) b.ensure(ix->code_stage);
+    LGPU_CUDA(cudaMemsetAsync(ctr, 0, nc * 4, st));
+    ws->stage.open(ws, st, nc, deadline, nullptr, [&](uint64_t c, void *buf, cudaStream_t fs) {
+        launch_codes_copy_gated(static_cast<const uint8_t *>(ix->codes_host.dev), static_cast<uint8_t *>(buf), rb,
+                                ix->part_off.as<uint64_t>(), ga.part_cnt, cut[c], cut[c + 1],
+                                (ix->h_part_off[cut[c + 1]] - ix->h_part_off[cut[c]]) * rb, moved, ix->num_sms, fs);
+    });
+    for (uint64_t c = 0; c < nc; c++) {
+        rows(a, ws->stage.take(c));
+        a.range = {ga.tile_off + cut[c], ga.tile_off_b + cut[c], cut[c + 1] - cut[c], (uint32_t)ix->h_part_off[cut[c]]};
+        a.tile_counter = ctr + c;
+        launch(a, 2 * ix->num_sms, st);
+        ws->stage.release(c);
+    }
+    ws->stage.close();
+}
+
 // IvfScan::exact_pq / sq / rq / pq4 / ham: the exact scan of every regrouped tile, then the PQ top-kk
 static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu_search_params &sp,
                       const IvfQueries &q, const GroupArgs &ga, RowFilter rf, const uint32_t *only, TopkOut pq,
-                      cudaStream_t st, const StageMarks &mark)
+                      cudaStream_t st, const StageMarks &mark, const Deadline *deadline)
 {
     if (p.scan == IvfScan::sq) {
         SqScanArgs qa{};
-        qa.codes = ix->codes.as<uint8_t>(); qa.xx = ix->sq_xx.as<uint32_t>();
+        qa.xx = ix->sq_xx.as<uint32_t>();
         qa.qcodes = ws->sq_q.as<uint8_t>(); qa.qq = ws->sq_qq.as<uint32_t>(); qa.dim_pad = ix->dim_pad;
-        qa.total_tiles = ga.total_tiles; qa.tile_counter = ga.tile_counter; qa.tile_desc = ga.tile_desc;
-        qa.dist_out = ws->dist_out.as<float>();
-        launch_sq_scan(qa, 2 * ix->num_sms, st);
+        scan_codes(ix, ws, ga, qa, [](SqScanArgs &a, void *X) { a.codes = static_cast<const uint8_t *>(X); },
+                   launch_sq_scan, deadline, st);
     } else if (p.scan == IvfScan::rq) {
         RqScanArgs ra{};
-        ra.codes = ix->codes.as<uint32_t>(); ra.add = ix->rq_add.as<float>(); ra.scale = ix->rq_scale.as<float>();
+        ra.add = ix->rq_add.as<float>(); ra.scale = ix->rq_scale.as<float>();
         ra.popc = ix->rq_popc.as<uint32_t>();
         ra.planes = ws->rq_planes.as<uint32_t>(); ra.slots = ws->rq_slots.as<RqSlot>();
         ra.dim = ix->dim; ra.wpr = ix->rq_wpr; ra.cosine = ix->metric == LGPU_COSINE;
-        ra.total_tiles = ga.total_tiles; ra.tile_counter = ga.tile_counter; ra.tile_desc = ga.tile_desc;
-        ra.dist_out = ws->dist_out.as<float>();
-        launch_rq_scan(ra, 2 * ix->num_sms, st);
+        scan_codes(ix, ws, ga, ra, [](RqScanArgs &a, void *X) { a.codes = static_cast<const uint32_t *>(X); },
+                   launch_rq_scan, deadline, st);
     } else if (p.scan == IvfScan::pq4) {
         launch_pq4_scan(pq4_args(ix, ws, ga), 2 * ix->num_sms, st);
     } else if (p.scan == IvfScan::ham) {
         HamScanArgs ha{};
-        ha.rows = ix->codes.as<uint8_t>(); ha.row_pop = ix->row_pop.as<uint32_t>(); ha.queries = q.h; ha.qpop = q.pop;
+        ha.row_pop = ix->row_pop.as<uint32_t>(); ha.queries = q.h; ha.qpop = q.pop;
         ha.nbytes_pad = ix->nbytes_pad;
-        ha.total_tiles = ga.total_tiles; ha.tile_counter = ga.tile_counter; ha.tile_desc = ga.tile_desc;
-        ha.dist_out = ws->dist_out.as<float>();
-        launch_ivf_ham_scan(ha, 2 * ix->num_sms, st);
+        scan_codes(ix, ws, ga, ha, [](HamScanArgs &a, void *X) { a.rows = static_cast<const uint8_t *>(X); },
+                   launch_ivf_ham_scan, deadline, st);
     } else {
         launch_scan2(scan_args(ix, ws, q.f, ga), ix->dsub, ix->num_sms, st);
     }
@@ -1664,7 +1719,7 @@ static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const fl
 // the flagged queries (maximum_nprobes widening) -- exact kernels, the other queries' outputs are left untouched.
 void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const IvfQueries &q, uint32_t B,
                    const lgpu_search_params &sp, uint32_t nprobes, TopkOut out, bool prof, RowFilter rf,
-                   const uint32_t *only = nullptr)
+                   const Deadline *deadline, const uint32_t *only = nullptr)
 {
     const IvfPlan p = ivf_plan(ix, B, nprobes, sp, rf.bits != nullptr, only != nullptr, scan_modes());
     const StageMarks mark{ws, prof};
@@ -1707,7 +1762,7 @@ void ivf_sub_batch(lgpu_index *ix, Workspace *ws, cudaStream_t st, const IvfQuer
             filter_fixup(ix, ws, p, ga, sc, rf, pq, st);
             mark(IVF_TOPK, st);
         } else {
-            ivf_exact(ix, ws, p, sp, prep, ga, rf, only, pq, st, mark);
+            ivf_exact(ix, ws, p, sp, prep, ga, rf, only, pq, st, mark, deadline);
         }
     }
     if (!p.refine) return;
@@ -1725,7 +1780,9 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32
     size_t per_q = std::max<size_t>(ix->pad_prefix[np_eff] * 4 + (size_t)ix->nlist * 4 + (size_t)ix->nch * 256 * 8 * 4, 4) +
                    ivf_kind_query_bytes(ix, nprobes, np_eff, kk) + large_k_query_bytes(kk) +
                    (kk > SELECT_KMAX ? (size_t)kk * 28 : 0);
-    size_t bs = workspace_budget() / per_q;
+    // an index whose codes are in pinned host memory leases its two staging buffers from the same budget
+    const size_t budget = workspace_budget(), stage = ix->codes_host.p ? 2 * ix->code_stage : 0;
+    size_t bs = (budget > stage ? budget - stage : 0) / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
     bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
     bs = std::max<size_t>(1, std::min<size_t>(bs, 65535));
@@ -1801,19 +1858,29 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const voi
         memset(g_stage_ms, 0, sizeof(g_stage_ms));
         memset(g_filter_stats, 0, sizeof(g_filter_stats));
         g_scanned_bytes = 0;
+        g_streamed_bytes = 0;
+    }
+    if (ix->codes_host.p) {        // the walk's byte count (code_ctr[0]) and one tile counter per chunk (scan_codes)
+        ws->code_ctr.ensure(8 + ix->code_cut.size() * 4);
+        LGPU_CUDA(cudaMemsetAsync(ws->code_ctr.p, 0, 8, st));
     }
     const IvfQueries qs = ivf_call_queries(ix, ws, st, d_q, B);
     const TopkOut out{d_ids, d_dist, d_cnt};
     for (uint32_t q0 = 0; q0 < B; q0 += bs) {
         uint32_t b = std::min(bs, B - q0);
         if (deadline && q0 > 0) deadline->wait(st, ws->ev[7]);      // the previous sub-batch, or LGPU_TIMEOUT
-        ivf_sub_batch(ix, ws, st, qs.at(q0), b, sp, nprobes, out.at(q0, sp.k), prof, rf);
+        ivf_sub_batch(ix, ws, st, qs.at(q0), b, sp, nprobes, out.at(q0, sp.k), prof, rf, deadline);
         if (prof) g_scanned_bytes += add_ivf_profile(ws, st, b) * ivf_row_bytes(ix);
         if (widen) {
             ws->widen.ensure((size_t)b * 4);
             launch_count_below(out.at(q0, sp.k).cnt, b, sp.k, ws->widen.as<uint32_t>(), st);
-            ivf_sub_batch(ix, ws, st, qs.at(q0), b, sp, np_max, out.at(q0, sp.k), false, rf, ws->widen.as<uint32_t>());
+            ivf_sub_batch(ix, ws, st, qs.at(q0), b, sp, np_max, out.at(q0, sp.k), false, rf, deadline,
+                          ws->widen.as<uint32_t>());
         }
+    }
+    if (prof && ix->codes_host.p) {   // every pass's copies, the maximum_nprobes widening's included
+        LGPU_CUDA(cudaMemcpyAsync(&g_streamed_bytes, ws->code_ctr.p, 8, cudaMemcpyDeviceToHost, st));
+        LGPU_CUDA(cudaStreamSynchronize(st));
     }
 }
 
@@ -2782,10 +2849,12 @@ static Route filtered_route(const uint32_t *allow, uint64_t allow_bits)
 static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, stream}; }
 
 // Whether the host route may capture a handle's calls into a CUDA graph: not a handle whose rows are on the host,
-// whose calls stream from pinned memory that an append moves, on a side stream (RowStore::walk)
+// whose calls stream from pinned memory that an append moves, on a side stream (RowStore::walk), nor an IVF index whose
+// codes are on the host, whose calls stage them on a side stream too (scan_codes) and check timeout_ms between chunks
 template <class H> static bool graph_capturable(const H *h)
 {
     if constexpr (std::is_base_of_v<lgpu_rows, H>) return !h->rows.on_host;
+    else if constexpr (std::is_base_of_v<lgpu_index, H>) return !h->codes_host.p;
     else return true;
 }
 
@@ -3143,6 +3212,17 @@ static uint64_t index_device_bytes(const lgpu_index *ix)
     return n;
 }
 
+// lgpu_index_code_bytes, lgpu_ivf_binary_code_bytes: the pinned bytes of an index's codes and where they are
+template <class H> static int code_bytes(const H *hp, uint64_t *bytes, int *placement)
+{
+    return guarded([&] {
+        LGPU_REQUIRE(bytes || placement, "null argument");
+        HandleRef<H> ix(const_cast<H *>(hp));
+        if (bytes) *bytes = ix->codes_host.bytes;
+        if (placement) *placement = ix->codes_host.p ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+    });
+}
+
 // Whether `bytes` of a handle's rows go to HBM at open: at most the cap the variable `cap_var` sets (read at every open;
 // unset = no cap, 0 = never HBM), and the device's free memory covers them plus the workspace budget (LGPU_WS_BYTES)
 // the handle's searches may lease
@@ -3153,6 +3233,73 @@ static bool rows_fit_hbm(const char *cap_var, uint64_t bytes)
     size_t free_b = 0, total_b = 0;
     LGPU_CUDA(cudaMemGetInfo(&free_b, &total_b));
     return cap > 0 && bytes <= cap && (uint64_t)free_b >= bytes + workspace_budget();
+}
+
+// Where an IVF_SQ, IVF_RQ or binary IVF_FLAT index keeps its codes, nrows x row_bytes in the scan's layout.  HBM when
+// they fit with room to spare (rows_fit_hbm under LGPU_CODES_HBM_BYTES): `codes` is allocated exactly, so that device
+// bytes of the two placements differ by the code bytes, and `hbm()` fills it as the kind always has.  Otherwise pinned,
+// mapped host memory the index owns, in the same layout, built in chunks of rows staged through one HBM buffer (never a
+// device copy of the whole index): fill(dst, r0, n) lays rows r0 .. r0 + n out at dst -- the HBM chunk, copied back
+// afterwards (fill_on_device), or the pinned memory, uploaded into the chunk -- and prep(chunk, r0, n) runs the kind's
+// per-row kernel on it: the kernel the HBM placement runs, so the stored bytes and the per-row terms are the same.  The chunks
+// of consecutive partitions a search stages (code_cut, each at most code_stage bytes: FLAT_STAGE_BYTES, or an eighth of
+// the workspace budget when that is smaller, never less than the largest partition) are cut here; two staging buffers
+// of the largest partition must fit the budget, or the open fails with LGPU_OOM.  IVF_HNSW_SQ (its graph walk reads
+// rows at random) and the PQ kinds keep their codes in HBM: they never come here.
+constexpr size_t CODE_PREP_BYTES = (size_t)64 << 20;
+
+template <class Hbm, class Fill, class Prep>
+static void place_codes(lgpu_index *ix, uint32_t row_bytes, bool fill_on_device, Hbm &&hbm, Fill &&fill, Prep &&prep)
+{
+    const uint64_t n = ix->nrows, bytes = n * row_bytes;
+    ix->code_row_bytes = row_bytes;
+    if (rows_fit_hbm("LGPU_CODES_HBM_BYTES", bytes)) {
+        ix->codes.ensure(std::max<size_t>(bytes, 16), true);
+        hbm();
+        return;
+    }
+    const uint32_t nlist = ix->nlist;
+    ix->h_part_off.assign(nlist + 1, 0);
+    uint64_t largest = 0;
+    for (uint32_t p = 0; p < nlist; p++) {
+        ix->h_part_off[p + 1] = ix->h_part_off[p] + ix->h_part_n[p];
+        largest = std::max<uint64_t>(largest, (uint64_t)ix->h_part_n[p] * row_bytes);
+    }
+    const size_t budget = workspace_budget();
+    if (2 * largest > budget) {
+        set_error("the largest partition's codes (" + std::to_string(largest) + " bytes) do not fit twice in the " +
+                  "workspace budget (LGPU_WS_BYTES) that stages an index whose codes are in host memory");
+        throw Failure{LGPU_OOM};
+    }
+    ix->code_stage = std::max<size_t>(std::min(FLAT_STAGE_BYTES, budget / 8), std::max<size_t>(largest, 16));
+    ix->code_cut.assign(1, 0);
+    uint64_t in_chunk = 0;
+    for (uint32_t p = 0; p < nlist; p++) {
+        const uint64_t b = (uint64_t)ix->h_part_n[p] * row_bytes;
+        if (in_chunk && in_chunk + b > ix->code_stage) { ix->code_cut.push_back(p); in_chunk = 0; }
+        in_chunk += b;
+    }
+    ix->code_cut.push_back(nlist);
+    ix->codes_host.alloc(bytes);
+    uint8_t *host = static_cast<uint8_t *>(ix->codes_host.p);
+    const uint64_t C = std::max<uint64_t>(1, CODE_PREP_BYTES / row_bytes);
+    DevBuf tmp;
+    tmp.ensure((size_t)std::min(n, C) * row_bytes + 16);
+    cudaStream_t st = nullptr;
+    for (uint64_t r0 = 0; r0 < n; r0 += C) {
+        const uint64_t c = std::min(C, n - r0);
+        uint8_t *chunk = tmp.as<uint8_t>();
+        if (fill_on_device) {
+            fill(chunk, r0, c);
+        } else {
+            fill(host + r0 * row_bytes, r0, c);
+            LGPU_CUDA(cudaMemcpyAsync(chunk, host + r0 * row_bytes, c * row_bytes, cudaMemcpyHostToDevice, st));
+        }
+        prep(chunk, r0, c);
+        if (fill_on_device)
+            LGPU_CUDA(cudaMemcpyAsync(host + r0 * row_bytes, chunk, c * row_bytes, cudaMemcpyDeviceToHost, st));
+        LGPU_CUDA(cudaStreamSynchronize(st));
+    }
 }
 
 // Where an index keeps its raw vectors ([nrows][dim] f32 on the host, borrowed for the open call), decided after
@@ -3278,7 +3425,18 @@ int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
         ix->dim_pad = sq_dim_pad(d->dim);
         ix->sq_lo = d->lo; ix->sq_hi = d->hi;
         open_ivf_common(ix, d, SQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
-        upload_sq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->sq_xx);
+        const uint32_t dim = d->dim, dim_pad = ix->dim_pad;
+        ix->sq_xx.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));       // (as upload_sq_rows sizes it)
+        place_codes(
+            ix, dim_pad, true, [&] { upload_sq_rows(d->codes, d->nrows, dim, ix->codes, ix->sq_xx); },
+            [&](uint8_t *dst, uint64_t r0, uint64_t n) {
+                LGPU_CUDA(cudaMemsetAsync(dst, 0, n * dim_pad, nullptr));
+                LGPU_CUDA(cudaMemcpy2DAsync(dst, dim_pad, d->codes + r0 * dim, dim, dim, n, cudaMemcpyHostToDevice,
+                                            nullptr));
+            },
+            [&](uint8_t *rows, uint64_t r0, uint64_t n) {
+                launch_sq_row_norms(rows, n, dim_pad, ix->sq_xx.as<uint32_t>() + r0, nullptr);
+            });
         return d->vectors;
     });
 }
@@ -3423,7 +3581,20 @@ int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
         ix = new_ivf(d->device, IvfKind::rq);
         ix->rq_wpr = rq_wpr(d->dim);
         open_ivf_common(ix, d, RQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
-        upload_rq_rows(d->codes, d->nrows, d->dim, ix->codes, ix->rq_popc);
+        const uint32_t dim = d->dim, wpr = ix->rq_wpr, nb = (dim + 7) / 8;
+        ix->rq_popc.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));     // (as upload_rq_rows sizes it)
+        place_codes(
+            ix, wpr * 4, true, [&] { upload_rq_rows(d->codes, d->nrows, dim, ix->codes, ix->rq_popc); },
+            [&](uint8_t *dst, uint64_t r0, uint64_t n) {
+                LGPU_CUDA(cudaMemsetAsync(dst, 0, n * wpr * 4, nullptr));
+                LGPU_CUDA(cudaMemcpy2DAsync(dst, (size_t)wpr * 4, d->codes + r0 * nb, nb, nb, n, cudaMemcpyHostToDevice,
+                                            nullptr));
+            },
+            [&](uint8_t *rows, uint64_t r0, uint64_t n) {
+                launch_rq_row_prep(reinterpret_cast<uint32_t *>(rows), n, dim, wpr, ix->rq_popc.as<uint32_t>() + r0,
+                                   nullptr);
+            });
+
         upload(ix->rq_add, d->add_factors, (size_t)d->nrows * 4);
         upload(ix->rq_scale, d->scale_factors, (size_t)d->nrows * 4);
         upload(ix->rq_rot, d->rotation, (size_t)d->dim * d->dim * 4);
@@ -3502,6 +3673,11 @@ int lgpu_index_host_bytes(const lgpu_index *ixh, uint64_t *bytes, int *placement
     });
 }
 
+int lgpu_index_code_bytes(const lgpu_index *ix, uint64_t *host_bytes, int *placement)
+{
+    return code_bytes(ix, host_bytes, placement);
+}
+
 int lgpu_debug_refine_host(const float *queries, uint32_t B, const float *rows, uint64_t N, uint32_t dim,
                            const uint64_t *pos, uint32_t nc, int metric, int device, float *out)
 {
@@ -3533,6 +3709,11 @@ int lgpu_debug_refine_host(const float *queries, uint32_t B, const float *rows, 
 int lgpu_last_scanned_code_bytes(uint64_t *bytes)
 {
     return guarded([&] { LGPU_REQUIRE(bytes, "null argument"); *bytes = g_scanned_bytes; });
+}
+
+int lgpu_last_streamed_code_bytes(uint64_t *bytes)
+{
+    return guarded([&] { LGPU_REQUIRE(bytes, "null argument"); *bytes = g_streamed_bytes; });
 }
 
 int lgpu_kernel_launch_count(uint64_t *count)
@@ -4080,12 +4261,27 @@ int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
             }
         };
         pack(d->centroids, d->nlist, ix->centroids, ix->cent_pop);
-        pack(d->vectors, d->nrows, ix->codes, ix->row_pop);
+        // the rows: in HBM as above, or packed on the host as a host binary handle packs them (ham_pack_host), their
+        // popcounts taken from chunks staged through HBM
+        ix->row_pop.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));     // (as `pack` sizes it)
+        place_codes(
+            ix, nbp, false, [&] { pack(d->vectors, d->nrows, ix->codes, ix->row_pop); },
+            [&](uint8_t *dst, uint64_t r0, uint64_t n) {
+                ham_pack_host(d->vectors + r0 * nb, n, nb, nbp, dst);
+            },
+            [&](uint8_t *rows, uint64_t r0, uint64_t n) {
+                launch_ham_pack(rows, nbp, nbp, n, nullptr, nbp, ix->row_pop.as<uint32_t>() + r0, nullptr);
+            });
         return nullptr;             // the packed rows are the index: no separate raw vectors
     });
 }
 
 void lgpu_ivf_binary_close(lgpu_ivf_binary *ix) { close_handle(ix); }
+
+int lgpu_ivf_binary_code_bytes(const lgpu_ivf_binary *ix, uint64_t *host_bytes, int *placement)
+{
+    return code_bytes(ix, host_bytes, placement);
+}
 
 static int ivf_binary_call(lgpu_ivf_binary *ixh, const Route &r, const uint8_t *q, uint32_t B,
                            const lgpu_search_params *p, uint64_t *ids, float *dist, uint32_t *cnt)

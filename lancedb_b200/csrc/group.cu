@@ -3,8 +3,11 @@
 // groups of up to 8 queries against one read of that partition's codes.  This is the
 // structural change versus the reference, which plans and runs each query vector
 // independently (rust/lancedb/src/table/query.rs:201-215, 334-381: "B independent
-// plans + UnionExec"); all of it is index arithmetic and exact.
+// plans + UnionExec"); all of it is index arithmetic and exact.  An index whose codes are in pinned host memory then
+// copies the probed partitions of each chunk into HBM by the part_cnt the regroup leaves (codes_copy_gated_kernel).
 #include "kernels.cuh"
+
+#include <algorithm>
 
 namespace lgpu {
 
@@ -214,7 +217,66 @@ __global__ void tile_desc_kernel(GroupArgs a)
     }
 }
 
+// One chunk of a host-resident index's codes into its staging buffer (launch_codes_copy_gated).  The chunk's bytes are
+// cut into CODES_SEG-byte segments, grid-strided over the CTAs; a segment's partitions are found by a binary search over
+// part_off, and only the bytes of the probed ones (part_cnt[p] > 0) are read from the mapped host memory, 4 x 16 bytes
+// per thread in flight.  An unprobed partition costs its segments one search and no transfer.
+constexpr uint64_t CODES_SEG = 32768;
+constexpr int CODES_NT = 256;
+
+__global__ void __launch_bounds__(CODES_NT) codes_copy_gated_kernel(const uint4 *__restrict__ src, uint4 *__restrict__ dst,
+                                                                    uint64_t row_bytes, const uint64_t *__restrict__ part_off,
+                                                                    const uint32_t *__restrict__ part_cnt, uint32_t p0,
+                                                                    uint32_t p1, uint64_t chunk_bytes,
+                                                                    unsigned long long *moved)
+{
+    pdl_entry();
+    const uint64_t row0 = part_off[p0];
+    const uint4 *from = src + row0 * row_bytes / 16;
+    const uint64_t nseg = (chunk_bytes + CODES_SEG - 1) / CODES_SEG;
+    for (uint64_t sg = blockIdx.x; sg < nseg; sg += gridDim.x) {
+        const uint64_t s0 = sg * CODES_SEG, s1 = min(chunk_bytes, s0 + CODES_SEG);
+        uint32_t lo = p0, hi = p1 - 1;                     // the last partition starting at or before s0
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if ((part_off[mid] - row0) * row_bytes <= s0) lo = mid; else hi = mid - 1;
+        }
+        for (uint32_t p = lo; p < p1; p++) {
+            const uint64_t pa = (part_off[p] - row0) * row_bytes, pb = (part_off[p + 1] - row0) * row_bytes;
+            if (pa >= s1) break;
+            if (!part_cnt[p]) continue;
+            const uint64_t w0 = max(pa, s0) / 16, w1 = min(pb, s1) / 16;
+            if (w0 >= w1) continue;
+            for (uint64_t w = w0 + threadIdx.x; w < w1; w += 4 * CODES_NT) {
+                uint4 v[4];
+#pragma unroll
+                for (int j = 0; j < 4; j++) if (w + j * CODES_NT < w1) v[j] = from[w + j * CODES_NT];
+#pragma unroll
+                for (int j = 0; j < 4; j++) if (w + j * CODES_NT < w1) dst[w + j * CODES_NT] = v[j];
+            }
+            if (moved && threadIdx.x == 0) atomicAdd(moved, (unsigned long long)(w1 - w0) * 16);
+        }
+    }
+}
+
 }  // namespace
+
+void launch_codes_copy_gated(const uint8_t *src, uint8_t *dst, uint64_t row_bytes, const uint64_t *part_off,
+                             const uint32_t *part_cnt, uint32_t p0, uint32_t p1, uint64_t chunk_bytes,
+                             unsigned long long *moved, int num_sms, cudaStream_t st)
+{
+    if (p1 <= p0 || chunk_bytes == 0) return;
+    if (row_bytes % 16) {
+        set_error("internal: staged code rows must be a multiple of 16 bytes");
+        throw Failure{LGPU_RUNTIME};
+    }
+    const uint64_t nseg = (chunk_bytes + CODES_SEG - 1) / CODES_SEG;
+    const unsigned grid = (unsigned)std::min<uint64_t>(nseg, 4ull * num_sms);
+    launch_k(codes_copy_gated_kernel, dim3(grid), dim3(CODES_NT), 0, st, reinterpret_cast<const uint4 *>(src),
+             reinterpret_cast<uint4 *>(dst), row_bytes, part_off, part_cnt, p0, p1, chunk_bytes, moved);
+    LGPU_COUNT_LAUNCH();
+    LGPU_CUDA(cudaGetLastError());
+}
 
 void launch_group(const GroupArgs &a, cudaStream_t st)
 {

@@ -40,7 +40,7 @@ __device__ __forceinline__ void ham_rows(const HamScanArgs &a, const TileDesc &T
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         const uint32_t r = min(r0 + (uint32_t)(g + 8 * i), row_end - 1u);
-        arow[i] = reinterpret_cast<const uint2 *>(a.rows + ((uint64_t)T.part_off32 + r) * nbp + 8 * t);
+        arow[i] = reinterpret_cast<const uint2 *>(a.rows + ((uint64_t)(T.part_off32 - a.range.row_shift) + r) * nbp + 8 * t);
     }
     const uint32_t qg = (uint32_t)g < T.ng ? T.q[g] : T.q[0];
     const uint2 *bq = reinterpret_cast<const uint2 *>(a.queries + (uint64_t)qg * nbp + 8 * t);
@@ -95,12 +95,13 @@ __global__ void __launch_bounds__(HAM_NT, 2) ivf_ham_scan_kernel(HamScanArgs a)
     __shared__ TileDesc s_tile;
     __shared__ uint32_t s_t;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t total = *a.total_tiles;
+    const uint32_t total = tile_range_total(a.range, a.total_tiles);
     if (tid == 0) s_t = atomicAdd(a.tile_counter, 1u);
     __syncthreads();
     for (uint32_t t = s_t; t < total;) {
+        const TileDesc *d = a.tile_desc + tile_range_at(a.range, t);
         if (tid < (int)(sizeof(TileDesc) / 4))
-            reinterpret_cast<uint32_t *>(&s_tile)[tid] = __ldg(reinterpret_cast<const uint32_t *>(a.tile_desc + t) + tid);
+            reinterpret_cast<uint32_t *>(&s_tile)[tid] = __ldg(reinterpret_cast<const uint32_t *>(d) + tid);
         __syncthreads();                                   // s_tile written; every thread has read s_t
         uint32_t next = 0;
         if (tid == 0) next = atomicAdd(a.tile_counter, 1u);

@@ -39,6 +39,30 @@ struct alignas(16) TileDesc {
 };
 static_assert(sizeof(TileDesc) == 128, "TileDesc layout");
 
+// The tiles of one chunk of consecutive partitions [p0, p0 + n) of a row-major IVF index whose codes are staged through
+// HBM (IVF_SQ, IVF_RQ and binary IVF_FLAT with codes in pinned host memory): the regroup numbers each partition's tiles
+// in two contiguous ranges, so the chunk's tiles are [a[0], a[n]) and [b[0], b[n]) (a = tile_off + p0, b = tile_off_b +
+// p0, device).  The staged rows start at row `row_shift` of the index: a tile's row r of partition p is read at
+// part_off[p] + r - row_shift of the staging buffer, while the per-row terms keep their absolute row.  a == nullptr: the
+// whole tile queue (*total_tiles tiles) over the index's own rows.
+struct TileRange {
+    const uint32_t *a, *b;
+    uint32_t n;
+    uint32_t row_shift;
+};
+// tiles the scan claims: the chunk's, or the whole queue's
+__device__ __forceinline__ uint32_t tile_range_total(const TileRange &r, const uint32_t *total_tiles)
+{
+    return r.a ? (r.a[r.n] - r.a[0]) + (r.b[r.n] - r.b[0]) : *total_tiles;
+}
+// the tile descriptor of claim t < tile_range_total
+__device__ __forceinline__ uint32_t tile_range_at(const TileRange &r, uint32_t t)
+{
+    if (!r.a) return t;
+    const uint32_t a0 = r.a[0], na = r.a[r.n] - a0;
+    return t < na ? a0 + t : r.b[0] + (t - na);
+}
+
 // one surviving row of the filter scan's candidate mode
 struct alignas(16) CandRec {
     float lb;                     // lower bound L of the row's distance
@@ -107,6 +131,7 @@ struct SqScanArgs {
     const TileDesc *tile_desc;    // built with rows_tile == SQ_ROWS_TILE
     float *dist_out;              // segment of slot e at out[e]: (float) sum_i (k_i - q_i)^2 of row r at out[e] + r
     int out_u32;                  // 1: write the exact u32 sums instead (lgpu_debug_sq_distances)
+    TileRange range;              // optional: one staged chunk's tiles, `codes` its staging buffer
 };
 // qc[b] = the codes of query b (sat_u8(((double)q - lo) * 255 / (hi - lo)), zero-padded to dim_pad), qq[b] = |qc[b]|^2
 void launch_sq_encode(const float *Q, uint32_t B, uint32_t dim, uint32_t dim_pad, double lo, double hi, uint8_t *qc,
@@ -161,6 +186,7 @@ struct RqScanArgs {
     const TileDesc *tile_desc;    // built with rows_tile == RQ_ROWS_TILE; slot[] addresses planes / slots
     float *dist_out;              // segment of slot e at out[e]: the estimate of row r at out[e] + r
     int out_ip;                   // 1: write the exact u32 ip = sum_i b_i u_i instead (lgpu_debug_rq_distances)
+    TileRange range;              // optional: one staged chunk's tiles, `codes` its staging buffer
 };
 // out[v][i] = lance_dot(P row i, x[v]): the rotation of n vectors by P [dim][dim]
 void launch_rq_rotate(const float *P, const float *x, uint32_t n, uint32_t dim, float *out, cudaStream_t st);
@@ -185,8 +211,16 @@ struct HamScanArgs {
     const TileDesc *tile_desc;    // built with rows_tile == HAM_ROWS_TILE; q[] addresses queries / qpop
     float *dist_out;              // segment of slot e at out[e]: popc(q XOR x) of row r at out[e] + r, as f32
     int out_u32;                  // 1: write the u32 distances instead (lgpu_debug_ivf_hamming_scan)
+    TileRange range;              // optional: one staged chunk's tiles, `rows` its staging buffer
 };
 void launch_ivf_ham_scan(const HamScanArgs &a, int grid, cudaStream_t st);
+// One chunk of a row-major IVF index's codes (rows [part_off[p0], part_off[p1]), row_bytes each, a multiple of 16) from
+// pinned host memory (src: the mapped alias of the whole store) into the staging buffer dst, which holds row
+// part_off[p0] at byte 0: only the partitions some probe slot scans (part_cnt[p] > 0), the others skipped at once.
+// *moved (optional) += the bytes copied.  Reads the offsets and counts on the device: no host synchronisation.
+void launch_codes_copy_gated(const uint8_t *src, uint8_t *dst, uint64_t row_bytes, const uint64_t *part_off,
+                             const uint32_t *part_cnt, uint32_t p0, uint32_t p1, uint64_t chunk_bytes,
+                             unsigned long long *moved, int num_sms, cudaStream_t st);
 // probes[q][j] = j for q < B, j < nlist: every partition, for nprobes >= nlist (no coarse step, no top-nprobes select)
 void launch_ham_all_probes(uint64_t *probes, uint32_t B, uint32_t nlist, cudaStream_t st);
 

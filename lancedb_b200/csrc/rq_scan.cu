@@ -210,7 +210,7 @@ __device__ __forceinline__ void rq_tile(const RqScanArgs &a, const TileDesc &T, 
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         const uint32_t r = min(r0 + (uint32_t)(g + 8 * i), row_end - 1u);      // rows past the tile: re-read, not written
-        arow[i] = reinterpret_cast<const uint2 *>(a.codes + ((uint64_t)T.part_off32 + r) * wpr + 2 * t);
+        arow[i] = reinterpret_cast<const uint2 *>(a.codes + ((uint64_t)(T.part_off32 - a.range.row_shift) + r) * wpr + 2 * t);
     }
     const uint32_t eg = (uint32_t)g < T.ng ? T.slot[g] : T.slot[0];
     const uint2 *bp = reinterpret_cast<const uint2 *>(a.planes + (uint64_t)eg * 4 * wpr + 2 * t);
@@ -287,12 +287,13 @@ __global__ void __launch_bounds__(RQ_NT, 2) rq_scan_kernel(RqScanArgs a)
     __shared__ TileDesc s_tile;
     __shared__ uint32_t s_t;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t total = *a.total_tiles;
+    const uint32_t total = tile_range_total(a.range, a.total_tiles);
     if (tid == 0) s_t = atomicAdd(a.tile_counter, 1u);
     __syncthreads();
     for (uint32_t t = s_t; t < total;) {
+        const TileDesc *d = a.tile_desc + tile_range_at(a.range, t);
         if (tid < (int)(sizeof(TileDesc) / 4))
-            reinterpret_cast<uint32_t *>(&s_tile)[tid] = __ldg(reinterpret_cast<const uint32_t *>(a.tile_desc + t) + tid);
+            reinterpret_cast<uint32_t *>(&s_tile)[tid] = __ldg(reinterpret_cast<const uint32_t *>(d) + tid);
         __syncthreads();                                   // s_tile written; every thread has read s_t
         uint32_t next = 0;
         if (tid == 0) next = atomicAdd(a.tile_counter, 1u);

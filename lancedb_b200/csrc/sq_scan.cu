@@ -101,7 +101,7 @@ __device__ __forceinline__ void sq_tile(const SqScanArgs &a, const TileDesc &T, 
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         const uint32_t r = min(r0 + (uint32_t)(g + 8 * i), row_end - 1u);      // rows past the tile: re-read, not written
-        arow[i] = a.codes + ((uint64_t)T.part_off32 + r) * a.dim_pad + 16 * t;
+        arow[i] = a.codes + ((uint64_t)(T.part_off32 - a.range.row_shift) + r) * a.dim_pad + 16 * t;
     }
     const uint32_t qg = (uint32_t)g < T.ng ? T.q[g] : T.q[0];
     const uint8_t *brow = a.qcodes + (uint64_t)qg * a.dim_pad + 16 * t;
@@ -147,14 +147,15 @@ __global__ void __launch_bounds__(SQ_NT, 2) sq_scan_kernel(SqScanArgs a)
     __shared__ TileDesc s_tile;
     __shared__ uint32_t s_t;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t total = *a.total_tiles;
+    const uint32_t total = tile_range_total(a.range, a.total_tiles);
     for (;;) {
         if (tid == 0) s_t = atomicAdd(a.tile_counter, 1u);
         __syncthreads();
         const uint32_t t = s_t;
         if (t >= total) break;
+        const TileDesc *d = a.tile_desc + tile_range_at(a.range, t);
         if (tid < (int)(sizeof(TileDesc) / 4))
-            reinterpret_cast<uint32_t *>(&s_tile)[tid] = __ldg(reinterpret_cast<const uint32_t *>(a.tile_desc + t) + tid);
+            reinterpret_cast<uint32_t *>(&s_tile)[tid] = __ldg(reinterpret_cast<const uint32_t *>(d) + tid);
         __syncthreads();
         sq_tile(a, s_tile, warp, lane);
         __syncthreads();                                   // s_t and s_tile are rewritten by the next claim
