@@ -303,15 +303,17 @@ class _Handle:
     __del__ = close
 
 
+def _placement(h, fn: str):
+    """(pinned host bytes, placement) of handle `h` from `fn`, its lgpu_*_host_bytes or lgpu_*_code_bytes."""
+    b, where = C.c_uint64(0), C.c_int(0)
+    check(getattr(load(), fn)(h, C.byref(b), C.byref(where)))
+    return b.value, where.value
+
+
 class _Placed:
     """A handle that reports where it keeps its rows, through lgpu_*_device_bytes and lgpu_*_host_bytes, `_bytes` the
     lgpu_* prefix."""
     _bytes = ""
-
-    def _host(self):
-        b, where = C.c_uint64(0), C.c_int(0)
-        check(getattr(load(), self._bytes + "_host_bytes")(self._h, C.byref(b), C.byref(where)))
-        return b.value, where.value
 
     def _device_bytes(self) -> int:
         n = C.c_uint64(0)
@@ -321,7 +323,7 @@ class _Placed:
     def host_bytes(self) -> int:
         """The pinned host memory the handle holds: the row data that did not fit in HBM at open, else 0
         (lgpu_*_host_bytes)."""
-        return self._host()[0]
+        return _placement(self._h, self._bytes + "_host_bytes")[0]
 
 
 class _Codes:
@@ -330,19 +332,14 @@ class _Codes:
     memory, the probed partitions streamed through the GPU by every search, with the same results."""
     _codes = ""
 
-    def _code_placement(self):
-        b, where = C.c_uint64(0), C.c_int(0)
-        check(getattr(load(), self._codes)(self._h, C.byref(b), C.byref(where)))
-        return b.value, where.value
-
     @property
     def codes_on_host(self) -> bool:
         """True when the codes are kept in pinned host memory and every search stages its probed partitions."""
-        return self._code_placement()[1] == VECTORS_HOST
+        return _placement(self._h, self._codes)[1] == VECTORS_HOST
 
     def code_host_bytes(self) -> int:
         """The pinned host memory the index holds for its codes (their padded layout), 0 when they are in HBM."""
-        return self._code_placement()[0]
+        return _placement(self._h, self._codes)[0]
 
 
 class _RowsHandle(_Handle):
@@ -370,7 +367,7 @@ class _Column(_Placed, _RowsHandle):
     @property
     def rows_on_host(self) -> bool:
         """True when the rows are kept in pinned host memory and every search streams them through the GPU."""
-        return self._host()[1] == VECTORS_HOST
+        return _placement(self._h, self._bytes + "_host_bytes")[1] == VECTORS_HOST
 
 
 def _host_search(fn: str, head, B: int, k: int, p: SearchParams, allow, allow_bits):
@@ -483,7 +480,7 @@ class GpuIvfPq(_Placed, _Codes, _RowsHandle):
     @property
     def vectors_on_host(self) -> bool:
         """True when the raw vectors (refine_factor) are kept in pinned host memory and refine reads them over PCIe."""
-        return self._host()[1] == VECTORS_HOST
+        return _placement(self._h, self._bytes + "_host_bytes")[1] == VECTORS_HOST
 
     def search(self, queries, k=10, nprobes=20, refine_factor=0, lower=None, upper=None, allow=None, allow_bits=0,
                max_nprobes=0, timeout_ms=0, ef=0):

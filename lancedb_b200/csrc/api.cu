@@ -154,16 +154,13 @@ struct Deadline {
 
 struct Workspace;
 
-// Rows streamed from pinned host memory through HBM (the search of a host flat, binary or multivector handle).  Between open
-// and close, chunk s of `steps` is copied into buf[s & 1] by cudaMemcpyAsync on the workspace's side stream (`front`,
-// forked from the call's stream and joined back to it), chunk s + 1 while chunk s is used on the call's stream:
-// take(s) hands over chunk s once the copy of chunk s + 1 is issued, release(s) marks every use of it enqueued.
-// copied[i]: buf[i] holds its chunk (side stream); freed[i]: the uses of its chunk are enqueued (call's stream), so the
-// copy two steps later may overwrite it.  timeout_ms is checked between chunks.  A walk that copies by a kernel of its
-// own instead (an IVF index's probed partitions, launch_codes_copy_gated) passes `copier`, which enqueues chunk s into
-// the buffer it is given on the side stream, in place of the cudaMemcpyAsync of src(s).
+// Rows streamed from pinned host memory through HBM (RowStore::walk).  Between open and close, chunk s of `steps` is
+// copied into buf[s & 1] by copier(s, buf, front) on the workspace's side stream (`front`, forked from the call's
+// stream and joined back to it), chunk s + 1 while chunk s is used on the call's stream: take(s) hands over chunk s
+// once the copy of chunk s + 1 is issued, release(s) marks every use of it enqueued.  copied[i]: buf[i] holds its chunk
+// (side stream); freed[i]: the uses of its chunk are enqueued (call's stream), so the copy two steps later may
+// overwrite it.  timeout_ms is checked between chunks.
 struct Staging {
-    using Source = std::function<std::pair<const void *, size_t>(uint64_t)>;   // chunk s: its pinned rows and bytes
     using Copier = std::function<void(uint64_t, void *, cudaStream_t)>;        // chunk s into a buffer, on a stream
     DevBuf buf[2];
     cudaEvent_t copied[2] = {}, freed[2] = {};
@@ -181,8 +178,7 @@ struct Staging {
             if (freed[i]) cudaEventDestroy(freed[i]);
         }
     }
-    void open(Workspace *ws, cudaStream_t st, uint64_t steps, const Deadline *deadline, Source src,
-              Copier copier = nullptr);
+    void open(Workspace *ws, cudaStream_t st, uint64_t steps, const Deadline *deadline, Copier copier);
     void *take(uint64_t s);
     void release(uint64_t s) { LGPU_CUDA(cudaEventRecord(freed[s & 1], st)); }
     void close();
@@ -192,7 +188,6 @@ struct Staging {
     cudaStream_t st = nullptr;
     uint64_t steps = 0;
     const Deadline *deadline = nullptr;
-    Source src;
     Copier copier;
 };
 
@@ -266,9 +261,9 @@ struct Workspace {
     }
 };
 
-void Staging::open(Workspace *w, cudaStream_t s, uint64_t n, const Deadline *dl, Source source, Copier cp)
+void Staging::open(Workspace *w, cudaStream_t s, uint64_t n, const Deadline *dl, Copier cp)
 {
-    ws = w; st = s; steps = n; deadline = dl; src = std::move(source); copier = std::move(cp);
+    ws = w; st = s; steps = n; deadline = dl; copier = std::move(cp);
     LGPU_CUDA(cudaEventRecord(ws->ev_fork, st));
     LGPU_CUDA(cudaStreamWaitEvent(ws->front, ws->ev_fork, 0));
     ws->front_open = true;
@@ -280,12 +275,7 @@ void Staging::copy(uint64_t s)
 {
     const int i = (int)(s & 1);
     if (s >= 2) LGPU_CUDA(cudaStreamWaitEvent(ws->front, freed[i], 0));
-    if (copier) {
-        copier(s, buf[i].p, ws->front);
-    } else {
-        const auto [rows, bytes] = src(s);
-        if (bytes) LGPU_CUDA(cudaMemcpyAsync(buf[i].p, rows, bytes, cudaMemcpyHostToDevice, ws->front));
-    }
+    copier(s, buf[i].p, ws->front);
     LGPU_CUDA(cudaEventRecord(copied[i], ws->front));
 }
 
@@ -348,9 +338,9 @@ struct RowChunk {
     bool resident;
 };
 
-// The stored rows of a flat, binary or multivector handle, [n][row bytes]: in HBM, or -- when the open found they do
-// not fit there (rows_fit_hbm) -- in pinned host memory mapped into the device's address space, which searches stream
-// through HBM.  The placement is fixed at open.
+// Stored rows, [n][row bytes] -- a flat, binary or multivector handle's rows, an IVF index's codes or raw vectors: in
+// HBM, or -- when the open found they do not fit there (rows_fit_hbm) -- in pinned host memory mapped into the device's
+// address space, which searches stream through HBM or read over PCIe.  The placement is fixed at open.
 struct RowStore {
     bool on_host = false;
     DevBuf hbm;
@@ -395,10 +385,11 @@ struct RowStore {
     // use(RowChunk) for `passes` passes over the chunks cut[c]..cut[c + 1] (row r at byte at(r)), then after(s) once
     // step s's staging buffer is released.  An HBM store is one resident chunk [cut.front(), cut.back()) per pass, the
     // deadline checked between passes; a host store streams each chunk through Workspace::stage, which checks it
-    // between steps.
+    // between steps.  Chunk s is copied into its staging buffer by `copier` when the caller gives one, else by a
+    // cudaMemcpyAsync of its pinned rows.
     template <class At, class Use, class After>
     void walk(Workspace *ws, cudaStream_t st, const std::vector<uint64_t> &cut, uint64_t passes, At &&at,
-              const Deadline *deadline, Use &&use, After &&after) const
+              const Deadline *deadline, Use &&use, After &&after, Staging::Copier copier = nullptr) const
     {
         const uint64_t nc = cut.size() - 1;
         if (!on_host) {
@@ -409,10 +400,14 @@ struct RowStore {
             }
             return;
         }
-        ws->stage.open(ws, st, passes * nc, deadline, [&](uint64_t s) -> std::pair<const void *, size_t> {
-            const uint64_t c = s % nc;
-            return {static_cast<const char *>(host.p) + at(cut[c]), at(cut[c + 1]) - at(cut[c])};
-        });
+        if (!copier)
+            copier = [&](uint64_t s, void *buf, cudaStream_t fs) {
+                const uint64_t c = s % nc, bytes = at(cut[c + 1]) - at(cut[c]);
+                if (bytes)
+                    LGPU_CUDA(cudaMemcpyAsync(buf, static_cast<const char *>(host.p) + at(cut[c]), bytes,
+                                              cudaMemcpyHostToDevice, fs));
+            };
+        ws->stage.open(ws, st, passes * nc, deadline, std::move(copier));
         for (uint64_t s = 0; s < passes * nc; s++) {
             const uint64_t c = s % nc;
             use(RowChunk{s, cut[c], cut[c + 1], ws->stage.take(s), false});
@@ -423,9 +418,9 @@ struct RowStore {
     }
     template <class At, class Use>
     void walk(Workspace *ws, cudaStream_t st, const std::vector<uint64_t> &cut, At &&at, const Deadline *deadline,
-              Use &&use) const
+              Use &&use, Staging::Copier copier = nullptr) const
     {
-        walk(ws, st, cut, 1, at, deadline, use, [](uint64_t) {});
+        walk(ws, st, cut, 1, at, deadline, use, [](uint64_t) {}, std::move(copier));
     }
 };
 
@@ -600,7 +595,16 @@ struct lgpu_index {
     uint32_t max_nrb = 1;          // row blocks (of 1536 rows) of the largest partition: bounds the tile count
     int metric = 0;
     uint64_t nrows = 0, device_bytes = 0;
-    DevBuf centroids, cb_tiled, codes, code_base, part_n, part_npad, part_off, row_ids, vectors;
+    DevBuf centroids, cb_tiled, code_base, part_n, part_npad, part_off, row_ids;
+    // the stored codes, in the scan's layout.  IVF_SQ, IVF_RQ and binary IVF_FLAT place them at open (place_codes):
+    // [nrows][code_row_bytes] in HBM, or in pinned host memory, which a search stages through HBM in chunks of
+    // consecutive partitions, code_cut[c] .. code_cut[c + 1] (rows code_rows[c] .. code_rows[c + 1]), at most
+    // code_stage bytes each.  The PQ kinds and IVF_HNSW_SQ keep them in `codes.hbm`.
+    RowStore codes;
+    uint32_t code_row_bytes = 0;
+    size_t code_stage = 0;
+    std::vector<uint32_t> code_cut;
+    std::vector<uint64_t> code_rows;
     DevBuf row_R, rmax_bits;            // filter scan: per-row constant 2 b.c and max |R| (tables.cu)
     DevBuf cb_n2;                       // filter scan: |b|^2 of every tiled codebook entry
     float cb2 = 0.f;                    // sum_i max_c |codebook_i[c]|^2 (error budget of the filter's table entries)
@@ -611,9 +615,9 @@ struct lgpu_index {
     float cent_max = 0.f, cent_err = 0.f;   // max |c|, max |bf16(c) - c| (the error band, kernels.cuh tc_band)
     bool has_tc = false;
     bool has_vectors = false;
-    // the raw vectors (refine_factor) live in `vectors` (HBM, [nrows][dim]) or, when they do not fit there
-    // (place_vectors), in `vectors_host`: [nrows][vec_stride] f32, vec_stride = dim rounded up to 4, padding zero
-    PinnedBuf vectors_host;
+    // the raw vectors (refine_factor), placed by place_vectors: [nrows][vec_stride] f32, vec_stride = dim in HBM, or dim
+    // rounded up to 4 (padding zero) in pinned host memory
+    RowStore vectors;
     uint32_t vec_stride = 0;
     // IVF_SQ (lgpu_ivf_sq_open): `codes` holds [nrows][dim_pad] u8 row codes, `sq_xx` the sum of each row's squared codes
     uint32_t dim_pad = 0;
@@ -633,15 +637,6 @@ struct lgpu_index {
     // and `codes` the packed rows [nrows][nbytes_pad] in partition order, both zero-padded, and their popcounts
     uint32_t nbytes = 0, nbytes_pad = 0;
     DevBuf cent_pop, row_pop;
-    // IVF_SQ, IVF_RQ and binary IVF_FLAT whose codes did not fit in HBM at open (place_codes): `codes_host` holds them,
-    // pinned and mapped, in the layout `codes` would ([nrows][code_row_bytes]), and `codes` stays empty.  A search
-    // stages them through HBM in chunks of consecutive partitions, code_cut[c] .. code_cut[c + 1], at most code_stage
-    // bytes of rows each
-    PinnedBuf codes_host;
-    uint32_t code_row_bytes = 0;
-    size_t code_stage = 0;
-    std::vector<uint32_t> code_cut;
-    std::vector<uint64_t> h_part_off;
     std::vector<uint64_t> pad_prefix;   // prefix sums of pad4(n_p) sorted descending
     std::vector<uint32_t> h_part_n;
     RowLive live;
@@ -1398,7 +1393,7 @@ static void ivf_small(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
     ws->dist_out.ensure((size_t)p.slots * stride * 4);
     SmallScanArgs ss{};
     ss.centroids = ix->centroids.as<float>(); ss.cb_tiled = ix->cb_tiled.as<float>();
-    ss.codes = ix->codes.as<unsigned char>(); ss.code_base = ix->code_base.as<uint64_t>();
+    ss.codes = ix->codes.hbm.as<unsigned char>(); ss.code_base = ix->code_base.as<uint64_t>();
     ss.part_n = ix->part_n.as<uint32_t>(); ss.part_npad = ix->part_npad.as<uint32_t>();
     ss.dim = ix->dim; ss.m = ix->m; ss.nch = ix->nch; ss.metric = (uint32_t)ix->metric; ss.nlist = ix->nlist;
     ss.nprobes = p.nprobes;
@@ -1454,7 +1449,7 @@ static ScanArgs scan_args(lgpu_index *ix, Workspace *ws, const float *qs, const 
 {
     ScanArgs sc{};
     sc.centroids = ix->centroids.as<float>(); sc.cb_tiled = ix->cb_tiled.as<float>();
-    sc.codes = ix->codes.as<unsigned char>(); sc.code_base = ix->code_base.as<uint64_t>();
+    sc.codes = ix->codes.hbm.as<unsigned char>(); sc.code_base = ix->code_base.as<uint64_t>();
     sc.part_n = ix->part_n.as<uint32_t>(); sc.part_npad = ix->part_npad.as<uint32_t>();
     sc.dim = ix->dim; sc.m = ix->m; sc.nch = ix->nch; sc.metric = (uint32_t)ix->metric; sc.nlist = ix->nlist;
     sc.rows_tile = ga.rows_tile; sc.fzero2 = 0ull;
@@ -1479,7 +1474,7 @@ static void pq4_tables(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const fl
 static Pq4ScanArgs pq4_args(lgpu_index *ix, Workspace *ws, const GroupArgs &ga)
 {
     Pq4ScanArgs a{};
-    a.codes = ix->codes.as<uint32_t>(); a.tables = ws->pq4_tab.as<uint8_t>(); a.slots = ws->pq4_slots.as<Pq4Slot>();
+    a.codes = ix->codes.hbm.as<uint32_t>(); a.tables = ws->pq4_tab.as<uint8_t>(); a.slots = ws->pq4_slots.as<Pq4Slot>();
     a.m = ix->m; a.metric = (uint32_t)ix->metric;
     a.total_tiles = ga.total_tiles; a.tile_counter = ga.tile_counter; a.tile_desc = ga.tile_desc;
     a.dist_out = ws->dist_out.as<float>();
@@ -1531,7 +1526,7 @@ static void filter_candidates(lgpu_index *ix, Workspace *ws, const IvfPlan &p, c
     FinalizeArgs fa{};
     fa.Q = qs; fa.cand = sc.cand; fa.cand_cnt = sc.cand_cnt; fa.cand_cap = cap; fa.cand_key = sc.cand_key; fa.thr = sc.thr;
     fa.slack = sc.slack; fa.bad = ws->qt_bad.as<uint32_t>();
-    fa.codes = ix->codes.as<unsigned char>(); fa.code_base = ix->code_base.as<uint64_t>();
+    fa.codes = ix->codes.hbm.as<unsigned char>(); fa.code_base = ix->code_base.as<uint64_t>();
     fa.part_npad = ix->part_npad.as<uint32_t>(); fa.part_off = ix->part_off.as<uint64_t>();
     fa.row_ids = ix->row_ids.as<uint64_t>(); fa.centroids = ix->centroids.as<float>();
     fa.cb_tiled = ix->cb_tiled.as<float>();
@@ -1570,7 +1565,7 @@ static void filter_dense(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const 
                        dot ? nullptr : ws->amax.as<float>(), dot ? nullptr : ix->rmax_bits.as<int>(),
                        ws->qt_bad.as<uint32_t>(), ws->qn2.as<float>(), ix->cb2, mscale, ix->m, dot, B, p.kk, kp,
                        ws->flags.as<uint32_t>(), ws->c_wcnt.as<uint32_t>() + 1, ws->c_surv.as<uint32_t>(), st);
-    launch_pq_rescore(qs, ws->s_pos.as<uint64_t>(), B, kp, ix->codes.as<unsigned char>(), ix->code_base.as<uint64_t>(),
+    launch_pq_rescore(qs, ws->s_pos.as<uint64_t>(), B, kp, ix->codes.hbm.as<unsigned char>(), ix->code_base.as<uint64_t>(),
                       ix->part_npad.as<uint32_t>(), ix->part_off.as<uint64_t>(), ix->nlist, ix->centroids.as<float>(),
                       ix->cb_tiled.as<float>(), ix->dim, ix->m, ix->dsub, ix->metric, ws->c_surv.as<uint32_t>(),
                       ws->s_exact.as<float>(), st);
@@ -1595,42 +1590,39 @@ static void filter_fixup(lgpu_index *ix, Workspace *ws, const IvfPlan &p, GroupA
     launch_select(sf, st);
 }
 
-// The scan of a row-major kind (sq, rq, ham) with `rows(a, X)` setting its rows to X.  An HBM index: one launch over
-// the whole tile queue of its own rows.  An index whose codes are in pinned host memory: a walk over the chunks of
-// code_cut through Workspace::stage.  Chunk c's probed partitions (part_cnt of the regroup, so the flagged queries'
-// probes in the maximum_nprobes pass) are copied into a staging buffer by launch_codes_copy_gated on the side stream
-// while chunk c - 1 is scanned; then the scan runs over chunk c's tiles alone (TileRange, its own claim counter), its
-// rows read from the buffer.  Nothing waits on the host but the deadline, checked between chunks.
+// The scan of a row-major kind (sq, rq, ham) with `rows(a, X)` setting its rows to X, over the walk of its codes.  An
+// HBM index: one launch over the whole tile queue of its own rows.  An index whose codes are in pinned host memory:
+// chunk c's probed partitions (part_cnt of the regroup, so the flagged queries' probes in the maximum_nprobes pass) are
+// copied into a staging buffer by launch_codes_copy_gated on the side stream while chunk c - 1 is scanned; then the
+// scan runs over chunk c's tiles alone (TileRange, its own claim counter in code_ctr, after the walk's byte count),
+// its rows read from the buffer.  Nothing waits on the host but the deadline, checked between chunks.
 template <class Args, class Rows, class Launch>
 static void scan_codes(lgpu_index *ix, Workspace *ws, const GroupArgs &ga, Args a, Rows &&rows, Launch &&launch,
                        const Deadline *deadline, cudaStream_t st)
 {
     a.total_tiles = ga.total_tiles; a.tile_counter = ga.tile_counter; a.tile_desc = ga.tile_desc;
     a.dist_out = ws->dist_out.as<float>();
-    if (!ix->codes_host.p) {
-        rows(a, ix->codes.p);
-        launch(a, 2 * ix->num_sms, st);
-        return;
-    }
     const std::vector<uint32_t> &cut = ix->code_cut;
-    const uint64_t nc = cut.size() - 1, rb = ix->code_row_bytes;
-    unsigned long long *moved = ws->code_ctr.as<unsigned long long>();      // [0]: bytes copied; then the counters
-    uint32_t *ctr = ws->code_ctr.as<uint32_t>() + 2;
-    for (auto &b : ws->stage.buf) b.ensure(ix->code_stage);
-    LGPU_CUDA(cudaMemsetAsync(ctr, 0, nc * 4, st));
-    ws->stage.open(ws, st, nc, deadline, nullptr, [&](uint64_t c, void *buf, cudaStream_t fs) {
-        launch_codes_copy_gated(static_cast<const uint8_t *>(ix->codes_host.dev), static_cast<uint8_t *>(buf), rb,
-                                ix->part_off.as<uint64_t>(), ga.part_cnt, cut[c], cut[c + 1],
-                                (ix->h_part_off[cut[c + 1]] - ix->h_part_off[cut[c]]) * rb, moved, ix->num_sms, fs);
-    });
-    for (uint64_t c = 0; c < nc; c++) {
-        rows(a, ws->stage.take(c));
-        a.range = {ga.tile_off + cut[c], ga.tile_off_b + cut[c], cut[c + 1] - cut[c], (uint32_t)ix->h_part_off[cut[c]]};
-        a.tile_counter = ctr + c;
-        launch(a, 2 * ix->num_sms, st);
-        ws->stage.release(c);
-    }
-    ws->stage.close();
+    const uint64_t rb = ix->code_row_bytes;
+    ix->codes.reserve_stage(ws, ix->code_stage);
+    if (ix->codes.on_host) LGPU_CUDA(cudaMemsetAsync(ws->code_ctr.as<uint32_t>() + 2, 0, (cut.size() - 1) * 4, st));
+    ix->codes.walk(
+        ws, st, ix->code_rows, [&](uint64_t r) { return r * rb; }, deadline,
+        [&](const RowChunk &ch) {
+            rows(a, ch.X);
+            if (!ch.resident) {
+                const uint64_t c = ch.s;
+                a.range = {ga.tile_off + cut[c], ga.tile_off_b + cut[c], cut[c + 1] - cut[c], (uint32_t)ch.r0};
+                a.tile_counter = ws->code_ctr.as<uint32_t>() + 2 + c;
+            }
+            launch(a, 2 * ix->num_sms, st);
+        },
+        [&](uint64_t c, void *buf, cudaStream_t fs) {
+            launch_codes_copy_gated(static_cast<const uint8_t *>(ix->codes.dev()), static_cast<uint8_t *>(buf), rb,
+                                    ix->part_off.as<uint64_t>(), ga.part_cnt, cut[c], cut[c + 1],
+                                    (ix->code_rows[c + 1] - ix->code_rows[c]) * rb,
+                                    ws->code_ctr.as<unsigned long long>(), ix->num_sms, fs);
+        });
 }
 
 // IvfScan::exact_pq / sq / rq / pq4 / ham: the exact scan of every regrouped tile, then the PQ top-kk
@@ -1642,7 +1634,7 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
         SqScanArgs qa{};
         qa.xx = ix->sq_xx.as<uint32_t>();
         qa.qcodes = ws->sq_q.as<uint8_t>(); qa.qq = ws->sq_qq.as<uint32_t>(); qa.dim_pad = ix->dim_pad;
-        scan_codes(ix, ws, ga, qa, [](SqScanArgs &a, void *X) { a.codes = static_cast<const uint8_t *>(X); },
+        scan_codes(ix, ws, ga, qa, [](SqScanArgs &a, const void *X) { a.codes = static_cast<const uint8_t *>(X); },
                    launch_sq_scan, deadline, st);
     } else if (p.scan == IvfScan::rq) {
         RqScanArgs ra{};
@@ -1650,7 +1642,7 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
         ra.popc = ix->rq_popc.as<uint32_t>();
         ra.planes = ws->rq_planes.as<uint32_t>(); ra.slots = ws->rq_slots.as<RqSlot>();
         ra.dim = ix->dim; ra.wpr = ix->rq_wpr; ra.cosine = ix->metric == LGPU_COSINE;
-        scan_codes(ix, ws, ga, ra, [](RqScanArgs &a, void *X) { a.codes = static_cast<const uint32_t *>(X); },
+        scan_codes(ix, ws, ga, ra, [](RqScanArgs &a, const void *X) { a.codes = static_cast<const uint32_t *>(X); },
                    launch_rq_scan, deadline, st);
     } else if (p.scan == IvfScan::pq4) {
         launch_pq4_scan(pq4_args(ix, ws, ga), 2 * ix->num_sms, st);
@@ -1658,7 +1650,7 @@ static void ivf_exact(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgp
         HamScanArgs ha{};
         ha.row_pop = ix->row_pop.as<uint32_t>(); ha.queries = q.h; ha.qpop = q.pop;
         ha.nbytes_pad = ix->nbytes_pad;
-        scan_codes(ix, ws, ga, ha, [](HamScanArgs &a, void *X) { a.rows = static_cast<const uint8_t *>(X); },
+        scan_codes(ix, ws, ga, ha, [](HamScanArgs &a, const void *X) { a.rows = static_cast<const uint8_t *>(X); },
                    launch_ivf_ham_scan, deadline, st);
     } else {
         launch_scan2(scan_args(ix, ws, q.f, ga), ix->dsub, ix->num_sms, st);
@@ -1680,7 +1672,7 @@ static void ivf_hnsw(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu
     ws->hn_ids.ensure(n * 8); ws->hn_dist.ensure(n * 4); ws->hn_pos.ensure(n * 8); ws->hn_ctr.ensure(16);
     LGPU_CUDA(cudaMemsetAsync(ws->hn_ctr.p, 0, 4, st));
     HnswArgs a{};
-    a.codes = ix->codes.as<uint8_t>(); a.qcodes = ws->sq_q.as<uint8_t>(); a.dim_pad = ix->dim_pad;
+    a.codes = ix->codes.hbm.as<uint8_t>(); a.qcodes = ws->sq_q.as<uint8_t>(); a.dim_pad = ix->dim_pad;
     a.probes = ws->probes.as<uint64_t>(); a.slots = p.slots; a.nprobes = p.nprobes; a.nlist = ix->nlist;
     a.part_off = ix->part_off.as<uint64_t>(); a.row_ids = ix->row_ids.as<uint64_t>();
     a.levels = ix->hn_levels.as<uint8_t>(); a.adj0 = ix->hn_adj0.as<uint32_t>();
@@ -1703,13 +1695,13 @@ static void ivf_hnsw(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const lgpu
 static void ivf_refine(lgpu_index *ix, Workspace *ws, const IvfPlan &p, const float *d_q, TopkOut out,
                        const uint32_t *only, cudaStream_t st)
 {
-    if (ix->vectors_host.p)
-        launch_refine_host(d_q, static_cast<const float *>(ix->vectors_host.dev), ix->vec_stride,
-                           ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric, ws->t_exact.as<float>(),
-                           ix->num_sms, st);
+    const float *X = static_cast<const float *>(ix->vectors.dev());
+    if (ix->vectors.on_host)
+        launch_refine_host(d_q, X, ix->vec_stride, ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric,
+                           ws->t_exact.as<float>(), ix->num_sms, st);
     else
-        launch_pair_distance(d_q, ix->vectors.as<float>(), ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric,
-                             ws->t_exact.as<float>(), st);
+        launch_pair_distance(d_q, X, ws->t_pos.as<uint64_t>(), p.B, p.kk, ix->dim, ix->metric, ws->t_exact.as<float>(),
+                             st);
     SelectArgs sr = select_cands(ws->t_exact.as<float>(), ws->t_ids.as<uint64_t>(), p.kk, p.B, p.k, out);
     sr.only = only;
     launch_select(with_scratch(ws, sr), st);
@@ -1781,7 +1773,7 @@ uint32_t ivf_sub_batch_size(lgpu_index *ix, uint32_t B, uint32_t nprobes, uint32
                    ivf_kind_query_bytes(ix, nprobes, np_eff, kk) + large_k_query_bytes(kk) +
                    (kk > SELECT_KMAX ? (size_t)kk * 28 : 0);
     // an index whose codes are in pinned host memory leases its two staging buffers from the same budget
-    const size_t budget = workspace_budget(), stage = ix->codes_host.p ? 2 * ix->code_stage : 0;
+    const size_t budget = workspace_budget(), stage = ix->codes.on_host ? 2 * ix->code_stage : 0;
     size_t bs = (budget > stage ? budget - stage : 0) / per_q;
     // tile descriptors address the distance segments with 32-bit float offsets
     bs = std::min<size_t>(bs, (size_t)0xffffffffull / std::max<size_t>(ix->pad_prefix[np_eff], 1));
@@ -1860,7 +1852,7 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const voi
         g_scanned_bytes = 0;
         g_streamed_bytes = 0;
     }
-    if (ix->codes_host.p) {        // the walk's byte count (code_ctr[0]) and one tile counter per chunk (scan_codes)
+    if (ix->codes.on_host) {       // the walk's byte count (code_ctr[0]) and one tile counter per chunk (scan_codes)
         ws->code_ctr.ensure(8 + ix->code_cut.size() * 4);
         LGPU_CUDA(cudaMemsetAsync(ws->code_ctr.p, 0, 8, st));
     }
@@ -1878,7 +1870,7 @@ void ivf_search_device(lgpu_index *ix, Workspace *ws, cudaStream_t st, const voi
                           ws->widen.as<uint32_t>());
         }
     }
-    if (prof && ix->codes_host.p) {   // every pass's copies, the maximum_nprobes widening's included
+    if (prof && ix->codes.on_host) {  // every pass's copies, the maximum_nprobes widening's included
         LGPU_CUDA(cudaMemcpyAsync(&g_streamed_bytes, ws->code_ctr.p, 8, cudaMemcpyDeviceToHost, st));
         LGPU_CUDA(cudaStreamSynchronize(st));
     }
@@ -2854,7 +2846,7 @@ static Route device_route(void *stream) { return {Route::DEVICE, 0, nullptr, 0, 
 template <class H> static bool graph_capturable(const H *h)
 {
     if constexpr (std::is_base_of_v<lgpu_rows, H>) return !h->rows.on_host;
-    else if constexpr (std::is_base_of_v<lgpu_index, H>) return !h->codes_host.p;
+    else if constexpr (std::is_base_of_v<lgpu_index, H>) return !h->codes.on_host;
     else return true;
 }
 
@@ -2932,14 +2924,22 @@ template <class H> static int rows_device_bytes(const H *hp, uint64_t *bytes)
         *bytes = h->rows.device_bytes() + h->row_ids.bytes + h->live.bits.bytes + own_device_bytes(h.h);
     });
 }
-template <class H> static int rows_host_bytes(const H *hp, uint64_t *bytes, int *placement)
+// lgpu_*_host_bytes, lgpu_*_code_bytes: of(h) gives a handle's row store (null: it keeps none, LGPU_VECTORS_NONE) and
+// the pinned bytes it holds beside it; the call reports the store's pinned bytes plus those, and where the store is
+template <class H, class Of> static int host_placement(const H *hp, uint64_t *bytes, int *placement, Of &&of)
 {
     return guarded([&] {
         LGPU_REQUIRE(bytes || placement, "null argument");
         HandleRef<H> h(const_cast<H *>(hp));
-        if (bytes) *bytes = h->rows.host_bytes() + own_host_bytes(h.h);
-        if (placement) *placement = h->rows.on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+        const auto [s, extra] = of(h.h);
+        if (bytes) *bytes = (s ? s->host_bytes() : 0) + extra;
+        if (placement) *placement = !s ? LGPU_VECTORS_NONE : s->on_host ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
     });
+}
+template <class H> static int rows_host_bytes(const H *hp, uint64_t *bytes, int *placement)
+{
+    return host_placement(hp, bytes, placement,
+                          [](const H *h) { return std::pair<const RowStore *, uint64_t>{&h->rows, own_host_bytes(h)}; });
 }
 
 // the partition layout every IVF index shares (lgpu_index_open, lgpu_ivf_sq_open): checked before any device work
@@ -3034,37 +3034,41 @@ static void open_ivf_common(lgpu_index *ix, const Desc *d, uint32_t rows_tile, c
 // IVF_SQ stored rows: dim zero-padded to the scan's K step
 static uint32_t sq_dim_pad(uint32_t dim) { return (uint32_t)round_up64(dim, SQ_K_CHUNK); }
 
-// codes [n][dim] (host) -> dst [n][dim_pad] (device, zero padding) and xx[r] = sum of row r's squared codes
-static void upload_sq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBuf &dst, DevBuf &xx)
+// codes [n][dim] (host) -> dst [n][dim_pad] (device, zero padding) and xx[r] = sum of row r's squared codes, on the
+// legacy stream
+static void fill_sq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, uint8_t *dst, uint32_t *xx)
 {
     const uint32_t dim_pad = sq_dim_pad(dim);
-    dst.ensure(std::max<size_t>((size_t)n * dim_pad, 16));
+    LGPU_CUDA(cudaMemsetAsync(dst, 0, n * dim_pad, nullptr));
+    LGPU_CUDA(cudaMemcpy2DAsync(dst, dim_pad, codes, dim, dim, n, cudaMemcpyHostToDevice, nullptr));
+    launch_sq_row_norms(dst, n, dim_pad, xx, nullptr);
+}
+static void upload_sq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBuf &dst, DevBuf &xx)
+{
+    dst.ensure(std::max<size_t>((size_t)n * sq_dim_pad(dim), 16));
     xx.ensure(std::max<size_t>((size_t)n * 4, 16));
-    cudaStream_t st = nullptr;
-    LGPU_CUDA(cudaMemsetAsync(dst.p, 0, dst.bytes, st));
-    if (n) {
-        LGPU_CUDA(cudaMemcpy2DAsync(dst.p, dim_pad, codes, dim, dim, n, cudaMemcpyHostToDevice, st));
-        launch_sq_row_norms(dst.as<uint8_t>(), n, dim_pad, xx.as<uint32_t>(), st);
-    }
-    LGPU_CUDA(cudaStreamSynchronize(st));
+    if (n) fill_sq_rows(codes, n, dim, dst.as<uint8_t>(), xx.as<uint32_t>());
+    LGPU_CUDA(cudaStreamSynchronize(nullptr));
 }
 
 // IVF_RQ stored rows: dim zero-padded to the scan's K step, in 32-bit words
 static uint32_t rq_wpr(uint32_t dim) { return (uint32_t)round_up64(dim, RQ_K_BITS) / 32; }
 
-// codes [n][ceil(dim / 8)] (host) -> dst [n][wpr] u32 (device, zero padding, bits past dim cleared) and popc[r]
-static void upload_rq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBuf &dst, DevBuf &popc)
+// codes [n][ceil(dim / 8)] (host) -> dst [n][wpr] u32 (device, zero padding, bits past dim cleared) and popc[r], on the
+// legacy stream
+static void fill_rq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, uint32_t *dst, uint32_t *popc)
 {
     const uint32_t wpr = rq_wpr(dim), nb = (dim + 7) / 8;
-    dst.ensure(std::max<size_t>((size_t)n * wpr * 4, 16));
+    LGPU_CUDA(cudaMemsetAsync(dst, 0, n * wpr * 4, nullptr));
+    LGPU_CUDA(cudaMemcpy2DAsync(dst, (size_t)wpr * 4, codes, nb, nb, n, cudaMemcpyHostToDevice, nullptr));
+    launch_rq_row_prep(dst, n, dim, wpr, popc, nullptr);
+}
+static void upload_rq_rows(const uint8_t *codes, uint64_t n, uint32_t dim, DevBuf &dst, DevBuf &popc)
+{
+    dst.ensure(std::max<size_t>((size_t)n * rq_wpr(dim) * 4, 16));
     popc.ensure(std::max<size_t>((size_t)n * 4, 16));
-    cudaStream_t st = nullptr;
-    LGPU_CUDA(cudaMemsetAsync(dst.p, 0, dst.bytes, st));
-    if (n) {
-        LGPU_CUDA(cudaMemcpy2DAsync(dst.p, (size_t)wpr * 4, codes, nb, nb, n, cudaMemcpyHostToDevice, st));
-        launch_rq_row_prep(dst.as<uint32_t>(), n, dim, wpr, popc.as<uint32_t>(), st);
-    }
-    LGPU_CUDA(cudaStreamSynchronize(st));
+    if (n) fill_rq_rows(codes, n, dim, dst.as<uint32_t>(), popc.as<uint32_t>());
+    LGPU_CUDA(cudaStreamSynchronize(nullptr));
 }
 
 // The padded PQ layouts: partition p's codes at code_base[p] = row_bytes x the 32-row padded heights of the partitions
@@ -3130,14 +3134,14 @@ static void open_pq8(const lgpu_index_desc *d, lgpu_index *&ix)
         LGPU_CUDA(cudaStreamSynchronize(st));
     }
     {   // codes -> skewed streams
-        ix->codes.ensure(std::max<uint64_t>(cb, 16));
-        LGPU_CUDA(cudaMemsetAsync(ix->codes.p, 0, ix->codes.bytes, st));
+        ix->codes.hbm.ensure(std::max<uint64_t>(cb, 16));
+        LGPU_CUDA(cudaMemsetAsync(ix->codes.hbm.p, 0, ix->codes.hbm.bytes, st));
         DevBuf tmp;
         if (d->nrows) {
             upload(tmp, d->codes, (size_t)d->nrows * d->m);
             launch_retile_codes(tmp.as<unsigned char>(), d->codes_layout, ix->part_off.as<uint64_t>(), nlist, d->nrows,
                                 d->m, ix->nch, ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(),
-                                ix->codes.as<unsigned char>(), st);
+                                ix->codes.hbm.as<unsigned char>(), st);
         }
         LGPU_CUDA(cudaStreamSynchronize(st));
     }
@@ -3161,7 +3165,7 @@ static void open_pq8(const lgpu_index_desc *d, lgpu_index *&ix)
     if (d->metric != LGPU_DOT) {   // per-row constants of the filter scan (tables.cu)
         ix->row_R.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));
         ix->rmax_bits.ensure(16);
-        launch_row_const(ix->codes.as<unsigned char>(), ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(),
+        launch_row_const(ix->codes.hbm.as<unsigned char>(), ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(),
                          ix->part_off.as<uint64_t>(), nlist, d->nrows, ix->centroids.as<float>(),
                          ix->cb_tiled.as<float>(), d->dim, d->m, ix->dsub, ix->row_R.as<float>(),
                          ix->rmax_bits.as<int>(), st);
@@ -3195,32 +3199,25 @@ static void open_pq4(const lgpu_index_desc *d, lgpu_index *&ix)
                 cbt[((size_t)i * dsub + t) * 16 + j] = d->codebook[((size_t)i * 16 + j) * dsub + t];
     upload(ix->pq4_cb, cbt.data(), cbt.size() * 4);
     upload_pq4_codes(d->codes, d->codes_layout, d->nrows, d->m, d->nlist, ix->part_off.as<uint64_t>(),
-                     ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(), total, ix->codes);
+                     ix->code_base.as<uint64_t>(), ix->part_npad.as<uint32_t>(), total, ix->codes.hbm);
 }
 
 // the HBM an index holds: every buffer its open allocated
 static uint64_t index_device_bytes(const lgpu_index *ix)
 {
-    uint64_t n = 0;
-    for (const DevBuf *b : {&ix->centroids, &ix->cb_tiled, &ix->codes, &ix->code_base, &ix->part_n, &ix->part_npad,
-                            &ix->part_off, &ix->row_ids, &ix->vectors, &ix->row_R, &ix->rmax_bits, &ix->cb_n2,
-                            &ix->cent_b, &ix->cent_n2, &ix->cent_sb, &ix->cent_sn2, &ix->sq_xx, &ix->rq_rot, &ix->rq_rc,
-                            &ix->rq_add, &ix->rq_scale, &ix->rq_popc, &ix->pq4_cb, &ix->cent_pop, &ix->row_pop,
-                            &ix->hn_levels, &ix->hn_adj0, &ix->hn_upper_index, &ix->hn_upper_adj, &ix->hn_entry,
-                            &ix->hn_top})
-        n += b->bytes;
-    return n;
+    return ix->codes.device_bytes() + ix->vectors.device_bytes() +
+           sum_bytes({&ix->centroids, &ix->cb_tiled, &ix->code_base, &ix->part_n, &ix->part_npad, &ix->part_off,
+                      &ix->row_ids, &ix->row_R, &ix->rmax_bits, &ix->cb_n2, &ix->cent_b, &ix->cent_n2, &ix->cent_sb,
+                      &ix->cent_sn2, &ix->sq_xx, &ix->rq_rot, &ix->rq_rc, &ix->rq_add, &ix->rq_scale, &ix->rq_popc,
+                      &ix->pq4_cb, &ix->cent_pop, &ix->row_pop, &ix->hn_levels, &ix->hn_adj0, &ix->hn_upper_index,
+                      &ix->hn_upper_adj, &ix->hn_entry, &ix->hn_top});
 }
 
 // lgpu_index_code_bytes, lgpu_ivf_binary_code_bytes: the pinned bytes of an index's codes and where they are
 template <class H> static int code_bytes(const H *hp, uint64_t *bytes, int *placement)
 {
-    return guarded([&] {
-        LGPU_REQUIRE(bytes || placement, "null argument");
-        HandleRef<H> ix(const_cast<H *>(hp));
-        if (bytes) *bytes = ix->codes_host.bytes;
-        if (placement) *placement = ix->codes_host.p ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
-    });
+    return host_placement(hp, bytes, placement,
+                          [](const H *ix) { return std::pair<const RowStore *, uint64_t>{&ix->codes, 0}; });
 }
 
 // Whether `bytes` of a handle's rows go to HBM at open: at most the cap the variable `cap_var` sets (read at every open;
@@ -3235,70 +3232,63 @@ static bool rows_fit_hbm(const char *cap_var, uint64_t bytes)
     return cap > 0 && bytes <= cap && (uint64_t)free_b >= bytes + workspace_budget();
 }
 
-// Where an IVF_SQ, IVF_RQ or binary IVF_FLAT index keeps its codes, nrows x row_bytes in the scan's layout.  HBM when
-// they fit with room to spare (rows_fit_hbm under LGPU_CODES_HBM_BYTES): `codes` is allocated exactly, so that device
-// bytes of the two placements differ by the code bytes, and `hbm()` fills it as the kind always has.  Otherwise pinned,
-// mapped host memory the index owns, in the same layout, built in chunks of rows staged through one HBM buffer (never a
-// device copy of the whole index): fill(dst, r0, n) lays rows r0 .. r0 + n out at dst -- the HBM chunk, copied back
-// afterwards (fill_on_device), or the pinned memory, uploaded into the chunk -- and prep(chunk, r0, n) runs the kind's
-// per-row kernel on it: the kernel the HBM placement runs, so the stored bytes and the per-row terms are the same.  The chunks
-// of consecutive partitions a search stages (code_cut, each at most code_stage bytes: FLAT_STAGE_BYTES, or an eighth of
-// the workspace budget when that is smaller, never less than the largest partition) are cut here; two staging buffers
-// of the largest partition must fit the budget, or the open fails with LGPU_OOM.  IVF_HNSW_SQ (its graph walk reads
-// rows at random) and the PQ kinds keep their codes in HBM: they never come here.
+// Where an IVF_SQ, IVF_RQ or binary IVF_FLAT index keeps its codes, nrows x row_bytes in the scan's layout: in HBM when
+// they fit with room to spare (rows_fit_hbm under LGPU_CODES_HBM_BYTES), allocated exactly, so that device bytes of the
+// two placements differ by the code bytes; otherwise in pinned, mapped host memory the index owns, in the same layout.
+// fill(dst, r0, n) lays rows r0 .. r0 + n out at device address dst and runs the kind's per-row kernel on them.  An HBM
+// store is one chunk of every row, laid out in place; a host store is built in chunks of CODE_PREP_BYTES in one HBM
+// buffer, each copied into the pinned rows (never a device copy of the whole index), so the stored bytes and the
+// per-row terms of the two placements are the same.  The chunks of consecutive partitions a search walks are cut here:
+// one for an HBM store; for a host store, each at most code_stage bytes (FLAT_STAGE_BYTES, or an eighth of the
+// workspace budget when that is smaller, never less than the largest partition), and two staging buffers of the
+// largest partition must fit the budget, or the open fails with LGPU_OOM.  IVF_HNSW_SQ (its graph walk reads rows at
+// random) and the PQ kinds keep their codes in HBM: they never come here.
 constexpr size_t CODE_PREP_BYTES = (size_t)64 << 20;
 
-template <class Hbm, class Fill, class Prep>
-static void place_codes(lgpu_index *ix, uint32_t row_bytes, bool fill_on_device, Hbm &&hbm, Fill &&fill, Prep &&prep)
+template <class Fill> static void place_codes(lgpu_index *ix, uint32_t row_bytes, Fill &&fill)
 {
     const uint64_t n = ix->nrows, bytes = n * row_bytes;
-    ix->code_row_bytes = row_bytes;
-    if (rows_fit_hbm("LGPU_CODES_HBM_BYTES", bytes)) {
-        ix->codes.ensure(std::max<size_t>(bytes, 16), true);
-        hbm();
-        return;
-    }
     const uint32_t nlist = ix->nlist;
-    ix->h_part_off.assign(nlist + 1, 0);
-    uint64_t largest = 0;
-    for (uint32_t p = 0; p < nlist; p++) {
-        ix->h_part_off[p + 1] = ix->h_part_off[p] + ix->h_part_n[p];
-        largest = std::max<uint64_t>(largest, (uint64_t)ix->h_part_n[p] * row_bytes);
-    }
-    const size_t budget = workspace_budget();
-    if (2 * largest > budget) {
-        set_error("the largest partition's codes (" + std::to_string(largest) + " bytes) do not fit twice in the " +
-                  "workspace budget (LGPU_WS_BYTES) that stages an index whose codes are in host memory");
-        throw Failure{LGPU_OOM};
-    }
-    ix->code_stage = std::max<size_t>(std::min(FLAT_STAGE_BYTES, budget / 8), std::max<size_t>(largest, 16));
+    const bool host = !rows_fit_hbm("LGPU_CODES_HBM_BYTES", bytes);
+    ix->code_row_bytes = row_bytes;
     ix->code_cut.assign(1, 0);
-    uint64_t in_chunk = 0;
-    for (uint32_t p = 0; p < nlist; p++) {
-        const uint64_t b = (uint64_t)ix->h_part_n[p] * row_bytes;
-        if (in_chunk && in_chunk + b > ix->code_stage) { ix->code_cut.push_back(p); in_chunk = 0; }
-        in_chunk += b;
+    ix->code_rows.assign(1, 0);
+    if (host) {
+        uint64_t largest = 0;
+        for (uint32_t p = 0; p < nlist; p++) largest = std::max<uint64_t>(largest, (uint64_t)ix->h_part_n[p] * row_bytes);
+        const size_t budget = workspace_budget();
+        if (2 * largest > budget) {
+            set_error("the largest partition's codes (" + std::to_string(largest) + " bytes) do not fit twice in the " +
+                      "workspace budget (LGPU_WS_BYTES) that stages an index whose codes are in host memory");
+            throw Failure{LGPU_OOM};
+        }
+        ix->code_stage = std::max<size_t>(std::min(FLAT_STAGE_BYTES, budget / 8), std::max<size_t>(largest, 16));
+        uint64_t in_chunk = 0, r = 0;
+        for (uint32_t p = 0; p < nlist; p++) {
+            const uint64_t b = (uint64_t)ix->h_part_n[p] * row_bytes;
+            if (in_chunk && in_chunk + b > ix->code_stage) {
+                ix->code_cut.push_back(p);
+                ix->code_rows.push_back(r);
+                in_chunk = 0;
+            }
+            in_chunk += b;
+            r += ix->h_part_n[p];
+        }
     }
     ix->code_cut.push_back(nlist);
-    ix->codes_host.alloc(bytes);
-    uint8_t *host = static_cast<uint8_t *>(ix->codes_host.p);
-    const uint64_t C = std::max<uint64_t>(1, CODE_PREP_BYTES / row_bytes);
+    ix->code_rows.push_back(n);
+    ix->codes.open(host, bytes);
+    const uint64_t C = host ? std::max<uint64_t>(1, CODE_PREP_BYTES / row_bytes) : n;
     DevBuf tmp;
-    tmp.ensure((size_t)std::min(n, C) * row_bytes + 16);
-    cudaStream_t st = nullptr;
+    if (host) tmp.ensure((size_t)std::min(n, C) * row_bytes + 16);
+    uint8_t *rows = reinterpret_cast<uint8_t *>(ix->codes.data());
     for (uint64_t r0 = 0; r0 < n; r0 += C) {
         const uint64_t c = std::min(C, n - r0);
-        uint8_t *chunk = tmp.as<uint8_t>();
-        if (fill_on_device) {
-            fill(chunk, r0, c);
-        } else {
-            fill(host + r0 * row_bytes, r0, c);
-            LGPU_CUDA(cudaMemcpyAsync(chunk, host + r0 * row_bytes, c * row_bytes, cudaMemcpyHostToDevice, st));
-        }
-        prep(chunk, r0, c);
-        if (fill_on_device)
-            LGPU_CUDA(cudaMemcpyAsync(host + r0 * row_bytes, chunk, c * row_bytes, cudaMemcpyDeviceToHost, st));
-        LGPU_CUDA(cudaStreamSynchronize(st));
+        uint8_t *dst = host ? tmp.as<uint8_t>() : rows;
+        fill(dst, r0, c);
+        if (host)
+            LGPU_CUDA(cudaMemcpyAsync(rows + r0 * row_bytes, dst, c * row_bytes, cudaMemcpyDeviceToHost, nullptr));
+        LGPU_CUDA(cudaStreamSynchronize(nullptr));
     }
 }
 
@@ -3312,24 +3302,17 @@ static void place_vectors(lgpu_index *ix, const float *vectors)
 {
     if (!vectors) return;
     ix->has_vectors = true;
-    const uint64_t n = ix->nrows, dim = ix->dim, bytes = n * dim * 4;
-    if (rows_fit_hbm("LGPU_VECTORS_HBM_BYTES", bytes)) {
-        ix->vectors.ensure(std::max<size_t>(bytes, 16), true);
-        if (bytes) LGPU_CUDA(cudaMemcpy(ix->vectors.p, vectors, bytes, cudaMemcpyHostToDevice));
-        return;
+    const uint64_t n = ix->nrows, dim = ix->dim;
+    const bool host = !rows_fit_hbm("LGPU_VECTORS_HBM_BYTES", n * dim * 4);
+    const uint64_t stride = host ? round_up64(dim, 4) : dim;
+    ix->vec_stride = (uint32_t)stride;
+    ix->vectors.open(host, n * stride * 4);
+    if (stride == dim) return ix->vectors.fill(0, vectors, n * dim * 4);
+    float *dst = reinterpret_cast<float *>(ix->vectors.data());
+    for (uint64_t r = 0; r < n; r++) {
+        memcpy(dst + r * stride, vectors + r * dim, dim * 4);
+        memset(dst + r * stride + dim, 0, (stride - dim) * 4);
     }
-    const uint32_t stride = (uint32_t)round_up64(dim, 4);
-    ix->vectors_host.alloc((size_t)n * stride * 4);
-    float *dst = static_cast<float *>(ix->vectors_host.p);
-    if (stride == dim) {
-        memcpy(dst, vectors, bytes);
-    } else {
-        for (uint64_t r = 0; r < n; r++) {
-            memcpy(dst + r * stride, vectors + r * dim, dim * 4);
-            memset(dst + r * stride + dim, 0, (stride - dim) * 4);
-        }
-    }
-    ix->vec_stride = stride;
 }
 
 // The sequence of every IVF open: `open(ix)` checks the desc, then creates the index (new_ivf) and fills it, and returns
@@ -3425,18 +3408,11 @@ int lgpu_ivf_sq_open(const lgpu_ivf_sq_desc *d, lgpu_index **out)
         ix->dim_pad = sq_dim_pad(d->dim);
         ix->sq_lo = d->lo; ix->sq_hi = d->hi;
         open_ivf_common(ix, d, SQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
-        const uint32_t dim = d->dim, dim_pad = ix->dim_pad;
+        const uint32_t dim = d->dim;
         ix->sq_xx.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));       // (as upload_sq_rows sizes it)
-        place_codes(
-            ix, dim_pad, true, [&] { upload_sq_rows(d->codes, d->nrows, dim, ix->codes, ix->sq_xx); },
-            [&](uint8_t *dst, uint64_t r0, uint64_t n) {
-                LGPU_CUDA(cudaMemsetAsync(dst, 0, n * dim_pad, nullptr));
-                LGPU_CUDA(cudaMemcpy2DAsync(dst, dim_pad, d->codes + r0 * dim, dim, dim, n, cudaMemcpyHostToDevice,
-                                            nullptr));
-            },
-            [&](uint8_t *rows, uint64_t r0, uint64_t n) {
-                launch_sq_row_norms(rows, n, dim_pad, ix->sq_xx.as<uint32_t>() + r0, nullptr);
-            });
+        place_codes(ix, ix->dim_pad, [&](uint8_t *dst, uint64_t r0, uint64_t n) {
+            fill_sq_rows(d->codes + r0 * dim, n, dim, dst, ix->sq_xx.as<uint32_t>() + r0);
+        });
         return d->vectors;
     });
 }
@@ -3496,7 +3472,7 @@ int lgpu_ivf_hnsw_sq_open(const lgpu_ivf_hnsw_sq_desc *d, lgpu_index **out)
         ix->sq_lo = s->lo; ix->sq_hi = s->hi;
         ix->hnsw_m = d->m;
         open_ivf_common(ix, s, SQ_ROWS_TILE, std::vector<uint64_t>(s->nlist));
-        upload_sq_rows(s->codes, s->nrows, s->dim, ix->codes, ix->sq_xx);
+        upload_sq_rows(s->codes, s->nrows, s->dim, ix->codes.hbm, ix->sq_xx);
         upload(ix->hn_levels, d->levels, (size_t)s->nrows);
         upload(ix->hn_adj0, d->adj0, (size_t)s->nrows * 2 * d->m * 4);
         upload(ix->hn_upper_index, d->upper_index, (size_t)s->nrows * 4);
@@ -3581,20 +3557,11 @@ int lgpu_ivf_rq_open(const lgpu_ivf_rq_desc *d, lgpu_index **out)
         ix = new_ivf(d->device, IvfKind::rq);
         ix->rq_wpr = rq_wpr(d->dim);
         open_ivf_common(ix, d, RQ_ROWS_TILE, std::vector<uint64_t>(d->nlist));
-        const uint32_t dim = d->dim, wpr = ix->rq_wpr, nb = (dim + 7) / 8;
+        const uint32_t dim = d->dim, nb = (dim + 7) / 8;
         ix->rq_popc.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));     // (as upload_rq_rows sizes it)
-        place_codes(
-            ix, wpr * 4, true, [&] { upload_rq_rows(d->codes, d->nrows, dim, ix->codes, ix->rq_popc); },
-            [&](uint8_t *dst, uint64_t r0, uint64_t n) {
-                LGPU_CUDA(cudaMemsetAsync(dst, 0, n * wpr * 4, nullptr));
-                LGPU_CUDA(cudaMemcpy2DAsync(dst, (size_t)wpr * 4, d->codes + r0 * nb, nb, nb, n, cudaMemcpyHostToDevice,
-                                            nullptr));
-            },
-            [&](uint8_t *rows, uint64_t r0, uint64_t n) {
-                launch_rq_row_prep(reinterpret_cast<uint32_t *>(rows), n, dim, wpr, ix->rq_popc.as<uint32_t>() + r0,
-                                   nullptr);
-            });
-
+        place_codes(ix, ix->rq_wpr * 4, [&](uint8_t *dst, uint64_t r0, uint64_t n) {
+            fill_rq_rows(d->codes + r0 * nb, n, dim, reinterpret_cast<uint32_t *>(dst), ix->rq_popc.as<uint32_t>() + r0);
+        });
         upload(ix->rq_add, d->add_factors, (size_t)d->nrows * 4);
         upload(ix->rq_scale, d->scale_factors, (size_t)d->nrows * 4);
         upload(ix->rq_rot, d->rotation, (size_t)d->dim * d->dim * 4);
@@ -3664,12 +3631,8 @@ int lgpu_index_device_bytes(const lgpu_index *ixh, uint64_t *bytes)
 
 int lgpu_index_host_bytes(const lgpu_index *ixh, uint64_t *bytes, int *placement)
 {
-    return guarded([&] {
-        LGPU_REQUIRE(bytes || placement, "null argument");
-        HandleRef<lgpu_index> ix(const_cast<lgpu_index *>(ixh));
-        if (bytes) *bytes = ix->vectors_host.bytes;
-        if (placement)
-            *placement = !ix->has_vectors ? LGPU_VECTORS_NONE : ix->vectors_host.p ? LGPU_VECTORS_HOST : LGPU_VECTORS_HBM;
+    return host_placement(ixh, bytes, placement, [](const lgpu_index *ix) {
+        return std::pair<const RowStore *, uint64_t>{ix->has_vectors ? &ix->vectors : nullptr, 0};
     });
 }
 
@@ -3692,15 +3655,16 @@ int lgpu_debug_refine_host(const float *queries, uint32_t B, const float *rows, 
         int sms = 0;
         LGPU_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
         const uint32_t stride = (uint32_t)round_up64(dim, 4);
-        PinnedBuf h;
-        h.alloc((size_t)N * stride * 4);
-        memset(h.p, 0, h.bytes);
-        for (uint64_t r = 0; r < N; r++) memcpy(static_cast<float *>(h.p) + r * stride, rows + r * dim, (size_t)dim * 4);
+        RowStore h;
+        h.open(true, (size_t)N * stride * 4);
+        float *X = reinterpret_cast<float *>(h.data());
+        memset(X, 0, h.host_bytes());
+        for (uint64_t r = 0; r < N; r++) memcpy(X + r * stride, rows + r * dim, (size_t)dim * 4);
         DevBuf q, p, o;
         upload(q, queries, (size_t)B * dim * 4);
         upload(p, pos, (size_t)B * nc * 8);
         o.ensure((size_t)B * nc * 4);
-        launch_refine_host(q.as<float>(), static_cast<const float *>(h.dev), stride, p.as<uint64_t>(), B, nc, dim, metric,
+        launch_refine_host(q.as<float>(), static_cast<const float *>(h.dev()), stride, p.as<uint64_t>(), B, nc, dim, metric,
                            o.as<float>(), sms, nullptr);
         LGPU_CUDA(cudaMemcpy(out, o.p, (size_t)B * nc * 4, cudaMemcpyDeviceToHost));
     });
@@ -4248,30 +4212,21 @@ int lgpu_ivf_binary_open(const lgpu_ivf_binary_desc *d, lgpu_ivf_binary **out)
         ix->nbytes = d->nbytes; ix->nbytes_pad = (d->nbytes + 31) & ~31u;
         ix->dim = d->nbytes;
         open_ivf_partitions(ix, d, HAM_ROWS_TILE, std::vector<uint64_t>(d->nlist));
-        // centroids and rows zero-padded to nbytes_pad, with their popcounts (ham_pack)
+        // centroids and rows zero-padded to nbytes_pad at dst, with their popcounts (ham_pack), from an upload
         const uint32_t nb = d->nbytes, nbp = ix->nbytes_pad;
-        auto pack = [&](const uint8_t *src, uint64_t n, DevBuf &dst, DevBuf &pop) {
-            dst.ensure(std::max<size_t>((size_t)n * nbp, 16));
-            pop.ensure(std::max<size_t>((size_t)n * 4, 16));
-            if (n) {
-                DevBuf raw;
-                upload(raw, src, (size_t)n * nb);
-                launch_ham_pack(raw.as<uint8_t>(), nb, nb, n, dst.as<uint8_t>(), nbp, pop.as<uint32_t>(), nullptr);
-                LGPU_CUDA(cudaStreamSynchronize(nullptr));
-            }
+        auto pack = [&](const uint8_t *src, uint64_t n, uint8_t *dst, uint32_t *pop) {
+            DevBuf raw;
+            upload(raw, src, (size_t)n * nb);
+            launch_ham_pack(raw.as<uint8_t>(), nb, nb, n, dst, nbp, pop, nullptr);
+            LGPU_CUDA(cudaStreamSynchronize(nullptr));
         };
-        pack(d->centroids, d->nlist, ix->centroids, ix->cent_pop);
-        // the rows: in HBM as above, or packed on the host as a host binary handle packs them (ham_pack_host), their
-        // popcounts taken from chunks staged through HBM
-        ix->row_pop.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));     // (as `pack` sizes it)
-        place_codes(
-            ix, nbp, false, [&] { pack(d->vectors, d->nrows, ix->codes, ix->row_pop); },
-            [&](uint8_t *dst, uint64_t r0, uint64_t n) {
-                ham_pack_host(d->vectors + r0 * nb, n, nb, nbp, dst);
-            },
-            [&](uint8_t *rows, uint64_t r0, uint64_t n) {
-                launch_ham_pack(rows, nbp, nbp, n, nullptr, nbp, ix->row_pop.as<uint32_t>() + r0, nullptr);
-            });
+        ix->centroids.ensure(std::max<size_t>((size_t)d->nlist * nbp, 16));
+        ix->cent_pop.ensure(std::max<size_t>((size_t)d->nlist * 4, 16));
+        pack(d->centroids, d->nlist, ix->centroids.as<uint8_t>(), ix->cent_pop.as<uint32_t>());
+        ix->row_pop.ensure(std::max<size_t>((size_t)d->nrows * 4, 16));
+        place_codes(ix, nbp, [&](uint8_t *dst, uint64_t r0, uint64_t n) {
+            pack(d->vectors + r0 * nb, n, dst, ix->row_pop.as<uint32_t>() + r0);
+        });
         return nullptr;             // the packed rows are the index: no separate raw vectors
     });
 }
