@@ -330,8 +330,12 @@ static void grow_keep(DevBuf &b, size_t used, size_t need)
     std::swap(b.bytes, nb.bytes);
 }
 
-// One chunk of a RowStore walk: step s, rows [r0, r1), X the rows as a kernel reads them.  resident: X is the store's
-// own HBM (the handle's per-row terms apply as they are); else a staging buffer (the chunk's terms are built for it).
+// the most rows of a host handle one staging buffer holds, in bytes: large enough that the copy engine runs at the
+// PCIe rate and a chunk's fixed scoring cost is small, small enough that the unoverlapped first copy is short
+constexpr size_t FLAT_STAGE_BYTES = (size_t)128 << 20;
+
+// One chunk of a RowStore walk or visit: step s, rows [r0, r1), X the rows as a kernel reads them.  resident: X is the
+// store's own HBM (the handle's per-row terms apply as they are); else an HBM copy (the chunk's terms are built for it).
 struct RowChunk {
     uint64_t s, r0, r1;
     const void *X;
@@ -421,6 +425,22 @@ struct RowStore {
               Use &&use, Staging::Copier copier = nullptr) const
     {
         walk(ws, st, cut, 1, at, deadline, use, [](uint64_t) {}, std::move(copier));
+    }
+    // f(RowChunk) over rows [r0, r1) of `row_bytes` each, at open or append, synchronously on the legacy stream: an HBM
+    // store once, X its resident row r0; a host store in chunks of at most FLAT_STAGE_BYTES, each copied into one
+    // temporary HBM buffer.  Nothing runs for no rows.
+    template <class F> void visit(uint64_t r0, uint64_t r1, size_t row_bytes, F &&f) const
+    {
+        if (r1 <= r0) return;
+        if (!on_host) return f(RowChunk{0, r0, r1, static_cast<const char *>(hbm.p) + r0 * row_bytes, true});
+        const uint64_t C = std::max<uint64_t>(1, std::min<uint64_t>(r1 - r0, FLAT_STAGE_BYTES / row_bytes));
+        DevBuf x;
+        x.ensure(C * row_bytes);
+        for (uint64_t r = r0, s = 0; r < r1; r += C, s++) {
+            const uint64_t m = std::min(C, r1 - r);
+            LGPU_CUDA(cudaMemcpy(x.p, data() + r * row_bytes, m * row_bytes, cudaMemcpyHostToDevice));
+            f(RowChunk{s, r, r + m, x.p, false});
+        }
     }
 };
 
@@ -700,6 +720,10 @@ struct lgpu_multivec : lgpu_rows {
     std::vector<uint64_t> h_offsets;       // host copy: the row chunks of a search are cut on the host
 };
 
+// the bytes of one stored row
+static size_t stored_row_bytes(const lgpu_flat *fl) { return (size_t)fl->dim * (fl->f16 ? 2 : 4); }
+static size_t stored_row_bytes(const lgpu_binary *bx) { return bx->nbytes_pad; }
+
 
 // ---- NCCL, bound at run time (dlopen): single-GPU hosts need no libnccl, and inside a process that already
 // loaded one (torch) the same library instance is used ----
@@ -860,17 +884,12 @@ static bool tc_operand_rows(const void *X, bool f16, uint64_t n, uint32_t d, voi
     xerr = me;
     return finite && std::isfinite(xmax);
 }
-static bool prepare_tc_operand(const void *X, bool f16, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax,
-                               float &xerr, cudaStream_t st)
-{
-    if (!f16) Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
-    n2.ensure(std::max<size_t>((size_t)n * 4, 16), f16);
-    return tc_operand_rows(X, f16, n, d, Xb.p, n2.as<float>(), xmax, xerr, st);
-}
 static bool prepare_tc_operand(const float *X, uint64_t n, uint32_t d, DevBuf &Xb, DevBuf &n2, float &xmax, float &xerr,
                                cudaStream_t st)
 {
-    return prepare_tc_operand(X, false, n, d, Xb, n2, xmax, xerr, st);
+    Xb.ensure(std::max<size_t>((size_t)n * d * 2, 16));
+    n2.ensure(std::max<size_t>((size_t)n * 4, 16));
+    return tc_operand_rows(X, false, n, d, Xb.p, n2.as<float>(), xmax, xerr, st);
 }
 
 // where a top-k goes: [B][k] ids and distances, [B] counts and, optionally, [B][k] storage positions
@@ -1926,10 +1945,6 @@ static void flat_score(lgpu_flat *fl, Workspace *ws, cudaStream_t st, int metric
     select_dense(ws, ws->D.as<float>(), N, ld, r.cols, b, sp, rf, out, st);
 }
 
-// the most rows of a host handle one staging buffer holds, in bytes: large enough that the copy engine runs at the
-// PCIe rate and a chunk's fixed scoring cost is small, small enough that the unoverlapped first copy is short
-constexpr size_t FLAT_STAGE_BYTES = (size_t)128 << 20;
-
 // The dense search of a flat or binary handle (stream_topk) reads its rows in chunks of C rows.  An HBM store is one
 // resident chunk of all N rows, the queries in passes of P = bs that the budget holds the scores of.  A host store's
 // chunks cross PCIe, copied into the workspace's two staging buffers on its side stream (RowStore::walk), chunk i + 1
@@ -2118,12 +2133,14 @@ static uint32_t ham_list_cap(uint32_t k, uint64_t N, uint64_t ns)
     return cap;
 }
 
-// The threshold sample of the list path, taken from the handle's rows at open and after every append (which hold the
-// handle alone): every (nrows / HAM_SAMPLE)-th row, packed, with its popcount and its id.  A host handle's sample rows
-// are gathered on the host and uploaded, so the sample is in HBM for both placements.  Enqueued on the legacy stream;
-// the caller synchronises.
-static void ham_sample(lgpu_binary *bx, uint64_t nrows)
+// The per-row terms of a binary handle once rows [n0, n0 + n) are stored, at open (n0 = 0) or append (which hold the
+// handle alone): the threshold sample of the list path, taken again from all nrows = n0 + n rows, every
+// (nrows / HAM_SAMPLE)-th row, packed, with its popcount and its id.  A host handle's sample rows are gathered on the
+// host and uploaded, so the sample is in HBM for both placements.  Enqueued on the legacy stream; the caller
+// synchronises.
+static void ham_sample(lgpu_binary *bx, uint64_t n0, uint64_t n)
 {
+    const uint64_t nrows = n0 + n;
     if (nrows <= HAM_SAMPLE) return;
     const uint64_t stride = nrows / HAM_SAMPLE;
     const uint32_t nbp = bx->nbytes_pad;
@@ -2198,9 +2215,9 @@ static void ham_list_select(Workspace *ws, cudaStream_t st, uint32_t B, uint32_t
 // the lists need no merge.  The dense fix-up of the overflowed queries differs by placement.  An HBM store: chunks of
 // `bf` queries over a [bf][N] matrix; one launch lists each chunk's flagged queries, and each chunk's two launches
 // return at once when its list is empty.  A host store: one list of all B flagged queries (its count gates every
-// launch below), then per chunk a gated copy of its rows out of the mapped pinned memory into staging buffer 0, the
-// dense Hamming scores of the flagged queries ([B][C] matrix) and their top-k, merged into a running top-k of the
-// flagged queries; with nothing flagged each launch returns at once, and nothing waits on the host.
+// launch below), then a second walk of the chunks, each copied out of the mapped pinned memory by a gated copier,
+// scored densely for the flagged queries ([B][C] matrix), and its top-k merged into a running top-k of the flagged
+// queries; with nothing flagged each launch returns at once, and nothing waits on the host.
 static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const uint8_t *Q, const uint32_t *qpop,
                           uint32_t B, uint32_t k, uint32_t cap, uint64_t C, uint32_t bf, TopkOut out, RowFilter rf,
                           const Deadline *deadline)
@@ -2246,18 +2263,22 @@ static void ham_topk_list(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
     RunningTopk run{ws, cut.size() - 1, B, k, out};
     run.only = ws->flags.as<uint32_t>(); run.gate = gate;
     const uint8_t *mapped = static_cast<const uint8_t *>(bx->rows.dev());
-    for (uint64_t c = 0; c + 1 < cut.size(); c++) {
-        const uint64_t n = cut[c + 1] - cut[c];
-        launch_mv_copy_gated(mapped + cut[c] * nbp, ws->stage.buf[0].as<uint8_t>(), n * nbp, gate, bx->num_sms, st);
-        launch_ham_dense(Q, ws->stage.buf[0].as<uint8_t>(), B, n, nbp, ws->D.as<float>(), ldc, bx->num_sms, st,
-                         ws->h_list.as<uint32_t>(), gate);
-        SelectArgs sc = select_rows(ws->D.as<float>(), n, ldc, B, k, run.dst(c));
-        with_cols(sc, row_cols(bx, cut[c]));
-        sc.only = run.only; sc.gate = gate;
-        sc.allow = rf.bits; sc.allow_bits = rf.nbits;
-        launch_select(sc, st);
-        run.merge(c, st);
-    }
+    bx->rows.walk(ws, st, cut, 1, [&](uint64_t r) { return r * nbp; }, nullptr,
+        [&](const RowChunk &ch) {
+            const uint64_t n = ch.r1 - ch.r0;
+            launch_ham_dense(Q, static_cast<const uint8_t *>(ch.X), B, n, nbp, ws->D.as<float>(), ldc, bx->num_sms, st,
+                             ws->h_list.as<uint32_t>(), gate);
+            SelectArgs sc = select_rows(ws->D.as<float>(), n, ldc, B, k, run.dst(ch.s));
+            with_cols(sc, row_cols(bx, ch.r0));
+            sc.only = run.only; sc.gate = gate;
+            sc.allow = rf.bits; sc.allow_bits = rf.nbits;
+            launch_select(sc, st);
+        },
+        [&](uint64_t s) { run.merge(s, st); },
+        [&](uint64_t s, void *buf, cudaStream_t fs) {
+            launch_mv_copy_gated(mapped + cut[s] * nbp, static_cast<uint8_t *>(buf), (cut[s + 1] - cut[s]) * nbp, gate,
+                                 bx->num_sms, fs);
+        });
 }
 
 // b queries (Q, qpop) against N rows X of a binary handle (ids from cols) by the dense route of an HBM handle of those
@@ -2315,7 +2336,7 @@ void binary_search_device(lgpu_binary *bx, Workspace *ws, cudaStream_t st, const
             const size_t per_q = per_q0 + (size_t)k * 48 + 16 + ldc * 4;
             const size_t left = budget > C * row_b ? budget - C * row_b : 0;
             bs = bf = (uint32_t)std::max<size_t>(1, std::min<size_t>(left / per_q, B));
-            for (auto &b : ws->stage.buf) b.ensure(C * nbp);
+            bx->rows.reserve_stage(ws, C * nbp);
             ws->chunk_pop.ensure(C * 4);
             RunningTopk::reserve(ws, (N + C - 1) / C, bs, k);
             ws->D.ensure((size_t)bs * ldc * 4);
@@ -2493,8 +2514,8 @@ static std::vector<uint64_t> mv_chunks(const lgpu_multivec *mv, uint64_t cap_vec
 // resident chunk [0, N); a host handle's mv_chunks of one staging buffer each, streamed through Workspace::stage in
 // every sub-batch, so each vector crosses PCIe once per sub-batch.  The tensor-core GEMM keeps chunk-local keys
 // (row_base = the chunk's first row) and fills the chunk's columns of A.  A host handle re-scores the shortlist from the
-// pinned vectors, and its fix-up copies each chunk of them into staging buffer 0 by a kernel that returns at once when
-// the gate is 0: no host synchronisation decides anything.  The vectors are in the row type (es bytes per element); an
+// pinned vectors, and its fix-up walks the chunks again with a copier kernel that returns at once when the gate is 0:
+// no host synchronisation decides anything.  The vectors are in the row type (es bytes per element); an
 // fp16 handle's vectors are also its tensor-core operand, so both routes stream the same 2-byte rows.  Half the budget
 // goes to the distance blocks of mv_exact_dense; the other half, less a host handle's two staging buffers, is `left`.
 void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, const float *d_q, const uint32_t *h_qoff,
@@ -2608,25 +2629,22 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             else rescore(static_cast<const float *>(V));
             launch_select(select_cands(ws->mv_ex.as<float>(), ws->mv_exid.as<uint64_t>(), cap, b, k, out.at(qa, k)), st);
             // exact fix-up of the flagged queries into A (free again: it holds their exact distances).  A host handle's
-            // rows go through staging buffer 0 on the call's stream; with no query flagged, every launch returns at
-            // once
+            // chunks are copied by a gated copier; with no query flagged, every launch returns at once
             const uint32_t *gate = ws->mv_gate.as<uint32_t>();
-            for (size_t c = 0; c + 1 < cutv.size(); c++) {
-                const uint64_t ra = cutv[c], rb = cutv[c + 1];
-                const void *X = static_cast<const char *>(V) + off[ra] * dim * es;
-                if (mv->rows.on_host) {
-                    const uint64_t n = (off[rb] - off[ra]) * dim;
+            mv->rows.walk(ws, st, cutv, at((size_t)dim * es), nullptr,
+                [&](const RowChunk &ch) {
+                    mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, A, ld, ch.X, ch.r0, ch.r1,
+                                   ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), gate);
+                },
+                [&](uint64_t s, void *buf, cudaStream_t fs) {
+                    const uint64_t j0 = off[cutv[s]], n = (off[cutv[s + 1]] - j0) * dim;
                     if (mv->f16)
-                        launch_mv_copy_gated(static_cast<const __half *>(X), ws->stage.buf[0].as<__half>(), n, gate,
-                                             mv->num_sms, st);
+                        launch_mv_copy_gated(static_cast<const __half *>(V) + j0 * dim, static_cast<__half *>(buf), n,
+                                             gate, mv->num_sms, fs);
                     else
-                        launch_mv_copy_gated(static_cast<const float *>(X), ws->stage.buf[0].as<float>(), n, gate,
-                                             mv->num_sms, st);
-                    X = ws->stage.buf[0].p;
-                }
-                mv_exact_dense(mv, ws, st, d_q, h_qoff, qa, qb, A, ld, X, ra, rb, ws->mv_flags.as<uint32_t>(),
-                               ws->mv_vflags.as<uint32_t>(), gate);
-            }
+                        launch_mv_copy_gated(static_cast<const float *>(V) + j0 * dim, static_cast<float *>(buf), n,
+                                             gate, mv->num_sms, fs);
+                });
             SelectArgs sc = select_rows(A, N, ld, b, k, out.at(qa, k));
             sc.col_ids = ids;
             sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = gate;
@@ -3992,33 +4010,67 @@ static uint64_t flat_row_data_bytes(uint64_t n, uint32_t d, bool f16)
     return rows + (f16 ? 0 : n * d * 2) + n * 4;
 }
 
-// The tensor-core band of n rows in host memory (a host handle's rows at open or append): tc_operand_rows over chunks
-// staged through HBM, the maxima of their constants, so xmax and xerr are those of the whole rows.  False when a row
-// has no finite band.
-static bool host_rows_band(const void *rows, bool f16, uint64_t n, uint32_t d, float &xmax, float &xerr)
+// n of the caller's rows into rows n0.. of a flat handle's store
+static void flat_store_rows(lgpu_flat *fl, const void *src, uint64_t n0, uint64_t n)
 {
-    const size_t es = f16 ? 2 : 4;
-    const uint64_t C = std::max<uint64_t>(1, std::min<uint64_t>(n, FLAT_STAGE_BYTES / ((size_t)d * es)));
-    DevBuf x, xb, n2;
-    x.ensure(C * d * es);
-    if (!f16) xb.ensure(C * d * 2);
-    n2.ensure(C * 4);
-    bool finite = true;
-    xmax = xerr = 0.f;
-    for (uint64_t r = 0; r < n; r += C) {
-        const uint64_t m = std::min(C, n - r);
-        LGPU_CUDA(cudaMemcpy(x.p, static_cast<const char *>(rows) + r * d * es, m * d * es, cudaMemcpyHostToDevice));
-        float a = 0.f, e = 0.f;
-        finite &= tc_operand_rows(x.p, f16, m, d, xb.p, n2.as<float>(), a, e, nullptr);
-        xmax = std::max(xmax, a);
-        xerr = std::max(xerr, e);
+    const size_t row = stored_row_bytes(fl);
+    fl->rows.fill(n0 * row, src, n * row);
+}
+
+// The per-row terms of a flat handle once rows [n0, n0 + n) are stored, at open (n0 = 0) or append.  In HBM, |x| once
+// a cosine search built it.  Once a column of a GEMM shape holds 4096 rows, the tensor-core band (vec_max and vec_err,
+// the maxima over every row) and, in HBM, the operand (vec_b, vec_n2): of every row when the column first gets there,
+// else of the new rows while the band is finite.  Each chunk of the row store's visit gets tc_operand_rows, into the
+// operand at its rows when the chunk is resident, else into scratch that only the band outlives.  A non-finite or
+// overflowing row leaves the column to the exact kernels.
+static void flat_row_terms(lgpu_flat *fl, uint64_t n0, uint64_t n)
+{
+    const uint64_t n1 = n0 + n;
+    const uint32_t d = fl->dim;
+    const bool f16 = fl->f16;
+    const bool hbm = !fl->rows.on_host;
+    if (hbm && fl->has_norms) {
+        grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
+        const char *x = fl->rows.data() + n0 * stored_row_bytes(fl);
+        if (f16) launch_row_norms(reinterpret_cast<const __half *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
+        else launch_row_norms(reinterpret_cast<const float *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
     }
-    return finite;
+    if (!gemm_shape_supported(d) || n1 < 4096) return;
+    const uint64_t a = n0 < 4096 ? 0 : n0;          // the first row whose terms are taken
+    if (a > 0 && !fl->has_tc) return;
+    if (hbm) {
+        // room for the operand of rows [a, n1): an open has sized it exactly; an append that first reaches 4096 rows
+        // gives the bf16 copy headroom (fp16 |x|^2 none), and later appends grow it as the rows grow
+        if (!f16) grow_keep(fl->vec_b, (size_t)a * d * 2, (size_t)n1 * d * 2);
+        if (a == 0) fl->vec_n2.ensure((size_t)n1 * 4, f16);
+        else grow_keep(fl->vec_n2, (size_t)a * 4, (size_t)n1 * 4);
+    }
+    DevBuf xb, n2;
+    bool finite = true;
+    float xmax = 0.f, xerr = 0.f;
+    fl->rows.visit(a, n1, stored_row_bytes(fl), [&](const RowChunk &ch) {
+        const uint64_t m = ch.r1 - ch.r0;
+        if (!ch.resident) {
+            if (!f16) xb.ensure(m * d * 2);
+            n2.ensure(m * 4);
+        }
+        void *b = f16 ? nullptr : ch.resident ? fl->vec_b.as<char>() + ch.r0 * d * 2 : xb.p;
+        float *q = ch.resident ? fl->vec_n2.as<float>() + ch.r0 : n2.as<float>();
+        float cm = 0.f, ce = 0.f;
+        finite &= tc_operand_rows(ch.X, f16, m, d, b, q, cm, ce, nullptr);
+        xmax = std::max(xmax, cm);
+        xerr = std::max(xerr, ce);
+    });
+    fl->has_tc = finite;
+    fl->vec_max = std::max(fl->vec_max, xmax);      // (both 0 before the column first reaches 4096 rows)
+    fl->vec_err = std::max(fl->vec_err, xerr);
+    if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
 }
 
 // lgpu_flat_open and lgpu_flat_open_f16: rows f32 or fp16 (f16), kept as given in HBM when their row data fits there
-// (LGPU_FLAT_HBM_BYTES, rows_fit_hbm), else in pinned host memory the handle owns.  HBM rows and their operand are
-// allocated exactly, so that device bytes of the two placements differ by the row data.
+// (LGPU_FLAT_HBM_BYTES, rows_fit_hbm), else in pinned host memory the handle owns: an append of nrows rows to an empty
+// store.  HBM rows and their operand are allocated exactly, so that device bytes of the two placements differ by the
+// row data.
 static int flat_open(const void *vectors, bool f16, uint64_t nrows, uint32_t dim, const uint64_t *row_ids, int device,
                      lgpu_flat **out)
 {
@@ -4029,21 +4081,15 @@ static int flat_open(const void *vectors, bool f16, uint64_t nrows, uint32_t dim
         require_device(device);
         fl = new lgpu_flat();
         fl->device = device; fl->nrows = nrows; fl->dim = dim; fl->f16 = f16;
-        const size_t es = f16 ? 2 : 4, bytes = (size_t)nrows * dim * es;
-        const bool tc_shape = gemm_shape_supported(dim) && nrows >= 4096;
-        fl->rows.open(!rows_fit_hbm("LGPU_FLAT_HBM_BYTES", flat_row_data_bytes(nrows, dim, f16)), bytes);
-        fl->rows.fill(0, vectors, bytes);
-        // the band (a non-finite or overflowing row: the exact kernels serve the column), and in HBM the operand
-        if (tc_shape && fl->rows.on_host) {
-            fl->has_tc = host_rows_band(fl->rows.data(), f16, nrows, dim, fl->vec_max, fl->vec_err);
-        } else if (tc_shape) {
+        fl->rows.open(!rows_fit_hbm("LGPU_FLAT_HBM_BYTES", flat_row_data_bytes(nrows, dim, f16)),
+                      nrows * stored_row_bytes(fl));
+        if (!fl->rows.on_host && gemm_shape_supported(dim) && nrows >= 4096) {
             if (!f16) fl->vec_b.ensure((size_t)nrows * dim * 2, true);
             fl->vec_n2.ensure((size_t)nrows * 4, true);
-            fl->has_tc = prepare_tc_operand(fl->rows.data(), f16, nrows, dim, fl->vec_b, fl->vec_n2, fl->vec_max,
-                                            fl->vec_err, nullptr);
-            if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
         }
+        flat_store_rows(fl, vectors, 0, nrows);
         open_rows(fl, row_ids, nrows);
+        flat_row_terms(fl, 0, nrows);
         register_handle(fl);
         *out = fl;
     });
@@ -4120,20 +4166,22 @@ static void ham_pack_host(const uint8_t *src, uint64_t n, uint32_t nbytes, uint3
 }
 
 // n of the caller's rows [n][nbytes] into rows n0.. of a binary handle's store, packed: on the host into pinned memory,
-// or in HBM from an upload, with their popcounts into `pop`
-static void ham_store_rows(lgpu_binary *bx, const uint8_t *src, uint64_t n0, uint64_t n)
+// or in HBM from an upload, with their popcounts into `pop` (grown to hold them)
+static void ham_store_rows(lgpu_binary *bx, const void *src, uint64_t n0, uint64_t n)
 {
     const uint32_t nbytes = bx->nbytes, nbp = bx->nbytes_pad;
     uint8_t *dst = reinterpret_cast<uint8_t *>(bx->rows.data()) + (size_t)n0 * nbp;
-    if (bx->rows.on_host) return ham_pack_host(src, n, nbytes, nbp, dst);
+    if (bx->rows.on_host) return ham_pack_host(static_cast<const uint8_t *>(src), n, nbytes, nbp, dst);
+    grow_keep(bx->pop, (size_t)n0 * 4, (size_t)(n0 + n) * 4);
     DevBuf raw;
     upload(raw, src, (size_t)n * nbytes);
     launch_ham_pack(raw.as<uint8_t>(), nbytes, nbytes, n, dst, nbp, bx->pop.as<uint32_t>() + n0, nullptr);
 }
 
 // The packed rows and their popcounts go to HBM when they fit there (LGPU_BINARY_HBM_BYTES, rows_fit_hbm), else the
-// rows are packed into pinned host memory the handle owns.  HBM rows and popcounts are allocated exactly, so that
-// device bytes of the two placements differ by nrows x (nbytes_pad + 4).
+// rows are packed into pinned host memory the handle owns: an append of nrows rows to an empty store.  HBM rows and
+// popcounts are allocated exactly, so that device bytes of the two placements differ by nrows x (nbytes_pad + 4); an
+// empty HBM handle holds 16 bytes of each, with headroom.
 int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, const uint64_t *row_ids, int device,
                      lgpu_binary **out)
 {
@@ -4147,16 +4195,12 @@ int lgpu_binary_open(const uint8_t *vectors, uint64_t nrows, uint32_t nbytes, co
         bx->device = device; bx->nrows = nrows; bx->nbytes = nbytes; bx->nbytes_pad = (nbytes + 31) & ~31u;
         const uint32_t nbp = bx->nbytes_pad;
         const bool host = !rows_fit_hbm("LGPU_BINARY_HBM_BYTES", nrows * (nbp + 4));
-        if (host || nrows) {
-            bx->rows.open(host, (size_t)nrows * nbp);
-            if (!host) bx->pop.ensure((size_t)nrows * 4, true);
-            ham_store_rows(bx, vectors, 0, nrows);
-        } else {
-            bx->rows.hbm.ensure(16);
-            bx->pop.ensure(16);
-        }
+        if (host || nrows) bx->rows.open(host, (size_t)nrows * nbp);
+        else bx->rows.hbm.ensure(16);
+        if (!host) bx->pop.ensure(nrows ? (size_t)nrows * 4 : 16, nrows > 0);
+        ham_store_rows(bx, vectors, 0, nrows);
         open_rows(bx, row_ids, nrows);
-        ham_sample(bx, nrows);
+        ham_sample(bx, 0, nrows);
         LGPU_CUDA(cudaDeviceSynchronize());
         register_handle(bx);
         *out = bx;
@@ -4405,13 +4449,10 @@ template <class H> static int delete_rows(H *hp, const uint64_t *row_ids, uint64
     });
 }
 
-// the bytes of one stored row
-static size_t stored_row_bytes(const lgpu_flat *fl) { return (size_t)fl->dim * (fl->f16 ? 2 : 4); }
-static size_t stored_row_bytes(const lgpu_binary *bx) { return bx->nbytes_pad; }
-
 // The sequence of a flat or binary append of n rows (row_ids: host, null = the positions that follow): hold the handle
-// alone, `check(h)`, grow the row store and `store(h, n0, n)` the rows into it, set their ids and live bits, then the
-// kind's per-row terms `terms(h, n0, n)`, drain the device and publish the new row count.
+// alone, `check(h)`, grow the row store and `store(h, rows, n0, n)` the rows into it, set their ids and live bits,
+// then the kind's per-row terms `terms(h, n0, n)`, drain the device and publish the new row count.  The kind's open
+// runs the same store and terms on an empty store of the placement it chose.
 template <class H, class Check, class Store, class Terms>
 static int append_rows(H *hp, const void *rows, uint64_t n, const uint64_t *row_ids, Check &&check, Store &&store,
                        Terms &&terms)
@@ -4425,7 +4466,7 @@ static int append_rows(H *hp, const void *rows, uint64_t n, const uint64_t *row_
         begin_append(h->device);
         const uint64_t n0 = h->nrows, n1 = n0 + n;
         h->rows.grow(n0 * stored_row_bytes(h.h), n1 * stored_row_bytes(h.h));
-        store(h.h, n0, n);
+        store(h.h, rows, n0, n);
         append_ids(h.h, n0, n, row_ids);
         grow_live(h.h, n0, n, bound);
         terms(h.h, n0, n);
@@ -4436,54 +4477,15 @@ static int append_rows(H *hp, const void *rows, uint64_t n, const uint64_t *row_
 
 extern "C" {
 
-// lgpu_flat_append and lgpu_flat_append_f16: the rows must have the handle's row type (f16).  The terms, as
-// lgpu_flat_open takes them from n1 rows: the whole column's when it first reaches 4096 rows, else the new rows', the
-// band constants the max over both parts.  In HBM: |x| once a cosine search built it, and the tensor-core operand
+// lgpu_flat_append and lgpu_flat_append_f16: the rows must have the handle's row type (f16)
 static int flat_append(lgpu_flat *flh, const void *rows, bool f16, uint64_t n, const uint64_t *row_ids)
 {
-    const size_t es = f16 ? 2 : 4;
     return append_rows(flh, rows, n, row_ids,
         [&](lgpu_flat *fl) {
             LGPU_REQUIRE(fl->f16 == f16, fl->f16 ? "the handle holds fp16 rows: append them with lgpu_flat_append_f16"
                                                  : "the handle holds f32 rows: append them with lgpu_flat_append");
         },
-        [&](lgpu_flat *fl, uint64_t n0, uint64_t n) { fl->rows.fill(n0 * es * fl->dim, rows, n * es * fl->dim); },
-        [&](lgpu_flat *fl, uint64_t n0, uint64_t n) {
-            const uint64_t n1 = n0 + n;
-            const uint32_t d = fl->dim;
-            const char *x = fl->rows.data() + (size_t)n0 * d * es;
-            if (fl->rows.on_host) {
-                if (!gemm_shape_supported(d) || n1 < 4096) return;
-                if (n0 < 4096) {
-                    fl->has_tc = host_rows_band(fl->rows.data(), f16, n1, d, fl->vec_max, fl->vec_err);
-                } else if (fl->has_tc) {
-                    float xmax = 0.f, xerr = 0.f;
-                    fl->has_tc = host_rows_band(x, f16, n, d, xmax, xerr);
-                    fl->vec_max = std::max(fl->vec_max, xmax);
-                    fl->vec_err = std::max(fl->vec_err, xerr);
-                }
-                return;
-            }
-            if (fl->has_norms) {
-                grow_keep(fl->ysqrt, (size_t)n0 * 4, (size_t)n1 * 4);
-                if (f16) launch_row_norms(reinterpret_cast<const __half *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
-                else launch_row_norms(reinterpret_cast<const float *>(x), n, d, fl->ysqrt.as<float>() + n0, nullptr);
-            }
-            if (!gemm_shape_supported(d) || n1 < 4096) return;
-            if (n0 < 4096) {
-                fl->has_tc = prepare_tc_operand(fl->rows.data(), f16, n1, d, fl->vec_b, fl->vec_n2, fl->vec_max,
-                                                fl->vec_err, nullptr);
-            } else if (fl->has_tc) {
-                if (!f16) grow_keep(fl->vec_b, (size_t)n0 * d * 2, (size_t)n1 * d * 2);
-                grow_keep(fl->vec_n2, (size_t)n0 * 4, (size_t)n1 * 4);
-                float xmax = 0.f, xerr = 0.f;
-                fl->has_tc = tc_operand_rows(x, f16, n, d, f16 ? nullptr : fl->vec_b.as<char>() + (size_t)n0 * d * 2,
-                                             fl->vec_n2.as<float>() + n0, xmax, xerr, nullptr);
-                fl->vec_max = std::max(fl->vec_max, xmax);
-                fl->vec_err = std::max(fl->vec_err, xerr);
-            }
-            if (!fl->has_tc) { fl->vec_b.reset(); fl->vec_n2.reset(); }
-        });
+        flat_store_rows, flat_row_terms);
 }
 
 int lgpu_flat_append(lgpu_flat *flh, const float *rows, uint64_t n, const uint64_t *row_ids)
@@ -4496,16 +4498,9 @@ int lgpu_flat_append_f16(lgpu_flat *flh, const uint16_t *rows, uint64_t n, const
     return flat_append(flh, rows, true, n, row_ids);
 }
 
-// the terms: an HBM store's popcounts (stored with the rows), and the threshold sample lgpu_binary_open takes from n1
-// rows
 int lgpu_binary_append(lgpu_binary *bxh, const uint8_t *rows, uint64_t n, const uint64_t *row_ids)
 {
-    return append_rows(bxh, rows, n, row_ids, [](lgpu_binary *) {},
-        [&](lgpu_binary *bx, uint64_t n0, uint64_t n) {
-            if (!bx->rows.on_host) grow_keep(bx->pop, (size_t)n0 * 4, (size_t)(n0 + n) * 4);
-            ham_store_rows(bx, rows, n0, n);
-        },
-        [](lgpu_binary *bx, uint64_t n0, uint64_t n) { ham_sample(bx, n0 + n); });
+    return append_rows(bxh, rows, n, row_ids, [](lgpu_binary *) {}, ham_store_rows, ham_sample);
 }
 
 int lgpu_index_delete(lgpu_index *ix, const uint64_t *row_ids, uint64_t n, uint64_t *n_deleted)
@@ -4757,26 +4752,18 @@ static int multivec_open(const void *values, bool f16, const uint64_t *offsets, 
         mv->rows.open(host, xbytes);
         mv->rows.fill(0, values, xbytes);
         if (hbytes) mv->ops.open(host, hbytes);
-        if (host) {
-            // |v| (and an f32 handle's fp16 operand) computed chunk by chunk of whole rows staged through HBM (each
-            // vector's terms depend on that vector alone)
-            const std::vector<uint64_t> cut = mv_chunks(mv, std::max<uint64_t>(1, FLAT_STAGE_BYTES / ((size_t)dim * es)));
-            DevBuf xs, hs;
-            for (size_t c = 0; c + 1 < cut.size(); c++) {
-                const uint64_t j0 = offsets[cut[c]], n = offsets[cut[c + 1]] - j0;
-                if (!n) continue;
-                xs.ensure(n * dim * es);
-                if (hbytes) hs.ensure(n * dim * 2);
-                LGPU_CUDA(cudaMemcpy(xs.p, static_cast<const char *>(values) + j0 * dim * es, n * dim * es,
-                                     cudaMemcpyHostToDevice));
-                ok &= mv_vector_terms(xs.p, f16, n, dim, mv->ysqrt.as<float>() + j0, tc_shape, hbytes ? hs.p : nullptr);
-                if (hbytes)
-                    LGPU_CUDA(cudaMemcpy(mv->ops.data() + j0 * dim * 2, hs.p, n * dim * 2, cudaMemcpyDeviceToHost));
-            }
-        } else if (T) {
-            ok = mv_vector_terms(mv->rows.data(), f16, T, dim, mv->ysqrt.as<float>(), tc_shape,
-                                 hbytes ? mv->ops.data() : nullptr);
-        }
+        // |v| (and an f32 handle's fp16 operand) of each chunk of vectors the row store visits (each vector's terms
+        // depend on that vector alone): a resident chunk's operand is written in place, a staged chunk's copied back
+        // into the pinned operand
+        DevBuf hs;
+        mv->rows.visit(0, T, (size_t)dim * es, [&](const RowChunk &ch) {
+            const uint64_t n = ch.r1 - ch.r0;
+            char *h = hbytes ? mv->ops.data() + ch.r0 * dim * 2 : nullptr;      // the chunk's stored operand
+            const bool copy = h && !ch.resident;
+            if (copy) hs.ensure(n * dim * 2);
+            ok &= mv_vector_terms(ch.X, f16, n, dim, mv->ysqrt.as<float>() + ch.r0, tc_shape, copy ? hs.p : h);
+            if (copy) LGPU_CUDA(cudaMemcpy(h, hs.p, n * dim * 2, cudaMemcpyDeviceToHost));
+        });
         if (tc_shape) {
             std::vector<uint32_t> cr(T);
             for (uint64_t r = 0; r < nrows; r++)
