@@ -593,9 +593,11 @@ int  lgpu_ivf_binary_search_unindexed_device(lgpu_ivf_binary *ix, lgpu_binary *t
  * queries: [Tq][dim] f32, Tq = q_offsets[B]; q_offsets: [B+1] u32 HOST array (also for the device entry point: it is
  * the batch's shape), q_offsets[0] = 0, query b's vectors are queries[q_offsets[b] .. q_offsets[b+1]), 1..4096 each.
  * Columns of at least 65536 vectors, all finite and non-zero, with dim a multiple of 8, are scored on the tensor cores
- * (fp16 copies of the normalised vectors) when the call has no prefilter or distance_range: every row within a
- * rigorous error band of the k-th approximate distance is re-scored exactly, and a query whose shortlist overflows or
- * that holds a zero / non-finite vector is redone exactly, so the results are the exact ones either way.
+ * (fp16 copies of the normalised vectors) when the call has no distance_range: every row within a rigorous error band
+ * of the k-th approximate distance is re-scored exactly, and a query whose shortlist overflows or that holds a zero /
+ * non-finite vector is redone exactly, so the results are the exact ones either way.  Under a prefilter or deleted rows
+ * the k-th distance is taken over the allowed rows and only allowed rows are re-scored; with fewer than k allowed rows
+ * every allowed row is.
  * lgpu_last_filter_stats after a profiled multivector call: [0] rows admitted to the shortlists, [1] rows scored
  * exactly (on the exact path: B x nrows), [2] queries redone densely after the shortlist, [3] queries. */
 int  lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
@@ -612,6 +614,23 @@ int  lgpu_multivec_open(const float *values, const uint64_t *offsets, uint64_t n
  * values: IEEE binary16 bits, [T][dim].  Every other lgpu_multivec_* function takes both row types. */
 int  lgpu_multivec_open_f16(const uint16_t *values, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
                             const uint64_t *row_ids /* NULL => 0..nrows-1 */, int device, lgpu_multivec **out);
+/* Append n rows to the column: values HOST [offsets[n]][dim] in the handle's row type (IEEE binary16 bits for
+ * lgpu_multivec_append_f16), offsets HOST [n + 1] as lgpu_multivec_open takes them (offsets[0] = 0, non-decreasing,
+ * rows of 0..2^20 vectors, the column at most 2^40 vectors); row_ids NULL => the positions that follow (nrows,
+ * nrows + 1, ...).  Afterwards the handle returns, on every entry point, exactly what lgpu_multivec_open[_f16] on the
+ * concatenated rows (and ids) returns, and takes the same route: the tensor-core route once the column holds 65536
+ * vectors, all finite and non-zero (an append that first gets there builds the fp16 operand of every vector), the exact
+ * route from the first appended zero or non-finite vector on.  As lgpu_flat_append: explicit ids stay explicit (ids
+ * given to a handle that had none make the old rows' positions explicit); an appended id equal to a deleted id the
+ * handle still holds, lgpu_multivec_append on an fp16 handle or lgpu_multivec_append_f16 on an f32 handle, and rows
+ * the open would refuse, fail with LGPU_INVALID_INPUT; n = 0 changes nothing.  A refused call changes nothing.  The
+ * handle keeps its placement for life: the vectors (and the operand) grow geometrically in HBM or in pinned host
+ * memory, and a pinned allocation that fails is LGPU_OOM.  |v|, the row of each vector and the operand are computed
+ * for the new vectors only.  The call takes the handle alone, as lgpu_flat_append does. */
+int  lgpu_multivec_append(lgpu_multivec *mv, const float *values, const uint64_t *offsets, uint64_t n,
+                          const uint64_t *row_ids /* NULL => the positions that follow */);
+int  lgpu_multivec_append_f16(lgpu_multivec *mv, const uint16_t *values, const uint64_t *offsets, uint64_t n,
+                              const uint64_t *row_ids);
 void lgpu_multivec_close(lgpu_multivec *mv);
 int  lgpu_multivec_search(lgpu_multivec *mv, const float *queries, const uint32_t *q_offsets, uint32_t B,
                           const lgpu_search_params *params, uint64_t *out_ids, float *out_dist, uint32_t *out_count);
@@ -641,11 +660,12 @@ int  lgpu_multivec_device_bytes(const lgpu_multivec *mv, uint64_t *bytes);
  * fp16 operand and re-scores its shortlist from the pinned vectors.  A staging buffer holds the longest row: a search
  * of a handle whose longest row does not fit twice in LGPU_WS_BYTES fails with LGPU_OOM before any device work.
  * Results are identical to an HBM handle's on the same rows -- same ids, counts and distance bits -- for every k,
- * distance_range, prefilter and deleted rows, and lgpu_last_filter_stats means the same.  A handle keeps its placement
- * for life.  A pinned allocation that fails is LGPU_OOM.  The caller's buffers are borrowed for the open call only,
+ * distance_range, prefilter, deleted rows and append, and lgpu_last_filter_stats means the same.  A handle keeps its
+ * placement for life; lgpu_multivec_append grows the pinned row data geometrically.  A pinned allocation that fails is
+ * LGPU_OOM.  The caller's buffers are borrowed for the open call only,
  * either way.
  * *bytes = the pinned host memory the handle holds (T x dim x 4, plus T x dim x 2 for the operand, for an f32 handle; T
- * x dim x 2 for an fp16 handle; 0 for an HBM handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output
+ * x dim x 2 for an fp16 handle; capacity kept for appends included; 0 for an HBM handle), *placement = LGPU_VECTORS_HBM or LGPU_VECTORS_HOST; either output
  * may be NULL. */
 int  lgpu_multivec_host_bytes(const lgpu_multivec *mv, uint64_t *bytes, int *placement);
 

@@ -51,7 +51,7 @@ EXPORTS = [
     "lgpu_flat_open_f16", "lgpu_flat_append_f16", "lgpu_flat_device_bytes",
     "lgpu_index_host_bytes", "lgpu_debug_refine_host", "lgpu_flat_host_bytes",
     "lgpu_multivec_device_bytes", "lgpu_multivec_host_bytes",
-    "lgpu_multivec_open_f16", "lgpu_debug_maxsim_gemm_f16",
+    "lgpu_multivec_open_f16", "lgpu_debug_maxsim_gemm_f16", "lgpu_multivec_append", "lgpu_multivec_append_f16",
     "lgpu_binary_device_bytes", "lgpu_binary_host_bytes",
     "lgpu_index_code_bytes", "lgpu_ivf_binary_code_bytes", "lgpu_last_streamed_code_bytes",
 ]
@@ -216,6 +216,8 @@ def load():
     lib.lgpu_debug_hamming_gemm.argtypes = [vp, vp, u32, C.c_uint64, u32, i32, vp]
     lib.lgpu_multivec_open.argtypes = [vp, vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
     lib.lgpu_multivec_open_f16.argtypes = [vp, vp, C.c_uint64, u32, vp, i32, C.POINTER(vp)]
+    lib.lgpu_multivec_append.argtypes = [vp, vp, vp, C.c_uint64, vp]
+    lib.lgpu_multivec_append_f16.argtypes = [vp, vp, vp, C.c_uint64, vp]
     lib.lgpu_multivec_close.argtypes = [vp]
     lib.lgpu_multivec_close.restype = None
     lib.lgpu_multivec_search.argtypes = [vp, vp, vp, u32, C.POINTER(SearchParams), vp, vp, vp]
@@ -771,16 +773,7 @@ class GpuMultivec(_Column):
 
     def __init__(self, values, offsets, row_ids=None, device: int = 0):
         self.dtype = np.dtype(np.float16 if getattr(values, "dtype", None) == np.float16 else np.float32)
-        v = np.ascontiguousarray(values, self.dtype)
-        off = np.ascontiguousarray(offsets, np.uint64)
-        if v.ndim != 2:
-            raise ValueError("multivector values must be a [vectors, dim] array")
-        if off.ndim != 1 or off.size < 1 or off[0] != 0 or int(off[-1]) != v.shape[0]:
-            raise ValueError("row offsets must be [rows + 1], start at 0 and end at the number of vectors")
-        if np.any(off[1:] < off[:-1]):
-            raise ValueError("row offsets must not decrease")
-        if off.size > 1 and int(np.max(off[1:] - off[:-1])) > MULTIVEC_MAX_ROW:
-            raise ValueError(f"a multivector row holds at most {MULTIVEC_MAX_ROW} vectors")
+        v, off = self._rows(values, offsets)
         if not 1 <= v.shape[1] <= MULTIVEC_MAX_DIM:
             raise ValueError(f"multivector dimension must be in [1, {MULTIVEC_MAX_DIM}]")
         self.nrows, self.dim = off.size - 1, v.shape[1]
@@ -792,6 +785,35 @@ class GpuMultivec(_Column):
         check(getattr(load(), opener)(_ptr(v), _ptr(off), self.nrows, self.dim, _ptr(rid), device, C.byref(h)))
         self._h = h
         self.device = device
+
+    def _rows(self, values, offsets):
+        """(values [T, dim] in the handle's row type, offsets [n+1] u64) of rows to open or append, checked."""
+        v = np.ascontiguousarray(values, self.dtype)
+        off = np.ascontiguousarray(offsets, np.uint64)
+        if v.ndim != 2:
+            raise ValueError("multivector values must be a [vectors, dim] array")
+        if off.ndim != 1 or off.size < 1 or off[0] != 0 or int(off[-1]) != v.shape[0]:
+            raise ValueError("row offsets must be [rows + 1], start at 0 and end at the number of vectors")
+        if np.any(off[1:] < off[:-1]):
+            raise ValueError("row offsets must not decrease")
+        if off.size > 1 and int(np.max(off[1:] - off[:-1])) > MULTIVEC_MAX_ROW:
+            raise ValueError(f"a multivector row holds at most {MULTIVEC_MAX_ROW} vectors")
+        return v, off
+
+    def append(self, values, offsets, row_ids=None):
+        """Append rows in place (lgpu_multivec_append[_f16]): values [T, dim] and offsets [n+1] as the constructor
+        takes them; row_ids None = the positions that follow.  An fp16 handle takes float16 values only, and an f32
+        handle no float16 values: a vector is never rounded to fit the handle.  Checked before any device call."""
+        if (getattr(values, "dtype", None) == np.float16) != (self.dtype == np.float16):
+            raise ValueError(f"append to a {self.dtype.name} multivector handle needs values of that type, not "
+                             f"{getattr(values, 'dtype', type(values).__name__)}")
+        v, off = self._rows(values, offsets)
+        if v.shape[1] != self.dim:
+            raise ValueError(f"multivector values must have dimension {self.dim}, got shape {v.shape}")
+        rid = _rows_ids(off[1:], row_ids)
+        appender = "lgpu_multivec_append_f16" if self.dtype == np.float16 else "lgpu_multivec_append"
+        check(getattr(load(), appender)(self._h, _ptr(v), _ptr(off), off.size - 1, _ptr(rid)))
+        self.nrows += off.size - 1
 
     def _queries(self, queries, q_offsets):
         """(values [Tq, dim] f32, offsets [B+1] u32).  queries: a list with one [nq_b, dim] (or [dim]) array per

@@ -722,7 +722,6 @@ struct lgpu_multivec : lgpu_rows {
 
 // the bytes of one stored row
 static size_t stored_row_bytes(const lgpu_flat *fl) { return (size_t)fl->dim * (fl->f16 ? 2 : 4); }
-static size_t stored_row_bytes(const lgpu_binary *bx) { return bx->nbytes_pad; }
 
 
 // ---- NCCL, bound at run time (dlopen): single-GPU hosts need no libnccl, and inside a process that already
@@ -2416,8 +2415,16 @@ constexpr uint32_t MV_MAX_DIM = 65536;
 //                 those rows (dist.cu) -> select mode 2; a query whose list overflowed or that holds a zero /
 //                 non-finite vector is redone by the exact path below in the same stream (flags / gate: nothing runs
 //                 when no query is flagged).  Taken when the column holds at least MV_TC_MIN_T vectors (all of them
-//                 finite and non-zero), dim is a multiple of 8, there is no prefilter or distance_range,
-//                 LGPU_NO_TENSOR_CORE is not set and one query's scores fit the workspace.
+//                 finite and non-zero), dim is a multiple of 8, there is no distance_range, LGPU_NO_TENSOR_CORE is
+//                 not set and one query's scores fit the workspace.  Under a row filter (a prefilter, deleted rows:
+//                 the RowFilter of the call) the k-th select sees the allowed rows only and mv_admit_kernel admits
+//                 only allowed rows, so a filtered row never costs a shortlist slot or a re-score.  The band is
+//                 unchanged: leaving rows out of the select can only raise the k-th approximate distance tau, and
+//                 the k allowed rows with A <= tau have D <= tau + E, so the allowed exact k-th distance D_k is at
+//                 most tau + E and every allowed row of the exact top-k has A <= D + E <= D_k + E <= tau + 2 E.
+//                 With fewer than k allowed rows the select returns fewer than k, tau is +inf and every
+//                 allowed row is admitted; a list that overflows goes to the fix-up, which filters as the exact
+//                 route does.
 //   exact         for every sub-batch of queries, blocks of consecutive query vectors against chunks of whole rows --
 //                 dist_matrix_kernel (cosine, lance order) -> per-row minimum -> in-order running sum into D[b][N] --
 //                 then select mode 1 (distance_range, prefilter, (_distance, _rowid) order, NaN dropped).
@@ -2537,7 +2544,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
     uint32_t max_nq = 0;
     for (uint32_t b = 0; b < B; b++) max_nq = std::max(max_nq, h_qoff[b + 1] - h_qoff[b]);
     const size_t quarter = budget / 4;
-    const bool tc = mv->tc_ok && tc_enabled() && !rf.bits && !sp.has_lower && !sp.has_upper && k <= SELECT_KMAX &&
+    const bool tc = mv->tc_ok && tc_enabled() && !sp.has_lower && !sp.has_upper && k <= SELECT_KMAX &&
                     (size_t)(max_nq + 1) * ld * 4 <= quarter;
     const size_t S = mv->rows.on_host ? mv_stage_bytes(mv) : 0, left = budget / 2 > 2 * S ? budget / 2 - 2 * S : 0;
     mv->rows.reserve_stage(ws, S);
@@ -2603,14 +2610,17 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
                 launch_mv_approx_sum(ws->mv_Mk.as<uint32_t>(), ldc, ws->mv_qoff.as<uint32_t>(), qa, qb, va, rb - ra,
                                      A + ra, ld, mv->num_sms, st);
             });
-            // the k-th smallest approximate distance of each query
-            launch_select(select_rows(A, N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
-                                                      ws->mv_kc.as<uint32_t>()}), st);
+            // the k-th smallest approximate distance of each query over the allowed rows (A's column r is row r of
+            // the handle in both placements, so its id is ids[r], or r)
+            SelectArgs sk = select_rows(A, N, ld, b, k, {ws->mv_ki.as<uint64_t>(), ws->mv_kd.as<float>(),
+                                                         ws->mv_kc.as<uint32_t>()});
+            if (rf.bits) { with_cols(sk, ids); sk.allow = rf.bits; sk.allow_bits = rf.nbits; }
+            launch_select(sk, st);
             launch_mv_threshold(ws->mv_kd.as<float>(), ws->mv_kc.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b, k, dim,
                                 mv->f16, ws->mv_thr.as<float>(), st);
             LGPU_CUDA(cudaMemsetAsync(ws->mv_cnt.p, 0, (size_t)b * 4, st));
             launch_mv_admit(A, ld, b, N, ws->mv_thr.as<float>(), cap, ws->mv_cnt.as<uint32_t>(),
-                            ws->mv_cand.as<uint32_t>(), st);
+                            ws->mv_cand.as<uint32_t>(), ids, rf.bits, rf.nbits, st);
             launch_mv_flags(ws->mv_cnt.as<uint32_t>(), cap, ws->mv_qbad.as<uint32_t>(), ws->mv_qoff.as<uint32_t>(), qa, b,
                             ws->mv_flags.as<uint32_t>(), ws->mv_vflags.as<uint32_t>(), ws->mv_gate.as<uint32_t>(), st);
             auto rescore = [&](auto *v) {
@@ -2648,6 +2658,7 @@ void multivec_search_device(lgpu_multivec *mv, Workspace *ws, cudaStream_t st, c
             SelectArgs sc = select_rows(A, N, ld, b, k, out.at(qa, k));
             sc.col_ids = ids;
             sc.only = ws->mv_flags.as<uint32_t>(); sc.gate = gate;
+            sc.allow = rf.bits; sc.allow_bits = rf.nbits;
             launch_select(sc, st);
             if (prof) {             // [0] rows admitted, [1] rows re-scored exactly, [2] queries redone densely
                 std::vector<uint32_t> cnt(b), fl(b);
@@ -4010,10 +4021,11 @@ static uint64_t flat_row_data_bytes(uint64_t n, uint32_t d, bool f16)
     return rows + (f16 ? 0 : n * d * 2) + n * 4;
 }
 
-// n of the caller's rows into rows n0.. of a flat handle's store
+// n of the caller's rows into rows n0.. of a flat handle's store, grown to hold them
 static void flat_store_rows(lgpu_flat *fl, const void *src, uint64_t n0, uint64_t n)
 {
     const size_t row = stored_row_bytes(fl);
+    fl->rows.grow(n0 * row, (n0 + n) * row);
     fl->rows.fill(n0 * row, src, n * row);
 }
 
@@ -4165,11 +4177,12 @@ static void ham_pack_host(const uint8_t *src, uint64_t n, uint32_t nbytes, uint3
     }
 }
 
-// n of the caller's rows [n][nbytes] into rows n0.. of a binary handle's store, packed: on the host into pinned memory,
-// or in HBM from an upload, with their popcounts into `pop` (grown to hold them)
+// n of the caller's rows [n][nbytes] into rows n0.. of a binary handle's store (grown to hold them), packed: on the host
+// into pinned memory, or in HBM from an upload, with their popcounts into `pop` (grown to hold them)
 static void ham_store_rows(lgpu_binary *bx, const void *src, uint64_t n0, uint64_t n)
 {
     const uint32_t nbytes = bx->nbytes, nbp = bx->nbytes_pad;
+    bx->rows.grow((size_t)n0 * nbp, (size_t)(n0 + n) * nbp);
     uint8_t *dst = reinterpret_cast<uint8_t *>(bx->rows.data()) + (size_t)n0 * nbp;
     if (bx->rows.on_host) return ham_pack_host(static_cast<const uint8_t *>(src), n, nbytes, nbp, dst);
     grow_keep(bx->pop, (size_t)n0 * 4, (size_t)(n0 + n) * 4);
@@ -4449,12 +4462,12 @@ template <class H> static int delete_rows(H *hp, const uint64_t *row_ids, uint64
     });
 }
 
-// The sequence of a flat or binary append of n rows (row_ids: host, null = the positions that follow): hold the handle
-// alone, `check(h)`, grow the row store and `store(h, rows, n0, n)` the rows into it, set their ids and live bits,
-// then the kind's per-row terms `terms(h, n0, n)`, drain the device and publish the new row count.  The kind's open
-// runs the same store and terms on an empty store of the placement it chose.
-template <class H, class Check, class Store, class Terms>
-static int append_rows(H *hp, const void *rows, uint64_t n, const uint64_t *row_ids, Check &&check, Store &&store,
+// The sequence of a flat, binary or multivector append of n rows (row_ids: host, null = the positions that follow):
+// hold the handle alone, `check(h)`, `store(h, rows, n0, n)` the rows into the row store, grown to hold them, set
+// their ids and live bits, then the kind's per-row terms `terms(h, n0, n)`, drain the device and publish the new row
+// count.  The kind's open runs the same store and terms on an empty store of the placement it chose.
+template <class H, class R, class Check, class Store, class Terms>
+static int append_rows(H *hp, const R *rows, uint64_t n, const uint64_t *row_ids, Check &&check, Store &&store,
                        Terms &&terms)
 {
     return guarded([&] {
@@ -4465,7 +4478,6 @@ static int append_rows(H *hp, const void *rows, uint64_t n, const uint64_t *row_
         const uint64_t bound = live_bound_after(h.h, n, row_ids);
         begin_append(h->device);
         const uint64_t n0 = h->nrows, n1 = n0 + n;
-        h->rows.grow(n0 * stored_row_bytes(h.h), n1 * stored_row_bytes(h.h));
         store(h.h, rows, n0, n);
         append_ids(h.h, n0, n, row_ids);
         grow_live(h.h, n0, n, bound);
@@ -4697,14 +4709,16 @@ int lgpu_debug_ivf_hamming_scan(const uint8_t *queries, uint32_t B, const uint8_
     });
 }
 
-// |v| of n stored vectors in HBM (f32, or fp16 when f16) into ysqrt and, when `check`, whether every one of them is
+// |v| of stored vectors [skip, n) of n in HBM (f32, or fp16 when f16) into ysqrt and, when `check`, whether every one of
+// the n is
 // finite and non-zero (false: the tensor-core path may not run), with the fp16 normalised operand of f32 vectors into
 // Xh.  fp16 vectors are their own operand: the same kernels read their exact f32 upcast, so |v| and the check are an
 // f32 handle's on those values.
-static bool mv_vector_terms(const void *X, bool f16, uint64_t n, uint32_t dim, float *ysqrt, bool check, void *Xh)
+static bool mv_vector_terms(const void *X, bool f16, uint64_t n, uint32_t dim, float *ysqrt, uint64_t skip, bool check,
+                            void *Xh)
 {
-    if (f16) launch_row_norms(static_cast<const __half *>(X), n, dim, ysqrt, nullptr);
-    else launch_row_norms(static_cast<const float *>(X), n, dim, ysqrt, nullptr);
+    if (f16) launch_row_norms(static_cast<const __half *>(X) + skip * dim, n - skip, dim, ysqrt + skip, nullptr);
+    else launch_row_norms(static_cast<const float *>(X) + skip * dim, n - skip, dim, ysqrt + skip, nullptr);
     if (!check) return true;
     DevBuf bad;
     bad.ensure(n * 4);
@@ -4715,7 +4729,101 @@ static bool mv_vector_terms(const void *X, bool f16, uint64_t n, uint32_t dim, f
     return std::none_of(hb.begin(), hb.end(), [](uint32_t b) { return b != 0; });
 }
 
-// lgpu_multivec_open and lgpu_multivec_open_f16: vectors f32 or fp16 (f16), kept as given
+// the rows an open or append hands a multivector handle: values [offsets[n]][dim] in the row type, offsets [n + 1]
+struct MvRows {
+    const void *values;
+    const uint64_t *offsets;
+};
+
+// The checks of n rows an open or append hands a handle that holds `held` vectors, before anything changes: offsets
+// that start at 0 and do not decrease, rows of at most MV_MAX_ROW vectors, a column of at most 2^40 vectors, and
+// values for any vector.
+static void check_multivec_rows(const MvRows &src, uint64_t n, uint64_t held)
+{
+    const uint64_t *offsets = src.offsets;
+    LGPU_REQUIRE(offsets != nullptr, "null argument");
+    LGPU_REQUIRE(offsets[0] == 0, "row offsets must start at 0");
+    for (uint64_t r = 0; r < n; r++) {
+        LGPU_REQUIRE(offsets[r + 1] >= offsets[r], "row offsets must not decrease");
+        LGPU_REQUIRE(offsets[r + 1] - offsets[r] <= MV_MAX_ROW, "a multivector row holds at most 2^20 vectors");
+    }
+    const uint64_t T = offsets[n];
+    LGPU_REQUIRE(T <= ((uint64_t)1 << 40) - held, "a multivector column holds at most 2^40 vectors");
+    LGPU_REQUIRE(T == 0 || src.values != nullptr, "null vectors");
+}
+
+// whether a column of T vectors in nrows rows has the tensor-core shape
+static bool mv_tc_shape(uint64_t T, uint64_t nrows, uint32_t dim)
+{
+    return T >= MV_TC_MIN_T && T < ((uint64_t)1 << 31) && nrows < 0xffffffffull && gemm_shape_supported(dim);
+}
+
+// n of the caller's rows into rows n0.. of a multivector handle: their offsets (host and device) and their vectors into
+// the row store, grown to hold them
+static void mv_store_rows(lgpu_multivec *mv, const MvRows *src, uint64_t n0, uint64_t n)
+{
+    const uint64_t T0 = mv->h_offsets[n0], T = src->offsets[n];
+    const size_t vb = (size_t)mv->dim * mv_elem_bytes(mv);
+    mv->h_offsets.resize(n0 + 1);                         // (a failed append may have left more)
+    for (uint64_t r = 1; r <= n; r++) mv->h_offsets.push_back(T0 + src->offsets[r]);
+    grow_keep(mv->offsets, (n0 + 1) * 8, (n0 + n + 1) * 8);
+    LGPU_CUDA(cudaMemcpy(mv->offsets.as<uint64_t>() + n0, mv->h_offsets.data() + n0, (n + 1) * 8,
+                         cudaMemcpyHostToDevice));
+    mv->rows.grow(T0 * vb, (T0 + T) * vb);
+    mv->rows.fill(T0 * vb, src->values, T * vb);
+}
+
+// The per-vector terms of a multivector handle once rows [n0, n0 + n) are stored, at open (n0 = 0) or append: |v| of
+// their vectors, the longest row and the vector count.  Once the column has the tensor-core shape (mv_tc_shape), the row
+// of each vector (col_row), an f32 handle's fp16 normalised operand (`ops`, the rows' placement) and tc_ok, whether
+// every stored vector normalises (a zero or non-finite vector has NaN pairs, which the approximate score cannot skip as
+// the exact min does): of every vector when the column first gets there, else of the new vectors while tc_ok holds, so
+// tc_ok ends as an open of the whole column sets it.  Each chunk of the row store's visit gets mv_vector_terms (each
+// vector's terms depend on that vector alone): a resident chunk's operand is written in place, a staged chunk's copied
+// back into the pinned operand.
+static void mv_row_terms(lgpu_multivec *mv, uint64_t n0, uint64_t n)
+{
+    const uint64_t n1 = n0 + n, *off = mv->h_offsets.data(), T0 = off[n0], T1 = off[n1];
+    const uint32_t dim = mv->dim;
+    const bool f16 = mv->f16;
+    const uint64_t a = T0 < MV_TC_MIN_T ? 0 : T0;          // the first vector whose operand is taken
+    const bool tc = mv_tc_shape(T1, n1, dim) && (a == 0 || mv->tc_ok);
+    grow_keep(mv->ysqrt, T0 * 4, T1 * 4);
+    if (tc) {
+        if (a == 0) {                                      // the column gets there: operand of every vector
+            mv->col_row.ensure(T1 * 4);
+            if (!f16) mv->ops.open(mv->rows.on_host, T1 * dim * 2);
+        } else {
+            grow_keep(mv->col_row, a * 4, T1 * 4);
+            if (!f16) mv->ops.grow(a * dim * 2, T1 * dim * 2);
+        }
+    }
+    bool ok = true;
+    DevBuf hs;
+    mv->rows.visit(tc ? a : T0, T1, (size_t)dim * mv_elem_bytes(mv), [&](const RowChunk &ch) {
+        const uint64_t m = ch.r1 - ch.r0;
+        char *h = tc && !f16 ? mv->ops.data() + ch.r0 * dim * 2 : nullptr;   // the chunk's stored operand
+        const bool copy = h && !ch.resident;
+        if (copy) hs.ensure(m * dim * 2);
+        const uint64_t skip = std::min(m, T0 > ch.r0 ? T0 - ch.r0 : 0);  // old vectors: their |v| is kept
+        ok &= mv_vector_terms(ch.X, f16, m, dim, mv->ysqrt.as<float>() + ch.r0, skip, tc, copy ? hs.p : h);
+        if (copy) LGPU_CUDA(cudaMemcpy(h, hs.p, m * dim * 2, cudaMemcpyDeviceToHost));
+    });
+    if (tc && T1 > a) {
+        std::vector<uint32_t> cr(T1 - a);
+        for (uint64_t r = a ? n0 : 0; r < n1; r++)
+            for (uint64_t j = off[r]; j < off[r + 1]; j++) cr[j - a] = (uint32_t)r;
+        LGPU_CUDA(cudaMemcpy(mv->col_row.as<uint32_t>() + a, cr.data(), (T1 - a) * 4, cudaMemcpyHostToDevice));
+    }
+    mv->tc_ok = tc && ok;
+    for (uint64_t r = n0; r < n1; r++) mv->max_row = std::max(mv->max_row, off[r + 1] - off[r]);
+    mv->total = T1;
+}
+
+// lgpu_multivec_open and lgpu_multivec_open_f16: vectors f32 or fp16 (f16), kept as given, in HBM when the row data --
+// the vectors, and an f32 handle's operand when the column has the tensor-core shape -- fits there
+// (LGPU_MULTIVEC_HBM_BYTES, rows_fit_hbm), else in pinned host memory the handle owns: an append of nrows rows to an
+// empty store.  The rows and the operand are allocated exactly.
 static int multivec_open(const void *values, bool f16, const uint64_t *offsets, uint64_t nrows, uint32_t dim,
                          const uint64_t *row_ids, int device, lgpu_multivec **out)
 {
@@ -4723,57 +4831,22 @@ static int multivec_open(const void *values, bool f16, const uint64_t *offsets, 
     int rc = guarded([&] {
         LGPU_REQUIRE(out != nullptr && offsets != nullptr, "null argument");
         LGPU_REQUIRE(dim >= 1 && dim <= MV_MAX_DIM, "multivector dimension must be in [1, 65536]");
-        LGPU_REQUIRE(offsets[0] == 0, "row offsets must start at 0");
-        uint64_t max_row = 0;
-        for (uint64_t r = 0; r < nrows; r++) {
-            LGPU_REQUIRE(offsets[r + 1] >= offsets[r], "row offsets must not decrease");
-            LGPU_REQUIRE(offsets[r + 1] - offsets[r] <= MV_MAX_ROW, "a multivector row holds at most 2^20 vectors");
-            max_row = std::max<uint64_t>(max_row, offsets[r + 1] - offsets[r]);
-        }
-        const uint64_t T = offsets[nrows];
-        LGPU_REQUIRE(T <= ((uint64_t)1 << 40), "a multivector column holds at most 2^40 vectors");
-        LGPU_REQUIRE(T == 0 || values != nullptr, "null vectors");
+        const MvRows src{values, offsets};
+        check_multivec_rows(src, nrows, 0);
         require_device(device);
         mv = new lgpu_multivec();
-        mv->device = device; mv->nrows = nrows; mv->total = T; mv->dim = dim; mv->max_row = max_row; mv->f16 = f16;
-        mv->h_offsets.assign(offsets, offsets + nrows + 1);
-        // the tensor-core operand: only when every stored vector normalises (a zero or non-finite vector has NaN pairs,
-        // which the approximate score cannot skip as the exact min does) and the shape suits the GEMM.  An fp16
-        // handle's vectors are their own operand: no copy
-        const bool tc_shape = T >= MV_TC_MIN_T && T < ((uint64_t)1 << 31) && nrows < 0xffffffffull &&
-                              gemm_shape_supported(dim);
-        const size_t es = f16 ? 2 : 4;
-        const size_t xbytes = (size_t)T * dim * es, hbytes = tc_shape && !f16 ? (size_t)T * dim * 2 : 0;
+        mv->device = device; mv->nrows = nrows; mv->dim = dim; mv->f16 = f16;
+        mv->h_offsets.assign(1, 0);
+        const uint64_t T = offsets[nrows];
+        const size_t xbytes = (size_t)T * dim * mv_elem_bytes(mv);
+        const size_t hbytes = mv_tc_shape(T, nrows, dim) && !f16 ? (size_t)T * dim * 2 : 0;
+        mv->rows.open(!rows_fit_hbm("LGPU_MULTIVEC_HBM_BYTES", xbytes + hbytes), xbytes);
         mv->ysqrt.ensure(std::max<size_t>((size_t)T * 4, 16));
         mv->offsets.ensure((size_t)(nrows + 1) * 8);
-        LGPU_CUDA(cudaMemcpy(mv->offsets.p, offsets, (size_t)(nrows + 1) * 8, cudaMemcpyHostToDevice));
-        bool ok = true;
-        const bool host = !rows_fit_hbm("LGPU_MULTIVEC_HBM_BYTES", xbytes + hbytes);
-        mv->rows.open(host, xbytes);
-        mv->rows.fill(0, values, xbytes);
-        if (hbytes) mv->ops.open(host, hbytes);
-        // |v| (and an f32 handle's fp16 operand) of each chunk of vectors the row store visits (each vector's terms
-        // depend on that vector alone): a resident chunk's operand is written in place, a staged chunk's copied back
-        // into the pinned operand
-        DevBuf hs;
-        mv->rows.visit(0, T, (size_t)dim * es, [&](const RowChunk &ch) {
-            const uint64_t n = ch.r1 - ch.r0;
-            char *h = hbytes ? mv->ops.data() + ch.r0 * dim * 2 : nullptr;      // the chunk's stored operand
-            const bool copy = h && !ch.resident;
-            if (copy) hs.ensure(n * dim * 2);
-            ok &= mv_vector_terms(ch.X, f16, n, dim, mv->ysqrt.as<float>() + ch.r0, tc_shape, copy ? hs.p : h);
-            if (copy) LGPU_CUDA(cudaMemcpy(h, hs.p, n * dim * 2, cudaMemcpyDeviceToHost));
-        });
-        if (tc_shape) {
-            std::vector<uint32_t> cr(T);
-            for (uint64_t r = 0; r < nrows; r++)
-                for (uint64_t j = offsets[r]; j < offsets[r + 1]; j++) cr[j] = (uint32_t)r;
-            mv->col_row.ensure((size_t)T * 4);
-            LGPU_CUDA(cudaMemcpy(mv->col_row.p, cr.data(), (size_t)T * 4, cudaMemcpyHostToDevice));
-            mv->tc_ok = ok;
-        }
-        LGPU_CUDA(cudaDeviceSynchronize());
+        mv_store_rows(mv, &src, 0, nrows);
         open_rows(mv, row_ids, nrows);
+        mv_row_terms(mv, 0, nrows);
+        LGPU_CUDA(cudaDeviceSynchronize());
         register_handle(mv);
         *out = mv;
     });
@@ -4791,6 +4864,32 @@ int lgpu_multivec_open_f16(const uint16_t *values, const uint64_t *offsets, uint
                            const uint64_t *row_ids, int device, lgpu_multivec **out)
 {
     return multivec_open(values, true, offsets, nrows, dim, row_ids, device, out);
+}
+
+// lgpu_multivec_append and lgpu_multivec_append_f16: the vectors must have the handle's row type (f16)
+static int multivec_append(lgpu_multivec *mvh, const void *values, bool f16, const uint64_t *offsets, uint64_t n,
+                           const uint64_t *row_ids)
+{
+    const MvRows src{values, offsets};
+    return append_rows(mvh, &src, n, row_ids,
+        [&](lgpu_multivec *mv) {
+            LGPU_REQUIRE(mv->f16 == f16, mv->f16 ? "the handle holds fp16 vectors: append them with lgpu_multivec_append_f16"
+                                                 : "the handle holds f32 vectors: append them with lgpu_multivec_append");
+            check_multivec_rows(src, n, mv->total);
+        },
+        mv_store_rows, mv_row_terms);
+}
+
+int lgpu_multivec_append(lgpu_multivec *mvh, const float *values, const uint64_t *offsets, uint64_t n,
+                         const uint64_t *row_ids)
+{
+    return multivec_append(mvh, values, false, offsets, n, row_ids);
+}
+
+int lgpu_multivec_append_f16(lgpu_multivec *mvh, const uint16_t *values, const uint64_t *offsets, uint64_t n,
+                             const uint64_t *row_ids)
+{
+    return multivec_append(mvh, values, true, offsets, n, row_ids);
 }
 
 int lgpu_multivec_device_bytes(const lgpu_multivec *mv, uint64_t *bytes) { return rows_device_bytes(mv, bytes); }

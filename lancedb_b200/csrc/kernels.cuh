@@ -520,9 +520,11 @@ void launch_mv_approx_sum(const uint32_t *M, uint64_t ldM, const uint32_t *q_off
 // thr[b] = dist[b][k-1] + 2 E_b when cnt[b] >= k, else +inf; E_b = mv_band(nq_b, d), or mv_band_f16 when f16
 void launch_mv_threshold(const float *dist, const uint32_t *cnt, const uint32_t *q_off, uint32_t qa, uint32_t B,
                          uint32_t k, uint32_t d, bool f16, float *thr, cudaStream_t st);
-// every row r with A[b][r] <= thr[b] is appended to cand[b][.] (count[b] zeroed by the caller, may exceed cap)
+// every row r with A[b][r] <= thr[b] that passes the row filter (allow null: none; the bit of its id col_ids[r], or r
+// without ids, set and below allow_bits) is appended to cand[b][.] (count[b] zeroed by the caller, may exceed cap)
 void launch_mv_admit(const float *A, uint64_t ldA, uint32_t B, uint64_t N, const float *thr, uint32_t cap,
-                     uint32_t *count, uint32_t *cand, cudaStream_t st);
+                     uint32_t *count, uint32_t *cand, const uint64_t *col_ids, const uint32_t *allow,
+                     uint64_t allow_bits, cudaStream_t st);
 // flags[b] = count[b] > cap or a vector of query b is bad; vflags[i] = flags of the query of vector i; *gate = any flag
 void launch_mv_flags(const uint32_t *count, uint32_t cap, const uint32_t *qbad, const uint32_t *q_off, uint32_t qa,
                      uint32_t B, uint32_t *flags, uint32_t *vflags, uint32_t *gate, cudaStream_t st);

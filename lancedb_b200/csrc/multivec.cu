@@ -8,7 +8,8 @@
 // policy of gemm_dist_kernel, whose epilogue keeps the largest approximate similarity per (query vector, document)
 // (an fp16 handle: the F16RowMaxSim policy, fp16 normalised queries against the stored fp16 vectors, each similarity
 // scaled by 1 / |v|); mv_approx_sum_kernel turns those into approximate distances, a shortlist admits every row within
-// 2 E of the k-th approximate distance (mv_band below, mv_band_f16 for an fp16 handle), dist.cu's mv_rescore_kernel
+// 2 E of the k-th approximate distance over the rows that pass the call's row filter (mv_band below, mv_band_f16 for
+// an fp16 handle; mv_admit_kernel admits only such rows), dist.cu's mv_rescore_kernel
 // re-scores the admitted rows exactly, and a query whose list overflowed (or that holds a zero / non-finite vector)
 // is redone by the exact path.
 //
@@ -138,18 +139,26 @@ __global__ void mv_threshold_kernel(const float *__restrict__ dist, const uint32
     thr[b] = cnt[b] >= k ? __fadd_ru(dist[(size_t)b * k + k - 1], __fmul_ru(2.0f, E)) : CUDART_INF_F;   // rounded up
 }
 
+// allow: the row filter (null: none), tested by the id of row r -- col_ids[r], or r without ids -- only for a row
+// under the threshold, so that a filtered row never takes a shortlist slot
 __global__ void mv_admit_kernel(const float *__restrict__ A, uint64_t ldA, uint64_t N, const float *__restrict__ thr,
-                                uint32_t cap, uint32_t *__restrict__ count, uint32_t *__restrict__ cand)
+                                uint32_t cap, uint32_t *__restrict__ count, uint32_t *__restrict__ cand,
+                                const uint64_t *__restrict__ col_ids, const uint32_t *__restrict__ allow,
+                                uint64_t allow_bits)
 {
     pdl_entry();
     const uint32_t b = blockIdx.y;
     const float t = thr[b];
     const float *row = A + (size_t)b * ldA;
-    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < N; r += (uint64_t)gridDim.x * blockDim.x)
-        if (row[r] <= t) {
-            const uint32_t slot = atomicAdd(count + b, 1u);
-            if (slot < cap) cand[(size_t)b * cap + slot] = (uint32_t)r;
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < N; r += (uint64_t)gridDim.x * blockDim.x) {
+        if (!(row[r] <= t)) continue;
+        if (allow) {
+            const uint64_t id = col_ids ? __ldg(col_ids + r) : r;
+            if (!(id < allow_bits && ((__ldg(allow + (id >> 5)) >> (id & 31)) & 1u))) continue;
         }
+        const uint32_t slot = atomicAdd(count + b, 1u);
+        if (slot < cap) cand[(size_t)b * cap + slot] = (uint32_t)r;
+    }
 }
 
 // one block
@@ -316,11 +325,12 @@ void launch_mv_threshold(const float *dist, const uint32_t *cnt, const uint32_t 
 }
 
 void launch_mv_admit(const float *A, uint64_t ldA, uint32_t B, uint64_t N, const float *thr, uint32_t cap,
-                     uint32_t *count, uint32_t *cand, cudaStream_t st)
+                     uint32_t *count, uint32_t *cand, const uint64_t *col_ids, const uint32_t *allow,
+                     uint64_t allow_bits, cudaStream_t st)
 {
     if (B == 0 || N == 0) return;
     launch_k(mv_admit_kernel, dim3((unsigned)std::min<uint64_t>((N + 1023) / 1024, 64), B), dim3(256), 0, st, A, ldA, N,
-             thr, cap, count, cand); LGPU_COUNT_LAUNCH();
+             thr, cap, count, cand, col_ids, allow, allow_bits); LGPU_COUNT_LAUNCH();
     LGPU_CUDA(cudaGetLastError());
 }
 

@@ -176,10 +176,15 @@ class Table:
         return _is_multivec_type(self._data.schema.field(column).type)
 
     def _multivec_rows(self, column: str):
-        """(values [T, dim], offsets [N+1] u64) of a multivector column; a null row holds no vectors.  float16 elements
-        stay float16 (GpuMultivec keeps them so, with the results of their exact f32 upcast); float64 elements are
-        converted to f32."""
-        col = self._data.column(column).combine_chunks()
+        """(values [T, dim], offsets [N+1] u64) of a multivector column (_multivec_rows_of)."""
+        return self._multivec_rows_of(self._data, column)
+
+    @staticmethod
+    def _multivec_rows_of(table: pa.Table, column: str):
+        """(values [T, dim], offsets [N+1] u64) of a multivector column of `table`; a null row holds no vectors.
+        float16 elements stay float16 (GpuMultivec keeps them so, with the results of their exact f32 upcast); float64
+        elements are converted to f32."""
+        col = table.column(column).combine_chunks()
         lens = col.value_lengths().fill_null(0).to_numpy(zero_copy_only=False).astype(np.int64)
         inner = col.flatten()                               # skips the values behind null rows
         if inner.null_count:
@@ -272,7 +277,8 @@ class Table:
         (unless fast_search()), until optimize() folds them into the index.
         on_bad_vectors="error" (the reference's default, and the only policy served): a float vector holding a NaN is
         refused (python/python/lancedb/table.py:4429-4445), and so is a row the column's index could not take at
-        optimize(): an infinite component, or a zero vector under a cosine index.  A refused call changes nothing."""
+        optimize(): an infinite component, or a zero vector under a cosine index.  A multivector row holding a null vector
+        is refused too.  A refused call changes nothing."""
         if mode == "overwrite":
             raise NotImplementedError("add(mode='overwrite') is not supported: only appends are")
         if mode != "append":
@@ -293,6 +299,9 @@ class Table:
         rows = {c: self._rows_of(new, c) for c in _vector_columns(self.schema) if not self._is_multivec(c)}
         for c, x in rows.items():
             self._check_new_rows(c, x)
+        # (values, offsets) of every multivector column: a row holding a null vector is refused here, before anything
+        # changes, as a search of the column would refuse it
+        mv_rows = {c: self._multivec_rows_of(new, c) for c in _vector_columns(self.schema) if self._is_multivec(c)}
         ids = np.arange(n0, n0 + n, dtype=np.uint64)
         done = []                   # the tails grow before the table does: a failure leaves the table as it was
         try:
@@ -314,16 +323,14 @@ class Table:
         self._data = pa.concat_tables([self._data, new]).combine_chunks()
         if self._live is not None:
             self._live = np.concatenate([self._live, np.ones(n, bool)])
-        for cache in (self._flat, self._binary):         # full-column caches grow in place (ids = positions)
+        for cache in (self._flat, self._binary, self._multivec):    # full-column caches grow in place (ids = positions)
             for column in list(cache):
+                new_rows = mv_rows[column] if cache is self._multivec else (rows[column],)
                 try:   # (a cache opened over the live rows holds explicit ids: the new ones are passed)
-                    cache[column].append(rows[column], None if self._live is None else ids)
+                    cache[column].append(*new_rows, row_ids=None if self._live is None else ids)
                 except BaseException:
                     cache.pop(column).close()             # reopened from the table on the next search
                     raise
-        for mv in self._multivec.values():               # reopened on the next search
-            mv.close()
-        self._multivec.clear()
         self.version += 1
 
     def _check_new_rows(self, column: str, x: np.ndarray) -> None:

@@ -6,7 +6,7 @@ Workloads (fixed row lengths, latent-factor vectors as in bench_multivector.py, 
   colbert_b1   50 000 rows x 128 vectors x d 128, nq 32, B 1        (tensor-core route)
   colbert      the same at B 64                                     (tensor-core route)
   colpali      10 000 rows x 1030 vectors x d 128, nq 24, B 16      (tensor-core route)
-  colbert_pf   the colbert column with a 10 % prefilter at B 8      (exact route)
+  colbert_pf   the colbert column with a 10 % prefilter at B 8      (tensor-core route under the prefilter)
 Each column is opened with both placements at a size that fits HBM.
 
 Prints one JSON line each for

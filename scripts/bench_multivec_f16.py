@@ -6,8 +6,8 @@ Columns (fixed row lengths, latent-factor vectors as in bench_multivector.py, st
   colbert   20 000 rows x 128 vectors x d 128, nq 32
   colpali    2 000 rows x 1030 vectors x d 128, nq 24
 Each column is opened four times: fp16 and f32, in HBM and in pinned host memory (LGPU_MULTIVEC_HBM_BYTES=0).
-Workloads per placement: colbert at B 1 and B 64 and colpali at B 16, on the tensor-core route (no filter) and on the
-exact route (a 10 % prefilter, which forces it).
+Workloads per placement: colbert at B 1 and B 64 and colpali at B 16, with no filter and with a 10 % prefilter (the
+route each call took is reported; run with LGPU_NO_TENSOR_CORE=1 for the exact route).
 
 Prints one JSON line each for
   device     the card's name and power limit, read in this run
