@@ -17,9 +17,11 @@
 // them, re-scores those few rows in the oracle's arithmetic (pq_rescore_kernel) and redoes unproven queries with
 // the exact kernel, so the reported ids and distances are bit-identical to the exact path.
 //
-// Pipeline: identical hand-over protocol to scan2.cu (tests/test_scan2_protocol.py models it): persistent CTAs,
-// a ring of three shared chunk buffers, named barriers FULL/EMPTY between 8 stager warps and 8 scanner warps, the
-// stage counter running on across tiles, tile descriptors claimed two tiles ahead.
+// Pipeline: persistent CTAs, a ring of three shared chunk buffers between 8 stager warps and 8 scanner warps (FULL
+// mbarriers, EMPTY named barriers), the stage counter running on across tiles, tile descriptors claimed two tiles
+// ahead.  A tile of nch chunks takes nch stages, and every buffer goes back to the stagers as soon as its stage has
+// been read -- a tile's last buffer only after the tile's epilogue -- so the stagers can fill all three buffers ahead
+// of the scanners (tests/test_scan3_ring_protocol.py models the hand-over).
 //   tile    = (partition, <= 8 of the queries probing it, <= 1536 rows); two CTAs per SM
 //   chunk   = 8 sub-spaces: shared [256 codes][8 sub-spaces][8 queries] u16 = 32 KB
 //   stagers : thread c owns code c.  It loads the 16 bytes (8 sub-spaces) of each of the tile's queries for code c
@@ -28,14 +30,17 @@
 //             stored ROTATED -- position j of code c holds sub-space (j + c) mod 8 -- so that in step j the eight
 //             lanes of a quarter-warp write eight different 16-byte slots: conflict-free without a per-lane
 //             register rotation.
-//   scanners: thread = rows row0 + ct + 256 r (r < 6); the skewed code stream (retile.cu) makes the eight lanes of
-//             a quarter-warp read eight different sub-space slots, so every LDS.128 is conflict-free whatever the
-//             codes are; accumulators are 4 x u32 per row (8 queries x u16).
-//   candidate epilogue (k <= 32): the scanners keep the tile's last data buffer after the zero stage, park the sums
-//             in it ([8 queries][1536 rows] u16 + the row terms) behind two scanner barriers, and warp g then runs
-//             query g alone with warp reductions; each warp hands the buffer back when its query is done.  The
-//             stagers need it for the next tile's chunk 1 only (tests/test_scan3_epilogue_protocol.py).  k > 32 keeps
-//             the block-wide epilogue, one query after the other, because of its list tightening.
+//   scanners: thread = rows row0 + ct + 256 r (r < 6), sig = row % 8; at step e of stage `it` the lane reads
+//             sub-space (e - sig) & 7 of chunk `it`, so the eight lanes of a quarter-warp read eight different
+//             sub-space slots and every LDS.128 is conflict-free whatever the codes are.  The code stream (retile.cu)
+//             delays row r's bytes by sig, so those codes are byte e of block `it` for e >= sig and byte e of block
+//             it + 1 for e < sig: one per-byte select of the two blocks per stage.  The sums are integers that cannot
+//             overflow, so their order does not matter.  Accumulators are 4 x u32 per row (8 queries x u16).
+//   candidate epilogue (k <= 32): the scanners keep the tile's last buffer, park the sums in it ([8 queries][1536
+//             rows] u16 + the row terms) behind two scanner barriers, and warp g then runs query g alone with warp
+//             reductions; each warp hands the buffer back when its query is done.  Meanwhile the stagers fill the
+//             next tile's chunks 0 and 1 into the other two buffers.  k > 32 keeps the block-wide epilogue, one query
+//             after the other, because of its list tightening.
 // Algorithmic bytes per tile row and query: m code bytes (SURVEY.md 8d), as for the exact kernel.
 #include "kernels.cuh"
 #include "scan_common.cuh"
@@ -66,7 +71,7 @@ constexpr int BAR_SCAN = 8;                         // named barrier of the 256 
 // FULL hand-over (stagers -> scanners) as mbarriers, one per ring buffer: a named barrier made the 8 scanner warps
 // wait for EACH OTHER at every stage (bar.sync counts all of them), so a stage took as long as its slowest warp; with
 // an mbarrier only the stagers arrive (one elected lane per warp) and every scanner warp goes on as soon as the
-// buffer is full.  The scanners can then drift apart by at most two stages (the EMPTY barrier, which the stagers
+// buffer is full.  The scanners can then drift apart by at most three stages (the EMPTY barrier, which the stagers
 // wait on, needs all of them).  LGPU_S3_NAMED_FULL=1 at build time restores the named barrier (A/B).
 #ifndef LGPU_S3_NAMED_FULL
 #define LGPU_S3_NAMED_FULL 0
@@ -74,7 +79,7 @@ constexpr int BAR_SCAN = 8;                         // named barrier of the 256 
 constexpr size_t S3_MBAR_OFF = S3_TILES + S3_SLOTS * S3_SLOT_BYTES + 2 * S3_SCR * 4;   // 3 x 8 bytes, 8-byte aligned
 constexpr size_t S3_QS_OFF = S3_MBAR_OFF + 32;     // [SCAN_G][step, cst, slack, -] f32
 static_assert(S3_QS_OFF + SCAN_G * 16 == S3_SMEM, "shared-memory layout");
-// The k <= 32 candidate epilogue parks the tile's sums in the chunk buffer its last data stage used:
+// The k <= 32 candidate epilogue parks the tile's sums in the chunk buffer its last stage used:
 // [SCAN_G queries][SCAN3_ROWS_TILE rows] u16, then the row terms R(row) as [SCAN3_ROWS_TILE] f32.
 constexpr int S3_SUMS_BYTES = SCAN_G * SCAN3_ROWS_TILE * 2;
 static_assert(S3_SUMS_BYTES + SCAN3_ROWS_TILE * 4 <= S3_BUF, "sum area inside one chunk buffer");
@@ -177,46 +182,38 @@ __device__ __forceinline__ void stager_loop(const ScanArgs &a, uint32_t total, i
     const int lane = tid & 31, pw = tid >> 5;
     const uint32_t nch = a.nch, c = (uint32_t)tid;
 
-    // One slab in registers.  The loads of the next data stage are issued right after this stage's slab has been
-    // written to shared memory, i.e. a whole scanner stage before they are needed: they land while the stagers
-    // wait for the ring buffer to come free.
+    // One slab in registers.  The loads of the next stage are issued right after this stage's slab has been written
+    // to shared memory, i.e. a whole scanner stage before they are needed: they land while the stagers wait for the
+    // ring buffer to come free.
     Slab cur;
     {
         const TileDesc *T0 = slot3(tiles, 0);
         if (T0->ng) slab_load(cur, a, T0, 0, c);
     }
+    constexpr int TD_WORDS = (int)(sizeof(TileDesc) / 4);
     int b = 0;
-    uint32_t gs = 0;
+    uint32_t gs = 0, t_claim = 0, t_word = 0;
     for (uint32_t n = 0;; n++) {
         const TileDesc *T = slot3(tiles, n);
         if (T->ng == 0) break;
-        const TileDesc *Tn = slot3(tiles, n + 1);
-        const bool next_tile = Tn->ng != 0;
-        uint32_t t_claim = 0, t_word = 0;
-        for (uint32_t ch = 0; ch <= nch; ch++) {
-            // --- tile look-ahead (warp 0): claim at stage 0, read the descriptor at stage 1 ---
-            if (pw == 0) {
-                if (ch == 0) {
-                    if (lane == 0) t_claim = atomicAdd(a.tile_counter, 1u);
-                    t_claim = __shfl_sync(0xffffffffu, t_claim, 0);
-                } else if (ch == 1) {
-                    t_word = 0;
-                    if (lane < (int)(sizeof(TileDesc) / 4) && t_claim < total)
-                        t_word = __ldg(reinterpret_cast<const uint32_t *>(a.tile_desc + t_claim) + lane);
-                }
+        for (uint32_t ch = 0; ch < nch; ch++) {
+            if (gs >= 3) bar_sync(BAR_EMPTY + b, S3_NT);           // scanners are done with stage gs-3
+            // --- tile look-ahead (warp 0): at stage 0 publish tile n+1 (claimed during tile n-1; the kernel's prologue
+            // wrote tiles 0 and 1) and claim tile n+2; read the claimed descriptor at the tile's last stage.  Slot n+1
+            // last held tile n-3, which every scanner has left: the EMPTY wait above saw them arrive for stage gs-3, and
+            // a tile's last stage is released only after its epilogue.
+            if (pw == 0 && ch == 0) {
+                if (n > 0 && lane < TD_WORDS)
+                    reinterpret_cast<uint32_t *>(const_cast<TileDesc *>(slot3(tiles, n + 1)))[lane] = t_word;
+                if (lane == 0) t_claim = atomicAdd(a.tile_counter, 1u);
+                t_claim = __shfl_sync(0xffffffffu, t_claim, 0);
             }
-            if (gs >= 2) bar_sync(BAR_EMPTY + b, S3_NT);           // scanners are done with stage gs-2
-            if (ch == nch) {                                       // all-zero code-0 row for the lagging lanes
-                if (tid < 32) reinterpret_cast<uint32_t *>(smem + b * S3_BUF)[tid] = 0u;
-            } else {
-                slab_store(cur, lut + (uint32_t)b * S3_BUF, c);
-                // the next data stage: the next chunk of this tile, or chunk 0 of the next tile (which then
-                // rides through the zero stage)
-                if (ch + 1 < nch) slab_load(cur, a, T, ch + 1, c);
-                else if (next_tile) slab_load(cur, a, Tn, 0, c);
+            if (pw == 0 && ch + 1 == nch) {
+                t_word = 0;
+                if (lane < TD_WORDS && t_claim < total)
+                    t_word = __ldg(reinterpret_cast<const uint32_t *>(a.tile_desc + t_claim) + lane);
             }
-            if (pw == 0 && ch == 1 && lane < (int)(sizeof(TileDesc) / 4))   // publish tile n+2 before FULL(stage 1)
-                reinterpret_cast<uint32_t *>(const_cast<TileDesc *>(slot3(tiles, n + 2)))[lane] = t_word;
+            slab_store(cur, lut + (uint32_t)b * S3_BUF, c);
 #if LGPU_S3_NAMED_FULL
             bar_arrive(BAR_FULL + b, S3_NT);
 #else
@@ -224,10 +221,21 @@ __device__ __forceinline__ void stager_loop(const ScanArgs &a, uint32_t total, i
             if (lane == 0) mbar_arrive(lut + (uint32_t)S3_MBAR_OFF + 8u * (uint32_t)b);
 #endif
             bar_sync(BAR_PROD, S3_PT);
+            // the next stage: the next chunk of this tile, or chunk 0 of the next tile, whose descriptor warp 0
+            // published at stage 0 (before the barrier above)
+            if (ch + 1 < nch) {
+                slab_load(cur, a, T, ch + 1, c);
+            } else {
+                const TileDesc *Tn = slot3(tiles, n + 1);
+                if (Tn->ng) slab_load(cur, a, Tn, 0, c);
+            }
             b = ring_next3(b);
             gs++;
         }
     }
+    // The scanners arrive on EMPTY after every stage, the last three included; take those arrivals so that no named
+    // barrier is left part-way when the CTA exits.
+    for (uint32_t s = gs >= 3 ? gs - 3 : 0; s < gs; s++) bar_sync(BAR_EMPTY + (int)(s % 3), S3_NT);
 }
 
 // ---------------------------------------------------------------- scanner side
@@ -276,7 +284,7 @@ __device__ __noinline__ uint32_t tighten_from_list(const uint32_t *keys, uint32_
     return tkey;
 }
 
-// ---- candidate epilogue for k <= 32: one warp per query, on sums parked in the last data buffer.
+// ---- candidate epilogue for k <= 32: one warp per query, on sums parked in the tile's last buffer.
 // tau_q (global, atomicMin) is any value such that at least k rows of the query have L <= tau_q: then the k-th
 // smallest exact distance is <= tau_q + W + E and every row of the exact top-k has L <= tau_q + W + 2E =
 // tau_q + slack_q.  A tile tightens tau_q from its own rows (an upper bound of their k-th smallest L, by 8 counting
@@ -288,11 +296,11 @@ __device__ __noinline__ uint32_t tighten_from_list(const uint32_t *keys, uint32_
 // area behind one scanner barrier (every warp has read the buffer) and read them back behind a second one, so that
 // warp g handles query g alone: its counts are warp reductions, and the only block barriers of the epilogue are those
 // two.  The buffer goes back to the stagers when every warp is done with its query; the stagers need it for the next
-// tile's chunk 1 only, which no scanner can use before then.  tests/test_scan3_epilogue_protocol.py models the hold.
+// tile's chunk 2 only, which no scanner can use before then.  tests/test_scan3_ring_protocol.py models the hold.
 // One query of a tile (query g), by one warp, over the sums and row terms parked in ring buffer bp.  Out of line, like
 // tighten_from_list, with only pointers and two indices as arguments: of the forms tried (inlined into the three gather
 // variants, out of line with the query's values as arguments) this one adds the fewest spill reloads to the gather
-// loops, though still 1-2 per stage (DESIGN.md §3).  `a` is the kernel's __grid_constant__ parameter, read in place.
+// loops (DESIGN.md §3).  `a` is the kernel's __grid_constant__ parameter, read in place.
 __device__ __noinline__ void cand_query_warp(const ScanArgs *ap, const TileDesc *T, int g, int bp)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -420,13 +428,13 @@ __device__ __noinline__ void cand_query_warp(const ScanArgs *ap, const TileDesc 
 }
 
 template <int R>
-__device__ __forceinline__ void cand_epilogue_warp(const ScanArgs &a, const TileDesc *T, bool next_exists, int bp, int ct,
+__device__ __forceinline__ void cand_epilogue_warp(const ScanArgs &a, const TileDesc *T, int bp, int ct,
                                                    const uint32_t (&acc)[R][4], const bool (&valid)[R], const float (&rr)[R])
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int ng = (int)T->ng, lane = ct & 31, g = ct >> 5;
     unsigned char *const area = smem + bp * S3_BUF;
-    bar_sync(BAR_SCAN, S3_CT);                            // every warp has read the last data buffer
+    bar_sync(BAR_SCAN, S3_CT);                            // every warp has read the last buffer
     {
         unsigned short *const sums = reinterpret_cast<unsigned short *>(area);
         float *const rrs = reinterpret_cast<float *>(area + S3_SUMS_BYTES);
@@ -443,14 +451,12 @@ __device__ __forceinline__ void cand_epilogue_warp(const ScanArgs &a, const Tile
     }
     bar_sync(BAR_SCAN, S3_CT);
     if (g < ng) cand_query_warp(&a, T, g, bp);
-    if (next_exists) {                                    // hand the buffer back for the next tile's chunk 1
-        __syncwarp();
-        bar_arrive(BAR_EMPTY + bp, S3_NT);
-    }
+    __syncwarp();                                         // hand the buffer back for the next tile's chunk 2
+    bar_arrive(BAR_EMPTY + bp, S3_NT);
 }
 
 template <int R, bool LIST>
-__device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, bool next_exists, int b, int ct, uint32_t &ph)
+__device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, int b, int ct, uint32_t &ph)
 {
     extern __shared__ __align__(1024) unsigned char smem[];
     const uint32_t lut = (uint32_t)__cvta_generic_to_shared(smem);
@@ -460,29 +466,33 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
     const int sig = ct & 7;                               // this lane's skew (== row % 8)
     const uint32_t n_p = T->n_p, npad = T->npad;                                    // (copied into the descriptor)
     const uint2 *cs = reinterpret_cast<const uint2 *>(a.codes + ((uint64_t)T->code_base8 << 3));   // [nch+1][npad]
+    // Row r's block j holds stream positions 8j..8j+7, i.e. codes 8j - sig .. 8j + 7 - sig.  In stage `it` the lane
+    // reads sub-space (e - sig) & 7 of chunk `it` at step e: for e >= sig that code is byte e of block it, for e < sig
+    // byte e of block it + 1.  So a stage's code word is a per-byte select of the two blocks, by these masks.
+    const uint32_t sel_x = sig >= 4 ? 0xffffffffu : (1u << (8 * sig)) - 1u;
+    const uint32_t sel_y = sig <= 4 ? 0u : (1u << (8 * (sig - 4))) - 1u;
 
     uint32_t acc[R][4];
     bool valid[R];
-    uint2 wn[R];
+    uint2 w[R], wn[R];                                    // blocks it and it + 1 of each row
 #pragma unroll
     for (int r = 0; r < R; r++) {
 #pragma unroll
         for (int g = 0; g < 4; g++) acc[r][g] = 0u;
         const uint32_t row = row0 + ct + r * S3_CT;
         valid[r] = row < row0 + nrows && row < n_p;
-        wn[r] = valid[r] ? __ldg(cs + row) : make_uint2(0u, 0u);
+        w[r] = valid[r] ? __ldg(cs + row) : make_uint2(0u, 0u);
     }
 
-    for (uint32_t it = 0; it <= nch; it++) {
-        uint2 w[R];
+    int bl = b;                                           // buffer of the tile's last stage
+    for (uint32_t it = 0; it < nch; it++) {
+        // Block it + 1 (block nch, the stream's last, for the last chunk), loaded while the stage's buffer fills.
+        // Loading it a stage earlier instead, as a third block in registers, measured slower: the 6-row loop then
+        // reloads more spilled registers per stage than the load's latency costs here.
 #pragma unroll
-        for (int r = 0; r < R; r++) w[r] = wn[r];
-        if (it < nch) {                                    // prefetch the next block of code bytes
-#pragma unroll
-            for (int r = 0; r < R; r++) {
-                const uint32_t row = row0 + ct + r * S3_CT;
-                wn[r] = valid[r] ? __ldg(cs + (size_t)(it + 1) * npad + row) : make_uint2(0u, 0u);
-            }
+        for (int r = 0; r < R; r++) {
+            const uint32_t row = row0 + ct + r * S3_CT;
+            wn[r] = valid[r] ? __ldg(cs + (size_t)(it + 1) * npad + row) : make_uint2(0u, 0u);
         }
 #if LGPU_S3_NAMED_FULL
         bar_sync(BAR_FULL + b, S3_NT);
@@ -490,22 +500,28 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
         mbar_wait(lut + (uint32_t)S3_MBAR_OFF + 8u * (uint32_t)b, (ph >> b) & 1u);
         ph ^= 1u << b;
 #endif
-        const int bp = b == 0 ? 2 : b - 1;                 // buffer of the previous stage
-        const uint32_t base_cur = lut + (uint32_t)b * S3_BUF;
-        const uint32_t base_prev = lut + (uint32_t)bp * S3_BUF;
+        uint2 cw[R];                                       // the codes of chunk `it`, byte e for step e
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+            cw[r].x = (w[r].x & ~sel_x) | (wn[r].x & sel_x);
+            cw[r].y = (w[r].y & ~sel_y) | (wn[r].y & sel_y);
+            w[r] = wn[r];
+        }
+        const uint32_t base = lut + (uint32_t)b * S3_BUF;
 #pragma unroll
         for (int e = 0; e < 8; e++) {
-            const uint32_t off = ((e < sig) ? base_prev : base_cur) + (uint32_t)(((e - sig) & 7) << 4);
+            const uint32_t off = base + (uint32_t)(((e - sig) & 7) << 4);
 #pragma unroll
             for (int r = 0; r < R; r++) {
-                const uint32_t word = (e < 4) ? w[r].x : w[r].y;
+                const uint32_t word = (e < 4) ? cw[r].x : cw[r].y;
                 const uint32_t code = (word >> (8 * (e & 3))) & 0xffu;
                 const uint4 v = lds128u(off + (code << 7));
                 acc[r][0] += v.x; acc[r][1] += v.y; acc[r][2] += v.z; acc[r][3] += v.w;
             }
         }
-        // the k <= 32 candidate epilogue keeps the last data buffer (the zero stage's bp) and hands it back itself
-        if (it + 2 <= nch || (next_exists && (it < nch || a.cand == nullptr || LIST))) bar_arrive(BAR_EMPTY + bp, S3_NT);
+        // every stage's buffer goes back at once, except the last: that one is released after the epilogue
+        if (it + 1 < nch) bar_arrive(BAR_EMPTY + b, S3_NT);
+        else bl = b;
         b = ring_next3(b);
     }
 
@@ -534,11 +550,12 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
                 }
             }
         }
+        __syncwarp();
+        bar_arrive(BAR_EMPTY + bl, S3_NT);
         return b;
     }
     if constexpr (!LIST) {
-        // the zero stage's previous buffer: two stages before the next tile's, i.e. b + 1 in the ring of three
-        cand_epilogue_warp<R>(a, T, next_exists, ring_next3(b), ct, acc, valid, rr);
+        cand_epilogue_warp<R>(a, T, bl, ct, acc, valid, rr);
         return b;
     }
     // candidate mode with the list tightening (k > 32), the same threshold policy as cand_epilogue_warp, run by the
@@ -676,6 +693,8 @@ __device__ __forceinline__ int scan_tile(const ScanArgs &a, const TileDesc *T, b
             }
         }
     }
+    __syncwarp();
+    bar_arrive(BAR_EMPTY + bl, S3_NT);
     return b;
 }
 
@@ -690,9 +709,8 @@ __device__ __forceinline__ void scanner_loop(const ScanArgs &a, int tid)
     for (uint32_t n = 0;; n++) {
         const TileDesc *T = slot3(tiles, n);
         if (T->ng == 0) break;
-        const bool next_exists = slot3(tiles, n + 1)->ng != 0;
         const int R = (int)((T->nrows + S3_CT - 1) / S3_CT);
-#define LGPU_SCAN3(RR) b = scan_tile<RR, LIST>(a, T, next_exists, b, ct, ph)
+#define LGPU_SCAN3(RR) b = scan_tile<RR, LIST>(a, T, b, ct, ph)
         if (R <= 2) LGPU_SCAN3(2);
         else if (R <= 4) LGPU_SCAN3(4);
         else LGPU_SCAN3(6);
@@ -712,8 +730,6 @@ __global__ void __launch_bounds__(S3_NT, 2) scan3_kernel(const __grid_constant__
     const uint32_t total = *a.total_tiles;
     unsigned char *const tiles = smem + S3_TILES;
 
-    // "stage -1" of the first tile: zero code-0 row in ring buffer 2
-    if (tid < 32) reinterpret_cast<uint32_t *>(smem + 2 * S3_BUF)[tid] = 0u;
 #if !LGPU_S3_NAMED_FULL
     if (tid == 0) {
         const uint32_t mb = (uint32_t)__cvta_generic_to_shared(smem) + (uint32_t)S3_MBAR_OFF;
